@@ -16,9 +16,13 @@ metric  = nvlink_probe_ms (lower is better): time to produce the N x N reachabil
           (median of the K timed steps, max over ranks; buffers resident in HBM; the mean and the worst
           step are in `value_mean_ms` / `value_max_ms`); `e2e.value` is the same probe through the
           public C ABI call from the host: launch, kernel, result rows written to pinned host
-          memory and read back.  Per-pair GB/s vs the 900 GB/s/dir NVLink-5 peak is in
+          memory and read back.  Per-pair GB/s vs the 450 GB/s/dir NVLink-4 peak of an H100 SXM is in
           `per_link_gbps`; `roofline` is the dominant kernel against its bound (HBM at N = 1,
           NVLink at N > 1).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller
+(reachability, mapping status and the 64-bit checksums of every cell) as .npy files, so that two builds
+can be compared output for output; with the same arguments the inputs (seeded patterns) are identical.
 """
 from __future__ import annotations
 
@@ -36,16 +40,10 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GIB = 1 << 30
-NVLINK_PEAK_GBPS = 900.0        # nominal per direction per GPU (BASELINE.md §2)
-# (the profiling guide quotes a 770 GB/s peer copy; it is not used: every N > 1 line carries the SAME-BOX copy-engine
-#  figures measured next to the probe on the probe's own buffers, roofline.peak_measured_ce_{uni,bidi})
-HBM_FALLBACK_GBPS = 6650.0
-# Bytes on the NVLink wire per payload byte of SM-issued traffic, from ncu's nvltx/nvlrx counters on the solo probe
-# kernel (profiles/r02_ncu_nvlink_{read,write}.csv; 1 GiB of payload each): a read costs 1.125 B of response in the
-# payload direction (32 B per 256-B response) and 0.1875 B of request in the opposite one (48 B per 256 B); a write
-# costs 1.1875 B in the payload direction and ~0.003 B of acknowledgement back.
-WIRE = {"read_rx": 1207959648 / 1073741888, "read_tx_req": 201326656 / 1073741888,
-        "write_tx": 1275068544 / 1073741888, "write_rx_ack": 3453312 / 1073741888}
+NVLINK_PEAK_GBPS = 450.0        # nominal NVLink 4 per direction per GPU, H100 SXM data sheet (18 links x 25 GB/s)
+# (every N > 1 line also carries the SAME-BOX copy-engine figures measured next to the probe on the probe's own
+#  buffers, roofline.peak_measured_ce_{uni,bidi})
+HBM_FALLBACK_GBPS = 3350.0      # H100 SXM data sheet HBM3 bandwidth (700 W card); used when no measured peak is present
 
 
 def measured_peaks():
@@ -53,7 +51,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": HBM_FALLBACK_GBPS}, "fallback"
+        return {"hbm_gbs": HBM_FALLBACK_GBPS}, "data-sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -169,7 +167,7 @@ def cpu_poll_timing(n_gpus: int, steps: int, warmup: int, budget_s: float, flags
     per GPU."""
     from oracle import oracle as o
 
-    o.build()
+    o.lib()
     times, last = [], None
     t_stop = time.perf_counter() + budget_s
     for i in range(warmup + steps):
@@ -404,6 +402,8 @@ def run_probe(args):
     rc = abi.load_library().cdprobe_gather(probe._h, ctypes.byref(out))
     if rc != abi.OK:
         raise RuntimeError(f"cdprobe_gather rc={rc}")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     res = pkg.Result.from_c(out)
     warmed_steps = max_over_ranks(float(warmed))
 
@@ -413,7 +413,7 @@ def run_probe(args):
     if rank == 0:
         from oracle import oracle as o  # the checker: never on the measured path
 
-        o.build()
+        o.lib()
         parity = parity_block(pkg, o, res, n, args.bytes, mode_id, uuids, o.DEFAULT_SEED)
     parity_ok = grp.gather_objects(None if parity is None else
                                    bool(parity["checksum_ok"] and parity["reach_vs_nvml_ok"] is not False))[0]
@@ -458,7 +458,7 @@ def run_probe(args):
         u_w = [statistics.median(u.gbps_write[i][j] for u in ur) for i in range(n) for j in range(n) if i != j]
         uni = {"read_min": min(u_r), "read_median": statistics.median(u_r), "write_min": min(u_w),
                "write_median": statistics.median(u_w), "probe_ms": statistics.median(u.probe_ms for u in ur),
-               "frac_min_of_900": min(min(u_r), min(u_w)) / NVLINK_PEAK_GBPS,
+               "frac_min_of_peak": min(min(u_r), min(u_w)) / NVLINK_PEAK_GBPS,
                "reach_all_ones": all(all(all(c == 1 for c in row) for row in u.reach) for u in ur)}
         # ---- the same-box ceiling: the copy engine on the very same buffers, ranks 0 <-> 1 (untimed for the
         # headline).  One way: rank 0 pushes alone.  Both ways: ranks 0 and 1 push to each other at once (each
@@ -482,18 +482,11 @@ def run_probe(args):
     a_gpu = (n - 1 if n > 1 else 1) * bpp
     algo_bytes = passes * a_gpu  # per launch (= per GPU per probe)
     achieved = algo_bytes / (value * 1e-3) / 1e9
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            t = json.load(f).get(f"n{n}_{args.path}")
-        if t and args.bytes == GIB and args.mode == "sliced":
-            traffic = t["dram_bytes_read"] + t["dram_bytes_write"]
-    except Exception:
-        traffic = None
+    traffic = None  # DRAM bytes from hardware counters: no counter source is read here
     if n == 1:
         roofline = {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                     "frac": achieved / peaks["hbm_gbs"], "traffic": traffic,
-                    "traffic_source": "profiles/ncu_traffic.json (ncu --set full capture of this kernel)" if traffic else None, "peak_kind": f"{peak_kind} copy bandwidth",
+                    "peak_kind": f"{peak_kind} HBM bandwidth",
                     "kernel": "cdprobe_kernel", "algorithmic_bytes_per_launch": algo_bytes,
                     "note": "N=1 loop-back: read 1 GiB + write 1 GiB + verify 1 GiB of local HBM per launch"}
     else:
@@ -502,29 +495,17 @@ def run_probe(args):
         link_achieved = min(min(pairs_r), min(pairs_w))
         roofline = {"bound": "nvlink", "achieved": link_achieved, "peak": NVLINK_PEAK_GBPS, "unit": "GB/s",
                     "frac": link_achieved / NVLINK_PEAK_GBPS, "traffic": None,
-                    "peak_kind": "nominal NVLink 5 per direction per GPU; the same-box copy-engine ceilings are beside it",
+                    "peak_kind": "nominal NVLink 4 per direction per GPU; the same-box copy-engine ceilings are beside it",
                     "peak_measured_ce_uni": max(ce["uni_push"], ce["uni_pull"]), "peak_measured_ce_bidi": ce["bidi_push_min"],
                     "frac_of_ce_bidi": link_achieved / ce["bidi_push_min"],
                     "frac_read_of_ce_bidi": min(pairs_r) / ce["bidi_push_min"],
                     "frac_write_of_ce_bidi": min(pairs_w) / ce["bidi_push_min"],
                     "ce": ce,
-                    # wire-level view: with both directions loaded a port's direction carries, per payload byte of its own
-                    # op, the payload + protocol of that op plus the requests/acks of the opposite direction's op
-                    "wire_bytes_per_payload_byte": WIRE,
-                    "wire_gbps_read_phase": min(pairs_r) * (WIRE["read_rx"] + WIRE["read_tx_req"]),
-                    "wire_gbps_write_phase": min(pairs_w) * (WIRE["write_tx"] + WIRE["write_rx_ack"]),
-                    "frac_wire_read_phase_of_900": min(pairs_r) * (WIRE["read_rx"] + WIRE["read_tx_req"]) / NVLINK_PEAK_GBPS,
-                    "frac_wire_write_phase_of_900": min(pairs_w) * (WIRE["write_tx"] + WIRE["write_rx_ack"]) / NVLINK_PEAK_GBPS,
-                    "payload_ceiling_read_bidi": NVLINK_PEAK_GBPS / (WIRE["read_rx"] + WIRE["read_tx_req"]),
-                    "payload_ceiling_write_bidi": NVLINK_PEAK_GBPS / (WIRE["write_tx"] + WIRE["write_rx_ack"]),
-                    "wire_source": "profiles/r02_ncu_nvlink_read.csv, profiles/r02_ncu_nvlink_write.csv (ncu nvltx__/nvlrx__ "
-                                   "bytes of the solo probe kernel)",
                     "kernel": "cdprobe_kernel", "algorithmic_bytes_per_launch": algo_bytes,
                     "nvlink_bytes_per_launch_per_direction": a_gpu,
                     "aggregate_link_gbps_per_gpu": link_bytes / (value * 1e-3) / 1e9,
                     "note": "achieved = slowest ordered pair with exclusive endpoints (tournament round), both "
-                            "directions of every port loaded; SM-issued peer stores cap at ~715 GB/s one way on "
-                            "every store shape (profiles/r02_linkbench_n2.jsonl)"}
+                            "directions of every port loaded"}
 
     if rank == 0:
         wl = conf["name"].format(n=n, cycles=0) if conf else workload_name(n, args.mode, args.bytes)
@@ -539,7 +520,7 @@ def run_probe(args):
                 "ctas": int(info.ctas[0]), "rounds": res.rounds, "phases": res.phases,
                 "barriers": "all-rank" if args.all_rank_barriers else "neighbourhood",
                 "parallelism": f"{n} ranks, one process per GPU, no data-path collective",
-                "l2": "inputs (1 GiB per pass) exceed the 126 MB L2; no explicit flush",
+                "l2": "inputs (1 GiB per pass) exceed the 50 MB L2; no explicit flush",
                 "handle_type": int(info.handle_type),
             },
             "device_ms_globaltimer": device_ms, "kernel_ms_globaltimer": kernel_ms, "barrier_us": barrier_us,
@@ -598,6 +579,25 @@ def run_probe(args):
             sys.stderr.write("PARITY FAILURE: " + json.dumps(parity) + "\n")
         return 3
     return 0
+
+
+def dump_outputs(dirname: str, out) -> None:
+    """What one cdprobe_run hands its caller, cut to the n x n domain: reach bits and mapping status as float32,
+    each 64-bit checksum as its (high, low) 32-bit halves in float64, which holds them exactly.  Measured rates and
+    times are left out: they differ from run to run by design."""
+    import numpy as np
+
+    os.makedirs(dirname, exist_ok=True)
+    n, m = out.n, int(len(out.reach_read) ** 0.5)
+
+    def cells(field):
+        return np.ctypeslib.as_array(getattr(out, field)).reshape(m, m)[:n, :n]
+
+    for name in ("reach_read", "reach_write", "status"):
+        np.save(os.path.join(dirname, name + ".npy"), cells(name).astype(np.float32))
+    for name in ("sum_read", "xor_read", "sum_write", "xor_write"):
+        v = cells(name).astype(np.uint64)
+        np.save(os.path.join(dirname, name + ".npy"), np.stack([v >> np.uint64(32), v & np.uint64(0xFFFFFFFF)], -1).astype(np.float64))
 
 
 def daemon_once(n: int):
@@ -717,7 +717,7 @@ def run_storm(args, pkg, probe, grp, info, n, rank, local, daemon_cost, conf):
     if rank == 0:
         from oracle import oracle as o
 
-        o.build()
+        o.lib()
         parity = parity_block(pkg, o, res, n, args.bytes, 1, uuids, o.DEFAULT_SEED)
         line = {"metric": "nvlink_probe_ms", "value": stats["probe_ms_p50"], "unit": "ms", "n_gpus": n, "steps": cycles,
                 "warmup": max(args.warmup, 3), "ms_per_step": stats["wall_ms"] / cycles, "higher_is_better": False,
@@ -755,6 +755,8 @@ def main():
                     help="BASELINE.json configs beyond the headline: c2 (2 GPUs, 64 MiB, full), c3-full (1 GiB per ordered "
                          "pair), c5 (reconcile storm: --steps cycles)")
     ap.add_argument("--all-rank-barriers", action="store_true", help="round-1 barrier schedule (comparison)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step returned (reach bits, status, checksums) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

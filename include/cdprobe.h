@@ -19,7 +19,7 @@
  *   - the library never prints and never aborts (klog owns stdout/stderr in
  *     the daemon: cmd/compute-domain-daemon/process.go:92-96);
  *   - a handle is not thread-safe; distinct handles are independent;
- *   - there is NO CPU fallback: without a CUDA driver + sm_100 device
+ *   - there is NO CPU fallback: without a CUDA driver + sm_90 device
  *     cdprobe_open() fails with CDPROBE_ERR_NO_DEVICE / _UNSUPPORTED.
  *
  * All integer results (reachability bits, checksums, schedule) are exact;
@@ -41,7 +41,7 @@ extern "C" {
 #endif
 
 #define CDPROBE_ABI_VERSION 2u         /* 2: neighbourhood barriers (sync_mask), calibrated gate, ce_copy */
-#define CDPROBE_MAX_GPUS 16          /* ranks in one probe domain (8 on HGX B200) */
+#define CDPROBE_MAX_GPUS 16          /* ranks in one probe domain (8 on HGX H100) */
 #define CDPROBE_MAX_PHASES 64
 #define CDPROBE_NVLINK_MAX_LINKS 18  /* == NVML_NVLINK_MAX_LINKS (nvml.h:389) */
 
@@ -54,7 +54,7 @@ extern "C" {
 #define CDPROBE_ERR_TIMEOUT (-5)     /* timeout_ms expired (device or host watchdog) */
 #define CDPROBE_ERR_RENDEZVOUS (-6)  /* multi-process handle exchange failed */
 #define CDPROBE_ERR_NOMEM (-7)
-#define CDPROBE_ERR_UNSUPPORTED (-8) /* device lacks VMM / cooperative launch / sm_100 */
+#define CDPROBE_ERR_UNSUPPORTED (-8) /* device lacks VMM / cooperative launch / sm_90 */
 #define CDPROBE_ERR_STATE (-9)       /* handle unusable after a sticky CUDA error */
 #define CDPROBE_ERR_INTEGRITY (-10)  /* self-check of published checksums failed */
 
@@ -99,18 +99,15 @@ typedef struct {
   uint32_t flags;                       /* CDPROBE_FLAG_* */
   uint64_t seed;                        /* 0 = 0xCD5EED0000000001 */
   float min_fraction;                   /* verdict threshold on pair GB/s, as a fraction of the reference figure below;
-                                           0 = default (0.90 with the calibrated reference, see link_peak_gbps) */
+                                           0 = default (0.65) */
   float link_peak_gbps;                 /* reference figure of the gate.
-                                           0 (default) = CALIBRATED: what a healthy B200 NVLink-5 port delivers to
-                                           SM-issued traffic of that op and schedule, measured next to the copy engine
-                                           on the same box (profiles/r02_linkbench_n2.jsonl: both directions loaded,
-                                           reads 672 / writes 703 GB/s; one way, reads 785 / writes 714.7 — SM stores
-                                           cap there on every store shape and CTA count; the copy engine moves
-                                           773-778), de-rated for the ~8 us a phase spends ramping and draining:
-                                               expected(bytes_per_pair) = bytes_per_pair / (bytes_per_pair / rate + 8 us)
-                                           >0 = absolute: threshold = min_fraction x link_peak_gbps (900 = nominal
-                                           NVLink 5 per direction; the north_star's "0.85 x 900 = 765" is above what
-                                           any SM write and any bidirectional transfer reaches on healthy hardware) */
+                                           0 (default) = nominal H100 SXM NVLink 4 per direction (450 GB/s, data
+                                           sheet) for every op and schedule, de-rated for the 6 us a phase spends
+                                           ramping and draining (measured on an H100 at N = 1):
+                                               expected(bytes_per_pair) = bytes_per_pair / (bytes_per_pair / 450 + 6 us)
+                                           What healthy H100 NVLink delivers to SM-issued traffic has not been
+                                           measured; the default fraction leaves room below nominal for it.
+                                           >0 = absolute: threshold = min_fraction x link_peak_gbps */
   uint32_t ctas;                        /* CTAs of the persistent kernel; 0 = one per SM */
   uint32_t world_size;                  /* processes in the probe domain; 0/1 = single process */
   uint32_t rank;                        /* this process's index in [0, world_size) */
@@ -275,7 +272,7 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
 /* Runtime options (no reopen needed; the bench sweeps them). */
 #define CDPROBE_OPT_EVENT_TIMING 1u  /* value 0/1: bracket each kernel with CUDA events, report event_ms */
 #define CDPROBE_OPT_CTAS 2u          /* CTAs of the persistent kernel (0 = one per SM) */
-#define CDPROBE_OPT_PATH 3u          /* 0 = TMA bulk copies, 1 = ld/st.global.v4 (128-bit), 2 = ld/st.global.v8 (256-bit) */
+#define CDPROBE_OPT_PATH 3u          /* 0 = TMA bulk copies, 1 = ld/st.global.v4 (128-bit), 2 = ld/st.global.v4, 32 contiguous bytes per lane */
 #define CDPROBE_OPT_TIMEOUT_MS 4u
 #define CDPROBE_OPT_OVERLAP_VERIFY 5u /* value 0/1 */
 #define CDPROBE_OPT_VERIFY_CTAS 6u   /* CTAs given to the overlapped verify (default 32) */
@@ -285,7 +282,7 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
 #define CDPROBE_OPT_WARMUP_BYTES 9u  /* bytes each rank streams from its first partner when warming (default 8 MiB, capped at bytes_per_pair) */
 #define CDPROBE_OPT_CTAS_RANK 11u    /* value = ((local rank + 1) << 16) | ctas: CTA count of ONE local rank (tests: a throttled issuer) */
 #define CDPROBE_OPT_MIN_FRACTION_PPM 12u /* min_fraction x 1e6 (0 = default) */
-#define CDPROBE_OPT_LINK_PEAK_MBPS 13u   /* link_peak_gbps x 1e3 (0 = calibrated reference) */
+#define CDPROBE_OPT_LINK_PEAK_MBPS 13u   /* link_peak_gbps x 1e3 (0 = default reference) */
 #define CDPROBE_OPT_SOLO_RANK 14u    /* profiling: 1-based local rank that runs ALONE — only its own read/write jobs, no
                                         cross-GPU barrier, nobody verifies its writes (reach_write stays 0).  A single
                                         self-contained kernel is what `ncu` can replay: NVLink byte counters per launch. */

@@ -86,7 +86,7 @@ func fabricProbeCLIFlags() []cli.Flag {
 		},
 		&cli.Float64Flag{
 			Name:        "fabric-probe-link-peak-gbps",
-			Usage:       "Reference figure of the gate in GB/s; 0 = the library's calibrated B200 reference.",
+			Usage:       "Reference figure of the gate in GB/s; 0 = the library's default (nominal NVLink 4, include/cdprobe.h).",
 			EnvVars:     []string{"FABRIC_PROBE_LINK_PEAK_GBPS"},
 			Destination: &fpOpts.linkPeakGBps,
 		},
@@ -200,14 +200,14 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		Bytes:        fpOpts.bytes,                 // FABRIC_PROBE_BYTES, default 1 GiB
 		Mode:         fpOpts.modeID(),              // FABRIC_PROBE_MODE, default sliced
 		MinFraction:  float32(fpOpts.minFraction),  // FABRIC_PROBE_MIN_FRACTION, 0 = library default
-		LinkPeakGBps: float32(fpOpts.linkPeakGBps), // FABRIC_PROBE_LINK_PEAK_GBPS, 0 = calibrated reference
+		LinkPeakGBps: float32(fpOpts.linkPeakGBps), // FABRIC_PROBE_LINK_PEAK_GBPS, 0 = library default reference
 		TimeoutMs:    5000,
 		Flags:        fabricprobe.FlagFabricHandles | fabricprobe.FlagMigAware,
 	}
 	probe, err := fabricprobe.Open(cfg)
 	switch {
 	case errors.Is(err, fabricprobe.ErrUnsupported):
-		// No libcdprobe.so / no CUDA driver / not sm_100: there is no CPU stand-in.  No verdict is
+		// No libcdprobe.so / no CUDA driver / not sm_90: there is no CPU stand-in.  No verdict is
 		// written and check() does not gate on a missing verdict.
 		klog.Infof("fabric probe not supported on this node: %v", err)
 		return p

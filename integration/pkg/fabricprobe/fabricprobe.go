@@ -76,7 +76,7 @@ const (
 )
 
 // ErrUnsupported is returned when the probe cannot run on this node (no libcdprobe.so, no CUDA
-// driver, no sm_100 GPU).  There is no CPU fallback: callers decide whether that gates Ready.
+// driver, no sm_90 GPU).  There is no CPU fallback: callers decide whether that gates Ready.
 var ErrUnsupported = errors.New("fabricprobe: not supported on this node")
 
 // Errors a Run can wrap (errors.Is).  After ErrTimeout, ErrState or ErrCUDA the handle may be
@@ -95,9 +95,9 @@ type Config struct {
 	Ops         uint32
 	TimeoutMs   uint32
 	Flags       uint32
-	MinFraction float32 // FABRIC_PROBE_MIN_FRACTION; 0 = library default (0.90 of the calibrated reference)
-	// FABRIC_PROBE_LINK_PEAK_GBPS; 0 = calibrated reference (what a healthy B200 port delivers to SM-issued
-	// traffic, include/cdprobe.h), > 0 = absolute: the gate is MinFraction x LinkPeakGBps.
+	MinFraction float32 // FABRIC_PROBE_MIN_FRACTION; 0 = library default (0.65 of the reference)
+	// FABRIC_PROBE_LINK_PEAK_GBPS; 0 = the library's default reference (nominal NVLink 4, include/cdprobe.h),
+	// > 0 = absolute: the gate is MinFraction x LinkPeakGBps.
 	LinkPeakGBps float32
 }
 

@@ -1,6 +1,6 @@
-"""cdprobe — B200-native ComputeDomain fabric-validation probe.
+"""cdprobe — H100-native ComputeDomain fabric-validation probe.
 
-The product is ``libcdprobe.so`` (hand-written sm_100a CUDA + a C++ host
+The product is ``libcdprobe.so`` (hand-written sm_90a CUDA + a C++ host
 runtime behind the C ABI in ``include/cdprobe.h``).  This package is the thin
 host-side mirror of the Go shim ``pkg/fabricprobe`` a maintainer would add to
 NVIDIA/k8s-dra-driver-gpu (SURVEY.md §8b, INTEGRATION.md): same names, same

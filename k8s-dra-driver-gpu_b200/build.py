@@ -1,4 +1,4 @@
-"""Builds libcdprobe.so (sm_100a only) in-tree with nvcc.
+"""Builds libcdprobe.so (sm_90a only) in-tree with nvcc.
 
 The library is the product: hand-written CUDA kernels + the C++ host runtime
 behind include/cdprobe.h.  It links the static CUDA runtime and reaches
@@ -18,7 +18,7 @@ LIB = os.path.join(HERE, "libcdprobe.so")
 DAEMON = os.path.join(HERE, "cdprobe-daemon")
 SOURCES = ["probe_kernels.cu", "handle.cc", "plan.cc", "schedule.cc", "rendezvous.cc", "vmm.cc", "topo.cc"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unknown-pragmas",
     "-cudart", "static", "-shared",

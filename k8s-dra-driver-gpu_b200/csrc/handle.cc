@@ -2,7 +2,7 @@
 //
 // Who calls this: the compute-domain-daemon's `run()` owns one handle for the
 // life of the pod (reference: cmd/compute-domain-daemon/main.go:212-347; the
-// cliqueID == "" branch main.go:244-250 is the single-node HGX B200 case) and
+// cliqueID == "" branch main.go:244-250 is the single-node HGX case) and
 // re-runs the probe on every daemon-set change; `check()` (main.go:435-459)
 // only reads the cached verdict.  bench.py drives the same ABI with one process
 // per GPU (world_size > 1).
@@ -93,8 +93,8 @@ struct cdprobe {
   bool event_timing = false;
   uint32_t path = 0;          // 0 TMA bulk, 1 ld/st 128-bit, 2 ld/st 256-bit
   uint32_t warm_mode = 1;     // 0 never, 1 auto (after an idle gap), 2 always
-  uint64_t warm_bytes = 8ull << 20;   // measured: the wake-up costs a fixed ~115 us whatever the byte count
-  double warm_idle_ms = 5.0;  // auto: no penalty after 10 ms idle, full penalty after 50 ms (profiles/r01_cold_start_n2.jsonl)
+  uint64_t warm_bytes = 8ull << 20;   // untimed wake-up prefix per rank
+  double warm_idle_ms = 5.0;  // auto: wake the links when the previous run ended longer ago than this
   double last_run_end_ms = -1.0;
   bool warm_now = false;
   uint32_t debug_skip_rank = 0;  // 1-based local rank whose kernel is NOT launched (fault injection)
@@ -492,9 +492,9 @@ static int open_impl(const cdprobe_config_t* cfg, cdprobe* h) {
     CDP_RT(cudaFree(0));
     cudaDeviceProp prop;
     CDP_RT(cudaGetDeviceProperties(&prop, L.ordinal));
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {
       set_err(std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-              "; libcdprobe carries sm_100a code only");
+              "; libcdprobe carries sm_90a code only");
       return CDPROBE_ERR_UNSUPPORTED;
     }
     L.sm_count = prop.multiProcessorCount;
@@ -640,25 +640,22 @@ static int open_impl(const cdprobe_config_t* cfg, cdprobe* h) {
 // The GB/s an ordered pair must reach for a passing verdict (0: bandwidth is not judged).
 //   link_peak_gbps > 0 : absolute, min_fraction x link_peak_gbps (default fraction 0.65: the round-1 gate
 //                        against nominal 900).
-//   link_peak_gbps == 0: calibrated.  What a healthy B200 port delivers to SM-issued traffic, measured on
-//                        the same box next to the copy engine (tools/linkbench.cu ->
-//                        profiles/r02_linkbench_n2.jsonl), de-rated for the ~8 us a phase spends ramping and
-//                        draining; default fraction 0.90.  Run-to-run spread of a pair is 0.2-0.7 %, spread
-//                        across pairs and boxes ~3 %: 0.90 leaves healthy hardware a 7 % margin, while a
-//                        port that lost 2 of its 18 links (-11 %) fails.
-struct HealthyRates {  // GB/s per direction per GPU, 1 GiB transfers
-  double read_bidi = 672.0, write_bidi = 703.0, read_uni = 785.0, write_uni = 714.7;
-  double phase_overhead_ns = 8000.0;
-};
+//   link_peak_gbps == 0: the nominal NVLink 4 rate of an H100 SXM (450 GB/s per direction, data sheet) for every
+//                        op and schedule, de-rated for the fixed cost of a phase (ramp and drain: 6 us, the
+//                        fixed cost of a read phase measured on an H100 at N = 1); default fraction 0.65.  What
+//                        healthy H100 NVLink delivers to SM-issued traffic has not been measured, so the default
+//                        fraction leaves a wide margin below nominal; set link_peak_gbps / min_fraction to gate
+//                        tighter once a domain's healthy rate is known.
+constexpr double kNominalLinkGbps = 450.0;
+constexpr double kPhaseOverheadNs = 6000.0;
 static float gate_gbps_for(const cdprobe_config_t& cfg, uint32_t n_total, uint64_t bpp, bool is_read) {
+  (void)is_read;
   if (cfg.mode == CDPROBE_MODE_REACH_ONLY || n_total <= 1) return 0.f;
-  if (cfg.link_peak_gbps > 0.f) return (cfg.min_fraction > 0.f ? cfg.min_fraction : 0.65f) * cfg.link_peak_gbps;
-  const HealthyRates hr;
-  const bool uni = (cfg.flags & CDPROBE_FLAG_UNIDIRECTIONAL) != 0;
-  const double rate = is_read ? (uni ? hr.read_uni : hr.read_bidi) : (uni ? hr.write_uni : hr.write_bidi);
+  const float fraction = cfg.min_fraction > 0.f ? cfg.min_fraction : 0.65f;
+  if (cfg.link_peak_gbps > 0.f) return fraction * cfg.link_peak_gbps;
   const double b = (double)bpp;
-  const double expected = b / (b / rate + hr.phase_overhead_ns);  // bytes per ns == GB/s
-  return (float)((cfg.min_fraction > 0.f ? cfg.min_fraction : 0.90f) * expected);
+  const double expected = b / (b / kNominalLinkGbps + kPhaseOverheadNs);  // bytes per ns == GB/s
+  return (float)(fraction * expected);
 }
 static float gate_gbps(const cdprobe* h, bool is_read) { return gate_gbps_for(h->cfg, h->n_total, h->plan.bpp, is_read); }
 

@@ -1,13 +1,14 @@
-// probe_kernels.cu — sm_100a kernels of the ComputeDomain fabric probe.
+// probe_kernels.cu — sm_90a kernels of the ComputeDomain fabric probe.
 //
 // K1 read probe   : every warp streams 8 KiB units of a peer's source slice
 //                   into shared memory with 1-D TMA bulk copies
 //                   (cp.async.bulk.shared::cluster.global + mbarrier complete_tx,
-//                   3 stages in flight per warp) or with 128-/256-bit
-//                   ld.global loads, and folds them into the (S, X) checksum.
+//                   3 stages in flight per warp) or with ld.global.v4 loads
+//                   (16 or 32 contiguous bytes per lane), and folds them into
+//                   the (S, X) checksum.
 // K2 write probe  : every warp generates the write pattern into shared memory
 //                   and pushes it into the peer's landing slot with TMA bulk
-//                   stores (cp.async.bulk.global.shared::cta) or st.global.v4/.v8.
+//                   stores (cp.async.bulk.global.shared::cta) or st.global.v4.
 // K3 barrier      : grid barrier (atomic arrive / release word) whose last
 //                   arriver runs the cross-GPU flag exchange with the ranks the
 //                   phase table names (at most four between rounds, nobody between
@@ -127,20 +128,16 @@ __device__ __forceinline__ void stg_v4(uint4* p, const uint4& v) {
 struct U8 {
   uint32_t r[8];
 };
-// 256-bit global accesses (sm_100+: LDG.E.256 / STG.E.256) — 1 KiB contiguous per warp instruction.
+// 32 contiguous bytes per lane (1 KiB per warp access pair).  sm_90 has no 256-bit global access, so each
+// 32-byte chunk moves as two 128-bit accesses (LDG.E.128 / STG.E.128) issued back to back.
 __device__ __forceinline__ U8 ldg_v8(const void* p) {
-  U8 v;
-  asm volatile("ld.global.L1::no_allocate.v8.u32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v.r[0]), "=r"(v.r[1]), "=r"(v.r[2]), "=r"(v.r[3]), "=r"(v.r[4]), "=r"(v.r[5]), "=r"(v.r[6]),
-                 "=r"(v.r[7])
-               : "l"(p)
-               : "memory");
-  return v;
+  const uint4 a = ldg_stream_v4(reinterpret_cast<const uint4*>(p));
+  const uint4 b = ldg_stream_v4(reinterpret_cast<const uint4*>(p) + 1);
+  return U8{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}};
 }
 __device__ __forceinline__ void stg_v8(void* p, const U8& v) {
-  asm volatile("st.global.L1::no_allocate.v8.u32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v.r[0]),
-               "r"(v.r[1]), "r"(v.r[2]), "r"(v.r[3]), "r"(v.r[4]), "r"(v.r[5]), "r"(v.r[6]), "r"(v.r[7])
-               : "memory");
+  stg_v4(reinterpret_cast<uint4*>(p), make_uint4(v.r[0], v.r[1], v.r[2], v.r[3]));
+  stg_v4(reinterpret_cast<uint4*>(p) + 1, make_uint4(v.r[4], v.r[5], v.r[6], v.r[7]));
 }
 __device__ __forceinline__ uint4 lds_v4(uint32_t addr) {
   uint4 r;
@@ -740,7 +737,7 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
     }
     // The row lives in pinned host memory.  One release at system scope by thread 0 publishes it: the other
     // threads' stores are ordered before it through the CTA barrier (cumulativity), so no per-thread
-    // fence.sys — each one is a round trip over PCIe (round 1 had three of them here: ~5 us per run, 512 -> 507 us at N = 1).
+    // fence.sys — each one is a round trip over PCIe.
     __syncthreads();
     if (t == 0) {
       row->t_first = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_rel[0]);

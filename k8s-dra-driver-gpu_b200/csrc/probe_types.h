@@ -1,4 +1,4 @@
-// probe_types.h — structures shared by the host runtime and the sm_100a kernels.
+// probe_types.h — structures shared by the host runtime and the sm_90a kernels.
 //
 // HBM layout of one rank's probe allocation (one cuMemCreate handle, mapped
 // into every peer's address space with cuMemMap/cuMemSetAccess):

@@ -77,9 +77,9 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
   // with its two ports carrying payload one way only (the classic per-link figure).
   const bool uni = (in.flags & CDPROBE_FLAG_UNIDIRECTIONAL) != 0;
   if (pl.rounds > 0) {
-    // Phase 0: link wake-up.  After >= ~50 ms of idleness the first NVLink transfer of a B200 pays a
-    // fixed ~115 us before data flows (measured, profiles/r01_cold_start_n2.jsonl; with 38 MB per pair
-    // that made the first read of a cold probe report 160 GB/s and failed healthy pairs).  Every rank
+    // Phase 0: link wake-up.  After a stretch of idleness the first NVLink transfer can pay a fixed
+    // start-up cost before data flows, which would make the first timed phase of a cold probe report a
+    // fraction of the link's rate and fail healthy pairs.  Every rank
     // streams a small prefix of its round-0 partner's slice, untimed; the phase always exists (all
     // ranks need the same barrier sequence) and each rank decides its own byte count at launch (0 when
     // its previous run ended less than warm_idle_ms ago).

@@ -31,7 +31,7 @@ class ProbeError(RuntimeError):
 
 
 class ErrUnsupported(ProbeError):
-    """No CUDA driver / no sm_100 GPU: the probe cannot run and nothing stands in for it."""
+    """No CUDA driver / no sm_90 GPU: the probe cannot run and nothing stands in for it."""
 
 
 @dataclasses.dataclass
@@ -43,8 +43,8 @@ class Config:
     timeout_ms: int = 5000
     flags: int = 0
     seed: int = 0
-    min_fraction: float = 0.0  # 0 = library default (0.90 of the calibrated reference; 0.65 of an explicit peak)
-    link_peak_gbps: float = 0.0  # 0 = calibrated reference (include/cdprobe.h); > 0 = absolute GB/s
+    min_fraction: float = 0.0  # 0 = library default (0.65 of the reference)
+    link_peak_gbps: float = 0.0  # 0 = nominal NVLink 4 reference (include/cdprobe.h); > 0 = absolute GB/s
     ctas: int = 0
     world_size: int = 1
     rank: int = 0

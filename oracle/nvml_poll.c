@@ -325,11 +325,13 @@ int cdoracle_nvml_poll(uint32_t n_max, uint32_t flags, cdoracle_nvml_t* out) {
       }
       ret = nv.DeviceGetPciInfo(dev[i], &pci);
       calls++;
-      if (ret != NVML_SUCCESS) {
+      /* NOT_SUPPORTED where the GPU sits behind a virtualised PCI layer: no bus id (as libcdprobe's topology
+       * walk), the rest of the poll still answers */
+      if (ret == NVML_SUCCESS) snprintf(out->pci_bus_id[i], sizeof(out->pci_bus_id[i]), "%s", pci.busId);
+      else if (ret != NVML_ERROR_NOT_SUPPORTED) {
         rc = (int)ret;
         goto done;
       }
-      snprintf(out->pci_bus_id[i], sizeof(out->pci_bus_id[i]), "%s", pci.busId);
     }
   }
   out->enumerate_ms = now_ms() - t0;

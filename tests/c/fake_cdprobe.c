@@ -69,7 +69,7 @@ CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out) {
   g_err[0] = 0;
   if (!cfg || !out || cfg->abi != CDPROBE_ABI_VERSION) return CDPROBE_ERR_ABI;
   if (s && strncmp(s, "unsupported", 11) == 0) {
-    snprintf(g_err, sizeof(g_err), "fake: no sm_100 device");
+    snprintf(g_err, sizeof(g_err), "fake: no sm_90 device");
     return CDPROBE_ERR_UNSUPPORTED;
   }
   if (s && strncmp(s, "openfail", 8) == 0) {

@@ -144,12 +144,12 @@ nvmlReturn_t nvmlDeviceGetMinorNumber(nvmlDevice_t d, unsigned int* m) {
 }
 nvmlReturn_t nvmlDeviceGetName(nvmlDevice_t d, char* buf, unsigned int len) {
   (void)d;
-  snprintf(buf, len, "NVIDIA B200 (fake)");
+  snprintf(buf, len, "NVIDIA H100 80GB HBM3 (fake)");
   return NVML_SUCCESS;
 }
 nvmlReturn_t nvmlDeviceGetMemoryInfo(nvmlDevice_t d, nvmlMemory_t* m) {
   (void)d;
-  m->total = 183359ull << 20;
+  m->total = 81559ull << 20;
   m->free = m->total;
   m->used = 0;
   return NVML_SUCCESS;
@@ -161,13 +161,13 @@ nvmlReturn_t nvmlDeviceGetPciInfo_v3(nvmlDevice_t d, nvmlPciInfo_t* p) {
 }
 nvmlReturn_t nvmlDeviceGetCudaComputeCapability(nvmlDevice_t d, int* major, int* minor) {
   (void)d;
-  *major = 10;
+  *major = 9;
   *minor = 0;
   return NVML_SUCCESS;
 }
 nvmlReturn_t nvmlDeviceGetArchitecture(nvmlDevice_t d, nvmlDeviceArchitecture_t* a) {
   (void)d;
-  *a = 10; /* NVML_DEVICE_ARCH_BLACKWELL */
+  *a = NVML_DEVICE_ARCH_HOPPER;
   return NVML_SUCCESS;
 }
 nvmlReturn_t nvmlDeviceGetBrand(nvmlDevice_t d, nvmlBrandType_t* b) {

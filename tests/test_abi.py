@@ -125,22 +125,22 @@ def test_product_does_not_reference_the_oracle():
 
 def test_gate_arithmetic_without_a_gpu(pkg):
     """cdprobe_gate: the verdict's bandwidth threshold as host arithmetic (include/cdprobe.h: link_peak_gbps).
-    Calibrated reference = healthy SM-path rate de-rated for the ~8 us a phase spends ramping and draining."""
+    Default reference = nominal NVLink 4 rate (450 GB/s per direction) de-rated for the 6 us of a phase's ramp and drain."""
     import pytest
 
     GIB = 1 << 30
     r, w = pkg.gate(pkg.Config(bytes=GIB), 8)                      # the headline config: defaults
     bpp = GIB // 7 // 128 * 128
-    assert r == pytest.approx(0.90 * bpp / (bpp / 672.0 + 8000.0), rel=1e-5)
-    assert w == pytest.approx(0.90 * bpp / (bpp / 703.0 + 8000.0), rel=1e-5)
-    assert 580 < r < 590 and 605 < w < 615                         # N = 8 measures 650-655 / 688-690: ~7-10 % of margin
+    assert r == pytest.approx(0.65 * bpp / (bpp / 450.0 + 6000.0), rel=1e-5)
+    assert w == pytest.approx(0.65 * bpp / (bpp / 450.0 + 6000.0), rel=1e-5)
+    assert 285 < r < 290 and 285 < w < 290
     r1, w1 = pkg.gate(pkg.Config(bytes=GIB, flags=pkg.abi.FLAG_UNIDIRECTIONAL), 8)
-    assert r1 == pytest.approx(0.90 * bpp / (bpp / 785.0 + 8000.0), rel=1e-5) and w1 == pytest.approx(0.90 * bpp / (bpp / 714.7 + 8000.0), rel=1e-5)
+    assert r1 == pytest.approx(0.65 * bpp / (bpp / 450.0 + 6000.0), rel=1e-5) and w1 == pytest.approx(r1, rel=1e-6)
     assert pkg.gate(pkg.Config(bytes=GIB, min_fraction=0.85, link_peak_gbps=900.0), 8) == (pytest.approx(765.0), pytest.approx(765.0))
-    assert pkg.gate(pkg.Config(bytes=GIB, link_peak_gbps=900.0), 8) == (pytest.approx(585.0), pytest.approx(585.0))  # round-1 gate
+    assert pkg.gate(pkg.Config(bytes=GIB, link_peak_gbps=900.0), 8) == (pytest.approx(585.0), pytest.approx(585.0))  # absolute rule
     assert pkg.gate(pkg.Config(bytes=GIB), 1) == (0.0, 0.0)        # loop-back: HBM speed is not a fabric property
     assert pkg.gate(pkg.Config(bytes=GIB, mode=pkg.abi.MODE_REACH_ONLY), 8) == (0.0, 0.0)
-    small = pkg.gate(pkg.Config(bytes=64 << 20), 8)[0]             # small slices: the fixed overhead dominates, the gate follows
+    small = pkg.gate(pkg.Config(bytes=16 << 20), 8)[0]             # small slices: the fixed overhead dominates, the gate follows
     assert small < 0.75 * r
     with pytest.raises(pkg.ProbeError):
         pkg.gate(pkg.Config(bytes=GIB, min_fraction=-1.0), 8)

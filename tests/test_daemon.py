@@ -371,7 +371,7 @@ def test_open_failure_is_not_ready_but_unsupported_does_not_gate(tmp_path, fake_
     d = json.loads(v.read_text())
     assert d["ok"] is False and "cdprobe_open: CUDA call failed" in d["error"] and d["pod_uid"] == "pod-9"
     assert daemon(["check"], {"CLIQUE_ID": "", "FABRIC_PROBE_VERDICT_PATH": str(v), "POD_UID": "pod-9"}).returncode == 1
-    # unsupported (no sm_100 GPU): no verdict at all, check does not gate — and the stale file is gone too
+    # unsupported (no sm_90 GPU): no verdict at all, check does not gate — and the stale file is gone too
     v.write_text(json.dumps({"ok": False, "time_unix": 5, "unreachable_pairs": 3}))
     r = subprocess.run([DAEMON, "run", "--once"], env=fake_env(tmp_path, fake_lib, "unsupported"), capture_output=True, text=True, timeout=60)
     assert r.returncode == 0 and "fabric probe not supported on this node" in r.stderr and not v.exists()

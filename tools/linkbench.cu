@@ -1,9 +1,9 @@
-// linkbench.cu — development microbenchmark (not product): what can one NVLink-5 port of a B200 carry,
-// and which SM-side access shape gets closest?  Round-2 question (VERDICT r01 "weak #2"): SM-issued peer
-// writes sat at 692-716 GB/s one-way on every path; the copy engine was never timed on the same box.
+// linkbench.cu — development microbenchmark (not product): what can one H100 NVLink-4 port carry,
+// and which SM-side access shape gets closest?  The copy engine is timed next to the SM paths on the same
+// buffers, so the SM figures can be read against the same-box ceiling.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo tools/linkbench.cu -o tools/linkbench
-//   tools/linkbench [bytes] [reps]  > profiles/r02_linkbench_n2.jsonl      (needs >= 2 GPUs with P2P)
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo tools/linkbench.cu -o tools/linkbench
+//   tools/linkbench [bytes] [reps]  > linkbench_n2.jsonl      (needs >= 2 GPUs with P2P)
 //
 // Every line of output is one JSON record:
 //   {"name": ..., "dir": "uni"|"bidi", "bytes": per-GPU payload of ONE op, "gbps": [min, median, max], ...}
@@ -128,11 +128,13 @@ __device__ uint64_t read_ldg(const uint8_t* src, uint64_t bytes, uint32_t gthrea
         const uint64_t i = v + (uint64_t)k * nthreads;
 #pragma unroll
         for (int q = 0; q < 8; ++q) r[k][q] = 0;
-        if (i < nvec)
-          asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(r[k][0]), "=r"(r[k][1]), "=r"(r[k][2]), "=r"(r[k][3]), "=r"(r[k][4]), "=r"(r[k][5]),
-                         "=r"(r[k][6]), "=r"(r[k][7])
-                       : "l"(src + i * 32));
+        if (i < nvec)  // 32 contiguous bytes per thread as two 128-bit loads (sm_90 has no 256-bit access)
+          asm volatile(
+              "ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+              "ld.global.L1::no_allocate.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+              : "=r"(r[k][0]), "=r"(r[k][1]), "=r"(r[k][2]), "=r"(r[k][3]), "=r"(r[k][4]), "=r"(r[k][5]),
+                "=r"(r[k][6]), "=r"(r[k][7])
+              : "l"(src + i * 32));
       }
 #pragma unroll
       for (int k = 0; k < UNROLL; ++k)
@@ -167,9 +169,11 @@ __device__ void write_stg(uint8_t* dst, uint64_t bytes, uint32_t gthread, uint32
                          "r"(z ^ 2u), "r"(z ^ 3u)
                          : "memory");
         } else {
-          asm volatile("st.global.L1::no_allocate.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + i * 32), "r"(z),
-                       "r"(z ^ 1u), "r"(z ^ 2u), "r"(z ^ 3u), "r"(z ^ 4u), "r"(z ^ 5u), "r"(z ^ 6u), "r"(z ^ 7u)
-                       : "memory");
+          asm volatile(
+              "st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};\n\t"
+              "st.global.L1::no_allocate.v4.u32 [%0+16], {%5,%6,%7,%8};" ::"l"(dst + i * 32), "r"(z),
+              "r"(z ^ 1u), "r"(z ^ 2u), "r"(z ^ 3u), "r"(z ^ 4u), "r"(z ^ 5u), "r"(z ^ 6u), "r"(z ^ 7u)
+              : "memory");
         }
       }
     }
@@ -351,7 +355,7 @@ Med med(std::vector<double> v) {
 
 // Runs variant v on the GPUs in `who` (issuer -> peer = issuer ^ 1) with the given op mix.
 void run_kernel(const Variant& v, const char* dir, std::vector<int> who, int opA, int opB, double fracA, int flags,
-                uint64_t bytes, int ctas = 148, const char* extra = "") {
+                uint64_t bytes, int ctas = 132, const char* extra = "") {
   std::vector<double> rd, wr, tms;
   const int grid = ctas * v.ctas_per_sm;
   int split = (int)(grid * fracA + 0.5);

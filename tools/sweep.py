@@ -17,7 +17,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--gpus", type=int, default=1)
 ap.add_argument("--bytes", type=int, default=1 << 30)
 ap.add_argument("--mode", default="sliced")
-ap.add_argument("--ctas", default="148,128,96,74,64,48,32")
+ap.add_argument("--ctas", default="132,128,96,66,64,48,32")
 ap.add_argument("--iters", type=int, default=8)
 ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "sweep.jsonl"))
 ap.add_argument("--overlap", default="0")
