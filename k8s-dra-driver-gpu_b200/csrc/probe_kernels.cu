@@ -22,7 +22,8 @@
 // One persistent cooperative kernel per GPU runs every phase of a probe
 // (wake-up, tournament rounds x {write, read + overlapped verify}) so a run
 // costs one launch per GPU; phases are timed with %globaltimer on the issuing
-// GPU (SURVEY.md H7).  The phase table comes from schedule.cc.
+// GPU (SURVEY.md H7).  The phase table comes from schedule.cc.  The single-GPU loop-back table runs as one
+// streamed pass without barriers instead (loopback_pass).
 //
 // The reference has no kernel for this path (SURVEY.md F1/F3); the gate it
 // implements is cmd/compute-domain-daemon/main.go:435-459.
@@ -209,6 +210,49 @@ __device__ __noinline__ void mbar_drain(Ctx& c, int stage) {
   c.parity_bits ^= (1u << stage);
 }
 
+// ---------------------------------------------------------- unit walks -----
+// The 8 KiB units one warp works on.  Strided (the phase walk): units gwarp, gwarp + nwarps, ...  Claimed (the
+// loop-back pass): runs of kClaimUnits consecutive units taken from a counter shared by every warp of the grid,
+// so no warp idles while another still has a backlog.  take() is warp-uniform; once it returns false it keeps
+// doing so.  A claimed walk also stops when the run is aborted.
+// 2 units (16 KiB) per atomic.  The size sets how far the last write lands after the first warps have moved on
+// to reading, and HBM streams slower while reads and writes mix.  On an H100 at a 400 W limit (1 GiB, median of 300
+// probes, two runs each) the kernel took 1017.6-1017.9 us with 2, 1023-1024 us with 4, 1033 us with 8 and
+// 1038 us with 16; with 1 it varied from 1031 to 1054 us.
+constexpr uint32_t kClaimUnits = 2;
+
+template <bool kClaimed>
+struct Walk {
+  uint64_t n_units, next, end;
+  uint32_t stride;
+  unsigned long long* claim;
+
+  __device__ __forceinline__ bool take(const Ctx& c, uint64_t& u) {
+    if (kClaimed && next == end && next < n_units) {
+      unsigned long long b = 0;
+      if (c.lane == 0) {
+        const bool ab = aborted(c);
+        b = atomicAdd(claim, (unsigned long long)kClaimUnits);
+        if (ab) b = n_units;
+      }
+      b = __shfl_sync(0xffffffffu, b, 0);
+      next = b < n_units ? b : n_units;
+      end = next + kClaimUnits < n_units ? next + kClaimUnits : n_units;
+    }
+    if (next >= n_units) return false;
+    u = next;
+    next += kClaimed ? 1u : stride;
+    return true;
+  }
+};
+__device__ __forceinline__ uint64_t units_of(uint64_t bytes) { return (bytes + kUnitBytes - 1) / kUnitBytes; }
+__device__ __forceinline__ Walk<false> strided(uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {
+  return Walk<false>{units_of(bytes), gwarp, 0ull, nwarps, nullptr};
+}
+__device__ __forceinline__ Walk<true> claimed(uint64_t bytes, unsigned long long* counter) {
+  return Walk<true>{units_of(bytes), 0ull, 0ull, 1u, counter};
+}
+
 // ------------------------------------------------------------ checksum -----
 struct Sum {
   uint64_t s0, s1;  // two partial sums (ILP), folded at the end
@@ -230,30 +274,37 @@ __device__ __forceinline__ void issue_load(const Ctx& c, const uint8_t* base, ui
   bulk_load(c.stage_smem + stage * kUnitBytes, base + off, n, bar);
 }
 
-__device__ void job_read_tma(Ctx& c, const uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
-  uint64_t u_issue = gwarp;
+// Every read job returns the number of units it folded in.
+template <bool kClaimed>
+__device__ uint32_t job_read_tma(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
+  uint64_t q[kStages];     // units in flight, oldest first; the oldest sits on stage s (constant indices only)
   uint32_t in_flight = 0;  // loads issued and not yet waited for (warp-uniform)
+  uint32_t it = 0;
   if (c.lane == 0) fence_proxy_async_global();  // data may have been written through the generic proxy
 #pragma unroll
   for (int s = 0; s < kStages; ++s) {
-    if (u_issue < n_units) {
-      if (c.lane == 0) issue_load(c, base, bytes, u_issue, s);
-      u_issue += nwarps;
+    uint64_t u;
+    if (walk.take(c, u)) {
+      if (c.lane == 0) issue_load(c, base, bytes, u, s);
+      q[s] = u;
       ++in_flight;
     }
   }
   int s = 0;
-  for (uint64_t u = gwarp; u < n_units; u += nwarps) {
+  while (in_flight > 0) {
+    const uint64_t u = q[0];
     if (!mbar_wait(c, s)) {
       // aborted: stop issuing, but every load already in flight must land before this CTA can exit
       for (; in_flight > 0; --in_flight) {
         mbar_drain(c, s);
         s = (s + 1 == kStages) ? 0 : s + 1;
       }
-      return;
+      return it;
     }
     --in_flight;
+    ++it;
+#pragma unroll
+    for (int k = 0; k + 1 < kStages; ++k) q[k] = q[k + 1];
     const uint64_t left = bytes - u * kUnitBytes;
     const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
     const uint32_t sbase = c.stage_smem + s * kUnitBytes + c.lane * 16u;
@@ -278,21 +329,26 @@ __device__ void job_read_tma(Ctx& c, const uint8_t* base, uint64_t bytes, uint32
     }
     fold_unit(a, ux, u);
     __syncwarp();
-    if (u_issue < n_units) {
+    uint64_t un;
+    if (walk.take(c, un)) {
       if (c.lane == 0) {
         fence_proxy_async_smem();
-        issue_load(c, base, bytes, u_issue, s);
+        issue_load(c, base, bytes, un, s);
       }
-      u_issue += nwarps;
+#pragma unroll
+      for (int k = 0; k < kStages; ++k)
+        if (k == (int)in_flight) q[k] = un;
       ++in_flight;
     }
     s = (s + 1 == kStages) ? 0 : s + 1;
   }
+  return it;
 }
 
-__device__ void job_read_ldg(Ctx& c, const uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
-  for (uint64_t u = gwarp; u < n_units; u += nwarps) {
+template <bool kClaimed>
+__device__ uint32_t job_read_ldg(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
+  uint32_t it = 0;
+  for (uint64_t u; walk.take(c, u); ++it) {
     const uint64_t left = bytes - u * kUnitBytes;
     const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
     const uint4* gp = reinterpret_cast<const uint4*>(base + u * kUnitBytes) + c.lane;
@@ -317,12 +373,14 @@ __device__ void job_read_ldg(Ctx& c, const uint8_t* base, uint64_t bytes, uint32
     }
     fold_unit(a, ux, u);
   }
+  return it;
 }
 
-__device__ void job_read_ldg256(Ctx& c, const uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
+template <bool kClaimed>
+__device__ uint32_t job_read_ldg256(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
   constexpr int kV = kUnitBytes / 32 / 32;  // 32-byte vectors per lane per full unit
-  for (uint64_t u = gwarp; u < n_units; u += nwarps) {
+  uint32_t it = 0;
+  for (uint64_t u; walk.take(c, u); ++it) {
     const uint64_t left = bytes - u * kUnitBytes;
     const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 5;
     const uint8_t* gp = base + u * kUnitBytes + c.lane * 32u;
@@ -349,15 +407,16 @@ __device__ void job_read_ldg256(Ctx& c, const uint8_t* base, uint64_t bytes, uin
     }
     fold_unit(a, ux, u);
   }
+  return it;
 }
 
 // ---------------------------------------------------------- K2: writing ----
-__device__ void job_write_tma(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, uint64_t salt,
-                              Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
+// Every write job returns the number of units it stored.
+template <bool kClaimed>
+__device__ uint32_t job_write_tma(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
   uint32_t it = 0;
   int s = 0;
-  for (uint64_t u = gwarp; u < n_units; u += nwarps, ++it) {
+  for (uint64_t u; walk.take(c, u); ++it) {
     if (it >= (uint32_t)kStages) {
       if (c.lane == 0) bulk_wait_read<kStages - 1>();  // the store that used stage s has drained it
     }
@@ -388,12 +447,13 @@ __device__ void job_write_tma(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t gw
   }
   if (c.lane == 0) bulk_wait_all();  // stores complete (not just smem drained)
   __syncwarp();
+  return it;
 }
 
-__device__ void job_write_stg(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, uint64_t salt,
-                              Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
-  for (uint64_t u = gwarp; u < n_units; u += nwarps) {
+template <bool kClaimed>
+__device__ uint32_t job_write_stg(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
+  uint32_t it = 0;
+  for (uint64_t u; walk.take(c, u); ++it) {
     const uint64_t left = bytes - u * kUnitBytes;
     const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
     uint4* gp = reinterpret_cast<uint4*>(base + u * kUnitBytes);
@@ -411,12 +471,13 @@ __device__ void job_write_stg(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t gw
     }
     fold_unit(a, ux, u);
   }
+  return it;
 }
 
-__device__ void job_write_stg256(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t gwarp, uint32_t nwarps, uint64_t salt,
-                                 Sum& a) {
-  const uint64_t n_units = (bytes + kUnitBytes - 1) / kUnitBytes;
-  for (uint64_t u = gwarp; u < n_units; u += nwarps) {
+template <bool kClaimed>
+__device__ uint32_t job_write_stg256(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
+  uint32_t it = 0;
+  for (uint64_t u; walk.take(c, u); ++it) {
     const uint64_t left = bytes - u * kUnitBytes;
     const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 5;
     uint8_t* gp = base + u * kUnitBytes;
@@ -441,6 +502,23 @@ __device__ void job_write_stg256(Ctx& c, uint8_t* base, uint64_t bytes, uint32_t
     }
     fold_unit(a, ux, u);
   }
+  return it;
+}
+
+// The data path picked at run time (ProbeParams::use_ldst): 0 TMA bulk copies, 1 16-byte ld/st, 2 32-byte ld/st.
+template <bool kClaimed>
+__device__ __forceinline__ uint32_t read_units(Ctx& c, uint32_t path, const uint8_t* base, uint64_t bytes,
+                                               Walk<kClaimed> walk, Sum& a) {
+  if (path == 2u) return job_read_ldg256(c, base, bytes, walk, a);
+  if (path == 1u) return job_read_ldg(c, base, bytes, walk, a);
+  return job_read_tma(c, base, bytes, walk, a);
+}
+template <bool kClaimed>
+__device__ __forceinline__ uint32_t write_units(Ctx& c, uint32_t path, uint8_t* base, uint64_t bytes,
+                                                Walk<kClaimed> walk, uint64_t salt, Sum& a) {
+  if (path == 2u) return job_write_stg256(c, base, bytes, walk, salt, a);
+  if (path == 1u) return job_write_stg(c, base, bytes, walk, salt, a);
+  return job_write_tma(c, base, bytes, walk, salt, a);
 }
 
 // ---------------------------------------------------------- K3: barrier ----
@@ -503,7 +581,9 @@ __device__ void barrier(const ProbeParams& P, Ctx& c, int b, uint32_t sync, uint
   __syncthreads();
   if (threadIdx.x == 0) {
     Ctrl* ctrl = c.ctrl;
-    const bool ab = aborted(c);
+    // the deadline is checked at every arrival, not only inside long waits: a run whose waits all stay short
+    // would otherwise finish past timeout_ms without the watchdog ever firing
+    const bool ab = check_abort(c);
     if (!ab) {
       const unsigned long long target = P.seq_base + (unsigned long long)b + 1ull;
       // This CTA's accumulator atomics precede the arrive.  Remote stores of a write job were already
@@ -576,6 +656,201 @@ __device__ __forceinline__ uint64_t warp_xor64(uint64_t v) {
   return v;
 }
 
+// The result row, written into pinned host memory by one whole CTA (every thread calls this), then the
+// accumulators are cleared for the next run.  Phase p ran from t_rel[p] to t_arr[p + 1].
+__device__ void write_row(const ProbeParams& P, const Ctx& c, uint64_t t_enter) {
+  Ctrl* ctrl = c.ctrl;
+  ResultRow* row = P.row;
+  const bool ab = aborted(c);
+  const uint32_t t = threadIdx.x;
+  if (t < P.n_phases) {
+    PhaseOut o;
+    o.t_start = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_rel[t]);
+    o.t_arrive = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_arr[t + 1]);
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb) {
+      const Job job = P.phase[t].job[jb];
+      const volatile Acc* acc = &ctrl->acc[t][jb];
+      o.t_end[jb] = acc->t_end;
+      o.sum[jb] = acc->sum;
+      o.xr[jb] = acc->xr;
+      o.exp_sum[jb] = 0;
+      o.exp_xr[jb] = 0;
+      o.verdict[jb] = 0;
+      o.code[jb] = job.kind == kJobNone ? kCodeSkipped : (ab ? kCodeAborted : kCodeOk);
+      if (!ab) {
+        if (job.kind == kJobRead) {
+          const Ctrl* pc = reinterpret_cast<const Ctrl*>(P.base_peer[job.peer]);
+          const uint32_t slice = P.full_mode ? 0u : job.slot;
+          o.exp_sum[jb] = ld_relaxed_sys(&pc->src_sum[slice]);
+          o.exp_xr[jb] = ld_relaxed_sys(&pc->src_xor[slice]);
+        } else if (job.kind == kJobVerify) {
+          o.exp_sum[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].sum);
+          o.exp_xr[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].xr);
+          o.verdict[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].seq);
+        } else if (job.kind == kJobWrite) {
+          o.verdict[jb] = ld_relaxed_sys(&ctrl->verdict[job.peer]);
+        }
+      }
+    }
+    row->ph[t] = o;
+  }
+  __syncthreads();
+  // reset the accumulators for the next run
+  if (t < P.n_phases) {
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb) {
+      Acc* acc = &ctrl->acc[t][jb];
+      acc->sum = 0ull;
+      acc->xr = 0ull;
+      acc->t_end = 0ull;
+    }
+  }
+  // The row lives in pinned host memory.  One release at system scope by thread 0 publishes it: the other
+  // threads' stores are ordered before it through the CTA barrier (cumulativity), so no per-thread
+  // fence.sys — each one is a round trip over PCIe.
+  __syncthreads();
+  if (t == 0) {
+    row->t_first = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_rel[0]);
+    row->t_last = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_arr[P.n_phases]);
+    row->aborted = ab ? 1u : 0u;
+    row->n_phases = P.n_phases;
+    row->t_enter = t_enter;
+    row->t_exit = gtimer();
+    st_release_sys(const_cast<uint64_t*>(&row->done), P.run_seq);
+  }
+}
+
+// ------------------------------------------------- N = 1: one streamed pass ----
+// The loop-back phase table (schedule.cc) is [write diag] [read diag || verify diag] and only the verify depends
+// on the write.  So instead of walking it with barriers in between, every warp claims write units until none are
+// left, then source-read units, then verify units (Walk<true>).  The phase table still names the jobs, the slot
+// and the salt, and the row keeps its two phases.
+__device__ __forceinline__ bool is_loopback(const ProbeParams& P) {
+  if (P.peer_mask != 0u || P.n_phases != 2u) return false;
+  const Job& w = P.phase[0].job[0];
+  const Job& r = P.phase[1].job[0];
+  const Job& v = P.phase[1].job[1];
+  const int8_t me = (int8_t)P.rank;
+  return w.kind == kJobWrite && P.phase[0].job[1].kind == kJobNone && r.kind == kJobRead && v.kind == kJobVerify &&
+         w.peer == me && r.peer == me && v.peer == me && v.writer == P.rank && v.slot == w.slot && v.salt == 0;
+}
+
+// Ordering of the verify after the write (the grid barrier's job in the phase walk):
+//   writer warp:   its stores complete (bulk: cp.async.bulk.wait_group 0 by the issuing lane; ld/st: every lane's
+//                  st.global) -> __syncwarp -> lane 0: fence.proxy.async.global, __threadfence, atomicAdd of the
+//                  units it stored onto lb.written (a gpu-scope release)
+//   verifier warp: lane 0 spins on ld.acquire.gpu of lb.written until it reaches the slot's unit count ->
+//                  __syncwarp -> loads (the bulk path issues fence.proxy.async.global before its first load).
+// Counting units rather than warps means no warp waits for a CTA that has not started: the units are all claimed
+// by CTAs that are running.  The CTA that finishes last (lb.done) publishes the write checksum and the verdict,
+// writes the row and zeroes the counters for the next run.
+__device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint64_t t_enter) {
+  constexpr int kRed = 11;  // per warp: (sum, xor) x 3 jobs, end time x 3 jobs, first issue x 2 jobs
+  static_assert(kWarpsPerCta * (kStages + kRed) * 8 <= kSmemBytes - kWarpsPerCta * kStages * kUnitBytes,
+                "mbarriers + reduction slots fit the tail of the dynamic shared memory");
+  __shared__ bool s_last;
+  __shared__ uint64_t s_t_enter;
+  Ctrl* ctrl = c.ctrl;
+  LoopBack* lb = &ctrl->lb;
+  const Job wj = P.phase[0].job[0];
+  uint8_t* self = P.base_peer[P.rank];
+  uint8_t* slot = self + P.land_off + (uint64_t)wj.slot * P.bpp;
+  const uint8_t* src = self + P.src_off + (P.full_mode ? 0ull : (uint64_t)P.phase[1].job[0].slot * P.bpp);
+  const uint64_t n_units = units_of(P.bpp);
+  if (threadIdx.x == 0) atomicMax(&lb->t_enter_n, ~t_enter);
+
+  Sum a[3] = {};                    // write, source read, verify
+  uint64_t t_end[3] = {0ull, 0ull, 0ull};  // per job: when this warp's last unit was done (0: it did none)
+  uint64_t t_first[2];              // when this warp started the write and the source read
+
+  t_first[0] = gtimer();
+  const uint32_t n_wr = write_units(c, P.use_ldst, slot, P.bpp, claimed(P.bpp, &lb->claim[0].v), wj.salt, a[0]);
+  __syncwarp();
+  if (n_wr) {
+    if (c.lane == 0) {
+      fence_proxy_async_global();
+      __threadfence();
+      atomicAdd(&lb->written.v, (unsigned long long)n_wr);
+    }
+    t_end[0] = gtimer();
+  }
+
+  t_first[1] = gtimer();
+  if (read_units(c, P.use_ldst, src, P.bpp, claimed(P.bpp, &lb->claim[1].v), a[1])) t_end[1] = gtimer();
+
+  bool go = true;
+  if (c.lane == 0) {
+    uint32_t spins = 0;
+    go = !check_abort(c);  // deadline checked at the transition too, as at a barrier arrival
+    while (go && ld_acquire_gpu(&lb->written.v) < n_units) {
+      if ((++spins & 63u) == 0u && check_abort(c)) go = false;
+    }
+  }
+  go = __shfl_sync(0xffffffffu, go, 0);
+  if (go && read_units(c, P.use_ldst, slot, P.bpp, claimed(P.bpp, &lb->claim[2].v), a[2])) t_end[2] = gtimer();
+
+  // CTA reduce -> one set of atomics per CTA
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const uint64_t ws = warp_sum64(a[j].s0 + a[j].s1);
+    const uint64_t wx = warp_xor64(a[j].x);
+    if (c.lane == 0) {
+      red[c.warp * kRed + 2 * j] = ws;
+      red[c.warp * kRed + 2 * j + 1] = wx;
+      red[c.warp * kRed + 6 + j] = t_end[j];
+      if (j < 2) red[c.warp * kRed + 9 + j] = t_first[j];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    Acc* acc[3] = {&ctrl->acc[0][0], &ctrl->acc[1][0], &ctrl->acc[1][1]};
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      uint64_t ts = 0, tx = 0, te = 0, tf = ~0ull;
+#pragma unroll
+      for (int w = 0; w < kWarpsPerCta; ++w) {
+        ts += red[w * kRed + 2 * j];
+        tx ^= red[w * kRed + 2 * j + 1];
+        te = max(te, red[w * kRed + 6 + j]);
+        if (j < 2) tf = min(tf, red[w * kRed + 9 + j]);
+      }
+      atomicAdd(&acc[j]->sum, (unsigned long long)ts);
+      atomicXor(&acc[j]->xr, (unsigned long long)tx);
+      if (te) atomicMax(&acc[j]->t_end, (unsigned long long)te);
+      if (j < 2) atomicMax(&lb->t_first_n[j], ~tf);
+    }
+    __threadfence();
+    const bool last = atomicAdd(&lb->done.v, 1ull) == gridDim.x - 1;
+    if (last) {
+      // every CTA is done: its accumulator atomics precede its arrival on lb.done
+      __threadfence();
+      const volatile LoopBack* vlb = lb;
+      ctrl->t_rel[0] = ~vlb->t_first_n[0];
+      ctrl->t_rel[1] = ~vlb->t_first_n[1];
+      ctrl->t_arr[1] = *reinterpret_cast<volatile unsigned long long*>(&ctrl->acc[0][0].t_end);
+      ctrl->t_arr[2] = gtimer();
+      s_t_enter = ~vlb->t_enter_n;
+      if (!aborted(c)) {
+        publish_writes(P, ctrl, 0);  // the owner of the slot is this GPU
+        publish_verdicts(P, ctrl);
+      }
+      __threadfence();
+    }
+    s_last = last;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  write_row(P, c, s_t_enter);
+  if (threadIdx.x == 0) {
+    for (int j = 0; j < 3; ++j) lb->claim[j].v = 0ull;
+    lb->written.v = 0ull;
+    lb->done.v = 0ull;
+    lb->t_first_n[0] = lb->t_first_n[1] = 0ull;
+    lb->t_enter_n = 0ull;
+  }
+}
+
 }  // namespace
 
 // ------------------------------------------------- the persistent kernel ----
@@ -605,6 +880,11 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
   __syncthreads();
   c.deadline = s_deadline;
 
+  if (is_loopback(P)) {
+    loopback_pass(P, c, red, s_enter);
+    return;
+  }
+
   barrier(P, c, 0, P.peer_mask, 0u, false);
 
   for (uint32_t ph = 0; ph < P.n_phases; ++ph) {
@@ -623,16 +903,10 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
           // untimed link wake-up: stream a prefix of the partner's slice (result ignored)
           const uint8_t* src = pb + P.src_off + (P.full_mode ? 0ull : (uint64_t)job.slot * P.bpp);
           const uint64_t nb = job.salt < P.bpp ? job.salt : P.bpp;
-          if (nb) {
-            if (P.use_ldst == 2u) job_read_ldg256(c, src, nb, gwarp, nwarps, a);
-            else if (P.use_ldst == 1u) job_read_ldg(c, src, nb, gwarp, nwarps, a);
-            else job_read_tma(c, src, nb, gwarp, nwarps, a);
-          }
+          if (nb) read_units(c, P.use_ldst, src, nb, strided(nb, gwarp, nwarps), a);
         } else if (job.kind == kJobRead) {
           const uint8_t* src = pb + P.src_off + (P.full_mode ? 0ull : (uint64_t)job.slot * P.bpp);
-          if (P.use_ldst == 2u) job_read_ldg256(c, src, P.bpp, gwarp, nwarps, a);
-          else if (P.use_ldst == 1u) job_read_ldg(c, src, P.bpp, gwarp, nwarps, a);
-          else job_read_tma(c, src, P.bpp, gwarp, nwarps, a);
+          read_units(c, P.use_ldst, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
         } else if (job.kind == kJobVerify) {
           // the slot's writer signals when its write phase is over (and its checksums are published); where the
           // schedule put no wait between that phase and this one (post_mask), this job does the waiting
@@ -650,15 +924,11 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
           }
           if (go) {
             const uint8_t* src = pb + P.land_off + (uint64_t)job.slot * P.bpp;
-            if (P.use_ldst == 2u) job_read_ldg256(c, src, P.bpp, gwarp, nwarps, a);
-            else if (P.use_ldst == 1u) job_read_ldg(c, src, P.bpp, gwarp, nwarps, a);
-            else job_read_tma(c, src, P.bpp, gwarp, nwarps, a);
+            read_units(c, P.use_ldst, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
           }
         } else {
           uint8_t* dst = pb + P.land_off + (uint64_t)job.slot * P.bpp;
-          if (P.use_ldst == 2u) job_write_stg256(c, dst, P.bpp, gwarp, nwarps, job.salt, a);
-          else if (P.use_ldst == 1u) job_write_stg(c, dst, P.bpp, gwarp, nwarps, job.salt, a);
-          else job_write_tma(c, dst, P.bpp, gwarp, nwarps, job.salt, a);
+          write_units(c, P.use_ldst, dst, P.bpp, strided(P.bpp, gwarp, nwarps), job.salt, a);
         }
       }
       // CTA reduce -> one atomic per CTA into the phase accumulator
@@ -686,69 +956,8 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
     barrier(P, c, (int)ph + 1, phd.sync_mask & P.peer_mask, phd.post_mask & P.peer_mask, ph + 1 == P.n_phases);
   }
 
-  // ---- output: CTA 0 writes the result row into pinned host memory ----------
-  if (blockIdx.x == 0) {
-    Ctrl* ctrl = c.ctrl;
-    ResultRow* row = P.row;
-    const bool ab = aborted(c);
-    const uint32_t t = threadIdx.x;
-    if (t < P.n_phases) {
-      PhaseOut o;
-      o.t_start = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_rel[t]);
-      o.t_arrive = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_arr[t + 1]);
-#pragma unroll
-      for (int jb = 0; jb < 2; ++jb) {
-        const Job job = P.phase[t].job[jb];
-        const volatile Acc* acc = &ctrl->acc[t][jb];
-        o.t_end[jb] = acc->t_end;
-        o.sum[jb] = acc->sum;
-        o.xr[jb] = acc->xr;
-        o.exp_sum[jb] = 0;
-        o.exp_xr[jb] = 0;
-        o.verdict[jb] = 0;
-        o.code[jb] = job.kind == kJobNone ? kCodeSkipped : (ab ? kCodeAborted : kCodeOk);
-        if (!ab) {
-          if (job.kind == kJobRead) {
-            const Ctrl* pc = reinterpret_cast<const Ctrl*>(P.base_peer[job.peer]);
-            const uint32_t slice = P.full_mode ? 0u : job.slot;
-            o.exp_sum[jb] = ld_relaxed_sys(&pc->src_sum[slice]);
-            o.exp_xr[jb] = ld_relaxed_sys(&pc->src_xor[slice]);
-          } else if (job.kind == kJobVerify) {
-            o.exp_sum[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].sum);
-            o.exp_xr[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].xr);
-            o.verdict[jb] = ld_relaxed_sys(&ctrl->wr[job.slot].seq);
-          } else if (job.kind == kJobWrite) {
-            o.verdict[jb] = ld_relaxed_sys(&ctrl->verdict[job.peer]);
-          }
-        }
-      }
-      row->ph[t] = o;
-    }
-    __syncthreads();
-    // reset the accumulators for the next run
-    if (t < P.n_phases) {
-#pragma unroll
-      for (int jb = 0; jb < 2; ++jb) {
-        Acc* acc = &ctrl->acc[t][jb];
-        acc->sum = 0ull;
-        acc->xr = 0ull;
-        acc->t_end = 0ull;
-      }
-    }
-    // The row lives in pinned host memory.  One release at system scope by thread 0 publishes it: the other
-    // threads' stores are ordered before it through the CTA barrier (cumulativity), so no per-thread
-    // fence.sys — each one is a round trip over PCIe.
-    __syncthreads();
-    if (t == 0) {
-      row->t_first = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_rel[0]);
-      row->t_last = *reinterpret_cast<volatile uint64_t*>(&ctrl->t_arr[P.n_phases]);
-      row->aborted = ab ? 1u : 0u;
-      row->n_phases = P.n_phases;
-      row->t_enter = s_enter;
-      row->t_exit = gtimer();
-      st_release_sys(const_cast<uint64_t*>(&row->done), P.run_seq);
-    }
-  }
+  // ---- output: CTA 0 writes the result row ----------------------------------
+  if (blockIdx.x == 0) write_row(P, c, s_enter);
 }
 
 // ------------------------------------------------------- source pattern ----

@@ -53,6 +53,20 @@ struct alignas(32) Acc {
   unsigned long long sum, xr, t_end, pad;
 };
 
+// Work counters of the single-GPU loop-back pass (probe_kernels.cu, loopback_pass).  Every run starts from
+// zero: the CTA that writes the result row clears them again (open and an aborted run zero all of Ctrl from
+// grid_arrive on).  Each hot word has its own 128-byte line.
+struct LoopBack {
+  struct alignas(128) Counter {
+    unsigned long long v;
+  };
+  Counter claim[3];                   // next unclaimed unit of the write, the source read and the verify
+  Counter written;                    // units whose stores have completed
+  Counter done;                       // CTAs that have finished all their work
+  unsigned long long t_first_n[2];    // ~(earliest first issue) of the write and of the source read (0 = none yet)
+  unsigned long long t_enter_n;       // ~(earliest CTA entry)
+};
+
 struct Ctrl {
   // ---- written by peers over NVLink ------------------------------------
   FlagLine flags[kMaxRanks];          // flags[j].v = last barrier target rank j signalled
@@ -68,6 +82,7 @@ struct Ctrl {
   alignas(128) uint64_t t_rel[kMaxPhases + 2];   // release time of barrier b
   uint64_t t_arr[kMaxPhases + 2];                // arrive time of barrier b (all local CTAs done)
   Acc acc[kMaxPhases][2];
+  LoopBack lb;
 };
 static_assert(sizeof(Ctrl) <= kCtrlBytes, "Ctrl must fit its granule");
 

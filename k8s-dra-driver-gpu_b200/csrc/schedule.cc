@@ -124,6 +124,9 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
   // Loop-back (N = 1, or CDPROBE_FLAG_LOCAL_DIAG): same shape as a round — write the diagonal slot,
   // then read the source slice on half the CTAs while the other half verifies what was just written
   // (both jobs are HBM-bound, hence the near-even split).  One barrier fewer than read / write / verify.
+  // At N = 1 the kernel recognises this two-phase table and runs it as one streamed pass in which every
+  // warp claims units of the three jobs in turn (probe_kernels.cu, loopback_pass): the CTA split below is
+  // then unused.  It still applies to CDPROBE_FLAG_LOCAL_DIAG in a multi-rank domain.
   cur_round = -1;
   const bool diag_overlap = pl.diag && (in.flags & CDPROBE_FLAG_OVERLAP_VERIFY) && (ops & CDPROBE_OP_WRITE) &&
                             (ops & CDPROBE_OP_READ);  // not a function of ctas: see `overlap` above
