@@ -232,7 +232,7 @@ static void fill_params(const cdprobe* h, uint32_t li, const Phase* phases, uint
   P->n_ranks = h->n_total;
   P->n_phases = n_phases;
   P->peer_mask = peer_mask;
-  P->use_ldst = h->path;
+  P->path = h->path;
   P->full_mode = h->plan.full ? 1u : 0u;
   for (uint32_t p = 0; p < n_phases; ++p) {
     P->phase[p] = phases[p];

@@ -45,17 +45,16 @@ __device__ __forceinline__ uint64_t gtimer() {
 __device__ __forceinline__ void st_release_sys(uint64_t* p, uint64_t v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) {
-  uint64_t v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ void st_release_gpu(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ unsigned long long ld_acquire_gpu(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+enum Scope { kScopeGpu, kScopeSys };
+// Acquire load of a 64-bit word at gpu scope (a word only this GPU's CTAs write) or sys scope (peers write it).
+template <Scope S>
+__device__ __forceinline__ uint64_t ld_acquire(const void* p) {
+  uint64_t v;
+  if constexpr (S == kScopeSys) asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  else asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
   return v;
 }
 __device__ __forceinline__ uint64_t ld_relaxed_sys(const uint64_t* p) {
@@ -126,20 +125,6 @@ __device__ __forceinline__ void stg_v4(uint4* p, const uint4& v) {
                "r"(v.w)
                : "memory");
 }
-struct U8 {
-  uint32_t r[8];
-};
-// 32 contiguous bytes per lane (1 KiB per warp access pair).  sm_90 has no 256-bit global access, so each
-// 32-byte chunk moves as two 128-bit accesses (LDG.E.128 / STG.E.128) issued back to back.
-__device__ __forceinline__ U8 ldg_v8(const void* p) {
-  const uint4 a = ldg_stream_v4(reinterpret_cast<const uint4*>(p));
-  const uint4 b = ldg_stream_v4(reinterpret_cast<const uint4*>(p) + 1);
-  return U8{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}};
-}
-__device__ __forceinline__ void stg_v8(void* p, const U8& v) {
-  stg_v4(reinterpret_cast<uint4*>(p), make_uint4(v.r[0], v.r[1], v.r[2], v.r[3]));
-  stg_v4(reinterpret_cast<uint4*>(p) + 1, make_uint4(v.r[4], v.r[5], v.r[6], v.r[7]));
-}
 __device__ __forceinline__ uint4 lds_v4(uint32_t addr) {
   uint4 r;
   asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
@@ -172,6 +157,16 @@ __device__ __noinline__ bool check_abort(const Ctx& c) {
     return true;
   }
   return false;
+}
+// Spins until the 64-bit word at p reaches target (acquire loads at scope S), checking abort and the deadline
+// every 64 spins.  Returns whether the target was reached; false means the run is aborted.
+template <Scope S>
+__device__ __forceinline__ bool spin_until(const Ctx& c, const void* p, uint64_t target) {
+  uint32_t spins = 0;
+  while (ld_acquire<S>(p) < target) {
+    if ((++spins & 63u) == 0u && check_abort(c)) return false;
+  }
+  return true;
 }
 
 // Waits for the bulk load armed on `stage`.  Returns false when the run was aborted while waiting —
@@ -246,6 +241,11 @@ struct Walk {
   }
 };
 __device__ __forceinline__ uint64_t units_of(uint64_t bytes) { return (bytes + kUnitBytes - 1) / kUnitBytes; }
+// Bytes in unit u: kUnitBytes, or what is left of the buffer for its last unit.
+__device__ __forceinline__ uint32_t unit_len(uint64_t bytes, uint64_t u) {
+  const uint64_t left = bytes - u * kUnitBytes;
+  return left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes;
+}
 __device__ __forceinline__ Walk<false> strided(uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {
   return Walk<false>{units_of(bytes), gwarp, 0ull, nwarps, nullptr};
 }
@@ -259,6 +259,35 @@ struct Sum {
   uint64_t x;       // position-folded xor
 };
 
+// Adds two consecutive 64-bit words into the sums and into the xor of the unit they belong to.
+__device__ __forceinline__ void add_pair(Sum& a, uint64_t& ux, uint64_t w0, uint64_t w1) {
+  a.s0 += w0;
+  a.s1 += w1;
+  ux ^= w0 ^ w1;
+}
+
+// The write pattern one lane generates: word k of a slot is write_word(salt, k) = z ^ (z >> 32) with
+// z = (salt + k) * kGolden.  A lane stores kLaneBytes of consecutive words per access, and the 32 lanes of a warp
+// store consecutive runs, so after each access a lane moves on by 32 * kLaneBytes / 8 words.
+template <uint32_t kLaneBytes>
+struct Pattern {
+  static constexpr int kV = kLaneBytes / 16;  // 16-byte vectors per access
+  uint64_t z;                                 // (salt + k) * kGolden of the lane's next word k
+  __device__ __forceinline__ Pattern(uint64_t salt, uint64_t u, int lane)
+      : z((salt + u * (kUnitBytes / 8) + 2ull * kV * lane) * kGolden) {}
+  // The lane's next access, added into the checksum.
+  __device__ __forceinline__ void next(uint4 (&v)[kV], Sum& a, uint64_t& ux) {
+#pragma unroll
+    for (int h = 0; h < kV; ++h) {
+      const uint64_t z0 = z + 2ull * h * kGolden, z1 = z0 + kGolden;
+      const uint64_t w0 = z0 ^ (z0 >> 32), w1 = z1 ^ (z1 >> 32);
+      add_pair(a, ux, w0, w1);
+      v[h] = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
+    }
+    z += 64ull * kV * kGolden;
+  }
+};
+
 __device__ __forceinline__ void fold_unit(Sum& a, uint64_t unit_xor, uint64_t unit) {
   const uint32_t g = static_cast<uint32_t>(unit / (kGranuleBytes / kUnitBytes));
   a.x ^= rotl64(unit_xor, fold6(g));
@@ -266,12 +295,10 @@ __device__ __forceinline__ void fold_unit(Sum& a, uint64_t unit_xor, uint64_t un
 
 // ------------------------------------------------------- K1/K4: reading ----
 __device__ __forceinline__ void issue_load(const Ctx& c, const uint8_t* base, uint64_t bytes, uint64_t u, int stage) {
-  const uint64_t off = u * kUnitBytes;
-  const uint64_t left = bytes - off;
-  const uint32_t n = left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes;
+  const uint32_t n = unit_len(bytes, u);
   const uint32_t bar = c.bar_smem + 8u * stage;
   mbar_arrive_expect_tx(bar, n);
-  bulk_load(c.stage_smem + stage * kUnitBytes, base + off, n, bar);
+  bulk_load(c.stage_smem + stage * kUnitBytes, base + u * kUnitBytes, n, bar);
 }
 
 // Every read job returns the number of units it folded in.
@@ -305,26 +332,19 @@ __device__ uint32_t job_read_tma(Ctx& c, const uint8_t* base, uint64_t bytes, Wa
     ++it;
 #pragma unroll
     for (int k = 0; k + 1 < kStages; ++k) q[k] = q[k + 1];
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
+    const uint32_t nvec = unit_len(bytes, u) >> 4;
     const uint32_t sbase = c.stage_smem + s * kUnitBytes + c.lane * 16u;
     uint64_t ux = 0;
     if (nvec == kUnitBytes / 16) {
 #pragma unroll
       for (int k = 0; k < (int)(kUnitBytes / 16 / 32); ++k) {
         const uint4 v = lds_v4(sbase + k * 512u);
-        const uint64_t w0 = pack64(v.x, v.y), w1 = pack64(v.z, v.w);
-        a.s0 += w0;
-        a.s1 += w1;
-        ux ^= w0 ^ w1;
+        add_pair(a, ux, pack64(v.x, v.y), pack64(v.z, v.w));
       }
     } else {
       for (uint32_t i = c.lane; i < nvec; i += 32) {
         const uint4 v = lds_v4(c.stage_smem + s * kUnitBytes + i * 16u);
-        const uint64_t w0 = pack64(v.x, v.y), w1 = pack64(v.z, v.w);
-        a.s0 += w0;
-        a.s1 += w1;
-        ux ^= w0 ^ w1;
+        add_pair(a, ux, pack64(v.x, v.y), pack64(v.z, v.w));
       }
     }
     fold_unit(a, ux, u);
@@ -345,66 +365,31 @@ __device__ uint32_t job_read_tma(Ctx& c, const uint8_t* base, uint64_t bytes, Wa
   return it;
 }
 
-template <bool kClaimed>
-__device__ uint32_t job_read_ldg(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
+// The ld/st data paths: a lane moves kLaneBytes contiguous bytes per access, lane l at kLaneBytes * l +
+// 32 * kLaneBytes * k of the unit.  sm_90 has no 256-bit global access, so 32 bytes move as two 16-byte accesses
+// issued back to back.  A full unit is kLdstVecs 16-byte loads in flight per lane on either path.
+template <uint32_t kLaneBytes, bool kClaimed>
+__device__ uint32_t job_read_ldst(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
+  constexpr int kV = kLaneBytes / 16;  // 16-byte vectors per access; vector i is the (i % kV)-th of access i / kV
+  static_assert(kLdstVecs * 16 * 32 == kUnitBytes, "a warp's loads cover one unit");
   uint32_t it = 0;
   for (uint64_t u; walk.take(c, u); ++it) {
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
-    const uint4* gp = reinterpret_cast<const uint4*>(base + u * kUnitBytes) + c.lane;
+    const uint32_t n = unit_len(bytes, u) / kLaneBytes;  // lane accesses in this unit
+    const uint4* gp = reinterpret_cast<const uint4*>(base + u * kUnitBytes) + kV * c.lane;
     uint4 v[kLdstVecs];
-    if (nvec == kUnitBytes / 16) {
+    if (n == kUnitBytes / kLaneBytes) {
 #pragma unroll
-      for (int k = 0; k < (int)kLdstVecs; ++k) v[k] = ldg_stream_v4(gp + k * 32);
+      for (int i = 0; i < (int)kLdstVecs; ++i) v[i] = ldg_stream_v4(gp + 32 * kV * (i / kV) + i % kV);
     } else {
 #pragma unroll
-      for (int k = 0; k < (int)kLdstVecs; ++k) {
-        v[k] = make_uint4(0u, 0u, 0u, 0u);
-        if (c.lane + k * 32u < nvec) v[k] = ldg_stream_v4(gp + k * 32);
+      for (int i = 0; i < (int)kLdstVecs; ++i) {
+        v[i] = make_uint4(0u, 0u, 0u, 0u);
+        if (c.lane + (i / kV) * 32u < n) v[i] = ldg_stream_v4(gp + 32 * kV * (i / kV) + i % kV);
       }
     }
     uint64_t ux = 0;
 #pragma unroll
-    for (int k = 0; k < (int)kLdstVecs; ++k) {
-      const uint64_t w0 = pack64(v[k].x, v[k].y), w1 = pack64(v[k].z, v[k].w);
-      a.s0 += w0;
-      a.s1 += w1;
-      ux ^= w0 ^ w1;
-    }
-    fold_unit(a, ux, u);
-  }
-  return it;
-}
-
-template <bool kClaimed>
-__device__ uint32_t job_read_ldg256(Ctx& c, const uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, Sum& a) {
-  constexpr int kV = kUnitBytes / 32 / 32;  // 32-byte vectors per lane per full unit
-  uint32_t it = 0;
-  for (uint64_t u; walk.take(c, u); ++it) {
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 5;
-    const uint8_t* gp = base + u * kUnitBytes + c.lane * 32u;
-    U8 v[kV];
-    if (nvec == kUnitBytes / 32) {
-#pragma unroll
-      for (int k = 0; k < kV; ++k) v[k] = ldg_v8(gp + k * 1024);
-    } else {
-#pragma unroll
-      for (int k = 0; k < kV; ++k) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) v[k].r[q] = 0u;
-        if (c.lane + k * 32u < nvec) v[k] = ldg_v8(gp + k * 1024);
-      }
-    }
-    uint64_t ux = 0;
-#pragma unroll
-    for (int k = 0; k < kV; ++k) {
-      const uint64_t w0 = pack64(v[k].r[0], v[k].r[1]), w1 = pack64(v[k].r[2], v[k].r[3]);
-      const uint64_t w2 = pack64(v[k].r[4], v[k].r[5]), w3 = pack64(v[k].r[6], v[k].r[7]);
-      a.s0 += w0 + w2;
-      a.s1 += w1 + w3;
-      ux ^= w0 ^ w1 ^ w2 ^ w3;
-    }
+    for (int i = 0; i < (int)kLdstVecs; ++i) add_pair(a, ux, pack64(v[i].x, v[i].y), pack64(v[i].z, v[i].w));
     fold_unit(a, ux, u);
   }
   return it;
@@ -421,20 +406,14 @@ __device__ uint32_t job_write_tma(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kC
       if (c.lane == 0) bulk_wait_read<kStages - 1>();  // the store that used stage s has drained it
     }
     __syncwarp();
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nb = left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes;
-    const uint32_t nvec = nb >> 4;
+    const uint32_t nb = unit_len(bytes, u);
     const uint32_t sbase = c.stage_smem + s * kUnitBytes;
-    uint64_t z = (salt + u * (kUnitBytes / 8) + 2ull * c.lane) * kGolden;
+    Pattern<16> pat(salt, u, c.lane);
     uint64_t ux = 0;
-    for (uint32_t i = c.lane; i < nvec; i += 32) {
-      const uint64_t z1 = z + kGolden;
-      const uint64_t w0 = z ^ (z >> 32), w1 = z1 ^ (z1 >> 32);
-      z += 64ull * kGolden;
-      sts_v4(sbase + i * 16u, make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
-      a.s0 += w0;
-      a.s1 += w1;
-      ux ^= w0 ^ w1;
+    for (uint32_t i = c.lane; i < nb >> 4; i += 32) {
+      uint4 v[1];
+      pat.next(v, a, ux);
+      sts_v4(sbase + i * 16u, v[0]);
     }
     fold_unit(a, ux, u);
     fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the async proxy
@@ -450,74 +429,41 @@ __device__ uint32_t job_write_tma(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kC
   return it;
 }
 
-template <bool kClaimed>
-__device__ uint32_t job_write_stg(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
+// Stores the write pattern to the addresses job_read_ldst loads from.
+template <uint32_t kLaneBytes, bool kClaimed>
+__device__ uint32_t job_write_ldst(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
+  constexpr int kV = Pattern<kLaneBytes>::kV;
   uint32_t it = 0;
   for (uint64_t u; walk.take(c, u); ++it) {
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 4;
+    const uint32_t n = unit_len(bytes, u) / kLaneBytes;
     uint4* gp = reinterpret_cast<uint4*>(base + u * kUnitBytes);
-    uint64_t z = (salt + u * (kUnitBytes / 8) + 2ull * c.lane) * kGolden;
+    Pattern<kLaneBytes> pat(salt, u, c.lane);
     uint64_t ux = 0;
 #pragma unroll 4
-    for (uint32_t i = c.lane; i < nvec; i += 32) {
-      const uint64_t z1 = z + kGolden;
-      const uint64_t w0 = z ^ (z >> 32), w1 = z1 ^ (z1 >> 32);
-      z += 64ull * kGolden;
-      stg_v4(gp + i, make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
-      a.s0 += w0;
-      a.s1 += w1;
-      ux ^= w0 ^ w1;
-    }
-    fold_unit(a, ux, u);
-  }
-  return it;
-}
-
-template <bool kClaimed>
-__device__ uint32_t job_write_stg256(Ctx& c, uint8_t* base, uint64_t bytes, Walk<kClaimed> walk, uint64_t salt, Sum& a) {
-  uint32_t it = 0;
-  for (uint64_t u; walk.take(c, u); ++it) {
-    const uint64_t left = bytes - u * kUnitBytes;
-    const uint32_t nvec = (left < kUnitBytes ? static_cast<uint32_t>(left) : kUnitBytes) >> 5;
-    uint8_t* gp = base + u * kUnitBytes;
-    uint64_t z = (salt + u * (kUnitBytes / 8) + 4ull * c.lane) * kGolden;
-    uint64_t ux = 0;
-#pragma unroll 4
-    for (uint32_t i = c.lane; i < nvec; i += 32) {
-      U8 v;
-      uint64_t zz = z;
+    for (uint32_t i = c.lane; i < n; i += 32) {
+      uint4 v[kV];
+      pat.next(v, a, ux);
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint64_t w = zz ^ (zz >> 32);
-        zz += kGolden;
-        v.r[2 * q] = (uint32_t)w;
-        v.r[2 * q + 1] = (uint32_t)(w >> 32);
-        if (q & 1) a.s1 += w;
-        else a.s0 += w;
-        ux ^= w;
-      }
-      z += 128ull * kGolden;
-      stg_v8(gp + (uint64_t)i * 32u, v);
+      for (int h = 0; h < kV; ++h) stg_v4(gp + kV * i + h, v[h]);
     }
     fold_unit(a, ux, u);
   }
   return it;
 }
 
-// The data path picked at run time (ProbeParams::use_ldst): 0 TMA bulk copies, 1 16-byte ld/st, 2 32-byte ld/st.
+// The data path picked at run time (ProbeParams::path): 0 TMA bulk copies, 1 16-byte ld/st, 2 32-byte ld/st.
 template <bool kClaimed>
 __device__ __forceinline__ uint32_t read_units(Ctx& c, uint32_t path, const uint8_t* base, uint64_t bytes,
                                                Walk<kClaimed> walk, Sum& a) {
-  if (path == 2u) return job_read_ldg256(c, base, bytes, walk, a);
-  if (path == 1u) return job_read_ldg(c, base, bytes, walk, a);
+  if (path == 2u) return job_read_ldst<32>(c, base, bytes, walk, a);
+  if (path == 1u) return job_read_ldst<16>(c, base, bytes, walk, a);
   return job_read_tma(c, base, bytes, walk, a);
 }
 template <bool kClaimed>
 __device__ __forceinline__ uint32_t write_units(Ctx& c, uint32_t path, uint8_t* base, uint64_t bytes,
                                                 Walk<kClaimed> walk, uint64_t salt, Sum& a) {
-  if (path == 2u) return job_write_stg256(c, base, bytes, walk, salt, a);
-  if (path == 1u) return job_write_stg(c, base, bytes, walk, salt, a);
+  if (path == 2u) return job_write_ldst<32>(c, base, bytes, walk, salt, a);
+  if (path == 1u) return job_write_ldst<16>(c, base, bytes, walk, salt, a);
   return job_write_tma(c, base, bytes, walk, salt, a);
 }
 
@@ -610,13 +556,7 @@ __device__ void barrier(const ProbeParams& P, Ctx& c, int b, uint32_t sync, uint
           bool timed_out = false;
           for (uint32_t j = 0; j < P.n_ranks && !timed_out; ++j) {
             if (j == P.rank || !((sync >> j) & 1u)) continue;
-            uint32_t spins = 0;
-            while (ld_acquire_sys(&ctrl->flags[j].v) < target) {
-              if ((++spins & 63u) == 0u && check_abort(c)) {
-                timed_out = true;
-                break;
-              }
-            }
+            timed_out = !spin_until<kScopeSys>(c, &ctrl->flags[j].v, target);
           }
         } else if (last) {
           publish_verdicts(P, ctrl);  // single-rank domains: the verdict word is local
@@ -635,10 +575,7 @@ __device__ void barrier(const ProbeParams& P, Ctx& c, int b, uint32_t sync, uint
           if (publish_writes(P, ctrl, b - 1)) __threadfence_system();  // loop-back write: the owner is this GPU
         }
       } else {
-        uint32_t spins = 0;
-        while (ld_acquire_gpu(&ctrl->grid_release) < target) {
-          if ((++spins & 63u) == 0u && check_abort(c)) break;
-        }
+        spin_until<kScopeGpu>(c, &ctrl->grid_release, target);
       }
     }
   }
@@ -654,6 +591,35 @@ __device__ __forceinline__ uint64_t warp_xor64(uint64_t v) {
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) v ^= __shfl_xor_sync(0xffffffffu, v, m);
   return v;
+}
+// CTA reduction of the checksums of kJobs jobs, called by every thread: thread 0 adds the CTA's totals into acc[j],
+// one atomicAdd and one atomicXor per job.  The warps' partials take the first 2 * kJobs * kWarpsPerCta slots of
+// red; what a warp stores into later slots before the call, thread 0 may read after it.
+template <int kJobs>
+__device__ __forceinline__ void cta_reduce(const Ctx& c, uint64_t* red, const Sum* a, Acc* const* acc) {
+#pragma unroll
+  for (int j = 0; j < kJobs; ++j) {
+    const uint64_t ws = warp_sum64(a[j].s0 + a[j].s1);
+    const uint64_t wx = warp_xor64(a[j].x);
+    if (c.lane == 0) {
+      red[(c.warp * kJobs + j) * 2] = ws;
+      red[(c.warp * kJobs + j) * 2 + 1] = wx;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int j = 0; j < kJobs; ++j) {
+      uint64_t ts = 0, tx = 0;
+#pragma unroll
+      for (int w = 0; w < kWarpsPerCta; ++w) {
+        ts += red[(w * kJobs + j) * 2];
+        tx ^= red[(w * kJobs + j) * 2 + 1];
+      }
+      atomicAdd(&acc[j]->sum, (unsigned long long)ts);
+      atomicXor(&acc[j]->xr, (unsigned long long)tx);
+    }
+  }
 }
 
 // The result row, written into pinned host memory by one whole CTA (every thread calls this), then the
@@ -746,7 +712,7 @@ __device__ __forceinline__ bool is_loopback(const ProbeParams& P) {
 // by CTAs that are running.  The CTA that finishes last (lb.done) publishes the write checksum and the verdict,
 // writes the row and zeroes the counters for the next run.
 __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint64_t t_enter) {
-  constexpr int kRed = 11;  // per warp: (sum, xor) x 3 jobs, end time x 3 jobs, first issue x 2 jobs
+  constexpr int kRed = 6 + 5;  // per warp: (sum, xor) x 3 jobs (cta_reduce), end time x 3 jobs, first issue x 2 jobs
   static_assert(kWarpsPerCta * (kStages + kRed) * 8 <= kSmemBytes - kWarpsPerCta * kStages * kUnitBytes,
                 "mbarriers + reduction slots fit the tail of the dynamic shared memory");
   __shared__ bool s_last;
@@ -765,7 +731,7 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
   uint64_t t_first[2];              // when this warp started the write and the source read
 
   t_first[0] = gtimer();
-  const uint32_t n_wr = write_units(c, P.use_ldst, slot, P.bpp, claimed(P.bpp, &lb->claim[0].v), wj.salt, a[0]);
+  const uint32_t n_wr = write_units(c, P.path, slot, P.bpp, claimed(P.bpp, &lb->claim[0].v), wj.salt, a[0]);
   __syncwarp();
   if (n_wr) {
     if (c.lane == 0) {
@@ -777,46 +743,33 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
   }
 
   t_first[1] = gtimer();
-  if (read_units(c, P.use_ldst, src, P.bpp, claimed(P.bpp, &lb->claim[1].v), a[1])) t_end[1] = gtimer();
+  if (read_units(c, P.path, src, P.bpp, claimed(P.bpp, &lb->claim[1].v), a[1])) t_end[1] = gtimer();
 
   bool go = true;
-  if (c.lane == 0) {
-    uint32_t spins = 0;
-    go = !check_abort(c);  // deadline checked at the transition too, as at a barrier arrival
-    while (go && ld_acquire_gpu(&lb->written.v) < n_units) {
-      if ((++spins & 63u) == 0u && check_abort(c)) go = false;
-    }
-  }
+  // deadline checked at the transition too, as at a barrier arrival
+  if (c.lane == 0) go = !check_abort(c) && spin_until<kScopeGpu>(c, &lb->written.v, n_units);
   go = __shfl_sync(0xffffffffu, go, 0);
-  if (go && read_units(c, P.use_ldst, slot, P.bpp, claimed(P.bpp, &lb->claim[2].v), a[2])) t_end[2] = gtimer();
+  if (go && read_units(c, P.path, slot, P.bpp, claimed(P.bpp, &lb->claim[2].v), a[2])) t_end[2] = gtimer();
 
-  // CTA reduce -> one set of atomics per CTA
+  // CTA reduce -> one set of atomics per CTA; the times take the slots after the checksums'
+  uint64_t* red_t = red + 6 * kWarpsPerCta;
+  if (c.lane == 0) {
 #pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    const uint64_t ws = warp_sum64(a[j].s0 + a[j].s1);
-    const uint64_t wx = warp_xor64(a[j].x);
-    if (c.lane == 0) {
-      red[c.warp * kRed + 2 * j] = ws;
-      red[c.warp * kRed + 2 * j + 1] = wx;
-      red[c.warp * kRed + 6 + j] = t_end[j];
-      if (j < 2) red[c.warp * kRed + 9 + j] = t_first[j];
-    }
+    for (int j = 0; j < 3; ++j) red_t[c.warp * 5 + j] = t_end[j];
+    red_t[c.warp * 5 + 3] = t_first[0];
+    red_t[c.warp * 5 + 4] = t_first[1];
   }
-  __syncthreads();
+  Acc* const acc[3] = {&ctrl->acc[0][0], &ctrl->acc[1][0], &ctrl->acc[1][1]};
+  cta_reduce<3>(c, red, a, acc);
   if (threadIdx.x == 0) {
-    Acc* acc[3] = {&ctrl->acc[0][0], &ctrl->acc[1][0], &ctrl->acc[1][1]};
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
-      uint64_t ts = 0, tx = 0, te = 0, tf = ~0ull;
+      uint64_t te = 0, tf = ~0ull;
 #pragma unroll
       for (int w = 0; w < kWarpsPerCta; ++w) {
-        ts += red[w * kRed + 2 * j];
-        tx ^= red[w * kRed + 2 * j + 1];
-        te = max(te, red[w * kRed + 6 + j]);
-        if (j < 2) tf = min(tf, red[w * kRed + 9 + j]);
+        te = max(te, red_t[w * 5 + j]);
+        if (j < 2) tf = min(tf, red_t[w * 5 + 3 + j]);
       }
-      atomicAdd(&acc[j]->sum, (unsigned long long)ts);
-      atomicXor(&acc[j]->xr, (unsigned long long)tx);
       if (te) atomicMax(&acc[j]->t_end, (unsigned long long)te);
       if (j < 2) atomicMax(&lb->t_first_n[j], ~tf);
     }
@@ -857,7 +810,7 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
 __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_constant__ ProbeParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
-  uint64_t* red = bars + kWarpsPerCta * kStages;  // [kWarpsPerCta][2]
+  uint64_t* red = bars + kWarpsPerCta * kStages;  // CTA reduction slots: 2 per warp, 11 in the loop-back pass
   __shared__ uint64_t s_deadline;
 
   Ctx c;
@@ -903,52 +856,32 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
           // untimed link wake-up: stream a prefix of the partner's slice (result ignored)
           const uint8_t* src = pb + P.src_off + (P.full_mode ? 0ull : (uint64_t)job.slot * P.bpp);
           const uint64_t nb = job.salt < P.bpp ? job.salt : P.bpp;
-          if (nb) read_units(c, P.use_ldst, src, nb, strided(nb, gwarp, nwarps), a);
+          if (nb) read_units(c, P.path, src, nb, strided(nb, gwarp, nwarps), a);
         } else if (job.kind == kJobRead) {
           const uint8_t* src = pb + P.src_off + (P.full_mode ? 0ull : (uint64_t)job.slot * P.bpp);
-          read_units(c, P.use_ldst, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
+          read_units(c, P.path, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
         } else if (job.kind == kJobVerify) {
           // the slot's writer signals when its write phase is over (and its checksums are published); where the
           // schedule put no wait between that phase and this one (post_mask), this job does the waiting
           bool go = true;
           if (job.salt != 0 && job.writer != P.rank && P.base_peer[job.writer] != nullptr) {
-            if (threadIdx.x == 0) {
-              const uint64_t need = P.seq_base + job.salt + 1ull;
-              uint32_t spins = 0;
-              while (ld_acquire_sys(&c.ctrl->flags[job.writer].v) < need) {
-                if ((++spins & 63u) == 0u && check_abort(c)) break;
-              }
-            }
+            if (threadIdx.x == 0) spin_until<kScopeSys>(c, &c.ctrl->flags[job.writer].v, P.seq_base + job.salt + 1ull);
             __syncthreads();
             go = !aborted(c);
           }
           if (go) {
             const uint8_t* src = pb + P.land_off + (uint64_t)job.slot * P.bpp;
-            read_units(c, P.use_ldst, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
+            read_units(c, P.path, src, P.bpp, strided(P.bpp, gwarp, nwarps), a);
           }
         } else {
           uint8_t* dst = pb + P.land_off + (uint64_t)job.slot * P.bpp;
-          write_units(c, P.use_ldst, dst, P.bpp, strided(P.bpp, gwarp, nwarps), job.salt, a);
+          write_units(c, P.path, dst, P.bpp, strided(P.bpp, gwarp, nwarps), job.salt, a);
         }
       }
       // CTA reduce -> one atomic per CTA into the phase accumulator
-      const uint64_t ws = warp_sum64(a.s0 + a.s1);
-      const uint64_t wx = warp_xor64(a.x);
-      if (c.lane == 0) {
-        red[c.warp * 2 + 0] = ws;
-        red[c.warp * 2 + 1] = wx;
-      }
-      __syncthreads();
+      Acc* const acc = &c.ctrl->acc[ph][jb];
+      cta_reduce<1>(c, red, &a, &acc);
       if (threadIdx.x == 0) {
-        uint64_t ts = 0, tx = 0;
-#pragma unroll
-        for (int w = 0; w < kWarpsPerCta; ++w) {
-          ts += red[w * 2 + 0];
-          tx ^= red[w * 2 + 1];
-        }
-        Acc* acc = &c.ctrl->acc[ph][jb];
-        atomicAdd(&acc->sum, (unsigned long long)ts);
-        atomicXor(&acc->xr, (unsigned long long)tx);
         if (job.kind == kJobWrite) __threadfence_system();  // stores have reached the peer
         atomicMax(&acc->t_end, (unsigned long long)gtimer());
       }

@@ -132,7 +132,8 @@ struct ProbeParams {
   uint64_t src_off, land_off;
   uint32_t rank, n_ranks, n_phases;
   uint32_t peer_mask;              // ranks taking part in the cross-GPU barrier with this rank
-  uint32_t use_ldst;               // 0 TMA bulk, 1 ld/st.global.v4
+  uint32_t path;                   // data path: 0 TMA bulk copies, 1 ld/st.global.v4 with 16 bytes per lane,
+                                   // 2 ld/st.global.v4 with 32 contiguous bytes per lane (two accesses)
   uint32_t full_mode;              // source has a single slice
   Phase phase[kMaxPhases];
 };
