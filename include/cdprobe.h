@@ -238,6 +238,42 @@ typedef struct {
   char clique_error[160];                         /* non-empty: getCliqueID would return this error */
 } cdprobe_topology_t;
 
+/* Diagnosis of one cell (cdprobe_diagnose): its region re-read after a run and compared word for word with the
+ * pattern it must hold.  A word that differs is classified, in this order: */
+#define CDPROBE_DIAG_SAMPLES 16
+#define CDPROBE_DIAG_FLIP 0u       /* none of the below: bits of the expected word flipped */
+#define CDPROBE_DIAG_ZERO 1u       /* word is 0 (never written since open) */
+#define CDPROBE_DIAG_DISPLACED 2u  /* the expected pattern's word from another index */
+#define CDPROBE_DIAG_STALE 3u      /* write cells: this writer's pattern from one of the 8 runs before */
+#define CDPROBE_DIAG_FOREIGN 4u    /* another rank's pattern */
+typedef struct {
+  uint64_t offset;                      /* bytes from the region start */
+  uint64_t expected, observed;
+  uint64_t word;                        /* DISPLACED/STALE/FOREIGN: the pattern index that produced `observed`
+                                           (read cells: index in that rank's source buffer; write cells: in the slot) */
+  uint64_t run_seq;                     /* STALE: the run that wrote it (0 otherwise) */
+  uint32_t kind;                        /* CDPROBE_DIAG_* */
+  int32_t rank;                         /* whose pattern it is (-1 for FLIP/ZERO) */
+} cdprobe_diag_sample_t;
+
+typedef struct {
+  uint32_t abi;
+  uint32_t op;                          /* CDPROBE_OP_READ or CDPROBE_OP_WRITE */
+  uint32_t issuer, target, reader;
+  uint32_t n_samples;                   /* min(CDPROBE_DIAG_SAMPLES, bad_words) */
+  uint64_t run_seq;                     /* the run whose pattern is expected (the last cdprobe_run) */
+  uint64_t region_offset;               /* region start in the target's allocation */
+  uint64_t bytes;                       /* region size (bytes_per_pair) */
+  uint64_t bad_words;                   /* 64-bit words that differ from the pattern */
+  uint64_t bad_granules;                /* 16 KiB granules (from the region start) holding a bad word */
+  uint64_t zero_words;                  /* bad words that read 0 */
+  uint64_t first_bad, last_bad;         /* byte offsets of the first / last bad word; UINT64_MAX / 0 when clean */
+  uint64_t kind_count[5];               /* bad words per CDPROBE_DIAG_* class */
+  uint64_t bit_flips[64];               /* FLIP words only: how often bit b differed */
+  double ms;                            /* CUDA-event time of the diagnosis on the reader's stream */
+  cdprobe_diag_sample_t sample[CDPROBE_DIAG_SAMPLES]; /* the lowest-offset bad words, in offset order */
+} cdprobe_diag_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -260,8 +296,9 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_remap_peer / cdprobe_unmap_peer  emulate NodeUnprepare/NodePrepare churn around a live domain:
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_plan,
- *   cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest: diagnostics, benches, fault injection; the reference has
- *   no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose: diagnostics,
+ *   benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose is optional for callers: a daemon binds it with dlsym and works without it.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -302,6 +339,14 @@ CDPROBE_API int cdprobe_remap_peer(cdprobe_t* h, uint32_t local, uint32_t peer);
 CDPROBE_API int cdprobe_unmap_peer(cdprobe_t* h, uint32_t local, uint32_t peer);
 /* Fault injection: XOR one 64-bit word of local rank's source slice / force a bad write salt. */
 CDPROBE_API int cdprobe_corrupt(cdprobe_t* h, uint32_t local, uint64_t byte_offset, uint64_t xor_mask);
+/* Where and how cell (op, issuer, target) of the last cdprobe_run went wrong: reader (a global rank, local to this
+ * process, that maps the target) re-reads the cell's region — the source slice the issuer reads, or the landing slot
+ * it writes — and compares it on its GPU with the pattern of that run.  reader = the issuer: what crossed the
+ * fabric; reader = the target: what is at rest.  Touches no result, verdict or pattern.  *out is filled with abi, op
+ * and the ranks whatever the return code.  CDPROBE_ERR_ARG: bad op, a rank >= n, a reader that is not local;
+ * CDPROBE_ERR_STATE: sticky handle, no run yet, or the reader does not map the target. */
+CDPROBE_API int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target, uint32_t reader,
+                                 cdprobe_diag_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

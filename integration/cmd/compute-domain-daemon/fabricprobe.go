@@ -29,6 +29,7 @@ import (
 	"fmt"
 	"os"
 	"path/filepath"
+	"sort"
 	"strings"
 	"time"
 
@@ -235,6 +236,9 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		metrics.ObserveFabricProbe(flags.nodeName, d, v.OK, v.UnreachablePairs, v.SlowPairs, res.N, res.GBpsRead, res.GBpsWrite)
 		klog.Infof("fabric probe: verdict ok=%t, %d GPU(s), %d unreachable pair(s), %d slow pair(s), min read %.0f GB/s, min write %.0f GB/s, %.3f ms",
 			v.OK, v.N, v.UnreachablePairs, v.SlowPairs, v.MinGBpsRead, v.MinGBpsWrite, v.ProbeMs)
+		if err == nil && !res.Aborted && !res.Verdict && res.UnreachablePairs > 0 {
+			logDiagnoses(probe, res)
+		}
 		if err != nil && (errors.Is(err, fabricprobe.ErrTimeout) || errors.Is(err, fabricprobe.ErrState) || errors.Is(err, fabricprobe.ErrCUDA)) {
 			// a timed-out pass may leave the handle sticky (Run then only returns ErrState): start afresh
 			probe.Close()
@@ -270,6 +274,73 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		}
 	}()
 	return p
+}
+
+// logDiagnoses logs one line per cell, for at most 8 unreachable cells whose mapping is up (an integrity failure,
+// not a torn-down peer): where the cell's bytes went wrong and how.  Read cells are re-read by the issuer (what
+// crossed the fabric) and by the target (what is at rest); write cells by the target, which holds the landing slot.
+// The same line as the C++ twin's (daemon_main.cc, log_diagnoses).  Libraries without cdprobe_diagnose log nothing.
+func logDiagnoses(probe *fabricprobe.Probe, res fabricprobe.Result) {
+	left := 8
+	for i := 0; i < res.N; i++ {
+		for j := 0; j < res.N; j++ {
+			for _, op := range []uint32{fabricprobe.OpRead, fabricprobe.OpWrite} {
+				c := i*res.N + j
+				if (i == j && res.N > 1) || left == 0 || res.Status[c] != 0 || res.Status[j*res.N+i] != 0 {
+					continue
+				}
+				if (op == fabricprobe.OpRead && res.ReachRead[c]) || (op == fabricprobe.OpWrite && res.ReachWrite[c]) {
+					continue
+				}
+				left--
+				opName, reader := "read", i
+				if op == fabricprobe.OpWrite {
+					opName, reader = "write", j
+				}
+				diag, err := probe.Diagnose(op, i, j, reader)
+				if errors.Is(err, fabricprobe.ErrUnsupported) {
+					return
+				}
+				if err != nil {
+					klog.Warningf("fabric probe diagnosis: %s %d -> %d, reader %d: %v", opName, i, j, reader, err)
+					continue
+				}
+				first := "none"
+				if diag.BadWords != 0 {
+					first = fmt.Sprint(diag.FirstBad)
+				}
+				order := make([]int, 64)
+				for b := range order {
+					order[b] = b
+				}
+				sort.SliceStable(order, func(a, b int) bool { return diag.BitFlips[order[a]] > diag.BitFlips[order[b]] })
+				bits := ""
+				for k := 0; k < 8 && diag.BitFlips[order[k]] != 0; k++ {
+					bits += fmt.Sprintf(" %d:%d", order[k], diag.BitFlips[order[k]])
+				}
+				if bits == "" {
+					bits = " none"
+				}
+				where := ""
+				if op == fabricprobe.OpRead && i != j {
+					if at, err := probe.Diagnose(op, i, j, j); err == nil {
+						switch {
+						case diag.BadWords != 0 && at.BadWords == 0:
+							where = "; in transit"
+						case at.BadWords == diag.BadWords && at.FirstBad == diag.FirstBad && at.LastBad == diag.LastBad:
+							where = "; at rest"
+						default:
+							where = fmt.Sprintf("; the target reads %d bad word(s)", at.BadWords)
+						}
+					}
+				}
+				klog.Infof("fabric probe diagnosis: %s %d -> %d, reader %d: %d/%d bad words, %d bad granule(s), first bad byte %s; "+
+					"flip %d zero %d displaced %d stale %d foreign %d; bits%s%s",
+					opName, i, j, reader, diag.BadWords, diag.Words, diag.BadGranules, first,
+					diag.KindCount[0], diag.KindCount[1], diag.KindCount[2], diag.KindCount[3], diag.KindCount[4], bits, where)
+			}
+		}
+	}
 }
 
 func writeVerdict(res fabricprobe.Result, runErr error, flags *Flags) fabricProbeVerdict {

@@ -29,10 +29,12 @@ typedef void (*close_fn)(cdprobe_t*);
 typedef const char* (*str_fn)(int);
 typedef const char* (*last_fn)(void);
 typedef uint32_t (*abi_fn)(void);
+typedef int (*diag_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
 static str_fn cdp_strerror; static last_fn cdp_last; static abi_fn cdp_abi;
+static diag_fn cdp_diag;  // optional: absent from libraries that predate cdprobe_diagnose
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -44,6 +46,7 @@ static int cdp_load(const char* path) {
   cdp_strerror = (str_fn)dlsym(cdp_dl, "cdprobe_strerror");
   cdp_last = (last_fn)dlsym(cdp_dl, "cdprobe_last_error");
   cdp_abi = (abi_fn)dlsym(cdp_dl, "cdprobe_abi_version");
+  cdp_diag = (diag_fn)dlsym(cdp_dl, "cdprobe_diagnose");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -52,6 +55,10 @@ static int cdp_call_run(cdprobe_t* h, cdprobe_result_t* r) { return cdp_run(h, r
 static void cdp_call_close(cdprobe_t* h) { cdp_close(h); }
 static const char* cdp_call_strerror(int rc) { return cdp_strerror(rc); }
 static const char* cdp_call_last(void) { return cdp_last(); }
+static int cdp_has_diagnose(void) { return cdp_diag != NULL; }
+static int cdp_call_diagnose(cdprobe_t* h, uint32_t op, uint32_t i, uint32_t j, uint32_t reader, cdprobe_diag_t* d) {
+  return cdp_diag(h, op, i, j, reader, d);
+}
 */
 import "C"
 
@@ -121,6 +128,34 @@ type Result struct {
 
 type Probe struct {
 	h *C.cdprobe_t
+}
+
+// DiagKinds names the classes of a bad word, indexed by CDPROBE_DIAG_*.
+var DiagKinds = [5]string{"flip", "zero", "displaced", "stale", "foreign"}
+
+// DiagSample is one bad word (cdprobe_diag_sample_t).
+type DiagSample struct {
+	Offset             uint64 // bytes from the region start
+	Expected, Observed uint64
+	Word               uint64 // displaced/stale/foreign: the pattern index that produced Observed
+	RunSeq             uint64 // stale: the run that wrote it
+	Kind               string // one of DiagKinds
+	Rank               int    // whose pattern it is (-1 for flip/zero)
+}
+
+// Diagnosis is what Diagnose found in one cell's region (cdprobe_diag_t).
+type Diagnosis struct {
+	Op                     string // "read" or "write"
+	Issuer, Target, Reader int
+	RunSeq                 uint64
+	Words                  uint64 // 64-bit words in the region
+	BadWords, BadGranules  uint64
+	ZeroWords              uint64
+	FirstBad, LastBad      uint64    // byte offsets of the first / last bad word (meaningless when BadWords == 0)
+	KindCount              [5]uint64 // indexed like DiagKinds
+	BitFlips               [64]uint64 // flip words only: how often bit b differed
+	Ms                     float64
+	Samples                []DiagSample // the lowest-offset bad words, in offset order
 }
 
 func Open(cfg Config) (*Probe, error) {
@@ -208,6 +243,46 @@ func (p *Probe) Run(ctx context.Context) (Result, error) {
 			err = fmt.Errorf("%w: %v", ErrCUDA, err)
 		}
 		return out, err
+	}
+	return out, nil
+}
+
+// Diagnose re-reads cell (op, issuer, target) of the last Run on reader's GPU and diffs it word for word against
+// the pattern: reader = issuer is what crossed the fabric, reader = target what is at rest.  ErrUnsupported when
+// the library predates cdprobe_diagnose.
+func (p *Probe) Diagnose(op uint32, issuer, target, reader int) (Diagnosis, error) {
+	if C.cdp_has_diagnose() == 0 {
+		return Diagnosis{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_diagnose", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	var d C.cdprobe_diag_t
+	rc := C.cdp_call_diagnose(p.h, C.uint32_t(op), C.uint32_t(issuer), C.uint32_t(target), C.uint32_t(reader), &d)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_diagnose: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return Diagnosis{}, err
+	}
+	out := Diagnosis{Op: "read", Issuer: int(d.issuer), Target: int(d.target), Reader: int(d.reader),
+		RunSeq: uint64(d.run_seq), Words: uint64(d.bytes) / 8, BadWords: uint64(d.bad_words),
+		BadGranules: uint64(d.bad_granules), ZeroWords: uint64(d.zero_words),
+		FirstBad: uint64(d.first_bad), LastBad: uint64(d.last_bad), Ms: float64(d.ms)}
+	if d.op == C.CDPROBE_OP_WRITE {
+		out.Op = "write"
+	}
+	for k := range out.KindCount {
+		out.KindCount[k] = uint64(d.kind_count[k])
+	}
+	for b := range out.BitFlips {
+		out.BitFlips[b] = uint64(d.bit_flips[b])
+	}
+	for k := 0; k < int(d.n_samples); k++ {
+		s := d.sample[k]
+		out.Samples = append(out.Samples, DiagSample{Offset: uint64(s.offset), Expected: uint64(s.expected),
+			Observed: uint64(s.observed), Word: uint64(s.word), RunSeq: uint64(s.run_seq),
+			Kind: DiagKinds[int(s.kind)%len(DiagKinds)], Rank: int(s.rank)})
 	}
 	return out, nil
 }

@@ -49,6 +49,31 @@ type Result struct {
 
 type Probe struct{}
 
+var DiagKinds = [5]string{"flip", "zero", "displaced", "stale", "foreign"}
+
+type DiagSample struct {
+	Offset, Expected, Observed, Word, RunSeq uint64
+	Kind                                     string
+	Rank                                     int
+}
+
+type Diagnosis struct {
+	Op                     string
+	Issuer, Target, Reader int
+	RunSeq                 uint64
+	Words                  uint64
+	BadWords, BadGranules  uint64
+	ZeroWords              uint64
+	FirstBad, LastBad      uint64
+	KindCount              [5]uint64
+	BitFlips               [64]uint64
+	Ms                     float64
+	Samples                []DiagSample
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
-func (*Probe) Close()                              {}
+func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
+	return Diagnosis{}, ErrUnsupported
+}
+func (*Probe) Close() {}

@@ -14,6 +14,7 @@ through ``cdprobe_pkg.load()`` at the repo root, which registers it as
 from . import abi, build, distutil  # noqa: F401
 from .fabricprobe import (  # noqa: F401
     Config,
+    Diagnosis,
     ErrUnsupported,
     Probe,
     ProbeError,
@@ -24,4 +25,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Open", "gate", "plan", "topology"]

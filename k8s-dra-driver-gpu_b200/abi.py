@@ -33,6 +33,10 @@ OPT_WARMUP, OPT_WARMUP_BYTES, OPT_DEBUG_SKIP_RANK = 8, 9, 10
 OPT_CTAS_RANK, OPT_MIN_FRACTION_PPM, OPT_LINK_PEAK_MBPS, OPT_SOLO_RANK, OPT_ALL_RANK_BARRIERS = 11, 12, 13, 14, 15
 OPT_PAIR_BARRIERS = 16
 
+DIAG_SAMPLES = 16
+DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
+DIAG_KIND_NAMES = ("flip", "zero", "displaced", "stale", "foreign")
+
 _N2 = MAX_GPUS * MAX_GPUS
 
 
@@ -185,6 +189,41 @@ class ScheduleT(C.Structure):
     ]
 
 
+class DiagSampleT(C.Structure):
+    _fields_ = [
+        ("offset", C.c_uint64),
+        ("expected", C.c_uint64),
+        ("observed", C.c_uint64),
+        ("word", C.c_uint64),
+        ("run_seq", C.c_uint64),
+        ("kind", C.c_uint32),
+        ("rank", C.c_int32),
+    ]
+
+
+class DiagT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("op", C.c_uint32),
+        ("issuer", C.c_uint32),
+        ("target", C.c_uint32),
+        ("reader", C.c_uint32),
+        ("n_samples", C.c_uint32),
+        ("run_seq", C.c_uint64),
+        ("region_offset", C.c_uint64),
+        ("bytes", C.c_uint64),
+        ("bad_words", C.c_uint64),
+        ("bad_granules", C.c_uint64),
+        ("zero_words", C.c_uint64),
+        ("first_bad", C.c_uint64),
+        ("last_bad", C.c_uint64),
+        ("kind_count", C.c_uint64 * 5),
+        ("bit_flips", C.c_uint64 * 64),
+        ("ms", C.c_double),
+        ("sample", DiagSampleT * DIAG_SAMPLES),
+    ]
+
+
 # Every symbol include/cdprobe.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "cdprobe_abi_version": (C.c_uint32, []),
@@ -201,6 +240,7 @@ SYMBOLS = {
     "cdprobe_corrupt": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64]),
     "cdprobe_ce_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32,
                                   C.c_uint64, C.c_uint32, C.POINTER(C.c_double)]),
+    "cdprobe_diagnose": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(DiagT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

@@ -42,6 +42,7 @@
 #include <time.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <string>
 
 #include "../../include/cdprobe.h"
@@ -191,6 +192,7 @@ struct Lib {
   const char* (*last_error)(void) = nullptr;
   uint32_t (*abi)(void) = nullptr;
   int (*topology)(uint32_t, cdprobe_topology_t*) = nullptr;
+  int (*diagnose)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*) = nullptr;  // optional
 };
 
 bool load_lib(Lib* L, std::string* why) {
@@ -207,6 +209,7 @@ bool load_lib(Lib* L, std::string* why) {
   *(void**)&L->last_error = dlsym(L->dl, "cdprobe_last_error");
   *(void**)&L->abi = dlsym(L->dl, "cdprobe_abi_version");
   *(void**)&L->topology = dlsym(L->dl, "cdprobe_topology");
+  *(void**)&L->diagnose = dlsym(L->dl, "cdprobe_diagnose");
   if (!L->open || !L->run || !L->close || !L->strerror_ || !L->last_error || !L->abi) {
     *why = "libcdprobe.so lacks an ABI symbol";
     return false;
@@ -286,6 +289,55 @@ bool write_verdict(const std::string& path, const cdprobe_result_t* r, int rc, c
     }
   }
   return true;
+}
+
+// One log line per cell, for at most 8 unreachable cells whose mapping is up (an integrity failure, not a torn-down
+// peer): where the cell's bytes went wrong and how (cdprobe_diagnose).  Read cells are re-read by the issuer (what
+// crossed the fabric) and, when the target is a rank of this process, by the target too (what is at rest); write
+// cells by the target, which holds the landing slot.
+void log_diagnoses(const Lib& L, cdprobe_t* h, const cdprobe_result_t& r) {
+  int left = 8;
+  for (uint32_t i = 0; i < r.n; ++i)
+    for (uint32_t j = 0; j < r.n; ++j)
+      for (uint32_t op = CDPROBE_OP_READ; op <= CDPROBE_OP_WRITE; ++op) {
+        const uint32_t c = i * CDPROBE_MAX_GPUS + j;
+        if ((i == j && r.n > 1) || !((r.row_mask >> i) & 1u) || left == 0) continue;
+        if (r.status[c] != 0 || r.status[j * CDPROBE_MAX_GPUS + i] != 0) continue;
+        if ((op == CDPROBE_OP_READ ? r.reach_read[c] : r.reach_write[c]) != 0) continue;
+        --left;
+        const char* opname = op == CDPROBE_OP_READ ? "read" : "write";
+        const uint32_t reader = op == CDPROBE_OP_READ ? i : j;
+        cdprobe_diag_t d;
+        int rc = L.diagnose(h, op, i, j, reader, &d);
+        if (rc != CDPROBE_OK) {
+          fprintf(stderr, "fabric probe diagnosis: %s %u -> %u, reader %u: %s: %s\n", opname, i, j, reader, L.strerror_(rc),
+                  L.last_error());
+          continue;
+        }
+        std::string first = d.bad_words ? std::to_string((unsigned long long)d.first_bad) : "none";
+        std::string bits;
+        int order[64];
+        for (int b = 0; b < 64; ++b) order[b] = b;
+        std::stable_sort(order, order + 64, [&](int a, int b) { return d.bit_flips[a] > d.bit_flips[b]; });
+        for (int k = 0; k < 8 && d.bit_flips[order[k]] != 0; ++k)
+          bits += " " + std::to_string(order[k]) + ":" + std::to_string((unsigned long long)d.bit_flips[order[k]]);
+        if (bits.empty()) bits = " none";
+        std::string where;
+        cdprobe_diag_t t;
+        if (op == CDPROBE_OP_READ && i != j && L.diagnose(h, op, i, j, j, &t) == CDPROBE_OK) {
+          if (d.bad_words != 0 && t.bad_words == 0) where = "; in transit";
+          else if (t.bad_words == d.bad_words && t.first_bad == d.first_bad && t.last_bad == d.last_bad) where = "; at rest";
+          else where = "; the target reads " + std::to_string((unsigned long long)t.bad_words) + " bad word(s)";
+        }
+        fprintf(stderr,
+                "fabric probe diagnosis: %s %u -> %u, reader %u: %llu/%llu bad words, %llu bad granule(s), first bad byte %s; "
+                "flip %llu zero %llu displaced %llu stale %llu foreign %llu; bits%s%s\n",
+                opname, i, j, reader, (unsigned long long)d.bad_words, (unsigned long long)(d.bytes / 8),
+                (unsigned long long)d.bad_granules, first.c_str(), (unsigned long long)d.kind_count[CDPROBE_DIAG_FLIP],
+                (unsigned long long)d.kind_count[CDPROBE_DIAG_ZERO], (unsigned long long)d.kind_count[CDPROBE_DIAG_DISPLACED],
+                (unsigned long long)d.kind_count[CDPROBE_DIAG_STALE], (unsigned long long)d.kind_count[CDPROBE_DIAG_FOREIGN],
+                bits.c_str(), where.c_str());
+      }
 }
 
 // Signals are blocked for the whole of run() and only delivered inside sigsuspend/sigtimedwait-style waits:
@@ -398,6 +450,8 @@ int cmd_run(bool once) {
               (rc == CDPROBE_OK && res.verdict) ? "ok" : "FAILED", res.n, res.unreachable_pairs, res.slow_pairs,
               res.min_gbps_read, res.min_gbps_write, res.probe_ms);
       status = (rc == CDPROBE_OK && res.verdict) ? 0 : 2;
+      if (L.diagnose && rc == CDPROBE_OK && !res.aborted && !res.verdict && res.unreachable_pairs > 0)
+        log_diagnoses(L, h, res);
       if (rc == CDPROBE_ERR_TIMEOUT || rc == CDPROBE_ERR_STATE || rc == CDPROBE_ERR_CUDA) {
         // a timed-out or failed pass may leave the handle sticky (cdprobe_run then only returns ERR_STATE):
         // close it; the next pass opens a fresh one

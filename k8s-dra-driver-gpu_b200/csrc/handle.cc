@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "../../include/cdprobe.h"
+#include "diagnose.h"
 #include "plan.h"
 #include "probe_launch.h"
 #include "probe_types.h"
@@ -68,6 +69,8 @@ struct LocalRank {
   Phase phases[kMaxPhases];
   uint32_t n_phases = 0;
   uint32_t peer_mask = 0;
+  void* diag_scratch = nullptr;  // cdprobe_diagnose: allocated on this rank's first diagnosis
+  size_t diag_scratch_bytes = 0;
 };
 
 }  // namespace cdp
@@ -86,6 +89,7 @@ struct cdprobe {
   bool has_import[kMaxRanks] = {};
   int32_t status[kMaxRanks][kMaxRanks];  // [issuer][owner] mapping status, all ranks
   uint64_t launch_seq = 0;
+  uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
   uint64_t seed = 0;
   uint64_t src_sum[kMaxRanks][kMaxRanks] = {};
   uint64_t src_xor[kMaxRanks][kMaxRanks] = {};
@@ -391,6 +395,7 @@ static void destroy(cdprobe* h) {
     if (L.has_own) h->drv.MemRelease(L.own);
     if (L.own_fd >= 0) ::close(L.own_fd);
     if (L.row) cudaFreeHost(L.row);
+    if (L.diag_scratch) cudaFree(L.diag_scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
     if (L.stream) cudaStreamDestroy(L.stream);
@@ -803,6 +808,7 @@ int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out) {
   }
   const double t0 = cdp::now_ms();
   h->launch_seq++;
+  h->last_run_seq = h->launch_seq;
   out->run_seq = h->launch_seq;
   h->warm_now = h->warm_mode == 2 ||
                 (h->warm_mode == 1 && (h->last_run_end_ms < 0 || t0 - h->last_run_end_ms > h->warm_idle_ms));
@@ -1182,6 +1188,104 @@ int cdprobe_gate(const cdprobe_config_t* cfg, uint32_t n_total, float* gate_read
   if (rc != CDPROBE_OK) return rc;
   *gate_read_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, true);
   *gate_write_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, false);
+  return CDPROBE_OK;
+}
+
+static_assert(CDPROBE_DIAG_FLIP == cdp::kDiagFlip && CDPROBE_DIAG_ZERO == cdp::kDiagZero &&
+                  CDPROBE_DIAG_DISPLACED == cdp::kDiagDisplaced && CDPROBE_DIAG_STALE == cdp::kDiagStale &&
+                  CDPROBE_DIAG_FOREIGN == cdp::kDiagForeign && CDPROBE_DIAG_SAMPLES == cdp::kDiagSamples,
+              "diagnosis classes");
+static_assert(sizeof(cdp::DiagSample) == sizeof(cdprobe_diag_sample_t) &&
+                  offsetof(cdp::DiagSample, run_seq) == offsetof(cdprobe_diag_sample_t, run_seq) &&
+                  offsetof(cdp::DiagSample, rank) == offsetof(cdprobe_diag_sample_t, rank),
+              "the kernel writes samples in the ABI layout");
+
+int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target, uint32_t reader, cdprobe_diag_t* out) {
+  cdp::g_last_error.clear();
+  if (h == nullptr || out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->op = op;
+  out->issuer = issuer;
+  out->target = target;
+  out->reader = reader;
+  out->first_bad = UINT64_MAX;
+  const cdp::Plan& pl = h->plan;
+  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE) {
+    cdp::set_err("op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE");
+    return CDPROBE_ERR_ARG;
+  }
+  if (issuer >= h->n_total || target >= h->n_total || reader >= h->n_total) {
+    cdp::set_err("rank out of range");
+    return CDPROBE_ERR_ARG;
+  }
+  if (issuer == target && !pl.diag) {
+    cdp::set_err("cell (i, i) exists only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG)");
+    return CDPROBE_ERR_ARG;
+  }
+  if (reader < h->first || reader >= h->first + h->n_local) {
+    cdp::set_err("reader is not a rank of this process");
+    return CDPROBE_ERR_ARG;
+  }
+  if (h->sticky) {
+    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
+    return CDPROBE_ERR_STATE;
+  }
+  if (h->last_run_seq == 0) {
+    cdp::set_err("no cdprobe_run yet: there is no pattern to compare with");
+    return CDPROBE_ERR_STATE;
+  }
+  cdp::LocalRank& L = h->lr[reader - h->first];
+  if (h->status[reader][target] != 0 || !L.mapped[target]) {  // never read through a mapping that is down
+    cdp::set_err("reader does not map the target");
+    return CDPROBE_ERR_STATE;
+  }
+  const uint64_t run_seq = h->last_run_seq;
+  out->run_seq = run_seq;
+  out->region_offset = cdp::cell_offset(pl, op, issuer, target);
+  out->bytes = pl.bpp;
+
+  const cdp::DiagSpec s =
+      op == CDPROBE_OP_WRITE
+          ? cdp::diag_write_spec(h->seed, h->n_total, issuer, target, run_seq, pl.bpp / 8)
+          : cdp::diag_read_spec(h->seed, h->n_total, target, (uint64_t)cdp::cell_slice(pl, issuer, target) * (pl.bpp / 8),
+                                pl.bpp / 8, pl.src_bytes / 8);
+
+  CDP_RT(cudaSetDevice(L.ordinal));
+  const size_t need = cdp::diag_scratch_bytes(pl.bpp);
+  if (L.diag_scratch_bytes < need) {
+    if (L.diag_scratch) cudaFree(L.diag_scratch);
+    L.diag_scratch = nullptr;
+    L.diag_scratch_bytes = 0;
+    CDP_RT(cudaMalloc(&L.diag_scratch, need));
+    L.diag_scratch_bytes = need;
+  }
+  const uint8_t* region = reinterpret_cast<const uint8_t*>(L.va[target]) + out->region_offset;
+  cdp::DiagOut d;
+  float ms = 0.f;
+  cudaError_t e = cudaEventRecord(L.ev0, L.stream);
+  if (e == cudaSuccess) e = (cudaError_t)cdp::diag_launch(region, s, L.diag_scratch, L.sm_count, L.stream);
+  if (e == cudaSuccess) e = cudaEventRecord(L.ev1, L.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&d, L.diag_scratch, sizeof(d), cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L.ev0, L.ev1);
+  if (e != cudaSuccess) {
+    h->sticky = true;  // a failed kernel leaves the context unusable
+    return cdp::fail_cuda("cdprobe_diagnose", e);
+  }
+  out->ms = ms;
+  out->bad_words = d.bad_words;
+  out->bad_granules = d.bad_granules;
+  out->zero_words = d.kind_count[cdp::kDiagZero];
+  if (d.bad_words) {
+    out->first_bad = ~d.first_bad_n;
+    out->last_bad = d.last_bad;
+  }
+  for (int k = 0; k < cdp::kDiagKinds; ++k) out->kind_count[k] = d.kind_count[k];
+  for (int b = 0; b < 64; ++b) out->bit_flips[b] = d.bit_flips[b];
+  out->n_samples = d.bad_words < (uint64_t)CDPROBE_DIAG_SAMPLES ? (uint32_t)d.bad_words : (uint32_t)CDPROBE_DIAG_SAMPLES;
+  memcpy(out->sample, d.sample, sizeof(out->sample[0]) * out->n_samples);
   return CDPROBE_OK;
 }
 

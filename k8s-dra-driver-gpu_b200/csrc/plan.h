@@ -29,6 +29,15 @@ struct Plan {
 int partner_of(uint32_t n, uint32_t r, uint32_t i);
 // Slot of issuer i inside owner j's buffers (its index among j's peers).
 inline uint32_t slot_of(uint32_t i, uint32_t j) { return i < j ? i : i - 1; }
+// Where cell (issuer i, target j) lives in j's allocation: the landing slot i writes and the source slice i reads
+// (in full mode every reader reads slice 0).  The loop-back cell i == j uses the diagonal slot.
+inline uint32_t cell_slot(const Plan& pl, uint32_t i, uint32_t j) { return i == j ? pl.diag_slot : slot_of(i, j); }
+inline uint32_t cell_slice(const Plan& pl, uint32_t i, uint32_t j) { return pl.full ? 0u : cell_slot(pl, i, j); }
+// Byte offset of the cell's region (bpp bytes) from the start of j's allocation.
+inline uint64_t cell_offset(const Plan& pl, uint32_t op, uint32_t i, uint32_t j) {
+  return op == CDPROBE_OP_WRITE ? pl.land_off + (uint64_t)cell_slot(pl, i, j) * pl.bpp
+                                : pl.src_off + (uint64_t)cell_slice(pl, i, j) * pl.bpp;
+}
 // Returns CDPROBE_OK or CDPROBE_ERR_ARG.
 int make_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, Plan* out);
 

@@ -172,4 +172,134 @@ CDP_HD inline uint64_t rotl64(uint64_t x, uint32_t r) {
 //   X = xor over granules g of rotl64(xor of the words of granule g, fold6(g)),
 //       granule = 16 KiB = 2048 words, g counted from the slice start.
 
+// ---- inverses of the pattern functions (cdprobe_diagnose) -------------------------------------------------
+// Both patterns are bijections of a 64-bit word, so an observed word names the (rank, index) or (salt + index)
+// that produced it.  The odd multipliers have these inverses mod 2^64.
+constexpr uint64_t kInvGolden = 0xF1DE83E19937733Dull;
+constexpr uint64_t kInvMix1 = 0x96DE1B173F119089ull;  // of 0xBF58476D1CE4E5B9
+constexpr uint64_t kInvMix2 = 0x319642B2D24D8EC3ull;  // of 0x94D049BB133111EB
+static_assert(kGolden * kInvGolden == 1ull && 0xBF58476D1CE4E5B9ull * kInvMix1 == 1ull &&
+                  0x94D049BB133111EBull * kInvMix2 == 1ull, "modular inverses");
+CDP_HD inline uint64_t unsplitmix64(uint64_t z) {
+  z = z ^ (z >> 31) ^ (z >> 62);
+  z *= kInvMix2;
+  z = z ^ (z >> 27) ^ (z >> 54);
+  z *= kInvMix1;
+  z = z ^ (z >> 30) ^ (z >> 60);
+  return z - kGolden;
+}
+// salt + k of a write-pattern word: y = z ^ (z >> 32) keeps the high half of z, so z = y ^ (y >> 32).
+CDP_HD inline uint64_t unwrite_word(uint64_t y) { return (y ^ (y >> 32)) * kInvGolden; }
+
+// Classes of a word that differs from the pattern (include/cdprobe.h CDPROBE_DIAG_*, same values).
+enum DiagKind : uint32_t { kDiagFlip = 0, kDiagZero = 1, kDiagDisplaced = 2, kDiagStale = 3, kDiagForeign = 4 };
+constexpr int kDiagKinds = 5;
+constexpr int kDiagMaxCand = 1 + 8 + kMaxRanks;  // write cells: current salt, 8 earlier runs, every other writer
+
+struct DiagCand {       // a write salt the cell's slot may hold words of
+  uint64_t salt;
+  uint64_t run_seq;     // the run that writes with it
+  uint32_t kind;        // kDiagDisplaced (this writer, this run), kDiagStale or kDiagForeign
+  int32_t rank;         // the writer
+};
+
+// What one cell's region must hold.  Word k of the region is
+//   read cells:  src_word(seed, target, first_word + k)
+//   write cells: write_word(cand[0].salt, k)   (cand[0] is the current salt)
+struct DiagSpec {
+  uint64_t seed;
+  uint64_t first_word;  // read: index of the region's word 0 in the target's source pattern
+  uint64_t n_words;     // words in the region
+  uint64_t src_words;   // read: words in one rank's source buffer
+  uint32_t is_write;
+  uint32_t target;
+  uint32_t n_ranks;
+  uint32_t n_cand;      // write: entries of cand
+  DiagCand cand[kDiagMaxCand];
+};
+
+struct DiagClass {
+  uint32_t kind;        // DiagKind
+  int32_t rank;         // whose pattern the word is (-1 for FLIP / ZERO)
+  uint64_t word;        // DISPLACED / STALE / FOREIGN: the pattern index that produced it
+  uint64_t run_seq;     // STALE: the run that wrote it
+};
+
+constexpr uint64_t kDiagStaleRuns = 8;  // earlier runs of the same writer a STALE word is traced back to
+
+// Read cell: the region is words [first_word, first_word + n_words) of target's source buffer of src_words words.
+inline DiagSpec diag_read_spec(uint64_t seed, uint32_t n_ranks, uint32_t target, uint64_t first_word, uint64_t n_words,
+                               uint64_t src_words) {
+  DiagSpec s = {};
+  s.seed = seed;
+  s.n_ranks = n_ranks;
+  s.target = target;
+  s.first_word = first_word;
+  s.n_words = n_words;
+  s.src_words = src_words;
+  return s;
+}
+// Write cell: the n_words slot issuer fills in target in run run_seq.  Candidates, in the order they are tried:
+// this run's salt (DISPLACED), the issuer's salts of the kDiagStaleRuns runs before (STALE), and every other
+// rank's salt into the target in this run (FOREIGN).
+inline DiagSpec diag_write_spec(uint64_t seed, uint32_t n_ranks, uint32_t issuer, uint32_t target, uint64_t run_seq,
+                                uint64_t n_words) {
+  DiagSpec s = {};
+  s.seed = seed;
+  s.n_ranks = n_ranks;
+  s.target = target;
+  s.n_words = n_words;
+  s.is_write = 1;
+  auto cand = [&](uint32_t writer, uint64_t seq, uint32_t kind) {
+    DiagCand& c = s.cand[s.n_cand++];
+    c.salt = write_salt(seed, writer, target, seq);
+    c.run_seq = seq;
+    c.kind = kind;
+    c.rank = (int32_t)writer;
+  };
+  cand(issuer, run_seq, kDiagDisplaced);
+  for (uint64_t d = 1; d <= kDiagStaleRuns && d < run_seq; ++d) cand(issuer, run_seq - d, kDiagStale);
+  for (uint32_t r = 0; r < n_ranks && r < (uint32_t)kMaxRanks; ++r)
+    if (r != issuer) cand(r, run_seq, kDiagForeign);
+  return s;
+}
+
+CDP_HD inline uint64_t diag_expected(const DiagSpec& s, uint64_t k) {
+  return s.is_write ? write_word(s.cand[0].salt, k) : src_word(s.seed, s.target, s.first_word + k);
+}
+
+// Class of an observed word that differs from the expected one, in this order: ZERO; a word of some rank's
+// source pattern (read cells) or of a candidate write salt (write cells) whose index lies inside that buffer;
+// anything else is a FLIP of the expected word.
+CDP_HD inline DiagClass diag_classify(const DiagSpec& s, uint64_t observed) {
+  DiagClass c = {kDiagFlip, -1, 0, 0};
+  if (observed == 0) {
+    c.kind = kDiagZero;
+    return c;
+  }
+  if (!s.is_write) {
+    const uint64_t x = unsplitmix64(observed) ^ s.seed;  // = rank << 56 ^ k
+    const uint32_t r = (uint32_t)(x >> 56);
+    const uint64_t k = x & ((1ull << 56) - 1);
+    if (r < s.n_ranks && k < s.src_words) {
+      c.kind = r == s.target ? kDiagDisplaced : kDiagForeign;
+      c.rank = (int32_t)r;
+      c.word = k;
+    }
+    return c;
+  }
+  const uint64_t z = unwrite_word(observed);  // = salt + k
+  for (uint32_t i = 0; i < s.n_cand; ++i) {
+    const uint64_t k = z - s.cand[i].salt;
+    if (k < s.n_words) {
+      c.kind = s.cand[i].kind;
+      c.rank = s.cand[i].rank;
+      c.word = k;
+      c.run_seq = c.kind == kDiagStale ? s.cand[i].run_seq : 0;
+      return c;
+    }
+  }
+  return c;
+}
+
 }  // namespace cdp

@@ -86,13 +86,13 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
     cur_round = 0;
     const int p0 = pl.partner[0][g];
     const bool ok0 = p0 >= 0 && pair_ok(g, (uint32_t)p0);
-    push(ok0 ? kJobWarm : kJobNone, ok0 ? p0 : (int)g, ok0 ? slot_of(g, (uint32_t)p0) : 0, 0);
+    push(ok0 ? kJobWarm : kJobNone, ok0 ? p0 : (int)g, ok0 ? cell_slot(pl, g, (uint32_t)p0) : 0, 0);
   }
   for (uint32_t r = 0; r < pl.rounds; ++r) {
     cur_round = (int)r;
     const int p = pl.partner[r][g];
     const bool ok = p >= 0 && pair_ok(g, (uint32_t)p);
-    const uint32_t slot = ok ? slot_of(g, (uint32_t)p) : 0;
+    const uint32_t slot = ok ? cell_slot(pl, g, (uint32_t)p) : 0;
     for (int half = 0; half < (uni ? 2 : 1); ++half) {
       const bool i_active = !uni || ((half == 0) == ((int)g < p));
       const bool p_active = !uni || !i_active;
@@ -101,14 +101,14 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
       // spare CTAs during the read phase of the SAME round, so no verify is left over at the end
       if (ops & CDPROBE_OP_WRITE) {
         Phase& ph = push(mine ? kJobWrite : kJobNone, mine ? p : (int)g, slot, 0);
-        if (p >= 0 && p_active) write_phase_into[slot_of((uint32_t)p, g)] = n - 1;
+        if (p >= 0 && p_active) write_phase_into[cell_slot(pl, (uint32_t)p, g)] = n - 1;
         if (!overflow) is_write_phase[n - 1] = true;
         if (overlap) {
           attach(ph);
           if (p >= 0 && p_active) {  // what the partner stores into my landing area during this phase
             pend.have = true;
             pend.ok = ok;
-            pend.slot = slot_of((uint32_t)p, g);
+            pend.slot = cell_slot(pl, (uint32_t)p, g);
             pend.writer = (uint32_t)p;
             pend.wphase = n - 1;
           }
@@ -131,9 +131,9 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
   const bool diag_overlap = pl.diag && (in.flags & CDPROBE_FLAG_OVERLAP_VERIFY) && (ops & CDPROBE_OP_WRITE) &&
                             (ops & CDPROBE_OP_READ);  // not a function of ctas: see `overlap` above
   if (pl.diag) {
-    if (ops & CDPROBE_OP_WRITE) push(kJobWrite, (int)g, pl.diag_slot, 0);
+    if (ops & CDPROBE_OP_WRITE) push(kJobWrite, (int)g, cell_slot(pl, g, g), 0);
     if (ops & CDPROBE_OP_READ) {
-      Phase& ph = push(kJobRead, (int)g, pl.diag_slot, 0);
+      Phase& ph = push(kJobRead, (int)g, cell_slot(pl, g, g), 0);
       if (diag_overlap) {
         // measured at N = 1 with an even split: the verify half (reading lines that were just written)
         // runs ~5 % slower than the source read, so it gets 33/64 of the CTAs (76 of 148)
@@ -142,9 +142,9 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
           if (half < 1) half = 1;
           if (half >= ctas) half = ctas - 1;
           ph.job[0].nctas = (uint16_t)(ctas - half);
-          set_job(ph.job[1], kJobVerify, (int)g, pl.diag_slot, g, ctas - half, half);
+          set_job(ph.job[1], kJobVerify, (int)g, cell_slot(pl, g, g), g, ctas - half, half);
         } else {
-          set_job(ph.job[1], kJobVerify, (int)g, pl.diag_slot, g, 0, 1);  // one CTA: read, then verify
+          set_job(ph.job[1], kJobVerify, (int)g, cell_slot(pl, g, g), g, 0, 1);  // one CTA: read, then verify
         }
       }
     }
@@ -160,7 +160,7 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
         if (ph.job[0].kind == kJobVerify && pend.writer != g) ph.job[0].salt = pend.wphase + 1;
       }
       pend.have = false;
-      if (pl.diag && !diag_overlap) push(kJobVerify, (int)g, pl.diag_slot, g);
+      if (pl.diag && !diag_overlap) push(kJobVerify, (int)g, cell_slot(pl, g, g), g);
     } else {
       for (uint32_t s = 0; s < pl.n_slots; ++s) {
         uint32_t writer;

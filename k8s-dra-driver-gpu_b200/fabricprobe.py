@@ -155,6 +155,49 @@ class Result:
         )
 
 
+@dataclasses.dataclass
+class Diagnosis:
+    """What cdprobe_diagnose found in one cell's region: exact counts, the classes of the bad words, the bit-flip
+    histogram of FLIP words and the lowest-offset bad words (dicts with kind names)."""
+    op: str                   # "read" or "write"
+    issuer: int
+    target: int
+    reader: int
+    run_seq: int
+    region_offset: int
+    bytes: int
+    bad_words: int
+    bad_granules: int
+    zero_words: int
+    first_bad: Optional[int]  # byte offset; None when the region is clean
+    last_bad: Optional[int]
+    kinds: dict               # {"flip": n, "zero": n, "displaced": n, "stale": n, "foreign": n}
+    bit_flips: List[int]      # [64]
+    ms: float
+    samples: List[dict]
+    raw: abi.DiagT = dataclasses.field(repr=False, default=None)
+
+    @property
+    def words(self) -> int:
+        return self.bytes // 8
+
+    @staticmethod
+    def from_c(d: abi.DiagT) -> "Diagnosis":
+        clean = d.bad_words == 0
+        return Diagnosis(
+            op={abi.OP_READ: "read", abi.OP_WRITE: "write"}.get(d.op, str(d.op)),
+            issuer=d.issuer, target=d.target, reader=d.reader, run_seq=d.run_seq,
+            region_offset=d.region_offset, bytes=d.bytes, bad_words=d.bad_words, bad_granules=d.bad_granules,
+            zero_words=d.zero_words, first_bad=None if clean else d.first_bad, last_bad=None if clean else d.last_bad,
+            kinds={name: d.kind_count[k] for k, name in enumerate(abi.DIAG_KIND_NAMES)},
+            bit_flips=list(d.bit_flips), ms=d.ms,
+            samples=[{"offset": s.offset, "expected": s.expected, "observed": s.observed, "word": s.word,
+                      "run_seq": s.run_seq, "kind": abi.DIAG_KIND_NAMES[s.kind], "rank": s.rank}
+                     for s in d.sample[:d.n_samples]],
+            raw=d,
+        )
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -243,6 +286,22 @@ class Probe:
         rc = self._lib.cdprobe_corrupt(self._h, local, byte_offset, xor_mask)
         if rc != abi.OK:
             _raise(self._lib, rc, "cdprobe_corrupt")
+
+    def Diagnose(self, op, issuer: int, target: int, reader: Optional[int] = None) -> Diagnosis:
+        """Go: (*Probe).Diagnose.  Re-reads cell (op, issuer, target) of the last Run on `reader`'s GPU (default: the
+        issuer, i.e. through the fabric; the target reads it at rest) and diffs it against the pattern.
+        op: abi.OP_READ / abi.OP_WRITE or "read" / "write"."""
+        op = {"read": abi.OP_READ, "write": abi.OP_WRITE}.get(op, op)
+        rc, d = self.diagnose_raw(op, issuer, target, issuer if reader is None else reader)
+        if rc != abi.OK:
+            _raise(self._lib, rc, "cdprobe_diagnose")
+        return Diagnosis.from_c(d)
+
+    def diagnose_raw(self, op: int, issuer: int, target: int, reader: int):
+        """The bare ABI call: (return code, abi.DiagT as the library left it)."""
+        d = abi.DiagT()
+        rc = self._lib.cdprobe_diagnose(self._h, op, issuer, target, reader, C.byref(d))
+        return rc, d
 
     def Close(self) -> None:
         if self._h:
