@@ -274,6 +274,27 @@ typedef struct {
   cdprobe_diag_sample_t sample[CDPROBE_DIAG_SAMPLES]; /* the lowest-offset bad words, in offset order */
 } cdprobe_diag_t;
 
+/* Dependent-load latency per ordered pair (cdprobe_latency): issuer i's GPU chases `hops` 8-byte loads through its
+ * own mapping of target j's source slice, each address taken from the word the load before returned (DESIGN §5c).
+ * Matrices are row-major [issuer * CDPROBE_MAX_GPUS + target], like cdprobe_result_t. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t hops, reps;                  /* as applied: 0 -> 1024 and 8; hops in [1, 1 << 20], reps in [1, 64] */
+  uint32_t reserved;
+  uint64_t region_bytes;                /* bytes one chase ranges over (bytes_per_pair) */
+  uint8_t measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];  /* 1: the cell was chased */
+  int32_t status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 0 ok; CDPROBE_ERR_INTEGRITY: the digest differs from the
+                                                             pattern's; CDPROBE_ERR_TIMEOUT: the chase passed timeout_ms;
+                                                             else the mapping's status as in cdprobe_result_t */
+  float ns_min[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];      /* ns per hop over the timed reps (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];
+  uint64_t digest[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* xor of every loaded word, warm-up rep included */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_latency_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -296,9 +317,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_remap_peer / cdprobe_unmap_peer  emulate NodeUnprepare/NodePrepare churn around a live domain:
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_plan,
- *   cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose: diagnostics,
- *   benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
- *   cdprobe_diagnose is optional for callers: a daemon binds it with dlsym and works without it.
+ *   cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
+ *   cdprobe_latency: diagnostics, benches, fault injection; the reference has no counterpart (it has no probe,
+ *   SURVEY.md F1).
+ *   cdprobe_diagnose and cdprobe_latency are optional for callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -347,6 +369,15 @@ CDPROBE_API int cdprobe_corrupt(cdprobe_t* h, uint32_t local, uint64_t byte_offs
  * CDPROBE_ERR_STATE: sticky handle, no run yet, or the reader does not map the target. */
 CDPROBE_API int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target, uint32_t reader,
                                  cdprobe_diag_t* out);
+/* Dependent-load latency of every cell whose issuer is local to this process: one untimed warm-up rep, then `reps`
+ * timed reps of `hops` dependent loads over the source slice the issuer reads (written only at open, so no run is
+ * needed first).  ns per hop by %globaltimer on the issuer; the digest of the loaded words is checked against the
+ * pattern (CDPROBE_ERR_INTEGRITY in the cell's status).  A cell whose mapping is down is not read (measured = 0, the
+ * mapping status); the diagonal is chased only with a loop-back slice (n == 1 or CDPROBE_FLAG_LOCAL_DIAG).  One-sided,
+ * not collective: fills the local rows (row_mask).  Touches no result, pattern, landing slot or run_seq.  *out
+ * carries abi and n whatever the return code.  CDPROBE_ERR_ARG: null argument, hops > 1 << 20 or reps > 64;
+ * CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

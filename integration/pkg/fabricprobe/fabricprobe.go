@@ -30,11 +30,13 @@ typedef const char* (*str_fn)(int);
 typedef const char* (*last_fn)(void);
 typedef uint32_t (*abi_fn)(void);
 typedef int (*diag_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*);
+typedef int (*lat_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_latency_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
 static str_fn cdp_strerror; static last_fn cdp_last; static abi_fn cdp_abi;
 static diag_fn cdp_diag;  // optional: absent from libraries that predate cdprobe_diagnose
+static lat_fn cdp_lat;    // optional: absent from libraries that predate cdprobe_latency
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -47,6 +49,7 @@ static int cdp_load(const char* path) {
   cdp_last = (last_fn)dlsym(cdp_dl, "cdprobe_last_error");
   cdp_abi = (abi_fn)dlsym(cdp_dl, "cdprobe_abi_version");
   cdp_diag = (diag_fn)dlsym(cdp_dl, "cdprobe_diagnose");
+  cdp_lat = (lat_fn)dlsym(cdp_dl, "cdprobe_latency");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -58,6 +61,10 @@ static const char* cdp_call_last(void) { return cdp_last(); }
 static int cdp_has_diagnose(void) { return cdp_diag != NULL; }
 static int cdp_call_diagnose(cdprobe_t* h, uint32_t op, uint32_t i, uint32_t j, uint32_t reader, cdprobe_diag_t* d) {
   return cdp_diag(h, op, i, j, reader, d);
+}
+static int cdp_has_latency(void) { return cdp_lat != NULL; }
+static int cdp_call_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* l) {
+  return cdp_lat(h, hops, reps, l);
 }
 */
 import "C"
@@ -156,6 +163,20 @@ type Diagnosis struct {
 	BitFlips               [64]uint64 // flip words only: how often bit b differed
 	Ms                     float64
 	Samples                []DiagSample // the lowest-offset bad words, in offset order
+}
+
+// Latency is the dependent-load latency matrix of the local rows (cdprobe_latency_t).  Matrices are N x N
+// row-major, [issuer*N + target]; the Ns* entries are 0 where a cell was not measured or its chase timed out.
+type Latency struct {
+	N                      int
+	RowMask                uint32    // rows of this process's ranks
+	Hops, Reps             int       // as applied
+	RegionBytes            uint64    // bytes one chase ranges over
+	Measured               []bool
+	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the mapping's status
+	NsMin, NsMedian, NsMax []float32 // ns per hop over the timed reps
+	Digest                 []uint64  // xor of every loaded word
+	Ms                     float64
 }
 
 func Open(cfg Config) (*Probe, error) {
@@ -283,6 +304,47 @@ func (p *Probe) Diagnose(op uint32, issuer, target, reader int) (Diagnosis, erro
 		out.Samples = append(out.Samples, DiagSample{Offset: uint64(s.offset), Expected: uint64(s.expected),
 			Observed: uint64(s.observed), Word: uint64(s.word), RunSeq: uint64(s.run_seq),
 			Kind: DiagKinds[int(s.kind)%len(DiagKinds)], Rank: int(s.rank)})
+	}
+	return out, nil
+}
+
+// Latency chases hops dependent 8-byte loads from every local issuer through its mapping of each target's source
+// slice and reports ns per hop (0, 0: 1024 hops, 8 timed reps).  One-sided: only the local rows are filled.
+// ErrUnsupported when the library predates cdprobe_latency.
+func (p *Probe) Latency(hops, reps int) (Latency, error) {
+	if C.cdp_has_latency() == 0 {
+		return Latency{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_latency", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	var lt C.cdprobe_latency_t
+	rc := C.cdp_call_latency(p.h, C.uint32_t(hops), C.uint32_t(reps), &lt)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_latency: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return Latency{}, err
+	}
+	n := int(lt.n)
+	out := Latency{N: n, RowMask: uint32(lt.row_mask), Hops: int(lt.hops), Reps: int(lt.reps),
+		RegionBytes: uint64(lt.region_bytes), Ms: float64(lt.ms)}
+	out.Measured = make([]bool, n*n)
+	out.Status = make([]int32, n*n)
+	out.NsMin = make([]float32, n*n)
+	out.NsMedian = make([]float32, n*n)
+	out.NsMax = make([]float32, n*n)
+	out.Digest = make([]uint64, n*n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < n; j++ {
+			k := i*C.CDPROBE_MAX_GPUS + j
+			out.Measured[i*n+j] = lt.measured[k] != 0
+			out.Status[i*n+j] = int32(lt.status[k])
+			out.NsMin[i*n+j] = float32(lt.ns_min[k])
+			out.NsMedian[i*n+j] = float32(lt.ns_median[k])
+			out.NsMax[i*n+j] = float32(lt.ns_max[k])
+			out.Digest[i*n+j] = uint64(lt.digest[k])
+		}
 	}
 	return out, nil
 }

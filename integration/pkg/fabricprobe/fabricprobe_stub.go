@@ -71,9 +71,22 @@ type Diagnosis struct {
 	Samples                []DiagSample
 }
 
+type Latency struct {
+	N                      int
+	RowMask                uint32
+	Hops, Reps             int
+	RegionBytes            uint64
+	Measured               []bool
+	Status                 []int32
+	NsMin, NsMedian, NsMax []float32
+	Digest                 []uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
 	return Diagnosis{}, ErrUnsupported
 }
-func (*Probe) Close() {}
+func (*Probe) Latency(int, int) (Latency, error) { return Latency{}, ErrUnsupported }
+func (*Probe) Close()                            {}

@@ -16,6 +16,7 @@ from .fabricprobe import (  # noqa: F401
     Config,
     Diagnosis,
     ErrUnsupported,
+    Latency,
     Probe,
     ProbeError,
     Result,
@@ -25,4 +26,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "Open", "gate", "plan", "topology"]

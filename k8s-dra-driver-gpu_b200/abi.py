@@ -37,6 +37,9 @@ DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
 DIAG_KIND_NAMES = ("flip", "zero", "displaced", "stale", "foreign")
 
+LATENCY_DEFAULT_HOPS, LATENCY_DEFAULT_REPS = 1024, 8
+LATENCY_MAX_HOPS, LATENCY_MAX_REPS = 1 << 20, 64
+
 _N2 = MAX_GPUS * MAX_GPUS
 
 
@@ -224,6 +227,25 @@ class DiagT(C.Structure):
     ]
 
 
+class LatencyT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("hops", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("region_bytes", C.c_uint64),
+        ("measured", C.c_uint8 * _N2),
+        ("status", C.c_int32 * _N2),
+        ("ns_min", C.c_float * _N2),
+        ("ns_median", C.c_float * _N2),
+        ("ns_max", C.c_float * _N2),
+        ("digest", C.c_uint64 * _N2),
+        ("ms", C.c_double),
+    ]
+
+
 # Every symbol include/cdprobe.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "cdprobe_abi_version": (C.c_uint32, []),
@@ -241,6 +263,7 @@ SYMBOLS = {
     "cdprobe_ce_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32,
                                   C.c_uint64, C.c_uint32, C.POINTER(C.c_double)]),
     "cdprobe_diagnose": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(DiagT)]),
+    "cdprobe_latency": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(LatencyT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

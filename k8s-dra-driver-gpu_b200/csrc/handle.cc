@@ -22,12 +22,14 @@
 #include <time.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <new>
 #include <string>
 #include <vector>
 
 #include "../../include/cdprobe.h"
 #include "diagnose.h"
+#include "latency.h"
 #include "plan.h"
 #include "probe_launch.h"
 #include "probe_types.h"
@@ -71,6 +73,7 @@ struct LocalRank {
   uint32_t peer_mask = 0;
   void* diag_scratch = nullptr;  // cdprobe_diagnose: allocated on this rank's first diagnosis
   size_t diag_scratch_bytes = 0;
+  LatencyRep* lat_scratch = nullptr;  // cdprobe_latency: allocated on this rank's first chase
 };
 
 }  // namespace cdp
@@ -396,6 +399,7 @@ static void destroy(cdprobe* h) {
     if (L.own_fd >= 0) ::close(L.own_fd);
     if (L.row) cudaFreeHost(L.row);
     if (L.diag_scratch) cudaFree(L.diag_scratch);
+    if (L.lat_scratch) cudaFree(L.lat_scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
     if (L.stream) cudaStreamDestroy(L.stream);
@@ -1286,6 +1290,125 @@ int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target
   for (int b = 0; b < 64; ++b) out->bit_flips[b] = d.bit_flips[b];
   out->n_samples = d.bad_words < (uint64_t)CDPROBE_DIAG_SAMPLES ? (uint32_t)d.bad_words : (uint32_t)CDPROBE_DIAG_SAMPLES;
   memcpy(out->sample, d.sample, sizeof(out->sample[0]) * out->n_samples);
+  return CDPROBE_OK;
+}
+
+static_assert(sizeof(cdp::LatencyRep) == 24, "latency rep slot");
+
+int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->hops = hops != 0 ? hops : cdp::kLatencyDefaultHops;
+  out->reps = reps != 0 ? reps : cdp::kLatencyDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  out->n = h->n_total;
+  out->region_bytes = pl.bpp;
+  if (out->hops > cdp::kLatencyMaxHops || out->reps > cdp::kLatencyMaxReps) {
+    cdp::set_err("hops must be at most 1 << 20 and reps at most 64");
+    return CDPROBE_ERR_ARG;
+  }
+  if (h->sticky) {
+    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
+    return CDPROBE_ERR_STATE;
+  }
+  hops = out->hops;
+  reps = out->reps;
+  const uint64_t lines = pl.bpp / (cdp::kLineWords * 8);
+
+  // 1. every local issuer's chases, all launched before any is waited for
+  cdp::LatencyParams P[cdp::kMaxRanks];
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    out->row_mask |= 1u << g;
+    cdp::LatencyParams& p = P[li];
+    memset(&p, 0, sizeof(p));
+    p.seed = h->seed;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.hops = hops;
+    p.reps = reps;
+    for (uint32_t j = 0; j < h->n_total; ++j) {
+      if (j == g && !pl.diag) continue;  // no loop-back slice to chase
+      const uint32_t idx = g * CDPROBE_MAX_GPUS + j;
+      if (h->status[g][j] != 0 || !L.mapped[j]) {  // never read through a mapping that is down
+        out->status[idx] = h->status[g][j] != 0 ? h->status[g][j] : cdp::kStatusUnmapped;
+        continue;
+      }
+      cdp::LatencyCell& c = p.cell[p.n_cells++];
+      c.region = reinterpret_cast<const uint8_t*>(L.va[j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
+      c.lines = lines;
+      c.issuer = g;
+      c.target = j;
+    }
+    if (p.n_cells == 0) continue;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    if (L.lat_scratch == nullptr)
+      CDP_RT(cudaMalloc(&L.lat_scratch, sizeof(cdp::LatencyRep) * cdp::kMaxRanks * cdp::kLatencyRepSlots));
+    const cudaError_t e = (cudaError_t)cdp::latency_launch(p, L.lat_scratch, L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch latency_kernel", e);
+    }
+  }
+
+  // 2. while they run: the digest each chase gives over an intact region
+  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t k = 0; k < P[li].n_cells; ++k) {
+      const cdp::LatencyCell& c = P[li].cell[k];
+      const uint64_t first = (uint64_t)cdp::cell_slice(pl, c.issuer, c.target) * (pl.bpp / 8);
+      for (uint32_t r = 0; r <= reps; ++r)
+        want[li][k] ^= cdp::latency_rep_digest(h->seed, c.issuer, c.target, first, lines, r, hops);
+    }
+  }
+
+  // 3. collect: ns per hop of the timed reps, the digest of all of them
+  std::vector<cdp::LatencyRep> got((size_t)cdp::kMaxRanks * cdp::kLatencyRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::LatencyParams& p = P[li];
+    if (p.n_cells == 0) continue;
+    cdp::LocalRank& L = h->lr[li];
+    cudaError_t e = cudaSetDevice(L.ordinal);
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(got.data(), L.lat_scratch, sizeof(cdp::LatencyRep) * p.n_cells * cdp::kLatencyRepSlots,
+                          cudaMemcpyDeviceToHost, L.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;  // a failed kernel leaves the context unusable
+      return cdp::fail_cuda("cdprobe_latency", e);
+    }
+    for (uint32_t k = 0; k < p.n_cells; ++k) {
+      const uint32_t idx = p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target;
+      const cdp::LatencyRep* rep = got.data() + (size_t)k * cdp::kLatencyRepSlots;
+      uint64_t digest = 0;
+      int32_t st = 0;
+      float ns[cdp::kLatencyMaxReps];
+      for (uint32_t r = 0; r <= reps; ++r) {
+        digest ^= rep[r].digest;
+        if (rep[r].status != 0) {
+          st = rep[r].status;
+          break;
+        }
+        if (r > 0) ns[r - 1] = (float)((double)rep[r].ns / hops);
+      }
+      out->measured[idx] = 1;
+      out->digest[idx] = digest;
+      if (st == 0) {
+        std::sort(ns, ns + reps);
+        out->ns_min[idx] = ns[0];
+        out->ns_median[idx] = ns[reps / 2];
+        out->ns_max[idx] = ns[reps - 1];
+        if (digest != want[li][k]) st = CDPROBE_ERR_INTEGRITY;
+      }
+      out->status[idx] = st;
+    }
+  }
+  out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
 

@@ -302,4 +302,40 @@ CDP_HD inline DiagClass diag_classify(const DiagSpec& s, uint64_t observed) {
   return c;
 }
 
+// ---- the dependent-load chase (cdprobe_latency, DESIGN §5c) ----------------------------------------------------
+// A chase ranges over the L = bytes / 128 lines of the source slice issuer i reads from target j.  Hop h loads
+// v = word 16 * line of that region (src_word(seed, j, first_word + 16 * line)); the next line is drawn from v, so
+// every load waits for the one before.  Mixing in h + 1 keeps a chase that revisits a line from repeating its path.
+constexpr uint64_t kLatencyTag = 0x4C4154454E4359ull;  // "LATENCY"
+constexpr uint32_t kLineWords = 16;                    // one 128-byte line
+
+// (x * n) >> 64: maps x uniformly into [0, n) without a division, so every line lies inside the region whatever
+// word the previous load returned.
+CDP_HD inline uint64_t fastrange64(uint64_t x, uint64_t n) {
+#if defined(__CUDA_ARCH__)
+  return __umul64hi(x, n);
+#else
+  return (uint64_t)(((unsigned __int128)x * n) >> 64);
+#endif
+}
+// First line of rep r of cell (i, j); r = 0 is the untimed warm-up.
+CDP_HD inline uint64_t latency_start(uint64_t seed, uint32_t i, uint32_t j, uint32_t r, uint64_t lines) {
+  return fastrange64(splitmix64(seed ^ kLatencyTag ^ ((uint64_t)i << 56) ^ ((uint64_t)j << 48) ^ r), lines);
+}
+// The line after hop h loaded v.
+CDP_HD inline uint64_t latency_next(uint64_t v, uint32_t h, uint64_t lines) {
+  return fastrange64(v ^ ((uint64_t)(h + 1) * kGolden), lines);
+}
+// Xor of every word one rep of the chase loads from an intact region (host side of the digest check).
+inline uint64_t latency_rep_digest(uint64_t seed, uint32_t i, uint32_t j, uint64_t first_word, uint64_t lines,
+                                   uint32_t rep, uint32_t hops) {
+  uint64_t line = latency_start(seed, i, j, rep, lines), digest = 0;
+  for (uint32_t h = 0; h < hops; ++h) {
+    const uint64_t v = src_word(seed, j, first_word + kLineWords * line);
+    digest ^= v;
+    line = latency_next(v, h, lines);
+  }
+  return digest;
+}
+
 }  // namespace cdp

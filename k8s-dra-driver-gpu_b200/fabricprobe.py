@@ -198,6 +198,50 @@ class Diagnosis:
         )
 
 
+@dataclasses.dataclass
+class Latency:
+    """What cdprobe_latency measured: n x n matrices [issuer][target] of ns per dependent 8-byte load (min, median and
+    max over the timed reps) and the digest of the loaded words.  A cell that was not chased (a row of another
+    process, a mapping that is down, the diagonal without a loop-back slice) is None in every matrix but `status`;
+    a chase that passed timeout_ms has a digest but no times."""
+    n: int
+    row_mask: int
+    hops: int
+    reps: int
+    region_bytes: int
+    measured: List[List[bool]]
+    status: List[List[int]]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the mapping's status
+    ns_min: List[List[Optional[float]]]
+    ns_median: List[List[Optional[float]]]
+    ns_max: List[List[Optional[float]]]
+    digest: List[List[Optional[int]]]
+    ms: float
+    raw: abi.LatencyT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.LatencyT) -> "Latency":
+        n = t.n
+
+        def mat(a, timed=False):
+            out = []
+            for i in range(n):
+                row = []
+                for j in range(n):
+                    k = i * abi.MAX_GPUS + j
+                    ok = t.measured[k] and not (timed and t.status[k] == abi.ERR_TIMEOUT)
+                    row.append(a[k] if ok else None)
+                out.append(row)
+            return out
+
+        return Latency(
+            n=n, row_mask=t.row_mask, hops=t.hops, reps=t.reps, region_bytes=t.region_bytes,
+            measured=[[bool(t.measured[i * abi.MAX_GPUS + j]) for j in range(n)] for i in range(n)],
+            status=[[t.status[i * abi.MAX_GPUS + j] for j in range(n)] for i in range(n)],
+            ns_min=mat(t.ns_min, True), ns_median=mat(t.ns_median, True), ns_max=mat(t.ns_max, True),
+            digest=mat(t.digest), ms=t.ms, raw=t,
+        )
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -302,6 +346,20 @@ class Probe:
         d = abi.DiagT()
         rc = self._lib.cdprobe_diagnose(self._h, op, issuer, target, reader, C.byref(d))
         return rc, d
+
+    def Latency(self, hops: int = 0, reps: int = 0) -> Latency:
+        """Go: (*Probe).Latency.  Dependent-load latency of every cell whose issuer is local (0: 1024 hops, 8 timed
+        reps).  Needs no Run first and disturbs none."""
+        rc, t = self.latency_raw(hops, reps)
+        if rc != abi.OK:
+            _raise(self._lib, rc, "cdprobe_latency")
+        return Latency.from_c(t)
+
+    def latency_raw(self, hops: int, reps: int):
+        """The bare ABI call: (return code, abi.LatencyT as the library left it)."""
+        t = abi.LatencyT()
+        rc = self._lib.cdprobe_latency(self._h, hops, reps, C.byref(t))
+        return rc, t
 
     def Close(self) -> None:
         if self._h:
