@@ -316,8 +316,8 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_strerror / cdprobe_last_error   text of the Go error:   fmt.Errorf convention of main.go
  *   cdprobe_remap_peer / cdprobe_unmap_peer  emulate NodeUnprepare/NodePrepare churn around a live domain:
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
- *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_plan,
- *   cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
+ *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
+ *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency: diagnostics, benches, fault injection; the reference has no counterpart (it has no probe,
  *   SURVEY.md F1).
  *   cdprobe_diagnose and cdprobe_latency are optional for callers: a daemon binds them with dlsym and works without.
@@ -359,8 +359,17 @@ CDPROBE_API int cdprobe_ce_copy(cdprobe_t* h, uint32_t n_copies, const uint32_t*
 CDPROBE_API int cdprobe_remap_peer(cdprobe_t* h, uint32_t local, uint32_t peer);
 /* Fault injection for parity tests: drop local rank's mapping of `peer` (cell becomes unreachable, run still returns). */
 CDPROBE_API int cdprobe_unmap_peer(cdprobe_t* h, uint32_t local, uint32_t peer);
-/* Fault injection: XOR one 64-bit word of local rank's source slice / force a bad write salt. */
+/* Fault injection: XOR one 64-bit word of local rank's source buffer (byte_offset from its start) at rest. */
 CDPROBE_API int cdprobe_corrupt(cdprobe_t* h, uint32_t local, uint64_t byte_offset, uint64_t xor_mask);
+/* Fault injection for tests: on every cdprobe_run until disarmed, right after local rank `local`'s write into
+ * `target`'s landing slot has completed and before any rank verifies it, XOR xor_mask[e] into word word[e] of that
+ * slot (e < n <= 8).  The writer's published (S, X) is untouched: to the verifier this is a fault in transit, and the
+ * run completes normally with that write cell failing.  One cell is armed per handle; arming replaces the previous
+ * arming, n = 0 disarms.  While disarmed the kernel only loads the descriptor's count.  CDPROBE_ERR_ARG: bad local or target, n > 8, a
+ * word >= bytes_per_pair / 8, a repeated word, a zero mask, or target == the issuer without a loop-back slot;
+ * CDPROBE_ERR_STATE: sticky handle, or the issuer does not map the target. */
+CDPROBE_API int cdprobe_corrupt_landing(cdprobe_t* h, uint32_t local, uint32_t target, uint32_t n,
+                                        const uint64_t* word, const uint64_t* xor_mask);
 /* Where and how cell (op, issuer, target) of the last cdprobe_run went wrong: reader (a global rank, local to this
  * process, that maps the target) re-reads the cell's region — the source slice the issuer reads, or the landing slot
  * it writes — and compares it on its GPU with the pattern of that run.  reader = the issuer: what crossed the

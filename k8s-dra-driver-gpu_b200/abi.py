@@ -260,6 +260,8 @@ SYMBOLS = {
     "cdprobe_remap_peer": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     "cdprobe_unmap_peer": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     "cdprobe_corrupt": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64]),
+    "cdprobe_corrupt_landing": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64),
+                                          C.POINTER(C.c_uint64)]),
     "cdprobe_ce_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32,
                                   C.c_uint64, C.c_uint32, C.POINTER(C.c_double)]),
     "cdprobe_diagnose": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(DiagT)]),

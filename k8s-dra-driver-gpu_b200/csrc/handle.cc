@@ -108,6 +108,7 @@ struct cdprobe {
   uint32_t solo_rank = 0;        // 1-based local rank that runs alone, no cross-GPU barrier (ncu captures)
   double last_probe_ms = 0.0;    // host wall clock of the previous run (wait_rows: how long to spin hot)
   uint32_t verify_ctas = 32;  // CTAs that verify landing slots under CDPROBE_FLAG_OVERLAP_VERIFY
+  int32_t fault_local = -1;   // local rank whose Ctrl holds the armed landing fault (cdprobe_corrupt_landing), -1: none
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -307,6 +308,16 @@ static int reset_ctrl_local(cdprobe* h, uint32_t li) {
   uint8_t* base = reinterpret_cast<uint8_t*>(L.va[L.grank]);
   const size_t off = offsetof(Ctrl, grid_arrive);
   CDP_RT(cudaMemsetAsync(base + off, 0, sizeof(Ctrl) - off, L.stream));
+  CDP_RT(cudaStreamSynchronize(L.stream));
+  return CDPROBE_OK;
+}
+
+// Writes local rank li's landing-fault descriptor (cdprobe_corrupt_landing), stream-ordered after the last run.
+static int write_fault(cdprobe* h, uint32_t li, const LandingFault& f) {
+  LocalRank& L = h->lr[li];
+  CDP_RT(cudaSetDevice(L.ordinal));
+  uint8_t* p = reinterpret_cast<uint8_t*>(L.va[L.grank]) + offsetof(Ctrl, fault);
+  CDP_RT(cudaMemcpyAsync(p, &f, sizeof(f), cudaMemcpyHostToDevice, L.stream));
   CDP_RT(cudaStreamSynchronize(L.stream));
   return CDPROBE_OK;
 }
@@ -1137,6 +1148,51 @@ int cdprobe_corrupt(cdprobe_t* h, uint32_t local, uint64_t byte_offset, uint64_t
   w ^= xor_mask;
   CDP_RT(cudaMemcpyAsync(p, &w, 8, cudaMemcpyHostToDevice, L.stream));
   CDP_RT(cudaStreamSynchronize(L.stream));
+  return CDPROBE_OK;
+}
+
+int cdprobe_corrupt_landing(cdprobe_t* h, uint32_t local, uint32_t target, uint32_t n, const uint64_t* word,
+                            const uint64_t* xor_mask) {
+  cdp::g_last_error.clear();
+  if (h == nullptr || local >= h->n_local || target >= h->n_total || n > cdp::kMaxLandingFaults) return CDPROBE_ERR_ARG;
+  if (n > 0 && (word == nullptr || xor_mask == nullptr)) return CDPROBE_ERR_ARG;
+  const uint32_t g = h->lr[local].grank;
+  const uint64_t words = h->plan.bpp / 8;
+  cdp::LandingFault f;
+  memset(&f, 0, sizeof(f));
+  f.n = n;
+  f.target = target;
+  for (uint32_t e = 0; e < n; ++e) {
+    if (word[e] >= words || xor_mask[e] == 0) return CDPROBE_ERR_ARG;
+    for (uint32_t q = 0; q < e; ++q)
+      if (word[q] == word[e]) return CDPROBE_ERR_ARG;
+    f.word[e] = word[e];
+    f.mask[e] = xor_mask[e];
+  }
+  if (n > 0 && target == g && !h->plan.diag) {
+    cdp::set_err("cell (i, i) exists only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG)");
+    return CDPROBE_ERR_ARG;
+  }
+  if (h->sticky) {
+    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
+    return CDPROBE_ERR_STATE;
+  }
+  if (n > 0 && (h->status[g][target] != 0 || !h->lr[local].mapped[target])) {
+    cdp::set_err("the issuer does not map the target");
+    return CDPROBE_ERR_STATE;
+  }
+  // one armed cell per handle: clear the previous one, wherever it is
+  if (h->fault_local >= 0) {
+    cdp::LandingFault off;
+    memset(&off, 0, sizeof(off));
+    const int rc = cdp::write_fault(h, (uint32_t)h->fault_local, off);
+    if (rc != CDPROBE_OK) return rc;
+    h->fault_local = -1;
+  }
+  if (n == 0) return CDPROBE_OK;
+  const int rc = cdp::write_fault(h, local, f);
+  if (rc != CDPROBE_OK) return rc;
+  h->fault_local = (int32_t)local;
   return CDPROBE_OK;
 }
 

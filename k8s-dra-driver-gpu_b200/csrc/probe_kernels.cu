@@ -507,6 +507,34 @@ __device__ void publish_verdicts(const ProbeParams& P, Ctrl* ctrl) {
   }
 }
 
+// ------------------------------------------------------ test-only fault injection ----
+// cdprobe_corrupt_landing arms ctrl->fault in the issuer's Ctrl.  The fault is applied by one thread after the write
+// into the armed target's slot has completed and before anything that lets a verifier read the slot, so to the
+// verifier it is a fault in transit; the writer's published (S, X) is untouched.  Every store stays inside the slot
+// (the host checks word[e] < bytes_per_pair / 8).
+__device__ __forceinline__ bool fault_armed(const ProbeParams& P, const Ctrl* ctrl, uint32_t target) {
+  return ctrl->fault.n != 0u && ctrl->fault.target == target && P.base_peer[target] != nullptr;
+}
+__device__ __forceinline__ void xor_landing(const LandingFault* f, uint8_t* slot) {
+  fence_proxy_async_global();  // the slot may hold TMA bulk stores
+  const uint32_t n = f->n;
+  for (uint32_t e = 0; e < n && e < kMaxLandingFaults; ++e) {
+    uint64_t* w = reinterpret_cast<uint64_t*>(slot) + f->word[e];
+    st_relaxed_sys(w, ld_relaxed_sys(w) ^ f->mask[e]);
+  }
+}
+// Phase walk: phase ph has a write job into the armed target (either job slot, as in publish_writes).  Called by the
+// barrier leader before its publications, signals and release, which the target's verify waits for.
+__device__ __noinline__ void fault_phase_write(const ProbeParams& P, Ctrl* ctrl, int ph) {
+#pragma unroll
+  for (int jb = 0; jb < 2; ++jb) {
+    const Job job = P.phase[ph].job[jb];
+    if (job.kind != kJobWrite || !fault_armed(P, ctrl, (uint32_t)job.peer)) continue;
+    xor_landing(&ctrl->fault, P.base_peer[job.peer] + P.land_off + (uint64_t)job.slot * P.bpp);
+    __threadfence_system();
+  }
+}
+
 __device__ __forceinline__ void signal_ranks(const ProbeParams& P, uint32_t mask, uint64_t target) {
   for (uint32_t j = 0; j < P.n_ranks; ++j) {
     if (j == P.rank || !((mask >> j) & 1u)) continue;
@@ -541,6 +569,7 @@ __device__ void barrier(const ProbeParams& P, Ctx& c, int b, uint32_t sync, uint
         *reinterpret_cast<volatile unsigned int*>(&ctrl->grid_arrive) = 0u;
         __threadfence();
         const uint64_t t_arr = gtimer();
+        if (b >= 1 && ctrl->fault.n != 0u) fault_phase_write(P, ctrl, b - 1);
         bool published = false, wrote_done = false;
         if (sync) {
           if (b >= 1) {
@@ -709,7 +738,9 @@ __device__ __forceinline__ bool is_loopback(const ProbeParams& P) {
 //   verifier warp: lane 0 spins on ld.acquire.gpu of lb.written until it reaches the slot's unit count ->
 //                  __syncwarp -> loads (the bulk path issues fence.proxy.async.global before its first load).
 // Counting units rather than warps means no warp waits for a CTA that has not started: the units are all claimed
-// by CTAs that are running.  The CTA that finishes last (lb.done) publishes the write checksum and the verdict,
+// by CTAs that are running.  An armed landing fault counts as one more unit: the writer warp whose atomicAdd
+// completes the slot's count applies it between two __threadfence and then adds 1, and the verifiers wait for that.
+// The CTA that finishes last (lb.done) publishes the write checksum and the verdict,
 // writes the row and zeroes the counters for the next run.
 __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint64_t t_enter) {
   constexpr int kRed = 6 + 5;  // per warp: (sum, xor) x 3 jobs (cta_reduce), end time x 3 jobs, first issue x 2 jobs
@@ -737,7 +768,15 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
     if (c.lane == 0) {
       fence_proxy_async_global();
       __threadfence();
-      atomicAdd(&lb->written.v, (unsigned long long)n_wr);
+      const unsigned long long before = atomicAdd(&lb->written.v, (unsigned long long)n_wr);
+      if (before + n_wr == n_units && fault_armed(P, ctrl, P.rank)) {
+        // the whole slot is stored: an armed landing fault goes in now and counts as one more unit, so the
+        // verifiers, which wait for n_units + 1, read it (acquire of every writer's release, then release again)
+        __threadfence();
+        xor_landing(&ctrl->fault, slot);
+        __threadfence();
+        atomicAdd(&lb->written.v, 1ull);
+      }
     }
     t_end[0] = gtimer();
   }
@@ -747,7 +786,9 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
 
   bool go = true;
   // deadline checked at the transition too, as at a barrier arrival
-  if (c.lane == 0) go = !check_abort(c) && spin_until<kScopeGpu>(c, &lb->written.v, n_units);
+  if (c.lane == 0)
+    go = !check_abort(c) &&
+         spin_until<kScopeGpu>(c, &lb->written.v, n_units + (fault_armed(P, ctrl, P.rank) ? 1u : 0u));
   go = __shfl_sync(0xffffffffu, go, 0);
   if (go && read_units(c, P.path, slot, P.bpp, claimed(P.bpp, &lb->claim[2].v), a[2])) t_end[2] = gtimer();
 

@@ -67,6 +67,16 @@ struct LoopBack {
   unsigned long long t_enter_n;       // ~(earliest CTA entry)
 };
 
+// Test-only fault injection (cdprobe_corrupt_landing): after this rank's write into `target`'s landing slot has
+// completed and before anyone verifies it, the kernel xors mask[e] into word word[e] of the slot, e < n.  n = 0:
+// disarmed.  Written by the host between runs only.
+constexpr uint32_t kMaxLandingFaults = 8;
+struct LandingFault {
+  uint32_t n, target;
+  uint64_t word[kMaxLandingFaults];
+  uint64_t mask[kMaxLandingFaults];
+};
+
 struct Ctrl {
   // ---- written by peers over NVLink ------------------------------------
   FlagLine flags[kMaxRanks];          // flags[j].v = last barrier target rank j signalled
@@ -75,6 +85,8 @@ struct Ctrl {
   // ---- published by the owner at open (read by peers) ------------------
   uint64_t src_sum[kMaxRanks];        // per source slice
   uint64_t src_xor[kMaxRanks];
+  // ---- written by the host; before grid_arrive, so the reset after an aborted run keeps it ----
+  LandingFault fault;
   // ---- local only ------------------------------------------------------
   alignas(128) unsigned int grid_arrive;
   alignas(128) unsigned long long grid_release;

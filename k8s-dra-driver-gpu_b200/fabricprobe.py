@@ -331,6 +331,20 @@ class Probe:
         if rc != abi.OK:
             _raise(self._lib, rc, "cdprobe_corrupt")
 
+    def CorruptLanding(self, local: int, target: int, faults) -> None:
+        """Test-only fault in transit: on every Run until disarmed, xor each (word index, mask) of `faults` into
+        the landing slot local rank `local` writes in `target`, after the write and before the verify.  [] disarms."""
+        rc = self.corrupt_landing_raw(local, target, faults)
+        if rc != abi.OK:
+            _raise(self._lib, rc, "cdprobe_corrupt_landing")
+
+    def corrupt_landing_raw(self, local: int, target: int, faults) -> int:
+        """The bare ABI call: its return code."""
+        k = len(faults)
+        word = (C.c_uint64 * max(k, 1))(*[int(w) for w, _ in faults])
+        mask = (C.c_uint64 * max(k, 1))(*[int(m) for _, m in faults])
+        return self._lib.cdprobe_corrupt_landing(self._h, local, target, k, word, mask)
+
     def Diagnose(self, op, issuer: int, target: int, reader: Optional[int] = None) -> Diagnosis:
         """Go: (*Probe).Diagnose.  Re-reads cell (op, issuer, target) of the last Run on `reader`'s GPU (default: the
         issuer, i.e. through the fabric; the target reads it at rest) and diffs it against the pattern.

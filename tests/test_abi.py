@@ -101,6 +101,43 @@ def test_open_rejects_bad_abi_and_null(pkg):
     lib.cdprobe_close(None)  # must be a no-op
 
 
+def test_corrupt_landing_null_handle_and_wrapper_packing(pkg):
+    """cdprobe_corrupt_landing refuses a null handle; Probe.CorruptLanding hands the library the local rank, the
+    target, the count and the (word, mask) pairs as two uint64 arrays, [] as n = 0, and raises on an error code."""
+    a = pkg.abi
+    lib = a.load_library()
+    assert a.SYMBOLS["cdprobe_corrupt_landing"] == (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)])
+    w, m = (C.c_uint64 * 1)(3), (C.c_uint64 * 1)(1)
+    assert lib.cdprobe_corrupt_landing(None, 0, 1, 1, w, m) == a.ERR_ARG
+    assert lib.cdprobe_corrupt_landing(None, 0, 1, 0, None, None) == a.ERR_ARG
+
+    calls = []
+
+    class FakeLib:
+        def cdprobe_corrupt_landing(self, h, local, target, n, word, mask):
+            calls.append((h.value, local, target, n, [word[e] for e in range(n)], [mask[e] for e in range(n)]))
+            return a.ERR_ARG if n > 8 else a.OK
+
+        def cdprobe_strerror(self, rc):
+            return b"invalid argument"
+
+        def cdprobe_last_error(self):
+            return b""
+
+    p = object.__new__(pkg.Probe)
+    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
+    try:
+        p.CorruptLanding(1, 3, [(0, 1), (1 << 40, (1 << 63) | 5)])
+        p.CorruptLanding(0, 0, [])
+        assert calls == [(0x1234, 1, 3, 2, [0, 1 << 40], [1, (1 << 63) | 5]), (0x1234, 0, 0, 0, [], [])]
+        with pytest.raises(pkg.ProbeError) as e:
+            p.CorruptLanding(0, 1, [(k, 1) for k in range(9)])
+        assert e.value.code == a.ERR_ARG and calls[-1][3] == 9
+    finally:
+        p._h = C.c_void_p()
+
+
 @pytest.mark.skipif(gpu_count() > 0, reason="this box has a GPU; the loud-failure path needs a CPU-only box")
 def test_open_fails_loudly_without_a_gpu(pkg):
     """No CUDA driver => CDPROBE_ERR_NO_DEVICE with a reason; there is no CPU fallback to fall into."""
