@@ -295,6 +295,29 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_latency_t;
 
+/* Signal round trip per ordered pair (cdprobe_pingpong): initiator i stores a word into its line in target j's
+ * memory, j polls its local copy and stores the echo into its line in i's memory, i polls for the echo — the K3
+ * barrier's signal, both ways (DESIGN §5d).  Matrices are row-major [initiator * CDPROBE_MAX_GPUS + target]. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t trips, reps;                 /* as applied: 0 -> 256 and 8; trips in [1, 1 << 16], reps in [1, 64] */
+  uint32_t fenced;                      /* 1: fence.sys before every store (the barrier's signal after a publication) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_pingpong calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint8_t measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];  /* 1: the cell's round trips ran */
+  int32_t status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 0 ok; CDPROBE_ERR_INTEGRITY: an echo or the digest differs
+                                                             from the expected words; CDPROBE_ERR_TIMEOUT: a poll passed
+                                                             timeout_ms; else the pair's mapping status */
+  float ns_min[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];      /* ns per round trip over the timed reps (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];
+  uint64_t digest[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* xor of every echo word the initiator received, warm-up
+                                                             rep included */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_pingpong_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -318,9 +341,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency: diagnostics, benches, fault injection; the reference has no counterpart (it has no probe,
- *   SURVEY.md F1).
- *   cdprobe_diagnose and cdprobe_latency are optional for callers: a daemon binds them with dlsym and works without.
+ *   cdprobe_latency, cdprobe_pingpong: diagnostics, benches, fault injection; the reference has no counterpart (it
+ *   has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose, cdprobe_latency and cdprobe_pingpong are optional for callers: a daemon binds them with dlsym
+ *   and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -347,6 +371,10 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                         self-contained kernel is what `ncu` can replay: NVLink byte counters per launch. */
 #define CDPROBE_OPT_ALL_RANK_BARRIERS 15u /* value 0/1: see CDPROBE_FLAG_ALL_RANK_BARRIERS */
 #define CDPROBE_OPT_PAIR_BARRIERS 16u     /* value 0/1: see CDPROBE_FLAG_PAIR_BARRIERS */
+#define CDPROBE_OPT_PINGPONG_FAULT 17u    /* tests: value = ((initiator + 1) << 32) | ((target + 1) << 16) | trip arms a
+                                             skip-ahead echo in cdprobe_pingpong: the responder `target`, in the
+                                             process that hosts it, answers that trip of timed rep 1 of cell
+                                             (initiator, target) with the echo of trip + 1; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -387,6 +415,19 @@ CDPROBE_API int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uin
  * carries abi and n whatever the return code.  CDPROBE_ERR_ARG: null argument, hops > 1 << 20 or reps > 64;
  * CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out);
+/* Signal round trip of every off-diagonal cell, over the pairs of the tournament (cdprobe_plan partner table): in
+ * each round a rank and its partner run two legs, the lower rank initiating first.  A leg is one untimed warm-up rep,
+ * then `reps` timed reps of `trips` round trips; ns per round trip by %globaltimer on the initiator.  fenced = 0:
+ * st.relaxed.sys stores and ld.acquire.sys polls (the barrier's signal when nothing was published); fenced = 1: a
+ * fence.sys before every store (the signal after a publication).  The digest of the echo words is checked against
+ * the expected one (CDPROBE_ERR_INTEGRITY in the cell's status).  A pair is exchanged only when both directions are
+ * mapped; otherwise both its cells are skipped on both sides (measured = 0, the mapping status).  n == 1 measures
+ * nothing.  Collective when world_size > 1: every process calls it with the same arguments, and fills the rows of
+ * its own ranks (row_mask).  Touches no result, pattern, landing slot, Ctrl word or run_seq; needs no run first.
+ * *out carries abi, n, trips and reps whatever the return code.  CDPROBE_ERR_ARG: null argument, trips > 1 << 16,
+ * reps > 64, fenced > 1, arguments that differ between processes, or an armed CDPROBE_OPT_PINGPONG_FAULT whose cell
+ * is out of range or whose trip is >= trips - 1 (or == trips - 2 with reps == 1); CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

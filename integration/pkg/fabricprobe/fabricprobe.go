@@ -31,12 +31,14 @@ typedef const char* (*last_fn)(void);
 typedef uint32_t (*abi_fn)(void);
 typedef int (*diag_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*);
 typedef int (*lat_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_latency_t*);
+typedef int (*pp_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_pingpong_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
 static str_fn cdp_strerror; static last_fn cdp_last; static abi_fn cdp_abi;
 static diag_fn cdp_diag;  // optional: absent from libraries that predate cdprobe_diagnose
 static lat_fn cdp_lat;    // optional: absent from libraries that predate cdprobe_latency
+static pp_fn cdp_pp;      // optional: absent from libraries that predate cdprobe_pingpong
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -50,6 +52,7 @@ static int cdp_load(const char* path) {
   cdp_abi = (abi_fn)dlsym(cdp_dl, "cdprobe_abi_version");
   cdp_diag = (diag_fn)dlsym(cdp_dl, "cdprobe_diagnose");
   cdp_lat = (lat_fn)dlsym(cdp_dl, "cdprobe_latency");
+  cdp_pp = (pp_fn)dlsym(cdp_dl, "cdprobe_pingpong");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -65,6 +68,10 @@ static int cdp_call_diagnose(cdprobe_t* h, uint32_t op, uint32_t i, uint32_t j, 
 static int cdp_has_latency(void) { return cdp_lat != NULL; }
 static int cdp_call_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* l) {
   return cdp_lat(h, hops, reps, l);
+}
+static int cdp_has_pingpong(void) { return cdp_pp != NULL; }
+static int cdp_call_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* pp) {
+  return cdp_pp(h, trips, reps, fenced, pp);
 }
 */
 import "C"
@@ -176,6 +183,21 @@ type Latency struct {
 	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the mapping's status
 	NsMin, NsMedian, NsMax []float32 // ns per hop over the timed reps
 	Digest                 []uint64  // xor of every loaded word
+	Ms                     float64
+}
+
+// PingPong is the signal round-trip matrix of the local rows (cdprobe_pingpong_t).  Matrices are N x N row-major,
+// [initiator*N + target]; the Ns* entries are 0 where a cell was not measured or its round trips timed out.
+type PingPong struct {
+	N                      int
+	RowMask                uint32    // rows of this process's ranks
+	Trips, Reps            int       // as applied
+	Fenced                 bool      // a fence.sys before every store
+	CallSeq                uint64    // 1-based count of PingPong calls, equal in every process
+	Measured               []bool
+	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the pair's mapping status
+	NsMin, NsMedian, NsMax []float32 // ns per round trip over the timed reps
+	Digest                 []uint64  // xor of every echo word the initiator received
 	Ms                     float64
 }
 
@@ -344,6 +366,52 @@ func (p *Probe) Latency(hops, reps int) (Latency, error) {
 			out.NsMedian[i*n+j] = float32(lt.ns_median[k])
 			out.NsMax[i*n+j] = float32(lt.ns_max[k])
 			out.Digest[i*n+j] = uint64(lt.digest[k])
+		}
+	}
+	return out, nil
+}
+
+// PingPong times the barrier's cross-GPU signal as a round trip over every pair of the tournament and reports ns
+// per round trip (0, 0: 256 round trips, 8 timed reps); fenced puts a fence.sys before every store.  Collective when
+// the domain spans processes: every process calls it with the same arguments and gets its own rows.
+// ErrUnsupported when the library predates cdprobe_pingpong.
+func (p *Probe) PingPong(trips, reps int, fenced bool) (PingPong, error) {
+	if C.cdp_has_pingpong() == 0 {
+		return PingPong{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_pingpong", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	f := 0
+	if fenced {
+		f = 1
+	}
+	var pp C.cdprobe_pingpong_t
+	rc := C.cdp_call_pingpong(p.h, C.uint32_t(trips), C.uint32_t(reps), C.uint32_t(f), &pp)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_pingpong: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return PingPong{}, err
+	}
+	n := int(pp.n)
+	out := PingPong{N: n, RowMask: uint32(pp.row_mask), Trips: int(pp.trips), Reps: int(pp.reps),
+		Fenced: pp.fenced != 0, CallSeq: uint64(pp.call_seq), Ms: float64(pp.ms)}
+	out.Measured = make([]bool, n*n)
+	out.Status = make([]int32, n*n)
+	out.NsMin = make([]float32, n*n)
+	out.NsMedian = make([]float32, n*n)
+	out.NsMax = make([]float32, n*n)
+	out.Digest = make([]uint64, n*n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < n; j++ {
+			k := i*C.CDPROBE_MAX_GPUS + j
+			out.Measured[i*n+j] = pp.measured[k] != 0
+			out.Status[i*n+j] = int32(pp.status[k])
+			out.NsMin[i*n+j] = float32(pp.ns_min[k])
+			out.NsMedian[i*n+j] = float32(pp.ns_median[k])
+			out.NsMax[i*n+j] = float32(pp.ns_max[k])
+			out.Digest[i*n+j] = uint64(pp.digest[k])
 		}
 	}
 	return out, nil

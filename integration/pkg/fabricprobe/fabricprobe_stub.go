@@ -83,10 +83,26 @@ type Latency struct {
 	Ms                     float64
 }
 
+type PingPong struct {
+	N                      int
+	RowMask                uint32
+	Trips, Reps            int
+	Fenced                 bool
+	CallSeq                uint64
+	Measured               []bool
+	Status                 []int32
+	NsMin, NsMedian, NsMax []float32
+	Digest                 []uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
 	return Diagnosis{}, ErrUnsupported
 }
 func (*Probe) Latency(int, int) (Latency, error) { return Latency{}, ErrUnsupported }
-func (*Probe) Close()                            {}
+func (*Probe) PingPong(int, int, bool) (PingPong, error) {
+	return PingPong{}, ErrUnsupported
+}
+func (*Probe) Close() {}

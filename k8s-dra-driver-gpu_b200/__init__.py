@@ -17,6 +17,7 @@ from .fabricprobe import (  # noqa: F401
     Diagnosis,
     ErrUnsupported,
     Latency,
+    PingPong,
     Probe,
     ProbeError,
     Result,
@@ -26,4 +27,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Open", "gate", "plan", "topology"]

@@ -32,6 +32,7 @@ OPT_UNIDIRECTIONAL = 7
 OPT_WARMUP, OPT_WARMUP_BYTES, OPT_DEBUG_SKIP_RANK = 8, 9, 10
 OPT_CTAS_RANK, OPT_MIN_FRACTION_PPM, OPT_LINK_PEAK_MBPS, OPT_SOLO_RANK, OPT_ALL_RANK_BARRIERS = 11, 12, 13, 14, 15
 OPT_PAIR_BARRIERS = 16
+OPT_PINGPONG_FAULT = 17
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -39,6 +40,9 @@ DIAG_KIND_NAMES = ("flip", "zero", "displaced", "stale", "foreign")
 
 LATENCY_DEFAULT_HOPS, LATENCY_DEFAULT_REPS = 1024, 8
 LATENCY_MAX_HOPS, LATENCY_MAX_REPS = 1 << 20, 64
+
+PINGPONG_DEFAULT_TRIPS, PINGPONG_DEFAULT_REPS = 256, 8
+PINGPONG_MAX_TRIPS, PINGPONG_MAX_REPS = 1 << 16, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
 
@@ -246,6 +250,31 @@ class LatencyT(C.Structure):
     ]
 
 
+class PingPongT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("trips", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("fenced", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("measured", C.c_uint8 * _N2),
+        ("status", C.c_int32 * _N2),
+        ("ns_min", C.c_float * _N2),
+        ("ns_median", C.c_float * _N2),
+        ("ns_max", C.c_float * _N2),
+        ("digest", C.c_uint64 * _N2),
+        ("ms", C.c_double),
+    ]
+
+
+def pingpong_fault(initiator: int, target: int, trip: int) -> int:
+    """The CDPROBE_OPT_PINGPONG_FAULT value that arms a skip-ahead echo at `trip` of timed rep 1 of cell
+    (initiator, target)."""
+    return ((initiator + 1) << 32) | ((target + 1) << 16) | trip
+
+
 # Every symbol include/cdprobe.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "cdprobe_abi_version": (C.c_uint32, []),
@@ -266,6 +295,7 @@ SYMBOLS = {
                                   C.c_uint64, C.c_uint32, C.POINTER(C.c_double)]),
     "cdprobe_diagnose": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(DiagT)]),
     "cdprobe_latency": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(LatencyT)]),
+    "cdprobe_pingpong": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PingPongT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

@@ -30,6 +30,7 @@
 #include "../../include/cdprobe.h"
 #include "diagnose.h"
 #include "latency.h"
+#include "pingpong.h"
 #include "plan.h"
 #include "probe_launch.h"
 #include "probe_types.h"
@@ -74,6 +75,7 @@ struct LocalRank {
   void* diag_scratch = nullptr;  // cdprobe_diagnose: allocated on this rank's first diagnosis
   size_t diag_scratch_bytes = 0;
   LatencyRep* lat_scratch = nullptr;  // cdprobe_latency: allocated on this rank's first chase
+  PingPongRep* pp_scratch = nullptr;  // cdprobe_pingpong: allocated on this rank's first round trip
 };
 
 }  // namespace cdp
@@ -109,6 +111,8 @@ struct cdprobe {
   double last_probe_ms = 0.0;    // host wall clock of the previous run (wait_rows: how long to spin hot)
   uint32_t verify_ctas = 32;  // CTAs that verify landing slots under CDPROBE_FLAG_OVERLAP_VERIFY
   int32_t fault_local = -1;   // local rank whose Ctrl holds the armed landing fault (cdprobe_corrupt_landing), -1: none
+  uint64_t pp_calls = 0;      // cdprobe_pingpong calls that ran (call_seq of the last one)
+  uint64_t pp_fault = 0;      // CDPROBE_OPT_PINGPONG_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -411,6 +415,7 @@ static void destroy(cdprobe* h) {
     if (L.row) cudaFreeHost(L.row);
     if (L.diag_scratch) cudaFree(L.diag_scratch);
     if (L.lat_scratch) cudaFree(L.lat_scratch);
+    if (L.pp_scratch) cudaFree(L.pp_scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
     if (L.stream) cudaStreamDestroy(L.stream);
@@ -1101,6 +1106,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       if (value == 0 || value > 65535) return CDPROBE_ERR_ARG;
       h->verify_ctas = (uint32_t)value;
       return cdp::rebuild_all(h);
+    case CDPROBE_OPT_PINGPONG_FAULT:  // checked against the call's arguments by cdprobe_pingpong
+      h->pp_fault = value;
+      return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;
   }
@@ -1462,6 +1470,207 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
         if (digest != want[li][k]) st = CDPROBE_ERR_INTEGRITY;
       }
       out->status[idx] = st;
+    }
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+static_assert(sizeof(cdp::PingPongRep) == 24, "pingpong rep slot");
+
+// What each process contributes at the start of cdprobe_pingpong, so that every process refuses or runs the same call
+// over the same pair set (cdprobe_unmap_peer changes only the local view).
+struct PingPongAgree {
+  uint64_t call_seq;
+  uint32_t trips, reps, fenced, ok;
+  int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [local rank][rank]: mapping status, unmapped cells folded in
+};
+
+int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->trips = trips != 0 ? trips : cdp::kPingPongDefaultTrips;
+  out->reps = reps != 0 ? reps : cdp::kPingPongDefaultReps;
+  out->fenced = fenced;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  trips = out->trips;
+  reps = out->reps;
+  if (h->sticky) {
+    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
+    return CDPROBE_ERR_STATE;
+  }
+  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together
+  std::string bad;
+  if (trips > cdp::kPingPongMaxTrips || reps > cdp::kPingPongMaxReps || fenced > 1)
+    bad = "trips must be at most 1 << 16, reps at most 64 and fenced 0 or 1";
+  uint32_t f_init = cdp::kPingPongNoFault, f_target = cdp::kPingPongNoFault, f_trip = cdp::kPingPongNoFault;
+  if (h->pp_fault != 0) {
+    const uint64_t fi = h->pp_fault >> 32, ft = (h->pp_fault >> 16) & 0xffffu, trip = h->pp_fault & 0xffffu;
+    if (fi == 0 || ft == 0 || fi > n || ft > n || fi == ft) {
+      bad = "the armed pingpong fault names no off-diagonal cell";
+    } else if (trip + 1 >= trips || (reps == 1 && trip + 2 == trips)) {
+      // the initiator runs one trip ahead until the responder catches up; that must happen inside the leg
+      bad = "the armed pingpong fault's trip must be below trips - 1, and below trips - 2 when reps is 1";
+    } else {
+      f_init = (uint32_t)fi - 1;
+      f_target = (uint32_t)ft - 1;
+      f_trip = (uint32_t)trip;
+    }
+  }
+  PingPongAgree mine;
+  memset(&mine, 0, sizeof(mine));
+  mine.call_seq = h->pp_calls + 1;
+  mine.trips = trips;
+  mine.reps = reps;
+  mine.fenced = fenced;
+  mine.ok = bad.empty() ? 1u : 0u;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  memcpy(st, h->status, sizeof(st));
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::LocalRank& L = h->lr[li];
+    for (uint32_t j = 0; j < n; ++j) {
+      int32_t s = h->status[L.grank][j];
+      if (s == 0 && !L.mapped[j]) s = cdp::kStatusUnmapped;
+      st[L.grank][j] = mine.status[li][j] = s;
+    }
+  }
+  if (h->cfg.world_size > 1) {
+    std::vector<PingPongAgree> all(h->cfg.world_size);
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    for (uint32_t r = 0; r < h->cfg.world_size; ++r) {
+      const PingPongAgree& o = all[r];
+      if (!o.ok && bad.empty()) bad = "another process called cdprobe_pingpong with invalid arguments";
+      if ((o.call_seq != mine.call_seq || o.trips != trips || o.reps != reps || o.fenced != fenced) && bad.empty())
+        bad = "cdprobe_pingpong is collective: every process must call it with the same arguments";
+      for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], o.status[li], sizeof(st[0]));
+    }
+  }
+  if (!bad.empty()) {
+    cdp::set_err(bad);
+    return CDPROBE_ERR_ARG;
+  }
+  h->pp_calls = mine.call_seq;
+  out->call_seq = h->pp_calls;
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+  if (n == 1) {
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+  if (h->cfg.world_size > 1) {  // every process has agreed before any kernel polls a peer
+    std::string err;
+    if (h->rdv.barrier(&err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  // a pair is exchanged only when both directions are mapped; the status of its cells is the pair's mapping status
+  auto pair_status = [&](uint32_t i, uint32_t j) { return st[i][j] != 0 ? st[i][j] : st[j][i]; };
+
+  // 2. one block per local rank, every one launched before any is waited for
+  cdp::PingPongParams P[cdp::kMaxRanks];
+  bool launched[cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::PingPongParams& p = P[li];
+    memset(&p, 0, sizeof(p));
+    p.call_seq = h->pp_calls;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.n_rounds = pl.rounds;
+    p.trips = trips;
+    p.reps = reps;
+    p.fault_round = cdp::kPingPongNoFault;
+    p.fault_trip = f_trip;
+    for (uint32_t j = 0; j < n; ++j)
+      if (j != g) out->status[g * CDPROBE_MAX_GPUS + j] = pair_status(g, j);
+    uint32_t active = 0;
+    for (uint32_t r = 0; r < pl.rounds; ++r) {
+      const int q = pl.partner[r][g];
+      if (q < 0 || pair_status(g, (uint32_t)q) != 0) continue;
+      cdp::PingPongRound& R = p.round[r];
+      R.remote = reinterpret_cast<uint64_t*>(L.va[q] + cdp::kPingOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      R.local = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kPingOff + (uint64_t)q * sizeof(cdp::FlagLine));
+      R.partner = (uint32_t)q;
+      R.first = g < (uint32_t)q ? 1u : 0u;
+      if (g == f_target && (uint32_t)q == f_init) p.fault_round = r;
+      ++active;
+    }
+    if (active == 0) continue;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    if (L.pp_scratch == nullptr)
+      CDP_RT(cudaMalloc(&L.pp_scratch, sizeof(cdp::PingPongRep) * cdp::kMaxRanks * cdp::kPingPongRepSlots));
+    const cudaError_t e = (cudaError_t)cdp::pingpong_launch(p, fenced != 0, L.pp_scratch, L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch pingpong_kernel", e);
+    }
+    launched[li] = true;
+  }
+
+  // 3. while they run: the digest of a clean leg for every cell a local rank initiates
+  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // [local rank][round]
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t r = 0; r < pl.rounds; ++r) {
+      const cdp::PingPongRound& R = P[li].round[r];
+      if (R.remote == nullptr) continue;
+      const uint32_t leg = R.first ? 0u : 1u;
+      for (uint32_t rep = 0; rep <= reps; ++rep) want[li][r] ^= cdp::pingpong_rep_digest(h->pp_calls, r, leg, rep, trips);
+    }
+  }
+
+  // 4. collect: ns per round trip of the timed reps, the digest of all of them
+  std::vector<cdp::PingPongRep> got((size_t)cdp::kMaxRanks * cdp::kPingPongRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (!launched[li]) continue;
+    cdp::LocalRank& L = h->lr[li];
+    const cdp::PingPongParams& p = P[li];
+    cudaError_t e = cudaSetDevice(L.ordinal);
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(got.data(), L.pp_scratch, sizeof(cdp::PingPongRep) * p.n_rounds * cdp::kPingPongRepSlots,
+                          cudaMemcpyDeviceToHost, L.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;  // a failed kernel leaves the context unusable
+      return cdp::fail_cuda("cdprobe_pingpong", e);
+    }
+    for (uint32_t r = 0; r < p.n_rounds; ++r) {
+      const cdp::PingPongRound& R = p.round[r];
+      if (R.remote == nullptr) continue;
+      const uint32_t idx = L.grank * CDPROBE_MAX_GPUS + R.partner;
+      const cdp::PingPongRep* rep = got.data() + (size_t)r * cdp::kPingPongRepSlots;
+      uint64_t digest = 0;
+      int32_t s = 0;
+      float ns[cdp::kPingPongMaxReps];
+      for (uint32_t k = 0; k <= reps; ++k) {
+        digest ^= rep[k].digest;
+        if (rep[k].status == CDPROBE_ERR_TIMEOUT) {
+          s = CDPROBE_ERR_TIMEOUT;
+          break;
+        }
+        if (rep[k].status != 0) s = rep[k].status;
+        if (k > 0) ns[k - 1] = (float)((double)rep[k].ns / trips);
+      }
+      out->measured[idx] = 1;
+      out->digest[idx] = digest;
+      if (s != CDPROBE_ERR_TIMEOUT) {
+        std::sort(ns, ns + reps);
+        out->ns_min[idx] = ns[0];
+        out->ns_median[idx] = ns[reps / 2];
+        out->ns_max[idx] = ns[reps - 1];
+        if (digest != want[li][r]) s = CDPROBE_ERR_INTEGRITY;
+      }
+      out->status[idx] = s;
     }
   }
   out->ms = cdp::now_ms() - t_begin;

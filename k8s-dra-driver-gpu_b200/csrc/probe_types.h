@@ -350,4 +350,30 @@ inline uint64_t latency_rep_digest(uint64_t seed, uint32_t i, uint32_t j, uint64
   return digest;
 }
 
+// ---- the signal round trip (cdprobe_pingpong, DESIGN §5d) -----------------------------------------------------
+// One 128-byte line per sender after Ctrl in the Ctrl granule: ping[s] in rank o's memory holds the last word s sent
+// to o.  Open zeroes the whole granule; the reset after an aborted run zeroes only [grid_arrive, sizeof(Ctrl)), so
+// these lines are never touched by it, and cdprobe_pingpong touches no Ctrl word.
+constexpr uint64_t kPingOff = 64ull << 10;
+static_assert(sizeof(Ctrl) <= kPingOff && kPingOff % 128 == 0 && kPingOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the pingpong lines sit after Ctrl inside its granule");
+
+// A pingpong word.  Bits [0, 17): 2 * trip + echo; [17, 24): rep (0 = the warm-up); 24: leg; [25, 29): round;
+// [29, 64): call_seq.  Words rise strictly along (call, round, leg, rep, trip, echo), so a word of an earlier call,
+// round, leg, rep or trip never satisfies a wait for a later one.
+constexpr uint32_t kPingTripBits = 17, kPingRepShift = 17, kPingLegShift = 24, kPingRoundShift = 25, kPingCallShift = 29;
+CDP_HD inline uint64_t pingpong_word(uint64_t call_seq, uint32_t round, uint32_t leg, uint32_t rep, uint32_t trip,
+                                     uint32_t echo) {
+  return (call_seq << kPingCallShift) | ((uint64_t)round << kPingRoundShift) | ((uint64_t)leg << kPingLegShift) |
+         ((uint64_t)rep << kPingRepShift) | (uint64_t)(2u * trip + echo);
+}
+// Xor of the echo words trips 0 .. trips - 1 of one rep return: the initiator's digest of a clean rep.  The trip
+// field holds 2t + 1 below the rep's base, so the xor is base (when trips is odd) | the xor of 2t + 1 over t < trips.
+CDP_HD inline uint64_t pingpong_rep_digest(uint64_t call_seq, uint32_t round, uint32_t leg, uint32_t rep, uint32_t trips) {
+  const uint64_t base = pingpong_word(call_seq, round, leg, rep, 0, 0);
+  const uint64_t m = trips - 1u;  // xor of 0 .. m
+  const uint64_t x = (m & 3u) == 0 ? m : (m & 3u) == 1 ? 1 : (m & 3u) == 2 ? m + 1 : 0;
+  return ((trips & 1u) ? base : 0ull) | (x << 1) | (uint64_t)(trips & 1u);
+}
+
 }  // namespace cdp

@@ -242,6 +242,51 @@ class Latency:
         )
 
 
+@dataclasses.dataclass
+class PingPong:
+    """What cdprobe_pingpong measured: n x n matrices [initiator][target] of ns per signal round trip (min, median and
+    max over the timed reps) and the digest of the echo words the initiator received.  A cell that did not run (a row
+    of another process, the diagonal, a pair whose mapping is down) is None in every matrix but `status`; a cell that
+    passed timeout_ms has a digest but no times."""
+    n: int
+    row_mask: int
+    trips: int
+    reps: int
+    fenced: bool
+    call_seq: int
+    measured: List[List[bool]]
+    status: List[List[int]]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the pair's mapping status
+    ns_min: List[List[Optional[float]]]
+    ns_median: List[List[Optional[float]]]
+    ns_max: List[List[Optional[float]]]
+    digest: List[List[Optional[int]]]
+    ms: float
+    raw: abi.PingPongT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.PingPongT) -> "PingPong":
+        n = t.n
+
+        def mat(a, timed=False):
+            out = []
+            for i in range(n):
+                row = []
+                for j in range(n):
+                    k = i * abi.MAX_GPUS + j
+                    ok = t.measured[k] and not (timed and t.status[k] == abi.ERR_TIMEOUT)
+                    row.append(a[k] if ok else None)
+                out.append(row)
+            return out
+
+        return PingPong(
+            n=n, row_mask=t.row_mask, trips=t.trips, reps=t.reps, fenced=bool(t.fenced), call_seq=t.call_seq,
+            measured=[[bool(t.measured[i * abi.MAX_GPUS + j]) for j in range(n)] for i in range(n)],
+            status=[[t.status[i * abi.MAX_GPUS + j] for j in range(n)] for i in range(n)],
+            ns_min=mat(t.ns_min, True), ns_median=mat(t.ns_median, True), ns_max=mat(t.ns_max, True),
+            digest=mat(t.digest), ms=t.ms, raw=t,
+        )
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -373,6 +418,21 @@ class Probe:
         """The bare ABI call: (return code, abi.LatencyT as the library left it)."""
         t = abi.LatencyT()
         rc = self._lib.cdprobe_latency(self._h, hops, reps, C.byref(t))
+        return rc, t
+
+    def PingPong(self, trips: int = 0, reps: int = 0, fenced: bool = False) -> PingPong:
+        """Go: (*Probe).PingPong.  Signal round trip of every off-diagonal cell over the tournament's pairs (0: 256
+        round trips, 8 timed reps); fenced: a fence.sys before every store.  Collective when world_size > 1.  Needs no
+        Run first and disturbs none."""
+        rc, t = self.pingpong_raw(trips, reps, 1 if fenced else 0)
+        if rc != abi.OK:
+            _raise(self._lib, rc, "cdprobe_pingpong")
+        return PingPong.from_c(t)
+
+    def pingpong_raw(self, trips: int, reps: int, fenced: int):
+        """The bare ABI call: (return code, abi.PingPongT as the library left it)."""
+        t = abi.PingPongT()
+        rc = self._lib.cdprobe_pingpong(self._h, trips, reps, fenced, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
