@@ -1,4 +1,5 @@
-// handle.cc — the probe handle behind the C ABI (include/cdprobe.h).
+// handle.cc — the probe handle behind the C ABI (include/cdprobe.h): open and close, peer mappings, options, fault
+// hooks and the run path.  The on-demand measurements (diagnose, latency, pingpong) are in measure.cc.
 //
 // Who calls this: the compute-domain-daemon's `run()` owns one handle for the
 // life of the pod (reference: cmd/compute-domain-daemon/main.go:212-347; the
@@ -11,8 +12,6 @@
 // calling thread (a launch is ~4 us; the first device barrier absorbs the
 // skew) and then polls the pinned result rows the kernels write.  No thread
 // survives a call.
-#include <cuda.h>
-#include <cuda_runtime.h>
 #include <errno.h>
 #include <fcntl.h>
 #include <sched.h>
@@ -22,113 +21,15 @@
 #include <time.h>
 #include <unistd.h>
 
-#include <algorithm>
 #include <new>
 #include <string>
 #include <vector>
 
-#include "../../include/cdprobe.h"
-#include "diagnose.h"
-#include "latency.h"
-#include "pingpong.h"
-#include "plan.h"
+#include "handle.h"
 #include "probe_launch.h"
-#include "probe_types.h"
-#include "rendezvous.h"
 #include "schedule.h"
-#include "vmm.h"
 
 namespace cdp {
-
-thread_local std::string g_last_error;
-
-static void set_err(const std::string& s) { g_last_error = s; }
-
-static double now_ms() {
-  timespec ts;
-  clock_gettime(CLOCK_MONOTONIC, &ts);
-  return ts.tv_sec * 1e3 + ts.tv_nsec / 1e6;
-}
-
-constexpr int32_t kStatusUnmapped = CDPROBE_ERR_STATE;  // fault-injected / torn-down mapping
-
-struct LocalRank {
-  uint32_t grank = 0;
-  int ordinal = -1;
-  int sm_count = 0;
-  uint32_t ctas = 0;
-  bool coop = false;
-  bool mig = false;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int max_ctas = 0;
-  CUmemGenericAllocationHandle own = 0;
-  bool has_own = false;
-  int own_fd = -1;
-  CUdeviceptr va[kMaxRanks] = {};
-  bool mapped[kMaxRanks] = {};
-  ResultRow* row = nullptr;
-  char uuid[48] = {};
-  Phase phases[kMaxPhases];
-  uint32_t n_phases = 0;
-  uint32_t peer_mask = 0;
-  void* diag_scratch = nullptr;  // cdprobe_diagnose: allocated on this rank's first diagnosis
-  size_t diag_scratch_bytes = 0;
-  LatencyRep* lat_scratch = nullptr;  // cdprobe_latency: allocated on this rank's first chase
-  PingPongRep* pp_scratch = nullptr;  // cdprobe_pingpong: allocated on this rank's first round trip
-};
-
-}  // namespace cdp
-
-using namespace cdp;
-
-struct cdprobe {
-  cdprobe_config_t cfg;
-  Plan plan;
-  Driver drv;
-  Rendezvous rdv;
-  uint32_t n_total = 0, n_local = 0, first = 0;
-  uint32_t handle_type = 0;  // 0 none, 1 posix fd, 8 fabric
-  LocalRank lr[kMaxRanks];
-  CUmemGenericAllocationHandle imported[kMaxRanks] = {};
-  bool has_import[kMaxRanks] = {};
-  int32_t status[kMaxRanks][kMaxRanks];  // [issuer][owner] mapping status, all ranks
-  uint64_t launch_seq = 0;
-  uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
-  uint64_t seed = 0;
-  uint64_t src_sum[kMaxRanks][kMaxRanks] = {};
-  uint64_t src_xor[kMaxRanks][kMaxRanks] = {};
-  bool sticky = false;
-  bool event_timing = false;
-  uint32_t path = 0;          // 0 TMA bulk, 1 ld/st 128-bit, 2 ld/st 256-bit
-  uint32_t warm_mode = 1;     // 0 never, 1 auto (after an idle gap), 2 always
-  uint64_t warm_bytes = 8ull << 20;   // untimed wake-up prefix per rank
-  double warm_idle_ms = 5.0;  // auto: wake the links when the previous run ended longer ago than this
-  double last_run_end_ms = -1.0;
-  bool warm_now = false;
-  uint32_t debug_skip_rank = 0;  // 1-based local rank whose kernel is NOT launched (fault injection)
-  uint32_t solo_rank = 0;        // 1-based local rank that runs alone, no cross-GPU barrier (ncu captures)
-  double last_probe_ms = 0.0;    // host wall clock of the previous run (wait_rows: how long to spin hot)
-  uint32_t verify_ctas = 32;  // CTAs that verify landing slots under CDPROBE_FLAG_OVERLAP_VERIFY
-  int32_t fault_local = -1;   // local rank whose Ctrl holds the armed landing fault (cdprobe_corrupt_landing), -1: none
-  uint64_t pp_calls = 0;      // cdprobe_pingpong calls that ran (call_seq of the last one)
-  uint64_t pp_fault = 0;      // CDPROBE_OPT_PINGPONG_FAULT value, 0: disarmed
-  double open_ms = 0, fill_ms = 0;
-};
-
-namespace cdp {
-
-static int fail_cuda(const char* what, cudaError_t e) {
-  set_err(std::string(what) + ": " + cudaGetErrorName(e) + " (" + cudaGetErrorString(e) + ")");
-  if (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver || e == cudaErrorInitializationError ||
-      e == cudaErrorSystemDriverMismatch || e == cudaErrorSystemNotReady || e == cudaErrorNotSupported)
-    return CDPROBE_ERR_NO_DEVICE;
-  if (e == cudaErrorNoKernelImageForDevice || e == cudaErrorInvalidDeviceFunction ||
-      e == cudaErrorCooperativeLaunchTooLarge)
-    return CDPROBE_ERR_UNSUPPORTED;
-  if (e == cudaErrorMemoryAllocation) return CDPROBE_ERR_NOMEM;
-  return CDPROBE_ERR_CUDA;
-}
 
 static int fail_drv(const cdprobe* h, const char* what, CUresult r) {
   set_err(std::string(what) + ": " + h->drv.error_name(r));
@@ -136,12 +37,6 @@ static int fail_drv(const cdprobe* h, const char* what, CUresult r) {
   if (r == CUDA_ERROR_NOT_SUPPORTED) return CDPROBE_ERR_UNSUPPORTED;
   return CDPROBE_ERR_CUDA;
 }
-
-#define CDP_RT(call)                                       \
-  do {                                                     \
-    cudaError_t e_ = (call);                               \
-    if (e_ != cudaSuccess) return cdp::fail_cuda(#call, e_);    \
-  } while (0)
 
 static void format_uuid(const cudaUUID_t& u, bool mig, char out[48]) {
   const unsigned char* b = reinterpret_cast<const unsigned char*>(u.bytes);
@@ -226,6 +121,18 @@ static int rebuild_all(cdprobe* h) {
     if (rc != CDPROBE_OK) return rc;
   }
   return CDPROBE_OK;
+}
+
+// Sets or clears one schedule flag and rebuilds every phase table; on failure the old flags and tables come back.
+static int set_flag(cdprobe* h, uint32_t flag, bool on) {
+  const uint32_t old = h->cfg.flags;
+  h->cfg.flags = (old & ~flag) | (on ? flag : 0u);
+  const int rc = rebuild_all(h);
+  if (rc != CDPROBE_OK) {
+    h->cfg.flags = old;
+    rebuild_all(h);
+  }
+  return rc;
 }
 
 static void fill_params(const cdprobe* h, uint32_t li, const Phase* phases, uint32_t n_phases, uint32_t peer_mask,
@@ -413,9 +320,7 @@ static void destroy(cdprobe* h) {
     if (L.has_own) h->drv.MemRelease(L.own);
     if (L.own_fd >= 0) ::close(L.own_fd);
     if (L.row) cudaFreeHost(L.row);
-    if (L.diag_scratch) cudaFree(L.diag_scratch);
-    if (L.lat_scratch) cudaFree(L.lat_scratch);
-    if (L.pp_scratch) cudaFree(L.pp_scratch);
+    if (L.scratch) cudaFree(L.scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
     if (L.stream) cudaStreamDestroy(L.stream);
@@ -822,10 +727,7 @@ int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out) {
   out->n = h->n_total;
   out->bytes_per_pair = h->plan.bpp;
   out->rounds = h->plan.rounds;
-  if (h->sticky) {
-    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
-    return CDPROBE_ERR_STATE;
-  }
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   const double t0 = cdp::now_ms();
   h->launch_seq++;
   h->last_run_seq = h->launch_seq;
@@ -1028,49 +930,13 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       h->cfg.timeout_ms = (uint32_t)value;
       return CDPROBE_OK;
     case CDPROBE_OPT_OVERLAP_VERIFY:
-    {
-      const uint32_t old = h->cfg.flags;
-      h->cfg.flags = (h->cfg.flags & ~CDPROBE_FLAG_OVERLAP_VERIFY) | (value ? CDPROBE_FLAG_OVERLAP_VERIFY : 0u);
-      const int rc = cdp::rebuild_all(h);
-      if (rc != CDPROBE_OK) {
-        h->cfg.flags = old;
-        cdp::rebuild_all(h);
-      }
-      return rc;
-    }
+      return cdp::set_flag(h, CDPROBE_FLAG_OVERLAP_VERIFY, value != 0);
     case CDPROBE_OPT_UNIDIRECTIONAL:
-    {
-      const uint32_t old = h->cfg.flags;
-      h->cfg.flags = (h->cfg.flags & ~CDPROBE_FLAG_UNIDIRECTIONAL) | (value ? CDPROBE_FLAG_UNIDIRECTIONAL : 0u);
-      const int rc = cdp::rebuild_all(h);
-      if (rc != CDPROBE_OK) {
-        h->cfg.flags = old;
-        cdp::rebuild_all(h);
-      }
-      return rc;
-    }
+      return cdp::set_flag(h, CDPROBE_FLAG_UNIDIRECTIONAL, value != 0);
     case CDPROBE_OPT_ALL_RANK_BARRIERS:
-    {
-      const uint32_t old = h->cfg.flags;
-      h->cfg.flags = (h->cfg.flags & ~CDPROBE_FLAG_ALL_RANK_BARRIERS) | (value ? CDPROBE_FLAG_ALL_RANK_BARRIERS : 0u);
-      const int rc = cdp::rebuild_all(h);
-      if (rc != CDPROBE_OK) {
-        h->cfg.flags = old;
-        cdp::rebuild_all(h);
-      }
-      return rc;
-    }
+      return cdp::set_flag(h, CDPROBE_FLAG_ALL_RANK_BARRIERS, value != 0);
     case CDPROBE_OPT_PAIR_BARRIERS:
-    {
-      const uint32_t old = h->cfg.flags;
-      h->cfg.flags = (h->cfg.flags & ~CDPROBE_FLAG_PAIR_BARRIERS) | (value ? CDPROBE_FLAG_PAIR_BARRIERS : 0u);
-      const int rc = cdp::rebuild_all(h);
-      if (rc != CDPROBE_OK) {
-        h->cfg.flags = old;
-        cdp::rebuild_all(h);
-      }
-      return rc;
-    }
+      return cdp::set_flag(h, CDPROBE_FLAG_PAIR_BARRIERS, value != 0);
     case CDPROBE_OPT_CTAS_RANK:
     {
       const uint32_t li = (uint32_t)(value >> 16), c = (uint32_t)(value & 0xffffu);
@@ -1128,7 +994,7 @@ int cdprobe_remap_peer(cdprobe_t* h, uint32_t local, uint32_t peer) {
   if (h == nullptr || local >= h->n_local || peer >= h->n_total) return CDPROBE_ERR_ARG;
   const uint32_t g = h->lr[local].grank;
   if (peer == g) return CDPROBE_ERR_ARG;
-  if (h->sticky) return CDPROBE_ERR_STATE;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   cdp::unmap_peer(h, local, peer);
   const int32_t st = cdp::map_peer(h, local, peer);
   if (st != 0 && h->cfg.world_size > 1) {
@@ -1181,11 +1047,8 @@ int cdprobe_corrupt_landing(cdprobe_t* h, uint32_t local, uint32_t target, uint3
     cdp::set_err("cell (i, i) exists only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG)");
     return CDPROBE_ERR_ARG;
   }
-  if (h->sticky) {
-    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
-    return CDPROBE_ERR_STATE;
-  }
-  if (n > 0 && (h->status[g][target] != 0 || !h->lr[local].mapped[target])) {
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  if (n > 0 && cdp::cell_status(h, local, target) != 0) {
     cdp::set_err("the issuer does not map the target");
     return CDPROBE_ERR_STATE;
   }
@@ -1210,7 +1073,7 @@ int cdprobe_ce_copy(cdprobe_t* h, uint32_t n_copies, const uint32_t* local, cons
   if (h == nullptr || local == nullptr || peer == nullptr || ms_out == nullptr || n_copies == 0 ||
       n_copies > h->n_local || reps == 0 || reps > 1024)
     return CDPROBE_ERR_ARG;
-  if (h->sticky) return CDPROBE_ERR_STATE;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   const cdp::Plan& pl = h->plan;
   uint64_t nb = bytes;
   if (nb == 0 || nb > pl.src_bytes) nb = pl.src_bytes;
@@ -1256,424 +1119,6 @@ int cdprobe_gate(const cdprobe_config_t* cfg, uint32_t n_total, float* gate_read
   if (rc != CDPROBE_OK) return rc;
   *gate_read_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, true);
   *gate_write_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, false);
-  return CDPROBE_OK;
-}
-
-static_assert(CDPROBE_DIAG_FLIP == cdp::kDiagFlip && CDPROBE_DIAG_ZERO == cdp::kDiagZero &&
-                  CDPROBE_DIAG_DISPLACED == cdp::kDiagDisplaced && CDPROBE_DIAG_STALE == cdp::kDiagStale &&
-                  CDPROBE_DIAG_FOREIGN == cdp::kDiagForeign && CDPROBE_DIAG_SAMPLES == cdp::kDiagSamples,
-              "diagnosis classes");
-static_assert(sizeof(cdp::DiagSample) == sizeof(cdprobe_diag_sample_t) &&
-                  offsetof(cdp::DiagSample, run_seq) == offsetof(cdprobe_diag_sample_t, run_seq) &&
-                  offsetof(cdp::DiagSample, rank) == offsetof(cdprobe_diag_sample_t, rank),
-              "the kernel writes samples in the ABI layout");
-
-int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target, uint32_t reader, cdprobe_diag_t* out) {
-  cdp::g_last_error.clear();
-  if (h == nullptr || out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
-  out->op = op;
-  out->issuer = issuer;
-  out->target = target;
-  out->reader = reader;
-  out->first_bad = UINT64_MAX;
-  const cdp::Plan& pl = h->plan;
-  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE) {
-    cdp::set_err("op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE");
-    return CDPROBE_ERR_ARG;
-  }
-  if (issuer >= h->n_total || target >= h->n_total || reader >= h->n_total) {
-    cdp::set_err("rank out of range");
-    return CDPROBE_ERR_ARG;
-  }
-  if (issuer == target && !pl.diag) {
-    cdp::set_err("cell (i, i) exists only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG)");
-    return CDPROBE_ERR_ARG;
-  }
-  if (reader < h->first || reader >= h->first + h->n_local) {
-    cdp::set_err("reader is not a rank of this process");
-    return CDPROBE_ERR_ARG;
-  }
-  if (h->sticky) {
-    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
-    return CDPROBE_ERR_STATE;
-  }
-  if (h->last_run_seq == 0) {
-    cdp::set_err("no cdprobe_run yet: there is no pattern to compare with");
-    return CDPROBE_ERR_STATE;
-  }
-  cdp::LocalRank& L = h->lr[reader - h->first];
-  if (h->status[reader][target] != 0 || !L.mapped[target]) {  // never read through a mapping that is down
-    cdp::set_err("reader does not map the target");
-    return CDPROBE_ERR_STATE;
-  }
-  const uint64_t run_seq = h->last_run_seq;
-  out->run_seq = run_seq;
-  out->region_offset = cdp::cell_offset(pl, op, issuer, target);
-  out->bytes = pl.bpp;
-
-  const cdp::DiagSpec s =
-      op == CDPROBE_OP_WRITE
-          ? cdp::diag_write_spec(h->seed, h->n_total, issuer, target, run_seq, pl.bpp / 8)
-          : cdp::diag_read_spec(h->seed, h->n_total, target, (uint64_t)cdp::cell_slice(pl, issuer, target) * (pl.bpp / 8),
-                                pl.bpp / 8, pl.src_bytes / 8);
-
-  CDP_RT(cudaSetDevice(L.ordinal));
-  const size_t need = cdp::diag_scratch_bytes(pl.bpp);
-  if (L.diag_scratch_bytes < need) {
-    if (L.diag_scratch) cudaFree(L.diag_scratch);
-    L.diag_scratch = nullptr;
-    L.diag_scratch_bytes = 0;
-    CDP_RT(cudaMalloc(&L.diag_scratch, need));
-    L.diag_scratch_bytes = need;
-  }
-  const uint8_t* region = reinterpret_cast<const uint8_t*>(L.va[target]) + out->region_offset;
-  cdp::DiagOut d;
-  float ms = 0.f;
-  cudaError_t e = cudaEventRecord(L.ev0, L.stream);
-  if (e == cudaSuccess) e = (cudaError_t)cdp::diag_launch(region, s, L.diag_scratch, L.sm_count, L.stream);
-  if (e == cudaSuccess) e = cudaEventRecord(L.ev1, L.stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&d, L.diag_scratch, sizeof(d), cudaMemcpyDeviceToHost, L.stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L.ev0, L.ev1);
-  if (e != cudaSuccess) {
-    h->sticky = true;  // a failed kernel leaves the context unusable
-    return cdp::fail_cuda("cdprobe_diagnose", e);
-  }
-  out->ms = ms;
-  out->bad_words = d.bad_words;
-  out->bad_granules = d.bad_granules;
-  out->zero_words = d.kind_count[cdp::kDiagZero];
-  if (d.bad_words) {
-    out->first_bad = ~d.first_bad_n;
-    out->last_bad = d.last_bad;
-  }
-  for (int k = 0; k < cdp::kDiagKinds; ++k) out->kind_count[k] = d.kind_count[k];
-  for (int b = 0; b < 64; ++b) out->bit_flips[b] = d.bit_flips[b];
-  out->n_samples = d.bad_words < (uint64_t)CDPROBE_DIAG_SAMPLES ? (uint32_t)d.bad_words : (uint32_t)CDPROBE_DIAG_SAMPLES;
-  memcpy(out->sample, d.sample, sizeof(out->sample[0]) * out->n_samples);
-  return CDPROBE_OK;
-}
-
-static_assert(sizeof(cdp::LatencyRep) == 24, "latency rep slot");
-
-int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
-  out->hops = hops != 0 ? hops : cdp::kLatencyDefaultHops;
-  out->reps = reps != 0 ? reps : cdp::kLatencyDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
-  const cdp::Plan& pl = h->plan;
-  out->n = h->n_total;
-  out->region_bytes = pl.bpp;
-  if (out->hops > cdp::kLatencyMaxHops || out->reps > cdp::kLatencyMaxReps) {
-    cdp::set_err("hops must be at most 1 << 20 and reps at most 64");
-    return CDPROBE_ERR_ARG;
-  }
-  if (h->sticky) {
-    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
-    return CDPROBE_ERR_STATE;
-  }
-  hops = out->hops;
-  reps = out->reps;
-  const uint64_t lines = pl.bpp / (cdp::kLineWords * 8);
-
-  // 1. every local issuer's chases, all launched before any is waited for
-  cdp::LatencyParams P[cdp::kMaxRanks];
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    out->row_mask |= 1u << g;
-    cdp::LatencyParams& p = P[li];
-    memset(&p, 0, sizeof(p));
-    p.seed = h->seed;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
-    p.hops = hops;
-    p.reps = reps;
-    for (uint32_t j = 0; j < h->n_total; ++j) {
-      if (j == g && !pl.diag) continue;  // no loop-back slice to chase
-      const uint32_t idx = g * CDPROBE_MAX_GPUS + j;
-      if (h->status[g][j] != 0 || !L.mapped[j]) {  // never read through a mapping that is down
-        out->status[idx] = h->status[g][j] != 0 ? h->status[g][j] : cdp::kStatusUnmapped;
-        continue;
-      }
-      cdp::LatencyCell& c = p.cell[p.n_cells++];
-      c.region = reinterpret_cast<const uint8_t*>(L.va[j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
-      c.lines = lines;
-      c.issuer = g;
-      c.target = j;
-    }
-    if (p.n_cells == 0) continue;
-    CDP_RT(cudaSetDevice(L.ordinal));
-    if (L.lat_scratch == nullptr)
-      CDP_RT(cudaMalloc(&L.lat_scratch, sizeof(cdp::LatencyRep) * cdp::kMaxRanks * cdp::kLatencyRepSlots));
-    const cudaError_t e = (cudaError_t)cdp::latency_launch(p, L.lat_scratch, L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch latency_kernel", e);
-    }
-  }
-
-  // 2. while they run: the digest each chase gives over an intact region
-  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    for (uint32_t k = 0; k < P[li].n_cells; ++k) {
-      const cdp::LatencyCell& c = P[li].cell[k];
-      const uint64_t first = (uint64_t)cdp::cell_slice(pl, c.issuer, c.target) * (pl.bpp / 8);
-      for (uint32_t r = 0; r <= reps; ++r)
-        want[li][k] ^= cdp::latency_rep_digest(h->seed, c.issuer, c.target, first, lines, r, hops);
-    }
-  }
-
-  // 3. collect: ns per hop of the timed reps, the digest of all of them
-  std::vector<cdp::LatencyRep> got((size_t)cdp::kMaxRanks * cdp::kLatencyRepSlots);
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    const cdp::LatencyParams& p = P[li];
-    if (p.n_cells == 0) continue;
-    cdp::LocalRank& L = h->lr[li];
-    cudaError_t e = cudaSetDevice(L.ordinal);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(got.data(), L.lat_scratch, sizeof(cdp::LatencyRep) * p.n_cells * cdp::kLatencyRepSlots,
-                          cudaMemcpyDeviceToHost, L.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;  // a failed kernel leaves the context unusable
-      return cdp::fail_cuda("cdprobe_latency", e);
-    }
-    for (uint32_t k = 0; k < p.n_cells; ++k) {
-      const uint32_t idx = p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target;
-      const cdp::LatencyRep* rep = got.data() + (size_t)k * cdp::kLatencyRepSlots;
-      uint64_t digest = 0;
-      int32_t st = 0;
-      float ns[cdp::kLatencyMaxReps];
-      for (uint32_t r = 0; r <= reps; ++r) {
-        digest ^= rep[r].digest;
-        if (rep[r].status != 0) {
-          st = rep[r].status;
-          break;
-        }
-        if (r > 0) ns[r - 1] = (float)((double)rep[r].ns / hops);
-      }
-      out->measured[idx] = 1;
-      out->digest[idx] = digest;
-      if (st == 0) {
-        std::sort(ns, ns + reps);
-        out->ns_min[idx] = ns[0];
-        out->ns_median[idx] = ns[reps / 2];
-        out->ns_max[idx] = ns[reps - 1];
-        if (digest != want[li][k]) st = CDPROBE_ERR_INTEGRITY;
-      }
-      out->status[idx] = st;
-    }
-  }
-  out->ms = cdp::now_ms() - t_begin;
-  return CDPROBE_OK;
-}
-
-static_assert(sizeof(cdp::PingPongRep) == 24, "pingpong rep slot");
-
-// What each process contributes at the start of cdprobe_pingpong, so that every process refuses or runs the same call
-// over the same pair set (cdprobe_unmap_peer changes only the local view).
-struct PingPongAgree {
-  uint64_t call_seq;
-  uint32_t trips, reps, fenced, ok;
-  int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [local rank][rank]: mapping status, unmapped cells folded in
-};
-
-int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
-  out->trips = trips != 0 ? trips : cdp::kPingPongDefaultTrips;
-  out->reps = reps != 0 ? reps : cdp::kPingPongDefaultReps;
-  out->fenced = fenced;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
-  const cdp::Plan& pl = h->plan;
-  const uint32_t n = h->n_total;
-  out->n = n;
-  trips = out->trips;
-  reps = out->reps;
-  if (h->sticky) {
-    cdp::set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
-    return CDPROBE_ERR_STATE;
-  }
-  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together
-  std::string bad;
-  if (trips > cdp::kPingPongMaxTrips || reps > cdp::kPingPongMaxReps || fenced > 1)
-    bad = "trips must be at most 1 << 16, reps at most 64 and fenced 0 or 1";
-  uint32_t f_init = cdp::kPingPongNoFault, f_target = cdp::kPingPongNoFault, f_trip = cdp::kPingPongNoFault;
-  if (h->pp_fault != 0) {
-    const uint64_t fi = h->pp_fault >> 32, ft = (h->pp_fault >> 16) & 0xffffu, trip = h->pp_fault & 0xffffu;
-    if (fi == 0 || ft == 0 || fi > n || ft > n || fi == ft) {
-      bad = "the armed pingpong fault names no off-diagonal cell";
-    } else if (trip + 1 >= trips || (reps == 1 && trip + 2 == trips)) {
-      // the initiator runs one trip ahead until the responder catches up; that must happen inside the leg
-      bad = "the armed pingpong fault's trip must be below trips - 1, and below trips - 2 when reps is 1";
-    } else {
-      f_init = (uint32_t)fi - 1;
-      f_target = (uint32_t)ft - 1;
-      f_trip = (uint32_t)trip;
-    }
-  }
-  PingPongAgree mine;
-  memset(&mine, 0, sizeof(mine));
-  mine.call_seq = h->pp_calls + 1;
-  mine.trips = trips;
-  mine.reps = reps;
-  mine.fenced = fenced;
-  mine.ok = bad.empty() ? 1u : 0u;
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  memcpy(st, h->status, sizeof(st));
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    const cdp::LocalRank& L = h->lr[li];
-    for (uint32_t j = 0; j < n; ++j) {
-      int32_t s = h->status[L.grank][j];
-      if (s == 0 && !L.mapped[j]) s = cdp::kStatusUnmapped;
-      st[L.grank][j] = mine.status[li][j] = s;
-    }
-  }
-  if (h->cfg.world_size > 1) {
-    std::vector<PingPongAgree> all(h->cfg.world_size);
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    for (uint32_t r = 0; r < h->cfg.world_size; ++r) {
-      const PingPongAgree& o = all[r];
-      if (!o.ok && bad.empty()) bad = "another process called cdprobe_pingpong with invalid arguments";
-      if ((o.call_seq != mine.call_seq || o.trips != trips || o.reps != reps || o.fenced != fenced) && bad.empty())
-        bad = "cdprobe_pingpong is collective: every process must call it with the same arguments";
-      for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], o.status[li], sizeof(st[0]));
-    }
-  }
-  if (!bad.empty()) {
-    cdp::set_err(bad);
-    return CDPROBE_ERR_ARG;
-  }
-  h->pp_calls = mine.call_seq;
-  out->call_seq = h->pp_calls;
-  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
-  if (n == 1) {
-    out->ms = cdp::now_ms() - t_begin;
-    return CDPROBE_OK;
-  }
-  if (h->cfg.world_size > 1) {  // every process has agreed before any kernel polls a peer
-    std::string err;
-    if (h->rdv.barrier(&err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-  }
-  // a pair is exchanged only when both directions are mapped; the status of its cells is the pair's mapping status
-  auto pair_status = [&](uint32_t i, uint32_t j) { return st[i][j] != 0 ? st[i][j] : st[j][i]; };
-
-  // 2. one block per local rank, every one launched before any is waited for
-  cdp::PingPongParams P[cdp::kMaxRanks];
-  bool launched[cdp::kMaxRanks] = {};
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    cdp::PingPongParams& p = P[li];
-    memset(&p, 0, sizeof(p));
-    p.call_seq = h->pp_calls;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
-    p.n_rounds = pl.rounds;
-    p.trips = trips;
-    p.reps = reps;
-    p.fault_round = cdp::kPingPongNoFault;
-    p.fault_trip = f_trip;
-    for (uint32_t j = 0; j < n; ++j)
-      if (j != g) out->status[g * CDPROBE_MAX_GPUS + j] = pair_status(g, j);
-    uint32_t active = 0;
-    for (uint32_t r = 0; r < pl.rounds; ++r) {
-      const int q = pl.partner[r][g];
-      if (q < 0 || pair_status(g, (uint32_t)q) != 0) continue;
-      cdp::PingPongRound& R = p.round[r];
-      R.remote = reinterpret_cast<uint64_t*>(L.va[q] + cdp::kPingOff + (uint64_t)g * sizeof(cdp::FlagLine));
-      R.local = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kPingOff + (uint64_t)q * sizeof(cdp::FlagLine));
-      R.partner = (uint32_t)q;
-      R.first = g < (uint32_t)q ? 1u : 0u;
-      if (g == f_target && (uint32_t)q == f_init) p.fault_round = r;
-      ++active;
-    }
-    if (active == 0) continue;
-    CDP_RT(cudaSetDevice(L.ordinal));
-    if (L.pp_scratch == nullptr)
-      CDP_RT(cudaMalloc(&L.pp_scratch, sizeof(cdp::PingPongRep) * cdp::kMaxRanks * cdp::kPingPongRepSlots));
-    const cudaError_t e = (cudaError_t)cdp::pingpong_launch(p, fenced != 0, L.pp_scratch, L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch pingpong_kernel", e);
-    }
-    launched[li] = true;
-  }
-
-  // 3. while they run: the digest of a clean leg for every cell a local rank initiates
-  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // [local rank][round]
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    for (uint32_t r = 0; r < pl.rounds; ++r) {
-      const cdp::PingPongRound& R = P[li].round[r];
-      if (R.remote == nullptr) continue;
-      const uint32_t leg = R.first ? 0u : 1u;
-      for (uint32_t rep = 0; rep <= reps; ++rep) want[li][r] ^= cdp::pingpong_rep_digest(h->pp_calls, r, leg, rep, trips);
-    }
-  }
-
-  // 4. collect: ns per round trip of the timed reps, the digest of all of them
-  std::vector<cdp::PingPongRep> got((size_t)cdp::kMaxRanks * cdp::kPingPongRepSlots);
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    if (!launched[li]) continue;
-    cdp::LocalRank& L = h->lr[li];
-    const cdp::PingPongParams& p = P[li];
-    cudaError_t e = cudaSetDevice(L.ordinal);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(got.data(), L.pp_scratch, sizeof(cdp::PingPongRep) * p.n_rounds * cdp::kPingPongRepSlots,
-                          cudaMemcpyDeviceToHost, L.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;  // a failed kernel leaves the context unusable
-      return cdp::fail_cuda("cdprobe_pingpong", e);
-    }
-    for (uint32_t r = 0; r < p.n_rounds; ++r) {
-      const cdp::PingPongRound& R = p.round[r];
-      if (R.remote == nullptr) continue;
-      const uint32_t idx = L.grank * CDPROBE_MAX_GPUS + R.partner;
-      const cdp::PingPongRep* rep = got.data() + (size_t)r * cdp::kPingPongRepSlots;
-      uint64_t digest = 0;
-      int32_t s = 0;
-      float ns[cdp::kPingPongMaxReps];
-      for (uint32_t k = 0; k <= reps; ++k) {
-        digest ^= rep[k].digest;
-        if (rep[k].status == CDPROBE_ERR_TIMEOUT) {
-          s = CDPROBE_ERR_TIMEOUT;
-          break;
-        }
-        if (rep[k].status != 0) s = rep[k].status;
-        if (k > 0) ns[k - 1] = (float)((double)rep[k].ns / trips);
-      }
-      out->measured[idx] = 1;
-      out->digest[idx] = digest;
-      if (s != CDPROBE_ERR_TIMEOUT) {
-        std::sort(ns, ns + reps);
-        out->ns_min[idx] = ns[0];
-        out->ns_median[idx] = ns[reps / 2];
-        out->ns_max[idx] = ns[reps - 1];
-        if (digest != want[li][r]) s = CDPROBE_ERR_INTEGRITY;
-      }
-      out->status[idx] = s;
-    }
-  }
-  out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
 

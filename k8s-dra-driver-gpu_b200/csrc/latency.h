@@ -4,14 +4,13 @@
 #include <stdint.h>
 
 #include "probe_types.h"
+#include "timed_rep.cuh"
 
 namespace cdp {
 
 constexpr uint32_t kLatencyDefaultHops = 1024;
 constexpr uint32_t kLatencyDefaultReps = 8;
 constexpr uint32_t kLatencyMaxHops = 1u << 20;
-constexpr uint32_t kLatencyMaxReps = 64;              // timed reps; one untimed warm-up rep runs before them
-constexpr uint32_t kLatencyRepSlots = kLatencyMaxReps + 1;
 
 struct LatencyCell {
   const uint8_t* region;  // the source slice the issuer reads, through the issuer's mapping of the target
@@ -26,14 +25,8 @@ struct LatencyParams {
   uint32_t n_cells, hops, reps; // reps: timed reps (rep 0, the warm-up, comes on top)
 };
 
-struct LatencyRep {             // what the kernel leaves per cell and rep, at [cell * kLatencyRepSlots + rep]
-  unsigned long long ns;        // %globaltimer: last load returned - chase started
-  unsigned long long digest;    // xor of the words this rep loaded
-  int32_t status;               // 0, or CDPROBE_ERR_TIMEOUT (the chase stopped; later reps did not run)
-  uint32_t pad;
-};
-
-// Enqueues the chases of p.n_cells cells on `stream`.  Returns a cudaError_t.
-int latency_launch(const LatencyParams& p, LatencyRep* out, cudaStream_t stream);
+// Enqueues the chases of p.n_cells cells on `stream`; cell k leaves its reps at out[k * kRepSlots + rep], each with a
+// status of 0 or CDPROBE_ERR_TIMEOUT.  Returns a cudaError_t.
+int latency_launch(const LatencyParams& p, TimedRep* out, cudaStream_t stream);
 
 }  // namespace cdp

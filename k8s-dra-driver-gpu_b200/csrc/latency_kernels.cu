@@ -22,25 +22,10 @@ __device__ __forceinline__ uint64_t ld_relaxed_sys(const uint8_t* p) {
   asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ uint64_t globaltimer() {
-  uint64_t t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
-  return t;
-}
-// The closing timer read.  `v`, the last loaded word, is an operand, so the compiler cannot place the read ahead of
-// the load.  In the SASS the read follows the loop body, whose xor of v into the digest waits for the load, and
-// instructions issue in order: the read cannot issue before the last load has returned
-// (tests/test_latency_cpu.py checks that order in the compiled kernel).
-__device__ __forceinline__ uint64_t globaltimer_after(uint64_t v) {
-  uint64_t t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) : "l"(v) : "memory");
-  return t;
-}
-
-__global__ void __launch_bounds__(32) latency_kernel(const __grid_constant__ LatencyParams p, LatencyRep* out) {
+__global__ void __launch_bounds__(32) latency_kernel(const __grid_constant__ LatencyParams p, TimedRep* out) {
   if (threadIdx.x != 0) return;
   const LatencyCell c = p.cell[blockIdx.x];
-  LatencyRep* o = out + (size_t)blockIdx.x * kLatencyRepSlots;
+  TimedRep* o = out + (size_t)blockIdx.x * kRepSlots;
   const uint64_t deadline = globaltimer() + p.timeout_ns;
   for (uint32_t r = 0; r <= p.reps; ++r) {
     uint64_t line = latency_start(p.seed, c.issuer, c.target, r, c.lines);
@@ -66,7 +51,7 @@ __global__ void __launch_bounds__(32) latency_kernel(const __grid_constant__ Lat
 
 }  // namespace
 
-int latency_launch(const LatencyParams& p, LatencyRep* out, cudaStream_t stream) {
+int latency_launch(const LatencyParams& p, TimedRep* out, cudaStream_t stream) {
   if (p.n_cells == 0) return (int)cudaSuccess;
   latency_kernel<<<p.n_cells, 32, 0, stream>>>(p, out);
   return (int)cudaGetLastError();

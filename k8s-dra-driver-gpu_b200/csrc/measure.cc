@@ -1,0 +1,423 @@
+// measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency and cdprobe_pingpong.
+// Each runs on the local ranks' own streams, between probe runs, and has its results on the host before it returns.
+#include <string.h>
+
+#include <algorithm>
+#include <string>
+#include <vector>
+
+#include "diagnose.h"
+#include "handle.h"
+#include "latency.h"
+#include "pingpong.h"
+
+namespace cdp {
+
+// Grows local rank L's scratch to at least `bytes`, on its device (the caller has selected it); the old buffer is freed
+// first.  The measurements share it: each runs on L's one stream, copies its results out before it returns, and reads
+// back only what its own kernels wrote in the same call.  diag_launch clears its DiagOut and the compare pass writes
+// every granule count; a rep table is read up to its first TIMEOUT slot, and the kernels write one for every cell they
+// leave unfinished.
+static int ensure_scratch(LocalRank& L, size_t bytes) {
+  if (L.scratch_bytes >= bytes) return CDPROBE_OK;
+  if (L.scratch) cudaFree(L.scratch);
+  L.scratch = nullptr;
+  L.scratch_bytes = 0;
+  CDP_RT(cudaMalloc(&L.scratch, bytes));
+  L.scratch_bytes = bytes;
+  return CDPROBE_OK;
+}
+
+// Grows every local rank's scratch to hold its rep tables before any kernel is launched.  cudaFree synchronizes the
+// device, and local ranks may share one: a pingpong kernel launched for an earlier rank would wait on this rank's.
+static int ensure_rep_tables(cdprobe* h) {
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    CDP_RT(cudaSetDevice(h->lr[li].ordinal));
+    const int rc = ensure_scratch(h->lr[li], sizeof(TimedRep) * kMaxRanks * kRepSlots);
+    if (rc != CDPROBE_OK) return rc;
+  }
+  return CDPROBE_OK;
+}
+
+// Copies local rank L's first `cells` rep tables to `got` once its kernel is done.
+static int fetch_reps(cdprobe* h, LocalRank& L, uint32_t cells, TimedRep* got, const char* what) {
+  cudaError_t e = cudaSetDevice(L.ordinal);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(got, L.scratch, sizeof(TimedRep) * cells * kRepSlots, cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+  if (e != cudaSuccess) {
+    h->sticky = true;  // a failed kernel leaves the context unusable
+    return fail_cuda(what, e);
+  }
+  return CDPROBE_OK;
+}
+
+// Fills cell idx of a cdprobe_latency_t or cdprobe_pingpong_t from its rep table: the warm-up rep, then `reps` timed
+// reps of `per_rep` hops or round trips each.  The digest covers every rep that ran; a CDPROBE_ERR_TIMEOUT rep ends the
+// cell, which then has no times.  Any other non-zero rep status is kept, and a digest other than `want` makes the cell
+// CDPROBE_ERR_INTEGRITY.  The latency kernel writes only 0 or CDPROBE_ERR_TIMEOUT, so for latency this is the rule
+// "stop at the first non-zero status".
+template <typename Out>
+static void summarize(const TimedRep* rep, uint32_t reps, uint32_t per_rep, uint64_t want, uint32_t idx, Out* out) {
+  uint64_t digest = 0;
+  int32_t s = 0;
+  float ns[kMaxTimedReps];
+  for (uint32_t k = 0; k <= reps; ++k) {
+    digest ^= rep[k].digest;
+    if (rep[k].status == CDPROBE_ERR_TIMEOUT) {
+      s = CDPROBE_ERR_TIMEOUT;
+      break;
+    }
+    if (rep[k].status != 0) s = rep[k].status;
+    if (k > 0) ns[k - 1] = (float)((double)rep[k].ns / per_rep);
+  }
+  out->measured[idx] = 1;
+  out->digest[idx] = digest;
+  if (s != CDPROBE_ERR_TIMEOUT) {
+    std::sort(ns, ns + reps);
+    out->ns_min[idx] = ns[0];
+    out->ns_median[idx] = ns[reps / 2];
+    out->ns_max[idx] = ns[reps - 1];
+    if (digest != want) s = CDPROBE_ERR_INTEGRITY;
+  }
+  out->status[idx] = s;
+}
+
+}  // namespace cdp
+
+extern "C" {
+
+static_assert(CDPROBE_DIAG_FLIP == cdp::kDiagFlip && CDPROBE_DIAG_ZERO == cdp::kDiagZero &&
+                  CDPROBE_DIAG_DISPLACED == cdp::kDiagDisplaced && CDPROBE_DIAG_STALE == cdp::kDiagStale &&
+                  CDPROBE_DIAG_FOREIGN == cdp::kDiagForeign && CDPROBE_DIAG_SAMPLES == cdp::kDiagSamples,
+              "diagnosis classes");
+static_assert(sizeof(cdp::DiagSample) == sizeof(cdprobe_diag_sample_t) &&
+                  offsetof(cdp::DiagSample, run_seq) == offsetof(cdprobe_diag_sample_t, run_seq) &&
+                  offsetof(cdp::DiagSample, rank) == offsetof(cdprobe_diag_sample_t, rank),
+              "the kernel writes samples in the ABI layout");
+
+int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target, uint32_t reader, cdprobe_diag_t* out) {
+  cdp::g_last_error.clear();
+  if (h == nullptr || out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->op = op;
+  out->issuer = issuer;
+  out->target = target;
+  out->reader = reader;
+  out->first_bad = UINT64_MAX;
+  const cdp::Plan& pl = h->plan;
+  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE) {
+    cdp::set_err("op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE");
+    return CDPROBE_ERR_ARG;
+  }
+  if (issuer >= h->n_total || target >= h->n_total || reader >= h->n_total) {
+    cdp::set_err("rank out of range");
+    return CDPROBE_ERR_ARG;
+  }
+  if (issuer == target && !pl.diag) {
+    cdp::set_err("cell (i, i) exists only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG)");
+    return CDPROBE_ERR_ARG;
+  }
+  if (reader < h->first || reader >= h->first + h->n_local) {
+    cdp::set_err("reader is not a rank of this process");
+    return CDPROBE_ERR_ARG;
+  }
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  if (h->last_run_seq == 0) {
+    cdp::set_err("no cdprobe_run yet: there is no pattern to compare with");
+    return CDPROBE_ERR_STATE;
+  }
+  cdp::LocalRank& L = h->lr[reader - h->first];
+  if (cdp::cell_status(h, reader - h->first, target) != 0) {  // never read through a mapping that is down
+    cdp::set_err("reader does not map the target");
+    return CDPROBE_ERR_STATE;
+  }
+  const uint64_t run_seq = h->last_run_seq;
+  out->run_seq = run_seq;
+  out->region_offset = cdp::cell_offset(pl, op, issuer, target);
+  out->bytes = pl.bpp;
+
+  const cdp::DiagSpec s =
+      op == CDPROBE_OP_WRITE
+          ? cdp::diag_write_spec(h->seed, h->n_total, issuer, target, run_seq, pl.bpp / 8)
+          : cdp::diag_read_spec(h->seed, h->n_total, target, (uint64_t)cdp::cell_slice(pl, issuer, target) * (pl.bpp / 8),
+                                pl.bpp / 8, pl.src_bytes / 8);
+
+  CDP_RT(cudaSetDevice(L.ordinal));
+  if (const int rc = cdp::ensure_scratch(L, cdp::diag_scratch_bytes(pl.bpp)); rc != CDPROBE_OK) return rc;
+  const uint8_t* region = reinterpret_cast<const uint8_t*>(L.va[target]) + out->region_offset;
+  cdp::DiagOut d;
+  float ms = 0.f;
+  cudaError_t e = cudaEventRecord(L.ev0, L.stream);
+  if (e == cudaSuccess) e = (cudaError_t)cdp::diag_launch(region, s, L.scratch, L.sm_count, L.stream);
+  if (e == cudaSuccess) e = cudaEventRecord(L.ev1, L.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&d, L.scratch, sizeof(d), cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L.ev0, L.ev1);
+  if (e != cudaSuccess) {
+    h->sticky = true;  // a failed kernel leaves the context unusable
+    return cdp::fail_cuda("cdprobe_diagnose", e);
+  }
+  out->ms = ms;
+  out->bad_words = d.bad_words;
+  out->bad_granules = d.bad_granules;
+  out->zero_words = d.kind_count[cdp::kDiagZero];
+  if (d.bad_words) {
+    out->first_bad = ~d.first_bad_n;
+    out->last_bad = d.last_bad;
+  }
+  for (int k = 0; k < cdp::kDiagKinds; ++k) out->kind_count[k] = d.kind_count[k];
+  for (int b = 0; b < 64; ++b) out->bit_flips[b] = d.bit_flips[b];
+  out->n_samples = d.bad_words < (uint64_t)CDPROBE_DIAG_SAMPLES ? (uint32_t)d.bad_words : (uint32_t)CDPROBE_DIAG_SAMPLES;
+  memcpy(out->sample, d.sample, sizeof(out->sample[0]) * out->n_samples);
+  return CDPROBE_OK;
+}
+
+int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->hops = hops != 0 ? hops : cdp::kLatencyDefaultHops;
+  out->reps = reps != 0 ? reps : cdp::kLatencyDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  out->n = h->n_total;
+  out->region_bytes = pl.bpp;
+  if (out->hops > cdp::kLatencyMaxHops || out->reps > cdp::kMaxTimedReps) {
+    cdp::set_err("hops must be at most 1 << 20 and reps at most 64");
+    return CDPROBE_ERR_ARG;
+  }
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  hops = out->hops;
+  reps = out->reps;
+  const uint64_t lines = pl.bpp / (cdp::kLineWords * 8);
+  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+
+  // 1. every local issuer's chases, all launched before any is waited for
+  cdp::LatencyParams P[cdp::kMaxRanks];
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    out->row_mask |= 1u << g;
+    cdp::LatencyParams& p = P[li];
+    memset(&p, 0, sizeof(p));
+    p.seed = h->seed;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.hops = hops;
+    p.reps = reps;
+    for (uint32_t j = 0; j < h->n_total; ++j) {
+      if (j == g && !pl.diag) continue;  // no loop-back slice to chase
+      const int32_t s = cdp::cell_status(h, li, j);
+      if (s != 0) {  // never read through a mapping that is down
+        out->status[g * CDPROBE_MAX_GPUS + j] = s;
+        continue;
+      }
+      cdp::LatencyCell& c = p.cell[p.n_cells++];
+      c.region = reinterpret_cast<const uint8_t*>(L.va[j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
+      c.lines = lines;
+      c.issuer = g;
+      c.target = j;
+    }
+    if (p.n_cells == 0) continue;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    const cudaError_t e = (cudaError_t)cdp::latency_launch(p, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch latency_kernel", e);
+    }
+  }
+
+  // 2. while they run: the digest each chase gives over an intact region
+  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t k = 0; k < P[li].n_cells; ++k) {
+      const cdp::LatencyCell& c = P[li].cell[k];
+      const uint64_t first = (uint64_t)cdp::cell_slice(pl, c.issuer, c.target) * (pl.bpp / 8);
+      for (uint32_t r = 0; r <= reps; ++r)
+        want[li][k] ^= cdp::latency_rep_digest(h->seed, c.issuer, c.target, first, lines, r, hops);
+    }
+  }
+
+  // 3. collect: ns per hop of the timed reps, the digest of all of them
+  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::LatencyParams& p = P[li];
+    if (p.n_cells == 0) continue;
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_cells, got.data(), "cdprobe_latency"); rc != CDPROBE_OK)
+      return rc;
+    for (uint32_t k = 0; k < p.n_cells; ++k)
+      cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, hops, want[li][k],
+                     p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+// What each process contributes at the start of cdprobe_pingpong, so that every process refuses or runs the same call
+// over the same pair set (cdprobe_unmap_peer changes only the local view).
+struct PingPongAgree {
+  uint64_t call_seq;
+  uint32_t trips, reps, fenced, ok;
+  int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [local rank][rank]: mapping status, unmapped cells folded in
+};
+
+int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->trips = trips != 0 ? trips : cdp::kPingPongDefaultTrips;
+  out->reps = reps != 0 ? reps : cdp::kPingPongDefaultReps;
+  out->fenced = fenced;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  trips = out->trips;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together
+  std::string bad;
+  if (trips > cdp::kPingPongMaxTrips || reps > cdp::kMaxTimedReps || fenced > 1)
+    bad = "trips must be at most 1 << 16, reps at most 64 and fenced 0 or 1";
+  uint32_t f_init = cdp::kPingPongNoFault, f_target = cdp::kPingPongNoFault, f_trip = cdp::kPingPongNoFault;
+  if (h->pp_fault != 0) {
+    const uint64_t fi = h->pp_fault >> 32, ft = (h->pp_fault >> 16) & 0xffffu, trip = h->pp_fault & 0xffffu;
+    if (fi == 0 || ft == 0 || fi > n || ft > n || fi == ft) {
+      bad = "the armed pingpong fault names no off-diagonal cell";
+    } else if (trip + 1 >= trips || (reps == 1 && trip + 2 == trips)) {
+      // the initiator runs one trip ahead until the responder catches up; that must happen inside the leg
+      bad = "the armed pingpong fault's trip must be below trips - 1, and below trips - 2 when reps is 1";
+    } else {
+      f_init = (uint32_t)fi - 1;
+      f_target = (uint32_t)ft - 1;
+      f_trip = (uint32_t)trip;
+    }
+  }
+  PingPongAgree mine;
+  memset(&mine, 0, sizeof(mine));
+  mine.call_seq = h->pp_calls + 1;
+  mine.trips = trips;
+  mine.reps = reps;
+  mine.fenced = fenced;
+  mine.ok = bad.empty() ? 1u : 0u;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  memcpy(st, h->status, sizeof(st));
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::LocalRank& L = h->lr[li];
+    for (uint32_t j = 0; j < n; ++j) st[L.grank][j] = mine.status[li][j] = cdp::cell_status(h, li, j);
+  }
+  if (h->cfg.world_size > 1) {
+    std::vector<PingPongAgree> all(h->cfg.world_size);
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    for (uint32_t r = 0; r < h->cfg.world_size; ++r) {
+      const PingPongAgree& o = all[r];
+      if (!o.ok && bad.empty()) bad = "another process called cdprobe_pingpong with invalid arguments";
+      if ((o.call_seq != mine.call_seq || o.trips != trips || o.reps != reps || o.fenced != fenced) && bad.empty())
+        bad = "cdprobe_pingpong is collective: every process must call it with the same arguments";
+      for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], o.status[li], sizeof(st[0]));
+    }
+  }
+  if (!bad.empty()) {
+    cdp::set_err(bad);
+    return CDPROBE_ERR_ARG;
+  }
+  h->pp_calls = mine.call_seq;
+  out->call_seq = h->pp_calls;
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+  if (n == 1) {
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+  if (h->cfg.world_size > 1) {  // every process has agreed before any kernel polls a peer
+    std::string err;
+    if (h->rdv.barrier(&err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+  // a pair is exchanged only when both directions are mapped; the status of its cells is the pair's mapping status
+  auto pair_status = [&](uint32_t i, uint32_t j) { return st[i][j] != 0 ? st[i][j] : st[j][i]; };
+
+  // 2. one block per local rank, every one launched before any is waited for
+  cdp::PingPongParams P[cdp::kMaxRanks];
+  bool launched[cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::PingPongParams& p = P[li];
+    memset(&p, 0, sizeof(p));
+    p.call_seq = h->pp_calls;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.n_rounds = pl.rounds;
+    p.trips = trips;
+    p.reps = reps;
+    p.fault_round = cdp::kPingPongNoFault;
+    p.fault_trip = f_trip;
+    for (uint32_t j = 0; j < n; ++j)
+      if (j != g) out->status[g * CDPROBE_MAX_GPUS + j] = pair_status(g, j);
+    uint32_t active = 0;
+    for (uint32_t r = 0; r < pl.rounds; ++r) {
+      const int q = pl.partner[r][g];
+      if (q < 0 || pair_status(g, (uint32_t)q) != 0) continue;
+      cdp::PingPongRound& R = p.round[r];
+      R.remote = reinterpret_cast<uint64_t*>(L.va[q] + cdp::kPingOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      R.local = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kPingOff + (uint64_t)q * sizeof(cdp::FlagLine));
+      R.partner = (uint32_t)q;
+      R.first = g < (uint32_t)q ? 1u : 0u;
+      if (g == f_target && (uint32_t)q == f_init) p.fault_round = r;
+      ++active;
+    }
+    if (active == 0) continue;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    const cudaError_t e =
+        (cudaError_t)cdp::pingpong_launch(p, fenced != 0, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch pingpong_kernel", e);
+    }
+    launched[li] = true;
+  }
+
+  // 3. while they run: the digest of a clean leg for every cell a local rank initiates
+  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // [local rank][round]
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t r = 0; r < pl.rounds; ++r) {
+      const cdp::PingPongRound& R = P[li].round[r];
+      if (R.remote == nullptr) continue;
+      const uint32_t leg = R.first ? 0u : 1u;
+      for (uint32_t rep = 0; rep <= reps; ++rep) want[li][r] ^= cdp::pingpong_rep_digest(h->pp_calls, r, leg, rep, trips);
+    }
+  }
+
+  // 4. collect: ns per round trip of the timed reps, the digest of all of them
+  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (!launched[li]) continue;
+    const cdp::PingPongParams& p = P[li];
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_rounds, got.data(), "cdprobe_pingpong"); rc != CDPROBE_OK)
+      return rc;
+    for (uint32_t r = 0; r < p.n_rounds; ++r) {
+      const cdp::PingPongRound& R = p.round[r];
+      if (R.remote == nullptr) continue;
+      cdp::summarize(got.data() + (size_t)r * cdp::kRepSlots, reps, trips, want[li][r],
+                     h->lr[li].grank * CDPROBE_MAX_GPUS + R.partner, out);
+    }
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+}  // extern "C"

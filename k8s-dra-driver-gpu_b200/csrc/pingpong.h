@@ -4,14 +4,13 @@
 #include <stdint.h>
 
 #include "probe_types.h"
+#include "timed_rep.cuh"
 
 namespace cdp {
 
 constexpr uint32_t kPingPongDefaultTrips = 256;
 constexpr uint32_t kPingPongDefaultReps = 8;
 constexpr uint32_t kPingPongMaxTrips = 1u << 16;
-constexpr uint32_t kPingPongMaxReps = 64;             // timed reps; one untimed warm-up rep runs before them
-constexpr uint32_t kPingPongRepSlots = kPingPongMaxReps + 1;
 constexpr uint32_t kPingPongNoFault = 0xFFFFFFFFu;
 
 struct PingPongRound {    // what one rank does in one round of the tournament
@@ -30,15 +29,8 @@ struct PingPongParams {
   uint32_t fault_trip;      // ... and the trip of timed rep 1 it answers with the next trip's echo (kPingPongNoFault: none)
 };
 
-struct PingPongRep {            // what the kernel leaves per initiated cell and rep, at [round * kPingPongRepSlots + rep]
-  unsigned long long ns;        // %globaltimer: last echo used - first ping about to be stored
-  unsigned long long digest;    // xor of the echo words this rep received
-  int32_t status;               // 0; CDPROBE_ERR_INTEGRITY: an echo differed from the expected word;
-                                // CDPROBE_ERR_TIMEOUT: a poll passed the deadline (later reps did not run)
-  uint32_t pad;
-};
-
-// Enqueues one 32-thread block for one rank on `stream`.  Returns a cudaError_t.
-int pingpong_launch(const PingPongParams& p, bool fenced, PingPongRep* out, cudaStream_t stream);
+// Enqueues one 32-thread block for one rank on `stream`; the cell it initiates in round r leaves its reps at
+// out[r * kRepSlots + rep], CDPROBE_ERR_INTEGRITY marking a rep with an unexpected echo.  Returns a cudaError_t.
+int pingpong_launch(const PingPongParams& p, bool fenced, TimedRep* out, cudaStream_t stream);
 
 }  // namespace cdp

@@ -34,20 +34,6 @@ __device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) {
 __device__ __forceinline__ void st_relaxed_sys(uint64_t* p, uint64_t v) {
   asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ uint64_t globaltimer() {
-  uint64_t t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
-  return t;
-}
-// The closing timer read.  `v`, the last echo, is an operand, so the compiler cannot place the read ahead of the
-// poll that returned it; in the SASS the read follows the trip loop, whose compare of v with the expected word waits
-// for the load (tests/test_pingpong_cpu.py checks that order in the compiled kernel).
-__device__ __forceinline__ uint64_t globaltimer_after(uint64_t v) {
-  uint64_t t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) : "l"(v) : "memory");
-  return t;
-}
-
 // Spins until the word at p is >= want; v gets the word that ended the wait.  False: the deadline passed.
 __device__ __forceinline__ bool poll(const uint64_t* p, uint64_t want, uint64_t deadline, uint64_t& v) {
   uint32_t spins = 0;
@@ -66,7 +52,7 @@ __device__ __forceinline__ void signal(uint64_t* p, uint64_t w) {
 // The initiator's side of one leg: the warm-up rep, then p.reps timed reps of p.trips round trips.
 template <bool kFenced>
 __device__ bool initiate(const PingPongParams& p, const PingPongRound& R, uint32_t r, uint32_t leg, uint64_t deadline,
-                         PingPongRep* o) {
+                         TimedRep* o) {
   for (uint32_t rep = 0; rep <= p.reps; ++rep) {
     const uint64_t base = pingpong_word(p.call_seq, r, leg, rep, 0, 0);
     uint64_t digest = 0, v = 0;
@@ -109,13 +95,13 @@ __device__ bool respond(const PingPongParams& p, const PingPongRound& R, uint32_
 }
 
 template <bool kFenced>
-__global__ void __launch_bounds__(32) pingpong_kernel(const __grid_constant__ PingPongParams p, PingPongRep* out) {
+__global__ void __launch_bounds__(32) pingpong_kernel(const __grid_constant__ PingPongParams p, TimedRep* out) {
   if (threadIdx.x != 0) return;
   const uint64_t deadline = globaltimer() + p.timeout_ns;
   for (uint32_t r = 0; r < p.n_rounds; ++r) {
     const PingPongRound& R = p.round[r];
     if (R.remote == nullptr) continue;
-    PingPongRep* o = out + (size_t)r * kPingPongRepSlots;
+    TimedRep* o = out + (size_t)r * kRepSlots;
     // Leg 1's first ping goes into the line that carried leg 0's echoes, so it must not be stored before leg 0's
     // last echo has been read: leg 0's initiator hands the pair over with this word, which leg 1's initiator awaits.
     // Its echo bit is 0, so it lies above every leg-0 ping and below every leg-1 echo of its sender.
@@ -144,7 +130,7 @@ __global__ void __launch_bounds__(32) pingpong_kernel(const __grid_constant__ Pi
     // timed out: every cell this rank has not initiated yet is marked, and the kernel exits
     for (uint32_t q = initiated ? r + 1 : r; q < p.n_rounds; ++q) {
       if (p.round[q].remote == nullptr) continue;
-      PingPongRep& first = out[(size_t)q * kPingPongRepSlots];
+      TimedRep& first = out[(size_t)q * kRepSlots];
       first.ns = 0;
       first.digest = 0;
       first.status = CDPROBE_ERR_TIMEOUT;
@@ -155,7 +141,7 @@ __global__ void __launch_bounds__(32) pingpong_kernel(const __grid_constant__ Pi
 
 }  // namespace
 
-int pingpong_launch(const PingPongParams& p, bool fenced, PingPongRep* out, cudaStream_t stream) {
+int pingpong_launch(const PingPongParams& p, bool fenced, TimedRep* out, cudaStream_t stream) {
   if (fenced) pingpong_kernel<true><<<1, 32, 0, stream>>>(p, out);
   else pingpong_kernel<false><<<1, 32, 0, stream>>>(p, out);
   return (int)cudaGetLastError();

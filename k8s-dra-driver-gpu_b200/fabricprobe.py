@@ -74,6 +74,26 @@ class Config:
         return c
 
 
+def _mat(t, a, keep=None):
+    """The n x n matrix [i][j] of a CDPROBE_MAX_GPUS-strided array of result `t`; None where keep(k) is false."""
+    return [[a[k] if keep is None or keep(k) else None for k in range(i * abi.MAX_GPUS, i * abi.MAX_GPUS + t.n)]
+            for i in range(t.n)]
+
+
+def _timed_cells(t) -> dict:
+    """The per-cell fields of a Latency or a PingPong.  A cell that was not measured is None in every matrix but
+    `status`; a cell that timed out keeps its digest but has no times."""
+    def measured(k):
+        return t.measured[k]
+
+    def timed(k):
+        return t.measured[k] and t.status[k] != abi.ERR_TIMEOUT
+
+    return dict(measured=_mat(t, [bool(m) for m in t.measured]), status=_mat(t, t.status),
+                ns_min=_mat(t, t.ns_min, timed), ns_median=_mat(t, t.ns_median, timed), ns_max=_mat(t, t.ns_max, timed),
+                digest=_mat(t, t.digest, measured), ms=t.ms, raw=t)
+
+
 @dataclasses.dataclass
 class Result:
     n: int
@@ -116,23 +136,19 @@ class Result:
     @staticmethod
     def from_c(r: abi.ResultT) -> "Result":
         n = r.n
-
-        def mat(a):
-            return [[a[i * abi.MAX_GPUS + j] for j in range(n)] for i in range(n)]
-
         return Result(
             n=n,
             row_mask=r.row_mask,
             verdict=bool(r.verdict),
-            reach_read=mat(r.reach_read),
-            reach_write=mat(r.reach_write),
-            gbps_read=mat(r.gbps_read),
-            gbps_write=mat(r.gbps_write),
-            status=mat(r.status),
-            sum_read=mat(r.sum_read),
-            xor_read=mat(r.xor_read),
-            sum_write=mat(r.sum_write),
-            xor_write=mat(r.xor_write),
+            reach_read=_mat(r, r.reach_read),
+            reach_write=_mat(r, r.reach_write),
+            gbps_read=_mat(r, r.gbps_read),
+            gbps_write=_mat(r, r.gbps_write),
+            status=_mat(r, r.status),
+            sum_read=_mat(r, r.sum_read),
+            xor_read=_mat(r, r.xor_read),
+            sum_write=_mat(r, r.sum_write),
+            xor_write=_mat(r, r.xor_write),
             bytes_per_pair=r.bytes_per_pair,
             run_seq=r.run_seq,
             rounds=r.rounds,
@@ -220,26 +236,8 @@ class Latency:
 
     @staticmethod
     def from_c(t: abi.LatencyT) -> "Latency":
-        n = t.n
-
-        def mat(a, timed=False):
-            out = []
-            for i in range(n):
-                row = []
-                for j in range(n):
-                    k = i * abi.MAX_GPUS + j
-                    ok = t.measured[k] and not (timed and t.status[k] == abi.ERR_TIMEOUT)
-                    row.append(a[k] if ok else None)
-                out.append(row)
-            return out
-
-        return Latency(
-            n=n, row_mask=t.row_mask, hops=t.hops, reps=t.reps, region_bytes=t.region_bytes,
-            measured=[[bool(t.measured[i * abi.MAX_GPUS + j]) for j in range(n)] for i in range(n)],
-            status=[[t.status[i * abi.MAX_GPUS + j] for j in range(n)] for i in range(n)],
-            ns_min=mat(t.ns_min, True), ns_median=mat(t.ns_median, True), ns_max=mat(t.ns_max, True),
-            digest=mat(t.digest), ms=t.ms, raw=t,
-        )
+        return Latency(n=t.n, row_mask=t.row_mask, hops=t.hops, reps=t.reps, region_bytes=t.region_bytes,
+                       **_timed_cells(t))
 
 
 @dataclasses.dataclass
@@ -265,26 +263,8 @@ class PingPong:
 
     @staticmethod
     def from_c(t: abi.PingPongT) -> "PingPong":
-        n = t.n
-
-        def mat(a, timed=False):
-            out = []
-            for i in range(n):
-                row = []
-                for j in range(n):
-                    k = i * abi.MAX_GPUS + j
-                    ok = t.measured[k] and not (timed and t.status[k] == abi.ERR_TIMEOUT)
-                    row.append(a[k] if ok else None)
-                out.append(row)
-            return out
-
-        return PingPong(
-            n=n, row_mask=t.row_mask, trips=t.trips, reps=t.reps, fenced=bool(t.fenced), call_seq=t.call_seq,
-            measured=[[bool(t.measured[i * abi.MAX_GPUS + j]) for j in range(n)] for i in range(n)],
-            status=[[t.status[i * abi.MAX_GPUS + j] for j in range(n)] for i in range(n)],
-            ns_min=mat(t.ns_min, True), ns_median=mat(t.ns_median, True), ns_max=mat(t.ns_max, True),
-            digest=mat(t.digest), ms=t.ms, raw=t,
-        )
+        return PingPong(n=t.n, row_mask=t.row_mask, trips=t.trips, reps=t.reps, fenced=bool(t.fenced),
+                        call_seq=t.call_seq, **_timed_cells(t))
 
 
 def _raise(lib, rc: int, what: str):
@@ -292,6 +272,11 @@ def _raise(lib, rc: int, what: str):
     detail = lib.cdprobe_last_error().decode()
     cls = ErrUnsupported if rc in (abi.ERR_NO_DEVICE, abi.ERR_UNSUPPORTED) else ProbeError
     raise cls(rc, f"{what}: {msg}", detail)
+
+
+def _check(lib, rc: int, what: str):
+    if rc != abi.OK:
+        _raise(lib, rc, what)
 
 
 class Probe:
@@ -314,9 +299,7 @@ class Probe:
         if rc != abi.OK and not (allow_timeout and rc == abi.ERR_TIMEOUT):
             _raise(self._lib, rc, "cdprobe_run")
         if gather:
-            rc2 = self._lib.cdprobe_gather(self._h, C.byref(r))
-            if rc2 != abi.OK:
-                _raise(self._lib, rc2, "cdprobe_gather")
+            _check(self._lib, self._lib.cdprobe_gather(self._h, C.byref(r)), "cdprobe_gather")
         return Result.from_c(r)
 
     def run_raw(self, out: abi.ResultT) -> int:
@@ -325,36 +308,26 @@ class Probe:
 
     def Info(self) -> abi.InfoT:
         i = abi.InfoT()
-        rc = self._lib.cdprobe_info(self._h, C.byref(i))
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_info")
+        _check(self._lib, self._lib.cdprobe_info(self._h, C.byref(i)), "cdprobe_info")
         return i
 
     def Trace(self, local: int = 0):
         """Per-phase timeline of the last run: list of dicts (ns relative to the first barrier release)."""
         t = abi.TraceT()
-        rc = self._lib.cdprobe_trace(self._h, local, C.byref(t))
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_trace")
+        _check(self._lib, self._lib.cdprobe_trace(self._h, local, C.byref(t)), "cdprobe_trace")
         names = {0: "-", 1: "read", 2: "write", 3: "verify", 4: "warm"}
         return [{"job0": names[t.kind0[p]], "peer0": t.peer0[p], "job1": names[t.kind1[p]], "peer1": t.peer1[p],
                  "sync_all": int(t.sync_all[p]), "sync_mask": int(t.sync_mask[p]), "post_mask": int(t.post_mask[p]), "t_start": t.t_start[p], "t_end0": t.t_end0[p], "t_end1": t.t_end1[p],
                  "t_arrive": t.t_arrive[p]} for p in range(t.n_phases)]
 
     def SetOption(self, option: int, value: int) -> None:
-        rc = self._lib.cdprobe_set_option(self._h, option, value)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_set_option")
+        _check(self._lib, self._lib.cdprobe_set_option(self._h, option, value), "cdprobe_set_option")
 
     def UnmapPeer(self, local: int, peer: int) -> None:
-        rc = self._lib.cdprobe_unmap_peer(self._h, local, peer)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_unmap_peer")
+        _check(self._lib, self._lib.cdprobe_unmap_peer(self._h, local, peer), "cdprobe_unmap_peer")
 
     def RemapPeer(self, local: int, peer: int) -> None:
-        rc = self._lib.cdprobe_remap_peer(self._h, local, peer)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_remap_peer")
+        _check(self._lib, self._lib.cdprobe_remap_peer(self._h, local, peer), "cdprobe_remap_peer")
 
     def CeCopy(self, copies, push: bool = True, nbytes: int = 0, reps: int = 4):
         """Copy-engine reference on the probe's buffers: `copies` = [(local rank, peer rank), ...] run concurrently;
@@ -363,25 +336,20 @@ class Probe:
         loc = (C.c_uint32 * k)(*[c[0] for c in copies])
         peer = (C.c_uint32 * k)(*[c[1] for c in copies])
         ms = (C.c_double * k)()
-        rc = self._lib.cdprobe_ce_copy(self._h, k, loc, peer, 1 if push else 0, nbytes, reps, ms)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_ce_copy")
+        _check(self._lib, self._lib.cdprobe_ce_copy(self._h, k, loc, peer, 1 if push else 0, nbytes, reps, ms),
+               "cdprobe_ce_copy")
         info = self.Info()
         pl = plan(info.n, self.cfg.bytes, self.cfg.mode, self.cfg.flags)
         nb = min(x for x in (nbytes or pl.src_bytes, pl.src_bytes, pl.land_bytes))
         return [(ms[i], nb * reps / (ms[i] * 1e-3) / 1e9 if ms[i] > 0 else 0.0) for i in range(k)]
 
     def Corrupt(self, local: int, byte_offset: int, xor_mask: int) -> None:
-        rc = self._lib.cdprobe_corrupt(self._h, local, byte_offset, xor_mask)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_corrupt")
+        _check(self._lib, self._lib.cdprobe_corrupt(self._h, local, byte_offset, xor_mask), "cdprobe_corrupt")
 
     def CorruptLanding(self, local: int, target: int, faults) -> None:
         """Test-only fault in transit: on every Run until disarmed, xor each (word index, mask) of `faults` into
         the landing slot local rank `local` writes in `target`, after the write and before the verify.  [] disarms."""
-        rc = self.corrupt_landing_raw(local, target, faults)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_corrupt_landing")
+        _check(self._lib, self.corrupt_landing_raw(local, target, faults), "cdprobe_corrupt_landing")
 
     def corrupt_landing_raw(self, local: int, target: int, faults) -> int:
         """The bare ABI call: its return code."""
@@ -396,8 +364,7 @@ class Probe:
         op: abi.OP_READ / abi.OP_WRITE or "read" / "write"."""
         op = {"read": abi.OP_READ, "write": abi.OP_WRITE}.get(op, op)
         rc, d = self.diagnose_raw(op, issuer, target, issuer if reader is None else reader)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_diagnose")
+        _check(self._lib, rc, "cdprobe_diagnose")
         return Diagnosis.from_c(d)
 
     def diagnose_raw(self, op: int, issuer: int, target: int, reader: int):
@@ -410,8 +377,7 @@ class Probe:
         """Go: (*Probe).Latency.  Dependent-load latency of every cell whose issuer is local (0: 1024 hops, 8 timed
         reps).  Needs no Run first and disturbs none."""
         rc, t = self.latency_raw(hops, reps)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_latency")
+        _check(self._lib, rc, "cdprobe_latency")
         return Latency.from_c(t)
 
     def latency_raw(self, hops: int, reps: int):
@@ -425,8 +391,7 @@ class Probe:
         round trips, 8 timed reps); fenced: a fence.sys before every store.  Collective when world_size > 1.  Needs no
         Run first and disturbs none."""
         rc, t = self.pingpong_raw(trips, reps, 1 if fenced else 0)
-        if rc != abi.OK:
-            _raise(self._lib, rc, "cdprobe_pingpong")
+        _check(self._lib, rc, "cdprobe_pingpong")
         return PingPong.from_c(t)
 
     def pingpong_raw(self, trips: int, reps: int, fenced: int):
@@ -461,9 +426,7 @@ def topology(strict: bool = True) -> abi.TopologyT:
     """internal/common topology enumeration (NVML only, no CUDA)."""
     lib = abi.load_library()
     t = abi.TopologyT()
-    rc = lib.cdprobe_topology(1 if strict else 0, C.byref(t))
-    if rc != abi.OK:
-        _raise(lib, rc, "cdprobe_topology")
+    _check(lib, lib.cdprobe_topology(1 if strict else 0, C.byref(t)), "cdprobe_topology")
     return t
 
 
@@ -472,16 +435,12 @@ def gate(cfg: Config, n_total: int):
     lib = abi.load_library()
     r, w = C.c_float(), C.c_float()
     c = cfg.to_c()
-    rc = lib.cdprobe_gate(C.byref(c), n_total, C.byref(r), C.byref(w))
-    if rc != abi.OK:
-        _raise(lib, rc, "cdprobe_gate")
+    _check(lib, lib.cdprobe_gate(C.byref(c), n_total, C.byref(r), C.byref(w)), "cdprobe_gate")
     return r.value, w.value
 
 
 def plan(n: int, nbytes: int, mode: int, flags: int = 0) -> abi.PlanT:
     lib = abi.load_library()
     p = abi.PlanT()
-    rc = lib.cdprobe_plan(n, nbytes, mode, flags, C.byref(p))
-    if rc != abi.OK:
-        _raise(lib, rc, "cdprobe_plan")
+    _check(lib, lib.cdprobe_plan(n, nbytes, mode, flags, C.byref(p)), "cdprobe_plan")
     return p
