@@ -318,6 +318,38 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_pingpong_t;
 
+/* Remote atomics per ordered pair (cdprobe_atomics): issuer i's GPU runs system-scope 64-bit atomics on cell (i, j)'s
+ * own word in target j's memory, through i's mapping of j; the owner's L2 performs them and returns each result to i
+ * (DESIGN §5e).  Matrices are row-major [issuer * CDPROBE_MAX_GPUS + target]. */
+#define CDPROBE_ATOMIC_FETCH_ADD 0u   /* one lane: a dependent atom.add chain, op k returns start + k */
+#define CDPROBE_ATOMIC_CAS 1u         /* one lane: a dependent atom.cas chain, every CAS must succeed */
+#define CDPROBE_ATOMIC_CONTENDED 2u   /* 32 lanes of one warp: fetch-add chains on the same word */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t kind;                        /* CDPROBE_ATOMIC_* */
+  uint32_t ops, reps;                   /* as applied: 0 -> 1024 and 8; ops in [1, 1 << 16] per lane, reps in [1, 64] */
+  uint32_t lanes;                       /* lanes issuing atomics: 1, or 32 for CDPROBE_ATOMIC_CONTENDED */
+  uint32_t reserved;
+  uint64_t call_seq;                    /* 1-based count of cdprobe_atomics calls on this handle (0: refused) */
+  uint8_t measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];  /* 1: the cell's atomics ran */
+  uint8_t native[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 1: same device, or CUDA reports native atomics for the pair;
+                                                             0: CUDA reports none (the cell is not run); 2: the target's
+                                                             device is not visible in this process (the cell runs) */
+  int32_t status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 0 ok; CDPROBE_ERR_INTEGRITY: a return, the read-back or the
+                                                             digest differs from the expected values; CDPROBE_ERR_TIMEOUT:
+                                                             the cell passed timeout_ms; CDPROBE_ERR_UNSUPPORTED: no
+                                                             native atomics; else the mapping's status */
+  float ns_min[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];      /* ns per atomic over the timed reps (0 when not timed);
+                                                             CONTENDED: per atomic on one word under 32-way contention */
+  float ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];
+  uint64_t digest[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* xor of every value the atomics returned, warm-up rep
+                                                             included */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_atomics_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -341,10 +373,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency, cdprobe_pingpong: diagnostics, benches, fault injection; the reference has no counterpart (it
- *   has no probe, SURVEY.md F1).
- *   cdprobe_diagnose, cdprobe_latency and cdprobe_pingpong are optional for callers: a daemon binds them with dlsym
- *   and works without.
+ *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics: diagnostics, benches, fault injection; the reference has no
+ *   counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong and cdprobe_atomics are optional for callers: a daemon binds
+ *   them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -375,6 +407,10 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              skip-ahead echo in cdprobe_pingpong: the responder `target`, in the
                                              process that hosts it, answers that trip of timed rep 1 of cell
                                              (initiator, target) with the echo of trip + 1; 0 disarms */
+#define CDPROBE_OPT_ATOMICS_FAULT 18u     /* tests: value = ((issuer + 1) << 16) | (target + 1) arms a lost-step fault in
+                                             cdprobe_atomics: in the process that hosts the issuer, the first op of timed
+                                             rep 1 of cell (issuer, target) adds 2 (CAS: swaps in v + 2), so exactly
+                                             that cell fails its checks; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -428,6 +464,19 @@ CDPROBE_API int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdpr
  * reps > 64, fenced > 1, arguments that differ between processes, or an armed CDPROBE_OPT_PINGPONG_FAULT whose cell
  * is out of range or whose trip is >= trips - 1 (or == trips - 2 with reps == 1); CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out);
+/* Remote atomics of every cell whose issuer is local to this process, on the cell's own 8-byte word in the target's
+ * memory (no other cell or process touches it).  Each rep opens with an atom.exch of its start value, then `ops`
+ * dependent atomics per lane follow: FETCH_ADD and CAS chains on one lane, 32 fetch-add chains on one word for
+ * CONTENDED; one untimed warm-up rep, then `reps` timed reps; ns per atomic by %globaltimer on the issuer.  Every
+ * return is checked (FETCH_ADD: op k returns start + k; CAS: every compare succeeds; CONTENDED: the warp's returns sum
+ * to the range's sum), the word is read back (start + lanes x ops), and the host checks the digest: any difference is
+ * CDPROBE_ERR_INTEGRITY in the cell's status.  A cell whose mapping is down, or whose pair CUDA reports without native
+ * atomics, is not run; the diagonal runs only with a loop-back slot (n == 1 or CDPROBE_FLAG_LOCAL_DIAG).  One-sided,
+ * not collective: fills the local rows (row_mask) and never waits on another rank.  Touches no result, pattern,
+ * landing slot, source buffer, Ctrl word, pingpong line or run_seq; needs no run first.  *out carries abi, n, kind,
+ * ops and reps whatever the return code.  CDPROBE_ERR_ARG: null argument, kind > 2, ops > 1 << 16, reps > 64, or an
+ * armed CDPROBE_OPT_ATOMICS_FAULT that names no cell of the domain; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

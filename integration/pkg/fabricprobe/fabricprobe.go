@@ -32,6 +32,7 @@ typedef uint32_t (*abi_fn)(void);
 typedef int (*diag_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*);
 typedef int (*lat_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_latency_t*);
 typedef int (*pp_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_pingpong_t*);
+typedef int (*at_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_atomics_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -39,6 +40,7 @@ static str_fn cdp_strerror; static last_fn cdp_last; static abi_fn cdp_abi;
 static diag_fn cdp_diag;  // optional: absent from libraries that predate cdprobe_diagnose
 static lat_fn cdp_lat;    // optional: absent from libraries that predate cdprobe_latency
 static pp_fn cdp_pp;      // optional: absent from libraries that predate cdprobe_pingpong
+static at_fn cdp_at;      // optional: absent from libraries that predate cdprobe_atomics
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -53,6 +55,7 @@ static int cdp_load(const char* path) {
   cdp_diag = (diag_fn)dlsym(cdp_dl, "cdprobe_diagnose");
   cdp_lat = (lat_fn)dlsym(cdp_dl, "cdprobe_latency");
   cdp_pp = (pp_fn)dlsym(cdp_dl, "cdprobe_pingpong");
+  cdp_at = (at_fn)dlsym(cdp_dl, "cdprobe_atomics");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -72,6 +75,10 @@ static int cdp_call_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_
 static int cdp_has_pingpong(void) { return cdp_pp != NULL; }
 static int cdp_call_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* pp) {
   return cdp_pp(h, trips, reps, fenced, pp);
+}
+static int cdp_has_atomics(void) { return cdp_at != NULL; }
+static int cdp_call_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* at) {
+  return cdp_at(h, kind, ops, reps, at);
 }
 */
 import "C"
@@ -198,6 +205,29 @@ type PingPong struct {
 	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the pair's mapping status
 	NsMin, NsMedian, NsMax []float32 // ns per round trip over the timed reps
 	Digest                 []uint64  // xor of every echo word the initiator received
+	Ms                     float64
+}
+
+// Kinds of Atomics (CDPROBE_ATOMIC_*).
+const (
+	AtomicFetchAdd  = 0 // one lane: a dependent atom.add chain
+	AtomicCAS       = 1 // one lane: a dependent atom.cas chain, every CAS must succeed
+	AtomicContended = 2 // 32 lanes of one warp: fetch-add chains on the same word
+)
+
+// Atomics is the remote-atomics matrix of the local rows (cdprobe_atomics_t).  Matrices are N x N row-major,
+// [issuer*N + target]; the Ns* entries are 0 where a cell was not measured or timed out.
+type Atomics struct {
+	N                      int
+	RowMask                uint32    // rows of this process's ranks
+	Kind                   int       // AtomicFetchAdd, AtomicCAS or AtomicContended
+	Ops, Reps, Lanes       int       // as applied; ops per lane
+	CallSeq                uint64    // 1-based count of Atomics calls on this handle
+	Native                 []uint8   // 1 native atomics (or same device); 0 none reported: not run; 2 peer device not visible
+	Measured               []bool
+	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; CDPROBE_ERR_UNSUPPORTED; else the mapping's status
+	NsMin, NsMedian, NsMax []float32 // ns per atomic over the timed reps
+	Digest                 []uint64  // xor of every value the atomics returned
 	Ms                     float64
 }
 
@@ -412,6 +442,50 @@ func (p *Probe) PingPong(trips, reps int, fenced bool) (PingPong, error) {
 			out.NsMedian[i*n+j] = float32(pp.ns_median[k])
 			out.NsMax[i*n+j] = float32(pp.ns_max[k])
 			out.Digest[i*n+j] = uint64(pp.digest[k])
+		}
+	}
+	return out, nil
+}
+
+// Atomics runs system-scope 64-bit atomics from every local issuer on each cell's own word in the target's memory
+// and reports ns per atomic (ops, reps 0, 0: 1024 ops per lane, 8 timed reps); every returned value is checked.
+// One-sided: only the local rows are filled and no process waits on another.  ErrUnsupported when the library
+// predates cdprobe_atomics.
+func (p *Probe) Atomics(kind, ops, reps int) (Atomics, error) {
+	if C.cdp_has_atomics() == 0 {
+		return Atomics{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_atomics", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	var at C.cdprobe_atomics_t
+	rc := C.cdp_call_atomics(p.h, C.uint32_t(kind), C.uint32_t(ops), C.uint32_t(reps), &at)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_atomics: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return Atomics{}, err
+	}
+	n := int(at.n)
+	out := Atomics{N: n, RowMask: uint32(at.row_mask), Kind: int(at.kind), Ops: int(at.ops), Reps: int(at.reps),
+		Lanes: int(at.lanes), CallSeq: uint64(at.call_seq), Ms: float64(at.ms)}
+	out.Native = make([]uint8, n*n)
+	out.Measured = make([]bool, n*n)
+	out.Status = make([]int32, n*n)
+	out.NsMin = make([]float32, n*n)
+	out.NsMedian = make([]float32, n*n)
+	out.NsMax = make([]float32, n*n)
+	out.Digest = make([]uint64, n*n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < n; j++ {
+			k := i*C.CDPROBE_MAX_GPUS + j
+			out.Native[i*n+j] = uint8(at.native[k])
+			out.Measured[i*n+j] = at.measured[k] != 0
+			out.Status[i*n+j] = int32(at.status[k])
+			out.NsMin[i*n+j] = float32(at.ns_min[k])
+			out.NsMedian[i*n+j] = float32(at.ns_median[k])
+			out.NsMax[i*n+j] = float32(at.ns_max[k])
+			out.Digest[i*n+j] = uint64(at.digest[k])
 		}
 	}
 	return out, nil

@@ -96,6 +96,22 @@ type PingPong struct {
 	Ms                     float64
 }
 
+const AtomicFetchAdd, AtomicCAS, AtomicContended = 0, 1, 2
+
+type Atomics struct {
+	N                      int
+	RowMask                uint32
+	Kind                   int
+	Ops, Reps, Lanes       int
+	CallSeq                uint64
+	Native                 []uint8
+	Measured               []bool
+	Status                 []int32
+	NsMin, NsMedian, NsMax []float32
+	Digest                 []uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
@@ -105,4 +121,5 @@ func (*Probe) Latency(int, int) (Latency, error) { return Latency{}, ErrUnsuppor
 func (*Probe) PingPong(int, int, bool) (PingPong, error) {
 	return PingPong{}, ErrUnsupported
 }
+func (*Probe) Atomics(int, int, int) (Atomics, error) { return Atomics{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -33,6 +33,7 @@ OPT_WARMUP, OPT_WARMUP_BYTES, OPT_DEBUG_SKIP_RANK = 8, 9, 10
 OPT_CTAS_RANK, OPT_MIN_FRACTION_PPM, OPT_LINK_PEAK_MBPS, OPT_SOLO_RANK, OPT_ALL_RANK_BARRIERS = 11, 12, 13, 14, 15
 OPT_PAIR_BARRIERS = 16
 OPT_PINGPONG_FAULT = 17
+OPT_ATOMICS_FAULT = 18
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -43,6 +44,11 @@ LATENCY_MAX_HOPS, LATENCY_MAX_REPS = 1 << 20, 64
 
 PINGPONG_DEFAULT_TRIPS, PINGPONG_DEFAULT_REPS = 256, 8
 PINGPONG_MAX_TRIPS, PINGPONG_MAX_REPS = 1 << 16, 64
+
+ATOMIC_FETCH_ADD, ATOMIC_CAS, ATOMIC_CONTENDED = 0, 1, 2
+ATOMIC_KIND_NAMES = ("fetch_add", "cas", "contended")
+ATOMICS_DEFAULT_OPS, ATOMICS_DEFAULT_REPS = 1024, 8
+ATOMICS_MAX_OPS, ATOMICS_MAX_REPS = 1 << 16, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
 
@@ -269,6 +275,33 @@ class PingPongT(C.Structure):
     ]
 
 
+class AtomicsT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("kind", C.c_uint32),
+        ("ops", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("lanes", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("measured", C.c_uint8 * _N2),
+        ("native", C.c_uint8 * _N2),
+        ("status", C.c_int32 * _N2),
+        ("ns_min", C.c_float * _N2),
+        ("ns_median", C.c_float * _N2),
+        ("ns_max", C.c_float * _N2),
+        ("digest", C.c_uint64 * _N2),
+        ("ms", C.c_double),
+    ]
+
+
+def atomics_fault(issuer: int, target: int) -> int:
+    """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
+    return ((issuer + 1) << 16) | (target + 1)
+
+
 def pingpong_fault(initiator: int, target: int, trip: int) -> int:
     """The CDPROBE_OPT_PINGPONG_FAULT value that arms a skip-ahead echo at `trip` of timed rep 1 of cell
     (initiator, target)."""
@@ -296,6 +329,7 @@ SYMBOLS = {
     "cdprobe_diagnose": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(DiagT)]),
     "cdprobe_latency": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(LatencyT)]),
     "cdprobe_pingpong": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PingPongT)]),
+    "cdprobe_atomics": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(AtomicsT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

@@ -975,6 +975,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_PINGPONG_FAULT:  // checked against the call's arguments by cdprobe_pingpong
       h->pp_fault = value;
       return CDPROBE_OK;
+    case CDPROBE_OPT_ATOMICS_FAULT:  // checked against the domain by cdprobe_atomics
+      h->at_fault = value;
+      return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;
   }

@@ -85,6 +85,8 @@ struct cdprobe {
   int32_t fault_local = -1;   // local rank whose Ctrl holds the armed landing fault (cdprobe_corrupt_landing), -1: none
   uint64_t pp_calls = 0;      // cdprobe_pingpong calls that ran (call_seq of the last one)
   uint64_t pp_fault = 0;      // CDPROBE_OPT_PINGPONG_FAULT value, 0: disarmed
+  uint64_t at_calls = 0;      // cdprobe_atomics calls that ran (call_seq of the last one)
+  uint64_t at_fault = 0;      // CDPROBE_OPT_ATOMICS_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 

@@ -1,11 +1,13 @@
-// measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency and cdprobe_pingpong.
-// Each runs on the local ranks' own streams, between probe runs, and has its results on the host before it returns.
+// measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong and
+// cdprobe_atomics.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
+// before it returns.
 #include <string.h>
 
 #include <algorithm>
 #include <string>
 #include <vector>
 
+#include "atomics.h"
 #include "diagnose.h"
 #include "handle.h"
 #include "latency.h"
@@ -52,8 +54,8 @@ static int fetch_reps(cdprobe* h, LocalRank& L, uint32_t cells, TimedRep* got, c
   return CDPROBE_OK;
 }
 
-// Fills cell idx of a cdprobe_latency_t or cdprobe_pingpong_t from its rep table: the warm-up rep, then `reps` timed
-// reps of `per_rep` hops or round trips each.  The digest covers every rep that ran; a CDPROBE_ERR_TIMEOUT rep ends the
+// Fills cell idx of a cdprobe_latency_t, cdprobe_pingpong_t or cdprobe_atomics_t from its rep table: the warm-up rep,
+// then `reps` timed reps of `per_rep` hops, round trips or atomics each.  The digest covers every rep that ran; a CDPROBE_ERR_TIMEOUT rep ends the
 // cell, which then has no times.  Any other non-zero rep status is kept, and a digest other than `want` makes the cell
 // CDPROBE_ERR_INTEGRITY.  The latency kernel writes only 0 or CDPROBE_ERR_TIMEOUT, so for latency this is the rule
 // "stop at the first non-zero status".
@@ -415,6 +417,111 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
       cdp::summarize(got.data() + (size_t)r * cdp::kRepSlots, reps, trips, want[li][r],
                      h->lr[li].grank * CDPROBE_MAX_GPUS + R.partner, out);
     }
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->kind = kind;
+  out->ops = ops != 0 ? ops : cdp::kAtomicsDefaultOps;
+  out->reps = reps != 0 ? reps : cdp::kAtomicsDefaultReps;
+  out->lanes = kind == CDPROBE_ATOMIC_CONTENDED ? 32u : 1u;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  if (kind > CDPROBE_ATOMIC_CONTENDED || out->ops > cdp::kAtomicsMaxOps || out->reps > cdp::kMaxTimedReps) {
+    cdp::set_err("kind must be a CDPROBE_ATOMIC_*, ops at most 1 << 16 and reps at most 64");
+    return CDPROBE_ERR_ARG;
+  }
+  uint32_t f_issuer = cdp::kMaxRanks, f_target = cdp::kMaxRanks;
+  if (h->at_fault != 0) {
+    const uint64_t fi = h->at_fault >> 16, ft = h->at_fault & 0xffffu;
+    if (fi == 0 || ft == 0 || fi > n || ft > n || (fi == ft && !pl.diag)) {
+      cdp::set_err("the armed atomics fault names no cell of this domain");
+      return CDPROBE_ERR_ARG;
+    }
+    f_issuer = (uint32_t)fi - 1;
+    f_target = (uint32_t)ft - 1;
+  }
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  ops = out->ops;
+  reps = out->reps;
+  const uint64_t total = (uint64_t)out->lanes * ops;  // increments per rep
+  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++h->at_calls;
+
+  // 1. every local issuer's cells, all launched before any is waited for; no kernel waits on another rank
+  cdp::AtomicsParams P[cdp::kMaxRanks];
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    out->row_mask |= 1u << g;
+    cdp::AtomicsParams& p = P[li];
+    memset(&p, 0, sizeof(p));
+    p.call_seq = h->at_calls;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.ops = ops;
+    p.reps = reps;
+    p.fault_cell = cdp::kAtomicsNoFault;
+    for (uint32_t j = 0; j < n; ++j) {
+      const uint32_t idx = g * CDPROBE_MAX_GPUS + j;
+      // native atomics: a device is atomic with itself; a peer in another process has a device this one cannot see
+      const cdp::LocalRank* peer = j >= h->first && j < h->first + h->n_local ? &h->lr[j - h->first] : nullptr;
+      int native = 1;
+      if (peer == nullptr) {
+        native = 2;
+      } else if (peer->ordinal != L.ordinal) {
+        CDP_RT(cudaDeviceGetP2PAttribute(&native, cudaDevP2PAttrNativeAtomicSupported, L.ordinal, peer->ordinal));
+        native = native != 0 ? 1 : 0;
+      }
+      out->native[idx] = (uint8_t)native;
+      if (j == g && !pl.diag) continue;  // no loop-back slot
+      const int32_t s = cdp::cell_status(h, li, j);
+      if (s != 0) {  // never touch a mapping that is down
+        out->status[idx] = s;
+        continue;
+      }
+      if (native == 0) {
+        out->status[idx] = CDPROBE_ERR_UNSUPPORTED;
+        continue;
+      }
+      if (g == f_issuer && j == f_target) p.fault_cell = p.n_cells;
+      cdp::AtomicsCell& c = p.cell[p.n_cells++];
+      c.word = reinterpret_cast<unsigned long long*>(L.va[j] + cdp::kAtomOff + (uint64_t)g * sizeof(cdp::AtomLine));
+      c.issuer = g;
+      c.target = j;
+    }
+    if (p.n_cells == 0) continue;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    const cudaError_t e = (cudaError_t)cdp::atomics_launch(p, kind, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch atomics kernel", e);
+    }
+  }
+
+  // 2. while they run: the digest of clean reps, the same for every cell
+  uint64_t want = 0;
+  for (uint32_t r = 0; r <= reps; ++r) want ^= cdp::atomics_rep_digest(cdp::atomics_start(h->at_calls, kind, r), total);
+
+  // 3. collect: ns per atomic of the timed reps, the digest of all of them
+  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::AtomicsParams& p = P[li];
+    if (p.n_cells == 0) continue;
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_cells, got.data(), "cdprobe_atomics"); rc != CDPROBE_OK)
+      return rc;
+    for (uint32_t k = 0; k < p.n_cells; ++k)
+      cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, (uint32_t)total, want,
+                     p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
   }
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;

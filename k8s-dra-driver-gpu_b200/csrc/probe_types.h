@@ -376,4 +376,39 @@ CDP_HD inline uint64_t pingpong_rep_digest(uint64_t call_seq, uint32_t round, ui
   return ((trips & 1u) ? base : 0ull) | (x << 1) | (uint64_t)(trips & 1u);
 }
 
+// ---- remote atomics (cdprobe_atomics, DESIGN §5e) ------------------------------------------------------------
+// One 128-byte line per issuer after the pingpong lines: word 0 of atom[i] in rank j's Ctrl granule is cell (i, j)'s
+// word, and only issuer i ever touches it, so no two cells or processes contend.  Open zeroes the whole granule; the
+// reset after an aborted run and every other call leave these lines alone.
+struct alignas(128) AtomLine {
+  unsigned long long v;
+  unsigned long long pad[15];
+};
+constexpr uint64_t kAtomOff = kPingOff + kMaxRanks * sizeof(FlagLine);  // 66 KiB
+static_assert(kAtomOff >= kPingOff + kMaxRanks * sizeof(FlagLine) && kAtomOff % 128 == 0 &&
+                  kAtomOff + kMaxRanks * sizeof(AtomLine) <= kCtrlBytes,
+              "the atomics lines sit after the pingpong lines inside the Ctrl granule");
+
+// The value a rep's opening exch stores.  Bits [0, 22): zero, room for the 32 x 2^16 increments of the largest rep;
+// [22, 29): rep (0 = the warm-up); [29, 31): kind; [31, 63): the low 32 bits of call_seq.  Bit 63 is always 0, so
+// `1 + (r >> 63)` is 1 for every value the word holds.
+constexpr uint32_t kAtomRepShift = 22, kAtomKindShift = 29, kAtomCallShift = 31;
+CDP_HD inline uint64_t atomics_start(uint64_t call_seq, uint32_t kind, uint32_t rep) {
+  return ((call_seq & 0xFFFFFFFFull) << kAtomCallShift) | ((uint64_t)(kind & 3u) << kAtomKindShift) |
+         ((uint64_t)(rep & 127u) << kAtomRepShift);
+}
+// Xor of start, start + 1, ..., start + total - 1: the values one clean rep's increments return, over every lane
+// (total = lanes x ops < 2^22).  The low bits of start are zero, so start + k = start | k, and the xor is start (when
+// total is odd) | the xor of 0 .. total - 1.
+CDP_HD inline uint64_t atomics_rep_digest(uint64_t start, uint64_t total) {
+  if (total == 0) return 0;
+  const uint64_t m = total - 1;  // xor of 0 .. m
+  const uint64_t x = (m & 3u) == 0 ? m : (m & 3u) == 1 ? 1 : (m & 3u) == 2 ? m + 1 : 0;
+  return ((total & 1u) ? start : 0ull) | x;
+}
+// Sum of the same values mod 2^64: what the warp's returns add up to in a clean CONTENDED rep.
+CDP_HD inline uint64_t atomics_rep_sum(uint64_t start, uint64_t total) {
+  return total * start + (total & 1u ? total * ((total - 1) / 2) : (total / 2) * (total - 1));
+}
+
 }  // namespace cdp

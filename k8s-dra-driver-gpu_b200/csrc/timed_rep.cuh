@@ -1,5 +1,5 @@
 // timed_rep.cuh — the per-rep record the timed measurements leave in device memory (cdprobe_latency,
-// cdprobe_pingpong), and the %globaltimer reads their kernels time a rep with.
+// cdprobe_pingpong, cdprobe_atomics), and the %globaltimer reads their kernels time a rep with.
 #pragma once
 #include <stdint.h>
 

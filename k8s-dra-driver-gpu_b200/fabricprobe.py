@@ -267,6 +267,38 @@ class PingPong:
                         call_seq=t.call_seq, **_timed_cells(t))
 
 
+@dataclasses.dataclass
+class Atomics:
+    """What cdprobe_atomics measured: n x n matrices [issuer][target] of ns per system-scope atomic on the cell's own
+    word in the target's memory (min, median and max over the timed reps) and the digest of the values the atomics
+    returned.  `native` is 1 (same device, or CUDA reports native atomics), 0 (CUDA reports none: not run) or 2 (the
+    target's device is not visible in this process) for the local rows, None elsewhere.  A cell that did not run is
+    None in every matrix but `status` and `native`; a cell that passed timeout_ms has a digest but no times."""
+    n: int
+    row_mask: int
+    kind: int
+    ops: int
+    reps: int
+    lanes: int
+    call_seq: int
+    native: List[List[Optional[int]]]
+    measured: List[List[bool]]
+    status: List[List[int]]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; ERR_UNSUPPORTED; else the mapping's status
+    ns_min: List[List[Optional[float]]]
+    ns_median: List[List[Optional[float]]]
+    ns_max: List[List[Optional[float]]]
+    digest: List[List[Optional[int]]]
+    ms: float
+    raw: abi.AtomicsT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.AtomicsT) -> "Atomics":
+        return Atomics(n=t.n, row_mask=t.row_mask, kind=t.kind, ops=t.ops, reps=t.reps, lanes=t.lanes,
+                       call_seq=t.call_seq,
+                       native=_mat(t, t.native, lambda k: t.row_mask >> (k // abi.MAX_GPUS) & 1),
+                       **_timed_cells(t))
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -398,6 +430,19 @@ class Probe:
         """The bare ABI call: (return code, abi.PingPongT as the library left it)."""
         t = abi.PingPongT()
         rc = self._lib.cdprobe_pingpong(self._h, trips, reps, fenced, C.byref(t))
+        return rc, t
+
+    def Atomics(self, kind: int, ops: int = 0, reps: int = 0) -> Atomics:
+        """Go: (*Probe).Atomics.  Remote atomics of every cell whose issuer is local (kind: abi.ATOMIC_*; 0: 1024 ops
+        per lane, 8 timed reps).  One-sided, not collective.  Needs no Run first and disturbs none."""
+        rc, t = self.atomics_raw(kind, ops, reps)
+        _check(self._lib, rc, "cdprobe_atomics")
+        return Atomics.from_c(t)
+
+    def atomics_raw(self, kind: int, ops: int, reps: int):
+        """The bare ABI call: (return code, abi.AtomicsT as the library left it)."""
+        t = abi.AtomicsT()
+        rc = self._lib.cdprobe_atomics(self._h, kind, ops, reps, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
