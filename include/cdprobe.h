@@ -140,7 +140,8 @@ typedef struct {
   uint32_t aborted;                     /* 1: a device watchdog fired */
   uint32_t warmed;                      /* 1: this run streamed the link wake-up prefix (phase 0) */
   uint32_t reserved1;
-  double probe_ms;                      /* host wall clock of this cdprobe_run call */
+  double probe_ms;                      /* host wall clock of this cdprobe_run call, up to the moment every local row is
+                                           published; the kernels retire after it, so event_ms may exceed it by a few us */
   double device_ms[CDPROBE_MAX_GPUS];   /* per local rank: first barrier release -> last arrive (%globaltimer) */
   double barrier_us[CDPROBE_MAX_GPUS];  /* per local rank: sum of (release - arrive) over all barriers */
   double event_ms[CDPROBE_MAX_GPUS];    /* per local rank: kernel duration by CUDA events on the launch stream
