@@ -351,6 +351,42 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_atomics_t;
 
+/* Bandwidth versus transfer size per ordered pair (cdprobe_bwcurve): issuer i's GPU reads growing prefixes of the
+ * source slice it reads from target j, through i's mapping of j, on the probe's read data path and grid (DESIGN §5f).
+ * Cells are row-major [issuer * CDPROBE_MAX_GPUS + target]; size k of a cell is [cell][k]. */
+#define CDPROBE_BWCURVE_MAX_SIZES 24  /* bytes_per_pair up to 32 GiB */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
+  uint32_t n_sizes;                     /* entries of size[] */
+  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_bwcurve calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes read per rep: 4096 << k for every 4096 << k < bytes_per_pair,
+                                               then bytes_per_pair */
+  uint8_t measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];  /* 1: the cell ran */
+  int32_t status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) differs from
+                                                             the pattern's; CDPROBE_ERR_TIMEOUT: the cell's kernel passed
+                                                             timeout_ms (no times); else the mapping's status */
+  uint32_t bad_sizes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* bit k set: a rep of size[k], warm-up included, read a
+                                                              checksum other than the pattern's */
+  float t0_ns[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];       /* ns_median of size[0] */
+  float peak_gbps[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* max over k of size[k] / ns_median[k] (bytes per ns) */
+  uint64_t half_bytes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* the smallest size[k] whose size[k] / ns_median[k]
+                                                               reaches peak / 2 (computed before peak is rounded) */
+  float ns_min[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* ns per rep over the timed reps
+                                                                                      (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* element reps / 2 of the sorted
+                                                                                      reps */
+  float ns_max[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];
+  uint64_t sum[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* checksum S the last timed rep
+                                                                                      read */
+  uint64_t xr[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];     /* checksum X */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_bwcurve_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -374,10 +410,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics: diagnostics, benches, fault injection; the reference has no
- *   counterpart (it has no probe, SURVEY.md F1).
- *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong and cdprobe_atomics are optional for callers: a daemon binds
- *   them with dlsym and works without.
+ *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve: diagnostics, benches, fault injection; the
+ *   reference has no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics and cdprobe_bwcurve are optional for callers:
+ *   a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -478,6 +514,21 @@ CDPROBE_API int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, ui
  * ops and reps whatever the return code.  CDPROBE_ERR_ARG: null argument, kind > 2, ops > 1 << 16, reps > 64, or an
  * armed CDPROBE_OPT_ATOMICS_FAULT that names no cell of the domain; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* out);
+/* Bandwidth versus transfer size of every cell whose issuer is local to this process: for each size of the ladder,
+ * one untimed warm-up rep, then `reps` timed reps, each reading the first size bytes of the source slice the issuer
+ * reads from the target (written only at open, so no run is needed first) with the issuer's whole probe grid on the
+ * CDPROBE_OPT_PATH data path.  A rep runs between two grid barriers and is timed as a probe phase is, by %globaltimer
+ * from the barrier's release to the last CTA's completion.  Every rep's (S, X) is checked against the pattern
+ * (bad_sizes, CDPROBE_ERR_INTEGRITY).  The cells run in the tournament's rounds (cdprobe_plan partner table), both
+ * ranks of a pair at once, every round after every kernel of the round before has finished in every process; with a
+ * loop-back slice (n == 1 or CDPROBE_FLAG_LOCAL_DIAG) a last round reads the diagonal.  A cell whose mapping is down
+ * is not read (measured = 0, the mapping status).  A cell whose kernel passes timeout_ms is CDPROBE_ERR_TIMEOUT and the
+ * handle stays usable.  Collective when world_size > 1: every process calls it with the same reps, and fills the rows
+ * of its own ranks (row_mask).  Touches no result, pattern, landing slot, Ctrl word, pingpong or atomics line, run_seq
+ * or warm-up state.  *out carries abi, n and reps whatever the return code.  CDPROBE_ERR_ARG: null argument,
+ * reps > 64, bytes_per_pair > 32 GiB, or arguments that differ between processes; CDPROBE_ERR_STATE: sticky
+ * handle. */
+CDPROBE_API int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -33,6 +33,7 @@ typedef int (*diag_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdpro
 typedef int (*lat_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_latency_t*);
 typedef int (*pp_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_pingpong_t*);
 typedef int (*at_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_atomics_t*);
+typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -41,6 +42,7 @@ static diag_fn cdp_diag;  // optional: absent from libraries that predate cdprob
 static lat_fn cdp_lat;    // optional: absent from libraries that predate cdprobe_latency
 static pp_fn cdp_pp;      // optional: absent from libraries that predate cdprobe_pingpong
 static at_fn cdp_at;      // optional: absent from libraries that predate cdprobe_atomics
+static bw_fn cdp_bw;      // optional: absent from libraries that predate cdprobe_bwcurve
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -56,6 +58,7 @@ static int cdp_load(const char* path) {
   cdp_lat = (lat_fn)dlsym(cdp_dl, "cdprobe_latency");
   cdp_pp = (pp_fn)dlsym(cdp_dl, "cdprobe_pingpong");
   cdp_at = (at_fn)dlsym(cdp_dl, "cdprobe_atomics");
+  cdp_bw = (bw_fn)dlsym(cdp_dl, "cdprobe_bwcurve");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -80,6 +83,8 @@ static int cdp_has_atomics(void) { return cdp_at != NULL; }
 static int cdp_call_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* at) {
   return cdp_at(h, kind, ops, reps, at);
 }
+static int cdp_has_bwcurve(void) { return cdp_bw != NULL; }
+static int cdp_call_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* bw) { return cdp_bw(h, reps, bw); }
 */
 import "C"
 
@@ -228,6 +233,26 @@ type Atomics struct {
 	Status                 []int32   // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; CDPROBE_ERR_UNSUPPORTED; else the mapping's status
 	NsMin, NsMedian, NsMax []float32 // ns per atomic over the timed reps
 	Digest                 []uint64  // xor of every value the atomics returned
+	Ms                     float64
+}
+
+// BwCurve is the bandwidth-versus-size curve of the local rows (cdprobe_bwcurve_t).  Per-cell slices are N x N
+// row-major, [issuer*N + target]; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
+// cell was not measured or timed out.
+type BwCurve struct {
+	N                      int
+	RowMask                uint32      // rows of this process's ranks
+	Reps                   int         // timed reps per size, as applied
+	Path                   int         // the read data path (CDPROBE_OPT_PATH)
+	CallSeq                uint64      // 1-based count of BwCurve calls on this handle, equal in every process
+	Sizes                  []uint64    // bytes read per rep
+	Measured               []bool
+	Status                 []int32     // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the mapping's status
+	BadSizes               []uint32    // bit k: a rep of Sizes[k] read a checksum other than the pattern's
+	T0Ns, PeakGBps         []float32   // median ns of the smallest size; max over sizes of size / median ns
+	HalfBytes              []uint64    // the smallest size reaching half the peak
+	NsMin, NsMedian, NsMax [][]float32 // [cell][size]: ns per rep over the timed reps
+	Sum, Xr                [][]uint64  // [cell][size]: (S, X) of the last timed rep
 	Ms                     float64
 }
 
@@ -486,6 +511,65 @@ func (p *Probe) Atomics(kind, ops, reps int) (Atomics, error) {
 			out.NsMedian[i*n+j] = float32(at.ns_median[k])
 			out.NsMax[i*n+j] = float32(at.ns_max[k])
 			out.Digest[i*n+j] = uint64(at.digest[k])
+		}
+	}
+	return out, nil
+}
+
+// BwCurve reads growing prefixes of every local issuer's source slices on the probe's read path and grid, in the
+// tournament's rounds, and reports ns per rep for each size (reps 0: 8 timed reps); every rep's checksum is checked.
+// Collective when the domain spans processes.  ErrUnsupported when the library predates cdprobe_bwcurve.
+func (p *Probe) BwCurve(reps int) (BwCurve, error) {
+	if C.cdp_has_bwcurve() == 0 {
+		return BwCurve{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_bwcurve", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	bw := new(C.cdprobe_bwcurve_t)
+	rc := C.cdp_call_bwcurve(p.h, C.uint32_t(reps), bw)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_bwcurve: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return BwCurve{}, err
+	}
+	n, ns := int(bw.n), int(bw.n_sizes)
+	out := BwCurve{N: n, RowMask: uint32(bw.row_mask), Reps: int(bw.reps), Path: int(bw.path),
+		CallSeq: uint64(bw.call_seq), Ms: float64(bw.ms)}
+	out.Sizes = make([]uint64, ns)
+	for s := 0; s < ns; s++ {
+		out.Sizes[s] = uint64(bw.size[s])
+	}
+	out.Measured = make([]bool, n*n)
+	out.Status = make([]int32, n*n)
+	out.BadSizes = make([]uint32, n*n)
+	out.T0Ns = make([]float32, n*n)
+	out.PeakGBps = make([]float32, n*n)
+	out.HalfBytes = make([]uint64, n*n)
+	out.NsMin = make([][]float32, n*n)
+	out.NsMedian = make([][]float32, n*n)
+	out.NsMax = make([][]float32, n*n)
+	out.Sum = make([][]uint64, n*n)
+	out.Xr = make([][]uint64, n*n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < n; j++ {
+			k, c := i*C.CDPROBE_MAX_GPUS+j, i*n+j
+			out.Measured[c] = bw.measured[k] != 0
+			out.Status[c] = int32(bw.status[k])
+			out.BadSizes[c] = uint32(bw.bad_sizes[k])
+			out.T0Ns[c] = float32(bw.t0_ns[k])
+			out.PeakGBps[c] = float32(bw.peak_gbps[k])
+			out.HalfBytes[c] = uint64(bw.half_bytes[k])
+			out.NsMin[c], out.NsMedian[c], out.NsMax[c] = make([]float32, ns), make([]float32, ns), make([]float32, ns)
+			out.Sum[c], out.Xr[c] = make([]uint64, ns), make([]uint64, ns)
+			for s := 0; s < ns; s++ {
+				out.NsMin[c][s] = float32(bw.ns_min[k][s])
+				out.NsMedian[c][s] = float32(bw.ns_median[k][s])
+				out.NsMax[c][s] = float32(bw.ns_max[k][s])
+				out.Sum[c][s] = uint64(bw.sum[k][s])
+				out.Xr[c][s] = uint64(bw.xr[k][s])
+			}
 		}
 	}
 	return out, nil

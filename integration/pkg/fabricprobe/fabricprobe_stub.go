@@ -112,6 +112,23 @@ type Atomics struct {
 	Ms                     float64
 }
 
+type BwCurve struct {
+	N                      int
+	RowMask                uint32
+	Reps                   int
+	Path                   int
+	CallSeq                uint64
+	Sizes                  []uint64
+	Measured               []bool
+	Status                 []int32
+	BadSizes               []uint32
+	T0Ns, PeakGBps         []float32
+	HalfBytes              []uint64
+	NsMin, NsMedian, NsMax [][]float32
+	Sum, Xr                [][]uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
@@ -122,4 +139,5 @@ func (*Probe) PingPong(int, int, bool) (PingPong, error) {
 	return PingPong{}, ErrUnsupported
 }
 func (*Probe) Atomics(int, int, int) (Atomics, error) { return Atomics{}, ErrUnsupported }
+func (*Probe) BwCurve(int) (BwCurve, error) { return BwCurve{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -50,6 +50,9 @@ ATOMIC_KIND_NAMES = ("fetch_add", "cas", "contended")
 ATOMICS_DEFAULT_OPS, ATOMICS_DEFAULT_REPS = 1024, 8
 ATOMICS_MAX_OPS, ATOMICS_MAX_REPS = 1 << 16, 64
 
+BWCURVE_MAX_SIZES = 24
+BWCURVE_DEFAULT_REPS, BWCURVE_MAX_REPS = 8, 64
+
 _N2 = MAX_GPUS * MAX_GPUS
 
 
@@ -297,6 +300,31 @@ class AtomicsT(C.Structure):
     ]
 
 
+class BwCurveT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("n_sizes", C.c_uint32),
+        ("path", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("size", C.c_uint64 * BWCURVE_MAX_SIZES),
+        ("measured", C.c_uint8 * _N2),
+        ("status", C.c_int32 * _N2),
+        ("bad_sizes", C.c_uint32 * _N2),
+        ("t0_ns", C.c_float * _N2),
+        ("peak_gbps", C.c_float * _N2),
+        ("half_bytes", C.c_uint64 * _N2),
+        ("ns_min", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("ns_median", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("ns_max", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("sum", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("xr", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("ms", C.c_double),
+    ]
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -330,6 +358,7 @@ SYMBOLS = {
     "cdprobe_latency": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(LatencyT)]),
     "cdprobe_pingpong": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PingPongT)]),
     "cdprobe_atomics": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(AtomicsT)]),
+    "cdprobe_bwcurve": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(BwCurveT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

@@ -1,6 +1,6 @@
-// measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong and
-// cdprobe_atomics.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
-// before it returns.
+// measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
+// cdprobe_atomics and cdprobe_bwcurve.  Each runs on the local ranks' own streams, between probe runs, and has its
+// results on the host before it returns.
 #include <string.h>
 
 #include <algorithm>
@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "atomics.h"
+#include "bwcurve.h"
 #include "diagnose.h"
 #include "handle.h"
 #include "latency.h"
@@ -41,11 +42,10 @@ static int ensure_rep_tables(cdprobe* h) {
   return CDPROBE_OK;
 }
 
-// Copies local rank L's first `cells` rep tables to `got` once its kernel is done.
-static int fetch_reps(cdprobe* h, LocalRank& L, uint32_t cells, TimedRep* got, const char* what) {
+// Copies the first `bytes` of local rank L's scratch (its rep tables) to `got` once its kernel is done.
+static int fetch_reps(cdprobe* h, LocalRank& L, size_t bytes, void* got, const char* what) {
   cudaError_t e = cudaSetDevice(L.ordinal);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(got, L.scratch, sizeof(TimedRep) * cells * kRepSlots, cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(got, L.scratch, bytes, cudaMemcpyDeviceToHost, L.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
   if (e != cudaSuccess) {
     h->sticky = true;  // a failed kernel leaves the context unusable
@@ -83,6 +83,46 @@ static void summarize(const TimedRep* rep, uint32_t reps, uint32_t per_rep, uint
     if (digest != want) s = CDPROBE_ERR_INTEGRITY;
   }
   out->status[idx] = s;
+}
+
+// Fills cell idx of a cdprobe_bwcurve_t from the records bwcurve_kernel left in `s`: per size, ns of the timed reps
+// and the (S, X) of the last one, every rep's (S, X) compared with want[k] (bad_sizes), and the model-free summary of
+// the medians.  A cell whose kernel was aborted at the deadline has no times.
+static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes,
+                         uint32_t reps, uint32_t idx, cdprobe_bwcurve_t* out) {
+  out->measured[idx] = 1;
+  if (s.abort_flag != 0) {
+    out->status[idx] = CDPROBE_ERR_TIMEOUT;
+    return;
+  }
+  uint32_t bad = 0;
+  double rate[kBwMaxSizes], peak = 0.0;
+  for (uint32_t k = 0; k < n_sizes; ++k) {
+    float ns[kMaxTimedReps];
+    for (uint32_t r = 0; r <= reps; ++r) {
+      const Acc& a = s.rep[k][r];
+      if (a.sum != want[k][0] || a.xr != want[k][1]) bad |= 1u << k;
+      if (r > 0) ns[r - 1] = (float)(a.t_end - s.t_rel[k][r]);
+    }
+    std::sort(ns, ns + reps);
+    out->ns_min[idx][k] = ns[0];
+    out->ns_median[idx][k] = ns[reps / 2];
+    out->ns_max[idx][k] = ns[reps - 1];
+    out->sum[idx][k] = s.rep[k][reps].sum;
+    out->xr[idx][k] = s.rep[k][reps].xr;
+    rate[k] = ns[reps / 2] > 0.f ? (double)size[k] / (double)ns[reps / 2] : 0.0;
+    peak = std::max(peak, rate[k]);
+  }
+  out->t0_ns[idx] = out->ns_median[idx][0];
+  out->peak_gbps[idx] = (float)peak;
+  for (uint32_t k = 0; k < n_sizes; ++k) {
+    if (rate[k] >= peak / 2) {
+      out->half_bytes[idx] = size[k];
+      break;
+    }
+  }
+  out->bad_sizes[idx] = bad;
+  out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
 }
 
 }  // namespace cdp
@@ -250,8 +290,8 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
   for (uint32_t li = 0; li < h->n_local; ++li) {
     const cdp::LatencyParams& p = P[li];
     if (p.n_cells == 0) continue;
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_cells, got.data(), "cdprobe_latency"); rc != CDPROBE_OK)
-      return rc;
+    const size_t bytes = sizeof(cdp::TimedRep) * p.n_cells * cdp::kRepSlots;
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_latency"); rc != CDPROBE_OK) return rc;
     for (uint32_t k = 0; k < p.n_cells; ++k)
       cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, hops, want[li][k],
                      p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
@@ -409,8 +449,8 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
   for (uint32_t li = 0; li < h->n_local; ++li) {
     if (!launched[li]) continue;
     const cdp::PingPongParams& p = P[li];
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_rounds, got.data(), "cdprobe_pingpong"); rc != CDPROBE_OK)
-      return rc;
+    const size_t bytes = sizeof(cdp::TimedRep) * p.n_rounds * cdp::kRepSlots;
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_pingpong"); rc != CDPROBE_OK) return rc;
     for (uint32_t r = 0; r < p.n_rounds; ++r) {
       const cdp::PingPongRound& R = p.round[r];
       if (R.remote == nullptr) continue;
@@ -517,11 +557,157 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
   for (uint32_t li = 0; li < h->n_local; ++li) {
     const cdp::AtomicsParams& p = P[li];
     if (p.n_cells == 0) continue;
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], p.n_cells, got.data(), "cdprobe_atomics"); rc != CDPROBE_OK)
-      return rc;
+    const size_t bytes = sizeof(cdp::TimedRep) * p.n_cells * cdp::kRepSlots;
+    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_atomics"); rc != CDPROBE_OK) return rc;
     for (uint32_t k = 0; k < p.n_cells; ++k)
       cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, (uint32_t)total, want,
                      p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+// What each process contributes at the start of cdprobe_bwcurve, so that every process refuses or runs the same call.
+// Every cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree.
+struct BwCurveAgree {
+  uint64_t call_seq;
+  uint32_t reps, ok;
+};
+
+int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->reps = reps != 0 ? reps : cdp::kBwDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  out->path = h->path;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together
+  std::string bad;
+  uint64_t size[cdp::kBwMaxSizes];
+  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
+  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
+  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
+  BwCurveAgree mine = {h->bw_calls + 1, reps, bad.empty() ? 1u : 0u};
+  if (h->cfg.world_size > 1) {
+    std::vector<BwCurveAgree> all(h->cfg.world_size);
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    for (const BwCurveAgree& o : all) {
+      if (!o.ok && bad.empty()) bad = "another process called cdprobe_bwcurve with invalid arguments";
+      if ((o.call_seq != mine.call_seq || o.reps != reps) && bad.empty())
+        bad = "cdprobe_bwcurve is collective: every process must call it with the same arguments";
+    }
+  }
+  if (!bad.empty()) {
+    cdp::set_err(bad);
+    return CDPROBE_ERR_ARG;
+  }
+  h->bw_calls = mine.call_seq;
+  out->call_seq = h->bw_calls;
+  out->n_sizes = n_sizes;
+  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+
+  // 2. scratch for the rep records and one cell's granule table, grown on every local rank before any kernel runs
+  const uint64_t granules = pl.bpp / cdp::kGranuleBytes;
+  const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    CDP_RT(cudaSetDevice(h->lr[li].ordinal));
+    if (const int rc = cdp::ensure_scratch(h->lr[li], table_off + 16 * granules); rc != CDPROBE_OK) return rc;
+  }
+
+  // 3. the (S, X) each size of each cell that runs must read, from the pattern definition: the per-granule sums of the
+  //    slice on the issuer's GPU, folded into every prefix on the host
+  bool runs[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  std::vector<uint64_t> want((size_t)cdp::kMaxRanks * cdp::kMaxRanks * cdp::kBwMaxSizes * 2);
+  auto want_of = [&](uint32_t li, uint32_t j) {
+    return reinterpret_cast<uint64_t(*)[2]>(want.data() + ((size_t)li * cdp::kMaxRanks + j) * cdp::kBwMaxSizes * 2);
+  };
+  std::vector<uint64_t> table(2 * granules);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g && !pl.diag) continue;  // no loop-back slice
+      const int32_t s = cdp::cell_status(h, li, j);
+      if (s != 0) {  // never read through a mapping that is down
+        out->status[g * CDPROBE_MAX_GPUS + j] = s;
+        continue;
+      }
+      runs[li][j] = true;
+      const uint64_t first = (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8);
+      uint64_t* gsum = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(L.scratch) + table_off);
+      cudaError_t e = (cudaError_t)cdp::bwcurve_granules_launch(gsum, gsum + granules, h->seed, j, first, granules,
+                                                                 (unsigned)L.sm_count * 8u, L.stream);
+      if (e == cudaSuccess && granules)
+        e = cudaMemcpyAsync(table.data(), gsum, 16 * granules, cudaMemcpyDeviceToHost, L.stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+      if (e != cudaSuccess) {
+        h->sticky = true;
+        return cdp::fail_cuda("cdprobe_bwcurve: granule checksums", e);
+      }
+      uint64_t(*w)[2] = want_of(li, j);
+      for (uint32_t k = 0; k < n_sizes; ++k)
+        cdp::bwcurve_prefix_checksum(table.data(), table.data() + granules, h->seed, j, first, size[k] / 8, &w[k][0],
+                                     &w[k][1]);
+    }
+  }
+
+  // 4. the rounds: the tournament's, then the loop-back; every local kernel of a round is launched before any is
+  //    waited for, and no process starts a round before every process has finished the one before
+  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
+  std::vector<cdp::BwScratch> got(1);
+  const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
+  for (uint32_t r = 0; r < n_rounds; ++r) {
+    if (h->cfg.world_size > 1) {
+      std::string err;
+      if (h->rdv.barrier(&err) != 0) {
+        cdp::set_err(err);
+        return CDPROBE_ERR_RENDEZVOUS;
+      }
+    }
+    int32_t target[cdp::kMaxRanks];
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      cdp::LocalRank& L = h->lr[li];
+      const int q = r < pl.rounds ? pl.partner[r][L.grank] : (int)L.grank;
+      target[li] = q >= 0 && runs[li][q] ? q : -1;
+      if (target[li] < 0) continue;
+      cdp::BwCurveParams p;
+      memset(&p, 0, sizeof(p));
+      p.region = reinterpret_cast<const uint8_t*>(L.va[q]) + cdp::cell_offset(pl, CDPROBE_OP_READ, L.grank, (uint32_t)q);
+      p.scratch = static_cast<cdp::BwScratch*>(L.scratch);
+      memcpy(p.size, size, sizeof(size));
+      p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+      p.n_sizes = n_sizes;
+      p.reps = reps;
+      p.path = h->path;
+      CDP_RT(cudaSetDevice(L.ordinal));
+      cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::BwScratch), L.stream);
+      if (e == cudaSuccess) e = (cudaError_t)cdp::bwcurve_launch(p, L.ctas, L.coop && coop_ok, L.stream);
+      if (e != cudaSuccess) {
+        h->sticky = true;
+        return cdp::fail_cuda("launch bwcurve_kernel", e);
+      }
+    }
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      if (target[li] < 0) continue;
+      cdp::LocalRank& L = h->lr[li];
+      if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::BwScratch), got.data(), "cdprobe_bwcurve"); rc != CDPROBE_OK)
+        return rc;
+      cdp::bw_summarize(got[0], want_of(li, (uint32_t)target[li]), size, n_sizes, reps,
+                        L.grank * CDPROBE_MAX_GPUS + (uint32_t)target[li], out);
+    }
   }
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;

@@ -18,6 +18,9 @@
 //                   ld.acquire.sys on the local copy.
 // K4 verify/local : the read probe pointed at local HBM (landing slots, source
 //                   slices at open, the N = 1 loop-back).
+// K5 bwcurve      : cdprobe_bwcurve's reads of growing prefixes of one source
+//                   slice through the K1 read path, one launch per cell, each
+//                   rep between two grid barriers (bwcurve_kernel).
 //
 // One persistent cooperative kernel per GPU runs every phase of a probe
 // (wake-up, tournament rounds x {write, read + overlapped verify}) so a run
@@ -30,6 +33,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "bwcurve.h"
 #include "probe_launch.h"
 #include "probe_types.h"
 
@@ -138,7 +142,7 @@ __device__ __forceinline__ uint64_t pack64(uint32_t lo, uint32_t hi) { return (u
 
 // ------------------------------------------------------------- context -----
 struct Ctx {
-  Ctrl* ctrl;
+  unsigned int* abort_word;  // the launch's abort flag: Ctrl::abort_flag, or BwScratch::abort_flag (bwcurve_kernel)
   uint64_t deadline;
   uint32_t stage_smem;   // shared address of this warp's stage 0
   uint32_t bar_smem;     // shared address of this warp's mbarrier 0
@@ -147,13 +151,13 @@ struct Ctx {
 };
 
 __device__ __forceinline__ bool aborted(const Ctx& c) {
-  return *reinterpret_cast<volatile unsigned int*>(&c.ctrl->abort_flag) != 0u;
+  return *reinterpret_cast<volatile unsigned int*>(c.abort_word) != 0u;
 }
 // Slow-path check used inside spin loops: watchdog + abort propagation.
 __device__ __noinline__ bool check_abort(const Ctx& c) {
   if (aborted(c)) return true;
   if (gtimer() > c.deadline) {
-    atomicExch(&c.ctrl->abort_flag, 1u);
+    atomicExch(c.abort_word, 1u);
     return true;
   }
   return false;
@@ -551,10 +555,9 @@ __device__ __forceinline__ void signal_ranks(const ProbeParams& P, uint32_t mask
 // A system-scope fence precedes the flag stores only when this rank published something the receiver acts on at
 // this barrier (write checksums; the verdicts at the last barrier): reads leave nothing in flight, and each CTA
 // already fenced its own remote stores before it arrived.
-__device__ void barrier(const ProbeParams& P, Ctx& c, int b, uint32_t sync, uint32_t post, bool last) {
+__device__ void barrier(const ProbeParams& P, Ctx& c, Ctrl* ctrl, int b, uint32_t sync, uint32_t post, bool last) {
   __syncthreads();
   if (threadIdx.x == 0) {
-    Ctrl* ctrl = c.ctrl;
     // the deadline is checked at every arrival, not only inside long waits: a run whose waits all stay short
     // would otherwise finish past timeout_ms without the watchdog ever firing
     const bool ab = check_abort(c);
@@ -653,8 +656,7 @@ __device__ __forceinline__ void cta_reduce(const Ctx& c, uint64_t* red, const Su
 
 // The result row, written into pinned host memory by one whole CTA (every thread calls this), then the
 // accumulators are cleared for the next run.  Phase p ran from t_rel[p] to t_arr[p + 1].
-__device__ void write_row(const ProbeParams& P, const Ctx& c, uint64_t t_enter) {
-  Ctrl* ctrl = c.ctrl;
+__device__ void write_row(const ProbeParams& P, const Ctx& c, Ctrl* ctrl, uint64_t t_enter) {
   ResultRow* row = P.row;
   const bool ab = aborted(c);
   const uint32_t t = threadIdx.x;
@@ -742,13 +744,12 @@ __device__ __forceinline__ bool is_loopback(const ProbeParams& P) {
 // completes the slot's count applies it between two __threadfence and then adds 1, and the verifiers wait for that.
 // The CTA that finishes last (lb.done) publishes the write checksum and the verdict,
 // writes the row and zeroes the counters for the next run.
-__device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint64_t t_enter) {
+__device__ void loopback_pass(const ProbeParams& P, Ctx& c, Ctrl* ctrl, uint64_t* red, uint64_t t_enter) {
   constexpr int kRed = 6 + 5;  // per warp: (sum, xor) x 3 jobs (cta_reduce), end time x 3 jobs, first issue x 2 jobs
   static_assert(kWarpsPerCta * (kStages + kRed) * 8 <= kSmemBytes - kWarpsPerCta * kStages * kUnitBytes,
                 "mbarriers + reduction slots fit the tail of the dynamic shared memory");
   __shared__ bool s_last;
   __shared__ uint64_t s_t_enter;
-  Ctrl* ctrl = c.ctrl;
   LoopBack* lb = &ctrl->lb;
   const Job wj = P.phase[0].job[0];
   uint8_t* self = P.base_peer[P.rank];
@@ -835,7 +836,7 @@ __device__ void loopback_pass(const ProbeParams& P, Ctx& c, uint64_t* red, uint6
   }
   __syncthreads();
   if (!s_last) return;
-  write_row(P, c, s_t_enter);
+  write_row(P, c, ctrl, s_t_enter);
   if (threadIdx.x == 0) {
     for (int j = 0; j < 3; ++j) lb->claim[j].v = 0ull;
     lb->written.v = 0ull;
@@ -855,7 +856,8 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
   __shared__ uint64_t s_deadline;
 
   Ctx c;
-  c.ctrl = reinterpret_cast<Ctrl*>(P.base_peer[P.rank]);
+  Ctrl* const ctrl = reinterpret_cast<Ctrl*>(P.base_peer[P.rank]);
+  c.abort_word = &ctrl->abort_flag;
   c.warp = threadIdx.x >> 5;
   c.lane = threadIdx.x & 31;
   c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
@@ -875,11 +877,11 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
   c.deadline = s_deadline;
 
   if (is_loopback(P)) {
-    loopback_pass(P, c, red, s_enter);
+    loopback_pass(P, c, ctrl, red, s_enter);
     return;
   }
 
-  barrier(P, c, 0, P.peer_mask, 0u, false);
+  barrier(P, c, ctrl, 0, P.peer_mask, 0u, false);
 
   for (uint32_t ph = 0; ph < P.n_phases; ++ph) {
     const Phase& phd = P.phase[ph];
@@ -906,7 +908,7 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
           // schedule put no wait between that phase and this one (post_mask), this job does the waiting
           bool go = true;
           if (job.salt != 0 && job.writer != P.rank && P.base_peer[job.writer] != nullptr) {
-            if (threadIdx.x == 0) spin_until<kScopeSys>(c, &c.ctrl->flags[job.writer].v, P.seq_base + job.salt + 1ull);
+            if (threadIdx.x == 0) spin_until<kScopeSys>(c, &ctrl->flags[job.writer].v, P.seq_base + job.salt + 1ull);
             __syncthreads();
             go = !aborted(c);
           }
@@ -920,18 +922,18 @@ __global__ void __launch_bounds__(kThreads, 1) cdprobe_kernel(const __grid_const
         }
       }
       // CTA reduce -> one atomic per CTA into the phase accumulator
-      Acc* const acc = &c.ctrl->acc[ph][jb];
+      Acc* const acc = &ctrl->acc[ph][jb];
       cta_reduce<1>(c, red, &a, &acc);
       if (threadIdx.x == 0) {
         if (job.kind == kJobWrite) __threadfence_system();  // stores have reached the peer
         atomicMax(&acc->t_end, (unsigned long long)gtimer());
       }
     }
-    barrier(P, c, (int)ph + 1, phd.sync_mask & P.peer_mask, phd.post_mask & P.peer_mask, ph + 1 == P.n_phases);
+    barrier(P, c, ctrl, (int)ph + 1, phd.sync_mask & P.peer_mask, phd.post_mask & P.peer_mask, ph + 1 == P.n_phases);
   }
 
   // ---- output: CTA 0 writes the result row ----------------------------------
-  if (blockIdx.x == 0) write_row(P, c, s_enter);
+  if (blockIdx.x == 0) write_row(P, c, ctrl, s_enter);
 }
 
 // ------------------------------------------------------- source pattern ----
@@ -940,6 +942,98 @@ __global__ void __launch_bounds__(256) cdprobe_fill_src_kernel(uint4* dst, uint6
   for (uint64_t v = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
     const uint64_t w0 = src_word(seed, rank, 2 * v), w1 = src_word(seed, rank, 2 * v + 1);
     dst[v] = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
+  }
+}
+
+// ------------------------------------------- K5: bandwidth versus size ----
+namespace {
+// Grid barrier b of a bwcurve_kernel launch, called by every thread.  Arrivals count on one word that only rises, so
+// barrier b is complete at (b + 1) x gridDim.x arrivals; the CTA that completes it stamps *t_rel and releases b + 1.
+// Returns false in every thread once the launch is aborted (the deadline is checked at every arrival, as in barrier()).
+__device__ bool grid_sync(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long long* t_rel) {
+  __shared__ bool s_go;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    bool go = !check_abort(c);
+    if (go) {
+      const unsigned int prev = atomicAdd(&bs->arrive, 1u);
+      if (prev == (b + 1u) * gridDim.x - 1u) {
+        *t_rel = gtimer();
+        st_release_gpu(&bs->release, b + 1ull);
+      } else {
+        go = spin_until<kScopeGpu>(c, &bs->release, b + 1ull);
+      }
+    }
+    s_go = go;
+  }
+  __syncthreads();
+  return s_go;
+}
+}  // namespace
+
+// One cell of cdprobe_bwcurve: for every size of the ladder, one warm-up and P.reps timed reps, each reading the first
+// size bytes of the cell's source slice with every warp of the grid (the strided walk of a probe phase, on the data
+// path the probe uses) and folding them into the (S, X) checksum.  Reps are separated by grid barriers, so a rep is
+// timed as a probe phase is: from the barrier's release stamp to the latest CTA completion stamp.  Every piece of
+// state (barrier, stamps, checksums, abort word) is in the rank's scratch buffer; Ctrl is not touched.
+__global__ void __launch_bounds__(kThreads, 1) bwcurve_kernel(const __grid_constant__ BwCurveParams P) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
+  uint64_t* red = bars + kWarpsPerCta * kStages;
+  __shared__ uint64_t s_deadline;
+  BwScratch* bs = P.scratch;
+
+  Ctx c;
+  c.abort_word = &bs->abort_flag;
+  c.warp = threadIdx.x >> 5;
+  c.lane = threadIdx.x & 31;
+  c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
+  c.bar_smem = smem_u32(bars) + c.warp * kStages * 8u;
+  c.parity_bits = 0u;
+  if (threadIdx.x == 0) s_deadline = gtimer() + P.timeout_ns;
+  if (c.lane == 0) {
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) mbar_init(c.bar_smem + 8u * s, 1u);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  c.deadline = s_deadline;
+
+  const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
+  const uint32_t nwarps = gridDim.x * kWarpsPerCta;
+  uint32_t b = 0;
+  for (uint32_t k = 0; k < P.n_sizes; ++k) {
+    const uint64_t bytes = P.size[k];
+    for (uint32_t r = 0; r <= P.reps; ++r, ++b) {
+      if (!grid_sync(c, bs, b, &bs->t_rel[k][r])) return;
+      Sum a{0ull, 0ull, 0ull};
+      read_units(c, P.path, P.region, bytes, strided(bytes, gwarp, nwarps), a);
+      Acc* const acc = &bs->rep[k][r];
+      cta_reduce<1>(c, red, &a, &acc);
+      if (threadIdx.x == 0) atomicMax(&acc->t_end, (unsigned long long)gtimer());
+    }
+  }
+}
+
+// The per-granule (sum, xor) of a source region from the pattern definition: one warp per 16 KiB granule.
+__global__ void __launch_bounds__(256) bwcurve_granules_kernel(uint64_t* gsum, uint64_t* gxor, uint64_t seed,
+                                                                uint32_t rank, uint64_t first_word, uint64_t n_granules) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+  for (uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n_granules; g += nwarps) {
+    const uint64_t w0 = first_word + g * kGranuleWords;
+    uint64_t s = 0, x = 0;
+    for (uint32_t k = lane; k < kGranuleWords; k += 32) {
+      const uint64_t w = src_word(seed, rank, w0 + k);
+      s += w;
+      x ^= w;
+    }
+    s = warp_sum64(s);
+    x = warp_xor64(x);
+    if (lane == 0) {
+      gsum[g] = s;
+      gxor[g] = x;
+    }
   }
 }
 
@@ -967,6 +1061,27 @@ int probe_kernel_launch(const ProbeParams* p, unsigned grid, bool cooperative, c
 
 int probe_fill_launch(void* dst, uint64_t bytes, uint64_t seed, uint32_t rank, unsigned grid, cudaStream_t stream) {
   cdprobe_fill_src_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<uint4*>(dst), bytes / 16, seed, rank);
+  return (int)cudaGetLastError();
+}
+
+int bwcurve_launch(const BwCurveParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
+  cudaError_t e = cudaFuncSetAttribute(bwcurve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  if (e != cudaSuccess) return (int)e;
+  void* args[] = {const_cast<BwCurveParams*>(&p)};
+  if (cooperative) {
+    e = cudaLaunchCooperativeKernel((const void*)bwcurve_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
+  } else {
+    e = cudaLaunchKernel((const void*)bwcurve_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
+  }
+  return (int)e;
+}
+
+int bwcurve_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t rank, uint64_t first_word,
+                            uint64_t n_granules, unsigned grid, cudaStream_t stream) {
+  if (n_granules == 0) return (int)cudaSuccess;
+  const uint64_t need = (n_granules + 7) / 8;  // eight warps per block
+  bwcurve_granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, seed, rank, first_word,
+                                                                                    n_granules);
   return (int)cudaGetLastError();
 }
 

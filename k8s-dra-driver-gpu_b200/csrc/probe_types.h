@@ -411,4 +411,42 @@ CDP_HD inline uint64_t atomics_rep_sum(uint64_t start, uint64_t total) {
   return total * start + (total & 1u ? total * ((total - 1) / 2) : (total / 2) * (total - 1));
 }
 
+// ---- the bandwidth-versus-size curve (cdprobe_bwcurve, DESIGN §5f) -------------------------------------------------
+constexpr uint32_t kBwMaxSizes = 24;     // CDPROBE_BWCURVE_MAX_SIZES
+constexpr uint64_t kBwMinSize = 4096;
+constexpr uint64_t kGranuleWords = kGranuleBytes / 8;
+
+// The sizes a cell is read at: 4096 << k for every k with 4096 << k < bpp, then bpp itself.  Returns how many, or 0
+// when that is more than kBwMaxSizes (bpp > 32 GiB).  size has room for kBwMaxSizes.
+CDP_HD inline uint32_t bwcurve_ladder(uint64_t bpp, uint64_t* size) {
+  uint32_t n = 0;
+  for (uint64_t s = kBwMinSize; s < bpp; s <<= 1) {
+    if (n == kBwMaxSizes) return 0;
+    size[n++] = s;
+  }
+  if (n == kBwMaxSizes) return 0;
+  size[n++] = bpp;
+  return n;
+}
+
+// (S, X) of the first n_words words of a source region, words first_word... of rank's pattern, from gsum[g] and gxor[g],
+// the sum and xor of the words of each whole granule g of the region.  The words of a last, partial granule (at most
+// kGranuleWords - 1) are generated from src_word here.
+CDP_HD inline void bwcurve_prefix_checksum(const uint64_t* gsum, const uint64_t* gxor, uint64_t seed, uint32_t rank,
+                                           uint64_t first_word, uint64_t n_words, uint64_t* sum, uint64_t* xr) {
+  const uint64_t whole = n_words / kGranuleWords;
+  uint64_t s = 0, x = 0, px = 0;
+  for (uint64_t g = 0; g < whole; ++g) {
+    s += gsum[g];
+    x ^= rotl64(gxor[g], fold6((uint32_t)g));
+  }
+  for (uint64_t k = whole * kGranuleWords; k < n_words; ++k) {
+    const uint64_t w = src_word(seed, rank, first_word + k);
+    s += w;
+    px ^= w;
+  }
+  *sum = s;
+  *xr = x ^ rotl64(px, fold6((uint32_t)whole));
+}
+
 }  // namespace cdp

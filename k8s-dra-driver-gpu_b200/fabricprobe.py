@@ -299,6 +299,52 @@ class Atomics:
                        **_timed_cells(t))
 
 
+@dataclasses.dataclass
+class BwCurve:
+    """What cdprobe_bwcurve measured: per cell [issuer][target], ns per rep (min, median and max over the timed reps)
+    of reading each size of the ladder `sizes` from the source slice the issuer reads, the (S, X) of the last timed
+    rep, the sizes whose reads did not match the pattern (`bad_sizes`, bit k for sizes[k]) and the summary of the
+    medians: t0_ns (the smallest size), peak_gbps and half_bytes.  Per-size values are lists over `sizes`.  A cell
+    that did not run is None everywhere but `status`; a cell that passed timeout_ms has no times."""
+    n: int
+    row_mask: int
+    reps: int
+    path: int
+    call_seq: int
+    sizes: List[int]
+    measured: List[List[bool]]
+    status: List[List[int]]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the mapping's status
+    bad_sizes: List[List[Optional[int]]]
+    t0_ns: List[List[Optional[float]]]
+    peak_gbps: List[List[Optional[float]]]
+    half_bytes: List[List[Optional[int]]]
+    ns_min: List[List[Optional[List[float]]]]
+    ns_median: List[List[Optional[List[float]]]]
+    ns_max: List[List[Optional[List[float]]]]
+    sum: List[List[Optional[List[int]]]]
+    xr: List[List[Optional[List[int]]]]
+    ms: float
+    raw: abi.BwCurveT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.BwCurveT) -> "BwCurve":
+        k = t.n_sizes
+
+        def timed(c):
+            return t.measured[c] and t.status[c] != abi.ERR_TIMEOUT
+
+        def per_size(a):
+            return [list(x)[:k] for x in a]
+
+        return BwCurve(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
+                       sizes=list(t.size)[:k], measured=_mat(t, [bool(m) for m in t.measured]),
+                       status=_mat(t, t.status), bad_sizes=_mat(t, t.bad_sizes, timed),
+                       t0_ns=_mat(t, t.t0_ns, timed), peak_gbps=_mat(t, t.peak_gbps, timed),
+                       half_bytes=_mat(t, t.half_bytes, timed), ns_min=_mat(t, per_size(t.ns_min), timed),
+                       ns_median=_mat(t, per_size(t.ns_median), timed), ns_max=_mat(t, per_size(t.ns_max), timed),
+                       sum=_mat(t, per_size(t.sum), timed), xr=_mat(t, per_size(t.xr), timed), ms=t.ms, raw=t)
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -443,6 +489,20 @@ class Probe:
         """The bare ABI call: (return code, abi.AtomicsT as the library left it)."""
         t = abi.AtomicsT()
         rc = self._lib.cdprobe_atomics(self._h, kind, ops, reps, C.byref(t))
+        return rc, t
+
+    def BwCurve(self, reps: int = 0) -> BwCurve:
+        """Go: (*Probe).BwCurve.  Bandwidth versus transfer size of every cell whose issuer is local, on the probe's
+        read path and grid (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first and
+        disturbs none."""
+        rc, t = self.bwcurve_raw(reps)
+        _check(self._lib, rc, "cdprobe_bwcurve")
+        return BwCurve.from_c(t)
+
+    def bwcurve_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.BwCurveT as the library left it)."""
+        t = abi.BwCurveT()
+        rc = self._lib.cdprobe_bwcurve(self._h, reps, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
