@@ -133,7 +133,8 @@ typedef struct {
   uint64_t sum_write[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* checksum of the pattern the issuer generated */
   uint64_t xor_write[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];
   uint64_t bytes_per_pair;
-  uint64_t run_seq;                     /* 1-based count of cdprobe_run on this handle */
+  uint64_t run_seq;                     /* sequence number of this run on the handle: the source checksum pass of
+                                           cdprobe_open is 1, so the first cdprobe_run is 2, and each run adds 1 */
   uint32_t rounds;                      /* tournament rounds (N-1 for even N) */
   uint32_t phases;                      /* device phases executed */
   uint32_t launches;                    /* kernels launched by this call (one per local rank) */
@@ -423,7 +424,8 @@ CDPROBE_API int cdprobe_info(cdprobe_t* h, cdprobe_info_t* out);
 CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out);
 /* Runtime options (no reopen needed; the bench sweeps them). */
 #define CDPROBE_OPT_EVENT_TIMING 1u  /* value 0/1: bracket each kernel with CUDA events, report event_ms */
-#define CDPROBE_OPT_CTAS 2u          /* CTAs of the persistent kernel (0 = one per SM) */
+#define CDPROBE_OPT_CTAS 2u          /* CTAs of the persistent kernel (0 = one per SM; capped at what fits the device);
+                                        CDPROBE_ERR_ARG and the handle unchanged for a value over UINT32_MAX */
 #define CDPROBE_OPT_PATH 3u          /* 0 = TMA bulk copies, 1 = ld/st.global.v4 (128-bit), 2 = ld/st.global.v4, 32 contiguous bytes per lane */
 #define CDPROBE_OPT_TIMEOUT_MS 4u
 #define CDPROBE_OPT_OVERLAP_VERIFY 5u /* value 0/1 */
@@ -432,7 +434,9 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
 #define CDPROBE_OPT_WARMUP 8u        /* link wake-up phase: 0 never, 1 auto = after > 5 ms idle (default), 2 always */
 #define CDPROBE_OPT_DEBUG_SKIP_RANK 10u /* fault injection: 1-based local rank whose kernel is not launched (0 = off) */
 #define CDPROBE_OPT_WARMUP_BYTES 9u  /* bytes each rank streams from its first partner when warming (default 8 MiB, capped at bytes_per_pair) */
-#define CDPROBE_OPT_CTAS_RANK 11u    /* value = ((local rank + 1) << 16) | ctas: CTA count of ONE local rank (tests: a throttled issuer) */
+#define CDPROBE_OPT_CTAS_RANK 11u    /* value = ((local rank + 1) << 16) | ctas: CTA count of ONE local rank (tests: a throttled issuer);
+                                        CDPROBE_ERR_ARG and the handle unchanged when ctas is 0 or value >> 16 is not a
+                                        local rank + 1 (bits above 16 included) */
 #define CDPROBE_OPT_MIN_FRACTION_PPM 12u /* min_fraction x 1e6 (0 = default) */
 #define CDPROBE_OPT_LINK_PEAK_MBPS 13u   /* link_peak_gbps x 1e3 (0 = default reference) */
 #define CDPROBE_OPT_SOLO_RANK 14u    /* profiling: 1-based local rank that runs ALONE — only its own read/write jobs, no

@@ -914,6 +914,8 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       h->event_timing = value != 0;
       return CDPROBE_OK;
     case CDPROBE_OPT_CTAS:
+      // a value truncated to 32 bits could become 0 CTAs: a grid no launch accepts
+      if (value > UINT32_MAX) return CDPROBE_ERR_ARG;
       for (uint32_t li = 0; li < h->n_local; ++li) {
         cdp::LocalRank& L = h->lr[li];
         uint32_t c = value ? (uint32_t)value : (uint32_t)L.sm_count;
@@ -939,7 +941,8 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return cdp::set_flag(h, CDPROBE_FLAG_PAIR_BARRIERS, value != 0);
     case CDPROBE_OPT_CTAS_RANK:
     {
-      const uint32_t li = (uint32_t)(value >> 16), c = (uint32_t)(value & 0xffffu);
+      const uint64_t li = value >> 16;  // not truncated: stray high bits must not name another rank
+      const uint32_t c = (uint32_t)(value & 0xffffu);
       if (li == 0 || li > h->n_local || c == 0) return CDPROBE_ERR_ARG;
       cdp::LocalRank& L = h->lr[li - 1];
       L.ctas = c > (uint32_t)L.max_ctas ? (uint32_t)L.max_ctas : c;
