@@ -76,7 +76,11 @@ extern "C" {
 #define CDPROBE_FLAG_OVERLAP_VERIFY 0x20u  /* verify landing slots on spare CTAs while the next round runs (default) */
 #define CDPROBE_FLAG_SIMULATE_MIG 0x200u   /* treat every local GPU as a MIG instance (BASELINE config 4 without MIG hardware) */
 #define CDPROBE_FLAG_SERIAL_VERIFY 0x100u  /* opt out of the overlapped verify: verify every slot after the rounds */
-#define CDPROBE_FLAG_ALLOW_SAME_DEVICE 0x40u /* several ranks may name the same CUDA ordinal (testing) */
+#define CDPROBE_FLAG_ALLOW_SAME_DEVICE 0x40u /* several ranks may name the same CUDA ordinal (testing).  Each rank
+                                              has its own stream; with more than 8 ranks on one device in one
+                                              process, set CUDA_DEVICE_MAX_CONNECTIONS >= the rank count before the
+                                              process creates its CUDA context, or two ranks' kernels may share a
+                                              hardware queue and one wait behind the other at a barrier */
 #define CDPROBE_FLAG_ALL_RANK_BARRIERS 0x400u /* every tournament phase closes with an all-rank flag exchange (round-1
                                               behaviour); default: only the ranks whose traffic shares an NVLink
                                               port with this rank's in the two phases either side of the barrier */

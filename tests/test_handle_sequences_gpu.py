@@ -17,6 +17,7 @@ model alone, so rerunning that one test reproduces it.  Several ranks share GPU 
 rank's persistent kernel stays resident), so the file runs on one H100.  No step aborts a run, injects a watchdog
 timeout or touches more than 4 GiB.
 """
+import ctypes as C
 import json
 import random
 import subprocess
@@ -127,6 +128,18 @@ class Driver:
                     if f in w:
                         assert getattr(got, f)[i][j] == w[f], (what, f, i, j, getattr(got, f)[i][j], w[f])
 
+    def table_fits(self, name, value):
+        """Whether cdprobe_schedule accepts every local rank's table with schedule option `name` set to `value`
+        (UNIDIRECTIONAL with the serial verify overflows the phase table from N = 13)."""
+        if name not in ("OPT_UNIDIRECTIONAL", "OPT_OVERLAP_VERIFY", "OPT_ALL_RANK_BARRIERS", "OPT_PAIR_BARRIERS"):
+            return True
+        m, flag = self.m, getattr(self.a, "FLAG" + name[3:])
+        flags = (m.flags & ~flag) | (flag if value else 0)
+        flags = flags if flags & hm.FLAG_OVERLAP_VERIFY else flags | hm.FLAG_SERIAL_VERIFY
+        s = self.a.ScheduleT()
+        return all(self.p._lib.cdprobe_schedule(self.n, g, self.nbytes, m.mode, m.ops, flags, m.ctas_of(g),
+                                                m.verify_ctas, C.byref(s)) == 0 for g in m.local)
+
     # ---- steps -----------------------------------------------------------------------------------------------
     def set_option(self, name, value):
         rc = self.p._lib.cdprobe_set_option(self.p._h, getattr(self.a, name), value)
@@ -162,7 +175,12 @@ class Driver:
             else:
                 self.check_run(p.Run(), exp)
         elif kind == "opt":
-            self.set_option(step[1], step[2])
+            if self.table_fits(step[1], step[2]):
+                self.set_option(step[1], step[2])
+            else:  # the schedule has no room for the phase table these flags ask for: refused, nothing changes
+                with pytest.raises(Refused) as e:
+                    self.set_option(step[1], step[2])
+                assert e.value.args[0] == a.ERR_ARG, (step, e.value.args)
             self.check_info()
         elif kind == "bad_opt":  # an out-of-range value: refused, nothing changes
             before = [p.Info().ctas[li] for li in range(self.n_local)]
@@ -243,21 +261,23 @@ class Driver:
 
 
 # ---- the seeded walk -------------------------------------------------------------------------------------------
-def gen_step(rng, m, same_device=True, two_procs=False, me=0):
-    """One step drawn from `rng` and the model's state alone (never from a device result)."""
+def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
+    """One step drawn from `rng` and the model's state alone (never from a device result).  `ctas_cap` bounds the
+    grids it may ask for, so that many same-device ranks stay resident together."""
     n, W = m.n, m.W
+    grids = [c for c in (1, 2, 3, 7, 8) if ctas_cap is None or c <= ctas_cap]
     x = rng.random()
     if x < 0.28:
         return ("run",)
     if x < 0.48:
-        ctas = [1, 2, 3, 7, 8] + ([0] if n == 1 or not same_device else [])
+        ctas = grids + ([0] if n == 1 or not same_device else [])
         name, values = rng.choice([
             ("OPT_PATH", [0, 1, 2]), ("OPT_CTAS", ctas), ("OPT_VERIFY_CTAS", [1, 2, 3, 32]),
             ("OPT_UNIDIRECTIONAL", [0, 1]), ("OPT_OVERLAP_VERIFY", [0, 1]), ("OPT_ALL_RANK_BARRIERS", [0, 1]),
             ("OPT_PAIR_BARRIERS", [0, 1]), ("OPT_WARMUP", [0, 2]), ("OPT_WARMUP_BYTES", [0, 128, m.bpp + 4096]),
             ("OPT_CTAS_RANK", None)])
         if name == "OPT_CTAS_RANK":
-            return ("opt", name, (rng.randrange(1, len(m.local) + 1) << 16) | rng.choice([1, 2, 3, 7, 8]))
+            return ("opt", name, (rng.randrange(1, len(m.local) + 1) << 16) | rng.choice(grids))
         return ("opt", name, rng.choice(values))
     if x < 0.51:
         return ("bad_opt",) + rng.choice([("OPT_PATH", 3), ("OPT_VERIFY_CTAS", 0), ("OPT_WARMUP", 3),
