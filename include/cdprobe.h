@@ -392,6 +392,43 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_bwcurve_t;
 
+/* One-shot all-reduce across the domain (cdprobe_allreduce): every rank r reads the first size bytes of every rank's
+ * source buffer, its own and the peers' through its mappings, and sums them word by word mod 2^64 into its own memory
+ * (DESIGN §5g).  Rows are ranks: entry [r] is rank r, and size k of rank r is [r][k].  The times are per rank; the
+ * algorithm bandwidth is size / ns, and each rank's NVLink ingress is (n - 1) x that. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
+  uint32_t n_sizes;                     /* entries of size[] */
+  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_allreduce calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per input and of the output per rep: the cdprobe_bwcurve ladder */
+  uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank ran */
+  int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) or the word check differs from
+                                           the pattern's sum; CDPROBE_ERR_TIMEOUT: the rank's kernel passed timeout_ms
+                                           (no times); else the mapping status of the domain's first cell that is down,
+                                           row-major, which stops every rank */
+  uint32_t bad_sizes[CDPROBE_MAX_GPUS]; /* bit k set: a rep of size[k], warm-up included, stored an output whose (S, X)
+                                           differs, or the word check of size[k] found a bad word */
+  float t0_ns[CDPROBE_MAX_GPUS];        /* ns_median of size[0] */
+  float peak_gbps[CDPROBE_MAX_GPUS];    /* max over k of size[k] / ns_median[k] (bytes per ns): algorithm bandwidth */
+  uint64_t half_bytes[CDPROBE_MAX_GPUS]; /* the smallest size[k] whose size[k] / ns_median[k] reaches peak / 2
+                                            (computed before peak is rounded) */
+  float ns_min[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* ns per rep over the timed reps (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];
+  uint64_t sum[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* checksum S of the output the last timed rep stored */
+  uint64_t xr[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];     /* checksum X */
+  uint64_t bad_words[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* words of that output that differ from the sum of
+                                                                      the pattern words (the word check) */
+  uint64_t first_bad[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* byte offset of the first of them; UINT64_MAX when
+                                                                      clean */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_allreduce_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -415,10 +452,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve: diagnostics, benches, fault injection; the
- *   reference has no counterpart (it has no probe, SURVEY.md F1).
- *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics and cdprobe_bwcurve are optional for callers:
- *   a daemon binds them with dlsym and works without.
+ *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce: diagnostics, benches,
+ *   fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve and cdprobe_allreduce are
+ *   optional for callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -456,6 +493,11 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              cdprobe_atomics: in the process that hosts the issuer, the first op of timed
                                              rep 1 of cell (issuer, target) adds 2 (CAS: swaps in v + 2), so exactly
                                              that cell fails its checks; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_FAULT 19u   /* tests: value = ((rank + 1) << 32) | ((k + 1) << 24) | word arms an off-by-one
+                                             in cdprobe_allreduce: in the process that hosts `rank`, timed rep 1 of
+                                             size[k] adds 1 to output word `word` (< 2^24) before it is stored and
+                                             folded, so exactly that row and size fail the checksum (and the word check
+                                             when reps == 1); 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -537,6 +579,24 @@ CDPROBE_API int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint3
  * reps > 64, bytes_per_pair > 32 GiB, or arguments that differ between processes; CDPROBE_ERR_STATE: sticky
  * handle. */
 CDPROBE_API int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out);
+/* One-shot all-reduce of every rank's source buffer, on every rank at once: for each size of the cdprobe_bwcurve
+ * ladder, one untimed warm-up rep, then `reps` timed reps.  In a rep, rank r reads the first size bytes of every rank's
+ * source buffer (written only at open, so no run is needed first), adding rank r, r + 1, ... (mod n) in that order, on
+ * the CDPROBE_OPT_PATH read path with its whole probe grid, and stores the sums with st.global.v4 into its scratch
+ * buffer.  A domain barrier opens every rep (flags in the Ctrl granule; only a grid barrier at n == 1), and a rep is
+ * timed per rank by %globaltimer from that rank's release to its last CTA's completion; ranks are released a signal
+ * latency apart, so no time is domain-wide.  Every rep's (S, X) is checked against the pattern's sum, and after the
+ * last rep of a size every output word is (bad_sizes, bad_words, CDPROBE_ERR_INTEGRITY).  If any cell of the domain
+ * is down (cdprobe_unmap_peer, a failed mapping, MIG), nothing runs: every filled row has measured = 0 and the status
+ * of the first such cell, and the call returns CDPROBE_OK.  A rank whose kernel passes timeout_ms is
+ * CDPROBE_ERR_TIMEOUT and the handle stays usable.  Collective when world_size > 1: every process calls it with the
+ * same reps and fills the rows of its own ranks (row_mask).  The output is bytes_per_pair per rank, so the scratch
+ * buffer grows by that much until close (1 GiB at n == 1 with 1 GiB).  Touches no result, pattern, landing slot, Ctrl
+ * word, pingpong or atomics line, run_seq, warm-up or bwcurve state.  *out carries abi, n and reps whatever the return
+ * code.  CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes,
+ * or an armed CDPROBE_OPT_ALLREDUCE_FAULT whose rank is >= n, whose k is >= n_sizes or whose word is
+ * >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

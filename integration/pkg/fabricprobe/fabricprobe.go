@@ -34,6 +34,7 @@ typedef int (*lat_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_latency_t*);
 typedef int (*pp_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_pingpong_t*);
 typedef int (*at_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_atomics_t*);
 typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
+typedef int (*ar_fn)(cdprobe_t*, uint32_t, cdprobe_allreduce_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -43,6 +44,7 @@ static lat_fn cdp_lat;    // optional: absent from libraries that predate cdprob
 static pp_fn cdp_pp;      // optional: absent from libraries that predate cdprobe_pingpong
 static at_fn cdp_at;      // optional: absent from libraries that predate cdprobe_atomics
 static bw_fn cdp_bw;      // optional: absent from libraries that predate cdprobe_bwcurve
+static ar_fn cdp_ar;      // optional: absent from libraries that predate cdprobe_allreduce
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -59,6 +61,7 @@ static int cdp_load(const char* path) {
   cdp_pp = (pp_fn)dlsym(cdp_dl, "cdprobe_pingpong");
   cdp_at = (at_fn)dlsym(cdp_dl, "cdprobe_atomics");
   cdp_bw = (bw_fn)dlsym(cdp_dl, "cdprobe_bwcurve");
+  cdp_ar = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -85,6 +88,8 @@ static int cdp_call_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t 
 }
 static int cdp_has_bwcurve(void) { return cdp_bw != NULL; }
 static int cdp_call_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* bw) { return cdp_bw(h, reps, bw); }
+static int cdp_has_allreduce(void) { return cdp_ar != NULL; }
+static int cdp_call_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) { return cdp_ar(h, reps, ar); }
 */
 import "C"
 
@@ -253,6 +258,26 @@ type BwCurve struct {
 	HalfBytes              []uint64    // the smallest size reaching half the peak
 	NsMin, NsMedian, NsMax [][]float32 // [cell][size]: ns per rep over the timed reps
 	Sum, Xr                [][]uint64  // [cell][size]: (S, X) of the last timed rep
+	Ms                     float64
+}
+
+// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t).  Every slice is indexed by rank; the
+// per-size ones hold one entry per Sizes element, and every timing is 0 where a rank was not measured or timed out.
+type AllReduce struct {
+	N                      int
+	RowMask                uint32      // rows of this process's ranks
+	Reps                   int         // timed reps per size, as applied
+	Path                   int         // the read data path (CDPROBE_OPT_PATH)
+	CallSeq                uint64      // 1-based count of AllReduce calls on this handle, equal in every process
+	Sizes                  []uint64    // bytes per input and of the output per rep
+	Measured               []bool
+	Status                 []int32     // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the first down cell's status
+	BadSizes               []uint32    // bit k: Sizes[k] failed the checksum or the word check
+	T0Ns, PeakGBps         []float32   // median ns of the smallest size; max over sizes of size / median ns (algbw)
+	HalfBytes              []uint64    // the smallest size reaching half the peak
+	NsMin, NsMedian, NsMax [][]float32 // [rank][size]: ns per rep over the timed reps
+	Sum, Xr                [][]uint64  // [rank][size]: (S, X) of the output of the last timed rep
+	BadWords, FirstBad     [][]uint64  // [rank][size]: the word check; FirstBad is MaxUint64 when clean
 	Ms                     float64
 }
 
@@ -570,6 +595,64 @@ func (p *Probe) BwCurve(reps int) (BwCurve, error) {
 				out.Sum[c][s] = uint64(bw.sum[k][s])
 				out.Xr[c][s] = uint64(bw.xr[k][s])
 			}
+		}
+	}
+	return out, nil
+}
+
+// AllReduce runs the one-shot all-reduce of every rank's source buffer on every rank at once, at each size of the
+// bwcurve ladder, and reports ns per rep for each size (reps 0: 8 timed reps); every rep's checksum and the last rep's
+// every word are checked.  Collective when the domain spans processes.  ErrUnsupported when the library predates
+// cdprobe_allreduce.
+func (p *Probe) AllReduce(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	ar := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce(p.h, C.uint32_t(reps), ar)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	n, ns := int(ar.n), int(ar.n_sizes)
+	out := AllReduce{N: n, RowMask: uint32(ar.row_mask), Reps: int(ar.reps), Path: int(ar.path),
+		CallSeq: uint64(ar.call_seq), Ms: float64(ar.ms)}
+	out.Sizes = make([]uint64, ns)
+	for s := 0; s < ns; s++ {
+		out.Sizes[s] = uint64(ar.size[s])
+	}
+	out.Measured = make([]bool, n)
+	out.Status = make([]int32, n)
+	out.BadSizes = make([]uint32, n)
+	out.T0Ns = make([]float32, n)
+	out.PeakGBps = make([]float32, n)
+	out.HalfBytes = make([]uint64, n)
+	out.NsMin, out.NsMedian, out.NsMax = make([][]float32, n), make([][]float32, n), make([][]float32, n)
+	out.Sum, out.Xr = make([][]uint64, n), make([][]uint64, n)
+	out.BadWords, out.FirstBad = make([][]uint64, n), make([][]uint64, n)
+	for r := 0; r < n; r++ {
+		out.Measured[r] = ar.measured[r] != 0
+		out.Status[r] = int32(ar.status[r])
+		out.BadSizes[r] = uint32(ar.bad_sizes[r])
+		out.T0Ns[r] = float32(ar.t0_ns[r])
+		out.PeakGBps[r] = float32(ar.peak_gbps[r])
+		out.HalfBytes[r] = uint64(ar.half_bytes[r])
+		out.NsMin[r], out.NsMedian[r], out.NsMax[r] = make([]float32, ns), make([]float32, ns), make([]float32, ns)
+		out.Sum[r], out.Xr[r] = make([]uint64, ns), make([]uint64, ns)
+		out.BadWords[r], out.FirstBad[r] = make([]uint64, ns), make([]uint64, ns)
+		for s := 0; s < ns; s++ {
+			out.NsMin[r][s] = float32(ar.ns_min[r][s])
+			out.NsMedian[r][s] = float32(ar.ns_median[r][s])
+			out.NsMax[r][s] = float32(ar.ns_max[r][s])
+			out.Sum[r][s] = uint64(ar.sum[r][s])
+			out.Xr[r][s] = uint64(ar.xr[r][s])
+			out.BadWords[r][s] = uint64(ar.bad_words[r][s])
+			out.FirstBad[r][s] = uint64(ar.first_bad[r][s])
 		}
 	}
 	return out, nil

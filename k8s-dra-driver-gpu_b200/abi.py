@@ -34,6 +34,7 @@ OPT_CTAS_RANK, OPT_MIN_FRACTION_PPM, OPT_LINK_PEAK_MBPS, OPT_SOLO_RANK, OPT_ALL_
 OPT_PAIR_BARRIERS = 16
 OPT_PINGPONG_FAULT = 17
 OPT_ATOMICS_FAULT = 18
+OPT_ALLREDUCE_FAULT = 19
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -52,6 +53,7 @@ ATOMICS_MAX_OPS, ATOMICS_MAX_REPS = 1 << 16, 64
 
 BWCURVE_MAX_SIZES = 24
 BWCURVE_DEFAULT_REPS, BWCURVE_MAX_REPS = 8, 64
+ALLREDUCE_DEFAULT_REPS, ALLREDUCE_MAX_REPS = 8, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
 
@@ -325,6 +327,38 @@ class BwCurveT(C.Structure):
     ]
 
 
+class AllReduceT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("n_sizes", C.c_uint32),
+        ("path", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("size", C.c_uint64 * BWCURVE_MAX_SIZES),
+        ("measured", C.c_uint8 * MAX_GPUS),
+        ("status", C.c_int32 * MAX_GPUS),
+        ("bad_sizes", C.c_uint32 * MAX_GPUS),
+        ("t0_ns", C.c_float * MAX_GPUS),
+        ("peak_gbps", C.c_float * MAX_GPUS),
+        ("half_bytes", C.c_uint64 * MAX_GPUS),
+        ("ns_min", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("ns_median", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("ns_max", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("sum", C.c_uint64 * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("xr", C.c_uint64 * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("bad_words", C.c_uint64 * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("first_bad", C.c_uint64 * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("ms", C.c_double),
+    ]
+
+
+def allreduce_fault(rank: int, k: int, word: int) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_FAULT value that makes timed rep 1 of size[k] add 1 to output word `word` on `rank`."""
+    return ((rank + 1) << 32) | ((k + 1) << 24) | word
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -359,6 +393,7 @@ SYMBOLS = {
     "cdprobe_pingpong": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PingPongT)]),
     "cdprobe_atomics": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(AtomicsT)]),
     "cdprobe_bwcurve": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(BwCurveT)]),
+    "cdprobe_allreduce": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

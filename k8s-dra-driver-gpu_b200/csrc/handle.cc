@@ -981,6 +981,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_ATOMICS_FAULT:  // checked against the domain by cdprobe_atomics
       h->at_fault = value;
       return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_FAULT:  // checked against the domain and the size ladder by cdprobe_allreduce
+      h->ar_fault = value;
+      return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;
   }

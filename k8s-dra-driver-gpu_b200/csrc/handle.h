@@ -88,6 +88,8 @@ struct cdprobe {
   uint64_t at_calls = 0;      // cdprobe_atomics calls that ran (call_seq of the last one)
   uint64_t at_fault = 0;      // CDPROBE_OPT_ATOMICS_FAULT value, 0: disarmed
   uint64_t bw_calls = 0;      // cdprobe_bwcurve calls that ran (call_seq of the last one)
+  uint64_t ar_calls = 0;      // cdprobe_allreduce calls that ran (call_seq of the last one)
+  uint64_t ar_fault = 0;      // CDPROBE_OPT_ALLREDUCE_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 

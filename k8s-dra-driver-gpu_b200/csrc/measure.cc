@@ -1,12 +1,13 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
-// cdprobe_atomics and cdprobe_bwcurve.  Each runs on the local ranks' own streams, between probe runs, and has its
-// results on the host before it returns.
+// cdprobe_atomics, cdprobe_bwcurve and cdprobe_allreduce.  Each runs on the local ranks' own streams, between probe
+// runs, and has its results on the host before it returns.
 #include <string.h>
 
 #include <algorithm>
 #include <string>
 #include <vector>
 
+#include "allreduce.h"
 #include "atomics.h"
 #include "bwcurve.h"
 #include "diagnose.h"
@@ -85,11 +86,13 @@ static void summarize(const TimedRep* rep, uint32_t reps, uint32_t per_rep, uint
   out->status[idx] = s;
 }
 
-// Fills cell idx of a cdprobe_bwcurve_t from the records bwcurve_kernel left in `s`: per size, ns of the timed reps
-// and the (S, X) of the last one, every rep's (S, X) compared with want[k] (bad_sizes), and the model-free summary of
-// the medians.  A cell whose kernel was aborted at the deadline has no times.
+// Fills entry idx of a cdprobe_bwcurve_t (a cell) or a cdprobe_allreduce_t (a row) from the records bwcurve_kernel or
+// allreduce_kernel left in `s`: per size, ns of the timed reps and the (S, X) of the last one, every rep's (S, X)
+// compared with want[k] (bad_sizes), and the model-free summary of the medians.  An entry whose kernel was aborted at
+// the deadline has no times.
+template <typename Out>
 static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes,
-                         uint32_t reps, uint32_t idx, cdprobe_bwcurve_t* out) {
+                         uint32_t reps, uint32_t idx, Out* out) {
   out->measured[idx] = 1;
   if (s.abort_flag != 0) {
     out->status[idx] = CDPROBE_ERR_TIMEOUT;
@@ -707,6 +710,191 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
         return rc;
       cdp::bw_summarize(got[0], want_of(li, (uint32_t)target[li]), size, n_sizes, reps,
                         L.grank * CDPROBE_MAX_GPUS + (uint32_t)target[li], out);
+    }
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+// What each process contributes at the start of cdprobe_allreduce, so that every process refuses, skips or runs the
+// same call.  The mapping verdict must agree too: a process that ran while another skipped would wait at the first
+// domain barrier until its watchdog fired.
+struct AllReduceAgree {
+  uint64_t call_seq;
+  uint32_t reps, ok;
+  uint32_t down_cell;    // issuer * kMaxRanks + target of this process's first cell whose mapping is down (kNoCell: none)
+  int32_t down_status;   // that cell's mapping status
+};
+static constexpr uint32_t kNoCell = ~0u;
+
+int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  cdp::g_last_error.clear();
+  if (out == nullptr) return CDPROBE_ERR_ARG;
+  // like cdprobe_run: the caller may read *out whatever the return code
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  out->path = h->path;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments, the armed fault and the mapping verdict; in a multi-process domain all three are shared below,
+  //    so every process refuses, skips or runs together
+  std::string bad;
+  uint64_t size[cdp::kBwMaxSizes];
+  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
+  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
+  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
+  uint32_t f_rank = cdp::kArNoFault, f_k = cdp::kArNoFault;
+  uint64_t f_word = 0;
+  if (h->ar_fault != 0 && bad.empty()) {
+    const uint64_t fr = h->ar_fault >> 32, fk = (h->ar_fault >> 24) & 0xffu;
+    f_word = h->ar_fault & 0xffffffu;
+    if (fr == 0 || fr > n || fk == 0 || fk > n_sizes || f_word >= size[fk - 1] / 8) {
+      bad = "the armed all-reduce fault names no rank, size or output word of this call";
+    } else {
+      f_rank = (uint32_t)fr - 1;
+      f_k = (uint32_t)fk - 1;
+    }
+  }
+  AllReduceAgree mine;
+  memset(&mine, 0, sizeof(mine));
+  mine.call_seq = h->ar_calls + 1;
+  mine.reps = reps;
+  mine.ok = bad.empty() ? 1u : 0u;
+  mine.down_cell = kNoCell;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t j = 0; j < n; ++j) {
+      const int32_t s = cdp::cell_status(h, li, j);
+      const uint32_t cell = h->lr[li].grank * cdp::kMaxRanks + j;
+      if (s != 0 && cell < mine.down_cell) {
+        mine.down_cell = cell;
+        mine.down_status = s;
+      }
+    }
+  }
+  AllReduceAgree down = mine;
+  if (h->cfg.world_size > 1) {
+    std::vector<AllReduceAgree> all(h->cfg.world_size);
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    for (const AllReduceAgree& o : all) {
+      if (!o.ok && bad.empty()) bad = "another process called cdprobe_allreduce with invalid arguments";
+      if ((o.call_seq != mine.call_seq || o.reps != reps) && bad.empty())
+        bad = "cdprobe_allreduce is collective: every process must call it with the same arguments";
+      if (o.down_cell < down.down_cell) down = o;
+    }
+  }
+  if (!bad.empty()) {
+    cdp::set_err(bad);
+    return CDPROBE_ERR_ARG;
+  }
+  h->ar_calls = mine.call_seq;
+  out->call_seq = h->ar_calls;
+  out->n_sizes = n_sizes;
+  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+  if (down.down_cell != kNoCell) {  // some rank cannot read some input: nothing runs, in any process
+    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = down.down_status;
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 2. scratch for the records, the output and the granule table, grown on every local rank before any kernel runs
+  const uint64_t granules = pl.bpp / cdp::kGranuleBytes;
+  const size_t table_off = cdp::kArOutOff + (pl.bpp + 255) / 256 * 256;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    CDP_RT(cudaSetDevice(h->lr[li].ordinal));
+    if (const int rc = cdp::ensure_scratch(h->lr[li], table_off + 16 * granules); rc != CDPROBE_OK) return rc;
+  }
+
+  // 3. the (S, X) every prefix of the output must have, from the pattern definition: the per-granule sums of the
+  //    summed words on the first local rank's GPU, folded into every prefix on the host
+  uint64_t want[cdp::kBwMaxSizes][2] = {};
+  {
+    cdp::LocalRank& L = h->lr[0];
+    std::vector<uint64_t> table(2 * granules);
+    uint64_t* gsum = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(L.scratch) + table_off);
+    CDP_RT(cudaSetDevice(L.ordinal));
+    cudaError_t e = (cudaError_t)cdp::allreduce_granules_launch(gsum, gsum + granules, h->seed, n, granules,
+                                                                 (unsigned)L.sm_count * 8u, L.stream);
+    if (e == cudaSuccess && granules)
+      e = cudaMemcpyAsync(table.data(), gsum, 16 * granules, cudaMemcpyDeviceToHost, L.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("cdprobe_allreduce: granule checksums", e);
+    }
+    for (uint32_t k = 0; k < n_sizes; ++k)
+      cdp::allreduce_prefix_checksum(table.data(), table.data() + granules, h->seed, n, size[k] / 8, &want[k][0],
+                                     &want[k][1]);
+  }
+
+  // 4. no process launches before every process is ready, so that no kernel waits at the first domain barrier for a
+  //    process still setting up; then every local kernel is launched before any is waited for
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.barrier(&err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::AllReduceParams p;
+    memset(&p, 0, sizeof(p));
+    for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + pl.src_off;
+    for (uint32_t j = 0; j < n; ++j)
+      if (j != g) p.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kArOff + (uint64_t)g * sizeof(cdp::FlagLine));
+    p.sig_in = reinterpret_cast<const cdp::FlagLine*>(L.va[g] + cdp::kArOff);
+    p.scratch = static_cast<cdp::ArScratch*>(L.scratch);
+    p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
+    memcpy(p.size, size, sizeof(size));
+    p.seed = h->seed;
+    p.call_seq = h->ar_calls;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.fault_k = g == f_rank ? f_k : cdp::kArNoFault;
+    p.fault_word = f_word;
+    p.rank = g;
+    p.n = n;
+    p.n_sizes = n_sizes;
+    p.reps = reps;
+    p.path = h->path;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::ArScratch), L.stream);
+    if (e == cudaSuccess) e = (cudaError_t)cdp::allreduce_launch(p, L.ctas, L.coop && coop_ok, L.stream);
+    if (e != cudaSuccess) {
+      h->sticky = true;
+      return cdp::fail_cuda("launch allreduce_kernel", e);
+    }
+  }
+
+  // 5. collect: per row, the times and checksums of every size, then the word checks
+  std::vector<cdp::ArScratch> got(1);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::ArScratch), got.data(), "cdprobe_allreduce"); rc != CDPROBE_OK)
+      return rc;
+    const cdp::ArScratch& s = got[0];
+    cdp::bw_summarize(s.rep, want, size, n_sizes, reps, g, out);
+    if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
+    for (uint32_t k = 0; k < n_sizes; ++k) {
+      out->bad_words[g][k] = s.bad_words[k];
+      out->first_bad[g][k] = s.bad_words[k] != 0 ? ~s.first_bad_n[k] : UINT64_MAX;
+      if (s.bad_words[k] != 0) {
+        out->bad_sizes[g] |= 1u << k;
+        out->status[g] = CDPROBE_ERR_INTEGRITY;
+      }
     }
   }
   out->ms = cdp::now_ms() - t_begin;

@@ -21,6 +21,11 @@
 // K5 bwcurve      : cdprobe_bwcurve's reads of growing prefixes of one source
 //                   slice through the K1 read path, one launch per cell, each
 //                   rep between two grid barriers (bwcurve_kernel).
+// K6 allreduce    : cdprobe_allreduce's one-shot all-reduce: every warp
+//                   streams one output unit of all n ranks' source buffers
+//                   (TMA ring or ld.global.v4), adds them in registers and
+//                   stores the sum with st.global.v4; each rep opens with a
+//                   domain barrier (allreduce_kernel).
 //
 // One persistent cooperative kernel per GPU runs every phase of a probe
 // (wake-up, tournament rounds x {write, read + overlapped verify}) so a run
@@ -33,6 +38,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "allreduce.h"
 #include "bwcurve.h"
 #include "probe_launch.h"
 #include "probe_types.h"
@@ -1037,6 +1043,291 @@ __global__ void __launch_bounds__(256) bwcurve_granules_kernel(uint64_t* gsum, u
   }
 }
 
+// ------------------------------------------- K6: one-shot all-reduce ----
+namespace {
+constexpr int kArWords = 2 * kLdstVecs;  // uint64 accumulators per lane: a warp holds one 8 KiB output unit
+
+// Byte offset in a unit of the lane's 16-byte vector i when each access moves kLaneBytes contiguous bytes: the layout
+// job_read_ldst loads in, and for kLaneBytes = 16 also the one job_read_tma reads a stage in.
+template <uint32_t kLaneBytes>
+__device__ __forceinline__ uint32_t ar_vec_off(int lane, int i) {
+  constexpr int kV = kLaneBytes / 16;
+  return kLaneBytes * (uint32_t)lane + 32u * kLaneBytes * (uint32_t)(i / kV) + 16u * (uint32_t)(i % kV);
+}
+
+__device__ __forceinline__ void ar_add(uint64_t (&acc)[kArWords], int i, const uint4& v) {
+  acc[2 * i] += pack64(v.x, v.y);
+  acc[2 * i + 1] += pack64(v.z, v.w);
+}
+
+// Unit u of the output is complete in the accumulators: the armed fault goes in (fw, an output word index; ~0 when
+// none), every vector of the unit leaves with st.global.v4 and is folded into the (S, X) by its place in the output,
+// and the accumulators are cleared for the next unit.
+template <uint32_t kLaneBytes>
+__device__ __forceinline__ void ar_store(const Ctx& c, uint8_t* out, uint64_t u, uint32_t len, uint64_t fw,
+                                         uint64_t (&acc)[kArWords], Sum& a) {
+  if (fw / (kUnitBytes / 8) == u) {  // rare: this unit holds the armed word
+    const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
+#pragma unroll
+    for (int i = 0; i < kArWords / 2; ++i) {
+      if (ar_vec_off<kLaneBytes>(c.lane, i) != (fb & ~15u)) continue;
+      if (fb & 8u) acc[2 * i + 1] += 1ull;
+      else acc[2 * i] += 1ull;
+    }
+  }
+  uint8_t* base = out + u * kUnitBytes;
+  uint64_t ux = 0;
+#pragma unroll
+  for (int i = 0; i < kArWords / 2; ++i) {
+    const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+    const uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
+    if (off < len) {
+      stg_v4(reinterpret_cast<uint4*>(base + off),
+             make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+      add_pair(a, ux, w0, w1);
+    }
+    acc[2 * i] = 0ull;
+    acc[2 * i + 1] = 0ull;
+  }
+  fold_unit(a, ux, u);
+}
+
+// TMA read side: the warp walks (unit, input) pairs, the n inputs of a unit in a row, through its kStages-deep ring of
+// bulk loads, one load per pair.  Each stage is added into the accumulators and then refilled with the next pair, so
+// the ring runs on across unit boundaries.  Aborted: stops issuing and drains what is in flight.
+__device__ void ar_units_tma(Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw, Sum& a) {
+  const uint32_t n = P.n;
+  Walk<false> iw = walk;  // the issue side: up to kStages pairs ahead of the consume side, over the same pairs
+  uint64_t iu = 0;
+  bool imore = iw.take(c, iu);
+  uint32_t isrc = 0, in_flight = 0;
+  if (c.lane == 0) fence_proxy_async_global();  // data may have been written through the generic proxy
+#pragma unroll
+  for (int s = 0; s < kStages; ++s) {
+    if (!imore) break;
+    if (c.lane == 0) issue_load(c, P.src[isrc], bytes, iu, s);
+    ++in_flight;
+    if (++isrc == n) {
+      isrc = 0;
+      imore = iw.take(c, iu);
+    }
+  }
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  int s = 0;
+  uint32_t csrc = 0;
+  uint64_t u = 0;
+  bool more = walk.take(c, u);
+  while (more) {
+    if (!mbar_wait(c, s)) {
+      for (; in_flight > 0; --in_flight) {
+        mbar_drain(c, s);
+        s = (s + 1 == kStages) ? 0 : s + 1;
+      }
+      return;
+    }
+    --in_flight;
+    const uint32_t len = unit_len(bytes, u);
+    const uint32_t sbase = c.stage_smem + s * kUnitBytes;
+    if (len == kUnitBytes) {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    } else {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i)
+        if (ar_vec_off<16>(c.lane, i) < len) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    }
+    __syncwarp();
+    if (imore) {
+      if (c.lane == 0) {
+        fence_proxy_async_smem();
+        issue_load(c, P.src[isrc], bytes, iu, s);
+      }
+      ++in_flight;
+      if (++isrc == n) {
+        isrc = 0;
+        imore = iw.take(c, iu);
+      }
+    }
+    s = (s + 1 == kStages) ? 0 : s + 1;
+    if (++csrc == n) {
+      ar_store<16>(c, P.out, u, len, fw, acc, a);
+      csrc = 0;
+      more = walk.take(c, u);
+    }
+  }
+}
+
+// ld/st read side: for each unit, the n inputs one after another, kLdstVecs 16-byte loads in flight per lane each.
+template <uint32_t kLaneBytes>
+__device__ void ar_units_ldst(const Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw,
+                              Sum& a) {
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  for (uint64_t u; walk.take(c, u);) {
+    const uint32_t len = unit_len(bytes, u);
+    for (uint32_t t = 0; t < P.n; ++t) {
+      const uint8_t* base = P.src[t] + u * kUnitBytes;
+      uint4 v[kLdstVecs];
+      if (len == kUnitBytes) {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i)
+          v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + ar_vec_off<kLaneBytes>(c.lane, i)));
+      } else {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i) {
+          v[i] = make_uint4(0u, 0u, 0u, 0u);
+          const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+          if (off < len) v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + off));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < (int)kLdstVecs; ++i) ar_add(acc, i, v[i]);
+    }
+    ar_store<kLaneBytes>(c, P.out, u, len, fw, acc, a);
+  }
+}
+
+__device__ __forceinline__ uint64_t warp_min64(uint64_t v) {
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) v = min(v, (uint64_t)__shfl_xor_sync(0xffffffffu, v, m));
+  return v;
+}
+
+// The untimed word check of the output the last rep of size k stored: each lane compares every 32nd word of its
+// warp's share with allreduce_word, reading at L2 (other SMs stored them).  One atomic pair per warp with a bad word.
+__device__ void ar_check(const Ctx& c, const AllReduceParams& P, ArScratch* as, uint32_t k, uint64_t bytes,
+                         uint32_t gwarp, uint32_t nwarps) {
+  const unsigned long long* out = reinterpret_cast<const unsigned long long*>(P.out);
+  const uint64_t words = bytes / 8;
+  uint64_t bad = 0, first = ~0ull;
+  for (uint64_t w = (uint64_t)gwarp * 32u + (uint32_t)c.lane; w < words; w += (uint64_t)nwarps * 32u) {
+    if (__ldcg(out + w) != allreduce_word(P.seed, P.n, w)) {
+      ++bad;
+      first = min(first, w * 8u);
+    }
+  }
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
+}
+
+// Barrier b of an allreduce_kernel launch, called by every thread: grid_sync's grid barrier on the same rising
+// counter.  At a domain barrier with peers, the CTA that completes it first stores (call_seq << 16) | (b + 1) into this
+// rank's line in every peer's Ctrl granule (st.relaxed.sys) and waits until every peer's line in this rank's granule
+// holds at least that (ld.acquire.sys); then it stamps *t_rel and releases the grid.  Nothing is published at it (the
+// inputs are written at open, the output is local), so no fence precedes the stores.  Returns false in every thread
+// once the launch is aborted (the deadline is checked at every arrival).
+__device__ bool ar_sync(const Ctx& c, const AllReduceParams& P, BwScratch* bs, uint32_t b, bool domain,
+                        unsigned long long* t_rel) {
+  __shared__ bool s_go;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    bool go = !check_abort(c);
+    if (go) {
+      const unsigned int prev = atomicAdd(&bs->arrive, 1u);
+      if (prev == (b + 1u) * gridDim.x - 1u) {
+        if (domain && P.n > 1) {
+          const uint64_t v = (P.call_seq << kArBarrierBits) | (b + 1ull);
+          for (uint32_t j = 0; j < P.n; ++j)
+            if (j != P.rank) st_relaxed_sys(P.sig_out[j], v);
+          for (uint32_t j = 0; j < P.n && go; ++j)
+            if (j != P.rank) go = spin_until<kScopeSys>(c, &P.sig_in[j].v, v);
+        }
+        if (go) {
+          if (t_rel != nullptr) *t_rel = gtimer();
+          st_release_gpu(&bs->release, b + 1ull);
+        }
+      } else {
+        go = spin_until<kScopeGpu>(c, &bs->release, b + 1ull);
+      }
+    }
+    s_go = go;
+  }
+  __syncthreads();
+  return s_go;
+}
+}  // namespace
+
+// One rank of cdprobe_allreduce: for every size of the ladder, one warm-up and P.reps timed reps, each summing the
+// first size bytes of all P.n inputs into P.out with every warp of the grid (the strided walk of a probe phase) and
+// folding the sum into the (S, X) checksum.  A domain barrier opens every rep, so a rep is timed as a probe phase is,
+// per rank: from this rank's release stamp to its latest CTA completion stamp (ranks see a release one signal latency
+// apart).  After the last rep of a size and a grid barrier, the word check.  Its state (barrier, stamps, checksums,
+// word-check counters, abort word) is in the rank's scratch buffer; outside it only its barrier lines are written.
+__global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_constant__ AllReduceParams P) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
+  uint64_t* red = bars + kWarpsPerCta * kStages;
+  __shared__ uint64_t s_deadline;
+  ArScratch* as = P.scratch;
+  BwScratch* bs = &as->rep;
+
+  Ctx c;
+  c.abort_word = &bs->abort_flag;
+  c.warp = threadIdx.x >> 5;
+  c.lane = threadIdx.x & 31;
+  c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
+  c.bar_smem = smem_u32(bars) + c.warp * kStages * 8u;
+  c.parity_bits = 0u;
+  if (threadIdx.x == 0) s_deadline = gtimer() + P.timeout_ns;
+  if (c.lane == 0) {
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) mbar_init(c.bar_smem + 8u * s, 1u);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  c.deadline = s_deadline;
+
+  const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
+  const uint32_t nwarps = gridDim.x * kWarpsPerCta;
+  uint32_t b = 0;
+  for (uint32_t k = 0; k < P.n_sizes; ++k) {
+    const uint64_t bytes = P.size[k];
+    for (uint32_t r = 0; r <= P.reps; ++r) {
+      if (!ar_sync(c, P, bs, b++, true, &bs->t_rel[k][r])) return;
+      const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
+      Sum a{0ull, 0ull, 0ull};
+      const Walk<false> walk = strided(bytes, gwarp, nwarps);
+      if (P.path == 2u) ar_units_ldst<32>(c, P, bytes, walk, fw, a);
+      else if (P.path == 1u) ar_units_ldst<16>(c, P, bytes, walk, fw, a);
+      else ar_units_tma(c, P, bytes, walk, fw, a);
+      __threadfence();  // this warp's stores are performed before the CTA's completion stamp
+      Acc* const acc = &bs->rep[k][r];
+      cta_reduce<1>(c, red, &a, &acc);
+      if (threadIdx.x == 0) atomicMax(&acc->t_end, (unsigned long long)gtimer());
+    }
+    if (!ar_sync(c, P, bs, b++, false, nullptr)) return;
+    ar_check(c, P, as, k, bytes, gwarp, nwarps);
+  }
+}
+
+// The per-granule (sum, xor) of the all-reduce output from the pattern definition: one warp per 16 KiB granule.
+__global__ void __launch_bounds__(256) allreduce_granules_kernel(uint64_t* gsum, uint64_t* gxor, uint64_t seed,
+                                                                  uint32_t n, uint64_t n_granules) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+  for (uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n_granules; g += nwarps) {
+    uint64_t s = 0, x = 0;
+    for (uint32_t k = lane; k < kGranuleWords; k += 32) {
+      const uint64_t w = allreduce_word(seed, n, g * kGranuleWords + k);
+      s += w;
+      x ^= w;
+    }
+    s = warp_sum64(s);
+    x = warp_xor64(x);
+    if (lane == 0) {
+      gsum[g] = s;
+      gxor[g] = x;
+    }
+  }
+}
+
 // ----------------------------------------------------------- launchers -----
 int probe_kernel_prepare(int* max_ctas_per_sm) {
   cudaError_t e = cudaFuncSetAttribute(cdprobe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
@@ -1082,6 +1373,27 @@ int bwcurve_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint3
   const uint64_t need = (n_granules + 7) / 8;  // eight warps per block
   bwcurve_granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, seed, rank, first_word,
                                                                                     n_granules);
+  return (int)cudaGetLastError();
+}
+
+int allreduce_launch(const AllReduceParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
+  cudaError_t e = cudaFuncSetAttribute(allreduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  if (e != cudaSuccess) return (int)e;
+  void* args[] = {const_cast<AllReduceParams*>(&p)};
+  if (cooperative) {
+    e = cudaLaunchCooperativeKernel((const void*)allreduce_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes,
+                                    stream);
+  } else {
+    e = cudaLaunchKernel((const void*)allreduce_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
+  }
+  return (int)e;
+}
+
+int allreduce_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t n, uint64_t n_granules,
+                              unsigned grid, cudaStream_t stream) {
+  if (n_granules == 0) return (int)cudaSuccess;
+  const uint64_t need = (n_granules + 7) / 8;  // eight warps per block
+  allreduce_granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, seed, n, n_granules);
   return (int)cudaGetLastError();
 }
 

@@ -429,11 +429,12 @@ CDP_HD inline uint32_t bwcurve_ladder(uint64_t bpp, uint64_t* size) {
   return n;
 }
 
-// (S, X) of the first n_words words of a source region, words first_word... of rank's pattern, from gsum[g] and gxor[g],
-// the sum and xor of the words of each whole granule g of the region.  The words of a last, partial granule (at most
-// kGranuleWords - 1) are generated from src_word here.
-CDP_HD inline void bwcurve_prefix_checksum(const uint64_t* gsum, const uint64_t* gxor, uint64_t seed, uint32_t rank,
-                                           uint64_t first_word, uint64_t n_words, uint64_t* sum, uint64_t* xr) {
+// (S, X) of the first n_words words of a region from gsum[g] and gxor[g], the sum and xor of the words of each whole
+// granule g of the region.  The words of a last, partial granule (at most kGranuleWords - 1) come from word(k), word k
+// of the region.
+template <typename Word>
+CDP_HD inline void prefix_checksum(const uint64_t* gsum, const uint64_t* gxor, uint64_t n_words, const Word& word,
+                                   uint64_t* sum, uint64_t* xr) {
   const uint64_t whole = n_words / kGranuleWords;
   uint64_t s = 0, x = 0, px = 0;
   for (uint64_t g = 0; g < whole; ++g) {
@@ -441,12 +442,53 @@ CDP_HD inline void bwcurve_prefix_checksum(const uint64_t* gsum, const uint64_t*
     x ^= rotl64(gxor[g], fold6((uint32_t)g));
   }
   for (uint64_t k = whole * kGranuleWords; k < n_words; ++k) {
-    const uint64_t w = src_word(seed, rank, first_word + k);
+    const uint64_t w = word(k);
     s += w;
     px ^= w;
   }
   *sum = s;
   *xr = x ^ rotl64(px, fold6((uint32_t)whole));
 }
+
+struct SrcRegionWord {  // word k of a source region: words first_word... of rank's pattern
+  uint64_t seed, first_word;
+  uint32_t rank;
+  CDP_HD uint64_t operator()(uint64_t k) const { return src_word(seed, rank, first_word + k); }
+};
+
+// (S, X) of the first n_words words of a source region, words first_word... of rank's pattern (prefix_checksum).
+CDP_HD inline void bwcurve_prefix_checksum(const uint64_t* gsum, const uint64_t* gxor, uint64_t seed, uint32_t rank,
+                                           uint64_t first_word, uint64_t n_words, uint64_t* sum, uint64_t* xr) {
+  prefix_checksum(gsum, gxor, n_words, SrcRegionWord{seed, first_word, rank}, sum, xr);
+}
+
+// ---- the one-shot all-reduce (cdprobe_allreduce, DESIGN §5g) -------------------------------------------------------
+// Word w of the output every rank computes: the sum mod 2^64 of word w of every rank's source buffer.  Integer addition
+// wraps exactly and commutes, so the order in which a rank adds its inputs does not change the result.
+CDP_HD inline uint64_t allreduce_word(uint64_t seed, uint32_t n, uint64_t w) {
+  uint64_t s = 0;
+  for (uint32_t j = 0; j < n; ++j) s += src_word(seed, j, w);
+  return s;
+}
+struct AllReduceWord {
+  uint64_t seed;
+  uint32_t n;
+  CDP_HD uint64_t operator()(uint64_t k) const { return allreduce_word(seed, n, k); }
+};
+// (S, X) of the first n_words words of the output, from the per-granule sums of the summed words (prefix_checksum).
+// S is the sum of the ranks' prefix sums; X is not made of the ranks' X, since xor does not distribute over the sum.
+CDP_HD inline void allreduce_prefix_checksum(const uint64_t* gsum, const uint64_t* gxor, uint64_t seed, uint32_t n,
+                                             uint64_t n_words, uint64_t* sum, uint64_t* xr) {
+  prefix_checksum(gsum, gxor, n_words, AllReduceWord{seed, n}, sum, xr);
+}
+
+// The domain barrier of cdprobe_allreduce: one 128-byte line per sender after the atomics lines, in the Ctrl granule.
+// line[s] in rank o's memory holds the last (call_seq << 16) | (b + 1) rank s signalled to o.  The values rise across
+// calls and barriers, so no call resets them; open zeroes the granule, and nothing else touches these lines.
+constexpr uint64_t kArOff = kAtomOff + kMaxRanks * sizeof(AtomLine);  // 68 KiB
+static_assert(kArOff % 128 == 0 && kArOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the all-reduce lines sit after the atomics lines inside the Ctrl granule");
+constexpr uint32_t kArBarrierBits = 16;  // barriers per call: at most kBwMaxSizes x (kMaxTimedReps + 2) < 2^16
+constexpr uint32_t kArNoFault = ~0u;
 
 }  // namespace cdp

@@ -345,6 +345,56 @@ class BwCurve:
                        sum=_mat(t, per_size(t.sum), timed), xr=_mat(t, per_size(t.xr), timed), ms=t.ms, raw=t)
 
 
+@dataclasses.dataclass
+class AllReduce:
+    """What cdprobe_allreduce measured: per rank r, ns per rep (min, median and max over the timed reps) of the one-shot
+    all-reduce of each size of the ladder `sizes`, the (S, X) of the output the last timed rep stored, the word check
+    of that output (`bad_words`, and `first_bad`, the byte offset of the first bad word or U64_MAX), the sizes that
+    failed either check (`bad_sizes`, bit k for sizes[k]) and the summary of the medians: t0_ns (the smallest size),
+    peak_gbps (algorithm bandwidth: size / ns; each rank's ingress is (n - 1) x that) and half_bytes.  Per-size values
+    are lists over `sizes`, and every list is indexed by rank.  A rank that did not run is None everywhere but
+    `status`; a rank that passed timeout_ms has no times."""
+    n: int
+    row_mask: int
+    reps: int
+    path: int
+    call_seq: int
+    sizes: List[int]
+    measured: List[bool]
+    status: List[int]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the mapping status of the domain's first cell down
+    bad_sizes: List[Optional[int]]
+    t0_ns: List[Optional[float]]
+    peak_gbps: List[Optional[float]]
+    half_bytes: List[Optional[int]]
+    ns_min: List[Optional[List[float]]]
+    ns_median: List[Optional[List[float]]]
+    ns_max: List[Optional[List[float]]]
+    sum: List[Optional[List[int]]]
+    xr: List[Optional[List[int]]]
+    bad_words: List[Optional[List[int]]]
+    first_bad: List[Optional[List[int]]]
+    ms: float
+    raw: abi.AllReduceT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.AllReduceT) -> "AllReduce":
+        k = t.n_sizes
+
+        def timed(r):
+            return t.measured[r] and t.status[r] != abi.ERR_TIMEOUT
+
+        def row(a, per_size=False):
+            return [(list(a[r])[:k] if per_size else a[r]) if timed(r) else None for r in range(t.n)]
+
+        return AllReduce(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
+                         sizes=list(t.size)[:k], measured=[bool(t.measured[r]) for r in range(t.n)],
+                         status=list(t.status)[:t.n], bad_sizes=row(t.bad_sizes), t0_ns=row(t.t0_ns),
+                         peak_gbps=row(t.peak_gbps), half_bytes=row(t.half_bytes), ns_min=row(t.ns_min, True),
+                         ns_median=row(t.ns_median, True), ns_max=row(t.ns_max, True), sum=row(t.sum, True),
+                         xr=row(t.xr, True), bad_words=row(t.bad_words, True), first_bad=row(t.first_bad, True),
+                         ms=t.ms, raw=t)
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -503,6 +553,20 @@ class Probe:
         """The bare ABI call: (return code, abi.BwCurveT as the library left it)."""
         t = abi.BwCurveT()
         rc = self._lib.cdprobe_bwcurve(self._h, reps, C.byref(t))
+        return rc, t
+
+    def AllReduce(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReduce.  One-shot all-reduce of every rank's source buffer on every rank at once, at each
+        size of the bwcurve ladder, on the probe's read path and grid (0: 8 timed reps per size).  Collective when
+        world_size > 1.  Needs no Run first and disturbs none."""
+        rc, t = self.allreduce_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce")
+        return AllReduce.from_c(t)
+
+    def allreduce_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce(self._h, reps, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
