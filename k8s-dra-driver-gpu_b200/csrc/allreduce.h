@@ -44,9 +44,6 @@ struct AllReduceParams {
 // not as the probe launches them.  For every size, one warm-up and p.reps timed reps, each opened by a domain barrier,
 // then the word check of the last one.  Returns a cudaError_t.
 int allreduce_launch(const AllReduceParams& p, unsigned grid, bool cooperative, cudaStream_t stream);
-// Writes gsum[g] / gxor[g], the sum and the xor of the words of whole granule g of the n-rank all-reduce output, for
-// its first n_granules granules, computed from allreduce_word.  Returns a cudaError_t.
-int allreduce_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t n, uint64_t n_granules,
-                              unsigned grid, cudaStream_t stream);
+// The expected output's per-granule sums come from granules_launch (bwcurve.h) with AllReduceWord.
 
 }  // namespace cdp

@@ -35,9 +35,11 @@ struct BwCurveParams {
 // not as the probe launches them.  For every size, one warm-up and p.reps timed reps, separated by grid barriers,
 // each reading the first size bytes of p.region through the probe's read path p.path.  Returns a cudaError_t.
 int bwcurve_launch(const BwCurveParams& p, unsigned grid, bool cooperative, cudaStream_t stream);
-// Writes gsum[g] / gxor[g], the sum and the xor of the words of whole granule g, for the n_granules granules of the
-// source region of `rank` that starts at word first_word, computed from src_word.  Returns a cudaError_t.
-int bwcurve_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t rank, uint64_t first_word,
-                            uint64_t n_granules, unsigned grid, cudaStream_t stream);
+// Writes gsum[g] / gxor[g], the sum and the xor of the words of whole granule g, for the first n_granules granules of
+// the region whose word k is word(k).  Defined for SrcRegionWord (a cell's source slice) and AllReduceWord (the
+// all-reduce output).  Returns a cudaError_t.
+template <typename Word>
+int granules_launch(uint64_t* gsum, uint64_t* gxor, const Word& word, uint64_t n_granules, unsigned grid,
+                    cudaStream_t stream);
 
 }  // namespace cdp

@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <string>
 #include <vector>
 
@@ -32,15 +33,21 @@ static int ensure_scratch(LocalRank& L, size_t bytes) {
   return CDPROBE_OK;
 }
 
-// Grows every local rank's scratch to hold its rep tables before any kernel is launched.  cudaFree synchronizes the
-// device, and local ranks may share one: a pingpong kernel launched for an earlier rank would wait on this rank's.
-static int ensure_rep_tables(cdprobe* h) {
+// Grows every local rank's scratch to at least `bytes` before any kernel is launched.  cudaFree synchronizes the
+// device, and local ranks may share one: a kernel launched for an earlier rank would wait on this rank's.
+static int ensure_scratch_all(cdprobe* h, size_t bytes) {
   for (uint32_t li = 0; li < h->n_local; ++li) {
     CDP_RT(cudaSetDevice(h->lr[li].ordinal));
-    const int rc = ensure_scratch(h->lr[li], sizeof(TimedRep) * kMaxRanks * kRepSlots);
-    if (rc != CDPROBE_OK) return rc;
+    if (const int rc = ensure_scratch(h->lr[li], bytes); rc != CDPROBE_OK) return rc;
   }
   return CDPROBE_OK;
+}
+constexpr size_t kRepTableBytes = sizeof(TimedRep) * kMaxRanks * kRepSlots;  // latency, pingpong, atomics
+
+// A launch, a copy or a kernel failed: the context is unusable, and so is the handle.
+static int fail_sticky(cdprobe* h, const char* what, cudaError_t e) {
+  h->sticky = true;
+  return fail_cuda(what, e);
 }
 
 // Copies the first `bytes` of local rank L's scratch (its rep tables) to `got` once its kernel is done.
@@ -48,10 +55,90 @@ static int fetch_reps(cdprobe* h, LocalRank& L, size_t bytes, void* got, const c
   cudaError_t e = cudaSetDevice(L.ordinal);
   if (e == cudaSuccess) e = cudaMemcpyAsync(got, L.scratch, bytes, cudaMemcpyDeviceToHost, L.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-  if (e != cudaSuccess) {
-    h->sticky = true;  // a failed kernel leaves the context unusable
-    return fail_cuda(what, e);
+  return e != cudaSuccess ? fail_sticky(h, what, e) : CDPROBE_OK;
+}
+
+// Clears the last error and *out and stamps the ABI version, as cdprobe_run does: the caller may read *out whatever
+// the return code.  False when out is null.
+template <typename Out>
+static bool begin_output(Out* out) {
+  g_last_error.clear();
+  if (out == nullptr) return false;
+  memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
+  return true;
+}
+
+// What each process contributes at the start of a collective measurement (cdprobe_pingpong, cdprobe_bwcurve,
+// cdprobe_allreduce), so that every process refuses, skips or runs the same call: the call number it is about to
+// make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and what the call
+// folds in from every process.
+template <typename Extra>
+struct Agreement {
+  uint64_t call_seq;
+  std::array<uint32_t, 3> args;
+  uint32_t ok;
+  Extra extra;
+};
+struct NoExtra {};
+
+// The handshake of collective measurement `fn`: every process contributes `mine` (ok: its own verdict `bad` on its
+// arguments is empty) and gets all[r], process r's contribution, back (in a single process, all = {mine}).  The first
+// error wins: this process's own arguments, then another process's, then a call number or arguments that differ.
+// Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and CDPROBE_ERR_ARG on a refusal, with the message set.
+template <typename Extra>
+static int agree(cdprobe* h, const char* fn, std::string bad, Agreement<Extra>& mine,
+                 std::vector<Agreement<Extra>>& all) {
+  mine.ok = bad.empty() ? 1u : 0u;
+  all.assign(h->cfg.world_size, mine);
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
   }
+  for (const Agreement<Extra>& o : all) {
+    if (!o.ok && bad.empty()) bad = std::string("another process called ") + fn + " with invalid arguments";
+    if ((o.call_seq != mine.call_seq || o.args != mine.args) && bad.empty())
+      bad = std::string(fn) + " is collective: every process must call it with the same arguments";
+  }
+  if (!bad.empty()) {
+    set_err(bad);
+    return CDPROBE_ERR_ARG;
+  }
+  return CDPROBE_OK;
+}
+
+// Waits until every process of the domain has got here; nothing to wait for in a single process.
+static int domain_barrier(cdprobe* h) {
+  if (h->cfg.world_size == 1) return CDPROBE_OK;
+  std::string err;
+  if (h->rdv.barrier(&err) != 0) {
+    set_err(err);
+    return CDPROBE_ERR_RENDEZVOUS;
+  }
+  return CDPROBE_OK;
+}
+
+// want[k], the (S, X) of the first size[k] bytes of the region whose word k is word(k), for every size: the
+// per-granule sums of its whole bpp granules, computed from the pattern definition on local rank L's GPU into its
+// scratch at table_off (grown by the caller), then folded into every prefix on the host.
+template <typename Word>
+static int expected_sums(cdprobe* h, LocalRank& L, size_t table_off, const Word& word, const uint64_t* size,
+                         uint32_t n_sizes, uint64_t (*want)[2], const char* what) {
+  const uint64_t granules = h->plan.bpp / kGranuleBytes;
+  std::vector<uint64_t> table(2 * granules);
+  uint64_t* gsum = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(L.scratch) + table_off);
+  CDP_RT(cudaSetDevice(L.ordinal));
+  cudaError_t e = (cudaError_t)granules_launch(gsum, gsum + granules, word, granules, (unsigned)L.sm_count * 8u,
+                                               L.stream);
+  if (e == cudaSuccess && granules)
+    e = cudaMemcpyAsync(table.data(), gsum, 16 * granules, cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+  if (e != cudaSuccess) return fail_sticky(h, what, e);
+  for (uint32_t k = 0; k < n_sizes; ++k)
+    prefix_checksum(table.data(), table.data() + granules, size[k] / 8, word, &want[k][0], &want[k][1]);
   return CDPROBE_OK;
 }
 
@@ -201,10 +288,7 @@ int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target
   if (e == cudaSuccess) e = cudaMemcpyAsync(&d, L.scratch, sizeof(d), cudaMemcpyDeviceToHost, L.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
   if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L.ev0, L.ev1);
-  if (e != cudaSuccess) {
-    h->sticky = true;  // a failed kernel leaves the context unusable
-    return cdp::fail_cuda("cdprobe_diagnose", e);
-  }
+  if (e != cudaSuccess) return cdp::fail_sticky(h, "cdprobe_diagnose", e);
   out->ms = ms;
   out->bad_words = d.bad_words;
   out->bad_granules = d.bad_granules;
@@ -221,11 +305,7 @@ int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target
 }
 
 int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
   out->hops = hops != 0 ? hops : cdp::kLatencyDefaultHops;
   out->reps = reps != 0 ? reps : cdp::kLatencyDefaultReps;
   if (h == nullptr) return CDPROBE_ERR_ARG;
@@ -241,7 +321,7 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
   hops = out->hops;
   reps = out->reps;
   const uint64_t lines = pl.bpp / (cdp::kLineWords * 8);
-  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::ensure_scratch_all(h, cdp::kRepTableBytes); rc != CDPROBE_OK) return rc;
 
   // 1. every local issuer's chases, all launched before any is waited for
   cdp::LatencyParams P[cdp::kMaxRanks];
@@ -271,10 +351,7 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
     if (p.n_cells == 0) continue;
     CDP_RT(cudaSetDevice(L.ordinal));
     const cudaError_t e = (cudaError_t)cdp::latency_launch(p, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch latency_kernel", e);
-    }
+    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch latency_kernel", e);
   }
 
   // 2. while they run: the digest each chase gives over an intact region
@@ -303,20 +380,8 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
   return CDPROBE_OK;
 }
 
-// What each process contributes at the start of cdprobe_pingpong, so that every process refuses or runs the same call
-// over the same pair set (cdprobe_unmap_peer changes only the local view).
-struct PingPongAgree {
-  uint64_t call_seq;
-  uint32_t trips, reps, fenced, ok;
-  int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [local rank][rank]: mapping status, unmapped cells folded in
-};
-
 int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fenced, cdprobe_pingpong_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
   out->trips = trips != 0 ? trips : cdp::kPingPongDefaultTrips;
   out->reps = reps != 0 ? reps : cdp::kPingPongDefaultReps;
   out->fenced = fenced;
@@ -346,38 +411,17 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
       f_trip = (uint32_t)trip;
     }
   }
-  PingPongAgree mine;
-  memset(&mine, 0, sizeof(mine));
-  mine.call_seq = h->pp_calls + 1;
-  mine.trips = trips;
-  mine.reps = reps;
-  mine.fenced = fenced;
-  mine.ok = bad.empty() ? 1u : 0u;
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  memcpy(st, h->status, sizeof(st));
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    const cdp::LocalRank& L = h->lr[li];
-    for (uint32_t j = 0; j < n; ++j) st[L.grank][j] = mine.status[li][j] = cdp::cell_status(h, li, j);
-  }
-  if (h->cfg.world_size > 1) {
-    std::vector<PingPongAgree> all(h->cfg.world_size);
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    for (uint32_t r = 0; r < h->cfg.world_size; ++r) {
-      const PingPongAgree& o = all[r];
-      if (!o.ok && bad.empty()) bad = "another process called cdprobe_pingpong with invalid arguments";
-      if ((o.call_seq != mine.call_seq || o.trips != trips || o.reps != reps || o.fenced != fenced) && bad.empty())
-        bad = "cdprobe_pingpong is collective: every process must call it with the same arguments";
-      for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], o.status[li], sizeof(st[0]));
-    }
-  }
-  if (!bad.empty()) {
-    cdp::set_err(bad);
-    return CDPROBE_ERR_ARG;
-  }
+  // every process runs over the same pair set: each contributes its local ranks' rows of mapping status, [local
+  // rank][rank] with unmapped cells folded in (cdprobe_unmap_peer changes only the local view)
+  using Rows = int32_t[cdp::kMaxRanks][cdp::kMaxRanks];
+  cdp::Agreement<Rows> mine = {h->pp_calls + 1, {trips, reps, fenced}, 0u, {}};
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < n; ++j) mine.extra[li][j] = cdp::cell_status(h, li, j);
+  std::vector<cdp::Agreement<Rows>> all;
+  if (const int rc = cdp::agree(h, "cdprobe_pingpong", bad, mine, all); rc != CDPROBE_OK) return rc;
+  Rows st = {};  // [rank][rank]
+  for (uint32_t r = 0; r < all.size(); ++r)
+    for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].extra[li], sizeof(st[0]));
   h->pp_calls = mine.call_seq;
   out->call_seq = h->pp_calls;
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
@@ -385,14 +429,9 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
     out->ms = cdp::now_ms() - t_begin;
     return CDPROBE_OK;
   }
-  if (h->cfg.world_size > 1) {  // every process has agreed before any kernel polls a peer
-    std::string err;
-    if (h->rdv.barrier(&err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-  }
-  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+  // every process has agreed before any kernel polls a peer
+  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::ensure_scratch_all(h, cdp::kRepTableBytes); rc != CDPROBE_OK) return rc;
   // a pair is exchanged only when both directions are mapped; the status of its cells is the pair's mapping status
   auto pair_status = [&](uint32_t i, uint32_t j) { return st[i][j] != 0 ? st[i][j] : st[j][i]; };
 
@@ -429,10 +468,7 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
     CDP_RT(cudaSetDevice(L.ordinal));
     const cudaError_t e =
         (cudaError_t)cdp::pingpong_launch(p, fenced != 0, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch pingpong_kernel", e);
-    }
+    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch pingpong_kernel", e);
     launched[li] = true;
   }
 
@@ -466,11 +502,7 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
 }
 
 int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cdprobe_atomics_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
   out->kind = kind;
   out->ops = ops != 0 ? ops : cdp::kAtomicsDefaultOps;
   out->reps = reps != 0 ? reps : cdp::kAtomicsDefaultReps;
@@ -498,7 +530,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
   ops = out->ops;
   reps = out->reps;
   const uint64_t total = (uint64_t)out->lanes * ops;  // increments per rep
-  if (const int rc = cdp::ensure_rep_tables(h); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::ensure_scratch_all(h, cdp::kRepTableBytes); rc != CDPROBE_OK) return rc;
   out->call_seq = ++h->at_calls;
 
   // 1. every local issuer's cells, all launched before any is waited for; no kernel waits on another rank
@@ -545,10 +577,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
     if (p.n_cells == 0) continue;
     CDP_RT(cudaSetDevice(L.ordinal));
     const cudaError_t e = (cudaError_t)cdp::atomics_launch(p, kind, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch atomics kernel", e);
-    }
+    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch atomics kernel", e);
   }
 
   // 2. while they run: the digest of clean reps, the same for every cell
@@ -570,19 +599,8 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
   return CDPROBE_OK;
 }
 
-// What each process contributes at the start of cdprobe_bwcurve, so that every process refuses or runs the same call.
-// Every cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree.
-struct BwCurveAgree {
-  uint64_t call_seq;
-  uint32_t reps, ok;
-};
-
 int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
   out->reps = reps != 0 ? reps : cdp::kBwDefaultReps;
   if (h == nullptr) return CDPROBE_ERR_ARG;
   const double t_begin = cdp::now_ms();
@@ -598,24 +616,10 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
   if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
   else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
-  BwCurveAgree mine = {h->bw_calls + 1, reps, bad.empty() ? 1u : 0u};
-  if (h->cfg.world_size > 1) {
-    std::vector<BwCurveAgree> all(h->cfg.world_size);
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    for (const BwCurveAgree& o : all) {
-      if (!o.ok && bad.empty()) bad = "another process called cdprobe_bwcurve with invalid arguments";
-      if ((o.call_seq != mine.call_seq || o.reps != reps) && bad.empty())
-        bad = "cdprobe_bwcurve is collective: every process must call it with the same arguments";
-    }
-  }
-  if (!bad.empty()) {
-    cdp::set_err(bad);
-    return CDPROBE_ERR_ARG;
-  }
+  // every cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree
+  cdp::Agreement<cdp::NoExtra> mine = {h->bw_calls + 1, {reps, 0u, 0u}, 0u, {}};
+  std::vector<cdp::Agreement<cdp::NoExtra>> all;
+  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", bad, mine, all); rc != CDPROBE_OK) return rc;
   h->bw_calls = mine.call_seq;
   out->call_seq = h->bw_calls;
   out->n_sizes = n_sizes;
@@ -623,12 +627,9 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
 
   // 2. scratch for the rep records and one cell's granule table, grown on every local rank before any kernel runs
-  const uint64_t granules = pl.bpp / cdp::kGranuleBytes;
   const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    CDP_RT(cudaSetDevice(h->lr[li].ordinal));
-    if (const int rc = cdp::ensure_scratch(h->lr[li], table_off + 16 * granules); rc != CDPROBE_OK) return rc;
-  }
+  const size_t scratch = table_off + 16 * (pl.bpp / cdp::kGranuleBytes);
+  if (const int rc = cdp::ensure_scratch_all(h, scratch); rc != CDPROBE_OK) return rc;
 
   // 3. the (S, X) each size of each cell that runs must read, from the pattern definition: the per-granule sums of the
   //    slice on the issuer's GPU, folded into every prefix on the host
@@ -637,7 +638,6 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   auto want_of = [&](uint32_t li, uint32_t j) {
     return reinterpret_cast<uint64_t(*)[2]>(want.data() + ((size_t)li * cdp::kMaxRanks + j) * cdp::kBwMaxSizes * 2);
   };
-  std::vector<uint64_t> table(2 * granules);
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
@@ -649,21 +649,11 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
         continue;
       }
       runs[li][j] = true;
-      const uint64_t first = (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8);
-      uint64_t* gsum = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(L.scratch) + table_off);
-      cudaError_t e = (cudaError_t)cdp::bwcurve_granules_launch(gsum, gsum + granules, h->seed, j, first, granules,
-                                                                 (unsigned)L.sm_count * 8u, L.stream);
-      if (e == cudaSuccess && granules)
-        e = cudaMemcpyAsync(table.data(), gsum, 16 * granules, cudaMemcpyDeviceToHost, L.stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-      if (e != cudaSuccess) {
-        h->sticky = true;
-        return cdp::fail_cuda("cdprobe_bwcurve: granule checksums", e);
-      }
-      uint64_t(*w)[2] = want_of(li, j);
-      for (uint32_t k = 0; k < n_sizes; ++k)
-        cdp::bwcurve_prefix_checksum(table.data(), table.data() + granules, h->seed, j, first, size[k] / 8, &w[k][0],
-                                     &w[k][1]);
+      const cdp::SrcRegionWord word{h->seed, (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8), j};
+      if (const int rc = cdp::expected_sums(h, L, table_off, word, size, n_sizes, want_of(li, j),
+                                            "cdprobe_bwcurve: granule checksums");
+          rc != CDPROBE_OK)
+        return rc;
     }
   }
 
@@ -673,13 +663,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   std::vector<cdp::BwScratch> got(1);
   const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
   for (uint32_t r = 0; r < n_rounds; ++r) {
-    if (h->cfg.world_size > 1) {
-      std::string err;
-      if (h->rdv.barrier(&err) != 0) {
-        cdp::set_err(err);
-        return CDPROBE_ERR_RENDEZVOUS;
-      }
-    }
+    if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
     int32_t target[cdp::kMaxRanks];
     for (uint32_t li = 0; li < h->n_local; ++li) {
       cdp::LocalRank& L = h->lr[li];
@@ -698,10 +682,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       CDP_RT(cudaSetDevice(L.ordinal));
       cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::BwScratch), L.stream);
       if (e == cudaSuccess) e = (cudaError_t)cdp::bwcurve_launch(p, L.ctas, L.coop && coop_ok, L.stream);
-      if (e != cudaSuccess) {
-        h->sticky = true;
-        return cdp::fail_cuda("launch bwcurve_kernel", e);
-      }
+      if (e != cudaSuccess) return cdp::fail_sticky(h, "launch bwcurve_kernel", e);
     }
     for (uint32_t li = 0; li < h->n_local; ++li) {
       if (target[li] < 0) continue;
@@ -716,23 +697,16 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   return CDPROBE_OK;
 }
 
-// What each process contributes at the start of cdprobe_allreduce, so that every process refuses, skips or runs the
-// same call.  The mapping verdict must agree too: a process that ran while another skipped would wait at the first
-// domain barrier until its watchdog fired.
-struct AllReduceAgree {
-  uint64_t call_seq;
-  uint32_t reps, ok;
-  uint32_t down_cell;    // issuer * kMaxRanks + target of this process's first cell whose mapping is down (kNoCell: none)
-  int32_t down_status;   // that cell's mapping status
+// What each process adds to the cdprobe_allreduce handshake: the mapping verdict must agree too, since a process that
+// ran while another skipped would wait at the first domain barrier until its watchdog fired.
+struct DownCell {
+  uint32_t cell;   // issuer * kMaxRanks + target of this process's first cell whose mapping is down (kNoCell: none)
+  int32_t status;  // that cell's mapping status
 };
 static constexpr uint32_t kNoCell = ~0u;
 
 int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
-  cdp::g_last_error.clear();
-  if (out == nullptr) return CDPROBE_ERR_ARG;
-  // like cdprobe_run: the caller may read *out whatever the return code
-  memset(out, 0, sizeof(*out));
-  out->abi = CDPROBE_ABI_VERSION;
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
   out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
   if (h == nullptr) return CDPROBE_ERR_ARG;
   const double t_begin = cdp::now_ms();
@@ -761,91 +735,46 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
       f_k = (uint32_t)fk - 1;
     }
   }
-  AllReduceAgree mine;
-  memset(&mine, 0, sizeof(mine));
-  mine.call_seq = h->ar_calls + 1;
-  mine.reps = reps;
-  mine.ok = bad.empty() ? 1u : 0u;
-  mine.down_cell = kNoCell;
+  cdp::Agreement<DownCell> mine = {h->ar_calls + 1, {reps, 0u, 0u}, 0u, {kNoCell, 0}};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     for (uint32_t j = 0; j < n; ++j) {
       const int32_t s = cdp::cell_status(h, li, j);
       const uint32_t cell = h->lr[li].grank * cdp::kMaxRanks + j;
-      if (s != 0 && cell < mine.down_cell) {
-        mine.down_cell = cell;
-        mine.down_status = s;
-      }
+      if (s != 0 && cell < mine.extra.cell) mine.extra = {cell, s};
     }
   }
-  AllReduceAgree down = mine;
-  if (h->cfg.world_size > 1) {
-    std::vector<AllReduceAgree> all(h->cfg.world_size);
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    for (const AllReduceAgree& o : all) {
-      if (!o.ok && bad.empty()) bad = "another process called cdprobe_allreduce with invalid arguments";
-      if ((o.call_seq != mine.call_seq || o.reps != reps) && bad.empty())
-        bad = "cdprobe_allreduce is collective: every process must call it with the same arguments";
-      if (o.down_cell < down.down_cell) down = o;
-    }
-  }
-  if (!bad.empty()) {
-    cdp::set_err(bad);
-    return CDPROBE_ERR_ARG;
-  }
+  std::vector<cdp::Agreement<DownCell>> all;
+  if (const int rc = cdp::agree(h, "cdprobe_allreduce", bad, mine, all); rc != CDPROBE_OK) return rc;
+  DownCell down = mine.extra;
+  for (const cdp::Agreement<DownCell>& o : all)
+    if (o.extra.cell < down.cell) down = o.extra;
   h->ar_calls = mine.call_seq;
   out->call_seq = h->ar_calls;
   out->n_sizes = n_sizes;
   memcpy(out->size, size, sizeof(size[0]) * n_sizes);
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
-  if (down.down_cell != kNoCell) {  // some rank cannot read some input: nothing runs, in any process
-    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = down.down_status;
+  if (down.cell != kNoCell) {  // some rank cannot read some input: nothing runs, in any process
+    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = down.status;
     out->ms = cdp::now_ms() - t_begin;
     return CDPROBE_OK;
   }
 
   // 2. scratch for the records, the output and the granule table, grown on every local rank before any kernel runs
-  const uint64_t granules = pl.bpp / cdp::kGranuleBytes;
   const size_t table_off = cdp::kArOutOff + (pl.bpp + 255) / 256 * 256;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    CDP_RT(cudaSetDevice(h->lr[li].ordinal));
-    if (const int rc = cdp::ensure_scratch(h->lr[li], table_off + 16 * granules); rc != CDPROBE_OK) return rc;
-  }
+  const size_t scratch = table_off + 16 * (pl.bpp / cdp::kGranuleBytes);
+  if (const int rc = cdp::ensure_scratch_all(h, scratch); rc != CDPROBE_OK) return rc;
 
   // 3. the (S, X) every prefix of the output must have, from the pattern definition: the per-granule sums of the
   //    summed words on the first local rank's GPU, folded into every prefix on the host
   uint64_t want[cdp::kBwMaxSizes][2] = {};
-  {
-    cdp::LocalRank& L = h->lr[0];
-    std::vector<uint64_t> table(2 * granules);
-    uint64_t* gsum = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(L.scratch) + table_off);
-    CDP_RT(cudaSetDevice(L.ordinal));
-    cudaError_t e = (cudaError_t)cdp::allreduce_granules_launch(gsum, gsum + granules, h->seed, n, granules,
-                                                                 (unsigned)L.sm_count * 8u, L.stream);
-    if (e == cudaSuccess && granules)
-      e = cudaMemcpyAsync(table.data(), gsum, 16 * granules, cudaMemcpyDeviceToHost, L.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("cdprobe_allreduce: granule checksums", e);
-    }
-    for (uint32_t k = 0; k < n_sizes; ++k)
-      cdp::allreduce_prefix_checksum(table.data(), table.data() + granules, h->seed, n, size[k] / 8, &want[k][0],
-                                     &want[k][1]);
-  }
+  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
+                                        "cdprobe_allreduce: granule checksums");
+      rc != CDPROBE_OK)
+    return rc;
 
   // 4. no process launches before every process is ready, so that no kernel waits at the first domain barrier for a
   //    process still setting up; then every local kernel is launched before any is waited for
-  if (h->cfg.world_size > 1) {
-    std::string err;
-    if (h->rdv.barrier(&err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-  }
+  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
   const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
@@ -872,10 +801,7 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
     CDP_RT(cudaSetDevice(L.ordinal));
     cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::ArScratch), L.stream);
     if (e == cudaSuccess) e = (cudaError_t)cdp::allreduce_launch(p, L.ctas, L.coop && coop_ok, L.stream);
-    if (e != cudaSuccess) {
-      h->sticky = true;
-      return cdp::fail_cuda("launch allreduce_kernel", e);
-    }
+    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch allreduce_kernel", e);
   }
 
   // 5. collect: per row, the times and checksums of every size, then the word checks

@@ -953,10 +953,41 @@ __global__ void __launch_bounds__(256) cdprobe_fill_src_kernel(uint4* dst, uint6
 
 // ------------------------------------------- K5: bandwidth versus size ----
 namespace {
-// Grid barrier b of a bwcurve_kernel launch, called by every thread.  Arrivals count on one word that only rises, so
-// barrier b is complete at (b + 1) x gridDim.x arrivals; the CTA that completes it stamps *t_rel and releases b + 1.
-// Returns false in every thread once the launch is aborted (the deadline is checked at every arrival, as in barrier()).
-__device__ bool grid_sync(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long long* t_rel) {
+// The entry of bwcurve_kernel and allreduce_kernel, in the probe kernel's shared-memory layout: the warp's stages and
+// mbarriers (initialised here), the launch's abort word and the deadline timeout_ns from now.  *red gets the CTA
+// reduction slots.  cdprobe_kernel has its own copy, which also stamps its entry time.
+__device__ __forceinline__ Ctx enter(uint8_t* smem, unsigned int* abort_word, uint64_t timeout_ns, uint64_t** red) {
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
+  *red = bars + kWarpsPerCta * kStages;
+  __shared__ uint64_t s_deadline;
+  Ctx c;
+  c.abort_word = abort_word;
+  c.warp = threadIdx.x >> 5;
+  c.lane = threadIdx.x & 31;
+  c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
+  c.bar_smem = smem_u32(bars) + c.warp * kStages * 8u;
+  c.parity_bits = 0u;
+  if (threadIdx.x == 0) s_deadline = gtimer() + timeout_ns;
+  if (c.lane == 0) {
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) mbar_init(c.bar_smem + 8u * s, 1u);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  c.deadline = s_deadline;
+  return c;
+}
+
+// Grid barrier b of a bwcurve_kernel or allreduce_kernel launch, called by every thread.  Arrivals count on one word
+// that only rises, so barrier b is complete at (b + 1) x gridDim.x arrivals; the CTA that completes it stamps *t_rel
+// (unless null) and releases b + 1.  Given the all-reduce's peer lines (dom) and more than one rank, it is a domain
+// barrier: before the stamp, that CTA stores (call_seq << 16) | (b + 1) into this rank's line in every peer's Ctrl
+// granule (st.relaxed.sys) and waits until every peer's line in this rank's granule holds at least that
+// (ld.acquire.sys).  Nothing is published at it (the inputs are written at open, the output is local), so no fence
+// precedes the stores.  Returns false in every thread once the launch is aborted (the deadline is checked at every
+// arrival, as in barrier()).
+__device__ bool grid_barrier(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long long* t_rel,
+                             const AllReduceParams* dom) {
   __shared__ bool s_go;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -964,8 +995,17 @@ __device__ bool grid_sync(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long
     if (go) {
       const unsigned int prev = atomicAdd(&bs->arrive, 1u);
       if (prev == (b + 1u) * gridDim.x - 1u) {
-        *t_rel = gtimer();
-        st_release_gpu(&bs->release, b + 1ull);
+        if (dom != nullptr && dom->n > 1) {
+          const uint64_t v = (dom->call_seq << kArBarrierBits) | (b + 1ull);
+          for (uint32_t j = 0; j < dom->n; ++j)
+            if (j != dom->rank) st_relaxed_sys(dom->sig_out[j], v);
+          for (uint32_t j = 0; j < dom->n && go; ++j)
+            if (j != dom->rank) go = spin_until<kScopeSys>(c, &dom->sig_in[j].v, v);
+        }
+        if (go) {
+          if (t_rel != nullptr) *t_rel = gtimer();
+          st_release_gpu(&bs->release, b + 1ull);
+        }
       } else {
         go = spin_until<kScopeGpu>(c, &bs->release, b + 1ull);
       }
@@ -984,26 +1024,9 @@ __device__ bool grid_sync(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long
 // state (barrier, stamps, checksums, abort word) is in the rank's scratch buffer; Ctrl is not touched.
 __global__ void __launch_bounds__(kThreads, 1) bwcurve_kernel(const __grid_constant__ BwCurveParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
-  uint64_t* red = bars + kWarpsPerCta * kStages;
-  __shared__ uint64_t s_deadline;
   BwScratch* bs = P.scratch;
-
-  Ctx c;
-  c.abort_word = &bs->abort_flag;
-  c.warp = threadIdx.x >> 5;
-  c.lane = threadIdx.x & 31;
-  c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
-  c.bar_smem = smem_u32(bars) + c.warp * kStages * 8u;
-  c.parity_bits = 0u;
-  if (threadIdx.x == 0) s_deadline = gtimer() + P.timeout_ns;
-  if (c.lane == 0) {
-#pragma unroll
-    for (int s = 0; s < kStages; ++s) mbar_init(c.bar_smem + 8u * s, 1u);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  c.deadline = s_deadline;
+  uint64_t* red;
+  Ctx c = enter(smem, &bs->abort_flag, P.timeout_ns, &red);
 
   const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
   const uint32_t nwarps = gridDim.x * kWarpsPerCta;
@@ -1011,7 +1034,7 @@ __global__ void __launch_bounds__(kThreads, 1) bwcurve_kernel(const __grid_const
   for (uint32_t k = 0; k < P.n_sizes; ++k) {
     const uint64_t bytes = P.size[k];
     for (uint32_t r = 0; r <= P.reps; ++r, ++b) {
-      if (!grid_sync(c, bs, b, &bs->t_rel[k][r])) return;
+      if (!grid_barrier(c, bs, b, &bs->t_rel[k][r], nullptr)) return;
       Sum a{0ull, 0ull, 0ull};
       read_units(c, P.path, P.region, bytes, strided(bytes, gwarp, nwarps), a);
       Acc* const acc = &bs->rep[k][r];
@@ -1021,16 +1044,16 @@ __global__ void __launch_bounds__(kThreads, 1) bwcurve_kernel(const __grid_const
   }
 }
 
-// The per-granule (sum, xor) of a source region from the pattern definition: one warp per 16 KiB granule.
-__global__ void __launch_bounds__(256) bwcurve_granules_kernel(uint64_t* gsum, uint64_t* gxor, uint64_t seed,
-                                                                uint32_t rank, uint64_t first_word, uint64_t n_granules) {
+// The per-granule (sum, xor) of a region whose word k is word(k), from the pattern definition: one warp per 16 KiB
+// granule.  Instantiated for bwcurve's source slices (SrcRegionWord) and the all-reduce output (AllReduceWord).
+template <typename Word>
+__global__ void __launch_bounds__(256) granules_kernel(uint64_t* gsum, uint64_t* gxor, Word word, uint64_t n_granules) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
   for (uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n_granules; g += nwarps) {
-    const uint64_t w0 = first_word + g * kGranuleWords;
     uint64_t s = 0, x = 0;
     for (uint32_t k = lane; k < kGranuleWords; k += 32) {
-      const uint64_t w = src_word(seed, rank, w0 + k);
+      const uint64_t w = word(g * kGranuleWords + k);
       s += w;
       x ^= w;
     }
@@ -1216,42 +1239,6 @@ __device__ void ar_check(const Ctx& c, const AllReduceParams& P, ArScratch* as, 
     atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
   }
 }
-
-// Barrier b of an allreduce_kernel launch, called by every thread: grid_sync's grid barrier on the same rising
-// counter.  At a domain barrier with peers, the CTA that completes it first stores (call_seq << 16) | (b + 1) into this
-// rank's line in every peer's Ctrl granule (st.relaxed.sys) and waits until every peer's line in this rank's granule
-// holds at least that (ld.acquire.sys); then it stamps *t_rel and releases the grid.  Nothing is published at it (the
-// inputs are written at open, the output is local), so no fence precedes the stores.  Returns false in every thread
-// once the launch is aborted (the deadline is checked at every arrival).
-__device__ bool ar_sync(const Ctx& c, const AllReduceParams& P, BwScratch* bs, uint32_t b, bool domain,
-                        unsigned long long* t_rel) {
-  __shared__ bool s_go;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    bool go = !check_abort(c);
-    if (go) {
-      const unsigned int prev = atomicAdd(&bs->arrive, 1u);
-      if (prev == (b + 1u) * gridDim.x - 1u) {
-        if (domain && P.n > 1) {
-          const uint64_t v = (P.call_seq << kArBarrierBits) | (b + 1ull);
-          for (uint32_t j = 0; j < P.n; ++j)
-            if (j != P.rank) st_relaxed_sys(P.sig_out[j], v);
-          for (uint32_t j = 0; j < P.n && go; ++j)
-            if (j != P.rank) go = spin_until<kScopeSys>(c, &P.sig_in[j].v, v);
-        }
-        if (go) {
-          if (t_rel != nullptr) *t_rel = gtimer();
-          st_release_gpu(&bs->release, b + 1ull);
-        }
-      } else {
-        go = spin_until<kScopeGpu>(c, &bs->release, b + 1ull);
-      }
-    }
-    s_go = go;
-  }
-  __syncthreads();
-  return s_go;
-}
 }  // namespace
 
 // One rank of cdprobe_allreduce: for every size of the ladder, one warm-up and P.reps timed reps, each summing the
@@ -1262,27 +1249,10 @@ __device__ bool ar_sync(const Ctx& c, const AllReduceParams& P, BwScratch* bs, u
 // word-check counters, abort word) is in the rank's scratch buffer; outside it only its barrier lines are written.
 __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_constant__ AllReduceParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWarpsPerCta * kStages * kUnitBytes);
-  uint64_t* red = bars + kWarpsPerCta * kStages;
-  __shared__ uint64_t s_deadline;
   ArScratch* as = P.scratch;
   BwScratch* bs = &as->rep;
-
-  Ctx c;
-  c.abort_word = &bs->abort_flag;
-  c.warp = threadIdx.x >> 5;
-  c.lane = threadIdx.x & 31;
-  c.stage_smem = smem_u32(smem) + c.warp * kStages * kUnitBytes;
-  c.bar_smem = smem_u32(bars) + c.warp * kStages * 8u;
-  c.parity_bits = 0u;
-  if (threadIdx.x == 0) s_deadline = gtimer() + P.timeout_ns;
-  if (c.lane == 0) {
-#pragma unroll
-    for (int s = 0; s < kStages; ++s) mbar_init(c.bar_smem + 8u * s, 1u);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  c.deadline = s_deadline;
+  uint64_t* red;
+  Ctx c = enter(smem, &bs->abort_flag, P.timeout_ns, &red);
 
   const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
   const uint32_t nwarps = gridDim.x * kWarpsPerCta;
@@ -1290,7 +1260,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_con
   for (uint32_t k = 0; k < P.n_sizes; ++k) {
     const uint64_t bytes = P.size[k];
     for (uint32_t r = 0; r <= P.reps; ++r) {
-      if (!ar_sync(c, P, bs, b++, true, &bs->t_rel[k][r])) return;
+      if (!grid_barrier(c, bs, b++, &bs->t_rel[k][r], &P)) return;
       const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
       Sum a{0ull, 0ull, 0ull};
       const Walk<false> walk = strided(bytes, gwarp, nwarps);
@@ -1302,33 +1272,24 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_con
       cta_reduce<1>(c, red, &a, &acc);
       if (threadIdx.x == 0) atomicMax(&acc->t_end, (unsigned long long)gtimer());
     }
-    if (!ar_sync(c, P, bs, b++, false, nullptr)) return;
+    if (!grid_barrier(c, bs, b++, nullptr, nullptr)) return;
     ar_check(c, P, as, k, bytes, gwarp, nwarps);
   }
 }
 
-// The per-granule (sum, xor) of the all-reduce output from the pattern definition: one warp per 16 KiB granule.
-__global__ void __launch_bounds__(256) allreduce_granules_kernel(uint64_t* gsum, uint64_t* gxor, uint64_t seed,
-                                                                  uint32_t n, uint64_t n_granules) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
-  for (uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n_granules; g += nwarps) {
-    uint64_t s = 0, x = 0;
-    for (uint32_t k = lane; k < kGranuleWords; k += 32) {
-      const uint64_t w = allreduce_word(seed, n, g * kGranuleWords + k);
-      s += w;
-      x ^= w;
-    }
-    s = warp_sum64(s);
-    x = warp_xor64(x);
-    if (lane == 0) {
-      gsum[g] = s;
-      gxor[g] = x;
-    }
-  }
-}
-
 // ----------------------------------------------------------- launchers -----
+namespace {
+// Launches a persistent kernel (cdprobe_kernel, bwcurve_kernel or allreduce_kernel) on `stream` of the current device:
+// `grid` CTAs of kThreads threads and kSmemBytes of dynamic shared memory, cooperative or not.  Returns a cudaError_t.
+template <typename Params>
+int grid_launch(void (*kernel)(Params), const Params& p, unsigned grid, bool cooperative, cudaStream_t stream) {
+  void* args[] = {const_cast<Params*>(&p)};
+  const void* f = reinterpret_cast<const void*>(kernel);
+  return (int)(cooperative ? cudaLaunchCooperativeKernel(f, dim3(grid), dim3(kThreads), args, kSmemBytes, stream)
+                           : cudaLaunchKernel(f, dim3(grid), dim3(kThreads), args, kSmemBytes, stream));
+}
+}  // namespace
+
 int probe_kernel_prepare(int* max_ctas_per_sm) {
   cudaError_t e = cudaFuncSetAttribute(cdprobe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
   if (e != cudaSuccess) return (int)e;
@@ -1340,14 +1301,7 @@ int probe_kernel_prepare(int* max_ctas_per_sm) {
 }
 
 int probe_kernel_launch(const ProbeParams* p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  void* args[] = {const_cast<ProbeParams*>(p)};
-  cudaError_t e;
-  if (cooperative) {
-    e = cudaLaunchCooperativeKernel((const void*)cdprobe_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
-  } else {
-    e = cudaLaunchKernel((const void*)cdprobe_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
-  }
-  return (int)e;
+  return grid_launch(cdprobe_kernel, *p, grid, cooperative, stream);
 }
 
 int probe_fill_launch(void* dst, uint64_t bytes, uint64_t seed, uint32_t rank, unsigned grid, cudaStream_t stream) {
@@ -1356,45 +1310,26 @@ int probe_fill_launch(void* dst, uint64_t bytes, uint64_t seed, uint32_t rank, u
 }
 
 int bwcurve_launch(const BwCurveParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(bwcurve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e != cudaSuccess) return (int)e;
-  void* args[] = {const_cast<BwCurveParams*>(&p)};
-  if (cooperative) {
-    e = cudaLaunchCooperativeKernel((const void*)bwcurve_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
-  } else {
-    e = cudaLaunchKernel((const void*)bwcurve_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
-  }
-  return (int)e;
-}
-
-int bwcurve_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t rank, uint64_t first_word,
-                            uint64_t n_granules, unsigned grid, cudaStream_t stream) {
-  if (n_granules == 0) return (int)cudaSuccess;
-  const uint64_t need = (n_granules + 7) / 8;  // eight warps per block
-  bwcurve_granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, seed, rank, first_word,
-                                                                                    n_granules);
-  return (int)cudaGetLastError();
+  const cudaError_t e =
+      cudaFuncSetAttribute(bwcurve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  return e != cudaSuccess ? (int)e : grid_launch(bwcurve_kernel, p, grid, cooperative, stream);
 }
 
 int allreduce_launch(const AllReduceParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(allreduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e != cudaSuccess) return (int)e;
-  void* args[] = {const_cast<AllReduceParams*>(&p)};
-  if (cooperative) {
-    e = cudaLaunchCooperativeKernel((const void*)allreduce_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes,
-                                    stream);
-  } else {
-    e = cudaLaunchKernel((const void*)allreduce_kernel, dim3(grid), dim3(kThreads), args, kSmemBytes, stream);
-  }
-  return (int)e;
+  const cudaError_t e =
+      cudaFuncSetAttribute(allreduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  return e != cudaSuccess ? (int)e : grid_launch(allreduce_kernel, p, grid, cooperative, stream);
 }
 
-int allreduce_granules_launch(uint64_t* gsum, uint64_t* gxor, uint64_t seed, uint32_t n, uint64_t n_granules,
-                              unsigned grid, cudaStream_t stream) {
+template <typename Word>
+int granules_launch(uint64_t* gsum, uint64_t* gxor, const Word& word, uint64_t n_granules, unsigned grid,
+                    cudaStream_t stream) {
   if (n_granules == 0) return (int)cudaSuccess;
   const uint64_t need = (n_granules + 7) / 8;  // eight warps per block
-  allreduce_granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, seed, n, n_granules);
+  granules_kernel<<<need < grid ? (unsigned)need : grid, 256, 0, stream>>>(gsum, gxor, word, n_granules);
   return (int)cudaGetLastError();
 }
+template int granules_launch(uint64_t*, uint64_t*, const SrcRegionWord&, uint64_t, unsigned, cudaStream_t);
+template int granules_launch(uint64_t*, uint64_t*, const AllReduceWord&, uint64_t, unsigned, cudaStream_t);
 
 }  // namespace cdp

@@ -1,6 +1,7 @@
 // allreduce_fold.cc — runs the expected-checksum fold of probe_types.h that cdprobe_allreduce's host uses on cases
 // given on stdin, for tests/test_allreduce_cpu.py.  The per-granule table the fold reads is computed here as
-// allreduce_granules_kernel computes it on the GPU: the sum and the xor of the 2048 summed words of each whole granule.
+// granules_kernel<AllReduceWord> computes it on the GPU: the sum and the xor of the 2048 summed words of each whole
+// granule.
 //
 // One case per line, numbers in decimal:
 //   F <seed> <n> <output_words> <m> <w_0> ... <w_m-1>    prints per prefix of w_k words: <S> <X>

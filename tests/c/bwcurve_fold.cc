@@ -1,7 +1,7 @@
 // bwcurve_fold.cc — runs the size ladder and the expected-checksum fold of probe_types.h (what cdprobe_bwcurve's host
 // uses) on cases given on stdin, for tests/test_bwcurve_cpu.py.  The per-granule table the fold reads is computed here
-// as bwcurve_granules_kernel computes it on the GPU: the sum and the xor of the 2048 pattern words of each whole
-// granule.
+// as granules_kernel<SrcRegionWord> computes it on the GPU: the sum and the xor of the 2048 pattern words of each
+// whole granule.
 //
 // One case per line, numbers in decimal:
 //   L <bpp>                                            prints: <n> <size 0> ... <size n-1>   (n = 0: refused)

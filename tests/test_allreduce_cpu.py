@@ -242,7 +242,7 @@ def test_the_closing_timer_read_follows_the_last_store(kernel):
     assert len(reds) == 2
 
 
-def test_ptxas_reports_no_spills(tmp_path):
+def test_ptxas_reports_no_spills_in_allreduce_and_its_granule_kernel(tmp_path):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not found")
@@ -251,7 +251,7 @@ def test_ptxas_reports_no_spills(tmp_path):
                           capture_output=True, text=True, check=True)
     props = dict(re.findall(r"Function properties for (\S+)\n\s*\d+ bytes stack frame, (\d+ bytes spill stores, "
                             r"\d+ bytes spill loads)", proc.stderr))
-    ar = [k for k in props if "allreduce" in k]
+    ar = [k for k in props if "allreduce" in k or "granules_kernelINS_13AllReduceWord" in k]
     assert len(ar) == 2, proc.stderr
     assert all(props[k] == "0 bytes spill stores, 0 bytes spill loads" for k in ar), props
 

@@ -219,7 +219,7 @@ def test_the_closing_timer_read_follows_the_reps_loads_and_fold(kernel):
     assert len(reds) == 2 and bar < min(reds) and max(reds) < timer
 
 
-def test_ptxas_reports_no_spills(tmp_path):
+def test_ptxas_reports_no_spills_in_bwcurve_and_its_granule_kernel(tmp_path):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not found")
@@ -228,7 +228,7 @@ def test_ptxas_reports_no_spills(tmp_path):
                           capture_output=True, text=True, check=True)
     props = dict(re.findall(r"Function properties for (\S+)\n\s*\d+ bytes stack frame, (\d+ bytes spill stores, "
                             r"\d+ bytes spill loads)", proc.stderr))
-    bw = [k for k in props if "bwcurve" in k]
+    bw = [k for k in props if "bwcurve" in k or "granules_kernelINS_13SrcRegionWord" in k]
     assert len(bw) == 2, proc.stderr
     assert all(v == "0 bytes spill stores, 0 bytes spill loads" for v in props.values()), props
 
