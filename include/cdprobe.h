@@ -429,6 +429,52 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_allreduce_t;
 
+/* One-shot all-to-all across the domain (cdprobe_alltoall): every rank pushes one block to every peer at once, into the
+ * peer's exchange area, and every rank checks every word it receives (DESIGN §5h).  Per-rank entries [r] describe rank
+ * r as a sender and are filled by the process that hosts r; per-cell entries [s * CDPROBE_MAX_GPUS + d] describe the
+ * block from sender s to receiver d and are filled by the process that hosts the receiver d, which checks them (a cell
+ * that does not run also has its cell_status filled by the sender's process).  Size k of an entry is [..][k]. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: rank r's entries, and the cells it receives, are filled in */
+  uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
+  uint32_t n_sizes;                     /* entries of size[] */
+  uint32_t path;                        /* the write data path used (CDPROBE_OPT_PATH) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_alltoall calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint64_t area_bytes;                  /* this rank's exchange area: n x bytes_per_pair rounded up to 2 MiB */
+  uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per block per rep: the cdprobe_bwcurve ladder */
+  /* per rank, as the sender */
+  uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank's kernel ran */
+  int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_TIMEOUT: the rank's kernel passed timeout_ms (no times) */
+  uint32_t blocks[CDPROBE_MAX_GPUS];    /* blocks the rank pushes per rep: its cells that run */
+  float t0_ns[CDPROBE_MAX_GPUS];        /* ns_median of size[0] */
+  float peak_gbps[CDPROBE_MAX_GPUS];    /* max over k of blocks x size[k] / ns_median[k] (bytes per ns): egress */
+  uint64_t half_bytes[CDPROBE_MAX_GPUS]; /* the smallest size[k] whose egress rate reaches peak / 2 (computed before
+                                            peak is rounded) */
+  float ns_min[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* ns per rep over the timed reps (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];
+  /* per cell [sender * CDPROBE_MAX_GPUS + receiver] */
+  uint8_t cell_measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* 1: the block was pushed and checked */
+  int32_t cell_status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* 0 ok; CDPROBE_ERR_INTEGRITY: a word check found a bad
+                                                                 word; CDPROBE_ERR_TIMEOUT: the receiver's kernel passed
+                                                                 timeout_ms; else (cell_measured 0) the sender's mapping
+                                                                 status of the receiver, probe allocation or exchange
+                                                                 area */
+  uint32_t bad_sizes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* bit k set: some rep of size[k], warm-up included,
+                                                                 delivered a bad word */
+  uint64_t bad_words[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* words of the block that differ
+                                                                 from the pattern, summed over every rep of size[k] */
+  uint64_t first_bad[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* byte offset of the lowest of
+                                                                 them; UINT64_MAX when clean */
+  uint64_t sum[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* checksum S of the block as the
+                                                                 receiver read it in the last timed rep */
+  uint64_t xr[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];  /* checksum X */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_alltoall_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -452,10 +498,10 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce: diagnostics, benches,
- *   fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
- *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve and cdprobe_allreduce are
- *   optional for callers: a daemon binds them with dlsym and works without.
+ *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_alltoall:
+ *   diagnostics, benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce and
+ *   cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -498,6 +544,11 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              size[k] adds 1 to output word `word` (< 2^24) before it is stored and
                                              folded, so exactly that row and size fail the checksum (and the word check
                                              when reps == 1); 0 disarms */
+#define CDPROBE_OPT_ALLTOALL_FAULT 20u    /* tests: value = ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24)
+                                             | word arms a fault in transit in cdprobe_alltoall: in the process that
+                                             hosts `sender`, timed rep 1 of size[k] stores word `word` (< 2^24) of
+                                             block (sender -> receiver) xored with 1, so exactly that cell and size
+                                             fail the receiver's word check; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -597,6 +648,27 @@ CDPROBE_API int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* 
  * or an armed CDPROBE_OPT_ALLREDUCE_FAULT whose rank is >= n, whose k is >= n_sizes or whose word is
  * >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* One-shot all-to-all: every rank pushes a block to every peer at once.  For each size of the cdprobe_bwcurve ladder,
+ * one untimed warm-up rep, then `reps` timed reps.  In rep r of size k, sender i writes the first size bytes of block
+ * (i -> j) at offset i x bytes_per_pair of receiver j's exchange area: the probe's write pattern with the salt
+ * write_salt(seed, i, j, alltoall_seq(call_seq, k, r)), whose sequence value has its top bit set, so no rep repeats
+ * another's words or a run's.  The blocks of a rank are interleaved unit by unit (rank + 1, rank + 2, ... mod n, then
+ * the diagonal) on the CDPROBE_OPT_PATH write path with the rank's whole probe grid.  A rep runs between two domain
+ * barriers (flags in the Ctrl granule) and is timed per rank as a probe write phase: from the rank's release to its last
+ * CTA's completion stamp, which follows its stores and a fence.sys.  After every rep, warm-up included, every receiver
+ * compares every word it received with the pattern.  There is one cell per off-diagonal pair, plus (i, i) with a
+ * loop-back slice (n == 1 or CDPROBE_FLAG_LOCAL_DIAG); a cell runs when the sender maps the receiver's probe allocation
+ * and exchange area, and otherwise nobody writes or checks it.  If no cell of the domain runs (MIG), no kernel is
+ * launched and the call returns CDPROBE_OK.  The exchange area (n x bytes_per_pair per rank, rounded up to 2 MiB) is
+ * created on the first call with the probe allocation's handle type, mapped wherever the probe mapping is then up, and
+ * kept until close; if creating it fails in any process, every process returns that error, nothing runs, and the next
+ * call tries again.  A rank whose kernel passes timeout_ms is CDPROBE_ERR_TIMEOUT and the handle stays usable.
+ * Collective when world_size > 1: every process calls it with the same reps.  Needs no run first and touches no
+ * result, pattern, source buffer, landing slot, run_seq, warm-up state or other measurement's state.  *out carries abi,
+ * n and reps whatever the return code.  CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments
+ * that differ between processes, or an armed CDPROBE_OPT_ALLTOALL_FAULT that names no cell of the domain, a k >=
+ * n_sizes or a word >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -35,6 +35,7 @@ typedef int (*pp_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_pingpong_
 typedef int (*at_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_atomics_t*);
 typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
 typedef int (*ar_fn)(cdprobe_t*, uint32_t, cdprobe_allreduce_t*);
+typedef int (*a2a_fn)(cdprobe_t*, uint32_t, cdprobe_alltoall_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -45,6 +46,7 @@ static pp_fn cdp_pp;      // optional: absent from libraries that predate cdprob
 static at_fn cdp_at;      // optional: absent from libraries that predate cdprobe_atomics
 static bw_fn cdp_bw;      // optional: absent from libraries that predate cdprobe_bwcurve
 static ar_fn cdp_ar;      // optional: absent from libraries that predate cdprobe_allreduce
+static a2a_fn cdp_a2a;    // optional: absent from libraries that predate cdprobe_alltoall
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -62,6 +64,7 @@ static int cdp_load(const char* path) {
   cdp_at = (at_fn)dlsym(cdp_dl, "cdprobe_atomics");
   cdp_bw = (bw_fn)dlsym(cdp_dl, "cdprobe_bwcurve");
   cdp_ar = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce");
+  cdp_a2a = (a2a_fn)dlsym(cdp_dl, "cdprobe_alltoall");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -90,6 +93,8 @@ static int cdp_has_bwcurve(void) { return cdp_bw != NULL; }
 static int cdp_call_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* bw) { return cdp_bw(h, reps, bw); }
 static int cdp_has_allreduce(void) { return cdp_ar != NULL; }
 static int cdp_call_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) { return cdp_ar(h, reps, ar); }
+static int cdp_has_alltoall(void) { return cdp_a2a != NULL; }
+static int cdp_call_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* aa) { return cdp_a2a(h, reps, aa); }
 */
 import "C"
 
@@ -278,6 +283,31 @@ type AllReduce struct {
 	NsMin, NsMedian, NsMax [][]float32 // [rank][size]: ns per rep over the timed reps
 	Sum, Xr                [][]uint64  // [rank][size]: (S, X) of the output of the last timed rep
 	BadWords, FirstBad     [][]uint64  // [rank][size]: the word check; FirstBad is MaxUint64 when clean
+	Ms                     float64
+}
+
+// AllToAll is the one-shot all-to-all (cdprobe_alltoall_t).  Per-rank slices are indexed by the sender and filled for
+// this process's ranks; per-cell ones are [sender][receiver] and filled for the cells this process's ranks receive.  The
+// per-size ones hold one entry per Sizes element; every timing is 0 where a rank was not measured or timed out.
+type AllToAll struct {
+	N                      int
+	RowMask                uint32      // this process's ranks
+	Reps                   int         // timed reps per size, as applied
+	Path                   int         // the write data path (CDPROBE_OPT_PATH)
+	CallSeq                uint64      // 1-based count of AllToAll calls on this handle, equal in every process
+	AreaBytes              uint64      // this rank's exchange area
+	Sizes                  []uint64    // bytes per block per rep
+	Measured               []bool      // [rank]
+	Status                 []int32     // [rank]: 0 ok; CDPROBE_ERR_TIMEOUT
+	Blocks                 []uint32    // [rank]: blocks pushed per rep
+	T0Ns, PeakGBps         []float32   // [rank]: median ns of the smallest size; max over sizes of egress GB/s
+	HalfBytes              []uint64    // [rank]: the smallest size reaching half the peak
+	NsMin, NsMedian, NsMax [][]float32 // [rank][size]: ns per rep over the timed reps
+	CellMeasured           [][]bool    // [sender][receiver]
+	CellStatus             [][]int32   // [sender][receiver]: 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the mapping status
+	BadSizes               [][]uint32  // [sender][receiver]: bit k: Sizes[k] delivered a bad word
+	BadWords, FirstBad     [][][]uint64 // [sender][receiver][size]: the word check; FirstBad is MaxUint64 when clean
+	Sum, Xr                [][][]uint64 // [sender][receiver][size]: (S, X) of the block in the last timed rep
 	Ms                     float64
 }
 
@@ -653,6 +683,71 @@ func (p *Probe) AllReduce(reps int) (AllReduce, error) {
 			out.Xr[r][s] = uint64(ar.xr[r][s])
 			out.BadWords[r][s] = uint64(ar.bad_words[r][s])
 			out.FirstBad[r][s] = uint64(ar.first_bad[r][s])
+		}
+	}
+	return out, nil
+}
+
+// AllToAll runs the one-shot all-to-all: every rank pushes a block to every peer at once, at each size of the bwcurve
+// ladder, and every receiver checks every word (reps 0: 8 timed reps).  Collective when the domain spans processes.
+// ErrUnsupported when the library predates cdprobe_alltoall.
+func (p *Probe) AllToAll(reps int) (AllToAll, error) {
+	if C.cdp_has_alltoall() == 0 {
+		return AllToAll{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_alltoall", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	aa := new(C.cdprobe_alltoall_t)
+	rc := C.cdp_call_alltoall(p.h, C.uint32_t(reps), aa)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_alltoall: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllToAll{}, err
+	}
+	n, ns := int(aa.n), int(aa.n_sizes)
+	out := AllToAll{N: n, RowMask: uint32(aa.row_mask), Reps: int(aa.reps), Path: int(aa.path),
+		CallSeq: uint64(aa.call_seq), AreaBytes: uint64(aa.area_bytes), Ms: float64(aa.ms)}
+	out.Sizes = make([]uint64, ns)
+	for s := 0; s < ns; s++ {
+		out.Sizes[s] = uint64(aa.size[s])
+	}
+	out.Measured, out.Status, out.Blocks = make([]bool, n), make([]int32, n), make([]uint32, n)
+	out.T0Ns, out.PeakGBps, out.HalfBytes = make([]float32, n), make([]float32, n), make([]uint64, n)
+	out.NsMin, out.NsMedian, out.NsMax = make([][]float32, n), make([][]float32, n), make([][]float32, n)
+	out.CellMeasured, out.CellStatus, out.BadSizes = make([][]bool, n), make([][]int32, n), make([][]uint32, n)
+	out.BadWords, out.FirstBad = make([][][]uint64, n), make([][][]uint64, n)
+	out.Sum, out.Xr = make([][][]uint64, n), make([][][]uint64, n)
+	for r := 0; r < n; r++ {
+		out.Measured[r] = aa.measured[r] != 0
+		out.Status[r] = int32(aa.status[r])
+		out.Blocks[r] = uint32(aa.blocks[r])
+		out.T0Ns[r] = float32(aa.t0_ns[r])
+		out.PeakGBps[r] = float32(aa.peak_gbps[r])
+		out.HalfBytes[r] = uint64(aa.half_bytes[r])
+		out.NsMin[r], out.NsMedian[r], out.NsMax[r] = make([]float32, ns), make([]float32, ns), make([]float32, ns)
+		for s := 0; s < ns; s++ {
+			out.NsMin[r][s] = float32(aa.ns_min[r][s])
+			out.NsMedian[r][s] = float32(aa.ns_median[r][s])
+			out.NsMax[r][s] = float32(aa.ns_max[r][s])
+		}
+		out.CellMeasured[r], out.CellStatus[r], out.BadSizes[r] = make([]bool, n), make([]int32, n), make([]uint32, n)
+		out.BadWords[r], out.FirstBad[r] = make([][]uint64, n), make([][]uint64, n)
+		out.Sum[r], out.Xr[r] = make([][]uint64, n), make([][]uint64, n)
+		for d := 0; d < n; d++ {
+			c := r*C.CDPROBE_MAX_GPUS + d
+			out.CellMeasured[r][d] = aa.cell_measured[c] != 0
+			out.CellStatus[r][d] = int32(aa.cell_status[c])
+			out.BadSizes[r][d] = uint32(aa.bad_sizes[c])
+			out.BadWords[r][d], out.FirstBad[r][d] = make([]uint64, ns), make([]uint64, ns)
+			out.Sum[r][d], out.Xr[r][d] = make([]uint64, ns), make([]uint64, ns)
+			for s := 0; s < ns; s++ {
+				out.BadWords[r][d][s] = uint64(aa.bad_words[c][s])
+				out.FirstBad[r][d][s] = uint64(aa.first_bad[c][s])
+				out.Sum[r][d][s] = uint64(aa.sum[c][s])
+				out.Xr[r][d][s] = uint64(aa.xr[c][s])
+			}
 		}
 	}
 	return out, nil

@@ -147,6 +147,28 @@ type AllReduce struct {
 	Ms                     float64
 }
 
+type AllToAll struct {
+	N                      int
+	RowMask                uint32
+	Reps                   int
+	Path                   int
+	CallSeq                uint64
+	AreaBytes              uint64
+	Sizes                  []uint64
+	Measured               []bool
+	Status                 []int32
+	Blocks                 []uint32
+	T0Ns, PeakGBps         []float32
+	HalfBytes              []uint64
+	NsMin, NsMedian, NsMax [][]float32
+	CellMeasured           [][]bool
+	CellStatus             [][]int32
+	BadSizes               [][]uint32
+	BadWords, FirstBad     [][][]uint64
+	Sum, Xr                [][][]uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
@@ -159,4 +181,5 @@ func (*Probe) PingPong(int, int, bool) (PingPong, error) {
 func (*Probe) Atomics(int, int, int) (Atomics, error) { return Atomics{}, ErrUnsupported }
 func (*Probe) BwCurve(int) (BwCurve, error) { return BwCurve{}, ErrUnsupported }
 func (*Probe) AllReduce(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -14,6 +14,7 @@ through ``cdprobe_pkg.load()`` at the repo root, which registers it as
 from . import abi, build, distutil  # noqa: F401
 from .fabricprobe import (  # noqa: F401
     AllReduce,
+    AllToAll,
     Atomics,
     BwCurve,
     Config,
@@ -30,4 +31,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "AllToAll", "Open", "gate", "plan", "topology"]

@@ -26,13 +26,11 @@ constexpr size_t kArOutOff = (sizeof(ArScratch) + 255) / 256 * 256;
 struct AllReduceParams {
   const uint8_t* src[kMaxRanks];  // the n inputs in the order this rank adds them: rank + t (mod n) at src[t], each
                                   // through this rank's mapping, src[0] its own source buffer
-  uint64_t* sig_out[kMaxRanks];   // this rank's line in rank j's Ctrl granule (null for j == rank)
-  const FlagLine* sig_in;         // this rank's own lines: sig_in[j].v is the last barrier value rank j signalled
+  DomainLines dom;                // the domain barrier: push to and wait for every other rank through the kArOff lines
   ArScratch* scratch;
   uint8_t* out;                   // the output, in this rank's scratch
   uint64_t size[kBwMaxSizes];     // the ladder (bwcurve_ladder)
   uint64_t seed;                  // the pattern seed (the word check)
-  uint64_t call_seq;              // the barrier values' high bits
   uint64_t timeout_ns;            // device deadline from kernel entry
   uint64_t fault_word;            // the armed fault: timed rep 1 of size fault_k adds 1 to this output word
   uint32_t fault_k;               // kArNoFault: disarmed

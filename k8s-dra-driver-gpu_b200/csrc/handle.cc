@@ -51,21 +51,21 @@ static bool imex_channel0_present() {
   return true;
 }
 
-// Map rank j's allocation into local rank i's address space.
-static int32_t map_peer(cdprobe* h, uint32_t li, uint32_t j) {
+// Map rank j's allocation of m into local rank li's address space.
+static int32_t map_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   LocalRank& L = h->lr[li];
-  if (L.mapped[j]) return 0;
+  if ((L.*m.mapped)[j]) return 0;
   CUmemGenericAllocationHandle hnd;
   if (j >= h->first && j < h->first + h->n_local) {
-    hnd = h->lr[j - h->first].own;
-  } else if (h->has_import[j]) {
-    hnd = h->imported[j];
+    hnd = m.own[j - h->first];
+  } else if (m.has_import[j]) {
+    hnd = m.imported[j];
   } else {
     return CDPROBE_ERR_RENDEZVOUS;
   }
   if (cudaSetDevice(L.ordinal) != cudaSuccess) return CDPROBE_ERR_CUDA;
   CUdeviceptr va = 0;
-  const size_t sz = h->plan.alloc_bytes;
+  const size_t sz = m.bytes;
   CUresult r = h->drv.MemAddressReserve(&va, sz, kVmmGranule, 0, 0);
   if (r != CUDA_SUCCESS) return (int32_t)r;
   r = h->drv.MemMap(va, sz, 0, hnd, 0);
@@ -84,19 +84,191 @@ static int32_t map_peer(cdprobe* h, uint32_t li, uint32_t j) {
     h->drv.MemAddressFree(va, sz);
     return (int32_t)r;
   }
-  L.va[j] = va;
-  L.mapped[j] = true;
+  (L.*m.va)[j] = va;
+  (L.*m.mapped)[j] = true;
   return 0;
 }
 
-static void unmap_peer(cdprobe* h, uint32_t li, uint32_t j) {
+static void unmap_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   LocalRank& L = h->lr[li];
-  if (!L.mapped[j]) return;
+  if (!(L.*m.mapped)[j]) return;
   cudaSetDevice(L.ordinal);
-  h->drv.MemUnmap(L.va[j], h->plan.alloc_bytes);
-  h->drv.MemAddressFree(L.va[j], h->plan.alloc_bytes);
-  L.va[j] = 0;
-  L.mapped[j] = false;
+  h->drv.MemUnmap((L.*m.va)[j], m.bytes);
+  h->drv.MemAddressFree((L.*m.va)[j], m.bytes);
+  (L.*m.va)[j] = 0;
+  (L.*m.mapped)[j] = false;
+}
+
+// Unmaps m everywhere and releases every handle of it: its imports, then the local allocations and their fds.
+static void release_shared(cdprobe* h, SharedAlloc& m) {
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (h->lr[li].ordinal < 0) continue;
+    for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j) unmap_peer(h, m, li, j);
+  }
+  for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j)
+    if (m.has_import[j]) {
+      h->drv.MemRelease(m.imported[j]);
+      m.has_import[j] = false;
+    }
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (h->lr[li].ordinal < 0) continue;
+    cudaSetDevice(h->lr[li].ordinal);
+    if (m.has_own[li]) h->drv.MemRelease(m.own[li]);
+    m.has_own[li] = false;
+    if (m.own_fd[li] >= 0) ::close(m.own_fd[li]);
+    m.own_fd[li] = -1;
+  }
+  m.bytes = 0;
+}
+
+// Local rank li's allocation of m: m.bytes of its device's memory, exportable as the handle type chosen at open.
+static int create_own(cdprobe* h, SharedAlloc& m, uint32_t li) {
+  LocalRank& L = h->lr[li];
+  CDP_RT(cudaSetDevice(L.ordinal));
+  CUmemAllocationProp ap;
+  memset(&ap, 0, sizeof(ap));
+  ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  ap.location.id = L.ordinal;
+  ap.requestedHandleTypes = h->handle_type == 8u   ? CU_MEM_HANDLE_TYPE_FABRIC
+                            : h->handle_type == 1u ? CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR
+                                                   : CU_MEM_HANDLE_TYPE_NONE;
+  size_t gran = 0;
+  CUresult r = h->drv.MemGetAllocationGranularity(&gran, &ap, CU_MEM_ALLOC_GRANULARITY_MINIMUM);
+  if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemGetAllocationGranularity", r);
+  if (gran == 0 || kVmmGranule % gran != 0) {
+    set_err("unexpected VMM granularity " + std::to_string(gran));
+    return CDPROBE_ERR_UNSUPPORTED;
+  }
+  r = h->drv.MemCreate(&m.own[li], m.bytes, &ap, 0);
+  if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemCreate", r);
+  m.has_own[li] = true;
+  if (h->handle_type == 1u) {
+    int fd = -1;
+    r = h->drv.MemExportToShareableHandle(&fd, m.own[li], CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
+    if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemExportToShareableHandle(fd)", r);
+    m.own_fd[li] = fd;
+  }
+  return CDPROBE_OK;
+}
+
+// Creates m with allocations of `bytes`: one per local rank, exported and exchanged with every process over the
+// rendezvous, the other processes' imported, and rank j's mapped into local rank li wherever st[its rank][j] is 0 on
+// entry.  st[its rank][j] then holds the outcome: the import's CUresult, CDPROBE_ERR_UNSUPPORTED between MIG
+// instances, or map_peer's status.  With `agree`, the processes first share whether each created its allocations and
+// all return the first failure, so that none waits in an exchange another has left; without it (open, whose failure
+// ends the handle), a failure returns at once.  On failure the caller releases m.
+static int share_alloc(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*st)[kMaxRanks], bool agree) {
+  const cdprobe_config_t& c = h->cfg;
+  std::string err;
+  m.bytes = bytes;
+  int rc = CDPROBE_OK;
+  for (uint32_t li = 0; li < h->n_local && rc == CDPROBE_OK; ++li) rc = create_own(h, m, li);
+  if (agree && c.world_size > 1) {
+    int32_t mine = rc, all[kMaxRanks];
+    if (h->rdv.allgather(&mine, sizeof(mine), all, &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    for (uint32_t r = 0; r < c.world_size && rc == CDPROBE_OK; ++r)
+      if (all[r] != CDPROBE_OK) {
+        rc = all[r];
+        set_err("another process could not create its allocation");
+      }
+  }
+  if (rc != CDPROBE_OK) return rc;
+
+  // ---- exchange handles between processes ---------------------------------
+  if (c.world_size > 1) {
+    if (h->handle_type == 1u) {
+      int mine[kMaxRanks];
+      for (uint32_t li = 0; li < h->n_local; ++li) mine[li] = m.own_fd[li];
+      std::vector<int> all;
+      if (h->rdv.allgather_fds(mine, h->n_local, &all, &err) != 0) {
+        set_err(err);
+        return CDPROBE_ERR_RENDEZVOUS;
+      }
+      for (uint32_t j = 0; j < h->n_total; ++j) {
+        const bool local = j >= h->first && j < h->first + h->n_local;
+        if (!local) {
+          CUresult r = h->drv.MemImportFromShareableHandle(&m.imported[j], (void*)(uintptr_t)all[j],
+                                                           CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
+          if (r == CUDA_SUCCESS) m.has_import[j] = true;
+          else
+            for (uint32_t li = 0; li < h->n_local; ++li) st[h->first + li][j] = (int32_t)r;
+        }
+        ::close(all[j]);
+      }
+    } else {
+      CUmemFabricHandle mine[kMaxRanks], all[kMaxRanks];
+      memset(mine, 0, sizeof(mine));
+      for (uint32_t li = 0; li < h->n_local; ++li) {
+        CUresult r = h->drv.MemExportToShareableHandle(&mine[li], m.own[li], CU_MEM_HANDLE_TYPE_FABRIC, 0);
+        if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemExportToShareableHandle(fabric)", r);
+      }
+      if (h->rdv.allgather(mine, sizeof(CUmemFabricHandle) * h->n_local, all, &err) != 0) {
+        set_err(err);
+        return CDPROBE_ERR_RENDEZVOUS;
+      }
+      for (uint32_t j = 0; j < h->n_total; ++j) {
+        const bool local = j >= h->first && j < h->first + h->n_local;
+        if (local) continue;
+        CUresult r = h->drv.MemImportFromShareableHandle(&m.imported[j], &all[j], CU_MEM_HANDLE_TYPE_FABRIC);
+        if (r == CUDA_SUCCESS) m.has_import[j] = true;
+        else
+          for (uint32_t li = 0; li < h->n_local; ++li) st[h->first + li][j] = (int32_t)r;
+      }
+    }
+  }
+
+  // ---- map every rank's allocation into every local rank's address space --
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    for (uint32_t j = 0; j < h->n_total; ++j) {
+      int32_t s = st[L.grank][j];
+      if (s == 0) {
+        if (j != L.grank && L.mig && (c.flags & (CDPROBE_FLAG_MIG_AWARE | CDPROBE_FLAG_SIMULATE_MIG)))
+          s = CDPROBE_ERR_UNSUPPORTED;  // no P2P under MIG (SURVEY H8): identity matrix, "not applicable"
+        else s = map_peer(h, m, li, j);
+      }
+      st[L.grank][j] = s;
+    }
+  }
+  return CDPROBE_OK;
+}
+
+// Every process's rows of a mapping-status matrix (local ranks' rows filled in), gathered into every row of st.
+static int gather_status(cdprobe* h, int32_t (*st)[kMaxRanks]) {
+  if (h->cfg.world_size == 1) return CDPROBE_OK;
+  std::string err;
+  int32_t mine[kMaxRanks][kMaxRanks], all[kMaxRanks][kMaxRanks][kMaxRanks];
+  memset(mine, 0, sizeof(mine));
+  for (uint32_t li = 0; li < h->n_local; ++li) memcpy(mine[li], st[h->first + li], sizeof(mine[li]));
+  if (h->rdv.allgather(mine, sizeof(int32_t) * kMaxRanks * h->n_local, all, &err) != 0) {
+    set_err(err);
+    return CDPROBE_ERR_RENDEZVOUS;
+  }
+  const int32_t* flat = &all[0][0][0];
+  for (uint32_t g = 0; g < h->n_total; ++g) memcpy(st[g], flat + (size_t)g * kMaxRanks, sizeof(st[g]));
+  return CDPROBE_OK;
+}
+
+int ensure_area(cdprobe* h) {
+  if (h->area.bytes != 0) return CDPROBE_OK;
+  const size_t bytes = ((size_t)h->n_total * h->plan.bpp + kVmmGranule - 1) / kVmmGranule * kVmmGranule;
+  int32_t st[kMaxRanks][kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < h->n_total; ++j) st[h->lr[li].grank][j] = cell_status(h, li, j);
+  int rc = share_alloc(h, h->area, bytes, st, true);
+  if (rc == CDPROBE_OK) rc = gather_status(h, st);
+  if (rc != CDPROBE_OK) {
+    const std::string keep = g_last_error;
+    release_shared(h, h->area);
+    g_last_error = keep;
+    return rc;
+  }
+  memcpy(h->area_status, st, sizeof(st));
+  return CDPROBE_OK;
 }
 
 // Phase table of local rank li: see schedule.cc.
@@ -306,19 +478,13 @@ static void destroy(cdprobe* h) {
     if (L.ordinal < 0) continue;
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
-    for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j) unmap_peer(h, li, j);
   }
-  for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j)
-    if (h->has_import[j]) {
-      h->drv.MemRelease(h->imported[j]);
-      h->has_import[j] = false;
-    }
+  release_shared(h, h->area);
+  release_shared(h, h->mem);
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
     if (L.ordinal < 0) continue;
     cudaSetDevice(L.ordinal);
-    if (L.has_own) h->drv.MemRelease(L.own);
-    if (L.own_fd >= 0) ::close(L.own_fd);
     if (L.row) cudaFreeHost(L.row);
     if (L.scratch) cudaFree(L.scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
@@ -450,107 +616,24 @@ static int open_impl(const cdprobe_config_t* cfg, cdprobe* h) {
     CDP_RT(cudaEventCreate(&L.ev0));
     CDP_RT(cudaEventCreate(&L.ev1));
 
-    CUmemAllocationProp ap;
-    memset(&ap, 0, sizeof(ap));
-    ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-    ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    ap.location.id = L.ordinal;
-    ap.requestedHandleTypes = h->handle_type == 8u   ? CU_MEM_HANDLE_TYPE_FABRIC
-                              : h->handle_type == 1u ? CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR
-                                                     : CU_MEM_HANDLE_TYPE_NONE;
-    size_t gran = 0;
-    CUresult r = h->drv.MemGetAllocationGranularity(&gran, &ap, CU_MEM_ALLOC_GRANULARITY_MINIMUM);
-    if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemGetAllocationGranularity", r);
-    if (gran == 0 || kVmmGranule % gran != 0) {
-      set_err("unexpected VMM granularity " + std::to_string(gran));
-      return CDPROBE_ERR_UNSUPPORTED;
-    }
-    r = h->drv.MemCreate(&L.own, h->plan.alloc_bytes, &ap, 0);
-    if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemCreate", r);
-    L.has_own = true;
-    if (h->handle_type == 1u) {
-      int fd = -1;
-      r = h->drv.MemExportToShareableHandle(&fd, L.own, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
-      if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemExportToShareableHandle(fd)", r);
-      L.own_fd = fd;
-    }
     void* row = nullptr;
     CDP_RT(cudaHostAlloc(&row, sizeof(ResultRow), cudaHostAllocPortable | cudaHostAllocMapped));
     memset(row, 0, sizeof(ResultRow));
     L.row = static_cast<ResultRow*>(row);
   }
 
-  // ---- exchange handles between processes ---------------------------------
-  if (c.world_size > 1) {
-    if (h->handle_type == 1u) {
-      int mine[kMaxRanks];
-      for (uint32_t li = 0; li < h->n_local; ++li) mine[li] = h->lr[li].own_fd;
-      std::vector<int> all;
-      if (h->rdv.allgather_fds(mine, h->n_local, &all, &err) != 0) {
-        set_err(err);
-        return CDPROBE_ERR_RENDEZVOUS;
-      }
-      for (uint32_t j = 0; j < h->n_total; ++j) {
-        const bool local = j >= h->first && j < h->first + h->n_local;
-        if (!local) {
-          CUresult r = h->drv.MemImportFromShareableHandle(&h->imported[j], (void*)(uintptr_t)all[j],
-                                                           CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
-          if (r == CUDA_SUCCESS) h->has_import[j] = true;
-          else
-            for (uint32_t li = 0; li < h->n_local; ++li) h->status[h->first + li][j] = (int32_t)r;
-        }
-        ::close(all[j]);
-      }
-    } else {
-      CUmemFabricHandle mine[kMaxRanks], all[kMaxRanks];
-      memset(mine, 0, sizeof(mine));
-      for (uint32_t li = 0; li < h->n_local; ++li) {
-        CUresult r = h->drv.MemExportToShareableHandle(&mine[li], h->lr[li].own, CU_MEM_HANDLE_TYPE_FABRIC, 0);
-        if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemExportToShareableHandle(fabric)", r);
-      }
-      if (h->rdv.allgather(mine, sizeof(CUmemFabricHandle) * h->n_local, all, &err) != 0) {
-        set_err(err);
-        return CDPROBE_ERR_RENDEZVOUS;
-      }
-      for (uint32_t j = 0; j < h->n_total; ++j) {
-        const bool local = j >= h->first && j < h->first + h->n_local;
-        if (local) continue;
-        CUresult r = h->drv.MemImportFromShareableHandle(&h->imported[j], &all[j], CU_MEM_HANDLE_TYPE_FABRIC);
-        if (r == CUDA_SUCCESS) h->has_import[j] = true;
-        else
-          for (uint32_t li = 0; li < h->n_local; ++li) h->status[h->first + li][j] = (int32_t)r;
-      }
-    }
-  }
-
-  // ---- map every rank's allocation into every local rank's address space --
+  // ---- the probe allocations, shared with every process and mapped ---------
+  rc = share_alloc(h, h->mem, h->plan.alloc_bytes, h->status, false);
+  if (rc != CDPROBE_OK) return rc;
   for (uint32_t li = 0; li < h->n_local; ++li) {
-    LocalRank& L = h->lr[li];
-    for (uint32_t j = 0; j < h->n_total; ++j) {
-      int32_t st = h->status[L.grank][j];
-      if (st == 0) {
-        if (j != L.grank && L.mig && (c.flags & (CDPROBE_FLAG_MIG_AWARE | CDPROBE_FLAG_SIMULATE_MIG)))
-          st = CDPROBE_ERR_UNSUPPORTED;  // no P2P under MIG (SURVEY H8): identity matrix, "not applicable"
-        else st = map_peer(h, li, j);
-      }
-      h->status[L.grank][j] = st;
-    }
+    const LocalRank& L = h->lr[li];
     if (h->status[L.grank][L.grank] != 0) {
       set_err("cannot map own allocation: " + h->drv.error_name((CUresult)h->status[L.grank][L.grank]));
       return CDPROBE_ERR_CUDA;
     }
   }
-  if (c.world_size > 1) {
-    int32_t mine[kMaxRanks][kMaxRanks], all[kMaxRanks][kMaxRanks][kMaxRanks];
-    memset(mine, 0, sizeof(mine));
-    for (uint32_t li = 0; li < h->n_local; ++li) memcpy(mine[li], h->status[h->first + li], sizeof(mine[li]));
-    if (h->rdv.allgather(mine, sizeof(int32_t) * kMaxRanks * h->n_local, all, &err) != 0) {
-      set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    const int32_t* flat = &all[0][0][0];
-    for (uint32_t g = 0; g < h->n_total; ++g) memcpy(h->status[g], flat + (size_t)g * kMaxRanks, sizeof(h->status[g]));
-  }
+  rc = gather_status(h, h->status);
+  if (rc != CDPROBE_OK) return rc;
   rc = rebuild_all(h);
   if (rc != CDPROBE_OK) return rc;
   h->open_ms = now_ms() - t0;
@@ -984,6 +1067,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_ALLREDUCE_FAULT:  // checked against the domain and the size ladder by cdprobe_allreduce
       h->ar_fault = value;
       return CDPROBE_OK;
+    case CDPROBE_OPT_ALLTOALL_FAULT:  // checked against the domain and the size ladder by cdprobe_alltoall
+      h->a2a_fault = value;
+      return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;
   }
@@ -994,7 +1080,7 @@ int cdprobe_unmap_peer(cdprobe_t* h, uint32_t local, uint32_t peer) {
   if (h->cfg.world_size > 1) return CDPROBE_ERR_UNSUPPORTED;  // peers would not learn about it
   const uint32_t g = h->lr[local].grank;
   if (peer == g) return CDPROBE_ERR_ARG;
-  cdp::unmap_peer(h, local, peer);
+  cdp::unmap_peer(h, h->mem, local, peer);
   h->status[g][peer] = cdp::kStatusUnmapped;
   return cdp::rebuild_all(h);
 }
@@ -1004,8 +1090,8 @@ int cdprobe_remap_peer(cdprobe_t* h, uint32_t local, uint32_t peer) {
   const uint32_t g = h->lr[local].grank;
   if (peer == g) return CDPROBE_ERR_ARG;
   if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
-  cdp::unmap_peer(h, local, peer);
-  const int32_t st = cdp::map_peer(h, local, peer);
+  cdp::unmap_peer(h, h->mem, local, peer);
+  const int32_t st = cdp::map_peer(h, h->mem, local, peer);
   if (st != 0 && h->cfg.world_size > 1) {
     // the other processes build their phase tables from the mapping status exchanged at open and would
     // not learn that this pair is gone: the domain has to be reopened

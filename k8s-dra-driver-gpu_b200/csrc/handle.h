@@ -38,11 +38,10 @@ struct LocalRank {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int max_ctas = 0;
-  CUmemGenericAllocationHandle own = 0;
-  bool has_own = false;
-  int own_fd = -1;
-  CUdeviceptr va[kMaxRanks] = {};
+  CUdeviceptr va[kMaxRanks] = {};  // rank j's probe allocation as mapped here
   bool mapped[kMaxRanks] = {};
+  CUdeviceptr area_va[kMaxRanks] = {};  // rank j's exchange area (cdprobe_alltoall) as mapped here
+  bool area_mapped[kMaxRanks] = {};
   ResultRow* row = nullptr;
   char uuid[48] = {};
   Phase phases[kMaxPhases];
@@ -50,6 +49,23 @@ struct LocalRank {
   uint32_t peer_mask = 0;
   void* scratch = nullptr;  // device output of the on-demand measurements (measure.cc), grown on demand
   size_t scratch_bytes = 0;
+};
+
+// One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
+// exports them, takes the other processes' over the rendezvous, imports them and maps every rank's into every local
+// rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area is another.
+struct SharedAlloc {
+  size_t bytes = 0;                                       // of each allocation; 0: not created
+  CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
+  bool (LocalRank::*mapped)[kMaxRanks];
+  CUmemGenericAllocationHandle own[kMaxRanks] = {};       // [local rank]
+  bool has_own[kMaxRanks] = {};
+  int own_fd[kMaxRanks];                                  // [local rank] exported POSIX fd, -1: none
+  CUmemGenericAllocationHandle imported[kMaxRanks] = {};  // [rank] of another process
+  bool has_import[kMaxRanks] = {};
+  SharedAlloc(CUdeviceptr (LocalRank::*v)[kMaxRanks], bool (LocalRank::*m)[kMaxRanks]) : va(v), mapped(m) {
+    for (int& f : own_fd) f = -1;
+  }
 };
 
 }  // namespace cdp
@@ -62,9 +78,10 @@ struct cdprobe {
   uint32_t n_total = 0, n_local = 0, first = 0;
   uint32_t handle_type = 0;  // 0 none, 1 posix fd, 8 fabric
   cdp::LocalRank lr[cdp::kMaxRanks];
-  CUmemGenericAllocationHandle imported[cdp::kMaxRanks] = {};
-  bool has_import[cdp::kMaxRanks] = {};
+  cdp::SharedAlloc mem{&cdp::LocalRank::va, &cdp::LocalRank::mapped};             // the probe allocation
+  cdp::SharedAlloc area{&cdp::LocalRank::area_va, &cdp::LocalRank::area_mapped};  // cdprobe_alltoall's exchange area
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
+  int32_t area_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the exchange area, once it exists
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
   uint64_t seed = 0;
@@ -90,6 +107,8 @@ struct cdprobe {
   uint64_t bw_calls = 0;      // cdprobe_bwcurve calls that ran (call_seq of the last one)
   uint64_t ar_calls = 0;      // cdprobe_allreduce calls that ran (call_seq of the last one)
   uint64_t ar_fault = 0;      // CDPROBE_OPT_ALLREDUCE_FAULT value, 0: disarmed
+  uint64_t a2a_calls = 0;     // cdprobe_alltoall calls that ran (call_seq of the last one)
+  uint64_t a2a_fault = 0;     // CDPROBE_OPT_ALLTOALL_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -119,6 +138,13 @@ inline int require_usable(const cdprobe* h) {
   set_err("handle is unusable after an earlier timeout or CUDA error: close it and open a new one");
   return CDPROBE_ERR_STATE;
 }
+
+// cdprobe_alltoall's exchange area (handle.cc): on the first call, every local rank creates n_total x bytes_per_pair of
+// device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every local rank
+// wherever the probe mapping is then up; area_status gets every rank's mapping statuses.  Collective.  If creating it
+// fails in any process, every process returns that error with nothing kept, and the next call tries again.  Kept
+// until close.
+int ensure_area(cdprobe* h);
 
 // The mapping status of local rank li's cell [its rank][j]: kStatusUnmapped when that status is 0 but the peer is not
 // mapped.  Non-zero: never read or write through that mapping.

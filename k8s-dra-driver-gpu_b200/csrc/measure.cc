@@ -1,6 +1,6 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
-// cdprobe_atomics, cdprobe_bwcurve and cdprobe_allreduce.  Each runs on the local ranks' own streams, between probe
-// runs, and has its results on the host before it returns.
+// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce and cdprobe_alltoall.  Each runs on the local ranks' own streams,
+// between probe runs, and has its results on the host before it returns.
 #include <string.h>
 
 #include <algorithm>
@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "allreduce.h"
+#include "alltoall.h"
 #include "atomics.h"
 #include "bwcurve.h"
 #include "diagnose.h"
@@ -70,9 +71,9 @@ static bool begin_output(Out* out) {
 }
 
 // What each process contributes at the start of a collective measurement (cdprobe_pingpong, cdprobe_bwcurve,
-// cdprobe_allreduce), so that every process refuses, skips or runs the same call: the call number it is about to
-// make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and what the call
-// folds in from every process.
+// cdprobe_allreduce, cdprobe_alltoall), so that every process refuses, skips or runs the same call: the call number it
+// is about to make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and what
+// the call folds in from every process.
 template <typename Extra>
 struct Agreement {
   uint64_t call_seq;
@@ -173,34 +174,27 @@ static void summarize(const TimedRep* rep, uint32_t reps, uint32_t per_rep, uint
   out->status[idx] = s;
 }
 
-// Fills entry idx of a cdprobe_bwcurve_t (a cell) or a cdprobe_allreduce_t (a row) from the records bwcurve_kernel or
-// allreduce_kernel left in `s`: per size, ns of the timed reps and the (S, X) of the last one, every rep's (S, X)
-// compared with want[k] (bad_sizes), and the model-free summary of the medians.  An entry whose kernel was aborted at
-// the deadline has no times.
+// Fills the times of entry idx of a cdprobe_bwcurve_t (a cell), a cdprobe_allreduce_t (a row) or a cdprobe_alltoall_t
+// (a row) from the rep records bwcurve_kernel, allreduce_kernel or alltoall_kernel left in `s`: per size, ns of the
+// timed reps, and the model-free summary of the medians, whose rates are scale x size[k] / ns_median[k].  An entry
+// whose kernel was aborted at the deadline has no times and is CDPROBE_ERR_TIMEOUT; returns whether it has times.
 template <typename Out>
-static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes,
-                         uint32_t reps, uint32_t idx, Out* out) {
+static bool bw_times(const BwScratch& s, const uint64_t* size, uint32_t n_sizes, uint32_t reps, double scale,
+                     uint32_t idx, Out* out) {
   out->measured[idx] = 1;
   if (s.abort_flag != 0) {
     out->status[idx] = CDPROBE_ERR_TIMEOUT;
-    return;
+    return false;
   }
-  uint32_t bad = 0;
   double rate[kBwMaxSizes], peak = 0.0;
   for (uint32_t k = 0; k < n_sizes; ++k) {
     float ns[kMaxTimedReps];
-    for (uint32_t r = 0; r <= reps; ++r) {
-      const Acc& a = s.rep[k][r];
-      if (a.sum != want[k][0] || a.xr != want[k][1]) bad |= 1u << k;
-      if (r > 0) ns[r - 1] = (float)(a.t_end - s.t_rel[k][r]);
-    }
+    for (uint32_t r = 1; r <= reps; ++r) ns[r - 1] = (float)(s.rep[k][r].t_end - s.t_rel[k][r]);
     std::sort(ns, ns + reps);
     out->ns_min[idx][k] = ns[0];
     out->ns_median[idx][k] = ns[reps / 2];
     out->ns_max[idx][k] = ns[reps - 1];
-    out->sum[idx][k] = s.rep[k][reps].sum;
-    out->xr[idx][k] = s.rep[k][reps].xr;
-    rate[k] = ns[reps / 2] > 0.f ? (double)size[k] / (double)ns[reps / 2] : 0.0;
+    rate[k] = ns[reps / 2] > 0.f ? scale * (double)size[k] / (double)ns[reps / 2] : 0.0;
     peak = std::max(peak, rate[k]);
   }
   out->t0_ns[idx] = out->ns_median[idx][0];
@@ -210,6 +204,25 @@ static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const ui
       out->half_bytes[idx] = size[k];
       break;
     }
+  }
+  out->status[idx] = 0;
+  return true;
+}
+
+// Fills entry idx of a cdprobe_bwcurve_t (a cell) or a cdprobe_allreduce_t (a row): the times (bw_times), the (S, X) of
+// each size's last rep, and every rep's (S, X) compared with want[k] (bad_sizes).
+template <typename Out>
+static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes,
+                         uint32_t reps, uint32_t idx, Out* out) {
+  if (!bw_times(s, size, n_sizes, reps, 1.0, idx, out)) return;
+  uint32_t bad = 0;
+  for (uint32_t k = 0; k < n_sizes; ++k) {
+    for (uint32_t r = 0; r <= reps; ++r) {
+      const Acc& a = s.rep[k][r];
+      if (a.sum != want[k][0] || a.xr != want[k][1]) bad |= 1u << k;
+    }
+    out->sum[idx][k] = s.rep[k][reps].sum;
+    out->xr[idx][k] = s.rep[k][reps].xr;
   }
   out->bad_sizes[idx] = bad;
   out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
@@ -782,14 +795,16 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
     cdp::AllReduceParams p;
     memset(&p, 0, sizeof(p));
     for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + pl.src_off;
-    for (uint32_t j = 0; j < n; ++j)
-      if (j != g) p.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kArOff + (uint64_t)g * sizeof(cdp::FlagLine));
-    p.sig_in = reinterpret_cast<const cdp::FlagLine*>(L.va[g] + cdp::kArOff);
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g) continue;
+      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kArOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kArOff + (uint64_t)j * sizeof(cdp::FlagLine));
+    }
+    p.dom.call_seq = h->ar_calls;
     p.scratch = static_cast<cdp::ArScratch*>(L.scratch);
     p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
     memcpy(p.size, size, sizeof(size));
     p.seed = h->seed;
-    p.call_seq = h->ar_calls;
     p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
     p.fault_k = g == f_rank ? f_k : cdp::kArNoFault;
     p.fault_word = f_word;
@@ -821,6 +836,173 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
         out->bad_sizes[g] |= 1u << k;
         out->status[g] = CDPROBE_ERR_INTEGRITY;
       }
+    }
+  }
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
+  out->reps = reps != 0 ? reps : cdp::kA2aDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  out->path = h->path;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
+  //    every process refuses or runs together over the same cells
+  std::string bad;
+  uint64_t size[cdp::kBwMaxSizes];
+  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
+  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
+  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
+  uint32_t f_send = cdp::kA2aNoFault, f_recv = cdp::kA2aNoFault, f_k = cdp::kA2aNoFault;
+  uint64_t f_word = 0;
+  if (h->a2a_fault != 0 && bad.empty()) {
+    const uint64_t fs = h->a2a_fault >> 40, fr = (h->a2a_fault >> 32) & 0xffu, fk = (h->a2a_fault >> 24) & 0xffu;
+    f_word = h->a2a_fault & 0xffffffu;
+    if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || fk == 0 || fk > n_sizes ||
+        f_word >= size[fk - 1] / 8) {
+      bad = "the armed all-to-all fault names no cell, size or word of this call";
+    } else {
+      f_send = (uint32_t)fs - 1;
+      f_recv = (uint32_t)fr - 1;
+      f_k = (uint32_t)fk - 1;
+    }
+  }
+  using Rows = int32_t[cdp::kMaxRanks][cdp::kMaxRanks];
+  cdp::Agreement<Rows> mine = {h->a2a_calls + 1, {reps, 0u, 0u}, 0u, {}};
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < n; ++j) mine.extra[li][j] = cdp::cell_status(h, li, j);
+  std::vector<cdp::Agreement<Rows>> all;
+  if (const int rc = cdp::agree(h, "cdprobe_alltoall", bad, mine, all); rc != CDPROBE_OK) return rc;
+  // 2. the exchange area, built once, by every process in the same call
+  if (const int rc = cdp::ensure_area(h); rc != CDPROBE_OK) return rc;
+  h->a2a_calls = mine.call_seq;
+  out->call_seq = h->a2a_calls;
+  out->area_bytes = h->area.bytes;
+  out->n_sizes = n_sizes;
+  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+
+  // 3. which cells run: st[s][d], the probe mapping status of sender s's cell to receiver d, or else its exchange-area
+  //    mapping status; 0 runs.  Every process derives the same matrix.
+  Rows st = {};
+  for (uint32_t r = 0; r < all.size(); ++r)
+    for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].extra[li], sizeof(st[0]));
+  bool any = false;
+  for (uint32_t s = 0; s < n; ++s) {
+    for (uint32_t d = 0; d < n; ++d) {
+      if (st[s][d] == 0) st[s][d] = h->area_status[s][d];
+      if (s == d && !pl.diag) st[s][d] = CDPROBE_ERR_ARG;  // no such cell
+      any |= st[s][d] == 0;
+    }
+  }
+  auto runs = [&](uint32_t s, uint32_t d) { return st[s][d] == 0; };
+  const bool local_fault = f_send >= h->first && f_send < h->first + h->n_local;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const uint32_t g = h->lr[li].grank;
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g && !pl.diag) continue;
+      if (!runs(g, j)) out->cell_status[g * CDPROBE_MAX_GPUS + j] = st[g][j];
+      if (!runs(j, g)) out->cell_status[j * CDPROBE_MAX_GPUS + g] = st[j][g];
+    }
+  }
+  if (!any) {  // e.g. MIG instances: nothing to exchange anywhere, so no kernel is launched in any process
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 4. the records, grown on every local rank; then no process launches before every process is ready, and every local
+  //    kernel is launched before any is waited for
+  if (const int rc = cdp::ensure_scratch_all(h, sizeof(cdp::A2aScratch)); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
+  bool launched[cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::AllToAllParams p;
+    memset(&p, 0, sizeof(p));
+    // the barrier: with every rank a cell joins to this one; rank j pushes to this rank when it maps it, else this
+    // rank polls line j of j's own memory through its own mapping
+    bool joined = runs(g, g);
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g || !(runs(g, j) || runs(j, g))) continue;
+      joined = true;
+      if (runs(g, j))
+        p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(
+          runs(j, g) ? L.va[g] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine)
+                     : L.va[j] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine));
+    }
+    if (!joined) continue;
+    p.dom.self = reinterpret_cast<uint64_t*>(L.va[g] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
+    p.dom.call_seq = h->a2a_calls;
+    // the blocks, in the order rank + 1, rank + 2, ... (mod n), then the diagonal
+    p.fault_k = cdp::kA2aNoFault;
+    for (uint32_t d = 1; d <= n; ++d) {
+      const uint32_t j = (g + d) % n;
+      if (!runs(g, j)) continue;
+      if (local_fault && g == f_send && j == f_recv) {
+        p.fault_k = f_k;
+        p.fault_block = p.blocks;
+        p.fault_word = f_word;
+      }
+      p.to[p.blocks] = j;
+      p.dst[p.blocks++] = reinterpret_cast<uint8_t*>(L.area_va[j]) + (uint64_t)g * pl.bpp;
+    }
+    for (uint32_t s = 0; s < n; ++s) {
+      if (!runs(s, g)) continue;
+      p.from[p.n_in] = s;
+      p.in[p.n_in++] = reinterpret_cast<const uint8_t*>(L.area_va[g]) + (uint64_t)s * pl.bpp;
+    }
+    p.scratch = static_cast<cdp::A2aScratch*>(L.scratch);
+    memcpy(p.size, size, sizeof(size));
+    p.seed = h->seed;
+    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.rank = g;
+    p.n_sizes = n_sizes;
+    p.reps = reps;
+    p.path = h->path;
+    out->blocks[g] = p.blocks;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::A2aScratch), L.stream);
+    if (e == cudaSuccess) e = (cudaError_t)cdp::alltoall_launch(p, L.ctas, L.coop && coop_ok, L.stream);
+    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch alltoall_kernel", e);
+    launched[li] = true;
+  }
+
+  // 5. collect: per rank, the egress times; per cell it receives, the word checks and the last rep's (S, X)
+  std::vector<cdp::A2aScratch> got(1);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (!launched[li]) continue;
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::A2aScratch), got.data(), "cdprobe_alltoall"); rc != CDPROBE_OK)
+      return rc;
+    const cdp::A2aScratch& s = got[0];
+    const bool timed = cdp::bw_times(s.rep, size, n_sizes, reps, (double)out->blocks[g], g, out);
+    for (uint32_t i = 0; i < n; ++i) {
+      if (!runs(i, g)) continue;
+      const uint32_t cell = i * CDPROBE_MAX_GPUS + g;
+      out->cell_measured[cell] = 1;
+      if (!timed) {
+        out->cell_status[cell] = CDPROBE_ERR_TIMEOUT;
+        continue;
+      }
+      for (uint32_t k = 0; k < n_sizes; ++k) {
+        out->bad_words[cell][k] = s.bad_words[i][k];
+        out->first_bad[cell][k] = s.bad_words[i][k] != 0 ? ~s.first_bad_n[i][k] : UINT64_MAX;
+        out->sum[cell][k] = s.sum[i][k];
+        out->xr[cell][k] = s.xr[i][k];
+        if (s.bad_words[i][k] != 0) out->bad_sizes[cell] |= 1u << k;
+      }
+      out->cell_status[cell] = out->bad_sizes[cell] ? CDPROBE_ERR_INTEGRITY : 0;
     }
   }
   out->ms = cdp::now_ms() - t_begin;

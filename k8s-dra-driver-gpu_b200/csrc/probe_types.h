@@ -168,6 +168,11 @@ CDP_HD inline uint64_t src_word(uint64_t seed, uint32_t rank, uint64_t k) {
 CDP_HD inline uint64_t write_salt(uint64_t seed, uint32_t src, uint32_t dst, uint64_t run_seq) {
   return splitmix64(seed ^ 0x5752495445ull ^ ((uint64_t)src << 56) ^ ((uint64_t)dst << 48) ^ run_seq);
 }
+// The sequence value of rep r (0: the warm-up) of size k of cdprobe_alltoall call call_seq, used in place of run_seq in
+// write_salt.  Bit 63 is set, and a run_seq never has it, so no block of an all-to-all shares a salt with a probe run.
+CDP_HD inline uint64_t alltoall_seq(uint64_t call_seq, uint32_t k, uint32_t r) {
+  return (1ull << 63) | ((call_seq & ((1ull << 51) - 1)) << 12) | ((uint64_t)(k & 31u) << 7) | (uint64_t)(r & 127u);
+}
 CDP_HD inline uint64_t write_word(uint64_t salt, uint64_t k) {
   uint64_t z = (salt + k) * kGolden;
   return z ^ (z >> 32);
@@ -490,5 +495,24 @@ static_assert(kArOff % 128 == 0 && kArOff + kMaxRanks * sizeof(FlagLine) <= kCtr
               "the all-reduce lines sit after the atomics lines inside the Ctrl granule");
 constexpr uint32_t kArBarrierBits = 16;  // barriers per call: at most kBwMaxSizes x (kMaxTimedReps + 2) < 2^16
 constexpr uint32_t kArNoFault = ~0u;
+
+// The domain barrier of cdprobe_alltoall: one 128-byte line per rank after the all-reduce lines.  line[s] in rank o's
+// memory (s != o) holds the last (call_seq << 16) | (b + 1) rank s pushed to o; line[o] in its own memory holds the
+// last value o reached, for the peers that map o but are not mapped by it and so poll it.  Same rules as kArOff.
+constexpr uint64_t kA2aOff = kArOff + kMaxRanks * sizeof(FlagLine);  // 70 KiB
+static_assert(kA2aOff % 128 == 0 && kA2aOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the all-to-all lines sit after the all-reduce lines inside the Ctrl granule");
+static_assert(kBwMaxSizes * (64 + 1) * 2 < (1u << kArBarrierBits), "all-to-all barriers per call fit the low bits");
+
+// The flag lines a domain barrier exchanges (probe_kernels.cu, grid_barrier): its leader stores (call_seq << 16) |
+// (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
+// least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own
+// memory when this rank polls it.  All null: a grid barrier only.
+struct DomainLines {
+  uint64_t* sig_out[kMaxRanks];
+  const uint64_t* sig_in[kMaxRanks];
+  uint64_t* self;
+  uint64_t call_seq;
+};
 
 }  // namespace cdp

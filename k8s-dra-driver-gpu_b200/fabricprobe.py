@@ -395,6 +395,70 @@ class AllReduce:
                          ms=t.ms, raw=t)
 
 
+@dataclasses.dataclass
+class AllToAll:
+    """What cdprobe_alltoall measured.  Per rank r, as the sender: `blocks` pushed per rep, ns per rep (min, median and
+    max over the timed reps) of each size of the ladder `sizes`, and the summary of the medians: t0_ns (the smallest
+    size), peak_gbps (egress: blocks x size / ns) and half_bytes.  Per cell [s][d] (sender, receiver), as the receiver
+    checked it: `cell_status`, the sizes that delivered a bad word (`bad_sizes`, bit k for sizes[k]), `bad_words` and
+    `first_bad` (the byte offset of the lowest bad word, or U64_MAX) per size, and the (S, X) of the block in the last
+    timed rep.  Per-size values are lists over `sizes`.  A rank that did not run, or timed out, is None everywhere but
+    `measured` and `status`; a cell its receiver did not check is None everywhere but `cell_measured` and
+    `cell_status`."""
+    n: int
+    row_mask: int
+    reps: int
+    path: int
+    call_seq: int
+    area_bytes: int
+    sizes: List[int]
+    measured: List[bool]
+    status: List[int]     # 0 ok; ERR_TIMEOUT
+    blocks: List[Optional[int]]
+    t0_ns: List[Optional[float]]
+    peak_gbps: List[Optional[float]]
+    half_bytes: List[Optional[int]]
+    ns_min: List[Optional[List[float]]]
+    ns_median: List[Optional[List[float]]]
+    ns_max: List[Optional[List[float]]]
+    cell_measured: List[List[bool]]
+    cell_status: List[List[int]]  # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the sender's mapping status of the receiver
+    bad_sizes: List[List[Optional[int]]]
+    bad_words: List[List[Optional[List[int]]]]
+    first_bad: List[List[Optional[List[int]]]]
+    sum: List[List[Optional[List[int]]]]
+    xr: List[List[Optional[List[int]]]]
+    ms: float
+    raw: abi.AllToAllT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.AllToAllT) -> "AllToAll":
+        k, n, M = t.n_sizes, t.n, abi.MAX_GPUS
+
+        def timed(r):
+            return t.measured[r] and t.status[r] != abi.ERR_TIMEOUT
+
+        def row(a, per_size=False):
+            return [(list(a[r])[:k] if per_size else a[r]) if timed(r) else None for r in range(n)]
+
+        def checked(c):
+            return t.cell_measured[c] and t.cell_status[c] != abi.ERR_TIMEOUT
+
+        def cells(a, per_size=True):
+            return [[(list(a[s * M + d])[:k] if per_size else a[s * M + d]) if checked(s * M + d) else None
+                     for d in range(n)] for s in range(n)]
+
+        return AllToAll(n=n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
+                        area_bytes=t.area_bytes, sizes=list(t.size)[:k], measured=[bool(t.measured[r]) for r in range(n)],
+                        status=list(t.status)[:n], blocks=[t.blocks[r] if t.measured[r] else None for r in range(n)],
+                        t0_ns=row(t.t0_ns), peak_gbps=row(t.peak_gbps), half_bytes=row(t.half_bytes),
+                        ns_min=row(t.ns_min, True), ns_median=row(t.ns_median, True), ns_max=row(t.ns_max, True),
+                        cell_measured=[[bool(t.cell_measured[s * M + d]) for d in range(n)] for s in range(n)],
+                        cell_status=[[t.cell_status[s * M + d] for d in range(n)] for s in range(n)],
+                        bad_sizes=cells(t.bad_sizes, False), bad_words=cells(t.bad_words),
+                        first_bad=cells(t.first_bad), sum=cells(t.sum), xr=cells(t.xr), ms=t.ms, raw=t)
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -567,6 +631,20 @@ class Probe:
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
         t = abi.AllReduceT()
         rc = self._lib.cdprobe_allreduce(self._h, reps, C.byref(t))
+        return rc, t
+
+    def AllToAll(self, reps: int = 0) -> AllToAll:
+        """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
+        the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps
+        per size).  Collective when world_size > 1.  Needs no Run first and disturbs none."""
+        rc, t = self.alltoall_raw(reps)
+        _check(self._lib, rc, "cdprobe_alltoall")
+        return AllToAll.from_c(t)
+
+    def alltoall_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllToAllT as the library left it)."""
+        t = abi.AllToAllT()
+        rc = self._lib.cdprobe_alltoall(self._h, reps, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
