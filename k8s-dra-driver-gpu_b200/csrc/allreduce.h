@@ -1,5 +1,5 @@
-// allreduce.h — host-callable launchers of the one-shot all-reduce kernels in probe_kernels.cu (cdprobe_allreduce), and
-// the layout of the scratch buffer they share with the host.
+// allreduce.h — host-callable launchers of the one-shot all-reduce kernels in allreduce_kernels.cu (cdprobe_allreduce),
+// and the layout of the scratch buffer they share with the host.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

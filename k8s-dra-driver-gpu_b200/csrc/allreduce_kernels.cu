@@ -1,0 +1,226 @@
+// allreduce_kernels.cu — sm_90a kernels of cdprobe_allreduce's one-shot all-reduce: every warp streams one output unit
+// of all n ranks' source buffers (TMA ring or ld.global.v4), adds them in registers and stores the sum with
+// st.global.v4; each rep opens with a domain barrier (allreduce_kernel).  And the per-granule sums of the output that
+// the expected checksums are folded from (granules_kernel<AllReduceWord>).  The shared data path is in datapath.cuh.
+//
+// probe_kernels.cu is untouched: the probe kernel's code generation does not depend on this file.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "allreduce.h"
+#include "datapath.cuh"
+
+namespace cdp {
+namespace {
+constexpr int kArWords = 2 * kLdstVecs;  // uint64 accumulators per lane: a warp holds one 8 KiB output unit
+
+// Byte offset in a unit of the lane's 16-byte vector i when each access moves kLaneBytes contiguous bytes: the layout
+// job_read_ldst loads in, and for kLaneBytes = 16 also the one job_read_tma reads a stage in.
+template <uint32_t kLaneBytes>
+__device__ __forceinline__ uint32_t ar_vec_off(int lane, int i) {
+  constexpr int kV = kLaneBytes / 16;
+  return kLaneBytes * (uint32_t)lane + 32u * kLaneBytes * (uint32_t)(i / kV) + 16u * (uint32_t)(i % kV);
+}
+
+__device__ __forceinline__ void ar_add(uint64_t (&acc)[kArWords], int i, const uint4& v) {
+  acc[2 * i] += pack64(v.x, v.y);
+  acc[2 * i + 1] += pack64(v.z, v.w);
+}
+
+// Unit u of the output is complete in the accumulators: the armed fault goes in (fw, an output word index; ~0 when
+// none), every vector of the unit leaves with st.global.v4 and is folded into the (S, X) by its place in the output,
+// and the accumulators are cleared for the next unit.
+template <uint32_t kLaneBytes>
+__device__ __forceinline__ void ar_store(const Ctx& c, uint8_t* out, uint64_t u, uint32_t len, uint64_t fw,
+                                         uint64_t (&acc)[kArWords], Sum& a) {
+  if (fw / (kUnitBytes / 8) == u) {  // rare: this unit holds the armed word
+    const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
+#pragma unroll
+    for (int i = 0; i < kArWords / 2; ++i) {
+      if (ar_vec_off<kLaneBytes>(c.lane, i) != (fb & ~15u)) continue;
+      if (fb & 8u) acc[2 * i + 1] += 1ull;
+      else acc[2 * i] += 1ull;
+    }
+  }
+  uint8_t* base = out + u * kUnitBytes;
+  uint64_t ux = 0;
+#pragma unroll
+  for (int i = 0; i < kArWords / 2; ++i) {
+    const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+    const uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
+    if (off < len) {
+      stg_v4(reinterpret_cast<uint4*>(base + off),
+             make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+      add_pair(a, ux, w0, w1);
+    }
+    acc[2 * i] = 0ull;
+    acc[2 * i + 1] = 0ull;
+  }
+  fold_unit(a, ux, u);
+}
+
+// TMA read side: the warp walks (unit, input) pairs, the n inputs of a unit in a row, through its kStages-deep ring of
+// bulk loads, one load per pair.  Each stage is added into the accumulators and then refilled with the next pair, so
+// the ring runs on across unit boundaries.  Aborted: stops issuing and drains what is in flight.
+__device__ void ar_units_tma(Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw, Sum& a) {
+  const uint32_t n = P.n;
+  Walk<false> iw = walk;  // the issue side: up to kStages pairs ahead of the consume side, over the same pairs
+  uint64_t iu = 0;
+  bool imore = iw.take(c, iu);
+  uint32_t isrc = 0, in_flight = 0;
+  if (c.lane == 0) fence_proxy_async_global();  // data may have been written through the generic proxy
+#pragma unroll
+  for (int s = 0; s < kStages; ++s) {
+    if (!imore) break;
+    if (c.lane == 0) issue_load(c, P.src[isrc], bytes, iu, s);
+    ++in_flight;
+    if (++isrc == n) {
+      isrc = 0;
+      imore = iw.take(c, iu);
+    }
+  }
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  int s = 0;
+  uint32_t csrc = 0;
+  uint64_t u = 0;
+  bool more = walk.take(c, u);
+  while (more) {
+    if (!mbar_wait(c, s)) {
+      for (; in_flight > 0; --in_flight) {
+        mbar_drain(c, s);
+        s = (s + 1 == kStages) ? 0 : s + 1;
+      }
+      return;
+    }
+    --in_flight;
+    const uint32_t len = unit_len(bytes, u);
+    const uint32_t sbase = c.stage_smem + s * kUnitBytes;
+    if (len == kUnitBytes) {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    } else {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i)
+        if (ar_vec_off<16>(c.lane, i) < len) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    }
+    __syncwarp();
+    if (imore) {
+      if (c.lane == 0) {
+        fence_proxy_async_smem();
+        issue_load(c, P.src[isrc], bytes, iu, s);
+      }
+      ++in_flight;
+      if (++isrc == n) {
+        isrc = 0;
+        imore = iw.take(c, iu);
+      }
+    }
+    s = (s + 1 == kStages) ? 0 : s + 1;
+    if (++csrc == n) {
+      ar_store<16>(c, P.out, u, len, fw, acc, a);
+      csrc = 0;
+      more = walk.take(c, u);
+    }
+  }
+}
+
+// ld/st read side: for each unit, the n inputs one after another, kLdstVecs 16-byte loads in flight per lane each.
+template <uint32_t kLaneBytes>
+__device__ void ar_units_ldst(const Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw,
+                              Sum& a) {
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  for (uint64_t u; walk.take(c, u);) {
+    const uint32_t len = unit_len(bytes, u);
+    for (uint32_t t = 0; t < P.n; ++t) {
+      const uint8_t* base = P.src[t] + u * kUnitBytes;
+      uint4 v[kLdstVecs];
+      if (len == kUnitBytes) {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i)
+          v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + ar_vec_off<kLaneBytes>(c.lane, i)));
+      } else {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i) {
+          v[i] = make_uint4(0u, 0u, 0u, 0u);
+          const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+          if (off < len) v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + off));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < (int)kLdstVecs; ++i) ar_add(acc, i, v[i]);
+    }
+    ar_store<kLaneBytes>(c, P.out, u, len, fw, acc, a);
+  }
+}
+
+// The untimed word check of the output the last rep of size k stored: each lane compares every 32nd word of its
+// warp's share with allreduce_word, reading at L2 (other SMs stored them).  One atomic pair per warp with a bad word.
+__device__ void ar_check(const Ctx& c, const AllReduceParams& P, ArScratch* as, uint32_t k, uint64_t bytes,
+                         uint32_t gwarp, uint32_t nwarps) {
+  const unsigned long long* out = reinterpret_cast<const unsigned long long*>(P.out);
+  const uint64_t words = bytes / 8;
+  uint64_t bad = 0, first = ~0ull;
+  for (uint64_t w = (uint64_t)gwarp * 32u + (uint32_t)c.lane; w < words; w += (uint64_t)nwarps * 32u) {
+    if (__ldcg(out + w) != allreduce_word(P.seed, P.n, w)) {
+      ++bad;
+      first = min(first, w * 8u);
+    }
+  }
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
+}
+}  // namespace
+
+// One rank of cdprobe_allreduce: for every size of the ladder, one warm-up and P.reps timed reps, each summing the
+// first size bytes of all P.n inputs into P.out with every warp of the grid (the strided walk of a probe phase) and
+// folding the sum into the (S, X) checksum.  A domain barrier opens every rep, so a rep is timed as a probe phase is,
+// per rank: from this rank's release stamp to its latest CTA completion stamp (ranks see a release one signal latency
+// apart).  After the last rep of a size and a grid barrier, the word check.  Its state (barrier, stamps, checksums,
+// word-check counters, abort word) is in the rank's scratch buffer; outside it only its barrier lines are written.
+__global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_constant__ AllReduceParams P) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  ArScratch* as = P.scratch;
+  BwScratch* bs = &as->rep;
+  uint64_t* red;
+  Ctx c = enter(smem, &bs->abort_flag, P.timeout_ns, &red);
+
+  const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
+  const uint32_t nwarps = gridDim.x * kWarpsPerCta;
+  uint32_t b = 0;
+  for (uint32_t k = 0; k < P.n_sizes; ++k) {
+    const uint64_t bytes = P.size[k];
+    for (uint32_t r = 0; r <= P.reps; ++r) {
+      if (!grid_barrier(c, bs, b++, &bs->t_rel[k][r], &P.dom, false)) return;
+      const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
+      Sum a{0ull, 0ull, 0ull};
+      const Walk<false> walk = strided(bytes, gwarp, nwarps);
+      if (P.path == 2u) ar_units_ldst<32>(c, P, bytes, walk, fw, a);
+      else if (P.path == 1u) ar_units_ldst<16>(c, P, bytes, walk, fw, a);
+      else ar_units_tma(c, P, bytes, walk, fw, a);
+      __threadfence();  // this warp's stores are performed before the CTA's completion stamp
+      Acc* const acc = &bs->rep[k][r];
+      cta_reduce<1>(c, red, &a, &acc);
+      if (threadIdx.x == 0) atomicMax(&acc->t_end, (unsigned long long)gtimer());
+    }
+    if (!grid_barrier(c, bs, b++, nullptr, nullptr, false)) return;
+    ar_check(c, P, as, k, bytes, gwarp, nwarps);
+  }
+}
+
+int allreduce_launch(const AllReduceParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
+  const cudaError_t e =
+      cudaFuncSetAttribute(allreduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  return e != cudaSuccess ? (int)e : grid_launch(allreduce_kernel, p, grid, cooperative, stream);
+}
+
+template int granules_launch(uint64_t*, uint64_t*, const AllReduceWord&, uint64_t, unsigned, cudaStream_t);
+
+}  // namespace cdp

@@ -1,5 +1,5 @@
-// alltoall.h — host-callable launcher of the one-shot all-to-all kernel in probe_kernels.cu (cdprobe_alltoall), and the
-// layout of the scratch buffer it shares with the host.
+// alltoall.h — host-callable launcher of the one-shot all-to-all kernel in alltoall_kernels.cu (cdprobe_alltoall), and
+// the layout of the scratch buffer it shares with the host.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
-// bwcurve.h — host-callable launchers of the bandwidth-versus-size kernels in probe_kernels.cu (cdprobe_bwcurve), and
-// the layout of the scratch buffer they share with the host.
+// bwcurve.h — host-callable launchers of the bandwidth-versus-size kernels in bwcurve_kernels.cu (cdprobe_bwcurve),
+// and the layout of the scratch buffer they share with the host.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -7,7 +7,7 @@
 // polls its local copy for the ping and stores the echo (received + 1) into its line in the initiator's memory.
 // Between the legs, leg 0's initiator stores a hand-over word once it has read the last echo, and leg 1's initiator
 // waits for it before its first ping (untimed, outside the digest).
-// These are the barrier's own operations (probe_kernels.cu, signal_ranks / spin_until): every store is
+// These are the barrier's own operations (probe_kernels.cu, signal_ranks; datapath.cuh, spin_until): every store is
 // st.relaxed.sys (STG.E.64.STRONG.SYS), every poll ld.acquire.sys, and the fenced variant puts the barrier's
 // system-scope fence (__threadfence_system, as after publish_writes / publish_verdicts) before each store.
 //

@@ -504,7 +504,7 @@ static_assert(kA2aOff % 128 == 0 && kA2aOff + kMaxRanks * sizeof(FlagLine) <= kC
               "the all-to-all lines sit after the all-reduce lines inside the Ctrl granule");
 static_assert(kBwMaxSizes * (64 + 1) * 2 < (1u << kArBarrierBits), "all-to-all barriers per call fit the low bits");
 
-// The flag lines a domain barrier exchanges (probe_kernels.cu, grid_barrier): its leader stores (call_seq << 16) |
+// The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own
 // memory when this rank polls it.  All null: a grid barrier only.

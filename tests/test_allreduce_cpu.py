@@ -13,6 +13,7 @@ import pytest
 
 import allreduce_ref as ref
 from conftest import ROOT
+from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -191,20 +192,9 @@ def test_wrapper_passes_its_arguments(pkg):
 
 
 # ---- the compiled kernel ------------------------------------------------------------------------------------------
-def cuobjdump():
-    return shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-
-
 @pytest.fixture(scope="module")
 def kernel(pkg):
-    exe = cuobjdump()
-    if exe is None:
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([exe, "-sass", pkg.abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    for f in re.split(r"\n\s*Function : ", sass):
-        if f.split("\n", 1)[0].strip().startswith("_ZN3cdp16allreduce_kernel"):
-            return [t.strip() for t in re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", f)]
-    pytest.fail("allreduce_kernel not in the library")
+    return kernel_sass(pkg.abi.LIB_PATH, r"^_ZN3cdp16allreduce_kernel")[1]
 
 
 def stamp(text):
@@ -242,18 +232,11 @@ def test_the_closing_timer_read_follows_the_last_store(kernel):
     assert len(reds) == 2
 
 
-def test_ptxas_reports_no_spills_in_allreduce_and_its_granule_kernel(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not found")
-    proc = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                           "-c", os.path.join(CSRC, "probe_kernels.cu"), "-o", str(tmp_path / "p.o")],
-                          capture_output=True, text=True, check=True)
-    props = dict(re.findall(r"Function properties for (\S+)\n\s*\d+ bytes stack frame, (\d+ bytes spill stores, "
-                            r"\d+ bytes spill loads)", proc.stderr))
-    ar = [k for k in props if "allreduce" in k or "granules_kernelINS_13AllReduceWord" in k]
-    assert len(ar) == 2, proc.stderr
-    assert all(props[k] == "0 bytes spill stores, 0 bytes spill loads" for k in ar), props
+def test_ptxas_reports_no_spills_in_the_allreduce_unit():
+    props = ptxas_report("allreduce_kernels.cu")
+    ar = [k for k in props if "allreduce_kernelE" in k or "granules_kernelINS_13AllReduceWord" in k]
+    assert len(ar) == 2, props
+    assert all(props[k][1:] == (0, 0) for k in ar), props
 
 
 # ---- Go mirror ----------------------------------------------------------------------------------------------------

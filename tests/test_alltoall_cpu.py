@@ -13,9 +13,9 @@ import pytest
 import alltoall_ref as ref
 import word_ref
 from conftest import ROOT
+from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 U64_MAX = (1 << 64) - 1
 
 
@@ -183,14 +183,7 @@ def test_wrapper_passes_its_arguments(pkg):
 # ---- the compiled kernel ------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def kernel(pkg):
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe):
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([exe, "-sass", pkg.abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    for f in re.split(r"\n\s*Function : ", sass):
-        if f.split("\n", 1)[0].strip().startswith("_ZN3cdp15alltoall_kernel"):
-            return [t.strip() for t in re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", f)]
-    pytest.fail("alltoall_kernel not in the library")
+    return kernel_sass(pkg.abi.LIB_PATH, r"^_ZN3cdp15alltoall_kernel")[1]
 
 
 def test_every_write_path_is_compiled_in(kernel):
@@ -202,18 +195,11 @@ def test_every_write_path_is_compiled_in(kernel):
     assert any(t.startswith("LDG.E.NA.128") for t in kernel)  # the word check
 
 
-def test_ptxas_reports_no_spills_in_alltoall(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not found")
-    proc = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                           "-c", os.path.join(CSRC, "probe_kernels.cu"), "-o", str(tmp_path / "p.o")],
-                          capture_output=True, text=True, check=True)
-    props = dict(re.findall(r"Function properties for (\S+)\n\s*\d+ bytes stack frame, (\d+ bytes spill stores, "
-                            r"\d+ bytes spill loads)", proc.stderr))
-    a2a = [k for k in props if "alltoall_kernel" in k]
-    assert len(a2a) == 1, proc.stderr
-    assert props[a2a[0]] == "0 bytes spill stores, 0 bytes spill loads", props
+def test_ptxas_reports_no_spills_in_the_alltoall_unit():
+    props = ptxas_report("alltoall_kernels.cu")
+    a2a = [k for k in props if "alltoall_kernelE" in k]
+    assert len(a2a) == 1, props
+    assert props[a2a[0]][1:] == (0, 0), props
 
 
 # ---- Go mirror ----------------------------------------------------------------------------------------------------

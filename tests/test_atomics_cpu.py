@@ -4,13 +4,13 @@ their register use, and the Go mirror."""
 import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 
 import pytest
 
 import atomics_ref as ref
 from conftest import ROOT
+from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -156,26 +156,10 @@ def test_wrapper_passes_its_arguments(pkg):
 
 
 # ---- the compiled kernels -----------------------------------------------------------------------------------------
-def cuobjdump():
-    return shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-
-
 @pytest.fixture(scope="module")
 def kernels(pkg):
-    exe = cuobjdump()
-    if exe is None:
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([exe, "-sass", pkg.abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    out = {}
-    for f in re.split(r"\n\s*Function : ", sass):
-        name = f.split("\n", 1)[0]
-        m = re.search(r"atomics_(chain_kernelILb([01])E|contended_kernel)", name)
-        if m:
-            kind = 2 if m.group(2) is None else int(m.group(2))
-            ins = re.findall(r"/\*([0-9a-f]{4,})\*/\s+([^;]*);", f)
-            out[kind] = ([int(a, 16) for a, _ in ins], [t.strip() for _, t in ins])
-    assert set(out) == {0, 1, 2}
-    return out
+    names = {0: r"atomics_chain_kernelILb0E", 1: r"atomics_chain_kernelILb1E", 2: r"atomics_contended_kernel"}
+    return {kind: kernel_sass(pkg.abi.LIB_PATH, name) for kind, name in names.items()}
 
 
 def regs(t):
@@ -284,16 +268,10 @@ def test_the_timer_reads_bracket_the_atomics(kernels, kind):
     assert readback > closing
 
 
-def test_ptxas_reports_no_spills(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not found")
-    proc = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                           "-c", os.path.join(CSRC, "atomics_kernels.cu"), "-o", str(tmp_path / "a.o")],
-                          capture_output=True, text=True, check=True)
-    props = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", proc.stderr)
-    assert len(props) == 3, proc.stderr
-    assert all(p == ("0", "0", "0") for p in props), props
+def test_ptxas_reports_no_spills():
+    props = ptxas_report("atomics_kernels.cu")
+    assert len(props) == 3, props
+    assert all(p == (0, 0, 0) for p in props.values()), props
 
 
 # ---- Go mirror ----------------------------------------------------------------------------------------------------

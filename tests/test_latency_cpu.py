@@ -4,13 +4,13 @@ import ctypes as C
 import os
 import random
 import re
-import shutil
 import subprocess
 
 import pytest
 
 import latency_ref as ref
 from conftest import ROOT
+from kernel_tools import kernel_sass
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -121,23 +121,10 @@ def test_latency_rejects_a_null_handle_and_fills_out(pkg):
 
 
 # ---- the compiled kernel ------------------------------------------------------------------------------------------
-def cuobjdump():
-    return shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-
-
 def test_chase_loads_are_strong_sys_and_the_closing_timer_follows_their_use(pkg):
     """Every load of the chase is LDG.E.64.STRONG.SYS (ld.relaxed.sys: no L1); a timer read precedes the first load,
     the loaded register is used before the loop branches, and the closing timer read comes after the hop loop."""
-    exe = cuobjdump()
-    if exe is None:
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([exe, "-sass", pkg.abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    funcs = re.split(r"\n\s*Function : ", sass)
-    body = [f for f in funcs if "latency_kernel" in f.split("\n", 1)[0]]
-    assert len(body) == 1
-    ins = re.findall(r"/\*([0-9a-f]{4,})\*/\s+([^;]*);", body[0])
-    addr = [int(a, 16) for a, _ in ins]
-    text = [t.strip() for _, t in ins]
+    addr, text = kernel_sass(pkg.abi.LIB_PATH, "latency_kernel")
     loads = [k for k, t in enumerate(text) if "LDG" in t or re.search(r"\bLD\b", t)]
     assert len(loads) == 1 and text[loads[0]].startswith("LDG.E.64.STRONG.SYS"), [text[k] for k in loads]
     ld = loads[0]

@@ -5,13 +5,13 @@ import ctypes as C
 import os
 import random
 import re
-import shutil
 import subprocess
 
 import pytest
 
 import pingpong_ref as ref
 from conftest import ROOT
+from kernel_tools import kernel_sass
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -175,26 +175,9 @@ def test_wrapper_passes_its_arguments(pkg):
 
 
 # ---- the compiled kernels -----------------------------------------------------------------------------------------
-def cuobjdump():
-    return shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-
-
 @pytest.fixture(scope="module")
 def kernels(pkg):
-    exe = cuobjdump()
-    if exe is None:
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([exe, "-sass", pkg.abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    funcs = re.split(r"\n\s*Function : ", sass)
-    out = {}
-    for f in funcs:
-        name = f.split("\n", 1)[0]
-        m = re.search(r"pingpong_kernelILb([01])E", name)
-        if m:
-            ins = re.findall(r"/\*([0-9a-f]{4,})\*/\s+([^;]*);", f)
-            out[m.group(1) == "1"] = ([int(a, 16) for a, _ in ins], [t.strip() for _, t in ins])
-    assert set(out) == {False, True}
-    return out
+    return {fenced: kernel_sass(pkg.abi.LIB_PATH, rf"pingpong_kernelILb{int(fenced)}E") for fenced in (False, True)}
 
 
 @pytest.mark.parametrize("fenced", [False, True], ids=["plain", "fenced"])
