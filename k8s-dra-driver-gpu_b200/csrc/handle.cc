@@ -315,7 +315,7 @@ static void fill_params(const cdprobe* h, uint32_t li, const Phase* phases, uint
   P->row = L.row;
   P->run_seq = h->launch_seq;
   P->seq_base = h->launch_seq * (uint64_t)(kMaxPhases + 2);
-  P->timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+  P->timeout_ns = timeout_ns(h);
   P->bpp = h->plan.bpp;
   P->src_off = h->plan.src_off;
   P->land_off = h->plan.land_off;
@@ -408,8 +408,7 @@ static int write_fault(cdprobe* h, uint32_t li, const LandingFault& f) {
 static int launch_one(cdprobe* h, uint32_t li, const ProbeParams& P) {
   LocalRank& L = h->lr[li];
   CDP_RT(cudaSetDevice(L.ordinal));
-  const bool coop = L.coop && !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
-  cudaError_t e = (cudaError_t)probe_kernel_launch(&P, L.ctas, coop, L.stream);
+  cudaError_t e = (cudaError_t)probe_kernel_launch(&P, L.ctas, launch_cooperatively(h, L), L.stream);
   if (e != cudaSuccess) return fail_cuda("launch cdprobe_kernel", e);
   return CDPROBE_OK;
 }

@@ -139,6 +139,15 @@ inline int require_usable(const cdprobe* h) {
   return CDPROBE_ERR_STATE;
 }
 
+// The device deadline every kernel gets, counted from its entry: timeout_ms.
+inline uint64_t timeout_ns(const cdprobe* h) { return (uint64_t)h->cfg.timeout_ms * 1000000ull; }
+
+// Whether local rank L's grid kernels (the probe and the ladder measurements) launch cooperatively: when its device
+// can and CDPROBE_FLAG_NO_COOPERATIVE is clear.
+inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
+  return L.coop && !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
+}
+
 // cdprobe_alltoall's exchange area (handle.cc): on the first call, every local rank creates n_total x bytes_per_pair of
 // device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every local rank
 // wherever the probe mapping is then up; area_status gets every rank's mapping statuses.  Collective.  If creating it

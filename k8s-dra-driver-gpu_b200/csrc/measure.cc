@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <array>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -51,10 +52,12 @@ static int fail_sticky(cdprobe* h, const char* what, cudaError_t e) {
   return fail_cuda(what, e);
 }
 
-// Copies the first `bytes` of local rank L's scratch (its rep tables) to `got` once its kernel is done.
-static int fetch_reps(cdprobe* h, LocalRank& L, size_t bytes, void* got, const char* what) {
+// Copies count T's from the head of local rank L's scratch (its rep tables, or the records a ladder kernel left) to
+// `got` once its kernel is done.
+template <typename T>
+static int fetch_reps(cdprobe* h, LocalRank& L, T* got, size_t count, const char* what) {
   cudaError_t e = cudaSetDevice(L.ordinal);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(got, L.scratch, bytes, cudaMemcpyDeviceToHost, L.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(got, L.scratch, sizeof(T) * count, cudaMemcpyDeviceToHost, L.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
   return e != cudaSuccess ? fail_sticky(h, what, e) : CDPROBE_OK;
 }
@@ -72,26 +75,27 @@ static bool begin_output(Out* out) {
 
 // What each process contributes at the start of a collective measurement (cdprobe_pingpong, cdprobe_bwcurve,
 // cdprobe_allreduce, cdprobe_alltoall), so that every process refuses, skips or runs the same call: the call number it
-// is about to make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and what
-// the call folds in from every process.
-template <typename Extra>
+// is about to make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and its
+// local ranks' rows of mapping status, [local rank][rank] with unmapped cells folded in (cdprobe_unmap_peer changes
+// only the local view).
 struct Agreement {
   uint64_t call_seq;
   std::array<uint32_t, 3> args;
   uint32_t ok;
-  Extra extra;
+  int32_t rows[kMaxRanks][kMaxRanks];
 };
-struct NoExtra {};
 
-// The handshake of collective measurement `fn`: every process contributes `mine` (ok: its own verdict `bad` on its
-// arguments is empty) and gets all[r], process r's contribution, back (in a single process, all = {mine}).  The first
-// error wins: this process's own arguments, then another process's, then a call number or arguments that differ.
-// Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and CDPROBE_ERR_ARG on a refusal, with the message set.
-template <typename Extra>
-static int agree(cdprobe* h, const char* fn, std::string bad, Agreement<Extra>& mine,
-                 std::vector<Agreement<Extra>>& all) {
-  mine.ok = bad.empty() ? 1u : 0u;
-  all.assign(h->cfg.world_size, mine);
+// The handshake of collective measurement `fn`: every process contributes its Agreement (ok: its own verdict `bad` on
+// its arguments is empty).  The first error wins: this process's own arguments, then another process's, then a call
+// number or arguments that differ.  Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and CDPROBE_ERR_ARG on a
+// refusal, with the message set.  Otherwise st, when given, gets the domain's matrix of mapping status, [rank][rank],
+// which every process derives alike.
+static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq, const std::array<uint32_t, 3>& args,
+                 int32_t (*st)[kMaxRanks]) {
+  Agreement mine = {call_seq, args, bad.empty() ? 1u : 0u, {}};
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < h->n_total; ++j) mine.rows[li][j] = cell_status(h, li, j);
+  std::vector<Agreement> all(h->cfg.world_size, mine);
   if (h->cfg.world_size > 1) {
     std::string err;
     if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
@@ -99,7 +103,7 @@ static int agree(cdprobe* h, const char* fn, std::string bad, Agreement<Extra>& 
       return CDPROBE_ERR_RENDEZVOUS;
     }
   }
-  for (const Agreement<Extra>& o : all) {
+  for (const Agreement& o : all) {
     if (!o.ok && bad.empty()) bad = std::string("another process called ") + fn + " with invalid arguments";
     if ((o.call_seq != mine.call_seq || o.args != mine.args) && bad.empty())
       bad = std::string(fn) + " is collective: every process must call it with the same arguments";
@@ -108,7 +112,23 @@ static int agree(cdprobe* h, const char* fn, std::string bad, Agreement<Extra>& 
     set_err(bad);
     return CDPROBE_ERR_ARG;
   }
+  if (st != nullptr) {
+    memset(st, 0, sizeof(int32_t) * kMaxRanks * kMaxRanks);
+    for (uint32_t r = 0; r < all.size(); ++r)
+      for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].rows[li], sizeof(st[0]));
+  }
   return CDPROBE_OK;
+}
+
+// The cell rule of the one-sided measurements (latency, atomics, bwcurve): whether local rank li's cell to rank j runs.
+// Cell (g, g) exists only with a loop-back slice; a cell whose mapping is down gets that status in status[] and is
+// never read or written through.
+static bool live_cell(const cdprobe* h, uint32_t li, uint32_t j, int32_t* status) {
+  const uint32_t g = h->lr[li].grank;
+  if (j == g && !h->plan.diag) return false;
+  const int32_t s = cell_status(h, li, j);
+  if (s != 0) status[g * CDPROBE_MAX_GPUS + j] = s;
+  return s == 0;
 }
 
 // Waits until every process of the domain has got here; nothing to wait for in a single process.
@@ -174,6 +194,35 @@ static void summarize(const TimedRep* rep, uint32_t reps, uint32_t per_rep, uint
   out->status[idx] = s;
 }
 
+// The cells one local rank's rep-table kernel measures: slot[k] of its table fills output cell idx[k], whose reps must
+// have the digest want[k].  n == 0: no kernel was launched.
+struct RepCells {
+  uint32_t n = 0;
+  uint32_t slot[kMaxRanks], idx[kMaxRanks];
+  uint64_t want[kMaxRanks] = {};
+  void add(uint32_t s, uint32_t i) {
+    slot[n] = s;
+    idx[n++] = i;
+  }
+};
+
+// Collects the rep table of every local rank that launched, once its kernel is done, and summarizes each of its cells:
+// ns per hop, round trip or atomic (`per_rep` of them per rep) of the timed reps, and the digest of all of them.
+template <typename Out>
+static int collect_reps(cdprobe* h, const RepCells* cells, uint32_t reps, uint32_t per_rep, const char* what, Out* out) {
+  std::vector<TimedRep> got((size_t)kMaxRanks * kRepSlots);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const RepCells& c = cells[li];
+    if (c.n == 0) continue;
+    if (const int rc = fetch_reps(h, h->lr[li], got.data(), (size_t)(c.slot[c.n - 1] + 1) * kRepSlots, what);
+        rc != CDPROBE_OK)
+      return rc;
+    for (uint32_t k = 0; k < c.n; ++k)
+      summarize(got.data() + (size_t)c.slot[k] * kRepSlots, reps, per_rep, c.want[k], c.idx[k], out);
+  }
+  return CDPROBE_OK;
+}
+
 // Fills the times of entry idx of a cdprobe_bwcurve_t (a cell), a cdprobe_allreduce_t (a row) or a cdprobe_alltoall_t
 // (a row) from the rep records bwcurve_kernel, allreduce_kernel or alltoall_kernel left in `s`: per size, ns of the
 // timed reps, and the model-free summary of the medians, whose rates are scale x size[k] / ns_median[k].  An entry
@@ -226,6 +275,40 @@ static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const ui
   }
   out->bad_sizes[idx] = bad;
   out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
+}
+
+// The size ladder of the ladder measurements (bwcurve, allreduce, alltoall), and their verdict on their arguments:
+// empty when they are valid.
+static std::string ladder(const cdprobe* h, uint32_t reps, uint64_t* size, uint32_t* n_sizes) {
+  *n_sizes = bwcurve_ladder(h->plan.bpp, size);
+  if (reps > kMaxTimedReps) return "reps must be at most 64";
+  if (*n_sizes == 0) return "bytes_per_pair must be at most 32 GiB";
+  return {};
+}
+
+// What a ladder measurement reports once every process has agreed to run it: the ladder and this process's rows.
+template <typename Out>
+static void put_ladder(const cdprobe* h, const uint64_t* size, uint32_t n_sizes, Out* out) {
+  out->n_sizes = n_sizes;
+  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
+  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+}
+
+// Launches a ladder kernel on local rank L: the parameters every ladder kernel takes, then its records at the head of
+// L's scratch cleared and the launch on L's stream.  A failed launch makes the handle sticky.
+template <typename Params>
+static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const uint64_t* size, uint32_t n_sizes, uint32_t reps,
+                         int (*launch)(const Params&, unsigned, bool, cudaStream_t), const char* what) {
+  p.scratch = static_cast<decltype(p.scratch)>(L.scratch);
+  memcpy(p.size, size, sizeof(p.size));
+  p.timeout_ns = timeout_ns(h);
+  p.n_sizes = n_sizes;
+  p.reps = reps;
+  p.path = h->path;
+  CDP_RT(cudaSetDevice(L.ordinal));
+  cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(*p.scratch), L.stream);
+  if (e == cudaSuccess) e = (cudaError_t)launch(p, L.ctas, launch_cooperatively(h, L), L.stream);
+  return e != cudaSuccess ? fail_sticky(h, what, e) : CDPROBE_OK;
 }
 
 }  // namespace cdp
@@ -338,6 +421,7 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
 
   // 1. every local issuer's chases, all launched before any is waited for
   cdp::LatencyParams P[cdp::kMaxRanks];
+  cdp::RepCells cells[cdp::kMaxRanks];
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
@@ -345,16 +429,12 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
     cdp::LatencyParams& p = P[li];
     memset(&p, 0, sizeof(p));
     p.seed = h->seed;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.timeout_ns = cdp::timeout_ns(h);
     p.hops = hops;
     p.reps = reps;
     for (uint32_t j = 0; j < h->n_total; ++j) {
-      if (j == g && !pl.diag) continue;  // no loop-back slice to chase
-      const int32_t s = cdp::cell_status(h, li, j);
-      if (s != 0) {  // never read through a mapping that is down
-        out->status[g * CDPROBE_MAX_GPUS + j] = s;
-        continue;
-      }
+      if (!cdp::live_cell(h, li, j, out->status)) continue;
+      cells[li].add(p.n_cells, g * CDPROBE_MAX_GPUS + j);
       cdp::LatencyCell& c = p.cell[p.n_cells++];
       c.region = reinterpret_cast<const uint8_t*>(L.va[j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
       c.lines = lines;
@@ -368,27 +448,17 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
   }
 
   // 2. while they run: the digest each chase gives over an intact region
-  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     for (uint32_t k = 0; k < P[li].n_cells; ++k) {
       const cdp::LatencyCell& c = P[li].cell[k];
       const uint64_t first = (uint64_t)cdp::cell_slice(pl, c.issuer, c.target) * (pl.bpp / 8);
       for (uint32_t r = 0; r <= reps; ++r)
-        want[li][k] ^= cdp::latency_rep_digest(h->seed, c.issuer, c.target, first, lines, r, hops);
+        cells[li].want[k] ^= cdp::latency_rep_digest(h->seed, c.issuer, c.target, first, lines, r, hops);
     }
   }
 
   // 3. collect: ns per hop of the timed reps, the digest of all of them
-  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    const cdp::LatencyParams& p = P[li];
-    if (p.n_cells == 0) continue;
-    const size_t bytes = sizeof(cdp::TimedRep) * p.n_cells * cdp::kRepSlots;
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_latency"); rc != CDPROBE_OK) return rc;
-    for (uint32_t k = 0; k < p.n_cells; ++k)
-      cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, hops, want[li][k],
-                     p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
-  }
+  if (const int rc = cdp::collect_reps(h, cells, reps, hops, "cdprobe_latency", out); rc != CDPROBE_OK) return rc;
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
@@ -424,19 +494,12 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
       f_trip = (uint32_t)trip;
     }
   }
-  // every process runs over the same pair set: each contributes its local ranks' rows of mapping status, [local
-  // rank][rank] with unmapped cells folded in (cdprobe_unmap_peer changes only the local view)
-  using Rows = int32_t[cdp::kMaxRanks][cdp::kMaxRanks];
-  cdp::Agreement<Rows> mine = {h->pp_calls + 1, {trips, reps, fenced}, 0u, {}};
-  for (uint32_t li = 0; li < h->n_local; ++li)
-    for (uint32_t j = 0; j < n; ++j) mine.extra[li][j] = cdp::cell_status(h, li, j);
-  std::vector<cdp::Agreement<Rows>> all;
-  if (const int rc = cdp::agree(h, "cdprobe_pingpong", bad, mine, all); rc != CDPROBE_OK) return rc;
-  Rows st = {};  // [rank][rank]
-  for (uint32_t r = 0; r < all.size(); ++r)
-    for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].extra[li], sizeof(st[0]));
-  h->pp_calls = mine.call_seq;
-  out->call_seq = h->pp_calls;
+  // every process runs over the same pair set: the domain's mapping status, from every process's rows
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_pingpong", bad, h->pp_calls + 1, {trips, reps, fenced}, st);
+      rc != CDPROBE_OK)
+    return rc;
+  out->call_seq = ++h->pp_calls;
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
   if (n == 1) {
     out->ms = cdp::now_ms() - t_begin;
@@ -450,14 +513,14 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
 
   // 2. one block per local rank, every one launched before any is waited for
   cdp::PingPongParams P[cdp::kMaxRanks];
-  bool launched[cdp::kMaxRanks] = {};
+  cdp::RepCells cells[cdp::kMaxRanks];
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
     cdp::PingPongParams& p = P[li];
     memset(&p, 0, sizeof(p));
     p.call_seq = h->pp_calls;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.timeout_ns = cdp::timeout_ns(h);
     p.n_rounds = pl.rounds;
     p.trips = trips;
     p.reps = reps;
@@ -465,7 +528,6 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
     p.fault_trip = f_trip;
     for (uint32_t j = 0; j < n; ++j)
       if (j != g) out->status[g * CDPROBE_MAX_GPUS + j] = pair_status(g, j);
-    uint32_t active = 0;
     for (uint32_t r = 0; r < pl.rounds; ++r) {
       const int q = pl.partner[r][g];
       if (q < 0 || pair_status(g, (uint32_t)q) != 0) continue;
@@ -475,41 +537,27 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
       R.partner = (uint32_t)q;
       R.first = g < (uint32_t)q ? 1u : 0u;
       if (g == f_target && (uint32_t)q == f_init) p.fault_round = r;
-      ++active;
+      cells[li].add(r, g * CDPROBE_MAX_GPUS + (uint32_t)q);
     }
-    if (active == 0) continue;
+    if (cells[li].n == 0) continue;
     CDP_RT(cudaSetDevice(L.ordinal));
     const cudaError_t e =
         (cudaError_t)cdp::pingpong_launch(p, fenced != 0, static_cast<cdp::TimedRep*>(L.scratch), L.stream);
     if (e != cudaSuccess) return cdp::fail_sticky(h, "launch pingpong_kernel", e);
-    launched[li] = true;
   }
 
   // 3. while they run: the digest of a clean leg for every cell a local rank initiates
-  uint64_t want[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // [local rank][round]
   for (uint32_t li = 0; li < h->n_local; ++li) {
-    for (uint32_t r = 0; r < pl.rounds; ++r) {
-      const cdp::PingPongRound& R = P[li].round[r];
-      if (R.remote == nullptr) continue;
-      const uint32_t leg = R.first ? 0u : 1u;
-      for (uint32_t rep = 0; rep <= reps; ++rep) want[li][r] ^= cdp::pingpong_rep_digest(h->pp_calls, r, leg, rep, trips);
+    cdp::RepCells& c = cells[li];
+    for (uint32_t k = 0; k < c.n; ++k) {
+      const uint32_t leg = P[li].round[c.slot[k]].first ? 0u : 1u;
+      for (uint32_t rep = 0; rep <= reps; ++rep)
+        c.want[k] ^= cdp::pingpong_rep_digest(h->pp_calls, c.slot[k], leg, rep, trips);
     }
   }
 
   // 4. collect: ns per round trip of the timed reps, the digest of all of them
-  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    if (!launched[li]) continue;
-    const cdp::PingPongParams& p = P[li];
-    const size_t bytes = sizeof(cdp::TimedRep) * p.n_rounds * cdp::kRepSlots;
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_pingpong"); rc != CDPROBE_OK) return rc;
-    for (uint32_t r = 0; r < p.n_rounds; ++r) {
-      const cdp::PingPongRound& R = p.round[r];
-      if (R.remote == nullptr) continue;
-      cdp::summarize(got.data() + (size_t)r * cdp::kRepSlots, reps, trips, want[li][r],
-                     h->lr[li].grank * CDPROBE_MAX_GPUS + R.partner, out);
-    }
-  }
+  if (const int rc = cdp::collect_reps(h, cells, reps, trips, "cdprobe_pingpong", out); rc != CDPROBE_OK) return rc;
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
@@ -548,6 +596,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
 
   // 1. every local issuer's cells, all launched before any is waited for; no kernel waits on another rank
   cdp::AtomicsParams P[cdp::kMaxRanks];
+  cdp::RepCells cells[cdp::kMaxRanks];
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
@@ -555,7 +604,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
     cdp::AtomicsParams& p = P[li];
     memset(&p, 0, sizeof(p));
     p.call_seq = h->at_calls;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
+    p.timeout_ns = cdp::timeout_ns(h);
     p.ops = ops;
     p.reps = reps;
     p.fault_cell = cdp::kAtomicsNoFault;
@@ -571,17 +620,13 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
         native = native != 0 ? 1 : 0;
       }
       out->native[idx] = (uint8_t)native;
-      if (j == g && !pl.diag) continue;  // no loop-back slot
-      const int32_t s = cdp::cell_status(h, li, j);
-      if (s != 0) {  // never touch a mapping that is down
-        out->status[idx] = s;
-        continue;
-      }
+      if (!cdp::live_cell(h, li, j, out->status)) continue;
       if (native == 0) {
         out->status[idx] = CDPROBE_ERR_UNSUPPORTED;
         continue;
       }
       if (g == f_issuer && j == f_target) p.fault_cell = p.n_cells;
+      cells[li].add(p.n_cells, idx);
       cdp::AtomicsCell& c = p.cell[p.n_cells++];
       c.word = reinterpret_cast<unsigned long long*>(L.va[j] + cdp::kAtomOff + (uint64_t)g * sizeof(cdp::AtomLine));
       c.issuer = g;
@@ -596,18 +641,11 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
   // 2. while they run: the digest of clean reps, the same for every cell
   uint64_t want = 0;
   for (uint32_t r = 0; r <= reps; ++r) want ^= cdp::atomics_rep_digest(cdp::atomics_start(h->at_calls, kind, r), total);
+  for (cdp::RepCells& c : cells) std::fill(c.want, c.want + c.n, want);
 
   // 3. collect: ns per atomic of the timed reps, the digest of all of them
-  std::vector<cdp::TimedRep> got((size_t)cdp::kMaxRanks * cdp::kRepSlots);
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    const cdp::AtomicsParams& p = P[li];
-    if (p.n_cells == 0) continue;
-    const size_t bytes = sizeof(cdp::TimedRep) * p.n_cells * cdp::kRepSlots;
-    if (const int rc = cdp::fetch_reps(h, h->lr[li], bytes, got.data(), "cdprobe_atomics"); rc != CDPROBE_OK) return rc;
-    for (uint32_t k = 0; k < p.n_cells; ++k)
-      cdp::summarize(got.data() + (size_t)k * cdp::kRepSlots, reps, (uint32_t)total, want,
-                     p.cell[k].issuer * CDPROBE_MAX_GPUS + p.cell[k].target, out);
-  }
+  if (const int rc = cdp::collect_reps(h, cells, reps, (uint32_t)total, "cdprobe_atomics", out); rc != CDPROBE_OK)
+    return rc;
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
@@ -623,21 +661,15 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   out->path = h->path;
   reps = out->reps;
   if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
-  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together
-  std::string bad;
+  // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together.  Every
+  //    cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree
   uint64_t size[cdp::kBwMaxSizes];
-  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
-  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
-  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
-  // every cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree
-  cdp::Agreement<cdp::NoExtra> mine = {h->bw_calls + 1, {reps, 0u, 0u}, 0u, {}};
-  std::vector<cdp::Agreement<cdp::NoExtra>> all;
-  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", bad, mine, all); rc != CDPROBE_OK) return rc;
-  h->bw_calls = mine.call_seq;
-  out->call_seq = h->bw_calls;
-  out->n_sizes = n_sizes;
-  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
-  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+  uint32_t n_sizes;
+  const std::string bad = cdp::ladder(h, reps, size, &n_sizes);
+  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", bad, h->bw_calls + 1, {reps, 0u, 0u}, nullptr); rc != CDPROBE_OK)
+    return rc;
+  out->call_seq = ++h->bw_calls;
+  cdp::put_ladder(h, size, n_sizes, out);
 
   // 2. scratch for the rep records and one cell's granule table, grown on every local rank before any kernel runs
   const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
@@ -655,12 +687,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
     for (uint32_t j = 0; j < n; ++j) {
-      if (j == g && !pl.diag) continue;  // no loop-back slice
-      const int32_t s = cdp::cell_status(h, li, j);
-      if (s != 0) {  // never read through a mapping that is down
-        out->status[g * CDPROBE_MAX_GPUS + j] = s;
-        continue;
-      }
+      if (!cdp::live_cell(h, li, j, out->status)) continue;
       runs[li][j] = true;
       const cdp::SrcRegionWord word{h->seed, (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8), j};
       if (const int rc = cdp::expected_sums(h, L, table_off, word, size, n_sizes, want_of(li, j),
@@ -672,8 +699,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
 
   // 4. the rounds: the tournament's, then the loop-back; every local kernel of a round is launched before any is
   //    waited for, and no process starts a round before every process has finished the one before
-  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
-  std::vector<cdp::BwScratch> got(1);
+  auto got = std::make_unique<cdp::BwScratch>();
   const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
   for (uint32_t r = 0; r < n_rounds; ++r) {
     if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
@@ -686,37 +712,21 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       cdp::BwCurveParams p;
       memset(&p, 0, sizeof(p));
       p.region = reinterpret_cast<const uint8_t*>(L.va[q]) + cdp::cell_offset(pl, CDPROBE_OP_READ, L.grank, (uint32_t)q);
-      p.scratch = static_cast<cdp::BwScratch*>(L.scratch);
-      memcpy(p.size, size, sizeof(size));
-      p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
-      p.n_sizes = n_sizes;
-      p.reps = reps;
-      p.path = h->path;
-      CDP_RT(cudaSetDevice(L.ordinal));
-      cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::BwScratch), L.stream);
-      if (e == cudaSuccess) e = (cudaError_t)cdp::bwcurve_launch(p, L.ctas, L.coop && coop_ok, L.stream);
-      if (e != cudaSuccess) return cdp::fail_sticky(h, "launch bwcurve_kernel", e);
+      if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::bwcurve_launch, "launch bwcurve_kernel");
+          rc != CDPROBE_OK)
+        return rc;
     }
     for (uint32_t li = 0; li < h->n_local; ++li) {
       if (target[li] < 0) continue;
       cdp::LocalRank& L = h->lr[li];
-      if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::BwScratch), got.data(), "cdprobe_bwcurve"); rc != CDPROBE_OK)
-        return rc;
-      cdp::bw_summarize(got[0], want_of(li, (uint32_t)target[li]), size, n_sizes, reps,
+      if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_bwcurve"); rc != CDPROBE_OK) return rc;
+      cdp::bw_summarize(*got, want_of(li, (uint32_t)target[li]), size, n_sizes, reps,
                         L.grank * CDPROBE_MAX_GPUS + (uint32_t)target[li], out);
     }
   }
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
-
-// What each process adds to the cdprobe_allreduce handshake: the mapping verdict must agree too, since a process that
-// ran while another skipped would wait at the first domain barrier until its watchdog fired.
-struct DownCell {
-  uint32_t cell;   // issuer * kMaxRanks + target of this process's first cell whose mapping is down (kNoCell: none)
-  int32_t status;  // that cell's mapping status
-};
-static constexpr uint32_t kNoCell = ~0u;
 
 int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
@@ -731,11 +741,9 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   // 1. the arguments, the armed fault and the mapping verdict; in a multi-process domain all three are shared below,
   //    so every process refuses, skips or runs together
-  std::string bad;
   uint64_t size[cdp::kBwMaxSizes];
-  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
-  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
-  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
+  uint32_t n_sizes;
+  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
   uint32_t f_rank = cdp::kArNoFault, f_k = cdp::kArNoFault;
   uint64_t f_word = 0;
   if (h->ar_fault != 0 && bad.empty()) {
@@ -748,26 +756,17 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
       f_k = (uint32_t)fk - 1;
     }
   }
-  cdp::Agreement<DownCell> mine = {h->ar_calls + 1, {reps, 0u, 0u}, 0u, {kNoCell, 0}};
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    for (uint32_t j = 0; j < n; ++j) {
-      const int32_t s = cdp::cell_status(h, li, j);
-      const uint32_t cell = h->lr[li].grank * cdp::kMaxRanks + j;
-      if (s != 0 && cell < mine.extra.cell) mine.extra = {cell, s};
-    }
-  }
-  std::vector<cdp::Agreement<DownCell>> all;
-  if (const int rc = cdp::agree(h, "cdprobe_allreduce", bad, mine, all); rc != CDPROBE_OK) return rc;
-  DownCell down = mine.extra;
-  for (const cdp::Agreement<DownCell>& o : all)
-    if (o.extra.cell < down.cell) down = o.extra;
-  h->ar_calls = mine.call_seq;
-  out->call_seq = h->ar_calls;
-  out->n_sizes = n_sizes;
-  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
-  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
-  if (down.cell != kNoCell) {  // some rank cannot read some input: nothing runs, in any process
-    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = down.status;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_allreduce", bad, h->ar_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
+    return rc;
+  out->call_seq = ++h->ar_calls;
+  cdp::put_ladder(h, size, n_sizes, out);
+  // a process that ran while another skipped would wait at the first domain barrier until its watchdog fired, so
+  // when some rank cannot read some input nothing runs, in any process: every row gets the domain's first down cell
+  const int32_t* down = std::find_if(&st[0][0], &st[0][0] + cdp::kMaxRanks * cdp::kMaxRanks,
+                                     [](int32_t s) { return s != 0; });
+  if (down != &st[0][0] + cdp::kMaxRanks * cdp::kMaxRanks) {
+    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = *down;
     out->ms = cdp::now_ms() - t_begin;
     return CDPROBE_OK;
   }
@@ -788,7 +787,6 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   // 4. no process launches before every process is ready, so that no kernel waits at the first domain barrier for a
   //    process still setting up; then every local kernel is launched before any is waited for
   if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
@@ -801,32 +799,24 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
       p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kArOff + (uint64_t)j * sizeof(cdp::FlagLine));
     }
     p.dom.call_seq = h->ar_calls;
-    p.scratch = static_cast<cdp::ArScratch*>(L.scratch);
     p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
-    memcpy(p.size, size, sizeof(size));
     p.seed = h->seed;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
     p.fault_k = g == f_rank ? f_k : cdp::kArNoFault;
     p.fault_word = f_word;
     p.rank = g;
     p.n = n;
-    p.n_sizes = n_sizes;
-    p.reps = reps;
-    p.path = h->path;
-    CDP_RT(cudaSetDevice(L.ordinal));
-    cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::ArScratch), L.stream);
-    if (e == cudaSuccess) e = (cudaError_t)cdp::allreduce_launch(p, L.ctas, L.coop && coop_ok, L.stream);
-    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch allreduce_kernel", e);
+    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_launch, "launch allreduce_kernel");
+        rc != CDPROBE_OK)
+      return rc;
   }
 
   // 5. collect: per row, the times and checksums of every size, then the word checks
-  std::vector<cdp::ArScratch> got(1);
+  auto got = std::make_unique<cdp::ArScratch>();
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
-    if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::ArScratch), got.data(), "cdprobe_allreduce"); rc != CDPROBE_OK)
-      return rc;
-    const cdp::ArScratch& s = got[0];
+    if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_allreduce"); rc != CDPROBE_OK) return rc;
+    const cdp::ArScratch& s = *got;
     cdp::bw_summarize(s.rep, want, size, n_sizes, reps, g, out);
     if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
     for (uint32_t k = 0; k < n_sizes; ++k) {
@@ -855,11 +845,9 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
   //    every process refuses or runs together over the same cells
-  std::string bad;
   uint64_t size[cdp::kBwMaxSizes];
-  const uint32_t n_sizes = cdp::bwcurve_ladder(pl.bpp, size);
-  if (reps > cdp::kMaxTimedReps) bad = "reps must be at most 64";
-  else if (n_sizes == 0) bad = "bytes_per_pair must be at most 32 GiB";
+  uint32_t n_sizes;
+  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
   uint32_t f_send = cdp::kA2aNoFault, f_recv = cdp::kA2aNoFault, f_k = cdp::kA2aNoFault;
   uint64_t f_word = 0;
   if (h->a2a_fault != 0 && bad.empty()) {
@@ -874,26 +862,17 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
       f_k = (uint32_t)fk - 1;
     }
   }
-  using Rows = int32_t[cdp::kMaxRanks][cdp::kMaxRanks];
-  cdp::Agreement<Rows> mine = {h->a2a_calls + 1, {reps, 0u, 0u}, 0u, {}};
-  for (uint32_t li = 0; li < h->n_local; ++li)
-    for (uint32_t j = 0; j < n; ++j) mine.extra[li][j] = cdp::cell_status(h, li, j);
-  std::vector<cdp::Agreement<Rows>> all;
-  if (const int rc = cdp::agree(h, "cdprobe_alltoall", bad, mine, all); rc != CDPROBE_OK) return rc;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_alltoall", bad, h->a2a_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
+    return rc;
   // 2. the exchange area, built once, by every process in the same call
   if (const int rc = cdp::ensure_area(h); rc != CDPROBE_OK) return rc;
-  h->a2a_calls = mine.call_seq;
-  out->call_seq = h->a2a_calls;
+  out->call_seq = ++h->a2a_calls;
   out->area_bytes = h->area.bytes;
-  out->n_sizes = n_sizes;
-  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
-  for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
+  cdp::put_ladder(h, size, n_sizes, out);
 
   // 3. which cells run: st[s][d], the probe mapping status of sender s's cell to receiver d, or else its exchange-area
   //    mapping status; 0 runs.  Every process derives the same matrix.
-  Rows st = {};
-  for (uint32_t r = 0; r < all.size(); ++r)
-    for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].extra[li], sizeof(st[0]));
   bool any = false;
   for (uint32_t s = 0; s < n; ++s) {
     for (uint32_t d = 0; d < n; ++d) {
@@ -921,7 +900,6 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   //    kernel is launched before any is waited for
   if (const int rc = cdp::ensure_scratch_all(h, sizeof(cdp::A2aScratch)); rc != CDPROBE_OK) return rc;
   if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-  const bool coop_ok = !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
   bool launched[cdp::kMaxRanks] = {};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
@@ -961,31 +939,23 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
       p.from[p.n_in] = s;
       p.in[p.n_in++] = reinterpret_cast<const uint8_t*>(L.area_va[g]) + (uint64_t)s * pl.bpp;
     }
-    p.scratch = static_cast<cdp::A2aScratch*>(L.scratch);
-    memcpy(p.size, size, sizeof(size));
     p.seed = h->seed;
-    p.timeout_ns = (uint64_t)h->cfg.timeout_ms * 1000000ull;
     p.rank = g;
-    p.n_sizes = n_sizes;
-    p.reps = reps;
-    p.path = h->path;
     out->blocks[g] = p.blocks;
-    CDP_RT(cudaSetDevice(L.ordinal));
-    cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(cdp::A2aScratch), L.stream);
-    if (e == cudaSuccess) e = (cudaError_t)cdp::alltoall_launch(p, L.ctas, L.coop && coop_ok, L.stream);
-    if (e != cudaSuccess) return cdp::fail_sticky(h, "launch alltoall_kernel", e);
+    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::alltoall_launch, "launch alltoall_kernel");
+        rc != CDPROBE_OK)
+      return rc;
     launched[li] = true;
   }
 
   // 5. collect: per rank, the egress times; per cell it receives, the word checks and the last rep's (S, X)
-  std::vector<cdp::A2aScratch> got(1);
+  auto got = std::make_unique<cdp::A2aScratch>();
   for (uint32_t li = 0; li < h->n_local; ++li) {
     if (!launched[li]) continue;
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
-    if (const int rc = cdp::fetch_reps(h, L, sizeof(cdp::A2aScratch), got.data(), "cdprobe_alltoall"); rc != CDPROBE_OK)
-      return rc;
-    const cdp::A2aScratch& s = got[0];
+    if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_alltoall"); rc != CDPROBE_OK) return rc;
+    const cdp::A2aScratch& s = *got;
     const bool timed = cdp::bw_times(s.rep, size, n_sizes, reps, (double)out->blocks[g], g, out);
     for (uint32_t i = 0; i < n; ++i) {
       if (!runs(i, g)) continue;
