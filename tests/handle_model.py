@@ -2,10 +2,13 @@
 
 A daemon keeps one handle for days and interleaves runs, option changes, remaps, fault injection and the on-demand
 measurements on it.  `HandleModel` follows the same calls and says, from the pattern spec alone, what each one must
-return: the expected values come from the CPU oracle (oracle/oracle.py), tests/word_ref.py, tests/latency_ref.py and
-tests/bwcurve_ref.py, never from the library.  It tracks:
+return: the expected values come from the CPU oracle (oracle/oracle.py), tests/word_ref.py, tests/latency_ref.py,
+tests/bwcurve_ref.py, tests/allreduce_ref.py and tests/alltoall_ref.py, never from the library.  It tracks:
 
-- the counters: run_seq and the call_seq of pingpong, atomics and bwcurve (a refused call advances none);
+- the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, allreduce and alltoall (a refused call
+  advances none);
+- the armed all-reduce and all-to-all faults of each process's handle, and which pairs were unmapped when the
+  all-to-all's exchange area was built;
 - the options in force: path, CTAs per rank, verify CTAs, the schedule flags, warm-up mode;
 - the phase table each rank must walk (cdprobe_schedule with the current options, with the jobs of an unmapped pair
   idled as the library's schedule does);
@@ -28,6 +31,8 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
+import allreduce_ref
+import alltoall_ref
 import bwcurve_ref
 import latency_ref
 import word_ref
@@ -70,6 +75,17 @@ def corrupted_checksum(base: Tuple[int, int], seed: int, rank: int, first: int, 
     return s, x
 
 
+def refold(base: Tuple[int, int], changed: Dict[int, Tuple[int, int]], n_words: int) -> Tuple[int, int]:
+    """(S, X) of the first n_words of a word array whose clean (S, X) is `base`, given the words that differ from the
+    clean ones ({word: (old, new)}): S += new - old and X ^= rotl64(old ^ new, fold6(word's granule))."""
+    s, x = base
+    for k, (old, new) in changed.items():
+        if k < n_words:
+            s = (s + new - old) & M64
+            x ^= rotl64(old ^ new, word_ref.fold6(k // word_ref.GRANULE_WORDS))
+    return s, x
+
+
 @dataclasses.dataclass
 class Slot:
     run_seq: Optional[int] = None              # the run that last wrote the slot; None: never (zeros of open)
@@ -101,7 +117,13 @@ class HandleModel:
         self.warm_mode = 1
         self.runs = 0                              # cdprobe_run calls that returned
         self.run_seq = 0                           # of the last run; 0: none yet
-        self.pp_calls = self.at_calls = self.bw_calls = 0
+        self.pp_calls = self.at_calls = self.bw_calls = self.ar_calls = self.a2a_calls = 0
+        # CDPROBE_OPT_ALLREDUCE_FAULT / CDPROBE_OPT_ALLTOALL_FAULT value of each process's handle (absent: disarmed)
+        self.ar_fault: Dict[int, int] = {}
+        self.a2a_fault: Dict[int, int] = {}
+        # the pairs unmapped when the first all-to-all built its exchange area (None: not built yet); the area is mapped
+        # only where the probe mapping was up then, and remaps do not map it later
+        self.area_down: Optional[frozenset] = None
         self.corrupt: Dict[Tuple[int, int], int] = {}      # (rank, word) -> mask, at rest
         # armed landing fault of each process's handle (one per handle): {process: (issuer, target, faults)}
         self.fault: Dict[int, Tuple[int, int, Tuple[Tuple[int, int], ...]]] = {}
@@ -277,6 +299,119 @@ class HandleModel:
                                sx=[self.read_checksum(i, j, s // 8) for s in sizes])
         return self.bw_calls, sizes, out
 
+    def ar_word(self, w: int) -> int:
+        """Word w of the clean all-reduce output: the sum of word w of every rank's pattern."""
+        return sum(src_word(self.seed, j, w) for j in range(self.n)) & M64
+
+    def allreduce(self, reps: int) -> Optional[dict]:
+        """What cdprobe_allreduce with `reps` timed reps must return: {"call_seq", "sizes", "rows": {local rank: {...}}},
+        or None when some process's armed fault names no rank, size or word of the ladder (CDPROBE_ERR_ARG; nothing
+        advances).  Any unmapped pair stops every rank, with the status of the first down cell, and call_seq still
+        advances.  Otherwise output word w is the sum of word w of every source buffer as it is at rest (slice 0 only),
+        a word is bad when that differs from the clean sum, and an armed fault adds 1 to its word in timed rep 1 of its
+        size on its rank: the word check and the reported (S, X) (both of the last rep) see it when reps is 1, and the
+        size fails at any reps since every rep's (S, X) is checked."""
+        sizes = bwcurve_ref.ladder(self.bpp)
+        faults = {}
+        for proc, v in self.ar_fault.items():
+            fr, fk, fw = v >> 32, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+                return None
+            if self.process_of(fr - 1) == proc:
+                faults[(fr - 1, fk - 1)] = fw
+        self.ar_calls += 1
+        out = dict(call_seq=self.ar_calls, sizes=sizes, rows={})
+        if self.unmapped:
+            for g in self.local:
+                out["rows"][g] = dict(measured=False, status=ERR_STATE)
+            return out
+        clean = allreduce_ref.expected(self.seed, self.n, tuple(sizes))
+        delta: Dict[int, int] = {}
+        for (r, k), m in self.corrupt.items():
+            if k < self.W:
+                w = src_word(self.seed, r, k)
+                delta[k] = (delta.get(k, 0) + (w ^ m) - w) & M64
+        at_rest = {}  # {output word: (clean, as summed)} of the words the corruptions change
+        for w, d in delta.items():
+            if d:
+                c = self.ar_word(w)
+                at_rest[w] = (c, (c + d) & M64)
+        for g in self.local:
+            row = dict(measured=True, bad_sizes=0, sx=[], bad_words=[], first_bad=[])
+            for k, s in enumerate(sizes):
+                nw = s // 8
+                rep1 = dict(at_rest)
+                fw = faults.get((g, k))
+                if fw is not None:
+                    old, cur = at_rest.get(fw, (self.ar_word(fw),) * 2)
+                    rep1[fw] = (old, (cur + 1) & M64)
+                last = rep1 if reps == 1 else at_rest
+                bad = sorted(w for w, (o, v) in last.items() if w < nw and o != v)
+                sx = refold(clean[k], last, nw)
+                row["sx"].append(sx)
+                row["bad_words"].append(len(bad))
+                row["first_bad"].append(8 * bad[0] if bad else word_ref.U64_MAX)
+                if bad or sx != clean[k] or refold(clean[k], rep1, nw) != clean[k]:
+                    row["bad_sizes"] |= 1 << k
+            row["status"] = ERR_INTEGRITY if row["bad_sizes"] else 0
+            out["rows"][g] = row
+        return out
+
+    def a2a_runs(self, s: int, d: int) -> bool:
+        """Whether all-to-all cell (sender s, receiver d) runs: it exists, s maps d now, and s's view of d's exchange
+        area was mapped when the area was built."""
+        return ((s != d or self.diag) and (s, d) not in self.unmapped and self.area_down is not None
+                and (s, d) not in self.area_down)
+
+    def alltoall(self, reps: int) -> Optional[dict]:
+        """What cdprobe_alltoall with `reps` timed reps must return, or None when some process's armed fault names no
+        cell, size or word (CDPROBE_ERR_ARG; nothing advances, and the exchange area is not built).  {"call_seq",
+        "sizes", "ranks": {local rank: {"measured", "blocks"}}, "cells": {(s, d): {...}}} with every cell whose receiver
+        is local, and every cell that does not run whose sender is local.  The area is built by the first call that
+        runs, so a pair unmapped then stays skipped after its remap.  Source corruptions and landing faults do not
+        touch the blocks; an armed fault fails exactly its cell and size (the word check of every rep sees rep 1; the
+        (S, X) of the last rep sees it when reps is 1)."""
+        n = self.n
+        sizes = bwcurve_ref.ladder(self.bpp)
+        faults = {}
+        for proc, v in self.a2a_fault.items():
+            fs, fr, fk, fw = v >> 40, (v >> 32) & 0xFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if (fs == 0 or fs > n or fr == 0 or fr > n or (fs == fr and not self.diag) or fk == 0 or fk > len(sizes)
+                    or fw >= sizes[fk - 1] // 8):
+                return None
+            if self.process_of(fs - 1) == proc:
+                faults[(fs - 1, fr - 1)] = (fk - 1, fw)
+        if self.area_down is None:
+            self.area_down = frozenset(self.unmapped)
+        self.a2a_calls += 1
+        seq = self.a2a_calls
+        runs = self.a2a_runs
+        ranks = {}
+        for g in self.local:
+            joined = any(runs(g, j) or runs(j, g) for j in range(n))
+            ranks[g] = dict(measured=joined, blocks=sum(runs(g, j) for j in range(n)))
+        cells = {}
+        for s in range(n):
+            for d in range(n):
+                if (s == d and not self.diag) or not (d in self.local or (s in self.local and not runs(s, d))):
+                    continue
+                if not runs(s, d):
+                    cells[(s, d)] = dict(cell_measured=False, cell_status=ERR_STATE)
+                    continue
+                sx = alltoall_ref.expected(self.seed, s, d, seq, reps, sizes)
+                bad_words, first_bad = [0] * len(sizes), [word_ref.U64_MAX] * len(sizes)
+                if (s, d) in faults:
+                    fk, fw = faults[(s, d)]
+                    bad_words[fk], first_bad[fk] = 1, 8 * fw
+                    if reps == 1:
+                        salt = word_ref.write_salt(self.seed, s, d, alltoall_ref.alltoall_seq(seq, fk, 1))
+                        w = int(word_ref.write_words(salt, fw, 1)[0])
+                        sx[fk] = refold(sx[fk], {fw: (w, w ^ 1)}, sizes[fk] // 8)
+                bad = sum(1 << k for k, b in enumerate(bad_words) if b)
+                cells[(s, d)] = dict(cell_measured=True, cell_status=ERR_INTEGRITY if bad else 0, bad_sizes=bad,
+                                     bad_words=bad_words, first_bad=first_bad, sx=sx)
+        return dict(call_seq=seq, sizes=sizes, ranks=ranks, cells=cells)
+
     # ---- state changes -------------------------------------------------------------------------------------
     def corrupt_word(self, rank: int, word: int, mask: int) -> None:
         m = self.corrupt.pop((rank, word), 0) ^ mask
@@ -292,6 +427,14 @@ class HandleModel:
             self.fault[self.process_of(i)] = (i, j, tuple(sorted(faults)))
         else:
             self.fault.pop(self.process_of(i), None)
+
+    def arm_measure(self, faults: Dict[int, int], proc: int, value: int) -> None:
+        """CDPROBE_OPT_ALLREDUCE_FAULT or CDPROBE_OPT_ALLTOALL_FAULT (`faults` is ar_fault or a2a_fault) set to `value`
+        in process proc's handle; 0 disarms it.  The value is only checked by the next call."""
+        if value:
+            faults[proc] = value
+        else:
+            faults.pop(proc, None)
 
     def set_flag(self, flag: int, on: bool) -> None:
         self.flags = (self.flags & ~flag) | (flag if on else 0)

@@ -1,6 +1,8 @@
 """Pins tests/handle_model.py against hand-built cases, without a GPU: the (S, X) of a slice with corrupted words, the
 latency chase over overridden words, what a landing slot holds after a history of runs, unmaps and landing faults
-(and so what cdprobe_diagnose must report on it), the counters and the unmapped-pair rule."""
+(and so what cdprobe_diagnose must report on it), the counters and the unmapped-pair rule, the all-reduce under
+corruptions (also cancelling ones) and faults against a direct recomputation, its skip rule, and the all-to-all's
+sticky exchange area."""
 import ctypes as C
 import random
 
@@ -8,6 +10,9 @@ import numpy as np
 import pytest
 
 import handle_model as hm
+import allreduce_ref
+import alltoall_ref
+import bwcurve_ref
 import latency_ref
 import word_ref as ref
 
@@ -158,3 +163,140 @@ def test_phase_table_idles_the_jobs_of_an_unmapped_pair(pkg, oracle):
                                  {"job0": "read", "peer0": 0, "job1": "verify", "peer1": 0}]
     m1.set_flag(hm.FLAG_OVERLAP_VERIFY, False)
     assert [ph["job0"] for ph in m1.phase_table(0)] == ["write", "read", "verify"]
+
+
+# ---- the all-reduce and the all-to-all -------------------------------------------------------------------------
+def allreduce_direct(n, sizes, corrupt, fault=None, reps=1):
+    """The all-reduce restated over whole word arrays (numpy): per size, (S, X) of the output of the last rep, its bad
+    words and first bad offset, given the corruptions at rest {(rank, word): mask} and a fault (k, word) of this row."""
+    W = sizes[-1] // 8
+    src = [ref.src_words(SEED, j, 0, W) for j in range(n)]
+    clean = sum(src[1:], src[0].copy())
+    for (r, k), m in corrupt.items():
+        if k < W:
+            src[r][k] ^= np.uint64(m)
+    at_rest = sum(src[1:], src[0].copy())
+    out = []
+    for k, s in enumerate(sizes):
+        words = at_rest[:s // 8].copy()
+        if fault is not None and fault[0] == k and reps == 1:
+            words[fault[1]] += np.uint64(1)
+        bad = np.flatnonzero(words != clean[:s // 8])
+        out.append((allreduce_ref.checksum(words), len(bad), 8 * int(bad[0]) if len(bad) else ref.U64_MAX))
+    return out
+
+
+def test_allreduce_under_one_corruption_equals_the_reference(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    for rank, word, mask in ((0, 0, 1), (2, 3 * G + 7, 1 << 63), (1, m.W - 1, 0xFFFF), (1, m.W + 5, 0xF0)):
+        m.corrupt_word(rank, word, mask)
+        got = m.allreduce(1)
+        want = allreduce_ref.expected_corrupted(SEED, n, tuple(sizes), rank, word, mask)
+        bits = 0 if word >= m.W else sum(1 << k for k, s in enumerate(sizes) if s // 8 > word)
+        for g in range(n):
+            row = got["rows"][g]
+            assert row["sx"] == want and row["bad_sizes"] == bits, (rank, word, g)
+            assert row["status"] == (hm.ERR_INTEGRITY if bits else 0)
+            assert row["bad_words"] == [(bits >> k) & 1 for k in range(len(sizes))]
+            assert row["first_bad"] == [8 * word if (bits >> k) & 1 else ref.U64_MAX for k in range(len(sizes))]
+        m.corrupt_word(rank, word, mask)  # restore
+        assert m.allreduce(1)["rows"][0]["sx"] == list(allreduce_ref.expected(SEED, n, tuple(sizes)))
+
+
+def test_allreduce_under_several_corruptions_and_a_fault_equals_a_direct_recomputation(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    rng = random.Random(5)
+    corrupt = {(0, 5): 1 << 40, (1, 5): 0x3, (2, 4 * G - 1): rng.getrandbits(64) | 1, (1, m.W - 1): 1 << 7,
+               (0, 2 * m.W + 3): 0xFF}
+    # a pair whose deltas cancel on word c: rank 2's change undoes rank 0's, so the sum there is clean
+    c = 3 * G + 100
+    wa, wb = hm.src_word(SEED, 0, c), hm.src_word(SEED, 2, c)
+    da = ((wa ^ 0x1234) - wa) & hm.M64
+    corrupt[(0, c)] = 0x1234
+    corrupt[(2, c)] = wb ^ ((wb - da) & hm.M64)
+    for (r, k), mask in corrupt.items():
+        m.corrupt_word(r, k, mask)
+    want = allreduce_direct(n, sizes, corrupt)
+    got = m.allreduce(1)["rows"]
+    for g in range(n):
+        assert [(sx, b, f) for sx, b, f in zip(got[g]["sx"], got[g]["bad_words"], got[g]["first_bad"])] == want, g
+    # the cancelled word is clean: a prefix ending just past it has exactly the bad words of the others
+    k = next(k for k, s in enumerate(sizes) if s // 8 > c)
+    assert want[k][1] == len({w for (r, w) in corrupt if w < min(sizes[k] // 8, m.W)} - {c})
+    # an armed fault on row 1, size 2, on a corrupted word: timed rep 1 adds 1 to the corrupted sum
+    fk = 2
+    m.arm_measure(m.ar_fault, 0, (2 << 32) | ((fk + 1) << 24) | 5)
+    for reps in (1, 3):
+        got = m.allreduce(reps)["rows"]
+        for g in range(n):
+            want = allreduce_direct(n, sizes, corrupt, (fk, 5) if g == 1 else None, reps)
+            assert [(sx, b, f) for sx, b, f in zip(got[g]["sx"], got[g]["bad_words"], got[g]["first_bad"])] == want
+        assert got[1]["bad_sizes"] == got[0]["bad_sizes"] | 1 << fk  # size 2 fails even when its last rep is clean
+
+
+def test_allreduce_skip_rule_refusals_and_counters(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    assert m.allreduce(2)["call_seq"] == 1
+    for bad in ((4 << 32) | (1 << 24), (1 << 24) | 5, (1 << 32) | ((len(sizes) + 1) << 24),
+                (1 << 32) | (1 << 24) | sizes[0] // 8, 1 << 32):
+        m.arm_measure(m.ar_fault, 0, bad)
+        assert m.allreduce(2) is None, hex(bad)
+    assert m.ar_calls == 1
+    m.arm_measure(m.ar_fault, 0, 0)
+    assert m.ar_fault == {}
+    m.unmapped.add((2, 1))
+    got = m.allreduce(2)
+    assert got["call_seq"] == 2 and got["rows"] == {g: dict(measured=False, status=hm.ERR_STATE) for g in range(n)}
+    assert (m.bw_calls, m.pp_calls, m.at_calls, m.a2a_calls, m.runs) == (0, 0, 0, 0, 0)
+    # a refusal is checked before the mapping verdict
+    m.arm_measure(m.ar_fault, 0, 1 << 32)
+    assert m.allreduce(2) is None and m.ar_calls == 2
+    m.arm_measure(m.ar_fault, 0, 0)
+    m.unmapped.discard((2, 1))
+    got = m.allreduce(2)
+    assert got["call_seq"] == 3 and all(r["status"] == 0 and r["bad_sizes"] == 0 for r in got["rows"].values())
+
+
+def test_alltoall_sticky_area_fault_and_counters(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    # a refused call builds no area
+    m.arm_measure(m.a2a_fault, 0, (1 << 40) | (1 << 32) | (1 << 24))  # the diagonal, which N = 3 does not have
+    assert m.alltoall(1) is None and m.area_down is None and m.a2a_calls == 0
+    m.arm_measure(m.a2a_fault, 0, 0)
+    m.unmapped.add((0, 2))
+    m.corrupt_word(1, 3, 1 << 5)                                       # source corruptions do not touch it
+    for step in ("first", "remapped", "again"):
+        got = m.alltoall(1)
+        assert got["sizes"] == sizes and m.area_down == {(0, 2)}, step
+        assert got["cells"][(0, 2)] == dict(cell_measured=False, cell_status=hm.ERR_STATE), step
+        assert [got["ranks"][g]["blocks"] for g in range(n)] == [1, 2, 2], step
+        assert all(r["measured"] for r in got["ranks"].values())
+        for (s, d), c in got["cells"].items():
+            if (s, d) != (0, 2):
+                assert c["cell_status"] == 0 and c["bad_sizes"] == 0
+                assert c["sx"] == [allreduce_ref.checksum(alltoall_ref.block_words(SEED, s, d, got["call_seq"], k, 1,
+                                                                                      sz // 8))
+                                   for k, sz in enumerate(sizes)]
+        m.unmapped.discard((0, 2))                                     # remap: the area stays unmapped for (0, 2)
+    assert m.a2a_calls == 3 and (m.ar_calls, m.bw_calls) == (0, 0)
+    # an armed fault fails exactly its cell and size; with reps = 1 the folded rep is the faulted one
+    fk, fw = len(sizes) - 1, m.W - 1
+    m.arm_measure(m.a2a_fault, 0, (3 << 40) | (1 << 32) | ((fk + 1) << 24) | fw)
+    for reps in (1, 2):
+        got = m.alltoall(reps)
+        c = got["cells"][(2, 0)]
+        assert c["bad_sizes"] == 1 << fk and c["cell_status"] == hm.ERR_INTEGRITY
+        assert c["bad_words"][fk] == 1 and c["first_bad"][fk] == 8 * fw
+        words = alltoall_ref.block_words(SEED, 2, 0, got["call_seq"], fk, reps, sizes[fk] // 8)
+        if reps == 1:
+            words[fw] ^= np.uint64(1)
+        assert c["sx"][fk] == allreduce_ref.checksum(words)
+        assert all(o["bad_sizes"] == 0 for key, o in got["cells"].items() if key not in ((2, 0), (0, 2)))

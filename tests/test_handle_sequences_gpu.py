@@ -10,6 +10,10 @@ one handle through many calls and compares the whole output of each call with th
   the verdict restatement (verdict_ref), the traced phase kinds and peers, and `warmed`;
 - Diagnose: the word_ref report of every cell, field for field, from the issuer and from the target;
 - Latency: status and digest; BwCurve: bad_sizes and (S, X) per size; PingPong and Atomics: clean cells, call_seq;
+- AllReduce: per row measured, status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest,
+  armed faults and the skip rule (any down pair stops every rank); AllToAll: per rank measured and blocks, per cell
+  status, bad_sizes and per size bad_words, first_bad and (S, X), under armed faults and the sticky exchange-area rule;
+  both with call_seq, the ladder and the path;
 - refused calls: the error code, and nothing they may not change.
 
 A divergence fails with the seed, the step index and every step so far; the walk is generated from the seed and the
@@ -27,6 +31,7 @@ import uuid
 
 import pytest
 
+import bwcurve_ref
 import handle_model as hm
 import verdict_ref
 import word_ref
@@ -46,6 +51,7 @@ UNIT = 1024  # words in one 8 KiB unit of the data paths
 HOPS, LAT_REPS = 64, 2
 TRIPS = 16
 ATOMIC_OPS = 64
+LADDER_REPS = 1  # the all-reduce and all-to-all fold timed rep 1, the faulted one, into their (S, X)
 
 
 class Refused(Exception):
@@ -158,6 +164,54 @@ class Driver:
             m.warm_mode = value
         elif name in ("OPT_UNIDIRECTIONAL", "OPT_OVERLAP_VERIFY", "OPT_ALL_RANK_BARRIERS", "OPT_PAIR_BARRIERS"):
             m.set_flag(getattr(self.a, "FLAG" + name[3:]), bool(value))
+        elif name == "OPT_ALLREDUCE_FAULT":
+            m.arm_measure(m.ar_fault, self.me, value)
+        elif name == "OPT_ALLTOALL_FAULT":
+            m.arm_measure(m.a2a_fault, self.me, value)
+
+    def check_allreduce(self):
+        a, m = self.a, self.m
+        want = m.allreduce(LADDER_REPS)
+        rc, t = self.p.allreduce_raw(LADDER_REPS)
+        if want is None:  # the armed fault names no rank, size or word of the ladder: refused, nothing advances
+            assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)
+            return
+        assert rc == a.OK, rc
+        ar = self.pkg.AllReduce.from_c(t)
+        assert (ar.call_seq, ar.sizes, ar.path, ar.reps) == (want["call_seq"], want["sizes"], m.path, LADDER_REPS), \
+            (ar.call_seq, want["call_seq"], ar.path, m.path)
+        assert ar.row_mask == sum(1 << g for g in m.local)
+        for g, w in want["rows"].items():
+            got = dict(measured=ar.measured[g], status=ar.status[g])
+            if w["measured"]:
+                got.update(bad_sizes=ar.bad_sizes[g], sx=list(zip(ar.sum[g], ar.xr[g])), bad_words=ar.bad_words[g],
+                           first_bad=ar.first_bad[g])
+            assert got == w, ("allreduce row", g, got, w)
+
+    def check_alltoall(self):
+        a, m = self.a, self.m
+        want = m.alltoall(LADDER_REPS)
+        rc, t = self.p.alltoall_raw(LADDER_REPS)
+        if want is None:  # the armed fault names no cell, size or word of the ladder: refused, nothing advances
+            assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)
+            return
+        assert rc == a.OK, rc
+        aa = self.pkg.AllToAll.from_c(t)
+        assert (aa.call_seq, aa.sizes, aa.path, aa.reps) == (want["call_seq"], want["sizes"], m.path, LADDER_REPS), \
+            (aa.call_seq, want["call_seq"], aa.path, m.path)
+        assert aa.area_bytes == (self.n * m.bpp + (2 << 20) - 1) // (2 << 20) * (2 << 20)
+        for g, w in want["ranks"].items():
+            assert aa.measured[g] == w["measured"], ("alltoall rank", g)
+            if w["measured"]:
+                assert aa.status[g] == 0 and aa.blocks[g] == w["blocks"], ("alltoall rank", g, aa.blocks[g], w)
+        for s in range(self.n):
+            for d in m.local:
+                w = want["cells"].get((s, d), dict(cell_measured=False, cell_status=0))
+                got = dict(cell_measured=aa.cell_measured[s][d], cell_status=aa.cell_status[s][d])
+                if w["cell_measured"]:
+                    got.update(bad_sizes=aa.bad_sizes[s][d], bad_words=aa.bad_words[s][d],
+                               first_bad=aa.first_bad[s][d], sx=list(zip(aa.sum[s][d], aa.xr[s][d])))
+                assert got == w, ("alltoall cell", s, d, got, w)
 
     def apply(self, step):
         a, m, p = self.a, self.m, self.p
@@ -236,10 +290,18 @@ class Driver:
             for (i, j), w in want.items():
                 if w["measured"]:
                     assert list(zip(bw.sum[i][j], bw.xr[i][j])) == w["sx"], ("bwcurve (S, X)", i, j)
+        elif kind == "allreduce":
+            self.check_allreduce()
+        elif kind == "alltoall":
+            self.check_alltoall()
         elif kind == "bad_call":  # refused measurement calls advance no call_seq
             what = step[1]
             if what == "bwcurve":
                 rc, _ = p.bwcurve_raw(a.BWCURVE_MAX_REPS + 1)
+            elif what == "allreduce":
+                rc, _ = p.allreduce_raw(a.ALLREDUCE_MAX_REPS + 1)
+            elif what == "alltoall":
+                rc, _ = p.alltoall_raw(a.ALLTOALL_MAX_REPS + 1)
             elif what == "pingpong":
                 rc, _ = p.pingpong_raw(a.PINGPONG_MAX_TRIPS + 1, 1, 0)
             else:
@@ -261,12 +323,48 @@ class Driver:
 
 
 # ---- the seeded walk -------------------------------------------------------------------------------------------
+def edge_word(rng, size):
+    """A word of the first `size` bytes where the ladder kernels go wrong: word 0, the last word, or a word of the last
+    partial 8 KiB unit (of the last unit when it is whole)."""
+    words = size // 8
+    lo = size // (UNIT * 8) * UNIT if size % (UNIT * 8) else words - UNIT
+    return rng.choice([0, words - 1, rng.randrange(lo, words)])
+
+
+def ladder_fault(rng, m, name, rank, peer):
+    """A valid OPT_ALLREDUCE_FAULT (on `rank`) or OPT_ALLTOALL_FAULT (cell rank -> peer) value at an edge word of a
+    size of the ladder: the last size or a random one."""
+    sizes = bwcurve_ref.ladder(m.bpp)
+    k = rng.choice([len(sizes) - 1, rng.randrange(len(sizes))])
+    word = edge_word(rng, sizes[k])
+    if name == "OPT_ALLREDUCE_FAULT":
+        return ((rank + 1) << 32) | ((k + 1) << 24) | word
+    return ((rank + 1) << 40) | ((peer + 1) << 32) | ((k + 1) << 24) | word
+
+
 def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
     """One step drawn from `rng` and the model's state alone (never from a device result).  `ctas_cap` bounds the
-    grids it may ask for, so that many same-device ranks stay resident together."""
+    grids it may ask for, so that many same-device ranks stay resident together.  A tenth of the steps are all-reduce
+    and all-to-all calls (each about as often as bwcurve) and their fault armings; the rest keep their weights."""
     n, W = m.n, m.W
     grids = [c for c in (1, 2, 3, 7, 8) if ctas_cap is None or c <= ctas_cap]
     x = rng.random()
+    if x < 0.035:
+        return ("allreduce",)
+    if x < 0.07:
+        return ("alltoall",)
+    if x < 0.10:
+        name = rng.choice(["OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"])
+        armed = m.ar_fault if name == "OPT_ALLREDUCE_FAULT" else m.a2a_fault
+        if armed and rng.random() < 0.4:
+            return ("opt", name, 0)
+        i = rng.choice(m.local)
+        j = rng.choice([c for c in range(n) if c != i] or [i])
+        value = ladder_fault(rng, m, name, i, j)
+        if rng.random() < 0.15:  # one word past its size: the next call is refused until the fault is re-armed
+            value += bwcurve_ref.ladder(m.bpp)[((value >> 24) & 0xFF) - 1] // 8 - (value & 0xFFFFFF)
+        return ("opt", name, value)
+    x = (x - 0.10) / 0.90
     if x < 0.28:
         return ("run",)
     if x < 0.48:
@@ -319,22 +417,32 @@ def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
         return ("atomics", rng.randrange(3))
     if x < 0.98:
         return ("bwcurve",)
-    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics"]))
+    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics", "allreduce", "alltoall"]))
+
+
+def walk_step(rng, m, steps, **kw):
+    """The next step of a walk: right after an unmap or a remap, an all-reduce or all-to-all call, so that every walk
+    with churn calls them while a pair is down and after a remap; else gen_step's."""
+    if steps and steps[-1][0] in ("unmap", "remap"):
+        return rng.choice([("allreduce",), ("alltoall",)])
+    return gen_step(rng, m, **kw)
 
 
 def walk(drv, seed, n_steps, **kw):
     rng = random.Random(seed)
     steps = []
     for k in range(n_steps):
-        step = gen_step(rng, drv.m, **kw)
+        step = walk_step(rng, drv.m, steps, **kw)
         steps.append(step)
         try:
             drv.apply(step)
         except Exception as e:
             raise AssertionError(f"seed {seed}: step {k} {step!r} diverged from the model: {e!r}\n"
                                  f"steps so far: {steps!r}") from e
-    drv.play([("run",), ("diagnose",)], f"seed {seed}: closing run")
-    return steps
+    # remap what is still down, so that every walk with churn also calls the ladder measurements after a remap
+    closing = [("remap",) + c for c in sorted(drv.m.unmapped)] + [("allreduce",), ("alltoall",), ("run",), ("diagnose",)]
+    drv.play(closing, f"seed {seed}: closing run")
+    return steps + closing
 
 
 def open_same(pkg, n, nbytes, ctas=8):
@@ -411,10 +519,48 @@ def test_measurements_between_a_corruption_and_its_restore(pkg, oracle, n):
     bpp = oracle.plan(n, BIG, 1, n == 1).bytes_per_pair
     W = bpp // 8
     word = W // G * G + 3  # inside the last, partial granule of slice 0
-    steps = [("bwcurve",), ("latency",), ("corrupt", 0, word, 0xFF00), ("bwcurve",), ("latency",), RUN, DIAG,
-             ("corrupt", 0, 5, 1 << 40), ("bwcurve",), ("latency",), ("corrupt", 0, word, 0xFF00), ("bwcurve",),
-             ("latency",), RUN, ("corrupt", 0, 5, 1 << 40), ("bwcurve",), ("latency",), RUN, DIAG]
+    AR, A2A = ("allreduce",), ("alltoall",)
+    steps = [("bwcurve",), ("latency",), AR, ("corrupt", 0, word, 0xFF00), ("bwcurve",), ("latency",), AR, A2A, RUN,
+             DIAG, ("corrupt", 0, 5, 1 << 40), ("bwcurve",), ("latency",), AR, ("corrupt", n - 1, 5, 1 << 41), AR,
+             ("corrupt", 0, word, 0xFF00), ("bwcurve",), ("latency",), AR, RUN, ("corrupt", 0, 5, 1 << 40),
+             ("corrupt", n - 1, 5, 1 << 41), ("bwcurve",), ("latency",), AR, A2A, RUN, DIAG]
     play(pkg, oracle, n, BIG, steps, f"n {n}")
+
+
+def test_alltoall_area_of_a_pair_unmapped_at_its_first_call_stays_unmapped_after_the_remap(pkg, oracle):
+    """The exchange area is mapped at the first all-to-all only where the probe mapping is up, and remaps leave it
+    alone: cell (0, 2) is skipped before and after its remap, until close, while runs use the remapped pair.  The
+    all-to-all leaves the landing slots as the last run wrote them."""
+    A2A = ("alltoall",)
+    steps = [RUN, ("unmap", 0, 2), A2A, ("allreduce",), ("remap", 0, 2), A2A, RUN, DIAG, A2A, DIAG,
+             ("opt", "OPT_ALLTOALL_FAULT", (3 << 40) | (1 << 32) | (1 << 24)), A2A, ("allreduce",), RUN, DIAG]
+    drv = play(pkg, oracle, 3, BIG, steps, "n 3")
+    assert drv.m.area_down == {(0, 2)} and drv.m.a2a_calls == 4
+
+
+@pytest.mark.parametrize("n", [1, 3])
+def test_grid_and_path_changes_between_ladder_calls_with_faults_armed(pkg, oracle, n):
+    """OPT_CTAS and OPT_CTAS_RANK change the grid the all-reduce and the all-to-all launch on, and with it which warp
+    walks which unit and stores the armed fault's word: on every path, with a fault armed on each, at an edge word."""
+    bpp = oracle.plan(n, SMALL, 1, n == 1).bytes_per_pair
+    sizes = bwcurve_ref.ladder(bpp)
+    last, W = len(sizes) - 1, bpp // 8
+    j = (n - 1) % n if n > 1 else 0
+    partial = W // UNIT * UNIT + 1  # in the last, partial unit of the last size
+    ar = [((n - 1 + 1) << 32) | ((last + 1) << 24) | (W - 1), (1 << 32) | (1 << 24) | 0]
+    a2a = [(1 << 40) | ((j + 1) << 32) | ((last + 1) << 24) | partial,
+           ((n - 1 + 1) << 40) | (1 << 32) | (1 << 24) | (sizes[0] // 8 - 1)]
+    grids = [("OPT_CTAS", 1), ("OPT_CTAS", 3), ("OPT_CTAS_RANK", (1 << 16) | 7), ("OPT_CTAS", 2),
+             ("OPT_CTAS_RANK", (n << 16) | 1), ("OPT_CTAS", 8)]
+    steps = []
+    for path in (0, 1, 2):
+        steps += [("opt", "OPT_PATH", path)]
+        for q, grid in enumerate(grids):
+            steps += [("opt", "OPT_ALLREDUCE_FAULT", ar[q % 2]), ("opt", "OPT_ALLTOALL_FAULT", a2a[q % 2]),
+                      ("allreduce",), ("alltoall",), ("opt",) + grid, ("allreduce",), ("alltoall",)]
+    steps += [("opt", "OPT_ALLREDUCE_FAULT", 0), ("opt", "OPT_ALLTOALL_FAULT", 0), ("allreduce",), ("alltoall",), RUN,
+              DIAG]
+    play(pkg, oracle, n, SMALL, steps, f"n {n}")
 
 
 def test_write_cell_of_a_writer_unmapped_for_one_run(pkg, oracle):
@@ -439,17 +585,18 @@ def test_out_of_range_ctas_are_refused(pkg, oracle, n):
 
 
 # ---- two processes, one rank each, on one GPU ------------------------------------------------------------------
-def two_proc_steps(seed, n_steps, bpp):
+def two_proc_steps(seed, n_steps, m):
     """The same list in both processes: collective steps ("all") and SetOption ("both") run in both; every other step
     belongs to one process.  Between two collective steps the processes are not ordered, so a stretch that corrupts a
     source buffer holds no step that reads another rank's memory outside a run."""
     rng = random.Random(seed)
-    W = bpp // 8
+    W = m.W
     out, mutating = [], False
     while len(out) < n_steps:
         x = rng.random()
         if x < 0.35:
-            out.append(("all", rng.choice([("run",), ("run",), ("pingpong", rng.randrange(2)), ("bwcurve",)])))
+            out.append(("all", rng.choice([("run",), ("run",), ("pingpong", rng.randrange(2)), ("bwcurve",),
+                                           ("allreduce",), ("alltoall",)])))
             mutating = rng.random() < 0.5
             continue
         if x < 0.5:
@@ -459,6 +606,11 @@ def two_proc_steps(seed, n_steps, bpp):
                                                        ("OPT_WARMUP", rng.choice([0, 2]))])))
             continue
         owner = rng.randrange(2)
+        if x < 0.58:  # a valid fault armed (or disarmed) only by the process that hosts its rank or sender
+            name = rng.choice(["OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"])
+            value = 0 if rng.random() < 0.3 else ladder_fault(rng, m, name, owner, 1 - owner)
+            out.append((owner, ("opt", name, value)))
+            continue
         if mutating:
             if rng.random() < 0.5:
                 out.append((owner, ("corrupt", owner, rng.choice([0, W - 1, W // G * G + 1]),
@@ -487,7 +639,7 @@ CHILD = textwrap.dedent(
                      timeout_ms=30000)
     with pkg.Open(cfg) as p:
         drv = t.Driver(pkg, oracle, p, cfg, 2, nbytes, me=rank, nprocs=2)
-        steps = t.two_proc_steps(seed, 40, drv.m.bpp)
+        steps = t.two_proc_steps(seed, 40, drv.m)
         done = []
         for k, (who, step) in enumerate(steps):
             done.append((who, step))
@@ -495,7 +647,7 @@ CHILD = textwrap.dedent(
                 if who in ("all", "both", rank):
                     drv.apply(step)
                 else:
-                    drv.mirror(step)
+                    drv.mirror(step, who)
             except Exception as e:
                 print("RESULT " + json.dumps({"ok": False, "error": f"process {rank}, seed {seed}: step {k} "
                                               f"{step!r} diverged from the model: {e!r}; steps so far: {done!r}"}))
@@ -505,14 +657,16 @@ CHILD = textwrap.dedent(
 ) % (ROOT, ROOT + "/tests")
 
 
-def mirror(self, step):
-    """The model's side of a step the other process executes: its state changes, not its checks."""
+def mirror(self, step, who):
+    """The model's side of a step process `who` executes: its state changes, not its checks."""
     m = self.m
     kind = step[0]
     if kind == "corrupt":
         m.corrupt_word(step[1], step[2], step[3])
     elif kind == "landing":
         m.arm(step[1], step[2], step[3])
+    elif kind == "opt" and step[1] in ("OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"):
+        m.arm_measure(m.ar_fault if step[1] == "OPT_ALLREDUCE_FAULT" else m.a2a_fault, who, step[2])
 
 
 Driver.mirror = mirror

@@ -30,6 +30,8 @@ import uuid
 
 import pytest
 
+import allreduce_ref
+import alltoall_ref
 import atomics_ref
 import bwcurve_ref
 import handle_model as hm
@@ -511,6 +513,8 @@ def mp_process(pkg, session, rank, world, n_local, what):
         out["at"] = [fields(p.Atomics(k, ops=ATOMIC_OPS, reps=AT_REPS)) for k in range(3)]
         out["pp"] = fields(p.PingPong(trips=MP_TRIPS, reps=PP_REPS))
         out["bw"] = fields(p.BwCurve(reps=BW_REPS))
+        out["ar"] = fields(p.AllReduce(reps=2))
+        out["a2a"] = fields(p.AllToAll(reps=2))
         # a landing fault armed in process 0 on a cell whose target lives in the last process
         W = info.bytes_per_pair // 8
         if rank == 0:
@@ -612,6 +616,27 @@ def test_processes_with_several_ranks_each(pkg, oracle, world, n_local):
                 first = slice_first_word(n, i, j, W * 8, False)
                 assert [[s, x] for s, x in zip(bw["sum"][i][j], bw["xr"][i][j])] == \
                     [list(oracle.src_checksum(SEED, j, first, s // 8)) for s in bw["sizes"]], (i, j)
+        # the all-reduce fills exactly the local rows, and the all-to-all exactly the cells a local rank receives, with
+        # the pattern's (S, X) at every size; both agree on call_seq in every process
+        ar, a2a = o["ar"], o["a2a"]
+        sizes = bwcurve_ref.ladder(W * 8)
+        for key in ("ar", "a2a"):
+            assert o[key]["call_seq"] == outs[0][key]["call_seq"] == 1 and o[key]["sizes"] == sizes, key
+            assert o[key]["row_mask"] == rows and o[key]["reps"] == 2, key
+        ar_want = [list(sx) for sx in allreduce_ref.expected(SEED, n, tuple(sizes))]
+        for r in range(n):
+            assert ar["measured"][r] == a2a["measured"][r] == (r in mine), r
+            if r in mine:
+                assert ar["status"][r] == 0 and ar["bad_sizes"][r] == 0 and ar["bad_words"][r] == [0] * len(sizes)
+                assert [[s, x] for s, x in zip(ar["sum"][r], ar["xr"][r])] == ar_want, r
+                assert a2a["status"][r] == 0 and a2a["blocks"][r] == n - 1, r
+        for s in range(n):
+            for d in range(n):
+                assert a2a["cell_measured"][s][d] == (d in mine and s != d), (s, d)
+                if a2a["cell_measured"][s][d]:
+                    assert a2a["cell_status"][s][d] == 0 and a2a["bad_words"][s][d] == [0] * len(sizes), (s, d)
+                    assert [[x, y] for x, y in zip(a2a["sum"][s][d], a2a["xr"][s][d])] == \
+                        [list(e) for e in alltoall_ref.expected(SEED, s, d, 1, 2, sizes)], (s, d)
         # the landing fault of process 0 fails exactly its cell, in every process's gathered result
         f = AsResult(o["faulted"])
         want_w = [[0 if (a, b) == (0, n - 1) else 1 for b in range(n)] for a in range(n)]
