@@ -549,6 +549,12 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              hosts `sender`, timed rep 1 of size[k] stores word `word` (< 2^24) of
                                              block (sender -> receiver) xored with 1, so exactly that cell and size
                                              fail the receiver's word check; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT 21u /* tests: value = (drop << 48) | ((receiver + 1) << 32) | ((k + 1) << 24)
+                                             | word arms a fault in cdprobe_allreduce_twoshot: in timed rep 1 of size[k],
+                                             in the process that hosts the rank whose chunk holds word `word`
+                                             (< 2^24), that rank stores the word into receiver's output xored with 1
+                                             (drop 0), or skips every store of the word's 8 KiB unit into receiver
+                                             (drop 1), so exactly that row and size fail; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -669,6 +675,35 @@ CDPROBE_API int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce
  * that differ between processes, or an armed CDPROBE_OPT_ALLTOALL_FAULT that names no cell of the domain, a k >=
  * n_sizes or a word >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out);
+/* Two-shot all-reduce of every rank's source buffer, on every rank at once: a reduce-scatter, then a pushed
+ * all-gather.  For each size of the cdprobe_bwcurve ladder, one untimed warm-up rep, then `reps` timed reps.  A size
+ * of U = ceil(size / 8 KiB) units is split into chunks: rank r owns units [floor(r U / n), floor((r + 1) U / n)),
+ * possibly none.  In a rep, rank r reads its units of every rank's source buffer, adding rank r, r + 1, ... (mod n) as
+ * cdprobe_allreduce does on the CDPROBE_OPT_PATH read path with its whole probe grid, and stores each summed unit with
+ * st.global.v4 into every rank's gather area, its own first, then r + 1, r + 2, ... (mod n).  Each rank's link
+ * traffic per rep is 2 (n - 1) / n x size, the all-reduce's.  Domain barriers open and close every rep (flags in the
+ * Ctrl granule; only grid barriers at n == 1), the closing one after a fence.sys in every CTA; a rep is timed per rank
+ * by %globaltimer from that rank's opening release to its closing release, when its output is complete.  After every
+ * rep, warm-up included and untimed, each rank reads back every word of its output, compares it with the pattern's sum
+ * and overwrites it with 0, so a unit that is not delivered in the next rep reads as 0s.  Every rep's (S, X) of that
+ * read-back is checked against the pattern's sum (bad_sizes, CDPROBE_ERR_INTEGRITY).  Row r of *out describes what
+ * rank r holds at the end of a rep:
+ *   sum, xr:              the (S, X) of rank r's whole output as rank r read it back after the last timed rep;
+ *   bad_words, first_bad: summed over every rep of the size, warm-up included (cdprobe_allreduce checks only the last);
+ *   peak_gbps:            the algorithm bandwidth, size / ns; the nccl-tests bus bandwidth is peak_gbps x 2 (n - 1) / n.
+ * The gather area (bytes_per_pair per rank, rounded up to 2 MiB) is created on the first call with the probe
+ * allocation's handle type, mapped wherever the probe mapping is then up, and kept until close; if creating it fails
+ * in any process, every process returns that error, nothing runs, and the next call tries again.  If any probe or
+ * gather-area mapping of the domain is down (cdprobe_unmap_peer, a failed mapping, MIG), nothing runs: every filled
+ * row has measured = 0 and the status of the first such cell, and the call returns CDPROBE_OK.  A rank whose kernel
+ * passes timeout_ms is CDPROBE_ERR_TIMEOUT and the handle stays usable.  Collective when world_size > 1: every process
+ * calls it with the same reps and fills the rows of its own ranks (row_mask); call_seq counts calls of this function.
+ * Needs no run first and touches no result, pattern, source buffer, landing slot, run_seq, warm-up state, exchange
+ * area or other measurement's state.  *out carries abi, n and reps whatever the return code.  CDPROBE_ERR_ARG: null
+ * argument, reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes, or an armed
+ * CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT whose receiver is >= n, whose k is >= n_sizes, whose word is >= size[k] / 8 or
+ * that has a bit above 48 set; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

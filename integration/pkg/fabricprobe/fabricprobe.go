@@ -47,6 +47,7 @@ static at_fn cdp_at;      // optional: absent from libraries that predate cdprob
 static bw_fn cdp_bw;      // optional: absent from libraries that predate cdprobe_bwcurve
 static ar_fn cdp_ar;      // optional: absent from libraries that predate cdprobe_allreduce
 static a2a_fn cdp_a2a;    // optional: absent from libraries that predate cdprobe_alltoall
+static ar_fn cdp_ar2;     // optional: absent from libraries that predate cdprobe_allreduce_twoshot
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -65,6 +66,7 @@ static int cdp_load(const char* path) {
   cdp_bw = (bw_fn)dlsym(cdp_dl, "cdprobe_bwcurve");
   cdp_ar = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce");
   cdp_a2a = (a2a_fn)dlsym(cdp_dl, "cdprobe_alltoall");
+  cdp_ar2 = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_twoshot");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -95,6 +97,10 @@ static int cdp_has_allreduce(void) { return cdp_ar != NULL; }
 static int cdp_call_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) { return cdp_ar(h, reps, ar); }
 static int cdp_has_alltoall(void) { return cdp_a2a != NULL; }
 static int cdp_call_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* aa) { return cdp_a2a(h, reps, aa); }
+static int cdp_has_allreduce_twoshot(void) { return cdp_ar2 != NULL; }
+static int cdp_call_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
+  return cdp_ar2(h, reps, ar);
+}
 */
 import "C"
 
@@ -266,8 +272,9 @@ type BwCurve struct {
 	Ms                     float64
 }
 
-// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t).  Every slice is indexed by rank; the
-// per-size ones hold one entry per Sizes element, and every timing is 0 where a rank was not measured or timed out.
+// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot).
+// Every slice is indexed by rank; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
+// rank was not measured or timed out.
 type AllReduce struct {
 	N                      int
 	RowMask                uint32      // rows of this process's ranks
@@ -649,6 +656,35 @@ func (p *Probe) AllReduce(reps int) (AllReduce, error) {
 		}
 		return AllReduce{}, err
 	}
+	return allReduceOf(ar), nil
+}
+
+// AllReduceTwoShot runs the two-shot all-reduce of every rank's source buffer on every rank at once, a reduce-scatter
+// then a pushed all-gather, at each size of the bwcurve ladder, and reports ns per rep for each size (reps 0: 8 timed
+// reps).  Every rep's output is read back, checked word for word and cleared: BadWords and FirstBad cover every rep.
+// PeakGBps is the algorithm bandwidth; the nccl-tests bus bandwidth is PeakGBps x 2(N - 1)/N.  Collective when the
+// domain spans processes.  ErrUnsupported when the library predates cdprobe_allreduce_twoshot.
+func (p *Probe) AllReduceTwoShot(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce_twoshot() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce_twoshot", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	ar := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce_twoshot(p.h, C.uint32_t(reps), ar)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce_twoshot: %s: %s", C.GoString(C.cdp_call_strerror(rc)),
+			C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	return allReduceOf(ar), nil
+}
+
+// allReduceOf copies a cdprobe_allreduce_t into an AllReduce.
+func allReduceOf(ar *C.cdprobe_allreduce_t) AllReduce {
 	n, ns := int(ar.n), int(ar.n_sizes)
 	out := AllReduce{N: n, RowMask: uint32(ar.row_mask), Reps: int(ar.reps), Path: int(ar.path),
 		CallSeq: uint64(ar.call_seq), Ms: float64(ar.ms)}
@@ -685,7 +721,7 @@ func (p *Probe) AllReduce(reps int) (AllReduce, error) {
 			out.FirstBad[r][s] = uint64(ar.first_bad[r][s])
 		}
 	}
-	return out, nil
+	return out
 }
 
 // AllToAll runs the one-shot all-to-all: every rank pushes a block to every peer at once, at each size of the bwcurve

@@ -181,5 +181,6 @@ func (*Probe) PingPong(int, int, bool) (PingPong, error) {
 func (*Probe) Atomics(int, int, int) (Atomics, error) { return Atomics{}, ErrUnsupported }
 func (*Probe) BwCurve(int) (BwCurve, error) { return BwCurve{}, ErrUnsupported }
 func (*Probe) AllReduce(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllReduceTwoShot(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

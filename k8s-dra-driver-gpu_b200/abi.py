@@ -36,6 +36,7 @@ OPT_PINGPONG_FAULT = 17
 OPT_ATOMICS_FAULT = 18
 OPT_ALLREDUCE_FAULT = 19
 OPT_ALLTOALL_FAULT = 20
+OPT_ALLREDUCE_TWOSHOT_FAULT = 21
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -398,6 +399,12 @@ def allreduce_fault(rank: int, k: int, word: int) -> int:
     return ((rank + 1) << 32) | ((k + 1) << 24) | word
 
 
+def allreduce_twoshot_fault(receiver: int, k: int, word: int, drop: bool = False) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT value that makes timed rep 1 of size[k] deliver output word `word` to
+    `receiver` xored with 1, or (drop) not deliver the word's 8 KiB unit to `receiver` at all."""
+    return ((1 if drop else 0) << 48) | ((receiver + 1) << 32) | ((k + 1) << 24) | word
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -433,6 +440,7 @@ SYMBOLS = {
     "cdprobe_atomics": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(AtomicsT)]),
     "cdprobe_bwcurve": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(BwCurveT)]),
     "cdprobe_allreduce": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
+    "cdprobe_allreduce_twoshot": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

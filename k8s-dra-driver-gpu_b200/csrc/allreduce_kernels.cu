@@ -1,32 +1,18 @@
 // allreduce_kernels.cu — sm_90a kernels of cdprobe_allreduce's one-shot all-reduce: every warp streams one output unit
 // of all n ranks' source buffers (TMA ring or ld.global.v4), adds them in registers and stores the sum with
 // st.global.v4; each rep opens with a domain barrier (allreduce_kernel).  And the per-granule sums of the output that
-// the expected checksums are folded from (granules_kernel<AllReduceWord>).  The shared data path is in datapath.cuh.
+// the expected checksums are folded from (granules_kernel<AllReduceWord>).  The shared data path is in datapath.cuh,
+// the read-and-add side in allreduce_path.cuh.
 //
 // probe_kernels.cu is untouched: the probe kernel's code generation does not depend on this file.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "allreduce.h"
-#include "datapath.cuh"
+#include "allreduce_path.cuh"
 
 namespace cdp {
 namespace {
-constexpr int kArWords = 2 * kLdstVecs;  // uint64 accumulators per lane: a warp holds one 8 KiB output unit
-
-// Byte offset in a unit of the lane's 16-byte vector i when each access moves kLaneBytes contiguous bytes: the layout
-// job_read_ldst loads in, and for kLaneBytes = 16 also the one job_read_tma reads a stage in.
-template <uint32_t kLaneBytes>
-__device__ __forceinline__ uint32_t ar_vec_off(int lane, int i) {
-  constexpr int kV = kLaneBytes / 16;
-  return kLaneBytes * (uint32_t)lane + 32u * kLaneBytes * (uint32_t)(i / kV) + 16u * (uint32_t)(i % kV);
-}
-
-__device__ __forceinline__ void ar_add(uint64_t (&acc)[kArWords], int i, const uint4& v) {
-  acc[2 * i] += pack64(v.x, v.y);
-  acc[2 * i + 1] += pack64(v.z, v.w);
-}
-
 // Unit u of the output is complete in the accumulators: the armed fault goes in (fw, an output word index; ~0 when
 // none), every vector of the unit leaves with st.global.v4 and is folded into the (S, X) by its place in the output,
 // and the accumulators are cleared for the next unit.
@@ -59,103 +45,14 @@ __device__ __forceinline__ void ar_store(const Ctx& c, uint8_t* out, uint64_t u,
   fold_unit(a, ux, u);
 }
 
-// TMA read side: the warp walks (unit, input) pairs, the n inputs of a unit in a row, through its kStages-deep ring of
-// bulk loads, one load per pair.  Each stage is added into the accumulators and then refilled with the next pair, so
-// the ring runs on across unit boundaries.  Aborted: stops issuing and drains what is in flight.
-__device__ void ar_units_tma(Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw, Sum& a) {
-  const uint32_t n = P.n;
-  Walk<false> iw = walk;  // the issue side: up to kStages pairs ahead of the consume side, over the same pairs
-  uint64_t iu = 0;
-  bool imore = iw.take(c, iu);
-  uint32_t isrc = 0, in_flight = 0;
-  if (c.lane == 0) fence_proxy_async_global();  // data may have been written through the generic proxy
-#pragma unroll
-  for (int s = 0; s < kStages; ++s) {
-    if (!imore) break;
-    if (c.lane == 0) issue_load(c, P.src[isrc], bytes, iu, s);
-    ++in_flight;
-    if (++isrc == n) {
-      isrc = 0;
-      imore = iw.take(c, iu);
-    }
-  }
-  uint64_t acc[kArWords];
-#pragma unroll
-  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
-  int s = 0;
-  uint32_t csrc = 0;
-  uint64_t u = 0;
-  bool more = walk.take(c, u);
-  while (more) {
-    if (!mbar_wait(c, s)) {
-      for (; in_flight > 0; --in_flight) {
-        mbar_drain(c, s);
-        s = (s + 1 == kStages) ? 0 : s + 1;
-      }
-      return;
-    }
-    --in_flight;
-    const uint32_t len = unit_len(bytes, u);
-    const uint32_t sbase = c.stage_smem + s * kUnitBytes;
-    if (len == kUnitBytes) {
-#pragma unroll
-      for (int i = 0; i < kArWords / 2; ++i) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
-    } else {
-#pragma unroll
-      for (int i = 0; i < kArWords / 2; ++i)
-        if (ar_vec_off<16>(c.lane, i) < len) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
-    }
-    __syncwarp();
-    if (imore) {
-      if (c.lane == 0) {
-        fence_proxy_async_smem();
-        issue_load(c, P.src[isrc], bytes, iu, s);
-      }
-      ++in_flight;
-      if (++isrc == n) {
-        isrc = 0;
-        imore = iw.take(c, iu);
-      }
-    }
-    s = (s + 1 == kStages) ? 0 : s + 1;
-    if (++csrc == n) {
-      ar_store<16>(c, P.out, u, len, fw, acc, a);
-      csrc = 0;
-      more = walk.take(c, u);
-    }
-  }
-}
-
-// ld/st read side: for each unit, the n inputs one after another, kLdstVecs 16-byte loads in flight per lane each.
-template <uint32_t kLaneBytes>
-__device__ void ar_units_ldst(const Ctx& c, const AllReduceParams& P, uint64_t bytes, Walk<false> walk, uint64_t fw,
-                              Sum& a) {
-  uint64_t acc[kArWords];
-#pragma unroll
-  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
-  for (uint64_t u; walk.take(c, u);) {
-    const uint32_t len = unit_len(bytes, u);
-    for (uint32_t t = 0; t < P.n; ++t) {
-      const uint8_t* base = P.src[t] + u * kUnitBytes;
-      uint4 v[kLdstVecs];
-      if (len == kUnitBytes) {
-#pragma unroll
-        for (int i = 0; i < (int)kLdstVecs; ++i)
-          v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + ar_vec_off<kLaneBytes>(c.lane, i)));
-      } else {
-#pragma unroll
-        for (int i = 0; i < (int)kLdstVecs; ++i) {
-          v[i] = make_uint4(0u, 0u, 0u, 0u);
-          const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
-          if (off < len) v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + off));
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < (int)kLdstVecs; ++i) ar_add(acc, i, v[i]);
-    }
+// The one-shot's store policy (allreduce_path.cuh): a summed unit goes to the rank's own output, P.out.
+struct ToOut {
+  template <uint32_t kLaneBytes>
+  __device__ __forceinline__ static void put(const Ctx& c, const AllReduceParams& P, uint64_t u, uint32_t len,
+                                             uint64_t fw, uint64_t (&acc)[kArWords], Sum& a) {
     ar_store<kLaneBytes>(c, P.out, u, len, fw, acc, a);
   }
-}
+};
 
 // The untimed word check of the output the last rep of size k stored: each lane compares every 32nd word of its
 // warp's share with allreduce_word, reading at L2 (other SMs stored them).  One atomic pair per warp with a bad word.
@@ -202,9 +99,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_con
       const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
       Sum a{0ull, 0ull, 0ull};
       const Walk<false> walk = strided(bytes, gwarp, nwarps);
-      if (P.path == 2u) ar_units_ldst<32>(c, P, bytes, walk, fw, a);
-      else if (P.path == 1u) ar_units_ldst<16>(c, P, bytes, walk, fw, a);
-      else ar_units_tma(c, P, bytes, walk, fw, a);
+      ar_units<ToOut>(c, P, bytes, walk, fw, a);
       __threadfence();  // this warp's stores are performed before the CTA's completion stamp
       Acc* const acc = &bs->rep[k][r];
       cta_reduce<1>(c, red, &a, &acc);

@@ -1,0 +1,143 @@
+// allreduce_path.cuh — the read-and-add side of the all-reduce kernels, shared by allreduce_kernel (one-shot,
+// allreduce_kernels.cu) and allreduce_twoshot_kernel (allreduce_twoshot_kernels.cu): every warp walks 8 KiB output
+// units, streams unit u of all P.n inputs (TMA ring or ld.global.v4) and adds them in registers (64-bit, wrapping).
+// Two things are parameters: the walk (which units a warp sums) and the store policy (where a summed unit goes).
+//
+// A store policy S has one member, called once per unit by every lane with the unit's sums in acc:
+//   template <uint32_t kLaneBytes> static void S::put(const Ctx&, const Params& P, uint64_t u, uint32_t len,
+//                                                      uint64_t fw, uint64_t (&acc)[kArWords], Sum& a)
+// It stores the len bytes of unit u, lane vector i at ar_vec_off<kLaneBytes>(lane, i), and leaves acc all zero.  fw is
+// the word index of the armed fault (~0: none).
+//
+// Internal linkage, as datapath.cuh: each unit that includes this header compiles its own copy.
+#pragma once
+#include <stdint.h>
+
+#include "datapath.cuh"
+
+namespace cdp {
+namespace {
+constexpr int kArWords = 2 * kLdstVecs;  // uint64 accumulators per lane: a warp holds one 8 KiB output unit
+
+// Byte offset in a unit of the lane's 16-byte vector i when each access moves kLaneBytes contiguous bytes: the layout
+// job_read_ldst loads in, and for kLaneBytes = 16 also the one job_read_tma reads a stage in.
+template <uint32_t kLaneBytes>
+__device__ __forceinline__ uint32_t ar_vec_off(int lane, int i) {
+  constexpr int kV = kLaneBytes / 16;
+  return kLaneBytes * (uint32_t)lane + 32u * kLaneBytes * (uint32_t)(i / kV) + 16u * (uint32_t)(i % kV);
+}
+
+__device__ __forceinline__ void ar_add(uint64_t (&acc)[kArWords], int i, const uint4& v) {
+  acc[2 * i] += pack64(v.x, v.y);
+  acc[2 * i + 1] += pack64(v.z, v.w);
+}
+
+// TMA read side: the warp walks (unit, input) pairs, the n inputs of a unit in a row, through its kStages-deep ring of
+// bulk loads, one load per pair.  Each stage is added into the accumulators and then refilled with the next pair, so
+// the ring runs on across unit boundaries.  Aborted: stops issuing and drains what is in flight.
+template <typename Store, typename Params>
+__device__ void ar_units_tma(Ctx& c, const Params& P, uint64_t bytes, Walk<false> walk, uint64_t fw, Sum& a) {
+  const uint32_t n = P.n;
+  Walk<false> iw = walk;  // the issue side: up to kStages pairs ahead of the consume side, over the same pairs
+  uint64_t iu = 0;
+  bool imore = iw.take(c, iu);
+  uint32_t isrc = 0, in_flight = 0;
+  if (c.lane == 0) fence_proxy_async_global();  // data may have been written through the generic proxy
+#pragma unroll
+  for (int s = 0; s < kStages; ++s) {
+    if (!imore) break;
+    if (c.lane == 0) issue_load(c, P.src[isrc], bytes, iu, s);
+    ++in_flight;
+    if (++isrc == n) {
+      isrc = 0;
+      imore = iw.take(c, iu);
+    }
+  }
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  int s = 0;
+  uint32_t csrc = 0;
+  uint64_t u = 0;
+  bool more = walk.take(c, u);
+  while (more) {
+    if (!mbar_wait(c, s)) {
+      for (; in_flight > 0; --in_flight) {
+        mbar_drain(c, s);
+        s = (s + 1 == kStages) ? 0 : s + 1;
+      }
+      return;
+    }
+    --in_flight;
+    const uint32_t len = unit_len(bytes, u);
+    const uint32_t sbase = c.stage_smem + s * kUnitBytes;
+    if (len == kUnitBytes) {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    } else {
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i)
+        if (ar_vec_off<16>(c.lane, i) < len) ar_add(acc, i, lds_v4(sbase + ar_vec_off<16>(c.lane, i)));
+    }
+    __syncwarp();
+    if (imore) {
+      if (c.lane == 0) {
+        fence_proxy_async_smem();
+        issue_load(c, P.src[isrc], bytes, iu, s);
+      }
+      ++in_flight;
+      if (++isrc == n) {
+        isrc = 0;
+        imore = iw.take(c, iu);
+      }
+    }
+    s = (s + 1 == kStages) ? 0 : s + 1;
+    if (++csrc == n) {
+      Store::template put<16>(c, P, u, len, fw, acc, a);
+      csrc = 0;
+      more = walk.take(c, u);
+    }
+  }
+}
+
+// ld/st read side: for each unit, the n inputs one after another, kLdstVecs 16-byte loads in flight per lane each.
+template <uint32_t kLaneBytes, typename Store, typename Params>
+__device__ void ar_units_ldst(const Ctx& c, const Params& P, uint64_t bytes, Walk<false> walk, uint64_t fw, Sum& a) {
+  uint64_t acc[kArWords];
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  for (uint64_t u; walk.take(c, u);) {
+    const uint32_t len = unit_len(bytes, u);
+    for (uint32_t t = 0; t < P.n; ++t) {
+      const uint8_t* base = P.src[t] + u * kUnitBytes;
+      uint4 v[kLdstVecs];
+      if (len == kUnitBytes) {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i)
+          v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + ar_vec_off<kLaneBytes>(c.lane, i)));
+      } else {
+#pragma unroll
+        for (int i = 0; i < (int)kLdstVecs; ++i) {
+          v[i] = make_uint4(0u, 0u, 0u, 0u);
+          const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+          if (off < len) v[i] = ldg_stream_v4(reinterpret_cast<const uint4*>(base + off));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < (int)kLdstVecs; ++i) ar_add(acc, i, v[i]);
+    }
+    Store::template put<kLaneBytes>(c, P, u, len, fw, acc, a);
+  }
+}
+
+// The read side on the data path picked at run time (ProbeParams::path): 0 TMA bulk copies, 1 16-byte ld/st, 2 32-byte
+// ld/st.
+template <typename Store, typename Params>
+__device__ __forceinline__ void ar_units(Ctx& c, const Params& P, uint64_t bytes, Walk<false> walk, uint64_t fw,
+                                         Sum& a) {
+  if (P.path == 2u) ar_units_ldst<32, Store>(c, P, bytes, walk, fw, a);
+  else if (P.path == 1u) ar_units_ldst<16, Store>(c, P, bytes, walk, fw, a);
+  else ar_units_tma<Store>(c, P, bytes, walk, fw, a);
+}
+}  // namespace
+}  // namespace cdp

@@ -1,0 +1,130 @@
+// allreduce_twoshot_kernels.cu — sm_90a kernel of cdprobe_allreduce_twoshot's two-shot all-reduce: every rank sums its
+// chunk of units of all n source buffers with the one-shot's read-and-add side (allreduce_path.cuh) and pushes each
+// summed unit with st.global.v4 into every rank's gather area; a fenced domain barrier closes the rep, and every rank
+// then checks and clears its own gather area (allreduce_twoshot_kernel).
+//
+// probe_kernels.cu is untouched: the probe kernel's code generation does not depend on this file.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "allreduce_path.cuh"
+#include "allreduce_twoshot.h"
+
+namespace cdp {
+namespace {
+// The two-shot's store policy (allreduce_path.cuh): a summed unit goes to every rank's gather area, dst[0] (this
+// rank's own) first.  The armed fault (fw, an output word index; ~0 when none) acts on the stores to dst[fault_dst]
+// only: the word leaves xored with 1, or (fault_drop) nothing of its unit leaves.  Nothing is folded into (S, X); the
+// word check reads the output back.
+struct ToGather {
+  template <uint32_t kLaneBytes>
+  __device__ __forceinline__ static void put(const Ctx& c, const TwoShotParams& P, uint64_t u, uint32_t len,
+                                             uint64_t fw, uint64_t (&acc)[kArWords], Sum&) {
+    const uint32_t hit_dst = fw / (kUnitBytes / 8) == u ? P.fault_dst : ~0u;  // rare: this unit holds the armed word
+    const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
+    for (uint32_t t = 0; t < P.n; ++t) {
+      if (t == hit_dst && P.fault_drop) continue;
+      uint8_t* base = P.dst[t] + u * kUnitBytes;
+#pragma unroll
+      for (int i = 0; i < kArWords / 2; ++i) {
+        const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+        if (off >= len) continue;
+        uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
+        if (t == hit_dst && off == (fb & ~15u)) {
+          if (fb & 8u) w1 ^= 1ull;
+          else w0 ^= 1ull;
+        }
+        stg_v4(reinterpret_cast<uint4*>(base + off),
+               make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+  }
+};
+
+// The untimed check of rep r of size k: every word of this rank's output (its gather area) is read at L2 (peers and
+// other SMs stored it), compared with allreduce_word, folded into the rep's (S, X) by its place in the output, and
+// then overwritten with 0, so a unit that is not delivered in a later rep reads as 0s rather than as this rep's sums.
+// One atomic pair per warp with a bad word, over every rep of the size.
+__device__ void ts_check(const Ctx& c, const TwoShotParams& P, ArScratch* as, uint64_t* red, uint32_t k, uint32_t r,
+                         uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {
+  uint4* const out = reinterpret_cast<uint4*>(P.dst[0]);
+  Sum a{0ull, 0ull, 0ull};
+  uint64_t bad = 0, first = ~0ull;
+  Walk<false> walk = strided(bytes, gwarp, nwarps);
+  for (uint64_t u; walk.take(c, u);) {
+    uint4* const p = out + u * (kUnitBytes / 16);
+    const uint32_t nvec = unit_len(bytes, u) / 16;
+    const uint64_t w_base = u * (kUnitBytes / 8);
+    uint64_t ux = 0;
+#pragma unroll 4
+    for (uint32_t v = c.lane; v < nvec; v += 32) {
+      const uint4 q = __ldcg(p + v);
+      const uint64_t w0 = pack64(q.x, q.y), w1 = pack64(q.z, q.w), k0 = w_base + 2 * v;
+      if (w0 != allreduce_word(P.seed, P.n, k0)) {
+        ++bad;
+        first = min(first, 8 * k0);
+      }
+      if (w1 != allreduce_word(P.seed, P.n, k0 + 1)) {
+        ++bad;
+        first = min(first, 8 * k0 + 8);
+      }
+      add_pair(a, ux, w0, w1);
+      stg_v4(p + v, make_uint4(0u, 0u, 0u, 0u));
+    }
+    fold_unit(a, ux, u);
+  }
+  __threadfence();  // the clearing stores are performed before the next opening barrier signals the peers
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
+  Acc* const acc = &as->rep.rep[k][r];
+  cta_reduce<1>(c, red, &a, &acc);
+}
+}  // namespace
+
+// One rank of cdprobe_allreduce_twoshot: for every size of the ladder, one warm-up and P.reps timed reps.  A rep opens
+// with a domain barrier whose leader fences first (the previous check's clearing stores precede every peer's pushes),
+// sums this rank's chunk (twoshot_chunk) of all P.n inputs with every warp of the grid and pushes each summed unit to
+// every rank (ToGather).  Every CTA then passes a CTA barrier and issues one fence.sys, and a fenced domain barrier
+// closes the rep: its release, stamped into rep[k][r].t_end, is when this rank's output is complete, so the rep runs
+// from the opening release to the closing release.  The word check and clear follow, untimed (DESIGN §5i).  State
+// lives in the rank's scratch buffer; outside it, only the gather areas and the barrier lines are written.
+__global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(const __grid_constant__ TwoShotParams P) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  ArScratch* as = P.scratch;
+  BwScratch* bs = &as->rep;
+  uint64_t* red;
+  Ctx c = enter(smem, &bs->abort_flag, P.timeout_ns, &red);
+
+  const uint32_t gwarp = blockIdx.x * kWarpsPerCta + c.warp;
+  const uint32_t nwarps = gridDim.x * kWarpsPerCta;
+  uint32_t b = 0;
+  for (uint32_t k = 0; k < P.n_sizes; ++k) {
+    const uint64_t bytes = P.size[k];
+    uint64_t lo, hi;
+    twoshot_chunk(units_of(bytes), P.n, P.rank, &lo, &hi);
+    for (uint32_t r = 0; r <= P.reps; ++r) {
+      if (!grid_barrier(c, bs, b++, &bs->t_rel[k][r], &P.dom, true)) return;
+      const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
+      Sum a{0ull, 0ull, 0ull};
+      ar_units<ToGather>(c, P, bytes, Walk<false>{hi, lo + gwarp, 0ull, nwarps, nullptr}, fw, a);
+      __syncthreads();
+      if (threadIdx.x == 0) __threadfence_system();  // every store of this CTA has reached its gather area
+      if (!grid_barrier(c, bs, b++, &bs->rep[k][r].t_end, &P.dom, true)) return;
+      ts_check(c, P, as, red, k, r, bytes, gwarp, nwarps);
+    }
+  }
+}
+
+int allreduce_twoshot_launch(const TwoShotParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
+  const cudaError_t e =
+      cudaFuncSetAttribute(allreduce_twoshot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  return e != cudaSuccess ? (int)e : grid_launch(allreduce_twoshot_kernel, p, grid, cooperative, stream);
+}
+
+}  // namespace cdp

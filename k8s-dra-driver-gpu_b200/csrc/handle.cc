@@ -253,21 +253,21 @@ static int gather_status(cdprobe* h, int32_t (*st)[kMaxRanks]) {
   return CDPROBE_OK;
 }
 
-int ensure_area(cdprobe* h) {
-  if (h->area.bytes != 0) return CDPROBE_OK;
-  const size_t bytes = ((size_t)h->n_total * h->plan.bpp + kVmmGranule - 1) / kVmmGranule * kVmmGranule;
+int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*status)[kMaxRanks]) {
+  if (m.bytes != 0) return CDPROBE_OK;
+  bytes = (bytes + kVmmGranule - 1) / kVmmGranule * kVmmGranule;
   int32_t st[kMaxRanks][kMaxRanks] = {};
   for (uint32_t li = 0; li < h->n_local; ++li)
     for (uint32_t j = 0; j < h->n_total; ++j) st[h->lr[li].grank][j] = cell_status(h, li, j);
-  int rc = share_alloc(h, h->area, bytes, st, true);
+  int rc = share_alloc(h, m, bytes, st, true);
   if (rc == CDPROBE_OK) rc = gather_status(h, st);
   if (rc != CDPROBE_OK) {
     const std::string keep = g_last_error;
-    release_shared(h, h->area);
+    release_shared(h, m);
     g_last_error = keep;
     return rc;
   }
-  memcpy(h->area_status, st, sizeof(st));
+  memcpy(status, st, sizeof(st));
   return CDPROBE_OK;
 }
 
@@ -478,6 +478,7 @@ static void destroy(cdprobe* h) {
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
   }
+  release_shared(h, h->gather);
   release_shared(h, h->area);
   release_shared(h, h->mem);
   for (uint32_t li = 0; li < h->n_local; ++li) {
@@ -1068,6 +1069,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return CDPROBE_OK;
     case CDPROBE_OPT_ALLTOALL_FAULT:  // checked against the domain and the size ladder by cdprobe_alltoall
       h->a2a_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT:  // checked against the domain and the ladder by cdprobe_allreduce_twoshot
+      h->ar2_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

@@ -1,5 +1,5 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
-// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce and cdprobe_alltoall.  Each runs on the local ranks' own streams,
+// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot and cdprobe_alltoall.  Each runs on the local ranks' own streams,
 // between probe runs, and has its results on the host before it returns.
 #include <string.h>
 
@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "allreduce.h"
+#include "allreduce_twoshot.h"
 #include "alltoall.h"
 #include "atomics.h"
 #include "bwcurve.h"
@@ -309,6 +310,41 @@ static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const uint64_t* si
   cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(*p.scratch), L.stream);
   if (e == cudaSuccess) e = (cudaError_t)launch(p, L.ctas, launch_cooperatively(h, L), L.stream);
   return e != cudaSuccess ? fail_sticky(h, what, e) : CDPROBE_OK;
+}
+
+// The skip rule of the all-reduces, on the domain's mapping status st ([rank][rank], 0: up): a process that ran while
+// another skipped would wait at the first domain barrier until its watchdog fired, so when some rank cannot reach some
+// other nothing runs, in any process: every local row gets the status of the domain's first down cell, row-major.
+// Returns whether the call skips.
+static bool skip_rows(const cdprobe* h, int32_t (*st)[kMaxRanks], cdprobe_allreduce_t* out) {
+  const int32_t* down = std::find_if(&st[0][0], &st[0][0] + kMaxRanks * kMaxRanks, [](int32_t s) { return s != 0; });
+  if (down == &st[0][0] + kMaxRanks * kMaxRanks) return false;
+  for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = *down;
+  return true;
+}
+
+// Collects the rows of the all-reduces once their kernels are done: per local row, the times and every rep's (S, X)
+// against want (bw_summarize), then the word checks of every size.
+static int collect_rows(cdprobe* h, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes, uint32_t reps,
+                        const char* what, cdprobe_allreduce_t* out) {
+  auto got = std::make_unique<ArScratch>();
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    if (const int rc = fetch_reps(h, L, got.get(), 1, what); rc != CDPROBE_OK) return rc;
+    const ArScratch& s = *got;
+    bw_summarize(s.rep, want, size, n_sizes, reps, g, out);
+    if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
+    for (uint32_t k = 0; k < n_sizes; ++k) {
+      out->bad_words[g][k] = s.bad_words[k];
+      out->first_bad[g][k] = s.bad_words[k] != 0 ? ~s.first_bad_n[k] : UINT64_MAX;
+      if (s.bad_words[k] != 0) {
+        out->bad_sizes[g] |= 1u << k;
+        out->status[g] = CDPROBE_ERR_INTEGRITY;
+      }
+    }
+  }
+  return CDPROBE_OK;
 }
 
 }  // namespace cdp
@@ -761,12 +797,8 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
     return rc;
   out->call_seq = ++h->ar_calls;
   cdp::put_ladder(h, size, n_sizes, out);
-  // a process that ran while another skipped would wait at the first domain barrier until its watchdog fired, so
-  // when some rank cannot read some input nothing runs, in any process: every row gets the domain's first down cell
-  const int32_t* down = std::find_if(&st[0][0], &st[0][0] + cdp::kMaxRanks * cdp::kMaxRanks,
-                                     [](int32_t s) { return s != 0; });
-  if (down != &st[0][0] + cdp::kMaxRanks * cdp::kMaxRanks) {
-    for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = *down;
+  // when some rank cannot read some input nothing runs, in any process
+  if (cdp::skip_rows(h, st, out)) {
     out->ms = cdp::now_ms() - t_begin;
     return CDPROBE_OK;
   }
@@ -811,23 +843,110 @@ int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   }
 
   // 5. collect: per row, the times and checksums of every size, then the word checks
-  auto got = std::make_unique<cdp::ArScratch>();
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_allreduce"); rc != CDPROBE_OK) return rc;
-    const cdp::ArScratch& s = *got;
-    cdp::bw_summarize(s.rep, want, size, n_sizes, reps, g, out);
-    if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
-    for (uint32_t k = 0; k < n_sizes; ++k) {
-      out->bad_words[g][k] = s.bad_words[k];
-      out->first_bad[g][k] = s.bad_words[k] != 0 ? ~s.first_bad_n[k] : UINT64_MAX;
-      if (s.bad_words[k] != 0) {
-        out->bad_sizes[g] |= 1u << k;
-        out->status[g] = CDPROBE_ERR_INTEGRITY;
+  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce", out); rc != CDPROBE_OK)
+    return rc;
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
+  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  out->path = h->path;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
+  //    every process refuses, skips or runs together.  The fault acts in the rank whose chunk holds its word
+  uint64_t size[cdp::kBwMaxSizes];
+  uint32_t n_sizes;
+  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
+  uint32_t f_owner = cdp::kArNoFault, f_recv = 0, f_k = cdp::kArNoFault, f_drop = 0;
+  uint64_t f_word = 0;
+  if (h->ar2_fault != 0 && bad.empty()) {
+    const uint64_t v = h->ar2_fault, fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu;
+    f_word = v & 0xffffffu;
+    if ((v >> 49) != 0 || fr == 0 || fr > n || fk == 0 || fk > n_sizes || f_word >= size[fk - 1] / 8) {
+      bad = "the armed two-shot all-reduce fault names no receiver, size or output word of this call";
+    } else {
+      f_recv = (uint32_t)fr - 1;
+      f_k = (uint32_t)fk - 1;
+      f_drop = (uint32_t)(v >> 48);
+      const uint64_t units = (size[f_k] + cdp::kUnitBytes - 1) / cdp::kUnitBytes, u = f_word / (cdp::kUnitBytes / 8);
+      for (uint32_t r = 0; r < n; ++r) {
+        uint64_t lo, hi;
+        cdp::twoshot_chunk(units, n, r, &lo, &hi);
+        if (u >= lo && u < hi) f_owner = r;
       }
     }
   }
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_allreduce_twoshot", bad, h->ar2_calls + 1, {reps, 0u, 0u}, st);
+      rc != CDPROBE_OK)
+    return rc;
+  // 2. the gather area, built once, by every process in the same call
+  if (const int rc = cdp::ensure_area(h, h->gather, pl.bpp, h->gather_status); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++h->ar2_calls;
+  cdp::put_ladder(h, size, n_sizes, out);
+  // 3. every rank reads every source buffer and writes every gather area: when some probe mapping or gather-area
+  //    mapping of the domain is down, nothing runs, in any process
+  for (uint32_t s = 0; s < n; ++s)
+    for (uint32_t d = 0; d < n; ++d)
+      if (st[s][d] == 0) st[s][d] = h->gather_status[s][d];
+  if (cdp::skip_rows(h, st, out)) {
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 4. scratch for the records and the granule table, grown on every local rank before any kernel runs; the (S, X)
+  //    every prefix of the output must have, as for the one-shot
+  const size_t table_off = cdp::kArOutOff;
+  if (const int rc = cdp::ensure_scratch_all(h, table_off + 16 * (pl.bpp / cdp::kGranuleBytes)); rc != CDPROBE_OK)
+    return rc;
+  uint64_t want[cdp::kBwMaxSizes][2] = {};
+  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
+                                        "cdprobe_allreduce_twoshot: granule checksums");
+      rc != CDPROBE_OK)
+    return rc;
+
+  // 5. no process launches before every process is ready; then every local kernel is launched before any is waited for
+  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::TwoShotParams p;
+    memset(&p, 0, sizeof(p));
+    for (uint32_t t = 0; t < n; ++t) {
+      p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + pl.src_off;
+      p.dst[t] = reinterpret_cast<uint8_t*>(L.gather_va[(g + t) % n]);
+    }
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g) continue;
+      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kAr2Off + (uint64_t)g * sizeof(cdp::FlagLine));
+      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kAr2Off + (uint64_t)j * sizeof(cdp::FlagLine));
+    }
+    p.dom.call_seq = h->ar2_calls;
+    p.seed = h->seed;
+    p.fault_k = g == f_owner ? f_k : cdp::kArNoFault;
+    p.fault_word = f_word;
+    p.fault_dst = (f_recv + n - g) % n;
+    p.fault_drop = f_drop;
+    p.rank = g;
+    p.n = n;
+    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_twoshot_launch,
+                                          "launch allreduce_twoshot_kernel");
+        rc != CDPROBE_OK)
+      return rc;
+  }
+
+  // 6. collect: per row, the times and every rep's checksums, then the word checks of every rep
+  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce_twoshot", out);
+      rc != CDPROBE_OK)
+    return rc;
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }
@@ -866,7 +985,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   if (const int rc = cdp::agree(h, "cdprobe_alltoall", bad, h->a2a_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
     return rc;
   // 2. the exchange area, built once, by every process in the same call
-  if (const int rc = cdp::ensure_area(h); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp, h->area_status); rc != CDPROBE_OK) return rc;
   out->call_seq = ++h->a2a_calls;
   out->area_bytes = h->area.bytes;
   cdp::put_ladder(h, size, n_sizes, out);

@@ -504,6 +504,20 @@ static_assert(kA2aOff % 128 == 0 && kA2aOff + kMaxRanks * sizeof(FlagLine) <= kC
               "the all-to-all lines sit after the all-reduce lines inside the Ctrl granule");
 static_assert(kBwMaxSizes * (64 + 1) * 2 < (1u << kArBarrierBits), "all-to-all barriers per call fit the low bits");
 
+// ---- the two-shot all-reduce (cdprobe_allreduce_twoshot, DESIGN §5i) -----------------------------------------------
+// The units rank r of n reduces in a prefix of `units` 8 KiB units: [*lo, *hi) = [floor(r units / n),
+// floor((r + 1) units / n)).  The chunks of the n ranks cover every unit once; with units < n some are empty.
+CDP_HD inline void twoshot_chunk(uint64_t units, uint32_t n, uint32_t r, uint64_t* lo, uint64_t* hi) {
+  *lo = units * r / n;
+  *hi = units * (r + 1) / n;
+}
+
+// The domain barrier of cdprobe_allreduce_twoshot: one 128-byte line per sender after the all-to-all lines, in the
+// Ctrl granule.  Same rules as kArOff; two barriers per rep, as the all-to-all's.
+constexpr uint64_t kAr2Off = kA2aOff + kMaxRanks * sizeof(FlagLine);  // 72 KiB
+static_assert(kAr2Off % 128 == 0 && kAr2Off + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the two-shot all-reduce lines sit after the all-to-all lines inside the Ctrl granule");
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -633,6 +633,22 @@ class Probe:
         rc = self._lib.cdprobe_allreduce(self._h, reps, C.byref(t))
         return rc, t
 
+    def AllReduceTwoShot(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReduceTwoShot.  Two-shot all-reduce (reduce-scatter, then a pushed all-gather) of every
+        rank's source buffer on every rank at once, at each size of the bwcurve ladder, on the probe's read path and
+        grid (0: 8 timed reps per size).  The result is an AllReduce whose bad_words and first_bad cover every rep;
+        the nccl-tests bus bandwidth is peak_gbps x 2 (n - 1) / n.  Collective when world_size > 1.  Needs no Run first
+        and disturbs none."""
+        rc, t = self.allreduce_twoshot_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce_twoshot")
+        return AllReduce.from_c(t)
+
+    def allreduce_twoshot_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce_twoshot(self._h, reps, C.byref(t))
+        return rc, t
+
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps

@@ -6,7 +6,13 @@ timed reps), the algorithm bandwidth of the median (size / ns) and the summary t
 Every row's checksums and words are checked by the library (status 0).  Sizes up to the 50 MB L2 come from L2 after
 the warm-up rep, larger ones from HBM.  With N ranks each rank's NVLink ingress is (n - 1) x the algorithm bandwidth;
 NVLink needs two GPUs and is not measured here.  Prints a table, then one JSON document with the card's name, power
-limit and SM clock read in the same call (read-only query); --out also writes the document to a file."""
+limit and SM clock read in the same call (read-only query); --out also writes the document to a file.
+
+--twoshot adds cdprobe_allreduce_twoshot in the same session: at N = 1 on each path next to the one-shot (the rank owns
+every unit, so a rep is the one-shot's reads plus a store to its own gather area and the untimed check), and with 2 and
+4 ranks sharing GPU 0 (`--multi-bytes` per rank) on the TMA path.  Each rank's link traffic in a two-shot rep is
+2 (n - 1) / n x size, so its bus bandwidth, busbw = algbw x 2 (n - 1) / n, is the figure nccl-tests reports; ranks on
+one device move that traffic through its own HBM, not NVLink."""
 import argparse
 import json
 import os
@@ -22,6 +28,8 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--bytes", type=int, default=1 << 30)
 ap.add_argument("--reps", type=int, default=16)
 ap.add_argument("--out", default=None, help="also write the JSON document to this file")
+ap.add_argument("--twoshot", action="store_true", help="also measure cdprobe_allreduce_twoshot")
+ap.add_argument("--multi-bytes", type=int, default=256 << 20, help="bytes_per_pair of the 2- and 4-rank two-shot runs")
 a = ap.parse_args()
 
 
@@ -32,15 +40,19 @@ def gpu():
     return dict(zip(q.split(","), [x.strip() for x in out.split(",")]))
 
 
-def rows(ar):
+def rows(ar, bus=None):
+    """Per rank: the summary and every size; bus: also busbw_gbps_median = algbw x bus."""
     out = {}
     for r in range(ar.n):
         assert ar.measured[r] and ar.status[r] == 0 and ar.bad_sizes[r] == 0, (r, ar.status[r])
         assert all(b == 0 for b in ar.bad_words[r]), r
         out[f"rank_{r}"] = {
             "t0_ns": ar.t0_ns[r], "peak_gbps": ar.peak_gbps[r], "half_bytes": ar.half_bytes[r],
-            "sizes": [{"bytes": s, "ns_min": lo, "ns_median": med, "ns_max": hi, "algbw_gbps_median": s / med}
+            "sizes": [{"bytes": s, "ns_min": lo, "ns_median": med, "ns_max": hi, "algbw_gbps_median": s / med,
+                       **({} if bus is None else {"busbw_gbps_median": s / med * bus})}
                       for s, lo, med, hi in zip(ar.sizes, ar.ns_min[r], ar.ns_median[r], ar.ns_max[r])]}
+        if bus is not None:
+            out[f"rank_{r}"]["peak_busbw_gbps"] = ar.peak_gbps[r] * bus
     return out
 
 
@@ -54,6 +66,22 @@ for path, name in enumerate(("tma", "ldst16", "ldst32")):
         p.SetOption(pkg.abi.OPT_PATH, path)
         ar = p.AllReduce(a.reps)
         res[f"n1_{name}"] = {**rows(ar), "call_ms": ar.ms}
+        if a.twoshot:
+            ts = p.AllReduceTwoShot(a.reps)
+            res[f"twoshot_n1_{name}"] = {**rows(ts, 0.0), "call_ms": ts.ms}
+if a.twoshot:
+    res["twoshot_what"] = ("the same for the two-shot all-reduce (cdprobe_allreduce_twoshot): a rep runs from the "
+                           "rank's opening domain-barrier release to its closing release, after every rank's pushes; "
+                           "busbw_gbps_median = algbw x 2 (n - 1) / n.  twoshot_n2 / twoshot_n4: 2 and 4 ranks on "
+                           "GPU 0 (ALLOW_SAME_DEVICE | NO_COOPERATIVE, 32 CTAs each, TMA path), bytes_per_pair = "
+                           "multi_bytes; their traffic stays in that GPU's HBM")
+    res["multi_bytes"] = a.multi_bytes
+    for n in (2, 4):
+        cfg = pkg.Config(ordinals=[0] * n, bytes=a.multi_bytes * (n - 1), flags=0x40 | 0x10, ctas=32,
+                         timeout_ms=20000)
+        with pkg.Open(cfg) as p:
+            ts = p.AllReduceTwoShot(a.reps)
+            res[f"twoshot_n{n}"] = {**rows(ts, 2 * (n - 1) / n), "call_ms": ts.ms}
 res["gpu"] = gpu()
 res["nvlink"] = "not measured (one GPU)"
 
@@ -62,6 +90,15 @@ for name in ("tma", "ldst16", "ldst32"):
     for s in res[f"n1_{name}"]["rank_0"]["sizes"]:
         print(f"{name:8} {s['bytes']:12d} {s['ns_min']:12.0f} {s['ns_median']:12.0f} {s['ns_max']:12.0f} "
               f"{s['algbw_gbps_median']:11.1f}")
+if a.twoshot:
+    print(f"\n{'two-shot':12} {'rank':>4} {'bytes':>12} {'ns_median':>12} {'algbw GB/s':>11} {'busbw GB/s':>11}")
+    for key in [f"twoshot_n1_{x}" for x in ("tma", "ldst16", "ldst32")] + ["twoshot_n2", "twoshot_n4"]:
+        for rk, row in res[key].items():
+            if not rk.startswith("rank_"):
+                continue
+            for s in row["sizes"]:
+                print(f"{key[8:]:12} {rk[5:]:>4} {s['bytes']:12d} {s['ns_median']:12.0f} "
+                      f"{s['algbw_gbps_median']:11.1f} {s['busbw_gbps_median']:11.1f}")
 print(f"gpu: {res['gpu']}")
 if a.out:
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
