@@ -402,9 +402,11 @@ typedef struct {
   uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
   uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
   uint32_t n_sizes;                     /* entries of size[] */
-  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH) */
+  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH); cdprobe_allreduce_ll has one
+                                           data path, ignores CDPROBE_OPT_PATH and reports CDPROBE_ALLREDUCE_PATH_LL */
   uint64_t call_seq;                    /* 1-based count of cdprobe_allreduce calls on this handle, equal in every
-                                           process (0 when the call was refused) */
+                                           process (0 when the call was refused); of cdprobe_allreduce_twoshot or
+                                           cdprobe_allreduce_ll calls for those */
   uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per input and of the output per rep: the cdprobe_bwcurve ladder */
   uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank ran */
   int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) or the word check differs from
@@ -428,6 +430,8 @@ typedef struct {
                                                                       clean */
   double ms;                            /* host wall clock of the call */
 } cdprobe_allreduce_t;
+/* cdprobe_allreduce_t.path of cdprobe_allreduce_ll: flag-carrying 16-byte packets (DESIGN §5j) */
+#define CDPROBE_ALLREDUCE_PATH_LL 3u
 
 /* One-shot all-to-all across the domain (cdprobe_alltoall): every rank pushes one block to every peer at once, into the
  * peer's exchange area, and every rank checks every word it receives (DESIGN §5h).  Per-rank entries [r] describe rank
@@ -498,10 +502,12 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *                                                                   cmd/compute-domain-kubelet-plugin/driver.go:165-232
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
- *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_alltoall:
+ *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_alltoall:
  *   diagnostics, benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
- *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce and
- *   cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works without.
+ *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll and cdprobe_alltoall are optional for callers: a daemon binds
+ *   them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -555,6 +561,13 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              (< 2^24), that rank stores the word into receiver's output xored with 1
                                              (drop 0), or skips every store of the word's 8 KiB unit into receiver
                                              (drop 1), so exactly that row and size fail; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_LL_FAULT 22u /* tests: value = (mode << 48) | ((sender + 1) << 40) | ((receiver + 1)
+                                             << 32) | ((k + 1) << 24) | arg arms a fault in cdprobe_allreduce_ll, in
+                                             timed rep 1 of size[k], in the process that hosts `sender`: mode 0, the
+                                             packet of word `arg` (< 2^24) from sender to receiver (!= sender) carries
+                                             its data xored with 1 and the right flags, so exactly that receiver's row
+                                             fails at that size; mode 1, the sender waits `arg` us (< timeout_ms / 2)
+                                             before its first push of the rep, and every row stays exact; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -704,6 +717,34 @@ CDPROBE_API int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t
  * CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT whose receiver is >= n, whose k is >= n_sizes, whose word is >= size[k] / 8 or
  * that has a bit above 48 set; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* Low-latency ("LL") all-reduce of every rank's source buffer, on every rank at once: no barrier and no fence per
+ * rep.  For each size of the LL ladder (the cdprobe_bwcurve ladder's sizes of at most 1 MiB; it ends at 1 MiB when
+ * bytes_per_pair is larger), one domain barrier (flags in the Ctrl granule; a grid barrier only at n == 1), then one
+ * untimed warm-up rep and `reps` timed reps back to back.  In a rep every 64-bit input word of rank r travels to every
+ * peer, r + 1, r + 2, ... (mod n), as one 16-byte packet (st.relaxed.sys.v2.u64) of two 8-byte elements, each 32 bits
+ * of data and the rep's 32-bit flag, into the peer's LL area; each rank polls its own area (ld.relaxed.sys.v2.u64)
+ * until both flags of every packet are the rep's, adds the packets to its own input and stores the sum into its
+ * output.  Rank j's input in a rep is its source word plus a per-rank, per-rep salt, subtracted again from the sum, so
+ * a packet of another rep that were accepted would leave a wrong word.  Every rank splits the words alike, over the
+ * warps of the domain's smallest grid.  A rep is timed per rank by %globaltimer from the end of that rank's previous
+ * rep (the warm-up: from the barrier release) to the moment its output is complete, the per-iteration figure
+ * nccl-tests reports.  Row r of *out is as cdprobe_allreduce's: every rep's (S, X) and the word check of the last rep;
+ * peak_gbps is the algorithm bandwidth, size / ns, and each rank's link ingress per rep is 2 (n - 1) x size (every 8
+ * bytes of data travel in a 16-byte packet).  The LL area (2 x n x 2 x the ladder's largest size per rank, rounded up
+ * to 2 MiB) is created on the first call with the probe allocation's handle type, zeroed, mapped wherever the probe
+ * mapping is then up, and kept until close; if creating it fails in any process, every process returns that error,
+ * nothing runs, and the next call tries again.  If any probe or LL-area mapping of the domain is down
+ * (cdprobe_unmap_peer, a failed mapping, MIG), nothing runs: every filled row has measured = 0 and the status of the
+ * first such cell, and the call returns CDPROBE_OK.  A rank whose kernel passes timeout_ms is CDPROBE_ERR_TIMEOUT
+ * with no times, the handle stays usable, and every LL area is zeroed before the next call runs.  Collective when
+ * world_size > 1: every process calls it with the same reps and fills the rows of its own ranks (row_mask); call_seq
+ * counts calls of this function.  Needs no run first and touches no result, pattern, source buffer, landing slot,
+ * run_seq, warm-up state, exchange or gather area or other measurement's state.  *out carries abi, n, reps and path
+ * whatever the return code.  CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments that
+ * differ between processes, or an armed CDPROBE_OPT_ALLREDUCE_LL_FAULT whose sender or receiver is >= n, whose k is
+ * >= n_sizes, whose mode is above 1, whose mode-0 receiver is its sender or word is >= size[k] / 8, or whose mode-1
+ * delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -48,6 +48,7 @@ static bw_fn cdp_bw;      // optional: absent from libraries that predate cdprob
 static ar_fn cdp_ar;      // optional: absent from libraries that predate cdprobe_allreduce
 static a2a_fn cdp_a2a;    // optional: absent from libraries that predate cdprobe_alltoall
 static ar_fn cdp_ar2;     // optional: absent from libraries that predate cdprobe_allreduce_twoshot
+static ar_fn cdp_arll;    // optional: absent from libraries that predate cdprobe_allreduce_ll
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -67,6 +68,7 @@ static int cdp_load(const char* path) {
   cdp_ar = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce");
   cdp_a2a = (a2a_fn)dlsym(cdp_dl, "cdprobe_alltoall");
   cdp_ar2 = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_twoshot");
+  cdp_arll = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ll");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -101,6 +103,8 @@ static int cdp_has_allreduce_twoshot(void) { return cdp_ar2 != NULL; }
 static int cdp_call_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
   return cdp_ar2(h, reps, ar);
 }
+static int cdp_has_allreduce_ll(void) { return cdp_arll != NULL; }
+static int cdp_call_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) { return cdp_arll(h, reps, ar); }
 */
 import "C"
 
@@ -272,7 +276,8 @@ type BwCurve struct {
 	Ms                     float64
 }
 
-// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot).
+// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot)
+// or the low-latency one's (AllReduceLL).
 // Every slice is indexed by rank; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
 // rank was not measured or timed out.
 type AllReduce struct {
@@ -681,6 +686,31 @@ func (p *Probe) AllReduceTwoShot(reps int) (AllReduce, error) {
 		return AllReduce{}, err
 	}
 	return allReduceOf(ar), nil
+}
+
+// AllReduceLL runs the low-latency all-reduce of every rank's source buffer on every rank at once: every input word
+// travels to every peer in a flag-carrying 16-byte packet, with no barrier or fence per rep, at each size of the LL
+// ladder (the bwcurve ladder up to 1 MiB), and reports ns per rep for each size (reps 0: 8 timed reps), timed from
+// the end of the rank's previous rep.  Path is CDPROBE_ALLREDUCE_PATH_LL.  Collective when the domain spans processes.
+// ErrUnsupported when the library predates cdprobe_allreduce_ll.
+func (p *Probe) AllReduceLL(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce_ll() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce_ll", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	ar := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce_ll(p.h, C.uint32_t(reps), ar)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce_ll: %s: %s", C.GoString(C.cdp_call_strerror(rc)),
+			C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	ll := allReduceOf(ar)
+	return ll, nil
 }
 
 // allReduceOf copies a cdprobe_allreduce_t into an AllReduce.

@@ -182,5 +182,6 @@ func (*Probe) Atomics(int, int, int) (Atomics, error) { return Atomics{}, ErrUns
 func (*Probe) BwCurve(int) (BwCurve, error) { return BwCurve{}, ErrUnsupported }
 func (*Probe) AllReduce(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceTwoShot(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllReduceLL(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -37,6 +37,7 @@ OPT_ATOMICS_FAULT = 18
 OPT_ALLREDUCE_FAULT = 19
 OPT_ALLTOALL_FAULT = 20
 OPT_ALLREDUCE_TWOSHOT_FAULT = 21
+OPT_ALLREDUCE_LL_FAULT = 22
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -56,6 +57,7 @@ ATOMICS_MAX_OPS, ATOMICS_MAX_REPS = 1 << 16, 64
 BWCURVE_MAX_SIZES = 24
 BWCURVE_DEFAULT_REPS, BWCURVE_MAX_REPS = 8, 64
 ALLREDUCE_DEFAULT_REPS, ALLREDUCE_MAX_REPS = 8, 64
+ALLREDUCE_PATH_LL = 3  # cdprobe_allreduce_t.path of cdprobe_allreduce_ll
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
@@ -405,6 +407,15 @@ def allreduce_twoshot_fault(receiver: int, k: int, word: int, drop: bool = False
     return ((1 if drop else 0) << 48) | ((receiver + 1) << 32) | ((k + 1) << 24) | word
 
 
+def allreduce_ll_fault(sender: int, receiver: int, k: int, arg: int, mode: int = 0) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_LL_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_ll: mode 0, the packet
+    of word `arg` from `sender` to `receiver` carries its data xored with 1; mode 1, `sender` waits `arg` us before its
+    first push (`receiver` must still name a rank).  Fields that do not fit are refused here."""
+    if mode not in (0, 1) or not (0 <= sender < 255 and 0 <= receiver < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
+        raise ValueError("allreduce_ll_fault: mode 0 or 1, ranks and k below 255, arg below 2^24")
+    return (mode << 48) | ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | arg
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -441,6 +452,7 @@ SYMBOLS = {
     "cdprobe_bwcurve": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(BwCurveT)]),
     "cdprobe_allreduce": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_twoshot": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
+    "cdprobe_allreduce_ll": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

@@ -53,27 +53,6 @@ struct ToOut {
     ar_store<kLaneBytes>(c, P.out, u, len, fw, acc, a);
   }
 };
-
-// The untimed word check of the output the last rep of size k stored: each lane compares every 32nd word of its
-// warp's share with allreduce_word, reading at L2 (other SMs stored them).  One atomic pair per warp with a bad word.
-__device__ void ar_check(const Ctx& c, const AllReduceParams& P, ArScratch* as, uint32_t k, uint64_t bytes,
-                         uint32_t gwarp, uint32_t nwarps) {
-  const unsigned long long* out = reinterpret_cast<const unsigned long long*>(P.out);
-  const uint64_t words = bytes / 8;
-  uint64_t bad = 0, first = ~0ull;
-  for (uint64_t w = (uint64_t)gwarp * 32u + (uint32_t)c.lane; w < words; w += (uint64_t)nwarps * 32u) {
-    if (__ldcg(out + w) != allreduce_word(P.seed, P.n, w)) {
-      ++bad;
-      first = min(first, w * 8u);
-    }
-  }
-  bad = warp_sum64(bad);
-  first = warp_min64(first);
-  if (c.lane == 0 && bad != 0) {
-    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
-    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
-  }
-}
 }  // namespace
 
 // One rank of cdprobe_allreduce: for every size of the ladder, one warm-up and P.reps timed reps, each summing the

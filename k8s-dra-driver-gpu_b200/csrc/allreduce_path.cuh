@@ -2,6 +2,8 @@
 // allreduce_kernels.cu) and allreduce_twoshot_kernel (allreduce_twoshot_kernels.cu): every warp walks 8 KiB output
 // units, streams unit u of all P.n inputs (TMA ring or ld.global.v4) and adds them in registers (64-bit, wrapping).
 // Two things are parameters: the walk (which units a warp sums) and the store policy (where a summed unit goes).
+// Also the word check of an output in the rank's scratch (ar_check), shared by the one-shot and allreduce_ll_kernel
+// (allreduce_ll_kernels.cu).
 //
 // A store policy S has one member, called once per unit by every lane with the unit's sums in acc:
 //   template <uint32_t kLaneBytes> static void S::put(const Ctx&, const Params& P, uint64_t u, uint32_t len,
@@ -13,6 +15,7 @@
 #pragma once
 #include <stdint.h>
 
+#include "allreduce.h"
 #include "datapath.cuh"
 
 namespace cdp {
@@ -138,6 +141,29 @@ __device__ __forceinline__ void ar_units(Ctx& c, const Params& P, uint64_t bytes
   if (P.path == 2u) ar_units_ldst<32, Store>(c, P, bytes, walk, fw, a);
   else if (P.path == 1u) ar_units_ldst<16, Store>(c, P, bytes, walk, fw, a);
   else ar_units_tma<Store>(c, P, bytes, walk, fw, a);
+}
+
+// The untimed word check of the output the last rep of size k stored at P.out (allreduce_kernel and
+// allreduce_ll_kernel): each lane compares every 32nd word of its warp's share with allreduce_word, reading at L2
+// (other SMs stored them).  One atomic pair per warp with a bad word.
+template <typename Params>
+__device__ void ar_check(const Ctx& c, const Params& P, ArScratch* as, uint32_t k, uint64_t bytes, uint32_t gwarp,
+                         uint32_t nwarps) {
+  const unsigned long long* out = reinterpret_cast<const unsigned long long*>(P.out);
+  const uint64_t words = bytes / 8;
+  uint64_t bad = 0, first = ~0ull;
+  for (uint64_t w = (uint64_t)gwarp * 32u + (uint32_t)c.lane; w < words; w += (uint64_t)nwarps * 32u) {
+    if (__ldcg(out + w) != allreduce_word(P.seed, P.n, w)) {
+      ++bad;
+      first = min(first, w * 8u);
+    }
+  }
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
 }
 }  // namespace
 }  // namespace cdp

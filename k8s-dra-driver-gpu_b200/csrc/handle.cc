@@ -478,6 +478,7 @@ static void destroy(cdprobe* h) {
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
   }
+  release_shared(h, h->ll);
   release_shared(h, h->gather);
   release_shared(h, h->area);
   release_shared(h, h->mem);
@@ -1072,6 +1073,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return CDPROBE_OK;
     case CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT:  // checked against the domain and the ladder by cdprobe_allreduce_twoshot
       h->ar2_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_LL_FAULT:  // checked against the domain, the ladder and timeout_ms by cdprobe_allreduce_ll
+      h->ll_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

@@ -44,6 +44,8 @@ struct LocalRank {
   bool area_mapped[kMaxRanks] = {};
   CUdeviceptr gather_va[kMaxRanks] = {};  // rank j's gather area (cdprobe_allreduce_twoshot) as mapped here
   bool gather_mapped[kMaxRanks] = {};
+  CUdeviceptr ll_va[kMaxRanks] = {};  // rank j's LL area (cdprobe_allreduce_ll) as mapped here
+  bool ll_mapped[kMaxRanks] = {};
   ResultRow* row = nullptr;
   char uuid[48] = {};
   Phase phases[kMaxPhases];
@@ -55,8 +57,8 @@ struct LocalRank {
 
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
 // exports them, takes the other processes' over the rendezvous, imports them and maps every rank's into every local
-// rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area and
-// cdprobe_allreduce_twoshot's gather area are others.
+// rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area,
+// cdprobe_allreduce_twoshot's gather area and cdprobe_allreduce_ll's LL area are others.
 struct SharedAlloc {
   size_t bytes = 0;                                       // of each allocation; 0: not created
   CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
@@ -84,9 +86,11 @@ struct cdprobe {
   cdp::SharedAlloc mem{&cdp::LocalRank::va, &cdp::LocalRank::mapped};             // the probe allocation
   cdp::SharedAlloc area{&cdp::LocalRank::area_va, &cdp::LocalRank::area_mapped};  // cdprobe_alltoall's exchange area
   cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};  // the two-shot's gather area
+  cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};  // cdprobe_allreduce_ll's LL area
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
   int32_t area_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the exchange area, once it exists
   int32_t gather_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the gather area, once it exists
+  int32_t ll_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the LL area, once it exists
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
   uint64_t seed = 0;
@@ -116,6 +120,9 @@ struct cdprobe {
   uint64_t a2a_fault = 0;     // CDPROBE_OPT_ALLTOALL_FAULT value, 0: disarmed
   uint64_t ar2_calls = 0;     // cdprobe_allreduce_twoshot calls that ran (call_seq of the last one)
   uint64_t ar2_fault = 0;     // CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT value, 0: disarmed
+  uint64_t ll_calls = 0;      // cdprobe_allreduce_ll calls that ran (call_seq of the last one)
+  uint64_t ll_fault = 0;      // CDPROBE_OPT_ALLREDUCE_LL_FAULT value, 0: disarmed
+  bool ll_dirty = false;      // a local rank's LL kernel timed out: its LL area may hold packets of any earlier call
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -155,8 +162,9 @@ inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
   return L.coop && !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
 }
 
-// A measurement's shared area m (handle.cc): cdprobe_alltoall's exchange area (h->area, n_total x bytes_per_pair) or
-// cdprobe_allreduce_twoshot's gather area (h->gather, bytes_per_pair).  On the first call, every local rank creates
+// A measurement's shared area m (handle.cc): cdprobe_alltoall's exchange area (h->area, n_total x bytes_per_pair),
+// cdprobe_allreduce_twoshot's gather area (h->gather, bytes_per_pair) or cdprobe_allreduce_ll's LL area (h->ll,
+// 2 x n_total x 2 x the LL ladder's largest size).  On the first call, every local rank creates
 // `bytes` of device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every
 // local rank wherever the probe mapping is then up; status gets every rank's mapping statuses.  Collective.  If
 // creating it fails in any process, every process returns that error with nothing kept, and the next call tries

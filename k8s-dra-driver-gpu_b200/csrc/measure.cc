@@ -1,6 +1,7 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
-// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot and cdprobe_alltoall.  Each runs on the local ranks' own streams,
-// between probe runs, and has its results on the host before it returns.
+// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll and
+// cdprobe_alltoall.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
+// before it returns.
 #include <string.h>
 
 #include <algorithm>
@@ -10,6 +11,7 @@
 #include <vector>
 
 #include "allreduce.h"
+#include "allreduce_ll.h"
 #include "allreduce_twoshot.h"
 #include "alltoall.h"
 #include "atomics.h"
@@ -278,10 +280,11 @@ static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const ui
   out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
 }
 
-// The size ladder of the ladder measurements (bwcurve, allreduce, alltoall), and their verdict on their arguments:
-// empty when they are valid.
-static std::string ladder(const cdprobe* h, uint32_t reps, uint64_t* size, uint32_t* n_sizes) {
-  *n_sizes = bwcurve_ladder(h->plan.bpp, size);
+// The size ladder of the ladder measurements (bwcurve, allreduce, alltoall: bwcurve_ladder; allreduce_ll: ll_ladder),
+// and their verdict on their arguments: empty when they are valid.
+static std::string ladder(const cdprobe* h, uint32_t reps, uint64_t* size, uint32_t* n_sizes,
+                          uint32_t (*rule)(uint64_t, uint64_t*) = bwcurve_ladder) {
+  *n_sizes = rule(h->plan.bpp, size);
   if (reps > kMaxTimedReps) return "reps must be at most 64";
   if (*n_sizes == 0) return "bytes_per_pair must be at most 32 GiB";
   return {};
@@ -947,6 +950,144 @@ int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* 
   if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce_twoshot", out);
       rc != CDPROBE_OK)
     return rc;
+  out->ms = cdp::now_ms() - t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
+  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  const double t_begin = cdp::now_ms();
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  out->n = n;
+  out->path = CDPROBE_ALLREDUCE_PATH_LL;
+  reps = out->reps;
+  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
+  //    every process refuses, skips or runs together.  The fault acts in the process that hosts its sender
+  uint64_t size[cdp::kBwMaxSizes];
+  uint32_t n_sizes;
+  std::string bad = cdp::ladder(h, reps, size, &n_sizes, cdp::ll_ladder);
+  uint32_t f_send = cdp::kArNoFault, f_recv = 0, f_k = cdp::kArNoFault, f_mode = 0;
+  uint64_t f_arg = 0;
+  if (h->ll_fault != 0 && bad.empty()) {
+    const uint64_t v = h->ll_fault, mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu,
+                   fk = (v >> 24) & 0xffu;
+    f_arg = v & 0xffffffu;
+    if (mode > 1 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > n_sizes ||
+        (mode == 0 && (fs == fr || f_arg >= size[fk - 1] / 8)) ||
+        (mode == 1 && 2 * f_arg >= 1000ull * h->cfg.timeout_ms)) {
+      bad = "the armed LL all-reduce fault names no packet, size or delay of this call";
+    } else {
+      f_send = (uint32_t)fs - 1;
+      f_recv = (uint32_t)fr - 1;
+      f_k = (uint32_t)fk - 1;
+      f_mode = (uint32_t)mode;
+    }
+  }
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_allreduce_ll", bad, h->ll_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
+    return rc;
+  // 2. the LL area, built once, by every process in the same call; it is zeroed before its first use
+  const uint64_t s_max = size[n_sizes - 1];
+  const bool fresh = h->ll.bytes == 0;
+  if (const int rc = cdp::ensure_area(h, h->ll, cdp::ll_area_bytes(n, s_max), h->ll_status); rc != CDPROBE_OK)
+    return rc;
+  h->ll_dirty |= fresh;
+  out->call_seq = ++h->ll_calls;
+  cdp::put_ladder(h, size, n_sizes, out);
+  // 3. every rank reads its own source buffer and writes every LL area: when some probe mapping or LL-area mapping of
+  //    the domain is down, nothing runs, in any process
+  for (uint32_t s = 0; s < n; ++s)
+    for (uint32_t d = 0; d < n; ++d)
+      if (st[s][d] == 0) st[s][d] = h->ll_status[s][d];
+  if (cdp::skip_rows(h, st, out)) {
+    out->ms = cdp::now_ms() - t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 4. the domain's smallest grid, which splits the words alike on every rank (DESIGN §5j), and whether any process
+  //    has an LL area that a timed-out call may have left holding packets of any earlier call: then every process
+  //    zeroes its local ranks' areas before any kernel of this call can push into them
+  struct {
+    uint32_t ctas, dirty;
+  } mine = {UINT32_MAX, h->ll_dirty ? 1u : 0u}, all[cdp::kMaxRanks];
+  for (uint32_t li = 0; li < h->n_local; ++li) mine.ctas = std::min(mine.ctas, h->lr[li].ctas);
+  all[0] = mine;
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all, &err) != 0) {
+      cdp::set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  uint32_t grid = UINT32_MAX;
+  bool dirty = false;
+  for (uint32_t r = 0; r < std::max(h->cfg.world_size, 1u); ++r) {
+    grid = std::min(grid, all[r].ctas);
+    dirty |= all[r].dirty != 0;
+  }
+  if (dirty) {
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      cdp::LocalRank& L = h->lr[li];
+      CDP_RT(cudaSetDevice(L.ordinal));
+      cudaError_t e = cudaMemsetAsync(reinterpret_cast<void*>(L.ll_va[L.grank]), 0, h->ll.bytes, L.stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+      if (e != cudaSuccess) return cdp::fail_sticky(h, "cdprobe_allreduce_ll: zero the LL area", e);
+    }
+    h->ll_dirty = false;
+  }
+
+  // 5. scratch for the records, the output and the granule table, grown on every local rank before any kernel runs;
+  //    the (S, X) every prefix of the output must have, as for the one-shot
+  const size_t table_off = cdp::kArOutOff + (s_max + 255) / 256 * 256;
+  if (const int rc = cdp::ensure_scratch_all(h, table_off + 16 * (pl.bpp / cdp::kGranuleBytes)); rc != CDPROBE_OK)
+    return rc;
+  uint64_t want[cdp::kBwMaxSizes][2] = {};
+  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
+                                        "cdprobe_allreduce_ll: granule checksums");
+      rc != CDPROBE_OK)
+    return rc;
+
+  // 6. no process launches before every process is ready; then every local kernel is launched before any is waited for
+  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    cdp::LlParams p;
+    memset(&p, 0, sizeof(p));
+    p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + pl.src_off;
+    for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.ll_va[(g + t) % n]);
+    p.in = reinterpret_cast<const uint8_t*>(L.ll_va[g]);
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j == g) continue;
+      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kLlOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kLlOff + (uint64_t)j * sizeof(cdp::FlagLine));
+    }
+    p.dom.call_seq = h->ll_calls;
+    p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
+    p.s_max = s_max;
+    p.seed = h->seed;
+    p.fault_k = g == f_send ? f_k : cdp::kArNoFault;
+    p.fault_mode = f_mode;
+    p.fault_dst = (f_recv + n - g) % n;
+    p.fault_arg = f_arg;
+    p.rank = g;
+    p.n = n;
+    p.ctas = grid;
+    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_ll_launch,
+                                          "launch allreduce_ll_kernel");
+        rc != CDPROBE_OK)
+      return rc;
+  }
+
+  // 7. collect: per row, the times and every rep's checksums, then the word check of the last rep; a row that timed
+  //    out leaves its LL area to be zeroed before the next call
+  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce_ll", out); rc != CDPROBE_OK)
+    return rc;
+  for (uint32_t li = 0; li < h->n_local; ++li) h->ll_dirty |= out->status[h->lr[li].grank] == CDPROBE_ERR_TIMEOUT;
   out->ms = cdp::now_ms() - t_begin;
   return CDPROBE_OK;
 }

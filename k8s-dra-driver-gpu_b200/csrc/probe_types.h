@@ -518,6 +518,40 @@ constexpr uint64_t kAr2Off = kA2aOff + kMaxRanks * sizeof(FlagLine);  // 72 KiB
 static_assert(kAr2Off % 128 == 0 && kAr2Off + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
               "the two-shot all-reduce lines sit after the all-to-all lines inside the Ctrl granule");
 
+// ---- the low-latency all-reduce (cdprobe_allreduce_ll, DESIGN §5j) --------------------------------------------------
+// The LL ladder: the bwcurve ladder's sizes of at most kLlMaxBytes (4096 ... 1 MiB when bytes_per_pair exceeds it).
+// Returns how many, or 0 when bwcurve_ladder does.  size has room for kBwMaxSizes.
+constexpr uint64_t kLlMaxBytes = 1ull << 20;
+CDP_HD inline uint32_t ll_ladder(uint64_t bpp, uint64_t* size) {
+  const uint32_t n = bwcurve_ladder(bpp, size);
+  uint32_t m = 0;
+  while (m < n && size[m] <= kLlMaxBytes) ++m;
+  return m;
+}
+// The flag every packet of rep r (0: the warm-up) of size k of call call_seq carries in both 32-bit halves.  r + 1 >= 1
+// makes it non-zero (the zeroed area holds 0); (k, r) < (24, 65) fit their bytes, so the flags of one call differ; and
+// the low 16 bits of call_seq differ between consecutive calls, so no flag of a call equals one of the call before.
+CDP_HD inline uint32_t ll_flag(uint64_t call_seq, uint32_t k, uint32_t r) {
+  return (uint32_t)((call_seq & 0xffffu) << 16) | ((k & 0xffu) << 8) | ((r + 1u) & 0xffu);
+}
+// What rank j adds to every input word in a rep whose flag is `flag`; the receiver subtracts the sum over all ranks.
+// Every rep's inputs differ, so a packet of another rep that were accepted would leave a wrong sum.
+CDP_HD inline uint64_t ll_salt(uint64_t seed, uint32_t j, uint32_t flag) {
+  return splitmix64(seed ^ 0x4C4C53414C54ull ^ ((uint64_t)j << 56) ^ ((uint64_t)flag << 8));
+}
+// Byte offset in a receiver's LL area of the 16-byte packet of word w from sender s in parity p (rep r uses r % 2),
+// for n ranks and a ladder whose largest size is s_max; the area is 2 x n x 2 x s_max bytes.
+CDP_HD inline uint64_t ll_slot(uint32_t p, uint32_t n, uint32_t s, uint64_t s_max, uint64_t w) {
+  return (((uint64_t)p * n + s) * (s_max / 8) + w) * 16;
+}
+CDP_HD inline uint64_t ll_area_bytes(uint32_t n, uint64_t s_max) { return 2ull * n * 2 * s_max; }
+
+// The opening domain barrier of every size of cdprobe_allreduce_ll: one 128-byte line per sender after the two-shot
+// lines, in the Ctrl granule.  Same rules as kArOff.
+constexpr uint64_t kLlOff = kAr2Off + kMaxRanks * sizeof(FlagLine);  // 74 KiB
+static_assert(kLlOff % 128 == 0 && kLlOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the LL all-reduce lines sit after the two-shot all-reduce lines inside the Ctrl granule");
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -649,6 +649,22 @@ class Probe:
         rc = self._lib.cdprobe_allreduce_twoshot(self._h, reps, C.byref(t))
         return rc, t
 
+    def AllReduceLL(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReduceLL.  Low-latency all-reduce of every rank's source buffer on every rank at once:
+        flag-carrying 16-byte packets pushed to every peer, no barrier or fence per rep, at each size of the LL ladder
+        (the bwcurve ladder up to 1 MiB), on the probe's grids (0: 8 timed reps per size).  A rep is timed from the end
+        of the rank's previous rep; path is abi.ALLREDUCE_PATH_LL.  Collective when world_size > 1.  Needs no Run
+        first and disturbs none."""
+        rc, t = self.allreduce_ll_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce_ll")
+        return AllReduce.from_c(t)
+
+    def allreduce_ll_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce_ll(self._h, reps, C.byref(t))
+        return rc, t
+
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps

@@ -12,7 +12,13 @@ limit and SM clock read in the same call (read-only query); --out also writes th
 every unit, so a rep is the one-shot's reads plus a store to its own gather area and the untimed check), and with 2 and
 4 ranks sharing GPU 0 (`--multi-bytes` per rank) on the TMA path.  Each rank's link traffic in a two-shot rep is
 2 (n - 1) / n x size, so its bus bandwidth, busbw = algbw x 2 (n - 1) / n, is the figure nccl-tests reports; ranks on
-one device move that traffic through its own HBM, not NVLink."""
+one device move that traffic through its own HBM, not NVLink.
+
+--ll measures cdprobe_allreduce_ll instead, next to the one-shot and the two-shot (TMA path) on the same handle in the
+same session: N = 1 and 2, 4 and 8 ranks sharing GPU 0 at `--ll-bytes` per pair (default 1 MiB, the LL ladder's
+largest size), so the ladder runs 4 KiB ... 1 MiB.  An LL rep runs from the end of the rank's previous rep to the end of
+its own (no barrier per rep); a one-shot rep from its opening barrier's release, a two-shot rep to its closing
+release.  Each rank's link ingress per LL rep is 2 (n - 1) x size: every 8 bytes of data travel in a 16-byte packet."""
 import argparse
 import json
 import os
@@ -30,6 +36,8 @@ ap.add_argument("--reps", type=int, default=16)
 ap.add_argument("--out", default=None, help="also write the JSON document to this file")
 ap.add_argument("--twoshot", action="store_true", help="also measure cdprobe_allreduce_twoshot")
 ap.add_argument("--multi-bytes", type=int, default=256 << 20, help="bytes_per_pair of the 2- and 4-rank two-shot runs")
+ap.add_argument("--ll", action="store_true", help="measure cdprobe_allreduce_ll next to the one-shot and the two-shot")
+ap.add_argument("--ll-bytes", type=int, default=1 << 20, help="bytes_per_pair of the --ll runs")
 a = ap.parse_args()
 
 
@@ -55,6 +63,42 @@ def rows(ar, bus=None):
             out[f"rank_{r}"]["peak_busbw_gbps"] = ar.peak_gbps[r] * bus
     return out
 
+
+if a.ll:
+    res = {"ll_bytes": a.ll_bytes, "reps": a.reps,
+           "what": "ns per rep of cdprobe_allreduce_ll (ll), cdprobe_allreduce (one_shot) and "
+                   "cdprobe_allreduce_twoshot (two_shot, TMA path) called one after another on the same handle: "
+                   "N = 1 with one CTA per SM, N = 2, 4, 8 ranks on GPU 0 (ALLOW_SAME_DEVICE | NO_COOPERATIVE, 16 "
+                   "CTAs each), bytes_per_pair = ll_bytes; the ll ladder is the bwcurve ladder up to 1 MiB and the "
+                   "others are reported at the same sizes.  An ll rep runs from the end of the rank's previous rep "
+                   "(the warm-up: its barrier release) to its latest CTA completion stamp; a one-shot rep from its "
+                   "opening barrier release to its latest CTA stamp; a two-shot rep from its opening to its closing "
+                   "barrier release.  algbw_gbps_median = bytes / ns_median; LL link ingress = 2 (n - 1) x bytes"}
+    for n in (1, 2, 4, 8):
+        cfg = pkg.Config(ordinals=[0] * n, bytes=a.ll_bytes * max(n - 1, 1), flags=0x40 | 0x10 if n > 1 else 0,
+                         ctas=16 if n > 1 else 0, timeout_ms=20000)
+        with pkg.Open(cfg) as p:
+            ll = p.AllReduceLL(a.reps)
+            one = p.AllReduce(a.reps)
+            ts = p.AllReduceTwoShot(a.reps)
+            res[f"n{n}"] = {"ll": {**rows(ll), "call_ms": ll.ms}, "one_shot": {**rows(one), "call_ms": one.ms},
+                            "two_shot": {**rows(ts), "call_ms": ts.ms}}
+    res["gpu"] = gpu()
+    res["nvlink"] = "not measured (one GPU)"
+    print(f"{'n':>2} {'rank':>4} {'bytes':>9} {'ll ns':>9} {'one-shot':>9} {'two-shot':>9} {'ll GB/s':>8}")
+    for n in (1, 2, 4, 8):
+        for r in range(n):
+            rk = f"rank_{r}"
+            for s, o, t in zip(*(res[f"n{n}"][x][rk]["sizes"] for x in ("ll", "one_shot", "two_shot"))):
+                print(f"{n:2d} {r:4d} {s['bytes']:9d} {s['ns_median']:9.0f} {o['ns_median']:9.0f} "
+                      f"{t['ns_median']:9.0f} {s['algbw_gbps_median']:8.1f}")
+    print(f"gpu: {res['gpu']}")
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(res))
+    sys.exit(0)
 
 res = {"bytes": a.bytes, "reps": a.reps,
        "what": "ns per rep of the one-shot all-reduce of the first `bytes` of every rank's source buffer into the "
