@@ -253,7 +253,7 @@ static int gather_status(cdprobe* h, int32_t (*st)[kMaxRanks]) {
   return CDPROBE_OK;
 }
 
-int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*status)[kMaxRanks]) {
+int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes) {
   if (m.bytes != 0) return CDPROBE_OK;
   bytes = (bytes + kVmmGranule - 1) / kVmmGranule * kVmmGranule;
   int32_t st[kMaxRanks][kMaxRanks] = {};
@@ -267,7 +267,7 @@ int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*status)[kMax
     g_last_error = keep;
     return rc;
   }
-  memcpy(status, st, sizeof(st));
+  memcpy(m.status, st, sizeof(st));
   return CDPROBE_OK;
 }
 

@@ -58,7 +58,8 @@ struct LocalRank {
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
 // exports them, takes the other processes' over the rendezvous, imports them and maps every rank's into every local
 // rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area,
-// cdprobe_allreduce_twoshot's gather area and cdprobe_allreduce_ll's LL area are others.
+// cdprobe_allreduce_twoshot's gather area and cdprobe_allreduce_ll's LL area are others (ensure_area), and keep their
+// state here.
 struct SharedAlloc {
   size_t bytes = 0;                                       // of each allocation; 0: not created
   CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
@@ -68,6 +69,10 @@ struct SharedAlloc {
   int own_fd[kMaxRanks];                                  // [local rank] exported POSIX fd, -1: none
   CUmemGenericAllocationHandle imported[kMaxRanks] = {};  // [rank] of another process
   bool has_import[kMaxRanks] = {};
+  int32_t status[kMaxRanks][kMaxRanks] = {};  // an area's [issuer][owner] mapping status, all ranks, once it exists
+                                              // (the probe allocation's is cdprobe::status)
+  bool stale = false;  // the LL area must be zeroed before its next use: it is new, or a local rank's kernel timed out
+                       // and it may hold packets of any earlier call
   SharedAlloc(CUdeviceptr (LocalRank::*v)[kMaxRanks], bool (LocalRank::*m)[kMaxRanks]) : va(v), mapped(m) {
     for (int& f : own_fd) f = -1;
   }
@@ -88,9 +93,6 @@ struct cdprobe {
   cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};  // the two-shot's gather area
   cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};  // cdprobe_allreduce_ll's LL area
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
-  int32_t area_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the exchange area, once it exists
-  int32_t gather_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the gather area, once it exists
-  int32_t ll_status[cdp::kMaxRanks][cdp::kMaxRanks] = {};  // the same for the LL area, once it exists
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
   uint64_t seed = 0;
@@ -122,7 +124,6 @@ struct cdprobe {
   uint64_t ar2_fault = 0;     // CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT value, 0: disarmed
   uint64_t ll_calls = 0;      // cdprobe_allreduce_ll calls that ran (call_seq of the last one)
   uint64_t ll_fault = 0;      // CDPROBE_OPT_ALLREDUCE_LL_FAULT value, 0: disarmed
-  bool ll_dirty = false;      // a local rank's LL kernel timed out: its LL area may hold packets of any earlier call
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -166,10 +167,10 @@ inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
 // cdprobe_allreduce_twoshot's gather area (h->gather, bytes_per_pair) or cdprobe_allreduce_ll's LL area (h->ll,
 // 2 x n_total x 2 x the LL ladder's largest size).  On the first call, every local rank creates
 // `bytes` of device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every
-// local rank wherever the probe mapping is then up; status gets every rank's mapping statuses.  Collective.  If
+// local rank wherever the probe mapping is then up; m.status gets every rank's mapping statuses.  Collective.  If
 // creating it fails in any process, every process returns that error with nothing kept, and the next call tries
 // again.  Kept until close.
-int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*status)[kMaxRanks]);
+int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes);
 
 // The mapping status of local rank li's cell [its rank][j]: kStatusUnmapped when that status is 0 but the peer is not
 // mapped.  Non-zero: never read or write through that mapping.

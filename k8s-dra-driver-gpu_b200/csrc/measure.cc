@@ -78,26 +78,30 @@ static bool begin_output(Out* out) {
 
 // What each process contributes at the start of a collective measurement (cdprobe_pingpong, cdprobe_bwcurve,
 // cdprobe_allreduce, cdprobe_alltoall), so that every process refuses, skips or runs the same call: the call number it
-// is about to make, the arguments every process must pass alike (unused ones 0), whether its own were valid, and its
-// local ranks' rows of mapping status, [local rank][rank] with unmapped cells folded in (cdprobe_unmap_peer changes
-// only the local view).
+// is about to make, the arguments every process must pass alike (unused ones 0), whether its own were valid, its local
+// ranks' smallest grid, whether its shared area must be zeroed before use, and its local ranks' rows of mapping status,
+// [local rank][rank] with unmapped cells folded in (cdprobe_unmap_peer changes only the local view).
 struct Agreement {
   uint64_t call_seq;
   std::array<uint32_t, 3> args;
   uint32_t ok;
+  uint32_t ctas, zero;
   int32_t rows[kMaxRanks][kMaxRanks];
 };
 
 // The handshake of collective measurement `fn`: every process contributes its Agreement (ok: its own verdict `bad` on
-// its arguments is empty).  The first error wins: this process's own arguments, then another process's, then a call
-// number or arguments that differ.  Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and CDPROBE_ERR_ARG on a
-// refusal, with the message set.  Otherwise st, when given, gets the domain's matrix of mapping status, [rank][rank],
-// which every process derives alike.
+// its arguments is empty; zero: *zero, when given).  The first error wins: this process's own arguments, then another
+// process's, then a call number or arguments that differ.  Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and
+// CDPROBE_ERR_ARG on a refusal, with the message set.  Otherwise st, when given, gets the domain's matrix of mapping
+// status, [rank][rank], which every process derives alike; grid, when given, the domain's smallest grid; and *zero
+// whether any process must zero its area.
 static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq, const std::array<uint32_t, 3>& args,
-                 int32_t (*st)[kMaxRanks]) {
-  Agreement mine = {call_seq, args, bad.empty() ? 1u : 0u, {}};
-  for (uint32_t li = 0; li < h->n_local; ++li)
+                 int32_t (*st)[kMaxRanks], uint32_t* grid = nullptr, bool* zero = nullptr) {
+  Agreement mine = {call_seq, args, bad.empty() ? 1u : 0u, UINT32_MAX, zero != nullptr && *zero ? 1u : 0u, {}};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    mine.ctas = std::min(mine.ctas, h->lr[li].ctas);
     for (uint32_t j = 0; j < h->n_total; ++j) mine.rows[li][j] = cell_status(h, li, j);
+  }
   std::vector<Agreement> all(h->cfg.world_size, mine);
   if (h->cfg.world_size > 1) {
     std::string err;
@@ -119,6 +123,11 @@ static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq,
     memset(st, 0, sizeof(int32_t) * kMaxRanks * kMaxRanks);
     for (uint32_t r = 0; r < all.size(); ++r)
       for (uint32_t li = 0; li < h->n_local; ++li) memcpy(st[r * h->n_local + li], all[r].rows[li], sizeof(st[0]));
+  }
+  if (grid != nullptr) *grid = UINT32_MAX;
+  for (const Agreement& o : all) {
+    if (grid != nullptr) *grid = std::min(*grid, o.ctas);
+    if (zero != nullptr) *zero |= o.zero != 0;
   }
   return CDPROBE_OK;
 }
@@ -280,34 +289,56 @@ static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const ui
   out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
 }
 
-// The size ladder of the ladder measurements (bwcurve, allreduce, alltoall: bwcurve_ladder; allreduce_ll: ll_ladder),
-// and their verdict on their arguments: empty when they are valid.
-static std::string ladder(const cdprobe* h, uint32_t reps, uint64_t* size, uint32_t* n_sizes,
-                          uint32_t (*rule)(uint64_t, uint64_t*) = bwcurve_ladder) {
-  *n_sizes = rule(h->plan.bpp, size);
-  if (reps > kMaxTimedReps) return "reps must be at most 64";
-  if (*n_sizes == 0) return "bytes_per_pair must be at most 32 GiB";
-  return {};
+// A ladder measurement as open_ladder lets it through: when it began, its reps, its size ladder, and the verdict on its
+// arguments, empty when they are valid.
+struct Ladder {
+  double t_begin;
+  uint32_t reps, n_sizes;
+  uint64_t size[kBwMaxSizes];
+  std::string bad;
+};
+
+// out->path of a ladder measurement that runs on the handle's data path (CDPROBE_OPT_PATH).
+constexpr uint32_t kHandlePath = UINT32_MAX;
+
+// The opening of the ladder measurements (bwcurve, the all-reduces, alltoall): *out cleared and stamped with reps (0:
+// default_reps); once the handle is known, n and the data path (`path`, or the handle's) before the handle is checked;
+// then the size ladder by `rule` (bwcurve_ladder; allreduce_ll: ll_ladder) and the verdict on the arguments.
+template <typename Out>
+static int open_ladder(cdprobe* h, Out* out, uint32_t reps, uint32_t default_reps, Ladder* lad,
+                       uint32_t path = kHandlePath, uint32_t (*rule)(uint64_t, uint64_t*) = bwcurve_ladder) {
+  if (!begin_output(out)) return CDPROBE_ERR_ARG;
+  out->reps = reps != 0 ? reps : default_reps;
+  if (h == nullptr) return CDPROBE_ERR_ARG;
+  lad->t_begin = now_ms();
+  out->n = h->n_total;
+  out->path = path == kHandlePath ? h->path : path;
+  lad->reps = out->reps;
+  if (const int rc = require_usable(h); rc != CDPROBE_OK) return rc;
+  lad->n_sizes = rule(h->plan.bpp, lad->size);
+  if (lad->reps > kMaxTimedReps) lad->bad = "reps must be at most 64";
+  else if (lad->n_sizes == 0) lad->bad = "bytes_per_pair must be at most 32 GiB";
+  return CDPROBE_OK;
 }
 
 // What a ladder measurement reports once every process has agreed to run it: the ladder and this process's rows.
 template <typename Out>
-static void put_ladder(const cdprobe* h, const uint64_t* size, uint32_t n_sizes, Out* out) {
-  out->n_sizes = n_sizes;
-  memcpy(out->size, size, sizeof(size[0]) * n_sizes);
+static void put_ladder(const cdprobe* h, const Ladder& lad, Out* out) {
+  out->n_sizes = lad.n_sizes;
+  memcpy(out->size, lad.size, sizeof(lad.size[0]) * lad.n_sizes);
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
 }
 
 // Launches a ladder kernel on local rank L: the parameters every ladder kernel takes, then its records at the head of
 // L's scratch cleared and the launch on L's stream.  A failed launch makes the handle sticky.
 template <typename Params>
-static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const uint64_t* size, uint32_t n_sizes, uint32_t reps,
+static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const Ladder& lad,
                          int (*launch)(const Params&, unsigned, bool, cudaStream_t), const char* what) {
   p.scratch = static_cast<decltype(p.scratch)>(L.scratch);
-  memcpy(p.size, size, sizeof(p.size));
+  memcpy(p.size, lad.size, sizeof(p.size));
   p.timeout_ns = timeout_ns(h);
-  p.n_sizes = n_sizes;
-  p.reps = reps;
+  p.n_sizes = lad.n_sizes;
+  p.reps = lad.reps;
   p.path = h->path;
   CDP_RT(cudaSetDevice(L.ordinal));
   cudaError_t e = cudaMemsetAsync(L.scratch, 0, sizeof(*p.scratch), L.stream);
@@ -328,17 +359,17 @@ static bool skip_rows(const cdprobe* h, int32_t (*st)[kMaxRanks], cdprobe_allred
 
 // Collects the rows of the all-reduces once their kernels are done: per local row, the times and every rep's (S, X)
 // against want (bw_summarize), then the word checks of every size.
-static int collect_rows(cdprobe* h, const uint64_t (*want)[2], const uint64_t* size, uint32_t n_sizes, uint32_t reps,
-                        const char* what, cdprobe_allreduce_t* out) {
+static int collect_rows(cdprobe* h, const uint64_t (*want)[2], const Ladder& lad, const char* what,
+                        cdprobe_allreduce_t* out) {
   auto got = std::make_unique<ArScratch>();
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
     if (const int rc = fetch_reps(h, L, got.get(), 1, what); rc != CDPROBE_OK) return rc;
     const ArScratch& s = *got;
-    bw_summarize(s.rep, want, size, n_sizes, reps, g, out);
+    bw_summarize(s.rep, want, lad.size, lad.n_sizes, lad.reps, g, out);
     if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
-    for (uint32_t k = 0; k < n_sizes; ++k) {
+    for (uint32_t k = 0; k < lad.n_sizes; ++k) {
       out->bad_words[g][k] = s.bad_words[k];
       out->first_bad[g][k] = s.bad_words[k] != 0 ? ~s.first_bad_n[k] : UINT64_MAX;
       if (s.bad_words[k] != 0) {
@@ -347,6 +378,227 @@ static int collect_rows(cdprobe* h, const uint64_t (*want)[2], const uint64_t* s
       }
     }
   }
+  return CDPROBE_OK;
+}
+
+// The barrier lines of local rank L in the FlagLine array at `off` in the Ctrl granule: it pushes into line L.grank of
+// every other rank's array and waits on line j of its own for rank j.
+static DomainLines domain_lines(const cdprobe* h, const LocalRank& L, uint64_t off, uint64_t call_seq) {
+  DomainLines d;
+  memset(&d, 0, sizeof(d));
+  const uint32_t g = L.grank;
+  for (uint32_t j = 0; j < h->n_total; ++j) {
+    if (j == g) continue;
+    d.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + off + (uint64_t)g * sizeof(FlagLine));
+    d.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + off + (uint64_t)j * sizeof(FlagLine));
+  }
+  d.call_seq = call_seq;
+  return d;
+}
+
+// An all-reduce's armed fault once its protocol has accepted it: in timed rep 1 of size k, rank `rank` (kArNoFault:
+// none) acts on word `word` towards receiver `recv`, in `mode`.  What each means is the protocol's.
+struct ArFault {
+  uint32_t rank = kArNoFault, recv = 0, k = kArNoFault, mode = 0;
+  uint64_t word = 0;
+};
+
+// One all-reduce protocol, as allreduce_call runs it.
+struct ArProtocol {
+  const char* fn;                                // the entry point, which names the call in every message
+  uint64_t cdprobe::*calls;                      // its calls that ran
+  uint64_t cdprobe::*fault;                      // its armed fault, 0: disarmed
+  uint32_t (*rule)(uint64_t, uint64_t*);         // its size ladder
+  uint32_t path;                                 // out->path: kHandlePath, or its own
+  SharedAlloc cdprobe::*area;                    // the shared area peers write, nullptr: none
+  uint64_t (*area_bytes)(uint32_t n, uint64_t s_max);  // its size per rank, for the ladder's largest size s_max
+  const char* zeroing;                           // the area must start zeroed: names the step in a CUDA failure
+  bool out_in_scratch;                           // the output takes s_max bytes of the scratch at kArOutOff
+  uint64_t lines;                                // its barrier lines in the Ctrl granule
+  // the fault's verdict for this call: nullptr with *f filled, or the refusal
+  const char* (*decode)(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f);
+  // fills its parameters for local rank L and launches its kernel (launch_ladder)
+  int (*launch)(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f, uint32_t grid);
+};
+
+static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint64_t fr = v >> 32, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  if (fr == 0 || fr > h->n_total || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+    return "the armed all-reduce fault names no rank, size or output word of this call";
+  *f = {(uint32_t)fr - 1, 0, (uint32_t)fk - 1, 0, word};
+  return nullptr;
+}
+
+static int oneshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                          uint32_t) {
+  const uint32_t g = L.grank, n = h->n_total;
+  AllReduceParams p;
+  memset(&p, 0, sizeof(p));
+  for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
+  p.dom = dom;
+  p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_word = f.word;
+  p.rank = g;
+  p.n = n;
+  return launch_ladder(h, L, p, lad, allreduce_launch, "launch allreduce_kernel");
+}
+
+// The fault acts in the rank whose chunk holds its word.
+static const char* twoshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint32_t n = h->n_total;
+  const uint64_t fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  if ((v >> 49) != 0 || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+    return "the armed two-shot all-reduce fault names no receiver, size or output word of this call";
+  *f = {kArNoFault, (uint32_t)fr - 1, (uint32_t)fk - 1, (uint32_t)(v >> 48), word};
+  const uint64_t units = (lad.size[f->k] + kUnitBytes - 1) / kUnitBytes, u = word / (kUnitBytes / 8);
+  for (uint32_t r = 0; r < n; ++r) {
+    uint64_t lo, hi;
+    twoshot_chunk(units, n, r, &lo, &hi);
+    if (u >= lo && u < hi) f->rank = r;
+  }
+  return nullptr;
+}
+
+static int twoshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                          uint32_t) {
+  const uint32_t g = L.grank, n = h->n_total;
+  TwoShotParams p;
+  memset(&p, 0, sizeof(p));
+  for (uint32_t t = 0; t < n; ++t) {
+    p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
+    p.dst[t] = reinterpret_cast<uint8_t*>(L.gather_va[(g + t) % n]);
+  }
+  p.dom = dom;
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_word = f.word;
+  p.fault_dst = (f.recv + n - g) % n;
+  p.fault_drop = f.mode;
+  p.rank = g;
+  p.n = n;
+  return launch_ladder(h, L, p, lad, allreduce_twoshot_launch, "launch allreduce_twoshot_kernel");
+}
+
+// The fault acts in the process that hosts its sender.
+static const char* ll_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint32_t n = h->n_total;
+  const uint64_t mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu, fk = (v >> 24) & 0xffu,
+                 arg = v & 0xffffffu;
+  if (mode > 1 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes ||
+      (mode == 0 && (fs == fr || arg >= lad.size[fk - 1] / 8)) || (mode == 1 && 2 * arg >= 1000ull * h->cfg.timeout_ms))
+    return "the armed LL all-reduce fault names no packet, size or delay of this call";
+  *f = {(uint32_t)fs - 1, (uint32_t)fr - 1, (uint32_t)fk - 1, (uint32_t)mode, arg};
+  return nullptr;
+}
+
+// Every rank splits the words over the domain's smallest grid, so that each word has the same owner everywhere.
+static int ll_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                     uint32_t grid) {
+  const uint32_t g = L.grank, n = h->n_total;
+  LlParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
+  for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.ll_va[(g + t) % n]);
+  p.in = reinterpret_cast<const uint8_t*>(L.ll_va[g]);
+  p.dom = dom;
+  p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
+  p.s_max = lad.size[lad.n_sizes - 1];
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_mode = f.mode;
+  p.fault_dst = (f.recv + n - g) % n;
+  p.fault_arg = f.word;
+  p.rank = g;
+  p.n = n;
+  p.ctas = grid;
+  return launch_ladder(h, L, p, lad, allreduce_ll_launch, "launch allreduce_ll_kernel");
+}
+
+constexpr ArProtocol kOneShot = {
+    "cdprobe_allreduce", &cdprobe::ar_calls, &cdprobe::ar_fault, bwcurve_ladder, kHandlePath, nullptr, nullptr,
+    nullptr, true, kArOff, oneshot_fault, oneshot_launch};
+constexpr ArProtocol kTwoShot = {
+    "cdprobe_allreduce_twoshot", &cdprobe::ar2_calls, &cdprobe::ar2_fault, bwcurve_ladder, kHandlePath,
+    &cdprobe::gather, [](uint32_t, uint64_t s_max) { return s_max; }, nullptr, false, kAr2Off, twoshot_fault,
+    twoshot_launch};
+constexpr ArProtocol kLl = {
+    "cdprobe_allreduce_ll", &cdprobe::ll_calls, &cdprobe::ll_fault, ll_ladder, CDPROBE_ALLREDUCE_PATH_LL, &cdprobe::ll,
+    ll_area_bytes, "cdprobe_allreduce_ll: zero the LL area", true, kLlOff, ll_fault, ll_launch};
+
+// The all-reduces (DESIGN §5g, §5i, §5j): one call of protocol P.
+static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, const ArProtocol& P) {
+  Ladder lad;
+  if (const int rc = open_ladder(h, out, reps, kArDefaultReps, &lad, P.path, P.rule); rc != CDPROBE_OK) return rc;
+  const uint32_t n = h->n_total;
+  // 1. the arguments, the armed fault, the probe mapping rows and whether any area must be zeroed; in a multi-process
+  //    domain all are shared, so every process refuses, skips, zeroes or runs together.  An area that must start zeroed
+  //    and is yet to be created is stale until it is zeroed
+  ArFault f;
+  if (h->*P.fault != 0 && lad.bad.empty())
+    if (const char* why = P.decode(h, h->*P.fault, lad, &f)) lad.bad = why;
+  SharedAlloc* m = P.area != nullptr ? &(h->*P.area) : nullptr;
+  if (P.zeroing != nullptr) m->stale |= m->bytes == 0;
+  bool zero = P.zeroing != nullptr && m->stale;
+  uint32_t grid;
+  int32_t st[kMaxRanks][kMaxRanks];
+  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero); rc != CDPROBE_OK)
+    return rc;
+  // 2. the area, built once, by every process in the same call
+  const uint64_t s_max = lad.size[lad.n_sizes - 1];
+  if (m != nullptr)
+    if (const int rc = ensure_area(h, *m, P.area_bytes(n, s_max)); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++(h->*P.calls);
+  put_ladder(h, lad, out);
+  // 3. every rank reads every input and writes every area: when some probe mapping or area mapping of the domain is
+  //    down, nothing runs, in any process
+  if (m != nullptr)
+    for (uint32_t s = 0; s < n; ++s)
+      for (uint32_t d = 0; d < n; ++d)
+        if (st[s][d] == 0) st[s][d] = m->status[s][d];
+  if (skip_rows(h, st, out)) {
+    out->ms = now_ms() - lad.t_begin;
+    return CDPROBE_OK;
+  }
+  // 4. every process zeroes its local ranks' areas before any kernel of this call can push into them
+  if (zero && P.zeroing != nullptr) {
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      LocalRank& L = h->lr[li];
+      CDP_RT(cudaSetDevice(L.ordinal));
+      cudaError_t e = cudaMemsetAsync(reinterpret_cast<void*>((L.*m->va)[L.grank]), 0, m->bytes, L.stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+      if (e != cudaSuccess) return fail_sticky(h, P.zeroing, e);
+    }
+    m->stale = false;
+  }
+
+  // 5. scratch for the records, the output (when it is there) and the granule table, grown on every local rank before
+  //    any kernel runs; the (S, X) every prefix of the output must have, from the pattern definition: the per-granule
+  //    sums of the summed words on the first local rank's GPU, folded into every prefix on the host
+  const size_t table_off = kArOutOff + (P.out_in_scratch ? (s_max + 255) / 256 * 256 : 0);
+  if (const int rc = ensure_scratch_all(h, table_off + 16 * (h->plan.bpp / kGranuleBytes)); rc != CDPROBE_OK) return rc;
+  uint64_t want[kBwMaxSizes][2] = {};
+  if (const int rc = expected_sums(h, h->lr[0], table_off, AllReduceWord{h->seed, n}, lad.size, lad.n_sizes, want,
+                                   (std::string(P.fn) + ": granule checksums").c_str());
+      rc != CDPROBE_OK)
+    return rc;
+
+  // 6. no process launches before every process is ready, so that no kernel waits at its first domain barrier for a
+  //    process still setting up; then every local kernel is launched before any is waited for
+  if (const int rc = domain_barrier(h); rc != CDPROBE_OK) return rc;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    if (const int rc = P.launch(h, L, domain_lines(h, L, P.lines, h->*P.calls), lad, f, grid); rc != CDPROBE_OK)
+      return rc;
+  }
+
+  // 7. collect: per row, the times and every rep's checksums, then the word checks; a row that timed out leaves an area
+  //    that must start zeroed stale, to be zeroed before the next call runs
+  if (const int rc = collect_rows(h, want, lad, P.fn, out); rc != CDPROBE_OK) return rc;
+  if (P.zeroing != nullptr)
+    for (uint32_t li = 0; li < h->n_local; ++li) m->stale |= out->status[h->lr[li].grank] == CDPROBE_ERR_TIMEOUT;
+  out->ms = now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }
 
@@ -690,25 +942,17 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
 }
 
 int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
-  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
-  out->reps = reps != 0 ? reps : cdp::kBwDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
+  cdp::Ladder lad;
+  if (const int rc = cdp::open_ladder(h, out, reps, cdp::kBwDefaultReps, &lad); rc != CDPROBE_OK) return rc;
   const cdp::Plan& pl = h->plan;
   const uint32_t n = h->n_total;
-  out->n = n;
-  out->path = h->path;
-  reps = out->reps;
-  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together.  Every
   //    cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree
-  uint64_t size[cdp::kBwMaxSizes];
-  uint32_t n_sizes;
-  const std::string bad = cdp::ladder(h, reps, size, &n_sizes);
-  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", bad, h->bw_calls + 1, {reps, 0u, 0u}, nullptr); rc != CDPROBE_OK)
+  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", lad.bad, h->bw_calls + 1, {lad.reps, 0u, 0u}, nullptr);
+      rc != CDPROBE_OK)
     return rc;
   out->call_seq = ++h->bw_calls;
-  cdp::put_ladder(h, size, n_sizes, out);
+  cdp::put_ladder(h, lad, out);
 
   // 2. scratch for the rep records and one cell's granule table, grown on every local rank before any kernel runs
   const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
@@ -729,7 +973,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       if (!cdp::live_cell(h, li, j, out->status)) continue;
       runs[li][j] = true;
       const cdp::SrcRegionWord word{h->seed, (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8), j};
-      if (const int rc = cdp::expected_sums(h, L, table_off, word, size, n_sizes, want_of(li, j),
+      if (const int rc = cdp::expected_sums(h, L, table_off, word, lad.size, lad.n_sizes, want_of(li, j),
                                             "cdprobe_bwcurve: granule checksums");
           rc != CDPROBE_OK)
         return rc;
@@ -751,7 +995,7 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       cdp::BwCurveParams p;
       memset(&p, 0, sizeof(p));
       p.region = reinterpret_cast<const uint8_t*>(L.va[q]) + cdp::cell_offset(pl, CDPROBE_OP_READ, L.grank, (uint32_t)q);
-      if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::bwcurve_launch, "launch bwcurve_kernel");
+      if (const int rc = cdp::launch_ladder(h, L, p, lad, cdp::bwcurve_launch, "launch bwcurve_kernel");
           rc != CDPROBE_OK)
         return rc;
     }
@@ -759,363 +1003,41 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       if (target[li] < 0) continue;
       cdp::LocalRank& L = h->lr[li];
       if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_bwcurve"); rc != CDPROBE_OK) return rc;
-      cdp::bw_summarize(*got, want_of(li, (uint32_t)target[li]), size, n_sizes, reps,
+      cdp::bw_summarize(*got, want_of(li, (uint32_t)target[li]), lad.size, lad.n_sizes, lad.reps,
                         L.grank * CDPROBE_MAX_GPUS + (uint32_t)target[li], out);
     }
   }
-  out->ms = cdp::now_ms() - t_begin;
+  out->ms = cdp::now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }
 
 int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
-  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
-  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
-  const cdp::Plan& pl = h->plan;
-  const uint32_t n = h->n_total;
-  out->n = n;
-  out->path = h->path;
-  reps = out->reps;
-  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
-  // 1. the arguments, the armed fault and the mapping verdict; in a multi-process domain all three are shared below,
-  //    so every process refuses, skips or runs together
-  uint64_t size[cdp::kBwMaxSizes];
-  uint32_t n_sizes;
-  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
-  uint32_t f_rank = cdp::kArNoFault, f_k = cdp::kArNoFault;
-  uint64_t f_word = 0;
-  if (h->ar_fault != 0 && bad.empty()) {
-    const uint64_t fr = h->ar_fault >> 32, fk = (h->ar_fault >> 24) & 0xffu;
-    f_word = h->ar_fault & 0xffffffu;
-    if (fr == 0 || fr > n || fk == 0 || fk > n_sizes || f_word >= size[fk - 1] / 8) {
-      bad = "the armed all-reduce fault names no rank, size or output word of this call";
-    } else {
-      f_rank = (uint32_t)fr - 1;
-      f_k = (uint32_t)fk - 1;
-    }
-  }
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_allreduce", bad, h->ar_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
-    return rc;
-  out->call_seq = ++h->ar_calls;
-  cdp::put_ladder(h, size, n_sizes, out);
-  // when some rank cannot read some input nothing runs, in any process
-  if (cdp::skip_rows(h, st, out)) {
-    out->ms = cdp::now_ms() - t_begin;
-    return CDPROBE_OK;
-  }
-
-  // 2. scratch for the records, the output and the granule table, grown on every local rank before any kernel runs
-  const size_t table_off = cdp::kArOutOff + (pl.bpp + 255) / 256 * 256;
-  const size_t scratch = table_off + 16 * (pl.bpp / cdp::kGranuleBytes);
-  if (const int rc = cdp::ensure_scratch_all(h, scratch); rc != CDPROBE_OK) return rc;
-
-  // 3. the (S, X) every prefix of the output must have, from the pattern definition: the per-granule sums of the
-  //    summed words on the first local rank's GPU, folded into every prefix on the host
-  uint64_t want[cdp::kBwMaxSizes][2] = {};
-  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
-                                        "cdprobe_allreduce: granule checksums");
-      rc != CDPROBE_OK)
-    return rc;
-
-  // 4. no process launches before every process is ready, so that no kernel waits at the first domain barrier for a
-  //    process still setting up; then every local kernel is launched before any is waited for
-  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    cdp::AllReduceParams p;
-    memset(&p, 0, sizeof(p));
-    for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + pl.src_off;
-    for (uint32_t j = 0; j < n; ++j) {
-      if (j == g) continue;
-      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kArOff + (uint64_t)g * sizeof(cdp::FlagLine));
-      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kArOff + (uint64_t)j * sizeof(cdp::FlagLine));
-    }
-    p.dom.call_seq = h->ar_calls;
-    p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
-    p.seed = h->seed;
-    p.fault_k = g == f_rank ? f_k : cdp::kArNoFault;
-    p.fault_word = f_word;
-    p.rank = g;
-    p.n = n;
-    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_launch, "launch allreduce_kernel");
-        rc != CDPROBE_OK)
-      return rc;
-  }
-
-  // 5. collect: per row, the times and checksums of every size, then the word checks
-  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce", out); rc != CDPROBE_OK)
-    return rc;
-  out->ms = cdp::now_ms() - t_begin;
-  return CDPROBE_OK;
+  return cdp::allreduce_call(h, reps, out, cdp::kOneShot);
 }
 
 int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
-  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
-  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
-  const cdp::Plan& pl = h->plan;
-  const uint32_t n = h->n_total;
-  out->n = n;
-  out->path = h->path;
-  reps = out->reps;
-  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
-  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
-  //    every process refuses, skips or runs together.  The fault acts in the rank whose chunk holds its word
-  uint64_t size[cdp::kBwMaxSizes];
-  uint32_t n_sizes;
-  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
-  uint32_t f_owner = cdp::kArNoFault, f_recv = 0, f_k = cdp::kArNoFault, f_drop = 0;
-  uint64_t f_word = 0;
-  if (h->ar2_fault != 0 && bad.empty()) {
-    const uint64_t v = h->ar2_fault, fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu;
-    f_word = v & 0xffffffu;
-    if ((v >> 49) != 0 || fr == 0 || fr > n || fk == 0 || fk > n_sizes || f_word >= size[fk - 1] / 8) {
-      bad = "the armed two-shot all-reduce fault names no receiver, size or output word of this call";
-    } else {
-      f_recv = (uint32_t)fr - 1;
-      f_k = (uint32_t)fk - 1;
-      f_drop = (uint32_t)(v >> 48);
-      const uint64_t units = (size[f_k] + cdp::kUnitBytes - 1) / cdp::kUnitBytes, u = f_word / (cdp::kUnitBytes / 8);
-      for (uint32_t r = 0; r < n; ++r) {
-        uint64_t lo, hi;
-        cdp::twoshot_chunk(units, n, r, &lo, &hi);
-        if (u >= lo && u < hi) f_owner = r;
-      }
-    }
-  }
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_allreduce_twoshot", bad, h->ar2_calls + 1, {reps, 0u, 0u}, st);
-      rc != CDPROBE_OK)
-    return rc;
-  // 2. the gather area, built once, by every process in the same call
-  if (const int rc = cdp::ensure_area(h, h->gather, pl.bpp, h->gather_status); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++h->ar2_calls;
-  cdp::put_ladder(h, size, n_sizes, out);
-  // 3. every rank reads every source buffer and writes every gather area: when some probe mapping or gather-area
-  //    mapping of the domain is down, nothing runs, in any process
-  for (uint32_t s = 0; s < n; ++s)
-    for (uint32_t d = 0; d < n; ++d)
-      if (st[s][d] == 0) st[s][d] = h->gather_status[s][d];
-  if (cdp::skip_rows(h, st, out)) {
-    out->ms = cdp::now_ms() - t_begin;
-    return CDPROBE_OK;
-  }
-
-  // 4. scratch for the records and the granule table, grown on every local rank before any kernel runs; the (S, X)
-  //    every prefix of the output must have, as for the one-shot
-  const size_t table_off = cdp::kArOutOff;
-  if (const int rc = cdp::ensure_scratch_all(h, table_off + 16 * (pl.bpp / cdp::kGranuleBytes)); rc != CDPROBE_OK)
-    return rc;
-  uint64_t want[cdp::kBwMaxSizes][2] = {};
-  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
-                                        "cdprobe_allreduce_twoshot: granule checksums");
-      rc != CDPROBE_OK)
-    return rc;
-
-  // 5. no process launches before every process is ready; then every local kernel is launched before any is waited for
-  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    cdp::TwoShotParams p;
-    memset(&p, 0, sizeof(p));
-    for (uint32_t t = 0; t < n; ++t) {
-      p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + pl.src_off;
-      p.dst[t] = reinterpret_cast<uint8_t*>(L.gather_va[(g + t) % n]);
-    }
-    for (uint32_t j = 0; j < n; ++j) {
-      if (j == g) continue;
-      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kAr2Off + (uint64_t)g * sizeof(cdp::FlagLine));
-      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kAr2Off + (uint64_t)j * sizeof(cdp::FlagLine));
-    }
-    p.dom.call_seq = h->ar2_calls;
-    p.seed = h->seed;
-    p.fault_k = g == f_owner ? f_k : cdp::kArNoFault;
-    p.fault_word = f_word;
-    p.fault_dst = (f_recv + n - g) % n;
-    p.fault_drop = f_drop;
-    p.rank = g;
-    p.n = n;
-    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_twoshot_launch,
-                                          "launch allreduce_twoshot_kernel");
-        rc != CDPROBE_OK)
-      return rc;
-  }
-
-  // 6. collect: per row, the times and every rep's checksums, then the word checks of every rep
-  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce_twoshot", out);
-      rc != CDPROBE_OK)
-    return rc;
-  out->ms = cdp::now_ms() - t_begin;
-  return CDPROBE_OK;
+  return cdp::allreduce_call(h, reps, out, cdp::kTwoShot);
 }
 
 int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
-  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
-  out->reps = reps != 0 ? reps : cdp::kArDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
-  const cdp::Plan& pl = h->plan;
-  const uint32_t n = h->n_total;
-  out->n = n;
-  out->path = CDPROBE_ALLREDUCE_PATH_LL;
-  reps = out->reps;
-  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
-  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
-  //    every process refuses, skips or runs together.  The fault acts in the process that hosts its sender
-  uint64_t size[cdp::kBwMaxSizes];
-  uint32_t n_sizes;
-  std::string bad = cdp::ladder(h, reps, size, &n_sizes, cdp::ll_ladder);
-  uint32_t f_send = cdp::kArNoFault, f_recv = 0, f_k = cdp::kArNoFault, f_mode = 0;
-  uint64_t f_arg = 0;
-  if (h->ll_fault != 0 && bad.empty()) {
-    const uint64_t v = h->ll_fault, mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu,
-                   fk = (v >> 24) & 0xffu;
-    f_arg = v & 0xffffffu;
-    if (mode > 1 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > n_sizes ||
-        (mode == 0 && (fs == fr || f_arg >= size[fk - 1] / 8)) ||
-        (mode == 1 && 2 * f_arg >= 1000ull * h->cfg.timeout_ms)) {
-      bad = "the armed LL all-reduce fault names no packet, size or delay of this call";
-    } else {
-      f_send = (uint32_t)fs - 1;
-      f_recv = (uint32_t)fr - 1;
-      f_k = (uint32_t)fk - 1;
-      f_mode = (uint32_t)mode;
-    }
-  }
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_allreduce_ll", bad, h->ll_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
-    return rc;
-  // 2. the LL area, built once, by every process in the same call; it is zeroed before its first use
-  const uint64_t s_max = size[n_sizes - 1];
-  const bool fresh = h->ll.bytes == 0;
-  if (const int rc = cdp::ensure_area(h, h->ll, cdp::ll_area_bytes(n, s_max), h->ll_status); rc != CDPROBE_OK)
-    return rc;
-  h->ll_dirty |= fresh;
-  out->call_seq = ++h->ll_calls;
-  cdp::put_ladder(h, size, n_sizes, out);
-  // 3. every rank reads its own source buffer and writes every LL area: when some probe mapping or LL-area mapping of
-  //    the domain is down, nothing runs, in any process
-  for (uint32_t s = 0; s < n; ++s)
-    for (uint32_t d = 0; d < n; ++d)
-      if (st[s][d] == 0) st[s][d] = h->ll_status[s][d];
-  if (cdp::skip_rows(h, st, out)) {
-    out->ms = cdp::now_ms() - t_begin;
-    return CDPROBE_OK;
-  }
-
-  // 4. the domain's smallest grid, which splits the words alike on every rank (DESIGN §5j), and whether any process
-  //    has an LL area that a timed-out call may have left holding packets of any earlier call: then every process
-  //    zeroes its local ranks' areas before any kernel of this call can push into them
-  struct {
-    uint32_t ctas, dirty;
-  } mine = {UINT32_MAX, h->ll_dirty ? 1u : 0u}, all[cdp::kMaxRanks];
-  for (uint32_t li = 0; li < h->n_local; ++li) mine.ctas = std::min(mine.ctas, h->lr[li].ctas);
-  all[0] = mine;
-  if (h->cfg.world_size > 1) {
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all, &err) != 0) {
-      cdp::set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-  }
-  uint32_t grid = UINT32_MAX;
-  bool dirty = false;
-  for (uint32_t r = 0; r < std::max(h->cfg.world_size, 1u); ++r) {
-    grid = std::min(grid, all[r].ctas);
-    dirty |= all[r].dirty != 0;
-  }
-  if (dirty) {
-    for (uint32_t li = 0; li < h->n_local; ++li) {
-      cdp::LocalRank& L = h->lr[li];
-      CDP_RT(cudaSetDevice(L.ordinal));
-      cudaError_t e = cudaMemsetAsync(reinterpret_cast<void*>(L.ll_va[L.grank]), 0, h->ll.bytes, L.stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
-      if (e != cudaSuccess) return cdp::fail_sticky(h, "cdprobe_allreduce_ll: zero the LL area", e);
-    }
-    h->ll_dirty = false;
-  }
-
-  // 5. scratch for the records, the output and the granule table, grown on every local rank before any kernel runs;
-  //    the (S, X) every prefix of the output must have, as for the one-shot
-  const size_t table_off = cdp::kArOutOff + (s_max + 255) / 256 * 256;
-  if (const int rc = cdp::ensure_scratch_all(h, table_off + 16 * (pl.bpp / cdp::kGranuleBytes)); rc != CDPROBE_OK)
-    return rc;
-  uint64_t want[cdp::kBwMaxSizes][2] = {};
-  if (const int rc = cdp::expected_sums(h, h->lr[0], table_off, cdp::AllReduceWord{h->seed, n}, size, n_sizes, want,
-                                        "cdprobe_allreduce_ll: granule checksums");
-      rc != CDPROBE_OK)
-    return rc;
-
-  // 6. no process launches before every process is ready; then every local kernel is launched before any is waited for
-  if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    cdp::LlParams p;
-    memset(&p, 0, sizeof(p));
-    p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + pl.src_off;
-    for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.ll_va[(g + t) % n]);
-    p.in = reinterpret_cast<const uint8_t*>(L.ll_va[g]);
-    for (uint32_t j = 0; j < n; ++j) {
-      if (j == g) continue;
-      p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kLlOff + (uint64_t)g * sizeof(cdp::FlagLine));
-      p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kLlOff + (uint64_t)j * sizeof(cdp::FlagLine));
-    }
-    p.dom.call_seq = h->ll_calls;
-    p.out = static_cast<uint8_t*>(L.scratch) + cdp::kArOutOff;
-    p.s_max = s_max;
-    p.seed = h->seed;
-    p.fault_k = g == f_send ? f_k : cdp::kArNoFault;
-    p.fault_mode = f_mode;
-    p.fault_dst = (f_recv + n - g) % n;
-    p.fault_arg = f_arg;
-    p.rank = g;
-    p.n = n;
-    p.ctas = grid;
-    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::allreduce_ll_launch,
-                                          "launch allreduce_ll_kernel");
-        rc != CDPROBE_OK)
-      return rc;
-  }
-
-  // 7. collect: per row, the times and every rep's checksums, then the word check of the last rep; a row that timed
-  //    out leaves its LL area to be zeroed before the next call
-  if (const int rc = cdp::collect_rows(h, want, size, n_sizes, reps, "cdprobe_allreduce_ll", out); rc != CDPROBE_OK)
-    return rc;
-  for (uint32_t li = 0; li < h->n_local; ++li) h->ll_dirty |= out->status[h->lr[li].grank] == CDPROBE_ERR_TIMEOUT;
-  out->ms = cdp::now_ms() - t_begin;
-  return CDPROBE_OK;
+  return cdp::allreduce_call(h, reps, out, cdp::kLl);
 }
 
 int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
-  if (!cdp::begin_output(out)) return CDPROBE_ERR_ARG;
-  out->reps = reps != 0 ? reps : cdp::kA2aDefaultReps;
-  if (h == nullptr) return CDPROBE_ERR_ARG;
-  const double t_begin = cdp::now_ms();
+  cdp::Ladder lad;
+  if (const int rc = cdp::open_ladder(h, out, reps, cdp::kA2aDefaultReps, &lad); rc != CDPROBE_OK) return rc;
   const cdp::Plan& pl = h->plan;
   const uint32_t n = h->n_total;
-  out->n = n;
-  out->path = h->path;
-  reps = out->reps;
-  if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
   // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
   //    every process refuses or runs together over the same cells
-  uint64_t size[cdp::kBwMaxSizes];
-  uint32_t n_sizes;
-  std::string bad = cdp::ladder(h, reps, size, &n_sizes);
   uint32_t f_send = cdp::kA2aNoFault, f_recv = cdp::kA2aNoFault, f_k = cdp::kA2aNoFault;
   uint64_t f_word = 0;
-  if (h->a2a_fault != 0 && bad.empty()) {
+  if (h->a2a_fault != 0 && lad.bad.empty()) {
     const uint64_t fs = h->a2a_fault >> 40, fr = (h->a2a_fault >> 32) & 0xffu, fk = (h->a2a_fault >> 24) & 0xffu;
     f_word = h->a2a_fault & 0xffffffu;
-    if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || fk == 0 || fk > n_sizes ||
-        f_word >= size[fk - 1] / 8) {
-      bad = "the armed all-to-all fault names no cell, size or word of this call";
+    if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || fk == 0 || fk > lad.n_sizes ||
+        f_word >= lad.size[fk - 1] / 8) {
+      lad.bad = "the armed all-to-all fault names no cell, size or word of this call";
     } else {
       f_send = (uint32_t)fs - 1;
       f_recv = (uint32_t)fr - 1;
@@ -1123,20 +1045,21 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     }
   }
   int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_alltoall", bad, h->a2a_calls + 1, {reps, 0u, 0u}, st); rc != CDPROBE_OK)
+  if (const int rc = cdp::agree(h, "cdprobe_alltoall", lad.bad, h->a2a_calls + 1, {lad.reps, 0u, 0u}, st);
+      rc != CDPROBE_OK)
     return rc;
   // 2. the exchange area, built once, by every process in the same call
-  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp, h->area_status); rc != CDPROBE_OK) return rc;
+  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
   out->call_seq = ++h->a2a_calls;
   out->area_bytes = h->area.bytes;
-  cdp::put_ladder(h, size, n_sizes, out);
+  cdp::put_ladder(h, lad, out);
 
   // 3. which cells run: st[s][d], the probe mapping status of sender s's cell to receiver d, or else its exchange-area
   //    mapping status; 0 runs.  Every process derives the same matrix.
   bool any = false;
   for (uint32_t s = 0; s < n; ++s) {
     for (uint32_t d = 0; d < n; ++d) {
-      if (st[s][d] == 0) st[s][d] = h->area_status[s][d];
+      if (st[s][d] == 0) st[s][d] = h->area.status[s][d];
       if (s == d && !pl.diag) st[s][d] = CDPROBE_ERR_ARG;  // no such cell
       any |= st[s][d] == 0;
     }
@@ -1152,7 +1075,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     }
   }
   if (!any) {  // e.g. MIG instances: nothing to exchange anywhere, so no kernel is launched in any process
-    out->ms = cdp::now_ms() - t_begin;
+    out->ms = cdp::now_ms() - lad.t_begin;
     return CDPROBE_OK;
   }
 
@@ -1202,7 +1125,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     p.seed = h->seed;
     p.rank = g;
     out->blocks[g] = p.blocks;
-    if (const int rc = cdp::launch_ladder(h, L, p, size, n_sizes, reps, cdp::alltoall_launch, "launch alltoall_kernel");
+    if (const int rc = cdp::launch_ladder(h, L, p, lad, cdp::alltoall_launch, "launch alltoall_kernel");
         rc != CDPROBE_OK)
       return rc;
     launched[li] = true;
@@ -1216,7 +1139,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     const uint32_t g = L.grank;
     if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_alltoall"); rc != CDPROBE_OK) return rc;
     const cdp::A2aScratch& s = *got;
-    const bool timed = cdp::bw_times(s.rep, size, n_sizes, reps, (double)out->blocks[g], g, out);
+    const bool timed = cdp::bw_times(s.rep, lad.size, lad.n_sizes, lad.reps, (double)out->blocks[g], g, out);
     for (uint32_t i = 0; i < n; ++i) {
       if (!runs(i, g)) continue;
       const uint32_t cell = i * CDPROBE_MAX_GPUS + g;
@@ -1225,7 +1148,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
         out->cell_status[cell] = CDPROBE_ERR_TIMEOUT;
         continue;
       }
-      for (uint32_t k = 0; k < n_sizes; ++k) {
+      for (uint32_t k = 0; k < lad.n_sizes; ++k) {
         out->bad_words[cell][k] = s.bad_words[i][k];
         out->first_bad[cell][k] = s.bad_words[i][k] != 0 ? ~s.first_bad_n[i][k] : UINT64_MAX;
         out->sum[cell][k] = s.sum[i][k];
@@ -1235,7 +1158,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
       out->cell_status[cell] = out->bad_sizes[cell] ? CDPROBE_ERR_INTEGRITY : 0;
     }
   }
-  out->ms = cdp::now_ms() - t_begin;
+  out->ms = cdp::now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }
 

@@ -1,8 +1,8 @@
 """What every on-demand measurement does when it refuses a call: the return code, the exact cdprobe_last_error() text,
 an output that holds the ABI version and the prologue fields the call fills before it refuses (everything else zero),
 and a call number that a refusal does not advance.  Where one call has two reasons to refuse, the one that wins is
-fixed: pingpong reports an invalid armed fault instead of its argument error, while atomics, all-reduce and
-all-to-all report the argument error.  Two processes refuse together: the one with invalid arguments gets its own
+fixed: pingpong reports an invalid armed fault instead of its argument error, while atomics, the three all-reduces
+and all-to-all report the argument error.  Two processes refuse together: the one with invalid arguments gets its own
 message, the other is told another process was at fault, and arguments that differ refuse both."""
 import ctypes as C
 import json
@@ -13,6 +13,7 @@ import uuid
 
 import pytest
 
+import allreduce_ll_ref
 import bwcurve_ref
 from conftest import ROOT
 
@@ -31,6 +32,8 @@ FAULT_PINGPONG_CELL = "the armed pingpong fault names no off-diagonal cell"
 FAULT_PINGPONG_TRIP = "the armed pingpong fault's trip must be below trips - 1, and below trips - 2 when reps is 1"
 FAULT_ATOMICS = "the armed atomics fault names no cell of this domain"
 FAULT_ALLREDUCE = "the armed all-reduce fault names no rank, size or output word of this call"
+FAULT_TWOSHOT = "the armed two-shot all-reduce fault names no receiver, size or output word of this call"
+FAULT_LL = "the armed LL all-reduce fault names no packet, size or delay of this call"
 FAULT_ALLTOALL = "the armed all-to-all fault names no cell, size or word of this call"
 
 
@@ -146,22 +149,27 @@ def test_atomics_reports_its_arguments_over_an_invalid_fault(pkg, probe):
     atomics_refusal(pkg, probe, a.ATOMIC_FETCH_ADD, 64, 65, ARGS_ATOMICS, (a.OPT_ATOMICS_FAULT, a.atomics_fault(0, 0)))
 
 
-# ---- bwcurve, all-reduce and all-to-all: the size ladder -------------------------------------------------------------
+# ---- bwcurve, the all-reduces and all-to-all: the size ladder --------------------------------------------------------
+
+LADDER_CALLS = ["bwcurve", "allreduce", "allreduce_twoshot", "allreduce_ll", "alltoall"]
+
 
 def ladder_refusal(pkg, p, what, reps, message, fault=None):
     a = pkg.abi
-    call = {"bwcurve": p.BwCurve, "allreduce": p.AllReduce, "alltoall": p.AllToAll}[what]
-    raw = {"bwcurve": p.bwcurve_raw, "allreduce": p.allreduce_raw, "alltoall": p.alltoall_raw}[what]
-    cls = {"bwcurve": a.BwCurveT, "allreduce": a.AllReduceT, "alltoall": a.AllToAllT}[what]
+    call = {"bwcurve": p.BwCurve, "allreduce": p.AllReduce, "allreduce_twoshot": p.AllReduceTwoShot,
+            "allreduce_ll": p.AllReduceLL, "alltoall": p.AllToAll}[what]
+    raw = getattr(p, what + "_raw")
+    cls = {"bwcurve": a.BwCurveT, "alltoall": a.AllToAllT}.get(what, a.AllReduceT)
+    path = a.ALLREDUCE_PATH_LL if what == "allreduce_ll" else 0
     seq = call(reps=1).call_seq
     disarm = arm(p, fault)
     rc, t = raw(reps)
-    check_refused(p, rc, t, message, expect(cls, n=N, reps=reps or 8, path=0))
+    check_refused(p, rc, t, message, expect(cls, n=N, reps=reps or 8, path=path))
     disarm()
     assert call(reps=1).call_seq == seq + 1
 
 
-@pytest.mark.parametrize("what", ["bwcurve", "allreduce", "alltoall"])
+@pytest.mark.parametrize("what", LADDER_CALLS)
 def test_ladder_calls_refuse_their_reps(pkg, probe, what):
     ladder_refusal(pkg, probe, what, 65, ARGS_REPS)
     ladder_refusal(pkg, probe, what, 1 << 31, ARGS_REPS)
@@ -175,6 +183,27 @@ def test_allreduce_refuses_an_armed_fault(pkg, probe):
         ladder_refusal(pkg, probe, "allreduce", 2, FAULT_ALLREDUCE, (a.OPT_ALLREDUCE_FAULT, fault))
 
 
+def test_allreduce_twoshot_refuses_an_armed_fault(pkg, probe):
+    a = pkg.abi
+    sizes = bwcurve_ref.ladder(bpp(pkg))
+    for fault in (a.allreduce_twoshot_fault(N, 0, 0), a.allreduce_twoshot_fault(0, len(sizes), 0),
+                  a.allreduce_twoshot_fault(0, 0, sizes[0] // 8), (1 << 24) | 5, (1 << 32) | 5,
+                  (1 << 49) | a.allreduce_twoshot_fault(0, 0, 0), (1 << 63) | a.allreduce_twoshot_fault(1, 1, 1)):
+        ladder_refusal(pkg, probe, "allreduce_twoshot", 2, FAULT_TWOSHOT, (a.OPT_ALLREDUCE_TWOSHOT_FAULT, fault))
+
+
+def test_allreduce_ll_refuses_an_armed_fault(pkg, probe):
+    """On LL's own ladder; a delay of 10 s is half the handle's 20 s timeout, which LL refuses."""
+    a = pkg.abi
+    sizes = allreduce_ll_ref.ladder(bpp(pkg))
+    for fault in (a.allreduce_ll_fault(N, 0, 0, 0), a.allreduce_ll_fault(0, N, 0, 0),
+                  a.allreduce_ll_fault(0, 1, len(sizes), 0), a.allreduce_ll_fault(0, 1, 0, sizes[0] // 8),
+                  a.allreduce_ll_fault(1, 1, 0, 0), a.allreduce_ll_fault(0, 1, 0, 10_000_000, mode=1),
+                  (2 << 48) | a.allreduce_ll_fault(0, 1, 0, 0), (1 << 63) | a.allreduce_ll_fault(0, 1, 0, 0),
+                  (1 << 24) | 5):
+        ladder_refusal(pkg, probe, "allreduce_ll", 2, FAULT_LL, (a.OPT_ALLREDUCE_LL_FAULT, fault))
+
+
 def test_alltoall_refuses_an_armed_fault(pkg, probe):
     a = pkg.abi
     sizes = bwcurve_ref.ladder(bpp(pkg))
@@ -183,11 +212,13 @@ def test_alltoall_refuses_an_armed_fault(pkg, probe):
         ladder_refusal(pkg, probe, "alltoall", 2, FAULT_ALLTOALL, (a.OPT_ALLTOALL_FAULT, fault))
 
 
-@pytest.mark.parametrize("what", ["allreduce", "alltoall"])
+@pytest.mark.parametrize("what", LADDER_CALLS[1:])
 def test_ladder_calls_report_their_reps_over_an_invalid_fault(pkg, probe, what):
     a = pkg.abi
-    fault = ((a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(N, 0, 0)) if what == "allreduce"
-             else (a.OPT_ALLTOALL_FAULT, a.alltoall_fault(0, 0, 0, 0)))
+    fault = {"allreduce": (a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(N, 0, 0)),
+             "allreduce_twoshot": (a.OPT_ALLREDUCE_TWOSHOT_FAULT, a.allreduce_twoshot_fault(N, 0, 0)),
+             "allreduce_ll": (a.OPT_ALLREDUCE_LL_FAULT, a.allreduce_ll_fault(N, 0, 0, 0)),
+             "alltoall": (a.OPT_ALLTOALL_FAULT, a.alltoall_fault(0, 0, 0, 0))}[what]
     ladder_refusal(pkg, probe, what, 65, ARGS_REPS, fault)
 
 
@@ -206,7 +237,8 @@ CHILD = textwrap.dedent(
     with m.Open(cfg) as p:
         lib = p._lib
         calls = {"pingpong": lambda reps: p.pingpong_raw(64, reps, 0), "bwcurve": p.bwcurve_raw,
-                 "allreduce": p.allreduce_raw, "alltoall": p.alltoall_raw}
+                 "allreduce": p.allreduce_raw, "allreduce_twoshot": p.allreduce_twoshot_raw,
+                 "allreduce_ll": p.allreduce_ll_raw, "alltoall": p.alltoall_raw}
         for name, call in calls.items():
             got = []
             for reps in (65 if rank == 0 else 2, 2 + rank, 2):  # invalid in one process, then different, then alike
@@ -240,7 +272,7 @@ def run_processes(world):
 def test_two_processes_refuse_together():
     outs = run_processes(2)
     for rank, o in enumerate(outs):
-        for name in ("pingpong", "bwcurve", "allreduce", "alltoall"):
+        for name in ["pingpong"] + LADDER_CALLS:
             fn = "cdprobe_" + name
             own = ARGS_PINGPONG if name == "pingpong" else ARGS_REPS
             bad, differ, ok = o[name]
