@@ -402,11 +402,12 @@ typedef struct {
   uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
   uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
   uint32_t n_sizes;                     /* entries of size[] */
-  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH); cdprobe_allreduce_ll has one
-                                           data path, ignores CDPROBE_OPT_PATH and reports CDPROBE_ALLREDUCE_PATH_LL */
+  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH); cdprobe_allreduce_ll and
+                                           cdprobe_allreduce_ring have one data path each, ignore CDPROBE_OPT_PATH and
+                                           report CDPROBE_ALLREDUCE_PATH_LL and CDPROBE_ALLREDUCE_PATH_RING */
   uint64_t call_seq;                    /* 1-based count of cdprobe_allreduce calls on this handle, equal in every
-                                           process (0 when the call was refused); of cdprobe_allreduce_twoshot or
-                                           cdprobe_allreduce_ll calls for those */
+                                           process (0 when the call was refused); of cdprobe_allreduce_twoshot,
+                                           cdprobe_allreduce_ll or cdprobe_allreduce_ring calls for those */
   uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per input and of the output per rep: the cdprobe_bwcurve ladder */
   uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank ran */
   int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) or the word check differs from
@@ -432,6 +433,8 @@ typedef struct {
 } cdprobe_allreduce_t;
 /* cdprobe_allreduce_t.path of cdprobe_allreduce_ll: flag-carrying 16-byte packets (DESIGN §5j) */
 #define CDPROBE_ALLREDUCE_PATH_LL 3u
+/* cdprobe_allreduce_t.path of cdprobe_allreduce_ring: 16-byte ld/st, one flag per 8 KiB unit (DESIGN §5k) */
+#define CDPROBE_ALLREDUCE_PATH_RING 4u
 
 /* One-shot all-to-all across the domain (cdprobe_alltoall): every rank pushes one block to every peer at once, into the
  * peer's exchange area, and every rank checks every word it receives (DESIGN §5h).  Per-rank entries [r] describe rank
@@ -503,11 +506,11 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_alltoall:
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_alltoall:
  *   diagnostics, benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll and cdprobe_alltoall are optional for callers: a daemon binds
- *   them with dlsym and works without.
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring and cdprobe_alltoall are optional for
+ *   callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -568,6 +571,16 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              its data xored with 1 and the right flags, so exactly that receiver's row
                                              fails at that size; mode 1, the sender waits `arg` us (< timeout_ms / 2)
                                              before its first push of the rep, and every row stays exact; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_RING_FAULT 23u /* tests: value = (mode << 48) | (phase << 40) | ((sender + 1) << 32) |
+                                             ((k + 1) << 24) | arg arms a fault in cdprobe_allreduce_ring, in timed rep
+                                             1 of size[k], in the process that hosts `sender`, in phase 0 (the
+                                             reduce-scatter) or 1 (the all-gather): mode 0, the sender's push of word
+                                             `arg` (< 2^24) to its successor carries it xored with 1 and the right
+                                             flag; mode 1, the push stores nothing of the word's 8 KiB unit but still
+                                             publishes its flag; mode 2, the sender waits `arg` us (< timeout_ms / 2)
+                                             before its first push of the rep, and every row stays exact.  Modes 0 and
+                                             1 fail every row in phase 0, and in phase 1 the rows from sender + 1 up to
+                                             the rank before the word's chunk owner; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -745,6 +758,36 @@ CDPROBE_API int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_a
  * >= n_sizes, whose mode is above 1, whose mode-0 receiver is its sender or word is >= size[k] / 8, or whose mode-1
  * delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* Ring all-reduce of every rank's source buffer, on every rank at once: each rank talks only to its successor
+ * r + 1 (mod n), to which it pushes, and its predecessor r - 1, which pushes to it.  For each size of the
+ * cdprobe_bwcurve ladder, one untimed warm-up rep and `reps` timed reps.  The size is cut into cdprobe_allreduce_twoshot's
+ * n chunks of 8 KiB units, and a rep is 2 (n - 1) steps: in the reduce-scatter, step s pushes the partial sum of chunk
+ * (r - 1 - s) mod n (the received partial plus rank r's own input) into the successor's ring area, so that rank r
+ * ends it holding the full sum of chunk r; in the all-gather, step s pushes the full chunk (r - s) mod n on.  Every
+ * 8 KiB unit goes with st.global.v4 and is published by its own flag (st.release.sys) that the receiver polls
+ * (ld.acquire.sys) before it reads the unit: no barrier and no fence across the domain between the steps, so a flag
+ * that overtook its data would leave stale or zero words.  A fenced domain barrier opens every rep (flags in the Ctrl
+ * granule; only a grid barrier at n == 1, where the rank stores its own input into its output).  A rep is timed per
+ * rank by %globaltimer from its opening release to the moment its output is complete and its pushes are issued, so a
+ * slow hop stretches every rank's rep.  After every rep, warm-up included and untimed, each rank reads back every word
+ * of its output, compares it with the pattern's sum and overwrites it with 0, as cdprobe_allreduce_twoshot does; row
+ * r of *out is as cdprobe_allreduce_twoshot's.  peak_gbps is the algorithm bandwidth, size / ns; the bus bandwidth is
+ * peak_gbps x 2 (n - 1) / n, and each rank sends and receives 2 (n - 1) / n x size per rep over one link each.  The
+ * ring area (bytes_per_pair per rank plus one 32-bit flag per 8 KiB of it, rounded up to 2 MiB) is created on the
+ * first call with the probe allocation's handle type, zeroed, mapped wherever the probe mapping is then up, and kept
+ * until close; if creating it fails in any process, every process returns that error, nothing runs, and the next call
+ * tries again.  If any probe or ring-area mapping of the domain is down (cdprobe_unmap_peer, a failed mapping, MIG),
+ * nothing runs: every filled row has measured = 0 and the status of the first such cell, and the call returns
+ * CDPROBE_OK.  A rank whose kernel passes timeout_ms is CDPROBE_ERR_TIMEOUT with no times, the handle stays usable,
+ * and every ring area is zeroed before the next call runs.  Collective when world_size > 1: every process calls it
+ * with the same reps and fills the rows of its own ranks (row_mask); call_seq counts calls of this function.  Needs no
+ * run first and touches no result, pattern, source buffer, landing slot, run_seq, warm-up state, exchange, gather or
+ * LL area or other measurement's state.  *out carries abi, n, reps and path whatever the return code.
+ * CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes, or an
+ * armed CDPROBE_OPT_ALLREDUCE_RING_FAULT whose mode is above 2, whose phase is above 1, whose sender is >= n, whose k
+ * is >= n_sizes, whose mode-0 or mode-1 word is >= size[k] / 8, lies in a chunk the sender does not push in that phase
+ * or is armed at n == 1, or whose mode-2 delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -49,6 +49,7 @@ static ar_fn cdp_ar;      // optional: absent from libraries that predate cdprob
 static a2a_fn cdp_a2a;    // optional: absent from libraries that predate cdprobe_alltoall
 static ar_fn cdp_ar2;     // optional: absent from libraries that predate cdprobe_allreduce_twoshot
 static ar_fn cdp_arll;    // optional: absent from libraries that predate cdprobe_allreduce_ll
+static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprobe_allreduce_ring
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -69,6 +70,7 @@ static int cdp_load(const char* path) {
   cdp_a2a = (a2a_fn)dlsym(cdp_dl, "cdprobe_alltoall");
   cdp_ar2 = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_twoshot");
   cdp_arll = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ll");
+  cdp_arring = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ring");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -105,6 +107,10 @@ static int cdp_call_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allre
 }
 static int cdp_has_allreduce_ll(void) { return cdp_arll != NULL; }
 static int cdp_call_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) { return cdp_arll(h, reps, ar); }
+static int cdp_has_allreduce_ring(void) { return cdp_arring != NULL; }
+static int cdp_call_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
+  return cdp_arring(h, reps, ar);
+}
 */
 import "C"
 
@@ -276,8 +282,8 @@ type BwCurve struct {
 	Ms                     float64
 }
 
-// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot)
-// or the low-latency one's (AllReduceLL).
+// AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot),
+// the low-latency one's (AllReduceLL) or the ring's (AllReduceRing).
 // Every slice is indexed by rank; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
 // rank was not measured or timed out.
 type AllReduce struct {
@@ -711,6 +717,32 @@ func (p *Probe) AllReduceLL(reps int) (AllReduce, error) {
 	}
 	ll := allReduceOf(ar)
 	return ll, nil
+}
+
+// AllReduceRing runs the ring all-reduce of every rank's source buffer on every rank at once: each rank passes every
+// 8 KiB unit to the next rank under its own flag, 2(N - 1) steps of reduce-scatter and all-gather with no barrier or
+// fence between them, at each size of the bwcurve ladder, and reports ns per rep for each size (reps 0: 8 timed reps),
+// timed from the rep's opening barrier to the moment the rank's output is complete.  Path is
+// CDPROBE_ALLREDUCE_PATH_RING.  Collective when the domain spans processes.  ErrUnsupported when the library predates
+// cdprobe_allreduce_ring.
+func (p *Probe) AllReduceRing(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce_ring() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce_ring", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	res := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce_ring(p.h, C.uint32_t(reps), res)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce_ring: %s: %s", C.GoString(C.cdp_call_strerror(rc)),
+			C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	ring := allReduceOf(res)
+	return ring, nil
 }
 
 // allReduceOf copies a cdprobe_allreduce_t into an AllReduce.

@@ -183,5 +183,6 @@ func (*Probe) BwCurve(int) (BwCurve, error) { return BwCurve{}, ErrUnsupported }
 func (*Probe) AllReduce(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceTwoShot(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceLL(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllReduceRing(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -38,6 +38,7 @@ OPT_ALLREDUCE_FAULT = 19
 OPT_ALLTOALL_FAULT = 20
 OPT_ALLREDUCE_TWOSHOT_FAULT = 21
 OPT_ALLREDUCE_LL_FAULT = 22
+OPT_ALLREDUCE_RING_FAULT = 23
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -58,6 +59,7 @@ BWCURVE_MAX_SIZES = 24
 BWCURVE_DEFAULT_REPS, BWCURVE_MAX_REPS = 8, 64
 ALLREDUCE_DEFAULT_REPS, ALLREDUCE_MAX_REPS = 8, 64
 ALLREDUCE_PATH_LL = 3  # cdprobe_allreduce_t.path of cdprobe_allreduce_ll
+ALLREDUCE_PATH_RING = 4  # cdprobe_allreduce_t.path of cdprobe_allreduce_ring
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
@@ -416,6 +418,16 @@ def allreduce_ll_fault(sender: int, receiver: int, k: int, arg: int, mode: int =
     return (mode << 48) | ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | arg
 
 
+def allreduce_ring_fault(sender: int, k: int, arg: int, phase: int = 0, mode: int = 0) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_RING_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_ring, in phase 0
+    (the reduce-scatter) or 1 (the all-gather): mode 0, `sender`'s push of word `arg` to its successor carries it xored
+    with 1; mode 1, that push stores nothing of the word's unit but still publishes its flag; mode 2, `sender` waits
+    `arg` us before its first push of the rep.  Fields that do not fit are refused here."""
+    if mode not in (0, 1, 2) or phase not in (0, 1) or not (0 <= sender < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
+        raise ValueError("allreduce_ring_fault: mode 0, 1 or 2, phase 0 or 1, sender and k below 255, arg below 2^24")
+    return (mode << 48) | (phase << 40) | ((sender + 1) << 32) | ((k + 1) << 24) | arg
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -453,6 +465,7 @@ SYMBOLS = {
     "cdprobe_allreduce": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_twoshot": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_ll": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
+    "cdprobe_allreduce_ring": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

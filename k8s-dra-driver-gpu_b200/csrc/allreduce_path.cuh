@@ -3,7 +3,8 @@
 // units, streams unit u of all P.n inputs (TMA ring or ld.global.v4) and adds them in registers (64-bit, wrapping).
 // Two things are parameters: the walk (which units a warp sums) and the store policy (where a summed unit goes).
 // Also the word check of an output in the rank's scratch (ar_check), shared by the one-shot and allreduce_ll_kernel
-// (allreduce_ll_kernels.cu).
+// (allreduce_ll_kernels.cu), and the word check and clear of an output peers store into (ar_check_clear), shared by
+// the two-shot and allreduce_ring_kernel (allreduce_ring_kernels.cu).
 //
 // A store policy S has one member, called once per unit by every lane with the unit's sums in acc:
 //   template <uint32_t kLaneBytes> static void S::put(const Ctx&, const Params& P, uint64_t u, uint32_t len,
@@ -164,6 +165,50 @@ __device__ void ar_check(const Ctx& c, const Params& P, ArScratch* as, uint32_t 
     atomicAdd(&as->bad_words[k], (unsigned long long)bad);
     atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
   }
+}
+
+// The untimed check of rep r of size k of an output peers store into (allreduce_twoshot_kernel's gather area,
+// allreduce_ring_kernel's ring area): every word of it is read at L2 (peers and other SMs stored it), compared with
+// allreduce_word, folded into the rep's (S, X) by its place in the output, and then overwritten with 0, so a unit that
+// is not delivered in a later rep reads as 0s rather than as this rep's sums.  One atomic pair per warp with a bad
+// word, over every rep of the size.
+template <typename Params>
+__device__ void ar_check_clear(const Ctx& c, const Params& P, uint4* const out, ArScratch* as, uint64_t* red,
+                               uint32_t k, uint32_t r, uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {
+  Sum a{0ull, 0ull, 0ull};
+  uint64_t bad = 0, first = ~0ull;
+  Walk<false> walk = strided(bytes, gwarp, nwarps);
+  for (uint64_t u; walk.take(c, u);) {
+    uint4* const p = out + u * (kUnitBytes / 16);
+    const uint32_t nvec = unit_len(bytes, u) / 16;
+    const uint64_t w_base = u * (kUnitBytes / 8);
+    uint64_t ux = 0;
+#pragma unroll 4
+    for (uint32_t v = c.lane; v < nvec; v += 32) {
+      const uint4 q = __ldcg(p + v);
+      const uint64_t w0 = pack64(q.x, q.y), w1 = pack64(q.z, q.w), k0 = w_base + 2 * v;
+      if (w0 != allreduce_word(P.seed, P.n, k0)) {
+        ++bad;
+        first = min(first, 8 * k0);
+      }
+      if (w1 != allreduce_word(P.seed, P.n, k0 + 1)) {
+        ++bad;
+        first = min(first, 8 * k0 + 8);
+      }
+      add_pair(a, ux, w0, w1);
+      stg_v4(p + v, make_uint4(0u, 0u, 0u, 0u));
+    }
+    fold_unit(a, ux, u);
+  }
+  __threadfence();  // the clearing stores are performed before the next opening barrier signals the peers
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
+  Acc* const acc = &as->rep.rep[k][r];
+  cta_reduce<1>(c, red, &a, &acc);
 }
 }  // namespace
 }  // namespace cdp

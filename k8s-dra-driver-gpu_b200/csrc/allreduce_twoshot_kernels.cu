@@ -1,7 +1,7 @@
 // allreduce_twoshot_kernels.cu — sm_90a kernel of cdprobe_allreduce_twoshot's two-shot all-reduce: every rank sums its
 // chunk of units of all n source buffers with the one-shot's read-and-add side (allreduce_path.cuh) and pushes each
 // summed unit with st.global.v4 into every rank's gather area; a fenced domain barrier closes the rep, and every rank
-// then checks and clears its own gather area (allreduce_twoshot_kernel).
+// then checks and clears its own gather area (allreduce_twoshot_kernel, with allreduce_path.cuh's ar_check_clear).
 //
 // probe_kernels.cu is untouched: the probe kernel's code generation does not depend on this file.
 #include <cuda_runtime.h>
@@ -42,49 +42,6 @@ struct ToGather {
     for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
   }
 };
-
-// The untimed check of rep r of size k: every word of this rank's output (its gather area) is read at L2 (peers and
-// other SMs stored it), compared with allreduce_word, folded into the rep's (S, X) by its place in the output, and
-// then overwritten with 0, so a unit that is not delivered in a later rep reads as 0s rather than as this rep's sums.
-// One atomic pair per warp with a bad word, over every rep of the size.
-__device__ void ts_check(const Ctx& c, const TwoShotParams& P, ArScratch* as, uint64_t* red, uint32_t k, uint32_t r,
-                         uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {
-  uint4* const out = reinterpret_cast<uint4*>(P.dst[0]);
-  Sum a{0ull, 0ull, 0ull};
-  uint64_t bad = 0, first = ~0ull;
-  Walk<false> walk = strided(bytes, gwarp, nwarps);
-  for (uint64_t u; walk.take(c, u);) {
-    uint4* const p = out + u * (kUnitBytes / 16);
-    const uint32_t nvec = unit_len(bytes, u) / 16;
-    const uint64_t w_base = u * (kUnitBytes / 8);
-    uint64_t ux = 0;
-#pragma unroll 4
-    for (uint32_t v = c.lane; v < nvec; v += 32) {
-      const uint4 q = __ldcg(p + v);
-      const uint64_t w0 = pack64(q.x, q.y), w1 = pack64(q.z, q.w), k0 = w_base + 2 * v;
-      if (w0 != allreduce_word(P.seed, P.n, k0)) {
-        ++bad;
-        first = min(first, 8 * k0);
-      }
-      if (w1 != allreduce_word(P.seed, P.n, k0 + 1)) {
-        ++bad;
-        first = min(first, 8 * k0 + 8);
-      }
-      add_pair(a, ux, w0, w1);
-      stg_v4(p + v, make_uint4(0u, 0u, 0u, 0u));
-    }
-    fold_unit(a, ux, u);
-  }
-  __threadfence();  // the clearing stores are performed before the next opening barrier signals the peers
-  bad = warp_sum64(bad);
-  first = warp_min64(first);
-  if (c.lane == 0 && bad != 0) {
-    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
-    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
-  }
-  Acc* const acc = &as->rep.rep[k][r];
-  cta_reduce<1>(c, red, &a, &acc);
-}
 }  // namespace
 
 // One rank of cdprobe_allreduce_twoshot: for every size of the ladder, one warm-up and P.reps timed reps.  A rep opens
@@ -116,7 +73,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(const __
       __syncthreads();
       if (threadIdx.x == 0) __threadfence_system();  // every store of this CTA has reached its gather area
       if (!grid_barrier(c, bs, b++, &bs->rep[k][r].t_end, &P.dom, true)) return;
-      ts_check(c, P, as, red, k, r, bytes, gwarp, nwarps);
+      ar_check_clear(c, P, reinterpret_cast<uint4*>(P.dst[0]), as, red, k, r, bytes, gwarp, nwarps);
     }
   }
 }

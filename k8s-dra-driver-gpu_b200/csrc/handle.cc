@@ -478,6 +478,7 @@ static void destroy(cdprobe* h) {
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
   }
+  release_shared(h, h->ring);
   release_shared(h, h->ll);
   release_shared(h, h->gather);
   release_shared(h, h->area);
@@ -1076,6 +1077,10 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return CDPROBE_OK;
     case CDPROBE_OPT_ALLREDUCE_LL_FAULT:  // checked against the domain, the ladder and timeout_ms by cdprobe_allreduce_ll
       h->ll_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_RING_FAULT:  // checked against the domain, the ladder, the chunks and timeout_ms by
+                                            // cdprobe_allreduce_ring
+      h->ring_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

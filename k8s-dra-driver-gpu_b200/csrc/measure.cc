@@ -1,6 +1,6 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
-// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll and
-// cdprobe_alltoall.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
+// cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll,
+// cdprobe_allreduce_ring and cdprobe_alltoall.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
 // before it returns.
 #include <string.h>
 
@@ -12,6 +12,7 @@
 
 #include "allreduce.h"
 #include "allreduce_ll.h"
+#include "allreduce_ring.h"
 #include "allreduce_twoshot.h"
 #include "alltoall.h"
 #include "atomics.h"
@@ -397,10 +398,12 @@ static DomainLines domain_lines(const cdprobe* h, const LocalRank& L, uint64_t o
 }
 
 // An all-reduce's armed fault once its protocol has accepted it: in timed rep 1 of size k, rank `rank` (kArNoFault:
-// none) acts on word `word` towards receiver `recv`, in `mode`.  What each means is the protocol's.
+// none) acts on word `word` towards receiver `recv`, in `mode` (and, for the ring, in `phase`).  What each means is the
+// protocol's.
 struct ArFault {
   uint32_t rank = kArNoFault, recv = 0, k = kArNoFault, mode = 0;
   uint64_t word = 0;
+  uint32_t phase = 0;
 };
 
 // One all-reduce protocol, as allreduce_call runs it.
@@ -516,6 +519,48 @@ static int ll_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Lad
   return launch_ladder(h, L, p, lad, allreduce_ll_launch, "launch allreduce_ll_kernel");
 }
 
+// The fault acts in the process that hosts its sender.  A corrupted or dropped word must lie in a chunk the sender
+// pushes in that phase: every chunk but its own in the reduce-scatter, every chunk but its successor's in the
+// all-gather.
+static const char* ring_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint32_t n = h->n_total;
+  const uint64_t mode = v >> 48, phase = (v >> 40) & 0xffu, fs = (v >> 32) & 0xffu, fk = (v >> 24) & 0xffu,
+                 arg = v & 0xffffffu;
+  const char* why = "the armed ring all-reduce fault names no pushed word, size or delay of this call";
+  if (mode > 2 || phase > 1 || fs == 0 || fs > n || fk == 0 || fk > lad.n_sizes) return why;
+  const uint32_t s = (uint32_t)fs - 1, k = (uint32_t)fk - 1;
+  if (mode == 2 && 2 * arg >= 1000ull * h->cfg.timeout_ms) return why;
+  if (mode < 2) {
+    if (n == 1 || arg >= lad.size[k] / 8) return why;
+    const uint64_t units = (lad.size[k] + kUnitBytes - 1) / kUnitBytes, u = arg / (kUnitBytes / 8);
+    uint64_t lo, hi;
+    twoshot_chunk(units, n, phase == 0 ? s : (s + 1) % n, &lo, &hi);
+    if (u >= lo && u < hi) return why;
+  }
+  *f = {s, 0, k, (uint32_t)mode, arg, (uint32_t)phase};
+  return nullptr;
+}
+
+static int ring_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                       uint32_t) {
+  const uint32_t g = L.grank, n = h->n_total;
+  RingParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
+  p.out = reinterpret_cast<uint8_t*>(L.ring_va[g]);
+  p.next = reinterpret_cast<uint8_t*>(L.ring_va[(g + 1) % n]);
+  p.dom = dom;
+  p.s_max = lad.size[lad.n_sizes - 1];
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_mode = f.mode;
+  p.fault_phase = f.phase;
+  p.fault_arg = f.word;
+  p.rank = g;
+  p.n = n;
+  return launch_ladder(h, L, p, lad, allreduce_ring_launch, "launch allreduce_ring_kernel");
+}
+
 constexpr ArProtocol kOneShot = {
     "cdprobe_allreduce", &cdprobe::ar_calls, &cdprobe::ar_fault, bwcurve_ladder, kHandlePath, nullptr, nullptr,
     nullptr, true, kArOff, oneshot_fault, oneshot_launch};
@@ -526,8 +571,12 @@ constexpr ArProtocol kTwoShot = {
 constexpr ArProtocol kLl = {
     "cdprobe_allreduce_ll", &cdprobe::ll_calls, &cdprobe::ll_fault, ll_ladder, CDPROBE_ALLREDUCE_PATH_LL, &cdprobe::ll,
     ll_area_bytes, "cdprobe_allreduce_ll: zero the LL area", true, kLlOff, ll_fault, ll_launch};
+constexpr ArProtocol kRing = {
+    "cdprobe_allreduce_ring", &cdprobe::ring_calls, &cdprobe::ring_fault, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_RING,
+    &cdprobe::ring, ring_area_bytes, "cdprobe_allreduce_ring: zero the ring area", false, kRingOff, ring_fault,
+    ring_launch};
 
-// The all-reduces (DESIGN §5g, §5i, §5j): one call of protocol P.
+// The all-reduces (DESIGN §5g, §5i, §5j, §5k): one call of protocol P.
 static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, const ArProtocol& P) {
   Ladder lad;
   if (const int rc = open_ladder(h, out, reps, kArDefaultReps, &lad, P.path, P.rule); rc != CDPROBE_OK) return rc;
@@ -1021,6 +1070,10 @@ int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* 
 
 int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   return cdp::allreduce_call(h, reps, out, cdp::kLl);
+}
+
+int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  return cdp::allreduce_call(h, reps, out, cdp::kRing);
 }
 
 int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {

@@ -552,6 +552,30 @@ constexpr uint64_t kLlOff = kAr2Off + kMaxRanks * sizeof(FlagLine);  // 74 KiB
 static_assert(kLlOff % 128 == 0 && kLlOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
               "the LL all-reduce lines sit after the two-shot all-reduce lines inside the Ctrl granule");
 
+// ---- the ring all-reduce (cdprobe_allreduce_ring, DESIGN §5k) -------------------------------------------------------
+// The flag a sender publishes for a flag grain it pushed in rep r (0: the warm-up) of size k of call call_seq, in
+// phase 0 (the reduce-scatter) or 1 (the all-gather): ll_flag with the phase in its bit 7, which r + 1 <= 65 leaves
+// free.  So it is never 0, differs across (k, r, phase) within a call, and differs from every flag of the call before.
+CDP_HD inline uint32_t ring_flag(uint64_t call_seq, uint32_t k, uint32_t r, uint32_t phase) {
+  return ll_flag(call_seq, k, r) | ((phase & 1u) << 7);
+}
+// The units one flag covers: a sender publishes one flag per kRingFlagUnits units of a chunk, after storing them all.
+// One 8 KiB unit per flag: a system-scope release per unit costs little next to the unit's stores (DESIGN §5k).
+constexpr uint32_t kRingFlagUnits = 1;
+// A rank's ring area for a ladder whose largest size is s_max: the output, every unit at its place, then from
+// ring_flags_off one 32-bit flag per 8 KiB unit of s_max (flag u: the grain that starts at unit u).
+CDP_HD inline uint64_t ring_flags_off(uint64_t s_max) { return (s_max + 127) / 128 * 128; }
+CDP_HD inline uint64_t ring_flag_off(uint64_t s_max, uint64_t u) { return ring_flags_off(s_max) + 4 * u; }
+CDP_HD inline uint64_t ring_area_bytes(uint32_t, uint64_t s_max) {
+  return ring_flag_off(s_max, (s_max + kUnitBytes - 1) / kUnitBytes);
+}
+
+// The opening domain barrier of every rep of cdprobe_allreduce_ring: one 128-byte line per sender after the LL lines,
+// in the Ctrl granule.  Same rules as kArOff.
+constexpr uint64_t kRingOff = kLlOff + kMaxRanks * sizeof(FlagLine);  // 76 KiB
+static_assert(kRingOff % 128 == 0 && kRingOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the ring all-reduce lines sit after the LL all-reduce lines inside the Ctrl granule");
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -665,6 +665,22 @@ class Probe:
         rc = self._lib.cdprobe_allreduce_ll(self._h, reps, C.byref(t))
         return rc, t
 
+    def AllReduceRing(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReduceRing.  Ring all-reduce of every rank's source buffer on every rank at once: each
+        8 KiB unit is passed to the next rank under its own flag, 2 (n - 1) steps of reduce-scatter and all-gather
+        with no barrier or fence between them, at each size of the bwcurve ladder, on the probe's grids (0: 8 timed
+        reps per size).  A rep is timed from its opening barrier to the moment the rank's output is complete; path is
+        abi.ALLREDUCE_PATH_RING.  Collective when world_size > 1.  Needs no Run first and disturbs none."""
+        rc, t = self.allreduce_ring_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce_ring")
+        return AllReduce.from_c(t)
+
+    def allreduce_ring_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce_ring(self._h, reps, C.byref(t))
+        return rc, t
+
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps

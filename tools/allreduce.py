@@ -18,7 +18,12 @@ one device move that traffic through its own HBM, not NVLink.
 same session: N = 1 and 2, 4 and 8 ranks sharing GPU 0 at `--ll-bytes` per pair (default 1 MiB, the LL ladder's
 largest size), so the ladder runs 4 KiB ... 1 MiB.  An LL rep runs from the end of the rank's previous rep to the end of
 its own (no barrier per rep); a one-shot rep from its opening barrier's release, a two-shot rep to its closing
-release.  Each rank's link ingress per LL rep is 2 (n - 1) x size: every 8 bytes of data travel in a 16-byte packet."""
+release.  Each rank's link ingress per LL rep is 2 (n - 1) x size: every 8 bytes of data travel in a 16-byte packet.
+
+--ring measures cdprobe_allreduce_ring instead, next to the one-shot and the two-shot (TMA path) on the same handle in
+the same session: N = 1 at `--bytes` per pair, and 2, 4 and 8 ranks sharing GPU 0 at `--multi-bytes` per pair.  A ring
+rep runs from its opening barrier's release to the moment the rank's output is complete.  Each rank sends and receives
+2 (n - 1) / n x size per ring rep, over one link each, so busbw = algbw x 2 (n - 1) / n is reported for all three."""
 import argparse
 import json
 import os
@@ -38,6 +43,7 @@ ap.add_argument("--twoshot", action="store_true", help="also measure cdprobe_all
 ap.add_argument("--multi-bytes", type=int, default=256 << 20, help="bytes_per_pair of the 2- and 4-rank two-shot runs")
 ap.add_argument("--ll", action="store_true", help="measure cdprobe_allreduce_ll next to the one-shot and the two-shot")
 ap.add_argument("--ll-bytes", type=int, default=1 << 20, help="bytes_per_pair of the --ll runs")
+ap.add_argument("--ring", action="store_true", help="measure cdprobe_allreduce_ring next to the one-shot and two-shot")
 a = ap.parse_args()
 
 
@@ -63,6 +69,45 @@ def rows(ar, bus=None):
             out[f"rank_{r}"]["peak_busbw_gbps"] = ar.peak_gbps[r] * bus
     return out
 
+
+if a.ring:
+    res = {"bytes": a.bytes, "multi_bytes": a.multi_bytes, "reps": a.reps,
+           "what": "ns per rep of cdprobe_allreduce_ring (ring), cdprobe_allreduce (one_shot) and "
+                   "cdprobe_allreduce_twoshot (two_shot, TMA path) called one after another on the same handle: "
+                   "N = 1 with one CTA per SM at bytes per pair, N = 2, 4, 8 ranks on GPU 0 (ALLOW_SAME_DEVICE | "
+                   "NO_COOPERATIVE, 16 CTAs each) at multi_bytes per pair; every size of the bwcurve ladder.  A ring "
+                   "rep runs from its opening barrier release to its latest CTA completion stamp; a one-shot rep from "
+                   "its opening barrier release to its latest CTA stamp; a two-shot rep from its opening to its "
+                   "closing barrier release.  algbw_gbps_median = bytes / ns_median; busbw_gbps_median = algbw x "
+                   "2 (n - 1) / n"}
+    for n in (1, 2, 4, 8):
+        bpp = a.bytes if n == 1 else a.multi_bytes
+        cfg = pkg.Config(ordinals=[0] * n, bytes=bpp * max(n - 1, 1), flags=0x40 | 0x10 if n > 1 else 0,
+                         ctas=16 if n > 1 else 0, timeout_ms=60000)
+        bus = 2 * (n - 1) / n
+        with pkg.Open(cfg) as p:
+            p.SetOption(pkg.abi.OPT_PATH, 0)
+            ring = p.AllReduceRing(a.reps)
+            one = p.AllReduce(a.reps)
+            ts = p.AllReduceTwoShot(a.reps)
+            res[f"n{n}"] = {"ring": {**rows(ring, bus), "call_ms": ring.ms},
+                            "one_shot": {**rows(one, bus), "call_ms": one.ms},
+                            "two_shot": {**rows(ts, bus), "call_ms": ts.ms}}
+    res["gpu"] = gpu()
+    res["nvlink"] = "not measured (one GPU)"
+    print(f"{'n':>2} {'bytes':>11} {'ring ns':>11} {'one-shot':>11} {'two-shot':>11} {'ring algbw':>10} "
+          f"{'ring busbw':>10}  (rank 0)")
+    for n in (1, 2, 4, 8):
+        for s, o, t in zip(*(res[f"n{n}"][x]["rank_0"]["sizes"] for x in ("ring", "one_shot", "two_shot"))):
+            print(f"{n:2d} {s['bytes']:11d} {s['ns_median']:11.0f} {o['ns_median']:11.0f} {t['ns_median']:11.0f} "
+                  f"{s['algbw_gbps_median']:10.1f} {s['busbw_gbps_median']:10.1f}")
+    print(f"gpu: {res['gpu']}")
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(res))
+    sys.exit(0)
 
 if a.ll:
     res = {"ll_bytes": a.ll_bytes, "reps": a.reps,
