@@ -407,7 +407,8 @@ typedef struct {
                                            report CDPROBE_ALLREDUCE_PATH_LL and CDPROBE_ALLREDUCE_PATH_RING */
   uint64_t call_seq;                    /* 1-based count of cdprobe_allreduce calls on this handle, equal in every
                                            process (0 when the call was refused); of cdprobe_allreduce_twoshot,
-                                           cdprobe_allreduce_ll or cdprobe_allreduce_ring calls for those */
+                                           cdprobe_allreduce_ll, cdprobe_allreduce_ring or cdprobe_allreduce_push
+                                           calls for those */
   uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per input and of the output per rep: the cdprobe_bwcurve ladder */
   uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank ran */
   int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) or the word check differs from
@@ -506,11 +507,11 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_alltoall:
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_alltoall:
  *   diagnostics, benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring and cdprobe_alltoall are optional for
- *   callers: a daemon binds them with dlsym and works without.
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push and
+ *   cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -581,6 +582,13 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              before its first push of the rep, and every row stays exact.  Modes 0 and
                                              1 fail every row in phase 0, and in phase 1 the rows from sender + 1 up to
                                              the rank before the word's chunk owner; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_PUSH_FAULT 24u /* tests: value = (mode << 48) | ((rank + 1) << 32) | ((k + 1) << 24) |
+                                             word arms a fault in cdprobe_allreduce_push, in timed rep 1 of size[k], on
+                                             output word `word` (< 2^24): mode 0, sender `rank` contributes its source
+                                             word + 1; mode 1, it skips the reduction of the word's 8 KiB unit; mode 2,
+                                             it issues that reduction twice (modes 0-2 fail every row); mode 3, the
+                                             owner of the word's chunk pushes the word xored with 1 to receiver `rank`
+                                             in the all-gather, so only row `rank` fails; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -788,6 +796,41 @@ CDPROBE_API int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allred
  * is >= n_sizes, whose mode-0 or mode-1 word is >= size[k] / 8, lies in a chunk the sender does not push in that phase
  * or is armed at n == 1, or whose mode-2 delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* Push all-reduce of every rank's source buffer, on every rank at once, in which every byte moves as a write: a
+ * reduce-scatter by remote reductions into each unit's owner, then a pushed all-gather.  For each size of the
+ * cdprobe_bwcurve ladder, one untimed warm-up rep and `reps` timed reps.  The size is cut into
+ * cdprobe_allreduce_twoshot's chunks of 8 KiB units.  In a rep, rank r first adds every unit u of its own source
+ * buffer into the push area of u's owner, at u's place: on the TMA path (CDPROBE_OPT_PATH 0) each unit is bulk-loaded
+ * into shared memory and sent with cp.reduce.async.bulk .add.u64, so the memory system that owns the target adds it
+ * in; on the ld/st paths (1, 2) each 8-byte word goes with its own red.relaxed.sys.global.add.u64, the paths differing
+ * only in the load layout.  Up to n ranks add into the same unit at once.  Once every reduction is performed and
+ * fenced, a fenced domain barrier leaves rank r's own chunk holding the full sum, and rank r pushes that chunk with
+ * st.global.v4 to every peer, r + 1, r + 2, ... (mod n).  The sums are 64-bit wrapping adds, so their order does not
+ * matter and the output is cdprobe_allreduce's word for word.  Each rank's link traffic per rep is
+ * 2 (n - 1) / n x size, the two-shot's, with every transfer a write.  Three domain barriers per rep (flags in the Ctrl
+ * granule; only grid barriers at n == 1, where the rank reduces its input into its own zeroed area and pushes
+ * nothing): a fenced one opens the rep, one follows the reductions and a fenced one closes the rep after a fence.sys
+ * in every CTA; a rep is timed per rank by %globaltimer from its opening release to its closing release.  After every
+ * rep, warm-up included and untimed, each rank reads back every word of its output, compares it with the pattern's
+ * sum and overwrites it with 0, the start the next rep's reductions need; row r of *out is as
+ * cdprobe_allreduce_twoshot's, and peak_gbps is the algorithm bandwidth, size / ns (bus bandwidth peak_gbps x
+ * 2 (n - 1) / n).  The push area (bytes_per_pair per rank, rounded up to 2 MiB) is created on the first call with the
+ * probe allocation's handle type, zeroed, mapped wherever the probe mapping is then up, and kept until close; if
+ * creating it fails in any process, every process returns that error, nothing runs, and the next call tries again.
+ * If any probe or push-area mapping of the domain is down (cdprobe_unmap_peer, a failed mapping, MIG), or two ranks
+ * on different devices this process sees lack native peer atomics (cudaDevP2PAttrNativeAtomicSupported; a rank in
+ * another process counts as native), nothing runs: every filled row has measured = 0 and the status of the first
+ * such cell (CDPROBE_ERR_UNSUPPORTED for missing atomics), and the call returns CDPROBE_OK.  A rank whose kernel
+ * passes timeout_ms is CDPROBE_ERR_TIMEOUT with no times, the handle stays usable, and every push area is zeroed
+ * before the next call runs.  Collective when world_size > 1: every process calls it with the same reps and fills the
+ * rows of its own ranks (row_mask); call_seq counts calls of this function.  Needs no run first and touches no
+ * result, pattern, source buffer, landing slot, run_seq, warm-up state, exchange, gather, LL or ring area or other
+ * measurement's state.  *out carries abi, n, reps and path whatever the return code.  CDPROBE_ERR_ARG: null argument,
+ * reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes, or an armed
+ * CDPROBE_OPT_ALLREDUCE_PUSH_FAULT whose mode is above 3, whose rank is >= n, whose k is >= n_sizes, whose word is
+ * >= size[k] / 8, or whose mode 3 is armed at n == 1 or names the word's owner as receiver; CDPROBE_ERR_STATE: sticky
+ * handle. */
+CDPROBE_API int cdprobe_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

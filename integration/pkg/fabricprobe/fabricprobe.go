@@ -50,6 +50,7 @@ static a2a_fn cdp_a2a;    // optional: absent from libraries that predate cdprob
 static ar_fn cdp_ar2;     // optional: absent from libraries that predate cdprobe_allreduce_twoshot
 static ar_fn cdp_arll;    // optional: absent from libraries that predate cdprobe_allreduce_ll
 static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprobe_allreduce_ring
+static ar_fn cdp_arpush;  // optional: absent from libraries that predate cdprobe_allreduce_push
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -71,6 +72,7 @@ static int cdp_load(const char* path) {
   cdp_ar2 = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_twoshot");
   cdp_arll = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ll");
   cdp_arring = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ring");
+  cdp_arpush = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_push");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -110,6 +112,10 @@ static int cdp_call_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_
 static int cdp_has_allreduce_ring(void) { return cdp_arring != NULL; }
 static int cdp_call_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
   return cdp_arring(h, reps, ar);
+}
+static int cdp_has_allreduce_push(void) { return cdp_arpush != NULL; }
+static int cdp_call_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
+  return cdp_arpush(h, reps, ar);
 }
 */
 import "C"
@@ -283,7 +289,7 @@ type BwCurve struct {
 }
 
 // AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot),
-// the low-latency one's (AllReduceLL) or the ring's (AllReduceRing).
+// the low-latency one's (AllReduceLL), the ring's (AllReduceRing) or the push one's (AllReducePush).
 // Every slice is indexed by rank; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
 // rank was not measured or timed out.
 type AllReduce struct {
@@ -743,6 +749,32 @@ func (p *Probe) AllReduceRing(reps int) (AllReduce, error) {
 	}
 	ring := allReduceOf(res)
 	return ring, nil
+}
+
+// AllReducePush runs the push all-reduce of every rank's source buffer on every rank at once, every byte moved as a
+// write: each rank reduces every 8 KiB unit of its input into the unit's owner (bulk reductions on the TMA path,
+// red.global per word on ld/st), then each owner pushes its finished chunk to every peer, at each size of the bwcurve
+// ladder, and reports ns per rep for each size (reps 0: 8 timed reps), timed from the rep's opening barrier to its
+// closing barrier.  Path is the handle's data path.  Collective when the domain spans processes.  ErrUnsupported when
+// the library predates cdprobe_allreduce_push.
+func (p *Probe) AllReducePush(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce_push() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce_push", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	res := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce_push(p.h, C.uint32_t(reps), res)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce_push: %s: %s", C.GoString(C.cdp_call_strerror(rc)),
+			C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	push := allReduceOf(res)
+	return push, nil
 }
 
 // allReduceOf copies a cdprobe_allreduce_t into an AllReduce.

@@ -184,5 +184,6 @@ func (*Probe) AllReduce(int) (AllReduce, error) { return AllReduce{}, ErrUnsuppo
 func (*Probe) AllReduceTwoShot(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceLL(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceRing(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllReducePush(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -39,6 +39,7 @@ OPT_ALLTOALL_FAULT = 20
 OPT_ALLREDUCE_TWOSHOT_FAULT = 21
 OPT_ALLREDUCE_LL_FAULT = 22
 OPT_ALLREDUCE_RING_FAULT = 23
+OPT_ALLREDUCE_PUSH_FAULT = 24
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -428,6 +429,16 @@ def allreduce_ring_fault(sender: int, k: int, arg: int, phase: int = 0, mode: in
     return (mode << 48) | (phase << 40) | ((sender + 1) << 32) | ((k + 1) << 24) | arg
 
 
+def allreduce_push_fault(rank: int, k: int, word: int, mode: int = 0) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_PUSH_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_push, on output word
+    `word`: mode 0, sender `rank` contributes its source word + 1; mode 1, it skips the reduction of the word's unit;
+    mode 2, it issues that reduction twice; mode 3, the owner of the word's chunk pushes the word xored with 1 to
+    receiver `rank` in the all-gather.  Fields that do not fit are refused here."""
+    if mode not in (0, 1, 2, 3) or not (0 <= rank < 0xffff and 0 <= k < 255 and 0 <= word < 1 << 24):
+        raise ValueError("allreduce_push_fault: mode 0 to 3, rank below 65535, k below 255, word below 2^24")
+    return (mode << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -466,6 +477,7 @@ SYMBOLS = {
     "cdprobe_allreduce_twoshot": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_ll": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_ring": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
+    "cdprobe_allreduce_push": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

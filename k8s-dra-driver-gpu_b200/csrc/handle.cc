@@ -478,6 +478,7 @@ static void destroy(cdprobe* h) {
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
   }
+  release_shared(h, h->push);
   release_shared(h, h->ring);
   release_shared(h, h->ll);
   release_shared(h, h->gather);
@@ -1081,6 +1082,10 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_ALLREDUCE_RING_FAULT:  // checked against the domain, the ladder, the chunks and timeout_ms by
                                             // cdprobe_allreduce_ring
       h->ring_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_PUSH_FAULT:  // checked against the domain, the ladder and the chunks by
+                                            // cdprobe_allreduce_push
+      h->push_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

@@ -48,6 +48,8 @@ struct LocalRank {
   bool ll_mapped[kMaxRanks] = {};
   CUdeviceptr ring_va[kMaxRanks] = {};  // rank j's ring area (cdprobe_allreduce_ring) as mapped here
   bool ring_mapped[kMaxRanks] = {};
+  CUdeviceptr push_va[kMaxRanks] = {};  // rank j's push area (cdprobe_allreduce_push) as mapped here
+  bool push_mapped[kMaxRanks] = {};
   ResultRow* row = nullptr;
   char uuid[48] = {};
   Phase phases[kMaxPhases];
@@ -60,8 +62,8 @@ struct LocalRank {
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
 // exports them, takes the other processes' over the rendezvous, imports them and maps every rank's into every local
 // rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area,
-// cdprobe_allreduce_twoshot's gather area, cdprobe_allreduce_ll's LL area and cdprobe_allreduce_ring's ring area are
-// others (ensure_area), and keep their state here.
+// cdprobe_allreduce_twoshot's gather area, cdprobe_allreduce_ll's LL area, cdprobe_allreduce_ring's ring area and
+// cdprobe_allreduce_push's push area are others (ensure_area), and keep their state here.
 struct SharedAlloc {
   size_t bytes = 0;                                       // of each allocation; 0: not created
   CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
@@ -73,8 +75,8 @@ struct SharedAlloc {
   bool has_import[kMaxRanks] = {};
   int32_t status[kMaxRanks][kMaxRanks] = {};  // an area's [issuer][owner] mapping status, all ranks, once it exists
                                               // (the probe allocation's is cdprobe::status)
-  bool stale = false;  // the LL or ring area must be zeroed before its next use: it is new, or a local rank's kernel
-                       // timed out and it may hold packets, data or flags of any earlier call
+  bool stale = false;  // the LL, ring or push area must be zeroed before its next use: it is new, or a local rank's
+                       // kernel timed out and it may hold packets, data, flags or partial sums of any earlier call
   SharedAlloc(CUdeviceptr (LocalRank::*v)[kMaxRanks], bool (LocalRank::*m)[kMaxRanks]) : va(v), mapped(m) {
     for (int& f : own_fd) f = -1;
   }
@@ -95,6 +97,7 @@ struct cdprobe {
   cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};  // the two-shot's gather area
   cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};  // cdprobe_allreduce_ll's LL area
   cdp::SharedAlloc ring{&cdp::LocalRank::ring_va, &cdp::LocalRank::ring_mapped};  // cdprobe_allreduce_ring's ring area
+  cdp::SharedAlloc push{&cdp::LocalRank::push_va, &cdp::LocalRank::push_mapped};  // cdprobe_allreduce_push's push area
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
@@ -129,6 +132,8 @@ struct cdprobe {
   uint64_t ll_fault = 0;      // CDPROBE_OPT_ALLREDUCE_LL_FAULT value, 0: disarmed
   uint64_t ring_calls = 0;    // cdprobe_allreduce_ring calls that ran (call_seq of the last one)
   uint64_t ring_fault = 0;    // CDPROBE_OPT_ALLREDUCE_RING_FAULT value, 0: disarmed
+  uint64_t push_calls = 0;    // cdprobe_allreduce_push calls that ran (call_seq of the last one)
+  uint64_t push_fault = 0;    // CDPROBE_OPT_ALLREDUCE_PUSH_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -170,8 +175,9 @@ inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
 
 // A measurement's shared area m (handle.cc): cdprobe_alltoall's exchange area (h->area, n_total x bytes_per_pair),
 // cdprobe_allreduce_twoshot's gather area (h->gather, bytes_per_pair), cdprobe_allreduce_ll's LL area (h->ll,
-// 2 x n_total x 2 x the LL ladder's largest size) or cdprobe_allreduce_ring's ring area (h->ring, bytes_per_pair and
-// one flag per 8 KiB of it).  On the first call, every local rank creates
+// 2 x n_total x 2 x the LL ladder's largest size), cdprobe_allreduce_ring's ring area (h->ring, bytes_per_pair and
+// one flag per 8 KiB of it) or cdprobe_allreduce_push's push area (h->push, bytes_per_pair).  On the first call, every
+// local rank creates
 // `bytes` of device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every
 // local rank wherever the probe mapping is then up; m.status gets every rank's mapping statuses.  Collective.  If
 // creating it fails in any process, every process returns that error with nothing kept, and the next call tries

@@ -1,7 +1,7 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
 // cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll,
-// cdprobe_allreduce_ring and cdprobe_alltoall.  Each runs on the local ranks' own streams, between probe runs, and has its results on the host
-// before it returns.
+// cdprobe_allreduce_ring, cdprobe_allreduce_push and cdprobe_alltoall.  Each runs on the local ranks' own streams,
+// between probe runs, and has its results on the host before it returns.
 #include <string.h>
 
 #include <algorithm>
@@ -12,6 +12,7 @@
 
 #include "allreduce.h"
 #include "allreduce_ll.h"
+#include "allreduce_push.h"
 #include "allreduce_ring.h"
 #include "allreduce_twoshot.h"
 #include "alltoall.h"
@@ -95,13 +96,24 @@ struct Agreement {
 // process's, then a call number or arguments that differ.  Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and
 // CDPROBE_ERR_ARG on a refusal, with the message set.  Otherwise st, when given, gets the domain's matrix of mapping
 // status, [rank][rank], which every process derives alike; grid, when given, the domain's smallest grid; and *zero
-// whether any process must zero its area.
+// whether any process must zero its area.  native: a measurement that needs remote atomics, so a live cell between two
+// devices this process sees and that CUDA reports without cudaDevP2PAttrNativeAtomicSupported is folded into the rows
+// as CDPROBE_ERR_UNSUPPORTED (a peer in another process counts as native, as in cdprobe_atomics).
 static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq, const std::array<uint32_t, 3>& args,
-                 int32_t (*st)[kMaxRanks], uint32_t* grid = nullptr, bool* zero = nullptr) {
+                 int32_t (*st)[kMaxRanks], uint32_t* grid = nullptr, bool* zero = nullptr, bool native = false) {
   Agreement mine = {call_seq, args, bad.empty() ? 1u : 0u, UINT32_MAX, zero != nullptr && *zero ? 1u : 0u, {}};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     mine.ctas = std::min(mine.ctas, h->lr[li].ctas);
-    for (uint32_t j = 0; j < h->n_total; ++j) mine.rows[li][j] = cell_status(h, li, j);
+    for (uint32_t j = 0; j < h->n_total; ++j) {
+      mine.rows[li][j] = cell_status(h, li, j);
+      const bool local = j >= h->first && j < h->first + h->n_local;
+      if (!native || mine.rows[li][j] != 0 || !local || h->lr[j - h->first].ordinal == h->lr[li].ordinal) continue;
+      // a query that fails counts as no native atomics: returning here would leave the other processes at the allgather
+      int ok = 0;
+      if (cudaDeviceGetP2PAttribute(&ok, cudaDevP2PAttrNativeAtomicSupported, h->lr[li].ordinal,
+                                    h->lr[j - h->first].ordinal) != cudaSuccess || ok == 0)
+        mine.rows[li][j] = CDPROBE_ERR_UNSUPPORTED;
+    }
   }
   std::vector<Agreement> all(h->cfg.world_size, mine);
   if (h->cfg.world_size > 1) {
@@ -422,6 +434,7 @@ struct ArProtocol {
   const char* (*decode)(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f);
   // fills its parameters for local rank L and launches its kernel (launch_ladder)
   int (*launch)(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f, uint32_t grid);
+  bool native = false;                           // it adds into peers' memory: every pair needs native atomics
 };
 
 static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
@@ -561,6 +574,45 @@ static int ring_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
   return launch_ladder(h, L, p, lad, allreduce_ring_launch, "launch allreduce_ring_kernel");
 }
 
+// Modes 0-2 act in the process that hosts the sender `rank`; mode 3 in the one that hosts the owner of the word's chunk,
+// towards receiver `rank`, which must be a peer of that owner.
+static const char* push_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint32_t n = h->n_total;
+  const uint64_t mode = v >> 48, fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  if (mode > 3) return "the armed push all-reduce fault has a mode above 3";
+  if (fr == 0 || fr > n) return "the armed push all-reduce fault names no rank of this domain";
+  if (fk == 0 || fk > lad.n_sizes) return "the armed push all-reduce fault names no size of this call";
+  if (word >= lad.size[fk - 1] / 8) return "the armed push all-reduce fault names no output word of its size";
+  const uint32_t r = (uint32_t)fr - 1, k = (uint32_t)fk - 1;
+  if (mode < 3) {
+    *f = {r, 0, k, (uint32_t)mode, word};
+    return nullptr;
+  }
+  if (n == 1) return "the armed push all-reduce fault's mode 3 has no peer to push to at n == 1";
+  const uint32_t owner = twoshot_owner((lad.size[k] + kUnitBytes - 1) / kUnitBytes, n, word / (kUnitBytes / 8));
+  if (owner == r) return "the armed push all-reduce fault's mode-3 receiver owns the word and is pushed no copy of it";
+  *f = {owner, r, k, 3u, word};
+  return nullptr;
+}
+
+static int push_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                       uint32_t) {
+  const uint32_t g = L.grank, n = h->n_total;
+  PushParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
+  for (uint32_t t = 0; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.push_va[(g + t) % n]);
+  p.dom = dom;
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_word = f.word;
+  p.fault_mode = f.mode;
+  p.fault_dst = (f.recv + n - g) % n;
+  p.rank = g;
+  p.n = n;
+  return launch_ladder(h, L, p, lad, allreduce_push_launch, "launch allreduce_push_kernel");
+}
+
 constexpr ArProtocol kOneShot = {
     "cdprobe_allreduce", &cdprobe::ar_calls, &cdprobe::ar_fault, bwcurve_ladder, kHandlePath, nullptr, nullptr,
     nullptr, true, kArOff, oneshot_fault, oneshot_launch};
@@ -575,8 +627,12 @@ constexpr ArProtocol kRing = {
     "cdprobe_allreduce_ring", &cdprobe::ring_calls, &cdprobe::ring_fault, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_RING,
     &cdprobe::ring, ring_area_bytes, "cdprobe_allreduce_ring: zero the ring area", false, kRingOff, ring_fault,
     ring_launch};
+constexpr ArProtocol kPush = {
+    "cdprobe_allreduce_push", &cdprobe::push_calls, &cdprobe::push_fault, bwcurve_ladder, kHandlePath, &cdprobe::push,
+    [](uint32_t, uint64_t s_max) { return s_max; }, "cdprobe_allreduce_push: zero the push area", false, kPushOff,
+    push_fault, push_launch, true};
 
-// The all-reduces (DESIGN §5g, §5i, §5j, §5k): one call of protocol P.
+// The all-reduces (DESIGN §5g, §5i, §5j, §5k, §5l): one call of protocol P.
 static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, const ArProtocol& P) {
   Ladder lad;
   if (const int rc = open_ladder(h, out, reps, kArDefaultReps, &lad, P.path, P.rule); rc != CDPROBE_OK) return rc;
@@ -592,7 +648,8 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   bool zero = P.zeroing != nullptr && m->stale;
   uint32_t grid;
   int32_t st[kMaxRanks][kMaxRanks];
-  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero); rc != CDPROBE_OK)
+  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero, P.native);
+      rc != CDPROBE_OK)
     return rc;
   // 2. the area, built once, by every process in the same call
   const uint64_t s_max = lad.size[lad.n_sizes - 1];
@@ -1074,6 +1131,10 @@ int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) 
 
 int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   return cdp::allreduce_call(h, reps, out, cdp::kRing);
+}
+
+int cdprobe_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  return cdp::allreduce_call(h, reps, out, cdp::kPush);
 }
 
 int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {

@@ -576,6 +576,20 @@ constexpr uint64_t kRingOff = kLlOff + kMaxRanks * sizeof(FlagLine);  // 76 KiB
 static_assert(kRingOff % 128 == 0 && kRingOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
               "the ring all-reduce lines sit after the LL all-reduce lines inside the Ctrl granule");
 
+// ---- the push all-reduce (cdprobe_allreduce_push, DESIGN §5l) -------------------------------------------------------
+// The rank whose two-shot chunk (twoshot_chunk) holds unit u < units of a prefix of `units` units: the largest r with
+// floor(r units / n) <= u, which is floor(((u + 1) n - 1) / units).  Every sender reduces unit u into that rank's area.
+CDP_HD inline uint32_t twoshot_owner(uint64_t units, uint32_t n, uint64_t u) {
+  return (uint32_t)(((u + 1) * n - 1) / units);
+}
+
+// The domain barriers of cdprobe_allreduce_push: one 128-byte line per sender after the ring lines, in the Ctrl
+// granule.  Same rules as kArOff; three barriers per rep.
+constexpr uint64_t kPushOff = kRingOff + kMaxRanks * sizeof(FlagLine);  // 78 KiB
+static_assert(kPushOff % 128 == 0 && kPushOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the push all-reduce lines sit after the ring all-reduce lines inside the Ctrl granule");
+static_assert(kBwMaxSizes * (64 + 1) * 3 < (1u << kArBarrierBits), "push all-reduce barriers per call fit the low bits");
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -681,6 +681,23 @@ class Probe:
         rc = self._lib.cdprobe_allreduce_ring(self._h, reps, C.byref(t))
         return rc, t
 
+    def AllReducePush(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReducePush.  Push all-reduce of every rank's source buffer on every rank at once, every byte
+        moved as a write: each rank reduces every 8 KiB unit of its input into the unit's owner (bulk reductions on the
+        TMA path, red.global per word on ld/st), then each owner pushes its finished chunk to every peer, at each size
+        of the bwcurve ladder, on the probe's data path and grids (0: 8 timed reps per size).  A rep is timed from its
+        opening to its closing barrier; path is the handle's.  Collective when world_size > 1.  Needs no Run first and
+        disturbs none."""
+        rc, t = self.allreduce_push_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce_push")
+        return AllReduce.from_c(t)
+
+    def allreduce_push_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce_push(self._h, reps, C.byref(t))
+        return rc, t
+
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps

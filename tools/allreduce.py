@@ -23,7 +23,13 @@ release.  Each rank's link ingress per LL rep is 2 (n - 1) x size: every 8 bytes
 --ring measures cdprobe_allreduce_ring instead, next to the one-shot and the two-shot (TMA path) on the same handle in
 the same session: N = 1 at `--bytes` per pair, and 2, 4 and 8 ranks sharing GPU 0 at `--multi-bytes` per pair.  A ring
 rep runs from its opening barrier's release to the moment the rank's output is complete.  Each rank sends and receives
-2 (n - 1) / n x size per ring rep, over one link each, so busbw = algbw x 2 (n - 1) / n is reported for all three."""
+2 (n - 1) / n x size per ring rep, over one link each, so busbw = algbw x 2 (n - 1) / n is reported for all three.
+
+--push measures cdprobe_allreduce_push instead, next to the one-shot and the two-shot on the same handle in the same
+session: N = 1 at `--bytes` per pair on each data path (TMA bulk reductions, and red.global per word behind 16-byte and
+32-byte loads), and 2, 4 and 8 ranks sharing GPU 0 at `--multi-bytes` per pair on the TMA path.  A push rep runs from
+its opening barrier's release to its closing release, as a two-shot rep does.  Each rank's link traffic per rep is the
+two-shot's, 2 (n - 1) / n x size, every transfer a write, so busbw = algbw x 2 (n - 1) / n is reported for all three."""
 import argparse
 import json
 import os
@@ -44,6 +50,7 @@ ap.add_argument("--multi-bytes", type=int, default=256 << 20, help="bytes_per_pa
 ap.add_argument("--ll", action="store_true", help="measure cdprobe_allreduce_ll next to the one-shot and the two-shot")
 ap.add_argument("--ll-bytes", type=int, default=1 << 20, help="bytes_per_pair of the --ll runs")
 ap.add_argument("--ring", action="store_true", help="measure cdprobe_allreduce_ring next to the one-shot and two-shot")
+ap.add_argument("--push", action="store_true", help="measure cdprobe_allreduce_push next to the one-shot and two-shot")
 a = ap.parse_args()
 
 
@@ -69,6 +76,47 @@ def rows(ar, bus=None):
             out[f"rank_{r}"]["peak_busbw_gbps"] = ar.peak_gbps[r] * bus
     return out
 
+
+if a.push:
+    res = {"bytes": a.bytes, "multi_bytes": a.multi_bytes, "reps": a.reps,
+           "what": "ns per rep of cdprobe_allreduce_push (push), cdprobe_allreduce (one_shot) and "
+                   "cdprobe_allreduce_twoshot (two_shot) called one after another on the same handle: n1_<path>: "
+                   "N = 1 with one CTA per SM at bytes per pair on the tma, ldst16 and ldst32 data paths; n2, n4, n8: "
+                   "2, 4, 8 ranks on GPU 0 (ALLOW_SAME_DEVICE | NO_COOPERATIVE, 16 CTAs each, TMA path) at "
+                   "multi_bytes per pair; every size of the bwcurve ladder.  A push or two-shot rep runs from its "
+                   "opening to its closing barrier release; a one-shot rep from its opening barrier release to its "
+                   "latest CTA stamp.  algbw_gbps_median = bytes / ns_median; busbw_gbps_median = algbw x "
+                   "2 (n - 1) / n"}
+    runs = [(1, path) for path in (0, 1, 2)] + [(n, 0) for n in (2, 4, 8)]
+    names = ("tma", "ldst16", "ldst32")
+    for n, path in runs:
+        bpp = a.bytes if n == 1 else a.multi_bytes
+        cfg = pkg.Config(ordinals=[0] * n, bytes=bpp * max(n - 1, 1), flags=0x40 | 0x10 if n > 1 else 0,
+                         ctas=16 if n > 1 else 0, timeout_ms=60000)
+        bus = 2 * (n - 1) / n
+        with pkg.Open(cfg) as p:
+            p.SetOption(pkg.abi.OPT_PATH, path)
+            push = p.AllReducePush(a.reps)
+            one = p.AllReduce(a.reps)
+            ts = p.AllReduceTwoShot(a.reps)
+            res[f"n1_{names[path]}" if n == 1 else f"n{n}"] = {"push": {**rows(push, bus), "call_ms": push.ms},
+                                                               "one_shot": {**rows(one, bus), "call_ms": one.ms},
+                                                               "two_shot": {**rows(ts, bus), "call_ms": ts.ms}}
+    res["gpu"] = gpu()
+    res["nvlink"] = "not measured (one GPU)"
+    print(f"{'run':>9} {'bytes':>11} {'push ns':>11} {'one-shot':>11} {'two-shot':>11} {'push algbw':>10} "
+          f"{'push busbw':>10}  (rank 0)")
+    for key in [f"n1_{x}" for x in names] + ["n2", "n4", "n8"]:
+        for s, o, t in zip(*(res[key][x]["rank_0"]["sizes"] for x in ("push", "one_shot", "two_shot"))):
+            print(f"{key:>9} {s['bytes']:11d} {s['ns_median']:11.0f} {o['ns_median']:11.0f} {t['ns_median']:11.0f} "
+                  f"{s['algbw_gbps_median']:10.1f} {s['busbw_gbps_median']:10.1f}")
+    print(f"gpu: {res['gpu']}")
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(res))
+    sys.exit(0)
 
 if a.ring:
     res = {"bytes": a.bytes, "multi_bytes": a.multi_bytes, "reps": a.reps,
