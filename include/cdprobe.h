@@ -402,13 +402,14 @@ typedef struct {
   uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
   uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
   uint32_t n_sizes;                     /* entries of size[] */
-  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH); cdprobe_allreduce_ll and
-                                           cdprobe_allreduce_ring have one data path each, ignore CDPROBE_OPT_PATH and
-                                           report CDPROBE_ALLREDUCE_PATH_LL and CDPROBE_ALLREDUCE_PATH_RING */
+  uint32_t path;                        /* the read data path used (CDPROBE_OPT_PATH); cdprobe_allreduce_ll,
+                                           cdprobe_allreduce_ring and cdprobe_allreduce_nvls have one data path each,
+                                           ignore CDPROBE_OPT_PATH and report CDPROBE_ALLREDUCE_PATH_LL,
+                                           CDPROBE_ALLREDUCE_PATH_RING and CDPROBE_ALLREDUCE_PATH_NVLS */
   uint64_t call_seq;                    /* 1-based count of cdprobe_allreduce calls on this handle, equal in every
                                            process (0 when the call was refused); of cdprobe_allreduce_twoshot,
-                                           cdprobe_allreduce_ll, cdprobe_allreduce_ring or cdprobe_allreduce_push
-                                           calls for those */
+                                           cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push or
+                                           cdprobe_allreduce_nvls calls for those */
   uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per input and of the output per rep: the cdprobe_bwcurve ladder */
   uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank ran */
   int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep's (S, X) or the word check differs from
@@ -436,6 +437,9 @@ typedef struct {
 #define CDPROBE_ALLREDUCE_PATH_LL 3u
 /* cdprobe_allreduce_t.path of cdprobe_allreduce_ring: 16-byte ld/st, one flag per 8 KiB unit (DESIGN §5k) */
 #define CDPROBE_ALLREDUCE_PATH_RING 4u
+/* cdprobe_allreduce_t.path of cdprobe_allreduce_nvls: multimem.ld_reduce and multimem.st through a multicast object
+ * (DESIGN §5m) */
+#define CDPROBE_ALLREDUCE_PATH_NVLS 5u
 
 /* One-shot all-to-all across the domain (cdprobe_alltoall): every rank pushes one block to every peer at once, into the
  * peer's exchange area, and every rank checks every word it receives (DESIGN §5h).  Per-rank entries [r] describe rank
@@ -507,11 +511,13 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_gather, cdprobe_info, cdprobe_trace, cdprobe_set_option, cdprobe_corrupt, cdprobe_corrupt_landing,
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_alltoall:
- *   diagnostics, benches, fault injection; the reference has no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall: diagnostics, benches, fault injection; the reference has no counterpart
+ *   (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
- *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push and
- *   cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works without.
+ *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
+ *   cdprobe_allreduce_nvls and cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works
+ *   without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -589,6 +595,12 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              it issues that reduction twice (modes 0-2 fail every row); mode 3, the
                                              owner of the word's chunk pushes the word xored with 1 to receiver `rank`
                                              in the all-gather, so only row `rank` fails; 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_NVLS_FAULT 25u /* tests: value = (mode << 48) | ((k + 1) << 24) | word arms a fault in
+                                             cdprobe_allreduce_nvls, in timed rep 1 of size[k], on output word `word`
+                                             (< 2^24), in the process hosting the owner of the word's chunk: mode 0,
+                                             the owner stores the word xored with 1 through the multicast address, so
+                                             every row fails at that word; mode 1, it skips the multicast store of the
+                                             word's 8 KiB unit, so every row reads that unit as 0s; 0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -831,6 +843,39 @@ CDPROBE_API int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allr
  * >= size[k] / 8, or whose mode 3 is armed at n == 1 or names the word's owner as receiver; CDPROBE_ERR_STATE: sticky
  * handle. */
 CDPROBE_API int cdprobe_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* Multicast (NVLS) all-reduce of every rank's source buffer, on every rank at once, through one multicast object that
+ * spans the domain: the switch sums and the switch fans out.  For each size of the cdprobe_bwcurve ladder, one untimed
+ * warm-up rep and `reps` timed reps.  Each rank has an NVLS area of 2 x s_max bytes (s_max: the ladder's largest
+ * size), rounded up to the VMM and multicast granularities, bound into the object at offset 0: its first half is the
+ * input, its second the output.  On every call, untimed and before any kernel runs, each rank copies the first s_max
+ * bytes of its source buffer into its input half and zeroes its output half.  The size is cut into
+ * cdprobe_allreduce_twoshot's chunks of 8 KiB units.  In a rep, rank r reads each word of its own chunk with
+ * multimem.ld_reduce .add.u64 through the object, which returns the wrapping 64-bit sum of that word over every
+ * member, and stores each summed 16 bytes with one multimem.st into every member's output half at once.  The sums are
+ * exact, so the output is cdprobe_allreduce's word for word.  A fenced domain barrier opens the rep, and one closes it
+ * after a fence.proxy.alias per thread and a fence.sys per CTA; a rep is timed per rank by %globaltimer from its
+ * opening release to its closing release.  After every rep, warm-up included and
+ * untimed, each rank reads back every word of its output through its own mapping, compares it with the pattern's sum
+ * and overwrites it with 0; row r of *out is as cdprobe_allreduce_twoshot's, path is CDPROBE_ALLREDUCE_PATH_NVLS
+ * whatever CDPROBE_OPT_PATH says, and peak_gbps is the algorithm bandwidth, size / ns (bus bandwidth peak_gbps x
+ * 2 (n - 1) / n).  The object and the areas are created on the first call that runs, with the probe allocation's
+ * handle type (the process hosting rank 0 creates the object and hands it to the others over the rendezvous), and kept
+ * until close; if a step fails in any process, every process returns that error, cdprobe_last_error names the step and
+ * the CUresult, nothing is kept, and the next call tries again.  When a rank's device reports no multicast support
+ * (CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED, or a MIG instance), the driver lacks the multicast entry points, or two
+ * ranks of the domain share a device (by UUID, across processes), nothing is created and nothing runs: every filled
+ * row has measured = 0 and status CDPROBE_ERR_UNSUPPORTED, and the call returns CDPROBE_OK.  The same holds, with
+ * cdprobe_last_error naming the CUresult, for a one-rank domain whose driver refuses a multicast object of one device
+ * (cuMulticastCreate returns CUDA_ERROR_INVALID_VALUE); that call asks the driver again each time.  Likewise, if any probe
+ * mapping of the domain is down, every filled row has the status of the first such cell.  A rank whose kernel passes
+ * timeout_ms is CDPROBE_ERR_TIMEOUT with no times and the handle stays usable.  Collective when world_size > 1: every
+ * process calls it with the same reps and fills the rows of its own ranks (row_mask); call_seq counts calls of this
+ * function.  Needs no run first and touches no result, pattern, source buffer, landing slot, run_seq, warm-up state or
+ * other measurement's state.  *out carries abi, n, reps and path whatever the return code.  CDPROBE_ERR_ARG: null
+ * argument, reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes, or an armed
+ * CDPROBE_OPT_ALLREDUCE_NVLS_FAULT whose mode is above 1, that sets any of bits 32 to 47, whose k is >= n_sizes or
+ * whose word is >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -51,6 +51,7 @@ static ar_fn cdp_ar2;     // optional: absent from libraries that predate cdprob
 static ar_fn cdp_arll;    // optional: absent from libraries that predate cdprobe_allreduce_ll
 static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprobe_allreduce_ring
 static ar_fn cdp_arpush;  // optional: absent from libraries that predate cdprobe_allreduce_push
+static ar_fn cdp_arnvls;  // optional: absent from libraries that predate cdprobe_allreduce_nvls
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -73,6 +74,7 @@ static int cdp_load(const char* path) {
   cdp_arll = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ll");
   cdp_arring = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ring");
   cdp_arpush = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_push");
+  cdp_arnvls = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_nvls");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -116,6 +118,10 @@ static int cdp_call_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduc
 static int cdp_has_allreduce_push(void) { return cdp_arpush != NULL; }
 static int cdp_call_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
   return cdp_arpush(h, reps, ar);
+}
+static int cdp_has_allreduce_nvls(void) { return cdp_arnvls != NULL; }
+static int cdp_call_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
+  return cdp_arnvls(h, reps, ar);
 }
 */
 import "C"
@@ -289,7 +295,8 @@ type BwCurve struct {
 }
 
 // AllReduce is the one-shot all-reduce of the local rows (cdprobe_allreduce_t), or the two-shot's (AllReduceTwoShot),
-// the low-latency one's (AllReduceLL), the ring's (AllReduceRing) or the push one's (AllReducePush).
+// the low-latency one's (AllReduceLL), the ring's (AllReduceRing), the push one's (AllReducePush) or the multicast one's
+// (AllReduceNVLS).
 // Every slice is indexed by rank; the per-size ones hold one entry per Sizes element, and every timing is 0 where a
 // rank was not measured or timed out.
 type AllReduce struct {
@@ -775,6 +782,33 @@ func (p *Probe) AllReducePush(reps int) (AllReduce, error) {
 	}
 	push := allReduceOf(res)
 	return push, nil
+}
+
+// AllReduceNVLS runs the multicast (NVLS) all-reduce of every rank's source buffer on every rank at once: each rank
+// sums its chunk of 8 KiB units with multimem.ld_reduce through one multicast object that spans the domain and stores
+// each sum to every rank with one multimem.st, at each size of the bwcurve ladder, and reports ns per rep for each size
+// (reps 0: 8 timed reps), timed from the rep's opening barrier to its closing barrier.  Path is
+// CDPROBE_ALLREDUCE_PATH_NVLS.  Rows are CDPROBE_ERR_UNSUPPORTED, with nothing run, when a device or the driver lacks
+// multicast or two ranks share a device.  Collective when the domain spans processes.  ErrUnsupported when the library
+// predates cdprobe_allreduce_nvls.
+func (p *Probe) AllReduceNVLS(reps int) (AllReduce, error) {
+	if C.cdp_has_allreduce_nvls() == 0 {
+		return AllReduce{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_allreduce_nvls", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	res := new(C.cdprobe_allreduce_t)
+	rc := C.cdp_call_allreduce_nvls(p.h, C.uint32_t(reps), res)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_allreduce_nvls: %s: %s", C.GoString(C.cdp_call_strerror(rc)),
+			C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return AllReduce{}, err
+	}
+	nvls := allReduceOf(res)
+	return nvls, nil
 }
 
 // allReduceOf copies a cdprobe_allreduce_t into an AllReduce.

@@ -185,5 +185,6 @@ func (*Probe) AllReduceTwoShot(int) (AllReduce, error) { return AllReduce{}, Err
 func (*Probe) AllReduceLL(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceRing(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReducePush(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
+func (*Probe) AllReduceNVLS(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -40,6 +40,7 @@ OPT_ALLREDUCE_TWOSHOT_FAULT = 21
 OPT_ALLREDUCE_LL_FAULT = 22
 OPT_ALLREDUCE_RING_FAULT = 23
 OPT_ALLREDUCE_PUSH_FAULT = 24
+OPT_ALLREDUCE_NVLS_FAULT = 25
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -61,6 +62,7 @@ BWCURVE_DEFAULT_REPS, BWCURVE_MAX_REPS = 8, 64
 ALLREDUCE_DEFAULT_REPS, ALLREDUCE_MAX_REPS = 8, 64
 ALLREDUCE_PATH_LL = 3  # cdprobe_allreduce_t.path of cdprobe_allreduce_ll
 ALLREDUCE_PATH_RING = 4  # cdprobe_allreduce_t.path of cdprobe_allreduce_ring
+ALLREDUCE_PATH_NVLS = 5  # cdprobe_allreduce_t.path of cdprobe_allreduce_nvls
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
@@ -439,6 +441,15 @@ def allreduce_push_fault(rank: int, k: int, word: int, mode: int = 0) -> int:
     return (mode << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
 
 
+def allreduce_nvls_fault(k: int, word: int, mode: int = 0) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_nvls, on output word
+    `word`, acted on by the owner of the word's chunk: mode 0, it stores the word xored with 1 through the multicast
+    address; mode 1, it skips the multicast store of the word's 8 KiB unit.  Fields that do not fit are refused here."""
+    if mode not in (0, 1) or not (0 <= k < 255 and 0 <= word < 1 << 24):
+        raise ValueError("allreduce_nvls_fault: mode 0 or 1, k below 255, word below 2^24")
+    return (mode << 48) | ((k + 1) << 24) | word
+
+
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
     return ((issuer + 1) << 16) | (target + 1)
@@ -478,6 +489,7 @@ SYMBOLS = {
     "cdprobe_allreduce_ll": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_ring": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_push": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
+    "cdprobe_allreduce_nvls": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

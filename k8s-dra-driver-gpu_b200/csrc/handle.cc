@@ -21,6 +21,7 @@
 #include <time.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <new>
 #include <string>
 #include <vector>
@@ -271,6 +272,222 @@ int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes) {
   return CDPROBE_OK;
 }
 
+// Unmaps the NVLS area in every local rank, unbinds every local device from the multicast object, then releases the
+// object and the allocations: no binding outlives its mapping, and no object its bindings.
+static void release_nvls(cdprobe* h) {
+  NvlsArea& a = h->nvls;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (h->lr[li].ordinal < 0) continue;
+    cudaSetDevice(h->lr[li].ordinal);
+    for (auto [va, mapped] : {std::pair{&a.mc_va[li], &a.mc_mapped[li]}, std::pair{&a.uc_va[li], &a.uc_mapped[li]}}) {
+      if (!*mapped) continue;
+      h->drv.MemUnmap(*va, a.bytes);
+      h->drv.MemAddressFree(*va, a.bytes);
+    }
+  }
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    CUdevice dev;
+    if (a.bound[li] && h->drv.DeviceGet(&dev, h->lr[li].ordinal) == CUDA_SUCCESS)
+      h->drv.MulticastUnbind(a.mc, dev, 0, a.bytes);
+  }
+  if (a.has_mc) h->drv.MemRelease(a.mc);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (!a.has_own[li]) continue;
+    cudaSetDevice(h->lr[li].ordinal);
+    h->drv.MemRelease(a.own[li]);
+  }
+  a = NvlsArea();
+}
+
+// Reserves `bytes` of address space on the current device, maps `hnd` there and opens it to device `ordinal`.
+static CUresult map_nvls(cdprobe* h, CUmemGenericAllocationHandle hnd, size_t bytes, size_t align, int ordinal,
+                         CUdeviceptr* va) {
+  CUresult r = h->drv.MemAddressReserve(va, bytes, align, 0, 0);
+  if (r != CUDA_SUCCESS) return r;
+  r = h->drv.MemMap(*va, bytes, 0, hnd, 0);
+  if (r != CUDA_SUCCESS) {
+    h->drv.MemAddressFree(*va, bytes);
+    return r;
+  }
+  CUmemAccessDesc ad;
+  memset(&ad, 0, sizeof(ad));
+  ad.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  ad.location.id = ordinal;
+  ad.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  r = h->drv.MemSetAccess(*va, bytes, &ad, 1);
+  if (r != CUDA_SUCCESS) {
+    h->drv.MemUnmap(*va, bytes);
+    h->drv.MemAddressFree(*va, bytes);
+  }
+  return r;
+}
+
+// What each process reports at a step of ensure_nvls: its return code and message, and from the process hosting rank
+// 0 the area's size and, for fabric handles, the multicast object's handle.
+struct NvlsOffer {
+  int32_t rc;
+  char msg[124];
+  uint64_t bytes;
+  CUmemFabricHandle fabric;
+};
+
+// Every process's rc, shared: the first failure in process order wins, with its message.  A failed exchange is
+// CDPROBE_ERR_RENDEZVOUS.  `offer` (optional) gets rank 0's process's report.
+static int nvls_agree(cdprobe* h, int rc, NvlsOffer* mine_in = nullptr, NvlsOffer* offer = nullptr) {
+  NvlsOffer mine;
+  memset(&mine, 0, sizeof(mine));
+  if (mine_in != nullptr) mine = *mine_in;
+  mine.rc = rc;
+  if (rc != CDPROBE_OK) snprintf(mine.msg, sizeof(mine.msg), "%s", g_last_error.c_str());
+  std::vector<NvlsOffer> all(h->cfg.world_size, mine);
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  if (offer != nullptr) *offer = all[0];
+  for (const NvlsOffer& o : all)
+    if (o.rc != CDPROBE_OK) {
+      set_err(o.msg);
+      return o.rc;
+    }
+  return CDPROBE_OK;
+}
+
+static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
+  NvlsArea& a = h->nvls;
+  // a multicast object needs a shareable handle type even in one process (cuMulticastCreate refuses none)
+  const CUmemAllocationHandleType ht =
+      h->handle_type == 8u ? CU_MEM_HANDLE_TYPE_FABRIC : CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
+  const bool host0 = h->first == 0;
+  CUmulticastObjectProp mp;
+  memset(&mp, 0, sizeof(mp));
+  mp.numDevices = h->n_total;
+  mp.handleTypes = ht;
+  // 1. the size, and in the process hosting rank 0 the object, exported for the others
+  NvlsOffer mine;
+  memset(&mine, 0, sizeof(mine));
+  int fd = -1;
+  int rc = CDPROBE_OK;
+  size_t gran = 0;
+  mp.size = bytes;
+  CUresult r = h->drv.MulticastGetGranularity(&gran, &mp, CU_MULTICAST_GRANULARITY_MINIMUM);
+  if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMulticastGetGranularity", r);
+  if (rc == CDPROBE_OK && (gran == 0 || gran % kVmmGranule != 0 && kVmmGranule % gran != 0)) {
+    set_err("unexpected multicast granularity " + std::to_string(gran));
+    rc = CDPROBE_ERR_UNSUPPORTED;
+  }
+  const size_t align = std::max<size_t>(gran, kVmmGranule);
+  mp.size = mine.bytes = (bytes + align - 1) / align * align;
+  if (rc == CDPROBE_OK && host0) {
+    r = h->drv.MulticastCreate(&a.mc, &mp);
+    if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMulticastCreate", r);
+    else a.has_mc = true;
+    *refused = h->n_total == 1 && r == CUDA_ERROR_INVALID_VALUE;
+    if (*refused) set_err(g_last_error + " (the driver refuses a multicast object of one device)");
+    if (rc == CDPROBE_OK && h->cfg.world_size > 1 && ht == CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR) {
+      r = h->drv.MemExportToShareableHandle(&fd, a.mc, ht, 0);
+      if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemExportToShareableHandle(multicast fd)", r);
+    } else if (rc == CDPROBE_OK && h->cfg.world_size > 1 && ht == CU_MEM_HANDLE_TYPE_FABRIC) {
+      r = h->drv.MemExportToShareableHandle(&mine.fabric, a.mc, ht, 0);
+      if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemExportToShareableHandle(multicast fabric)", r);
+    }
+  }
+  NvlsOffer offer;
+  rc = nvls_agree(h, rc, &mine, &offer);
+  if (rc != CDPROBE_OK) {
+    if (fd >= 0) ::close(fd);
+    return rc;
+  }
+  a.bytes = offer.bytes;
+  // 2. the handle to the other processes.  allgather_fds takes one descriptor from every process: the others send
+  //    their probe allocation's, which every receiver closes unread
+  if (h->cfg.world_size > 1 && ht == CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR) {
+    std::vector<int> all;
+    std::string err;
+    const int send = host0 ? fd : h->mem.own_fd[0];
+    const int xrc = h->rdv.allgather_fds(&send, 1, &all, &err);
+    if (fd >= 0) ::close(fd);
+    if (xrc != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    if (!host0) {
+      r = h->drv.MemImportFromShareableHandle(&a.mc, (void*)(uintptr_t)all[0], ht);
+      if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemImportFromShareableHandle(multicast fd)", r);
+      else a.has_mc = true;
+    }
+    for (int f : all) ::close(f);
+  } else if (h->cfg.world_size > 1 && !host0) {
+    r = h->drv.MemImportFromShareableHandle(&a.mc, &offer.fabric, ht);
+    if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemImportFromShareableHandle(multicast fabric)", r);
+    else a.has_mc = true;
+  }
+  // 3. every process adds its devices; binding or mapping blocks until every device is added, so nobody starts
+  //    before every process has reported that it did
+  for (uint32_t li = 0; li < h->n_local && rc == CDPROBE_OK; ++li) {
+    CUdevice dev;
+    r = h->drv.DeviceGet(&dev, h->lr[li].ordinal);
+    if (r == CUDA_SUCCESS) r = h->drv.MulticastAddDevice(a.mc, dev);
+    if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMulticastAddDevice", r);
+  }
+  if ((rc = nvls_agree(h, rc)) != CDPROBE_OK) return rc;
+  // 4. per local rank: its allocation, bound at offset 0, then the object and the allocation mapped into it
+  for (uint32_t li = 0; li < h->n_local && rc == CDPROBE_OK; ++li) {
+    LocalRank& L = h->lr[li];
+    if (cudaSetDevice(L.ordinal) != cudaSuccess) {
+      set_err("cudaSetDevice");
+      rc = CDPROBE_ERR_CUDA;
+      break;
+    }
+    CUmemAllocationProp ap;
+    memset(&ap, 0, sizeof(ap));
+    ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    ap.location.id = L.ordinal;
+    ap.requestedHandleTypes = ht;
+    r = h->drv.MemCreate(&a.own[li], a.bytes, &ap, 0);
+    if (r != CUDA_SUCCESS) {
+      rc = fail_drv(h, "cuMemCreate", r);
+      break;
+    }
+    a.has_own[li] = true;
+    r = h->drv.MulticastBindMem(a.mc, 0, a.own[li], 0, a.bytes, 0);
+    if (r != CUDA_SUCCESS) {
+      rc = fail_drv(h, "cuMulticastBindMem", r);
+      break;
+    }
+    a.bound[li] = true;
+    r = map_nvls(h, a.mc, a.bytes, align, L.ordinal, &a.mc_va[li]);
+    if (r != CUDA_SUCCESS) {
+      rc = fail_drv(h, "cuMemMap(multicast)", r);
+      break;
+    }
+    a.mc_mapped[li] = true;
+    r = map_nvls(h, a.own[li], a.bytes, align, L.ordinal, &a.uc_va[li]);
+    if (r != CUDA_SUCCESS) {
+      rc = fail_drv(h, "cuMemMap(unicast)", r);
+      break;
+    }
+    a.uc_mapped[li] = true;
+  }
+  return nvls_agree(h, rc);
+}
+
+int ensure_nvls(cdprobe* h, size_t bytes, bool* refused) {
+  *refused = false;
+  if (h->nvls.bytes != 0) return CDPROBE_OK;
+  const int rc = ensure_nvls_steps(h, bytes, refused);
+  if (rc != CDPROBE_OK) {
+    const std::string keep = g_last_error;
+    release_nvls(h);
+    g_last_error = keep;
+  }
+  return rc;
+}
+
 // Phase table of local rank li: see schedule.cc.
 static int build_phases(cdprobe* h, uint32_t li) {
   LocalRank& L = h->lr[li];
@@ -478,6 +695,7 @@ static void destroy(cdprobe* h) {
     cudaSetDevice(L.ordinal);
     if (L.stream) cudaStreamSynchronize(L.stream);
   }
+  release_nvls(h);
   release_shared(h, h->push);
   release_shared(h, h->ring);
   release_shared(h, h->ll);
@@ -1086,6 +1304,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_ALLREDUCE_PUSH_FAULT:  // checked against the domain, the ladder and the chunks by
                                             // cdprobe_allreduce_push
       h->push_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_ALLREDUCE_NVLS_FAULT:  // checked against the ladder and the chunks by cdprobe_allreduce_nvls
+      h->nvls_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

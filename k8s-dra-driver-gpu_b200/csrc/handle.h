@@ -82,6 +82,19 @@ struct SharedAlloc {
   }
 };
 
+// cdprobe_allreduce_nvls's NVLS area (handle.cc, ensure_nvls): one multicast object of `bytes` that spans the domain,
+// and per local rank an allocation of `bytes` on its device, bound into the object at offset 0, mapped into the rank
+// both through the object (multicast) and on its own (unicast).  Peers never map another rank's allocation.
+struct NvlsArea {
+  size_t bytes = 0;                         // of the object and of each allocation; 0: not created
+  CUmemGenericAllocationHandle mc = 0;      // the multicast object, created here or imported from rank 0's process
+  bool has_mc = false;
+  CUmemGenericAllocationHandle own[kMaxRanks] = {};  // [local rank]
+  bool has_own[kMaxRanks] = {}, bound[kMaxRanks] = {};
+  CUdeviceptr mc_va[kMaxRanks] = {}, uc_va[kMaxRanks] = {};  // [local rank] its multicast and unicast mappings
+  bool mc_mapped[kMaxRanks] = {}, uc_mapped[kMaxRanks] = {};
+};
+
 }  // namespace cdp
 
 struct cdprobe {
@@ -98,6 +111,7 @@ struct cdprobe {
   cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};  // cdprobe_allreduce_ll's LL area
   cdp::SharedAlloc ring{&cdp::LocalRank::ring_va, &cdp::LocalRank::ring_mapped};  // cdprobe_allreduce_ring's ring area
   cdp::SharedAlloc push{&cdp::LocalRank::push_va, &cdp::LocalRank::push_mapped};  // cdprobe_allreduce_push's push area
+  cdp::NvlsArea nvls;  // cdprobe_allreduce_nvls's multicast object and NVLS areas
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
@@ -134,6 +148,8 @@ struct cdprobe {
   uint64_t ring_fault = 0;    // CDPROBE_OPT_ALLREDUCE_RING_FAULT value, 0: disarmed
   uint64_t push_calls = 0;    // cdprobe_allreduce_push calls that ran (call_seq of the last one)
   uint64_t push_fault = 0;    // CDPROBE_OPT_ALLREDUCE_PUSH_FAULT value, 0: disarmed
+  uint64_t nvls_calls = 0;    // cdprobe_allreduce_nvls calls that ran (call_seq of the last one)
+  uint64_t nvls_fault = 0;    // CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value, 0: disarmed
   double open_ms = 0, fill_ms = 0;
 };
 
@@ -183,6 +199,17 @@ inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
 // creating it fails in any process, every process returns that error with nothing kept, and the next call tries
 // again.  Kept until close.
 int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes);
+
+// cdprobe_allreduce_nvls's NVLS area (h->nvls, DESIGN §5m): on the first call, `bytes` rounded up to the VMM granule
+// and to the multicast granularity.  The process hosting rank 0 creates the multicast object with the probe
+// allocation's handle type (POSIX fd within one process, which has none) and hands it to the others over the
+// rendezvous; every process adds its devices; once every process has reported that, each local rank creates its
+// allocation, binds it at offset 0 and maps the object and its allocation.  Collective, and only for a domain that
+// agree() found able to run it.  If a step fails in any process, every process returns that error with nothing kept
+// (cdprobe_last_error names the step and the CUresult), and the next call tries again.  *refused: the failure is the
+// driver refusing a multicast object of one device (cuMulticastCreate, CUDA_ERROR_INVALID_VALUE, n_total == 1), which
+// the caller reports as CDPROBE_ERR_UNSUPPORTED rows.  Kept until close.
+int ensure_nvls(cdprobe* h, size_t bytes, bool* refused);
 
 // The mapping status of local rank li's cell [its rank][j]: kStatusUnmapped when that status is 0 but the peer is not
 // mapped.  Non-zero: never read or write through that mapping.

@@ -1,7 +1,7 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
 // cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll,
-// cdprobe_allreduce_ring, cdprobe_allreduce_push and cdprobe_alltoall.  Each runs on the local ranks' own streams,
-// between probe runs, and has its results on the host before it returns.
+// cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_allreduce_nvls and cdprobe_alltoall.  Each runs on the local
+// ranks' own streams, between probe runs, and has its results on the host before it returns.
 #include <string.h>
 
 #include <algorithm>
@@ -12,6 +12,7 @@
 
 #include "allreduce.h"
 #include "allreduce_ll.h"
+#include "allreduce_nvls.h"
 #include "allreduce_push.h"
 #include "allreduce_ring.h"
 #include "allreduce_twoshot.h"
@@ -91,6 +92,28 @@ struct Agreement {
   int32_t rows[kMaxRanks][kMaxRanks];
 };
 
+// What each process adds for cdprobe_allreduce_nvls, in a second exchange that only that call makes: whether its driver
+// and every local device can take part in a multicast object (multicast_here), and its local ranks' device UUIDs.
+struct NvlsFacts {
+  uint32_t mc;
+  char uuid[kMaxRanks][48];
+};
+
+// Whether this process can put every local rank into a multicast object: the driver has the multicast entry points,
+// and every local device reports CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED (a MIG instance, or one simulated, never
+// does).  A query that fails counts as no.
+static bool multicast_here(cdprobe* h) {
+  if (!h->drv.load_multicast()) return false;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    CUdevice dev;
+    int on = 0;
+    if (h->lr[li].mig || h->drv.DeviceGet(&dev, h->lr[li].ordinal) != CUDA_SUCCESS ||
+        h->drv.DeviceGetAttribute(&on, CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED, dev) != CUDA_SUCCESS || on == 0)
+      return false;
+  }
+  return true;
+}
+
 // The handshake of collective measurement `fn`: every process contributes its Agreement (ok: its own verdict `bad` on
 // its arguments is empty; zero: *zero, when given).  The first error wins: this process's own arguments, then another
 // process's, then a call number or arguments that differ.  Returns CDPROBE_ERR_RENDEZVOUS when the exchange fails and
@@ -98,9 +121,12 @@ struct Agreement {
 // status, [rank][rank], which every process derives alike; grid, when given, the domain's smallest grid; and *zero
 // whether any process must zero its area.  native: a measurement that needs remote atomics, so a live cell between two
 // devices this process sees and that CUDA reports without cudaDevP2PAttrNativeAtomicSupported is folded into the rows
-// as CDPROBE_ERR_UNSUPPORTED (a peer in another process counts as native, as in cdprobe_atomics).
+// as CDPROBE_ERR_UNSUPPORTED (a peer in another process counts as native, as in cdprobe_atomics).  nvls, when given,
+// gets whether the domain can form one multicast object, from a second exchange (NvlsFacts): every process can put its
+// ranks in (multicast_here), and no two ranks of the domain share a device, by UUID; a team holds each device once.
 static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq, const std::array<uint32_t, 3>& args,
-                 int32_t (*st)[kMaxRanks], uint32_t* grid = nullptr, bool* zero = nullptr, bool native = false) {
+                 int32_t (*st)[kMaxRanks], uint32_t* grid = nullptr, bool* zero = nullptr, bool native = false,
+                 bool* nvls = nullptr) {
   Agreement mine = {call_seq, args, bad.empty() ? 1u : 0u, UINT32_MAX, zero != nullptr && *zero ? 1u : 0u, {}};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     mine.ctas = std::min(mine.ctas, h->lr[li].ctas);
@@ -141,6 +167,28 @@ static int agree(cdprobe* h, const char* fn, std::string bad, uint64_t call_seq,
   for (const Agreement& o : all) {
     if (grid != nullptr) *grid = std::min(*grid, o.ctas);
     if (zero != nullptr) *zero |= o.zero != 0;
+  }
+  if (nvls == nullptr) return CDPROBE_OK;
+  // every process has got here: the arguments agree everywhere
+  NvlsFacts facts;
+  memset(&facts, 0, sizeof(facts));
+  facts.mc = multicast_here(h) ? 1u : 0u;
+  for (uint32_t li = 0; li < h->n_local; ++li) memcpy(facts.uuid[li], h->lr[li].uuid, sizeof(facts.uuid[li]));
+  std::vector<NvlsFacts> each(h->cfg.world_size, facts);
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.allgather(&facts, sizeof(facts), each.data(), &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  *nvls = true;
+  for (uint32_t p = 0; p < each.size(); ++p) {
+    *nvls &= each[p].mc != 0;
+    for (uint32_t li = 0; li < h->n_local; ++li)
+      for (uint32_t q = 0; q <= p; ++q)
+        for (uint32_t lj = 0; lj < (q == p ? li : h->n_local); ++lj)
+          *nvls &= strncmp(each[p].uuid[li], each[q].uuid[lj], sizeof(each[p].uuid[li])) != 0;
   }
   return CDPROBE_OK;
 }
@@ -363,9 +411,13 @@ static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const Ladder& lad,
 // another skipped would wait at the first domain barrier until its watchdog fired, so when some rank cannot reach some
 // other nothing runs, in any process: every local row gets the status of the domain's first down cell, row-major.
 // Returns whether the call skips.
-static bool skip_rows(const cdprobe* h, int32_t (*st)[kMaxRanks], cdprobe_allreduce_t* out) {
+static const int32_t* first_down(int32_t (*st)[kMaxRanks]) {
   const int32_t* down = std::find_if(&st[0][0], &st[0][0] + kMaxRanks * kMaxRanks, [](int32_t s) { return s != 0; });
-  if (down == &st[0][0] + kMaxRanks * kMaxRanks) return false;
+  return down == &st[0][0] + kMaxRanks * kMaxRanks ? nullptr : down;
+}
+static bool skip_rows(const cdprobe* h, int32_t (*st)[kMaxRanks], cdprobe_allreduce_t* out) {
+  const int32_t* down = first_down(st);
+  if (down == nullptr) return false;
   for (uint32_t li = 0; li < h->n_local; ++li) out->status[h->lr[li].grank] = *down;
   return true;
 }
@@ -435,6 +487,7 @@ struct ArProtocol {
   // fills its parameters for local rank L and launches its kernel (launch_ladder)
   int (*launch)(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f, uint32_t grid);
   bool native = false;                           // it adds into peers' memory: every pair needs native atomics
+  bool nvls = false;                             // it runs through the multicast object (h->nvls, ensure_nvls)
 };
 
 static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
@@ -613,6 +666,39 @@ static int push_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
   return launch_ladder(h, L, p, lad, allreduce_push_launch, "launch allreduce_push_kernel");
 }
 
+// The fault acts in the process that hosts the owner of the word's chunk.
+static const char* nvls_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+  const uint64_t mode = v >> 48, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  if (mode > 1) return "the armed NVLS all-reduce fault has a mode above 1";
+  if (((v >> 32) & 0xffffu) != 0) return "the armed NVLS all-reduce fault sets bits 32 to 47, which name nothing";
+  if (fk == 0 || fk > lad.n_sizes) return "the armed NVLS all-reduce fault names no size of this call";
+  if (word >= lad.size[fk - 1] / 8) return "the armed NVLS all-reduce fault names no output word of its size";
+  const uint32_t k = (uint32_t)fk - 1;
+  const uint64_t units = (lad.size[k] + kUnitBytes - 1) / kUnitBytes;
+  *f = {twoshot_owner(units, h->n_total, word / (kUnitBytes / 8)), 0, k, (uint32_t)mode, word};
+  return nullptr;
+}
+
+// The input half is the first s_max bytes of the rank's NVLS area, the output half the next s_max.
+static int nvls_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
+                       uint32_t) {
+  const uint32_t g = L.grank, li = g - h->first;
+  const uint64_t s_max = lad.size[lad.n_sizes - 1];
+  NvlsParams p;
+  memset(&p, 0, sizeof(p));
+  p.mc_in = reinterpret_cast<const uint8_t*>(h->nvls.mc_va[li]);
+  p.mc_out = reinterpret_cast<uint8_t*>(h->nvls.mc_va[li] + s_max);
+  p.out = reinterpret_cast<uint8_t*>(h->nvls.uc_va[li] + s_max);
+  p.dom = dom;
+  p.seed = h->seed;
+  p.fault_k = g == f.rank ? f.k : kArNoFault;
+  p.fault_word = f.word;
+  p.fault_mode = f.mode;
+  p.rank = g;
+  p.n = h->n_total;
+  return launch_ladder(h, L, p, lad, allreduce_nvls_launch, "launch allreduce_nvls_kernel");
+}
+
 constexpr ArProtocol kOneShot = {
     "cdprobe_allreduce", &cdprobe::ar_calls, &cdprobe::ar_fault, bwcurve_ladder, kHandlePath, nullptr, nullptr,
     nullptr, true, kArOff, oneshot_fault, oneshot_launch};
@@ -631,8 +717,11 @@ constexpr ArProtocol kPush = {
     "cdprobe_allreduce_push", &cdprobe::push_calls, &cdprobe::push_fault, bwcurve_ladder, kHandlePath, &cdprobe::push,
     [](uint32_t, uint64_t s_max) { return s_max; }, "cdprobe_allreduce_push: zero the push area", false, kPushOff,
     push_fault, push_launch, true};
+constexpr ArProtocol kNvls = {
+    "cdprobe_allreduce_nvls", &cdprobe::nvls_calls, &cdprobe::nvls_fault, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_NVLS,
+    nullptr, nullptr, nullptr, false, kNvlsOff, nvls_fault, nvls_launch, false, true};
 
-// The all-reduces (DESIGN §5g, §5i, §5j, §5k, §5l): one call of protocol P.
+// The all-reduces (DESIGN §5g, §5i, §5j, §5k, §5l, §5m): one call of protocol P.
 static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, const ArProtocol& P) {
   Ladder lad;
   if (const int rc = open_ladder(h, out, reps, kArDefaultReps, &lad, P.path, P.rule); rc != CDPROBE_OK) return rc;
@@ -648,13 +737,29 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   bool zero = P.zeroing != nullptr && m->stale;
   uint32_t grid;
   int32_t st[kMaxRanks][kMaxRanks];
-  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero, P.native);
+  bool nvls = true;
+  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero, P.native,
+                           P.nvls ? &nvls : nullptr);
       rc != CDPROBE_OK)
     return rc;
-  // 2. the area, built once, by every process in the same call
+  // a domain that cannot form a multicast object runs nothing, whatever its mappings
+  const auto unsupported = [&] {
+    for (uint32_t s = 0; s < n; ++s)
+      for (uint32_t d = 0; d < n; ++d) st[s][d] = CDPROBE_ERR_UNSUPPORTED;
+  };
+  if (!nvls) unsupported();
+  // 2. the area, built once, by every process in the same call; the NVLS area only for a call that will run.  A
+  //    driver that refuses a multicast object of one device leaves a one-rank domain unsupported, with the CUresult in
+  //    cdprobe_last_error
   const uint64_t s_max = lad.size[lad.n_sizes - 1];
   if (m != nullptr)
     if (const int rc = ensure_area(h, *m, P.area_bytes(n, s_max)); rc != CDPROBE_OK) return rc;
+  if (P.nvls && first_down(st) == nullptr) {
+    bool refused = false;
+    const int rc = ensure_nvls(h, 2 * s_max, &refused);
+    if (refused) unsupported();
+    else if (rc != CDPROBE_OK) return rc;
+  }
   out->call_seq = ++(h->*P.calls);
   put_ladder(h, lad, out);
   // 3. every rank reads every input and writes every area: when some probe mapping or area mapping of the domain is
@@ -677,6 +782,19 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
       if (e != cudaSuccess) return fail_sticky(h, P.zeroing, e);
     }
     m->stale = false;
+  }
+  // the NVLS input is the first s_max bytes of each rank's source buffer, and its output starts zeroed, on every call
+  if (P.nvls) {
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      LocalRank& L = h->lr[li];
+      CDP_RT(cudaSetDevice(L.ordinal));
+      void* const in = reinterpret_cast<void*>(h->nvls.uc_va[li]);
+      cudaError_t e = cudaMemcpyAsync(in, reinterpret_cast<const void*>(L.va[L.grank] + h->plan.src_off), s_max,
+                                      cudaMemcpyDeviceToDevice, L.stream);
+      if (e == cudaSuccess) e = cudaMemsetAsync(static_cast<uint8_t*>(in) + s_max, 0, s_max, L.stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
+      if (e != cudaSuccess) return fail_sticky(h, "cdprobe_allreduce_nvls: fill the NVLS area", e);
+    }
   }
 
   // 5. scratch for the records, the output (when it is there) and the granule table, grown on every local rank before
@@ -1135,6 +1253,10 @@ int cdprobe_allreduce_ring(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out
 
 int cdprobe_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
   return cdp::allreduce_call(h, reps, out, cdp::kPush);
+}
+
+int cdprobe_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out) {
+  return cdp::allreduce_call(h, reps, out, cdp::kNvls);
 }
 
 int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {

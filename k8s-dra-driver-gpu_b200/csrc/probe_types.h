@@ -590,6 +590,13 @@ static_assert(kPushOff % 128 == 0 && kPushOff + kMaxRanks * sizeof(FlagLine) <= 
               "the push all-reduce lines sit after the ring all-reduce lines inside the Ctrl granule");
 static_assert(kBwMaxSizes * (64 + 1) * 3 < (1u << kArBarrierBits), "push all-reduce barriers per call fit the low bits");
 
+// ---- the multicast all-reduce (cdprobe_allreduce_nvls, DESIGN §5m) --------------------------------------------------
+// The domain barriers of cdprobe_allreduce_nvls: one 128-byte line per sender after the push lines, in the Ctrl
+// granule.  Same rules as kArOff; two barriers per rep.
+constexpr uint64_t kNvlsOff = kPushOff + kMaxRanks * sizeof(FlagLine);  // 80 KiB
+static_assert(kNvlsOff % 128 == 0 && kNvlsOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the multicast all-reduce lines sit after the push all-reduce lines inside the Ctrl granule");
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -41,6 +41,18 @@ cudaError_t Driver::load(std::string* err) {
   return cudaSuccess;
 }
 
+bool Driver::load_multicast() {
+  if (multicast < 0)
+    multicast = resolve("cuMulticastCreate", &MulticastCreate, nullptr) == cudaSuccess &&
+                resolve("cuMulticastAddDevice", &MulticastAddDevice, nullptr) == cudaSuccess &&
+                resolve("cuMulticastBindMem", &MulticastBindMem, nullptr) == cudaSuccess &&
+                resolve("cuMulticastUnbind", &MulticastUnbind, nullptr) == cudaSuccess &&
+                resolve("cuMulticastGetGranularity", &MulticastGetGranularity, nullptr) == cudaSuccess &&
+                resolve("cuDeviceGet", &DeviceGet, nullptr) == cudaSuccess &&
+                resolve("cuDeviceGetAttribute", &DeviceGetAttribute, nullptr) == cudaSuccess;
+  return multicast == 1;
+}
+
 std::string Driver::error_name(CUresult r) const {
   const char* s = nullptr;
   if (GetErrorName && GetErrorName(r, &s) == CUDA_SUCCESS && s) return s;

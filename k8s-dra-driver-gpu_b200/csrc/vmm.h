@@ -26,9 +26,22 @@ struct Driver {
                                          unsigned long long) = nullptr;
   CUresult (*MemImportFromShareableHandle)(CUmemGenericAllocationHandle*, void*, CUmemAllocationHandleType) = nullptr;
   CUresult (*GetErrorName)(CUresult, const char**) = nullptr;
+  // Multicast objects (cdprobe_allreduce_nvls): resolved by load_multicast, apart from load's set, so that a driver
+  // without them still opens a handle.
+  CUresult (*MulticastCreate)(CUmemGenericAllocationHandle*, const CUmulticastObjectProp*) = nullptr;
+  CUresult (*MulticastAddDevice)(CUmemGenericAllocationHandle, CUdevice) = nullptr;
+  CUresult (*MulticastBindMem)(CUmemGenericAllocationHandle, size_t, CUmemGenericAllocationHandle, size_t, size_t,
+                               unsigned long long) = nullptr;
+  CUresult (*MulticastUnbind)(CUmemGenericAllocationHandle, CUdevice, size_t, size_t) = nullptr;
+  CUresult (*MulticastGetGranularity)(size_t*, const CUmulticastObjectProp*, CUmulticastGranularity_flags) = nullptr;
+  CUresult (*DeviceGet)(CUdevice*, int) = nullptr;
+  CUresult (*DeviceGetAttribute)(int*, CUdevice_attribute, CUdevice) = nullptr;
+  int multicast = -1;  // load_multicast's verdict, -1: not asked yet
 
   // Returns cudaSuccess or the runtime error that prevented loading.
   cudaError_t load(std::string* err);
+  // Whether every multicast entry point above resolved; asked once.
+  bool load_multicast();
   std::string error_name(CUresult r) const;
 };
 

@@ -698,6 +698,23 @@ class Probe:
         rc = self._lib.cdprobe_allreduce_push(self._h, reps, C.byref(t))
         return rc, t
 
+    def AllReduceNVLS(self, reps: int = 0) -> AllReduce:
+        """Go: (*Probe).AllReduceNVLS.  Multicast (NVLS) all-reduce of every rank's source buffer on every rank at once:
+        each rank sums its chunk of 8 KiB units with multimem.ld_reduce through one multicast object that spans the
+        domain and stores each sum to every rank with one multimem.st, at each size of the bwcurve ladder (0: 8 timed
+        reps per size).  A rep is timed from its opening to its closing barrier; path is ALLREDUCE_PATH_NVLS.  Rows are
+        ERR_UNSUPPORTED, with nothing run, where the devices, the driver or a shared device rule multicast out.
+        Collective when world_size > 1.  Needs no Run first and disturbs none."""
+        rc, t = self.allreduce_nvls_raw(reps)
+        _check(self._lib, rc, "cdprobe_allreduce_nvls")
+        return AllReduce.from_c(t)
+
+    def allreduce_nvls_raw(self, reps: int):
+        """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
+        t = abi.AllReduceT()
+        rc = self._lib.cdprobe_allreduce_nvls(self._h, reps, C.byref(t))
+        return rc, t
+
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps

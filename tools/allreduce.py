@@ -29,7 +29,14 @@ rep runs from its opening barrier's release to the moment the rank's output is c
 session: N = 1 at `--bytes` per pair on each data path (TMA bulk reductions, and red.global per word behind 16-byte and
 32-byte loads), and 2, 4 and 8 ranks sharing GPU 0 at `--multi-bytes` per pair on the TMA path.  A push rep runs from
 its opening barrier's release to its closing release, as a two-shot rep does.  Each rank's link traffic per rep is the
-two-shot's, 2 (n - 1) / n x size, every transfer a write, so busbw = algbw x 2 (n - 1) / n is reported for all three."""
+two-shot's, 2 (n - 1) / n x size, every transfer a write, so busbw = algbw x 2 (n - 1) / n is reported for all three.
+
+--nvls measures cdprobe_allreduce_nvls instead, next to the one-shot and the two-shot (TMA path) on the same handle in
+the same session, one rank per visible device (up to 8) at `--bytes` per pair.  It records in the same call the
+device's CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED, the VMM and multicast minimum granularities, the CUresult of a
+direct cuMulticastCreate of a one-device object, and the card's name, power limit and SM clock.  Where the NVLS call
+runs nothing (a driver that refuses a one-device object, on one GPU), its rows' status and cdprobe_last_error are
+recorded next to the one-shot's and the two-shot's times."""
 import argparse
 import json
 import os
@@ -51,6 +58,7 @@ ap.add_argument("--ll", action="store_true", help="measure cdprobe_allreduce_ll 
 ap.add_argument("--ll-bytes", type=int, default=1 << 20, help="bytes_per_pair of the --ll runs")
 ap.add_argument("--ring", action="store_true", help="measure cdprobe_allreduce_ring next to the one-shot and two-shot")
 ap.add_argument("--push", action="store_true", help="measure cdprobe_allreduce_push next to the one-shot and two-shot")
+ap.add_argument("--nvls", action="store_true", help="measure cdprobe_allreduce_nvls next to the one-shot and two-shot")
 a = ap.parse_args()
 
 
@@ -76,6 +84,83 @@ def rows(ar, bus=None):
             out[f"rank_{r}"]["peak_busbw_gbps"] = ar.peak_gbps[r] * bus
     return out
 
+
+def multicast_facts():
+    """CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED of device 0, the minimum VMM and multicast granularities for a
+    one-device object of 2 MiB, and the CUresult of cuMulticastCreate for such an object (POSIX fd handle type; 0:
+    created, and released at once), read through the driver API on device 0's primary context."""
+    import ctypes as C
+
+    class McProp(C.Structure):
+        _fields_ = [("numDevices", C.c_uint), ("size", C.c_size_t), ("handleTypes", C.c_ulonglong),
+                    ("flags", C.c_ulonglong)]
+
+    class Loc(C.Structure):
+        _fields_ = [("type", C.c_int), ("id", C.c_int)]
+
+    class AllocProp(C.Structure):
+        _fields_ = [("type", C.c_int), ("requestedHandleTypes", C.c_int), ("location", Loc), ("win32HandleMetaData",
+                    C.c_void_p), ("compressionType", C.c_ubyte), ("gpuDirectRDMACapable", C.c_ubyte),
+                    ("usage", C.c_ushort), ("reserved", C.c_ubyte * 4)]
+
+    cu = C.CDLL("libcuda.so.1")
+    dev, on, mc, vmm = C.c_int(), C.c_int(), C.c_size_t(), C.c_size_t()
+    assert cu.cuInit(0) == 0 and cu.cuDeviceGet(C.byref(dev), 0) == 0
+    assert cu.cuDeviceGetAttribute(C.byref(on), 132, dev) == 0  # CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED
+    ap_ = AllocProp(1, 0, Loc(1, dev.value))  # pinned, on device 0
+    assert cu.cuMemGetAllocationGranularity(C.byref(vmm), C.byref(ap_), 0) == 0
+    rc = cu.cuMulticastGetGranularity(C.byref(mc), C.byref(McProp(1, 2 << 20, 0, 0)), 0)
+    ctx, obj, name = C.c_void_p(), C.c_ulonglong(), C.c_char_p()
+    assert cu.cuDevicePrimaryCtxRetain(C.byref(ctx), dev) == 0 and cu.cuCtxPushCurrent(ctx) == 0
+    created = cu.cuMulticastCreate(C.byref(obj), C.byref(McProp(1, 2 << 20, 1, 0)))  # 1: POSIX file descriptor
+    if created == 0:
+        cu.cuMemRelease(obj)
+    cu.cuGetErrorName(created, C.byref(name))
+    cu.cuCtxPopCurrent(C.byref(C.c_void_p()))
+    cu.cuDevicePrimaryCtxRelease(dev)
+    return {"multicast_supported": on.value, "vmm_granularity_min": vmm.value,
+            "multicast_granularity_min": mc.value if rc == 0 else f"CUresult {rc}",
+            "create_one_device_2mib": {"curesult": created, "name": name.value.decode() if name.value else None}}
+
+
+if a.nvls:
+    import torch
+
+    n_dev = torch.cuda.device_count()
+    res = {"bytes": a.bytes, "reps": a.reps, "devices": n_dev, "multicast": multicast_facts(),
+           "what": "cdprobe_allreduce_nvls (nvls), cdprobe_allreduce (one_shot) and cdprobe_allreduce_twoshot "
+                   "(two_shot, TMA path) called one after another on the same handle, one rank per visible device "
+                   "(N = 1 on one GPU) with one CTA per SM and bytes per pair: ns per rep of every size of the bwcurve "
+                   "ladder for every call that ran, and the NVLS call's per-rank status where it ran nothing.  An nvls "
+                   "or two-shot rep runs from its opening to its closing barrier release; a one-shot rep from its "
+                   "opening barrier release to its latest CTA stamp.  algbw_gbps_median = bytes / ns_median; "
+                   "busbw_gbps_median = algbw x 2 (n - 1) / n"}
+    n = min(n_dev, 8)
+    bus = 2 * (n - 1) / n
+    with pkg.Open(pkg.Config(ordinals=list(range(n)), bytes=a.bytes * max(n - 1, 1), timeout_ms=60000)) as p:
+        nvls = p.AllReduceNVLS(a.reps)
+        nvls_error = p._lib.cdprobe_last_error().decode()
+        one = p.AllReduce(a.reps)
+        ts = p.AllReduceTwoShot(a.reps)
+        ran = all(nvls.measured[r] for r in range(n))
+        res[f"n{n}"] = {"nvls": {**(rows(nvls, bus) if ran else {"status": nvls.status, "last_error": nvls_error}),
+                                 "call_ms": nvls.ms, "path": nvls.path},
+                        "one_shot": {**rows(one, bus), "call_ms": one.ms},
+                        "two_shot": {**rows(ts, bus), "call_ms": ts.ms}}
+    res["gpu"] = gpu()
+    res["nvlink"] = "not measured" if n == 1 else f"measured by the n{n} rows"
+    runs = res[f"n{n}"]
+    print(f"{'bytes':>11} {'nvls ns':>11} {'one-shot':>11} {'two-shot':>11}  (rank 0)")
+    for i, (o, t) in enumerate(zip(runs["one_shot"]["rank_0"]["sizes"], runs["two_shot"]["rank_0"]["sizes"])):
+        v = runs["nvls"]["rank_0"]["sizes"][i]["ns_median"] if ran else float("nan")
+        print(f"{o['bytes']:11d} {v:11.0f} {o['ns_median']:11.0f} {t['ns_median']:11.0f}")
+    print(f"nvls ran: {ran}  status: {nvls.status} {nvls_error}  multicast: {res['multicast']}  gpu: {res['gpu']}")
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(res))
+    sys.exit(0)
 
 if a.push:
     res = {"bytes": a.bytes, "multi_bytes": a.multi_bytes, "reps": a.reps,
