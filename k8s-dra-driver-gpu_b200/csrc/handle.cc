@@ -52,6 +52,53 @@ static bool imex_channel0_present() {
   return true;
 }
 
+// Pinned memory on device `ordinal`, exportable as handle type `ht`.
+static CUmemAllocationProp alloc_prop(int ordinal, CUmemAllocationHandleType ht) {
+  CUmemAllocationProp ap;
+  memset(&ap, 0, sizeof(ap));
+  ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  ap.location.id = ordinal;
+  ap.requestedHandleTypes = ht;
+  return ap;
+}
+
+// Creates `bytes` of alloc_prop(ordinal, ht) memory in *hnd.
+static CUresult create_alloc(const cdprobe* h, int ordinal, CUmemAllocationHandleType ht, size_t bytes,
+                             CUmemGenericAllocationHandle* hnd) {
+  const CUmemAllocationProp ap = alloc_prop(ordinal, ht);
+  return h->drv.MemCreate(hnd, bytes, &ap, 0);
+}
+
+// Reserves `bytes` of address space aligned to `align`, maps `hnd` there and opens it to device `ordinal` for reading
+// and writing.  On failure nothing of it is kept.
+static CUresult map_range(const cdprobe* h, CUmemGenericAllocationHandle hnd, size_t bytes, size_t align, int ordinal,
+                          CUdeviceptr* va) {
+  CUresult r = h->drv.MemAddressReserve(va, bytes, align, 0, 0);
+  if (r != CUDA_SUCCESS) return r;
+  r = h->drv.MemMap(*va, bytes, 0, hnd, 0);
+  if (r != CUDA_SUCCESS) {
+    h->drv.MemAddressFree(*va, bytes);
+    return r;
+  }
+  CUmemAccessDesc ad;
+  memset(&ad, 0, sizeof(ad));
+  ad.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  ad.location.id = ordinal;
+  ad.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  r = h->drv.MemSetAccess(*va, bytes, &ad, 1);
+  if (r != CUDA_SUCCESS) {
+    h->drv.MemUnmap(*va, bytes);
+    h->drv.MemAddressFree(*va, bytes);
+  }
+  return r;
+}
+
+static void unmap_range(const cdprobe* h, CUdeviceptr va, size_t bytes) {
+  h->drv.MemUnmap(va, bytes);
+  h->drv.MemAddressFree(va, bytes);
+}
+
 // Map rank j's allocation of m into local rank li's address space.
 static int32_t map_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   LocalRank& L = h->lr[li];
@@ -66,25 +113,8 @@ static int32_t map_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   }
   if (cudaSetDevice(L.ordinal) != cudaSuccess) return CDPROBE_ERR_CUDA;
   CUdeviceptr va = 0;
-  const size_t sz = m.bytes;
-  CUresult r = h->drv.MemAddressReserve(&va, sz, kVmmGranule, 0, 0);
+  const CUresult r = map_range(h, hnd, m.bytes, kVmmGranule, L.ordinal, &va);
   if (r != CUDA_SUCCESS) return (int32_t)r;
-  r = h->drv.MemMap(va, sz, 0, hnd, 0);
-  if (r != CUDA_SUCCESS) {
-    h->drv.MemAddressFree(va, sz);
-    return (int32_t)r;
-  }
-  CUmemAccessDesc ad;
-  memset(&ad, 0, sizeof(ad));
-  ad.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-  ad.location.id = L.ordinal;
-  ad.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-  r = h->drv.MemSetAccess(va, sz, &ad, 1);
-  if (r != CUDA_SUCCESS) {
-    h->drv.MemUnmap(va, sz);
-    h->drv.MemAddressFree(va, sz);
-    return (int32_t)r;
-  }
   (L.*m.va)[j] = va;
   (L.*m.mapped)[j] = true;
   return 0;
@@ -94,8 +124,7 @@ static void unmap_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   LocalRank& L = h->lr[li];
   if (!(L.*m.mapped)[j]) return;
   cudaSetDevice(L.ordinal);
-  h->drv.MemUnmap((L.*m.va)[j], m.bytes);
-  h->drv.MemAddressFree((L.*m.va)[j], m.bytes);
+  unmap_range(h, (L.*m.va)[j], m.bytes);
   (L.*m.va)[j] = 0;
   (L.*m.mapped)[j] = false;
 }
@@ -126,14 +155,10 @@ static void release_shared(cdprobe* h, SharedAlloc& m) {
 static int create_own(cdprobe* h, SharedAlloc& m, uint32_t li) {
   LocalRank& L = h->lr[li];
   CDP_RT(cudaSetDevice(L.ordinal));
-  CUmemAllocationProp ap;
-  memset(&ap, 0, sizeof(ap));
-  ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-  ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-  ap.location.id = L.ordinal;
-  ap.requestedHandleTypes = h->handle_type == 8u   ? CU_MEM_HANDLE_TYPE_FABRIC
-                            : h->handle_type == 1u ? CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR
-                                                   : CU_MEM_HANDLE_TYPE_NONE;
+  const CUmemAllocationHandleType ht = h->handle_type == 8u   ? CU_MEM_HANDLE_TYPE_FABRIC
+                                       : h->handle_type == 1u ? CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR
+                                                              : CU_MEM_HANDLE_TYPE_NONE;
+  const CUmemAllocationProp ap = alloc_prop(L.ordinal, ht);
   size_t gran = 0;
   CUresult r = h->drv.MemGetAllocationGranularity(&gran, &ap, CU_MEM_ALLOC_GRANULARITY_MINIMUM);
   if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemGetAllocationGranularity", r);
@@ -141,7 +166,7 @@ static int create_own(cdprobe* h, SharedAlloc& m, uint32_t li) {
     set_err("unexpected VMM granularity " + std::to_string(gran));
     return CDPROBE_ERR_UNSUPPORTED;
   }
-  r = h->drv.MemCreate(&m.own[li], m.bytes, &ap, 0);
+  r = create_alloc(h, L.ordinal, ht, m.bytes, &m.own[li]);
   if (r != CUDA_SUCCESS) return fail_drv(h, "cuMemCreate", r);
   m.has_own[li] = true;
   if (h->handle_type == 1u) {
@@ -153,30 +178,54 @@ static int create_own(cdprobe* h, SharedAlloc& m, uint32_t li) {
   return CDPROBE_OK;
 }
 
+// What each process reports at a step of a collective setup: its return code and message and, where the step hands
+// something over, a payload (ensure_nvls: the area's size and the multicast object's fabric handle).
+struct StepReport {
+  int32_t rc;
+  char msg[124];
+  uint64_t bytes;
+  CUmemFabricHandle fabric;
+};
+
+// Every process's rc, shared: the first failure in process order wins, with its message, so that no process goes on
+// to an exchange another has left.  A failed exchange is CDPROBE_ERR_RENDEZVOUS.  `mine_in` (optional) is this
+// process's payload, and `first` (optional) gets the report of the process hosting rank 0.
+static int agree_step(cdprobe* h, int rc, const StepReport* mine_in = nullptr, StepReport* first = nullptr) {
+  StepReport mine;
+  memset(&mine, 0, sizeof(mine));
+  if (mine_in != nullptr) mine = *mine_in;
+  mine.rc = rc;
+  if (rc != CDPROBE_OK) snprintf(mine.msg, sizeof(mine.msg), "%s", g_last_error.c_str());
+  std::vector<StepReport> all(h->cfg.world_size, mine);
+  if (h->cfg.world_size > 1) {
+    std::string err;
+    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+  }
+  if (first != nullptr) *first = all[0];
+  for (uint32_t p = 0; p < all.size(); ++p)
+    if (all[p].rc != CDPROBE_OK) {
+      if (p != h->cfg.rank) set_err(all[p].msg);  // this process's own message stays whole
+      return all[p].rc;
+    }
+  return CDPROBE_OK;
+}
+
 // Creates m with allocations of `bytes`: one per local rank, exported and exchanged with every process over the
 // rendezvous, the other processes' imported, and rank j's mapped into local rank li wherever st[its rank][j] is 0 on
 // entry.  st[its rank][j] then holds the outcome: the import's CUresult, CDPROBE_ERR_UNSUPPORTED between MIG
-// instances, or map_peer's status.  With `agree`, the processes first share whether each created its allocations and
-// all return the first failure, so that none waits in an exchange another has left; without it (open, whose failure
-// ends the handle), a failure returns at once.  On failure the caller releases m.
+// instances, or map_peer's status.  With `agree`, the processes first share whether each created its allocations
+// (agree_step); without it (open, whose failure ends the handle), a failure returns at once.  On failure the caller
+// releases m.
 static int share_alloc(cdprobe* h, SharedAlloc& m, size_t bytes, int32_t (*st)[kMaxRanks], bool agree) {
   const cdprobe_config_t& c = h->cfg;
   std::string err;
   m.bytes = bytes;
   int rc = CDPROBE_OK;
   for (uint32_t li = 0; li < h->n_local && rc == CDPROBE_OK; ++li) rc = create_own(h, m, li);
-  if (agree && c.world_size > 1) {
-    int32_t mine = rc, all[kMaxRanks];
-    if (h->rdv.allgather(&mine, sizeof(mine), all, &err) != 0) {
-      set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-    for (uint32_t r = 0; r < c.world_size && rc == CDPROBE_OK; ++r)
-      if (all[r] != CDPROBE_OK) {
-        rc = all[r];
-        set_err("another process could not create its allocation");
-      }
-  }
+  if (agree) rc = agree_step(h, rc);
   if (rc != CDPROBE_OK) return rc;
 
   // ---- exchange handles between processes ---------------------------------
@@ -254,6 +303,18 @@ static int gather_status(cdprobe* h, int32_t (*st)[kMaxRanks]) {
   return CDPROBE_OK;
 }
 
+// Returns a collective setup's rc.  On failure, first releases what the setup made, keeping its message in
+// cdprobe_last_error, so that nothing is kept and the next call tries again.
+template <class Release>
+static int release_on_failure(int rc, Release release) {
+  if (rc != CDPROBE_OK) {
+    const std::string keep = g_last_error;
+    release();
+    g_last_error = keep;
+  }
+  return rc;
+}
+
 int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes) {
   if (m.bytes != 0) return CDPROBE_OK;
   bytes = (bytes + kVmmGranule - 1) / kVmmGranule * kVmmGranule;
@@ -262,14 +323,8 @@ int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes) {
     for (uint32_t j = 0; j < h->n_total; ++j) st[h->lr[li].grank][j] = cell_status(h, li, j);
   int rc = share_alloc(h, m, bytes, st, true);
   if (rc == CDPROBE_OK) rc = gather_status(h, st);
-  if (rc != CDPROBE_OK) {
-    const std::string keep = g_last_error;
-    release_shared(h, m);
-    g_last_error = keep;
-    return rc;
-  }
-  memcpy(m.status, st, sizeof(st));
-  return CDPROBE_OK;
+  if (rc == CDPROBE_OK) memcpy(m.status, st, sizeof(st));
+  return release_on_failure(rc, [&] { release_shared(h, m); });
 }
 
 // Unmaps the NVLS area in every local rank, unbinds every local device from the multicast object, then releases the
@@ -279,11 +334,8 @@ static void release_nvls(cdprobe* h) {
   for (uint32_t li = 0; li < h->n_local; ++li) {
     if (h->lr[li].ordinal < 0) continue;
     cudaSetDevice(h->lr[li].ordinal);
-    for (auto [va, mapped] : {std::pair{&a.mc_va[li], &a.mc_mapped[li]}, std::pair{&a.uc_va[li], &a.uc_mapped[li]}}) {
-      if (!*mapped) continue;
-      h->drv.MemUnmap(*va, a.bytes);
-      h->drv.MemAddressFree(*va, a.bytes);
-    }
+    if (a.mc_mapped[li]) unmap_range(h, a.mc_va[li], a.bytes);
+    if (a.uc_mapped[li]) unmap_range(h, a.uc_va[li], a.bytes);
   }
   for (uint32_t li = 0; li < h->n_local; ++li) {
     CUdevice dev;
@@ -299,63 +351,6 @@ static void release_nvls(cdprobe* h) {
   a = NvlsArea();
 }
 
-// Reserves `bytes` of address space on the current device, maps `hnd` there and opens it to device `ordinal`.
-static CUresult map_nvls(cdprobe* h, CUmemGenericAllocationHandle hnd, size_t bytes, size_t align, int ordinal,
-                         CUdeviceptr* va) {
-  CUresult r = h->drv.MemAddressReserve(va, bytes, align, 0, 0);
-  if (r != CUDA_SUCCESS) return r;
-  r = h->drv.MemMap(*va, bytes, 0, hnd, 0);
-  if (r != CUDA_SUCCESS) {
-    h->drv.MemAddressFree(*va, bytes);
-    return r;
-  }
-  CUmemAccessDesc ad;
-  memset(&ad, 0, sizeof(ad));
-  ad.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-  ad.location.id = ordinal;
-  ad.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-  r = h->drv.MemSetAccess(*va, bytes, &ad, 1);
-  if (r != CUDA_SUCCESS) {
-    h->drv.MemUnmap(*va, bytes);
-    h->drv.MemAddressFree(*va, bytes);
-  }
-  return r;
-}
-
-// What each process reports at a step of ensure_nvls: its return code and message, and from the process hosting rank
-// 0 the area's size and, for fabric handles, the multicast object's handle.
-struct NvlsOffer {
-  int32_t rc;
-  char msg[124];
-  uint64_t bytes;
-  CUmemFabricHandle fabric;
-};
-
-// Every process's rc, shared: the first failure in process order wins, with its message.  A failed exchange is
-// CDPROBE_ERR_RENDEZVOUS.  `offer` (optional) gets rank 0's process's report.
-static int nvls_agree(cdprobe* h, int rc, NvlsOffer* mine_in = nullptr, NvlsOffer* offer = nullptr) {
-  NvlsOffer mine;
-  memset(&mine, 0, sizeof(mine));
-  if (mine_in != nullptr) mine = *mine_in;
-  mine.rc = rc;
-  if (rc != CDPROBE_OK) snprintf(mine.msg, sizeof(mine.msg), "%s", g_last_error.c_str());
-  std::vector<NvlsOffer> all(h->cfg.world_size, mine);
-  if (h->cfg.world_size > 1) {
-    std::string err;
-    if (h->rdv.allgather(&mine, sizeof(mine), all.data(), &err) != 0) {
-      set_err(err);
-      return CDPROBE_ERR_RENDEZVOUS;
-    }
-  }
-  if (offer != nullptr) *offer = all[0];
-  for (const NvlsOffer& o : all)
-    if (o.rc != CDPROBE_OK) {
-      set_err(o.msg);
-      return o.rc;
-    }
-  return CDPROBE_OK;
-}
-
 static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
   NvlsArea& a = h->nvls;
   // a multicast object needs a shareable handle type even in one process (cuMulticastCreate refuses none)
@@ -367,7 +362,7 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
   mp.numDevices = h->n_total;
   mp.handleTypes = ht;
   // 1. the size, and in the process hosting rank 0 the object, exported for the others
-  NvlsOffer mine;
+  StepReport mine;
   memset(&mine, 0, sizeof(mine));
   int fd = -1;
   int rc = CDPROBE_OK;
@@ -395,13 +390,13 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
       if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemExportToShareableHandle(multicast fabric)", r);
     }
   }
-  NvlsOffer offer;
-  rc = nvls_agree(h, rc, &mine, &offer);
+  StepReport host0_report;
+  rc = agree_step(h, rc, &mine, &host0_report);
   if (rc != CDPROBE_OK) {
     if (fd >= 0) ::close(fd);
     return rc;
   }
-  a.bytes = offer.bytes;
+  a.bytes = host0_report.bytes;
   // 2. the handle to the other processes.  allgather_fds takes one descriptor from every process: the others send
   //    their probe allocation's, which every receiver closes unread
   if (h->cfg.world_size > 1 && ht == CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR) {
@@ -421,7 +416,7 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
     }
     for (int f : all) ::close(f);
   } else if (h->cfg.world_size > 1 && !host0) {
-    r = h->drv.MemImportFromShareableHandle(&a.mc, &offer.fabric, ht);
+    r = h->drv.MemImportFromShareableHandle(&a.mc, &host0_report.fabric, ht);
     if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMemImportFromShareableHandle(multicast fabric)", r);
     else a.has_mc = true;
   }
@@ -433,7 +428,7 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
     if (r == CUDA_SUCCESS) r = h->drv.MulticastAddDevice(a.mc, dev);
     if (r != CUDA_SUCCESS) rc = fail_drv(h, "cuMulticastAddDevice", r);
   }
-  if ((rc = nvls_agree(h, rc)) != CDPROBE_OK) return rc;
+  if ((rc = agree_step(h, rc)) != CDPROBE_OK) return rc;
   // 4. per local rank: its allocation, bound at offset 0, then the object and the allocation mapped into it
   for (uint32_t li = 0; li < h->n_local && rc == CDPROBE_OK; ++li) {
     LocalRank& L = h->lr[li];
@@ -442,13 +437,7 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
       rc = CDPROBE_ERR_CUDA;
       break;
     }
-    CUmemAllocationProp ap;
-    memset(&ap, 0, sizeof(ap));
-    ap.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-    ap.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    ap.location.id = L.ordinal;
-    ap.requestedHandleTypes = ht;
-    r = h->drv.MemCreate(&a.own[li], a.bytes, &ap, 0);
+    r = create_alloc(h, L.ordinal, ht, a.bytes, &a.own[li]);
     if (r != CUDA_SUCCESS) {
       rc = fail_drv(h, "cuMemCreate", r);
       break;
@@ -460,32 +449,26 @@ static int ensure_nvls_steps(cdprobe* h, size_t bytes, bool* refused) {
       break;
     }
     a.bound[li] = true;
-    r = map_nvls(h, a.mc, a.bytes, align, L.ordinal, &a.mc_va[li]);
+    r = map_range(h, a.mc, a.bytes, align, L.ordinal, &a.mc_va[li]);
     if (r != CUDA_SUCCESS) {
       rc = fail_drv(h, "cuMemMap(multicast)", r);
       break;
     }
     a.mc_mapped[li] = true;
-    r = map_nvls(h, a.own[li], a.bytes, align, L.ordinal, &a.uc_va[li]);
+    r = map_range(h, a.own[li], a.bytes, align, L.ordinal, &a.uc_va[li]);
     if (r != CUDA_SUCCESS) {
       rc = fail_drv(h, "cuMemMap(unicast)", r);
       break;
     }
     a.uc_mapped[li] = true;
   }
-  return nvls_agree(h, rc);
+  return agree_step(h, rc);
 }
 
 int ensure_nvls(cdprobe* h, size_t bytes, bool* refused) {
   *refused = false;
   if (h->nvls.bytes != 0) return CDPROBE_OK;
-  const int rc = ensure_nvls_steps(h, bytes, refused);
-  if (rc != CDPROBE_OK) {
-    const std::string keep = g_last_error;
-    release_nvls(h);
-    g_last_error = keep;
-  }
-  return rc;
+  return release_on_failure(ensure_nvls_steps(h, bytes, refused), [h] { release_nvls(h); });
 }
 
 // Phase table of local rank li: see schedule.cc.

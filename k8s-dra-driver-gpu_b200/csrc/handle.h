@@ -61,9 +61,8 @@ struct LocalRank {
 
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
 // exports them, takes the other processes' over the rendezvous, imports them and maps every rank's into every local
-// rank (handle.cc, share_alloc).  The probe allocation is one (open); cdprobe_alltoall's exchange area,
-// cdprobe_allreduce_twoshot's gather area, cdprobe_allreduce_ll's LL area, cdprobe_allreduce_ring's ring area and
-// cdprobe_allreduce_push's push area are others (ensure_area), and keep their state here.
+// rank (handle.cc, share_alloc).  The probe allocation and the measurements' unicast areas are SharedAllocs (the
+// cdprobe members say which, how large and whose).
 struct SharedAlloc {
   size_t bytes = 0;                                       // of each allocation; 0: not created
   CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
@@ -75,16 +74,16 @@ struct SharedAlloc {
   bool has_import[kMaxRanks] = {};
   int32_t status[kMaxRanks][kMaxRanks] = {};  // an area's [issuer][owner] mapping status, all ranks, once it exists
                                               // (the probe allocation's is cdprobe::status)
-  bool stale = false;  // the LL, ring or push area must be zeroed before its next use: it is new, or a local rank's
-                       // kernel timed out and it may hold packets, data, flags or partial sums of any earlier call
+  bool stale = false;  // an area that must start zeroed must be zeroed before its next use: it is new, or a local
+                       // rank's kernel timed out and it may hold packets, data, flags or partial sums of any earlier call
   SharedAlloc(CUdeviceptr (LocalRank::*v)[kMaxRanks], bool (LocalRank::*m)[kMaxRanks]) : va(v), mapped(m) {
     for (int& f : own_fd) f = -1;
   }
 };
 
-// cdprobe_allreduce_nvls's NVLS area (handle.cc, ensure_nvls): one multicast object of `bytes` that spans the domain,
-// and per local rank an allocation of `bytes` on its device, bound into the object at offset 0, mapped into the rank
-// both through the object (multicast) and on its own (unicast).  Peers never map another rank's allocation.
+// The NVLS area (handle.cc, ensure_nvls): one multicast object of `bytes` that spans the domain, and per local rank an
+// allocation of `bytes` on its device, bound into the object at offset 0, mapped into the rank both through the object
+// (multicast) and on its own (unicast).  Peers never map another rank's allocation.
 struct NvlsArea {
   size_t bytes = 0;                         // of the object and of each allocation; 0: not created
   CUmemGenericAllocationHandle mc = 0;      // the multicast object, created here or imported from rank 0's process
@@ -105,13 +104,23 @@ struct cdprobe {
   uint32_t n_total = 0, n_local = 0, first = 0;
   uint32_t handle_type = 0;  // 0 none, 1 posix fd, 8 fabric
   cdp::LocalRank lr[cdp::kMaxRanks];
-  cdp::SharedAlloc mem{&cdp::LocalRank::va, &cdp::LocalRank::mapped};             // the probe allocation
-  cdp::SharedAlloc area{&cdp::LocalRank::area_va, &cdp::LocalRank::area_mapped};  // cdprobe_alltoall's exchange area
-  cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};  // the two-shot's gather area
-  cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};  // cdprobe_allreduce_ll's LL area
-  cdp::SharedAlloc ring{&cdp::LocalRank::ring_va, &cdp::LocalRank::ring_mapped};  // cdprobe_allreduce_ring's ring area
-  cdp::SharedAlloc push{&cdp::LocalRank::push_va, &cdp::LocalRank::push_mapped};  // cdprobe_allreduce_push's push area
-  cdp::NvlsArea nvls;  // cdprobe_allreduce_nvls's multicast object and NVLS areas
+  // The device memory shared across the domain, per rank.  The probe allocation is made at open; every other area on
+  // the first call of the measurement that owns it (ensure_area, ensure_nvls), rounded up to the VMM granule.  All are
+  // kept until close.
+  cdp::SharedAlloc mem{&cdp::LocalRank::va, &cdp::LocalRank::mapped};  // the probe allocation: plan.alloc_bytes
+  // cdprobe_alltoall's exchange area: n_total x bytes_per_pair
+  cdp::SharedAlloc area{&cdp::LocalRank::area_va, &cdp::LocalRank::area_mapped};
+  // cdprobe_allreduce_twoshot's gather area: bytes_per_pair
+  cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};
+  // cdprobe_allreduce_ll's LL area: 2 x n_total x 2 x the LL ladder's largest size
+  cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};
+  // cdprobe_allreduce_ring's ring area: bytes_per_pair and one flag per 8 KiB of it
+  cdp::SharedAlloc ring{&cdp::LocalRank::ring_va, &cdp::LocalRank::ring_mapped};
+  // cdprobe_allreduce_push's push area: bytes_per_pair
+  cdp::SharedAlloc push{&cdp::LocalRank::push_va, &cdp::LocalRank::push_mapped};
+  // cdprobe_allreduce_nvls's multicast object and NVLS areas: 2 x bytes_per_pair, also rounded up to the multicast
+  // granularity
+  cdp::NvlsArea nvls;
   int32_t status[cdp::kMaxRanks][cdp::kMaxRanks];  // [issuer][owner] mapping status, all ranks
   uint64_t launch_seq = 0;
   uint64_t last_run_seq = 0;  // launch_seq of the last cdprobe_run (0: none yet); the run a diagnosis checks
@@ -189,24 +198,20 @@ inline bool launch_cooperatively(const cdprobe* h, const LocalRank& L) {
   return L.coop && !(h->cfg.flags & CDPROBE_FLAG_NO_COOPERATIVE);
 }
 
-// A measurement's shared area m (handle.cc): cdprobe_alltoall's exchange area (h->area, n_total x bytes_per_pair),
-// cdprobe_allreduce_twoshot's gather area (h->gather, bytes_per_pair), cdprobe_allreduce_ll's LL area (h->ll,
-// 2 x n_total x 2 x the LL ladder's largest size), cdprobe_allreduce_ring's ring area (h->ring, bytes_per_pair and
-// one flag per 8 KiB of it) or cdprobe_allreduce_push's push area (h->push, bytes_per_pair).  On the first call, every
-// local rank creates
-// `bytes` of device memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every
-// local rank wherever the probe mapping is then up; m.status gets every rank's mapping statuses.  Collective.  If
-// creating it fails in any process, every process returns that error with nothing kept, and the next call tries
-// again.  Kept until close.
+// A measurement's unicast shared area m (handle.cc).  On the first call, every local rank creates `bytes` of device
+// memory (rounded up to the VMM granule), shared like the probe allocation and mapped into every local rank wherever
+// the probe mapping is then up; m.status gets every rank's mapping statuses.  Collective.  If creating it fails in any
+// process, every process returns the first failure in process order, with that process's message; nothing is kept,
+// and the next call tries again.  Kept until close.
 int ensure_area(cdprobe* h, SharedAlloc& m, size_t bytes);
 
-// cdprobe_allreduce_nvls's NVLS area (h->nvls, DESIGN §5m): on the first call, `bytes` rounded up to the VMM granule
-// and to the multicast granularity.  The process hosting rank 0 creates the multicast object with the probe
-// allocation's handle type (POSIX fd within one process, which has none) and hands it to the others over the
-// rendezvous; every process adds its devices; once every process has reported that, each local rank creates its
-// allocation, binds it at offset 0 and maps the object and its allocation.  Collective, and only for a domain that
-// agree() found able to run it.  If a step fails in any process, every process returns that error with nothing kept
-// (cdprobe_last_error names the step and the CUresult), and the next call tries again.  *refused: the failure is the
+// The NVLS area (h->nvls, DESIGN §5m): on the first call, `bytes` rounded up to the VMM granule and to the multicast
+// granularity.  The process hosting rank 0 creates the multicast object with the probe allocation's handle type
+// (POSIX fd within one process, which has none) and hands it to the others over the rendezvous; every process adds
+// its devices; once every process has reported that, each local rank creates its allocation, binds it at offset 0 and
+// maps the object and its allocation.  Collective, and only for a domain that agree() found able to run it.  If a step
+// fails in any process, every process returns the first failure as ensure_area does (cdprobe_last_error names the
+// step and the CUresult); nothing is kept, and the next call tries again.  *refused: the failure is the
 // driver refusing a multicast object of one device (cuMulticastCreate, CUDA_ERROR_INVALID_VALUE, n_total == 1), which
 // the caller reports as CDPROBE_ERR_UNSUPPORTED rows.  Kept until close.
 int ensure_nvls(cdprobe* h, size_t bytes, bool* refused);
