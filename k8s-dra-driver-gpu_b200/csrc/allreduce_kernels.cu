@@ -90,9 +90,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_con
 }
 
 int allreduce_launch(const AllReduceParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_kernel, p, grid, cooperative, stream);
 }
 
 template int granules_launch(uint64_t*, uint64_t*, const AllReduceWord&, uint64_t, unsigned, cudaStream_t);

@@ -33,11 +33,7 @@ __device__ bool ll_rep(const Ctx& c, const LlParams& P, uint32_t k, uint32_t r, 
   const uint64_t salt = ll_salt(P.seed, g, flag);
   const unsigned long long* src = reinterpret_cast<const unsigned long long*>(P.src);
   const bool armed = r == 1u && k == P.fault_k;
-  if (armed && P.fault_mode == 1u) {
-    const uint64_t until = gtimer() + P.fault_arg * 1000u;  // below timeout_ms / 2 (the host checks)
-    while (gtimer() < until) {
-    }
-  }
+  if (armed && P.fault_mode == 1u) delay_us(P.fault_arg);
   const uint64_t fw = armed && P.fault_mode == 0u ? P.fault_arg : ~0ull;
 
   // 1. push: one packet per owned word to rank g + 1, g + 2, ... (mod n)
@@ -120,9 +116,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(const __grid_
 }
 
 int allreduce_ll_launch(const LlParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_ll_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_ll_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_ll_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

@@ -111,9 +111,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_nvls_kernel(const __gri
 }
 
 int allreduce_nvls_launch(const NvlsParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_nvls_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_nvls_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_nvls_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

@@ -4,7 +4,10 @@
 // Two things are parameters: the walk (which units a warp sums) and the store policy (where a summed unit goes).
 // Also the word check of an output in the rank's scratch (ar_check), shared by the one-shot and allreduce_ll_kernel
 // (allreduce_ll_kernels.cu), and the word check and clear of an output peers store into (ar_check_clear), shared by
-// the two-shot and allreduce_ring_kernel (allreduce_ring_kernels.cu).
+// the two-shot and allreduce_ring_kernel (allreduce_ring_kernels.cu).  And the pieces the all-reduce kernels share
+// around those: the store of a unit to several ranks (put_ranks, the two-shot's and the push's store policies), the
+// pair store (stg_pair, also the ring's), the armed delay (delay_us, the LL's and the ring's) and the fenced close of
+// a phase (close_fenced, the two-shot's and the push's).
 //
 // A store policy S has one member, called once per unit by every lane with the unit's sums in acc:
 //   template <uint32_t kLaneBytes> static void S::put(const Ctx&, const Params& P, uint64_t u, uint32_t len,
@@ -34,6 +37,63 @@ __device__ __forceinline__ uint32_t ar_vec_off(int lane, int i) {
 __device__ __forceinline__ void ar_add(uint64_t (&acc)[kArWords], int i, const uint4& v) {
   acc[2 * i] += pack64(v.x, v.y);
   acc[2 * i + 1] += pack64(v.z, v.w);
+}
+
+// Two 64-bit words to global memory at p with one st.global.v4.
+__device__ __forceinline__ void stg_pair(uint8_t* p, uint64_t w0, uint64_t w1) {
+  stg_v4(reinterpret_cast<uint4*>(p),
+         make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+}
+
+// A store policy's body for a unit that goes to several ranks: the summed unit u (len bytes, lane vector i at
+// ar_vec_off<kLaneBytes>(lane, i)) goes to P.dst[t0], P.dst[t0 + 1], ..., P.dst[P.n - 1], and acc is cleared.  The
+// armed fault (fw, an output word index; ~0 when none) acts on the stores to P.dst[P.fault_dst] only: the word leaves
+// xored with 1, or (kDrop, for parameters with a fault_drop, and P.fault_drop) nothing of its unit goes there.  The
+// xor is written out here and in the ring's ring_unit rather than in a helper of its own: as a separate inline
+// function it compiled to a branch around every vector's store instead of predicated instructions, and this form
+// compiles to the same SASS as the store policies it replaced.
+template <uint32_t kLaneBytes, bool kDrop, typename Params>
+__device__ __forceinline__ void put_ranks(const Ctx& c, const Params& P, uint32_t t0, uint64_t u, uint32_t len,
+                                          uint64_t fw, uint64_t (&acc)[kArWords]) {
+  const uint32_t hit_dst = fw / (kUnitBytes / 8) == u ? P.fault_dst : ~0u;  // rare: this unit holds the armed word
+  const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
+  for (uint32_t t = t0; t < P.n; ++t) {
+    if constexpr (kDrop) {
+      if (t == hit_dst && P.fault_drop) continue;
+    }
+    uint8_t* base = P.dst[t] + u * kUnitBytes;
+#pragma unroll
+    for (int i = 0; i < kArWords / 2; ++i) {
+      const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
+      if (off >= len) continue;
+      uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
+      if (t == hit_dst && off == (fb & ~15u)) {
+        if (fb & 8u) w1 ^= 1ull;
+        else w0 ^= 1ull;
+      }
+      stg_pair(base + off, w0, w1);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+}
+
+// The armed delay of the LL and ring kernels: spins until `us` microseconds have passed (below timeout_ms / 2, which
+// the host checks).
+__device__ __forceinline__ void delay_us(uint64_t us) {
+  const uint64_t until = gtimer() + us * 1000u;
+  while (gtimer() < until) {
+  }
+}
+
+// Closes a phase whose stores go to peers (the two-shot and the push): after a CTA barrier, thread 0 issues one
+// fence.sys, so every store of the CTA has reached its peer before the fenced domain barrier b signals; its release
+// is stamped into *stamp (unless null).  Returns false in every thread once the launch is aborted.
+__device__ __forceinline__ bool close_fenced(const Ctx& c, BwScratch* bs, uint32_t b, unsigned long long* stamp,
+                                             const DomainLines* dom) {
+  __syncthreads();
+  if (threadIdx.x == 0) __threadfence_system();
+  return grid_barrier(c, bs, b, stamp, dom, true);
 }
 
 // TMA read side: the warp walks (unit, input) pairs, the n inputs of a unit in a row, through its kStages-deep ring of
@@ -144,6 +204,17 @@ __device__ __forceinline__ void ar_units(Ctx& c, const Params& P, uint64_t bytes
   else ar_units_tma<Store>(c, P, bytes, walk, fw, a);
 }
 
+// The end of a word check, by every lane with its own count of bad words and lowest bad word's byte offset: one atomic
+// pair per warp with a bad word into the counters of size k.
+__device__ __forceinline__ void ar_check_flush(const Ctx& c, ArScratch* as, uint32_t k, uint64_t bad, uint64_t first) {
+  bad = warp_sum64(bad);
+  first = warp_min64(first);
+  if (c.lane == 0 && bad != 0) {
+    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
+    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
+  }
+}
+
 // The untimed word check of the output the last rep of size k stored at P.out (allreduce_kernel and
 // allreduce_ll_kernel): each lane compares every 32nd word of its warp's share with allreduce_word, reading at L2
 // (other SMs stored them).  One atomic pair per warp with a bad word.
@@ -159,12 +230,7 @@ __device__ void ar_check(const Ctx& c, const Params& P, ArScratch* as, uint32_t 
       first = min(first, w * 8u);
     }
   }
-  bad = warp_sum64(bad);
-  first = warp_min64(first);
-  if (c.lane == 0 && bad != 0) {
-    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
-    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
-  }
+  ar_check_flush(c, as, k, bad, first);
 }
 
 // The untimed check of rep r of size k of an output peers store into (allreduce_twoshot_kernel's gather area,
@@ -201,12 +267,7 @@ __device__ void ar_check_clear(const Ctx& c, const Params& P, uint4* const out, 
     fold_unit(a, ux, u);
   }
   __threadfence();  // the clearing stores are performed before the next opening barrier signals the peers
-  bad = warp_sum64(bad);
-  first = warp_min64(first);
-  if (c.lane == 0 && bad != 0) {
-    atomicAdd(&as->bad_words[k], (unsigned long long)bad);
-    atomicMax(&as->first_bad_n[k], (unsigned long long)~first);
-  }
+  ar_check_flush(c, as, k, bad, first);
   Acc* const acc = &as->rep.rep[k][r];
   cta_reduce<1>(c, red, &a, &acc);
 }

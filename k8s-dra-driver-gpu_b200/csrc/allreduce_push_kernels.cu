@@ -144,26 +144,7 @@ struct ToPeers {
   template <uint32_t kLaneBytes>
   __device__ __forceinline__ static void put(const Ctx& c, const PeerView& V, uint64_t u, uint32_t len, uint64_t fw,
                                              uint64_t (&acc)[kArWords], Sum&) {
-    const PushParams& P = *V.P;
-    const uint32_t hit_dst = fw / (kUnitBytes / 8) == u ? P.fault_dst : ~0u;  // rare: this unit holds the armed word
-    const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
-    for (uint32_t t = 1; t < P.n; ++t) {
-      uint8_t* base = P.dst[t] + u * kUnitBytes;
-#pragma unroll
-      for (int i = 0; i < kArWords / 2; ++i) {
-        const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
-        if (off >= len) continue;
-        uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
-        if (t == hit_dst && off == (fb & ~15u)) {
-          if (fb & 8u) w1 ^= 1ull;
-          else w0 ^= 1ull;
-        }
-        stg_v4(reinterpret_cast<uint4*>(base + off),
-               make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+    put_ranks<kLaneBytes, false>(c, *V.P, 1u, u, len, fw, acc);
   }
 };
 }  // namespace
@@ -201,26 +182,20 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_push_kernel(const __gri
       if (P.path == 2u) reduce_ldst<32>(c, P, bytes, walk, fu, fb, P.fault_mode);
       else if (P.path == 1u) reduce_ldst<16>(c, P, bytes, walk, fu, fb, P.fault_mode);
       else reduce_tma(c, P, bytes, walk, fu, fb, P.fault_mode);  // aborted: the barrier below sees it
-      __syncthreads();
-      if (threadIdx.x == 0) __threadfence_system();  // every reduction of this CTA has reached its owner
-      if (!grid_barrier(c, bs, b++, nullptr, &P.dom, true)) return;
+      if (!close_fenced(c, bs, b++, nullptr, &P.dom)) return;  // this rank's chunk is complete in its area
       if (P.n > 1) {
         Sum a{0ull, 0ull, 0ull};
         ar_units<ToPeers>(c, V, bytes, Walk<false>{hi, lo + gwarp, 0ull, nwarps, nullptr},
                           armed && P.fault_mode == 3u ? P.fault_word : ~0ull, a);
       }
-      __syncthreads();
-      if (threadIdx.x == 0) __threadfence_system();  // every push of this CTA has reached its peer
-      if (!grid_barrier(c, bs, b++, &bs->rep[k][r].t_end, &P.dom, true)) return;
+      if (!close_fenced(c, bs, b++, &bs->rep[k][r].t_end, &P.dom)) return;
       ar_check_clear(c, P, reinterpret_cast<uint4*>(P.dst[0]), as, red, k, r, bytes, gwarp, nwarps);
     }
   }
 }
 
 int allreduce_push_launch(const PushParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_push_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_push_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_push_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

@@ -70,16 +70,13 @@ __device__ __forceinline__ void ring_unit(const Ctx& c, const RingParams& P, uin
     const uint32_t off = ar_vec_off<16>(c.lane, i);
     if (off >= len) continue;
     uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
-    if (st.own)
-      stg_v4(reinterpret_cast<uint4*>(P.out + base + off),
-             make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+    if (st.own) stg_pair(P.out + base + off, w0, w1);
     if (!st.push || drop) continue;
     if (off == (hit & ~15u)) {
       if (hit & 8u) w1 ^= 1ull;
       else w0 ^= 1ull;
     }
-    stg_v4(reinterpret_cast<uint4*>(P.next + base + off),
-           make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
+    stg_pair(P.next + base + off, w0, w1);
   }
 }
 
@@ -102,11 +99,7 @@ __device__ bool ring_rep(const Ctx& c, const RingParams& P, uint32_t k, uint32_t
   const uint32_t* const in_flags = reinterpret_cast<const uint32_t*>(P.out + ring_flags_off(P.s_max));
   uint32_t* const out_flags = reinterpret_cast<uint32_t*>(P.next + ring_flags_off(P.s_max));
   const bool armed = r == 1u && k == P.fault_k;
-  if (armed && P.fault_mode == 2u) {
-    const uint64_t until = gtimer() + P.fault_arg * 1000u;  // below timeout_ms / 2 (the host checks)
-    while (gtimer() < until) {
-    }
-  }
+  if (armed && P.fault_mode == 2u) delay_us(P.fault_arg);
   const uint64_t fw = armed && P.fault_mode < 2u ? P.fault_arg : ~0ull;
   for (uint64_t j = gwarp; j * kRingFlagUnits < span; j += nwarps) {
     for (uint32_t s = 0; s <= last; ++s) {
@@ -164,9 +157,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_ring_kernel(const __gri
 }
 
 int allreduce_ring_launch(const RingParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_ring_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_ring_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

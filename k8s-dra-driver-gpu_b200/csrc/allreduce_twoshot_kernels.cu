@@ -20,26 +20,7 @@ struct ToGather {
   template <uint32_t kLaneBytes>
   __device__ __forceinline__ static void put(const Ctx& c, const TwoShotParams& P, uint64_t u, uint32_t len,
                                              uint64_t fw, uint64_t (&acc)[kArWords], Sum&) {
-    const uint32_t hit_dst = fw / (kUnitBytes / 8) == u ? P.fault_dst : ~0u;  // rare: this unit holds the armed word
-    const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
-    for (uint32_t t = 0; t < P.n; ++t) {
-      if (t == hit_dst && P.fault_drop) continue;
-      uint8_t* base = P.dst[t] + u * kUnitBytes;
-#pragma unroll
-      for (int i = 0; i < kArWords / 2; ++i) {
-        const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
-        if (off >= len) continue;
-        uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
-        if (t == hit_dst && off == (fb & ~15u)) {
-          if (fb & 8u) w1 ^= 1ull;
-          else w0 ^= 1ull;
-        }
-        stg_v4(reinterpret_cast<uint4*>(base + off),
-               make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
+    put_ranks<kLaneBytes, true>(c, P, 0u, u, len, fw, acc);
   }
 };
 }  // namespace
@@ -70,18 +51,14 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(const __
       const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
       Sum a{0ull, 0ull, 0ull};
       ar_units<ToGather>(c, P, bytes, Walk<false>{hi, lo + gwarp, 0ull, nwarps, nullptr}, fw, a);
-      __syncthreads();
-      if (threadIdx.x == 0) __threadfence_system();  // every store of this CTA has reached its gather area
-      if (!grid_barrier(c, bs, b++, &bs->rep[k][r].t_end, &P.dom, true)) return;
+      if (!close_fenced(c, bs, b++, &bs->rep[k][r].t_end, &P.dom)) return;
       ar_check_clear(c, P, reinterpret_cast<uint4*>(P.dst[0]), as, red, k, r, bytes, gwarp, nwarps);
     }
   }
 }
 
 int allreduce_twoshot_launch(const TwoShotParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(allreduce_twoshot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(allreduce_twoshot_kernel, p, grid, cooperative, stream);
+  return grid_launch(allreduce_twoshot_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

@@ -161,9 +161,7 @@ __global__ void __launch_bounds__(kThreads, 1) alltoall_kernel(const __grid_cons
 }
 
 int alltoall_launch(const AllToAllParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(alltoall_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(alltoall_kernel, p, grid, cooperative, stream);
+  return grid_launch(alltoall_kernel, p, grid, cooperative, stream);
 }
 
 }  // namespace cdp

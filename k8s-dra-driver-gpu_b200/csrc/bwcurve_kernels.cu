@@ -39,9 +39,7 @@ __global__ void __launch_bounds__(kThreads, 1) bwcurve_kernel(const __grid_const
 }
 
 int bwcurve_launch(const BwCurveParams& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(bwcurve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e != cudaSuccess ? (int)e : grid_launch(bwcurve_kernel, p, grid, cooperative, stream);
+  return grid_launch(bwcurve_kernel, p, grid, cooperative, stream);
 }
 
 template int granules_launch(uint64_t*, uint64_t*, const SrcRegionWord&, uint64_t, unsigned, cudaStream_t);

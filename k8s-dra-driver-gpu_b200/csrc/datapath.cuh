@@ -607,13 +607,17 @@ int granules_launch(uint64_t* gsum, uint64_t* gxor, const Word& word, uint64_t n
 
 // ----------------------------------------------------------- launcher -----
 namespace {
-// Launches a persistent kernel (cdprobe_kernel, bwcurve_kernel, allreduce_kernel or alltoall_kernel) on `stream` of
-// the current device: `grid` CTAs of kThreads threads and kSmemBytes of dynamic shared memory, cooperative or not.
+// Launches a persistent kernel (cdprobe_kernel, bwcurve_kernel, alltoall_kernel or one of the six all-reduce kernels)
+// on `stream` of the current device: `grid` CTAs of kThreads threads and kSmemBytes of dynamic shared memory,
+// cooperative or not.  Sets the kernel's dynamic shared-memory limit to kSmemBytes first, on every launch; for
+// cdprobe_kernel, whose launcher has already set it before its occupancy check, that is one redundant driver call.
 // Returns a cudaError_t.
 template <typename Params>
 int grid_launch(void (*kernel)(Params), const Params& p, unsigned grid, bool cooperative, cudaStream_t stream) {
-  void* args[] = {const_cast<Params*>(&p)};
   const void* f = reinterpret_cast<const void*>(kernel);
+  const cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  if (e != cudaSuccess) return (int)e;
+  void* args[] = {const_cast<Params*>(&p)};
   return (int)(cooperative ? cudaLaunchCooperativeKernel(f, dim3(grid), dim3(kThreads), args, kSmemBytes, stream)
                            : cudaLaunchKernel(f, dim3(grid), dim3(kThreads), args, kSmemBytes, stream));
 }

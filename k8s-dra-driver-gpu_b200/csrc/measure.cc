@@ -490,6 +490,20 @@ struct ArProtocol {
   bool nvls = false;                             // it runs through the multicast object (h->nvls, ensure_nvls)
 };
 
+// The fields every all-reduce's parameters share, for local rank L, in parameters that start zeroed: the domain
+// barrier, the seed, the rank, the rank count and the armed fault's size, kArNoFault unless the fault acts in L.
+template <typename Params>
+static Params ar_params(const cdprobe* h, const LocalRank& L, const DomainLines& dom, const ArFault& f) {
+  Params p;
+  memset(&p, 0, sizeof(p));
+  p.dom = dom;
+  p.seed = h->seed;
+  p.rank = L.grank;
+  p.n = h->n_total;
+  p.fault_k = L.grank == f.rank ? f.k : kArNoFault;
+  return p;
+}
+
 static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
   const uint64_t fr = v >> 32, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
   if (fr == 0 || fr > h->n_total || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
@@ -501,16 +515,10 @@ static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad
 static int oneshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                           uint32_t) {
   const uint32_t g = L.grank, n = h->n_total;
-  AllReduceParams p;
-  memset(&p, 0, sizeof(p));
+  AllReduceParams p = ar_params<AllReduceParams>(h, L, dom, f);
   for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
-  p.dom = dom;
   p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_word = f.word;
-  p.rank = g;
-  p.n = n;
   return launch_ladder(h, L, p, lad, allreduce_launch, "launch allreduce_kernel");
 }
 
@@ -533,20 +541,14 @@ static const char* twoshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad
 static int twoshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                           uint32_t) {
   const uint32_t g = L.grank, n = h->n_total;
-  TwoShotParams p;
-  memset(&p, 0, sizeof(p));
+  TwoShotParams p = ar_params<TwoShotParams>(h, L, dom, f);
   for (uint32_t t = 0; t < n; ++t) {
     p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
     p.dst[t] = reinterpret_cast<uint8_t*>(L.gather_va[(g + t) % n]);
   }
-  p.dom = dom;
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_word = f.word;
   p.fault_dst = (f.recv + n - g) % n;
   p.fault_drop = f.mode;
-  p.rank = g;
-  p.n = n;
   return launch_ladder(h, L, p, lad, allreduce_twoshot_launch, "launch allreduce_twoshot_kernel");
 }
 
@@ -566,21 +568,15 @@ static const char* ll_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArF
 static int ll_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                      uint32_t grid) {
   const uint32_t g = L.grank, n = h->n_total;
-  LlParams p;
-  memset(&p, 0, sizeof(p));
+  LlParams p = ar_params<LlParams>(h, L, dom, f);
   p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
   for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.ll_va[(g + t) % n]);
   p.in = reinterpret_cast<const uint8_t*>(L.ll_va[g]);
-  p.dom = dom;
   p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
   p.s_max = lad.size[lad.n_sizes - 1];
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_mode = f.mode;
   p.fault_dst = (f.recv + n - g) % n;
   p.fault_arg = f.word;
-  p.rank = g;
-  p.n = n;
   p.ctas = grid;
   return launch_ladder(h, L, p, lad, allreduce_ll_launch, "launch allreduce_ll_kernel");
 }
@@ -610,20 +606,14 @@ static const char* ring_fault(const cdprobe* h, uint64_t v, const Ladder& lad, A
 static int ring_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                        uint32_t) {
   const uint32_t g = L.grank, n = h->n_total;
-  RingParams p;
-  memset(&p, 0, sizeof(p));
+  RingParams p = ar_params<RingParams>(h, L, dom, f);
   p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
   p.out = reinterpret_cast<uint8_t*>(L.ring_va[g]);
   p.next = reinterpret_cast<uint8_t*>(L.ring_va[(g + 1) % n]);
-  p.dom = dom;
   p.s_max = lad.size[lad.n_sizes - 1];
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_mode = f.mode;
   p.fault_phase = f.phase;
   p.fault_arg = f.word;
-  p.rank = g;
-  p.n = n;
   return launch_ladder(h, L, p, lad, allreduce_ring_launch, "launch allreduce_ring_kernel");
 }
 
@@ -651,18 +641,12 @@ static const char* push_fault(const cdprobe* h, uint64_t v, const Ladder& lad, A
 static int push_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                        uint32_t) {
   const uint32_t g = L.grank, n = h->n_total;
-  PushParams p;
-  memset(&p, 0, sizeof(p));
+  PushParams p = ar_params<PushParams>(h, L, dom, f);
   p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
   for (uint32_t t = 0; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.push_va[(g + t) % n]);
-  p.dom = dom;
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_word = f.word;
   p.fault_mode = f.mode;
   p.fault_dst = (f.recv + n - g) % n;
-  p.rank = g;
-  p.n = n;
   return launch_ladder(h, L, p, lad, allreduce_push_launch, "launch allreduce_push_kernel");
 }
 
@@ -684,18 +668,12 @@ static int nvls_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
                        uint32_t) {
   const uint32_t g = L.grank, li = g - h->first;
   const uint64_t s_max = lad.size[lad.n_sizes - 1];
-  NvlsParams p;
-  memset(&p, 0, sizeof(p));
+  NvlsParams p = ar_params<NvlsParams>(h, L, dom, f);
   p.mc_in = reinterpret_cast<const uint8_t*>(h->nvls.mc_va[li]);
   p.mc_out = reinterpret_cast<uint8_t*>(h->nvls.mc_va[li] + s_max);
   p.out = reinterpret_cast<uint8_t*>(h->nvls.uc_va[li] + s_max);
-  p.dom = dom;
-  p.seed = h->seed;
-  p.fault_k = g == f.rank ? f.k : kArNoFault;
   p.fault_word = f.word;
   p.fault_mode = f.mode;
-  p.rank = g;
-  p.n = h->n_total;
   return launch_ladder(h, L, p, lad, allreduce_nvls_launch, "launch allreduce_nvls_kernel");
 }
 

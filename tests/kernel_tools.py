@@ -1,6 +1,8 @@
 """What the CUDA tools report about the compiled kernels, for the tests that check them: ptxas's resource report of one
-translation unit, and one kernel's SASS in the built library.  Each skips the calling test when its tool is missing."""
+translation unit, one kernel's SASS in the built library, and the pins of every function's SASS.  Each skips the
+calling test when its tool is missing."""
 import functools
+import hashlib
 import os
 import re
 import shutil
@@ -57,3 +59,14 @@ def kernel_sass(lib, pattern):
     assert len(names) == 1, (pattern, names)
     addr, text = funcs[names[0]]
     return list(addr), list(text)
+
+
+def sass_pins(lib):
+    """{function: [instruction count, sha256 of the instructions joined by newlines]} for every function in the library
+    `lib`, as kernel_sass reads them.  A function in an anonymous namespace is keyed without the two hashes nvcc puts
+    in that namespace's name, which change with the build directory."""
+    pins = {}
+    for name, (_, text) in _sass(_tool("cuobjdump"), lib).items():
+        key = re.sub(r"_GLOBAL__N__[0-9a-f]{8}_(\w+?_cu)_[0-9a-f]{8}", r"_GLOBAL__N__\1", name)
+        pins[key] = [len(text), hashlib.sha256("\n".join(text).encode()).hexdigest()]
+    return pins
