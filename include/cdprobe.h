@@ -487,6 +487,49 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_alltoall_t;
 
+/* Copy-engine bandwidth versus transfer size per ordered pair (cdprobe_memcpy): issuer i's stream copies growing
+ * prefixes of a source slice with cudaMemcpyAsync, from target j into i's exchange area (a pull, CDPROBE_OP_READ) or
+ * from i into j's (a push, CDPROBE_OP_WRITE), and i's GPU checks every word that landed (DESIGN §5n).  Cells are
+ * row-major [issuer * CDPROBE_MAX_GPUS + target]; size k of a cell is [cell][k]. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: row r is filled in (the rows of this process's ranks) */
+  uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
+  uint32_t n_sizes;                     /* entries of size[] */
+  uint32_t op;                          /* as passed: CDPROBE_OP_READ (pull) or CDPROBE_OP_WRITE (push) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_memcpy calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint64_t area_bytes;                  /* this rank's exchange area (cdprobe_alltoall's): n x bytes_per_pair rounded
+                                           up to 2 MiB */
+  uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes copied per rep: the cdprobe_bwcurve ladder */
+  uint8_t measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];  /* 1: the cell ran */
+  int32_t status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep of some size landed a
+                                                             word other than the pattern's; CDPROBE_ERR_TIMEOUT: an
+                                                             (S, X) read of the cell passed timeout_ms (no times); else
+                                                             the status of the issuer's probe or exchange-area mapping */
+  uint32_t bad_sizes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* bit k set: a rep of size[k], warm-up included, landed a
+                                                              bad word or an (S, X) other than the pattern's */
+  float t0_ns[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];       /* ns_median of size[0] */
+  float peak_gbps[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* max over k of size[k] / ns_median[k] (bytes per ns) */
+  uint64_t half_bytes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* the smallest size[k] whose size[k] / ns_median[k]
+                                                               reaches peak / 2 (computed before peak is rounded) */
+  float ns_min[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* ns per copy over the timed reps, by
+                                                                                      CUDA events (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* element reps / 2 of the sorted
+                                                                                      reps */
+  float ns_max[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];
+  uint64_t sum[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* checksum S of the destination as
+                                                                                      the check read it, last timed rep */
+  uint64_t xr[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];     /* checksum X */
+  uint64_t bad_words[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* destination words that differ
+                                                                   from the pattern, summed over every rep of size[k],
+                                                                   warm-up included */
+  uint64_t first_bad[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* byte offset of the lowest of
+                                                                   them; UINT64_MAX when clean */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_memcpy_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -512,12 +555,12 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls, cdprobe_alltoall: diagnostics, benches, fault injection; the reference has no counterpart
- *   (it has no probe, SURVEY.md F1).
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy: diagnostics, benches, fault injection; the reference has
+ *   no counterpart (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls and cdprobe_alltoall are optional for callers: a daemon binds them with dlsym and works
- *   without.
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall and cdprobe_memcpy are optional for callers: a daemon binds them with
+ *   dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -601,6 +644,14 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              the owner stores the word xored with 1 through the multicast address, so
                                              every row fails at that word; mode 1, it skips the multicast store of the
                                              word's 8 KiB unit, so every row reads that unit as 0s; 0 disarms */
+#define CDPROBE_OPT_MEMCPY_FAULT 26u      /* tests: value = (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) |
+                                             ((k + 1) << 24) | word arms a fault in cdprobe_memcpy, in timed rep 1 of
+                                             size[k] of cell (issuer, target), in the process that hosts the issuer:
+                                             mode 0, between the copy and the checks, destination word `word` (< 2^24)
+                                             is overwritten with its pattern value xored with 1 (an 8-byte copy from
+                                             host memory); mode 1, no copy is queued, so the destination the previous
+                                             rep cleared reads as 0s.  Either fails exactly that cell and size; 0
+                                             disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -876,6 +927,37 @@ CDPROBE_API int cdprobe_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allr
  * CDPROBE_OPT_ALLREDUCE_NVLS_FAULT whose mode is above 1, that sets any of bits 32 to 47, whose k is >= n_sizes or
  * whose word is >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
+/* Copy-engine bandwidth versus transfer size of every cell whose issuer is local to this process, checked word for
+ * word: for each size of the cdprobe_bwcurve ladder, one untimed warm-up rep, then `reps` timed reps, each one
+ * cudaMemcpyAsync of the first size bytes of a source slice (written only at open, so no run is needed first) on the
+ * issuer's stream.  op = CDPROBE_OP_READ pulls: the slice issuer i reads from target j, from j's allocation into block j
+ * of i's exchange area.  op = CDPROBE_OP_WRITE pushes: the slice j reads from i, from i's own allocation into block i
+ * of j's exchange area.  The exchange area is cdprobe_alltoall's (n x bytes_per_pair per rank, created on the first
+ * call of either, collectively, and kept until close; cdprobe_alltoall salts and checks every word it uses, so the two
+ * may share it).  The timed part of a rep is queued whole before any of it may start: a stream wait
+ * (cuStreamWaitValue64) on a host-mapped ticket word, an event, the copy, an event.  The host then releases the ticket,
+ * so the events bracket the copy alone, without the host's enqueue time; ns per rep is their cudaEventElapsedTime,
+ * which resolves about 0.5 us, so t0_ns is indicative only.  Once the copy has completed, the untimed checks are queued
+ * on the issuer's GPU through its mapping: cdprobe_diagnose's comparison of every destination word with the pattern,
+ * cdprobe_bwcurve's (S, X) read of the destination on the issuer's grid and CDPROBE_OPT_PATH data path, and a memset
+ * of the destination to 0, so that a copy that does not land in a later rep reads as 0s.  The local ranks of one process are released together; across processes only the
+ * domain barrier before each size aligns them.  Every rep, warm-up included, is checked (bad_sizes, bad_words,
+ * first_bad, CDPROBE_ERR_INTEGRITY).  The cells run in the tournament's rounds (cdprobe_plan partner table), both ranks
+ * of a pair at once, then with a loop-back slice (n == 1 or CDPROBE_FLAG_LOCAL_DIAG) a last round copies the diagonal;
+ * a domain barrier opens every round and every size.  A cell runs when the issuer maps the target's probe allocation
+ * and exchange area; otherwise nothing is copied (measured = 0, the mapping status).  Nothing is written but the
+ * cells' blocks of the exchange area and the issuers' scratch buffers, which grow to hold a diagnosis of
+ * bytes_per_pair.  An (S, X) read that passes timeout_ms makes its cell CDPROBE_ERR_TIMEOUT and the handle stays
+ * usable; a copy whose closing event has not completed timeout_ms after its release returns CDPROBE_ERR_TIMEOUT and
+ * leaves the handle sticky (a copy cannot be aborted).  Collective when world_size > 1: every process calls it with the
+ * same op and reps, and fills the rows of its own ranks (row_mask).  Touches no result, pattern, source buffer, landing
+ * slot, Ctrl word, run_seq, warm-up state or other measurement's state.  *out carries abi, n, reps and op whatever the
+ * return code.  CDPROBE_ERR_ARG: null argument, an op other than CDPROBE_OP_READ or CDPROBE_OP_WRITE, reps > 64,
+ * bytes_per_pair > 32 GiB, arguments that differ between processes, or an armed CDPROBE_OPT_MEMCPY_FAULT that names no
+ * cell of the domain, a k >= n_sizes or a word >= size[k] / 8, or has a mode above 1; CDPROBE_ERR_TIMEOUT: a copy did
+ * not complete (sticky); CDPROBE_ERR_UNSUPPORTED: the driver has no cuStreamWaitValue64; CDPROBE_ERR_CUDA: it
+ * refused one (sticky); CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

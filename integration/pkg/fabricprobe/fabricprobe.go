@@ -36,6 +36,7 @@ typedef int (*at_fn)(cdprobe_t*, uint32_t, uint32_t, uint32_t, cdprobe_atomics_t
 typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
 typedef int (*ar_fn)(cdprobe_t*, uint32_t, cdprobe_allreduce_t*);
 typedef int (*a2a_fn)(cdprobe_t*, uint32_t, cdprobe_alltoall_t*);
+typedef int (*mc_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_memcpy_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -52,6 +53,7 @@ static ar_fn cdp_arll;    // optional: absent from libraries that predate cdprob
 static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprobe_allreduce_ring
 static ar_fn cdp_arpush;  // optional: absent from libraries that predate cdprobe_allreduce_push
 static ar_fn cdp_arnvls;  // optional: absent from libraries that predate cdprobe_allreduce_nvls
+static mc_fn cdp_mc;      // optional: absent from libraries that predate cdprobe_memcpy
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -75,6 +77,7 @@ static int cdp_load(const char* path) {
   cdp_arring = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_ring");
   cdp_arpush = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_push");
   cdp_arnvls = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_nvls");
+  cdp_mc = (mc_fn)dlsym(cdp_dl, "cdprobe_memcpy");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -122,6 +125,10 @@ static int cdp_call_allreduce_push(cdprobe_t* h, uint32_t reps, cdprobe_allreduc
 static int cdp_has_allreduce_nvls(void) { return cdp_arnvls != NULL; }
 static int cdp_call_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* ar) {
   return cdp_arnvls(h, reps, ar);
+}
+static int cdp_has_memcpy(void) { return cdp_mc != NULL; }
+static int cdp_call_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* mc) {
+  return cdp_mc(h, op, reps, mc);
 }
 */
 import "C"
@@ -339,6 +346,28 @@ type AllToAll struct {
 	BadSizes               [][]uint32  // [sender][receiver]: bit k: Sizes[k] delivered a bad word
 	BadWords, FirstBad     [][][]uint64 // [sender][receiver][size]: the word check; FirstBad is MaxUint64 when clean
 	Sum, Xr                [][][]uint64 // [sender][receiver][size]: (S, X) of the block in the last timed rep
+	Ms                     float64
+}
+
+// Memcpy is the copy-engine bandwidth curve of the local rows (cdprobe_memcpy_t), pulled (Op CDPROBE_OP_READ) or pushed
+// (CDPROBE_OP_WRITE).  Cells are [issuer * N + target], as in BwCurve; the per-size slices hold one entry per Sizes
+// element.
+type Memcpy struct {
+	N                      int
+	RowMask                uint32      // rows of this process's ranks
+	Reps                   int         // timed reps per size, as applied
+	Op                     uint32      // CDPROBE_OP_READ (pull) or CDPROBE_OP_WRITE (push)
+	CallSeq                uint64      // 1-based count of Memcpy calls on this handle, equal in every process
+	AreaBytes              uint64      // this rank's exchange area, where the copies land
+	Sizes                  []uint64    // bytes copied per rep
+	Measured               []bool
+	Status                 []int32     // 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else the mapping's status
+	BadSizes               []uint32    // bit k: a rep of Sizes[k] landed a bad word or checksum
+	T0Ns, PeakGBps         []float32   // median ns of the smallest size; max over sizes of size / median ns
+	HalfBytes              []uint64    // the smallest size reaching half the peak
+	NsMin, NsMedian, NsMax [][]float32 // [cell][size]: ns per copy over the timed reps, by CUDA events
+	Sum, Xr                [][]uint64  // [cell][size]: (S, X) of the destination in the last timed rep
+	BadWords, FirstBad     [][]uint64  // [cell][size]: the word check over every rep; FirstBad is MaxUint64 when clean
 	Ms                     float64
 }
 
@@ -911,6 +940,63 @@ func (p *Probe) AllToAll(reps int) (AllToAll, error) {
 				out.FirstBad[r][d][s] = uint64(aa.first_bad[c][s])
 				out.Sum[r][d][s] = uint64(aa.sum[c][s])
 				out.Xr[r][d][s] = uint64(aa.xr[c][s])
+			}
+		}
+	}
+	return out, nil
+}
+
+// Memcpy runs the copy-engine bandwidth curve: cudaMemcpyAsync of each size of the bwcurve ladder per cell, pulled from
+// the target into the issuer's exchange area (op CDPROBE_OP_READ) or pushed into the target's (CDPROBE_OP_WRITE), timed
+// by CUDA events, every landed word checked (reps 0: 8 timed reps).  Collective when the domain spans processes.
+// ErrUnsupported when the library predates cdprobe_memcpy.
+func (p *Probe) Memcpy(op uint32, reps int) (Memcpy, error) {
+	if C.cdp_has_memcpy() == 0 {
+		return Memcpy{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_memcpy", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	mc := new(C.cdprobe_memcpy_t)
+	rc := C.cdp_call_memcpy(p.h, C.uint32_t(op), C.uint32_t(reps), mc)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_memcpy: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		if rc == C.CDPROBE_ERR_STATE {
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		}
+		return Memcpy{}, err
+	}
+	n, ns := int(mc.n), int(mc.n_sizes)
+	out := Memcpy{N: n, RowMask: uint32(mc.row_mask), Reps: int(mc.reps), Op: uint32(mc.op),
+		CallSeq: uint64(mc.call_seq), AreaBytes: uint64(mc.area_bytes), Ms: float64(mc.ms)}
+	out.Sizes = make([]uint64, ns)
+	for s := 0; s < ns; s++ {
+		out.Sizes[s] = uint64(mc.size[s])
+	}
+	out.Measured, out.Status, out.BadSizes = make([]bool, n*n), make([]int32, n*n), make([]uint32, n*n)
+	out.T0Ns, out.PeakGBps, out.HalfBytes = make([]float32, n*n), make([]float32, n*n), make([]uint64, n*n)
+	out.NsMin, out.NsMedian, out.NsMax = make([][]float32, n*n), make([][]float32, n*n), make([][]float32, n*n)
+	out.Sum, out.Xr = make([][]uint64, n*n), make([][]uint64, n*n)
+	out.BadWords, out.FirstBad = make([][]uint64, n*n), make([][]uint64, n*n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < n; j++ {
+			k, c := i*C.CDPROBE_MAX_GPUS+j, i*n+j
+			out.Measured[c] = mc.measured[k] != 0
+			out.Status[c] = int32(mc.status[k])
+			out.BadSizes[c] = uint32(mc.bad_sizes[k])
+			out.T0Ns[c] = float32(mc.t0_ns[k])
+			out.PeakGBps[c] = float32(mc.peak_gbps[k])
+			out.HalfBytes[c] = uint64(mc.half_bytes[k])
+			out.NsMin[c], out.NsMedian[c], out.NsMax[c] = make([]float32, ns), make([]float32, ns), make([]float32, ns)
+			out.Sum[c], out.Xr[c] = make([]uint64, ns), make([]uint64, ns)
+			out.BadWords[c], out.FirstBad[c] = make([]uint64, ns), make([]uint64, ns)
+			for s := 0; s < ns; s++ {
+				out.NsMin[c][s] = float32(mc.ns_min[k][s])
+				out.NsMedian[c][s] = float32(mc.ns_median[k][s])
+				out.NsMax[c][s] = float32(mc.ns_max[k][s])
+				out.Sum[c][s] = uint64(mc.sum[k][s])
+				out.Xr[c][s] = uint64(mc.xr[k][s])
+				out.BadWords[c][s] = uint64(mc.bad_words[k][s])
+				out.FirstBad[c][s] = uint64(mc.first_bad[k][s])
 			}
 		}
 	}

@@ -169,6 +169,25 @@ type AllToAll struct {
 	Ms                     float64
 }
 
+type Memcpy struct {
+	N                      int
+	RowMask                uint32
+	Reps                   int
+	Op                     uint32
+	CallSeq                uint64
+	AreaBytes              uint64
+	Sizes                  []uint64
+	Measured               []bool
+	Status                 []int32
+	BadSizes               []uint32
+	T0Ns, PeakGBps         []float32
+	HalfBytes              []uint64
+	NsMin, NsMedian, NsMax [][]float32
+	Sum, Xr                [][]uint64
+	BadWords, FirstBad     [][]uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
@@ -187,4 +206,5 @@ func (*Probe) AllReduceRing(int) (AllReduce, error) { return AllReduce{}, ErrUns
 func (*Probe) AllReducePush(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllReduceNVLS(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
+func (*Probe) Memcpy(uint32, int) (Memcpy, error) { return Memcpy{}, ErrUnsupported }
 func (*Probe) Close() {}

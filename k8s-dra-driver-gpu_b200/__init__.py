@@ -21,6 +21,7 @@ from .fabricprobe import (  # noqa: F401
     Diagnosis,
     ErrUnsupported,
     Latency,
+    Memcpy,
     PingPong,
     Probe,
     ProbeError,
@@ -31,4 +32,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "AllToAll", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "AllToAll", "Memcpy", "Open", "gate", "plan", "topology"]

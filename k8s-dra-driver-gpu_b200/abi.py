@@ -41,6 +41,7 @@ OPT_ALLREDUCE_LL_FAULT = 22
 OPT_ALLREDUCE_RING_FAULT = 23
 OPT_ALLREDUCE_PUSH_FAULT = 24
 OPT_ALLREDUCE_NVLS_FAULT = 25
+OPT_MEMCPY_FAULT = 26
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -64,6 +65,7 @@ ALLREDUCE_PATH_LL = 3  # cdprobe_allreduce_t.path of cdprobe_allreduce_ll
 ALLREDUCE_PATH_RING = 4  # cdprobe_allreduce_t.path of cdprobe_allreduce_ring
 ALLREDUCE_PATH_NVLS = 5  # cdprobe_allreduce_t.path of cdprobe_allreduce_nvls
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
+MEMCPY_DEFAULT_REPS, MEMCPY_MAX_REPS = 8, 64
 
 _N2 = MAX_GPUS * MAX_GPUS
 
@@ -395,6 +397,43 @@ class AllToAllT(C.Structure):
     ]
 
 
+class MemcpyT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("n_sizes", C.c_uint32),
+        ("op", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("area_bytes", C.c_uint64),
+        ("size", C.c_uint64 * BWCURVE_MAX_SIZES),
+        ("measured", C.c_uint8 * _N2),
+        ("status", C.c_int32 * _N2),
+        ("bad_sizes", C.c_uint32 * _N2),
+        ("t0_ns", C.c_float * _N2),
+        ("peak_gbps", C.c_float * _N2),
+        ("half_bytes", C.c_uint64 * _N2),
+        ("ns_min", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("ns_median", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("ns_max", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("sum", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("xr", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("bad_words", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("first_bad", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("ms", C.c_double),
+    ]
+
+
+def memcpy_fault(issuer: int, target: int, k: int, word: int, mode: int = 0) -> int:
+    """The CDPROBE_OPT_MEMCPY_FAULT value for timed rep 1 of size[k] of cell (issuer, target) of cdprobe_memcpy: mode 0,
+    destination word `word` is xored with 1 between the copy and the check; mode 1, no copy is queued, so the cleared
+    destination reads as 0s.  Fields that do not fit are refused here."""
+    if mode not in (0, 1) or not (0 <= issuer < 255 and 0 <= target < 255 and 0 <= k < 255 and 0 <= word < 1 << 24):
+        raise ValueError("memcpy_fault: mode 0 or 1, ranks and k below 255, word below 2^24")
+    return (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | ((k + 1) << 24) | word
+
+
 def alltoall_fault(sender: int, receiver: int, k: int, word: int) -> int:
     """The CDPROBE_OPT_ALLTOALL_FAULT value that makes timed rep 1 of size[k] store word `word` of block
     (sender -> receiver) xored with 1."""
@@ -491,6 +530,7 @@ SYMBOLS = {
     "cdprobe_allreduce_push": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_allreduce_nvls": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
+    "cdprobe_memcpy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(MemcpyT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

@@ -693,8 +693,11 @@ static void destroy(cdprobe* h) {
     if (L.scratch) cudaFree(L.scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
+    for (cudaEvent_t ev : L.memcpy_ev)
+      if (ev) cudaEventDestroy(ev);
     if (L.stream) cudaStreamDestroy(L.stream);
   }
+  if (h->memcpy_host) cudaFreeHost(h->memcpy_host);
   h->rdv.close();
   delete h;
 }
@@ -1290,6 +1293,9 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return CDPROBE_OK;
     case CDPROBE_OPT_ALLREDUCE_NVLS_FAULT:  // checked against the ladder and the chunks by cdprobe_allreduce_nvls
       h->nvls_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_MEMCPY_FAULT:  // checked against the domain and the size ladder by cdprobe_memcpy
+      h->memcpy_fault = value;
       return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;

@@ -12,9 +12,12 @@
 #include "plan.h"
 #include "probe_types.h"
 #include "rendezvous.h"
+#include "timed_rep.cuh"
 #include "vmm.h"
 
 namespace cdp {
+
+struct MemcpyHost;
 
 inline thread_local std::string g_last_error;
 
@@ -57,6 +60,7 @@ struct LocalRank {
   uint32_t peer_mask = 0;
   void* scratch = nullptr;  // device output of the on-demand measurements (measure.cc), grown on demand
   size_t scratch_bytes = 0;
+  cudaEvent_t memcpy_ev[2 * kRepSlots] = {};  // cdprobe_memcpy, made on first use: rep r's copy is [2r] to [2r + 1]
 };
 
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
@@ -159,6 +163,11 @@ struct cdprobe {
   uint64_t push_fault = 0;    // CDPROBE_OPT_ALLREDUCE_PUSH_FAULT value, 0: disarmed
   uint64_t nvls_calls = 0;    // cdprobe_allreduce_nvls calls that ran (call_seq of the last one)
   uint64_t nvls_fault = 0;    // CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value, 0: disarmed
+  uint64_t memcpy_calls = 0;  // cdprobe_memcpy calls that ran (call_seq of the last one)
+  uint64_t memcpy_fault = 0;  // CDPROBE_OPT_MEMCPY_FAULT value, 0: disarmed
+  cdp::MemcpyHost* memcpy_host = nullptr;  // cdprobe_memcpy's pinned host block (measure.cc), made on first use:
+                                          // the ticket its streams wait on and what its checks leave
+  uint64_t memcpy_tickets = 0;        // tickets handed out so far
   double open_ms = 0, fill_ms = 0;
 };
 

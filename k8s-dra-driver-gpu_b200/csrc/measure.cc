@@ -1,8 +1,10 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
 // cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll,
-// cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_allreduce_nvls and cdprobe_alltoall.  Each runs on the local
-// ranks' own streams, between probe runs, and has its results on the host before it returns.
+// cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_allreduce_nvls, cdprobe_alltoall and cdprobe_memcpy.  Each
+// runs on the local ranks' own streams, between probe runs, and has its results on the host before it returns.
 #include <string.h>
+
+#include <stddef.h>
 
 #include <algorithm>
 #include <array>
@@ -296,27 +298,19 @@ static int collect_reps(cdprobe* h, const RepCells* cells, uint32_t reps, uint32
   return CDPROBE_OK;
 }
 
-// Fills the times of entry idx of a cdprobe_bwcurve_t (a cell), a cdprobe_allreduce_t (a row) or a cdprobe_alltoall_t
-// (a row) from the rep records bwcurve_kernel, allreduce_kernel or alltoall_kernel left in `s`: per size, ns of the
-// timed reps, and the model-free summary of the medians, whose rates are scale x size[k] / ns_median[k].  An entry
-// whose kernel was aborted at the deadline has no times and is CDPROBE_ERR_TIMEOUT; returns whether it has times.
+// Fills the times of entry idx of a ladder measurement from ns[k][r], ns of timed rep r + 1 of size k: per size, the
+// minimum, median and maximum, and the model-free summary of the medians, whose rates are
+// scale x size[k] / ns_median[k].  Sorts ns.
 template <typename Out>
-static bool bw_times(const BwScratch& s, const uint64_t* size, uint32_t n_sizes, uint32_t reps, double scale,
-                     uint32_t idx, Out* out) {
-  out->measured[idx] = 1;
-  if (s.abort_flag != 0) {
-    out->status[idx] = CDPROBE_ERR_TIMEOUT;
-    return false;
-  }
+static void ladder_times(float (*ns)[kMaxTimedReps], const uint64_t* size, uint32_t n_sizes, uint32_t reps,
+                         double scale, uint32_t idx, Out* out) {
   double rate[kBwMaxSizes], peak = 0.0;
   for (uint32_t k = 0; k < n_sizes; ++k) {
-    float ns[kMaxTimedReps];
-    for (uint32_t r = 1; r <= reps; ++r) ns[r - 1] = (float)(s.rep[k][r].t_end - s.t_rel[k][r]);
-    std::sort(ns, ns + reps);
-    out->ns_min[idx][k] = ns[0];
-    out->ns_median[idx][k] = ns[reps / 2];
-    out->ns_max[idx][k] = ns[reps - 1];
-    rate[k] = ns[reps / 2] > 0.f ? scale * (double)size[k] / (double)ns[reps / 2] : 0.0;
+    std::sort(ns[k], ns[k] + reps);
+    out->ns_min[idx][k] = ns[k][0];
+    out->ns_median[idx][k] = ns[k][reps / 2];
+    out->ns_max[idx][k] = ns[k][reps - 1];
+    rate[k] = ns[k][reps / 2] > 0.f ? scale * (double)size[k] / (double)ns[k][reps / 2] : 0.0;
     peak = std::max(peak, rate[k]);
   }
   out->t0_ns[idx] = out->ns_median[idx][0];
@@ -328,6 +322,23 @@ static bool bw_times(const BwScratch& s, const uint64_t* size, uint32_t n_sizes,
     }
   }
   out->status[idx] = 0;
+}
+
+// Fills the times of entry idx of a cdprobe_bwcurve_t (a cell), a cdprobe_allreduce_t (a row) or a cdprobe_alltoall_t
+// (a row) from the rep records bwcurve_kernel, allreduce_kernel or alltoall_kernel left in `s` (ladder_times).  An
+// entry whose kernel was aborted at the deadline has no times and is CDPROBE_ERR_TIMEOUT; returns whether it has times.
+template <typename Out>
+static bool bw_times(const BwScratch& s, const uint64_t* size, uint32_t n_sizes, uint32_t reps, double scale,
+                     uint32_t idx, Out* out) {
+  out->measured[idx] = 1;
+  if (s.abort_flag != 0) {
+    out->status[idx] = CDPROBE_ERR_TIMEOUT;
+    return false;
+  }
+  float ns[kBwMaxSizes][kMaxTimedReps];
+  for (uint32_t k = 0; k < n_sizes; ++k)
+    for (uint32_t r = 1; r <= reps; ++r) ns[k][r - 1] = (float)(s.rep[k][r].t_end - s.t_rel[k][r]);
+  ladder_times(ns, size, n_sizes, reps, scale, idx, out);
   return true;
 }
 
@@ -362,9 +373,16 @@ struct Ladder {
 // out->path of a ladder measurement that runs on the handle's data path (CDPROBE_OPT_PATH).
 constexpr uint32_t kHandlePath = UINT32_MAX;
 
-// The opening of the ladder measurements (bwcurve, the all-reduces, alltoall): *out cleared and stamped with reps (0:
-// default_reps); once the handle is known, n and the data path (`path`, or the handle's) before the handle is checked;
-// then the size ladder by `rule` (bwcurve_ladder; allreduce_ll: ll_ladder) and the verdict on the arguments.
+// out->path of a ladder measurement that reports one; cdprobe_memcpy_t has none (its copies use no data path).
+template <typename Out>
+static void put_path(Out* out, uint32_t path) {
+  out->path = path;
+}
+static void put_path(cdprobe_memcpy_t*, uint32_t) {}
+
+// The opening of the ladder measurements (bwcurve, the all-reduces, alltoall, memcpy): *out cleared and stamped with
+// reps (0: default_reps); once the handle is known, n and the data path (`path`, or the handle's) before the handle is
+// checked; then the size ladder by `rule` (bwcurve_ladder; allreduce_ll: ll_ladder) and the verdict on the arguments.
 template <typename Out>
 static int open_ladder(cdprobe* h, Out* out, uint32_t reps, uint32_t default_reps, Ladder* lad,
                        uint32_t path = kHandlePath, uint32_t (*rule)(uint64_t, uint64_t*) = bwcurve_ladder) {
@@ -373,7 +391,7 @@ static int open_ladder(cdprobe* h, Out* out, uint32_t reps, uint32_t default_rep
   if (h == nullptr) return CDPROBE_ERR_ARG;
   lad->t_begin = now_ms();
   out->n = h->n_total;
-  out->path = path == kHandlePath ? h->path : path;
+  put_path(out, path == kHandlePath ? h->path : path);
   lad->reps = out->reps;
   if (const int rc = require_usable(h); rc != CDPROBE_OK) return rc;
   lad->n_sizes = rule(h->plan.bpp, lad->size);
@@ -802,6 +820,180 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
     for (uint32_t li = 0; li < h->n_local; ++li) m->stale |= out->status[h->lr[li].grank] == CDPROBE_ERR_TIMEOUT;
   out->ms = now_ms() - lad.t_begin;
   return CDPROBE_OK;
+}
+
+constexpr uint32_t kMemcpyDefaultReps = 8;
+
+// cdprobe_memcpy's armed fault once the call has accepted it: timed rep 1 of size k of cell (issuer, target) flips
+// destination word `word` (mode 0) or queues no copy (mode 1).  issuer kMaxRanks: none.
+struct MemcpyFault {
+  uint32_t issuer = kMaxRanks, target = 0, k = 0, mode = 0;
+  uint64_t word = 0;
+};
+
+// What the checks of one rep of cdprobe_memcpy leave for the host, copied back on the issuer's stream behind them: the
+// head of the diagnosis (bad_words, bad_granules, first_bad_n of its DiagOut) and the (S, X) read of bwcurve_kernel
+// (its abort word and the Acc of its one rep).
+struct MemcpyRepOut {
+  unsigned long long diag[3];
+  unsigned int abort_flag;
+  Acc acc;
+};
+static_assert(offsetof(DiagOut, bad_words) == 0 && offsetof(DiagOut, first_bad_n) == 16, "the diagnosis head");
+static_assert(offsetof(BwScratch, abort_flag) == 0, "the (S, X) read's abort word");
+
+// cdprobe_memcpy's pinned, mapped and portable host block, made on first use and kept until close: the ticket every
+// local stream waits on (cuStreamWaitValue64, through its UVA address), the word the armed mode-0 fault stores per
+// local rank, and what each rep's checks left, per local rank and rep.
+struct MemcpyHost {
+  uint64_t ticket;
+  uint64_t flip[kMaxRanks];
+  MemcpyRepOut rep[kMaxRanks][kRepSlots];
+};
+
+// Where cdprobe_memcpy keeps its device state in a local rank's scratch: the BwScratch of the (S, X) read at 0, the
+// diagnosis of a destination of up to bytes_per_pair at diag_off, the granule table of expected_sums at table_off.
+struct MemcpyScratch {
+  size_t diag_off, table_off, bytes;
+  explicit MemcpyScratch(uint64_t bpp) {
+    diag_off = (sizeof(BwScratch) + 255) / 256 * 256;
+    table_off = diag_off + (diag_scratch_bytes(bpp) + 255) / 256 * 256;
+    bytes = table_off + 16 * (bpp / kGranuleBytes);
+  }
+};
+
+// The host block, the driver's stream wait and every local rank's event pool, made on first use.
+static int memcpy_setup(cdprobe* h) {
+  std::string err;
+  if (h->drv.load_stream_wait(&err) != cudaSuccess) {
+    set_err("cdprobe_memcpy: " + err);
+    return CDPROBE_ERR_UNSUPPORTED;
+  }
+  CDP_RT(cudaSetDevice(h->lr[0].ordinal));
+  if (h->memcpy_host == nullptr) {
+    void* p = nullptr;
+    CDP_RT(cudaHostAlloc(&p, sizeof(MemcpyHost), cudaHostAllocPortable | cudaHostAllocMapped));
+    memset(p, 0, sizeof(MemcpyHost));
+    h->memcpy_host = static_cast<MemcpyHost*>(p);
+    __atomic_store_n(&h->memcpy_host->ticket, h->memcpy_tickets, __ATOMIC_RELEASE);
+  }
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    CDP_RT(cudaSetDevice(L.ordinal));
+    for (cudaEvent_t& ev : L.memcpy_ev)
+      if (ev == nullptr) CDP_RT(cudaEventCreate(&ev));
+  }
+  return CDPROBE_OK;
+}
+
+// The timed part of rep `rep` of cdprobe_memcpy's cell (L.grank, j), queued on L's stream: the wait for the rep's
+// ticket, event A, the copy (none when `drop`), event B.  A failure of the stream wait itself is cudaErrorUnknown with
+// the driver's result in *cu.
+static cudaError_t memcpy_timed(cdprobe* h, LocalRank& L, uint32_t j, uint32_t op, uint64_t ticket, uint64_t bytes,
+                                uint32_t rep, bool drop, CUresult* cu) {
+  const MemcpyCell c = memcpy_cell(h->plan, op, L.grank, j);
+  cudaError_t e = cudaSetDevice(L.ordinal);
+  if (e != cudaSuccess) return e;
+  *cu = h->drv.StreamWaitValue64(L.stream, reinterpret_cast<CUdeviceptr>(&h->memcpy_host->ticket), ticket,
+                                 CU_STREAM_WAIT_VALUE_GEQ);
+  if (*cu != CUDA_SUCCESS) return cudaErrorUnknown;
+  e = cudaEventRecord(L.memcpy_ev[2 * rep], L.stream);
+  if (e == cudaSuccess && !drop)
+    e = cudaMemcpyAsync(reinterpret_cast<void*>(L.area_va[c.dst_rank] + c.dst_off),
+                        reinterpret_cast<const void*>(L.va[c.src_rank] + c.src_off), bytes, cudaMemcpyDeviceToDevice,
+                        L.stream);
+  if (e == cudaSuccess) e = cudaEventRecord(L.memcpy_ev[2 * rep + 1], L.stream);
+  return e;
+}
+
+// The untimed checks of rep `rep` of the cell, queued on L's stream behind its event B: the armed mode-0 fault's store
+// (`flip`: word flip_word), the diagnosis of every destination word against the source slice's pattern (diag_launch),
+// the (S, X) read of the destination (bwcurve_kernel, one rep of one size), the clearing of the destination to 0, and
+// the copies of what the checks left into rep's slot of the host block.
+static cudaError_t memcpy_check(cdprobe* h, LocalRank& L, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes,
+                                uint32_t rep, bool flip, uint64_t flip_word) {
+  const Plan& pl = h->plan;
+  const MemcpyCell c = memcpy_cell(pl, op, L.grank, j);
+  const MemcpyScratch ms(pl.bpp);
+  MemcpyHost* const host = h->memcpy_host;
+  MemcpyRepOut* const got = &host->rep[li][rep];
+  uint8_t* const dst = reinterpret_cast<uint8_t*>(L.area_va[c.dst_rank] + c.dst_off);
+  uint8_t* const scratch = static_cast<uint8_t*>(L.scratch);
+  cudaStream_t s = L.stream;
+  cudaError_t e = cudaSetDevice(L.ordinal);
+  if (e == cudaSuccess && flip) {
+    host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + flip_word) ^ 1ull;
+    e = cudaMemcpyAsync(dst + 8 * flip_word, &host->flip[li], 8, cudaMemcpyHostToDevice, s);
+  }
+  if (e == cudaSuccess)
+    e = (cudaError_t)diag_launch(dst, diag_read_spec(h->seed, h->n_total, c.src_rank, c.first_word, bytes / 8,
+                                                     pl.src_bytes / 8),
+                                 scratch + ms.diag_off, L.sm_count, s);
+  if (e == cudaSuccess) e = cudaMemsetAsync(scratch, 0, sizeof(BwScratch), s);
+  if (e == cudaSuccess) {
+    BwCurveParams p;
+    memset(&p, 0, sizeof(p));
+    p.region = dst;
+    p.scratch = reinterpret_cast<BwScratch*>(scratch);
+    p.size[0] = bytes;
+    p.timeout_ns = timeout_ns(h);
+    p.n_sizes = 1;
+    p.path = h->path;
+    e = (cudaError_t)bwcurve_launch(p, L.ctas, launch_cooperatively(h, L), s);
+  }
+  if (e == cudaSuccess) e = cudaMemsetAsync(dst, 0, bytes, s);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(got->diag, scratch + ms.diag_off, sizeof(got->diag), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(&got->abort_flag, scratch, sizeof(got->abort_flag), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(&got->acc, scratch + offsetof(BwScratch, rep), sizeof(got->acc), cudaMemcpyDeviceToHost, s);
+  return e;
+}
+
+// Rep `rep` of size k of cdprobe_memcpy on every local rank with a cell in this round (target[li] >= 0).  The timed
+// part of every rank's rep is queued (memcpy_timed) before the host releases the rep's ticket, so the events bracket
+// the copy alone, without the host's enqueue time; the ticket is released even when queuing fails, so no stream is
+// left waiting.  Then the host waits, polling, until every copy's event B has completed, and only then queues the
+// checks (memcpy_check): launching a kernel may have to load it, which must not wait behind a stream that waits on
+// the host, and no host submission overlaps a timed copy.  A copy cannot be aborted: one whose event B has not
+// completed timeout_ms after the release returns CDPROBE_ERR_TIMEOUT and makes the handle sticky.
+static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladder& lad, uint32_t k, uint32_t rep,
+                      const MemcpyFault& f) {
+  const uint64_t ticket = ++h->memcpy_tickets, bytes = lad.size[k];
+  auto armed = [&](uint32_t li) {
+    return rep == 1 && k == f.k && h->lr[li].grank == f.issuer && (uint32_t)target[li] == f.target;
+  };
+  cudaError_t e = cudaSuccess;
+  CUresult cu = CUDA_SUCCESS;
+  for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
+    if (target[li] >= 0)
+      e = memcpy_timed(h, h->lr[li], (uint32_t)target[li], op, ticket, bytes, rep, armed(li) && f.mode == 1, &cu);
+  __atomic_store_n(&h->memcpy_host->ticket, ticket, __ATOMIC_RELEASE);
+  if (cu != CUDA_SUCCESS) {
+    h->sticky = true;
+    set_err("cdprobe_memcpy: cuStreamWaitValue64: " + h->drv.error_name(cu));
+    return CDPROBE_ERR_CUDA;
+  }
+  if (e != cudaSuccess) return fail_sticky(h, "cdprobe_memcpy: queue a rep", e);
+  const double deadline = now_ms() + h->cfg.timeout_ms;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if (target[li] < 0) continue;
+    LocalRank& L = h->lr[li];
+    CDP_RT(cudaSetDevice(L.ordinal));
+    while ((e = cudaEventQuery(L.memcpy_ev[2 * rep + 1])) != cudaSuccess) {
+      if (e != cudaErrorNotReady) return fail_sticky(h, "cdprobe_memcpy: wait for a copy", e);
+      if (now_ms() > deadline) {
+        h->sticky = true;
+        set_err("cdprobe_memcpy: a copy did not complete within timeout_ms of its release");
+        return CDPROBE_ERR_TIMEOUT;
+      }
+    }
+  }
+  for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
+    if (target[li] >= 0)
+      e = memcpy_check(h, h->lr[li], li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.word);
+  return e != cudaSuccess ? fail_sticky(h, "cdprobe_memcpy: queue the checks", e) : CDPROBE_OK;
 }
 
 }  // namespace cdp
@@ -1370,6 +1562,145 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
         if (s.bad_words[i][k] != 0) out->bad_sizes[cell] |= 1u << k;
       }
       out->cell_status[cell] = out->bad_sizes[cell] ? CDPROBE_ERR_INTEGRITY : 0;
+    }
+  }
+  out->ms = cdp::now_ms() - lad.t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* out) {
+  cdp::Ladder lad;
+  const int opened = cdp::open_ladder(h, out, reps, cdp::kMemcpyDefaultReps, &lad);
+  if (out != nullptr) out->op = op;
+  if (opened != CDPROBE_OK) return opened;
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
+  //    every process refuses or runs together over the same rounds
+  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad.bad.empty())
+    lad.bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
+  cdp::MemcpyFault f;
+  if (h->memcpy_fault != 0 && lad.bad.empty()) {
+    const uint64_t v = h->memcpy_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu,
+                   fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+    if (mode > 1 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || fk == 0 ||
+        fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+      lad.bad = "the armed memcpy fault names no cell, size or word of this call, or has a mode above 1";
+    else
+      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, (uint32_t)fk - 1, (uint32_t)mode, word};
+  }
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::agree(h, "cdprobe_memcpy", lad.bad, h->memcpy_calls + 1, {lad.reps, op, 0u}, st);
+      rc != CDPROBE_OK)
+    return rc;
+  // 2. the exchange area (cdprobe_alltoall's), built once, by every process in the same call
+  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++h->memcpy_calls;
+  out->area_bytes = h->area.bytes;
+  cdp::put_ladder(h, lad, out);
+
+  // 3. which cells run: the issuer maps the target's probe allocation and exchange area (cdprobe_alltoall's rule);
+  //    whether any cell of the domain runs, from the status every process shares
+  bool any = false;
+  for (uint32_t s = 0; s < n; ++s)
+    for (uint32_t d = 0; d < n; ++d) any |= (s != d || pl.diag) && st[s][d] == 0 && h->area.status[s][d] == 0;
+  bool runs[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const cdp::LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    for (uint32_t j = 0; j < n; ++j) {
+      if (!cdp::live_cell(h, li, j, out->status)) continue;
+      const int32_t a = h->area.status[g][j] == 0 && !L.area_mapped[j] ? cdp::kStatusUnmapped : h->area.status[g][j];
+      if (a != 0) out->status[g * CDPROBE_MAX_GPUS + j] = a;
+      runs[li][j] = a == 0;
+    }
+  }
+  if (!any) {  // e.g. MIG instances: nothing to copy anywhere, so nothing is queued in any process
+    out->ms = cdp::now_ms() - lad.t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 4. the host block, the stream wait and the events; scratch for the checks and one cell's granule table, grown on
+  //    every local rank before anything is queued; the (S, X) each size of each cell must land, from the pattern
+  //    definition: the per-granule sums of the source slice on the issuer's GPU, folded into every prefix on the host
+  if (const int rc = cdp::memcpy_setup(h); rc != CDPROBE_OK) return rc;
+  const cdp::MemcpyScratch ms(pl.bpp);
+  if (const int rc = cdp::ensure_scratch_all(h, ms.bytes); rc != CDPROBE_OK) return rc;
+  std::vector<uint64_t> want((size_t)cdp::kMaxRanks * cdp::kMaxRanks * cdp::kBwMaxSizes * 2);
+  auto want_of = [&](uint32_t li, uint32_t j) {
+    return reinterpret_cast<uint64_t(*)[2]>(want.data() + ((size_t)li * cdp::kMaxRanks + j) * cdp::kBwMaxSizes * 2);
+  };
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    cdp::LocalRank& L = h->lr[li];
+    for (uint32_t j = 0; j < n; ++j) {
+      if (!runs[li][j]) continue;
+      const cdp::MemcpyCell c = cdp::memcpy_cell(pl, op, L.grank, j);
+      if (const int rc = cdp::expected_sums(h, L, ms.table_off, cdp::SrcRegionWord{h->seed, c.first_word, c.src_rank},
+                                            lad.size, lad.n_sizes, want_of(li, j), "cdprobe_memcpy: granule checksums");
+          rc != CDPROBE_OK)
+        return rc;
+    }
+  }
+
+  // 5. the rounds: the tournament's, then the loop-back.  No process starts a round or a size before every process has
+  //    finished the one before; within a size, one rep at a time on every local rank at once.  After a size, every
+  //    local stream is drained, and the checks' records and the events are read: per rep, the diagnosis's bad words
+  //    and the (S, X) read against the pattern's
+  auto ns = std::make_unique<float[][cdp::kBwMaxSizes][cdp::kMaxTimedReps]>(cdp::kMaxRanks);
+  const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
+  for (uint32_t r = 0; r < n_rounds; ++r) {
+    if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+    int32_t target[cdp::kMaxRanks];
+    bool local = false, aborted[cdp::kMaxRanks] = {};
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      const int q = r < pl.rounds ? pl.partner[r][h->lr[li].grank] : (int)h->lr[li].grank;
+      target[li] = q >= 0 && runs[li][q] ? q : -1;
+      local |= target[li] >= 0;
+    }
+    for (uint32_t k = 0; k < lad.n_sizes; ++k) {
+      if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+      if (!local) continue;
+      for (uint32_t rep = 0; rep <= lad.reps; ++rep)
+        if (const int rc = cdp::memcpy_rep(h, target, op, lad, k, rep, f); rc != CDPROBE_OK) return rc;
+      for (uint32_t li = 0; li < h->n_local; ++li) {
+        if (target[li] < 0) continue;
+        const cdp::LocalRank& L = h->lr[li];
+        const uint32_t j = (uint32_t)target[li], idx = L.grank * CDPROBE_MAX_GPUS + j;
+        CDP_RT(cudaSetDevice(L.ordinal));
+        if (const cudaError_t e = cudaStreamSynchronize(L.stream); e != cudaSuccess)
+          return cdp::fail_sticky(h, "cdprobe_memcpy: check a size", e);
+        const uint64_t(*w)[2] = want_of(li, j);
+        uint64_t first = UINT64_MAX;
+        for (uint32_t rep = 0; rep <= lad.reps; ++rep) {
+          const cdp::MemcpyRepOut& got = h->memcpy_host->rep[li][rep];
+          aborted[li] |= got.abort_flag != 0;
+          out->bad_words[idx][k] += got.diag[0];
+          if (got.diag[0] != 0) first = std::min(first, (uint64_t)~got.diag[2]);
+          if (got.diag[0] != 0 || got.acc.sum != w[k][0] || got.acc.xr != w[k][1]) out->bad_sizes[idx] |= 1u << k;
+          if (rep == lad.reps) {
+            out->sum[idx][k] = got.acc.sum;
+            out->xr[idx][k] = got.acc.xr;
+          }
+          if (rep == 0) continue;
+          float ms_rep = 0.f;
+          const cudaError_t e = cudaEventElapsedTime(&ms_rep, L.memcpy_ev[2 * rep], L.memcpy_ev[2 * rep + 1]);
+          if (e != cudaSuccess) return cdp::fail_sticky(h, "cdprobe_memcpy: event times", e);
+          ns[li][k][rep - 1] = ms_rep * 1e6f;
+        }
+        out->first_bad[idx][k] = first;
+      }
+    }
+    // per cell: the times, unless an (S, X) read passed its deadline, and the verdict of every size's checks
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      if (target[li] < 0) continue;
+      const uint32_t idx = h->lr[li].grank * CDPROBE_MAX_GPUS + (uint32_t)target[li];
+      out->measured[idx] = 1;
+      if (aborted[li]) {
+        out->status[idx] = CDPROBE_ERR_TIMEOUT;
+        continue;
+      }
+      cdp::ladder_times(ns[li], lad.size, lad.n_sizes, lad.reps, 1.0, idx, out);
+      out->status[idx] = out->bad_sizes[idx] ? CDPROBE_ERR_INTEGRITY : 0;
     }
   }
   out->ms = cdp::now_ms() - lad.t_begin;

@@ -61,6 +61,19 @@ int make_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, Plan* o
   return CDPROBE_OK;
 }
 
+MemcpyCell memcpy_cell(const Plan& pl, uint32_t op, uint32_t g, uint32_t j) {
+  // a pull moves the slice g reads from j to g; a push moves the slice j reads from g to j
+  const bool push = op == CDPROBE_OP_WRITE;
+  const uint32_t reader = push ? j : g, owner = push ? g : j;
+  MemcpyCell c;
+  c.src_rank = owner;
+  c.src_off = cell_offset(pl, CDPROBE_OP_READ, reader, owner);
+  c.first_word = (uint64_t)cell_slice(pl, reader, owner) * (pl.bpp / 8);
+  c.dst_rank = reader;
+  c.dst_off = (uint64_t)owner * pl.bpp;
+  return c;
+}
+
 }  // namespace cdp
 
 extern "C" int cdprobe_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, cdprobe_plan_t* out) {

@@ -38,6 +38,19 @@ inline uint64_t cell_offset(const Plan& pl, uint32_t op, uint32_t i, uint32_t j)
   return op == CDPROBE_OP_WRITE ? pl.land_off + (uint64_t)cell_slot(pl, i, j) * pl.bpp
                                 : pl.src_off + (uint64_t)cell_slice(pl, i, j) * pl.bpp;
 }
+// What cell (issuer g, target j) of cdprobe_memcpy copies with op (CDPROBE_OP_READ: a pull, CDPROBE_OP_WRITE: a
+// push) and where it lands (DESIGN §5n).  The source is a source slice: the one g reads from j, in j's allocation, for
+// a pull; the one j reads from g, in g's own allocation, for a push.  Its word k is src_word(seed, src_rank,
+// first_word + k).  The destination is the block of the sender (the slice's owner) in the receiver's exchange area,
+// so the cells of one round never land on the same bytes.
+struct MemcpyCell {
+  uint32_t src_rank;    // whose allocation holds the source slice
+  uint64_t src_off;     // the slice's byte offset in that allocation
+  uint64_t first_word;  // the slice's first word in src_rank's source buffer
+  uint32_t dst_rank;    // whose exchange area receives the copy
+  uint64_t dst_off;     // the block's byte offset in that area
+};
+MemcpyCell memcpy_cell(const Plan& pl, uint32_t op, uint32_t g, uint32_t j);
 // Returns CDPROBE_OK or CDPROBE_ERR_ARG.
 int make_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, Plan* out);
 

@@ -53,6 +53,10 @@ bool Driver::load_multicast() {
   return multicast == 1;
 }
 
+cudaError_t Driver::load_stream_wait(std::string* err) {
+  return StreamWaitValue64 != nullptr ? cudaSuccess : resolve("cuStreamWaitValue64", &StreamWaitValue64, err);
+}
+
 std::string Driver::error_name(CUresult r) const {
   const char* s = nullptr;
   if (GetErrorName && GetErrorName(r, &s) == CUDA_SUCCESS && s) return s;

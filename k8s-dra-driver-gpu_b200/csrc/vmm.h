@@ -37,11 +37,15 @@ struct Driver {
   CUresult (*DeviceGet)(CUdevice*, int) = nullptr;
   CUresult (*DeviceGetAttribute)(int*, CUdevice_attribute, CUdevice) = nullptr;
   int multicast = -1;  // load_multicast's verdict, -1: not asked yet
+  // The stream wait of cdprobe_memcpy: resolved by load_stream_wait on its first call, apart from load's set.
+  CUresult (*StreamWaitValue64)(CUstream, CUdeviceptr, cuuint64_t, unsigned int) = nullptr;
 
   // Returns cudaSuccess or the runtime error that prevented loading.
   cudaError_t load(std::string* err);
   // Whether every multicast entry point above resolved; asked once.
   bool load_multicast();
+  // Resolves StreamWaitValue64 once; returns cudaSuccess or why it is missing.
+  cudaError_t load_stream_wait(std::string* err);
   std::string error_name(CUresult r) const;
 };
 

@@ -459,6 +459,59 @@ class AllToAll:
                         first_bad=cells(t.first_bad), sum=cells(t.sum), xr=cells(t.xr), ms=t.ms, raw=t)
 
 
+@dataclasses.dataclass
+class Memcpy:
+    """What cdprobe_memcpy measured: per cell [issuer][target], ns per copy-engine copy (min, median and max over the
+    timed reps, by CUDA events) of each size of the ladder `sizes`, pulled from the target (op OP_READ) or pushed to it
+    (OP_WRITE), the word check of what landed (`bad_words` over every rep, and `first_bad`, the byte offset of the
+    lowest bad word or U64_MAX), the (S, X) of the last timed rep's destination, the sizes that failed either check
+    (`bad_sizes`, bit k for sizes[k]) and the summary of the medians: t0_ns (the smallest size; events resolve about
+    0.5 us), peak_gbps and half_bytes.  Per-size values are lists over `sizes`.  A cell that did not run is None
+    everywhere but `status`; a cell whose (S, X) read passed timeout_ms has no times."""
+    n: int
+    row_mask: int
+    reps: int
+    op: int
+    call_seq: int
+    area_bytes: int
+    sizes: List[int]
+    measured: List[List[bool]]
+    status: List[List[int]]     # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the issuer's mapping status
+    bad_sizes: List[List[Optional[int]]]
+    t0_ns: List[List[Optional[float]]]
+    peak_gbps: List[List[Optional[float]]]
+    half_bytes: List[List[Optional[int]]]
+    ns_min: List[List[Optional[List[float]]]]
+    ns_median: List[List[Optional[List[float]]]]
+    ns_max: List[List[Optional[List[float]]]]
+    sum: List[List[Optional[List[int]]]]
+    xr: List[List[Optional[List[int]]]]
+    bad_words: List[List[Optional[List[int]]]]
+    first_bad: List[List[Optional[List[int]]]]
+    ms: float
+    raw: abi.MemcpyT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.MemcpyT) -> "Memcpy":
+        k = t.n_sizes
+
+        def timed(c):
+            return t.measured[c] and t.status[c] != abi.ERR_TIMEOUT
+
+        def per_size(a):
+            return [list(x)[:k] for x in a]
+
+        return Memcpy(n=t.n, row_mask=t.row_mask, reps=t.reps, op=t.op, call_seq=t.call_seq, area_bytes=t.area_bytes,
+                      sizes=list(t.size)[:k], measured=_mat(t, [bool(m) for m in t.measured]),
+                      status=_mat(t, t.status), bad_sizes=_mat(t, t.bad_sizes, timed),
+                      t0_ns=_mat(t, t.t0_ns, timed), peak_gbps=_mat(t, t.peak_gbps, timed),
+                      half_bytes=_mat(t, t.half_bytes, timed), ns_min=_mat(t, per_size(t.ns_min), timed),
+                      ns_median=_mat(t, per_size(t.ns_median), timed), ns_max=_mat(t, per_size(t.ns_max), timed),
+                      sum=_mat(t, per_size(t.sum), timed), xr=_mat(t, per_size(t.xr), timed),
+                      bad_words=_mat(t, per_size(t.bad_words), timed),
+                      first_bad=_mat(t, per_size(t.first_bad), timed), ms=t.ms, raw=t)
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -727,6 +780,22 @@ class Probe:
         """The bare ABI call: (return code, abi.AllToAllT as the library left it)."""
         t = abi.AllToAllT()
         rc = self._lib.cdprobe_alltoall(self._h, reps, C.byref(t))
+        return rc, t
+
+    def Memcpy(self, op: int, reps: int = 0) -> Memcpy:
+        """Go: (*Probe).Memcpy.  Copy-engine bandwidth versus transfer size of every cell whose issuer is local:
+        cudaMemcpyAsync of each size of the bwcurve ladder from the target into the issuer's exchange area (op
+        abi.OP_READ, a pull) or from the issuer into the target's (abi.OP_WRITE, a push), each copy timed by CUDA events
+        and every landed word checked (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first
+        and disturbs none."""
+        rc, t = self.memcpy_raw(op, reps)
+        _check(self._lib, rc, "cdprobe_memcpy")
+        return Memcpy.from_c(t)
+
+    def memcpy_raw(self, op: int, reps: int):
+        """The bare ABI call: (return code, abi.MemcpyT as the library left it)."""
+        t = abi.MemcpyT()
+        rc = self._lib.cdprobe_memcpy(self._h, op, reps, C.byref(t))
         return rc, t
 
     def Close(self) -> None:
