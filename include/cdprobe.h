@@ -598,11 +598,11 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              cdprobe_atomics: in the process that hosts the issuer, the first op of timed
                                              rep 1 of cell (issuer, target) adds 2 (CAS: swaps in v + 2), so exactly
                                              that cell fails its checks; 0 disarms */
-#define CDPROBE_OPT_ALLREDUCE_FAULT 19u   /* tests: value = ((rank + 1) << 32) | ((k + 1) << 24) | word arms an off-by-one
-                                             in cdprobe_allreduce: in the process that hosts `rank`, timed rep 1 of
-                                             size[k] adds 1 to output word `word` (< 2^24) before it is stored and
-                                             folded, so exactly that row and size fail the checksum (and the word check
-                                             when reps == 1); 0 disarms */
+#define CDPROBE_OPT_ALLREDUCE_FAULT 19u   /* tests: value = (drop << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
+                                             arms a fault in cdprobe_allreduce: in the process that hosts `rank`, timed
+                                             rep 1 of size[k] adds 1 to output word `word` (< 2^24) before it is stored
+                                             (drop 0), or stores nothing of the word's 8 KiB unit (drop 1), so exactly
+                                             that row and size fail the word check and rep 1's checksum; 0 disarms */
 #define CDPROBE_OPT_ALLTOALL_FAULT 20u    /* tests: value = ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24)
                                              | word arms a fault in transit in cdprobe_alltoall: in the process that
                                              hosts `sender`, timed rep 1 of size[k] stores word `word` (< 2^24) of
@@ -620,7 +620,10 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              packet of word `arg` (< 2^24) from sender to receiver (!= sender) carries
                                              its data xored with 1 and the right flags, so exactly that receiver's row
                                              fails at that size; mode 1, the sender waits `arg` us (< timeout_ms / 2)
-                                             before its first push of the rep, and every row stays exact; 0 disarms */
+                                             before its first push of the rep, and every row stays exact; mode 2, in
+                                             every rep of size[k], warm-up included, the receiver (== sender) makes no
+                                             store to output word `arg` (< size[k] / 8) but still folds it into (S, X),
+                                             so exactly that row and size fail the word check; 0 disarms */
 #define CDPROBE_OPT_ALLREDUCE_RING_FAULT 23u /* tests: value = (mode << 48) | (phase << 40) | ((sender + 1) << 32) |
                                              ((k + 1) << 24) | arg arms a fault in cdprobe_allreduce_ring, in timed rep
                                              1 of size[k], in the process that hosts `sender`, in phase 0 (the
@@ -739,8 +742,11 @@ CDPROBE_API int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* 
  * the CDPROBE_OPT_PATH read path with its whole probe grid, and stores the sums with st.global.v4 into its scratch
  * buffer.  A domain barrier opens every rep (flags in the Ctrl granule; only a grid barrier at n == 1), and a rep is
  * timed per rank by %globaltimer from that rank's release to its last CTA's completion; ranks are released a signal
- * latency apart, so no time is domain-wide.  Every rep's (S, X) is checked against the pattern's sum, and after the
- * last rep of a size every output word is (bad_sizes, bad_words, CDPROBE_ERR_INTEGRITY).  If any cell of the domain
+ * latency apart, so no time is domain-wide.  After every rep, warm-up included and untimed, each rank reads back every
+ * word of its output, compares it with the pattern's sum and overwrites it with 0, as cdprobe_allreduce_twoshot does,
+ * so a unit that a rep does not store reads as 0s; the output also starts zeroed on every call.  Every rep's (S, X) of
+ * that read-back is checked against the pattern's sum (bad_sizes, CDPROBE_ERR_INTEGRITY); sum and xr are the last
+ * timed rep's, and bad_words and first_bad are summed over every rep of the size, warm-up included.  If any cell of the domain
  * is down (cdprobe_unmap_peer, a failed mapping, MIG), nothing runs: every filled row has measured = 0 and the status
  * of the first such cell, and the call returns CDPROBE_OK.  A rank whose kernel passes timeout_ms is
  * CDPROBE_ERR_TIMEOUT and the handle stays usable.  Collective when world_size > 1: every process calls it with the
@@ -748,8 +754,8 @@ CDPROBE_API int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* 
  * buffer grows by that much until close (1 GiB at n == 1 with 1 GiB).  Touches no result, pattern, landing slot, Ctrl
  * word, pingpong or atomics line, run_seq, warm-up or bwcurve state.  *out carries abi, n and reps whatever the return
  * code.  CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments that differ between processes,
- * or an armed CDPROBE_OPT_ALLREDUCE_FAULT whose rank is >= n, whose k is >= n_sizes or whose word is
- * >= size[k] / 8; CDPROBE_ERR_STATE: sticky handle. */
+ * or an armed CDPROBE_OPT_ALLREDUCE_FAULT whose rank is >= n, whose k is >= n_sizes, whose word is
+ * >= size[k] / 8 or that has a bit above 48 set; CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_allreduce(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 /* One-shot all-to-all: every rank pushes a block to every peer at once.  For each size of the cdprobe_bwcurve ladder,
  * one untimed warm-up rep, then `reps` timed reps.  In rep r of size k, sender i writes the first size bytes of block
@@ -786,7 +792,7 @@ CDPROBE_API int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t
  * read-back is checked against the pattern's sum (bad_sizes, CDPROBE_ERR_INTEGRITY).  Row r of *out describes what
  * rank r holds at the end of a rep:
  *   sum, xr:              the (S, X) of rank r's whole output as rank r read it back after the last timed rep;
- *   bad_words, first_bad: summed over every rep of the size, warm-up included (cdprobe_allreduce checks only the last);
+ *   bad_words, first_bad: summed over every rep of the size, warm-up included, as cdprobe_allreduce's;
  *   peak_gbps:            the algorithm bandwidth, size / ns; the nccl-tests bus bandwidth is peak_gbps x 2 (n - 1) / n.
  * The gather area (bytes_per_pair per rank, rounded up to 2 MiB) is created on the first call with the probe
  * allocation's handle type, mapped wherever the probe mapping is then up, and kept until close; if creating it fails
@@ -812,9 +818,12 @@ CDPROBE_API int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_a
  * a packet of another rep that were accepted would leave a wrong word.  Every rank splits the words alike, over the
  * warps of the domain's smallest grid.  A rep is timed per rank by %globaltimer from the end of that rank's previous
  * rep (the warm-up: from the barrier release) to the moment its output is complete, the per-iteration figure
- * nccl-tests reports.  Row r of *out is as cdprobe_allreduce's: every rep's (S, X) and the word check of the last rep;
- * peak_gbps is the algorithm bandwidth, size / ns, and each rank's link ingress per rep is 2 (n - 1) x size (every 8
- * bytes of data travel in a 16-byte packet).  The LL area (2 x n x 2 x the ladder's largest size per rank, rounded up
+ * nccl-tests reports.  Every rep's (S, X) is folded from the sums as they are stored and checked (bad_sizes).  After
+ * the last rep of a size, untimed, each rank reads back every word of its output, compares it with the pattern's sum
+ * and overwrites it with 0 (bad_words, first_bad: that one check), and the output starts zeroed on every call, so a
+ * word the last rep of a size does not store is seen; one that only earlier reps of the size miss is not.  sum and xr
+ * are the last timed rep's; peak_gbps is the algorithm bandwidth, size / ns, and each rank's link ingress per rep is
+ * 2 (n - 1) x size (every 8 bytes of data travel in a 16-byte packet).  The LL area (2 x n x 2 x the ladder's largest size per rank, rounded up
  * to 2 MiB) is created on the first call with the probe allocation's handle type, zeroed, mapped wherever the probe
  * mapping is then up, and kept until close; if creating it fails in any process, every process returns that error,
  * nothing runs, and the next call tries again.  If any probe or LL-area mapping of the domain is down
@@ -826,8 +835,9 @@ CDPROBE_API int cdprobe_allreduce_twoshot(cdprobe_t* h, uint32_t reps, cdprobe_a
  * run_seq, warm-up state, exchange or gather area or other measurement's state.  *out carries abi, n, reps and path
  * whatever the return code.  CDPROBE_ERR_ARG: null argument, reps > 64, bytes_per_pair > 32 GiB, arguments that
  * differ between processes, or an armed CDPROBE_OPT_ALLREDUCE_LL_FAULT whose sender or receiver is >= n, whose k is
- * >= n_sizes, whose mode is above 1, whose mode-0 receiver is its sender or word is >= size[k] / 8, or whose mode-1
- * delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky handle. */
+ * >= n_sizes, whose mode is above 2, whose mode-0 receiver is its sender, whose mode-2 receiver is not its sender,
+ * whose mode-0 or mode-2 word is >= size[k] / 8, or whose mode-1 delay is >= timeout_ms / 2; CDPROBE_ERR_STATE: sticky
+ * handle. */
 CDPROBE_API int cdprobe_allreduce_ll(cdprobe_t* h, uint32_t reps, cdprobe_allreduce_t* out);
 /* Ring all-reduce of every rank's source buffer, on every rank at once: each rank talks only to its successor
  * r + 1 (mod n), to which it pushes, and its predecessor r - 1, which pushes to it.  For each size of the

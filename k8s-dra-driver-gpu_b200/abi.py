@@ -440,9 +440,12 @@ def alltoall_fault(sender: int, receiver: int, k: int, word: int) -> int:
     return ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | word
 
 
-def allreduce_fault(rank: int, k: int, word: int) -> int:
-    """The CDPROBE_OPT_ALLREDUCE_FAULT value that makes timed rep 1 of size[k] add 1 to output word `word` on `rank`."""
-    return ((rank + 1) << 32) | ((k + 1) << 24) | word
+def allreduce_fault(rank: int, k: int, word: int, drop: bool = False) -> int:
+    """The CDPROBE_OPT_ALLREDUCE_FAULT value that makes timed rep 1 of size[k] on `rank` add 1 to output word `word`,
+    or (drop) store nothing of the word's 8 KiB unit.  Fields that do not fit are refused here."""
+    if not (0 <= rank < 0xffff and 0 <= k < 255 and 0 <= word < 1 << 24):
+        raise ValueError("allreduce_fault: rank below 65535, k below 255, word below 2^24")
+    return ((1 if drop else 0) << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
 
 
 def allreduce_twoshot_fault(receiver: int, k: int, word: int, drop: bool = False) -> int:
@@ -452,11 +455,12 @@ def allreduce_twoshot_fault(receiver: int, k: int, word: int, drop: bool = False
 
 
 def allreduce_ll_fault(sender: int, receiver: int, k: int, arg: int, mode: int = 0) -> int:
-    """The CDPROBE_OPT_ALLREDUCE_LL_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_ll: mode 0, the packet
+    """The CDPROBE_OPT_ALLREDUCE_LL_FAULT value for size[k] of cdprobe_allreduce_ll: in timed rep 1, mode 0, the packet
     of word `arg` from `sender` to `receiver` carries its data xored with 1; mode 1, `sender` waits `arg` us before its
-    first push (`receiver` must still name a rank).  Fields that do not fit are refused here."""
-    if mode not in (0, 1) or not (0 <= sender < 255 and 0 <= receiver < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
-        raise ValueError("allreduce_ll_fault: mode 0 or 1, ranks and k below 255, arg below 2^24")
+    first push (`receiver` must still name a rank); in every rep of the size, mode 2, `receiver` (which must be
+    `sender`) makes no store to output word `arg`.  Fields that do not fit are refused here."""
+    if mode not in (0, 1, 2) or not (0 <= sender < 255 and 0 <= receiver < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
+        raise ValueError("allreduce_ll_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
     return (mode << 48) | ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | arg
 
 

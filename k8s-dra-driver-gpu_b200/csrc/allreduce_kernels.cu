@@ -14,12 +14,14 @@
 namespace cdp {
 namespace {
 // Unit u of the output is complete in the accumulators: the armed fault goes in (fw, an output word index; ~0 when
-// none), every vector of the unit leaves with st.global.v4 and is folded into the (S, X) by its place in the output,
-// and the accumulators are cleared for the next unit.
+// none), every vector of the unit leaves with st.global.v4, and the accumulators are cleared for the next unit.  The
+// fault adds 1 to its word, or (P.fault_drop) nothing of its unit is stored.  Nothing is folded into (S, X): the word
+// check reads the output back.
 template <uint32_t kLaneBytes>
-__device__ __forceinline__ void ar_store(const Ctx& c, uint8_t* out, uint64_t u, uint32_t len, uint64_t fw,
-                                         uint64_t (&acc)[kArWords], Sum& a) {
-  if (fw / (kUnitBytes / 8) == u) {  // rare: this unit holds the armed word
+__device__ __forceinline__ void ar_store(const Ctx& c, const AllReduceParams& P, uint64_t u, uint32_t len, uint64_t fw,
+                                         uint64_t (&acc)[kArWords]) {
+  const bool hit = fw / (kUnitBytes / 8) == u;  // rare: this unit holds the armed word
+  if (hit) {
     const uint32_t fb = (uint32_t)(fw % (kUnitBytes / 8)) * 8u;
 #pragma unroll
     for (int i = 0; i < kArWords / 2; ++i) {
@@ -28,39 +30,40 @@ __device__ __forceinline__ void ar_store(const Ctx& c, uint8_t* out, uint64_t u,
       else acc[2 * i] += 1ull;
     }
   }
-  uint8_t* base = out + u * kUnitBytes;
-  uint64_t ux = 0;
+  if (hit && P.fault_drop) len = 0;  // no vector of the unit is stored
+  uint8_t* base = P.out + u * kUnitBytes;
+  if (len == kUnitBytes) {  // a whole unit: every lane stores every vector, with no guard
 #pragma unroll
-  for (int i = 0; i < kArWords / 2; ++i) {
-    const uint32_t off = ar_vec_off<kLaneBytes>(c.lane, i);
-    const uint64_t w0 = acc[2 * i], w1 = acc[2 * i + 1];
-    if (off < len) {
-      stg_v4(reinterpret_cast<uint4*>(base + off),
-             make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)));
-      add_pair(a, ux, w0, w1);
-    }
-    acc[2 * i] = 0ull;
-    acc[2 * i + 1] = 0ull;
+    for (int i = 0; i < kArWords / 2; ++i)
+      stg_pair(base + ar_vec_off<kLaneBytes>(c.lane, i), acc[2 * i], acc[2 * i + 1]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < kArWords / 2; ++i)
+      if (ar_vec_off<kLaneBytes>(c.lane, i) < len)
+        stg_pair(base + ar_vec_off<kLaneBytes>(c.lane, i), acc[2 * i], acc[2 * i + 1]);
   }
-  fold_unit(a, ux, u);
+#pragma unroll
+  for (int i = 0; i < kArWords; ++i) acc[i] = 0ull;
 }
 
 // The one-shot's store policy (allreduce_path.cuh): a summed unit goes to the rank's own output, P.out.
 struct ToOut {
   template <uint32_t kLaneBytes>
   __device__ __forceinline__ static void put(const Ctx& c, const AllReduceParams& P, uint64_t u, uint32_t len,
-                                             uint64_t fw, uint64_t (&acc)[kArWords], Sum& a) {
-    ar_store<kLaneBytes>(c, P.out, u, len, fw, acc, a);
+                                             uint64_t fw, uint64_t (&acc)[kArWords], Sum&) {
+    ar_store<kLaneBytes>(c, P, u, len, fw, acc);
   }
 };
 }  // namespace
 
 // One rank of cdprobe_allreduce: for every size of the ladder, one warm-up and P.reps timed reps, each summing the
-// first size bytes of all P.n inputs into P.out with every warp of the grid (the strided walk of a probe phase) and
-// folding the sum into the (S, X) checksum.  A domain barrier opens every rep, so a rep is timed as a probe phase is,
-// per rank: from this rank's release stamp to its latest CTA completion stamp (ranks see a release one signal latency
-// apart).  After the last rep of a size and a grid barrier, the word check.  Its state (barrier, stamps, checksums,
-// word-check counters, abort word) is in the rank's scratch buffer; outside it only its barrier lines are written.
+// first size bytes of all P.n inputs into P.out with every warp of the grid (the strided walk of a probe phase).  A
+// domain barrier opens every rep, so a rep is timed as a probe phase is, per rank: from this rank's release stamp to its
+// latest CTA completion stamp (ranks see a release one signal latency apart).  After every rep and a grid barrier, the
+// word check and clear of the output (allreduce_path.cuh's ar_check_clear), untimed: the rep's (S, X) is folded from
+// what the check read back, and a unit that a later rep does not store reads as 0s (DESIGN §5g).  Its state (barrier,
+// stamps, checksums, word-check counters, abort word) is in the rank's scratch buffer; outside it only its barrier
+// lines are written.
 __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_constant__ AllReduceParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];
   ArScratch* as = P.scratch;
@@ -77,15 +80,13 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_kernel(const __grid_con
       if (!grid_barrier(c, bs, b++, &bs->t_rel[k][r], &P.dom, false)) return;
       const uint64_t fw = (r == 1u && k == P.fault_k) ? P.fault_word : ~0ull;
       Sum a{0ull, 0ull, 0ull};
-      const Walk<false> walk = strided(bytes, gwarp, nwarps);
-      ar_units<ToOut>(c, P, bytes, walk, fw, a);
+      ar_units<ToOut>(c, P, bytes, strided(bytes, gwarp, nwarps), fw, a);
       __threadfence();  // this warp's stores are performed before the CTA's completion stamp
-      Acc* const acc = &bs->rep[k][r];
-      cta_reduce<1>(c, red, &a, &acc);
-      if (threadIdx.x == 0) atomicMax(&acc->t_end, (unsigned long long)gtimer());
+      __syncthreads();
+      if (threadIdx.x == 0) atomicMax(&bs->rep[k][r].t_end, (unsigned long long)gtimer());
+      if (!grid_barrier(c, bs, b++, nullptr, nullptr, false)) return;
+      ar_check_clear(c, P, reinterpret_cast<uint4*>(P.out), as, red, k, r, bytes, gwarp, nwarps);
     }
-    if (!grid_barrier(c, bs, b++, nullptr, nullptr, false)) return;
-    ar_check(c, P, as, k, bytes, gwarp, nwarps);
   }
 }
 

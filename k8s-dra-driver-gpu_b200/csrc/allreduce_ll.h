@@ -22,9 +22,10 @@ struct LlParams {
   uint64_t s_max;                 // its largest size: the LL area's slot layout (ll_slot)
   uint64_t seed;                  // the pattern seed (the inputs, the salts and the word check)
   uint64_t timeout_ns;            // device deadline from kernel entry
-  uint64_t fault_arg;             // the armed fault, in timed rep 1 of size fault_k (kArNoFault: disarmed): mode 0,
+  uint64_t fault_arg;             // the armed fault, in size fault_k (kArNoFault: disarmed): in timed rep 1, mode 0,
   uint32_t fault_k;               //   the packet of word fault_arg to dst[fault_dst] carries its data xored with 1;
-  uint32_t fault_mode, fault_dst; //   mode 1, this rank waits fault_arg us before its first push
+  uint32_t fault_mode, fault_dst; //   mode 1, this rank waits fault_arg us before its first push; in every rep,
+                                  //   mode 2, this rank makes no store to output word fault_arg
   uint32_t rank, n, n_sizes, reps;
   uint32_t ctas;                  // the domain's smallest grid: only CTAs below it move words
   uint32_t path;                  // set for every ladder kernel; LL has one data path and ignores it
@@ -33,7 +34,7 @@ struct LlParams {
 // Launches allreduce_ll_kernel on `stream` of the current device: `grid` (>= p.ctas) CTAs of the probe kernel's shape,
 // cooperative or not as the probe launches them.  For every size, one domain barrier, then one warm-up and p.reps
 // timed reps back to back, each pushing this rank's words as flag-carrying packets to every peer and summing the
-// packets that arrive, then the word check of the last one (DESIGN §5j).  Returns a cudaError_t.
+// packets that arrive, then the word check and clear of the last one's output (DESIGN §5j).  Returns a cudaError_t.
 int allreduce_ll_launch(const LlParams& p, unsigned grid, bool cooperative, cudaStream_t stream);
 
 }  // namespace cdp

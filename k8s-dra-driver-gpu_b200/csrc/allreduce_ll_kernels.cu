@@ -1,7 +1,8 @@
 // allreduce_ll_kernels.cu — sm_90a kernel of cdprobe_allreduce_ll's low-latency all-reduce: every 64-bit input word
 // travels to every peer as one 16-byte packet of two flag-carrying 8-byte elements (st.relaxed.sys.v2.u64), and the
 // receiver polls its own LL area (ld.relaxed.sys.v2.u64) until both flags of each packet are the rep's; no barrier and
-// no fence inside a size (allreduce_ll_kernel).  The word check is the one-shot's (allreduce_path.cuh).
+// no fence inside a size (allreduce_ll_kernel).  The word check and clear of the output after each size is
+// allreduce_path.cuh's ar_check.
 //
 // probe_kernels.cu is untouched: the probe kernel's code generation does not depend on this file.
 #include <cuda_runtime.h>
@@ -35,6 +36,7 @@ __device__ bool ll_rep(const Ctx& c, const LlParams& P, uint32_t k, uint32_t r, 
   const bool armed = r == 1u && k == P.fault_k;
   if (armed && P.fault_mode == 1u) delay_us(P.fault_arg);
   const uint64_t fw = armed && P.fault_mode == 0u ? P.fault_arg : ~0ull;
+  const uint64_t nw = k == P.fault_k && P.fault_mode == 2u ? P.fault_arg : ~0ull;  // mode 2: the word left unstored
 
   // 1. push: one packet per owned word to rank g + 1, g + 2, ... (mod n)
   for (uint64_t i = gwarp; i < lines; i += nwarps) {
@@ -69,7 +71,7 @@ __device__ bool ll_rep(const Ctx& c, const LlParams& P, uint32_t k, uint32_t r, 
       acc += (e0 & 0xffffffffull) | (e1 << 32);
     }
     const uint64_t v = acc - salts;
-    out[w] = v;
+    if (w != nw) out[w] = v;
     a.s0 += v;
     a.x ^= rotl64(v, fold6((uint32_t)(i / (kGranuleWords / 32))));
   }
@@ -81,8 +83,9 @@ __device__ bool ll_rep(const Ctx& c, const LlParams& P, uint32_t k, uint32_t r, 
 // then one warm-up and P.reps timed reps back to back with no barrier between them (ll_rep; rep r uses parity r % 2 of
 // the LL area).  A CTA's rep ends when its stores of the output are performed: its stamp goes into rep[k][r].t_end and
 // into t_rel[k][r + 1], where the next rep is timed from, so a rep runs from the end of this rank's previous rep to the
-// end of its own.  After the last rep of a size and a grid barrier, the one-shot's word check.  CTAs from P.ctas on
-// only join the barriers and the check.  State lives in the rank's scratch buffer; outside it, only the peers' LL areas
+// end of its own.  After the last rep of a size and a grid barrier, the word check and clear of the output (ar_check),
+// so the next size, and the next call, finds 0s wherever it stores nothing.  CTAs from P.ctas on only join the
+// barriers and the check.  State lives in the rank's scratch buffer; outside it, only the peers' LL areas
 // and the barrier lines are written.
 __global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(const __grid_constant__ LlParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];

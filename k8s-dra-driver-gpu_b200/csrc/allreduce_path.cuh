@@ -2,12 +2,12 @@
 // allreduce_kernels.cu) and allreduce_twoshot_kernel (allreduce_twoshot_kernels.cu): every warp walks 8 KiB output
 // units, streams unit u of all P.n inputs (TMA ring or ld.global.v4) and adds them in registers (64-bit, wrapping).
 // Two things are parameters: the walk (which units a warp sums) and the store policy (where a summed unit goes).
-// Also the word check of an output in the rank's scratch (ar_check), shared by the one-shot and allreduce_ll_kernel
-// (allreduce_ll_kernels.cu), and the word check and clear of an output peers store into (ar_check_clear), shared by
-// the two-shot and allreduce_ring_kernel (allreduce_ring_kernels.cu).  And the pieces the all-reduce kernels share
-// around those: the store of a unit to several ranks (put_ranks, the two-shot's and the push's store policies), the
-// pair store (stg_pair, also the ring's), the armed delay (delay_us, the LL's and the ring's) and the fenced close of
-// a phase (close_fenced, the two-shot's and the push's).
+// Also the word check and clear of allreduce_ll_kernel's output after the last rep of a size (ar_check,
+// allreduce_ll_kernels.cu), and the word check and clear of an output after every rep (ar_check_clear), shared by the
+// one-shot, the two-shot, allreduce_ring_kernel (allreduce_ring_kernels.cu) and allreduce_nvls_kernel.  And the pieces
+// the all-reduce kernels share around those: the store of a unit to several ranks (put_ranks, the two-shot's and the
+// push's store policies), the pair store (stg_pair, also the one-shot's and the ring's), the armed delay (delay_us, the
+// LL's and the ring's) and the fenced close of a phase (close_fenced, the two-shot's and the push's).
 //
 // A store policy S has one member, called once per unit by every lane with the unit's sums in acc:
 //   template <uint32_t kLaneBytes> static void S::put(const Ctx&, const Params& P, uint64_t u, uint32_t len,
@@ -215,13 +215,14 @@ __device__ __forceinline__ void ar_check_flush(const Ctx& c, ArScratch* as, uint
   }
 }
 
-// The untimed word check of the output the last rep of size k stored at P.out (allreduce_kernel and
-// allreduce_ll_kernel): each lane compares every 32nd word of its warp's share with allreduce_word, reading at L2
-// (other SMs stored them).  One atomic pair per warp with a bad word.
+// The untimed word check and clear of the output the last rep of size k stored at P.out (allreduce_ll_kernel): each
+// lane compares every 32nd word of its warp's share with allreduce_word, reading at L2 (other SMs stored them), and
+// overwrites it with 0, so a word that the next size or call does not store reads as 0 rather than as this size's
+// sum.  One atomic pair per warp with a bad word.
 template <typename Params>
 __device__ void ar_check(const Ctx& c, const Params& P, ArScratch* as, uint32_t k, uint64_t bytes, uint32_t gwarp,
                          uint32_t nwarps) {
-  const unsigned long long* out = reinterpret_cast<const unsigned long long*>(P.out);
+  unsigned long long* out = reinterpret_cast<unsigned long long*>(P.out);
   const uint64_t words = bytes / 8;
   uint64_t bad = 0, first = ~0ull;
   for (uint64_t w = (uint64_t)gwarp * 32u + (uint32_t)c.lane; w < words; w += (uint64_t)nwarps * 32u) {
@@ -229,15 +230,17 @@ __device__ void ar_check(const Ctx& c, const Params& P, ArScratch* as, uint32_t 
       ++bad;
       first = min(first, w * 8u);
     }
+    out[w] = 0ull;
   }
+  __threadfence();  // the clearing stores are performed before the next size's opening barrier
   ar_check_flush(c, as, k, bad, first);
 }
 
-// The untimed check of rep r of size k of an output peers store into (allreduce_twoshot_kernel's gather area,
-// allreduce_ring_kernel's ring area): every word of it is read at L2 (peers and other SMs stored it), compared with
-// allreduce_word, folded into the rep's (S, X) by its place in the output, and then overwritten with 0, so a unit that
-// is not delivered in a later rep reads as 0s rather than as this rep's sums.  One atomic pair per warp with a bad
-// word, over every rep of the size.
+// The untimed check of rep r of size k of an output (allreduce_kernel's in the rank's scratch,
+// allreduce_twoshot_kernel's gather area, allreduce_ring_kernel's ring area): every word of it is read at L2 (peers and
+// other SMs stored it), compared with allreduce_word, folded into the rep's (S, X) by its place in the output, and then
+// overwritten with 0, so a unit that is not delivered in a later rep reads as 0s rather than as this rep's sums.  One
+// atomic pair per warp with a bad word, over every rep of the size.
 template <typename Params>
 __device__ void ar_check_clear(const Ctx& c, const Params& P, uint4* const out, ArScratch* as, uint64_t* red,
                                uint32_t k, uint32_t r, uint64_t bytes, uint32_t gwarp, uint32_t nwarps) {

@@ -29,10 +29,11 @@
 namespace cdp {
 
 // Grows local rank L's scratch to at least `bytes`, on its device (the caller has selected it); the old buffer is freed
-// first.  The measurements share it: each runs on L's one stream, copies its results out before it returns, and reads
-// back only what its own kernels wrote in the same call.  diag_launch clears its DiagOut and the compare pass writes
-// every granule count; a rep table is read up to its first TIMEOUT slot, and the kernels write one for every cell they
-// leave unfinished.
+// first, and the new one is not zeroed.  The measurements share it: each runs on L's one stream, copies its results
+// out before it returns, and reads back only what its own kernels wrote in the same call.  diag_launch clears its
+// DiagOut and the compare pass writes every granule count; a rep table is read up to its first TIMEOUT slot, and the
+// kernels write one for every cell they leave unfinished; launch_ladder clears a ladder kernel's records; the one-shot
+// and LL all-reduces zero their output at the start of every call, and their word checks clear each word they read.
 static int ensure_scratch(LocalRank& L, size_t bytes) {
   if (L.scratch_bytes >= bytes) return CDPROBE_OK;
   if (L.scratch) cudaFree(L.scratch);
@@ -523,10 +524,10 @@ static Params ar_params(const cdprobe* h, const LocalRank& L, const DomainLines&
 }
 
 static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
-  const uint64_t fr = v >> 32, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
-  if (fr == 0 || fr > h->n_total || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+  const uint64_t fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  if ((v >> 49) != 0 || fr == 0 || fr > h->n_total || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
     return "the armed all-reduce fault names no rank, size or output word of this call";
-  *f = {(uint32_t)fr - 1, 0, (uint32_t)fk - 1, 0, word};
+  *f = {(uint32_t)fr - 1, 0, (uint32_t)fk - 1, (uint32_t)(v >> 48), word};
   return nullptr;
 }
 
@@ -537,6 +538,7 @@ static int oneshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, cons
   for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
   p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
   p.fault_word = f.word;
+  p.fault_drop = f.mode;
   return launch_ladder(h, L, p, lad, allreduce_launch, "launch allreduce_kernel");
 }
 
@@ -570,13 +572,14 @@ static int twoshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, cons
   return launch_ladder(h, L, p, lad, allreduce_twoshot_launch, "launch allreduce_twoshot_kernel");
 }
 
-// The fault acts in the process that hosts its sender.
+// The fault acts in the process that hosts its sender, which for mode 2 is its receiver.
 static const char* ll_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
   const uint32_t n = h->n_total;
   const uint64_t mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu, fk = (v >> 24) & 0xffu,
                  arg = v & 0xffffffu;
-  if (mode > 1 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes ||
-      (mode == 0 && (fs == fr || arg >= lad.size[fk - 1] / 8)) || (mode == 1 && 2 * arg >= 1000ull * h->cfg.timeout_ms))
+  if (mode > 2 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes ||
+      (mode != 1 && arg >= lad.size[fk - 1] / 8) || (mode == 0 && fs == fr) || (mode == 2 && fs != fr) ||
+      (mode == 1 && 2 * arg >= 1000ull * h->cfg.timeout_ms))
     return "the armed LL all-reduce fault names no packet, size or delay of this call";
   *f = {(uint32_t)fs - 1, (uint32_t)fr - 1, (uint32_t)fk - 1, (uint32_t)mode, arg};
   return nullptr;
@@ -798,6 +801,16 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   //    sums of the summed words on the first local rank's GPU, folded into every prefix on the host
   const size_t table_off = kArOutOff + (P.out_in_scratch ? (s_max + 255) / 256 * 256 : 0);
   if (const int rc = ensure_scratch_all(h, table_off + 16 * (h->plan.bpp / kGranuleBytes)); rc != CDPROBE_OK) return rc;
+  // an output in the scratch starts zeroed on every call, so a word this call does not store reads as 0 rather than
+  // as what an earlier call, an aborted one or another handle's left there
+  if (P.out_in_scratch) {
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      LocalRank& L = h->lr[li];
+      CDP_RT(cudaSetDevice(L.ordinal));
+      const cudaError_t e = cudaMemsetAsync(static_cast<uint8_t*>(L.scratch) + kArOutOff, 0, s_max, L.stream);
+      if (e != cudaSuccess) return fail_sticky(h, (std::string(P.fn) + ": zero the output").c_str(), e);
+    }
+  }
   uint64_t want[kBwMaxSizes][2] = {};
   if (const int rc = expected_sums(h, h->lr[0], table_off, AllReduceWord{h->seed, n}, lad.size, lad.n_sizes, want,
                                    (std::string(P.fn) + ": granule checksums").c_str());

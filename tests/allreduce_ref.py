@@ -15,6 +15,7 @@ import word_ref
 from bwcurve_ref import ladder, summary  # noqa: F401  (the all-reduce uses bwcurve's ladder and summary)
 
 GRANULE_WORDS = word_ref.GRANULE_WORDS
+UNIT_WORDS = 1024  # an 8 KiB output unit
 U64_MAX = word_ref.U64_MAX
 _u = np.uint64
 
@@ -56,3 +57,9 @@ def expected_corrupted(seed: int, n: int, sizes, rank: int, word: int, mask: int
         orig = int(word_ref.src_words(seed, rank, word, 1)[0])
         words[word] = _u((int(words[word]) - orig + (orig ^ mask)) % (1 << 64))
     return [checksum(words[:s // 8]) for s in sizes]
+
+
+def unit_words(word: int, size: int) -> range:
+    """The output words of the 8 KiB unit that holds `word` at a size of `size` bytes; the last unit may be partial."""
+    first = word // UNIT_WORDS * UNIT_WORDS
+    return range(first, min(first + UNIT_WORDS, size // 8))

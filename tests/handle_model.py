@@ -308,17 +308,19 @@ class HandleModel:
         or None when some process's armed fault names no rank, size or word of the ladder (CDPROBE_ERR_ARG; nothing
         advances).  Any unmapped pair stops every rank, with the status of the first down cell, and call_seq still
         advances.  Otherwise output word w is the sum of word w of every source buffer as it is at rest (slice 0 only),
-        a word is bad when that differs from the clean sum, and an armed fault adds 1 to its word in timed rep 1 of its
-        size on its rank: the word check and the reported (S, X) (both of the last rep) see it when reps is 1, and the
-        size fails at any reps since every rep's (S, X) is checked."""
+        a word is bad when that differs from the clean sum, and an armed fault acts in timed rep 1 of its size on its
+        rank: it adds 1 to its word, or (drop, bit 48) leaves its 8 KiB unit unstored, which the check after the rep
+        reads as 0s.  Every rep, warm-up included, is checked and cleared, so bad_words and first_bad cover every rep
+        and see the fault at any reps; the reported (S, X) is the last timed rep's, so it shows the fault when reps is
+        1, and the size fails at any reps since every rep's (S, X) is checked."""
         sizes = bwcurve_ref.ladder(self.bpp)
         faults = {}
         for proc, v in self.ar_fault.items():
-            fr, fk, fw = v >> 32, (v >> 24) & 0xFF, v & 0xFFFFFF
-            if fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+            fr, fk, fw = (v >> 32) & 0xFFFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if v >> 49 or fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
                 return None
             if self.process_of(fr - 1) == proc:
-                faults[(fr - 1, fk - 1)] = fw
+                faults[(fr - 1, fk - 1)] = (fw, bool(v >> 48))
         self.ar_calls += 1
         out = dict(call_seq=self.ar_calls, sizes=sizes, rows={})
         if self.unmapped:
@@ -341,17 +343,22 @@ class HandleModel:
             for k, s in enumerate(sizes):
                 nw = s // 8
                 rep1 = dict(at_rest)
-                fw = faults.get((g, k))
-                if fw is not None:
+                fw, drop = faults.get((g, k), (None, False))
+                if fw is not None and drop:
+                    for w in allreduce_ref.unit_words(fw, s):
+                        rep1[w] = (at_rest.get(w, (self.ar_word(w),))[0], 0)
+                elif fw is not None:
                     old, cur = at_rest.get(fw, (self.ar_word(fw),) * 2)
                     rep1[fw] = (old, (cur + 1) & M64)
                 last = rep1 if reps == 1 else at_rest
-                bad = sorted(w for w, (o, v) in last.items() if w < nw and o != v)
+                bad = sorted(w for w, (o, v) in at_rest.items() if w < nw and o != v)
+                bad1 = sorted(w for w, (o, v) in rep1.items() if w < nw and o != v)
                 sx = refold(clean[k], last, nw)
                 row["sx"].append(sx)
-                row["bad_words"].append(len(bad))
-                row["first_bad"].append(8 * bad[0] if bad else word_ref.U64_MAX)
-                if bad or sx != clean[k] or refold(clean[k], rep1, nw) != clean[k]:
+                row["bad_words"].append(reps * len(bad) + len(bad1))  # the warm-up and reps 2.. see the words at rest
+                first = min(bad[:1] + bad1[:1], default=None)
+                row["first_bad"].append(word_ref.U64_MAX if first is None else 8 * first)
+                if bad1 or sx != clean[k] or refold(clean[k], rep1, nw) != clean[k]:
                     row["bad_sizes"] |= 1 << k
             row["status"] = ERR_INTEGRITY if row["bad_sizes"] else 0
             out["rows"][g] = row

@@ -40,6 +40,13 @@ def test_allreduce_struct_layout_matches_c(pkg, tmp_path):
     assert int(got["opt"]) == a.OPT_ALLREDUCE_FAULT == 19
     assert "cdprobe_allreduce" in a.SYMBOLS
     assert a.allreduce_fault(2, 5, 77) == (3 << 32) | (6 << 24) | 77
+    assert a.allreduce_fault(2, 5, 77, drop=True) == (1 << 48) | (3 << 32) | (6 << 24) | 77
+    assert a.allreduce_fault(0xfffe, 254, (1 << 24) - 1, drop=True) >> 49 == 0
+    for bad in (dict(rank=0xffff), dict(rank=-1), dict(k=255), dict(k=-1), dict(word=1 << 24), dict(word=-1)):
+        args = dict(rank=0, k=0, word=0)
+        args.update(bad)
+        with pytest.raises(ValueError):
+            a.allreduce_fault(**args)
 
 
 def test_every_declared_symbol_is_exported(pkg):
@@ -197,6 +204,11 @@ def kernel(pkg):
     return kernel_sass(pkg.abi.LIB_PATH, r"^_ZN3cdp16allreduce_kernel")[1]
 
 
+def unpredicated(t):
+    """The instruction without its guard predicate (@P0, @!P1, ...)."""
+    return re.sub(r"^@!?U?P\w+\s+", "", t)
+
+
 def stamp(text):
     """Index of the rep's completion stamp: the 64-bit atomic max whose value is a %globaltimer read."""
     for k, t in enumerate(text):
@@ -218,18 +230,31 @@ def test_every_read_path_and_the_vector_stores_are_compiled_in(kernel):
     assert not any(t.startswith("UBLKCP.G.S") for t in kernel)  # the sum does not leave through TMA
 
 
-def test_the_closing_timer_read_follows_the_last_store(kernel):
-    """The completion stamp is a %globaltimer read made after every store of the rep, the fence that waits for them,
-    the CTA barrier and the CTA's (S, X) reductions; it is the value the atomic max stores."""
+def test_the_closing_timer_read_follows_the_last_store_and_precedes_the_checksum(kernel):
+    """The completion stamp is a %globaltimer read made after every store of the rep, the fence that waits for them
+    and the CTA barrier; it is the value the atomic max stores.  The rep's (S, X) is not folded in the timed window: its
+    reductions follow the stamp, in the word check that reads the output back."""
     mx = stamp(kernel)
     timer = mx - 1
-    stores = [k for k, t in enumerate(kernel[:mx]) if t.startswith("STG.E.NA.128")]
-    fence = max(k for k in range(timer) if kernel[k].startswith("MEMBAR.SC.GPU"))
-    bar = max(k for k in range(timer) if kernel[k].startswith("BAR.SYNC"))
-    loads = [k for k, t in enumerate(kernel[:mx]) if t.startswith(("LDG.E.NA.128", "SYNCS.PHASECHK"))]
+    text = [unpredicated(t) for t in kernel]
+    stores = [k for k, t in enumerate(text[:mx]) if t.startswith("STG.E.NA.128")]
+    fence = max(k for k in range(timer) if text[k].startswith("MEMBAR.SC.GPU"))
+    bar = max(k for k in range(timer) if text[k].startswith("BAR.SYNC"))
+    loads = [k for k, t in enumerate(text[:mx]) if t.startswith(("LDG.E.NA.128", "SYNCS.PHASECHK"))]
     assert stores and loads and max(loads) < max(stores) < fence < bar < timer
-    reds = [k for k in range(bar, timer) if re.match(r"(REDG|ATOMG)\.E\.(ADD|XOR)\.64", kernel[k])]
-    assert len(reds) == 2
+    assert not any(re.match(r"(REDG|ATOMG)\.E\.(ADD|XOR)\.64", t) for t in text[:mx])
+    reds = [k for k, t in enumerate(text) if k > mx and re.match(r"(REDG|ATOMG)\.E\.(ADD|XOR)\.64", t)]
+    assert any(".XOR." in text[k] for k in reds) and any(".ADD." in text[k] for k in reds)
+
+
+def test_every_rep_is_checked_and_cleared_after_its_stamp(kernel):
+    """After the completion stamp, the word check reads the output back at L2 (128-bit ld.global.cg) and overwrites
+    it with 0s (128-bit stores), so no rep can leave its words for a later one."""
+    text = [unpredicated(t) for t in kernel]
+    after = text[stamp(kernel):]
+    loads = [k for k, t in enumerate(after) if re.match(r"LDG\.E\.128\.STRONG\.GPU", t)]
+    clears = [k for k, t in enumerate(after) if t.startswith("STG.E.NA.128") and re.search(r", RZ$", t)]
+    assert loads and clears and min(loads) < min(clears)
 
 
 def test_ptxas_reports_no_spills_in_the_allreduce_unit():

@@ -1,7 +1,8 @@
 """cdprobe_allreduce on the GPU: every row's output at every size has the (S, X) of the pattern's sum and passes the
-word check, a word corrupted at rest fails exactly the sizes that cover it in every row, an armed fault fails exactly
-one row and size, a mapping that is down stops every rank without waiting, two processes agree, the call needs no run
-and disturbs none, and the times are ordered and bounded.  Several ranks share one device where a test needs N > 1,
+word check, a word corrupted at rest fails exactly the sizes that cover it in every row and every rep, an armed fault
+(a word off by one, or a unit not stored) fails exactly one row and size at any reps, whatever an earlier call or an
+earlier handle left in the output, a mapping that is down stops every rank without waiting, two processes agree, the
+call needs no run and disturbs none, and the times are ordered and bounded, at N = 1 no faster than HBM allows.  Several ranks share one device where a test needs N > 1,
 with CTA counts that let their grids be resident together (every rank waits for every other at each rep)."""
 import json
 import subprocess
@@ -26,6 +27,17 @@ ERR_ARG, ERR_UNSUPPORTED, ERR_STATE, ERR_INTEGRITY = -2, -8, -9, -10
 U64_MAX = (1 << 64) - 1
 GIB = 1 << 30
 REF_MAX = 64 << 20  # sizes up to this get their (S, X) from the numpy reference; larger ones (N = 1) from the oracle
+# NVIDIA H100 SXM data sheet: 3.35 TB/s of HBM3, with test_timing_gpu.py's margin for lines still in the 50 MB L2.  At
+# N = 1 a one-shot rep of 1 GiB reads its input and writes its output through HBM: 2 GiB.
+HBM_DATASHEET_GBPS = 3350.0
+HBM_MARGIN = 1.10
+
+
+def assert_hbm_floor(ar, hbm_bytes, size=GIB):
+    """Rank 0's fastest rep at `size` moved at least `hbm_bytes` through HBM, so it took no less than they need."""
+    k = ar.sizes.index(size)
+    floor_ns = hbm_bytes / (HBM_MARGIN * HBM_DATASHEET_GBPS)
+    assert ar.ns_min[0][k] >= floor_ns, (ar.ns_min[0][k], floor_ns)
 
 
 def open_same(pkg, n, flags=0, nbytes=1 << 20, mode=MODE_SLICED):
@@ -81,6 +93,9 @@ def test_single_rank_every_size_clean(pkg, oracle, nbytes, path):
         ar2 = p.AllReduce(reps=3)
         assert (ar2.reps, ar2.call_seq) == (3, 2)
         assert_all_clean(ar2, oracle, nbytes)
+        if nbytes == GIB:
+            for r in (ar, ar2):
+                assert_hbm_floor(r, 2 * GIB)
 
 
 @pytest.mark.parametrize("mode", [MODE_SLICED, MODE_FULL, MODE_REACH], ids=["sliced", "full", "reach"])
@@ -97,6 +112,29 @@ def test_same_device_every_row_clean(pkg, oracle, n, mode):
         assert p.AllReduce(reps=2).call_seq == 2
 
 
+def test_a_dropped_unit_is_seen_whatever_the_output_held_before(pkg, oracle):
+    """Every rep of every call stores the same sums into the same words, so a unit a rep does not store would still
+    hold what an earlier rep, an LL call on the same handle, or a closed handle's output in the same process left
+    there.  The check clears the output after every rep, so the drop fails exactly its row, size and unit each time."""
+    n, nbytes = 3, (1 << 20) + 768
+    a = pkg.abi
+    bpp = pkg.plan(n, nbytes, MODE_SLICED).bytes_per_pair
+    sizes = ref.ladder(bpp)
+    expect = want(oracle, n, sizes)
+    fault = (1, 2, 700, True)  # in the one unit of size 2, below the LL's largest size
+    with open_same(pkg, n, nbytes=nbytes) as p:
+        assert_all_clean(p.AllReduce(reps=2), oracle, bpp)
+        ll = p.AllReduceLL(reps=2)
+        assert all(ll.status[r] == 0 for r in range(n)) and ll.sizes == sizes[:len(ll.sizes)] and len(ll.sizes) > 2
+        p.SetOption(a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(*fault))
+        check_fault(p.AllReduce(reps=2), n, sizes, expect, 2, fault)
+    with open_same(pkg, n, nbytes=nbytes) as p:  # the same config and seed: its scratch may reuse the freed one
+        p.SetOption(a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(*fault))
+        ar = p.AllReduce(reps=1)
+        assert ar.call_seq == 1
+        check_fault(ar, n, sizes, expect, 1, fault)
+
+
 @pytest.mark.parametrize("path", [0, 1, 2], ids=["tma", "ldst16", "ldst32"])
 def test_a_corrupt_word_fails_exactly_the_sizes_that_cover_it_in_every_row(pkg, oracle, path):
     n, nbytes = 3, (2 << 20) + 5 * 1024 + 256  # bytes_per_pair is not a whole number of 16 KiB granules
@@ -107,17 +145,18 @@ def test_a_corrupt_word_fails_exactly_the_sizes_that_cover_it_in_every_row(pkg, 
         assert bpp % 16384 != 0
         last_partial = bpp // 16384 * 16384 + 1000
         x, mask = 2, 1 << 17
+        reps = 2
         for o in (40, 200000, last_partial):
             w = o // 8
             p.Corrupt(x, w * 8, mask)
-            ar = p.AllReduce(reps=2)
+            ar = p.AllReduce(reps=reps)
             bits = sum(1 << k for k, s in enumerate(sizes) if s > 8 * w)
             expect = ref.expected_corrupted(SEED, n, tuple(sizes), x, w, mask)
             for r in range(n):
                 assert ar.measured[r] and ar.status[r] == ERR_INTEGRITY and ar.bad_sizes[r] == bits, (o, r)
                 for k, s in enumerate(sizes):
                     covered = s > 8 * w
-                    assert ar.bad_words[r][k] == (1 if covered else 0), (o, r, s)
+                    assert ar.bad_words[r][k] == (reps + 1 if covered else 0), (o, r, s)  # every rep, warm-up too
                     assert ar.first_bad[r][k] == (8 * w if covered else U64_MAX), (o, r, s)
                     assert (ar.sum[r][k], ar.xr[r][k]) == expect[k], (o, r, s)
                     assert 0 < ar.ns_min[r][k] <= ar.ns_max[r][k]  # the times are still reported
@@ -125,32 +164,58 @@ def test_a_corrupt_word_fails_exactly_the_sizes_that_cover_it_in_every_row(pkg, 
             assert_all_clean(p.AllReduce(reps=2), oracle, bpp)
 
 
+def check_fault(ar, n, sizes, expect, reps, fault):
+    """fault (rank, k, word, drop): timed rep 1 of size k at `rank` adds 1 to the word, or stores nothing of its unit,
+    which the check after that rep reads as 0s.  Every rep is checked, so the word check finds it at any reps; (S, X)
+    is the last timed rep's, so it shows the fault only when reps == 1.  Every other row and size is clean."""
+    rank, k, word, drop = fault
+    for r in range(n):
+        if r != rank:
+            assert_row_clean(ar, r, expect)
+            continue
+        assert ar.status[r] == ERR_INTEGRITY and ar.bad_sizes[r] == 1 << k, (reps, fault, ar.bad_sizes[r])
+        for q, s in enumerate(sizes):
+            ctx = (reps, fault, q)
+            assert 0 < ar.ns_min[r][q] <= ar.ns_median[r][q] <= ar.ns_max[r][q], ctx
+            if q != k:
+                assert ar.bad_words[r][q] == 0 and ar.first_bad[r][q] == U64_MAX, ctx
+                assert (ar.sum[r][q], ar.xr[r][q]) == expect[q], ctx
+                continue
+            unit = ref.unit_words(word, s)
+            assert ar.bad_words[r][q] == (len(unit) if drop else 1), (ctx, ar.bad_words[r][q])
+            assert ar.first_bad[r][q] == 8 * (unit[0] if drop else word), (ctx, ar.first_bad[r][q])
+            if reps > 1:
+                assert (ar.sum[r][q], ar.xr[r][q]) == expect[q], ctx
+            else:
+                out = ref.output_words(SEED, n, s // 8)
+                if drop:
+                    out[unit[0]:unit[-1] + 1] = 0
+                else:
+                    out[word] += 1
+                assert (ar.sum[r][q], ar.xr[r][q]) == ref.checksum(out), ctx
+
+
 def test_an_armed_fault_fails_exactly_one_row_and_size(pkg, oracle):
-    n, nbytes = 3, 1 << 20
+    n, nbytes = 3, (1 << 20) + 768  # bytes_per_pair 512 KiB + 384: the last size ends in a partial unit
     a = pkg.abi
     with open_same(pkg, n, nbytes=nbytes) as p:
         bpp = pkg.plan(n, nbytes, MODE_SLICED).bytes_per_pair
         sizes = ref.ladder(bpp)
+        assert sizes[-1] % 8192  # the last size ends in a partial unit
         expect = want(oracle, n, sizes)
-        rank, k, word = 1, 3, sizes[3] // 8 - 5
-        p.SetOption(a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(rank, k, word))
-        for reps in (2, 3, 1):
-            ar = p.AllReduce(reps=reps)
-            for r in range(n):
-                if r != rank:
-                    assert_row_clean(ar, r, expect)
-                    continue
-                assert ar.status[r] == ERR_INTEGRITY and ar.bad_sizes[r] == 1 << k, (reps, ar.bad_sizes[r])
-                for q in range(len(sizes)):
-                    found = reps == 1 and q == k  # a later clean rep overwrites the faulted output
-                    assert ar.bad_words[r][q] == (1 if found else 0), (reps, q)
-                    assert ar.first_bad[r][q] == (8 * word if found else U64_MAX), (reps, q)
-                    if q != k or reps > 1:
-                        assert (ar.sum[r][q], ar.xr[r][q]) == expect[q], (reps, q)
+        last = len(sizes) - 1
+        for fault in ((1, 3, sizes[3] // 8 - 5, False), (1, 3, sizes[3] // 8 - 5, True), (2, 0, 0, True),
+                      (0, last, sizes[last] // 8 - 1, True), (2, last, 3 * 1024 + 7, True)):
+            p.SetOption(a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(*fault))
+            for reps in (1, 2, 3):
+                check_fault(p.AllReduce(reps=reps), n, sizes, expect, reps, fault)
+            ar = p.AllReduce(reps=2)
         # arming that names no rank, size or word of the call is refused, and refusing changes nothing
         seq = ar.call_seq
         for bad in (a.allreduce_fault(n, 0, 0), a.allreduce_fault(0, len(sizes), 0),
-                    a.allreduce_fault(0, 0, sizes[0] // 8), (1 << 24) | 5, (1 << 32) | 5):
+                    a.allreduce_fault(0, 0, sizes[0] // 8), a.allreduce_fault(n, 0, 0, drop=True),
+                    a.allreduce_fault(0, 0, sizes[0] // 8, drop=True), (1 << 49) | a.allreduce_fault(0, 0, 0),
+                    (1 << 63) | a.allreduce_fault(0, 0, 0, drop=True), (1 << 24) | 5, (1 << 32) | 5):
             p.SetOption(a.OPT_ALLREDUCE_FAULT, bad)
             rc, t = p.allreduce_raw(2)
             assert rc == ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, hex(bad)

@@ -36,7 +36,9 @@ def test_the_fault_encoder_and_its_refusals(pkg):
     assert a.allreduce_ll_fault(2, 0, 5, 77) == (3 << 40) | (1 << 32) | (6 << 24) | 77
     assert a.allreduce_ll_fault(0, 1, 0, 2000, mode=1) == (1 << 48) | (1 << 40) | (2 << 32) | (1 << 24) | 2000
     assert a.allreduce_ll_fault(15, 14, 23, (1 << 24) - 1, 1) >> 49 == 0
-    for bad in (dict(mode=2), dict(mode=-1), dict(arg=1 << 24), dict(arg=-1), dict(sender=255), dict(receiver=-1),
+    assert a.allreduce_ll_fault(1, 1, 3, 500, mode=2) == (2 << 48) | (2 << 40) | (2 << 32) | (4 << 24) | 500
+    assert a.allreduce_ll_fault(254, 254, 254, (1 << 24) - 1, 2) >> 50 == 0
+    for bad in (dict(mode=3), dict(mode=-1), dict(arg=1 << 24), dict(arg=-1), dict(sender=255), dict(receiver=-1),
                 dict(k=255)):
         args = dict(sender=0, receiver=1, k=0, arg=0, mode=0)
         args.update(bad)
@@ -210,6 +212,15 @@ def test_the_packets_are_single_128_bit_system_scope_accesses(kernel):
     assert not any(t.startswith(("UBLKCP", "SYNCS.PHASECHK")) for t in kernel)
     assert not any(re.match(r"MEMBAR\.(SC|ALL)\.SYS", t) for t in kernel)
     assert any(t.startswith("LDG.E.64.STRONG.GPU") for t in kernel)  # the word check's ld.global.cg
+
+
+def test_the_word_check_clears_every_word_it_reads(kernel):
+    """After its ld.global.cg of an output word, the word check stores 0 over it, so the next size or call finds 0s
+    wherever it makes no store; then a fence, before the next size's opening barrier."""
+    loads = [k for k, t in enumerate(kernel) if t.startswith("LDG.E.64.STRONG.GPU")]
+    clears = [k for k, t in enumerate(kernel) if re.match(r"STG\.E\.64 .*, RZ$", t)]
+    assert loads and clears and any(k > min(loads) for k in clears)
+    assert any(t.startswith("MEMBAR.SC.GPU") for t in kernel[min(clears):])
 
 
 def test_ptxas_reports_no_spills_in_the_ll_unit():

@@ -1,8 +1,9 @@
 """cdprobe_allreduce_ll on the GPU: every row's output at every size of the LL ladder is the pattern's sum, word for
 word and in (S, X), and equals the one-shot's and the two-shot's on the same handle; tiny ladders, ladders cut at
 1 MiB, small and unequal grids (the agreed word partition); a word corrupted at rest fails exactly the sizes that
-cover it in every row; a corrupted packet fails only its receiver's row and size; a delayed sender stretches every
-rank's rep and leaves every row exact; a mapping that is down stops every rank without waiting; two processes with
+cover it in every row; a corrupted packet fails only its receiver's row and size; an output word a rank never stores
+in a size fails exactly that row and size, whatever an earlier size, a one-shot call or a closed handle left there; a
+delayed sender stretches every rank's rep and leaves every row exact; a mapping that is down stops every rank without waiting; two processes with
 unequal grids agree; repeated calls stay exact and disturb nothing; the times are ordered and bounded.  Several ranks
 share one device where a test needs N > 1, with CTA counts that let their grids be resident together (every rank
 waits for every other's packets).  No test drives a kernel past its deadline."""
@@ -53,11 +54,13 @@ def src(rank, n_words):
     return w
 
 
-def check(ar, n, bpp, reps, corrupt=None, fault=None):
+def check(ar, n, bpp, reps, corrupt=None, fault=None, unstored=None):
     """Every row at every size, from the words at rest: corrupt {(rank, word): mask} is xored into the sources, and
     fault (sender, receiver, k, word) xors the data of that packet, the sender's salted input, with 1 in timed rep 1
-    only, which moves the receiver's output word by +1 or -1.  The word check and (S, X) are the last timed rep's;
-    bad_sizes also counts every earlier rep's (S, X)."""
+    only, which moves the receiver's output word by +1 or -1.  unstored (rank, k, word), the mode-2 fault: that rank
+    makes no store to the word in any rep of size k, so the word check after the size reads 0 there (the output
+    starts zeroed and every check clears it), while (S, X), folded from the sums, stays clean.  The word check and
+    (S, X) are the last timed rep's; bad_sizes also counts every earlier rep's (S, X)."""
     corrupt = corrupt or {}
     sizes = ref.ladder(bpp)
     assert ar.sizes == sizes and ar.reps == reps and ar.n == n and ar.path == PATH_LL
@@ -77,7 +80,11 @@ def check(ar, n, bpp, reps, corrupt=None, fault=None):
                     v = (int(src(fault[0], W)[fault[3]]) + ref.salt(SEED, fault[0], ref.flag(ar.call_seq, k, 1)))
                     last = last.copy()
                     last[fault[3]] = np.uint64((int(last[fault[3]]) + ((v ^ 1) - v)) % (1 << 64))
-            bad = np.flatnonzero(last != clean[:s // 8])
+            seen = last
+            if unstored is not None and (r, k) == unstored[:2]:
+                seen = last.copy()
+                seen[unstored[2]] = 0
+            bad = np.flatnonzero(seen != clean[:s // 8])
             if len(bad):
                 bits |= 1 << k
             ctx = (r, s, fault)
@@ -158,7 +165,15 @@ def test_grids_and_unequal_grids_split_the_words_alike(pkg, grid):
         f = (2, 0, len(sizes) - 1, bpp // 8 - 1)
         p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, a.allreduce_ll_fault(*f))
         check(p.AllReduceLL(reps=1), n, bpp, 1, fault=f)
+        # an output word left unstored: word 0 of size 0, a word below the previous size at k >= 1 (which that size
+        # stored and its check cleared), the last word of the largest LL size
+        for u in ((0, 0, 0), (2, 3, sizes[2] // 8 - 1), (1, len(sizes) - 1, sizes[-1] // 8 - 1)):
+            p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, a.allreduce_ll_fault(u[0], u[0], u[1], u[2], mode=2))
+            for reps in (1, 3):
+                ar = check(p.AllReduceLL(reps=reps), n, bpp, reps, unstored=u)
+                assert ar.bad_words[u[0]][u[1]] == 1 and ar.first_bad[u[0]][u[1]] == 8 * u[2], (u, reps)
         p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, 0)
+        check(p.AllReduceLL(reps=2), n, bpp, 2)
 
 
 def test_a_corrupt_word_fails_exactly_the_sizes_that_cover_it_in_every_row(pkg):
@@ -189,6 +204,25 @@ def test_a_corrupted_packet_fails_only_its_receiver_and_size(pkg):
         check(p.AllReduceLL(reps=2), n, bpp, 2)
 
 
+def test_an_unstored_word_is_seen_whatever_the_output_held_before(pkg):
+    """Every rep, size and call stores the same sums into the same words, so a word the LL leaves unstored would still
+    hold what a one-shot call on the same handle, or a closed handle's output in the same process, left there.  The
+    output is zeroed at the start of every call, so the unstored word fails exactly its row and size each time."""
+    a = pkg.abi
+    n, bpp = 3, EDGE_BPP
+    sizes = ref.ladder(bpp)
+    u = (1, 4, sizes[3] // 8 - 2)  # below size 3, so size 3 also stored it in this call
+    with open_bpp(pkg, n, bpp) as p:
+        one = p.AllReduce(reps=2)
+        assert all(one.status[r] == 0 for r in range(n)) and one.sizes[:len(sizes)] == sizes
+        p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, a.allreduce_ll_fault(u[0], u[0], u[1], u[2], mode=2))
+        check(p.AllReduceLL(reps=2), n, bpp, 2, unstored=u)
+    with open_bpp(pkg, n, bpp) as p:  # the same config and seed: its scratch may reuse the freed one
+        p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, a.allreduce_ll_fault(u[0], u[0], u[1], u[2], mode=2))
+        ar = check(p.AllReduceLL(reps=1), n, bpp, 1, unstored=u)
+        assert ar.call_seq == 1 and ar.bad_words[u[0]][u[1]] == 1
+
+
 def test_a_delayed_sender_stretches_every_rank_and_every_row_stays_exact(pkg):
     """The sender waits 2 ms before its first push of timed rep 1 of size k.  Its own rep 1 spans the wait; every
     other rank's rep 1 ends only after the sender's packets arrive, and starts when its rep 0 ended, at most a few
@@ -208,6 +242,9 @@ def test_a_delayed_sender_stretches_every_rank_and_every_row_stays_exact(pkg):
         p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, 0)
 
 
+NAMES_NOTHING = "the armed LL all-reduce fault names no packet, size or delay of this call"
+
+
 def test_an_armed_fault_that_names_nothing_is_refused(pkg):
     a = pkg.abi
     n = 3
@@ -218,11 +255,14 @@ def test_an_armed_fault_that_names_nothing_is_refused(pkg):
         for bad in (a.allreduce_ll_fault(n, 0, 0, 0), a.allreduce_ll_fault(0, n, 0, 0),
                     a.allreduce_ll_fault(0, 1, len(sizes), 0), a.allreduce_ll_fault(0, 1, 0, sizes[0] // 8),
                     a.allreduce_ll_fault(1, 1, 0, 0), a.allreduce_ll_fault(0, 1, 0, 10_000_000, mode=1),
-                    (2 << 48) | a.allreduce_ll_fault(0, 1, 0, 0), (1 << 63) | a.allreduce_ll_fault(0, 1, 0, 0),
-                    (1 << 24) | 5):
+                    (2 << 48) | a.allreduce_ll_fault(0, 1, 0, 0), (3 << 48) | a.allreduce_ll_fault(0, 0, 0, 0),
+                    (1 << 63) | a.allreduce_ll_fault(0, 1, 0, 0), a.allreduce_ll_fault(2, 0, len(sizes) - 1, 5, mode=2),
+                    a.allreduce_ll_fault(1, 1, 0, sizes[0] // 8, mode=2), a.allreduce_ll_fault(n, n, 0, 0, mode=2),
+                    a.allreduce_ll_fault(2, 2, len(sizes), 0, mode=2), (1 << 24) | 5):
             p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, bad)
             rc, t = p.allreduce_ll_raw(2)
             assert rc == ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, hex(bad)
+            assert p._lib.cdprobe_last_error().decode() == NAMES_NOTHING, hex(bad)
         p.SetOption(a.OPT_ALLREDUCE_LL_FAULT, 0)
         ar2 = check(p.AllReduceLL(reps=2), n, bpp, 2)
         assert ar2.call_seq == ar.call_seq + 1

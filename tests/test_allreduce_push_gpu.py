@@ -23,6 +23,7 @@ import allreduce_push_ref as ref
 import allreduce_ref
 import word_ref
 from conftest import ROOT
+from test_allreduce_gpu import assert_hbm_floor
 
 pytestmark = pytest.mark.gpu
 
@@ -138,7 +139,9 @@ def set_path(pkg, p, path):
 
 @pytest.mark.parametrize("path", PATHS)
 def test_single_rank_every_size_of_a_1_gib_ladder_clean(pkg, oracle, path):
-    """At N = 1 the rank reduces its input into its own zeroed area, and the all-gather has no targets."""
+    """At N = 1 the rank reduces its input into its own zeroed area, and the all-gather has no targets.  A 1 GiB rep
+    reads its 1 GiB input, and each bulk reduction (or red.global) makes the memory system read and write the area's
+    1 GiB: 3 GiB through HBM (allreduce_push_kernel at n == 1: reduce_tma / reduce_ldst, then no ar_units pass)."""
     with pkg.Open(pkg.Config(ordinals=[0], bytes=GIB, timeout_ms=60000)) as p:
         set_path(pkg, p, path)
         ar = p.AllReducePush(reps=2)
@@ -147,6 +150,7 @@ def test_single_rank_every_size_of_a_1_gib_ladder_clean(pkg, oracle, path):
         assert [(s, x) for s, x in zip(ar.sum[0], ar.xr[0])] == want(oracle, 1, ar.sizes)
         assert ar.bad_words[0] == [0] * len(ar.sizes) and ar.first_bad[0] == [U64_MAX] * len(ar.sizes)
         assert_fits_in_call(ar)
+        assert_hbm_floor(ar, 3 * GIB)
 
 
 @pytest.mark.parametrize("path", PATHS)

@@ -20,6 +20,7 @@ import allreduce_ref
 import allreduce_ring_ref as ref
 import word_ref
 from conftest import ROOT
+from test_allreduce_gpu import assert_hbm_floor
 
 pytestmark = pytest.mark.gpu
 
@@ -152,7 +153,9 @@ def want(oracle, n, sizes):
 
 @pytest.mark.parametrize("nbytes", [4 << 20, GIB], ids=["4MiB", "1GiB"])
 def test_single_rank_every_size_clean(pkg, oracle, nbytes):
-    """At N = 1 there are no steps: the rank stores its own prefix into its output, and the check runs as usual."""
+    """At N = 1 there are no steps: the rank stores its own prefix into its output, and the check runs as usual.  So
+    a 1 GiB rep reads 1 GiB and stores 1 GiB through HBM (ring_rep at n == 1: one step, s = 0, that neither receives
+    nor pushes), and takes no less than 2 GiB need at the data sheet's bandwidth."""
     with pkg.Open(pkg.Config(ordinals=[0], bytes=nbytes, timeout_ms=60000)) as p:
         ar = p.AllReduceRing(reps=2)
         assert ar.sizes == allreduce_ref.ladder(nbytes) and ar.path == PATH_RING and ar.call_seq == 1
@@ -161,6 +164,8 @@ def test_single_rank_every_size_clean(pkg, oracle, nbytes):
         assert [(s, x) for s, x in zip(ar.sum[0], ar.xr[0])] == expect
         assert ar.bad_words[0] == [0] * len(ar.sizes) and ar.first_bad[0] == [U64_MAX] * len(ar.sizes)
         assert_fits_in_call(ar)
+        if nbytes == GIB:
+            assert_hbm_floor(ar, 2 * GIB)
 
 
 @pytest.mark.parametrize("mode", [MODE_SLICED, MODE_FULL, MODE_REACH], ids=["sliced", "full", "reach"])

@@ -19,6 +19,7 @@ import allreduce_ref
 import allreduce_twoshot_ref as ref
 import word_ref
 from conftest import ROOT
+from test_allreduce_gpu import assert_hbm_floor
 
 pytestmark = pytest.mark.gpu
 
@@ -134,7 +135,8 @@ def assert_all_clean(ar, oracle, bpp):
 @pytest.mark.parametrize("path", PATHS, ids=["tma", "ldst16", "ldst32"])
 @pytest.mark.parametrize("nbytes", [4 << 20, GIB], ids=["4MiB", "1GiB"])
 def test_single_rank_every_size_clean(pkg, oracle, nbytes, path):
-    """At N = 1 the rank owns every unit and its output is a copy of its own prefix."""
+    """At N = 1 the rank owns every unit and its output is a copy of its own prefix: a 1 GiB rep reads 1 GiB and
+    stores 1 GiB through HBM, so it takes no less than 2 GiB need at the data sheet's bandwidth."""
     with pkg.Open(pkg.Config(ordinals=[0], bytes=nbytes, timeout_ms=20000)) as p:
         p.SetOption(pkg.abi.OPT_PATH, path)
         ar = p.AllReduceTwoShot()
@@ -143,6 +145,9 @@ def test_single_rank_every_size_clean(pkg, oracle, nbytes, path):
         ar2 = p.AllReduceTwoShot(reps=3)
         assert (ar2.reps, ar2.call_seq) == (3, 2)
         assert_all_clean(ar2, oracle, nbytes)
+        if nbytes == GIB:
+            for r in (ar, ar2):
+                assert_hbm_floor(r, 2 * GIB)
 
 
 @pytest.mark.parametrize("mode", [MODE_SLICED, MODE_FULL, MODE_REACH], ids=["sliced", "full", "reach"])

@@ -167,8 +167,9 @@ def test_phase_table_idles_the_jobs_of_an_unmapped_pair(pkg, oracle):
 
 # ---- the all-reduce and the all-to-all -------------------------------------------------------------------------
 def allreduce_direct(n, sizes, corrupt, fault=None, reps=1):
-    """The all-reduce restated over whole word arrays (numpy): per size, (S, X) of the output of the last rep, its bad
-    words and first bad offset, given the corruptions at rest {(rank, word): mask} and a fault (k, word) of this row."""
+    """The all-reduce restated over whole word arrays (numpy): per size, (S, X) of the output of the last rep, and the
+    bad words and first bad offset over every rep (the warm-up, then `reps` timed reps), given the corruptions at rest
+    {(rank, word): mask} and a fault (k, word, drop) of this row in timed rep 1: the word + 1, or its 8 KiB unit 0s."""
     W = sizes[-1] // 8
     src = [ref.src_words(SEED, j, 0, W) for j in range(n)]
     clean = sum(src[1:], src[0].copy())
@@ -178,11 +179,16 @@ def allreduce_direct(n, sizes, corrupt, fault=None, reps=1):
     at_rest = sum(src[1:], src[0].copy())
     out = []
     for k, s in enumerate(sizes):
-        words = at_rest[:s // 8].copy()
-        if fault is not None and fault[0] == k and reps == 1:
-            words[fault[1]] += np.uint64(1)
-        bad = np.flatnonzero(words != clean[:s // 8])
-        out.append((allreduce_ref.checksum(words), len(bad), 8 * int(bad[0]) if len(bad) else ref.U64_MAX))
+        outs = [at_rest[:s // 8].copy() for _ in range(reps + 1)]
+        if fault is not None and fault[0] == k:
+            if fault[2]:
+                outs[1][fault[1] // 1024 * 1024:(fault[1] // 1024 + 1) * 1024] = 0
+            else:
+                outs[1][fault[1]] += np.uint64(1)
+        bad = [np.flatnonzero(w != clean[:s // 8]) for w in outs]
+        first = min((int(b[0]) for b in bad if len(b)), default=None)
+        out.append((allreduce_ref.checksum(outs[-1]), sum(len(b) for b in bad),
+                    ref.U64_MAX if first is None else 8 * first))
     return out
 
 
@@ -199,7 +205,7 @@ def test_allreduce_under_one_corruption_equals_the_reference(oracle):
             row = got["rows"][g]
             assert row["sx"] == want and row["bad_sizes"] == bits, (rank, word, g)
             assert row["status"] == (hm.ERR_INTEGRITY if bits else 0)
-            assert row["bad_words"] == [(bits >> k) & 1 for k in range(len(sizes))]
+            assert row["bad_words"] == [2 * ((bits >> k) & 1) for k in range(len(sizes))]  # the warm-up and rep 1
             assert row["first_bad"] == [8 * word if (bits >> k) & 1 else ref.U64_MAX for k in range(len(sizes))]
         m.corrupt_word(rank, word, mask)  # restore
         assert m.allreduce(1)["rows"][0]["sx"] == list(allreduce_ref.expected(SEED, n, tuple(sizes)))
@@ -226,16 +232,20 @@ def test_allreduce_under_several_corruptions_and_a_fault_equals_a_direct_recompu
         assert [(sx, b, f) for sx, b, f in zip(got[g]["sx"], got[g]["bad_words"], got[g]["first_bad"])] == want, g
     # the cancelled word is clean: a prefix ending just past it has exactly the bad words of the others
     k = next(k for k, s in enumerate(sizes) if s // 8 > c)
-    assert want[k][1] == len({w for (r, w) in corrupt if w < min(sizes[k] // 8, m.W)} - {c})
-    # an armed fault on row 1, size 2, on a corrupted word: timed rep 1 adds 1 to the corrupted sum
-    fk = 2
-    m.arm_measure(m.ar_fault, 0, (2 << 32) | ((fk + 1) << 24) | 5)
-    for reps in (1, 3):
-        got = m.allreduce(reps)["rows"]
-        for g in range(n):
-            want = allreduce_direct(n, sizes, corrupt, (fk, 5) if g == 1 else None, reps)
-            assert [(sx, b, f) for sx, b, f in zip(got[g]["sx"], got[g]["bad_words"], got[g]["first_bad"])] == want
-        assert got[1]["bad_sizes"] == got[0]["bad_sizes"] | 1 << fk  # size 2 fails even when its last rep is clean
+    assert want[k][1] == 2 * len({w for (r, w) in corrupt if w < min(sizes[k] // 8, m.W)} - {c})  # warm-up, rep 1
+    # an armed fault on row 1, size 2, on a corrupted word: timed rep 1 adds 1 to the corrupted sum, or (drop) stores
+    # nothing of its unit; then a drop on row 2 in the last, partial unit of the last size
+    fk, last = 2, len(sizes) - 1
+    for g0, k0, w0, drop in ((1, fk, 5, False), (1, fk, 5, True), (2, last, m.W - 1, True)):
+        m.arm_measure(m.ar_fault, 0, (int(drop) << 48) | ((g0 + 1) << 32) | ((k0 + 1) << 24) | w0)
+        for reps in (1, 3):
+            got = m.allreduce(reps)["rows"]
+            for g in range(n):
+                want = allreduce_direct(n, sizes, corrupt, (k0, w0, drop) if g == g0 else None, reps)
+                assert [(sx, b, f) for sx, b, f in zip(got[g]["sx"], got[g]["bad_words"], got[g]["first_bad"])] == \
+                    want, (g0, k0, drop, reps, g)
+            # the size fails even when its last rep is clean
+            assert got[g0]["bad_sizes"] == got[(g0 + 1) % n]["bad_sizes"] | 1 << k0
 
 
 def test_allreduce_skip_rule_refusals_and_counters(oracle):
@@ -244,7 +254,8 @@ def test_allreduce_skip_rule_refusals_and_counters(oracle):
     sizes = bwcurve_ref.ladder(m.bpp)
     assert m.allreduce(2)["call_seq"] == 1
     for bad in ((4 << 32) | (1 << 24), (1 << 24) | 5, (1 << 32) | ((len(sizes) + 1) << 24),
-                (1 << 32) | (1 << 24) | sizes[0] // 8, 1 << 32):
+                (1 << 32) | (1 << 24) | sizes[0] // 8, 1 << 32, (1 << 49) | (1 << 32) | (1 << 24),
+                (1 << 63) | (1 << 48) | (1 << 32) | (1 << 24)):
         m.arm_measure(m.ar_fault, 0, bad)
         assert m.allreduce(2) is None, hex(bad)
     assert m.ar_calls == 1

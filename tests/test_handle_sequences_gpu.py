@@ -332,13 +332,14 @@ def edge_word(rng, size):
 
 
 def ladder_fault(rng, m, name, rank, peer):
-    """A valid OPT_ALLREDUCE_FAULT (on `rank`) or OPT_ALLTOALL_FAULT (cell rank -> peer) value at an edge word of a
-    size of the ladder: the last size or a random one."""
+    """A valid OPT_ALLREDUCE_FAULT (on `rank`; half of them drop the word's unit instead of adding 1) or
+    OPT_ALLTOALL_FAULT (cell rank -> peer) value at an edge word of a size of the ladder: the last size or a random
+    one."""
     sizes = bwcurve_ref.ladder(m.bpp)
     k = rng.choice([len(sizes) - 1, rng.randrange(len(sizes))])
     word = edge_word(rng, sizes[k])
     if name == "OPT_ALLREDUCE_FAULT":
-        return ((rank + 1) << 32) | ((k + 1) << 24) | word
+        return (rng.randrange(2) << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
     return ((rank + 1) << 40) | ((peer + 1) << 32) | ((k + 1) << 24) | word
 
 

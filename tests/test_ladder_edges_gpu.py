@@ -7,12 +7,14 @@ word for word against the numpy references (bwcurve_ref, allreduce_ref, alltoall
   expected sums with no whole granule;
 - grids of 1, 2, 3 and 7 CTAs per rank, the full grid at N = 1, and unequal per-rank grids (OPT_CTAS_RANK), which
   change which warp walks which unit;
-- faults placed at the edges: the all-reduce's at word 0 of size 0 and at the last word of the last, partial unit;
+- faults placed at the edges: the all-reduce's at word 0 of size 0 and at the last word of the last, partial unit,
+  each as a word off by one and as a unit not stored;
   the all-to-all's at the last word of a partial unit, at a word of the last warp of the grid and on the diagonal
   block; and a corrupted source word in a partial unit, which fails exactly the bwcurve cell and sizes that read it,
   every all-reduce row at those sizes, and no all-to-all cell.
 
-Every call uses one timed rep, so the faulted rep is the one folded into (S, X).  Several ranks share GPU 0 with at
+Every call uses one timed rep, so the faulted rep is the one folded into (S, X); the all-reduce's word check runs
+after the warm-up and after the timed rep, and its bad words are summed over both.  Several ranks share GPU 0 with at
 most 8 CTAs each, so every rank's grid stays resident."""
 import functools
 
@@ -101,7 +103,8 @@ def check_bwcurve(bw, src, n, bpp, diag, corrupt=None):
 
 def check_allreduce(ar, src, n, bpp, corrupt=None, fault=None):
     """Every row at every size holds the sum of the words at rest; a word is bad when that differs from the clean
-    sum.  fault (rank, k, word): timed rep 1 of size k on that rank adds 1 to the word."""
+    sum.  fault (rank, k, word, drop): timed rep 1 of size k on that rank adds 1 to the word, or (drop) stores
+    nothing of its 8 KiB unit, which then reads as 0s.  The warm-up and the timed rep are both checked."""
     corrupt = corrupt or {}
     sizes = bwcurve_ref.ladder(bpp)
     assert ar.sizes == sizes and ar.reps == 1
@@ -111,15 +114,21 @@ def check_allreduce(ar, src, n, bpp, corrupt=None, fault=None):
     for r in range(n):
         bits = 0
         for k, s in enumerate(sizes):
-            words = at_rest[:s // 8].copy()
+            warm = at_rest[:s // 8]
+            words = warm.copy()  # timed rep 1's output
             if fault is not None and (r, k) == fault[:2]:
-                words[fault[2]] += np.uint64(1)
-            bad = np.flatnonzero(words != clean[:s // 8])
+                if len(fault) > 3 and fault[3]:
+                    unit = allreduce_ref.unit_words(fault[2], s)
+                    words[unit[0]:unit[-1] + 1] = 0
+                else:
+                    words[fault[2]] += np.uint64(1)
+            bad = [np.flatnonzero(w != clean[:s // 8]) for w in (warm, words)]
             ctx = (r, s, fault)
             assert (ar.sum[r][k], ar.xr[r][k]) == allreduce_ref.checksum(words), ctx
-            assert ar.bad_words[r][k] == len(bad), (ctx, ar.bad_words[r][k])
-            assert ar.first_bad[r][k] == (8 * int(bad[0]) if len(bad) else U64_MAX), (ctx, ar.first_bad[r][k])
-            if len(bad):
+            assert ar.bad_words[r][k] == sum(len(b) for b in bad), (ctx, ar.bad_words[r][k])
+            first = min((int(b[0]) for b in bad if len(b)), default=None)
+            assert ar.first_bad[r][k] == (U64_MAX if first is None else 8 * first), (ctx, ar.first_bad[r][k])
+            if first is not None:
                 bits |= 1 << k
         assert ar.measured[r] and ar.bad_sizes[r] == bits, (r, ar.bad_sizes[r], bits)
         assert ar.status[r] == (ERR_INTEGRITY if bits else 0), r
@@ -228,8 +237,9 @@ def test_grids_and_faults_at_the_edges(pkg, src, n, grid):
         for path in PATHS:
             p.SetOption(a.OPT_PATH, path)
             check_bwcurve(p.BwCurve(reps=1), src, n, bpp, diag)
-            # the all-reduce: word 0 of size 0, and the last word of the last, partial unit of the last size
-            for fault in ((n - 1, 0, 0), (0, last, W - 1)):
+            # the all-reduce: word 0 of size 0, and the last word of the last, partial unit of the last size, each off
+            # by one and as its unit not stored (size 0's half unit, the last size's 384-byte unit)
+            for fault in ((n - 1, 0, 0, False), (0, last, W - 1, False), (n - 1, 0, 0, True), (0, last, W - 1, True)):
                 p.SetOption(a.OPT_ALLREDUCE_FAULT, a.allreduce_fault(*fault))
                 check_allreduce(p.AllReduce(reps=1), src, n, bpp, fault=fault)
             p.SetOption(a.OPT_ALLREDUCE_FAULT, 0)
