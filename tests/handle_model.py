@@ -3,12 +3,15 @@
 A daemon keeps one handle for days and interleaves runs, option changes, remaps, fault injection and the on-demand
 measurements on it.  `HandleModel` follows the same calls and says, from the pattern spec alone, what each one must
 return: the expected values come from the CPU oracle (oracle/oracle.py), tests/word_ref.py, tests/latency_ref.py,
-tests/bwcurve_ref.py, tests/allreduce_ref.py and tests/alltoall_ref.py, never from the library.  It tracks:
+tests/bwcurve_ref.py, tests/allreduce_ref.py, the all-reduce protocol references (allreduce_twoshot_ref,
+allreduce_ll_ref, allreduce_ring_ref, allreduce_push_ref), tests/alltoall_ref.py and tests/memcpy_ref.py, never from
+the library.  It tracks:
 
-- the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, allreduce and alltoall (a refused call
-  advances none);
-- the armed all-reduce and all-to-all faults of each process's handle, and which pairs were unmapped when the
-  all-to-all's exchange area was built;
+- the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, the five all-reduces (one-shot, two-shot, LL,
+  ring, push), alltoall and memcpy (a refused call advances none);
+- the armed fault of each of those ladder measurements in each process's handle; which pairs were unmapped when the
+  exchange area (shared by the all-to-all and memcpy, built by whichever is called first) was built, and the same for
+  the two-shot's gather area and the LL, ring and push areas;
 - the options in force: path, CTAs per rank, verify CTAs, the schedule flags, warm-up mode;
 - the phase table each rank must walk (cdprobe_schedule with the current options, with the jobs of an unmapped pair
   idled as the library's schedule does);
@@ -31,10 +34,15 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
+import allreduce_ll_ref
+import allreduce_push_ref
 import allreduce_ref
+import allreduce_ring_ref
+import allreduce_twoshot_ref
 import alltoall_ref
 import bwcurve_ref
 import latency_ref
+import memcpy_ref
 import word_ref
 
 M64 = (1 << 64) - 1
@@ -98,8 +106,9 @@ class HandleModel:
     returns an abi.ScheduleT (cdprobe_schedule)."""
 
     def __init__(self, oracle, schedule, n: int, nbytes: int, sm_count: int, ctas: int = 0, local=None,
-                 flags: int = 0, seed: int = SEED, mode: int = 1, ops: int = 3):
+                 flags: int = 0, seed: int = SEED, mode: int = 1, ops: int = 3, timeout_ms: int = 20000):
         self.oracle, self._schedule = oracle, schedule
+        self.timeout_ms = timeout_ms
         self.n, self.nbytes, self.mode, self.ops, self.seed = n, nbytes, mode, ops, seed
         self.local = list(range(n)) if local is None else list(local)
         pl = oracle.plan(n, nbytes, mode, n == 1)
@@ -117,13 +126,23 @@ class HandleModel:
         self.warm_mode = 1
         self.runs = 0                              # cdprobe_run calls that returned
         self.run_seq = 0                           # of the last run; 0: none yet
-        self.pp_calls = self.at_calls = self.bw_calls = self.ar_calls = self.a2a_calls = 0
-        # CDPROBE_OPT_ALLREDUCE_FAULT / CDPROBE_OPT_ALLTOALL_FAULT value of each process's handle (absent: disarmed)
+        self.pp_calls = self.at_calls = self.bw_calls = self.a2a_calls = self.mc_calls = 0
+        # the all-reduces' calls: one-shot, two-shot, LL, ring, push
+        self.ar_calls = self.ts_calls = self.ll_calls = self.ring_calls = self.push_calls = 0
+        # the armed fault option of each measurement in each process's handle, {process: value} (absent: disarmed):
+        # CDPROBE_OPT_ALLREDUCE_FAULT, _ALLREDUCE_{TWOSHOT,LL,RING,PUSH}_FAULT, _ALLTOALL_FAULT, _MEMCPY_FAULT
         self.ar_fault: Dict[int, int] = {}
+        self.ts_fault: Dict[int, int] = {}
+        self.ll_fault: Dict[int, int] = {}
+        self.ring_fault: Dict[int, int] = {}
+        self.push_fault: Dict[int, int] = {}
         self.a2a_fault: Dict[int, int] = {}
-        # the pairs unmapped when the first all-to-all built its exchange area (None: not built yet); the area is mapped
-        # only where the probe mapping was up then, and remaps do not map it later
+        self.mc_fault: Dict[int, int] = {}
+        # the pairs unmapped when the first all-to-all or memcpy built the exchange area they share (None: not built
+        # yet); the area is mapped only where the probe mapping was up then, and remaps do not map it later
         self.area_down: Optional[frozenset] = None
+        # the same for the gather, LL, ring and push areas, each built by its own all-reduce's first call
+        self.ar_area_down: Dict[str, Optional[frozenset]] = {"ts": None, "ll": None, "ring": None, "push": None}
         self.corrupt: Dict[Tuple[int, int], int] = {}      # (rank, word) -> mask, at rest
         # armed landing fault of each process's handle (one per handle): {process: (issuer, target, faults)}
         self.fault: Dict[int, Tuple[int, int, Tuple[Tuple[int, int], ...]]] = {}
@@ -303,27 +322,51 @@ class HandleModel:
         """Word w of the clean all-reduce output: the sum of word w of every rank's pattern."""
         return sum(src_word(self.seed, j, w) for j in range(self.n)) & M64
 
-    def allreduce(self, reps: int) -> Optional[dict]:
-        """What cdprobe_allreduce with `reps` timed reps must return: {"call_seq", "sizes", "rows": {local rank: {...}}},
-        or None when some process's armed fault names no rank, size or word of the ladder (CDPROBE_ERR_ARG; nothing
-        advances).  Any unmapped pair stops every rank, with the status of the first down cell, and call_seq still
-        advances.  Otherwise output word w is the sum of word w of every source buffer as it is at rest (slice 0 only),
-        a word is bad when that differs from the clean sum, and an armed fault acts in timed rep 1 of its size on its
-        rank: it adds 1 to its word, or (drop, bit 48) leaves its 8 KiB unit unstored, which the check after the rep
-        reads as 0s.  Every rep, warm-up included, is checked and cleared, so bad_words and first_bad cover every rep
-        and see the fault at any reps; the reported (S, X) is the last timed rep's, so it shows the fault when reps is
-        1, and the size fails at any reps since every rep's (S, X) is checked."""
-        sizes = bwcurve_ref.ladder(self.bpp)
-        faults = {}
-        for proc, v in self.ar_fault.items():
-            fr, fk, fw = (v >> 32) & 0xFFFF, (v >> 24) & 0xFF, v & 0xFFFFFF
-            if v >> 49 or fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+    def src_at_rest(self, rank: int, lo: int, hi: int) -> np.ndarray:
+        """Words [lo, hi) of rank's source buffer as they are at rest."""
+        w = word_ref.src_words(self.seed, rank, lo, hi - lo)
+        for k, m in self.corruptions_of(rank).items():
+            if lo <= k < hi:
+                w[k - lo] ^= np.uint64(m)
+        return w
+
+    def _ar_set(self, words: Dict[int, Tuple[int, int]], lo: int, hi: int, fn) -> None:
+        """Words [lo, hi) of one rep's all-reduce output {word: (clean, value)} (a word absent holds its clean sum)
+        become fn(word, value) mod 2^64."""
+        clean = sum(word_ref.src_words(self.seed, j, lo, hi - lo) for j in range(self.n))
+        for i, w in enumerate(range(lo, hi)):
+            c, v = words.get(w, (int(clean[i]),) * 2)
+            words[w] = (c, fn(w, v) & M64)
+
+    def _allreduce(self, name: str, reps: int, sizes: List[int], decode, effect, every_rep: bool = True):
+        """One call of an all-reduce, on the rules they share.  name: the prefix of its armed faults ({process: value},
+        `<name>_fault`) and its counter (`<name>_calls`); it has a shared area when ar_area_down has the name.
+        decode(value, sizes) is the call's verdict on an armed value: None refuses it (CDPROBE_ERR_ARG, nothing
+        advances), else a tuple whose first field is the rank in whose process it acts and whose second is its size.
+        effect(words, unstored, row, size, fault) applies the fault to that row's output of timed rep 1 of the size
+        ({word: (clean, value)}), or names output words the row never stores in the size (`unstored`).
+
+        The area is built by the first call that is not refused, mapped only where the probe mapping was up then.  Any
+        unmapped pair, or a pair down when the area was built, stops every rank, and call_seq still advances.  Otherwise
+        output word w is the sum of word w of every source buffer as it is at rest (slice 0 only), and a word is bad
+        when it differs from the clean sum.  every_rep: every rep, warm-up included, is checked and cleared, so
+        bad_words and first_bad cover every rep; else (the LL) only the last rep of a size is.  The reported (S, X) is
+        the last timed rep's, so it shows a fault of timed rep 1 when reps is 1, and a size fails when any rep's (S, X)
+        or any checked word is wrong."""
+        faults = []
+        for proc, v in getattr(self, name + "_fault").items():
+            f = decode(v, sizes)
+            if f is None:
                 return None
-            if self.process_of(fr - 1) == proc:
-                faults[(fr - 1, fk - 1)] = (fw, bool(v >> 48))
-        self.ar_calls += 1
-        out = dict(call_seq=self.ar_calls, sizes=sizes, rows={})
-        if self.unmapped:
+            if self.process_of(f[0]) == proc:
+                faults.append(f)
+        faults.sort(key=lambda f: f[-1])  # the push's all-gather fault (mode 3) acts after the contributions
+        if name in self.ar_area_down and self.ar_area_down[name] is None:
+            self.ar_area_down[name] = frozenset(self.unmapped)
+        seq = getattr(self, name + "_calls") + 1
+        setattr(self, name + "_calls", seq)
+        out = dict(call_seq=seq, sizes=sizes, rows={})
+        if self.unmapped or self.ar_area_down.get(name):
             for g in self.local:
                 out["rows"][g] = dict(measured=False, status=ERR_STATE)
             return out
@@ -342,27 +385,258 @@ class HandleModel:
             row = dict(measured=True, bad_sizes=0, sx=[], bad_words=[], first_bad=[])
             for k, s in enumerate(sizes):
                 nw = s // 8
-                rep1 = dict(at_rest)
-                fw, drop = faults.get((g, k), (None, False))
-                if fw is not None and drop:
-                    for w in allreduce_ref.unit_words(fw, s):
-                        rep1[w] = (at_rest.get(w, (self.ar_word(w),))[0], 0)
-                elif fw is not None:
-                    old, cur = at_rest.get(fw, (self.ar_word(fw),) * 2)
-                    rep1[fw] = (old, (cur + 1) & M64)
+                rep1, unstored = dict(at_rest), set()
+                for f in faults:
+                    if f[1] == k:
+                        effect(rep1, unstored, g, s, f)
                 last = rep1 if reps == 1 else at_rest
-                bad = sorted(w for w, (o, v) in at_rest.items() if w < nw and o != v)
-                bad1 = sorted(w for w, (o, v) in rep1.items() if w < nw and o != v)
+                if every_rep:
+                    bad = sorted(w for w, (o, v) in at_rest.items() if w < nw and o != v)
+                    bad1 = sorted(w for w, (o, v) in rep1.items() if w < nw and o != v)
+                    n_bad = reps * len(bad) + len(bad1)  # the warm-up and reps 2.. see the words at rest
+                    first = min(bad[:1] + bad1[:1], default=None)
+                else:
+                    seen = dict(last)
+                    for w in unstored:  # the output starts zeroed and every check clears it
+                        seen[w] = (seen.get(w, (self.ar_word(w),))[0], 0)
+                    bad = sorted(w for w, (o, v) in seen.items() if w < nw and o != v)
+                    n_bad, first = len(bad), (bad[0] if bad else None)
                 sx = refold(clean[k], last, nw)
                 row["sx"].append(sx)
-                row["bad_words"].append(reps * len(bad) + len(bad1))  # the warm-up and reps 2.. see the words at rest
-                first = min(bad[:1] + bad1[:1], default=None)
+                row["bad_words"].append(n_bad)
                 row["first_bad"].append(word_ref.U64_MAX if first is None else 8 * first)
-                if bad1 or sx != clean[k] or refold(clean[k], rep1, nw) != clean[k]:
+                if n_bad or refold(clean[k], rep1, nw) != clean[k] or refold(clean[k], at_rest, nw) != clean[k]:
                     row["bad_sizes"] |= 1 << k
             row["status"] = ERR_INTEGRITY if row["bad_sizes"] else 0
             out["rows"][g] = row
         return out
+
+    def allreduce(self, reps: int) -> Optional[dict]:
+        """What cdprobe_allreduce with `reps` timed reps must return: {"call_seq", "sizes", "rows": {local rank: {...}}},
+        or None when some process's armed fault names no rank, size or word of the ladder.  An armed fault acts in
+        timed rep 1 of its size on its rank: it adds 1 to its word, or (drop, bit 48) leaves its 8 KiB unit unstored,
+        which the check after the rep reads as 0s.  The rest is _allreduce's."""
+        sizes = bwcurve_ref.ladder(self.bpp)
+
+        def decode(v, sizes):
+            fr, fk, fw = (v >> 32) & 0xFFFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if v >> 49 or fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+                return None
+            return fr - 1, fk - 1, fw, bool(v >> 48)
+
+        def effect(words, unstored, g, s, f):
+            rank, _, fw, drop = f
+            if g != rank:
+                return
+            if drop:
+                unit = allreduce_ref.unit_words(fw, s)
+                self._ar_set(words, unit.start, unit.stop, lambda w, v: 0)
+            else:
+                self._ar_set(words, fw, fw + 1, lambda w, v: v + 1)
+
+        return self._allreduce("ar", reps, sizes, decode, effect)
+
+    def twoshot(self, reps: int) -> Optional[dict]:
+        """cdprobe_allreduce_twoshot, as allreduce().  Its fault (receiver, size, word, drop) acts in the process that
+        hosts the rank whose chunk holds the word: timed rep 1 delivers the word to the receiver xored with 1, or (drop)
+        none of its 8 KiB unit, which the receiver's check reads as 0s.  It has a gather area."""
+        sizes = bwcurve_ref.ladder(self.bpp)
+
+        def decode(v, sizes):
+            fr, fk, fw = (v >> 32) & 0xFFFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if v >> 49 or fr == 0 or fr > self.n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+                return None
+            return allreduce_twoshot_ref.owner(sizes[fk - 1], self.n, fw), fk - 1, fr - 1, fw, bool(v >> 48)
+
+        def effect(words, unstored, g, s, f):
+            _, _, recv, fw, drop = f
+            if g != recv:
+                return
+            if drop:
+                unit = allreduce_ref.unit_words(fw, s)
+                self._ar_set(words, unit.start, unit.stop, lambda w, v: 0)
+            else:
+                self._ar_set(words, fw, fw + 1, lambda w, v: v ^ 1)
+
+        return self._allreduce("ts", reps, sizes, decode, effect)
+
+    def ll(self, reps: int) -> Optional[dict]:
+        """cdprobe_allreduce_ll, on its own ladder (cut at 1 MiB).  Its fault (mode, sender, receiver, size, arg) acts
+        in the process that hosts the sender: mode 0, in timed rep 1 the packet of word arg to the receiver carries the
+        sender's salted input xored with 1, which moves the receiver's word by +1 or -1; mode 1, the sender waits arg us
+        (no value changes); mode 2, the receiver (which is the sender) stores nothing to word arg in any rep of the size
+        and still folds the word into (S, X).  Only the last rep of a size is word-checked.  It has an LL area."""
+        sizes = allreduce_ll_ref.ladder(self.bpp)
+
+        def decode(v, sizes):
+            mode, fs, fr, fk, arg = v >> 48, (v >> 40) & 0xFF, (v >> 32) & 0xFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if (mode > 2 or fs == 0 or fs > self.n or fr == 0 or fr > self.n or fk == 0 or fk > len(sizes)
+                    or (mode != 1 and arg >= sizes[fk - 1] // 8) or (mode == 0 and fs == fr) or (mode == 2 and fs != fr)
+                    or (mode == 1 and 2 * arg >= 1000 * self.timeout_ms)):
+                return None
+            return fs - 1, fk - 1, fr - 1, arg, mode
+
+        def effect(words, unstored, g, s, f):
+            sender, k, recv, arg, mode = f
+            if g != recv or mode == 1:
+                return
+            if mode == 2:
+                unstored.add(arg)
+                return
+            fl = allreduce_ll_ref.flag(self.ll_calls, k, 1)
+            v = (int(self.src_at_rest(sender, arg, arg + 1)[0]) + allreduce_ll_ref.salt(self.seed, sender, fl)) & M64
+            self._ar_set(words, arg, arg + 1, lambda w, x: x + (v ^ 1) - v)
+
+        return self._allreduce("ll", reps, sizes, decode, effect, every_rep=False)
+
+    def ring(self, reps: int) -> Optional[dict]:
+        """cdprobe_allreduce_ring.  Its fault (mode, phase, sender, size, arg) acts in the process that hosts the sender,
+        in timed rep 1: mode 0, the sender's push of word arg carries it xored with 1; mode 1, that push stores nothing
+        of the word's unit; mode 2, the sender waits arg us (no value changes).  The rows it fails and what they then
+        hold are allreduce_ring_ref's: in the reduce-scatter the sender's partial of the chunk is off in every row; in
+        the all-gather the rows downstream of the hop hold the word xored with 1, or in place of the unit what they got
+        in the reduce-scatter (the sender's partial, or the clear's 0s).  It has a ring area."""
+        sizes = bwcurve_ref.ladder(self.bpp)
+        n = self.n
+
+        def decode(v, sizes):
+            mode, phase, fs, fk, arg = v >> 48, (v >> 40) & 0xFF, (v >> 32) & 0xFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if mode > 2 or phase > 1 or fs == 0 or fs > n or fk == 0 or fk > len(sizes):
+                return None
+            if mode == 2 and 2 * arg >= 1000 * self.timeout_ms:
+                return None
+            if mode < 2 and (n == 1 or arg >= sizes[fk - 1] // 8 or allreduce_ring_ref.chunk_of(sizes[fk - 1], n, arg)
+                             not in allreduce_ring_ref.pushes(n, fs - 1, phase)):
+                return None
+            return fs - 1, fk - 1, arg, phase, mode
+
+        def effect(words, unstored, g, s, f):
+            sender, _, word, phase, mode = f
+            if mode == 2 or g not in allreduce_ring_ref.failing_rows(n, sender, phase, s, word):
+                return
+            if phase == 1 and mode == 0:
+                self._ar_set(words, word, word + 1, lambda w, v: v ^ 1)
+                return
+            unit = allreduce_ref.unit_words(word, s)
+            c = allreduce_ring_ref.chunk_of(s, n, word)
+            part = None  # the sender's partial of chunk c: the inputs of ranks sender - s' .. sender, as they are at rest
+            if sender != c:
+                part = sum(self.src_at_rest(j, unit.start, unit.stop)
+                           for j in allreduce_ring_ref.partial_ranks(n, sender, c))
+            p = {w: int(part[w - unit.start]) for w in unit} if part is not None else {w: 0 for w in unit}
+            if phase == 1:
+                self._ar_set(words, unit.start, unit.stop, lambda w, v: p[w])
+            elif mode == 0:
+                self._ar_set(words, word, word + 1, lambda w, v: v + (p[w] ^ 1) - p[w])
+            else:
+                self._ar_set(words, unit.start, unit.stop, lambda w, v: v - p[w])
+
+        return self._allreduce("ring", reps, sizes, decode, effect)
+
+    def push(self, reps: int) -> Optional[dict]:
+        """cdprobe_allreduce_push.  Its fault (mode, rank, size, word) acts in timed rep 1 (allreduce_push_ref): modes
+        0-2 in the process that hosts sender `rank`, which contributes its word + 1 (every row's word + 1), skips the
+        word's unit (every row's unit less the sender's input) or reduces it twice (plus the input); mode 3 in the
+        process that hosts the word's owner, which pushes the word xored with 1 to receiver `rank`.  It has a push
+        area."""
+        sizes = bwcurve_ref.ladder(self.bpp)
+        n = self.n
+
+        def decode(v, sizes):
+            mode, fr, fk, fw = v >> 48, (v >> 32) & 0xFFFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if mode > 3 or fr == 0 or fr > n or fk == 0 or fk > len(sizes) or fw >= sizes[fk - 1] // 8:
+                return None
+            if mode < 3:
+                return fr - 1, fk - 1, fr - 1, fw, mode
+            owner = allreduce_push_ref.word_owner(sizes[fk - 1], n, fw)
+            return None if n == 1 or owner == fr - 1 else (owner, fk - 1, fr - 1, fw, mode)
+
+        def effect(words, unstored, g, s, f):
+            _, _, rank, fw, mode = f
+            if mode == 0:
+                self._ar_set(words, fw, fw + 1, lambda w, v: v + 1)
+            elif mode == 3:
+                if g == rank:
+                    self._ar_set(words, fw, fw + 1, lambda w, v: v ^ 1)
+            else:
+                unit = allreduce_ref.unit_words(fw, s)
+                x = self.src_at_rest(rank, unit.start, unit.stop)
+                sign = -1 if mode == 1 else 1
+                self._ar_set(words, unit.start, unit.stop, lambda w, v: v + sign * int(x[w - unit.start]))
+
+        return self._allreduce("push", reps, sizes, decode, effect)
+
+    def build_area(self) -> None:
+        """The exchange area, built by the first all-to-all or memcpy call that is not refused."""
+        if self.area_down is None:
+            self.area_down = frozenset(self.unmapped)
+
+    def memcpy(self, op: int, reps: int) -> Optional[dict]:
+        """What cdprobe_memcpy with op and `reps` timed reps must return, or None when the op is neither OP_READ nor
+        OP_WRITE or some process's armed fault names no cell, size or word, or has a mode above 1 (CDPROBE_ERR_ARG;
+        nothing advances, and the exchange area is not built).  {"call_seq", "sizes", "cells": {(issuer, target):
+        {...}}} for every cell whose issuer is local.  A cell runs when its issuer maps the target now and mapped it
+        when the exchange area was built (by this call, an all-to-all or an earlier memcpy); else it is not measured and
+        carries CDPROBE_ERR_STATE.  The destination of a cell that runs holds its source slice (memcpy_ref.cell) as it
+        is at rest after every rep, warm-up included, and is checked and cleared then: a corrupted word is one bad word
+        per rep.  An armed fault acts in the process that hosts its issuer, in timed rep 1 of its cell and size: mode 0
+        overwrites one landed word with its pattern value xored with 1, mode 1 copies nothing, so the cleared
+        destination reads as 0s.  The (S, X) is the last timed rep's."""
+        n = self.n
+        sizes = bwcurve_ref.ladder(self.bpp)
+        if op not in (OP_READ, OP_WRITE):
+            return None
+        faults = {}
+        for proc, v in self.mc_fault.items():
+            mode, fi, ft, fk, fw = v >> 48, (v >> 40) & 0xFF, (v >> 32) & 0xFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if (mode > 1 or fi == 0 or fi > n or ft == 0 or ft > n or (fi == ft and not self.diag) or fk == 0
+                    or fk > len(sizes) or fw >= sizes[fk - 1] // 8):
+                return None
+            if self.process_of(fi - 1) == proc:
+                faults[(fi - 1, ft - 1)] = (fk - 1, fw, mode)
+        self.build_area()
+        self.mc_calls += 1
+        cells = {}
+        for g in self.local:
+            for j in range(n):
+                if g == j and not self.diag:
+                    continue
+                if (g, j) in self.unmapped or (g, j) in (self.area_down or ()):
+                    cells[(g, j)] = dict(measured=False, status=ERR_STATE)
+                    continue
+                c = memcpy_ref.cell(n, self.bpp, self.mode, op, g, j)
+                src, first = c["src_rank"], c["first_word"]
+                corr = {k - first: m for k, m in self.corruptions_of(src).items() if first <= k < first + self.W}
+                cell = dict(measured=True, bad_sizes=0, sx=[], bad_words=[], first_bad=[])
+                for k, s in enumerate(sizes):
+                    nw = s // 8
+                    clean_sx = self.clean_checksum(src, first, nw)
+                    rest = {}  # {destination word: (pattern, landed)} of the corrupted words of the prefix
+                    for w, m in corr.items():
+                        if w < nw:
+                            p = src_word(self.seed, src, first + w)
+                            rest[w] = (p, p ^ m)
+                    bad = sorted(rest)
+                    fk, fw, mode = faults.get((g, j), (None, None, None))
+                    if fk == k and mode == 1:  # nothing landed: every word the pattern does not make 0 is bad
+                        pattern = word_ref.src_words(self.seed, src, first, nw)
+                        bad1, sx1 = [int(w) for w in np.flatnonzero(pattern != 0)], (0, 0)
+                    else:
+                        rep1 = dict(rest)
+                        if fk == k:
+                            p = src_word(self.seed, src, first + fw)
+                            rep1[fw] = (p, p ^ 1)
+                        bad1, sx1 = sorted(rep1), refold(clean_sx, rep1, nw)
+                    sx_rest = refold(clean_sx, rest, nw)
+                    cell["sx"].append(sx1 if reps == 1 else sx_rest)
+                    cell["bad_words"].append(reps * len(bad) + len(bad1))
+                    first_bad = min(bad[:1] + bad1[:1], default=None)
+                    cell["first_bad"].append(word_ref.U64_MAX if first_bad is None else 8 * first_bad)
+                    if bad or bad1 or sx1 != clean_sx or sx_rest != clean_sx:
+                        cell["bad_sizes"] |= 1 << k
+                cell["status"] = ERR_INTEGRITY if cell["bad_sizes"] else 0
+                cells[(g, j)] = cell
+        return dict(call_seq=self.mc_calls, sizes=sizes, cells=cells)
 
     def a2a_runs(self, s: int, d: int) -> bool:
         """Whether all-to-all cell (sender s, receiver d) runs: it exists, s maps d now, and s's view of d's exchange
@@ -388,8 +662,7 @@ class HandleModel:
                 return None
             if self.process_of(fs - 1) == proc:
                 faults[(fs - 1, fr - 1)] = (fk - 1, fw)
-        if self.area_down is None:
-            self.area_down = frozenset(self.unmapped)
+        self.build_area()
         self.a2a_calls += 1
         seq = self.a2a_calls
         runs = self.a2a_runs

@@ -2,7 +2,10 @@
 latency chase over overridden words, what a landing slot holds after a history of runs, unmaps and landing faults
 (and so what cdprobe_diagnose must report on it), the counters and the unmapped-pair rule, the all-reduce under
 corruptions (also cancelling ones) and faults against a direct recomputation, its skip rule, and the all-to-all's
-sticky exchange area."""
+sticky exchange area; the same for the two-shot, LL, ring and push all-reduces (each protocol's faults at edge words,
+drop and unstored modes included, against whole-array recomputations from their references) and for memcpy (a
+corrupted source word fails exactly the cells and sizes that copy it), with their refusals, counters, skip rules and
+sticky areas, the exchange area shared by memcpy and the all-to-all in both orders."""
 import ctypes as C
 import random
 
@@ -10,10 +13,14 @@ import numpy as np
 import pytest
 
 import handle_model as hm
+import allreduce_ll_ref
+import allreduce_push_ref
 import allreduce_ref
+import allreduce_ring_ref
 import alltoall_ref
 import bwcurve_ref
 import latency_ref
+import memcpy_ref
 import word_ref as ref
 
 SEED = hm.SEED
@@ -311,3 +318,383 @@ def test_alltoall_sticky_area_fault_and_counters(oracle):
             words[fw] ^= np.uint64(1)
         assert c["sx"][fk] == allreduce_ref.checksum(words)
         assert all(o["bad_sizes"] == 0 for key, o in got["cells"].items() if key not in ((2, 0), (0, 2)))
+
+
+# ---- the two-shot, LL, ring and push all-reduces, and memcpy ----------------------------------------------------
+EDGE_BPP = 57 * 8192 + 384  # a partial last unit in a partial last granule: ladder 4096 ... 262144, 467328
+LADDERS = {"ts": bwcurve_ref.ladder, "ll": allreduce_ll_ref.ladder, "ring": bwcurve_ref.ladder,
+           "push": bwcurve_ref.ladder}
+
+
+def edge_model(oracle, n=3):
+    m = hm.HandleModel(oracle, no_schedule, n, EDGE_BPP * max(n - 1, 1), sm_count=132)
+    assert m.bpp == EDGE_BPP
+    return m
+
+
+def call(m, name, reps):
+    return {"ts": m.twoshot, "ll": m.ll, "ring": m.ring, "push": m.push}[name](reps)
+
+
+def sources(n, W, corrupt):
+    srcs = [ref.src_words(SEED, j, 0, W) for j in range(n)]
+    for (r, k), mask in corrupt.items():
+        if k < W:
+            srcs[r][k] ^= np.uint64(mask)
+    return srcs
+
+
+def ring_rep1(srcs, g, s, fault):
+    """Row g after timed rep 1 of a ring fault (sender, word, phase, mode), over whole arrays (test_allreduce_ring_gpu's
+    restatement, on the sources at rest)."""
+    n, nw = len(srcs), s // 8
+    sender, word, phase, mode = fault
+    out = sum(x[:nw] for x in srcs)
+    if mode == 2 or g not in allreduce_ring_ref.failing_rows(n, sender, phase, s, word):
+        return out
+    u0, u1 = word // 1024 * 1024, min(word // 1024 * 1024 + 1024, nw)
+    if phase == 1 and mode == 0:
+        out[word] ^= np.uint64(1)
+        return out
+    c = allreduce_ring_ref.chunk_of(s, n, word)
+    part = sum(srcs[j][:nw] for j in allreduce_ring_ref.partial_ranks(n, sender, c)) if sender != c else None
+    if phase == 1:
+        out[u0:u1] = 0 if part is None else part[u0:u1]
+    elif mode == 0:
+        p = int(part[word])
+        out[word] = np.uint64((int(out[word]) + (p ^ 1) - p) % (1 << 64))
+    else:
+        out[u0:u1] -= part[u0:u1]
+    return out
+
+
+def rep1_direct(name, srcs, g, k, s, fault, call_seq):
+    """Row g's output after timed rep 1 of size s, with `fault` (the option's fields, as the per-protocol suites name
+    them) or None, over whole arrays."""
+    nw = s // 8
+    out = sum(x[:nw] for x in srcs)
+    if fault is None or fault[0] != k:
+        return out
+    f = fault[1:]
+    if name == "ts":
+        recv, word, drop = f
+        if g == recv:
+            if drop:
+                out[word // 1024 * 1024:word // 1024 * 1024 + 1024] = 0
+            else:
+                out[word] ^= np.uint64(1)
+        return out
+    if name == "ll":
+        sender, recv, word, mode = f
+        if g == recv and mode == 0:
+            v = int(srcs[sender][word]) + allreduce_ll_ref.salt(SEED, sender, allreduce_ll_ref.flag(call_seq, k, 1))
+            out[word] = np.uint64((int(out[word]) + (v ^ 1) - v) % (1 << 64))
+        return out
+    if name == "ring":
+        return ring_rep1(srcs, g, s, f)
+    mode, rank, word = f
+    return allreduce_push_ref.rep([x[:nw] for x in srcs], s, (mode, rank, word))[g]
+
+
+def ar_direct(name, n, sizes, corrupt, g, fault=None, reps=1, call_seq=1):
+    """Per size of row g: ((S, X) of the last timed rep, bad words, first bad offset, whether the size fails), from
+    whole arrays: every rep checked (the LL: only the last, with a mode-2 word read as 0 in every rep of its size)."""
+    W = sizes[-1] // 8
+    clean = sum(ref.src_words(SEED, j, 0, W) for j in range(n))
+    srcs = sources(n, W, corrupt)
+    rest = sum(srcs[1:], srcs[0].copy())
+    out = []
+    for k, s in enumerate(sizes):
+        nw = s // 8
+        outs = [rest[:nw].copy() for _ in range(reps + 1)]
+        outs[1] = rep1_direct(name, srcs, g, k, s, fault, call_seq)
+        want = allreduce_ref.checksum(clean[:nw])
+        if name == "ll":
+            seen = outs[-1].copy()
+            if fault is not None and fault[0] == k and fault[-1] == 2 and fault[2] == g:
+                seen[fault[3]] = 0
+            bad = [np.flatnonzero(seen != clean[:nw])]
+        else:
+            bad = [np.flatnonzero(o != clean[:nw]) for o in outs]
+        n_bad = sum(len(b) for b in bad)
+        first = min((int(b[0]) for b in bad if len(b)), default=None)
+        fails = bool(n_bad) or any(allreduce_ref.checksum(o) != want for o in outs)
+        out.append((allreduce_ref.checksum(outs[-1]), n_bad, ref.U64_MAX if first is None else 8 * first, fails))
+    return out
+
+
+def model_rows(got, n):
+    return {g: [(sx, b, f, bool((got["rows"][g]["bad_sizes"] >> k) & 1))
+                for k, (sx, b, f) in enumerate(zip(got["rows"][g]["sx"], got["rows"][g]["bad_words"],
+                                                   got["rows"][g]["first_bad"]))] for g in range(n)}
+
+
+@pytest.mark.parametrize("name", ["ts", "ll", "ring", "push"])
+def test_ladder_allreduce_under_one_corruption_equals_the_reference(oracle, name):
+    n = 3
+    m = edge_model(oracle, n)
+    sizes = LADDERS[name](m.bpp)
+    for rank, word, mask in ((0, 0, 1), (2, 3 * G + 7, 1 << 63), (1, m.W - 1, 0xFFFF), (1, m.W + 5, 0xF0)):
+        m.corrupt_word(rank, word, mask)
+        got = call(m, name, 2)
+        assert got["sizes"] == sizes
+        want = allreduce_ref.expected_corrupted(SEED, n, tuple(sizes), rank, word, mask)
+        bits = 0 if word >= m.W else sum(1 << k for k, s in enumerate(sizes) if s // 8 > word)
+        checked = 1 if name == "ll" else 3  # the LL checks the last rep's words; the others every rep's
+        for g in range(n):
+            row = got["rows"][g]
+            assert row["sx"] == want and row["bad_sizes"] == bits, (rank, word, g)
+            assert row["status"] == (hm.ERR_INTEGRITY if bits else 0)
+            assert row["bad_words"] == [checked * ((bits >> k) & 1) for k in range(len(sizes))]
+            assert row["first_bad"] == [8 * word if (bits >> k) & 1 else ref.U64_MAX for k in range(len(sizes))]
+        m.corrupt_word(rank, word, mask)  # restore
+        assert call(m, name, 1)["rows"][0]["sx"] == list(allreduce_ref.expected(SEED, n, tuple(sizes)))
+
+
+def edge_faults(name, n, sizes, W):
+    """(option value, fault as ar_direct takes it) at the edges: word 0 of size 0, the last word of the last, partial
+    unit, and each protocol's drop or unstored mode."""
+    last = len(sizes) - 1
+    Wl = sizes[last] // 8
+    if name == "ts":
+        a = lambda recv, k, w, drop=False: (int(drop) << 48) | ((recv + 1) << 32) | ((k + 1) << 24) | w
+        cases = [(0, 0, 0, False), (n - 1, last, Wl - 1, False), (1, last, Wl - 1, True), (2, 0, 0, True)]
+        return [(a(r, k, w, d), (k, r, w, d)) for r, k, w, d in cases]
+    if name == "ll":
+        a = lambda s, r, k, w, mode=0: (mode << 48) | ((s + 1) << 40) | ((r + 1) << 32) | ((k + 1) << 24) | w
+        cases = [(0, 1, 0, 0, 0), (2, 0, last, Wl - 1, 0), (1, 1, 0, 0, 2), (2, 2, last, Wl - 1, 2),
+                 (0, 2, 1, 10, 1)]
+        return [(a(*c), (c[2], c[0], c[1], c[3], c[4])) for c in cases]
+    if name == "ring":
+        a = lambda s, k, w, ph, mode: (mode << 48) | (ph << 40) | ((s + 1) << 32) | ((k + 1) << 24) | w
+        out = []
+        for k, w in ((0, 0), (last, Wl - 1)):
+            for ph in (0, 1):
+                for mode in (0, 1):
+                    c = allreduce_ring_ref.chunk_of(sizes[k], n, w)
+                    s = next(s for s in range(n) if c in allreduce_ring_ref.pushes(n, s, ph))
+                    out.append((a(s, k, w, ph, mode), (k, s, w, ph, mode)))
+        return out
+    a = lambda r, k, w, mode: (mode << 48) | ((r + 1) << 32) | ((k + 1) << 24) | w
+    out = []
+    for k, w in ((0, 0), (last, Wl - 1)):
+        for mode in range(4):
+            r = 1
+            if mode == 3 and allreduce_push_ref.word_owner(sizes[k], n, w) == r:
+                r = 2
+            out.append((a(r, k, w, mode), (k, mode, r, w)))
+    return out
+
+
+@pytest.mark.parametrize("name", ["ts", "ll", "ring", "push"])
+def test_ladder_allreduce_under_cancelling_corruptions_and_edge_faults_equals_a_direct_recomputation(oracle, name):
+    n = 3
+    m = edge_model(oracle, n)
+    sizes = LADDERS[name](m.bpp)
+    W = m.W
+    corrupt = {(0, 5): 1 << 40, (1, 5): 0x3, (2, 4 * G - 1): 0x55 << 9, (1, W - 1): 1 << 7, (0, 2 * W + 3): 0xFF,
+               (2, 1): 1 << 3}
+    c = 3 * G + 100  # rank 2's change undoes rank 0's: the sum there is clean
+    wa, wb = hm.src_word(SEED, 0, c), hm.src_word(SEED, 2, c)
+    corrupt[(0, c)] = 0x1234
+    corrupt[(2, c)] = wb ^ ((wb - (((wa ^ 0x1234) - wa) & hm.M64)) & hm.M64)
+    for (r, k), mask in corrupt.items():
+        m.corrupt_word(r, k, mask)
+    got = model_rows(call(m, name, 1), n)
+    for g in range(n):
+        assert got[g] == ar_direct(name, n, sizes, corrupt, g), g
+    opt = name + "_fault"
+    for value, fault in edge_faults(name, n, sizes, W):
+        m.arm_measure(getattr(m, opt), 0, value)
+        for reps in (1, 3):
+            out = call(m, name, reps)
+            assert out is not None, hex(value)
+            got = model_rows(out, n)
+            for g in range(n):
+                assert got[g] == ar_direct(name, n, sizes, corrupt, g, fault, reps, out["call_seq"]), \
+                    (hex(value), reps, g)
+    m.arm_measure(getattr(m, opt), 0, 0)
+
+
+REFUSED = {
+    "ts": lambda n, sizes: [((n + 1) << 32) | (1 << 24), (1 << 24) | 5, (1 << 32) | ((len(sizes) + 1) << 24),
+                            (1 << 32) | (1 << 24) | sizes[0] // 8, 1 << 32, (1 << 49) | (1 << 32) | (1 << 24)],
+    "ll": lambda n, sizes: [(1 << 40) | (1 << 32) | (1 << 24), (3 << 48) | (1 << 40) | (2 << 32) | (1 << 24),
+                            (2 << 48) | (1 << 40) | (2 << 32) | (1 << 24), (1 << 40) | (2 << 32) | (1 << 24) | sizes[0] // 8,
+                            (1 << 48) | (1 << 40) | (2 << 32) | (1 << 24) | 10_000_000, ((n + 1) << 40) | (1 << 32) | (1 << 24),
+                            (1 << 40) | (2 << 32) | ((len(sizes) + 1) << 24)],
+    "ring": lambda n, sizes: [(3 << 48) | (1 << 32) | (1 << 24), (2 << 40) | (1 << 32) | (1 << 24),
+                              ((n + 1) << 32) | (1 << 24), (1 << 32) | ((len(sizes) + 1) << 24),
+                              (3 << 32) | (1 << 24),  # size 0 is one unit, rank 2's, which it never pushes in phase 0
+                              (2 << 48) | (1 << 32) | (1 << 24) | 10_000_000],
+    "push": lambda n, sizes: [(4 << 48) | (1 << 32) | (1 << 24), ((n + 1) << 32) | (1 << 24),
+                              (1 << 32) | ((len(sizes) + 1) << 24), (1 << 32) | (1 << 24) | sizes[0] // 8,
+                              (3 << 48) | (3 << 32) | (1 << 24)],  # mode 3 to the word's owner, rank 2
+}
+
+
+@pytest.mark.parametrize("name", ["ts", "ll", "ring", "push"])
+def test_ladder_allreduce_refusals_counters_skip_rule_and_sticky_area(oracle, name):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = LADDERS[name](m.bpp)
+    calls, opt = name + "_calls", name + "_fault"
+    for bad in REFUSED[name](n, sizes):
+        m.arm_measure(getattr(m, opt), 0, bad)
+        assert call(m, name, 2) is None, hex(bad)
+    assert getattr(m, calls) == 0 and m.ar_area_down[name] is None  # a refused call builds no area
+    m.arm_measure(getattr(m, opt), 0, 0)
+    assert call(m, name, 2)["call_seq"] == 1 and m.ar_area_down[name] == frozenset()
+    m.unmapped.add((2, 1))  # any down pair stops every rank
+    got = call(m, name, 2)
+    assert got["call_seq"] == 2 and got["rows"] == {g: dict(measured=False, status=hm.ERR_STATE) for g in range(n)}
+    m.unmapped.discard((2, 1))
+    assert all(r["status"] == 0 and r["measured"] for r in call(m, name, 2)["rows"].values())
+    assert (m.ar_calls, m.a2a_calls, m.mc_calls, m.bw_calls) == (0, 0, 0, 0)
+    assert all(getattr(m, o + "_calls") == 0 for o in LADDERS if o != name)
+    # an area built while a pair is down keeps every rank off after the remap, until the handle is closed; each
+    # measurement's area is its own
+    m2 = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    m2.unmapped.add((0, 2))
+    call(m2, name, 1)
+    m2.unmapped.discard((0, 2))
+    for _ in range(2):
+        got = call(m2, name, 1)
+        assert got["rows"] == {g: dict(measured=False, status=hm.ERR_STATE) for g in range(n)}
+    assert m2.ar_area_down[name] == {(0, 2)} and getattr(m2, calls) == 3
+    for other in LADDERS:
+        if other != name:
+            assert all(r["measured"] for r in call(m2, other, 1)["rows"].values()), other
+    assert all(r["measured"] for r in m2.allreduce(1)["rows"].values())
+
+
+def test_ll_and_ring_report_their_own_ladder_and_the_push_and_two_shot_the_bwcurve_one(oracle):
+    m = hm.HandleModel(oracle, no_schedule, 1, 3 << 20, sm_count=132)
+    assert m.ll(1)["sizes"] == [s for s in bwcurve_ref.ladder(3 << 20) if s <= 1 << 20]
+    for name in ("ts", "ring", "push"):
+        assert call(m, name, 1)["sizes"] == bwcurve_ref.ladder(3 << 20)
+    # at N = 1 the ring pushes nothing and the push has no peer: their word faults are refused
+    for name, v in (("ring", (1 << 32) | (1 << 24)), ("push", (3 << 48) | (1 << 32) | (1 << 24))):
+        m.arm_measure(getattr(m, name + "_fault"), 0, v)
+        assert call(m, name, 1) is None
+
+
+def memcpy_direct(oracle, n, bpp, op, g, j, corrupt, fault=None, reps=1):
+    """Per size of cell (g, j): ((S, X) of the last timed rep's destination, bad words, first bad offset, fails), from
+    whole arrays: the source slice as it is at rest, and in timed rep 1 the fault (k, word, mode)."""
+    c = memcpy_ref.cell(n, bpp, 1, op, g, j)
+    src = sources(n, c["first_word"] + bpp // 8, corrupt)[c["src_rank"]][c["first_word"]:]
+    out = []
+    for k, s in enumerate(memcpy_ref.ladder(bpp)):
+        nw = s // 8
+        want = memcpy_ref.words(SEED, c, s)
+        outs = [src[:nw].copy() for _ in range(reps + 1)]
+        if fault is not None and fault[0] == k:
+            if fault[2]:
+                outs[1][:] = 0
+            else:
+                outs[1][fault[1]] = want[fault[1]] ^ np.uint64(1)
+        bad = [np.flatnonzero(o != want) for o in outs]
+        first = min((int(b[0]) for b in bad if len(b)), default=None)
+        fails = any(len(b) for b in bad) or any(allreduce_ref.checksum(o) != allreduce_ref.checksum(want) for o in outs)
+        out.append((allreduce_ref.checksum(outs[-1]), sum(len(b) for b in bad),
+                    ref.U64_MAX if first is None else 8 * first, fails))
+    return out
+
+
+def memcpy_cells(got):
+    return {key: [(sx, b, f, bool((c["bad_sizes"] >> k) & 1))
+                  for k, (sx, b, f) in enumerate(zip(c["sx"], c["bad_words"], c["first_bad"]))]
+            for key, c in got["cells"].items() if c["measured"]}
+
+
+@pytest.mark.parametrize("op", [hm.OP_READ, hm.OP_WRITE], ids=["pull", "push"])
+def test_memcpy_under_one_corruption_fails_exactly_the_cells_and_sizes_that_copy_it(oracle, op):
+    n = 3
+    m = edge_model(oracle, n)
+    sizes = memcpy_ref.ladder(m.bpp)
+    W = m.W
+    for rank, word, mask in ((0, 0, 1), (2, W + 3 * G + 7, 1 << 63), (1, 2 * W - 1, 0xFFFF), (1, W - 1, 0xF0)):
+        m.corrupt_word(rank, word, mask)
+        got = m.memcpy(op, 2)
+        assert got["sizes"] == sizes and set(got["cells"]) == {(g, j) for g in range(n) for j in range(n) if g != j}
+        for (g, j), cell in got["cells"].items():
+            c = memcpy_ref.cell(n, m.bpp, 1, op, g, j)
+            at = word - c["first_word"]
+            hit = c["src_rank"] == rank and 0 <= at < W
+            bits = sum(1 << k for k, s in enumerate(sizes) if hit and s // 8 > at)
+            assert cell["bad_sizes"] == bits and cell["status"] == (hm.ERR_INTEGRITY if bits else 0), (g, j, word)
+            assert cell["bad_words"] == [3 * ((bits >> k) & 1) for k in range(len(sizes))]  # warm-up and two reps
+            assert cell["first_bad"] == [8 * at if (bits >> k) & 1 else ref.U64_MAX for k in range(len(sizes))]
+            words = memcpy_ref.words(SEED, c, m.bpp)
+            if hit:
+                words[at] ^= np.uint64(mask)
+            assert cell["sx"] == [allreduce_ref.checksum(words[:s // 8]) for s in sizes], (g, j)
+        m.corrupt_word(rank, word, mask)  # restore
+    assert m.mc_calls == 4
+
+
+@pytest.mark.parametrize("op", [hm.OP_READ, hm.OP_WRITE], ids=["pull", "push"])
+def test_memcpy_under_corruptions_and_edge_faults_equals_a_direct_recomputation(oracle, op):
+    n = 3
+    m = edge_model(oracle, n)
+    sizes = memcpy_ref.ladder(m.bpp)
+    W, last = m.W, len(sizes) - 1
+    corrupt = {(0, 5): 1 << 40, (1, W + 5): 0x3, (2, W - 1): 1 << 7, (0, 2 * W - 1): 0xFF, (1, 0): 1}
+    for (r, k), mask in corrupt.items():
+        m.corrupt_word(r, k, mask)
+    got = memcpy_cells(m.memcpy(op, 1))
+    for (g, j), cells in got.items():
+        assert cells == memcpy_direct(oracle, n, m.bpp, op, g, j, corrupt), (g, j)
+    # word 0 of size 0, the last word of the last, partial unit, and a word a corruption also changes; flip and drop
+    for (g, j, k, w) in ((0, 1, 0, 0), (2, 1, last, W - 1), (1, 0, last, 5), (1, 2, 0, 0)):
+        for mode in (0, 1):
+            m.arm_measure(m.mc_fault, 0, (mode << 48) | ((g + 1) << 40) | ((j + 1) << 32) | ((k + 1) << 24) | w)
+            for reps in (1, 2):
+                got = memcpy_cells(m.memcpy(op, reps))
+                for (gg, jj), cells in got.items():
+                    f = (k, w, mode) if (gg, jj) == (g, j) else None
+                    assert cells == memcpy_direct(oracle, n, m.bpp, op, gg, jj, corrupt, f, reps), (g, j, k, mode, reps)
+    m.arm_measure(m.mc_fault, 0, 0)
+
+
+def test_memcpy_refusals_counters_and_the_one_sided_skip_rule(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = memcpy_ref.ladder(m.bpp)
+    for op in (0, 3):
+        assert m.memcpy(op, 1) is None
+    for bad in ((2 << 48) | (1 << 40) | (2 << 32) | (1 << 24), (1 << 40) | (1 << 32) | (1 << 24),
+                ((n + 1) << 40) | (1 << 32) | (1 << 24), (1 << 40) | (2 << 32) | ((len(sizes) + 1) << 24),
+                (1 << 40) | (2 << 32) | (1 << 24) | sizes[0] // 8, (1 << 40) | (1 << 24)):
+        m.arm_measure(m.mc_fault, 0, bad)
+        assert m.memcpy(hm.OP_READ, 1) is None, hex(bad)
+    assert m.mc_calls == 0 and m.area_down is None  # a refused call builds no exchange area
+    m.arm_measure(m.mc_fault, 0, 0)
+    m.memcpy(hm.OP_WRITE, 1)
+    m.unmapped.add((2, 1))  # only the issuer's own direction stops, and only its cell
+    got = m.memcpy(hm.OP_READ, 1)
+    assert got["call_seq"] == 2 and got["cells"][(2, 1)] == dict(measured=False, status=hm.ERR_STATE)
+    assert all(c["measured"] and c["status"] == 0 for key, c in got["cells"].items() if key != (2, 1))
+    m.unmapped.discard((2, 1))
+    assert all(c["measured"] for c in m.memcpy(hm.OP_READ, 1)["cells"].values())
+    assert (m.a2a_calls, m.ar_calls, m.ts_calls, m.ll_calls, m.ring_calls, m.push_calls) == (0,) * 6
+
+
+@pytest.mark.parametrize("first", ["memcpy", "alltoall"])
+def test_the_exchange_area_is_built_by_whichever_of_memcpy_and_alltoall_comes_first(oracle, first):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    m.unmapped.add((0, 2))
+    m.memcpy(hm.OP_READ, 1) if first == "memcpy" else m.alltoall(1)
+    assert m.area_down == {(0, 2)}
+    m.unmapped.discard((0, 2))  # remap: the probe mapping is back, the exchange area's is not
+    for op in (hm.OP_READ, hm.OP_WRITE):
+        got = m.memcpy(op, 1)
+        assert got["cells"][(0, 2)] == dict(measured=False, status=hm.ERR_STATE), op
+        assert all(c["measured"] for key, c in got["cells"].items() if key != (0, 2))
+    aa = m.alltoall(1)
+    assert aa["cells"][(0, 2)] == dict(cell_measured=False, cell_status=hm.ERR_STATE)
+    assert m.area_down == {(0, 2)} and (m.mc_calls, m.a2a_calls) == ((3, 1) if first == "memcpy" else (2, 2))
+    # the all-reduces' areas are their own: built now, with every mapping up
+    assert all(r["measured"] for r in m.twoshot(1)["rows"].values()) and m.ar_area_down["ts"] == frozenset()

@@ -10,10 +10,13 @@ one handle through many calls and compares the whole output of each call with th
   the verdict restatement (verdict_ref), the traced phase kinds and peers, and `warmed`;
 - Diagnose: the word_ref report of every cell, field for field, from the issuer and from the target;
 - Latency: status and digest; BwCurve: bad_sizes and (S, X) per size; PingPong and Atomics: clean cells, call_seq;
-- AllReduce: per row measured, status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest,
-  armed faults and the skip rule (any down pair stops every rank); AllToAll: per rank measured and blocks, per cell
-  status, bad_sizes and per size bad_words, first_bad and (S, X), under armed faults and the sticky exchange-area rule;
-  both with call_seq, the ladder and the path;
+- the five all-reduces (AllReduce, AllReduceTwoShot, AllReduceLL, AllReduceRing, AllReducePush): per row measured,
+  status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest, each protocol's armed
+  faults (drop and unstored modes included), the skip rule (any down pair stops every rank) and each area's sticky
+  rule; AllToAll: per rank measured and blocks, per cell status, bad_sizes and per size bad_words, first_bad and
+  (S, X), under armed faults and the sticky exchange-area rule; Memcpy, both ops: per cell measured, status, bad_sizes
+  and per size bad_words, first_bad and (S, X), under corruptions at rest, armed faults and the exchange area it shares
+  with the all-to-all; all with call_seq, the ladder and the path (the LL and the ring report their own) or area_bytes;
 - refused calls: the error code, and nothing they may not change.
 
 A divergence fails with the seed, the step index and every step so far; the walk is generated from the seed and the
@@ -31,6 +34,9 @@ import uuid
 
 import pytest
 
+import allreduce_ll_ref
+import allreduce_push_ref
+import allreduce_ring_ref
 import bwcurve_ref
 import handle_model as hm
 import verdict_ref
@@ -51,7 +57,17 @@ UNIT = 1024  # words in one 8 KiB unit of the data paths
 HOPS, LAT_REPS = 64, 2
 TRIPS = 16
 ATOMIC_OPS = 64
-LADDER_REPS = 1  # the all-reduce and all-to-all fold timed rep 1, the faulted one, into their (S, X)
+LADDER_REPS = 1  # the ladder measurements fold timed rep 1, the faulted one, into their (S, X)
+# each ladder measurement's fault option and the model's {process: value} of it
+FAULTS = {"OPT_ALLREDUCE_FAULT": "ar_fault", "OPT_ALLREDUCE_TWOSHOT_FAULT": "ts_fault",
+          "OPT_ALLREDUCE_LL_FAULT": "ll_fault", "OPT_ALLREDUCE_RING_FAULT": "ring_fault",
+          "OPT_ALLREDUCE_PUSH_FAULT": "push_fault", "OPT_ALLTOALL_FAULT": "a2a_fault", "OPT_MEMCPY_FAULT": "mc_fault"}
+# each all-reduce step: the model's method, the raw binding and the path it reports (None: the handle's)
+ALLREDUCES = {"allreduce": ("allreduce", "allreduce_raw", None), "twoshot": ("twoshot", "allreduce_twoshot_raw", None),
+              "ll": ("ll", "allreduce_ll_raw", 3), "ring": ("ring", "allreduce_ring_raw", 4),
+              "push": ("push", "allreduce_push_raw", None)}
+LADDER_CALLS = [("allreduce",), ("twoshot",), ("ll",), ("ring",), ("push",), ("alltoall",), ("memcpy", 1),
+                ("memcpy", 2)]
 
 
 class Refused(Exception):
@@ -70,6 +86,7 @@ class Driver:
         self.m = hm.HandleModel(oracle, hm.schedule_fn(p._lib, pkg.abi), n, nbytes, info.sm_count[0], cfg.ctas,
                                 local=local, flags=cfg.flags)
         self.gate = pkg.gate(cfg, n)
+        self.area_bytes = None  # of the exchange area, once the all-to-all or memcpy has reported it
         self.check_info()
 
     # ---- checks ----------------------------------------------------------------------------------------------
@@ -164,22 +181,22 @@ class Driver:
             m.warm_mode = value
         elif name in ("OPT_UNIDIRECTIONAL", "OPT_OVERLAP_VERIFY", "OPT_ALL_RANK_BARRIERS", "OPT_PAIR_BARRIERS"):
             m.set_flag(getattr(self.a, "FLAG" + name[3:]), bool(value))
-        elif name == "OPT_ALLREDUCE_FAULT":
-            m.arm_measure(m.ar_fault, self.me, value)
-        elif name == "OPT_ALLTOALL_FAULT":
-            m.arm_measure(m.a2a_fault, self.me, value)
+        elif name in FAULTS:
+            m.arm_measure(getattr(m, FAULTS[name]), self.me, value)
 
-    def check_allreduce(self):
+    def check_allreduce(self, kind="allreduce"):
         a, m = self.a, self.m
-        want = m.allreduce(LADDER_REPS)
-        rc, t = self.p.allreduce_raw(LADDER_REPS)
+        model, raw, path = ALLREDUCES[kind]
+        want = getattr(m, model)(LADDER_REPS)
+        rc, t = getattr(self.p, raw)(LADDER_REPS)
         if want is None:  # the armed fault names no rank, size or word of the ladder: refused, nothing advances
             assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)
             return
         assert rc == a.OK, rc
         ar = self.pkg.AllReduce.from_c(t)
-        assert (ar.call_seq, ar.sizes, ar.path, ar.reps) == (want["call_seq"], want["sizes"], m.path, LADDER_REPS), \
-            (ar.call_seq, want["call_seq"], ar.path, m.path)
+        path = m.path if path is None else path
+        assert (ar.call_seq, ar.sizes, ar.path, ar.reps) == (want["call_seq"], want["sizes"], path, LADDER_REPS), \
+            (ar.call_seq, want["call_seq"], ar.path, path)
         assert ar.row_mask == sum(1 << g for g in m.local)
         for g, w in want["rows"].items():
             got = dict(measured=ar.measured[g], status=ar.status[g])
@@ -200,6 +217,7 @@ class Driver:
         assert (aa.call_seq, aa.sizes, aa.path, aa.reps) == (want["call_seq"], want["sizes"], m.path, LADDER_REPS), \
             (aa.call_seq, want["call_seq"], aa.path, m.path)
         assert aa.area_bytes == (self.n * m.bpp + (2 << 20) - 1) // (2 << 20) * (2 << 20)
+        self.check_area_bytes(aa.area_bytes)
         for g, w in want["ranks"].items():
             assert aa.measured[g] == w["measured"], ("alltoall rank", g)
             if w["measured"]:
@@ -212,6 +230,36 @@ class Driver:
                     got.update(bad_sizes=aa.bad_sizes[s][d], bad_words=aa.bad_words[s][d],
                                first_bad=aa.first_bad[s][d], sx=list(zip(aa.sum[s][d], aa.xr[s][d])))
                 assert got == w, ("alltoall cell", s, d, got, w)
+
+    def check_area_bytes(self, area_bytes):
+        """The all-to-all and memcpy share one exchange area: every call reports the same size, n blocks at least."""
+        if self.area_bytes is None:
+            assert area_bytes >= self.n * self.m.bpp, (area_bytes, self.n * self.m.bpp)
+            self.area_bytes = area_bytes
+        assert area_bytes == self.area_bytes, (area_bytes, self.area_bytes)
+
+    def check_memcpy(self, op):
+        a, m = self.a, self.m
+        want = m.memcpy(op, LADDER_REPS)
+        rc, t = self.p.memcpy_raw(op, LADDER_REPS)
+        if want is None:  # the op or the armed fault names nothing of this call: refused, nothing advances
+            assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)
+            return
+        assert rc == a.OK, rc
+        mc = self.pkg.Memcpy.from_c(t)
+        assert (mc.call_seq, mc.sizes, mc.op, mc.reps) == (want["call_seq"], want["sizes"], op, LADDER_REPS), \
+            (mc.call_seq, want["call_seq"])
+        self.check_area_bytes(mc.area_bytes)
+        assert mc.row_mask == sum(1 << g for g in m.local)
+        for g in m.local:
+            for j in range(self.n):
+                w = want["cells"].get((g, j), dict(measured=False, status=0))
+                got = dict(measured=mc.measured[g][j], status=mc.status[g][j])
+                assert got == {f: w[f] for f in got}, ("memcpy cell", op, g, j, got, w)
+                if w["measured"]:
+                    got.update(bad_sizes=mc.bad_sizes[g][j], sx=list(zip(mc.sum[g][j], mc.xr[g][j])),
+                               bad_words=mc.bad_words[g][j], first_bad=mc.first_bad[g][j])
+                assert got == w, ("memcpy cell", op, g, j, got, w)
 
     def apply(self, step):
         a, m, p = self.a, self.m, self.p
@@ -290,16 +338,22 @@ class Driver:
             for (i, j), w in want.items():
                 if w["measured"]:
                     assert list(zip(bw.sum[i][j], bw.xr[i][j])) == w["sx"], ("bwcurve (S, X)", i, j)
-        elif kind == "allreduce":
-            self.check_allreduce()
+        elif kind in ALLREDUCES:
+            self.check_allreduce(kind)
         elif kind == "alltoall":
             self.check_alltoall()
+        elif kind == "memcpy":
+            self.check_memcpy(step[1])
         elif kind == "bad_call":  # refused measurement calls advance no call_seq
             what = step[1]
             if what == "bwcurve":
                 rc, _ = p.bwcurve_raw(a.BWCURVE_MAX_REPS + 1)
-            elif what == "allreduce":
-                rc, _ = p.allreduce_raw(a.ALLREDUCE_MAX_REPS + 1)
+            elif what in ALLREDUCES:
+                rc, _ = getattr(p, ALLREDUCES[what][1])(a.ALLREDUCE_MAX_REPS + 1)
+            elif what == "memcpy":
+                rc, _ = p.memcpy_raw(a.OP_READ | a.OP_WRITE, 1)
+            elif what == "memcpy_reps":
+                rc, _ = p.memcpy_raw(a.OP_WRITE, a.MEMCPY_MAX_REPS + 1)
             elif what == "alltoall":
                 rc, _ = p.alltoall_raw(a.ALLTOALL_MAX_REPS + 1)
             elif what == "pingpong":
@@ -332,40 +386,72 @@ def edge_word(rng, size):
 
 
 def ladder_fault(rng, m, name, rank, peer):
-    """A valid OPT_ALLREDUCE_FAULT (on `rank`; half of them drop the word's unit instead of adding 1) or
-    OPT_ALLTOALL_FAULT (cell rank -> peer) value at an edge word of a size of the ladder: the last size or a random
-    one."""
-    sizes = bwcurve_ref.ladder(m.bpp)
+    """A valid value of a ladder measurement's fault option at an edge word of a size of its ladder (the last size or a
+    random one), acting in the process that hosts `rank`, about half of them in a drop or unstored mode:
+    OPT_ALLREDUCE_FAULT on `rank`, adding 1 or dropping the word's unit; OPT_ALLREDUCE_TWOSHOT_FAULT to receiver
+    `rank`, xor 1 or drop; OPT_ALLREDUCE_LL_FAULT, a corrupted packet rank -> peer, or a word `rank` never stores;
+    OPT_ALLREDUCE_RING_FAULT, a corrupted or dropped push by `rank` in a phase that pushes the word (at N = 1, where
+    nothing is pushed, a 5 us delay); OPT_ALLREDUCE_PUSH_FAULT, modes 0-2 by sender `rank` or mode 3 to receiver
+    `rank`; OPT_ALLTOALL_FAULT on block rank -> peer; OPT_MEMCPY_FAULT on cell rank -> peer, flipped or dropped."""
+    n = m.n
+    sizes = allreduce_ll_ref.ladder(m.bpp) if name == "OPT_ALLREDUCE_LL_FAULT" else bwcurve_ref.ladder(m.bpp)
     k = rng.choice([len(sizes) - 1, rng.randrange(len(sizes))])
     word = edge_word(rng, sizes[k])
-    if name == "OPT_ALLREDUCE_FAULT":
-        return (rng.randrange(2) << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
-    return ((rank + 1) << 40) | ((peer + 1) << 32) | ((k + 1) << 24) | word
+    low = ((k + 1) << 24) | word
+    drop = rng.randrange(2)
+    if name in ("OPT_ALLREDUCE_FAULT", "OPT_ALLREDUCE_TWOSHOT_FAULT"):
+        return (drop << 48) | ((rank + 1) << 32) | low
+    if name == "OPT_ALLREDUCE_LL_FAULT":
+        if drop or peer == rank:
+            return (2 << 48) | ((rank + 1) << 40) | ((rank + 1) << 32) | low
+        return ((rank + 1) << 40) | ((peer + 1) << 32) | low
+    if name == "OPT_ALLREDUCE_RING_FAULT":
+        if n == 1:
+            return (2 << 48) | (1 << 32) | ((k + 1) << 24) | 5
+        # `rank` pushes every chunk but its own in the reduce-scatter and every chunk but rank + 1's in the all-gather,
+        # so at N >= 2 one of the phases pushes the word's chunk
+        phase = rng.randrange(2)
+        if allreduce_ring_ref.chunk_of(sizes[k], n, word) not in allreduce_ring_ref.pushes(n, rank, phase):
+            phase ^= 1
+        return (drop << 48) | (phase << 40) | ((rank + 1) << 32) | low
+    if name == "OPT_ALLREDUCE_PUSH_FAULT":
+        mode = rng.randrange(4)
+        if mode == 3 and (n == 1 or allreduce_push_ref.word_owner(sizes[k], n, word) == rank):
+            mode = rng.randrange(3)
+        return (mode << 48) | ((rank + 1) << 32) | low
+    if name == "OPT_MEMCPY_FAULT":
+        return (drop << 48) | ((rank + 1) << 40) | ((peer + 1) << 32) | low
+    return ((rank + 1) << 40) | ((peer + 1) << 32) | low
+
+
+def past_its_size(m, name, value):
+    """The same fault one word past its size, which the next call refuses (a delay is left as it is)."""
+    if name == "OPT_ALLREDUCE_RING_FAULT" and value >> 48 == 2:
+        return value
+    return value + bwcurve_ref.ladder(m.bpp)[((value >> 24) & 0xFF) - 1] // 8 - (value & 0xFFFFFF)
 
 
 def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
     """One step drawn from `rng` and the model's state alone (never from a device result).  `ctas_cap` bounds the
-    grids it may ask for, so that many same-device ranks stay resident together.  A tenth of the steps are all-reduce
-    and all-to-all calls (each about as often as bwcurve) and their fault armings; the rest keep their weights."""
+    grids it may ask for, so that many same-device ranks stay resident together.  A sixth of the steps are calls of the
+    seven ladder collectives (the five all-reduces, the all-to-all and memcpy with either op, each about as often as
+    bwcurve) and their fault armings; the rest keep their weights."""
     n, W = m.n, m.W
     grids = [c for c in (1, 2, 3, 7, 8) if ctas_cap is None or c <= ctas_cap]
     x = rng.random()
-    if x < 0.035:
-        return ("allreduce",)
-    if x < 0.07:
-        return ("alltoall",)
-    if x < 0.10:
-        name = rng.choice(["OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"])
-        armed = m.ar_fault if name == "OPT_ALLREDUCE_FAULT" else m.a2a_fault
-        if armed and rng.random() < 0.4:
+    if x < 0.12:
+        return rng.choice(LADDER_CALLS)
+    if x < 0.16:
+        name = rng.choice(sorted(FAULTS))
+        if getattr(m, FAULTS[name]) and rng.random() < 0.4:
             return ("opt", name, 0)
         i = rng.choice(m.local)
         j = rng.choice([c for c in range(n) if c != i] or [i])
         value = ladder_fault(rng, m, name, i, j)
         if rng.random() < 0.15:  # one word past its size: the next call is refused until the fault is re-armed
-            value += bwcurve_ref.ladder(m.bpp)[((value >> 24) & 0xFF) - 1] // 8 - (value & 0xFFFFFF)
+            value = past_its_size(m, name, value)
         return ("opt", name, value)
-    x = (x - 0.10) / 0.90
+    x = (x - 0.16) / 0.84
     if x < 0.28:
         return ("run",)
     if x < 0.48:
@@ -418,14 +504,15 @@ def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
         return ("atomics", rng.randrange(3))
     if x < 0.98:
         return ("bwcurve",)
-    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics", "allreduce", "alltoall"]))
+    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics", "alltoall", "memcpy", "memcpy_reps"]
+                                   + sorted(ALLREDUCES)))
 
 
 def walk_step(rng, m, steps, **kw):
-    """The next step of a walk: right after an unmap or a remap, an all-reduce or all-to-all call, so that every walk
-    with churn calls them while a pair is down and after a remap; else gen_step's."""
+    """The next step of a walk: right after an unmap or a remap, a call of one of the seven ladder collectives, so that
+    every walk with churn calls them while a pair is down and after a remap; else gen_step's."""
     if steps and steps[-1][0] in ("unmap", "remap"):
-        return rng.choice([("allreduce",), ("alltoall",)])
+        return rng.choice(LADDER_CALLS)
     return gen_step(rng, m, **kw)
 
 
@@ -441,7 +528,7 @@ def walk(drv, seed, n_steps, **kw):
             raise AssertionError(f"seed {seed}: step {k} {step!r} diverged from the model: {e!r}\n"
                                  f"steps so far: {steps!r}") from e
     # remap what is still down, so that every walk with churn also calls the ladder measurements after a remap
-    closing = [("remap",) + c for c in sorted(drv.m.unmapped)] + [("allreduce",), ("alltoall",), ("run",), ("diagnose",)]
+    closing = [("remap",) + c for c in sorted(drv.m.unmapped)] + LADDER_CALLS + [("run",), ("diagnose",)]
     drv.play(closing, f"seed {seed}: closing run")
     return steps + closing
 
@@ -539,6 +626,106 @@ def test_alltoall_area_of_a_pair_unmapped_at_its_first_call_stays_unmapped_after
     assert drv.m.area_down == {(0, 2)} and drv.m.a2a_calls == 4
 
 
+@pytest.mark.parametrize("first", ["memcpy", "alltoall"])
+def test_exchange_area_built_while_a_pair_is_down_stays_unmapped_for_memcpy_and_alltoall(pkg, oracle, first):
+    """cdprobe_memcpy and cdprobe_alltoall share one exchange area, built by whichever is called first: with (0, 2)
+    down then, cell (0, 2) is skipped by both, with either op, until close, while runs use the remapped pair.  An armed
+    memcpy drop on another cell fails exactly that cell and size, and the next call is clean again."""
+    A2A, MC1, MC2 = ("alltoall",), ("memcpy", 1), ("memcpy", 2)
+    opener = MC1 if first == "memcpy" else A2A
+    bpp = oracle.plan(3, BIG, 1, False).bytes_per_pair
+    last = len(bwcurve_ref.ladder(bpp)) - 1
+    drop = (1 << 48) | (3 << 40) | (1 << 32) | ((last + 1) << 24) | (bpp // 8 - 1)
+    # the first calls after the remap are memcpy's, so a model that let only the all-to-all build the area diverges
+    steps = [RUN, ("unmap", 0, 2), opener, MC2, ("remap", 0, 2), MC1, MC2, A2A, RUN, DIAG,
+             ("opt", "OPT_MEMCPY_FAULT", drop), MC2, MC1, ("opt", "OPT_MEMCPY_FAULT", 0), MC2, A2A, RUN, DIAG]
+    drv = play(pkg, oracle, 3, BIG, steps, f"n 3, {first} first")
+    assert drv.m.area_down == {(0, 2)} and drv.m.mc_calls == (7 if first == "memcpy" else 6)
+
+
+def allreduce_edge_faults(m, drop):
+    """One armed fault per all-reduce at an edge word (word 0 of size 0, or the last word of the last, partial unit),
+    in its drop or unstored mode when `drop`, else as a corrupted word; each in a rank of this process."""
+    n, W = m.n, m.W
+    sizes, ll_sizes = bwcurve_ref.ladder(m.bpp), allreduce_ll_ref.ladder(m.bpp)
+    last, ll_last = len(sizes) - 1, len(ll_sizes) - 1
+    r, q = n - 1, 0
+    out = [("OPT_ALLREDUCE_FAULT", (drop << 48) | ((r + 1) << 32) | ((last + 1) << 24) | (W - 1)),
+           ("OPT_ALLREDUCE_TWOSHOT_FAULT", (drop << 48) | ((q + 1) << 32) | (1 << 24)),
+           ("OPT_ALLREDUCE_LL_FAULT", (2 << 48) | ((r + 1) << 40) | ((r + 1) << 32) | ((ll_last + 1) << 24)
+            | (ll_sizes[-1] // 8 - 1) if drop or n == 1 else ((r + 1) << 40) | ((q + 1) << 32) | (1 << 24)),
+           ("OPT_ALLREDUCE_PUSH_FAULT", ((1 if drop else 0) << 48) | ((r + 1) << 32) | ((last + 1) << 24) | (W - 1))]
+    if n > 1:  # the ring pushes the last word in the reduce-scatter from every rank but its chunk's owner, n - 1
+        out.append(("OPT_ALLREDUCE_RING_FAULT", (drop << 48) | ((q + 1) << 32) | ((last + 1) << 24) | (W - 1)))
+    return out
+
+
+@pytest.mark.parametrize("n", [1, 3])
+def test_five_allreduces_in_sequence_leave_nothing_another_could_hide_behind(pkg, oracle, n):
+    """The one-shot, two-shot, LL, ring and push, one after another in both orders, on every path and across grid
+    changes, between a corruption and its restore, with each one's fault armed once at an edge word, as a drop, an
+    unstored word or a corrupted one.  Each rep's check clears the output it read, so a unit one of them drops reads
+    as 0s rather than as the sums an earlier rep or call stored there.  (None of these calls leaves a correct sum in
+    the scratch for the next: what stays there is cleared output or granule tables, so the host's zeroing of the
+    LL's output at the start of a call is seen only through a memcpy diagnosis, in the test below.)"""
+    FIVE = [("allreduce",), ("twoshot",), ("ll",), ("ring",), ("push",)]
+    cfg, p = open_same(pkg, n, SMALL, 8)
+    with p:
+        drv = Driver(pkg, oracle, p, cfg, n, SMALL)
+        m = drv.m
+        word = m.W - 1  # in the last, partial unit of slice 0
+        grids = [("OPT_CTAS", 1), ("OPT_CTAS", 3), ("OPT_CTAS_RANK", (len(m.local) << 16) | 2), ("OPT_CTAS", 8)]
+        steps = []
+        for q, path in enumerate((0, 1, 2)):
+            steps += [("opt", "OPT_PATH", path), ("opt",) + grids[q]] + FIVE + [("corrupt", n - 1, word, 1 << 21)]
+            steps += FIVE[::-1]
+            for drop in (1, 0):
+                faults = allreduce_edge_faults(m, drop)
+                steps += [("opt",) + f for f in faults] + FIVE + [("opt",) + grids[q + 1]] + FIVE[::-1]
+                steps += [("opt", f[0], 0) for f in faults]
+            steps += [("corrupt", n - 1, word, 1 << 21)] + FIVE
+        steps += [RUN, DIAG]
+        drv.play(steps, f"n {n}")
+        assert (m.ar_calls, m.ts_calls, m.ll_calls, m.ring_calls, m.push_calls) == (21,) * 5
+
+
+# The LL's output lies at kArOutOff = 63232 bytes into the rank's scratch, and memcpy's last diagnosis (a DiagOut at
+# 62976) leaves its first sample's `expected`, the pattern word of the lowest bad word, at 63568: over output word 42.
+# At N = 1 that pattern word is the LL's sum for the word.  Each later sample's `expected` lies 48 bytes (6 words) on.
+LL_WORDS_UNDER_DIAG_SAMPLES = [42 + 6 * i for i in range(16)]
+
+
+@pytest.mark.parametrize("op", [1, 2], ids=["pull", "push"])
+def test_an_ll_word_never_stored_is_not_hidden_by_a_memcpy_diagnosis_left_in_the_scratch(pkg, oracle, op):
+    """A memcpy over corrupted source words leaves, in the scratch the LL writes its output to, the samples of its last
+    diagnosis: at N = 1 their `expected` words are the LL's correct sums for the very words they lie over.  An LL that
+    then never stores one of those words (mode 2) must still find it bad: the output is zeroed at the start of every LL
+    call, so the word reads 0 rather than the leftover.  A clean LL first grows the scratch to the LL's size, so the
+    memcpy and the faulted LL use the same buffer."""
+    words = LL_WORDS_UNDER_DIAG_SAMPLES
+    corrupt = [("corrupt", 0, w, 1 << 12) for w in words]
+    steps = [("ll",)]
+    for w in (words[0], words[-1]):
+        steps += corrupt + [("memcpy", op)] + corrupt  # the corruptions are restored before the LL runs
+        steps += [("opt", "OPT_ALLREDUCE_LL_FAULT", (2 << 48) | (1 << 40) | (1 << 32) | (1 << 24) | w), ("ll",),
+                  ("opt", "OPT_ALLREDUCE_LL_FAULT", 0), ("ll",)]
+    drv = play(pkg, oracle, 1, SMALL, steps, f"n 1, op {op}")
+    assert drv.m.ll_calls == 5 and drv.m.corrupt == {}
+
+
+@pytest.mark.parametrize("n", [1, 3])
+def test_memcpy_leaves_the_probe_state_alone(pkg, oracle, n):
+    """Memcpy copies into the exchange area and checks in the issuers' scratch: every landing slot and source checksum
+    stays as the runs and corruptions left them, and a corrupted source word fails exactly the cells that copy it."""
+    bpp = oracle.plan(n, BIG, 1, n == 1).bytes_per_pair
+    W, j = bpp // 8, (1 if n > 1 else 0)
+    faults = [(0, 1 << 63), (W - 1, 0xF0)]
+    steps = [RUN, ("memcpy", 1), DIAG, ("landing", 0, j, faults), RUN, ("memcpy", 2), DIAG,
+             ("corrupt", n - 1, W - 1, 1 << 30), ("memcpy", 1), ("memcpy", 2), RUN, DIAG, ("landing", 0, j, []),
+             ("memcpy", 2), ("corrupt", n - 1, W - 1, 1 << 30), RUN, ("memcpy", 1), DIAG]
+    play(pkg, oracle, n, BIG, steps, f"n {n}")
+
+
 @pytest.mark.parametrize("n", [1, 3])
 def test_grid_and_path_changes_between_ladder_calls_with_faults_armed(pkg, oracle, n):
     """OPT_CTAS and OPT_CTAS_RANK change the grid the all-reduce and the all-to-all launch on, and with it which warp
@@ -596,8 +783,8 @@ def two_proc_steps(seed, n_steps, m):
     while len(out) < n_steps:
         x = rng.random()
         if x < 0.35:
-            out.append(("all", rng.choice([("run",), ("run",), ("pingpong", rng.randrange(2)), ("bwcurve",),
-                                           ("allreduce",), ("alltoall",)])))
+            out.append(("all", rng.choice([("run",), ("run",), ("pingpong", rng.randrange(2)), ("bwcurve",)]
+                                          + LADDER_CALLS)))
             mutating = rng.random() < 0.5
             continue
         if x < 0.5:
@@ -607,8 +794,10 @@ def two_proc_steps(seed, n_steps, m):
                                                        ("OPT_WARMUP", rng.choice([0, 2]))])))
             continue
         owner = rng.randrange(2)
-        if x < 0.58:  # a valid fault armed (or disarmed) only by the process that hosts its rank or sender
-            name = rng.choice(["OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"])
+        if x < 0.58:  # a valid fault armed (or disarmed) only by the process that hosts its rank, sender or issuer
+            name = rng.choice(sorted(FAULTS))
+            if name == "OPT_ALLREDUCE_RING_FAULT":
+                owner = 0  # one process arms the ring, so no two of its pushes are faulted in one rep
             value = 0 if rng.random() < 0.3 else ladder_fault(rng, m, name, owner, 1 - owner)
             out.append((owner, ("opt", name, value)))
             continue
@@ -666,8 +855,8 @@ def mirror(self, step, who):
         m.corrupt_word(step[1], step[2], step[3])
     elif kind == "landing":
         m.arm(step[1], step[2], step[3])
-    elif kind == "opt" and step[1] in ("OPT_ALLREDUCE_FAULT", "OPT_ALLTOALL_FAULT"):
-        m.arm_measure(m.ar_fault if step[1] == "OPT_ALLREDUCE_FAULT" else m.a2a_fault, who, step[2])
+    elif kind == "opt" and step[1] in FAULTS:
+        m.arm_measure(getattr(m, FAULTS[step[1]]), who, step[2])
 
 
 Driver.mirror = mirror

@@ -1,5 +1,6 @@
-"""The ladder measurements (cdprobe_bwcurve, cdprobe_allreduce, cdprobe_alltoall) where their kernels go wrong, checked
-word for word against the numpy references (bwcurve_ref, allreduce_ref, alltoall_ref, word_ref) on every data path:
+"""The ladder measurements (cdprobe_bwcurve, cdprobe_allreduce, cdprobe_alltoall, cdprobe_memcpy) where their kernels
+go wrong, checked word for word against the numpy references (bwcurve_ref, allreduce_ref, alltoall_ref, memcpy_ref,
+word_ref) on every data path:
 
 - tiny ladders: bytes_per_pair below one 8 KiB unit, below the ladder's 4096-byte minimum, exactly one ladder step, one
   128-byte vector past a unit, one 16 KiB granule and one vector past it, and a partial unit in the second granule.
@@ -10,8 +11,13 @@ word for word against the numpy references (bwcurve_ref, allreduce_ref, alltoall
 - faults placed at the edges: the all-reduce's at word 0 of size 0 and at the last word of the last, partial unit,
   each as a word off by one and as a unit not stored;
   the all-to-all's at the last word of a partial unit, at a word of the last warp of the grid and on the diagonal
-  block; and a corrupted source word in a partial unit, which fails exactly the bwcurve cell and sizes that read it,
-  every all-reduce row at those sizes, and no all-to-all cell.
+  block; memcpy's at word 0 of size 0, at the last word of the last, partial unit and on the diagonal cell, each
+  flipped and dropped; and a corrupted source word in a partial unit, which fails exactly the bwcurve cell and sizes
+  that read it, every all-reduce row at those sizes, exactly the memcpy cells and sizes that copy it (pulled and
+  pushed), and no all-to-all cell.
+
+Memcpy's checks run diag_launch and bwcurve_kernel on the issuer's grid over a destination in the exchange area, so
+its tiny ladders and small grids reach the same partial-unit branches.
 
 Every call uses one timed rep, so the faulted rep is the one folded into (S, X); the all-reduce's word check runs
 after the warm-up and after the timed rep, and its bad words are summed over both.  Several ranks share GPU 0 with at
@@ -24,6 +30,7 @@ import pytest
 import allreduce_ref
 import alltoall_ref
 import bwcurve_ref
+import memcpy_ref
 import word_ref
 from test_bwcurve_gpu import slice_first_word
 
@@ -37,6 +44,7 @@ U64_MAX = word_ref.U64_MAX
 UNIT_WORDS = 1024   # 8 KiB
 WARPS_PER_CTA = 8
 PATHS = (0, 1, 2)   # TMA, 16-byte ld/st, 32-byte ld/st
+OPS = (memcpy_ref.OP_READ, memcpy_ref.OP_WRITE)
 # below one unit, below the 4096-byte minimum, exactly one ladder step, one vector past a unit, one granule, one vector
 # past a granule, a partial unit in the second granule
 TINY = (128, 3968, 4096, 4224, 8320, 16384, 16512, 24704)
@@ -136,6 +144,49 @@ def check_allreduce(ar, src, n, bpp, corrupt=None, fault=None):
     return ar
 
 
+def check_memcpy(mc, src, n, bpp, diag, op, corrupt=None, fault=None):
+    """Every cell at every size lands its source slice (memcpy_ref.cell) as it is at rest, in the warm-up and the timed
+    rep, and is checked after each: a corrupted source word is one FLIP per rep at its offset in every cell and size
+    that copies it.  fault (issuer, target, k, word, mode): timed rep 1 of that cell and size holds the word's pattern
+    value xored with 1 (mode 0), or nothing, as the clear's 0s (mode 1)."""
+    corrupt = corrupt or {}
+    sizes = memcpy_ref.ladder(bpp)
+    assert mc.sizes == sizes and mc.reps == 1 and mc.op == op
+    W = bpp // 8
+    for g in range(n):
+        for j in range(n):
+            if g == j and not diag:
+                assert not mc.measured[g][j] and mc.status[g][j] == 0, (g, j)
+                continue
+            c = memcpy_ref.cell(n, bpp, 1, op, g, j)
+            first = c["first_word"]
+            words = source(src, c["src_rank"], first + W, corrupt)[first:]
+            pattern = src(c["src_rank"], first + W)[first:]
+            bits = 0
+            for k, s in enumerate(sizes):
+                nw = s // 8
+                warm, rep1 = words[:nw], words[:nw].copy()
+                if fault is not None and (g, j, k) == fault[:3]:
+                    if fault[4]:
+                        rep1[:] = 0
+                    else:
+                        rep1[fault[3]] = pattern[fault[3]] ^ np.uint64(1)
+                bad = [np.flatnonzero(w != pattern[:nw]) for w in (warm, rep1)]
+                first_bad = min((int(b[0]) for b in bad if len(b)), default=None)
+                ctx = (g, j, s, op, fault)
+                assert (mc.sum[g][j][k], mc.xr[g][j][k]) == allreduce_ref.checksum(rep1), ctx
+                assert mc.bad_words[g][j][k] == sum(len(b) for b in bad), (ctx, mc.bad_words[g][j][k])
+                assert mc.first_bad[g][j][k] == (U64_MAX if first_bad is None else 8 * first_bad), \
+                    (ctx, mc.first_bad[g][j][k])
+                if first_bad is not None:
+                    bits |= 1 << k
+            assert mc.measured[g][j] and mc.bad_sizes[g][j] == bits, (g, j, mc.bad_sizes[g][j], bits)
+            assert mc.status[g][j] == (ERR_INTEGRITY if bits else 0), (g, j)
+            assert (mc.t0_ns[g][j], mc.peak_gbps[g][j], mc.half_bytes[g][j]) == \
+                memcpy_ref.summary(sizes, mc.ns_median[g][j])
+    return mc
+
+
 def check_alltoall(aa, n, bpp, diag, fault=None):
     """Every block at every size holds its sender's pattern of this call; fault (sender, receiver, k, word): timed rep
     1 of size k delivers that word xored with 1, and only there."""
@@ -200,6 +251,8 @@ def test_tiny_ladders_every_path_clean(pkg, src, n, bpp):
             check_bwcurve(p.BwCurve(reps=1), src, n, bpp, n == 1)
             check_allreduce(p.AllReduce(reps=1), src, n, bpp)
             check_alltoall(p.AllToAll(reps=1), n, bpp, n == 1)
+            for op in OPS:
+                check_memcpy(p.Memcpy(op, reps=1), src, n, bpp, n == 1, op)
 
 
 @pytest.mark.parametrize("bpp", TINY)
@@ -210,6 +263,8 @@ def test_tiny_ladders_with_the_diagonal_block(pkg, src, bpp):
             p.SetOption(pkg.abi.OPT_PATH, path)
             check_bwcurve(p.BwCurve(reps=1), src, n, bpp, True)
             check_alltoall(p.AllToAll(reps=1), n, bpp, True)
+            for op in OPS:
+                check_memcpy(p.Memcpy(op, reps=1), src, n, bpp, True, op)
 
 
 # ---- grids and edge-placed faults ----------------------------------------------------------------------------------
@@ -254,6 +309,15 @@ def test_grids_and_faults_at_the_edges(pkg, src, n, grid):
                 check_alltoall(p.AllToAll(reps=1), n, bpp, diag, fault)
             p.SetOption(a.OPT_ALLTOALL_FAULT, 0)
             check_alltoall(p.AllToAll(reps=1), n, bpp, diag)
+            # memcpy: word 0 of size 0, the last word of the last, partial unit, the diagonal cell; flipped, dropped
+            for op in OPS:
+                check_memcpy(p.Memcpy(op, reps=1), src, n, bpp, diag, op)
+            for q, (g, j, k, word) in enumerate(((0, 1 % n, 0, 0), (n - 1, 0, last, W - 1), (n - 1, n - 1, 1, 7))):
+                for mode in (0, 1):
+                    op = OPS[(q + mode) % 2]
+                    p.SetOption(a.OPT_MEMCPY_FAULT, a.memcpy_fault(g, j, k, word, mode))
+                    check_memcpy(p.Memcpy(op, reps=1), src, n, bpp, diag, op, fault=(g, j, k, word, mode))
+            p.SetOption(a.OPT_MEMCPY_FAULT, 0)
             if path != 2:
                 continue
             # a source word in a partial unit, on the 32-byte ld/st path: the last word of slice 0 of rank n - 1 (only
@@ -267,6 +331,9 @@ def test_grids_and_faults_at_the_edges(pkg, src, n, grid):
                 check_bwcurve(p.BwCurve(reps=1), src, n, bpp, diag, corrupt)
                 check_allreduce(p.AllReduce(reps=1), src, n, bpp, corrupt)
                 check_alltoall(p.AllToAll(reps=1), n, bpp, diag)
+                for op in OPS:
+                    mc = check_memcpy(p.Memcpy(op, reps=1), src, n, bpp, diag, op, corrupt)
+                    assert any(mc.bad_sizes[g][d] for g in range(n) for d in range(n) if mc.measured[g][d])
                 p.Corrupt(j, 8 * word, 1 << 33)  # restore: the next calls are clean
                 check_bwcurve(p.BwCurve(reps=1), src, n, bpp, diag)
                 check_allreduce(p.AllReduce(reps=1), src, n, bpp)

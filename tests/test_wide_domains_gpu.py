@@ -11,8 +11,9 @@ the form `rank * n_local + li` (first local rank, the fd exchange, the pingpong 
   table that overflows is refused at open and leaks nothing; every cell word for word; diagnose reports that name
   writers 8 to 15; landing faults on slots 14 and 15; the on-demand measurements; seeded model walks.
 - b. Several processes, several ranks each (2 x 8, 2 x 4, 3 x 3), on GPU 0 with fd handles: the gathered matrix, the
-  verdict, diagnose, the measurements' row masks and digests, a landing fault across processes, the pingpong status
-  merge, and the refusals of mismatched and oversized domains.
+  verdict, diagnose, the measurements' row masks and digests (every all-reduce's rows and the all-to-all's and memcpy's
+  cells against their references in every process), a landing fault across processes, the pingpong status merge,
+  and the refusals of mismatched and oversized domains.
 
 More than 8 ranks in one process put more than 8 streams on one device; every such test runs in a child process whose
 environment sets CUDA_DEVICE_MAX_CONNECTIONS=32 (include/cdprobe.h, CDPROBE_FLAG_ALLOW_SAME_DEVICE), since the test
@@ -30,12 +31,14 @@ import uuid
 
 import pytest
 
+import allreduce_ll_ref
 import allreduce_ref
 import alltoall_ref
 import atomics_ref
 import bwcurve_ref
 import handle_model as hm
 import latency_ref
+import memcpy_ref
 import pingpong_ref
 import verdict_ref
 import word_ref as ref
@@ -515,6 +518,10 @@ def mp_process(pkg, session, rank, world, n_local, what):
         out["bw"] = fields(p.BwCurve(reps=BW_REPS))
         out["ar"] = fields(p.AllReduce(reps=2))
         out["a2a"] = fields(p.AllToAll(reps=2))
+        for key, fn in (("ts", p.AllReduceTwoShot), ("ll", p.AllReduceLL), ("ring", p.AllReduceRing),
+                        ("push", p.AllReducePush)):
+            out[key] = fields(fn(reps=2))
+        out["mc"] = [fields(p.Memcpy(op, reps=2)) for op in (pkg.abi.OP_READ, pkg.abi.OP_WRITE)]
         # a landing fault armed in process 0 on a cell whose target lives in the last process
         W = info.bytes_per_pair // 8
         if rank == 0:
@@ -637,6 +644,30 @@ def test_processes_with_several_ranks_each(pkg, oracle, world, n_local):
                     assert a2a["cell_status"][s][d] == 0 and a2a["bad_words"][s][d] == [0] * len(sizes), (s, d)
                     assert [[x, y] for x, y in zip(a2a["sum"][s][d], a2a["xr"][s][d])] == \
                         [list(e) for e in alltoall_ref.expected(SEED, s, d, 1, 2, sizes)], (s, d)
+        # the two-shot, LL, ring and push fill exactly the local rows with the pattern's sums, on their own ladders and
+        # paths; memcpy fills exactly the cells a local rank issues, with its source slice's (S, X), for both ops
+        for key, ladder, path in (("ts", sizes, 0), ("ll", allreduce_ll_ref.ladder(W * 8), 3), ("ring", sizes, 4),
+                                  ("push", sizes, 0)):
+            got = o[key]
+            assert got["call_seq"] == outs[0][key]["call_seq"] == 1 and got["sizes"] == ladder, key
+            assert (got["row_mask"], got["reps"], got["path"]) == (rows, 2, path), key
+            want = [list(sx) for sx in allreduce_ref.expected(SEED, n, tuple(ladder))]
+            for r in range(n):
+                assert got["measured"][r] == (r in mine), (key, r)
+                if r in mine:
+                    assert got["status"][r] == 0 and got["bad_sizes"][r] == 0, (key, r)
+                    assert got["bad_words"][r] == [0] * len(ladder), (key, r)
+                    assert [[s, x] for s, x in zip(got["sum"][r], got["xr"][r])] == want, (key, r)
+        for call, mc in enumerate(o["mc"], 1):
+            assert (mc["call_seq"], mc["row_mask"], mc["reps"], mc["sizes"]) == (call, rows, 2, sizes), mc["op"]
+            for g in range(n):
+                for d in range(n):
+                    assert mc["measured"][g][d] == (g in mine and g != d), (mc["op"], g, d)
+                    if mc["measured"][g][d]:
+                        cell = memcpy_ref.cell(n, W * 8, 1, mc["op"], g, d)
+                        assert mc["status"][g][d] == 0 and mc["bad_words"][g][d] == [0] * len(sizes), (g, d)
+                        assert [[s, x] for s, x in zip(mc["sum"][g][d], mc["xr"][g][d])] == \
+                            [list(e) for e in memcpy_ref.expected(oracle, SEED, cell, sizes)], (mc["op"], g, d)
         # the landing fault of process 0 fails exactly its cell, in every process's gathered result
         f = AsResult(o["faulted"])
         want_w = [[0 if (a, b) == (0, n - 1) else 1 for b in range(n)] for a in range(n)]
