@@ -102,7 +102,7 @@ static void unmap_range(const cdprobe* h, CUdeviceptr va, size_t bytes) {
 // Map rank j's allocation of m into local rank li's address space.
 static int32_t map_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   LocalRank& L = h->lr[li];
-  if ((L.*m.mapped)[j]) return 0;
+  if (m.mapped[li][j]) return 0;
   CUmemGenericAllocationHandle hnd;
   if (j >= h->first && j < h->first + h->n_local) {
     hnd = m.own[j - h->first];
@@ -115,40 +115,34 @@ static int32_t map_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
   CUdeviceptr va = 0;
   const CUresult r = map_range(h, hnd, m.bytes, kVmmGranule, L.ordinal, &va);
   if (r != CUDA_SUCCESS) return (int32_t)r;
-  (L.*m.va)[j] = va;
-  (L.*m.mapped)[j] = true;
+  m.va[li][j] = va;
+  m.mapped[li][j] = true;
   return 0;
 }
 
 static void unmap_peer(cdprobe* h, SharedAlloc& m, uint32_t li, uint32_t j) {
-  LocalRank& L = h->lr[li];
-  if (!(L.*m.mapped)[j]) return;
-  cudaSetDevice(L.ordinal);
-  unmap_range(h, (L.*m.va)[j], m.bytes);
-  (L.*m.va)[j] = 0;
-  (L.*m.mapped)[j] = false;
+  if (!m.mapped[li][j]) return;
+  cudaSetDevice(h->lr[li].ordinal);
+  unmap_range(h, m.va[li][j], m.bytes);
+  m.va[li][j] = 0;
+  m.mapped[li][j] = false;
 }
 
-// Unmaps m everywhere and releases every handle of it: its imports, then the local allocations and their fds.
+// Unmaps m everywhere, releases its imports, then its local allocations and their fds, and leaves m as never created.
 static void release_shared(cdprobe* h, SharedAlloc& m) {
   for (uint32_t li = 0; li < h->n_local; ++li) {
     if (h->lr[li].ordinal < 0) continue;
     for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j) unmap_peer(h, m, li, j);
   }
   for (uint32_t j = 0; j < (uint32_t)kMaxRanks; ++j)
-    if (m.has_import[j]) {
-      h->drv.MemRelease(m.imported[j]);
-      m.has_import[j] = false;
-    }
+    if (m.has_import[j]) h->drv.MemRelease(m.imported[j]);
   for (uint32_t li = 0; li < h->n_local; ++li) {
     if (h->lr[li].ordinal < 0) continue;
     cudaSetDevice(h->lr[li].ordinal);
     if (m.has_own[li]) h->drv.MemRelease(m.own[li]);
-    m.has_own[li] = false;
     if (m.own_fd[li] >= 0) ::close(m.own_fd[li]);
-    m.own_fd[li] = -1;
   }
-  m.bytes = 0;
+  m = SharedAlloc();
 }
 
 // Local rank li's allocation of m: m.bytes of its device's memory, exportable as the handle type chosen at open.
@@ -511,7 +505,8 @@ static void fill_params(const cdprobe* h, uint32_t li, const Phase* phases, uint
                         ProbeParams* P) {
   const LocalRank& L = h->lr[li];
   memset(P, 0, sizeof(*P));
-  for (uint32_t j = 0; j < h->n_total; ++j) P->base_peer[j] = L.mapped[j] ? reinterpret_cast<uint8_t*>(L.va[j]) : nullptr;
+  for (uint32_t j = 0; j < h->n_total; ++j)
+    P->base_peer[j] = h->mem.mapped[li][j] ? reinterpret_cast<uint8_t*>(h->mem.va[li][j]) : nullptr;
   P->row = L.row;
   P->run_seq = h->launch_seq;
   P->seq_base = h->launch_seq * (uint64_t)(kMaxPhases + 2);
@@ -588,7 +583,7 @@ static bool wait_rows(cdprobe* h, uint64_t token) {
 static int reset_ctrl_local(cdprobe* h, uint32_t li) {
   LocalRank& L = h->lr[li];
   CDP_RT(cudaSetDevice(L.ordinal));
-  uint8_t* base = reinterpret_cast<uint8_t*>(L.va[L.grank]);
+  uint8_t* base = reinterpret_cast<uint8_t*>(h->mem.va[li][L.grank]);
   const size_t off = offsetof(Ctrl, grid_arrive);
   CDP_RT(cudaMemsetAsync(base + off, 0, sizeof(Ctrl) - off, L.stream));
   CDP_RT(cudaStreamSynchronize(L.stream));
@@ -599,7 +594,7 @@ static int reset_ctrl_local(cdprobe* h, uint32_t li) {
 static int write_fault(cdprobe* h, uint32_t li, const LandingFault& f) {
   LocalRank& L = h->lr[li];
   CDP_RT(cudaSetDevice(L.ordinal));
-  uint8_t* p = reinterpret_cast<uint8_t*>(L.va[L.grank]) + offsetof(Ctrl, fault);
+  uint8_t* p = reinterpret_cast<uint8_t*>(h->mem.va[li][L.grank]) + offsetof(Ctrl, fault);
   CDP_RT(cudaMemcpyAsync(p, &f, sizeof(f), cudaMemcpyHostToDevice, L.stream));
   CDP_RT(cudaStreamSynchronize(L.stream));
   return CDPROBE_OK;
@@ -621,7 +616,7 @@ static int fill_and_publish(cdprobe* h) {
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
     CDP_RT(cudaSetDevice(L.ordinal));
-    uint8_t* base = reinterpret_cast<uint8_t*>(L.va[L.grank]);
+    uint8_t* base = reinterpret_cast<uint8_t*>(h->mem.va[li][L.grank]);
     CDP_RT(cudaMemsetAsync(base, 0, kCtrlBytes, L.stream));
     CDP_RT(cudaMemsetAsync(base + pl.land_off, 0, pl.land_bytes, L.stream));
     cudaError_t e = (cudaError_t)probe_fill_launch(base + pl.src_off, pl.src_bytes, h->seed, L.grank,
@@ -662,7 +657,7 @@ static int fill_and_publish(cdprobe* h) {
       pub[0][s] = h->src_sum[li][s] = L.row->ph[s].sum[0];
       pub[1][s] = h->src_xor[li][s] = L.row->ph[s].xr[0];
     }
-    uint8_t* base = reinterpret_cast<uint8_t*>(L.va[L.grank]);
+    uint8_t* base = reinterpret_cast<uint8_t*>(h->mem.va[li][L.grank]);
     CDP_RT(cudaMemcpyAsync(base + offsetof(Ctrl, src_sum), pub[0], sizeof(pub[0]), cudaMemcpyHostToDevice, L.stream));
     CDP_RT(cudaMemcpyAsync(base + offsetof(Ctrl, src_xor), pub[1], sizeof(pub[1]), cudaMemcpyHostToDevice, L.stream));
     CDP_RT(cudaStreamSynchronize(L.stream));
@@ -1337,7 +1332,7 @@ int cdprobe_corrupt(cdprobe_t* h, uint32_t local, uint64_t byte_offset, uint64_t
   if (byte_offset % 8 != 0 || byte_offset + 8 > h->plan.src_bytes) return CDPROBE_ERR_ARG;
   cdp::LocalRank& L = h->lr[local];
   CDP_RT(cudaSetDevice(L.ordinal));
-  uint8_t* p = reinterpret_cast<uint8_t*>(L.va[L.grank]) + h->plan.src_off + byte_offset;
+  uint8_t* p = reinterpret_cast<uint8_t*>(h->mem.va[local][L.grank]) + h->plan.src_off + byte_offset;
   uint64_t w = 0;
   CDP_RT(cudaMemcpyAsync(&w, p, 8, cudaMemcpyDeviceToHost, L.stream));
   CDP_RT(cudaStreamSynchronize(L.stream));
@@ -1404,8 +1399,7 @@ int cdprobe_ce_copy(cdprobe_t* h, uint32_t n_copies, const uint32_t* local, cons
     if (local[k] >= h->n_local || peer[k] >= h->n_total) return CDPROBE_ERR_ARG;
     for (uint32_t q = 0; q < k; ++q)
       if (local[q] == local[k]) return CDPROBE_ERR_ARG;  // one copy per local rank: each has one stream and event pair
-    const cdp::LocalRank& L = h->lr[local[k]];
-    if (!L.mapped[peer[k]]) {
+    if (!h->mem.mapped[local[k]][peer[k]]) {
       cdp::set_err("peer is not mapped into this rank's address space");
       return CDPROBE_ERR_STATE;
     }
@@ -1413,8 +1407,8 @@ int cdprobe_ce_copy(cdprobe_t* h, uint32_t n_copies, const uint32_t* local, cons
   for (uint32_t k = 0; k < n_copies; ++k) {
     cdp::LocalRank& L = h->lr[local[k]];
     CDP_RT(cudaSetDevice(L.ordinal));
-    const uint8_t* mine = reinterpret_cast<const uint8_t*>(L.va[L.grank]);
-    const uint8_t* theirs = reinterpret_cast<const uint8_t*>(L.va[peer[k]]);
+    const uint8_t* mine = reinterpret_cast<const uint8_t*>(h->mem.va[local[k]][L.grank]);
+    const uint8_t* theirs = reinterpret_cast<const uint8_t*>(h->mem.va[local[k]][peer[k]]);
     const void* src = push ? mine + pl.src_off : theirs + pl.src_off;
     void* dst = const_cast<uint8_t*>(push ? theirs : mine) + pl.land_off;
     CDP_RT(cudaEventRecord(L.ev0, L.stream));

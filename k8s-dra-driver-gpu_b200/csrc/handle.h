@@ -41,18 +41,6 @@ struct LocalRank {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int max_ctas = 0;
-  CUdeviceptr va[kMaxRanks] = {};  // rank j's probe allocation as mapped here
-  bool mapped[kMaxRanks] = {};
-  CUdeviceptr area_va[kMaxRanks] = {};  // rank j's exchange area (cdprobe_alltoall) as mapped here
-  bool area_mapped[kMaxRanks] = {};
-  CUdeviceptr gather_va[kMaxRanks] = {};  // rank j's gather area (cdprobe_allreduce_twoshot) as mapped here
-  bool gather_mapped[kMaxRanks] = {};
-  CUdeviceptr ll_va[kMaxRanks] = {};  // rank j's LL area (cdprobe_allreduce_ll) as mapped here
-  bool ll_mapped[kMaxRanks] = {};
-  CUdeviceptr ring_va[kMaxRanks] = {};  // rank j's ring area (cdprobe_allreduce_ring) as mapped here
-  bool ring_mapped[kMaxRanks] = {};
-  CUdeviceptr push_va[kMaxRanks] = {};  // rank j's push area (cdprobe_allreduce_push) as mapped here
-  bool push_mapped[kMaxRanks] = {};
   ResultRow* row = nullptr;
   char uuid[48] = {};
   Phase phases[kMaxPhases];
@@ -69,8 +57,8 @@ struct LocalRank {
 // cdprobe members say which, how large and whose).
 struct SharedAlloc {
   size_t bytes = 0;                                       // of each allocation; 0: not created
-  CUdeviceptr (LocalRank::*va)[kMaxRanks];                // where a local rank keeps its mappings: (L.*va)[j]
-  bool (LocalRank::*mapped)[kMaxRanks];
+  CUdeviceptr va[kMaxRanks][kMaxRanks] = {};              // [local rank][rank] rank j's allocation as mapped there
+  bool mapped[kMaxRanks][kMaxRanks] = {};
   CUmemGenericAllocationHandle own[kMaxRanks] = {};       // [local rank]
   bool has_own[kMaxRanks] = {};
   int own_fd[kMaxRanks];                                  // [local rank] exported POSIX fd, -1: none
@@ -80,7 +68,7 @@ struct SharedAlloc {
                                               // (the probe allocation's is cdprobe::status)
   bool stale = false;  // an area that must start zeroed must be zeroed before its next use: it is new, or a local
                        // rank's kernel timed out and it may hold packets, data, flags or partial sums of any earlier call
-  SharedAlloc(CUdeviceptr (LocalRank::*v)[kMaxRanks], bool (LocalRank::*m)[kMaxRanks]) : va(v), mapped(m) {
+  SharedAlloc() {
     for (int& f : own_fd) f = -1;
   }
 };
@@ -111,17 +99,12 @@ struct cdprobe {
   // The device memory shared across the domain, per rank.  The probe allocation is made at open; every other area on
   // the first call of the measurement that owns it (ensure_area, ensure_nvls), rounded up to the VMM granule.  All are
   // kept until close.
-  cdp::SharedAlloc mem{&cdp::LocalRank::va, &cdp::LocalRank::mapped};  // the probe allocation: plan.alloc_bytes
-  // cdprobe_alltoall's exchange area: n_total x bytes_per_pair
-  cdp::SharedAlloc area{&cdp::LocalRank::area_va, &cdp::LocalRank::area_mapped};
-  // cdprobe_allreduce_twoshot's gather area: bytes_per_pair
-  cdp::SharedAlloc gather{&cdp::LocalRank::gather_va, &cdp::LocalRank::gather_mapped};
-  // cdprobe_allreduce_ll's LL area: 2 x n_total x 2 x the LL ladder's largest size
-  cdp::SharedAlloc ll{&cdp::LocalRank::ll_va, &cdp::LocalRank::ll_mapped};
-  // cdprobe_allreduce_ring's ring area: bytes_per_pair and one flag per 8 KiB of it
-  cdp::SharedAlloc ring{&cdp::LocalRank::ring_va, &cdp::LocalRank::ring_mapped};
-  // cdprobe_allreduce_push's push area: bytes_per_pair
-  cdp::SharedAlloc push{&cdp::LocalRank::push_va, &cdp::LocalRank::push_mapped};
+  cdp::SharedAlloc mem;     // the probe allocation: plan.alloc_bytes
+  cdp::SharedAlloc area;    // cdprobe_alltoall's exchange area: n_total x bytes_per_pair
+  cdp::SharedAlloc gather;  // cdprobe_allreduce_twoshot's gather area: bytes_per_pair
+  cdp::SharedAlloc ll;      // cdprobe_allreduce_ll's LL area: 2 x n_total x 2 x the LL ladder's largest size
+  cdp::SharedAlloc ring;    // cdprobe_allreduce_ring's ring area: bytes_per_pair and one flag per 8 KiB of it
+  cdp::SharedAlloc push;    // cdprobe_allreduce_push's push area: bytes_per_pair
   // cdprobe_allreduce_nvls's multicast object and NVLS areas: 2 x bytes_per_pair, also rounded up to the multicast
   // granularity
   cdp::NvlsArea nvls;
@@ -229,7 +212,7 @@ int ensure_nvls(cdprobe* h, size_t bytes, bool* refused);
 // mapped.  Non-zero: never read or write through that mapping.
 inline int32_t cell_status(const cdprobe* h, uint32_t li, uint32_t j) {
   const int32_t s = h->status[h->lr[li].grank][j];
-  return s == 0 && !h->lr[li].mapped[j] ? kStatusUnmapped : s;
+  return s == 0 && !h->mem.mapped[li][j] ? kStatusUnmapped : s;
 }
 
 }  // namespace cdp

@@ -362,6 +362,19 @@ static void bw_summarize(const BwScratch& s, const uint64_t (*want)[2], const ui
   out->status[idx] = bad ? CDPROBE_ERR_INTEGRITY : 0;
 }
 
+// Fills the word checks of entry idx of a cdprobe_allreduce_t (a row) or a cdprobe_alltoall_t (a cell) from its
+// kernel's per-size counts; an entry with a bad size gets CDPROBE_ERR_INTEGRITY in *status.
+template <typename Out>
+static void word_checks(const unsigned long long* bad_words, const unsigned long long* first_bad_n, uint32_t n_sizes,
+                        uint32_t idx, int32_t* status, Out* out) {
+  for (uint32_t k = 0; k < n_sizes; ++k) {
+    out->bad_words[idx][k] = bad_words[k];
+    out->first_bad[idx][k] = bad_words[k] != 0 ? ~first_bad_n[k] : UINT64_MAX;
+    if (bad_words[k] != 0) out->bad_sizes[idx] |= 1u << k;
+  }
+  if (out->bad_sizes[idx] != 0) *status = CDPROBE_ERR_INTEGRITY;
+}
+
 // A ladder measurement as open_ladder lets it through: when it began, its reps, its size ladder, and the verdict on its
 // arguments, empty when they are valid.
 struct Ladder {
@@ -370,6 +383,19 @@ struct Ladder {
   uint64_t size[kBwMaxSizes];
   std::string bad;
 };
+
+// Where an armed ladder fault acts, from its low 32 bits, (k + 1) << 24 | word: size k and word `word` (for some modes
+// a delay instead), and whether the call has that size and that size has that word.  k is valid only when size_ok.
+struct FaultSpot {
+  uint32_t k;
+  uint64_t word;
+  bool size_ok, word_ok;
+};
+static FaultSpot fault_spot(uint64_t v, const Ladder& lad) {
+  const uint64_t fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  const bool size_ok = fk != 0 && fk <= lad.n_sizes;
+  return {(uint32_t)fk - 1, word, size_ok, size_ok && word < lad.size[fk - 1] / 8};
+}
 
 // out->path of a ladder measurement that runs on the handle's data path (CDPROBE_OPT_PATH).
 constexpr uint32_t kHandlePath = UINT32_MAX;
@@ -426,6 +452,45 @@ static int launch_ladder(cdprobe* h, LocalRank& L, Params& p, const Ladder& lad,
   return e != cudaSuccess ? fail_sticky(h, what, e) : CDPROBE_OK;
 }
 
+// [local rank][rank][size]: the (S, X) each size of each cell of bwcurve or memcpy must give.
+using CellSums = uint64_t[kMaxRanks][kBwMaxSizes][2];
+// *want[li][j] for every cell that runs: expected_sums of the source slice its op moves (memcpy_cell; bwcurve reads the
+// slice a pull copies), on the issuer's GPU, with the granule table at table_off of its scratch, grown to hold it.
+static int cell_sums(cdprobe* h, const bool (*runs)[kMaxRanks], uint32_t op, size_t table_off, const Ladder& lad,
+                     const char* what, std::unique_ptr<CellSums[]>* want) {
+  if (const int rc = ensure_scratch_all(h, table_off + 16 * (h->plan.bpp / kGranuleBytes)); rc != CDPROBE_OK) return rc;
+  *want = std::make_unique<CellSums[]>(kMaxRanks);
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    for (uint32_t j = 0; j < h->n_total; ++j) {
+      if (!runs[li][j]) continue;
+      const MemcpyCell c = memcpy_cell(h->plan, op, h->lr[li].grank, j);
+      const int rc = expected_sums(h, h->lr[li], table_off, SrcRegionWord{h->seed, c.first_word, c.src_rank}, lad.size,
+                                   lad.n_sizes, (*want)[li][j], what);
+      if (rc != CDPROBE_OK) return rc;
+    }
+  }
+  return CDPROBE_OK;
+}
+
+// The rounds of bwcurve and memcpy, the tournament's then the loop-back, each behind a domain barrier: round(target),
+// target[li] the rank local rank li's cell of the round reaches, -1 when it has none that runs.
+template <typename Round>
+static int walk_rounds(cdprobe* h, const bool (*runs)[kMaxRanks], const Round& round) {
+  const Plan& pl = h->plan;
+  const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
+  for (uint32_t r = 0; r < n_rounds; ++r) {
+    if (const int rc = domain_barrier(h); rc != CDPROBE_OK) return rc;
+    int32_t target[kMaxRanks];
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      const uint32_t g = h->lr[li].grank;
+      const int q = r < pl.rounds ? pl.partner[r][g] : (int)g;
+      target[li] = q >= 0 && runs[li][q] ? q : -1;
+    }
+    if (const int rc = round(target); rc != CDPROBE_OK) return rc;
+  }
+  return CDPROBE_OK;
+}
+
 // The skip rule of the all-reduces, on the domain's mapping status st ([rank][rank], 0: up): a process that ran while
 // another skipped would wait at the first domain barrier until its watchdog fired, so when some rank cannot reach some
 // other nothing runs, in any process: every local row gets the status of the domain's first down cell, row-major.
@@ -452,15 +517,8 @@ static int collect_rows(cdprobe* h, const uint64_t (*want)[2], const Ladder& lad
     if (const int rc = fetch_reps(h, L, got.get(), 1, what); rc != CDPROBE_OK) return rc;
     const ArScratch& s = *got;
     bw_summarize(s.rep, want, lad.size, lad.n_sizes, lad.reps, g, out);
-    if (out->status[g] == CDPROBE_ERR_TIMEOUT) continue;
-    for (uint32_t k = 0; k < lad.n_sizes; ++k) {
-      out->bad_words[g][k] = s.bad_words[k];
-      out->first_bad[g][k] = s.bad_words[k] != 0 ? ~s.first_bad_n[k] : UINT64_MAX;
-      if (s.bad_words[k] != 0) {
-        out->bad_sizes[g] |= 1u << k;
-        out->status[g] = CDPROBE_ERR_INTEGRITY;
-      }
-    }
+    if (out->status[g] != CDPROBE_ERR_TIMEOUT)
+      word_checks(s.bad_words, s.first_bad_n, lad.n_sizes, g, &out->status[g], out);
   }
   return CDPROBE_OK;
 }
@@ -471,10 +529,11 @@ static DomainLines domain_lines(const cdprobe* h, const LocalRank& L, uint64_t o
   DomainLines d;
   memset(&d, 0, sizeof(d));
   const uint32_t g = L.grank;
+  const CUdeviceptr* va = h->mem.va[g - h->first];
   for (uint32_t j = 0; j < h->n_total; ++j) {
     if (j == g) continue;
-    d.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + off + (uint64_t)g * sizeof(FlagLine));
-    d.sig_in[j] = reinterpret_cast<const uint64_t*>(L.va[g] + off + (uint64_t)j * sizeof(FlagLine));
+    d.sig_out[j] = reinterpret_cast<uint64_t*>(va[j] + off + (uint64_t)g * sizeof(FlagLine));
+    d.sig_in[j] = reinterpret_cast<const uint64_t*>(va[g] + off + (uint64_t)j * sizeof(FlagLine));
   }
   d.call_seq = call_seq;
   return d;
@@ -501,8 +560,8 @@ struct ArProtocol {
   const char* zeroing;                           // the area must start zeroed: names the step in a CUDA failure
   bool out_in_scratch;                           // the output takes s_max bytes of the scratch at kArOutOff
   uint64_t lines;                                // its barrier lines in the Ctrl granule
-  // the fault's verdict for this call: nullptr with *f filled, or the refusal
-  const char* (*decode)(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f);
+  // the verdict on fault v, whose size and word are `at`, for this call: nullptr with *f filled, or the refusal
+  const char* (*decode)(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder& lad, ArFault* f);
   // fills its parameters for local rank L and launches its kernel (launch_ladder)
   int (*launch)(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f, uint32_t grid);
   bool native = false;                           // it adds into peers' memory: every pair needs native atomics
@@ -523,19 +582,20 @@ static Params ar_params(const cdprobe* h, const LocalRank& L, const DomainLines&
   return p;
 }
 
-static const char* oneshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
-  const uint64_t fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
-  if ((v >> 49) != 0 || fr == 0 || fr > h->n_total || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+static const char* oneshot_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder&, ArFault* f) {
+  const uint64_t fr = (v >> 32) & 0xffffu;
+  if ((v >> 49) != 0 || fr == 0 || fr > h->n_total || !at.word_ok)
     return "the armed all-reduce fault names no rank, size or output word of this call";
-  *f = {(uint32_t)fr - 1, 0, (uint32_t)fk - 1, (uint32_t)(v >> 48), word};
+  *f = {(uint32_t)fr - 1, 0, at.k, (uint32_t)(v >> 48), at.word};
   return nullptr;
 }
 
 static int oneshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                           uint32_t) {
-  const uint32_t g = L.grank, n = h->n_total;
+  const uint32_t g = L.grank, n = h->n_total, li = g - h->first;
   AllReduceParams p = ar_params<AllReduceParams>(h, L, dom, f);
-  for (uint32_t t = 0; t < n; ++t) p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
+  for (uint32_t t = 0; t < n; ++t)
+    p.src[t] = reinterpret_cast<const uint8_t*>(h->mem.va[li][(g + t) % n]) + h->plan.src_off;
   p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
   p.fault_word = f.word;
   p.fault_drop = f.mode;
@@ -543,13 +603,13 @@ static int oneshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, cons
 }
 
 // The fault acts in the rank whose chunk holds its word.
-static const char* twoshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+static const char* twoshot_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder& lad, ArFault* f) {
   const uint32_t n = h->n_total;
-  const uint64_t fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
-  if ((v >> 49) != 0 || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+  const uint64_t fr = (v >> 32) & 0xffffu;
+  if ((v >> 49) != 0 || fr == 0 || fr > n || !at.word_ok)
     return "the armed two-shot all-reduce fault names no receiver, size or output word of this call";
-  *f = {kArNoFault, (uint32_t)fr - 1, (uint32_t)fk - 1, (uint32_t)(v >> 48), word};
-  const uint64_t units = (lad.size[f->k] + kUnitBytes - 1) / kUnitBytes, u = word / (kUnitBytes / 8);
+  *f = {kArNoFault, (uint32_t)fr - 1, at.k, (uint32_t)(v >> 48), at.word};
+  const uint64_t units = (lad.size[f->k] + kUnitBytes - 1) / kUnitBytes, u = at.word / (kUnitBytes / 8);
   for (uint32_t r = 0; r < n; ++r) {
     uint64_t lo, hi;
     twoshot_chunk(units, n, r, &lo, &hi);
@@ -560,11 +620,11 @@ static const char* twoshot_fault(const cdprobe* h, uint64_t v, const Ladder& lad
 
 static int twoshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                           uint32_t) {
-  const uint32_t g = L.grank, n = h->n_total;
+  const uint32_t g = L.grank, n = h->n_total, li = g - h->first;
   TwoShotParams p = ar_params<TwoShotParams>(h, L, dom, f);
   for (uint32_t t = 0; t < n; ++t) {
-    p.src[t] = reinterpret_cast<const uint8_t*>(L.va[(g + t) % n]) + h->plan.src_off;
-    p.dst[t] = reinterpret_cast<uint8_t*>(L.gather_va[(g + t) % n]);
+    p.src[t] = reinterpret_cast<const uint8_t*>(h->mem.va[li][(g + t) % n]) + h->plan.src_off;
+    p.dst[t] = reinterpret_cast<uint8_t*>(h->gather.va[li][(g + t) % n]);
   }
   p.fault_word = f.word;
   p.fault_dst = (f.recv + n - g) % n;
@@ -573,26 +633,24 @@ static int twoshot_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, cons
 }
 
 // The fault acts in the process that hosts its sender, which for mode 2 is its receiver.
-static const char* ll_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+static const char* ll_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder&, ArFault* f) {
   const uint32_t n = h->n_total;
-  const uint64_t mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu, fk = (v >> 24) & 0xffu,
-                 arg = v & 0xffffffu;
-  if (mode > 2 || fs == 0 || fs > n || fr == 0 || fr > n || fk == 0 || fk > lad.n_sizes ||
-      (mode != 1 && arg >= lad.size[fk - 1] / 8) || (mode == 0 && fs == fr) || (mode == 2 && fs != fr) ||
-      (mode == 1 && 2 * arg >= 1000ull * h->cfg.timeout_ms))
+  const uint64_t mode = v >> 48, fs = (v >> 40) & 0xffu, fr = (v >> 32) & 0xffu;
+  if (mode > 2 || fs == 0 || fs > n || fr == 0 || fr > n || !at.size_ok || (mode != 1 && !at.word_ok) ||
+      (mode == 0 && fs == fr) || (mode == 2 && fs != fr) || (mode == 1 && 2 * at.word >= 1000ull * h->cfg.timeout_ms))
     return "the armed LL all-reduce fault names no packet, size or delay of this call";
-  *f = {(uint32_t)fs - 1, (uint32_t)fr - 1, (uint32_t)fk - 1, (uint32_t)mode, arg};
+  *f = {(uint32_t)fs - 1, (uint32_t)fr - 1, at.k, (uint32_t)mode, at.word};
   return nullptr;
 }
 
 // Every rank splits the words over the domain's smallest grid, so that each word has the same owner everywhere.
 static int ll_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                      uint32_t grid) {
-  const uint32_t g = L.grank, n = h->n_total;
+  const uint32_t g = L.grank, n = h->n_total, li = g - h->first;
   LlParams p = ar_params<LlParams>(h, L, dom, f);
-  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
-  for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.ll_va[(g + t) % n]);
-  p.in = reinterpret_cast<const uint8_t*>(L.ll_va[g]);
+  p.src = reinterpret_cast<const uint8_t*>(h->mem.va[li][g]) + h->plan.src_off;
+  for (uint32_t t = 1; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(h->ll.va[li][(g + t) % n]);
+  p.in = reinterpret_cast<const uint8_t*>(h->ll.va[li][g]);
   p.out = static_cast<uint8_t*>(L.scratch) + kArOutOff;
   p.s_max = lad.size[lad.n_sizes - 1];
   p.fault_mode = f.mode;
@@ -605,32 +663,31 @@ static int ll_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Lad
 // The fault acts in the process that hosts its sender.  A corrupted or dropped word must lie in a chunk the sender
 // pushes in that phase: every chunk but its own in the reduce-scatter, every chunk but its successor's in the
 // all-gather.
-static const char* ring_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+static const char* ring_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder& lad, ArFault* f) {
   const uint32_t n = h->n_total;
-  const uint64_t mode = v >> 48, phase = (v >> 40) & 0xffu, fs = (v >> 32) & 0xffu, fk = (v >> 24) & 0xffu,
-                 arg = v & 0xffffffu;
+  const uint64_t mode = v >> 48, phase = (v >> 40) & 0xffu, fs = (v >> 32) & 0xffu;
   const char* why = "the armed ring all-reduce fault names no pushed word, size or delay of this call";
-  if (mode > 2 || phase > 1 || fs == 0 || fs > n || fk == 0 || fk > lad.n_sizes) return why;
-  const uint32_t s = (uint32_t)fs - 1, k = (uint32_t)fk - 1;
-  if (mode == 2 && 2 * arg >= 1000ull * h->cfg.timeout_ms) return why;
+  if (mode > 2 || phase > 1 || fs == 0 || fs > n || !at.size_ok) return why;
+  const uint32_t s = (uint32_t)fs - 1, k = at.k;
+  if (mode == 2 && 2 * at.word >= 1000ull * h->cfg.timeout_ms) return why;
   if (mode < 2) {
-    if (n == 1 || arg >= lad.size[k] / 8) return why;
-    const uint64_t units = (lad.size[k] + kUnitBytes - 1) / kUnitBytes, u = arg / (kUnitBytes / 8);
+    if (n == 1 || !at.word_ok) return why;
+    const uint64_t units = (lad.size[k] + kUnitBytes - 1) / kUnitBytes, u = at.word / (kUnitBytes / 8);
     uint64_t lo, hi;
     twoshot_chunk(units, n, phase == 0 ? s : (s + 1) % n, &lo, &hi);
     if (u >= lo && u < hi) return why;
   }
-  *f = {s, 0, k, (uint32_t)mode, arg, (uint32_t)phase};
+  *f = {s, 0, k, (uint32_t)mode, at.word, (uint32_t)phase};
   return nullptr;
 }
 
 static int ring_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                        uint32_t) {
-  const uint32_t g = L.grank, n = h->n_total;
+  const uint32_t g = L.grank, n = h->n_total, li = g - h->first;
   RingParams p = ar_params<RingParams>(h, L, dom, f);
-  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
-  p.out = reinterpret_cast<uint8_t*>(L.ring_va[g]);
-  p.next = reinterpret_cast<uint8_t*>(L.ring_va[(g + 1) % n]);
+  p.src = reinterpret_cast<const uint8_t*>(h->mem.va[li][g]) + h->plan.src_off;
+  p.out = reinterpret_cast<uint8_t*>(h->ring.va[li][g]);
+  p.next = reinterpret_cast<uint8_t*>(h->ring.va[li][(g + 1) % n]);
   p.s_max = lad.size[lad.n_sizes - 1];
   p.fault_mode = f.mode;
   p.fault_phase = f.phase;
@@ -640,31 +697,31 @@ static int ring_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
 
 // Modes 0-2 act in the process that hosts the sender `rank`; mode 3 in the one that hosts the owner of the word's chunk,
 // towards receiver `rank`, which must be a peer of that owner.
-static const char* push_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
+static const char* push_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder& lad, ArFault* f) {
   const uint32_t n = h->n_total;
-  const uint64_t mode = v >> 48, fr = (v >> 32) & 0xffffu, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+  const uint64_t mode = v >> 48, fr = (v >> 32) & 0xffffu;
   if (mode > 3) return "the armed push all-reduce fault has a mode above 3";
   if (fr == 0 || fr > n) return "the armed push all-reduce fault names no rank of this domain";
-  if (fk == 0 || fk > lad.n_sizes) return "the armed push all-reduce fault names no size of this call";
-  if (word >= lad.size[fk - 1] / 8) return "the armed push all-reduce fault names no output word of its size";
-  const uint32_t r = (uint32_t)fr - 1, k = (uint32_t)fk - 1;
+  if (!at.size_ok) return "the armed push all-reduce fault names no size of this call";
+  if (!at.word_ok) return "the armed push all-reduce fault names no output word of its size";
+  const uint32_t r = (uint32_t)fr - 1, k = at.k;
   if (mode < 3) {
-    *f = {r, 0, k, (uint32_t)mode, word};
+    *f = {r, 0, k, (uint32_t)mode, at.word};
     return nullptr;
   }
   if (n == 1) return "the armed push all-reduce fault's mode 3 has no peer to push to at n == 1";
-  const uint32_t owner = twoshot_owner((lad.size[k] + kUnitBytes - 1) / kUnitBytes, n, word / (kUnitBytes / 8));
+  const uint32_t owner = twoshot_owner((lad.size[k] + kUnitBytes - 1) / kUnitBytes, n, at.word / (kUnitBytes / 8));
   if (owner == r) return "the armed push all-reduce fault's mode-3 receiver owns the word and is pushed no copy of it";
-  *f = {owner, r, k, 3u, word};
+  *f = {owner, r, k, 3u, at.word};
   return nullptr;
 }
 
 static int push_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const Ladder& lad, const ArFault& f,
                        uint32_t) {
-  const uint32_t g = L.grank, n = h->n_total;
+  const uint32_t g = L.grank, n = h->n_total, li = g - h->first;
   PushParams p = ar_params<PushParams>(h, L, dom, f);
-  p.src = reinterpret_cast<const uint8_t*>(L.va[g]) + h->plan.src_off;
-  for (uint32_t t = 0; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(L.push_va[(g + t) % n]);
+  p.src = reinterpret_cast<const uint8_t*>(h->mem.va[li][g]) + h->plan.src_off;
+  for (uint32_t t = 0; t < n; ++t) p.dst[t] = reinterpret_cast<uint8_t*>(h->push.va[li][(g + t) % n]);
   p.fault_word = f.word;
   p.fault_mode = f.mode;
   p.fault_dst = (f.recv + n - g) % n;
@@ -672,15 +729,14 @@ static int push_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
 }
 
 // The fault acts in the process that hosts the owner of the word's chunk.
-static const char* nvls_fault(const cdprobe* h, uint64_t v, const Ladder& lad, ArFault* f) {
-  const uint64_t mode = v >> 48, fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
+static const char* nvls_fault(const cdprobe* h, uint64_t v, const FaultSpot& at, const Ladder& lad, ArFault* f) {
+  const uint64_t mode = v >> 48;
   if (mode > 1) return "the armed NVLS all-reduce fault has a mode above 1";
   if (((v >> 32) & 0xffffu) != 0) return "the armed NVLS all-reduce fault sets bits 32 to 47, which name nothing";
-  if (fk == 0 || fk > lad.n_sizes) return "the armed NVLS all-reduce fault names no size of this call";
-  if (word >= lad.size[fk - 1] / 8) return "the armed NVLS all-reduce fault names no output word of its size";
-  const uint32_t k = (uint32_t)fk - 1;
-  const uint64_t units = (lad.size[k] + kUnitBytes - 1) / kUnitBytes;
-  *f = {twoshot_owner(units, h->n_total, word / (kUnitBytes / 8)), 0, k, (uint32_t)mode, word};
+  if (!at.size_ok) return "the armed NVLS all-reduce fault names no size of this call";
+  if (!at.word_ok) return "the armed NVLS all-reduce fault names no output word of its size";
+  const uint64_t units = (lad.size[at.k] + kUnitBytes - 1) / kUnitBytes;
+  *f = {twoshot_owner(units, h->n_total, at.word / (kUnitBytes / 8)), 0, at.k, (uint32_t)mode, at.word};
   return nullptr;
 }
 
@@ -730,7 +786,7 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   //    and is yet to be created is stale until it is zeroed
   ArFault f;
   if (h->*P.fault != 0 && lad.bad.empty())
-    if (const char* why = P.decode(h, h->*P.fault, lad, &f)) lad.bad = why;
+    if (const char* why = P.decode(h, h->*P.fault, fault_spot(h->*P.fault, lad), lad, &f)) lad.bad = why;
   SharedAlloc* m = P.area != nullptr ? &(h->*P.area) : nullptr;
   if (P.zeroing != nullptr) m->stale |= m->bytes == 0;
   bool zero = P.zeroing != nullptr && m->stale;
@@ -776,7 +832,7 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
     for (uint32_t li = 0; li < h->n_local; ++li) {
       LocalRank& L = h->lr[li];
       CDP_RT(cudaSetDevice(L.ordinal));
-      cudaError_t e = cudaMemsetAsync(reinterpret_cast<void*>((L.*m->va)[L.grank]), 0, m->bytes, L.stream);
+      cudaError_t e = cudaMemsetAsync(reinterpret_cast<void*>(m->va[li][L.grank]), 0, m->bytes, L.stream);
       if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
       if (e != cudaSuccess) return fail_sticky(h, P.zeroing, e);
     }
@@ -788,8 +844,8 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
       LocalRank& L = h->lr[li];
       CDP_RT(cudaSetDevice(L.ordinal));
       void* const in = reinterpret_cast<void*>(h->nvls.uc_va[li]);
-      cudaError_t e = cudaMemcpyAsync(in, reinterpret_cast<const void*>(L.va[L.grank] + h->plan.src_off), s_max,
-                                      cudaMemcpyDeviceToDevice, L.stream);
+      const void* const src = reinterpret_cast<const void*>(h->mem.va[li][L.grank] + h->plan.src_off);
+      cudaError_t e = cudaMemcpyAsync(in, src, s_max, cudaMemcpyDeviceToDevice, L.stream);
       if (e == cudaSuccess) e = cudaMemsetAsync(static_cast<uint8_t*>(in) + s_max, 0, s_max, L.stream);
       if (e == cudaSuccess) e = cudaStreamSynchronize(L.stream);
       if (e != cudaSuccess) return fail_sticky(h, "cdprobe_allreduce_nvls: fill the NVLS area", e);
@@ -867,11 +923,10 @@ struct MemcpyHost {
 // Where cdprobe_memcpy keeps its device state in a local rank's scratch: the BwScratch of the (S, X) read at 0, the
 // diagnosis of a destination of up to bytes_per_pair at diag_off, the granule table of expected_sums at table_off.
 struct MemcpyScratch {
-  size_t diag_off, table_off, bytes;
+  size_t diag_off, table_off;
   explicit MemcpyScratch(uint64_t bpp) {
     diag_off = (sizeof(BwScratch) + 255) / 256 * 256;
     table_off = diag_off + (diag_scratch_bytes(bpp) + 255) / 256 * 256;
-    bytes = table_off + 16 * (bpp / kGranuleBytes);
   }
 };
 
@@ -899,11 +954,12 @@ static int memcpy_setup(cdprobe* h) {
   return CDPROBE_OK;
 }
 
-// The timed part of rep `rep` of cdprobe_memcpy's cell (L.grank, j), queued on L's stream: the wait for the rep's
-// ticket, event A, the copy (none when `drop`), event B.  A failure of the stream wait itself is cudaErrorUnknown with
-// the driver's result in *cu.
-static cudaError_t memcpy_timed(cdprobe* h, LocalRank& L, uint32_t j, uint32_t op, uint64_t ticket, uint64_t bytes,
+// The timed part of rep `rep` of cdprobe_memcpy's cell (L.grank, j), L = h->lr[li], queued on L's stream: the wait
+// for the rep's ticket, event A, the copy (none when `drop`), event B.  A failure of the stream wait itself is
+// cudaErrorUnknown with the driver's result in *cu.
+static cudaError_t memcpy_timed(cdprobe* h, uint32_t li, uint32_t j, uint32_t op, uint64_t ticket, uint64_t bytes,
                                 uint32_t rep, bool drop, CUresult* cu) {
+  LocalRank& L = h->lr[li];
   const MemcpyCell c = memcpy_cell(h->plan, op, L.grank, j);
   cudaError_t e = cudaSetDevice(L.ordinal);
   if (e != cudaSuccess) return e;
@@ -912,9 +968,9 @@ static cudaError_t memcpy_timed(cdprobe* h, LocalRank& L, uint32_t j, uint32_t o
   if (*cu != CUDA_SUCCESS) return cudaErrorUnknown;
   e = cudaEventRecord(L.memcpy_ev[2 * rep], L.stream);
   if (e == cudaSuccess && !drop)
-    e = cudaMemcpyAsync(reinterpret_cast<void*>(L.area_va[c.dst_rank] + c.dst_off),
-                        reinterpret_cast<const void*>(L.va[c.src_rank] + c.src_off), bytes, cudaMemcpyDeviceToDevice,
-                        L.stream);
+    e = cudaMemcpyAsync(reinterpret_cast<void*>(h->area.va[li][c.dst_rank] + c.dst_off),
+                        reinterpret_cast<const void*>(h->mem.va[li][c.src_rank] + c.src_off), bytes,
+                        cudaMemcpyDeviceToDevice, L.stream);
   if (e == cudaSuccess) e = cudaEventRecord(L.memcpy_ev[2 * rep + 1], L.stream);
   return e;
 }
@@ -923,14 +979,15 @@ static cudaError_t memcpy_timed(cdprobe* h, LocalRank& L, uint32_t j, uint32_t o
 // (`flip`: word flip_word), the diagnosis of every destination word against the source slice's pattern (diag_launch),
 // the (S, X) read of the destination (bwcurve_kernel, one rep of one size), the clearing of the destination to 0, and
 // the copies of what the checks left into rep's slot of the host block.
-static cudaError_t memcpy_check(cdprobe* h, LocalRank& L, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes,
-                                uint32_t rep, bool flip, uint64_t flip_word) {
+static cudaError_t memcpy_check(cdprobe* h, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes, uint32_t rep,
+                                bool flip, uint64_t flip_word) {
+  LocalRank& L = h->lr[li];
   const Plan& pl = h->plan;
   const MemcpyCell c = memcpy_cell(pl, op, L.grank, j);
   const MemcpyScratch ms(pl.bpp);
   MemcpyHost* const host = h->memcpy_host;
   MemcpyRepOut* const got = &host->rep[li][rep];
-  uint8_t* const dst = reinterpret_cast<uint8_t*>(L.area_va[c.dst_rank] + c.dst_off);
+  uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
   uint8_t* const scratch = static_cast<uint8_t*>(L.scratch);
   cudaStream_t s = L.stream;
   cudaError_t e = cudaSetDevice(L.ordinal);
@@ -981,7 +1038,7 @@ static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladd
   CUresult cu = CUDA_SUCCESS;
   for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
     if (target[li] >= 0)
-      e = memcpy_timed(h, h->lr[li], (uint32_t)target[li], op, ticket, bytes, rep, armed(li) && f.mode == 1, &cu);
+      e = memcpy_timed(h, li, (uint32_t)target[li], op, ticket, bytes, rep, armed(li) && f.mode == 1, &cu);
   __atomic_store_n(&h->memcpy_host->ticket, ticket, __ATOMIC_RELEASE);
   if (cu != CUDA_SUCCESS) {
     h->sticky = true;
@@ -1005,7 +1062,7 @@ static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladd
   }
   for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
     if (target[li] >= 0)
-      e = memcpy_check(h, h->lr[li], li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.word);
+      e = memcpy_check(h, li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.word);
   return e != cudaSuccess ? fail_sticky(h, "cdprobe_memcpy: queue the checks", e) : CDPROBE_OK;
 }
 
@@ -1073,7 +1130,7 @@ int cdprobe_diagnose(cdprobe_t* h, uint32_t op, uint32_t issuer, uint32_t target
 
   CDP_RT(cudaSetDevice(L.ordinal));
   if (const int rc = cdp::ensure_scratch(L, cdp::diag_scratch_bytes(pl.bpp)); rc != CDPROBE_OK) return rc;
-  const uint8_t* region = reinterpret_cast<const uint8_t*>(L.va[target]) + out->region_offset;
+  const uint8_t* region = reinterpret_cast<const uint8_t*>(h->mem.va[reader - h->first][target]) + out->region_offset;
   cdp::DiagOut d;
   float ms = 0.f;
   cudaError_t e = cudaEventRecord(L.ev0, L.stream);
@@ -1134,7 +1191,7 @@ int cdprobe_latency(cdprobe_t* h, uint32_t hops, uint32_t reps, cdprobe_latency_
       if (!cdp::live_cell(h, li, j, out->status)) continue;
       cells[li].add(p.n_cells, g * CDPROBE_MAX_GPUS + j);
       cdp::LatencyCell& c = p.cell[p.n_cells++];
-      c.region = reinterpret_cast<const uint8_t*>(L.va[j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
+      c.region = reinterpret_cast<const uint8_t*>(h->mem.va[li][j]) + cdp::cell_offset(pl, CDPROBE_OP_READ, g, j);
       c.lines = lines;
       c.issuer = g;
       c.target = j;
@@ -1230,8 +1287,9 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
       const int q = pl.partner[r][g];
       if (q < 0 || pair_status(g, (uint32_t)q) != 0) continue;
       cdp::PingPongRound& R = p.round[r];
-      R.remote = reinterpret_cast<uint64_t*>(L.va[q] + cdp::kPingOff + (uint64_t)g * sizeof(cdp::FlagLine));
-      R.local = reinterpret_cast<const uint64_t*>(L.va[g] + cdp::kPingOff + (uint64_t)q * sizeof(cdp::FlagLine));
+      R.remote = reinterpret_cast<uint64_t*>(h->mem.va[li][q] + cdp::kPingOff + (uint64_t)g * sizeof(cdp::FlagLine));
+      R.local =
+          reinterpret_cast<const uint64_t*>(h->mem.va[li][g] + cdp::kPingOff + (uint64_t)q * sizeof(cdp::FlagLine));
       R.partner = (uint32_t)q;
       R.first = g < (uint32_t)q ? 1u : 0u;
       if (g == f_target && (uint32_t)q == f_init) p.fault_round = r;
@@ -1326,7 +1384,8 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
       if (g == f_issuer && j == f_target) p.fault_cell = p.n_cells;
       cells[li].add(p.n_cells, idx);
       cdp::AtomicsCell& c = p.cell[p.n_cells++];
-      c.word = reinterpret_cast<unsigned long long*>(L.va[j] + cdp::kAtomOff + (uint64_t)g * sizeof(cdp::AtomLine));
+      c.word =
+          reinterpret_cast<unsigned long long*>(h->mem.va[li][j] + cdp::kAtomOff + (uint64_t)g * sizeof(cdp::AtomLine));
       c.issuer = g;
       c.target = j;
     }
@@ -1361,47 +1420,28 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   out->call_seq = ++h->bw_calls;
   cdp::put_ladder(h, lad, out);
 
-  // 2. scratch for the rep records and one cell's granule table, grown on every local rank before any kernel runs
-  const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
-  const size_t scratch = table_off + 16 * (pl.bpp / cdp::kGranuleBytes);
-  if (const int rc = cdp::ensure_scratch_all(h, scratch); rc != CDPROBE_OK) return rc;
-
-  // 3. the (S, X) each size of each cell that runs must read, from the pattern definition: the per-granule sums of the
-  //    slice on the issuer's GPU, folded into every prefix on the host
+  // 2. which cells run; scratch for the rep records and one cell's granule table, grown on every local rank before any
+  //    kernel runs, and the (S, X) each size of each cell that runs must read, from the pattern definition
   bool runs[cdp::kMaxRanks][cdp::kMaxRanks] = {};
-  std::vector<uint64_t> want((size_t)cdp::kMaxRanks * cdp::kMaxRanks * cdp::kBwMaxSizes * 2);
-  auto want_of = [&](uint32_t li, uint32_t j) {
-    return reinterpret_cast<uint64_t(*)[2]>(want.data() + ((size_t)li * cdp::kMaxRanks + j) * cdp::kBwMaxSizes * 2);
-  };
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    const uint32_t g = L.grank;
-    for (uint32_t j = 0; j < n; ++j) {
-      if (!cdp::live_cell(h, li, j, out->status)) continue;
-      runs[li][j] = true;
-      const cdp::SrcRegionWord word{h->seed, (uint64_t)cdp::cell_slice(pl, g, j) * (pl.bpp / 8), j};
-      if (const int rc = cdp::expected_sums(h, L, table_off, word, lad.size, lad.n_sizes, want_of(li, j),
-                                            "cdprobe_bwcurve: granule checksums");
-          rc != CDPROBE_OK)
-        return rc;
-    }
-  }
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < n; ++j) runs[li][j] = cdp::live_cell(h, li, j, out->status);
+  const size_t table_off = (sizeof(cdp::BwScratch) + 255) / 256 * 256;
+  std::unique_ptr<cdp::CellSums[]> want;
+  if (const int rc = cdp::cell_sums(h, runs, CDPROBE_OP_READ, table_off, lad, "cdprobe_bwcurve: granule checksums",
+                                    &want);
+      rc != CDPROBE_OK)
+    return rc;
 
-  // 4. the rounds: the tournament's, then the loop-back; every local kernel of a round is launched before any is
-  //    waited for, and no process starts a round before every process has finished the one before
+  // 3. the rounds: every local kernel of a round is launched before any is waited for
   auto got = std::make_unique<cdp::BwScratch>();
-  const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
-  for (uint32_t r = 0; r < n_rounds; ++r) {
-    if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-    int32_t target[cdp::kMaxRanks];
+  const auto round = [&](const int32_t* target) -> int {
     for (uint32_t li = 0; li < h->n_local; ++li) {
-      cdp::LocalRank& L = h->lr[li];
-      const int q = r < pl.rounds ? pl.partner[r][L.grank] : (int)L.grank;
-      target[li] = q >= 0 && runs[li][q] ? q : -1;
       if (target[li] < 0) continue;
+      cdp::LocalRank& L = h->lr[li];
+      const uint32_t q = (uint32_t)target[li];
       cdp::BwCurveParams p;
       memset(&p, 0, sizeof(p));
-      p.region = reinterpret_cast<const uint8_t*>(L.va[q]) + cdp::cell_offset(pl, CDPROBE_OP_READ, L.grank, (uint32_t)q);
+      p.region = reinterpret_cast<const uint8_t*>(h->mem.va[li][q]) + cdp::cell_offset(pl, CDPROBE_OP_READ, L.grank, q);
       if (const int rc = cdp::launch_ladder(h, L, p, lad, cdp::bwcurve_launch, "launch bwcurve_kernel");
           rc != CDPROBE_OK)
         return rc;
@@ -1410,10 +1450,12 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
       if (target[li] < 0) continue;
       cdp::LocalRank& L = h->lr[li];
       if (const int rc = cdp::fetch_reps(h, L, got.get(), 1, "cdprobe_bwcurve"); rc != CDPROBE_OK) return rc;
-      cdp::bw_summarize(*got, want_of(li, (uint32_t)target[li]), lad.size, lad.n_sizes, lad.reps,
+      cdp::bw_summarize(*got, want[li][target[li]], lad.size, lad.n_sizes, lad.reps,
                         L.grank * CDPROBE_MAX_GPUS + (uint32_t)target[li], out);
     }
-  }
+    return CDPROBE_OK;
+  };
+  if (const int rc = cdp::walk_rounds(h, runs, round); rc != CDPROBE_OK) return rc;
   out->ms = cdp::now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }
@@ -1452,15 +1494,15 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   uint32_t f_send = cdp::kA2aNoFault, f_recv = cdp::kA2aNoFault, f_k = cdp::kA2aNoFault;
   uint64_t f_word = 0;
   if (h->a2a_fault != 0 && lad.bad.empty()) {
-    const uint64_t fs = h->a2a_fault >> 40, fr = (h->a2a_fault >> 32) & 0xffu, fk = (h->a2a_fault >> 24) & 0xffu;
-    f_word = h->a2a_fault & 0xffffffu;
-    if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || fk == 0 || fk > lad.n_sizes ||
-        f_word >= lad.size[fk - 1] / 8) {
+    const uint64_t fs = h->a2a_fault >> 40, fr = (h->a2a_fault >> 32) & 0xffu;
+    const cdp::FaultSpot at = cdp::fault_spot(h->a2a_fault, lad);
+    f_word = at.word;
+    if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || !at.word_ok) {
       lad.bad = "the armed all-to-all fault names no cell, size or word of this call";
     } else {
       f_send = (uint32_t)fs - 1;
       f_recv = (uint32_t)fr - 1;
-      f_k = (uint32_t)fk - 1;
+      f_k = at.k;
     }
   }
   int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
@@ -1506,6 +1548,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   for (uint32_t li = 0; li < h->n_local; ++li) {
     cdp::LocalRank& L = h->lr[li];
     const uint32_t g = L.grank;
+    const CUdeviceptr* va = h->mem.va[li];
     cdp::AllToAllParams p;
     memset(&p, 0, sizeof(p));
     // the barrier: with every rank a cell joins to this one; rank j pushes to this rank when it maps it, else this
@@ -1515,13 +1558,13 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
       if (j == g || !(runs(g, j) || runs(j, g))) continue;
       joined = true;
       if (runs(g, j))
-        p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(L.va[j] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
+        p.dom.sig_out[j] = reinterpret_cast<uint64_t*>(va[j] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
       p.dom.sig_in[j] = reinterpret_cast<const uint64_t*>(
-          runs(j, g) ? L.va[g] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine)
-                     : L.va[j] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine));
+          runs(j, g) ? va[g] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine)
+                     : va[j] + cdp::kA2aOff + (uint64_t)j * sizeof(cdp::FlagLine));
     }
     if (!joined) continue;
-    p.dom.self = reinterpret_cast<uint64_t*>(L.va[g] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
+    p.dom.self = reinterpret_cast<uint64_t*>(va[g] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
     p.dom.call_seq = h->a2a_calls;
     // the blocks, in the order rank + 1, rank + 2, ... (mod n), then the diagonal
     p.fault_k = cdp::kA2aNoFault;
@@ -1534,12 +1577,12 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
         p.fault_word = f_word;
       }
       p.to[p.blocks] = j;
-      p.dst[p.blocks++] = reinterpret_cast<uint8_t*>(L.area_va[j]) + (uint64_t)g * pl.bpp;
+      p.dst[p.blocks++] = reinterpret_cast<uint8_t*>(h->area.va[li][j]) + (uint64_t)g * pl.bpp;
     }
     for (uint32_t s = 0; s < n; ++s) {
       if (!runs(s, g)) continue;
       p.from[p.n_in] = s;
-      p.in[p.n_in++] = reinterpret_cast<const uint8_t*>(L.area_va[g]) + (uint64_t)s * pl.bpp;
+      p.in[p.n_in++] = reinterpret_cast<const uint8_t*>(h->area.va[li][g]) + (uint64_t)s * pl.bpp;
     }
     p.seed = h->seed;
     p.rank = g;
@@ -1568,13 +1611,10 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
         continue;
       }
       for (uint32_t k = 0; k < lad.n_sizes; ++k) {
-        out->bad_words[cell][k] = s.bad_words[i][k];
-        out->first_bad[cell][k] = s.bad_words[i][k] != 0 ? ~s.first_bad_n[i][k] : UINT64_MAX;
         out->sum[cell][k] = s.sum[i][k];
         out->xr[cell][k] = s.xr[i][k];
-        if (s.bad_words[i][k] != 0) out->bad_sizes[cell] |= 1u << k;
       }
-      out->cell_status[cell] = out->bad_sizes[cell] ? CDPROBE_ERR_INTEGRITY : 0;
+      cdp::word_checks(s.bad_words[i], s.first_bad_n[i], lad.n_sizes, cell, &out->cell_status[cell], out);
     }
   }
   out->ms = cdp::now_ms() - lad.t_begin;
@@ -1594,13 +1634,12 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
     lad.bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
   cdp::MemcpyFault f;
   if (h->memcpy_fault != 0 && lad.bad.empty()) {
-    const uint64_t v = h->memcpy_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu,
-                   fk = (v >> 24) & 0xffu, word = v & 0xffffffu;
-    if (mode > 1 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || fk == 0 ||
-        fk > lad.n_sizes || word >= lad.size[fk - 1] / 8)
+    const uint64_t v = h->memcpy_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
+    const cdp::FaultSpot at = cdp::fault_spot(v, lad);
+    if (mode > 1 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || !at.word_ok)
       lad.bad = "the armed memcpy fault names no cell, size or word of this call, or has a mode above 1";
     else
-      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, (uint32_t)fk - 1, (uint32_t)mode, word};
+      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, at.k, (uint32_t)mode, at.word};
   }
   int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
   if (const int rc = cdp::agree(h, "cdprobe_memcpy", lad.bad, h->memcpy_calls + 1, {lad.reps, op, 0u}, st);
@@ -1623,7 +1662,7 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
     const uint32_t g = L.grank;
     for (uint32_t j = 0; j < n; ++j) {
       if (!cdp::live_cell(h, li, j, out->status)) continue;
-      const int32_t a = h->area.status[g][j] == 0 && !L.area_mapped[j] ? cdp::kStatusUnmapped : h->area.status[g][j];
+      const int32_t s = h->area.status[g][j], a = s == 0 && !h->area.mapped[li][j] ? cdp::kStatusUnmapped : s;
       if (a != 0) out->status[g * CDPROBE_MAX_GPUS + j] = a;
       runs[li][j] = a == 0;
     }
@@ -1637,39 +1676,19 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
   //    every local rank before anything is queued; the (S, X) each size of each cell must land, from the pattern
   //    definition: the per-granule sums of the source slice on the issuer's GPU, folded into every prefix on the host
   if (const int rc = cdp::memcpy_setup(h); rc != CDPROBE_OK) return rc;
-  const cdp::MemcpyScratch ms(pl.bpp);
-  if (const int rc = cdp::ensure_scratch_all(h, ms.bytes); rc != CDPROBE_OK) return rc;
-  std::vector<uint64_t> want((size_t)cdp::kMaxRanks * cdp::kMaxRanks * cdp::kBwMaxSizes * 2);
-  auto want_of = [&](uint32_t li, uint32_t j) {
-    return reinterpret_cast<uint64_t(*)[2]>(want.data() + ((size_t)li * cdp::kMaxRanks + j) * cdp::kBwMaxSizes * 2);
-  };
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    cdp::LocalRank& L = h->lr[li];
-    for (uint32_t j = 0; j < n; ++j) {
-      if (!runs[li][j]) continue;
-      const cdp::MemcpyCell c = cdp::memcpy_cell(pl, op, L.grank, j);
-      if (const int rc = cdp::expected_sums(h, L, ms.table_off, cdp::SrcRegionWord{h->seed, c.first_word, c.src_rank},
-                                            lad.size, lad.n_sizes, want_of(li, j), "cdprobe_memcpy: granule checksums");
-          rc != CDPROBE_OK)
-        return rc;
-    }
-  }
+  std::unique_ptr<cdp::CellSums[]> want;
+  if (const int rc = cdp::cell_sums(h, runs, op, cdp::MemcpyScratch(pl.bpp).table_off, lad,
+                                    "cdprobe_memcpy: granule checksums", &want);
+      rc != CDPROBE_OK)
+    return rc;
 
-  // 5. the rounds: the tournament's, then the loop-back.  No process starts a round or a size before every process has
-  //    finished the one before; within a size, one rep at a time on every local rank at once.  After a size, every
-  //    local stream is drained, and the checks' records and the events are read: per rep, the diagnosis's bad words
-  //    and the (S, X) read against the pattern's
+  // 5. the rounds.  No process starts a size before every process has finished the one before; within a size, one rep
+  //    at a time on every local rank at once.  After a size, every local stream is drained, and the checks' records
+  //    and the events are read: per rep, the diagnosis's bad words and the (S, X) read against the pattern's
   auto ns = std::make_unique<float[][cdp::kBwMaxSizes][cdp::kMaxTimedReps]>(cdp::kMaxRanks);
-  const uint32_t n_rounds = pl.rounds + (pl.diag ? 1u : 0u);
-  for (uint32_t r = 0; r < n_rounds; ++r) {
-    if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
-    int32_t target[cdp::kMaxRanks];
+  const auto round = [&](const int32_t* target) -> int {
     bool local = false, aborted[cdp::kMaxRanks] = {};
-    for (uint32_t li = 0; li < h->n_local; ++li) {
-      const int q = r < pl.rounds ? pl.partner[r][h->lr[li].grank] : (int)h->lr[li].grank;
-      target[li] = q >= 0 && runs[li][q] ? q : -1;
-      local |= target[li] >= 0;
-    }
+    for (uint32_t li = 0; li < h->n_local; ++li) local |= target[li] >= 0;
     for (uint32_t k = 0; k < lad.n_sizes; ++k) {
       if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
       if (!local) continue;
@@ -1682,7 +1701,7 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
         CDP_RT(cudaSetDevice(L.ordinal));
         if (const cudaError_t e = cudaStreamSynchronize(L.stream); e != cudaSuccess)
           return cdp::fail_sticky(h, "cdprobe_memcpy: check a size", e);
-        const uint64_t(*w)[2] = want_of(li, j);
+        const uint64_t(*w)[2] = want[li][j];
         uint64_t first = UINT64_MAX;
         for (uint32_t rep = 0; rep <= lad.reps; ++rep) {
           const cdp::MemcpyRepOut& got = h->memcpy_host->rep[li][rep];
@@ -1715,7 +1734,9 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
       cdp::ladder_times(ns[li], lad.size, lad.n_sizes, lad.reps, 1.0, idx, out);
       out->status[idx] = out->bad_sizes[idx] ? CDPROBE_ERR_INTEGRITY : 0;
     }
-  }
+    return CDPROBE_OK;
+  };
+  if (const int rc = cdp::walk_rounds(h, runs, round); rc != CDPROBE_OK) return rc;
   out->ms = cdp::now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }
