@@ -530,6 +530,46 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_memcpy_t;
 
+/* Per-link NVLink counters of one local device over the last sampled cdprobe_run (cdprobe_links, DESIGN §5o): the
+ * difference of two NVML samples, one taken just before the run's clock starts, one just after it stops.  Link l is
+ * NVML's scopeId l. */
+#define CDPROBE_LINK_REPLAY 0u          /* errors[l][k]: NVML_FI_DEV_NVLINK_ERROR_DL_REPLAY */
+#define CDPROBE_LINK_RECOVERY 1u        /*               NVML_FI_DEV_NVLINK_ERROR_DL_RECOVERY */
+#define CDPROBE_LINK_CRC 2u             /*               NVML_FI_DEV_NVLINK_ERROR_DL_CRC */
+/* failed_fields[l] bits: the field of link l that returned an error in either sample (its delta reads 0) */
+#define CDPROBE_LINK_FIELD_TX 0x01u
+#define CDPROBE_LINK_FIELD_RX 0x02u
+#define CDPROBE_LINK_FIELD_REPLAY 0x04u
+#define CDPROBE_LINK_FIELD_RECOVERY 0x08u
+#define CDPROBE_LINK_FIELD_CRC 0x10u
+typedef struct {
+  int32_t status;                       /* 0 ok; CDPROBE_ERR_UNSUPPORTED: NVML is missing, lacks the field entry points,
+                                           or has no NVLink field for this GPU (PCIe card, MIG instance); > 0: the
+                                           nvmlReturn_t that failed (the handle lookup or the field call) */
+  uint32_t rank_mask;                   /* bit r set: rank r runs on this device */
+  char uuid[48];                        /* as cdprobe_info reports it */
+  uint32_t link_mask;                   /* bit l set: link l was ENABLED at the first sample */
+  uint32_t lost_mask;                   /* ENABLED at the first sample, not at the second */
+  uint32_t error_mask;                  /* some error counter of link l rose */
+  uint32_t reserved;
+  uint64_t expected_tx_kib;             /* payload the pass's plan sends from this device to other devices (KiB, rounded
+                                           down); barrier flags and read requests are not payload */
+  uint64_t expected_rx_kib;             /* payload it receives from other devices */
+  uint64_t tx_kib[CDPROBE_NVLINK_MAX_LINKS];  /* NVML_FI_DEV_NVLINK_THROUGHPUT_DATA_TX delta (KiB) */
+  uint64_t rx_kib[CDPROBE_NVLINK_MAX_LINKS];  /* NVML_FI_DEV_NVLINK_THROUGHPUT_DATA_RX delta (KiB) */
+  uint64_t errors[CDPROBE_NVLINK_MAX_LINKS][3]; /* [link][CDPROBE_LINK_*] deltas */
+  uint32_t failed_fields[CDPROBE_NVLINK_MAX_LINKS]; /* CDPROBE_LINK_FIELD_* bits */
+  char remote_bus_id[CDPROBE_NVLINK_MAX_LINKS][32]; /* nvmlDeviceGetNvLinkRemotePciInfo_v2 at the first sample: an
+                                                       NVSwitch or a peer GPU; "" when NVML does not say */
+} cdprobe_link_device_t;
+typedef struct {
+  uint32_t abi;
+  uint32_t n_devices;                   /* rows of dev[]: the distinct devices of this process's ranks */
+  uint64_t run_seq;                     /* the cdprobe_run the deltas cover; 0: no sampled run yet */
+  double sample_ms;                     /* host time both samples took */
+  cdprobe_link_device_t dev[CDPROBE_MAX_GPUS];
+} cdprobe_links_t;
+
 CDPROBE_API uint32_t cdprobe_abi_version(void);
 CDPROBE_API const char* cdprobe_strerror(int code);
 /* Detail of the last failure on the calling thread ("cuMemMap: CUDA_ERROR_..."), "" if none. */
@@ -555,12 +595,12 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy: diagnostics, benches, fault injection; the reference has
- *   no counterpart (it has no probe, SURVEY.md F1).
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy, cdprobe_links: diagnostics, benches, fault injection;
+ *   the reference has no counterpart (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls, cdprobe_alltoall and cdprobe_memcpy are optional for callers: a daemon binds them with
- *   dlsym and works without.
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy and cdprobe_links are optional for callers: a daemon binds
+ *   them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -655,6 +695,11 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              host memory); mode 1, no copy is queued, so the destination the previous
                                              rep cleared reads as 0s.  Either fails exactly that cell and size; 0
                                              disarms */
+#define CDPROBE_OPT_LINK_COUNTERS 27u     /* value 0/1 (default 0): sample every local device's per-link NVLink counters
+                                             through NVML around each cdprobe_run, for cdprobe_links.  Turning it on
+                                             loads and initialises NVML once and resolves each local device by UUID;
+                                             both stay until close.  An NVML failure never fails the call or a run: it
+                                             shows in cdprobe_links_t's status */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -968,6 +1013,14 @@ CDPROBE_API int cdprobe_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allr
  * not complete (sticky); CDPROBE_ERR_UNSUPPORTED: the driver has no cuStreamWaitValue64; CDPROBE_ERR_CUDA: it
  * refused one (sticky); CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* out);
+/* The per-link NVLink counters of the last cdprobe_run taken with CDPROBE_OPT_LINK_COUNTERS on: one row per distinct
+ * device of this process's ranks (ranks sharing a device share a row), with the payload the run's phase tables moved
+ * between devices next to what NVML counted.  The samples bracket probe_ms: the first is taken before its clock
+ * starts, the second after it stops (and after the event_timing round trip), so probe_ms, device_ms, kernel_ms and
+ * event_ms mean what they mean without the option.  Nothing here judges the numbers: the verdict is unchanged.  A run
+ * that fails before its rows are published takes no second sample and leaves the last report in place.  One-sided, not
+ * collective.  Before any sampled run: run_seq 0 and every other field 0.  CDPROBE_ERR_ARG: null argument. */
+CDPROBE_API int cdprobe_links(cdprobe_t* h, cdprobe_links_t* out);
 CDPROBE_API void cdprobe_close(cdprobe_t* h);
 
 /* Host-only helpers (no CUDA): schedule + slice arithmetic; the fd/blob rendezvous self-test. */

@@ -59,6 +59,7 @@ type fabricProbeOptions struct {
 	linkPeakGBps float64
 	intervalS    int
 	maxAgeS      int
+	linkCounters bool
 }
 
 var fpOpts fabricProbeOptions
@@ -102,6 +103,12 @@ func fabricProbeCLIFlags() []cli.Flag {
 			Usage:       "check fails when the verdict is older than this many seconds; 0 = 3 x interval + 60 when an interval is set, else never.",
 			EnvVars:     []string{"FABRIC_PROBE_MAX_AGE_S"},
 			Destination: &fpOpts.maxAgeS,
+		},
+		&cli.BoolFlag{
+			Name:        "fabric-probe-link-counters",
+			Usage:       "Report each GPU's per-link NVLink traffic and error counters over every probe pass (log and metrics; the verdict is unchanged).",
+			EnvVars:     []string{"FABRIC_PROBE_LINK_COUNTERS"},
+			Destination: &fpOpts.linkCounters,
 		},
 	}
 }
@@ -218,6 +225,8 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		writeVerdict(fabricprobe.Result{}, fmt.Errorf("cdprobe_open: %w", err), flags)
 		return p
 	}
+	enableLinkCounters(probe)
+	var lastLinks uint64 // RunSeq of the last link report logged, on the current handle
 
 	runOnce := func() {
 		if probe == nil { // the previous pass left the handle unusable
@@ -227,6 +236,8 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 				probe = nil
 				return
 			}
+			enableLinkCounters(probe)
+			lastLinks = 0
 		}
 		t0 := time.Now()
 		res, err := probe.Run(ctx)
@@ -236,6 +247,15 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		metrics.ObserveFabricProbe(flags.nodeName, d, v.OK, v.UnreachablePairs, v.SlowPairs, res.N, res.GBpsRead, res.GBpsWrite)
 		klog.Infof("fabric probe: verdict ok=%t, %d GPU(s), %d unreachable pair(s), %d slow pair(s), min read %.0f GB/s, min write %.0f GB/s, %.3f ms",
 			v.OK, v.N, v.UnreachablePairs, v.SlowPairs, v.MinGBpsRead, v.MinGBpsWrite, v.ProbeMs)
+		if fpOpts.linkCounters {
+			// a library without cdprobe_links (ErrUnsupported) reports nothing and leaves the pass as it was
+			// a pass that failed before its rows were published leaves the previous report in place: report each once
+			if links, lerr := probe.Links(); lerr == nil && links.RunSeq > lastLinks {
+				lastLinks = links.RunSeq
+				logLinks(links)
+				metrics.ObserveFabricProbeLinks(flags.nodeName, links)
+			}
+		}
 		if err == nil && !res.Aborted && !res.Verdict && res.UnreachablePairs > 0 {
 			logDiagnoses(probe, res)
 		}
@@ -274,6 +294,44 @@ func startFabricProbe(ctx context.Context, flags *Flags) *fabricProber {
 		}
 	}()
 	return p
+}
+
+// enableLinkCounters turns the per-link NVLink counters on for a freshly opened handle when
+// --fabric-probe-link-counters asks for them.  A library without them runs the pass unchanged.
+func enableLinkCounters(probe *fabricprobe.Probe) {
+	if !fpOpts.linkCounters {
+		return
+	}
+	if err := probe.SetOption(fabricprobe.OptLinkCounters, 1); err != nil && !errors.Is(err, fabricprobe.ErrUnsupported) {
+		klog.Warningf("fabric probe links: cannot enable the link counters: %v", err)
+	}
+}
+
+// logLinks logs one line per GPU with a link lost or an error counter risen over the pass, the C++ twin's line
+// (daemon_main.cc, log_links):
+//
+//	fabric probe links: GPU-… link 7 (remote 0000:05:00.0): replay +312 recovery +0 crc +41; link 11 lost
+func logLinks(links fabricprobe.Links) {
+	for _, d := range links.Devices {
+		if d.Status != 0 || (d.LostMask == 0 && d.ErrorMask == 0) {
+			continue
+		}
+		var items []string
+		for l := range d.TxKiB {
+			if d.ErrorMask>>l&1 != 0 {
+				remote := ""
+				if d.RemoteBusID[l] != "" {
+					remote = " (remote " + d.RemoteBusID[l] + ")"
+				}
+				items = append(items, fmt.Sprintf("link %d%s: replay +%d recovery +%d crc +%d", l, remote,
+					d.Errors[l][0], d.Errors[l][1], d.Errors[l][2]))
+			}
+			if d.LostMask>>l&1 != 0 {
+				items = append(items, fmt.Sprintf("link %d lost", l))
+			}
+		}
+		klog.Infof("fabric probe links: %s %s", d.UUID, strings.Join(items, "; "))
+	}
 }
 
 // logDiagnoses logs one line per cell, for at most 8 unreachable cells whose mapping is up (an integrity failure,

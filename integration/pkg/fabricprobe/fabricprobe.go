@@ -37,6 +37,8 @@ typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
 typedef int (*ar_fn)(cdprobe_t*, uint32_t, cdprobe_allreduce_t*);
 typedef int (*a2a_fn)(cdprobe_t*, uint32_t, cdprobe_alltoall_t*);
 typedef int (*mc_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_memcpy_t*);
+typedef int (*opt_fn)(cdprobe_t*, uint32_t, uint64_t);
+typedef int (*links_fn)(cdprobe_t*, cdprobe_links_t*);
 
 static void* cdp_dl;
 static open_fn cdp_open; static run_fn cdp_run; static close_fn cdp_close;
@@ -54,6 +56,8 @@ static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprob
 static ar_fn cdp_arpush;  // optional: absent from libraries that predate cdprobe_allreduce_push
 static ar_fn cdp_arnvls;  // optional: absent from libraries that predate cdprobe_allreduce_nvls
 static mc_fn cdp_mc;      // optional: absent from libraries that predate cdprobe_memcpy
+static opt_fn cdp_opt;    // optional: this binding did not need cdprobe_set_option before the link counters
+static links_fn cdp_links;  // optional: absent from libraries that predate cdprobe_links
 
 static int cdp_load(const char* path) {
   if (cdp_dl) return 0;
@@ -78,6 +82,8 @@ static int cdp_load(const char* path) {
   cdp_arpush = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_push");
   cdp_arnvls = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_nvls");
   cdp_mc = (mc_fn)dlsym(cdp_dl, "cdprobe_memcpy");
+  cdp_opt = (opt_fn)dlsym(cdp_dl, "cdprobe_set_option");
+  cdp_links = (links_fn)dlsym(cdp_dl, "cdprobe_links");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
   return cdp_abi() == CDPROBE_ABI_VERSION ? 0 : -3;
 }
@@ -130,6 +136,10 @@ static int cdp_has_memcpy(void) { return cdp_mc != NULL; }
 static int cdp_call_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* mc) {
   return cdp_mc(h, op, reps, mc);
 }
+static int cdp_has_set_option(void) { return cdp_opt != NULL; }
+static int cdp_call_set_option(cdprobe_t* h, uint32_t option, uint64_t value) { return cdp_opt(h, option, value); }
+static int cdp_has_links(void) { return cdp_links != NULL; }
+static int cdp_call_links(cdprobe_t* h, cdprobe_links_t* l) { return cdp_links(h, l); }
 */
 import "C"
 
@@ -151,7 +161,34 @@ const (
 	FlagFabricHandles = 0x01
 	FlagMigAware      = 0x02
 	FlagLocalDiag     = 0x04
+
+	// OptLinkCounters (value 0/1, default 0) samples every local GPU's per-link NVLink counters around each Run,
+	// for Links (CDPROBE_OPT_LINK_COUNTERS).
+	OptLinkCounters = 27
 )
+
+// The error counters of LinkDevice.Errors, in order (CDPROBE_LINK_*).
+var LinkCounterNames = [3]string{"replay", "recovery", "crc"}
+
+// LinkDevice is one local GPU's row of Links (cdprobe_link_device_t).  Per-link slices have 18 entries, index = link.
+type LinkDevice struct {
+	Status                        int32       // 0 ok; CDPROBE_ERR_UNSUPPORTED: no NVLink fields; > 0: the failing nvmlReturn_t
+	RankMask                      uint32      // ranks on this GPU
+	UUID                          string
+	LinkMask, LostMask, ErrorMask uint32      // enabled at the first sample; enabled then but not at the second; an error rose
+	ExpectedTxKiB, ExpectedRxKiB  uint64      // payload the pass's plan moved to / from other GPUs
+	TxKiB, RxKiB                  []uint64
+	Errors                        [][3]uint64 // [link][replay, recovery, crc]
+	FailedFields                  []uint32    // CDPROBE_LINK_FIELD_* bits
+	RemoteBusID                   []string    // "" when NVML does not say
+}
+
+// Links is the per-link NVLink counter report of the last Run taken with OptLinkCounters on (cdprobe_links_t).
+type Links struct {
+	RunSeq   uint64 // 0: no sampled run yet
+	SampleMs float64
+	Devices  []LinkDevice
+}
 
 // ErrUnsupported is returned when the probe cannot run on this node (no libcdprobe.so, no CUDA
 // driver, no sm_90 GPU).  There is no CPU fallback: callers decide whether that gates Ready.
@@ -999,6 +1036,53 @@ func (p *Probe) Memcpy(op uint32, reps int) (Memcpy, error) {
 				out.FirstBad[c][s] = uint64(mc.first_bad[k][s])
 			}
 		}
+	}
+	return out, nil
+}
+
+// SetOption sets one run option (CDPROBE_OPT_*).  ErrUnsupported when the library lacks cdprobe_set_option.
+func (p *Probe) SetOption(option uint32, value uint64) error {
+	if C.cdp_has_set_option() == 0 {
+		return fmt.Errorf("%w: libcdprobe.so has no cdprobe_set_option", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	if rc := C.cdp_call_set_option(p.h, C.uint32_t(option), C.uint64_t(value)); rc != 0 {
+		return fmt.Errorf("cdprobe_set_option: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+	}
+	return nil
+}
+
+// Links returns the per-link NVLink counters of the last Run taken with OptLinkCounters on, one row per local GPU.
+// One-sided, not collective.  ErrUnsupported when the library predates cdprobe_links.
+func (p *Probe) Links() (Links, error) {
+	if C.cdp_has_links() == 0 {
+		return Links{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_links", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	t := new(C.cdprobe_links_t)
+	if rc := C.cdp_call_links(p.h, t); rc != 0 {
+		return Links{}, fmt.Errorf("cdprobe_links: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+	}
+	out := Links{RunSeq: uint64(t.run_seq), SampleMs: float64(t.sample_ms)}
+	const nl = C.CDPROBE_NVLINK_MAX_LINKS
+	for k := 0; k < int(t.n_devices); k++ {
+		d := &t.dev[k]
+		x := LinkDevice{Status: int32(d.status), RankMask: uint32(d.rank_mask), UUID: C.GoString(&d.uuid[0]),
+			LinkMask: uint32(d.link_mask), LostMask: uint32(d.lost_mask), ErrorMask: uint32(d.error_mask),
+			ExpectedTxKiB: uint64(d.expected_tx_kib), ExpectedRxKiB: uint64(d.expected_rx_kib)}
+		x.TxKiB, x.RxKiB = make([]uint64, nl), make([]uint64, nl)
+		x.Errors, x.FailedFields, x.RemoteBusID = make([][3]uint64, nl), make([]uint32, nl), make([]string, nl)
+		for l := 0; l < nl; l++ {
+			x.TxKiB[l], x.RxKiB[l] = uint64(d.tx_kib[l]), uint64(d.rx_kib[l])
+			for c := 0; c < 3; c++ {
+				x.Errors[l][c] = uint64(d.errors[l][c])
+			}
+			x.FailedFields[l] = uint32(d.failed_fields[l])
+			x.RemoteBusID[l] = C.GoString(&d.remote_bus_id[l][0])
+		}
+		out.Devices = append(out.Devices, x)
 	}
 	return out, nil
 }

@@ -20,7 +20,28 @@ const (
 	ModeReachOnly, ModeSliced, ModeFull             = 0, 1, 2
 	OpRead, OpWrite                                 = 1, 2
 	FlagFabricHandles, FlagMigAware, FlagLocalDiag = 0x01, 0x02, 0x04
+	OptLinkCounters = 27
 )
+
+var LinkCounterNames = [3]string{"replay", "recovery", "crc"}
+
+type LinkDevice struct {
+	Status                        int32
+	RankMask                      uint32
+	UUID                          string
+	LinkMask, LostMask, ErrorMask uint32
+	ExpectedTxKiB, ExpectedRxKiB  uint64
+	TxKiB, RxKiB                  []uint64
+	Errors                        [][3]uint64
+	FailedFields                  []uint32
+	RemoteBusID                   []string
+}
+
+type Links struct {
+	RunSeq   uint64
+	SampleMs float64
+	Devices  []LinkDevice
+}
 
 type Config struct {
 	LibraryPath string
@@ -207,4 +228,6 @@ func (*Probe) AllReducePush(int) (AllReduce, error) { return AllReduce{}, ErrUns
 func (*Probe) AllReduceNVLS(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Memcpy(uint32, int) (Memcpy, error) { return Memcpy{}, ErrUnsupported }
+func (*Probe) SetOption(uint32, uint64) error { return ErrUnsupported }
+func (p *Probe) Links() (Links, error)         { return Links{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -12,6 +12,8 @@ import (
 
 	"k8s.io/component-base/metrics"
 	"k8s.io/component-base/metrics/legacyregistry"
+
+	"sigs.k8s.io/dra-driver-nvidia-gpu/pkg/fabricprobe"
 )
 
 var (
@@ -65,6 +67,22 @@ var (
 		},
 		[]string{"node", "outcome"},
 	)
+	fabricProbeLinkKiB = metrics.NewGaugeVec(
+		&metrics.GaugeOpts{
+			Namespace: "nvidia_dra",
+			Name:      "fabric_probe_link_kib",
+			Help:      "NVLink data a GPU link sent (dir tx) or received (dir rx) over the last fabric probe pass, in KiB, as NVML counts it.",
+		},
+		[]string{"node", "gpu", "link", "dir"},
+	)
+	fabricProbeLinkErrors = metrics.NewGaugeVec(
+		&metrics.GaugeOpts{
+			Namespace: "nvidia_dra",
+			Name:      "fabric_probe_link_errors",
+			Help:      "NVLink data-link errors (counter replay, recovery or crc) a GPU link counted over the last fabric probe pass.",
+		},
+		[]string{"node", "gpu", "link", "counter"},
+	)
 )
 
 func registerFabricProbe() {
@@ -76,6 +94,8 @@ func registerFabricProbe() {
 			fabricProbeSlowPairs,
 			fabricProbePairGBps,
 			fabricProbePassesTotal,
+			fabricProbeLinkKiB,
+			fabricProbeLinkErrors,
 		)
 	})
 }
@@ -102,6 +122,24 @@ func ObserveFabricProbe(node string, d time.Duration, ok bool, unreachable, slow
 			if k := i*n + j; k < len(gbpsRead) && k < len(gbpsWrite) {
 				fabricProbePairGBps.WithLabelValues(node, strconv.Itoa(i), strconv.Itoa(j), "read").Set(float64(gbpsRead[k]))
 				fabricProbePairGBps.WithLabelValues(node, strconv.Itoa(i), strconv.Itoa(j), "write").Set(float64(gbpsWrite[k]))
+			}
+		}
+	}
+}
+
+// ObserveFabricProbeLinks records the per-link NVLink counters of one pass, for every GPU NVML could sample.
+func ObserveFabricProbeLinks(node string, links fabricprobe.Links) {
+	registerFabricProbe()
+	for _, d := range links.Devices {
+		if d.Status != 0 {
+			continue
+		}
+		for l := range d.TxKiB {
+			link := strconv.Itoa(l)
+			fabricProbeLinkKiB.WithLabelValues(node, d.UUID, link, "tx").Set(float64(d.TxKiB[l]))
+			fabricProbeLinkKiB.WithLabelValues(node, d.UUID, link, "rx").Set(float64(d.RxKiB[l]))
+			for c, name := range fabricprobe.LinkCounterNames {
+				fabricProbeLinkErrors.WithLabelValues(node, d.UUID, link, name).Set(float64(d.Errors[l][c]))
 			}
 		}
 	}

@@ -42,6 +42,7 @@ OPT_ALLREDUCE_RING_FAULT = 23
 OPT_ALLREDUCE_PUSH_FAULT = 24
 OPT_ALLREDUCE_NVLS_FAULT = 25
 OPT_MEMCPY_FAULT = 26
+OPT_LINK_COUNTERS = 27
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -66,6 +67,11 @@ ALLREDUCE_PATH_RING = 4  # cdprobe_allreduce_t.path of cdprobe_allreduce_ring
 ALLREDUCE_PATH_NVLS = 5  # cdprobe_allreduce_t.path of cdprobe_allreduce_nvls
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
 MEMCPY_DEFAULT_REPS, MEMCPY_MAX_REPS = 8, 64
+
+NVLINK_MAX_LINKS = 18
+LINK_REPLAY, LINK_RECOVERY, LINK_CRC = 0, 1, 2
+LINK_ERROR_NAMES = ("replay", "recovery", "crc")
+LINK_FIELD_TX, LINK_FIELD_RX, LINK_FIELD_REPLAY, LINK_FIELD_RECOVERY, LINK_FIELD_CRC = 0x01, 0x02, 0x04, 0x08, 0x10
 
 _N2 = MAX_GPUS * MAX_GPUS
 
@@ -425,6 +431,35 @@ class MemcpyT(C.Structure):
     ]
 
 
+class LinkDeviceT(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("rank_mask", C.c_uint32),
+        ("uuid", C.c_char * 48),
+        ("link_mask", C.c_uint32),
+        ("lost_mask", C.c_uint32),
+        ("error_mask", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("expected_tx_kib", C.c_uint64),
+        ("expected_rx_kib", C.c_uint64),
+        ("tx_kib", C.c_uint64 * NVLINK_MAX_LINKS),
+        ("rx_kib", C.c_uint64 * NVLINK_MAX_LINKS),
+        ("errors", (C.c_uint64 * 3) * NVLINK_MAX_LINKS),
+        ("failed_fields", C.c_uint32 * NVLINK_MAX_LINKS),
+        ("remote_bus_id", (C.c_char * 32) * NVLINK_MAX_LINKS),
+    ]
+
+
+class LinksT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n_devices", C.c_uint32),
+        ("run_seq", C.c_uint64),
+        ("sample_ms", C.c_double),
+        ("dev", LinkDeviceT * MAX_GPUS),
+    ]
+
+
 def memcpy_fault(issuer: int, target: int, k: int, word: int, mode: int = 0) -> int:
     """The CDPROBE_OPT_MEMCPY_FAULT value for timed rep 1 of size[k] of cell (issuer, target) of cdprobe_memcpy: mode 0,
     destination word `word` is xored with 1 between the copy and the check; mode 1, no copy is queued, so the cleared
@@ -535,6 +570,7 @@ SYMBOLS = {
     "cdprobe_allreduce_nvls": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_memcpy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(MemcpyT)]),
+    "cdprobe_links": (C.c_int, [C.c_void_p, C.POINTER(LinksT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),
     "cdprobe_topology": (C.c_int, [C.c_uint32, C.POINTER(TopologyT)]),

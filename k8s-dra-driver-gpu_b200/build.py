@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcdprobe.so")
 DAEMON = os.path.join(HERE, "cdprobe-daemon")
-SOURCES = ["probe_kernels.cu", "bwcurve_kernels.cu", "allreduce_kernels.cu", "allreduce_twoshot_kernels.cu", "allreduce_ll_kernels.cu", "allreduce_ring_kernels.cu", "allreduce_push_kernels.cu", "allreduce_nvls_kernels.cu", "alltoall_kernels.cu", "diagnose_kernels.cu", "latency_kernels.cu", "pingpong_kernels.cu", "atomics_kernels.cu", "handle.cc", "measure.cc", "plan.cc", "schedule.cc", "rendezvous.cc", "vmm.cc", "topo.cc"]
+SOURCES = ["probe_kernels.cu", "bwcurve_kernels.cu", "allreduce_kernels.cu", "allreduce_twoshot_kernels.cu", "allreduce_ll_kernels.cu", "allreduce_ring_kernels.cu", "allreduce_push_kernels.cu", "allreduce_nvls_kernels.cu", "alltoall_kernels.cu", "diagnose_kernels.cu", "latency_kernels.cu", "pingpong_kernels.cu", "atomics_kernels.cu", "handle.cc", "measure.cc", "plan.cc", "schedule.cc", "rendezvous.cc", "vmm.cc", "topo.cc", "links.cc"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

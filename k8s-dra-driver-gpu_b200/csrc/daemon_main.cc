@@ -193,6 +193,8 @@ struct Lib {
   uint32_t (*abi)(void) = nullptr;
   int (*topology)(uint32_t, cdprobe_topology_t*) = nullptr;
   int (*diagnose)(cdprobe_t*, uint32_t, uint32_t, uint32_t, uint32_t, cdprobe_diag_t*) = nullptr;  // optional
+  int (*set_option)(cdprobe_t*, uint32_t, uint64_t) = nullptr;                                      // optional
+  int (*links)(cdprobe_t*, cdprobe_links_t*) = nullptr;                                             // optional
 };
 
 bool load_lib(Lib* L, std::string* why) {
@@ -210,6 +212,8 @@ bool load_lib(Lib* L, std::string* why) {
   *(void**)&L->abi = dlsym(L->dl, "cdprobe_abi_version");
   *(void**)&L->topology = dlsym(L->dl, "cdprobe_topology");
   *(void**)&L->diagnose = dlsym(L->dl, "cdprobe_diagnose");
+  *(void**)&L->set_option = dlsym(L->dl, "cdprobe_set_option");
+  *(void**)&L->links = dlsym(L->dl, "cdprobe_links");
   if (!L->open || !L->run || !L->close || !L->strerror_ || !L->last_error || !L->abi) {
     *why = "libcdprobe.so lacks an ABI symbol";
     return false;
@@ -226,7 +230,13 @@ int ppoll_nofd(const timespec* ts, const sigset_t* mask) { return ppoll(nullptr,
 void on_term(int) { g_stop = 1; }
 void on_usr1(int) { g_rerun = 1; }
 
-bool write_verdict(const std::string& path, const cdprobe_result_t* r, int rc, const char* err) {
+bool env_on(const char* name) {
+  const std::string v = env_or(name, "");
+  return v == "1" || v == "true" || v == "TRUE" || v == "True";
+}
+
+bool write_verdict(const std::string& path, const cdprobe_result_t* r, int rc, const char* err,
+                   const cdprobe_links_t* links = nullptr) {
   const std::string tmp = path + ".tmp";
   FILE* f = fopen(tmp.c_str(), "w");
   if (f == nullptr) return false;
@@ -284,6 +294,24 @@ bool write_verdict(const std::string& path, const cdprobe_result_t* r, int rc, c
           fprintf(m, "nvidia_dra_fabric_probe_pair_gbps{src=\"%u\",dst=\"%u\",op=\"read\"} %.1f\n", i, j, r->gbps_read[c]);
           fprintf(m, "nvidia_dra_fabric_probe_pair_gbps{src=\"%u\",dst=\"%u\",op=\"write\"} %.1f\n", i, j, r->gbps_write[c]);
         }
+      if (links != nullptr) {  // per-link NVLink counters of the pass, for the GPUs NVML could sample
+        const std::string node = env_or("NODE_NAME", "");
+        const char* dirs[2] = {"tx", "rx"};
+        const char* counters[3] = {"replay", "recovery", "crc"};
+        fprintf(m, "# TYPE nvidia_dra_fabric_probe_link_kib gauge\n");
+        for (uint32_t d = 0; d < links->n_devices; ++d)
+          for (int l = 0; l < CDPROBE_NVLINK_MAX_LINKS && links->dev[d].status == 0; ++l)
+            for (int k = 0; k < 2; ++k)
+              fprintf(m, "nvidia_dra_fabric_probe_link_kib{node=\"%s\",gpu=\"%s\",link=\"%d\",dir=\"%s\"} %llu\n",
+                      node.c_str(), links->dev[d].uuid, l, dirs[k],
+                      (unsigned long long)(k == 0 ? links->dev[d].tx_kib[l] : links->dev[d].rx_kib[l]));
+        fprintf(m, "# TYPE nvidia_dra_fabric_probe_link_errors gauge\n");
+        for (uint32_t d = 0; d < links->n_devices; ++d)
+          for (int l = 0; l < CDPROBE_NVLINK_MAX_LINKS && links->dev[d].status == 0; ++l)
+            for (int k = 0; k < 3; ++k)
+              fprintf(m, "nvidia_dra_fabric_probe_link_errors{node=\"%s\",gpu=\"%s\",link=\"%d\",counter=\"%s\"} %llu\n",
+                      node.c_str(), links->dev[d].uuid, l, counters[k], (unsigned long long)links->dev[d].errors[l][k]);
+      }
       fclose(m);
       rename(mtmp.c_str(), mpath.c_str());
     }
@@ -340,6 +368,35 @@ void log_diagnoses(const Lib& L, cdprobe_t* h, const cdprobe_result_t& r) {
       }
 }
 
+// One log line per GPU of the pass with a link lost or an error counter risen, e.g.
+//   fabric probe links: GPU-… link 7 (remote 0000:05:00.0): replay +312 recovery +0 crc +41; link 11 lost
+void log_links(const cdprobe_links_t& k) {
+  for (uint32_t d = 0; d < k.n_devices; ++d) {
+    const cdprobe_link_device_t& x = k.dev[d];
+    if (x.status != 0 || (x.lost_mask == 0 && x.error_mask == 0)) continue;
+    std::string line;
+    for (int l = 0; l < CDPROBE_NVLINK_MAX_LINKS; ++l) {
+      if ((x.error_mask >> l) & 1u) {
+        char buf[160];
+        snprintf(buf, sizeof(buf), "link %d%s%s%s: replay +%llu recovery +%llu crc +%llu", l,
+                 x.remote_bus_id[l][0] ? " (remote " : "", x.remote_bus_id[l], x.remote_bus_id[l][0] ? ")" : "",
+                 (unsigned long long)x.errors[l][CDPROBE_LINK_REPLAY],
+                 (unsigned long long)x.errors[l][CDPROBE_LINK_RECOVERY], (unsigned long long)x.errors[l][CDPROBE_LINK_CRC]);
+        line += (line.empty() ? "" : "; ") + std::string(buf);
+      }
+      if ((x.lost_mask >> l) & 1u) line += (line.empty() ? "" : "; ") + std::string("link ") + std::to_string(l) + " lost";
+    }
+    fprintf(stderr, "fabric probe links: %s %s\n", x.uuid, line.c_str());
+  }
+}
+
+// Turns the link counters on for a freshly opened handle, when asked for and the library has them.
+void enable_links(const Lib& L, cdprobe_t* h, bool want) {
+  if (!want || !L.set_option || !L.links) return;
+  if (L.set_option(h, CDPROBE_OPT_LINK_COUNTERS, 1) != CDPROBE_OK)
+    fprintf(stderr, "fabric probe links: cannot enable the link counters: %s\n", L.last_error());
+}
+
 // Signals are blocked for the whole of run() and only delivered inside sigsuspend/sigtimedwait-style waits:
 // the "check the flag, then sleep" sequence cannot lose a SIGTERM or SIGUSR1 that lands in between.
 int wait_for_signal(const sigset_t* unblocked, long timeout_s) {
@@ -381,6 +438,7 @@ int cmd_run(bool once) {
   cfg.timeout_ms = (uint32_t)atol(env_or("FABRIC_PROBE_TIMEOUT_MS", "5000").c_str());
   cfg.flags = CDPROBE_FLAG_FABRIC_HANDLES | CDPROBE_FLAG_MIG_AWARE;
   const long interval_s = atol(env_or("FABRIC_PROBE_INTERVAL_S", "0").c_str());
+  const bool want_links = env_on("FABRIC_PROBE_LINK_COUNTERS");
   if (L.topology) {
     cdprobe_topology_t topo;
     if (L.topology(1, &topo) == CDPROBE_OK && topo.clique_error[0] == '\0')
@@ -399,6 +457,7 @@ int cmd_run(bool once) {
     write_verdict(verdict_path, nullptr, rc, e.c_str());
     return 1;
   }
+  enable_links(L, h, want_links);
   sigset_t block, orig;
   sigemptyset(&block);
   sigaddset(&block, SIGTERM);
@@ -435,6 +494,7 @@ int cmd_run(bool once) {
           if (!g_stop) g_rerun = 1;
           continue;
         }
+        enable_links(L, h, want_links);
       }
       const timespec t0 = [] { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t; }();
       rc = L.run(h, &res);
@@ -442,7 +502,10 @@ int cmd_run(bool once) {
       clock_gettime(CLOCK_MONOTONIC, &t1);
       fprintf(stderr, "t_fabric_probe %.6f s\n", (t1.tv_sec - t0.tv_sec) + (t1.tv_nsec - t0.tv_nsec) / 1e9);
       const std::string run_err = rc == CDPROBE_OK ? "" : std::string(L.strerror_(rc)) + ": " + L.last_error();
-      if (!write_verdict(verdict_path, &res, rc, run_err.c_str()))
+      cdprobe_links_t links;
+      const bool have_links = want_links && L.set_option && L.links && L.links(h, &links) == CDPROBE_OK &&
+                              links.run_seq != 0 && links.run_seq == res.run_seq;
+      if (!write_verdict(verdict_path, &res, rc, run_err.c_str(), have_links ? &links : nullptr))
         fprintf(stderr, "cannot write %s: %s\n", verdict_path.c_str(), strerror(errno));
       fprintf(stderr,
               "fabric probe: verdict %s, %u GPU(s), %u unreachable pair(s), %u slow pair(s), min read %.0f GB/s, min write "
@@ -450,6 +513,7 @@ int cmd_run(bool once) {
               (rc == CDPROBE_OK && res.verdict) ? "ok" : "FAILED", res.n, res.unreachable_pairs, res.slow_pairs,
               res.min_gbps_read, res.min_gbps_write, res.probe_ms);
       status = (rc == CDPROBE_OK && res.verdict) ? 0 : 2;
+      if (have_links) log_links(links);
       if (L.diagnose && rc == CDPROBE_OK && !res.aborted && !res.verdict && res.unreachable_pairs > 0)
         log_diagnoses(L, h, res);
       if (rc == CDPROBE_ERR_TIMEOUT || rc == CDPROBE_ERR_STATE || rc == CDPROBE_ERR_CUDA) {

@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "handle.h"
+#include "links.h"
 #include "probe_launch.h"
 #include "schedule.h"
 
@@ -693,6 +694,7 @@ static void destroy(cdprobe* h) {
     if (L.stream) cudaStreamDestroy(L.stream);
   }
   if (h->memcpy_host) cudaFreeHost(h->memcpy_host);
+  delete h->links;
   h->rdv.close();
   delete h;
 }
@@ -822,6 +824,17 @@ static int open_impl(const cdprobe_config_t* cfg, cdprobe* h) {
     CDP_RT(cudaHostAlloc(&row, sizeof(ResultRow), cudaHostAllocPortable | cudaHostAllocMapped));
     memset(row, 0, sizeof(ResultRow));
     L.row = static_cast<ResultRow*>(row);
+  }
+
+  // ---- every rank's device, by UUID: which cells of a run cross a device boundary (cdprobe_links) ----
+  for (uint32_t li = 0; li < h->n_local; ++li) memcpy(h->rank_uuid[h->first + li], h->lr[li].uuid, 48);
+  if (c.world_size > 1) {
+    std::vector<char> all((size_t)c.world_size * c.n_gpus * 48);
+    if (h->rdv.allgather(h->rank_uuid[h->first], (size_t)c.n_gpus * 48, all.data(), &err) != 0) {
+      set_err(err);
+      return CDPROBE_ERR_RENDEZVOUS;
+    }
+    memcpy(h->rank_uuid, all.data(), all.size());
   }
 
   // ---- the probe allocations, shared with every process and mapped ---------
@@ -958,6 +971,78 @@ static void assemble(const cdprobe* h, cdprobe_result_t* out) {
   out->verdict = (verdict && !out->aborted) ? 1u : 0u;
 }
 
+// CDPROBE_OPT_LINK_COUNTERS, first enabling: one report row per distinct device of the local ranks, and NVML with a
+// handle for each.
+static int links_open(cdprobe* h) {
+  h->links = new (std::nothrow) LinkCounters();
+  if (h->links == nullptr) return CDPROBE_ERR_NOMEM;
+  cdprobe_links_t& rep = h->links->report;
+  char uuid[kMaxRanks][48] = {};
+  bool mig[kMaxRanks] = {};
+  uint32_t n = 0;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const LocalRank& L = h->lr[li];
+    uint32_t d = 0;
+    while (d < n && strncmp(uuid[d], L.uuid, 48) != 0) ++d;
+    if (d == n) {
+      memcpy(uuid[n], L.uuid, 48);
+      mig[n++] = L.mig;
+    }
+    rep.dev[d].rank_mask |= 1u << L.grank;
+  }
+  for (uint32_t d = 0; d < n; ++d) memcpy(rep.dev[d].uuid, uuid[d], 48);
+  h->links->sampler.open(n, uuid, mig);
+  return CDPROBE_OK;
+}
+
+// The first sample of a run, before probe_ms's clock starts.
+static void links_before(cdprobe* h) {
+  LinkCounters& lc = *h->links;
+  const double t = now_ms();
+  lc.sampler.sample(lc.before, true);
+  lc.before_ms = now_ms() - t;
+}
+
+// The second sample, after probe_ms's clock has stopped, and the report: the deltas next to the payload the run's
+// phase tables moved between devices.
+static void links_after(cdprobe* h, const cdprobe_result_t* out) {
+  LinkCounters& lc = *h->links;
+  const double t = now_ms();
+  lc.sampler.sample(lc.after, false);
+  cdprobe_links_t& rep = lc.report;
+  rep.sample_ms = lc.before_ms + (now_ms() - t);
+  rep.run_seq = h->launch_seq;
+  rep.n_devices = lc.sampler.n();
+  uint32_t dev[kMaxRanks];  // rank -> the lowest rank on the same device
+  for (uint32_t r = 0; r < h->n_total; ++r) {
+    dev[r] = r;
+    for (uint32_t q = 0; q < r; ++q)
+      if (strncmp(h->rank_uuid[q], h->rank_uuid[r], 48) == 0) {
+        dev[r] = q;
+        break;
+      }
+  }
+  uint32_t ran = h->n_total >= 32 ? 0xffffffffu : (1u << h->n_total) - 1u;
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    if (h->debug_skip_rank == li + 1 || (h->solo_rank != 0 && h->solo_rank != li + 1)) ran &= ~(1u << h->lr[li].grank);
+  ScheduleInput in;
+  in.plan = &h->plan;
+  in.ops = h->cfg.ops;
+  in.flags = h->cfg.flags;
+  in.ctas = h->lr[0].ctas;
+  in.verify_ctas = h->verify_ctas;
+  in.status = h->status;
+  uint64_t tx[kMaxRanks], rx[kMaxRanks];
+  link_payload(in, ran, dev, out->warmed ? h->warm_bytes : 0, tx, rx);
+  for (uint32_t d = 0; d < rep.n_devices; ++d) {
+    cdprobe_link_device_t& row = rep.dev[d];
+    link_delta(lc.before[d], lc.after[d], &row);
+    const uint32_t r = dev[__builtin_ctz(row.rank_mask)];
+    row.expected_tx_kib = tx[r] / 1024;
+    row.expected_rx_kib = rx[r] / 1024;
+  }
+}
+
 }  // namespace cdp
 
 // ------------------------------------------------------------------ C ABI ----
@@ -1013,6 +1098,7 @@ int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out) {
   out->bytes_per_pair = h->plan.bpp;
   out->rounds = h->plan.rounds;
   if (const int rc = cdp::require_usable(h); rc != CDPROBE_OK) return rc;
+  if (h->link_counters) cdp::links_before(h);  // before probe_ms: the samples are not part of the probe
   const double t0 = cdp::now_ms();
   h->launch_seq++;
   h->last_run_seq = h->launch_seq;
@@ -1080,6 +1166,7 @@ int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out) {
         out->event_ms[li] = ms;
     }
   }
+  if (h->link_counters) cdp::links_after(h, out);
   if (out->aborted) {
     for (uint32_t li = 0; li < h->n_local; ++li) {
       const int rc = cdp::reset_ctrl_local(h, li);
@@ -1292,6 +1379,12 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
     case CDPROBE_OPT_MEMCPY_FAULT:  // checked against the domain and the size ladder by cdprobe_memcpy
       h->memcpy_fault = value;
       return CDPROBE_OK;
+    case CDPROBE_OPT_LINK_COUNTERS:
+      if (value > 1) return CDPROBE_ERR_ARG;
+      if (value != 0 && h->links == nullptr)
+        if (const int rc = cdp::links_open(h); rc != CDPROBE_OK) return rc;
+      h->link_counters = value != 0;
+      return CDPROBE_OK;
     default:
       return CDPROBE_ERR_ARG;
   }
@@ -1435,6 +1528,14 @@ int cdprobe_gate(const cdprobe_config_t* cfg, uint32_t n_total, float* gate_read
   if (rc != CDPROBE_OK) return rc;
   *gate_read_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, true);
   *gate_write_gbps = cdp::gate_gbps_for(*cfg, n_total, pl.bpp, false);
+  return CDPROBE_OK;
+}
+
+int cdprobe_links(cdprobe_t* h, cdprobe_links_t* out) {
+  if (h == nullptr || out == nullptr) return CDPROBE_ERR_ARG;
+  if (h->links != nullptr && h->links->report.run_seq != 0) *out = h->links->report;
+  else memset(out, 0, sizeof(*out));
+  out->abi = CDPROBE_ABI_VERSION;
   return CDPROBE_OK;
 }
 

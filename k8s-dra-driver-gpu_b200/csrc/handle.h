@@ -18,6 +18,7 @@
 namespace cdp {
 
 struct MemcpyHost;
+struct LinkCounters;
 
 inline thread_local std::string g_last_error;
 
@@ -151,6 +152,10 @@ struct cdprobe {
   cdp::MemcpyHost* memcpy_host = nullptr;  // cdprobe_memcpy's pinned host block (measure.cc), made on first use:
                                           // the ticket its streams wait on and what its checks leave
   uint64_t memcpy_tickets = 0;        // tickets handed out so far
+  char rank_uuid[cdp::kMaxRanks][48] = {};  // every rank's device UUID, exchanged at open (cdprobe_links' payload)
+  bool link_counters = false;               // CDPROBE_OPT_LINK_COUNTERS
+  cdp::LinkCounters* links = nullptr;       // NVML, the local devices and the last report, from the option's first
+                                            // enabling until close
   double open_ms = 0, fill_ms = 0;
 };
 

@@ -228,6 +228,33 @@ int make_phases(const ScheduleInput& in, Phase* phases, uint32_t* n_phases, uint
   return CDPROBE_OK;
 }
 
+void link_payload(const ScheduleInput& in, uint32_t ran_mask, const uint32_t* dev, uint64_t warm_bytes, uint64_t* tx,
+                  uint64_t* rx) {
+  const Plan& pl = *in.plan;
+  for (uint32_t d = 0; d < pl.n; ++d) tx[d] = rx[d] = 0;
+  const uint64_t warm = warm_bytes < pl.bpp ? warm_bytes : pl.bpp;
+  for (uint32_t r = 0; r < pl.n; ++r) {
+    if (!((ran_mask >> r) & 1u)) continue;
+    ScheduleInput mine = in;
+    mine.rank = r;
+    Phase ph[kMaxPhases];
+    uint32_t np = 0, mask = 0;
+    if (make_phases(mine, ph, &np, &mask) != CDPROBE_OK) continue;
+    for (uint32_t p = 0; p < np; ++p)
+      for (const Job& j : ph[p].job) {
+        if (j.peer < 0 || dev[r] == dev[(uint32_t)j.peer]) continue;
+        const uint32_t peer = (uint32_t)j.peer;
+        if (j.kind == kJobRead || j.kind == kJobWarm) {
+          const uint64_t b = j.kind == kJobRead ? pl.bpp : warm;
+          tx[dev[peer]] += b;
+          rx[dev[r]] += b;
+        } else if (j.kind == kJobWrite) {
+          tx[dev[r]] += pl.bpp;
+          rx[dev[peer]] += pl.bpp;
+        }
+      }
+  }
+}
 
 }  // namespace cdp
 

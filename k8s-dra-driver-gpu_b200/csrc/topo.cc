@@ -11,66 +11,18 @@
 //     semantics of getCliqueIDStrict / getCliqueIDLegacy
 //     (cmd/compute-domain-kubelet-plugin/nvlib.go:208-363), so the daemon and
 //     the kubelet plugin agree on whether the IMEX gate applies.
-// NVML is reached the way go-nvml reaches it: lazy dlopen of
-// libnvidia-ml.so.1 (vendor/github.com/NVIDIA/go-nvml/pkg/nvml/lib.go:29-80),
-// nvmlInitWithFlags(NVML_INIT_FLAG_NO_GPUS) and an unconditional shutdown
-// (nvlib.go:107-123).  No CUDA here; this file makes no reachability claim —
-// reachability comes only from the kernels.
-#include <dlfcn.h>
-#include <nvml.h>
+// NVML is reached through nvml_loader.h.  No CUDA here; this file makes no
+// reachability claim — reachability comes only from the kernels.
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <set>
 #include <string>
 
 #include "../../include/cdprobe.h"
+#include "nvml_loader.h"
 
 namespace {
-
-class Nvml {
- public:
-  ~Nvml() {
-    if (inited_ && shutdown_) shutdown_();
-    if (dl_) dlclose(dl_);
-  }
-  int open() {
-    const char* path = getenv("CDPROBE_NVML_PATH");
-    if (path == nullptr || *path == '\0') path = "libnvidia-ml.so.1";
-    dl_ = dlopen(path, RTLD_LAZY | RTLD_GLOBAL);
-    if (dl_ == nullptr) return CDPROBE_ERR_NO_DEVICE;
-    bool ok = sym(init_, "nvmlInitWithFlags") && sym(shutdown_, "nvmlShutdown") &&
-              sym(count_, "nvmlDeviceGetCount_v2") && sym(by_index_, "nvmlDeviceGetHandleByIndex_v2") &&
-              sym(uuid_, "nvmlDeviceGetUUID") && sym(pci_, "nvmlDeviceGetPciInfo_v3") &&
-              sym(mig_, "nvmlDeviceGetMigMode") && sym(link_, "nvmlDeviceGetNvLinkState") &&
-              sym(fabric_, "nvmlDeviceGetGpuFabricInfo");
-    if (!ok) return CDPROBE_ERR_UNSUPPORTED;
-    const nvmlReturn_t r = init_(NVML_INIT_FLAG_NO_GPUS);
-    if (r != NVML_SUCCESS) return CDPROBE_ERR_NO_DEVICE;
-    inited_ = true;
-    return CDPROBE_OK;
-  }
-
-  nvmlReturn_t (*init_)(unsigned int) = nullptr;
-  nvmlReturn_t (*shutdown_)(void) = nullptr;
-  nvmlReturn_t (*count_)(unsigned int*) = nullptr;
-  nvmlReturn_t (*by_index_)(unsigned int, nvmlDevice_t*) = nullptr;
-  nvmlReturn_t (*uuid_)(nvmlDevice_t, char*, unsigned int) = nullptr;
-  nvmlReturn_t (*pci_)(nvmlDevice_t, nvmlPciInfo_t*) = nullptr;
-  nvmlReturn_t (*mig_)(nvmlDevice_t, unsigned int*, unsigned int*) = nullptr;
-  nvmlReturn_t (*link_)(nvmlDevice_t, unsigned int, nvmlEnableState_t*) = nullptr;
-  nvmlReturn_t (*fabric_)(nvmlDevice_t, nvmlGpuFabricInfo_t*) = nullptr;
-
- private:
-  template <typename Fn>
-  bool sym(Fn& fn, const char* name) {
-    fn = reinterpret_cast<Fn>(dlsym(dl_, name));
-    return fn != nullptr;
-  }
-  void* dl_ = nullptr;
-  bool inited_ = false;
-};
 
 std::string hex_uuid(const unsigned char* b) {
   char s[40];
@@ -91,7 +43,7 @@ extern "C" int cdprobe_topology(uint32_t strict, cdprobe_topology_t* out) {
   if (out == nullptr) return CDPROBE_ERR_ARG;
   memset(out, 0, sizeof(*out));
   out->abi = CDPROBE_ABI_VERSION;
-  Nvml nv;
+  cdp::Nvml nv;
   int rc = nv.open();
   if (rc != CDPROBE_OK) return rc;
   unsigned int n = 0;

@@ -512,6 +512,32 @@ class Memcpy:
                       first_bad=_mat(t, per_size(t.first_bad), timed), ms=t.ms, raw=t)
 
 
+@dataclasses.dataclass
+class Links:
+    """What cdprobe_links reported: per distinct local device, the per-link NVLink counter deltas NVML gave over the
+    last run taken with abi.OPT_LINK_COUNTERS on, next to the payload that run's plan moved between devices.  Each
+    device is a dict: status (0, abi.ERR_UNSUPPORTED or an nvmlReturn_t), rank_mask, uuid, link_mask, lost_mask,
+    error_mask, expected_tx_kib, expected_rx_kib, and per link (lists of 18) tx_kib, rx_kib, errors ({"replay",
+    "recovery", "crc"}), failed_fields (abi.LINK_FIELD_* bits) and remote_bus_id.  run_seq 0: no sampled run yet."""
+    n_devices: int
+    run_seq: int
+    sample_ms: float
+    devices: List[dict]
+    raw: abi.LinksT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.LinksT) -> "Links":
+        L = abi.NVLINK_MAX_LINKS
+        return Links(n_devices=t.n_devices, run_seq=t.run_seq, sample_ms=t.sample_ms, raw=t, devices=[
+            {"status": d.status, "rank_mask": d.rank_mask, "uuid": d.uuid.decode(), "link_mask": d.link_mask,
+             "lost_mask": d.lost_mask, "error_mask": d.error_mask, "expected_tx_kib": d.expected_tx_kib,
+             "expected_rx_kib": d.expected_rx_kib, "tx_kib": list(d.tx_kib), "rx_kib": list(d.rx_kib),
+             "errors": [dict(zip(abi.LINK_ERROR_NAMES, d.errors[l])) for l in range(L)],
+             "failed_fields": list(d.failed_fields),
+             "remote_bus_id": [d.remote_bus_id[l].value.decode() for l in range(L)]}
+            for d in t.dev[:t.n_devices]])
+
+
 def _raise(lib, rc: int, what: str):
     msg = lib.cdprobe_strerror(rc).decode()
     detail = lib.cdprobe_last_error().decode()
@@ -797,6 +823,13 @@ class Probe:
         t = abi.MemcpyT()
         rc = self._lib.cdprobe_memcpy(self._h, op, reps, C.byref(t))
         return rc, t
+
+    def Links(self) -> Links:
+        """Go: (*Probe).Links.  The per-link NVLink counters of the last Run taken with abi.OPT_LINK_COUNTERS on, one
+        entry per distinct local device.  One-sided, not collective."""
+        t = abi.LinksT()
+        _check(self._lib, self._lib.cdprobe_links(self._h, C.byref(t)), "cdprobe_links")
+        return Links.from_c(t)
 
     def Close(self) -> None:
         if self._h:
