@@ -10,13 +10,11 @@ import sys
 import pytest
 
 from conftest import ROOT, gpu_count
-
-HEADER = os.path.join(ROOT, "include", "cdprobe.h")
+from harness import FakeLib, assert_layout, declared_symbols, fake_probe
 
 
 def test_exports_every_declared_symbol(pkg):
-    text = open(HEADER).read()
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", text))
+    declared = declared_symbols()
     assert declared == set(pkg.abi.SYMBOLS), declared ^ set(pkg.abi.SYMBOLS)
     lib = pkg.abi.load_library()
     for name in declared:
@@ -43,21 +41,7 @@ def test_struct_layout_matches_c(pkg, tmp_path):
     structs = {"cdprobe_config_t": a.ConfigT, "cdprobe_result_t": a.ResultT, "cdprobe_info_t": a.InfoT,
                "cdprobe_plan_t": a.PlanT, "cdprobe_trace_t": a.TraceT,
                "cdprobe_topology_t": a.TopologyT, "cdprobe_schedule_t": a.ScheduleT}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{HEADER}"', "int main(void){"]
-    for cname, ct in structs.items():
-        lines.append(f'printf("{cname} %zu\\n", sizeof({cname}));')
-        for fname, _ in ct._fields_:
-            lines.append(f'printf("{cname}.{fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    for cname, ct in structs.items():
-        assert int(got[cname]) == C.sizeof(ct), cname
-        for fname, _ in ct._fields_:
-            assert int(got[f"{cname}.{fname}"]) == getattr(ct, fname).offset, f"{cname}.{fname}"
+    assert_layout(tmp_path, structs)
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
@@ -114,28 +98,18 @@ def test_corrupt_landing_null_handle_and_wrapper_packing(pkg):
 
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_corrupt_landing(self, h, local, target, n, word, mask):
             calls.append((h.value, local, target, n, [word[e] for e in range(n)], [mask[e] for e in range(n)]))
             return a.ERR_ARG if n > 8 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         p.CorruptLanding(1, 3, [(0, 1), (1 << 40, (1 << 63) | 5)])
         p.CorruptLanding(0, 0, [])
         assert calls == [(0x1234, 1, 3, 2, [0, 1 << 40], [1, (1 << 63) | 5]), (0x1234, 0, 0, 0, [], [])]
         with pytest.raises(pkg.ProbeError) as e:
             p.CorruptLanding(0, 1, [(k, 1) for k in range(9)])
         assert e.value.code == a.ERR_ARG and calls[-1][3] == 9
-    finally:
-        p._h = C.c_void_p()
 
 
 @pytest.mark.skipif(gpu_count() > 0, reason="this box has a GPU; the loud-failure path needs a CPU-only box")

@@ -5,39 +5,24 @@ import ctypes as C
 import os
 import random
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import allreduce_ref as ref
 from conftest import ROOT
+from harness import FakeLib, assert_layout, c_tool, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 G = 2048  # words per 16 KiB granule
 U64_MAX = (1 << 64) - 1
 
 
 def test_allreduce_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("sizeof %zu\\n", sizeof(cdprobe_allreduce_t));',
-             'printf("opt %u\\n", CDPROBE_OPT_ALLREDUCE_FAULT);']
-    for fname, _ in a.AllReduceT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_allreduce_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["sizeof"]) == C.sizeof(a.AllReduceT)
-    for fname, _ in a.AllReduceT._fields_:
-        assert int(got[fname]) == getattr(a.AllReduceT, fname).offset, fname
-    assert int(got["opt"]) == a.OPT_ALLREDUCE_FAULT == 19
+    assert_layout(tmp_path, {"cdprobe_allreduce_t": a.AllReduceT})
+    assert header_values(tmp_path, "CDPROBE_OPT_ALLREDUCE_FAULT") == [a.OPT_ALLREDUCE_FAULT] == [19]
     assert "cdprobe_allreduce" in a.SYMBOLS
     assert a.allreduce_fault(2, 5, 77) == (3 << 32) | (6 << 24) | 77
     assert a.allreduce_fault(2, 5, 77, drop=True) == (1 << 48) | (3 << 32) | (6 << 24) | 77
@@ -50,13 +35,8 @@ def test_allreduce_struct_layout_matches_c(pkg, tmp_path):
 
 
 def test_every_declared_symbol_is_exported(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_allreduce" in declared
     assert declared <= exported, declared - exported
 
@@ -82,17 +62,7 @@ def test_output_words_restatement_by_hand():
 
 @pytest.fixture(scope="module")
 def fold(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("ar") / "allreduce_fold"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "allreduce_fold.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(lines):
-        text = "".join(" ".join(str(x) for x in l) + "\n" for l in lines)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(lines)
-        return [[int(x) for x in l.split()] for l in out]
-
-    return run
+    return c_tool(tmp_path_factory, "allreduce_fold.cc")
 
 
 @pytest.mark.parametrize("n", [1, 2, 3, 8, 16])
@@ -155,7 +125,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_allreduce(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -169,15 +139,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.t0_ns[1], t.peak_gbps[1], t.half_bytes[1], t.bad_sizes[1] = 2.0, 2048.0, 4096, 2
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         ar = p.AllReduce()
         assert calls[-1] == (0x1234, 0)
         assert (ar.n, ar.row_mask, ar.reps, ar.call_seq, ar.path, ar.sizes) == (3, 2, 8, 4, 2, [4096, 8192])
@@ -194,8 +156,6 @@ def test_wrapper_passes_its_arguments(pkg):
             p.AllReduce(65)
         assert e.value.code == a.ERR_ARG
         assert pkg.AllReduce is type(ar)
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the compiled kernel ------------------------------------------------------------------------------------------

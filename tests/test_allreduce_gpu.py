@@ -4,11 +4,7 @@ word check, a word corrupted at rest fails exactly the sizes that cover it in ev
 earlier handle left in the output, a mapping that is down stops every rank without waiting, two processes agree, the
 call needs no run and disturbs none, and the times are ordered and bounded, at N = 1 no faster than HBM allows.  Several ranks share one device where a test needs N > 1,
 with CTA counts that let their grids be resident together (every rank waits for every other at each rep)."""
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
@@ -16,6 +12,7 @@ import allreduce_ref as ref
 import atomics_ref
 import pingpong_ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -334,24 +331,12 @@ CHILD = textwrap.dedent(
 ) % ROOT
 
 
-def run_processes(world, n_local, what):
-    session = f"ar-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local), what],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
-    return outs
-
-
 @pytest.mark.parametrize("n_local", [1, 2], ids=["2x1", "2x2"])
 def test_two_processes_agree_and_fill_their_own_rows(pkg, n_local):
     """Both processes drive GPU 0, so their contexts are time-sliced and the times only need to be positive."""
     world = 2
     n = world * n_local
-    outs = run_processes(world, n_local, "full")
+    outs = run_children(CHILD, world, n_local, "full")
     sizes = ref.ladder(pkg.plan(n, 1 << 20, MODE_SLICED).bytes_per_pair)
     expect = [list(sx) for sx in ref.expected(SEED, n, tuple(sizes))]
     masks = [o["calls"][0]["row_mask"] for o in outs]
@@ -377,7 +362,7 @@ def test_one_process_with_no_peer_mappings_stops_both():
     """A peer mapping cannot be dropped in one process of a multi-process domain (cdprobe_unmap_peer refuses), so the
     process whose mappings are down is one whose ranks are (simulated) MIG instances: neither process runs, both
     report the status of the domain's first down cell, and neither waits for a watchdog."""
-    outs = run_processes(2, 2, "mig")
+    outs = run_children(CHILD, 2, 2, "mig")
     for rank, o in enumerate(outs):
         c = o["calls"][0]
         assert c["call_seq"] == 1 and c["ms"] < 5000

@@ -4,30 +4,22 @@ restatement, the compiled kernel's packet stores and loads and its spills, and t
 import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
 import allreduce_ll_ref as ref
 from conftest import ROOT
+from harness import FakeLib, c_tool, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 U64_MAX = (1 << 64) - 1
 
 
 def test_option_path_and_symbol_match_the_header(pkg, tmp_path):
     a = pkg.abi
-    src = tmp_path / "opt.c"
-    src.write_text(f'#include <stdio.h>\n#include "{HEADER}"\n'
-                   'int main(void){printf("%u %u\\n", CDPROBE_OPT_ALLREDUCE_LL_FAULT, CDPROBE_ALLREDUCE_PATH_LL);'
-                   ' return 0;}\n')
-    exe = tmp_path / "opt"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
-    assert [int(x) for x in out] == [a.OPT_ALLREDUCE_LL_FAULT, a.ALLREDUCE_PATH_LL] == [22, 3]
+    out = header_values(tmp_path, "CDPROBE_OPT_ALLREDUCE_LL_FAULT", "CDPROBE_ALLREDUCE_PATH_LL")
+    assert out == [a.OPT_ALLREDUCE_LL_FAULT, a.ALLREDUCE_PATH_LL] == [22, 3]
     assert a.SYMBOLS["cdprobe_allreduce_ll"] == a.SYMBOLS["cdprobe_allreduce"]
 
 
@@ -47,13 +39,8 @@ def test_the_fault_encoder_and_its_refusals(pkg):
 
 
 def test_the_symbol_is_declared_and_exported(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_allreduce_ll" in declared and "cdprobe_allreduce_ll" in exported
 
 
@@ -86,7 +73,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_allreduce_ll(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -100,15 +87,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.t0_ns[1], t.peak_gbps[1], t.half_bytes[1], t.bad_sizes[1] = 2.0, 2048.0, 4096, 2
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         ar = p.AllReduceLL()
         assert calls[-1] == (0x1234, 0)
         assert type(ar) is pkg.AllReduce
@@ -125,24 +104,12 @@ def test_wrapper_passes_its_arguments(pkg):
         with pytest.raises(pkg.ProbeError) as e:
             p.AllReduceLL(65)
         assert e.value.code == a.ERR_ARG
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- ladder, flags, salts and slots ----------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def helper(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("ll") / "ll_flags"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "ll_flags.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(lines):
-        out = subprocess.run([str(exe)], input="".join(l + "\n" for l in lines), capture_output=True, text=True,
-                             check=True).stdout.splitlines()
-        assert len(out) == len(lines)
-        return [[int(x) for x in l.split()] for l in out]
-
-    return run
+    return c_tool(tmp_path_factory, "ll_flags.cc")
 
 
 def test_the_ladder_matches_the_restatement_from_128_bytes_to_32_gib(helper):

@@ -4,7 +4,6 @@ modes, the barrier lines, the compiled kernel's multicast instructions and spill
 import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -14,6 +13,7 @@ import allreduce_nvls_ref as ref
 import allreduce_ref
 import word_ref
 from conftest import ROOT
+from harness import FakeLib, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
@@ -22,18 +22,9 @@ U64_MAX = (1 << 64) - 1
 SEED = 0xCD5EED0000000001
 
 
-def header_values(tmp_path, names, sizes=()):
-    src = tmp_path / "v.c"
-    body = "".join(f'printf("%llu\\n", (unsigned long long){x});' for x in list(names) + [f"sizeof({t})" for t in sizes])
-    src.write_text(f'#include <stdio.h>\n#include "{HEADER}"\nint main(void){{{body} return 0;}}\n')
-    exe = tmp_path / "v"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    return [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-
-
 def test_option_path_and_symbol_match_the_header(pkg, tmp_path):
     a = pkg.abi
-    got = header_values(tmp_path, ["CDPROBE_OPT_ALLREDUCE_NVLS_FAULT", "CDPROBE_ALLREDUCE_PATH_NVLS"])
+    got = header_values(tmp_path, "CDPROBE_OPT_ALLREDUCE_NVLS_FAULT", "CDPROBE_ALLREDUCE_PATH_NVLS")
     assert got == [a.OPT_ALLREDUCE_NVLS_FAULT, a.ALLREDUCE_PATH_NVLS] == [25, 5]
     assert a.SYMBOLS["cdprobe_allreduce_nvls"] == a.SYMBOLS["cdprobe_allreduce"]
 
@@ -47,7 +38,7 @@ PARENT_SIZES = {"cdprobe_config_t": 192, "cdprobe_result_t": 12376, "cdprobe_inf
 
 def test_the_abi_version_and_every_struct_size_are_unchanged(pkg, tmp_path):
     a = pkg.abi
-    got = header_values(tmp_path, ["CDPROBE_ABI_VERSION"], list(PARENT_SIZES))
+    got = header_values(tmp_path, "CDPROBE_ABI_VERSION", *(f"sizeof({t})" for t in PARENT_SIZES))
     assert got[0] == a.ABI_VERSION == 2
     assert dict(zip(PARENT_SIZES, got[1:])) == PARENT_SIZES
     py = [a.ConfigT, a.ResultT, a.InfoT, a.PlanT, a.TraceT, a.ScheduleT, a.TopologyT, a.DiagSampleT, a.DiagT,
@@ -56,13 +47,8 @@ def test_the_abi_version_and_every_struct_size_are_unchanged(pkg, tmp_path):
 
 
 def test_the_symbol_is_declared_and_exported_and_the_abi_set_still_matches(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_allreduce_nvls" in declared and "cdprobe_allreduce_nvls" in exported
     assert declared == set(pkg.abi.SYMBOLS)
 
@@ -109,7 +95,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_allreduce_nvls(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -122,15 +108,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.bad_words[0][1], t.first_bad[0][0], t.first_bad[0][1] = 1, U64_MAX, 8
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         ar = p.AllReduceNVLS()
         assert calls[-1] == (0x1234, 0)
         assert type(ar) is pkg.AllReduce
@@ -144,8 +122,6 @@ def test_wrapper_passes_its_arguments(pkg):
         with pytest.raises(pkg.ProbeError) as e:
             p.AllReduceNVLS(65)
         assert e.value.code == a.ERR_ARG
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the restatement ------------------------------------------------------------------------------------------------

@@ -15,11 +15,7 @@ import of the multicast handle between processes, fabric handles, and a down pro
 two ranks, which on one GPU share the device and are refused for that first)."""
 import ctypes as C
 import functools
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import numpy as np
 import pytest
@@ -28,6 +24,7 @@ import allreduce_nvls_ref as ref
 import allreduce_ref
 import word_ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -377,14 +374,7 @@ def test_two_processes_sharing_a_device_agree_to_run_nothing(pkg, n_local):
     """Both processes drive GPU 0: their ranks' UUIDs are equal across processes, so every process refuses alike."""
     world = 2
     n = world * n_local
-    session = f"arnvls-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local)],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world, n_local)
     for rank, o in enumerate(outs):
         mine = set(range(rank * n_local, (rank + 1) * n_local))
         assert [c["call_seq"] for c in o["calls"]] == [1, 2]

@@ -4,42 +4,29 @@ probe_types.h against it, the compiled kernel's flag stores, polls and spills, a
 import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
 import allreduce_ring_ref as ref
 import bwcurve_ref
 from conftest import ROOT
+from harness import FakeLib, c_tool, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 U64_MAX = (1 << 64) - 1
 
 
 def test_option_path_and_symbol_match_the_header(pkg, tmp_path):
     a = pkg.abi
-    src = tmp_path / "opt.c"
-    src.write_text(f'#include <stdio.h>\n#include "{HEADER}"\n'
-                   'int main(void){printf("%u %u\\n", CDPROBE_OPT_ALLREDUCE_RING_FAULT, CDPROBE_ALLREDUCE_PATH_RING);'
-                   ' return 0;}\n')
-    exe = tmp_path / "opt"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
-    assert [int(x) for x in out] == [a.OPT_ALLREDUCE_RING_FAULT, a.ALLREDUCE_PATH_RING] == [23, 4]
+    out = header_values(tmp_path, "CDPROBE_OPT_ALLREDUCE_RING_FAULT", "CDPROBE_ALLREDUCE_PATH_RING")
+    assert out == [a.OPT_ALLREDUCE_RING_FAULT, a.ALLREDUCE_PATH_RING] == [23, 4]
     assert a.SYMBOLS["cdprobe_allreduce_ring"] == a.SYMBOLS["cdprobe_allreduce"]
 
 
 def test_the_symbol_is_declared_and_exported_and_the_abi_set_still_matches(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_allreduce_ring" in declared and "cdprobe_allreduce_ring" in exported
     assert declared == set(pkg.abi.SYMBOLS)
 
@@ -87,7 +74,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_allreduce_ring(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -101,15 +88,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.t0_ns[1], t.peak_gbps[1], t.half_bytes[1], t.bad_sizes[1] = 2.0, 2048.0, 4096, 2
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         ar = p.AllReduceRing()
         assert calls[-1] == (0x1234, 0)
         assert type(ar) is pkg.AllReduce
@@ -126,8 +105,6 @@ def test_wrapper_passes_its_arguments(pkg):
         with pytest.raises(pkg.ProbeError) as e:
             p.AllReduceRing(65)
         assert e.value.code == a.ERR_ARG
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the restatement ------------------------------------------------------------------------------------------------
@@ -175,17 +152,7 @@ def test_failing_rows_run_from_the_hop_to_the_rank_before_the_owner(n):
 # ---- flags and layout -------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def helper(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("ring") / "ring_flags"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "ring_flags.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(lines):
-        out = subprocess.run([str(exe)], input="".join(l + "\n" for l in lines), capture_output=True, text=True,
-                             check=True).stdout.splitlines()
-        assert len(out) == len(lines)
-        return [[int(x) for x in l.split()] for l in out]
-
-    return run
+    return c_tool(tmp_path_factory, "ring_flags.cc")
 
 
 def test_the_flag_grain_and_the_barrier_lines(helper):

@@ -7,11 +7,7 @@ without waiting; two processes agree; repeated calls stay exact and disturb noth
 where a test needs N > 1, with CTA counts that let their grids be resident together (every rank waits for its
 predecessor's flags).  No test drives a kernel past its deadline."""
 import functools
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import numpy as np
 import pytest
@@ -20,6 +16,7 @@ import allreduce_ref
 import allreduce_ring_ref as ref
 import word_ref
 from conftest import ROOT
+from harness import run_children
 from test_allreduce_gpu import assert_hbm_floor
 
 pytestmark = pytest.mark.gpu
@@ -419,14 +416,7 @@ def test_two_processes_agree_and_fill_their_own_rows(pkg, n_local):
     be positive."""
     world = 2
     n = world * n_local
-    session = f"arring-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local)],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world, n_local)
     sizes = allreduce_ref.ladder(pkg.plan(n, 1 << 20, MODE_SLICED).bytes_per_pair)
     expect = [list(sx) for sx in allreduce_ref.expected(SEED, n, tuple(sizes))]
     ns = len(sizes)

@@ -4,29 +4,21 @@ and register use, and the Go mirror."""
 import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
 import allreduce_twoshot_ref as ref
 from conftest import ROOT
+from harness import FakeLib, c_tool, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 U64_MAX = (1 << 64) - 1
 
 
 def test_option_and_symbol_match_the_header(pkg, tmp_path):
     a = pkg.abi
-    src = tmp_path / "opt.c"
-    src.write_text(f'#include <stdio.h>\n#include "{HEADER}"\n'
-                   'int main(void){printf("%u\\n", CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT); return 0;}\n')
-    exe = tmp_path / "opt"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    assert int(subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout) == \
-        a.OPT_ALLREDUCE_TWOSHOT_FAULT == 21
+    assert header_values(tmp_path, "CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT") == [a.OPT_ALLREDUCE_TWOSHOT_FAULT] == [21]
     assert a.SYMBOLS["cdprobe_allreduce_twoshot"] == a.SYMBOLS["cdprobe_allreduce"]
     assert a.allreduce_twoshot_fault(2, 5, 77) == (3 << 32) | (6 << 24) | 77
     assert a.allreduce_twoshot_fault(0, 0, 0, drop=True) == (1 << 48) | (1 << 32) | (1 << 24)
@@ -34,13 +26,8 @@ def test_option_and_symbol_match_the_header(pkg, tmp_path):
 
 
 def test_the_symbol_is_declared_and_exported(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_allreduce_twoshot" in declared and "cdprobe_allreduce_twoshot" in exported
 
 
@@ -65,7 +52,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_allreduce_twoshot(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -79,15 +66,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.t0_ns[1], t.peak_gbps[1], t.half_bytes[1], t.bad_sizes[1] = 2.0, 2048.0, 4096, 2
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         ar = p.AllReduceTwoShot()
         assert calls[-1] == (0x1234, 0)
         assert type(ar) is pkg.AllReduce
@@ -104,25 +83,13 @@ def test_wrapper_passes_its_arguments(pkg):
         with pytest.raises(pkg.ProbeError) as e:
             p.AllReduceTwoShot(65)
         assert e.value.code == a.ERR_ARG
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the chunk partition -------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def chunks(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("ts") / "twoshot_chunks"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "twoshot_chunks.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(f"{u} {n}\n" for u, n in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [[tuple(v[2 * r:2 * r + 2]) for r in range(len(v) // 2)] for v in ([int(x) for x in l.split()]
-                                                                                   for l in out)]
-
-    return run
+    run = c_tool(tmp_path_factory, "twoshot_chunks.cc")
+    return lambda cases: [[tuple(v[2 * r:2 * r + 2]) for r in range(len(v) // 2)] for v in run(cases)]
 
 
 def test_chunks_are_a_disjoint_cover_and_match_the_restatement(chunks):

@@ -6,11 +6,7 @@ without waiting; two processes agree; the call needs no run and disturbs none; t
 Several ranks share one device where a test needs N > 1, with CTA counts that let their grids be resident together
 (every rank waits for every other at each rep).  No test drives a kernel past its deadline."""
 import functools
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import numpy as np
 import pytest
@@ -19,6 +15,7 @@ import allreduce_ref
 import allreduce_twoshot_ref as ref
 import word_ref
 from conftest import ROOT
+from harness import run_children
 from test_allreduce_gpu import assert_hbm_floor
 
 pytestmark = pytest.mark.gpu
@@ -367,14 +364,7 @@ def test_two_processes_agree_and_fill_their_own_rows(pkg, n_local):
     """Both processes drive GPU 0, so their contexts are time-sliced and the times only need to be positive."""
     world = 2
     n = world * n_local
-    session = f"ar2-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local)],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world, n_local)
     sizes = allreduce_ref.ladder(pkg.plan(n, 1 << 20, MODE_SLICED).bytes_per_pair)
     expect = [list(sx) for sx in allreduce_ref.expected(SEED, n, tuple(sizes))]
     for rank, o in enumerate(outs):

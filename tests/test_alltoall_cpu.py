@@ -4,8 +4,6 @@ and register use, and the Go mirror."""
 import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,6 +11,7 @@ import pytest
 import alltoall_ref as ref
 import word_ref
 from conftest import ROOT
+from harness import FakeLib, assert_layout, declared_symbols, exported_symbols, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
@@ -21,33 +20,15 @@ U64_MAX = (1 << 64) - 1
 
 def test_alltoall_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("sizeof %zu\\n", sizeof(cdprobe_alltoall_t));',
-             'printf("opt %u\\n", CDPROBE_OPT_ALLTOALL_FAULT);']
-    for fname, _ in a.AllToAllT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_alltoall_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["sizeof"]) == C.sizeof(a.AllToAllT)
-    for fname, _ in a.AllToAllT._fields_:
-        assert int(got[fname]) == getattr(a.AllToAllT, fname).offset, fname
-    assert int(got["opt"]) == a.OPT_ALLTOALL_FAULT == 20
+    assert_layout(tmp_path, {"cdprobe_alltoall_t": a.AllToAllT})
+    assert header_values(tmp_path, "CDPROBE_OPT_ALLTOALL_FAULT") == [a.OPT_ALLTOALL_FAULT] == [20]
     assert "cdprobe_alltoall" in a.SYMBOLS
     assert a.alltoall_fault(2, 0, 5, 77) == (3 << 40) | (1 << 32) | (6 << 24) | 77
 
 
 def test_every_declared_symbol_is_exported(pkg):
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    out = subprocess.run([nm, "-D", "--defined-only", pkg.abi.LIB_PATH], capture_output=True, text=True,
-                         check=True).stdout
-    exported = {l.split()[-1] for l in out.splitlines() if l.strip()}
-    declared = set(re.findall(r"CDPROBE_API\s+[\w\s\*]+?\b(cdprobe_\w+)\s*\(", open(HEADER).read()))
+    exported = exported_symbols(pkg.abi.LIB_PATH)
+    declared = declared_symbols()
     assert "cdprobe_alltoall" in declared
     assert declared <= exported, declared - exported
 
@@ -130,7 +111,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_alltoall(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -148,15 +129,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.cell_status[2 * 16 + 1] = a.ERR_STATE
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         aa = p.AllToAll()
         assert calls[-1] == (0x1234, 0)
         assert (aa.n, aa.row_mask, aa.reps, aa.call_seq, aa.path, aa.sizes, aa.area_bytes) == \
@@ -176,8 +149,6 @@ def test_wrapper_passes_its_arguments(pkg):
             p.AllToAll(65)
         assert e.value.code == a.ERR_ARG
         assert pkg.AllToAll is type(aa)
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the compiled kernel ------------------------------------------------------------------------------------------

@@ -3,16 +3,13 @@ the pattern; an armed fault fails exactly its cell and size, also across process
 its cell; MIG launches nothing; the call needs no run and disturbs none; the times are ordered and bounded; and the
 exchange area leaks nothing.  Several ranks share one device where a test needs N > 1, with CTA counts that let their
 grids be resident together (every rank waits for its peers at each rep)."""
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import alltoall_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -272,18 +269,6 @@ CHILD = textwrap.dedent(
 ) % ROOT
 
 
-def run_processes(world, n_local, fault="none"):
-    session = f"a2a-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local), fault],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
-    return outs
-
-
 @pytest.mark.parametrize("n_local", [1, 2], ids=["2x1", "2x2"])
 def test_two_processes_agree_and_fill_their_own_entries(pkg, oracle, n_local):
     """Both processes drive GPU 0.  With two ranks per process, a fault is armed on a cell from process 0's second rank
@@ -291,7 +276,7 @@ def test_two_processes_agree_and_fill_their_own_entries(pkg, oracle, n_local):
     world = 2
     n = world * n_local
     fi, fj, fk, fw = (1, 2, 2, 77) if n_local == 2 else (0, 1, 2, 77)
-    outs = run_processes(world, n_local, str(pkg.abi.alltoall_fault(fi, fj, fk, fw)))
+    outs = run_children(CHILD, world, n_local, pkg.abi.alltoall_fault(fi, fj, fk, fw))
     sizes = ref.ladder(pkg.plan(n, 1 << 20, MODE_SLICED).bytes_per_pair)
     for rank, o in enumerate(outs):
         mine = set(range(rank * n_local, (rank + 1) * n_local))

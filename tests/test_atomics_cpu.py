@@ -4,37 +4,24 @@ their register use, and the Go mirror."""
 import ctypes as C
 import os
 import re
-import subprocess
 
 import pytest
 
 import atomics_ref as ref
 from conftest import ROOT
+from harness import FakeLib, assert_layout, c_tool, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 
 
 def test_atomics_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("size %zu\\n", sizeof(cdprobe_atomics_t));',
-             'printf("opt %u\\n", CDPROBE_OPT_ATOMICS_FAULT);',
-             'printf("kinds %u,%u,%u\\n", CDPROBE_ATOMIC_FETCH_ADD, CDPROBE_ATOMIC_CAS, CDPROBE_ATOMIC_CONTENDED);']
-    for fname, _ in a.AtomicsT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_atomics_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["size"]) == C.sizeof(a.AtomicsT)
-    for fname, _ in a.AtomicsT._fields_:
-        assert int(got[fname]) == getattr(a.AtomicsT, fname).offset, fname
-    assert int(got["opt"]) == a.OPT_ATOMICS_FAULT == 18
-    assert got["kinds"] == f"{a.ATOMIC_FETCH_ADD},{a.ATOMIC_CAS},{a.ATOMIC_CONTENDED}" == "0,1,2"
+    assert_layout(tmp_path, {"cdprobe_atomics_t": a.AtomicsT})
+    opt, *kinds = header_values(tmp_path, "CDPROBE_OPT_ATOMICS_FAULT", "CDPROBE_ATOMIC_FETCH_ADD", "CDPROBE_ATOMIC_CAS",
+                                "CDPROBE_ATOMIC_CONTENDED")
+    assert opt == a.OPT_ATOMICS_FAULT == 18
+    assert kinds == [a.ATOMIC_FETCH_ADD, a.ATOMIC_CAS, a.ATOMIC_CONTENDED] == [0, 1, 2]
     assert "cdprobe_atomics" in a.SYMBOLS
     assert a.atomics_fault(2, 5) == ref.fault_value(2, 5) == (3 << 16) | 6
 
@@ -42,17 +29,8 @@ def test_atomics_struct_layout_matches_c(pkg, tmp_path):
 # ---- start values and digests: probe_types.h against the restatement ---------------------------------------------
 @pytest.fixture(scope="module")
 def words(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("at") / "atomics_words"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "atomics_words.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [tuple(int(x) for x in l.split()) for l in out]
-
-    return run
+    run = c_tool(tmp_path_factory, "atomics_words.cc")
+    return lambda cases: [tuple(r) for r in run(cases)]
 
 
 CALLS = (1, 2, 3, (1 << 32) - 1, 1 << 32, (1 << 32) + 1, (1 << 40) + 5)
@@ -118,7 +96,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_atomics(self, h, kind, ops, reps, out):
             calls.append((h.value, kind, ops, reps))
             t = out._obj
@@ -130,15 +108,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.status[0] = a.ERR_STATE
             return a.ERR_ARG if kind > 2 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         at = p.Atomics(a.ATOMIC_CONTENDED)
         assert calls[-1] == (0x1234, 2, 0, 0)
         assert (at.kind, at.ops, at.reps, at.lanes, at.call_seq) == (2, 1024, 8, 32, 4)
@@ -151,8 +121,6 @@ def test_wrapper_passes_its_arguments(pkg):
             p.Atomics(3)
         assert e.value.code == a.ERR_ARG
         assert pkg.Atomics is type(at)
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the compiled kernels -----------------------------------------------------------------------------------------

@@ -2,16 +2,13 @@
 lost, duplicated or misplaced an update cannot pass; the times are plausible; cells whose mapping is down are not run;
 the armed fault fails exactly its cell; the call is one-sided, needs no run and disturbs none.  Several ranks share
 one device where a test needs N > 1."""
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import atomics_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -219,14 +216,7 @@ CHILD = textwrap.dedent(
 def test_two_processes_fill_their_own_rows(pkg):
     """Both processes drive GPU 0, so their contexts are time-sliced and the times only need to be positive."""
     world = 2
-    session = f"at-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world)], stdout=subprocess.PIPE,
-                              stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world)
     for rank, o in enumerate(outs):
         other = 1 - rank
         calls = o["calls"] + ([o["solo"]] if rank == 0 else [])

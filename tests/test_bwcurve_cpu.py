@@ -5,37 +5,23 @@ import ctypes as C
 import os
 import random
 import re
-import subprocess
 
 import pytest
 
 import bwcurve_ref as ref
 from conftest import ROOT
+from harness import FakeLib, assert_layout, c_tool, fake_probe, header_values
 from kernel_tools import kernel_sass, ptxas_report
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 GIB = 1 << 30
 G = 2048  # words per 16 KiB granule
 
 
 def test_bwcurve_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("sizeof %zu\\n", sizeof(cdprobe_bwcurve_t));',
-             'printf("max_sizes %u\\n", CDPROBE_BWCURVE_MAX_SIZES);']
-    for fname, _ in a.BwCurveT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_bwcurve_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["sizeof"]) == C.sizeof(a.BwCurveT)
-    for fname, _ in a.BwCurveT._fields_:
-        assert int(got[fname]) == getattr(a.BwCurveT, fname).offset, fname
-    assert int(got["max_sizes"]) == a.BWCURVE_MAX_SIZES == ref.MAX_SIZES == 24
+    assert_layout(tmp_path, {"cdprobe_bwcurve_t": a.BwCurveT})
+    assert header_values(tmp_path, "CDPROBE_BWCURVE_MAX_SIZES") == [a.BWCURVE_MAX_SIZES] == [ref.MAX_SIZES] == [24]
     assert "cdprobe_bwcurve" in a.SYMBOLS
 
 
@@ -67,17 +53,7 @@ def test_summary_restatement_by_hand():
 
 @pytest.fixture(scope="module")
 def fold(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("bw") / "bwcurve_fold"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "bwcurve_fold.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(lines):
-        text = "".join(" ".join(str(x) for x in l) + "\n" for l in lines)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(lines)
-        return [[int(x) for x in l.split()] for l in out]
-
-    return run
+    return c_tool(tmp_path_factory, "bwcurve_fold.cc")
 
 
 def test_library_ladder_matches_the_restatement(fold):
@@ -129,7 +105,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_bwcurve(self, h, reps, out):
             calls.append((h.value, reps))
             t = out._obj
@@ -142,15 +118,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.status[0], t.status[1] = a.ERR_STATE, a.ERR_INTEGRITY
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         bw = p.BwCurve()
         assert calls[-1] == (0x1234, 0)
         assert (bw.n, bw.reps, bw.call_seq, bw.path, bw.sizes) == (2, 8, 3, 1, [4096, 8192])
@@ -165,8 +133,6 @@ def test_wrapper_passes_its_arguments(pkg):
             p.BwCurve(65)
         assert e.value.code == a.ERR_ARG
         assert pkg.BwCurve is type(bw)
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the compiled kernel ------------------------------------------------------------------------------------------

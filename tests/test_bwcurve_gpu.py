@@ -3,16 +3,13 @@ corrupted at rest fails exactly the sizes that cover it, cells whose mapping is 
 and disturbs none, the times are plausible and bounded, and two processes agree.  Several ranks share one device where
 a test needs N > 1."""
 import functools
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import bwcurve_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -225,14 +222,7 @@ CHILD = textwrap.dedent(
 def test_two_processes_agree_and_fill_their_own_rows(pkg, oracle):
     """Both processes drive GPU 0, so their contexts are time-sliced and the times only need to be positive."""
     world = 2
-    session = f"bw-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world)], stdout=subprocess.PIPE,
-                              stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world)
     bpp = 1 << 20
     for rank, o in enumerate(outs):
         other = 1 - rank

@@ -9,6 +9,7 @@ import subprocess
 import pytest
 
 from conftest import ROOT
+from harness import assert_layout, c_tool, exported_symbols, header_values
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -20,43 +21,19 @@ FLIP, ZERO, DISPLACED, STALE, FOREIGN = 0, 1, 2, 3, 4
 def test_diag_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
     structs = {"cdprobe_diag_sample_t": a.DiagSampleT, "cdprobe_diag_t": a.DiagT}
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){"]
-    for cname, ct in structs.items():
-        lines.append(f'printf("{cname} %zu\\n", sizeof({cname}));')
-        for fname, _ in ct._fields_:
-            lines.append(f'printf("{cname}.{fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines += ['printf("samples %d\\n", CDPROBE_DIAG_SAMPLES);',
-              'printf("kinds %u %u %u %u %u\\n", CDPROBE_DIAG_FLIP, CDPROBE_DIAG_ZERO, CDPROBE_DIAG_DISPLACED, '
-              'CDPROBE_DIAG_STALE, CDPROBE_DIAG_FOREIGN);', "return 0;}"]
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines()
-    got = {l.split(" ", 1)[0]: l.split(" ", 1)[1] for l in out}
-    for cname, ct in structs.items():
-        assert int(got[cname]) == C.sizeof(ct), cname
-        for fname, _ in ct._fields_:
-            assert int(got[f"{cname}.{fname}"]) == getattr(ct, fname).offset, f"{cname}.{fname}"
-    assert int(got["samples"]) == a.DIAG_SAMPLES
-    assert got["kinds"] == " ".join(map(str, (a.DIAG_FLIP, a.DIAG_ZERO, a.DIAG_DISPLACED, a.DIAG_STALE, a.DIAG_FOREIGN)))
+    assert_layout(tmp_path, structs)
+    samples, *kinds = header_values(tmp_path, "CDPROBE_DIAG_SAMPLES", "CDPROBE_DIAG_FLIP", "CDPROBE_DIAG_ZERO",
+                                    "CDPROBE_DIAG_DISPLACED", "CDPROBE_DIAG_STALE", "CDPROBE_DIAG_FOREIGN")
+    assert samples == a.DIAG_SAMPLES
+    assert kinds == [a.DIAG_FLIP, a.DIAG_ZERO, a.DIAG_DISPLACED, a.DIAG_STALE, a.DIAG_FOREIGN]
     assert "cdprobe_diagnose" in a.SYMBOLS
 
 
 # ---- the classifier: known answers built with the oracle's forward functions ------------------------------------
 @pytest.fixture(scope="module")
 def classify(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("diag") / "diag_classify"
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "diag_classify.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [tuple(int(x) for x in l.split()) for l in out]
-
-    return run
+    run = c_tool(tmp_path_factory, "diag_classify.cc", "-O1")
+    return lambda cases: [tuple(r) for r in run(cases)]
 
 
 def test_read_cell_words_classify_to_their_rank_and_index(oracle, classify):
@@ -135,8 +112,8 @@ def fake_libs(pkg, tmp_path_factory):
     with_sym, without = str(d / "libfake_diag.so"), str(d / "libfake_nodiag.so")
     subprocess.run(["gcc", "-shared", "-fPIC", "-O1", "-Wall", src, "-o", with_sym], check=True)
     subprocess.run(["gcc", "-shared", "-fPIC", "-O1", "-Wall", "-DFAKE_CDPROBE_NO_DIAGNOSE", src, "-o", without], check=True)
-    assert "cdprobe_diagnose" in subprocess.run(["nm", "-D", with_sym], capture_output=True, text=True).stdout
-    assert "cdprobe_diagnose" not in subprocess.run(["nm", "-D", without], capture_output=True, text=True).stdout
+    assert "cdprobe_diagnose" in exported_symbols(with_sym)
+    assert "cdprobe_diagnose" not in exported_symbols(without)
     return with_sym, without
 
 

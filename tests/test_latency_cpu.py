@@ -4,51 +4,29 @@ import ctypes as C
 import os
 import random
 import re
-import subprocess
 
 import pytest
 
 import latency_ref as ref
 from conftest import ROOT
+from harness import assert_layout, c_tool
 from kernel_tools import kernel_sass
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 SEED = 0xCD5EED0000000001
 
 
 def test_latency_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("size %zu\\n", sizeof(cdprobe_latency_t));']
-    for fname, _ in a.LatencyT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_latency_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["size"]) == C.sizeof(a.LatencyT)
-    for fname, _ in a.LatencyT._fields_:
-        assert int(got[fname]) == getattr(a.LatencyT, fname).offset, fname
+    assert_layout(tmp_path, {"cdprobe_latency_t": a.LatencyT})
     assert "cdprobe_latency" in a.SYMBOLS
 
 
 # ---- the chase: probe_types.h against the restatement ------------------------------------------------------------
 @pytest.fixture(scope="module")
 def chain(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("lat") / "latency_chain"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "latency_chain.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [tuple(int(x) for x in l.split()) for l in out]
-
-    return run
+    run = c_tool(tmp_path_factory, "latency_chain.cc")
+    return lambda cases: [tuple(r) for r in run(cases)]
 
 
 def restated(seed, i, j, first, lines, hops, reps):

@@ -1,16 +1,13 @@
 """cdprobe_latency on the GPU: every chased cell's digest equals the restatement in tests/latency_ref.py, so a chase
 that read the wrong words cannot pass; the times are plausible; cells whose mapping is down are never read; the call
 needs no run and disturbs none.  Several ranks share one device where a test needs N > 1."""
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import latency_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -184,14 +181,7 @@ def test_two_processes_fill_their_own_rows(pkg, oracle):
     other context and only need to be positive, and the probe's bandwidth verdict is not judged (as in the other
     two-process tests); every pair must stay reachable around the latency calls."""
     world = 2
-    session = f"l-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world)], stdout=subprocess.PIPE,
-                              stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=300)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world, timeout=300)
     for rank, per_call in enumerate(outs):
         other = 1 - rank
         for o in per_call:

@@ -15,6 +15,7 @@ import pytest
 
 import links_ref
 from conftest import ROOT
+from harness import assert_layout
 from kernel_tools import CSRC
 
 FAKE_NVML_DIR = os.path.join(ROOT, "tests", "fake_nvml")
@@ -43,21 +44,7 @@ def fake_uuid(g):
 # ---- ABI --------------------------------------------------------------------------------------------------------
 def test_layout_matches_gcc_offsetof(pkg, tmp_path):
     abi = pkg.abi
-    lines = []
-    for cname, cls in (("cdprobe_links_t", abi.LinksT), ("cdprobe_link_device_t", abi.LinkDeviceT)):
-        lines.append(f'printf("{cname} %zu\\n", sizeof({cname}));')
-        for fname, _ in cls._fields_:
-            lines.append(f'printf("{cname}.{fname} %zu\\n", offsetof({cname}, {fname}));')
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "%s"\nint main(void) {\n%s\nreturn 0;\n}\n'
-                   % (HEADER, "\n".join(lines)))
-    subprocess.run(["gcc", "-std=c11", str(src), "-o", str(tmp_path / "layout")], check=True)
-    got = dict(l.split() for l in subprocess.run([str(tmp_path / "layout")], capture_output=True, text=True,
-                                                 check=True).stdout.splitlines())
-    for cname, cls in (("cdprobe_links_t", abi.LinksT), ("cdprobe_link_device_t", abi.LinkDeviceT)):
-        assert int(got[cname]) == C.sizeof(cls), cname
-        for fname, _ in cls._fields_:
-            assert int(got[f"{cname}.{fname}"]) == getattr(cls, fname).offset, (cname, fname)
+    assert_layout(tmp_path, {"cdprobe_links_t": abi.LinksT, "cdprobe_link_device_t": abi.LinkDeviceT})
 
 
 def test_option_number_and_symbol(pkg):

@@ -11,7 +11,7 @@ import pytest
 
 import memcpy_ref as ref
 from conftest import ROOT
-from kernel_tools import CSRC
+from harness import FakeLib, assert_layout, c_tool_exe, fake_probe, header_values
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
 U64_MAX = (1 << 64) - 1
@@ -21,29 +21,15 @@ MODES = (0, 1, 2)  # reach, sliced, full
 
 def test_memcpy_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("sizeof %zu\\n", sizeof(cdprobe_memcpy_t));', 'printf("opt %u\\n", CDPROBE_OPT_MEMCPY_FAULT);']
-    for fname, _ in a.MemcpyT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_memcpy_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["sizeof"]) == C.sizeof(a.MemcpyT)
-    for fname, _ in a.MemcpyT._fields_:
-        assert int(got[fname]) == getattr(a.MemcpyT, fname).offset, fname
-    assert int(got["opt"]) == a.OPT_MEMCPY_FAULT == 26
+    assert_layout(tmp_path, {"cdprobe_memcpy_t": a.MemcpyT})
+    assert header_values(tmp_path, "CDPROBE_OPT_MEMCPY_FAULT") == [a.OPT_MEMCPY_FAULT] == [26]
     assert a.SYMBOLS["cdprobe_memcpy"] == (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(a.MemcpyT)])
 
 
 # ---- the cell geometry ------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def cells(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("mc") / "memcpy_cells"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "memcpy_cells.cc"),
-                    os.path.join(CSRC, "plan.cc"), "-o", str(exe)], check=True)
+    exe = c_tool_exe(tmp_path_factory, "memcpy_cells.cc", csrc=["plan.cc"])
 
     def run(cases):
         text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
@@ -180,22 +166,14 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_memcpy(self, h, op, reps, out):
             calls.append((h.value, op, reps))
             t = out._obj
             t.abi, t.n, t.reps, t.op = 2, 2, reps or 8, op
             return a.ERR_ARG if reps > 64 else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         m = p.Memcpy(a.OP_WRITE)
         assert calls[-1] == (0x1234, a.OP_WRITE, 0) and (m.op, m.reps, m.n) == (a.OP_WRITE, 8, 2)
         p.Memcpy(a.OP_READ, reps=3)
@@ -204,8 +182,6 @@ def test_wrapper_passes_its_arguments(pkg):
             p.Memcpy(a.OP_READ, 65)
         assert e.value.code == a.ERR_ARG
         assert pkg.Memcpy is type(m)
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- Go mirror ------------------------------------------------------------------------------------------------------

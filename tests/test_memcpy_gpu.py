@@ -3,17 +3,14 @@ the (S, X) of the pattern; an armed fault fails exactly its cell and size, and t
 clean; a mapping that is down stops only its cell; MIG copies nothing; the call needs no run and disturbs none; the
 times are ordered and bounded; two processes agree; and nothing leaks.  Several ranks share one device where a test
 needs N > 1."""
-import json
 import os
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import memcpy_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -277,14 +274,7 @@ CHILD = textwrap.dedent(
 def test_two_processes_agree_and_fill_their_own_rows(pkg, oracle, n_local):
     world = 2
     n = world * n_local
-    session = f"mc-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world), str(n_local)],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world, n_local)
     bpp = pkg.plan(n, 1 << 20, MODE_SLICED).bytes_per_pair
     sizes = ref.ladder(bpp)
     for rank, o in enumerate(outs):

@@ -5,35 +5,21 @@ import ctypes as C
 import os
 import random
 import re
-import subprocess
 
 import pytest
 
 import pingpong_ref as ref
 from conftest import ROOT
+from harness import FakeLib, assert_layout, c_tool, fake_probe, header_values
 from kernel_tools import kernel_sass
 
 HEADER = os.path.join(ROOT, "include", "cdprobe.h")
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 
 
 def test_pingpong_struct_layout_matches_c(pkg, tmp_path):
     a = pkg.abi
-    lines = ["#include <stdio.h>", "#include <stddef.h>", f'#include "{HEADER}"', "int main(void){",
-             'printf("size %zu\\n", sizeof(cdprobe_pingpong_t));',
-             'printf("opt %u\\n", CDPROBE_OPT_PINGPONG_FAULT);']
-    for fname, _ in a.PingPongT._fields_:
-        lines.append(f'printf("{fname} %zu\\n", offsetof(cdprobe_pingpong_t, {fname}));')
-    lines.append("return 0;}")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-o", str(exe), str(src)], check=True)
-    got = dict(l.split() for l in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines())
-    assert int(got["size"]) == C.sizeof(a.PingPongT)
-    for fname, _ in a.PingPongT._fields_:
-        assert int(got[fname]) == getattr(a.PingPongT, fname).offset, fname
-    assert int(got["opt"]) == a.OPT_PINGPONG_FAULT == 17
+    assert_layout(tmp_path, {"cdprobe_pingpong_t": a.PingPongT})
+    assert header_values(tmp_path, "CDPROBE_OPT_PINGPONG_FAULT") == [a.OPT_PINGPONG_FAULT] == [17]
     assert "cdprobe_pingpong" in a.SYMBOLS
     assert a.pingpong_fault(2, 5, 7) == ref.fault_value(2, 5, 7) == (3 << 32) | (6 << 16) | 7
 
@@ -41,17 +27,8 @@ def test_pingpong_struct_layout_matches_c(pkg, tmp_path):
 # ---- words and digests: probe_types.h against the restatement ----------------------------------------------------
 @pytest.fixture(scope="module")
 def words(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("pp") / "pingpong_words"
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "pingpong_words.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [tuple(int(x) for x in l.split()) for l in out]
-
-    return run
+    run = c_tool(tmp_path_factory, "pingpong_words.cc")
+    return lambda cases: [tuple(r) for r in run(cases)]
 
 
 MAX_CALL = (1 << 35) - 1
@@ -141,7 +118,7 @@ def test_wrapper_passes_its_arguments(pkg):
     a = pkg.abi
     calls = []
 
-    class FakeLib:
+    class Lib(FakeLib):
         def cdprobe_pingpong(self, h, trips, reps, fenced, out):
             calls.append((h.value, trips, reps, fenced))
             t = out._obj
@@ -151,15 +128,7 @@ def test_wrapper_passes_its_arguments(pkg):
             t.status[16] = a.ERR_STATE
             return a.ERR_ARG if trips > a.PINGPONG_MAX_TRIPS else a.OK
 
-        def cdprobe_strerror(self, rc):
-            return b"invalid argument"
-
-        def cdprobe_last_error(self):
-            return b""
-
-    p = object.__new__(pkg.Probe)
-    p._lib, p._h = FakeLib(), C.c_void_p(0x1234)
-    try:
+    with fake_probe(pkg, Lib()) as p:
         pp = p.PingPong()
         assert calls[-1] == (0x1234, 0, 0, 0)
         assert (pp.trips, pp.reps, pp.fenced, pp.call_seq) == (256, 8, False, 4)
@@ -170,8 +139,6 @@ def test_wrapper_passes_its_arguments(pkg):
         with pytest.raises(pkg.ProbeError) as e:
             p.PingPong(trips=a.PINGPONG_MAX_TRIPS + 1)
         assert e.value.code == a.ERR_ARG
-    finally:
-        p._h = C.c_void_p()
 
 
 # ---- the compiled kernels -----------------------------------------------------------------------------------------

@@ -2,16 +2,13 @@
 round trip that returned the wrong words cannot pass; the times are plausible; pairs whose mapping is down are not
 exchanged; the skip-ahead fault fails exactly its cell; the call needs no run and disturbs none.  Several ranks share
 one device where a test needs N > 1."""
-import json
-import subprocess
-import sys
 import textwrap
-import uuid
 
 import pytest
 
 import pingpong_ref as ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -209,14 +206,7 @@ def test_two_processes_fill_their_own_rows(pkg):
     """Both processes drive GPU 0, so their contexts are time-sliced and every round trip may wait for a context
     switch: the counts stay small and the times only need to be positive."""
     world = 2
-    session = f"pp-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), str(world)], stdout=subprocess.PIPE,
-                              stderr=subprocess.PIPE, text=True) for r in range(world)]
-    outs = []
-    for pr in procs:
-        so, se = pr.communicate(timeout=600)
-        assert pr.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    outs = run_children(CHILD, world)
     pl = pkg.plan(world, 1 << 20, 1)
     for rank, o in enumerate(outs):
         other = 1 - rank

@@ -13,18 +13,16 @@ of the verdict (tests/verdict_ref.py).
 Several ranks share GPU 0 where a test needs N > 1, so the file runs on one H100.  The one-sided bounds in (b), (c)
 and (f) only ever tighten if other contexts share the device: they can stretch event and host times, never shrink them.
 """
-import json
 import subprocess
-import sys
 import textwrap
 import time
-import uuid
 
 import numpy as np
 import pytest
 
 import verdict_ref
 from conftest import ROOT
+from harness import run_children
 
 pytestmark = pytest.mark.gpu
 
@@ -338,16 +336,7 @@ class SimpleResult:
 
 
 def run_two_processes(nbytes, min_fraction, link_peak, corrupt):
-    session = f"t-{uuid.uuid4().hex[:12]}"
-    procs = [subprocess.Popen([sys.executable, "-c", CHILD, session, str(r), "2", str(nbytes), "64", "8",
-                               repr(min_fraction), repr(link_peak), str(int(corrupt))],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(2)]
-    outs = []
-    for p in procs:
-        so, se = p.communicate(timeout=300)
-        assert p.returncode == 0, se[-2000:]
-        outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
-    return outs
+    return run_children(CHILD, 2, nbytes, 64, 8, min_fraction, link_peak, int(corrupt), timeout=300)
 
 
 @pytest.mark.parametrize("case", ["healthy", "gate-nobody-meets", "corrupt-slice"])

@@ -1,17 +1,14 @@
 """The word-level reference (tests/word_ref.py) against the C oracle and the diagnosis classifier, and the exact blind
 spots of the probe's (S, X) checksum.  No GPU."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
 
 import word_ref as ref
-from conftest import ROOT
+from harness import c_tool
 
-CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
 SEED = 0xCD5EED0000000001
 INDICES = (0, 1, 2047, 2048, 1 << 32, (1 << 56) - 1)
 
@@ -65,17 +62,8 @@ def test_inverses_recover_the_pattern_index():
 # ---- the reference classifier against the C classifier the kernel compiles ------------------------------------
 @pytest.fixture(scope="module")
 def c_classify(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("words") / "diag_classify"
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-I", CSRC, os.path.join(ROOT, "tests", "c", "diag_classify.cc"),
-                    "-o", str(exe)], check=True)
-
-    def run(cases):
-        text = "".join(" ".join(str(x) for x in c) + "\n" for c in cases)
-        out = subprocess.run([str(exe)], input=text, capture_output=True, text=True, check=True).stdout.splitlines()
-        assert len(out) == len(cases)
-        return [tuple(int(x) for x in l.split()) for l in out]
-
-    return run
+    run = c_tool(tmp_path_factory, "diag_classify.cc", "-O1")
+    return lambda cases: [tuple(r) for r in run(cases)]
 
 
 def ref_answer(case):
