@@ -530,6 +530,63 @@ typedef struct {
   double ms;                            /* host wall clock of the call */
 } cdprobe_memcpy_t;
 
+/* Copy-engine all-to-all across the domain (cdprobe_ce_alltoall): in every rep, every cell of the domain copies its
+ * block at once, each on its issuer's copy stream of its own, and the ranks signal each other with stream memory
+ * operations, GPU to GPU (DESIGN §5p).  The cells are cdprobe_memcpy's.  Per-rank entries [r] describe rank r's rep,
+ * from its release until its own copies are complete and every block addressed to it has landed, and are filled by
+ * the process that hosts r.  Per-cell entries [issuer * CDPROBE_MAX_GPUS + target] describe the block of cell (issuer,
+ * target): its check fields (cell_measured, cell_status, bad_sizes, bad_words, first_bad, sum, xr) are filled by the
+ * process that hosts the rank that owns the block's destination and checks it (the issuer on a pull, the target on a
+ * push), its copy times (copy_ns_median) by the process that hosts the issuer.  Size k of an entry is [..][k]. */
+typedef struct {
+  uint32_t abi;
+  uint32_t n;                           /* total ranks in the domain */
+  uint32_t row_mask;                    /* bit r set: rank r's entries, the copy times of the cells it issues and the
+                                           checks of the blocks it owns are filled in */
+  uint32_t reps;                        /* as applied: 0 -> 8; in [1, 64] */
+  uint32_t n_sizes;                     /* entries of size[] */
+  uint32_t op;                          /* as passed: CDPROBE_OP_READ (pull) or CDPROBE_OP_WRITE (push) */
+  uint64_t call_seq;                    /* 1-based count of cdprobe_ce_alltoall calls on this handle, equal in every
+                                           process (0 when the call was refused) */
+  uint64_t area_bytes;                  /* this rank's exchange area (cdprobe_alltoall's): n x bytes_per_pair rounded
+                                           up to 2 MiB */
+  uint64_t size[CDPROBE_BWCURVE_MAX_SIZES]; /* bytes per block per rep: the cdprobe_bwcurve ladder */
+  /* per rank */
+  uint8_t measured[CDPROBE_MAX_GPUS];   /* 1: the rank's reps ran */
+  int32_t status[CDPROBE_MAX_GPUS];     /* 0 ok; else (measured 0) the status of the domain's first down probe or
+                                           exchange-area mapping, row-major */
+  uint32_t blocks[CDPROBE_MAX_GPUS];    /* blocks the rank copies per rep: the cells it issues */
+  float t0_ns[CDPROBE_MAX_GPUS];        /* ns_median of size[0] */
+  float peak_gbps[CDPROBE_MAX_GPUS];    /* max over k of blocks x size[k] / ns_median[k] (bytes per ns) */
+  uint64_t half_bytes[CDPROBE_MAX_GPUS]; /* the smallest size[k] whose rate reaches peak / 2 (computed before peak is
+                                            rounded) */
+  float ns_min[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];    /* ns per rep over the timed reps, by CUDA events A and
+                                                                   B on the rank's stream (0 when not timed) */
+  float ns_median[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* element reps / 2 of the sorted reps */
+  float ns_max[CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];
+  /* per cell [issuer * CDPROBE_MAX_GPUS + target] */
+  uint8_t cell_measured[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS]; /* 1: the block was copied and checked */
+  int32_t cell_status[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];   /* 0 ok; CDPROBE_ERR_INTEGRITY: some rep of some size
+                                                                 landed a bad word or an (S, X) other than the
+                                                                 pattern's; CDPROBE_ERR_TIMEOUT: an (S, X) read of the
+                                                                 block passed timeout_ms; else (cell_measured 0) the
+                                                                 status of the domain's first down mapping */
+  uint32_t bad_sizes[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS];    /* bit k set: a rep of size[k], warm-up included, landed
+                                                                 a bad word or an (S, X) other than the pattern's */
+  float copy_ns_median[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* median ns of the block's
+                                                                 copy over the timed reps, by CUDA events on its copy
+                                                                 stream */
+  uint64_t bad_words[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* words of the block that differ
+                                                                 from the pattern, summed over every rep of size[k],
+                                                                 warm-up included */
+  uint64_t first_bad[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* byte offset of the lowest of
+                                                                 them; UINT64_MAX when clean */
+  uint64_t sum[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES]; /* checksum S of the block as its owner
+                                                                 read it in the last timed rep */
+  uint64_t xr[CDPROBE_MAX_GPUS * CDPROBE_MAX_GPUS][CDPROBE_BWCURVE_MAX_SIZES];  /* checksum X */
+  double ms;                            /* host wall clock of the call */
+} cdprobe_ce_alltoall_t;
+
 /* Per-link NVLink counters of one local device over the last sampled cdprobe_run (cdprobe_links, DESIGN §5o): the
  * difference of two NVML samples, one taken just before the run's clock starts, one just after it stops.  Link l is
  * NVML's scopeId l. */
@@ -595,12 +652,13 @@ CDPROBE_API const char* cdprobe_last_error(void);
  *   cdprobe_plan, cdprobe_schedule, cdprobe_gate, cdprobe_ce_copy, cdprobe_rendezvous_selftest, cdprobe_diagnose,
  *   cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy, cdprobe_links: diagnostics, benches, fault injection;
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy, cdprobe_ce_alltoall, cdprobe_links: diagnostics, benches,
+ *   fault injection;
  *   the reference has no counterpart (it has no probe, SURVEY.md F1).
  *   cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong, cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce,
  *   cdprobe_allreduce_twoshot, cdprobe_allreduce_ll, cdprobe_allreduce_ring, cdprobe_allreduce_push,
- *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy and cdprobe_links are optional for callers: a daemon binds
- *   them with dlsym and works without.
+ *   cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy, cdprobe_ce_alltoall and cdprobe_links are optional for
+ *   callers: a daemon binds them with dlsym and works without.
  */
 CDPROBE_API int cdprobe_open(const cdprobe_config_t* cfg, cdprobe_t** out);
 CDPROBE_API int cdprobe_run(cdprobe_t* h, cdprobe_result_t* out);
@@ -700,6 +758,17 @@ CDPROBE_API int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out
                                              loads and initialises NVML once and resolves each local device by UUID;
                                              both stay until close.  An NVML failure never fails the call or a run: it
                                              shows in cdprobe_links_t's status */
+#define CDPROBE_OPT_CE_ALLTOALL_FAULT 28u /* tests: value = (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) |
+                                             ((k + 1) << 24) | arg arms a fault in cdprobe_ce_alltoall, in timed rep 1
+                                             of size[k] of cell (issuer, target), in the process that hosts the issuer,
+                                             on the cell's copy stream: mode 0, after the copy and before the landed
+                                             flag, destination word `arg` (< 2^24) is overwritten with its pattern value
+                                             xored with 1 (an 8-byte copy from host memory); mode 1, no copy is queued
+                                             but the landed flag is still published, so the destination its owner
+                                             cleared reads as 0s; either fails exactly that cell and size.  Mode 2
+                                             holds the copy stream on a second host ticket released `arg` us (below
+                                             timeout_ms / 2) after the rep's: every cell stays exact, and the rep of
+                                             the rank that waits for the block takes at least that long.  0 disarms */
 CDPROBE_API int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value);
 /* Copy-engine reference on the probe's own buffers (the same-box ceiling the roofline is quoted against; not part
  * of a probe): copy k moves `bytes` (capped at the source / landing size) `reps` times back to back between local
@@ -1013,6 +1082,35 @@ CDPROBE_API int cdprobe_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allr
  * not complete (sticky); CDPROBE_ERR_UNSUPPORTED: the driver has no cuStreamWaitValue64; CDPROBE_ERR_CUDA: it
  * refused one (sticky); CDPROBE_ERR_STATE: sticky handle. */
 CDPROBE_API int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* out);
+/* Copy-engine all-to-all across the domain, checked word for word (DESIGN §5p): for each size of the cdprobe_bwcurve
+ * ladder, one untimed warm-up rep, then `reps` timed reps, in each of which every cell of cdprobe_memcpy (the same
+ * source slice, the same block of the exchange area, the diagonal with a loop-back slice) copies the first size bytes
+ * of its slice with cudaMemcpyAsync, all at once.  Each local rank keeps one copy stream per cell it issues, made on
+ * the first call and kept until close; its own stream carries the barrier, the joins and the checks.  A rep of rank r,
+ * queued whole before the host releases the rep's ticket (cdprobe_memcpy's): its stream waits for the ticket, writes
+ * the opening value into line r of every peer's flag lines with cuStreamWriteValue64 through r's mapping and waits
+ * (cuStreamWaitValue64, GEQ) for every peer's in its own; event A; each copy stream waits for A, copies between
+ * events, and on a push then writes the landed value into line r of the receiver's lines (fenced, so it is ordered
+ * after the copy); the stream joins every copy stream and, on a push, waits for every sender's landed value; event B.
+ * ns per rep is B - A; copy_ns_median comes from each copy stream's own events (about 0.5 us resolution).  Once every
+ * local B has completed, the rank that owns each destination checks it on its own GPU, as cdprobe_memcpy's issuer does:
+ * the diagnosis against the pattern, the (S, X) read, the clearing to 0.  The next rep's opening write is queued behind
+ * those checks, so no block is copied into before its owner has checked and cleared the last one.  Only the domain
+ * barrier before each size is a host collective.  The exchange area is cdprobe_alltoall's and cdprobe_memcpy's. When
+ * any probe or exchange-area mapping of the domain is down, nothing runs: every local row and every cell a local rank
+ * issues or owns gets the status of the domain's first down cell, row-major, and the call returns CDPROBE_OK.  No
+ * kernel runs in the timed window.  Collective when world_size > 1: every process calls it with the same op and reps.
+ * Touches no result, pattern, source buffer, landing slot, run_seq, warm-up state or other measurement's lines or
+ * areas.  *out carries abi, n, reps and op whatever the return code.  CDPROBE_ERR_ARG: as cdprobe_memcpy, or an armed
+ * CDPROBE_OPT_CE_ALLTOALL_FAULT that names no cell of the domain, a k >= n_sizes, a word >= size[k] / 8 (modes 0 and
+ * 1), a delay of timeout_ms / 2 or more (mode 2) or a mode above 2; CDPROBE_ERR_UNSUPPORTED (every process): the
+ * driver lacks cuStreamWriteValue64 or cuStreamWaitValue64, or some process would hold more streams on one device
+ * (each local rank's own and its copy streams) than CUDA_DEVICE_MAX_CONNECTIONS (read at open, default 8) gives
+ * hardware queues, so that a stream wait could block a stream sharing its queue (cdprobe_last_error names the need and
+ * the limit); CDPROBE_ERR_CUDA: the driver refused a stream memory operation (sticky, the CUresult named);
+ * CDPROBE_ERR_TIMEOUT: some rep's B had not completed timeout_ms after its release (sticky; the host writes the awaited
+ * values into its own ranks' lines first, so no stream stays blocked); CDPROBE_ERR_STATE: sticky handle. */
+CDPROBE_API int cdprobe_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_alltoall_t* out);
 /* The per-link NVLink counters of the last cdprobe_run taken with CDPROBE_OPT_LINK_COUNTERS on: one row per distinct
  * device of this process's ranks (ranks sharing a device share a row), with the payload the run's phase tables moved
  * between devices next to what NVML counted.  The samples bracket probe_ms: the first is taken before its clock

@@ -37,6 +37,7 @@ typedef int (*bw_fn)(cdprobe_t*, uint32_t, cdprobe_bwcurve_t*);
 typedef int (*ar_fn)(cdprobe_t*, uint32_t, cdprobe_allreduce_t*);
 typedef int (*a2a_fn)(cdprobe_t*, uint32_t, cdprobe_alltoall_t*);
 typedef int (*mc_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_memcpy_t*);
+typedef int (*cea_fn)(cdprobe_t*, uint32_t, uint32_t, cdprobe_ce_alltoall_t*);
 typedef int (*opt_fn)(cdprobe_t*, uint32_t, uint64_t);
 typedef int (*links_fn)(cdprobe_t*, cdprobe_links_t*);
 
@@ -56,6 +57,7 @@ static ar_fn cdp_arring;  // optional: absent from libraries that predate cdprob
 static ar_fn cdp_arpush;  // optional: absent from libraries that predate cdprobe_allreduce_push
 static ar_fn cdp_arnvls;  // optional: absent from libraries that predate cdprobe_allreduce_nvls
 static mc_fn cdp_mc;      // optional: absent from libraries that predate cdprobe_memcpy
+static cea_fn cdp_cea;    // optional: absent from libraries that predate cdprobe_ce_alltoall
 static opt_fn cdp_opt;    // optional: this binding did not need cdprobe_set_option before the link counters
 static links_fn cdp_links;  // optional: absent from libraries that predate cdprobe_links
 
@@ -82,6 +84,7 @@ static int cdp_load(const char* path) {
   cdp_arpush = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_push");
   cdp_arnvls = (ar_fn)dlsym(cdp_dl, "cdprobe_allreduce_nvls");
   cdp_mc = (mc_fn)dlsym(cdp_dl, "cdprobe_memcpy");
+  cdp_cea = (cea_fn)dlsym(cdp_dl, "cdprobe_ce_alltoall");
   cdp_opt = (opt_fn)dlsym(cdp_dl, "cdprobe_set_option");
   cdp_links = (links_fn)dlsym(cdp_dl, "cdprobe_links");
   if (!cdp_open || !cdp_run || !cdp_close || !cdp_strerror || !cdp_last || !cdp_abi) return -2;
@@ -135,6 +138,10 @@ static int cdp_call_allreduce_nvls(cdprobe_t* h, uint32_t reps, cdprobe_allreduc
 static int cdp_has_memcpy(void) { return cdp_mc != NULL; }
 static int cdp_call_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* mc) {
   return cdp_mc(h, op, reps, mc);
+}
+static int cdp_has_ce_alltoall(void) { return cdp_cea != NULL; }
+static int cdp_call_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_alltoall_t* ca) {
+  return cdp_cea(h, op, reps, ca);
 }
 static int cdp_has_set_option(void) { return cdp_opt != NULL; }
 static int cdp_call_set_option(cdprobe_t* h, uint32_t option, uint64_t value) { return cdp_opt(h, option, value); }
@@ -405,6 +412,34 @@ type Memcpy struct {
 	NsMin, NsMedian, NsMax [][]float32 // [cell][size]: ns per copy over the timed reps, by CUDA events
 	Sum, Xr                [][]uint64  // [cell][size]: (S, X) of the destination in the last timed rep
 	BadWords, FirstBad     [][]uint64  // [cell][size]: the word check over every rep; FirstBad is MaxUint64 when clean
+	Ms                     float64
+}
+
+// CeAllToAll is the copy-engine all-to-all (cdprobe_ce_alltoall_t), pulled (Op CDPROBE_OP_READ) or pushed
+// (CDPROBE_OP_WRITE).  Per-rank slices are filled for this process's ranks; per-cell ones are [issuer][target]: the
+// check fields for the blocks this process's ranks own (the issuer's on a pull, the target's on a push), CopyNsMedian
+// for the cells they issue.  The per-size ones hold one entry per Sizes element; every timing is 0 where a rank did
+// not run.
+type CeAllToAll struct {
+	N                      int
+	RowMask                uint32       // this process's ranks
+	Reps                   int          // timed reps per size, as applied
+	Op                     uint32       // CDPROBE_OP_READ (pull) or CDPROBE_OP_WRITE (push)
+	CallSeq                uint64       // 1-based count of CeAllToAll calls on this handle, equal in every process
+	AreaBytes              uint64       // this rank's exchange area, where the blocks land
+	Sizes                  []uint64     // bytes per block per rep
+	Measured               []bool       // [rank]
+	Status                 []int32      // [rank]: 0 ok; else the status of the domain's first down mapping
+	Blocks                 []uint32     // [rank]: blocks copied per rep (the cells it issues)
+	T0Ns, PeakGBps         []float32    // [rank]: median ns of the smallest size; max over sizes of blocks x size / ns
+	HalfBytes              []uint64     // [rank]: the smallest size reaching half the peak
+	NsMin, NsMedian, NsMax [][]float32  // [rank][size]: ns per rep, release to every block landed, over the timed reps
+	CellMeasured           [][]bool     // [issuer][target]
+	CellStatus             [][]int32    // [issuer][target]: 0 ok; CDPROBE_ERR_INTEGRITY; CDPROBE_ERR_TIMEOUT; else a mapping status
+	BadSizes               [][]uint32   // [issuer][target]: bit k: Sizes[k] landed a bad word or checksum
+	CopyNsMedian           [][][]float32 // [issuer][target][size]: median ns of the cell's copy, by CUDA events
+	BadWords, FirstBad     [][][]uint64 // [issuer][target][size]: the word check; FirstBad is MaxUint64 when clean
+	Sum, Xr                [][][]uint64 // [issuer][target][size]: (S, X) of the block in the last timed rep
 	Ms                     float64
 }
 
@@ -1034,6 +1069,79 @@ func (p *Probe) Memcpy(op uint32, reps int) (Memcpy, error) {
 				out.Xr[c][s] = uint64(mc.xr[k][s])
 				out.BadWords[c][s] = uint64(mc.bad_words[k][s])
 				out.FirstBad[c][s] = uint64(mc.first_bad[k][s])
+			}
+		}
+	}
+	return out, nil
+}
+
+// CeAllToAll runs the copy-engine all-to-all: in every rep every cell copies its block at once on a copy stream of its
+// own, pulled (op CDPROBE_OP_READ) or pushed (CDPROBE_OP_WRITE), the ranks signalling each other with stream memory
+// operations, at each size of the bwcurve ladder; the owner of every block checks every word (reps 0: 8 timed reps).
+// Collective when the domain spans processes.  ErrUnsupported when the library predates cdprobe_ce_alltoall.
+func (p *Probe) CeAllToAll(op uint32, reps int) (CeAllToAll, error) {
+	if C.cdp_has_ce_alltoall() == 0 {
+		return CeAllToAll{}, fmt.Errorf("%w: libcdprobe.so has no cdprobe_ce_alltoall", ErrUnsupported)
+	}
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	ca := new(C.cdprobe_ce_alltoall_t)
+	rc := C.cdp_call_ce_alltoall(p.h, C.uint32_t(op), C.uint32_t(reps), ca)
+	if rc != 0 {
+		err := fmt.Errorf("cdprobe_ce_alltoall: %s: %s", C.GoString(C.cdp_call_strerror(rc)), C.GoString(C.cdp_call_last()))
+		switch rc {
+		case C.CDPROBE_ERR_STATE:
+			err = fmt.Errorf("%w: %v", ErrState, err)
+		case C.CDPROBE_ERR_UNSUPPORTED:
+			err = fmt.Errorf("%w: %v", ErrUnsupported, err)
+		}
+		return CeAllToAll{}, err
+	}
+	n, ns := int(ca.n), int(ca.n_sizes)
+	out := CeAllToAll{N: n, RowMask: uint32(ca.row_mask), Reps: int(ca.reps), Op: uint32(ca.op),
+		CallSeq: uint64(ca.call_seq), AreaBytes: uint64(ca.area_bytes), Ms: float64(ca.ms)}
+	out.Sizes = make([]uint64, ns)
+	for s := 0; s < ns; s++ {
+		out.Sizes[s] = uint64(ca.size[s])
+	}
+	out.Measured, out.Status, out.Blocks = make([]bool, n), make([]int32, n), make([]uint32, n)
+	out.T0Ns, out.PeakGBps, out.HalfBytes = make([]float32, n), make([]float32, n), make([]uint64, n)
+	out.NsMin, out.NsMedian, out.NsMax = make([][]float32, n), make([][]float32, n), make([][]float32, n)
+	out.CellMeasured, out.CellStatus, out.BadSizes = make([][]bool, n), make([][]int32, n), make([][]uint32, n)
+	out.CopyNsMedian = make([][][]float32, n)
+	out.BadWords, out.FirstBad = make([][][]uint64, n), make([][][]uint64, n)
+	out.Sum, out.Xr = make([][][]uint64, n), make([][][]uint64, n)
+	for r := 0; r < n; r++ {
+		out.Measured[r] = ca.measured[r] != 0
+		out.Status[r] = int32(ca.status[r])
+		out.Blocks[r] = uint32(ca.blocks[r])
+		out.T0Ns[r] = float32(ca.t0_ns[r])
+		out.PeakGBps[r] = float32(ca.peak_gbps[r])
+		out.HalfBytes[r] = uint64(ca.half_bytes[r])
+		out.NsMin[r], out.NsMedian[r], out.NsMax[r] = make([]float32, ns), make([]float32, ns), make([]float32, ns)
+		for s := 0; s < ns; s++ {
+			out.NsMin[r][s] = float32(ca.ns_min[r][s])
+			out.NsMedian[r][s] = float32(ca.ns_median[r][s])
+			out.NsMax[r][s] = float32(ca.ns_max[r][s])
+		}
+		out.CellMeasured[r], out.CellStatus[r], out.BadSizes[r] = make([]bool, n), make([]int32, n), make([]uint32, n)
+		out.CopyNsMedian[r] = make([][]float32, n)
+		out.BadWords[r], out.FirstBad[r] = make([][]uint64, n), make([][]uint64, n)
+		out.Sum[r], out.Xr[r] = make([][]uint64, n), make([][]uint64, n)
+		for d := 0; d < n; d++ {
+			c := r*C.CDPROBE_MAX_GPUS + d
+			out.CellMeasured[r][d] = ca.cell_measured[c] != 0
+			out.CellStatus[r][d] = int32(ca.cell_status[c])
+			out.BadSizes[r][d] = uint32(ca.bad_sizes[c])
+			out.CopyNsMedian[r][d] = make([]float32, ns)
+			out.BadWords[r][d], out.FirstBad[r][d] = make([]uint64, ns), make([]uint64, ns)
+			out.Sum[r][d], out.Xr[r][d] = make([]uint64, ns), make([]uint64, ns)
+			for s := 0; s < ns; s++ {
+				out.CopyNsMedian[r][d][s] = float32(ca.copy_ns_median[c][s])
+				out.BadWords[r][d][s] = uint64(ca.bad_words[c][s])
+				out.FirstBad[r][d][s] = uint64(ca.first_bad[c][s])
+				out.Sum[r][d][s] = uint64(ca.sum[c][s])
+				out.Xr[r][d][s] = uint64(ca.xr[c][s])
 			}
 		}
 	}

@@ -209,6 +209,29 @@ type Memcpy struct {
 	Ms                     float64
 }
 
+type CeAllToAll struct {
+	N                      int
+	RowMask                uint32
+	Reps                   int
+	Op                     uint32
+	CallSeq                uint64
+	AreaBytes              uint64
+	Sizes                  []uint64
+	Measured               []bool
+	Status                 []int32
+	Blocks                 []uint32
+	T0Ns, PeakGBps         []float32
+	HalfBytes              []uint64
+	NsMin, NsMedian, NsMax [][]float32
+	CellMeasured           [][]bool
+	CellStatus             [][]int32
+	BadSizes               [][]uint32
+	CopyNsMedian           [][][]float32
+	BadWords, FirstBad     [][][]uint64
+	Sum, Xr                [][][]uint64
+	Ms                     float64
+}
+
 func Open(Config) (*Probe, error)                  { return nil, ErrUnsupported }
 func (*Probe) Run(context.Context) (Result, error) { return Result{}, ErrUnsupported }
 func (*Probe) Diagnose(uint32, int, int, int) (Diagnosis, error) {
@@ -228,6 +251,7 @@ func (*Probe) AllReducePush(int) (AllReduce, error) { return AllReduce{}, ErrUns
 func (*Probe) AllReduceNVLS(int) (AllReduce, error) { return AllReduce{}, ErrUnsupported }
 func (*Probe) AllToAll(int) (AllToAll, error) { return AllToAll{}, ErrUnsupported }
 func (*Probe) Memcpy(uint32, int) (Memcpy, error) { return Memcpy{}, ErrUnsupported }
+func (*Probe) CeAllToAll(uint32, int) (CeAllToAll, error) { return CeAllToAll{}, ErrUnsupported }
 func (*Probe) SetOption(uint32, uint64) error { return ErrUnsupported }
 func (p *Probe) Links() (Links, error)         { return Links{}, ErrUnsupported }
 func (*Probe) Close() {}

@@ -17,6 +17,7 @@ from .fabricprobe import (  # noqa: F401
     AllToAll,
     Atomics,
     BwCurve,
+    CeAllToAll,
     Config,
     Diagnosis,
     ErrUnsupported,
@@ -32,4 +33,4 @@ from .fabricprobe import (  # noqa: F401
     topology,
 )
 
-__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "AllToAll", "Memcpy", "Open", "gate", "plan", "topology"]
+__all__ = ["abi", "build", "Config", "Probe", "ProbeError", "ErrUnsupported", "Result", "Diagnosis", "Latency", "PingPong", "Atomics", "BwCurve", "AllReduce", "AllToAll", "Memcpy", "CeAllToAll", "Open", "gate", "plan", "topology"]

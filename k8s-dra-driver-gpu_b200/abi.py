@@ -43,6 +43,7 @@ OPT_ALLREDUCE_PUSH_FAULT = 24
 OPT_ALLREDUCE_NVLS_FAULT = 25
 OPT_MEMCPY_FAULT = 26
 OPT_LINK_COUNTERS = 27
+OPT_CE_ALLTOALL_FAULT = 28
 
 DIAG_SAMPLES = 16
 DIAG_FLIP, DIAG_ZERO, DIAG_DISPLACED, DIAG_STALE, DIAG_FOREIGN = 0, 1, 2, 3, 4
@@ -67,6 +68,7 @@ ALLREDUCE_PATH_RING = 4  # cdprobe_allreduce_t.path of cdprobe_allreduce_ring
 ALLREDUCE_PATH_NVLS = 5  # cdprobe_allreduce_t.path of cdprobe_allreduce_nvls
 ALLTOALL_DEFAULT_REPS, ALLTOALL_MAX_REPS = 8, 64
 MEMCPY_DEFAULT_REPS, MEMCPY_MAX_REPS = 8, 64
+CE_ALLTOALL_DEFAULT_REPS, CE_ALLTOALL_MAX_REPS = 8, 64
 
 NVLINK_MAX_LINKS = 18
 LINK_REPLAY, LINK_RECOVERY, LINK_CRC = 0, 1, 2
@@ -431,6 +433,38 @@ class MemcpyT(C.Structure):
     ]
 
 
+class CeAllToAllT(C.Structure):
+    _fields_ = [
+        ("abi", C.c_uint32),
+        ("n", C.c_uint32),
+        ("row_mask", C.c_uint32),
+        ("reps", C.c_uint32),
+        ("n_sizes", C.c_uint32),
+        ("op", C.c_uint32),
+        ("call_seq", C.c_uint64),
+        ("area_bytes", C.c_uint64),
+        ("size", C.c_uint64 * BWCURVE_MAX_SIZES),
+        ("measured", C.c_uint8 * MAX_GPUS),
+        ("status", C.c_int32 * MAX_GPUS),
+        ("blocks", C.c_uint32 * MAX_GPUS),
+        ("t0_ns", C.c_float * MAX_GPUS),
+        ("peak_gbps", C.c_float * MAX_GPUS),
+        ("half_bytes", C.c_uint64 * MAX_GPUS),
+        ("ns_min", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("ns_median", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("ns_max", C.c_float * BWCURVE_MAX_SIZES * MAX_GPUS),
+        ("cell_measured", C.c_uint8 * _N2),
+        ("cell_status", C.c_int32 * _N2),
+        ("bad_sizes", C.c_uint32 * _N2),
+        ("copy_ns_median", C.c_float * BWCURVE_MAX_SIZES * _N2),
+        ("bad_words", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("first_bad", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("sum", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("xr", C.c_uint64 * BWCURVE_MAX_SIZES * _N2),
+        ("ms", C.c_double),
+    ]
+
+
 class LinkDeviceT(C.Structure):
     _fields_ = [
         ("status", C.c_int32),
@@ -467,6 +501,16 @@ def memcpy_fault(issuer: int, target: int, k: int, word: int, mode: int = 0) -> 
     if mode not in (0, 1) or not (0 <= issuer < 255 and 0 <= target < 255 and 0 <= k < 255 and 0 <= word < 1 << 24):
         raise ValueError("memcpy_fault: mode 0 or 1, ranks and k below 255, word below 2^24")
     return (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | ((k + 1) << 24) | word
+
+
+def ce_alltoall_fault(issuer: int, target: int, k: int, arg: int, mode: int = 0) -> int:
+    """The CDPROBE_OPT_CE_ALLTOALL_FAULT value for timed rep 1 of size[k] of cell (issuer, target) of
+    cdprobe_ce_alltoall: mode 0, destination word `arg` is xored with 1 after the copy and before the landed flag; mode
+    1, no copy is queued but the landed flag is published; mode 2, the copy stream is held `arg` us.  Fields that do not
+    fit are refused here."""
+    if mode not in (0, 1, 2) or not (0 <= issuer < 255 and 0 <= target < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
+        raise ValueError("ce_alltoall_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
+    return (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | ((k + 1) << 24) | arg
 
 
 def alltoall_fault(sender: int, receiver: int, k: int, word: int) -> int:
@@ -570,6 +614,7 @@ SYMBOLS = {
     "cdprobe_allreduce_nvls": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllReduceT)]),
     "cdprobe_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(AllToAllT)]),
     "cdprobe_memcpy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(MemcpyT)]),
+    "cdprobe_ce_alltoall": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(CeAllToAllT)]),
     "cdprobe_links": (C.c_int, [C.c_void_p, C.POINTER(LinksT)]),
     "cdprobe_close": (None, [C.c_void_p]),
     "cdprobe_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(PlanT)]),

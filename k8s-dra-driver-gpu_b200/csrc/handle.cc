@@ -17,6 +17,7 @@
 #include <sched.h>
 #include <stddef.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <time.h>
 #include <unistd.h>
@@ -691,9 +692,18 @@ static void destroy(cdprobe* h) {
     if (L.ev1) cudaEventDestroy(L.ev1);
     for (cudaEvent_t ev : L.memcpy_ev)
       if (ev) cudaEventDestroy(ev);
+    for (uint32_t i = 0; i < (uint32_t)kMaxRanks; ++i) {
+      if (L.cea_stream[i]) cudaStreamSynchronize(L.cea_stream[i]);
+      for (cudaEvent_t ev : L.cea_copy_ev[i])
+        if (ev) cudaEventDestroy(ev);
+      if (L.cea_stream[i]) cudaStreamDestroy(L.cea_stream[i]);
+    }
+    for (cudaEvent_t ev : L.cea_ev)
+      if (ev) cudaEventDestroy(ev);
     if (L.stream) cudaStreamDestroy(L.stream);
   }
   if (h->memcpy_host) cudaFreeHost(h->memcpy_host);
+  if (h->cea_host) cudaFreeHost(h->cea_host);
   delete h->links;
   h->rdv.close();
   delete h;
@@ -713,6 +723,12 @@ static int open_impl(const cdprobe_config_t* cfg, cdprobe* h) {
   h->path = (c.flags & CDPROBE_FLAG_PATH_LDST) ? 1u : 0u;
   if (!(c.flags & CDPROBE_FLAG_SERIAL_VERIFY)) c.flags |= CDPROBE_FLAG_OVERLAP_VERIFY;  // overlapped verify is the default
   h->seed = c.seed ? c.seed : kDefaultSeed;
+  // the hardware queues per device the CUDA runtime of this process gives its streams (cdprobe_ce_alltoall); it reads
+  // the variable once, at its initialisation, and clamps it to [1, 32]
+  if (const char* mc = getenv("CUDA_DEVICE_MAX_CONNECTIONS"); mc != nullptr && *mc != '\0') {
+    const long v = strtol(mc, nullptr, 10);
+    if (v > 0) h->max_connections = (uint32_t)std::min(v, 32L);
+  }
   c.session[sizeof(c.session) - 1] = '\0';
   memset(h->status, 0, sizeof(h->status));
 
@@ -1378,6 +1394,10 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       return CDPROBE_OK;
     case CDPROBE_OPT_MEMCPY_FAULT:  // checked against the domain and the size ladder by cdprobe_memcpy
       h->memcpy_fault = value;
+      return CDPROBE_OK;
+    case CDPROBE_OPT_CE_ALLTOALL_FAULT:  // checked against the domain, the size ladder and timeout_ms by
+                                         // cdprobe_ce_alltoall
+      h->cea_fault = value;
       return CDPROBE_OK;
     case CDPROBE_OPT_LINK_COUNTERS:
       if (value > 1) return CDPROBE_ERR_ARG;

@@ -1,8 +1,10 @@
 // measure.cc — the on-demand measurements behind the C ABI: cdprobe_diagnose, cdprobe_latency, cdprobe_pingpong,
 // cdprobe_atomics, cdprobe_bwcurve, cdprobe_allreduce, cdprobe_allreduce_twoshot, cdprobe_allreduce_ll,
-// cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_allreduce_nvls, cdprobe_alltoall and cdprobe_memcpy.  Each
+// cdprobe_allreduce_ring, cdprobe_allreduce_push, cdprobe_allreduce_nvls, cdprobe_alltoall, cdprobe_memcpy and
+// cdprobe_ce_alltoall.  Each
 // runs on the local ranks' own streams, between probe runs, and has its results on the host before it returns.
 #include <string.h>
+#include <unistd.h>
 
 #include <stddef.h>
 
@@ -400,12 +402,14 @@ static FaultSpot fault_spot(uint64_t v, const Ladder& lad) {
 // out->path of a ladder measurement that runs on the handle's data path (CDPROBE_OPT_PATH).
 constexpr uint32_t kHandlePath = UINT32_MAX;
 
-// out->path of a ladder measurement that reports one; cdprobe_memcpy_t has none (its copies use no data path).
+// out->path of a ladder measurement that reports one; cdprobe_memcpy_t and cdprobe_ce_alltoall_t have none (their
+// copies use no data path).
 template <typename Out>
 static void put_path(Out* out, uint32_t path) {
   out->path = path;
 }
 static void put_path(cdprobe_memcpy_t*, uint32_t) {}
+static void put_path(cdprobe_ce_alltoall_t*, uint32_t) {}
 
 // The opening of the ladder measurements (bwcurve, the all-reduces, alltoall, memcpy): *out cleared and stamped with
 // reps (0: default_reps); once the handle is known, n and the data path (`path`, or the handle's) before the handle is
@@ -975,30 +979,21 @@ static cudaError_t memcpy_timed(cdprobe* h, uint32_t li, uint32_t j, uint32_t op
   return e;
 }
 
-// The untimed checks of rep `rep` of the cell, queued on L's stream behind its event B: the armed mode-0 fault's store
-// (`flip`: word flip_word), the diagnosis of every destination word against the source slice's pattern (diag_launch),
-// the (S, X) read of the destination (bwcurve_kernel, one rep of one size), the clearing of the destination to 0, and
-// the copies of what the checks left into rep's slot of the host block.
-static cudaError_t memcpy_check(cdprobe* h, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes, uint32_t rep,
-                                bool flip, uint64_t flip_word) {
+// The untimed checks of the block cell `c` landed, queued on stream `s` of local rank L = h->lr[li], the block's
+// owner, on its own memory and scratch: the diagnosis of every destination word against the source slice's pattern
+// (diag_launch), the (S, X) read of the destination (bwcurve_kernel, one rep of one size), the clearing of the
+// destination to 0, and the copies of what the checks left into `got`.  cdprobe_memcpy's issuer and
+// cdprobe_ce_alltoall's owners check this way.
+static cudaError_t check_block(cdprobe* h, uint32_t li, const MemcpyCell& c, uint64_t bytes, MemcpyRepOut* got) {
   LocalRank& L = h->lr[li];
   const Plan& pl = h->plan;
-  const MemcpyCell c = memcpy_cell(pl, op, L.grank, j);
   const MemcpyScratch ms(pl.bpp);
-  MemcpyHost* const host = h->memcpy_host;
-  MemcpyRepOut* const got = &host->rep[li][rep];
   uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
   uint8_t* const scratch = static_cast<uint8_t*>(L.scratch);
   cudaStream_t s = L.stream;
-  cudaError_t e = cudaSetDevice(L.ordinal);
-  if (e == cudaSuccess && flip) {
-    host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + flip_word) ^ 1ull;
-    e = cudaMemcpyAsync(dst + 8 * flip_word, &host->flip[li], 8, cudaMemcpyHostToDevice, s);
-  }
-  if (e == cudaSuccess)
-    e = (cudaError_t)diag_launch(dst, diag_read_spec(h->seed, h->n_total, c.src_rank, c.first_word, bytes / 8,
-                                                     pl.src_bytes / 8),
-                                 scratch + ms.diag_off, L.sm_count, s);
+  cudaError_t e = (cudaError_t)diag_launch(
+      dst, diag_read_spec(h->seed, h->n_total, c.src_rank, c.first_word, bytes / 8, pl.src_bytes / 8),
+      scratch + ms.diag_off, L.sm_count, s);
   if (e == cudaSuccess) e = cudaMemsetAsync(scratch, 0, sizeof(BwScratch), s);
   if (e == cudaSuccess) {
     BwCurveParams p;
@@ -1018,6 +1013,23 @@ static cudaError_t memcpy_check(cdprobe* h, uint32_t li, uint32_t j, uint32_t op
     e = cudaMemcpyAsync(&got->abort_flag, scratch, sizeof(got->abort_flag), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess)
     e = cudaMemcpyAsync(&got->acc, scratch + offsetof(BwScratch, rep), sizeof(got->acc), cudaMemcpyDeviceToHost, s);
+  return e;
+}
+
+// The untimed checks of rep `rep` of the cell, queued on L's stream behind its event B: the armed mode-0 fault's store
+// (`flip`: word flip_word), then check_block into rep's slot of the host block.
+static cudaError_t memcpy_check(cdprobe* h, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes, uint32_t rep,
+                                bool flip, uint64_t flip_word) {
+  LocalRank& L = h->lr[li];
+  const MemcpyCell c = memcpy_cell(h->plan, op, L.grank, j);
+  MemcpyHost* const host = h->memcpy_host;
+  uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
+  cudaError_t e = cudaSetDevice(L.ordinal);
+  if (e == cudaSuccess && flip) {
+    host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + flip_word) ^ 1ull;
+    e = cudaMemcpyAsync(dst + 8 * flip_word, &host->flip[li], 8, cudaMemcpyHostToDevice, L.stream);
+  }
+  if (e == cudaSuccess) e = check_block(h, li, c, bytes, &host->rep[li][rep]);
   return e;
 }
 
@@ -1064,6 +1076,222 @@ static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladd
     if (target[li] >= 0)
       e = memcpy_check(h, li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.word);
   return e != cudaSuccess ? fail_sticky(h, "cdprobe_memcpy: queue the checks", e) : CDPROBE_OK;
+}
+
+constexpr uint32_t kCeA2aDefaultReps = 8;
+
+// cdprobe_ce_alltoall's armed fault once the call has accepted it: timed rep 1 of size k of cell (issuer, target), on
+// the cell's copy stream, flips destination word `arg` (mode 0), queues no copy (mode 1), or is held `arg` us (mode 2).
+// issuer kMaxRanks: none.
+struct CeA2aFault {
+  uint32_t issuer = kMaxRanks, target = 0, k = 0, mode = 0;
+  uint64_t arg = 0;
+};
+
+// cdprobe_ce_alltoall's pinned, mapped and portable host block, made on first use and kept until close: the ticket
+// every local stream waits on, the second ticket a mode-2 fault holds a copy stream on, the tickets handed out so far,
+// the word the armed mode-0 fault stores per local rank, the awaited values the host writes into its own ranks' lines
+// when it gives up on a rep, and what each rep's checks left, per local owner, block (its sender) and rep.
+struct CeA2aHost {
+  uint64_t ticket, hold, issued;
+  uint64_t flip[kMaxRanks];
+  uint64_t release[2];
+  MemcpyRepOut rep[kMaxRanks][kMaxRanks][kRepSlots];
+};
+
+// The cells local rank li issues, one per copy stream: its peers in the order rank + 1, rank + 2, ... (mod n), then
+// the diagonal with a loop-back slice.  Returns their count.
+static uint32_t ce_a2a_targets(const cdprobe* h, uint32_t li, uint32_t* target) {
+  const uint32_t g = h->lr[li].grank, n = h->n_total;
+  uint32_t c = 0;
+  for (uint32_t d = 1; d <= n; ++d)
+    if ((g + d) % n != g || h->plan.diag) target[c++] = (g + d) % n;
+  return c;
+}
+
+// Why this process cannot run cdprobe_ce_alltoall, empty when it can: the driver lacks a stream memory operation, or
+// its local ranks would hold more streams on one device than the hardware queues CUDA_DEVICE_MAX_CONNECTIONS gives.
+static std::string ce_a2a_refusal(cdprobe* h) {
+  std::string err;
+  if (h->drv.load_stream_wait(&err) != cudaSuccess || h->drv.load_stream_write(&err) != cudaSuccess)
+    return "cdprobe_ce_alltoall: " + err;
+  int ordinal[kMaxRanks], worst = 0;
+  for (uint32_t li = 0; li < h->n_local; ++li) ordinal[li] = h->lr[li].ordinal;
+  const uint32_t need = ce_a2a_queues(h->n_total, h->plan.diag, h->n_local, ordinal, &worst);
+  if (need <= h->max_connections) return "";
+  return "cdprobe_ce_alltoall: needs " + std::to_string(need) + " queues on ordinal " + std::to_string(worst) +
+         ", CUDA_DEVICE_MAX_CONNECTIONS allows " + std::to_string(h->max_connections);
+}
+
+// The host block, and every local rank's copy streams and events, made on the first call and kept until close.
+static int ce_a2a_setup(cdprobe* h) {
+  CDP_RT(cudaSetDevice(h->lr[0].ordinal));
+  if (h->cea_host == nullptr) {
+    void* p = nullptr;
+    CDP_RT(cudaHostAlloc(&p, sizeof(CeA2aHost), cudaHostAllocPortable | cudaHostAllocMapped));
+    memset(p, 0, sizeof(CeA2aHost));
+    h->cea_host = static_cast<CeA2aHost*>(p);
+  }
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    uint32_t target[kMaxRanks];
+    const uint32_t cells = ce_a2a_targets(h, li, target);
+    CDP_RT(cudaSetDevice(L.ordinal));
+    for (uint32_t i = 0; i < cells; ++i) {
+      if (L.cea_stream[i] == nullptr) CDP_RT(cudaStreamCreateWithFlags(&L.cea_stream[i], cudaStreamNonBlocking));
+      for (uint32_t x = 0; x < 3; ++x)
+        if (L.cea_copy_ev[i][x] == nullptr)
+          CDP_RT(cudaEventCreateWithFlags(&L.cea_copy_ev[i][x], x < 2 ? cudaEventDefault : cudaEventDisableTiming));
+    }
+    for (cudaEvent_t& ev : L.cea_ev)
+      if (ev == nullptr) CDP_RT(cudaEventCreate(&ev));
+  }
+  return CDPROBE_OK;
+}
+
+// Word `word` (0: opening, 1: landed) of `sender`'s line in `owner`'s flag lines, as local rank li maps them.
+static CUdeviceptr ce_a2a_line(const cdprobe* h, uint32_t li, uint32_t owner, uint32_t sender, uint32_t word) {
+  return h->mem.va[li][owner] + kCeA2aOff + (uint64_t)sender * sizeof(FlagLine) + 8ull * word;
+}
+
+// When the host gives up on a rep whose values are v: writes v into both words of every line of its own ranks, on a
+// stream of its own, so that no stream of theirs is left waiting at close.  Best effort: it waits at most timeout_ms.
+static void ce_a2a_unblock(cdprobe* h, uint64_t v) {
+  CeA2aHost* const host = h->cea_host;
+  host->release[0] = host->release[1] = v;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    cudaStream_t s = nullptr;
+    if (cudaSetDevice(L.ordinal) != cudaSuccess || cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess)
+      continue;
+    for (uint32_t j = 0; j < h->n_total; ++j)
+      cudaMemcpyAsync(reinterpret_cast<void*>(ce_a2a_line(h, li, L.grank, j, 0)), host->release, 16,
+                      cudaMemcpyHostToDevice, s);
+    const double deadline = now_ms() + h->cfg.timeout_ms;
+    while (cudaStreamQuery(s) == cudaErrorNotReady && now_ms() < deadline) {
+    }
+    cudaStreamDestroy(s);
+  }
+}
+
+// Rep `rep` of size k of cdprobe_ce_alltoall on every local rank, all queued before the host releases the rep's
+// ticket (DESIGN §5p): on each rank's stream the ticket wait, the opening barrier, event A, the joins of its copy
+// streams (and on a push the landed values of every sender), event B; on each copy stream the wait for A, the copy
+// between its two events, and on a push the landed value.  The ticket is released even when queuing fails.  Then the
+// host waits, polling, until every B has completed, reads the times of a timed rep into rank_ns[li][k] and
+// copy_ns[li][i][k], and only then queues the checks of every block each local rank owns, on its stream, so no kernel
+// launch waits behind a stream that waits on the host.
+static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, uint32_t rep, const CeA2aFault& f,
+                      float (*rank_ns)[kBwMaxSizes][kMaxTimedReps],
+                      float (*copy_ns)[kMaxRanks][kBwMaxSizes][kMaxTimedReps]) {
+  CeA2aHost* const host = h->cea_host;
+  const Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  const bool push = op == CDPROBE_OP_WRITE;
+  const uint64_t ticket = ++host->issued, v = ce_a2a_value(h->cea_calls, k, rep, lad.reps), bytes = lad.size[k];
+  const auto wait_value = [&](cudaStream_t s, CUdeviceptr a, uint64_t want) {
+    return h->drv.StreamWaitValue64(s, a, want, CU_STREAM_WAIT_VALUE_GEQ);
+  };
+  cudaError_t e = cudaSuccess;
+  CUresult cu = CUDA_SUCCESS;
+  const char* what = "";
+  bool held = false;
+  const auto ok = [&] { return e == cudaSuccess && cu == CUDA_SUCCESS; };
+  for (uint32_t li = 0; li < h->n_local && ok(); ++li) {
+    LocalRank& L = h->lr[li];
+    const uint32_t g = L.grank;
+    const cudaStream_t s = L.stream;
+    e = cudaSetDevice(L.ordinal);
+    what = "cuStreamWaitValue64";
+    if (ok()) cu = wait_value(s, reinterpret_cast<CUdeviceptr>(&host->ticket), ticket);
+    what = "cuStreamWriteValue64";
+    for (uint32_t p = 0; p < n && ok(); ++p)
+      if (p != g) cu = h->drv.StreamWriteValue64(s, ce_a2a_line(h, li, p, g, 0), v, CU_STREAM_WRITE_VALUE_DEFAULT);
+    what = "cuStreamWaitValue64";
+    for (uint32_t p = 0; p < n && ok(); ++p)
+      if (p != g) cu = wait_value(s, ce_a2a_line(h, li, g, p, 0), v);
+    if (ok()) e = cudaEventRecord(L.cea_ev[0], s);
+    uint32_t target[kMaxRanks];
+    const uint32_t cells = ce_a2a_targets(h, li, target);
+    for (uint32_t i = 0; i < cells && ok(); ++i) {
+      const uint32_t j = target[i];
+      const MemcpyCell c = memcpy_cell(pl, op, g, j);
+      const bool armed = rep == 1 && k == f.k && g == f.issuer && j == f.target;
+      const cudaStream_t cs = L.cea_stream[i];
+      cudaEvent_t* const ev = L.cea_copy_ev[i];
+      uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
+      e = cudaStreamWaitEvent(cs, L.cea_ev[0], 0);
+      what = "cuStreamWaitValue64";
+      if (ok() && armed && f.mode == 2) {
+        cu = wait_value(cs, reinterpret_cast<CUdeviceptr>(&host->hold), ticket);
+        held = true;
+      }
+      if (ok()) e = cudaEventRecord(ev[0], cs);
+      if (ok() && !(armed && f.mode == 1))
+        e = cudaMemcpyAsync(dst, reinterpret_cast<const void*>(h->mem.va[li][c.src_rank] + c.src_off), bytes,
+                            cudaMemcpyDeviceToDevice, cs);
+      if (ok()) e = cudaEventRecord(ev[1], cs);
+      if (ok() && armed && f.mode == 0) {
+        host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + f.arg) ^ 1ull;
+        e = cudaMemcpyAsync(dst + 8 * f.arg, &host->flip[li], 8, cudaMemcpyHostToDevice, cs);
+      }
+      what = "cuStreamWriteValue64";
+      if (ok() && push) cu = h->drv.StreamWriteValue64(cs, ce_a2a_line(h, li, j, g, 1), v, CU_STREAM_WRITE_VALUE_DEFAULT);
+      if (ok()) e = cudaEventRecord(ev[2], cs);
+      if (ok()) e = cudaStreamWaitEvent(s, ev[2], 0);
+    }
+    what = "cuStreamWaitValue64";
+    for (uint32_t p = 0; p < n && push && ok(); ++p)
+      if (p != g || pl.diag) cu = wait_value(s, ce_a2a_line(h, li, g, p, 1), v);
+    if (ok()) e = cudaEventRecord(L.cea_ev[1], s);
+  }
+  __atomic_store_n(&host->ticket, ticket, __ATOMIC_RELEASE);
+  if (held) usleep((useconds_t)f.arg);
+  __atomic_store_n(&host->hold, ticket, __ATOMIC_RELEASE);
+  if (!ok()) {
+    ce_a2a_unblock(h, v);
+    if (e != cudaSuccess) return fail_sticky(h, "cdprobe_ce_alltoall: queue a rep", e);
+    h->sticky = true;
+    set_err(std::string("cdprobe_ce_alltoall: ") + what + ": " + h->drv.error_name(cu));
+    return CDPROBE_ERR_CUDA;
+  }
+  const double deadline = now_ms() + h->cfg.timeout_ms;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    LocalRank& L = h->lr[li];
+    CDP_RT(cudaSetDevice(L.ordinal));
+    while ((e = cudaEventQuery(L.cea_ev[1])) != cudaSuccess) {
+      if (e != cudaErrorNotReady) return fail_sticky(h, "cdprobe_ce_alltoall: wait for a rep", e);
+      if (now_ms() > deadline) {
+        ce_a2a_unblock(h, v);
+        h->sticky = true;
+        set_err("cdprobe_ce_alltoall: a rep did not complete within timeout_ms of its release");
+        return CDPROBE_ERR_TIMEOUT;
+      }
+    }
+  }
+  for (uint32_t li = 0; li < h->n_local && rep > 0; ++li) {
+    LocalRank& L = h->lr[li];
+    uint32_t target[kMaxRanks];
+    const uint32_t cells = ce_a2a_targets(h, li, target);
+    float ms = 0.f;
+    CDP_RT(cudaSetDevice(L.ordinal));
+    if ((e = cudaEventElapsedTime(&ms, L.cea_ev[0], L.cea_ev[1])) != cudaSuccess)
+      return fail_sticky(h, "cdprobe_ce_alltoall: event times", e);
+    rank_ns[li][k][rep - 1] = ms * 1e6f;
+    for (uint32_t i = 0; i < cells; ++i) {
+      if ((e = cudaEventElapsedTime(&ms, L.cea_copy_ev[i][0], L.cea_copy_ev[i][1])) != cudaSuccess)
+        return fail_sticky(h, "cdprobe_ce_alltoall: event times", e);
+      copy_ns[li][i][k][rep - 1] = ms * 1e6f;
+    }
+  }
+  // every block in rank g's area holds the slice g reads from its sender j, whichever side copied it
+  for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li) {
+    const uint32_t g = h->lr[li].grank;
+    e = cudaSetDevice(h->lr[li].ordinal);
+    for (uint32_t j = 0; j < n && e == cudaSuccess; ++j)
+      if (j != g || pl.diag) e = check_block(h, li, memcpy_cell(pl, CDPROBE_OP_READ, g, j), bytes, &host->rep[li][j][rep]);
+  }
+  return e != cudaSuccess ? fail_sticky(h, "cdprobe_ce_alltoall: queue the checks", e) : CDPROBE_OK;
 }
 
 }  // namespace cdp
@@ -1737,6 +1965,146 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
     return CDPROBE_OK;
   };
   if (const int rc = cdp::walk_rounds(h, runs, round); rc != CDPROBE_OK) return rc;
+  out->ms = cdp::now_ms() - lad.t_begin;
+  return CDPROBE_OK;
+}
+
+int cdprobe_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_alltoall_t* out) {
+  cdp::Ladder lad;
+  const int opened = cdp::open_ladder(h, out, reps, cdp::kCeA2aDefaultReps, &lad);
+  if (out != nullptr) out->op = op;
+  if (opened != CDPROBE_OK) return opened;
+  const cdp::Plan& pl = h->plan;
+  const uint32_t n = h->n_total;
+  const bool push = op == CDPROBE_OP_WRITE;
+  // 1. the arguments, the armed fault, the probe mapping rows and whether every process can run it; in a multi-process
+  //    domain all are shared, so every process refuses, skips or runs together
+  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad.bad.empty())
+    lad.bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
+  cdp::CeA2aFault f;
+  if (h->cea_fault != 0 && lad.bad.empty()) {
+    const uint64_t v = h->cea_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
+    const cdp::FaultSpot at = cdp::fault_spot(v, lad);
+    if (mode > 2 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || !at.size_ok ||
+        (mode < 2 && !at.word_ok) || (mode == 2 && 2 * at.word >= 1000ull * h->cfg.timeout_ms))
+      lad.bad = "the armed copy-engine all-to-all fault names no cell, size, word or delay of this call, or has a mode "
+                "above 2";
+    else
+      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, at.k, (uint32_t)mode, at.word};
+  }
+  const std::string refusal = lad.bad.empty() ? cdp::ce_a2a_refusal(h) : std::string();
+  bool refused = !refusal.empty();
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  // agree() ors the refusal flag (its `zero`) over every process
+  if (const int rc = cdp::agree(h, "cdprobe_ce_alltoall", lad.bad, h->cea_calls + 1, {lad.reps, op, 0u}, st, nullptr,
+                                &refused);
+      rc != CDPROBE_OK)
+    return rc;
+  if (refused) {
+    cdp::set_err(!refusal.empty() ? refusal
+                                  : std::string("cdprobe_ce_alltoall: another process cannot run it (no stream memory "
+                                                "operations, or more streams than CUDA_DEVICE_MAX_CONNECTIONS)"));
+    return CDPROBE_ERR_UNSUPPORTED;
+  }
+  // 2. the exchange area (cdprobe_alltoall's and cdprobe_memcpy's), built once, by every process in the same call
+  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++h->cea_calls;
+  out->area_bytes = h->area.bytes;
+  cdp::put_ladder(h, lad, out);
+
+  // 3. every rank signals every other and every cell copies in every rep: when some probe or exchange-area mapping of
+  //    the domain is down, nothing runs, in any process (a stream barrier cannot skip a peer)
+  for (uint32_t s = 0; s < n; ++s)
+    for (uint32_t d = 0; d < n; ++d)
+      if (st[s][d] == 0) st[s][d] = h->area.status[s][d];
+  if (const int32_t* down = cdp::first_down(st); down != nullptr) {
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      const uint32_t g = h->lr[li].grank;
+      out->status[g] = *down;
+      for (uint32_t j = 0; j < n; ++j) {
+        if (j == g && !pl.diag) continue;
+        out->cell_status[g * CDPROBE_MAX_GPUS + j] = *down;
+        out->cell_status[j * CDPROBE_MAX_GPUS + g] = *down;
+      }
+    }
+    out->ms = cdp::now_ms() - lad.t_begin;
+    return CDPROBE_OK;
+  }
+
+  // 4. the host block, the copy streams and the events; scratch for the checks and one block's granule table, grown on
+  //    every local rank before anything is queued; the (S, X) each size of each block a local rank owns must have,
+  //    from the pattern definition: block j of rank g's area holds the slice g reads from j, on a pull and on a push
+  if (const int rc = cdp::ce_a2a_setup(h); rc != CDPROBE_OK) return rc;
+  bool owns[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  for (uint32_t li = 0; li < h->n_local; ++li)
+    for (uint32_t j = 0; j < n; ++j) owns[li][j] = j != h->lr[li].grank || pl.diag;
+  std::unique_ptr<cdp::CellSums[]> want;
+  if (const int rc = cdp::cell_sums(h, owns, CDPROBE_OP_READ, cdp::MemcpyScratch(pl.bpp).table_off, lad,
+                                    "cdprobe_ce_alltoall: granule checksums", &want);
+      rc != CDPROBE_OK)
+    return rc;
+
+  // 5. the sizes, each behind a domain barrier; within a size, one rep at a time, every rank and cell at once, each rep
+  //    behind the checks of the one before.  After a size, every local stream is drained and the checks' records read:
+  //    per rep, the diagnosis's bad words and the (S, X) read against the pattern's
+  auto rank_ns = std::make_unique<float[][cdp::kBwMaxSizes][cdp::kMaxTimedReps]>(cdp::kMaxRanks);
+  auto copy_ns = std::make_unique<float[][cdp::kMaxRanks][cdp::kBwMaxSizes][cdp::kMaxTimedReps]>(cdp::kMaxRanks);
+  bool aborted[cdp::kMaxRanks][cdp::kMaxRanks] = {};
+  for (uint32_t k = 0; k < lad.n_sizes; ++k) {
+    if (const int rc = cdp::domain_barrier(h); rc != CDPROBE_OK) return rc;
+    for (uint32_t rep = 0; rep <= lad.reps; ++rep)
+      if (const int rc = cdp::ce_a2a_rep(h, op, lad, k, rep, f, rank_ns.get(), copy_ns.get()); rc != CDPROBE_OK)
+        return rc;
+    for (uint32_t li = 0; li < h->n_local; ++li) {
+      const cdp::LocalRank& L = h->lr[li];
+      const uint32_t g = L.grank;
+      CDP_RT(cudaSetDevice(L.ordinal));
+      if (const cudaError_t e = cudaStreamSynchronize(L.stream); e != cudaSuccess)
+        return cdp::fail_sticky(h, "cdprobe_ce_alltoall: check a size", e);
+      for (uint32_t j = 0; j < n; ++j) {
+        if (!owns[li][j]) continue;
+        const uint32_t idx = push ? j * CDPROBE_MAX_GPUS + g : g * CDPROBE_MAX_GPUS + j;
+        const uint64_t(*w)[2] = want[li][j];
+        uint64_t first = UINT64_MAX;
+        for (uint32_t rep = 0; rep <= lad.reps; ++rep) {
+          const cdp::MemcpyRepOut& got = h->cea_host->rep[li][j][rep];
+          aborted[li][j] |= got.abort_flag != 0;
+          out->bad_words[idx][k] += got.diag[0];
+          if (got.diag[0] != 0) first = std::min(first, (uint64_t)~got.diag[2]);
+          if (got.diag[0] != 0 || got.acc.sum != w[k][0] || got.acc.xr != w[k][1]) out->bad_sizes[idx] |= 1u << k;
+          if (rep == lad.reps) {
+            out->sum[idx][k] = got.acc.sum;
+            out->xr[idx][k] = got.acc.xr;
+          }
+        }
+        out->first_bad[idx][k] = first;
+      }
+    }
+  }
+
+  // 6. per rank, the times of its reps (rate: blocks x size / ns); per cell it issues, the median copy time; per block
+  //    it owns, the verdict of every size's checks, unless an (S, X) read passed its deadline
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    const uint32_t g = h->lr[li].grank;
+    uint32_t target[cdp::kMaxRanks];
+    const uint32_t cells = cdp::ce_a2a_targets(h, li, target);
+    for (uint32_t i = 0; i < cells; ++i) {
+      for (uint32_t k = 0; k < lad.n_sizes; ++k) {
+        float* const t = copy_ns[li][i][k];
+        std::sort(t, t + lad.reps);
+        out->copy_ns_median[g * CDPROBE_MAX_GPUS + target[i]][k] = t[lad.reps / 2];
+      }
+    }
+    out->measured[g] = 1;
+    out->blocks[g] = cells;
+    cdp::ladder_times(rank_ns[li], lad.size, lad.n_sizes, lad.reps, (double)cells, g, out);
+    for (uint32_t j = 0; j < n; ++j) {
+      if (!owns[li][j]) continue;
+      const uint32_t idx = push ? j * CDPROBE_MAX_GPUS + g : g * CDPROBE_MAX_GPUS + j;
+      out->cell_measured[idx] = 1;
+      out->cell_status[idx] = aborted[li][j] ? CDPROBE_ERR_TIMEOUT : out->bad_sizes[idx] ? CDPROBE_ERR_INTEGRITY : 0;
+    }
+  }
   out->ms = cdp::now_ms() - lad.t_begin;
   return CDPROBE_OK;
 }

@@ -74,6 +74,21 @@ MemcpyCell memcpy_cell(const Plan& pl, uint32_t op, uint32_t g, uint32_t j) {
   return c;
 }
 
+uint32_t ce_a2a_queues(uint32_t n, bool diag, uint32_t n_local, const int* ordinal, int* worst) {
+  const uint32_t per_rank = 1u + (n - 1u) + (diag ? 1u : 0u);
+  uint32_t most = 0;
+  *worst = n_local ? ordinal[0] : -1;
+  for (uint32_t li = 0; li < n_local; ++li) {
+    uint32_t here = 0;
+    for (uint32_t lj = 0; lj < n_local; ++lj) here += ordinal[lj] == ordinal[li] ? per_rank : 0u;
+    if (here > most || (here == most && ordinal[li] < *worst)) {
+      most = here;
+      *worst = ordinal[li];
+    }
+  }
+  return most;
+}
+
 }  // namespace cdp
 
 extern "C" int cdprobe_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, cdprobe_plan_t* out) {

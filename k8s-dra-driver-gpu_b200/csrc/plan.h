@@ -51,6 +51,12 @@ struct MemcpyCell {
   uint64_t dst_off;     // the block's byte offset in that area
 };
 MemcpyCell memcpy_cell(const Plan& pl, uint32_t op, uint32_t g, uint32_t j);
+// The hardware queues cdprobe_ce_alltoall needs on the most loaded device of a process whose n_local ranks run on
+// ordinal[0 .. n_local) of an n-rank domain (diag: with a loop-back slice): each local rank holds its own stream and
+// one copy stream per cell it issues, n - 1 peers and the diagonal.  *worst gets that device's ordinal (the lowest on
+// a tie).  A stream wait blocks every stream that shares its queue, so the call needs at most
+// CUDA_DEVICE_MAX_CONNECTIONS of them per device.
+uint32_t ce_a2a_queues(uint32_t n, bool diag, uint32_t n_local, const int* ordinal, int* worst);
 // Returns CDPROBE_OK or CDPROBE_ERR_ARG.
 int make_plan(uint32_t n, uint64_t bytes, uint32_t mode, uint32_t flags, Plan* out);
 

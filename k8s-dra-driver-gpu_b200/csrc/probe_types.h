@@ -597,6 +597,19 @@ constexpr uint64_t kNvlsOff = kPushOff + kMaxRanks * sizeof(FlagLine);  // 80 Ki
 static_assert(kNvlsOff % 128 == 0 && kNvlsOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
               "the multicast all-reduce lines sit after the push all-reduce lines inside the Ctrl granule");
 
+// ---- the copy-engine all-to-all (cdprobe_ce_alltoall, DESIGN §5p) ----------------------------------------------------
+// One 128-byte line per sender after the NVLS lines, in the Ctrl granule, written only by stream memory operations:
+// word 0 holds the sender's opening value, word 1 its landed value (a push's).  Open zeroes them; nothing else does.
+constexpr uint64_t kCeA2aOff = kNvlsOff + kMaxRanks * sizeof(FlagLine);  // 82 KiB
+static_assert(kCeA2aOff % 128 == 0 && kCeA2aOff + kMaxRanks * sizeof(FlagLine) <= kCtrlBytes,
+              "the copy-engine all-to-all lines sit after the multicast all-reduce lines inside the Ctrl granule");
+static_assert(kBwMaxSizes * (64 + 1) < (1u << kArBarrierBits), "copy-engine all-to-all reps per call fit the low bits");
+// The value rep `rep` (0: the warm-up) of size k of call call_seq opens and lands with: (call_seq << 16) | (b + 1),
+// b = k x (reps + 1) + rep.  Values rise along (call, size, rep), so a GEQ wait is never satisfied by an earlier one.
+inline uint64_t ce_a2a_value(uint64_t call_seq, uint32_t k, uint32_t rep, uint32_t reps) {
+  return (call_seq << kArBarrierBits) | ((uint64_t)k * (reps + 1) + rep + 1);
+}
+
 // The flag lines a domain barrier exchanges (datapath.cuh, grid_barrier): its leader stores (call_seq << 16) |
 // (b + 1) into self (unless null) and into every non-null sig_out[j], then waits until every non-null sig_in[j] holds at
 // least that.  sig_in[j] is where rank j's value arrives: this rank's line j when j pushes it, or line j of rank j's own

@@ -57,6 +57,10 @@ cudaError_t Driver::load_stream_wait(std::string* err) {
   return StreamWaitValue64 != nullptr ? cudaSuccess : resolve("cuStreamWaitValue64", &StreamWaitValue64, err);
 }
 
+cudaError_t Driver::load_stream_write(std::string* err) {
+  return StreamWriteValue64 != nullptr ? cudaSuccess : resolve("cuStreamWriteValue64", &StreamWriteValue64, err);
+}
+
 std::string Driver::error_name(CUresult r) const {
   const char* s = nullptr;
   if (GetErrorName && GetErrorName(r, &s) == CUDA_SUCCESS && s) return s;

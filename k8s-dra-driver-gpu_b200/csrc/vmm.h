@@ -39,6 +39,8 @@ struct Driver {
   int multicast = -1;  // load_multicast's verdict, -1: not asked yet
   // The stream wait of cdprobe_memcpy: resolved by load_stream_wait on its first call, apart from load's set.
   CUresult (*StreamWaitValue64)(CUstream, CUdeviceptr, cuuint64_t, unsigned int) = nullptr;
+  // The stream write of cdprobe_ce_alltoall: resolved by load_stream_write on its first call, apart from load's set.
+  CUresult (*StreamWriteValue64)(CUstream, CUdeviceptr, cuuint64_t, unsigned int) = nullptr;
 
   // Returns cudaSuccess or the runtime error that prevented loading.
   cudaError_t load(std::string* err);
@@ -46,6 +48,8 @@ struct Driver {
   bool load_multicast();
   // Resolves StreamWaitValue64 once; returns cudaSuccess or why it is missing.
   cudaError_t load_stream_wait(std::string* err);
+  // Resolves StreamWriteValue64 once; returns cudaSuccess or why it is missing.
+  cudaError_t load_stream_write(std::string* err);
   std::string error_name(CUresult r) const;
 };
 

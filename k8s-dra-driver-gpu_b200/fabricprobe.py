@@ -513,6 +513,74 @@ class Memcpy:
 
 
 @dataclasses.dataclass
+class CeAllToAll:
+    """What cdprobe_ce_alltoall measured.  Per rank r: `blocks` it copies per rep (the cells it issues), ns per rep
+    (min, median and max over the timed reps, from its release until its own copies are complete and every block
+    addressed to it has landed) of each size of the ladder `sizes`, and the summary of the medians: t0_ns (the smallest
+    size), peak_gbps (blocks x size / ns) and half_bytes.  Per cell [issuer][target]: `copy_ns_median`, the median of
+    its copy stream's own timing per size, filled by the issuer's process; and, as the block's owner checked it (the
+    issuer on a pull, the target on a push), `cell_status`, the sizes that failed a check (`bad_sizes`, bit k for
+    sizes[k]), `bad_words` and `first_bad` (the byte offset of the lowest bad word, or U64_MAX) per size, and the (S, X)
+    of the block in the last timed rep.  Per-size values are lists over `sizes`.  A rank that did not run is None
+    everywhere but `measured` and `status`; a cell whose owner did not check it is None in the check fields, and one
+    whose issuer is not local has no `copy_ns_median`."""
+    n: int
+    row_mask: int
+    reps: int
+    op: int
+    call_seq: int
+    area_bytes: int
+    sizes: List[int]
+    measured: List[bool]
+    status: List[int]     # 0 ok; else the status of the domain's first down mapping
+    blocks: List[Optional[int]]
+    t0_ns: List[Optional[float]]
+    peak_gbps: List[Optional[float]]
+    half_bytes: List[Optional[int]]
+    ns_min: List[Optional[List[float]]]
+    ns_median: List[Optional[List[float]]]
+    ns_max: List[Optional[List[float]]]
+    cell_measured: List[List[bool]]
+    cell_status: List[List[int]]  # 0 ok; ERR_INTEGRITY; ERR_TIMEOUT; else the status of the first down mapping
+    bad_sizes: List[List[Optional[int]]]
+    copy_ns_median: List[List[Optional[List[float]]]]
+    bad_words: List[List[Optional[List[int]]]]
+    first_bad: List[List[Optional[List[int]]]]
+    sum: List[List[Optional[List[int]]]]
+    xr: List[List[Optional[List[int]]]]
+    ms: float
+    raw: abi.CeAllToAllT = dataclasses.field(repr=False, default=None)
+
+    @staticmethod
+    def from_c(t: abi.CeAllToAllT) -> "CeAllToAll":
+        k, n, M = t.n_sizes, t.n, abi.MAX_GPUS
+
+        def row(a, per_size=False):
+            return [(list(a[r])[:k] if per_size else a[r]) if t.measured[r] else None for r in range(n)]
+
+        def checked(c):
+            return t.cell_measured[c] and t.cell_status[c] != abi.ERR_TIMEOUT
+
+        def cells(a, per_size=True):
+            return [[(list(a[s * M + d])[:k] if per_size else a[s * M + d]) if checked(s * M + d) else None
+                     for d in range(n)] for s in range(n)]
+
+        # rank s issues a cell to every peer, and to itself only with a loop-back slice (then it copies n blocks)
+        copy = [[list(t.copy_ns_median[s * M + d])[:k] if t.measured[s] and (s != d or t.blocks[s] == n) else None
+                 for d in range(n)] for s in range(n)]
+        return CeAllToAll(n=n, row_mask=t.row_mask, reps=t.reps, op=t.op, call_seq=t.call_seq,
+                          area_bytes=t.area_bytes, sizes=list(t.size)[:k],
+                          measured=[bool(t.measured[r]) for r in range(n)], status=list(t.status)[:n],
+                          blocks=row(t.blocks), t0_ns=row(t.t0_ns), peak_gbps=row(t.peak_gbps),
+                          half_bytes=row(t.half_bytes), ns_min=row(t.ns_min, True), ns_median=row(t.ns_median, True),
+                          ns_max=row(t.ns_max, True),
+                          cell_measured=[[bool(t.cell_measured[s * M + d]) for d in range(n)] for s in range(n)],
+                          cell_status=[[t.cell_status[s * M + d] for d in range(n)] for s in range(n)],
+                          bad_sizes=cells(t.bad_sizes, False), copy_ns_median=copy, bad_words=cells(t.bad_words),
+                          first_bad=cells(t.first_bad), sum=cells(t.sum), xr=cells(t.xr), ms=t.ms, raw=t)
+
+
+@dataclasses.dataclass
 class Links:
     """What cdprobe_links reported: per distinct local device, the per-link NVLink counter deltas NVML gave over the
     last run taken with abi.OPT_LINK_COUNTERS on, next to the payload that run's plan moved between devices.  Each
@@ -822,6 +890,22 @@ class Probe:
         """The bare ABI call: (return code, abi.MemcpyT as the library left it)."""
         t = abi.MemcpyT()
         rc = self._lib.cdprobe_memcpy(self._h, op, reps, C.byref(t))
+        return rc, t
+
+    def CeAllToAll(self, op: int, reps: int = 0) -> CeAllToAll:
+        """Go: (*Probe).CeAllToAll.  Copy-engine all-to-all: in every rep every cell of Memcpy copies its block at
+        once, each on a copy stream of its own, pulled (op abi.OP_READ) or pushed (abi.OP_WRITE), with the ranks
+        signalling each other by stream memory operations, at each size of the bwcurve ladder; the owner of every block
+        checks every word (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first and disturbs
+        none."""
+        rc, t = self.ce_alltoall_raw(op, reps)
+        _check(self._lib, rc, "cdprobe_ce_alltoall")
+        return CeAllToAll.from_c(t)
+
+    def ce_alltoall_raw(self, op: int, reps: int):
+        """The bare ABI call: (return code, abi.CeAllToAllT as the library left it)."""
+        t = abi.CeAllToAllT()
+        rc = self._lib.cdprobe_ce_alltoall(self._h, op, reps, C.byref(t))
         return rc, t
 
     def Links(self) -> Links:
