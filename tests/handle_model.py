@@ -4,14 +4,15 @@ A daemon keeps one handle for days and interleaves runs, option changes, remaps,
 measurements on it.  `HandleModel` follows the same calls and says, from the pattern spec alone, what each one must
 return: the expected values come from the CPU oracle (oracle/oracle.py), tests/word_ref.py, tests/latency_ref.py,
 tests/bwcurve_ref.py, tests/allreduce_ref.py, the all-reduce protocol references (allreduce_twoshot_ref,
-allreduce_ll_ref, allreduce_ring_ref, allreduce_push_ref), tests/alltoall_ref.py and tests/memcpy_ref.py, never from
-the library.  It tracks:
+allreduce_ll_ref, allreduce_ring_ref, allreduce_push_ref), tests/alltoall_ref.py, tests/memcpy_ref.py and
+tests/ce_alltoall_ref.py, never from the library.  It tracks:
 
 - the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, the five all-reduces (one-shot, two-shot, LL,
-  ring, push), alltoall and memcpy (a refused call advances none);
+  ring, push), alltoall, memcpy and the copy-engine all-to-all (a refused call advances none);
+- each process's hardware queues per device, against which the copy-engine all-to-all is refused;
 - the armed fault of each of those ladder measurements in each process's handle; which pairs were unmapped when the
-  exchange area (shared by the all-to-all and memcpy, built by whichever is called first) was built, and the same for
-  the two-shot's gather area and the LL, ring and push areas;
+  exchange area (shared by the all-to-all, memcpy and the copy-engine all-to-all, built by whichever is called first)
+  was built, and the same for the two-shot's gather area and the LL, ring and push areas;
 - the options in force: path, CTAs per rank, verify CTAs, the schedule flags, warm-up mode;
 - the phase table each rank must walk (cdprobe_schedule with the current options, with the jobs of an unmapped pair
   idled as the library's schedule does);
@@ -30,6 +31,8 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import os
+import re
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -41,6 +44,7 @@ import allreduce_ring_ref
 import allreduce_twoshot_ref
 import alltoall_ref
 import bwcurve_ref
+import ce_alltoall_ref
 import latency_ref
 import memcpy_ref
 import word_ref
@@ -48,6 +52,8 @@ import word_ref
 M64 = (1 << 64) - 1
 SEED = 0xCD5EED0000000001
 OP_READ, OP_WRITE = 1, 2
+ERR_ARG = -2
+ERR_UNSUPPORTED = -8
 ERR_STATE = -9
 ERR_INTEGRITY = -10
 FLAG_OVERLAP_VERIFY = 0x20
@@ -59,6 +65,15 @@ KIND_NAMES = {0: "-", 1: "read", 2: "write", 3: "verify", 4: "warm"}
 JOB_NONE, JOB_READ, JOB_WRITE, JOB_VERIFY, JOB_WARM = 0, 1, 2, 3, 4
 # The checksum pass at open is the handle's first launch and takes sequence number 1, so the first run is 2.
 FIRST_RUN_SEQ = 2
+CE_A2A_DEFAULT_REPS = 8
+
+
+def max_connections(env) -> int:
+    """The hardware queues per device cdprobe_open reads from CUDA_DEVICE_MAX_CONNECTIONS in `env`: its leading
+    integer clamped to at most 32 when positive, else the CUDA runtime's default of 8."""
+    m = re.match(r"\s*([+-]?\d+)", env.get("CUDA_DEVICE_MAX_CONNECTIONS") or "")
+    v = int(m.group(1)) if m else 0
+    return min(v, 32) if v > 0 else ce_alltoall_ref.DEFAULT_QUEUES
 
 
 def rotl64(x: int, r: int) -> int:
@@ -138,8 +153,18 @@ class HandleModel:
         self.push_fault: Dict[int, int] = {}
         self.a2a_fault: Dict[int, int] = {}
         self.mc_fault: Dict[int, int] = {}
-        # the pairs unmapped when the first all-to-all or memcpy built the exchange area they share (None: not built
-        # yet); the area is mapped only where the probe mapping was up then, and remaps do not map it later
+        # the copy-engine all-to-all: its calls, its armed fault (CDPROBE_OPT_CE_ALLTOALL_FAULT) per process, each
+        # process's hardware queues per device (CUDA_DEVICE_MAX_CONNECTIONS as read by cdprobe_open; by default this
+        # process's, for every process) and each global rank's device ordinal (absent: 0), which the caller sets from
+        # the ordinals the handle was opened with
+        self.cea_calls = 0
+        self.cea_fault: Dict[int, int] = {}
+        limit = max_connections(os.environ)
+        self.max_connections: Dict[int, int] = {p: limit for p in range(n // len(self.local))}
+        self.ordinal: Dict[int, int] = {}
+        # the pairs unmapped when the first all-to-all, memcpy or copy-engine all-to-all built the exchange area they
+        # share (None: not built yet); the area is mapped only where the probe mapping was up then, and remaps do not
+        # map it later
         self.area_down: Optional[frozenset] = None
         # the same for the gather, LL, ring and push areas, each built by its own all-reduce's first call
         self.ar_area_down: Dict[str, Optional[frozenset]] = {"ts": None, "ll": None, "ring": None, "push": None}
@@ -567,9 +592,50 @@ class HandleModel:
         return self._allreduce("push", reps, sizes, decode, effect)
 
     def build_area(self) -> None:
-        """The exchange area, built by the first all-to-all or memcpy call that is not refused."""
+        """The exchange area, built by the first all-to-all, memcpy or copy-engine all-to-all call that is not
+        refused."""
         if self.area_down is None:
             self.area_down = frozenset(self.unmapped)
+
+    def _block(self, op: int, g: int, j: int, sizes: List[int], reps: int, fault=None) -> dict:
+        """What the checks of cell (issuer g, target j)'s block report when the block is copied and checked in every
+        rep, as cdprobe_memcpy and cdprobe_ce_alltoall both do: {"bad_sizes", "sx", "bad_words", "first_bad",
+        "status"}.  The block holds its source slice (memcpy_ref.cell) as it is at rest after every rep, warm-up
+        included, and is checked and cleared then: a corrupted word is one bad word per rep.  `fault` (k, word, mode)
+        acts in timed rep 1 of size k: mode 0 overwrites the landed word with its pattern value xored with 1, mode 1
+        copies nothing, so the cleared block reads as 0s.  The (S, X) is the last timed rep's."""
+        c = memcpy_ref.cell(self.n, self.bpp, self.mode, op, g, j)
+        src, first = c["src_rank"], c["first_word"]
+        corr = {k - first: m for k, m in self.corruptions_of(src).items() if first <= k < first + self.W}
+        cell = dict(bad_sizes=0, sx=[], bad_words=[], first_bad=[])
+        fk, fw, mode = fault if fault is not None else (None, None, None)
+        for k, s in enumerate(sizes):
+            nw = s // 8
+            clean_sx = self.clean_checksum(src, first, nw)
+            rest = {}  # {destination word: (pattern, landed)} of the corrupted words of the prefix
+            for w, m in corr.items():
+                if w < nw:
+                    p = src_word(self.seed, src, first + w)
+                    rest[w] = (p, p ^ m)
+            bad = sorted(rest)
+            if fk == k and mode == 1:  # nothing landed: every word the pattern does not make 0 is bad
+                pattern = word_ref.src_words(self.seed, src, first, nw)
+                bad1, sx1 = [int(w) for w in np.flatnonzero(pattern != 0)], (0, 0)
+            else:
+                rep1 = dict(rest)
+                if fk == k:
+                    p = src_word(self.seed, src, first + fw)
+                    rep1[fw] = (p, p ^ 1)
+                bad1, sx1 = sorted(rep1), refold(clean_sx, rep1, nw)
+            sx_rest = refold(clean_sx, rest, nw)
+            cell["sx"].append(sx1 if reps == 1 else sx_rest)
+            cell["bad_words"].append(reps * len(bad) + len(bad1))
+            first_bad = min(bad[:1] + bad1[:1], default=None)
+            cell["first_bad"].append(word_ref.U64_MAX if first_bad is None else 8 * first_bad)
+            if bad or bad1 or sx1 != clean_sx or sx_rest != clean_sx:
+                cell["bad_sizes"] |= 1 << k
+        cell["status"] = ERR_INTEGRITY if cell["bad_sizes"] else 0
+        return cell
 
     def memcpy(self, op: int, reps: int) -> Optional[dict]:
         """What cdprobe_memcpy with op and `reps` timed reps must return, or None when the op is neither OP_READ nor
@@ -604,38 +670,7 @@ class HandleModel:
                 if (g, j) in self.unmapped or (g, j) in (self.area_down or ()):
                     cells[(g, j)] = dict(measured=False, status=ERR_STATE)
                     continue
-                c = memcpy_ref.cell(n, self.bpp, self.mode, op, g, j)
-                src, first = c["src_rank"], c["first_word"]
-                corr = {k - first: m for k, m in self.corruptions_of(src).items() if first <= k < first + self.W}
-                cell = dict(measured=True, bad_sizes=0, sx=[], bad_words=[], first_bad=[])
-                for k, s in enumerate(sizes):
-                    nw = s // 8
-                    clean_sx = self.clean_checksum(src, first, nw)
-                    rest = {}  # {destination word: (pattern, landed)} of the corrupted words of the prefix
-                    for w, m in corr.items():
-                        if w < nw:
-                            p = src_word(self.seed, src, first + w)
-                            rest[w] = (p, p ^ m)
-                    bad = sorted(rest)
-                    fk, fw, mode = faults.get((g, j), (None, None, None))
-                    if fk == k and mode == 1:  # nothing landed: every word the pattern does not make 0 is bad
-                        pattern = word_ref.src_words(self.seed, src, first, nw)
-                        bad1, sx1 = [int(w) for w in np.flatnonzero(pattern != 0)], (0, 0)
-                    else:
-                        rep1 = dict(rest)
-                        if fk == k:
-                            p = src_word(self.seed, src, first + fw)
-                            rep1[fw] = (p, p ^ 1)
-                        bad1, sx1 = sorted(rep1), refold(clean_sx, rep1, nw)
-                    sx_rest = refold(clean_sx, rest, nw)
-                    cell["sx"].append(sx1 if reps == 1 else sx_rest)
-                    cell["bad_words"].append(reps * len(bad) + len(bad1))
-                    first_bad = min(bad[:1] + bad1[:1], default=None)
-                    cell["first_bad"].append(word_ref.U64_MAX if first_bad is None else 8 * first_bad)
-                    if bad or bad1 or sx1 != clean_sx or sx_rest != clean_sx:
-                        cell["bad_sizes"] |= 1 << k
-                cell["status"] = ERR_INTEGRITY if cell["bad_sizes"] else 0
-                cells[(g, j)] = cell
+                cells[(g, j)] = dict(measured=True, **self._block(op, g, j, sizes, reps, faults.get((g, j))))
         return dict(call_seq=self.mc_calls, sizes=sizes, cells=cells)
 
     def a2a_runs(self, s: int, d: int) -> bool:
@@ -691,6 +726,58 @@ class HandleModel:
                 cells[(s, d)] = dict(cell_measured=True, cell_status=ERR_INTEGRITY if bad else 0, bad_sizes=bad,
                                      bad_words=bad_words, first_bad=first_bad, sx=sx)
         return dict(call_seq=seq, sizes=sizes, ranks=ranks, cells=cells)
+
+    def ce_alltoall(self, op: int, reps: int):
+        """What cdprobe_ce_alltoall with op and `reps` timed reps (0: 8) must return, but the times.  A refused call
+        returns its error code and advances nothing, nor builds the exchange area: ERR_ARG when reps is above 64, else
+        when the op is neither OP_READ nor OP_WRITE, else when some process's armed fault names no cell, size or word
+        (modes 0 and 1) or delay (mode 2, below timeout_ms / 2), or has a mode above 2; ERR_UNSUPPORTED when some
+        process would hold more streams on one device than its CUDA_DEVICE_MAX_CONNECTIONS gives (ce_alltoall_ref.queues
+        against max_connections).  Otherwise the call builds the area and advances call_seq.  When any probe mapping is
+        down, or was down when the area was built, nothing runs: every local rank, and every cell with a local issuer or
+        target, carries CDPROBE_ERR_STATE.  Else every rank issues every cell, and per cell whose owner (the issuer on a
+        pull, the target on a push) is local the block's checks are memcpy's (_block) with the fault, of modes 0 and 1,
+        armed in the process that hosts the issuer; mode 2 only delays a copy.
+        {"call_seq", "sizes", "area_min_bytes" (n blocks; the area is that rounded up to the VMM granule the driver
+        reports), "ranks": {local rank: {"measured", "status", "blocks"}}, "cells":
+        {(issuer, target): {"cell_measured", "cell_status", ...}}}."""
+        n = self.n
+        sizes = bwcurve_ref.ladder(self.bpp)
+        if reps > 64 or op not in (OP_READ, OP_WRITE):
+            return ERR_ARG
+        reps = reps or CE_A2A_DEFAULT_REPS
+        faults = {}
+        for proc, v in self.cea_fault.items():
+            mode, fi, ft, fk, arg = v >> 48, (v >> 40) & 0xFF, (v >> 32) & 0xFF, (v >> 24) & 0xFF, v & 0xFFFFFF
+            if (mode > 2 or fi == 0 or fi > n or ft == 0 or ft > n or (fi == ft and not self.diag) or fk == 0
+                    or fk > len(sizes) or (mode < 2 and arg >= sizes[fk - 1] // 8)
+                    or (mode == 2 and 2 * arg >= 1000 * self.timeout_ms)):
+                return ERR_ARG
+            if self.process_of(fi - 1) == proc and mode < 2:
+                faults[(fi - 1, ft - 1)] = (fk - 1, arg, mode)
+        n_procs = n // len(self.local)
+        for proc in range(n_procs):
+            ranks = range(proc * len(self.local), (proc + 1) * len(self.local))
+            need, _ = ce_alltoall_ref.queues(n, self.diag, [self.ordinal.get(g, 0) for g in ranks])
+            if need > self.max_connections[proc]:
+                return ERR_UNSUPPORTED
+        self.build_area()
+        self.cea_calls += 1
+        out = dict(call_seq=self.cea_calls, sizes=sizes, area_min_bytes=n * self.bpp, ranks={}, cells={})
+        if self.unmapped or self.area_down:
+            for g in self.local:
+                out["ranks"][g] = dict(measured=False, status=ERR_STATE, blocks=0)
+                for j in range(n):
+                    if j != g or self.diag:
+                        out["cells"][(g, j)] = out["cells"][(j, g)] = dict(cell_measured=False, cell_status=ERR_STATE)
+            return out
+        for g in self.local:
+            out["ranks"][g] = dict(measured=True, status=0, blocks=n - 1 + self.diag)
+        for g, j in ce_alltoall_ref.cells(n, self.diag):
+            if ce_alltoall_ref.owner(op, g, j) in self.local:
+                b = self._block(op, g, j, sizes, reps, faults.get((g, j)))
+                out["cells"][(g, j)] = dict(cell_measured=True, cell_status=b.pop("status"), **b)
+        return out
 
     # ---- state changes -------------------------------------------------------------------------------------
     def corrupt_word(self, rank: int, word: int, mask: int) -> None:

@@ -3,8 +3,12 @@ with the (S, X) of the pattern, and every block is word-checked by its owner; ea
 process that would share hardware queues is refused and keeps its handle; an armed fault fails exactly its cell and
 size, or only delays it, and the next call is clean; a mapping that is down runs nothing; the neighbouring measurements
 stay clean; two processes give what one gives; and nothing leaks.  Several ranks share one device; domains whose
-streams exceed the default 8 hardware queues run in child processes with CUDA_DEVICE_MAX_CONNECTIONS=32."""
+streams exceed the default 8 hardware queues run in child processes with CUDA_DEVICE_MAX_CONNECTIONS=32, and three
+ranks run at exactly the queues they need, and are refused one queue below, in children with the limit set so."""
+import json
 import os
+import subprocess
+import sys
 import textwrap
 
 import pytest
@@ -282,3 +286,53 @@ def test_no_leak(pkg):
             assert torch.cuda.mem_get_info(0)[0] == free1 and len(os.listdir("/proc/self/fd")) == fds1
         assert torch.cuda.mem_get_info(0)[0] == free0
     assert len(os.listdir("/proc/self/fd")) == fds0
+
+
+# ---- the queue refusal at its edge ----------------------------------------------------------------------------------
+BOUNDARY = textwrap.dedent(
+    """
+    import json, sys
+    sys.path[:0] = [%r, %r]
+    sys.modules["torch"] = None
+    import cdprobe_pkg
+    from oracle import oracle
+    import test_ce_alltoall_gpu as t
+    t.case_boundary(cdprobe_pkg.load(), oracle, *json.loads(sys.argv[1]))
+    print("CHILD OK")
+    """
+) % (ROOT, os.path.join(ROOT, "tests"))
+
+
+def case_boundary(pkg, oracle, diag, limit):
+    """Three ranks on one device, each with its own stream and a copy stream per cell it issues: 9 queues, 12 with
+    LOCAL_DIAG.  At need = limit every stream has a hardware queue of its own and both ops run clean; one queue less
+    is refused with the need and the limit named, advances nothing, and memcpy still runs clean on the handle."""
+    n, nbytes = 3, 1 << 20
+    need, ordinal = ref.queues(n, bool(diag), [0] * n)
+    assert (need, ordinal) == (9 if not diag else 12, 0)
+    with open_same(pkg, n, flags=diag, nbytes=nbytes) as p:
+        bpp = pkg.plan(n, nbytes, MODE_SLICED, diag).bytes_per_pair
+        if limit >= need:
+            for call, op in enumerate(OPS, 1):
+                c = as_dict(p.CeAllToAll(op, reps=2))
+                assert (c["call_seq"], c["reps"]) == (call, 2)
+                check_call(c, oracle, bpp, MODE_SLICED, bool(diag))
+            return
+        for op in OPS:
+            rc, t = p.ce_alltoall_raw(op, 2)
+            assert rc == ERR_UNSUPPORTED and t.call_seq == 0 and sum(t.measured) == 0, rc
+            assert ref.queue_message(need, 0, limit) in pkg.abi.load_library().cdprobe_last_error().decode()
+        mc = p.Memcpy(ref.OP_WRITE, reps=1)
+        assert mc.call_seq == 1
+        assert all(mc.status[g][j] == 0 and mc.bad_sizes[g][j] == 0 for g, j in ref.cells(n, bool(diag)))
+
+
+BOUNDARY_CASES = [(0, 9), (0, 8), (LOCAL_DIAG, 12), (LOCAL_DIAG, 11)]
+
+
+@pytest.mark.parametrize("diag,limit", BOUNDARY_CASES, ids=["9-of-9", "9-of-8", "diag-12-of-12", "diag-12-of-11"])
+def test_three_ranks_run_at_exactly_their_queues_and_are_refused_one_below(pkg, oracle, diag, limit):
+    env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS=str(limit))
+    pr = subprocess.run([sys.executable, "-c", BOUNDARY, json.dumps([diag, limit])], env=env, capture_output=True,
+                        text=True, timeout=600)
+    assert pr.returncode == 0 and "CHILD OK" in pr.stdout, pr.stderr[-8000:]

@@ -5,7 +5,9 @@ corruptions (also cancelling ones) and faults against a direct recomputation, it
 sticky exchange area; the same for the two-shot, LL, ring and push all-reduces (each protocol's faults at edge words,
 drop and unstored modes included, against whole-array recomputations from their references) and for memcpy (a
 corrupted source word fails exactly the cells and sizes that copy it), with their refusals, counters, skip rules and
-sticky areas, the exchange area shared by memcpy and the all-to-all in both orders."""
+sticky areas, the exchange area shared by memcpy and the all-to-all in both orders; and for the copy-engine all-to-all
+(its blocks are memcpy's, checked by their owners: corruptions, edge faults of every mode, its refusals and their
+precedence, the queue limit of every process, its all-or-nothing down rule and its own counter)."""
 import ctypes as C
 import random
 
@@ -19,6 +21,7 @@ import allreduce_ref
 import allreduce_ring_ref
 import alltoall_ref
 import bwcurve_ref
+import ce_alltoall_ref
 import latency_ref
 import memcpy_ref
 import word_ref as ref
@@ -681,12 +684,14 @@ def test_memcpy_refusals_counters_and_the_one_sided_skip_rule(oracle):
     assert (m.a2a_calls, m.ar_calls, m.ts_calls, m.ll_calls, m.ring_calls, m.push_calls) == (0,) * 6
 
 
-@pytest.mark.parametrize("first", ["memcpy", "alltoall"])
+@pytest.mark.parametrize("first", ["memcpy", "alltoall", "ce_alltoall"])
 def test_the_exchange_area_is_built_by_whichever_of_memcpy_and_alltoall_comes_first(oracle, first):
     n = 3
     m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    m.max_connections[0] = 32
     m.unmapped.add((0, 2))
-    m.memcpy(hm.OP_READ, 1) if first == "memcpy" else m.alltoall(1)
+    {"memcpy": lambda: m.memcpy(hm.OP_READ, 1), "alltoall": lambda: m.alltoall(1),
+     "ce_alltoall": lambda: m.ce_alltoall(hm.OP_READ, 1)}[first]()
     assert m.area_down == {(0, 2)}
     m.unmapped.discard((0, 2))  # remap: the probe mapping is back, the exchange area's is not
     for op in (hm.OP_READ, hm.OP_WRITE):
@@ -695,6 +700,218 @@ def test_the_exchange_area_is_built_by_whichever_of_memcpy_and_alltoall_comes_fi
         assert all(c["measured"] for key, c in got["cells"].items() if key != (0, 2))
     aa = m.alltoall(1)
     assert aa["cells"][(0, 2)] == dict(cell_measured=False, cell_status=hm.ERR_STATE)
-    assert m.area_down == {(0, 2)} and (m.mc_calls, m.a2a_calls) == ((3, 1) if first == "memcpy" else (2, 2))
+    assert m.area_down == {(0, 2)}
+    assert (m.mc_calls, m.a2a_calls, m.cea_calls) == {"memcpy": (3, 1, 0), "alltoall": (2, 2, 0),
+                                                      "ce_alltoall": (2, 1, 1)}[first]
+    # the copy-engine all-to-all needs every pair of the area: it stays off until close
+    for op in (hm.OP_READ, hm.OP_WRITE):
+        got = m.ce_alltoall(op, 1)
+        assert got["ranks"] == {g: dict(measured=False, status=hm.ERR_STATE, blocks=0) for g in range(n)}
+        assert got["cells"] == {(g, j): dict(cell_measured=False, cell_status=hm.ERR_STATE)
+                                for g in range(n) for j in range(n) if g != j}
     # the all-reduces' areas are their own: built now, with every mapping up
     assert all(r["measured"] for r in m.twoshot(1)["rows"].values()) and m.ar_area_down["ts"] == frozenset()
+
+
+# ---- the copy-engine all-to-all ------------------------------------------------------------------------------------
+def ce_cells(got):
+    """{cell: [((S, X), bad words, first bad, fails) per size]} of the cells the model says were checked."""
+    return {key: [(sx, b, f, bool((c["bad_sizes"] >> k) & 1))
+                  for k, (sx, b, f) in enumerate(zip(c["sx"], c["bad_words"], c["first_bad"]))]
+            for key, c in got["cells"].items() if c["cell_measured"]}
+
+
+def check_ce(oracle, m, op, reps, corrupt, faults=None):
+    """One ce_alltoall call of the model against memcpy_direct for every block a local rank owns: the cell set, the
+    rank rows, the verdicts, and per size the (S, X), bad words and first bad offset.  faults: {cell: (k, word, mode)}
+    of modes 0 and 1."""
+    n = m.n
+    got = m.ce_alltoall(op, reps)
+    cells = [c for c in ce_alltoall_ref.cells(n, m.diag) if ce_alltoall_ref.owner(op, *c) in m.local]
+    assert sorted(got["cells"]) == sorted(cells)
+    assert got["ranks"] == {g: dict(measured=True, status=0, blocks=n - 1 + m.diag) for g in m.local}
+    assert got["area_min_bytes"] == n * m.bpp
+    for (g, j), sizes in ce_cells(got).items():
+        f = (faults or {}).get((g, j))
+        want = memcpy_direct(oracle, n, m.bpp, op, g, j, corrupt, f, reps or 8)
+        assert sizes == want, (g, j, f, reps)
+        c = got["cells"][(g, j)]
+        assert c["cell_status"] == (hm.ERR_INTEGRITY if c["bad_sizes"] else 0)
+    return got
+
+
+@pytest.mark.parametrize("op", [hm.OP_READ, hm.OP_WRITE], ids=["pull", "push"])
+def test_ce_alltoall_under_one_several_and_cancelling_corruptions_equals_a_direct_recomputation(oracle, op):
+    n = 3
+    m = edge_model(oracle, n)
+    m.max_connections[0] = 9
+    sizes = memcpy_ref.ladder(m.bpp)
+    W = m.W
+    # one corruption: exactly the cells and sizes that copy it, (reps + 1) bad words each (the warm-up too)
+    for reps in (1, 2, 0):
+        for rank, word, mask in ((0, 0, 1), (2, W + 3 * G + 7, 1 << 63), (1, 2 * W - 1, 0xFFFF), (1, W - 1, 0xF0)):
+            m.corrupt_word(rank, word, mask)
+            got = check_ce(oracle, m, op, reps, {(rank, word): mask})
+            for (g, j), cell in got["cells"].items():
+                c = memcpy_ref.cell(n, m.bpp, 1, op, g, j)
+                at = word - c["first_word"]
+                hit = c["src_rank"] == rank and 0 <= at < W
+                bits = sum(1 << k for k, s in enumerate(sizes) if hit and s // 8 > at)
+                assert cell["bad_sizes"] == bits, (g, j, word)
+                assert cell["bad_words"] == [((reps or 8) + 1) * ((bits >> k) & 1) for k in range(len(sizes))]
+                assert cell["first_bad"] == [8 * at if (bits >> k) & 1 else ref.U64_MAX for k in range(len(sizes))]
+            m.corrupt_word(rank, word, mask)  # restore
+    assert m.corrupt == {} and m.cea_calls == 12
+    # several at once, and two maskings of one word that cancel in part and then whole
+    corrupt = {(0, 5): 1 << 40, (1, W + 5): 0x3, (2, W - 1): 1 << 7, (0, 2 * W - 1): 0xFF, (1, 0): 1}
+    for (r, k), mask in corrupt.items():
+        m.corrupt_word(r, k, mask)
+    check_ce(oracle, m, op, 1, corrupt)
+    m.corrupt_word(0, 5, (1 << 40) | 1)
+    check_ce(oracle, m, op, 2, {**corrupt, (0, 5): 1})
+    m.corrupt_word(0, 5, 1)
+    check_ce(oracle, m, op, 2, {k: v for k, v in corrupt.items() if k != (0, 5)})
+    assert (0, 5) not in m.corrupt
+
+
+@pytest.mark.parametrize("op", [hm.OP_READ, hm.OP_WRITE], ids=["pull", "push"])
+@pytest.mark.parametrize("n", [1, 3])
+def test_ce_alltoall_edge_faults_of_every_mode_equal_a_direct_recomputation(oracle, n, op):
+    """Modes 0 and 1 at word 0 of size 0, the last word of the last, partial unit and a word of that unit a corruption
+    also changes (on the loop-back cell at N = 1), in timed rep 1 only; mode 2 changes no integrity field."""
+    m = edge_model(oracle, n)
+    m.max_connections[0] = 32
+    sizes = memcpy_ref.ladder(m.bpp)
+    W, last = m.W, len(sizes) - 1
+    corrupt = {(n - 1, 5): 1 << 40, (0, W - 1): 0xFF}
+    for (r, k), mask in corrupt.items():
+        m.corrupt_word(r, k, mask)
+    spots = [(0, 0, 0, 0), (0, 0, last, W - 1), (0, 0, last, W // 1024 * 1024 + 3), (0, 0, 0, 5)] if n == 1 else \
+        [(0, 1, 0, 0), (2, 1, last, W - 1), (1, 0, last, 5), (1, 2, last, W // 1024 * 1024 + 3)]
+    for g, j, k, w in spots:
+        for mode in (0, 1):
+            m.arm_measure(m.cea_fault, 0, (mode << 48) | ((g + 1) << 40) | ((j + 1) << 32) | ((k + 1) << 24) | w)
+            for reps in (1, 2):
+                got = check_ce(oracle, m, op, reps, corrupt, {(g, j): (k, w, mode)})
+                assert got["cells"][(g, j)]["bad_sizes"] >> k & 1
+        for reps in (1, 2):  # a hold of 3 ms: every block as if nothing were armed
+            m.arm_measure(m.cea_fault, 0, (2 << 48) | ((g + 1) << 40) | ((j + 1) << 32) | ((k + 1) << 24) | 3000)
+            check_ce(oracle, m, op, reps, corrupt)
+    m.arm_measure(m.cea_fault, 0, 0)
+    assert m.cea_calls == len(spots) * 6 and (m.mc_calls, m.a2a_calls) == (0, 0)
+
+
+@pytest.mark.parametrize("op", [hm.OP_READ, hm.OP_WRITE], ids=["pull", "push"])
+def test_ce_alltoall_fault_acts_only_in_the_process_that_hosts_its_issuer(oracle, op):
+    """Process 0 of two (one rank each) checks the blocks it owns: a fault armed in process 1 on issuer 1 reaches cell
+    (1, 0) when process 0 owns it (a push); the same fault armed in process 0 is validated but acts nowhere."""
+    m = hm.HandleModel(oracle, no_schedule, 2, 1 << 20, sm_count=132, local=[0])
+    sizes = memcpy_ref.ladder(m.bpp)
+    v = (2 << 40) | (1 << 32) | (2 << 24) | 7  # issuer 1, target 0, size 1, word 7
+    m.arm_measure(m.cea_fault, 1, v)
+    got = m.ce_alltoall(op, 1)
+    owned = {(0, 1)} if op == hm.OP_READ else {(1, 0)}
+    assert set(got["cells"]) == owned and set(got["ranks"]) == {0}
+    for key in owned:
+        f = (1, 7, 0) if key == (1, 0) else None
+        assert ce_cells(got)[key] == memcpy_direct(oracle, 2, m.bpp, op, *key, {}, f, 1)
+        assert got["cells"][key]["bad_sizes"] == (0b10 if f else 0)
+    m.arm_measure(m.cea_fault, 1, 0)
+    m.arm_measure(m.cea_fault, 0, v)
+    assert all(c["bad_sizes"] == 0 for c in m.ce_alltoall(op, 1)["cells"].values())
+    m.arm_measure(m.cea_fault, 1, v + sizes[1] // 8)  # one word past its size, in the other process: refused here too
+    assert m.ce_alltoall(op, 1) == hm.ERR_ARG and m.cea_calls == 2
+
+
+def test_ce_alltoall_refusals_their_precedence_and_the_queue_limit_of_every_process(oracle):
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    sizes = memcpy_ref.ladder(m.bpp)
+    m.max_connections[0] = 8  # 3 ranks on one device need 9 queues
+    bad_fault = (3 << 48) | (1 << 40) | (2 << 32) | (1 << 24)
+    m.arm_measure(m.cea_fault, 0, bad_fault)
+    assert m.ce_alltoall(hm.OP_READ, 65) == hm.ERR_ARG    # reps first
+    assert m.ce_alltoall(3, 2) == hm.ERR_ARG              # then the op
+    assert m.ce_alltoall(hm.OP_READ, 2) == hm.ERR_ARG     # then the fault, before the queues
+    for bad in ((1 << 40) | (1 << 32) | (1 << 24), ((n + 1) << 40) | (1 << 32) | (1 << 24),
+                (1 << 40) | ((n + 1) << 32) | (1 << 24), (1 << 40) | (2 << 32) | ((len(sizes) + 1) << 24),
+                (1 << 40) | (2 << 32) | (1 << 24) | sizes[0] // 8, (1 << 48) | (1 << 40) | (2 << 32) | (1 << 24)
+                | sizes[0] // 8, (2 << 48) | (1 << 40) | (2 << 32) | (1 << 24) | 10_000_000, (1 << 40) | (2 << 32)):
+        m.arm_measure(m.cea_fault, 0, bad)
+        assert m.ce_alltoall(hm.OP_WRITE, 1) == hm.ERR_ARG, hex(bad)
+    # a hold below timeout_ms / 2 names no word: accepted whatever its size
+    m.arm_measure(m.cea_fault, 0, (2 << 48) | (1 << 40) | (2 << 32) | (1 << 24) | 9_999_999)
+    assert m.ce_alltoall(hm.OP_WRITE, 1) == hm.ERR_UNSUPPORTED  # then the queues
+    m.arm_measure(m.cea_fault, 0, 0)
+    assert m.ce_alltoall(hm.OP_READ, 0) == hm.ERR_UNSUPPORTED
+    assert m.cea_calls == 0 and m.area_down is None  # no refusal advances anything or builds the area
+    m.max_connections[0] = 9  # need = limit runs
+    got = m.ce_alltoall(hm.OP_READ, 0)
+    assert got["call_seq"] == 1 and all(c["bad_words"] == [0] * len(sizes) for c in got["cells"].values())
+    assert m.area_down == frozenset()
+    # two processes of three ranks each: 18 queues; one process at 8 refuses both
+    for limits, want in (({0: 32, 1: 8}, hm.ERR_UNSUPPORTED), ({0: 8, 1: 32}, hm.ERR_UNSUPPORTED),
+                         ({0: 18, 1: 18}, None)):
+        for me in (0, 1):
+            mp = hm.HandleModel(oracle, no_schedule, 6, 5 << 20, sm_count=132, local=range(3 * me, 3 * me + 3))
+            mp.max_connections.update(limits)
+            got = mp.ce_alltoall(hm.OP_WRITE, 1)
+            if want is None:
+                assert got["call_seq"] == 1 and set(got["ranks"]) == set(mp.local)
+                assert {ce_alltoall_ref.owner(hm.OP_WRITE, *c) for c in got["cells"]} == set(mp.local)
+            else:
+                assert got == want and mp.cea_calls == 0 and mp.area_down is None, (limits, me)
+    # one rank per device, as a node of four GPUs opens them: 4 queues per device, which the default 8 allows
+    m4 = hm.HandleModel(oracle, no_schedule, 4, 3 << 20, sm_count=132)
+    m4.ordinal.update({g: g for g in range(4)})
+    m4.max_connections[0] = 8
+    assert m4.ce_alltoall(hm.OP_READ, 1)["call_seq"] == 1
+    m4.ordinal.clear()  # all four on device 0: 16
+    assert m4.ce_alltoall(hm.OP_READ, 1) == hm.ERR_UNSUPPORTED and m4.cea_calls == 1
+    # two ranks on each of two devices need what one rank per device needs, twice
+    m4 = hm.HandleModel(oracle, no_schedule, 4, 3 << 20, sm_count=132)
+    m4.ordinal.update({0: 0, 1: 1, 2: 0, 3: 1})
+    m4.max_connections[0] = 8
+    assert m4.ce_alltoall(hm.OP_READ, 1)["call_seq"] == 1
+    m4.ordinal[3] = 0
+    assert m4.ce_alltoall(hm.OP_READ, 1) == hm.ERR_UNSUPPORTED and m4.cea_calls == 1
+
+
+def test_max_connections_reads_the_variable_as_cdprobe_open_does():
+    for value, want in ((None, 8), ("", 8), ("9", 9), ("32", 32), ("64", 32), ("0", 8), ("-4", 8), ("abc", 8),
+                        ("12x", 12), (" 5", 5)):
+        env = {} if value is None else {"CUDA_DEVICE_MAX_CONNECTIONS": value}
+        assert hm.max_connections(env) == want, value
+
+
+def test_ce_alltoall_down_rule_counters_and_the_sticky_area(oracle):
+    """Any pair down stops every rank and reports every cell of a local rank, either way, as down; call_seq still
+    advances and the area is built.  A pair down when the area was built keeps it off after the remap, while memcpy
+    and the all-to-all skip only that cell.  Each measurement keeps its own counter."""
+    n = 3
+    m = hm.HandleModel(oracle, no_schedule, n, 1 << 20, sm_count=132)
+    m.max_connections[0] = 32
+    assert m.ce_alltoall(hm.OP_WRITE, 1)["call_seq"] == 1
+    m.unmapped.add((2, 1))  # after the area: stops the call while down, not after the remap
+    got = m.ce_alltoall(hm.OP_READ, 1)
+    assert got["call_seq"] == 2 and got["ranks"] == {g: dict(measured=False, status=hm.ERR_STATE, blocks=0)
+                                                     for g in range(n)}
+    assert got["cells"] == {(g, j): dict(cell_measured=False, cell_status=hm.ERR_STATE)
+                            for g in range(n) for j in range(n) if g != j}
+    m.unmapped.discard((2, 1))
+    assert all(r["measured"] for r in m.ce_alltoall(hm.OP_READ, 1)["ranks"].values())
+    # only rank 0 local, two processes: its row, and the cells it issues or receives, are down
+    m2 = hm.HandleModel(oracle, no_schedule, 2, 1 << 20, sm_count=132, local=[0])
+    m2.unmapped.add((0, 1))
+    got = m2.ce_alltoall(hm.OP_READ, 1)
+    assert got["ranks"] == {0: dict(measured=False, status=hm.ERR_STATE, blocks=0)} and m2.area_down == {(0, 1)}
+    assert set(got["cells"]) == {(0, 1), (1, 0)}
+    m2.unmapped.clear()
+    assert m2.ce_alltoall(hm.OP_WRITE, 1)["ranks"][0]["measured"] is False and m2.cea_calls == 2
+    # counters: each its own
+    m.alltoall(1)
+    m.memcpy(hm.OP_READ, 1)
+    m.memcpy(hm.OP_WRITE, 1)
+    assert (m.cea_calls, m.a2a_calls, m.mc_calls) == (3, 1, 2)
+    assert m.ce_alltoall(3, 1) == hm.ERR_ARG and m.ce_alltoall(hm.OP_READ, 2)["call_seq"] == 4
+    assert (m.cea_calls, m.a2a_calls, m.mc_calls) == (4, 1, 2)

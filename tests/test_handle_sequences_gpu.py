@@ -16,7 +16,11 @@ one handle through many calls and compares the whole output of each call with th
   rule; AllToAll: per rank measured and blocks, per cell status, bad_sizes and per size bad_words, first_bad and
   (S, X), under armed faults and the sticky exchange-area rule; Memcpy, both ops: per cell measured, status, bad_sizes
   and per size bad_words, first_bad and (S, X), under corruptions at rest, armed faults and the exchange area it shares
-  with the all-to-all; all with call_seq, the ladder and the path (the LL and the ring report their own) or area_bytes;
+  with the all-to-all; the copy-engine all-to-all, both ops: per rank measured, status and blocks, per cell status,
+  bad_sizes and per size bad_words, first_bad and (S, X) where its owner is local, under corruptions at rest, armed
+  flips, drops and holds, its all-or-nothing down rule, the shared exchange area and the hardware-queue refusal (walks
+  with N = 3 and 5 ranks on one device see it refused at 8 queues, and run it in a child process with 32); all with
+  call_seq, the ladder and the path (the LL and the ring report their own) or area_bytes;
 - refused calls: the error code, and nothing they may not change.
 
 A divergence fails with the seed, the step index and every step so far; the walk is generated from the seed and the
@@ -26,6 +30,7 @@ timeout or touches more than 4 GiB.
 """
 import ctypes as C
 import json
+import os
 import random
 import subprocess
 import sys
@@ -61,13 +66,14 @@ LADDER_REPS = 1  # the ladder measurements fold timed rep 1, the faulted one, in
 # each ladder measurement's fault option and the model's {process: value} of it
 FAULTS = {"OPT_ALLREDUCE_FAULT": "ar_fault", "OPT_ALLREDUCE_TWOSHOT_FAULT": "ts_fault",
           "OPT_ALLREDUCE_LL_FAULT": "ll_fault", "OPT_ALLREDUCE_RING_FAULT": "ring_fault",
-          "OPT_ALLREDUCE_PUSH_FAULT": "push_fault", "OPT_ALLTOALL_FAULT": "a2a_fault", "OPT_MEMCPY_FAULT": "mc_fault"}
+          "OPT_ALLREDUCE_PUSH_FAULT": "push_fault", "OPT_ALLTOALL_FAULT": "a2a_fault", "OPT_MEMCPY_FAULT": "mc_fault",
+          "OPT_CE_ALLTOALL_FAULT": "cea_fault"}
 # each all-reduce step: the model's method, the raw binding and the path it reports (None: the handle's)
 ALLREDUCES = {"allreduce": ("allreduce", "allreduce_raw", None), "twoshot": ("twoshot", "allreduce_twoshot_raw", None),
               "ll": ("ll", "allreduce_ll_raw", 3), "ring": ("ring", "allreduce_ring_raw", 4),
               "push": ("push", "allreduce_push_raw", None)}
 LADDER_CALLS = [("allreduce",), ("twoshot",), ("ll",), ("ring",), ("push",), ("alltoall",), ("memcpy", 1),
-                ("memcpy", 2)]
+                ("memcpy", 2), ("ce_alltoall", 1), ("ce_alltoall", 2)]
 
 
 class Refused(Exception):
@@ -85,6 +91,9 @@ class Driver:
         local = list(range(self.first, self.first + self.n_local))
         self.m = hm.HandleModel(oracle, hm.schedule_fn(p._lib, pkg.abi), n, nbytes, info.sm_count[0], cfg.ctas,
                                 local=local, flags=cfg.flags)
+        # every process of these tests opens its ranks on the same ordinals, so global rank g sits on ordinal
+        # cfg.ordinals[g % n_local] (the copy-engine all-to-all counts hardware queues per device)
+        self.m.ordinal.update({g: cfg.ordinals[g % self.n_local] for g in range(n)})
         self.gate = pkg.gate(cfg, n)
         self.area_bytes = None  # of the exchange area, once the all-to-all or memcpy has reported it
         self.check_info()
@@ -261,6 +270,36 @@ class Driver:
                                bad_words=mc.bad_words[g][j], first_bad=mc.first_bad[g][j])
                 assert got == w, ("memcpy cell", op, g, j, got, w)
 
+    def check_ce_alltoall(self, op):
+        """cdprobe_ce_alltoall against the model, field for field but the times: a refusal's code and nothing advanced;
+        else call_seq, the ladder, area_bytes, per rank measured, status and blocks, and per cell cell_measured,
+        cell_status and, where a local owner checked it, bad_sizes and per size bad_words, first_bad and (S, X)."""
+        a, m = self.a, self.m
+        want = m.ce_alltoall(op, LADDER_REPS)
+        rc, t = self.p.ce_alltoall_raw(op, LADDER_REPS)
+        if not isinstance(want, dict):  # ERR_ARG or the queue refusal: nothing advances, the area is not built
+            assert rc == want and t.call_seq == 0 and sum(t.measured) == 0, (rc, want, t.call_seq)
+            return
+        assert rc == a.OK, (rc, a.load_library().cdprobe_last_error())
+        ca = self.pkg.CeAllToAll.from_c(t)
+        assert (ca.call_seq, ca.sizes, ca.op, ca.reps) == (want["call_seq"], want["sizes"], op, LADDER_REPS), \
+            (ca.call_seq, want["call_seq"])
+        assert ca.area_bytes >= want["area_min_bytes"], (ca.area_bytes, want["area_min_bytes"])
+        self.check_area_bytes(ca.area_bytes)
+        assert ca.row_mask == sum(1 << g for g in m.local)
+        for g in range(self.n):
+            w = want["ranks"].get(g, dict(measured=False, status=0, blocks=0))
+            got = dict(measured=ca.measured[g], status=ca.status[g], blocks=ca.blocks[g] if ca.measured[g] else 0)
+            assert got == w, ("ce_alltoall rank", op, g, got, w)
+        for g in range(self.n):
+            for j in range(self.n):
+                w = want["cells"].get((g, j), dict(cell_measured=False, cell_status=0))
+                got = dict(cell_measured=ca.cell_measured[g][j], cell_status=ca.cell_status[g][j])
+                if w["cell_measured"]:
+                    got.update(bad_sizes=ca.bad_sizes[g][j], bad_words=ca.bad_words[g][j],
+                               first_bad=ca.first_bad[g][j], sx=list(zip(ca.sum[g][j], ca.xr[g][j])))
+                assert got == w, ("ce_alltoall cell", op, g, j, got, w)
+
     def apply(self, step):
         a, m, p = self.a, self.m, self.p
         kind = step[0]
@@ -344,6 +383,8 @@ class Driver:
             self.check_alltoall()
         elif kind == "memcpy":
             self.check_memcpy(step[1])
+        elif kind == "ce_alltoall":
+            self.check_ce_alltoall(step[1])
         elif kind == "bad_call":  # refused measurement calls advance no call_seq
             what = step[1]
             if what == "bwcurve":
@@ -356,6 +397,12 @@ class Driver:
                 rc, _ = p.memcpy_raw(a.OP_WRITE, a.MEMCPY_MAX_REPS + 1)
             elif what == "alltoall":
                 rc, _ = p.alltoall_raw(a.ALLTOALL_MAX_REPS + 1)
+            elif what == "ce_alltoall":
+                rc, t = p.ce_alltoall_raw(a.OP_READ | a.OP_WRITE, 1)
+                assert t.call_seq == 0
+            elif what == "ce_alltoall_reps":
+                rc, t = p.ce_alltoall_raw(a.OP_WRITE, 65)
+                assert t.call_seq == 0
             elif what == "pingpong":
                 rc, _ = p.pingpong_raw(a.PINGPONG_MAX_TRIPS + 1, 1, 0)
             else:
@@ -392,7 +439,8 @@ def ladder_fault(rng, m, name, rank, peer):
     `rank`, xor 1 or drop; OPT_ALLREDUCE_LL_FAULT, a corrupted packet rank -> peer, or a word `rank` never stores;
     OPT_ALLREDUCE_RING_FAULT, a corrupted or dropped push by `rank` in a phase that pushes the word (at N = 1, where
     nothing is pushed, a 5 us delay); OPT_ALLREDUCE_PUSH_FAULT, modes 0-2 by sender `rank` or mode 3 to receiver
-    `rank`; OPT_ALLTOALL_FAULT on block rank -> peer; OPT_MEMCPY_FAULT on cell rank -> peer, flipped or dropped."""
+    `rank`; OPT_ALLTOALL_FAULT on block rank -> peer; OPT_MEMCPY_FAULT on cell rank -> peer, flipped or dropped;
+    OPT_CE_ALLTOALL_FAULT on cell rank -> peer, flipped, dropped or held."""
     n = m.n
     sizes = allreduce_ll_ref.ladder(m.bpp) if name == "OPT_ALLREDUCE_LL_FAULT" else bwcurve_ref.ladder(m.bpp)
     k = rng.choice([len(sizes) - 1, rng.randrange(len(sizes))])
@@ -421,12 +469,16 @@ def ladder_fault(rng, m, name, rank, peer):
         return (mode << 48) | ((rank + 1) << 32) | low
     if name == "OPT_MEMCPY_FAULT":
         return (drop << 48) | ((rank + 1) << 40) | ((peer + 1) << 32) | low
+    if name == "OPT_CE_ALLTOALL_FAULT":  # a flip, a dropped copy, or a hold of at most 1 ms
+        mode = rng.randrange(3)
+        arg = rng.choice([50, 1000]) if mode == 2 else word
+        return (mode << 48) | ((rank + 1) << 40) | ((peer + 1) << 32) | ((k + 1) << 24) | arg
     return ((rank + 1) << 40) | ((peer + 1) << 32) | low
 
 
 def past_its_size(m, name, value):
     """The same fault one word past its size, which the next call refuses (a delay is left as it is)."""
-    if name == "OPT_ALLREDUCE_RING_FAULT" and value >> 48 == 2:
+    if name in ("OPT_ALLREDUCE_RING_FAULT", "OPT_CE_ALLTOALL_FAULT") and value >> 48 == 2:
         return value
     return value + bwcurve_ref.ladder(m.bpp)[((value >> 24) & 0xFF) - 1] // 8 - (value & 0xFFFFFF)
 
@@ -504,8 +556,8 @@ def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
         return ("atomics", rng.randrange(3))
     if x < 0.98:
         return ("bwcurve",)
-    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics", "alltoall", "memcpy", "memcpy_reps"]
-                                   + sorted(ALLREDUCES)))
+    return ("bad_call", rng.choice(["bwcurve", "pingpong", "atomics", "alltoall", "memcpy", "memcpy_reps", "ce_alltoall",
+                                    "ce_alltoall_reps"] + sorted(ALLREDUCES)))
 
 
 def walk_step(rng, m, steps, **kw):
@@ -559,6 +611,50 @@ def test_seeded_walk_real_peers(pkg, oracle, seed):
     cfg = pkg.Config(ordinals=list(range(n)), bytes=BIG, timeout_ms=20000)
     with pkg.Open(cfg) as p:
         walk(Driver(pkg, oracle, p, cfg, n, BIG, same_device=False), seed, STEPS, same_device=False)
+
+
+# The copy-engine all-to-all needs n x n hardware queues for n ranks on one device: above 2 ranks more than the
+# default 8 of CUDA_DEVICE_MAX_CONNECTIONS, so the walks above see its refusal at N = 3 and 5, and these see it run.
+# The CUDA runtime reads the variable once, at its start, so they run in a child process that has it from birth.
+CHILD_WALKS = [(3, BIG, 8, 34), (5, SMALL, 8, 54)]
+
+
+def case_walk(pkg, oracle, n, nbytes, ctas, seed):
+    cfg, p = open_same(pkg, n, nbytes, ctas)
+    with p:
+        drv = Driver(pkg, oracle, p, cfg, n, nbytes)
+        assert drv.m.max_connections == {0: 32}
+        walk(drv, seed, STEPS)
+
+
+@pytest.mark.parametrize("n,nbytes,ctas,seed", CHILD_WALKS,
+                         ids=[f"n{w[0]}-{'big' if w[1] == BIG else 'small'}-seed{w[3]}" for w in CHILD_WALKS])
+def test_seeded_walk_with_32_hardware_queues(pkg, oracle, n, nbytes, ctas, seed):
+    in_child("case_walk", n, nbytes, ctas, seed)
+
+
+SEQ_CHILD = textwrap.dedent(
+    """
+    import json, sys
+    sys.path[:0] = [%r, %r]
+    sys.modules["torch"] = None  # not needed here; conftest.gpu_count() then reports 0, which only feeds skip marks
+    import cdprobe_pkg
+    from oracle import oracle
+    import test_handle_sequences_gpu as t
+    pkg = cdprobe_pkg.load()
+    getattr(t, sys.argv[1])(pkg, oracle, *json.loads(sys.argv[2]))
+    print("CHILD OK")
+    """
+) % (ROOT, ROOT + "/tests")
+
+
+def in_child(case, *args, timeout=1200):
+    """Run case(pkg, oracle, *args) in a fresh process with 32 hardware queues per device; its assertion is the
+    failure message."""
+    env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32")
+    pr = subprocess.run([sys.executable, "-c", SEQ_CHILD, case, json.dumps(args)], env=env, capture_output=True,
+                        text=True, timeout=timeout)
+    assert pr.returncode == 0 and "CHILD OK" in pr.stdout, pr.stderr[-8000:]
 
 
 # ---- hand-written sequences: the transitions most likely to leave state behind ---------------------------------
@@ -626,21 +722,32 @@ def test_alltoall_area_of_a_pair_unmapped_at_its_first_call_stays_unmapped_after
     assert drv.m.area_down == {(0, 2)} and drv.m.a2a_calls == 4
 
 
-@pytest.mark.parametrize("first", ["memcpy", "alltoall"])
-def test_exchange_area_built_while_a_pair_is_down_stays_unmapped_for_memcpy_and_alltoall(pkg, oracle, first):
-    """cdprobe_memcpy and cdprobe_alltoall share one exchange area, built by whichever is called first: with (0, 2)
-    down then, cell (0, 2) is skipped by both, with either op, until close, while runs use the remapped pair.  An armed
-    memcpy drop on another cell fails exactly that cell and size, and the next call is clean again."""
-    A2A, MC1, MC2 = ("alltoall",), ("memcpy", 1), ("memcpy", 2)
-    opener = MC1 if first == "memcpy" else A2A
+def case_exchange_area_built_while_a_pair_is_down(pkg, oracle, first):
+    """cdprobe_memcpy, cdprobe_alltoall and cdprobe_ce_alltoall share one exchange area, built by whichever is called
+    first, even by a copy-engine all-to-all that then runs nothing: with (0, 2) down then, cell (0, 2) is skipped by
+    memcpy and the all-to-all, with either op, until close, while runs use the remapped pair, and the copy-engine
+    all-to-all stays off.  An armed memcpy drop on another cell fails exactly that cell and size, and the next call is
+    clean again.  Three ranks on one device need 9 hardware queues: it runs in a child process with 32."""
+    A2A, MC1, MC2, CE1, CE2 = ("alltoall",), ("memcpy", 1), ("memcpy", 2), ("ce_alltoall", 1), ("ce_alltoall", 2)
+    opener = {"memcpy": MC1, "alltoall": A2A, "ce_alltoall": CE1}[first]
     bpp = oracle.plan(3, BIG, 1, False).bytes_per_pair
     last = len(bwcurve_ref.ladder(bpp)) - 1
     drop = (1 << 48) | (3 << 40) | (1 << 32) | ((last + 1) << 24) | (bpp // 8 - 1)
     # the first calls after the remap are memcpy's, so a model that let only the all-to-all build the area diverges
-    steps = [RUN, ("unmap", 0, 2), opener, MC2, ("remap", 0, 2), MC1, MC2, A2A, RUN, DIAG,
-             ("opt", "OPT_MEMCPY_FAULT", drop), MC2, MC1, ("opt", "OPT_MEMCPY_FAULT", 0), MC2, A2A, RUN, DIAG]
+    # (a copy-engine all-to-all that runs nothing is the only call before the remap, so a library that built the area
+    # after its down check would build it at the next memcpy, with every pair up)
+    steps = [RUN, ("unmap", 0, 2), opener] + ([MC2] if first != "ce_alltoall" else []) + [
+        ("remap", 0, 2), MC1, MC2, A2A, CE2, RUN, DIAG, ("opt", "OPT_MEMCPY_FAULT", drop), MC2, MC1,
+        ("opt", "OPT_MEMCPY_FAULT", 0), MC2, A2A, CE1, RUN, DIAG]
     drv = play(pkg, oracle, 3, BIG, steps, f"n 3, {first} first")
-    assert drv.m.area_down == {(0, 2)} and drv.m.mc_calls == (7 if first == "memcpy" else 6)
+    assert drv.m.max_connections == {0: 32}
+    assert drv.m.area_down == {(0, 2)}
+    assert (drv.m.mc_calls, drv.m.cea_calls) == {"memcpy": (7, 2), "alltoall": (6, 2), "ce_alltoall": (5, 3)}[first]
+
+
+@pytest.mark.parametrize("first", ["memcpy", "alltoall", "ce_alltoall"])
+def test_exchange_area_built_while_a_pair_is_down_stays_unmapped_for_memcpy_and_alltoall(pkg, oracle, first):
+    in_child("case_exchange_area_built_while_a_pair_is_down", first)
 
 
 def allreduce_edge_faults(m, drop):

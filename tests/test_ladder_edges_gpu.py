@@ -17,12 +17,21 @@ word_ref) on every data path:
   pushed), and no all-to-all cell.
 
 Memcpy's checks run diag_launch and bwcurve_kernel on the issuer's grid over a destination in the exchange area, so
-its tiny ladders and small grids reach the same partial-unit branches.
+its tiny ladders and small grids reach the same partial-unit branches.  The copy-engine all-to-all's owners check its
+blocks, memcpy's blocks, the same way on their own grid and path: it runs the tiny ladders and EDGE_BPP at N = 1, 2
+(with and without LOCAL_DIAG) and 3, on every path and the grids of 1, 2, 3 and 7 CTAs, with flips at word 0 of size 0
+and at the last word of the last, partial unit and a drop at the last size, on the loop-back cell too, and a corrupted
+source word in a partial unit failing exactly the cells and sizes it fails for memcpy.
 
 Every call uses one timed rep, so the faulted rep is the one folded into (S, X); the all-reduce's word check runs
 after the warm-up and after the timed rep, and its bad words are summed over both.  Several ranks share GPU 0 with at
 most 8 CTAs each, so every rank's grid stays resident."""
 import functools
+import json
+import os
+import subprocess
+import sys
+import textwrap
 
 import numpy as np
 import pytest
@@ -32,6 +41,7 @@ import alltoall_ref
 import bwcurve_ref
 import memcpy_ref
 import word_ref
+from conftest import ROOT
 from test_bwcurve_gpu import slice_first_word
 
 pytestmark = pytest.mark.gpu
@@ -53,15 +63,17 @@ TINY = (128, 3968, 4096, 4224, 8320, 16384, 16512, 24704)
 EDGE_BPP = 57 * 8192 + 384
 
 
+@functools.lru_cache(maxsize=None)
+def src_words(rank, n_words):
+    """Words [0, n_words) of rank's source buffer, from the pattern definition (cached)."""
+    w = word_ref.src_words(SEED, rank, 0, n_words)
+    w.setflags(write=False)
+    return w
+
+
 @pytest.fixture(scope="module")
 def src():
-    """Words [0, n_words) of rank's source buffer, from the pattern definition (cached across the module's tests)."""
-    @functools.lru_cache(maxsize=None)
-    def words(rank, n_words):
-        w = word_ref.src_words(SEED, rank, 0, n_words)
-        w.setflags(write=False)
-        return w
-    return words
+    return src_words
 
 
 def open_probe(pkg, n, bpp, flags=0):
@@ -149,42 +161,68 @@ def check_memcpy(mc, src, n, bpp, diag, op, corrupt=None, fault=None):
     rep, and is checked after each: a corrupted source word is one FLIP per rep at its offset in every cell and size
     that copies it.  fault (issuer, target, k, word, mode): timed rep 1 of that cell and size holds the word's pattern
     value xored with 1 (mode 0), or nothing, as the clear's 0s (mode 1)."""
-    corrupt = corrupt or {}
     sizes = memcpy_ref.ladder(bpp)
     assert mc.sizes == sizes and mc.reps == 1 and mc.op == op
-    W = bpp // 8
     for g in range(n):
         for j in range(n):
             if g == j and not diag:
                 assert not mc.measured[g][j] and mc.status[g][j] == 0, (g, j)
                 continue
-            c = memcpy_ref.cell(n, bpp, 1, op, g, j)
-            first = c["first_word"]
-            words = source(src, c["src_rank"], first + W, corrupt)[first:]
-            pattern = src(c["src_rank"], first + W)[first:]
-            bits = 0
-            for k, s in enumerate(sizes):
-                nw = s // 8
-                warm, rep1 = words[:nw], words[:nw].copy()
-                if fault is not None and (g, j, k) == fault[:3]:
-                    if fault[4]:
-                        rep1[:] = 0
-                    else:
-                        rep1[fault[3]] = pattern[fault[3]] ^ np.uint64(1)
-                bad = [np.flatnonzero(w != pattern[:nw]) for w in (warm, rep1)]
-                first_bad = min((int(b[0]) for b in bad if len(b)), default=None)
-                ctx = (g, j, s, op, fault)
-                assert (mc.sum[g][j][k], mc.xr[g][j][k]) == allreduce_ref.checksum(rep1), ctx
-                assert mc.bad_words[g][j][k] == sum(len(b) for b in bad), (ctx, mc.bad_words[g][j][k])
-                assert mc.first_bad[g][j][k] == (U64_MAX if first_bad is None else 8 * first_bad), \
-                    (ctx, mc.first_bad[g][j][k])
-                if first_bad is not None:
-                    bits |= 1 << k
+            bits = check_block(mc, src, n, bpp, op, g, j, corrupt, fault)
             assert mc.measured[g][j] and mc.bad_sizes[g][j] == bits, (g, j, mc.bad_sizes[g][j], bits)
             assert mc.status[g][j] == (ERR_INTEGRITY if bits else 0), (g, j)
             assert (mc.t0_ns[g][j], mc.peak_gbps[g][j], mc.half_bytes[g][j]) == \
                 memcpy_ref.summary(sizes, mc.ns_median[g][j])
     return mc
+
+
+def check_block(out, src, n, bpp, op, g, j, corrupt=None, fault=None):
+    """The checks of cell (g, j)'s block in `out` (a Memcpy or a CeAllToAll: the same blocks, checked the same way)
+    against whole arrays: per size the (S, X) of timed rep 1, the bad words of the warm-up and rep 1 and the lowest
+    bad offset.  Returns the sizes that must fail, as bits."""
+    corrupt = corrupt or {}
+    W = bpp // 8
+    c = memcpy_ref.cell(n, bpp, 1, op, g, j)
+    first = c["first_word"]
+    words = source(src, c["src_rank"], first + W, corrupt)[first:]
+    pattern = src(c["src_rank"], first + W)[first:]
+    bits = 0
+    for k, s in enumerate(memcpy_ref.ladder(bpp)):
+        nw = s // 8
+        warm, rep1 = words[:nw], words[:nw].copy()
+        if fault is not None and (g, j, k) == fault[:3]:
+            if fault[4]:
+                rep1[:] = 0
+            else:
+                rep1[fault[3]] = pattern[fault[3]] ^ np.uint64(1)
+        bad = [np.flatnonzero(w != pattern[:nw]) for w in (warm, rep1)]
+        first_bad = min((int(b[0]) for b in bad if len(b)), default=None)
+        ctx = (g, j, s, op, fault)
+        assert (out.sum[g][j][k], out.xr[g][j][k]) == allreduce_ref.checksum(rep1), ctx
+        assert out.bad_words[g][j][k] == sum(len(b) for b in bad), (ctx, out.bad_words[g][j][k])
+        assert out.first_bad[g][j][k] == (U64_MAX if first_bad is None else 8 * first_bad), \
+            (ctx, out.first_bad[g][j][k])
+        if first_bad is not None:
+            bits |= 1 << k
+    return bits
+
+
+def check_ce_alltoall(ca, src, n, bpp, diag, op, corrupt=None, fault=None):
+    """Every rank issued every cell, and every block its owner checked holds, in the warm-up and the timed rep, what
+    memcpy's cell (issuer, target) lands (check_block); fault (issuer, target, k, word, mode) as memcpy's."""
+    sizes = memcpy_ref.ladder(bpp)
+    assert ca.sizes == sizes and ca.reps == 1 and ca.op == op
+    for r in range(n):
+        assert ca.measured[r] and ca.status[r] == 0 and ca.blocks[r] == n - 1 + diag, r
+    for g in range(n):
+        for j in range(n):
+            if g == j and not diag:
+                assert not ca.cell_measured[g][j] and ca.cell_status[g][j] == 0, (g, j)
+                continue
+            bits = check_block(ca, src, n, bpp, op, g, j, corrupt, fault)
+            assert ca.cell_measured[g][j] and ca.bad_sizes[g][j] == bits, (g, j, ca.bad_sizes[g][j], bits)
+            assert ca.cell_status[g][j] == (ERR_INTEGRITY if bits else 0), (g, j)
+    return ca
 
 
 def check_alltoall(aa, n, bpp, diag, fault=None):
@@ -347,3 +385,99 @@ def test_the_last_warp_placement_exists_on_small_grids():
         blocks = n
         t = word // UNIT_WORDS * blocks + block_index(n, s, d)
         assert t % (WARPS_PER_CTA * ctas) == WARPS_PER_CTA * ctas - 1 and word < bwcurve_ref.ladder(EDGE_BPP)[k] // 8
+
+
+# ---- the copy-engine all-to-all ---------------------------------------------------------------------------------------
+# Its owners check every block with memcpy's diag_launch and bwcurve_kernel, on the owner's grid and path.  N ranks on
+# one device need N x N streams (N x (N + 1) with the loop-back), so every case runs in a child process with 32 hardware
+# queues per device; the CUDA runtime reads the variable once, at its start.
+CE_CHILD = textwrap.dedent(
+    """
+    import json, sys
+    sys.path[:0] = [%r, %r]
+    sys.modules["torch"] = None
+    import cdprobe_pkg
+    import test_ladder_edges_gpu as t
+    getattr(t, sys.argv[1])(cdprobe_pkg.load(), *json.loads(sys.argv[2]))
+    print("CHILD OK")
+    """
+) % (ROOT, os.path.join(ROOT, "tests"))
+
+
+def ce_in_child(case, *args):
+    env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32")
+    pr = subprocess.run([sys.executable, "-c", CE_CHILD, case, json.dumps(args)], env=env, capture_output=True,
+                        text=True, timeout=1200)
+    assert pr.returncode == 0 and "CHILD OK" in pr.stdout, pr.stderr[-8000:]
+
+
+def case_ce_alltoall_tiny(pkg, n, flags):
+    """Both ops on every tiny ladder and on EDGE_BPP, on every path: every block clean."""
+    diag = n == 1 or bool(flags & LOCAL_DIAG)
+    for bpp in TINY + (EDGE_BPP,):
+        with open_probe(pkg, n, bpp, flags) as p:
+            for path in PATHS:
+                p.SetOption(pkg.abi.OPT_PATH, path)
+                for op in OPS:
+                    check_ce_alltoall(p.CeAllToAll(op, reps=1), src_words, n, bpp, diag, op)
+
+
+def case_ce_alltoall_grids_and_edges(pkg, n, flags):
+    """EDGE_BPP on grids of 1, 2, 3 and 7 CTAs per rank and every path: clean; a flip at word 0 of size 0, a flip at
+    the last word of the last, partial unit and a drop at the last size, on the loop-back cell too when there is one,
+    each failing exactly its cell and size; and a corrupted source word in a partial unit failing exactly the cells and
+    sizes memcpy fails for it on the same handle."""
+    a = pkg.abi
+    bpp = EDGE_BPP
+    diag = n == 1 or bool(flags & LOCAL_DIAG)
+    sizes = memcpy_ref.ladder(bpp)
+    last, W = len(sizes) - 1, bpp // 8
+    faults = [(0, 1 % n, 0, 0, 0), (n - 1, 0, last, W - 1, 0), (n - 1, 0, last, W // UNIT_WORDS * UNIT_WORDS + 5, 1)]
+    if diag:
+        faults += [(n - 1, n - 1, 0, 0, 0), (n - 1, n - 1, last, W - 1, 0), (0, 0, last, 0, 1)]
+    faults = [f for f in faults if f[0] != f[1] or diag]
+    with open_probe(pkg, n, bpp, flags) as p:
+        for q, ctas in enumerate((1, 2, 3, 7)):
+            p.SetOption(a.OPT_CTAS, ctas)
+            assert [p.Info().ctas[li] for li in range(n)] == [ctas] * n
+            for path in PATHS:
+                p.SetOption(a.OPT_PATH, path)
+                for op in OPS:
+                    check_ce_alltoall(p.CeAllToAll(op, reps=1), src_words, n, bpp, diag, op)
+            p.SetOption(a.OPT_PATH, q % 3)
+            for f, fault in enumerate(faults):
+                op = OPS[(q + f) % 2]
+                p.SetOption(a.OPT_CE_ALLTOALL_FAULT, a.ce_alltoall_fault(*fault))
+                ca = check_ce_alltoall(p.CeAllToAll(op, reps=1), src_words, n, bpp, diag, op, fault=fault)
+                assert ca.bad_sizes[fault[0]][fault[1]] == 1 << fault[2], fault
+            p.SetOption(a.OPT_CE_ALLTOALL_FAULT, 0)
+        # a source word in a partial unit, on the 32-byte ld/st path: the last word of slice 0 of rank n - 1, then the
+        # last word of size 0's half unit
+        p.SetOption(a.OPT_PATH, 2)
+        j = n - 1
+        for word in (W - 1, sizes[0] // 8 - 1):
+            corrupt = {(j, word): 1 << 33}
+            p.Corrupt(j, 8 * word, 1 << 33)
+            for op in OPS:
+                ca = check_ce_alltoall(p.CeAllToAll(op, reps=1), src_words, n, bpp, diag, op, corrupt)
+                mc = check_memcpy(p.Memcpy(op, reps=1), src_words, n, bpp, diag, op, corrupt)
+                cells = [(g, d) for g in range(n) for d in range(n) if g != d or diag]
+                assert [ca.bad_sizes[g][d] for g, d in cells] == [mc.bad_sizes[g][d] for g, d in cells], (word, op)
+                assert any(ca.bad_sizes[g][d] for g, d in cells), (word, op)
+            p.Corrupt(j, 8 * word, 1 << 33)  # restore: the next calls are clean
+            for op in OPS:
+                check_ce_alltoall(p.CeAllToAll(op, reps=1), src_words, n, bpp, diag, op)
+
+
+CE_SHAPES = [(1, 0), (2, 0), (2, LOCAL_DIAG), (3, 0)]
+CE_IDS = ["n1", "n2", "n2-local-diag", "n3"]
+
+
+@pytest.mark.parametrize("n,flags", CE_SHAPES, ids=CE_IDS)
+def test_ce_alltoall_tiny_ladders_every_path_clean(n, flags):
+    ce_in_child("case_ce_alltoall_tiny", n, flags)
+
+
+@pytest.mark.parametrize("n,flags", CE_SHAPES, ids=CE_IDS)
+def test_ce_alltoall_grids_and_faults_at_the_edges(n, flags):
+    ce_in_child("case_ce_alltoall_grids_and_edges", n, flags)

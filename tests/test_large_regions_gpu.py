@@ -287,6 +287,34 @@ def test_a_memcpy_every_size_and_a_word_past_2_32(pkg, op):
         assert mc.bad_sizes[0][0] == 0 and list(zip(mc.sum[0][0], mc.xr[0][0])) == want
 
 
+@pytest.mark.parametrize("op", [OP_READ, OP_WRITE], ids=["pull", "push"])
+def test_a_ce_alltoall_every_size_and_a_word_past_2_32(pkg, op):
+    """The copy-engine all-to-all's loop-back block at N = 1: every size clean; a source word past byte 2^32 fails
+    only the last size, the one that covers it, with one bad word in the warm-up and one in the timed rep and its own
+    byte offset as first_bad; restored, every size is clean again."""
+    guard(pkg, 1, A_BPP, extra=round_up(A_BPP, VMM))  # the exchange area
+    sizes = bwcurve_ref.ladder(A_BPP)
+    want = list(src_sums(0, A_BPP))
+    with open_a(pkg) as p:
+        ca = p.CeAllToAll(op, reps=2)
+        assert ca.sizes == sizes and ca.area_bytes == round_up(A_BPP, VMM) and ca.blocks == [1]
+        assert ca.cell_measured == [[True]] and ca.cell_status == [[0]] and ca.bad_sizes == [[0]]
+        assert ca.bad_words[0][0] == [0] * len(sizes) and ca.first_bad[0][0] == [U64_MAX] * len(sizes)
+        assert list(zip(ca.sum[0][0], ca.xr[0][0])) == want
+        off = (1 << 32) + 8 * 37
+        assert sizes[-2] <= off < sizes[-1]
+        p.Corrupt(0, off, 1 << 40)
+        ca = p.CeAllToAll(op, reps=1)
+        assert ca.cell_status[0][0] == ERR_INTEGRITY and ca.bad_sizes[0][0] == 1 << (len(sizes) - 1)
+        assert ca.bad_words[0][0] == [0] * (len(sizes) - 1) + [2]
+        assert ca.first_bad[0][0] == [U64_MAX] * (len(sizes) - 1) + [off]
+        assert list(zip(ca.sum[0][0], ca.xr[0][0]))[:-1] == want[:-1]
+        assert tuple(zip(ca.sum[0][0], ca.xr[0][0]))[-1] != want[-1]
+        p.Corrupt(0, off, 1 << 40)
+        ca = p.CeAllToAll(op, reps=1)
+        assert ca.bad_sizes[0][0] == 0 and list(zip(ca.sum[0][0], ca.xr[0][0])) == want
+
+
 def test_a_alltoall_row_clean_at_every_size(pkg):
     guard(pkg, 1, A_BPP, extra=round_up(A_BPP, VMM))
     sizes = bwcurve_ref.ladder(A_BPP)
@@ -510,3 +538,22 @@ def test_c_open_refuses_more_than_16_gib_and_allocates_nothing(pkg):
         assert e.value.code == pkg.abi.ERR_ARG, nbytes
     free1, _ = torch.cuda.mem_get_info(0)
     assert free1 >= free0 - (256 << 20), (free0, free1)  # others share the device: allow its own churn, not 16 GiB
+
+
+@pytest.mark.parametrize("op", [OP_READ, OP_WRITE], ids=["pull", "push"])
+def test_b_ce_alltoall_block_1_starts_past_2_32(pkg, op):
+    """Two ranks, sliced, A's 4 GiB + 8 KiB + 128 per pair, both copying at once: block 1 of each exchange area starts
+    past byte 2^32 of the area, and every block is clean at every size with its source slice's (S, X)."""
+    n = 2
+    guard(pkg, n, A_BPP, extra=round_up(n * A_BPP, VMM))
+    sizes = bwcurve_ref.ladder(A_BPP)
+    with pkg.Open(pkg.Config(ordinals=[0, 0], bytes=A_BPP, flags=SAME, ctas=8, timeout_ms=120000,
+                             link_peak_gbps=SAME_DEVICE_LINK_PEAK_GBPS)) as p:
+        ca = p.CeAllToAll(op, reps=1)
+        assert ca.sizes == sizes and ca.area_bytes == round_up(n * A_BPP, VMM)
+        assert ca.measured == [True, True] and ca.status == [0, 0] and ca.blocks == [1, 1]
+        for g, j in ((0, 1), (1, 0)):
+            src = g if op == OP_WRITE else j
+            assert ca.cell_measured[g][j] and ca.cell_status[g][j] == 0 and ca.bad_sizes[g][j] == 0, (g, j)
+            assert ca.bad_words[g][j] == [0] * len(sizes) and ca.first_bad[g][j] == [U64_MAX] * len(sizes), (g, j)
+            assert list(zip(ca.sum[g][j], ca.xr[g][j])) == list(src_sums(src, A_BPP)), (g, j)

@@ -2,10 +2,14 @@
 an output that holds the ABI version and the prologue fields the call fills before it refuses (everything else zero),
 and a call number that a refusal does not advance.  Where one call has two reasons to refuse, the one that wins is
 fixed: pingpong reports an invalid armed fault instead of its argument error, while atomics, the three all-reduces
-and all-to-all report the argument error.  Two processes refuse together: the one with invalid arguments gets its own
-message, the other is told another process was at fault, and arguments that differ refuse both."""
+and all-to-all report the argument error; memcpy and the copy-engine all-to-all refuse their reps, and the copy-engine
+all-to-all reports its reps over its op, its op over its armed fault, and all three over its hardware queues.  Two
+processes refuse together: the one with invalid arguments gets its own message, the other is told another process was
+at fault, and arguments that differ refuse both; a process without the hardware queues for the copy-engine all-to-all
+names its need and its limit, and the other is told another process cannot run it."""
 import ctypes as C
 import json
+import os
 import subprocess
 import sys
 import textwrap
@@ -35,6 +39,12 @@ FAULT_ALLREDUCE = "the armed all-reduce fault names no rank, size or output word
 FAULT_TWOSHOT = "the armed two-shot all-reduce fault names no receiver, size or output word of this call"
 FAULT_LL = "the armed LL all-reduce fault names no packet, size or delay of this call"
 FAULT_ALLTOALL = "the armed all-to-all fault names no cell, size or word of this call"
+ARGS_OP = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE"
+FAULT_CE_ALLTOALL = ("the armed copy-engine all-to-all fault names no cell, size, word or delay of this call, or has a "
+                     "mode above 2")
+QUEUES_OTHER = ("cdprobe_ce_alltoall: another process cannot run it (no stream memory operations, or more streams than "
+                "CUDA_DEVICE_MAX_CONNECTIONS)")
+ERR_UNSUPPORTED = -8
 
 
 @pytest.fixture(scope="module")
@@ -222,6 +232,44 @@ def test_ladder_calls_report_their_reps_over_an_invalid_fault(pkg, probe, what):
     ladder_refusal(pkg, probe, what, 65, ARGS_REPS, fault)
 
 
+# ---- memcpy and the copy-engine all-to-all: an op and the size ladder ------------------------------------------------
+
+def op_ladder_refusal(pkg, p, what, op, reps, message, fault=None):
+    """cdprobe_memcpy or cdprobe_ce_alltoall refused with `message`: the prologue holds n, reps and op, the call number
+    does not advance, and the next valid call runs."""
+    a = pkg.abi
+    call, raw, cls = {"memcpy": (p.Memcpy, p.memcpy_raw, a.MemcpyT),
+                      "ce_alltoall": (p.CeAllToAll, p.ce_alltoall_raw, a.CeAllToAllT)}[what]
+    seq = call(a.OP_READ, reps=1).call_seq
+    disarm = arm(p, fault)
+    rc, t = raw(op, reps)
+    check_refused(p, rc, t, message, expect(cls, n=N, reps=reps or 8, op=op))
+    disarm()
+    assert call(a.OP_WRITE, reps=1).call_seq == seq + 1
+
+
+@pytest.mark.parametrize("what", ["memcpy", "ce_alltoall"])
+def test_memcpy_and_ce_alltoall_refuse_their_reps(pkg, probe, what):
+    for op in (pkg.abi.OP_READ, pkg.abi.OP_WRITE):
+        op_ladder_refusal(pkg, probe, what, op, 65, ARGS_REPS)
+    op_ladder_refusal(pkg, probe, what, pkg.abi.OP_WRITE, 1 << 31, ARGS_REPS)
+
+
+def test_ce_alltoall_refuses_its_op_and_an_armed_fault_in_that_order(pkg, probe):
+    a = pkg.abi
+    sizes = bwcurve_ref.ladder(bpp(pkg))
+    for op in (0, 3, 4):
+        op_ladder_refusal(pkg, probe, "ce_alltoall", op, 2, ARGS_OP)
+    for fault in (a.ce_alltoall_fault(0, 0, 0, 0), a.ce_alltoall_fault(N, 0, 0, 0), a.ce_alltoall_fault(0, N, 0, 0),
+                  a.ce_alltoall_fault(0, 1, len(sizes), 0), a.ce_alltoall_fault(1, 0, 0, sizes[0] // 8),
+                  a.ce_alltoall_fault(1, 0, 0, sizes[0] // 8, mode=1), a.ce_alltoall_fault(0, 1, 0, 10_000_000, mode=2),
+                  (3 << 48) | a.ce_alltoall_fault(0, 1, 0, 0), (1 << 32) | (1 << 24), (1 << 40) | (1 << 24)):
+        op_ladder_refusal(pkg, probe, "ce_alltoall", a.OP_READ, 2, FAULT_CE_ALLTOALL, (a.OPT_CE_ALLTOALL_FAULT, fault))
+    bad = (a.OPT_CE_ALLTOALL_FAULT, a.ce_alltoall_fault(0, 0, 0, 0))
+    op_ladder_refusal(pkg, probe, "ce_alltoall", 3, 2, ARGS_OP, bad)  # the op over the fault
+    op_ladder_refusal(pkg, probe, "ce_alltoall", 3, 65, ARGS_REPS, bad)  # the reps over both
+
+
 # ---- two processes ---------------------------------------------------------------------------------------------------
 
 CHILD = textwrap.dedent(
@@ -281,3 +329,59 @@ def test_two_processes_refuse_together():
             assert differ == {"rc": ERR_ARG, "call_seq": 0,
                               "error": f"{fn} is collective: every process must call it with the same arguments"}
             assert ok == {"rc": 0, "error": "", "call_seq": 1}, (rank, name)
+
+
+QUEUES_CHILD = textwrap.dedent(
+    """
+    import json, sys
+    sys.path.insert(0, %r)
+    import cdprobe_pkg
+    m = cdprobe_pkg.load()
+    session, rank = sys.argv[1], int(sys.argv[2])
+    cfg = m.Config(ordinals=[0] * 3, bytes=1 << 20, world_size=2, rank=rank, session=session, flags=0x50, ctas=8,
+                   timeout_ms=30000)
+    out = []
+    with m.Open(cfg) as p:
+        lib = p._lib
+        for op, reps in ((m.abi.OP_WRITE, 65), (m.abi.OP_READ, 2), (m.abi.OP_WRITE, 1)):
+            rc, t = p.ce_alltoall_raw(op, reps)
+            out.append({"rc": rc, "error": lib.cdprobe_last_error().decode(), "call_seq": t.call_seq,
+                        "measured": sum(t.measured)})
+        mc = p.Memcpy(m.abi.OP_WRITE, reps=1)
+        out.append({"call_seq": mc.call_seq, "row_mask": mc.row_mask,
+                    "clean": all(mc.status[g][j] == 0 and mc.bad_sizes[g][j] == 0 for g in range(6) for j in range(6)
+                                 if mc.row_mask >> g & 1 and g != j),
+                    "measured": sum(mc.measured[g][j] for g in range(6) for j in range(6))})
+    print("RESULT " + json.dumps(out))
+    """
+) % ROOT
+
+
+def test_a_process_without_the_queues_refuses_the_copy_engine_alltoall_in_both():
+    """Two processes of three ranks each on one device (n = 6): each needs 18 hardware queues.  Process 0 has 8,
+    process 1 has 32.  Invalid reps are refused first in both, with their own text; then process 0 names its need and
+    its limit and process 1 is told another process cannot run it.  Nothing advances, and memcpy then runs clean."""
+    session = f"refuse-q-{uuid.uuid4().hex[:12]}"
+    procs = [subprocess.Popen([sys.executable, "-c", QUEUES_CHILD, session, str(r)], stdout=subprocess.PIPE,
+                              stderr=subprocess.PIPE, text=True,
+                              env=dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS=str(limit)))
+             for r, limit in enumerate((8, 32))]
+    outs = []
+    try:
+        for pr in procs:
+            so, se = pr.communicate(timeout=600)
+            assert pr.returncode == 0, se[-2000:]
+            outs.append(json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][7:]))
+    finally:
+        for pr in procs:
+            if pr.poll() is None:
+                pr.kill()
+                pr.wait()
+    own = "cdprobe_ce_alltoall: needs 18 queues on ordinal 0, CUDA_DEVICE_MAX_CONNECTIONS allows 8"
+    for rank, o in enumerate(outs):
+        reps, first, second, mc = o
+        assert reps == {"rc": ERR_ARG, "error": ARGS_REPS, "call_seq": 0, "measured": 0}, (rank, reps)
+        for got in (first, second):
+            assert got == {"rc": ERR_UNSUPPORTED, "error": own if rank == 0 else QUEUES_OTHER, "call_seq": 0,
+                           "measured": 0}, (rank, got)
+        assert mc == {"call_seq": 1, "row_mask": 0b111 << (3 * rank), "clean": True, "measured": 3 * 5}, (rank, mc)

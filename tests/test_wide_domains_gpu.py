@@ -36,7 +36,9 @@ import allreduce_ref
 import alltoall_ref
 import atomics_ref
 import bwcurve_ref
+import ce_alltoall_ref
 import handle_model as hm
+import test_ce_alltoall_gpu as ce_test
 import latency_ref
 import memcpy_ref
 import pingpong_ref
@@ -427,6 +429,23 @@ def case_measurements(pkg, oracle, n, flags):
                 assert_bwcurve_clean(bw, oracle, bpp, diag, skip={(i, j)})
                 p.Corrupt(j, base + o, 1 << 17)
             assert_bwcurve_clean(p.BwCurve(reps=BW_REPS), oracle, bpp, diag)
+        # the copy-engine all-to-all: n ranks on one device need n x n streams (n x (n + 1) with the loop-back),
+        # 81, 225 and 272 of the 32 this process has: refused with the need named, advancing nothing, and memcpy
+        # then runs clean on the handle
+        need, ordinal = ce_alltoall_ref.queues(n, diag, [0] * n)
+        assert (n, need, ordinal) in ((9, 81, 0), (15, 225, 0), (16, 272, 0))
+        for op in (pkg.abi.OP_READ, pkg.abi.OP_WRITE):
+            rc, t = p.ce_alltoall_raw(op, 2)
+            assert rc == ERR_UNSUPPORTED and t.call_seq == 0 and sum(t.measured) == 0, rc
+            assert p._lib.cdprobe_last_error().decode() == \
+                "cdprobe_ce_alltoall: " + ce_alltoall_ref.queue_message(need, 0, 32)
+        mc = p.Memcpy(pkg.abi.OP_WRITE, reps=1)
+        assert mc.call_seq == 1 and mc.sizes == bwcurve_ref.ladder(bpp)
+        for g, j in ce_alltoall_ref.cells(n, diag):
+            cell = memcpy_ref.cell(n, bpp, 1, pkg.abi.OP_WRITE, g, j)
+            assert mc.measured[g][j] and mc.status[g][j] == 0 and mc.bad_sizes[g][j] == 0, (g, j)
+            assert list(zip(mc.sum[g][j], mc.xr[g][j])) == \
+                [tuple(e) for e in memcpy_ref.expected(oracle, SEED, cell, mc.sizes)], (g, j)
         r = p.Run()  # the measurements disturbed nothing
         check_run(pkg, oracle, p, cfg, r, n, flags, 1)
 
@@ -522,6 +541,11 @@ def mp_process(pkg, session, rank, world, n_local, what):
                         ("push", p.AllReducePush)):
             out[key] = fields(fn(reps=2))
         out["mc"] = [fields(p.Memcpy(op, reps=2)) for op in (pkg.abi.OP_READ, pkg.abi.OP_WRITE)]
+        out["ce"] = []
+        for op in (pkg.abi.OP_READ, pkg.abi.OP_WRITE):
+            rc, t = p.ce_alltoall_raw(op, 2)
+            out["ce"].append({"rc": rc, "error": p._lib.cdprobe_last_error().decode() if rc else "",
+                              **({} if rc else ce_test.as_dict(pkg.CeAllToAll.from_c(t)))})
         # a landing fault armed in process 0 on a cell whose target lives in the last process
         W = info.bytes_per_pair // 8
         if rank == 0:
@@ -540,9 +564,13 @@ def mp_process(pkg, session, rank, world, n_local, what):
 
 
 def run_processes(world, n_local, what, timeout=900):
+    """The processes of the "full" case have 32 hardware queues per device, so the copy-engine all-to-all runs up to 32
+    streams on one; the others keep the runtime's default."""
     session = f"wd-{uuid.uuid4().hex[:12]}"
+    env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32") if what == "full" else None
     procs = [subprocess.Popen([sys.executable, "-c", MP_CHILD, session, str(r), str(world), str(n_local), what],
-                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True) for r in range(world)]
+                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, env=env)
+             for r in range(world)]
     outs = []
     for pr in procs:
         so, se = pr.communicate(timeout=timeout)
@@ -668,6 +696,20 @@ def test_processes_with_several_ranks_each(pkg, oracle, world, n_local):
                         assert mc["status"][g][d] == 0 and mc["bad_words"][g][d] == [0] * len(sizes), (g, d)
                         assert [[s, x] for s, x in zip(mc["sum"][g][d], mc["xr"][g][d])] == \
                             [list(e) for e in memcpy_ref.expected(oracle, SEED, cell, sizes)], (mc["op"], g, d)
+        # the copy-engine all-to-all: n_local x n streams per process on one device.  2 x 8 needs 128 of 32 and is
+        # refused in both processes, each naming its own need; 2 x 4 runs at exactly 32 and 3 x 3 at 27, every block
+        # checked by its owner's process and clean
+        need, _ = ce_alltoall_ref.queues(n, False, [0] * n_local)
+        assert need == n_local * n
+        for call, ce in enumerate(o["ce"], 1):
+            if need > 32:
+                assert ce == {"rc": ERR_UNSUPPORTED, "error": "cdprobe_ce_alltoall: " +
+                              ce_alltoall_ref.queue_message(need, 0, 32)}, ce
+                continue
+            assert ce["rc"] == 0 and ce["call_seq"] == call and ce["row_mask"] == rows, ce["rc"]
+            ce_test.check_call(ce, oracle, W * 8, 1, False)
+            for g, j in ce_alltoall_ref.cells(n, False):
+                assert ce["cell_measured"][g][j] == (ce_alltoall_ref.owner(ce["op"], g, j) in mine), (g, j)
         # the landing fault of process 0 fails exactly its cell, in every process's gathered result
         f = AsResult(o["faulted"])
         want_w = [[0 if (a, b) == (0, n - 1) else 1 for b in range(n)] for a in range(n)]
