@@ -7,8 +7,9 @@ tests/bwcurve_ref.py, tests/allreduce_ref.py, the all-reduce protocol references
 allreduce_ll_ref, allreduce_ring_ref, allreduce_push_ref), tests/alltoall_ref.py, tests/memcpy_ref.py and
 tests/ce_alltoall_ref.py, never from the library.  It tracks:
 
-- the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, the five all-reduces (one-shot, two-shot, LL,
-  ring, push), alltoall, memcpy and the copy-engine all-to-all (a refused call advances none);
+- the counters: run_seq and the call_seq of pingpong, atomics, bwcurve, the six all-reduces (one-shot, two-shot, LL,
+  ring, push, NVLS), alltoall, memcpy and the copy-engine all-to-all (a refused call advances none); the NVLS call as
+  it behaves where ranks share a device or a single rank's object is refused, so it runs nothing;
 - each process's hardware queues per device, against which the copy-engine all-to-all is refused;
 - the armed fault of each of those ladder measurements in each process's handle; which pairs were unmapped when the
   exchange area (shared by the all-to-all, memcpy and the copy-engine all-to-all, built by whichever is called first)
@@ -159,6 +160,11 @@ class HandleModel:
         # the ordinals the handle was opened with
         self.cea_calls = 0
         self.cea_fault: Dict[int, int] = {}
+        # the NVLS all-reduce: its calls, its armed fault (CDPROBE_OPT_ALLREDUCE_NVLS_FAULT) per process, and whether
+        # the driver refuses a multicast object of one device (the caller sets it from a one-rank call where it matters)
+        self.nvls_calls = 0
+        self.nvls_fault: Dict[int, int] = {}
+        self.one_device_nvls_refused = True
         limit = max_connections(os.environ)
         self.max_connections: Dict[int, int] = {p: limit for p in range(n // len(self.local))}
         self.ordinal: Dict[int, int] = {}
@@ -590,6 +596,49 @@ class HandleModel:
                 self._ar_set(words, unit.start, unit.stop, lambda w, v: v + sign * int(x[w - unit.start]))
 
         return self._allreduce("push", reps, sizes, decode, effect)
+
+    def nvls_modelled(self) -> bool:
+        """Whether the domain cannot form a multicast object, which is all allreduce_nvls models: two ranks share a
+        device (by ordinal; a team holds each device once), or one rank whose one-device object the driver refuses."""
+        if self.n == 1:
+            return self.one_device_nvls_refused
+        ordinals = [self.ordinal.get(g, 0) for g in range(self.n)]
+        return len(set(ordinals)) < len(ordinals)
+
+    def allreduce_nvls(self, reps: int, proc: int = 0):
+        """What cdprobe_allreduce_nvls with `reps` timed reps must return in process `proc`, on a domain that cannot
+        form a multicast object: every rank on one device (a team holds each device once), or one rank, whose
+        one-device object the driver refuses.  A refused call returns CDPROBE_ERR_ARG with the text cdprobe_last_error
+        then holds, which this returns, and advances nothing.  The refusals come in this order: reps above 64, then this
+        process's armed fault (a mode above 1, bits 32 to 47 set, no size of the ladder, no word of its size), then
+        another process's.  Otherwise the call advances its own call_seq and every local row reports
+        CDPROBE_ERR_UNSUPPORTED, unmeasured, whatever the mappings: no NVLS area is built and nothing else changes.
+        A domain that can form the object (nvls_modelled false) runs the kernel, which this does not model."""
+        assert self.nvls_modelled(), "the NVLS call runs on this domain; the model covers only domains that refuse it"
+        sizes = bwcurve_ref.ladder(self.bpp)
+        if reps > 64:
+            return "reps must be at most 64"
+
+        def refusal(v):
+            fk, word = (v >> 24) & 0xFF, v & 0xFFFFFF
+            if v >> 48 > 1:
+                return "the armed NVLS all-reduce fault has a mode above 1"
+            if (v >> 32) & 0xFFFF:
+                return "the armed NVLS all-reduce fault sets bits 32 to 47, which name nothing"
+            if fk == 0 or fk > len(sizes):
+                return "the armed NVLS all-reduce fault names no size of this call"
+            if word >= sizes[fk - 1] // 8:
+                return "the armed NVLS all-reduce fault names no output word of its size"
+            return None
+
+        why = {p: refusal(v) for p, v in self.nvls_fault.items()}
+        if why.get(proc):
+            return why[proc]
+        if any(why.values()):
+            return "another process called cdprobe_allreduce_nvls with invalid arguments"
+        self.nvls_calls += 1
+        return dict(call_seq=self.nvls_calls, sizes=sizes,
+                    rows={g: dict(measured=False, status=ERR_UNSUPPORTED) for g in self.local})
 
     def build_area(self) -> None:
         """The exchange area, built by the first all-to-all, memcpy or copy-engine all-to-all call that is not

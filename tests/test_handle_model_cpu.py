@@ -915,3 +915,94 @@ def test_ce_alltoall_down_rule_counters_and_the_sticky_area(oracle):
     assert (m.cea_calls, m.a2a_calls, m.mc_calls) == (3, 1, 2)
     assert m.ce_alltoall(3, 1) == hm.ERR_ARG and m.ce_alltoall(hm.OP_READ, 2)["call_seq"] == 4
     assert (m.cea_calls, m.a2a_calls, m.mc_calls) == (4, 1, 2)
+
+
+NVLS_TEXTS = {"reps": "reps must be at most 64",
+              "mode": "the armed NVLS all-reduce fault has a mode above 1",
+              "bits": "the armed NVLS all-reduce fault sets bits 32 to 47, which name nothing",
+              "size": "the armed NVLS all-reduce fault names no size of this call",
+              "word": "the armed NVLS all-reduce fault names no output word of its size",
+              "other": "another process called cdprobe_allreduce_nvls with invalid arguments"}
+
+
+def test_allreduce_nvls_refusals_in_their_order_with_their_texts(oracle):
+    """Reps first, then the fault's mode, its unused bits, its size and its word; a refused call advances nothing."""
+    m = hm.HandleModel(oracle, no_schedule, 3, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    K = len(sizes)
+    word_past = (K << 24) | sizes[-1] // 8
+    for v, want in (((2 << 48) | (1 << 32) | ((K + 1) << 24) | word_past, "mode"),
+                    ((1 << 63) | (1 << 24), "mode"),
+                    ((1 << 48) | (1 << 32) | ((K + 1) << 24), "bits"),
+                    ((1 << 47) | (1 << 24), "bits"),
+                    (((K + 1) << 24) | 0xFFFFFF, "size"),
+                    (5, "size"),
+                    (word_past, "word"),
+                    ((1 << 48) | (1 << 24) | sizes[0] // 8, "word")):
+        m.arm_measure(m.nvls_fault, 0, v)
+        assert m.allreduce_nvls(65) == NVLS_TEXTS["reps"], hex(v)
+        assert m.allreduce_nvls(2) == NVLS_TEXTS[want], hex(v)
+    assert m.nvls_calls == 0
+    m.arm_measure(m.nvls_fault, 0, (1 << 48) | (K << 24) | (sizes[-1] // 8 - 1))  # the last word: accepted
+    assert m.allreduce_nvls(2)["call_seq"] == 1
+    m.arm_measure(m.nvls_fault, 0, 0)
+    assert m.allreduce_nvls(0)["call_seq"] == 2 and m.allreduce_nvls(64)["call_seq"] == 3
+
+
+def test_allreduce_nvls_a_bad_fault_in_another_process_refuses_with_its_own_text(oracle):
+    sizes = bwcurve_ref.ladder(hm.HandleModel(oracle, no_schedule, 4, 3 << 20, sm_count=132).bpp)
+    for me in (0, 1):
+        m = hm.HandleModel(oracle, no_schedule, 4, 3 << 20, sm_count=132, local=range(2 * me, 2 * me + 2))
+        m.arm_measure(m.nvls_fault, 1, (1 << 24) | sizes[0] // 8)  # process 1's: one word past size 0
+        m.arm_measure(m.nvls_fault, 0, 1 << 24)                    # process 0's: word 0, valid
+        assert m.allreduce_nvls(1, proc=me) == (NVLS_TEXTS["word"] if me == 1 else NVLS_TEXTS["other"])
+        m.arm_measure(m.nvls_fault, 0, 2 << 48)                    # now both bad: each names its own
+        assert m.allreduce_nvls(1, proc=me) == (NVLS_TEXTS["word"] if me == 1 else NVLS_TEXTS["mode"])
+        m.arm_measure(m.nvls_fault, 1, 0)
+        m.arm_measure(m.nvls_fault, 0, 0)
+        got = m.allreduce_nvls(1, proc=me)
+        assert got["call_seq"] == 1 and set(got["rows"]) == set(m.local)
+
+
+def test_allreduce_nvls_runs_nothing_advances_only_its_own_counter_and_builds_nothing(oracle):
+    """Every local row is unmeasured with CDPROBE_ERR_UNSUPPORTED, whether or not a pair is down, a word is corrupted
+    or a valid fault is armed; no area is built and no other counter moves."""
+    m = hm.HandleModel(oracle, no_schedule, 3, 1 << 20, sm_count=132)
+    sizes = bwcurve_ref.ladder(m.bpp)
+    want_rows = {g: dict(measured=False, status=hm.ERR_UNSUPPORTED) for g in range(3)}
+    seq = 0
+    for step in ("clean", "corrupt", "unmap", "fault", "remap"):
+        if step == "corrupt":
+            m.corrupt_word(1, 5, 1 << 9)
+        elif step == "unmap":
+            m.unmapped.add((2, 0))
+        elif step == "fault":
+            m.arm_measure(m.nvls_fault, 0, (1 << 48) | (len(sizes) << 24))
+        elif step == "remap":
+            m.unmapped.clear()
+        seq += 1
+        assert m.allreduce_nvls(1) == dict(call_seq=seq, sizes=sizes, rows=want_rows), step
+    assert (m.ar_calls, m.ts_calls, m.ll_calls, m.ring_calls, m.push_calls, m.a2a_calls, m.mc_calls,
+            m.cea_calls) == (0,) * 8
+    assert m.area_down is None and all(v is None for v in m.ar_area_down.values())
+    assert m.allreduce(1)["call_seq"] == 1 and m.nvls_calls == 5
+    m1 = hm.HandleModel(oracle, no_schedule, 1, 1 << 20, sm_count=132)
+    assert m1.allreduce_nvls(3)["rows"] == {0: dict(measured=False, status=hm.ERR_UNSUPPORTED)}
+
+
+def test_allreduce_nvls_is_modelled_only_where_the_domain_cannot_form_a_multicast_object(oracle):
+    """Ranks that share a device, or one rank whose one-device object the driver refuses: the call runs nothing.  One
+    rank per device, or one rank the driver accepts, runs the kernel, which the model does not cover."""
+    m = hm.HandleModel(oracle, no_schedule, 4, 3 << 20, sm_count=132)
+    assert m.nvls_modelled()  # every rank on ordinal 0
+    m.ordinal.update({0: 0, 1: 1, 2: 2, 3: 1})
+    assert m.nvls_modelled()  # ranks 1 and 3 share a device
+    m.ordinal[3] = 3
+    assert not m.nvls_modelled()
+    with pytest.raises(AssertionError):
+        m.allreduce_nvls(1)
+    assert m.nvls_calls == 0
+    m1 = hm.HandleModel(oracle, no_schedule, 1, 1 << 20, sm_count=132)
+    assert m1.nvls_modelled()
+    m1.one_device_nvls_refused = False
+    assert not m1.nvls_modelled()

@@ -10,17 +10,23 @@ one handle through many calls and compares the whole output of each call with th
   the verdict restatement (verdict_ref), the traced phase kinds and peers, and `warmed`;
 - Diagnose: the word_ref report of every cell, field for field, from the issuer and from the target;
 - Latency: status and digest; BwCurve: bad_sizes and (S, X) per size; PingPong and Atomics: clean cells, call_seq;
-- the five all-reduces (AllReduce, AllReduceTwoShot, AllReduceLL, AllReduceRing, AllReducePush): per row measured,
-  status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest, each protocol's armed
-  faults (drop and unstored modes included), the skip rule (any down pair stops every rank) and each area's sticky
-  rule; AllToAll: per rank measured and blocks, per cell status, bad_sizes and per size bad_words, first_bad and
-  (S, X), under armed faults and the sticky exchange-area rule; Memcpy, both ops: per cell measured, status, bad_sizes
-  and per size bad_words, first_bad and (S, X), under corruptions at rest, armed faults and the exchange area it shares
-  with the all-to-all; the copy-engine all-to-all, both ops: per rank measured, status and blocks, per cell status,
-  bad_sizes and per size bad_words, first_bad and (S, X) where its owner is local, under corruptions at rest, armed
-  flips, drops and holds, its all-or-nothing down rule, the shared exchange area and the hardware-queue refusal (walks
-  with N = 3 and 5 ranks on one device see it refused at 8 queues, and run it in a child process with 32); all with
-  call_seq, the ladder and the path (the LL and the ring report their own) or area_bytes;
+- the five all-reduces that run on one GPU (AllReduce, AllReduceTwoShot, AllReduceLL, AllReduceRing, AllReducePush):
+  per row measured, status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest, each
+  protocol's armed faults (drop and unstored modes included), the skip rule (any down pair stops every rank) and each
+  area's sticky rule; AllToAll: per rank measured and blocks, per cell status, bad_sizes and per size bad_words,
+  first_bad and (S, X), under armed faults and the sticky exchange-area rule; Memcpy, both ops: per cell measured,
+  status, bad_sizes and per size bad_words, first_bad and (S, X), under corruptions at rest, armed faults and the
+  exchange area it shares with the all-to-all; the copy-engine all-to-all, both ops: per rank measured, status and
+  blocks, per cell status, bad_sizes and per size bad_words, first_bad and (S, X) where its owner is local, under
+  corruptions at rest, armed flips, drops and holds, its all-or-nothing down rule, the shared exchange area and the
+  hardware-queue refusal (walks with N = 3 and 5 ranks on one device see it refused at 8 queues, and run it in a child
+  process with 32); all with call_seq, the ladder and the path (the LL, the ring and the NVLS call report their own)
+  or area_bytes;
+- the NVLS all-reduce (AllReduceNVLS) with its fault option armed, where the domain cannot form a multicast object
+  (ranks sharing a device, or one rank whose one-device object the driver refuses, asked once per process): it runs
+  nothing, every row reports CDPROBE_ERR_UNSUPPORTED, its own call_seq advances, and its refusals name their reasons.
+  On a domain that can form the object (the walk over real peers) the call runs the kernel, which the model does not
+  cover, so no walk draws it there;
 - refused calls: the error code, and nothing they may not change.
 
 A divergence fails with the seed, the step index and every step so far; the walk is generated from the seed and the
@@ -29,6 +35,7 @@ rank's persistent kernel stays resident), so the file runs on one H100.  No step
 timeout or touches more than 4 GiB.
 """
 import ctypes as C
+import functools
 import json
 import os
 import random
@@ -67,13 +74,29 @@ LADDER_REPS = 1  # the ladder measurements fold timed rep 1, the faulted one, in
 FAULTS = {"OPT_ALLREDUCE_FAULT": "ar_fault", "OPT_ALLREDUCE_TWOSHOT_FAULT": "ts_fault",
           "OPT_ALLREDUCE_LL_FAULT": "ll_fault", "OPT_ALLREDUCE_RING_FAULT": "ring_fault",
           "OPT_ALLREDUCE_PUSH_FAULT": "push_fault", "OPT_ALLTOALL_FAULT": "a2a_fault", "OPT_MEMCPY_FAULT": "mc_fault",
-          "OPT_CE_ALLTOALL_FAULT": "cea_fault"}
+          "OPT_CE_ALLTOALL_FAULT": "cea_fault", "OPT_ALLREDUCE_NVLS_FAULT": "nvls_fault"}
 # each all-reduce step: the model's method, the raw binding and the path it reports (None: the handle's)
 ALLREDUCES = {"allreduce": ("allreduce", "allreduce_raw", None), "twoshot": ("twoshot", "allreduce_twoshot_raw", None),
               "ll": ("ll", "allreduce_ll_raw", 3), "ring": ("ring", "allreduce_ring_raw", 4),
-              "push": ("push", "allreduce_push_raw", None)}
-LADDER_CALLS = [("allreduce",), ("twoshot",), ("ll",), ("ring",), ("push",), ("alltoall",), ("memcpy", 1),
+              "push": ("push", "allreduce_push_raw", None), "nvls": ("allreduce_nvls", "allreduce_nvls_raw", 5)}
+LADDER_CALLS = [("allreduce",), ("twoshot",), ("ll",), ("ring",), ("push",), ("nvls",), ("alltoall",), ("memcpy", 1),
                 ("memcpy", 2), ("ce_alltoall", 1), ("ce_alltoall", 2)]
+
+
+def ladder_calls(m):
+    """LADDER_CALLS without the NVLS call where it would run: the model covers it only on a domain that cannot form a
+    multicast object (HandleModel.nvls_modelled)."""
+    return [c for c in LADDER_CALLS if c != ("nvls",) or m.nvls_modelled()]
+
+
+@functools.lru_cache(maxsize=None)
+def one_device_nvls_refused(pkg, ordinal):
+    """Whether a one-rank cdprobe_allreduce_nvls on `ordinal` runs nothing (CDPROBE_ERR_UNSUPPORTED): the device has no
+    multicast, or its driver refuses a multicast object of one device.  Asked once, on a handle of its own."""
+    with pkg.Open(pkg.Config(ordinals=[ordinal], bytes=1 << 20, ctas=8, timeout_ms=20000)) as p:
+        ar = p.AllReduceNVLS(reps=1)
+    assert ar.measured[0] or ar.status[0] == hm.ERR_UNSUPPORTED, ar.status
+    return not ar.measured[0]
 
 
 class Refused(Exception):
@@ -94,6 +117,8 @@ class Driver:
         # every process of these tests opens its ranks on the same ordinals, so global rank g sits on ordinal
         # cfg.ordinals[g % n_local] (the copy-engine all-to-all counts hardware queues per device)
         self.m.ordinal.update({g: cfg.ordinals[g % self.n_local] for g in range(n)})
+        if n == 1:
+            self.m.one_device_nvls_refused = one_device_nvls_refused(pkg, cfg.ordinals[0])
         self.gate = pkg.gate(cfg, n)
         self.area_bytes = None  # of the exchange area, once the all-to-all or memcpy has reported it
         self.check_info()
@@ -196,10 +221,12 @@ class Driver:
     def check_allreduce(self, kind="allreduce"):
         a, m = self.a, self.m
         model, raw, path = ALLREDUCES[kind]
-        want = getattr(m, model)(LADDER_REPS)
+        want = getattr(m, model)(LADDER_REPS, proc=self.me) if kind == "nvls" else getattr(m, model)(LADDER_REPS)
         rc, t = getattr(self.p, raw)(LADDER_REPS)
-        if want is None:  # the armed fault names no rank, size or word of the ladder: refused, nothing advances
-            assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)
+        if want is None or isinstance(want, str):  # the armed fault names nothing of the ladder: refused, nothing
+            assert rc == a.ERR_ARG and t.call_seq == 0 and sum(t.measured) == 0, (rc, t.call_seq)  # advances
+            if isinstance(want, str):  # the NVLS call's refusal names its reason
+                assert self.p._lib.cdprobe_last_error().decode() == want
             return
         assert rc == a.OK, rc
         ar = self.pkg.AllReduce.from_c(t)
@@ -439,7 +466,8 @@ def ladder_fault(rng, m, name, rank, peer):
     `rank`, xor 1 or drop; OPT_ALLREDUCE_LL_FAULT, a corrupted packet rank -> peer, or a word `rank` never stores;
     OPT_ALLREDUCE_RING_FAULT, a corrupted or dropped push by `rank` in a phase that pushes the word (at N = 1, where
     nothing is pushed, a 5 us delay); OPT_ALLREDUCE_PUSH_FAULT, modes 0-2 by sender `rank` or mode 3 to receiver
-    `rank`; OPT_ALLTOALL_FAULT on block rank -> peer; OPT_MEMCPY_FAULT on cell rank -> peer, flipped or dropped;
+    `rank`; OPT_ALLREDUCE_NVLS_FAULT, xor 1 or a skipped unit, by the word's owner; OPT_ALLTOALL_FAULT on block
+    rank -> peer; OPT_MEMCPY_FAULT on cell rank -> peer, flipped or dropped;
     OPT_CE_ALLTOALL_FAULT on cell rank -> peer, flipped, dropped or held."""
     n = m.n
     sizes = allreduce_ll_ref.ladder(m.bpp) if name == "OPT_ALLREDUCE_LL_FAULT" else bwcurve_ref.ladder(m.bpp)
@@ -467,6 +495,8 @@ def ladder_fault(rng, m, name, rank, peer):
         if mode == 3 and (n == 1 or allreduce_push_ref.word_owner(sizes[k], n, word) == rank):
             mode = rng.randrange(3)
         return (mode << 48) | ((rank + 1) << 32) | low
+    if name == "OPT_ALLREDUCE_NVLS_FAULT":  # no rank field: the word's owner acts on it
+        return (drop << 48) | low
     if name == "OPT_MEMCPY_FAULT":
         return (drop << 48) | ((rank + 1) << 40) | ((peer + 1) << 32) | low
     if name == "OPT_CE_ALLTOALL_FAULT":  # a flip, a dropped copy, or a hold of at most 1 ms
@@ -486,13 +516,14 @@ def past_its_size(m, name, value):
 def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
     """One step drawn from `rng` and the model's state alone (never from a device result).  `ctas_cap` bounds the
     grids it may ask for, so that many same-device ranks stay resident together.  A sixth of the steps are calls of the
-    seven ladder collectives (the five all-reduces, the all-to-all and memcpy with either op, each about as often as
+    ladder collectives (the six all-reduces where ladder_calls keeps the NVLS call, the all-to-all, memcpy and the
+    copy-engine all-to-all with either op, each about as often as
     bwcurve) and their fault armings; the rest keep their weights."""
     n, W = m.n, m.W
     grids = [c for c in (1, 2, 3, 7, 8) if ctas_cap is None or c <= ctas_cap]
     x = rng.random()
     if x < 0.12:
-        return rng.choice(LADDER_CALLS)
+        return rng.choice(ladder_calls(m))
     if x < 0.16:
         name = rng.choice(sorted(FAULTS))
         if getattr(m, FAULTS[name]) and rng.random() < 0.4:
@@ -502,6 +533,8 @@ def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
         value = ladder_fault(rng, m, name, i, j)
         if rng.random() < 0.15:  # one word past its size: the next call is refused until the fault is re-armed
             value = past_its_size(m, name, value)
+        elif name == "OPT_ALLREDUCE_NVLS_FAULT" and rng.random() < 0.1:  # a mode above 1, or bits that name nothing
+            value |= rng.choice([2 << 48, 1 << 32])
         return ("opt", name, value)
     x = (x - 0.16) / 0.84
     if x < 0.28:
@@ -561,10 +594,10 @@ def gen_step(rng, m, same_device=True, two_procs=False, me=0, ctas_cap=None):
 
 
 def walk_step(rng, m, steps, **kw):
-    """The next step of a walk: right after an unmap or a remap, a call of one of the seven ladder collectives, so that
+    """The next step of a walk: right after an unmap or a remap, a call of one of the ladder collectives (ladder_calls), so that
     every walk with churn calls them while a pair is down and after a remap; else gen_step's."""
     if steps and steps[-1][0] in ("unmap", "remap"):
-        return rng.choice(LADDER_CALLS)
+        return rng.choice(ladder_calls(m))
     return gen_step(rng, m, **kw)
 
 
@@ -580,7 +613,7 @@ def walk(drv, seed, n_steps, **kw):
             raise AssertionError(f"seed {seed}: step {k} {step!r} diverged from the model: {e!r}\n"
                                  f"steps so far: {steps!r}") from e
     # remap what is still down, so that every walk with churn also calls the ladder measurements after a remap
-    closing = [("remap",) + c for c in sorted(drv.m.unmapped)] + LADDER_CALLS + [("run",), ("diagnose",)]
+    closing = [("remap",) + c for c in sorted(drv.m.unmapped)] + ladder_calls(drv.m) + [("run",), ("diagnose",)]
     drv.play(closing, f"seed {seed}: closing run")
     return steps + closing
 
@@ -891,7 +924,7 @@ def two_proc_steps(seed, n_steps, m):
         x = rng.random()
         if x < 0.35:
             out.append(("all", rng.choice([("run",), ("run",), ("pingpong", rng.randrange(2)), ("bwcurve",)]
-                                          + LADDER_CALLS)))
+                                          + ladder_calls(m))))
             mutating = rng.random() < 0.5
             continue
         if x < 0.5:
