@@ -690,20 +690,17 @@ static void destroy(cdprobe* h) {
     if (L.scratch) cudaFree(L.scratch);
     if (L.ev0) cudaEventDestroy(L.ev0);
     if (L.ev1) cudaEventDestroy(L.ev1);
-    for (cudaEvent_t ev : L.memcpy_ev)
-      if (ev) cudaEventDestroy(ev);
     for (uint32_t i = 0; i < (uint32_t)kMaxRanks; ++i) {
       if (L.cea_stream[i]) cudaStreamSynchronize(L.cea_stream[i]);
       for (cudaEvent_t ev : L.cea_copy_ev[i])
         if (ev) cudaEventDestroy(ev);
       if (L.cea_stream[i]) cudaStreamDestroy(L.cea_stream[i]);
     }
-    for (cudaEvent_t ev : L.cea_ev)
+    for (cudaEvent_t ev : L.rep_ev)
       if (ev) cudaEventDestroy(ev);
     if (L.stream) cudaStreamDestroy(L.stream);
   }
-  if (h->memcpy_host) cudaFreeHost(h->memcpy_host);
-  if (h->cea_host) cudaFreeHost(h->cea_host);
+  if (h->copy_host) cudaFreeHost(h->copy_host);
   delete h->links;
   h->rdv.close();
   delete h;

@@ -17,8 +17,7 @@
 
 namespace cdp {
 
-struct MemcpyHost;
-struct CeA2aHost;
+struct CopyHost;
 struct LinkCounters;
 
 inline thread_local std::string g_last_error;
@@ -50,12 +49,12 @@ struct LocalRank {
   uint32_t peer_mask = 0;
   void* scratch = nullptr;  // device output of the on-demand measurements (measure.cc), grown on demand
   size_t scratch_bytes = 0;
-  cudaEvent_t memcpy_ev[2 * kRepSlots] = {};  // cdprobe_memcpy, made on first use: rep r's copy is [2r] to [2r + 1]
+  // cdprobe_memcpy and cdprobe_ce_alltoall, made on the first call of either: rep r is timed from [2r] to [2r + 1]
+  cudaEvent_t rep_ev[2 * kRepSlots] = {};
   // cdprobe_ce_alltoall, made on its first call and kept until close: one copy stream per cell the rank issues, each
-  // with the events of its copy ([0] to [1]) and of its join ([2]); events A and B of a rep on `stream`
+  // with the events of its copy ([0] to [1]) and of its join ([2])
   cudaStream_t cea_stream[kMaxRanks] = {};
   cudaEvent_t cea_copy_ev[kMaxRanks][3] = {};
-  cudaEvent_t cea_ev[2] = {};
 };
 
 // One allocation per local rank, shared with the whole domain: each process creates its local ranks' allocations,
@@ -155,12 +154,11 @@ struct cdprobe {
   uint64_t nvls_fault = 0;    // CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value, 0: disarmed
   uint64_t memcpy_calls = 0;  // cdprobe_memcpy calls that ran (call_seq of the last one)
   uint64_t memcpy_fault = 0;  // CDPROBE_OPT_MEMCPY_FAULT value, 0: disarmed
-  cdp::MemcpyHost* memcpy_host = nullptr;  // cdprobe_memcpy's pinned host block (measure.cc), made on first use:
-                                          // the ticket its streams wait on and what its checks leave
-  uint64_t memcpy_tickets = 0;        // tickets handed out so far
   uint64_t cea_calls = 0;             // cdprobe_ce_alltoall calls that ran (call_seq of the last one)
   uint64_t cea_fault = 0;             // CDPROBE_OPT_CE_ALLTOALL_FAULT value, 0: disarmed
-  cdp::CeA2aHost* cea_host = nullptr;  // cdprobe_ce_alltoall's pinned host block (measure.cc), made on first use
+  // the pinned host block of cdprobe_memcpy and cdprobe_ce_alltoall (measure.cc), made by the first call of either:
+  // the tickets their streams wait on and what their checks leave
+  cdp::CopyHost* copy_host = nullptr;
   uint32_t max_connections = 8;       // CUDA_DEVICE_MAX_CONNECTIONS as read at open: hardware queues per device
   char rank_uuid[cdp::kMaxRanks][48] = {};  // every rank's device UUID, exchanged at open (cdprobe_links' payload)
   bool link_counters = false;               // CDPROBE_OPT_LINK_COUNTERS

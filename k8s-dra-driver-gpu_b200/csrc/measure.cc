@@ -495,6 +495,14 @@ static int walk_rounds(cdprobe* h, const bool (*runs)[kMaxRanks], const Round& r
   return CDPROBE_OK;
 }
 
+// Folds area m's mapping status into the domain's mapping status st ([rank][rank]): a cell whose probe mapping is up
+// gets its mapping of m.
+static void fold_area_status(const cdprobe* h, const SharedAlloc& m, int32_t (*st)[kMaxRanks]) {
+  for (uint32_t s = 0; s < h->n_total; ++s)
+    for (uint32_t d = 0; d < h->n_total; ++d)
+      if (st[s][d] == 0) st[s][d] = m.status[s][d];
+}
+
 // The skip rule of the all-reduces, on the domain's mapping status st ([rank][rank], 0: up): a process that ran while
 // another skipped would wait at the first domain barrier until its watchdog fired, so when some rank cannot reach some
 // other nothing runs, in any process: every local row gets the status of the domain's first down cell, row-major.
@@ -823,10 +831,7 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   put_ladder(h, lad, out);
   // 3. every rank reads every input and writes every area: when some probe mapping or area mapping of the domain is
   //    down, nothing runs, in any process
-  if (m != nullptr)
-    for (uint32_t s = 0; s < n; ++s)
-      for (uint32_t d = 0; d < n; ++d)
-        if (st[s][d] == 0) st[s][d] = m->status[s][d];
+  if (m != nullptr) fold_area_status(h, *m, st);
   if (skip_rows(h, st, out)) {
     out->ms = now_ms() - lad.t_begin;
     return CDPROBE_OK;
@@ -895,18 +900,9 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   return CDPROBE_OK;
 }
 
-constexpr uint32_t kMemcpyDefaultReps = 8;
-
-// cdprobe_memcpy's armed fault once the call has accepted it: timed rep 1 of size k of cell (issuer, target) flips
-// destination word `word` (mode 0) or queues no copy (mode 1).  issuer kMaxRanks: none.
-struct MemcpyFault {
-  uint32_t issuer = kMaxRanks, target = 0, k = 0, mode = 0;
-  uint64_t word = 0;
-};
-
-// What the checks of one rep of cdprobe_memcpy leave for the host, copied back on the issuer's stream behind them: the
-// head of the diagnosis (bad_words, bad_granules, first_bad_n of its DiagOut) and the (S, X) read of bwcurve_kernel
-// (its abort word and the Acc of its one rep).
+// What the checks of one rep of a block leave for the host (check_block), copied back on the checking rank's stream
+// behind them: the head of the diagnosis (bad_words, bad_granules, first_bad_n of its DiagOut) and the (S, X) read of
+// bwcurve_kernel (its abort word and the Acc of its one rep).
 struct MemcpyRepOut {
   unsigned long long diag[3];
   unsigned int abort_flag;
@@ -915,13 +911,19 @@ struct MemcpyRepOut {
 static_assert(offsetof(DiagOut, bad_words) == 0 && offsetof(DiagOut, first_bad_n) == 16, "the diagnosis head");
 static_assert(offsetof(BwScratch, abort_flag) == 0, "the (S, X) read's abort word");
 
-// cdprobe_memcpy's pinned, mapped and portable host block, made on first use and kept until close: the ticket every
-// local stream waits on (cuStreamWaitValue64, through its UVA address), the word the armed mode-0 fault stores per
-// local rank, and what each rep's checks left, per local rank and rep.
-struct MemcpyHost {
-  uint64_t ticket;
+// The pinned, mapped and portable host block of the copy-engine measurements (cdprobe_memcpy, cdprobe_ce_alltoall),
+// made by the first call of either (copy_setup) and kept until close: the ticket every local stream waits on
+// (cuStreamWaitValue64, through its UVA address), the second ticket a CE all-to-all mode-2 fault holds a copy stream
+// on, the tickets handed out so far, the word an armed mode-0 fault stores per local rank, the awaited values the CE
+// all-to-all writes into its own ranks' lines when it gives up on a rep, and what each rep's checks left, per local
+// rank, block and rep: memcpy's cell [issuer][target], the CE all-to-all's block [owner][sender].  Both calls take
+// their tickets from `issued`; tickets only rise, and a handle runs one call at a time, so a GEQ wait on either ticket
+// is met only by the rep it was queued for.
+struct CopyHost {
+  uint64_t ticket, hold, issued;
   uint64_t flip[kMaxRanks];
-  MemcpyRepOut rep[kMaxRanks][kRepSlots];
+  uint64_t release[2];
+  MemcpyRepOut rep[kMaxRanks][kMaxRanks][kRepSlots];
 };
 
 // Where cdprobe_memcpy keeps its device state in a local rank's scratch: the BwScratch of the (S, X) read at 0, the
@@ -934,28 +936,144 @@ struct MemcpyScratch {
   }
 };
 
-// The host block, the driver's stream wait and every local rank's event pool, made on first use.
-static int memcpy_setup(cdprobe* h) {
-  std::string err;
-  if (h->drv.load_stream_wait(&err) != cudaSuccess) {
-    set_err("cdprobe_memcpy: " + err);
-    return CDPROBE_ERR_UNSUPPORTED;
-  }
+// The host block and every local rank's rep events, made on the first call of either copy-engine measurement.
+static int copy_setup(cdprobe* h) {
   CDP_RT(cudaSetDevice(h->lr[0].ordinal));
-  if (h->memcpy_host == nullptr) {
+  if (h->copy_host == nullptr) {
     void* p = nullptr;
-    CDP_RT(cudaHostAlloc(&p, sizeof(MemcpyHost), cudaHostAllocPortable | cudaHostAllocMapped));
-    memset(p, 0, sizeof(MemcpyHost));
-    h->memcpy_host = static_cast<MemcpyHost*>(p);
-    __atomic_store_n(&h->memcpy_host->ticket, h->memcpy_tickets, __ATOMIC_RELEASE);
+    CDP_RT(cudaHostAlloc(&p, sizeof(CopyHost), cudaHostAllocPortable | cudaHostAllocMapped));
+    memset(p, 0, sizeof(CopyHost));
+    h->copy_host = static_cast<CopyHost*>(p);
   }
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
     CDP_RT(cudaSetDevice(L.ordinal));
-    for (cudaEvent_t& ev : L.memcpy_ev)
+    for (cudaEvent_t& ev : L.rep_ev)
       if (ev == nullptr) CDP_RT(cudaEventCreate(&ev));
   }
   return CDPROBE_OK;
+}
+
+// A copy-engine measurement's armed fault once the call has accepted it: timed rep 1 of size k of cell (issuer,
+// target) flips destination word `arg` (mode 0), queues no copy (mode 1), or holds the copy `arg` us (mode 2, the CE
+// all-to-all's).  issuer kMaxRanks: none.
+struct CopyFault {
+  uint32_t issuer = kMaxRanks, target = 0, k = 0, mode = 0;
+  uint64_t arg = 0;
+};
+
+// One copy-engine measurement, as open_copy opens it.  (Its member pointers go through an alias: nvcc's host pass warns
+// about the bare declarator, as it does for ArProtocol's.)
+using HandleCount = uint64_t cdprobe::*;
+struct CopyCall {
+  const char* fn;                      // the entry point
+  uint32_t default_reps;
+  HandleCount calls;                   // its calls that ran
+  HandleCount fault;                   // its armed fault, 0: disarmed
+  uint64_t max_mode;                   // the highest fault mode it accepts
+  const char* bad_fault;               // its refusal of an armed fault
+  std::string (*refusal)(cdprobe* h);  // why this process cannot run it, empty when it can; nullptr: it always can
+  const char* refused_elsewhere;       // its refusal when only another process cannot run it
+};
+
+// The opening of the copy-engine measurements: open_ladder, with out->op; the verdict on op, then on the armed fault
+// (`(mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | fault_spot`: a mode below 2 names a word of its size,
+// mode 2 a size and a delay under timeout_ms / 2); then, with valid arguments, C.refusal.  All are agreed over every
+// process, so every process refuses or runs together, and a refusal is CDPROBE_ERR_UNSUPPORTED.  Then the exchange area
+// (cdprobe_alltoall's, built once, by every process in the same call), the call number and the ladder.  *st gets the
+// domain's probe mapping status.
+template <typename Out>
+static int open_copy(cdprobe* h, const CopyCall& C, uint32_t op, uint32_t reps, Out* out, Ladder* lad, CopyFault* f,
+                     int32_t (*st)[kMaxRanks]) {
+  const int opened = open_ladder(h, out, reps, C.default_reps, lad);
+  if (out != nullptr) out->op = op;
+  if (opened != CDPROBE_OK) return opened;
+  const uint32_t n = h->n_total;
+  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad->bad.empty())
+    lad->bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
+  if (const uint64_t v = h->*C.fault; v != 0 && lad->bad.empty()) {
+    const uint64_t mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
+    const FaultSpot at = fault_spot(v, *lad);
+    if (mode > C.max_mode || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !h->plan.diag) || !at.size_ok ||
+        (mode < 2 && !at.word_ok) || (mode == 2 && 2 * at.word >= 1000ull * h->cfg.timeout_ms))
+      lad->bad = C.bad_fault;
+    else
+      *f = {(uint32_t)fi - 1, (uint32_t)ft - 1, at.k, (uint32_t)mode, at.word};
+  }
+  const std::string refusal = C.refusal != nullptr && lad->bad.empty() ? C.refusal(h) : std::string();
+  bool refused = !refusal.empty();
+  // agree() ors the refusal flag (its `zero`) over every process
+  if (const int rc = agree(h, C.fn, lad->bad, h->*C.calls + 1, {lad->reps, op, 0u}, st, nullptr, &refused);
+      rc != CDPROBE_OK)
+    return rc;
+  if (refused) {
+    set_err(!refusal.empty() ? refusal : std::string(C.refused_elsewhere));
+    return CDPROBE_ERR_UNSUPPORTED;
+  }
+  if (const int rc = ensure_area(h, h->area, (size_t)n * h->plan.bpp); rc != CDPROBE_OK) return rc;
+  out->call_seq = ++(h->*C.calls);
+  out->area_bytes = h->area.bytes;
+  put_ladder(h, *lad, out);
+  return CDPROBE_OK;
+}
+
+// The armed mode-0 fault's store, queued on stream s of local rank li after cell c's copy: destination word `word`
+// overwritten, by an 8-byte copy from the host block, with its pattern value xored with 1.
+static cudaError_t store_flip(cdprobe* h, uint32_t li, const MemcpyCell& c, uint64_t word, cudaStream_t s) {
+  uint64_t* const w = &h->copy_host->flip[li];
+  *w = src_word(h->seed, c.src_rank, c.first_word + word) ^ 1ull;
+  return cudaMemcpyAsync(reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off) + 8 * word, w, 8,
+                         cudaMemcpyHostToDevice, s);
+}
+
+// Waits, polling, until event B of rep `rep` has completed on every local rank in `ranks` (bit li), from the rep's
+// release: a copy cannot be aborted, so never an unbounded synchronise.  A failed query returns its error (`failed`)
+// and a B not complete timeout_ms after the release CDPROBE_ERR_TIMEOUT (`late`); either makes the handle sticky.
+static int wait_reps(cdprobe* h, uint32_t ranks, uint32_t rep, const char* failed, const char* late) {
+  const double deadline = now_ms() + h->cfg.timeout_ms;
+  for (uint32_t li = 0; li < h->n_local; ++li) {
+    if ((ranks >> li & 1u) == 0) continue;
+    LocalRank& L = h->lr[li];
+    CDP_RT(cudaSetDevice(L.ordinal));
+    cudaError_t e;
+    while ((e = cudaEventQuery(L.rep_ev[2 * rep + 1])) != cudaSuccess) {
+      if (e != cudaErrorNotReady) return fail_sticky(h, failed, e);
+      if (now_ms() > deadline) {
+        h->sticky = true;
+        set_err(late);
+        return CDPROBE_ERR_TIMEOUT;
+      }
+    }
+  }
+  return CDPROBE_OK;
+}
+
+// Folds what the checks of size k of one block left, got[rep] for the warm-up and every timed rep, into entry idx of a
+// cdprobe_memcpy_t (a cell) or a cdprobe_ce_alltoall_t (a block): bad_words over every rep and first_bad, the lowest
+// bad offset of any; bit k of bad_sizes for a bad word or an (S, X) other than `want` in any rep; the last rep's
+// (S, X).  Returns whether any rep's (S, X) read was aborted at its deadline.
+template <typename Out>
+static bool fold_checks(const MemcpyRepOut* got, uint32_t reps, uint32_t k, const uint64_t* want, uint32_t idx,
+                        Out* out) {
+  bool aborted = false;
+  uint64_t first = UINT64_MAX;
+  for (uint32_t rep = 0; rep <= reps; ++rep) {
+    const MemcpyRepOut& g = got[rep];
+    aborted |= g.abort_flag != 0;
+    out->bad_words[idx][k] += g.diag[0];
+    if (g.diag[0] != 0) first = std::min(first, (uint64_t)~g.diag[2]);
+    if (g.diag[0] != 0 || g.acc.sum != want[0] || g.acc.xr != want[1]) out->bad_sizes[idx] |= 1u << k;
+  }
+  out->first_bad[idx][k] = first;
+  out->sum[idx][k] = got[reps].acc.sum;
+  out->xr[idx][k] = got[reps].acc.xr;
+  return aborted;
+}
+
+// The status of a block once every size is folded: an (S, X) read aborted at its deadline, else a size that failed
+// its checks, else 0.
+static int32_t copy_verdict(bool aborted, uint32_t bad_sizes) {
+  return aborted ? CDPROBE_ERR_TIMEOUT : bad_sizes != 0 ? CDPROBE_ERR_INTEGRITY : 0;
 }
 
 // The timed part of rep `rep` of cdprobe_memcpy's cell (L.grank, j), L = h->lr[li], queued on L's stream: the wait
@@ -967,15 +1085,15 @@ static cudaError_t memcpy_timed(cdprobe* h, uint32_t li, uint32_t j, uint32_t op
   const MemcpyCell c = memcpy_cell(h->plan, op, L.grank, j);
   cudaError_t e = cudaSetDevice(L.ordinal);
   if (e != cudaSuccess) return e;
-  *cu = h->drv.StreamWaitValue64(L.stream, reinterpret_cast<CUdeviceptr>(&h->memcpy_host->ticket), ticket,
+  *cu = h->drv.StreamWaitValue64(L.stream, reinterpret_cast<CUdeviceptr>(&h->copy_host->ticket), ticket,
                                  CU_STREAM_WAIT_VALUE_GEQ);
   if (*cu != CUDA_SUCCESS) return cudaErrorUnknown;
-  e = cudaEventRecord(L.memcpy_ev[2 * rep], L.stream);
+  e = cudaEventRecord(L.rep_ev[2 * rep], L.stream);
   if (e == cudaSuccess && !drop)
     e = cudaMemcpyAsync(reinterpret_cast<void*>(h->area.va[li][c.dst_rank] + c.dst_off),
                         reinterpret_cast<const void*>(h->mem.va[li][c.src_rank] + c.src_off), bytes,
                         cudaMemcpyDeviceToDevice, L.stream);
-  if (e == cudaSuccess) e = cudaEventRecord(L.memcpy_ev[2 * rep + 1], L.stream);
+  if (e == cudaSuccess) e = cudaEventRecord(L.rep_ev[2 * rep + 1], L.stream);
   return e;
 }
 
@@ -1017,87 +1135,57 @@ static cudaError_t check_block(cdprobe* h, uint32_t li, const MemcpyCell& c, uin
 }
 
 // The untimed checks of rep `rep` of the cell, queued on L's stream behind its event B: the armed mode-0 fault's store
-// (`flip`: word flip_word), then check_block into rep's slot of the host block.
+// (`flip`: word flip_word), then check_block into the cell's slot of the host block.
 static cudaError_t memcpy_check(cdprobe* h, uint32_t li, uint32_t j, uint32_t op, uint64_t bytes, uint32_t rep,
                                 bool flip, uint64_t flip_word) {
   LocalRank& L = h->lr[li];
   const MemcpyCell c = memcpy_cell(h->plan, op, L.grank, j);
-  MemcpyHost* const host = h->memcpy_host;
-  uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
   cudaError_t e = cudaSetDevice(L.ordinal);
-  if (e == cudaSuccess && flip) {
-    host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + flip_word) ^ 1ull;
-    e = cudaMemcpyAsync(dst + 8 * flip_word, &host->flip[li], 8, cudaMemcpyHostToDevice, L.stream);
-  }
-  if (e == cudaSuccess) e = check_block(h, li, c, bytes, &host->rep[li][rep]);
+  if (e == cudaSuccess && flip) e = store_flip(h, li, c, flip_word, L.stream);
+  if (e == cudaSuccess) e = check_block(h, li, c, bytes, &h->copy_host->rep[li][j][rep]);
   return e;
 }
 
 // Rep `rep` of size k of cdprobe_memcpy on every local rank with a cell in this round (target[li] >= 0).  The timed
 // part of every rank's rep is queued (memcpy_timed) before the host releases the rep's ticket, so the events bracket
 // the copy alone, without the host's enqueue time; the ticket is released even when queuing fails, so no stream is
-// left waiting.  Then the host waits, polling, until every copy's event B has completed, and only then queues the
+// left waiting.  Then the host waits until every copy's event B has completed (wait_reps), and only then queues the
 // checks (memcpy_check): launching a kernel may have to load it, which must not wait behind a stream that waits on
-// the host, and no host submission overlaps a timed copy.  A copy cannot be aborted: one whose event B has not
-// completed timeout_ms after the release returns CDPROBE_ERR_TIMEOUT and makes the handle sticky.
+// the host, and no host submission overlaps a timed copy.
 static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladder& lad, uint32_t k, uint32_t rep,
-                      const MemcpyFault& f) {
-  const uint64_t ticket = ++h->memcpy_tickets, bytes = lad.size[k];
+                      const CopyFault& f) {
+  const uint64_t ticket = ++h->copy_host->issued, bytes = lad.size[k];
   auto armed = [&](uint32_t li) {
     return rep == 1 && k == f.k && h->lr[li].grank == f.issuer && (uint32_t)target[li] == f.target;
   };
   cudaError_t e = cudaSuccess;
   CUresult cu = CUDA_SUCCESS;
-  for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
-    if (target[li] >= 0)
-      e = memcpy_timed(h, li, (uint32_t)target[li], op, ticket, bytes, rep, armed(li) && f.mode == 1, &cu);
-  __atomic_store_n(&h->memcpy_host->ticket, ticket, __ATOMIC_RELEASE);
+  uint32_t ranks = 0;
+  for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li) {
+    if (target[li] < 0) continue;
+    ranks |= 1u << li;
+    e = memcpy_timed(h, li, (uint32_t)target[li], op, ticket, bytes, rep, armed(li) && f.mode == 1, &cu);
+  }
+  __atomic_store_n(&h->copy_host->ticket, ticket, __ATOMIC_RELEASE);
   if (cu != CUDA_SUCCESS) {
     h->sticky = true;
     set_err("cdprobe_memcpy: cuStreamWaitValue64: " + h->drv.error_name(cu));
     return CDPROBE_ERR_CUDA;
   }
   if (e != cudaSuccess) return fail_sticky(h, "cdprobe_memcpy: queue a rep", e);
-  const double deadline = now_ms() + h->cfg.timeout_ms;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    if (target[li] < 0) continue;
-    LocalRank& L = h->lr[li];
-    CDP_RT(cudaSetDevice(L.ordinal));
-    while ((e = cudaEventQuery(L.memcpy_ev[2 * rep + 1])) != cudaSuccess) {
-      if (e != cudaErrorNotReady) return fail_sticky(h, "cdprobe_memcpy: wait for a copy", e);
-      if (now_ms() > deadline) {
-        h->sticky = true;
-        set_err("cdprobe_memcpy: a copy did not complete within timeout_ms of its release");
-        return CDPROBE_ERR_TIMEOUT;
-      }
-    }
-  }
+  if (const int rc = wait_reps(h, ranks, rep, "cdprobe_memcpy: wait for a copy",
+                               "cdprobe_memcpy: a copy did not complete within timeout_ms of its release");
+      rc != CDPROBE_OK)
+    return rc;
   for (uint32_t li = 0; li < h->n_local && e == cudaSuccess; ++li)
     if (target[li] >= 0)
-      e = memcpy_check(h, li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.word);
+      e = memcpy_check(h, li, (uint32_t)target[li], op, bytes, rep, armed(li) && f.mode == 0, f.arg);
   return e != cudaSuccess ? fail_sticky(h, "cdprobe_memcpy: queue the checks", e) : CDPROBE_OK;
 }
 
-constexpr uint32_t kCeA2aDefaultReps = 8;
-
-// cdprobe_ce_alltoall's armed fault once the call has accepted it: timed rep 1 of size k of cell (issuer, target), on
-// the cell's copy stream, flips destination word `arg` (mode 0), queues no copy (mode 1), or is held `arg` us (mode 2).
-// issuer kMaxRanks: none.
-struct CeA2aFault {
-  uint32_t issuer = kMaxRanks, target = 0, k = 0, mode = 0;
-  uint64_t arg = 0;
-};
-
-// cdprobe_ce_alltoall's pinned, mapped and portable host block, made on first use and kept until close: the ticket
-// every local stream waits on, the second ticket a mode-2 fault holds a copy stream on, the tickets handed out so far,
-// the word the armed mode-0 fault stores per local rank, the awaited values the host writes into its own ranks' lines
-// when it gives up on a rep, and what each rep's checks left, per local owner, block (its sender) and rep.
-struct CeA2aHost {
-  uint64_t ticket, hold, issued;
-  uint64_t flip[kMaxRanks];
-  uint64_t release[2];
-  MemcpyRepOut rep[kMaxRanks][kMaxRanks][kRepSlots];
-};
+constexpr CopyCall kMemcpy = {
+    "cdprobe_memcpy", 8, &cdprobe::memcpy_calls, &cdprobe::memcpy_fault, 1,
+    "the armed memcpy fault names no cell, size or word of this call, or has a mode above 1", nullptr, nullptr};
 
 // The cells local rank li issues, one per copy stream: its peers in the order rank + 1, rank + 2, ... (mod n), then
 // the diagonal with a loop-back slice.  Returns their count.
@@ -1123,15 +1211,17 @@ static std::string ce_a2a_refusal(cdprobe* h) {
          ", CUDA_DEVICE_MAX_CONNECTIONS allows " + std::to_string(h->max_connections);
 }
 
-// The host block, and every local rank's copy streams and events, made on the first call and kept until close.
+constexpr CopyCall kCeA2a = {
+    "cdprobe_ce_alltoall", 8, &cdprobe::cea_calls, &cdprobe::cea_fault, 2,
+    "the armed copy-engine all-to-all fault names no cell, size, word or delay of this call, or has a mode above 2",
+    ce_a2a_refusal,
+    "cdprobe_ce_alltoall: another process cannot run it (no stream memory operations, or more streams than "
+    "CUDA_DEVICE_MAX_CONNECTIONS)"};
+
+// The host block and the rep events (copy_setup), and every local rank's copy streams and their events, made on the
+// first call and kept until close.
 static int ce_a2a_setup(cdprobe* h) {
-  CDP_RT(cudaSetDevice(h->lr[0].ordinal));
-  if (h->cea_host == nullptr) {
-    void* p = nullptr;
-    CDP_RT(cudaHostAlloc(&p, sizeof(CeA2aHost), cudaHostAllocPortable | cudaHostAllocMapped));
-    memset(p, 0, sizeof(CeA2aHost));
-    h->cea_host = static_cast<CeA2aHost*>(p);
-  }
+  if (const int rc = copy_setup(h); rc != CDPROBE_OK) return rc;
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
     uint32_t target[kMaxRanks];
@@ -1143,8 +1233,6 @@ static int ce_a2a_setup(cdprobe* h) {
         if (L.cea_copy_ev[i][x] == nullptr)
           CDP_RT(cudaEventCreateWithFlags(&L.cea_copy_ev[i][x], x < 2 ? cudaEventDefault : cudaEventDisableTiming));
     }
-    for (cudaEvent_t& ev : L.cea_ev)
-      if (ev == nullptr) CDP_RT(cudaEventCreate(&ev));
   }
   return CDPROBE_OK;
 }
@@ -1157,7 +1245,7 @@ static CUdeviceptr ce_a2a_line(const cdprobe* h, uint32_t li, uint32_t owner, ui
 // When the host gives up on a rep whose values are v: writes v into both words of every line of its own ranks, on a
 // stream of its own, so that no stream of theirs is left waiting at close.  Best effort: it waits at most timeout_ms.
 static void ce_a2a_unblock(cdprobe* h, uint64_t v) {
-  CeA2aHost* const host = h->cea_host;
+  CopyHost* const host = h->copy_host;
   host->release[0] = host->release[1] = v;
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
@@ -1178,13 +1266,13 @@ static void ce_a2a_unblock(cdprobe* h, uint64_t v) {
 // ticket (DESIGN §5p): on each rank's stream the ticket wait, the opening barrier, event A, the joins of its copy
 // streams (and on a push the landed values of every sender), event B; on each copy stream the wait for A, the copy
 // between its two events, and on a push the landed value.  The ticket is released even when queuing fails.  Then the
-// host waits, polling, until every B has completed, reads the times of a timed rep into rank_ns[li][k] and
+// host waits until every B has completed (wait_reps), reads the times of a timed rep into rank_ns[li][k] and
 // copy_ns[li][i][k], and only then queues the checks of every block each local rank owns, on its stream, so no kernel
 // launch waits behind a stream that waits on the host.
-static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, uint32_t rep, const CeA2aFault& f,
+static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, uint32_t rep, const CopyFault& f,
                       float (*rank_ns)[kBwMaxSizes][kMaxTimedReps],
                       float (*copy_ns)[kMaxRanks][kBwMaxSizes][kMaxTimedReps]) {
-  CeA2aHost* const host = h->cea_host;
+  CopyHost* const host = h->copy_host;
   const Plan& pl = h->plan;
   const uint32_t n = h->n_total;
   const bool push = op == CDPROBE_OP_WRITE;
@@ -1210,7 +1298,7 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
     what = "cuStreamWaitValue64";
     for (uint32_t p = 0; p < n && ok(); ++p)
       if (p != g) cu = wait_value(s, ce_a2a_line(h, li, g, p, 0), v);
-    if (ok()) e = cudaEventRecord(L.cea_ev[0], s);
+    if (ok()) e = cudaEventRecord(L.rep_ev[2 * rep], s);
     uint32_t target[kMaxRanks];
     const uint32_t cells = ce_a2a_targets(h, li, target);
     for (uint32_t i = 0; i < cells && ok(); ++i) {
@@ -1220,7 +1308,7 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
       const cudaStream_t cs = L.cea_stream[i];
       cudaEvent_t* const ev = L.cea_copy_ev[i];
       uint8_t* const dst = reinterpret_cast<uint8_t*>(h->area.va[li][c.dst_rank] + c.dst_off);
-      e = cudaStreamWaitEvent(cs, L.cea_ev[0], 0);
+      e = cudaStreamWaitEvent(cs, L.rep_ev[2 * rep], 0);
       what = "cuStreamWaitValue64";
       if (ok() && armed && f.mode == 2) {
         cu = wait_value(cs, reinterpret_cast<CUdeviceptr>(&host->hold), ticket);
@@ -1231,10 +1319,7 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
         e = cudaMemcpyAsync(dst, reinterpret_cast<const void*>(h->mem.va[li][c.src_rank] + c.src_off), bytes,
                             cudaMemcpyDeviceToDevice, cs);
       if (ok()) e = cudaEventRecord(ev[1], cs);
-      if (ok() && armed && f.mode == 0) {
-        host->flip[li] = src_word(h->seed, c.src_rank, c.first_word + f.arg) ^ 1ull;
-        e = cudaMemcpyAsync(dst + 8 * f.arg, &host->flip[li], 8, cudaMemcpyHostToDevice, cs);
-      }
+      if (ok() && armed && f.mode == 0) e = store_flip(h, li, c, f.arg, cs);
       what = "cuStreamWriteValue64";
       if (ok() && push) cu = h->drv.StreamWriteValue64(cs, ce_a2a_line(h, li, j, g, 1), v, CU_STREAM_WRITE_VALUE_DEFAULT);
       if (ok()) e = cudaEventRecord(ev[2], cs);
@@ -1243,7 +1328,7 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
     what = "cuStreamWaitValue64";
     for (uint32_t p = 0; p < n && push && ok(); ++p)
       if (p != g || pl.diag) cu = wait_value(s, ce_a2a_line(h, li, g, p, 1), v);
-    if (ok()) e = cudaEventRecord(L.cea_ev[1], s);
+    if (ok()) e = cudaEventRecord(L.rep_ev[2 * rep + 1], s);
   }
   __atomic_store_n(&host->ticket, ticket, __ATOMIC_RELEASE);
   if (held) usleep((useconds_t)f.arg);
@@ -1255,19 +1340,11 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
     set_err(std::string("cdprobe_ce_alltoall: ") + what + ": " + h->drv.error_name(cu));
     return CDPROBE_ERR_CUDA;
   }
-  const double deadline = now_ms() + h->cfg.timeout_ms;
-  for (uint32_t li = 0; li < h->n_local; ++li) {
-    LocalRank& L = h->lr[li];
-    CDP_RT(cudaSetDevice(L.ordinal));
-    while ((e = cudaEventQuery(L.cea_ev[1])) != cudaSuccess) {
-      if (e != cudaErrorNotReady) return fail_sticky(h, "cdprobe_ce_alltoall: wait for a rep", e);
-      if (now_ms() > deadline) {
-        ce_a2a_unblock(h, v);
-        h->sticky = true;
-        set_err("cdprobe_ce_alltoall: a rep did not complete within timeout_ms of its release");
-        return CDPROBE_ERR_TIMEOUT;
-      }
-    }
+  if (const int rc = wait_reps(h, (1u << h->n_local) - 1u, rep, "cdprobe_ce_alltoall: wait for a rep",
+                               "cdprobe_ce_alltoall: a rep did not complete within timeout_ms of its release");
+      rc != CDPROBE_OK) {
+    if (rc == CDPROBE_ERR_TIMEOUT) ce_a2a_unblock(h, v);
+    return rc;
   }
   for (uint32_t li = 0; li < h->n_local && rep > 0; ++li) {
     LocalRank& L = h->lr[li];
@@ -1275,7 +1352,7 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
     const uint32_t cells = ce_a2a_targets(h, li, target);
     float ms = 0.f;
     CDP_RT(cudaSetDevice(L.ordinal));
-    if ((e = cudaEventElapsedTime(&ms, L.cea_ev[0], L.cea_ev[1])) != cudaSuccess)
+    if ((e = cudaEventElapsedTime(&ms, L.rep_ev[2 * rep], L.rep_ev[2 * rep + 1])) != cudaSuccess)
       return fail_sticky(h, "cdprobe_ce_alltoall: event times", e);
     rank_ns[li][k][rep - 1] = ms * 1e6f;
     for (uint32_t i = 0; i < cells; ++i) {
@@ -1745,10 +1822,10 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
 
   // 3. which cells run: st[s][d], the probe mapping status of sender s's cell to receiver d, or else its exchange-area
   //    mapping status; 0 runs.  Every process derives the same matrix.
+  cdp::fold_area_status(h, h->area, st);
   bool any = false;
   for (uint32_t s = 0; s < n; ++s) {
     for (uint32_t d = 0; d < n; ++d) {
-      if (st[s][d] == 0) st[s][d] = h->area.status[s][d];
       if (s == d && !pl.diag) st[s][d] = CDPROBE_ERR_ARG;  // no such cell
       any |= st[s][d] == 0;
     }
@@ -1850,40 +1927,21 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
 }
 
 int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* out) {
+  // 1-2. the arguments, the armed fault and the probe mapping rows, shared in a multi-process domain so that every
+  //      process refuses or runs together over the same rounds; then the exchange area
   cdp::Ladder lad;
-  const int opened = cdp::open_ladder(h, out, reps, cdp::kMemcpyDefaultReps, &lad);
-  if (out != nullptr) out->op = op;
-  if (opened != CDPROBE_OK) return opened;
+  cdp::CopyFault f;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::open_copy(h, cdp::kMemcpy, op, reps, out, &lad, &f, st); rc != CDPROBE_OK) return rc;
   const cdp::Plan& pl = h->plan;
   const uint32_t n = h->n_total;
-  // 1. the arguments, the armed fault and the probe mapping rows; in a multi-process domain all three are shared, so
-  //    every process refuses or runs together over the same rounds
-  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad.bad.empty())
-    lad.bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
-  cdp::MemcpyFault f;
-  if (h->memcpy_fault != 0 && lad.bad.empty()) {
-    const uint64_t v = h->memcpy_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
-    const cdp::FaultSpot at = cdp::fault_spot(v, lad);
-    if (mode > 1 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || !at.word_ok)
-      lad.bad = "the armed memcpy fault names no cell, size or word of this call, or has a mode above 1";
-    else
-      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, at.k, (uint32_t)mode, at.word};
-  }
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_memcpy", lad.bad, h->memcpy_calls + 1, {lad.reps, op, 0u}, st);
-      rc != CDPROBE_OK)
-    return rc;
-  // 2. the exchange area (cdprobe_alltoall's), built once, by every process in the same call
-  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++h->memcpy_calls;
-  out->area_bytes = h->area.bytes;
-  cdp::put_ladder(h, lad, out);
 
   // 3. which cells run: the issuer maps the target's probe allocation and exchange area (cdprobe_alltoall's rule);
   //    whether any cell of the domain runs, from the status every process shares
+  cdp::fold_area_status(h, h->area, st);
   bool any = false;
   for (uint32_t s = 0; s < n; ++s)
-    for (uint32_t d = 0; d < n; ++d) any |= (s != d || pl.diag) && st[s][d] == 0 && h->area.status[s][d] == 0;
+    for (uint32_t d = 0; d < n; ++d) any |= (s != d || pl.diag) && st[s][d] == 0;
   bool runs[cdp::kMaxRanks][cdp::kMaxRanks] = {};
   for (uint32_t li = 0; li < h->n_local; ++li) {
     const cdp::LocalRank& L = h->lr[li];
@@ -1900,10 +1958,15 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
     return CDPROBE_OK;
   }
 
-  // 4. the host block, the stream wait and the events; scratch for the checks and one cell's granule table, grown on
-  //    every local rank before anything is queued; the (S, X) each size of each cell must land, from the pattern
-  //    definition: the per-granule sums of the source slice on the issuer's GPU, folded into every prefix on the host
-  if (const int rc = cdp::memcpy_setup(h); rc != CDPROBE_OK) return rc;
+  // 4. the driver's stream wait, the host block and the events; scratch for the checks and one cell's granule table,
+  //    grown on every local rank before anything is queued; the (S, X) each size of each cell must land, from the
+  //    pattern definition: the per-granule sums of the source slice on the issuer's GPU, folded into every prefix on
+  //    the host.  A driver without the stream wait is refused here, by this process alone (DESIGN §5n)
+  if (std::string err; h->drv.load_stream_wait(&err) != cudaSuccess) {
+    cdp::set_err("cdprobe_memcpy: " + err);
+    return CDPROBE_ERR_UNSUPPORTED;
+  }
+  if (const int rc = cdp::copy_setup(h); rc != CDPROBE_OK) return rc;
   std::unique_ptr<cdp::CellSums[]> want;
   if (const int rc = cdp::cell_sums(h, runs, op, cdp::MemcpyScratch(pl.bpp).table_off, lad,
                                     "cdprobe_memcpy: granule checksums", &want);
@@ -1929,25 +1992,13 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
         CDP_RT(cudaSetDevice(L.ordinal));
         if (const cudaError_t e = cudaStreamSynchronize(L.stream); e != cudaSuccess)
           return cdp::fail_sticky(h, "cdprobe_memcpy: check a size", e);
-        const uint64_t(*w)[2] = want[li][j];
-        uint64_t first = UINT64_MAX;
-        for (uint32_t rep = 0; rep <= lad.reps; ++rep) {
-          const cdp::MemcpyRepOut& got = h->memcpy_host->rep[li][rep];
-          aborted[li] |= got.abort_flag != 0;
-          out->bad_words[idx][k] += got.diag[0];
-          if (got.diag[0] != 0) first = std::min(first, (uint64_t)~got.diag[2]);
-          if (got.diag[0] != 0 || got.acc.sum != w[k][0] || got.acc.xr != w[k][1]) out->bad_sizes[idx] |= 1u << k;
-          if (rep == lad.reps) {
-            out->sum[idx][k] = got.acc.sum;
-            out->xr[idx][k] = got.acc.xr;
-          }
-          if (rep == 0) continue;
+        for (uint32_t rep = 1; rep <= lad.reps; ++rep) {
           float ms_rep = 0.f;
-          const cudaError_t e = cudaEventElapsedTime(&ms_rep, L.memcpy_ev[2 * rep], L.memcpy_ev[2 * rep + 1]);
+          const cudaError_t e = cudaEventElapsedTime(&ms_rep, L.rep_ev[2 * rep], L.rep_ev[2 * rep + 1]);
           if (e != cudaSuccess) return cdp::fail_sticky(h, "cdprobe_memcpy: event times", e);
           ns[li][k][rep - 1] = ms_rep * 1e6f;
         }
-        out->first_bad[idx][k] = first;
+        aborted[li] |= cdp::fold_checks(h->copy_host->rep[li][j], lad.reps, k, want[li][j][k], idx, out);
       }
     }
     // per cell: the times, unless an (S, X) read passed its deadline, and the verdict of every size's checks
@@ -1955,12 +2006,8 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
       if (target[li] < 0) continue;
       const uint32_t idx = h->lr[li].grank * CDPROBE_MAX_GPUS + (uint32_t)target[li];
       out->measured[idx] = 1;
-      if (aborted[li]) {
-        out->status[idx] = CDPROBE_ERR_TIMEOUT;
-        continue;
-      }
-      cdp::ladder_times(ns[li], lad.size, lad.n_sizes, lad.reps, 1.0, idx, out);
-      out->status[idx] = out->bad_sizes[idx] ? CDPROBE_ERR_INTEGRITY : 0;
+      if (!aborted[li]) cdp::ladder_times(ns[li], lad.size, lad.n_sizes, lad.reps, 1.0, idx, out);
+      out->status[idx] = cdp::copy_verdict(aborted[li], out->bad_sizes[idx]);
     }
     return CDPROBE_OK;
   };
@@ -1970,53 +2017,19 @@ int cdprobe_memcpy(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_memcpy_t* o
 }
 
 int cdprobe_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_alltoall_t* out) {
+  // 1-2. the arguments, the armed fault, the probe mapping rows and whether every process can run it, shared in a
+  //      multi-process domain so that every process refuses, skips or runs together; then the exchange area
   cdp::Ladder lad;
-  const int opened = cdp::open_ladder(h, out, reps, cdp::kCeA2aDefaultReps, &lad);
-  if (out != nullptr) out->op = op;
-  if (opened != CDPROBE_OK) return opened;
+  cdp::CopyFault f;
+  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
+  if (const int rc = cdp::open_copy(h, cdp::kCeA2a, op, reps, out, &lad, &f, st); rc != CDPROBE_OK) return rc;
   const cdp::Plan& pl = h->plan;
   const uint32_t n = h->n_total;
   const bool push = op == CDPROBE_OP_WRITE;
-  // 1. the arguments, the armed fault, the probe mapping rows and whether every process can run it; in a multi-process
-  //    domain all are shared, so every process refuses, skips or runs together
-  if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad.bad.empty())
-    lad.bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
-  cdp::CeA2aFault f;
-  if (h->cea_fault != 0 && lad.bad.empty()) {
-    const uint64_t v = h->cea_fault, mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
-    const cdp::FaultSpot at = cdp::fault_spot(v, lad);
-    if (mode > 2 || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !pl.diag) || !at.size_ok ||
-        (mode < 2 && !at.word_ok) || (mode == 2 && 2 * at.word >= 1000ull * h->cfg.timeout_ms))
-      lad.bad = "the armed copy-engine all-to-all fault names no cell, size, word or delay of this call, or has a mode "
-                "above 2";
-    else
-      f = {(uint32_t)fi - 1, (uint32_t)ft - 1, at.k, (uint32_t)mode, at.word};
-  }
-  const std::string refusal = lad.bad.empty() ? cdp::ce_a2a_refusal(h) : std::string();
-  bool refused = !refusal.empty();
-  int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  // agree() ors the refusal flag (its `zero`) over every process
-  if (const int rc = cdp::agree(h, "cdprobe_ce_alltoall", lad.bad, h->cea_calls + 1, {lad.reps, op, 0u}, st, nullptr,
-                                &refused);
-      rc != CDPROBE_OK)
-    return rc;
-  if (refused) {
-    cdp::set_err(!refusal.empty() ? refusal
-                                  : std::string("cdprobe_ce_alltoall: another process cannot run it (no stream memory "
-                                                "operations, or more streams than CUDA_DEVICE_MAX_CONNECTIONS)"));
-    return CDPROBE_ERR_UNSUPPORTED;
-  }
-  // 2. the exchange area (cdprobe_alltoall's and cdprobe_memcpy's), built once, by every process in the same call
-  if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++h->cea_calls;
-  out->area_bytes = h->area.bytes;
-  cdp::put_ladder(h, lad, out);
 
   // 3. every rank signals every other and every cell copies in every rep: when some probe or exchange-area mapping of
   //    the domain is down, nothing runs, in any process (a stream barrier cannot skip a peer)
-  for (uint32_t s = 0; s < n; ++s)
-    for (uint32_t d = 0; d < n; ++d)
-      if (st[s][d] == 0) st[s][d] = h->area.status[s][d];
+  cdp::fold_area_status(h, h->area, st);
   if (const int32_t* down = cdp::first_down(st); down != nullptr) {
     for (uint32_t li = 0; li < h->n_local; ++li) {
       const uint32_t g = h->lr[li].grank;
@@ -2064,20 +2077,7 @@ int cdprobe_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_all
       for (uint32_t j = 0; j < n; ++j) {
         if (!owns[li][j]) continue;
         const uint32_t idx = push ? j * CDPROBE_MAX_GPUS + g : g * CDPROBE_MAX_GPUS + j;
-        const uint64_t(*w)[2] = want[li][j];
-        uint64_t first = UINT64_MAX;
-        for (uint32_t rep = 0; rep <= lad.reps; ++rep) {
-          const cdp::MemcpyRepOut& got = h->cea_host->rep[li][j][rep];
-          aborted[li][j] |= got.abort_flag != 0;
-          out->bad_words[idx][k] += got.diag[0];
-          if (got.diag[0] != 0) first = std::min(first, (uint64_t)~got.diag[2]);
-          if (got.diag[0] != 0 || got.acc.sum != w[k][0] || got.acc.xr != w[k][1]) out->bad_sizes[idx] |= 1u << k;
-          if (rep == lad.reps) {
-            out->sum[idx][k] = got.acc.sum;
-            out->xr[idx][k] = got.acc.xr;
-          }
-        }
-        out->first_bad[idx][k] = first;
+        aborted[li][j] |= cdp::fold_checks(h->copy_host->rep[li][j], lad.reps, k, want[li][j][k], idx, out);
       }
     }
   }
@@ -2102,7 +2102,7 @@ int cdprobe_ce_alltoall(cdprobe_t* h, uint32_t op, uint32_t reps, cdprobe_ce_all
       if (!owns[li][j]) continue;
       const uint32_t idx = push ? j * CDPROBE_MAX_GPUS + g : g * CDPROBE_MAX_GPUS + j;
       out->cell_measured[idx] = 1;
-      out->cell_status[idx] = aborted[li][j] ? CDPROBE_ERR_TIMEOUT : out->bad_sizes[idx] ? CDPROBE_ERR_INTEGRITY : 0;
+      out->cell_status[idx] = cdp::copy_verdict(aborted[li][j], out->bad_sizes[idx]);
     }
   }
   out->ms = cdp::now_ms() - lad.t_begin;
