@@ -22,6 +22,8 @@ import sys
 
 import numpy as np
 
+from mutants import replace_once
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "k8s-dra-driver-gpu_b200", "csrc")
@@ -76,9 +78,7 @@ def generate(text=None, mutation=None):
     assert " ".join(removed) == " ".join(" ".join(s.split()) for s in statements), removed
     assert added == [LD_REDUCE_CALL, STORE_CALL], added
     if mutation is not None:
-        old, new = MUTATIONS[mutation]
-        assert out.count(old) == 1, (mutation, out.count(old))
-        out = out.replace(old, new)
+        out = replace_once(out, *MUTATIONS[mutation], where=f"the copy ({mutation})")
     return out
 
 
