@@ -494,13 +494,27 @@ class LinksT(C.Structure):
     ]
 
 
+def _pack(biased, plain=(), mode: int = 0, modes: int = 1, message: str | None = None) -> int:
+    """A fault option value: `mode` at bit 48, and each (value, shift, width) of `biased` as value + 1 (so that 0 names
+    nothing) and of `plain` as value, in its width-bit field at `shift`.  With a message, a mode outside range(modes)
+    or a field that does not fit its width raises ValueError(message); without one nothing is checked."""
+    if message is not None and (mode not in range(modes) or not all(0 <= v < (1 << w) - 1 for v, _, w in biased)
+                                or not all(0 <= v < 1 << w for v, _, w in plain)):
+        raise ValueError(message)
+    word = mode << 48
+    for v, shift, _ in biased:
+        word |= (v + 1) << shift
+    for v, shift, _ in plain:
+        word |= v << shift
+    return word
+
+
 def memcpy_fault(issuer: int, target: int, k: int, word: int, mode: int = 0) -> int:
     """The CDPROBE_OPT_MEMCPY_FAULT value for timed rep 1 of size[k] of cell (issuer, target) of cdprobe_memcpy: mode 0,
     destination word `word` is xored with 1 between the copy and the check; mode 1, no copy is queued, so the cleared
     destination reads as 0s.  Fields that do not fit are refused here."""
-    if mode not in (0, 1) or not (0 <= issuer < 255 and 0 <= target < 255 and 0 <= k < 255 and 0 <= word < 1 << 24):
-        raise ValueError("memcpy_fault: mode 0 or 1, ranks and k below 255, word below 2^24")
-    return (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | ((k + 1) << 24) | word
+    return _pack([(issuer, 40, 8), (target, 32, 8), (k, 24, 8)], [(word, 0, 24)], mode, 2,
+                 "memcpy_fault: mode 0 or 1, ranks and k below 255, word below 2^24")
 
 
 def ce_alltoall_fault(issuer: int, target: int, k: int, arg: int, mode: int = 0) -> int:
@@ -508,29 +522,27 @@ def ce_alltoall_fault(issuer: int, target: int, k: int, arg: int, mode: int = 0)
     cdprobe_ce_alltoall: mode 0, destination word `arg` is xored with 1 after the copy and before the landed flag; mode
     1, no copy is queued but the landed flag is published; mode 2, the copy stream is held `arg` us.  Fields that do not
     fit are refused here."""
-    if mode not in (0, 1, 2) or not (0 <= issuer < 255 and 0 <= target < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
-        raise ValueError("ce_alltoall_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
-    return (mode << 48) | ((issuer + 1) << 40) | ((target + 1) << 32) | ((k + 1) << 24) | arg
+    return _pack([(issuer, 40, 8), (target, 32, 8), (k, 24, 8)], [(arg, 0, 24)], mode, 3,
+                 "ce_alltoall_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
 
 
 def alltoall_fault(sender: int, receiver: int, k: int, word: int) -> int:
     """The CDPROBE_OPT_ALLTOALL_FAULT value that makes timed rep 1 of size[k] store word `word` of block
     (sender -> receiver) xored with 1."""
-    return ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | word
+    return _pack([(sender, 40, 8), (receiver, 32, 8), (k, 24, 8)], [(word, 0, 24)])
 
 
 def allreduce_fault(rank: int, k: int, word: int, drop: bool = False) -> int:
     """The CDPROBE_OPT_ALLREDUCE_FAULT value that makes timed rep 1 of size[k] on `rank` add 1 to output word `word`,
     or (drop) store nothing of the word's 8 KiB unit.  Fields that do not fit are refused here."""
-    if not (0 <= rank < 0xffff and 0 <= k < 255 and 0 <= word < 1 << 24):
-        raise ValueError("allreduce_fault: rank below 65535, k below 255, word below 2^24")
-    return ((1 if drop else 0) << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
+    return _pack([(rank, 32, 16), (k, 24, 8)], [(word, 0, 24)], 1 if drop else 0, 2,
+                 "allreduce_fault: rank below 65535, k below 255, word below 2^24")
 
 
 def allreduce_twoshot_fault(receiver: int, k: int, word: int, drop: bool = False) -> int:
     """The CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT value that makes timed rep 1 of size[k] deliver output word `word` to
     `receiver` xored with 1, or (drop) not deliver the word's 8 KiB unit to `receiver` at all."""
-    return ((1 if drop else 0) << 48) | ((receiver + 1) << 32) | ((k + 1) << 24) | word
+    return _pack([(receiver, 32, 16), (k, 24, 8)], [(word, 0, 24)], 1 if drop else 0)
 
 
 def allreduce_ll_fault(sender: int, receiver: int, k: int, arg: int, mode: int = 0) -> int:
@@ -538,9 +550,8 @@ def allreduce_ll_fault(sender: int, receiver: int, k: int, arg: int, mode: int =
     of word `arg` from `sender` to `receiver` carries its data xored with 1; mode 1, `sender` waits `arg` us before its
     first push (`receiver` must still name a rank); in every rep of the size, mode 2, `receiver` (which must be
     `sender`) makes no store to output word `arg`.  Fields that do not fit are refused here."""
-    if mode not in (0, 1, 2) or not (0 <= sender < 255 and 0 <= receiver < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
-        raise ValueError("allreduce_ll_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
-    return (mode << 48) | ((sender + 1) << 40) | ((receiver + 1) << 32) | ((k + 1) << 24) | arg
+    return _pack([(sender, 40, 8), (receiver, 32, 8), (k, 24, 8)], [(arg, 0, 24)], mode, 3,
+                 "allreduce_ll_fault: mode 0, 1 or 2, ranks and k below 255, arg below 2^24")
 
 
 def allreduce_ring_fault(sender: int, k: int, arg: int, phase: int = 0, mode: int = 0) -> int:
@@ -548,9 +559,8 @@ def allreduce_ring_fault(sender: int, k: int, arg: int, phase: int = 0, mode: in
     (the reduce-scatter) or 1 (the all-gather): mode 0, `sender`'s push of word `arg` to its successor carries it xored
     with 1; mode 1, that push stores nothing of the word's unit but still publishes its flag; mode 2, `sender` waits
     `arg` us before its first push of the rep.  Fields that do not fit are refused here."""
-    if mode not in (0, 1, 2) or phase not in (0, 1) or not (0 <= sender < 255 and 0 <= k < 255 and 0 <= arg < 1 << 24):
-        raise ValueError("allreduce_ring_fault: mode 0, 1 or 2, phase 0 or 1, sender and k below 255, arg below 2^24")
-    return (mode << 48) | (phase << 40) | ((sender + 1) << 32) | ((k + 1) << 24) | arg
+    return _pack([(sender, 32, 8), (k, 24, 8)], [(phase, 40, 1), (arg, 0, 24)], mode, 3,
+                 "allreduce_ring_fault: mode 0, 1 or 2, phase 0 or 1, sender and k below 255, arg below 2^24")
 
 
 def allreduce_push_fault(rank: int, k: int, word: int, mode: int = 0) -> int:
@@ -558,29 +568,27 @@ def allreduce_push_fault(rank: int, k: int, word: int, mode: int = 0) -> int:
     `word`: mode 0, sender `rank` contributes its source word + 1; mode 1, it skips the reduction of the word's unit;
     mode 2, it issues that reduction twice; mode 3, the owner of the word's chunk pushes the word xored with 1 to
     receiver `rank` in the all-gather.  Fields that do not fit are refused here."""
-    if mode not in (0, 1, 2, 3) or not (0 <= rank < 0xffff and 0 <= k < 255 and 0 <= word < 1 << 24):
-        raise ValueError("allreduce_push_fault: mode 0 to 3, rank below 65535, k below 255, word below 2^24")
-    return (mode << 48) | ((rank + 1) << 32) | ((k + 1) << 24) | word
+    return _pack([(rank, 32, 16), (k, 24, 8)], [(word, 0, 24)], mode, 4,
+                 "allreduce_push_fault: mode 0 to 3, rank below 65535, k below 255, word below 2^24")
 
 
 def allreduce_nvls_fault(k: int, word: int, mode: int = 0) -> int:
     """The CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value for timed rep 1 of size[k] of cdprobe_allreduce_nvls, on output word
     `word`, acted on by the owner of the word's chunk: mode 0, it stores the word xored with 1 through the multicast
     address; mode 1, it skips the multicast store of the word's 8 KiB unit.  Fields that do not fit are refused here."""
-    if mode not in (0, 1) or not (0 <= k < 255 and 0 <= word < 1 << 24):
-        raise ValueError("allreduce_nvls_fault: mode 0 or 1, k below 255, word below 2^24")
-    return (mode << 48) | ((k + 1) << 24) | word
+    return _pack([(k, 24, 8)], [(word, 0, 24)], mode, 2,
+                 "allreduce_nvls_fault: mode 0 or 1, k below 255, word below 2^24")
 
 
 def atomics_fault(issuer: int, target: int) -> int:
     """The CDPROBE_OPT_ATOMICS_FAULT value that makes the first op of timed rep 1 of cell (issuer, target) step by 2."""
-    return ((issuer + 1) << 16) | (target + 1)
+    return _pack([(issuer, 16, 16), (target, 0, 16)])
 
 
 def pingpong_fault(initiator: int, target: int, trip: int) -> int:
     """The CDPROBE_OPT_PINGPONG_FAULT value that arms a skip-ahead echo at `trip` of timed rep 1 of cell
     (initiator, target)."""
-    return ((initiator + 1) << 32) | ((target + 1) << 16) | trip
+    return _pack([(initiator, 32, 16), (target, 16, 16)], [(trip, 0, 16)])
 
 
 # Every symbol include/cdprobe.h declares: name -> (restype, argtypes)

@@ -80,18 +80,63 @@ def _mat(t, a, keep=None):
             for i in range(t.n)]
 
 
+def _row(t, a, keep=None):
+    """The n entries [r] of a CDPROBE_MAX_GPUS-long array of result `t`; None where keep(r) is false."""
+    return [a[r] if keep is None or keep(r) else None for r in range(t.n)]
+
+
+def _sized(t, a):
+    """Each entry of the per-size array `a` of result `t`, as a list cut to the ladder's n_sizes."""
+    return [list(x)[:t.n_sizes] for x in a]
+
+
+def _measured(t):
+    """keep: entry k of `t` (a cell or a rank) was measured."""
+    return lambda k: t.measured[k]
+
+
+def _timed(t):
+    """keep: entry k of `t` (a cell or a rank) was measured and did not pass timeout_ms."""
+    return lambda k: t.measured[k] and t.status[k] != abi.ERR_TIMEOUT
+
+
 def _timed_cells(t) -> dict:
-    """The per-cell fields of a Latency or a PingPong.  A cell that was not measured is None in every matrix but
-    `status`; a cell that timed out keeps its digest but has no times."""
-    def measured(k):
-        return t.measured[k]
-
-    def timed(k):
-        return t.measured[k] and t.status[k] != abi.ERR_TIMEOUT
-
+    """The per-cell fields of a Latency, a PingPong or an Atomics.  A cell that was not measured is None in every
+    matrix but `status`; a cell that timed out keeps its digest but has no times."""
+    timed = _timed(t)
     return dict(measured=_mat(t, [bool(m) for m in t.measured]), status=_mat(t, t.status),
                 ns_min=_mat(t, t.ns_min, timed), ns_median=_mat(t, t.ns_median, timed), ns_max=_mat(t, t.ns_max, timed),
-                digest=_mat(t, t.digest, measured), ms=t.ms, raw=t)
+                digest=_mat(t, t.digest, _measured(t)), ms=t.ms, raw=t)
+
+
+def _ladder(t, shape, keep) -> dict:
+    """The fields every ladder measurement has, per cell (shape _mat) or per rank (shape _row): `sizes`, `measured`,
+    `status`, and where keep, the summary of the medians and the times per size."""
+    return dict(sizes=list(t.size)[:t.n_sizes], measured=shape(t, [bool(m) for m in t.measured]),
+                status=shape(t, t.status), t0_ns=shape(t, t.t0_ns, keep), peak_gbps=shape(t, t.peak_gbps, keep),
+                half_bytes=shape(t, t.half_bytes, keep), ns_min=shape(t, _sized(t, t.ns_min), keep),
+                ns_median=shape(t, _sized(t, t.ns_median), keep), ns_max=shape(t, _sized(t, t.ns_max), keep),
+                ms=t.ms, raw=t)
+
+
+def _curve(t, shape) -> dict:
+    """The fields a BwCurve, a Memcpy and an AllReduce share: the ladder's and the (S, X) check's, each None but
+    `measured` and `status` where the entry was not measured or timed out."""
+    timed = _timed(t)
+    return dict(_ladder(t, shape, timed), bad_sizes=shape(t, t.bad_sizes, timed),
+                sum=shape(t, _sized(t, t.sum), timed), xr=shape(t, _sized(t, t.xr), timed))
+
+
+def _cell_checks(t) -> dict:
+    """The per-cell check fields of an AllToAll and a CeAllToAll, each None but `cell_measured` and `cell_status`
+    where the block was not checked or its check timed out."""
+    def checked(c):
+        return t.cell_measured[c] and t.cell_status[c] != abi.ERR_TIMEOUT
+
+    return dict(cell_measured=_mat(t, [bool(m) for m in t.cell_measured]), cell_status=_mat(t, t.cell_status),
+                bad_sizes=_mat(t, t.bad_sizes, checked), bad_words=_mat(t, _sized(t, t.bad_words), checked),
+                first_bad=_mat(t, _sized(t, t.first_bad), checked), sum=_mat(t, _sized(t, t.sum), checked),
+                xr=_mat(t, _sized(t, t.xr), checked))
 
 
 @dataclasses.dataclass
@@ -328,21 +373,7 @@ class BwCurve:
 
     @staticmethod
     def from_c(t: abi.BwCurveT) -> "BwCurve":
-        k = t.n_sizes
-
-        def timed(c):
-            return t.measured[c] and t.status[c] != abi.ERR_TIMEOUT
-
-        def per_size(a):
-            return [list(x)[:k] for x in a]
-
-        return BwCurve(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
-                       sizes=list(t.size)[:k], measured=_mat(t, [bool(m) for m in t.measured]),
-                       status=_mat(t, t.status), bad_sizes=_mat(t, t.bad_sizes, timed),
-                       t0_ns=_mat(t, t.t0_ns, timed), peak_gbps=_mat(t, t.peak_gbps, timed),
-                       half_bytes=_mat(t, t.half_bytes, timed), ns_min=_mat(t, per_size(t.ns_min), timed),
-                       ns_median=_mat(t, per_size(t.ns_median), timed), ns_max=_mat(t, per_size(t.ns_max), timed),
-                       sum=_mat(t, per_size(t.sum), timed), xr=_mat(t, per_size(t.xr), timed), ms=t.ms, raw=t)
+        return BwCurve(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq, **_curve(t, _mat))
 
 
 @dataclasses.dataclass
@@ -378,21 +409,10 @@ class AllReduce:
 
     @staticmethod
     def from_c(t: abi.AllReduceT) -> "AllReduce":
-        k = t.n_sizes
-
-        def timed(r):
-            return t.measured[r] and t.status[r] != abi.ERR_TIMEOUT
-
-        def row(a, per_size=False):
-            return [(list(a[r])[:k] if per_size else a[r]) if timed(r) else None for r in range(t.n)]
-
+        timed = _timed(t)
         return AllReduce(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
-                         sizes=list(t.size)[:k], measured=[bool(t.measured[r]) for r in range(t.n)],
-                         status=list(t.status)[:t.n], bad_sizes=row(t.bad_sizes), t0_ns=row(t.t0_ns),
-                         peak_gbps=row(t.peak_gbps), half_bytes=row(t.half_bytes), ns_min=row(t.ns_min, True),
-                         ns_median=row(t.ns_median, True), ns_max=row(t.ns_max, True), sum=row(t.sum, True),
-                         xr=row(t.xr, True), bad_words=row(t.bad_words, True), first_bad=row(t.first_bad, True),
-                         ms=t.ms, raw=t)
+                         bad_words=_row(t, _sized(t, t.bad_words), timed),
+                         first_bad=_row(t, _sized(t, t.first_bad), timed), **_curve(t, _row))
 
 
 @dataclasses.dataclass
@@ -433,30 +453,9 @@ class AllToAll:
 
     @staticmethod
     def from_c(t: abi.AllToAllT) -> "AllToAll":
-        k, n, M = t.n_sizes, t.n, abi.MAX_GPUS
-
-        def timed(r):
-            return t.measured[r] and t.status[r] != abi.ERR_TIMEOUT
-
-        def row(a, per_size=False):
-            return [(list(a[r])[:k] if per_size else a[r]) if timed(r) else None for r in range(n)]
-
-        def checked(c):
-            return t.cell_measured[c] and t.cell_status[c] != abi.ERR_TIMEOUT
-
-        def cells(a, per_size=True):
-            return [[(list(a[s * M + d])[:k] if per_size else a[s * M + d]) if checked(s * M + d) else None
-                     for d in range(n)] for s in range(n)]
-
-        return AllToAll(n=n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
-                        area_bytes=t.area_bytes, sizes=list(t.size)[:k], measured=[bool(t.measured[r]) for r in range(n)],
-                        status=list(t.status)[:n], blocks=[t.blocks[r] if t.measured[r] else None for r in range(n)],
-                        t0_ns=row(t.t0_ns), peak_gbps=row(t.peak_gbps), half_bytes=row(t.half_bytes),
-                        ns_min=row(t.ns_min, True), ns_median=row(t.ns_median, True), ns_max=row(t.ns_max, True),
-                        cell_measured=[[bool(t.cell_measured[s * M + d]) for d in range(n)] for s in range(n)],
-                        cell_status=[[t.cell_status[s * M + d] for d in range(n)] for s in range(n)],
-                        bad_sizes=cells(t.bad_sizes, False), bad_words=cells(t.bad_words),
-                        first_bad=cells(t.first_bad), sum=cells(t.sum), xr=cells(t.xr), ms=t.ms, raw=t)
+        return AllToAll(n=t.n, row_mask=t.row_mask, reps=t.reps, path=t.path, call_seq=t.call_seq,
+                        area_bytes=t.area_bytes, blocks=_row(t, t.blocks, _measured(t)), **_ladder(t, _row, _timed(t)),
+                        **_cell_checks(t))
 
 
 @dataclasses.dataclass
@@ -493,23 +492,10 @@ class Memcpy:
 
     @staticmethod
     def from_c(t: abi.MemcpyT) -> "Memcpy":
-        k = t.n_sizes
-
-        def timed(c):
-            return t.measured[c] and t.status[c] != abi.ERR_TIMEOUT
-
-        def per_size(a):
-            return [list(x)[:k] for x in a]
-
+        timed = _timed(t)
         return Memcpy(n=t.n, row_mask=t.row_mask, reps=t.reps, op=t.op, call_seq=t.call_seq, area_bytes=t.area_bytes,
-                      sizes=list(t.size)[:k], measured=_mat(t, [bool(m) for m in t.measured]),
-                      status=_mat(t, t.status), bad_sizes=_mat(t, t.bad_sizes, timed),
-                      t0_ns=_mat(t, t.t0_ns, timed), peak_gbps=_mat(t, t.peak_gbps, timed),
-                      half_bytes=_mat(t, t.half_bytes, timed), ns_min=_mat(t, per_size(t.ns_min), timed),
-                      ns_median=_mat(t, per_size(t.ns_median), timed), ns_max=_mat(t, per_size(t.ns_max), timed),
-                      sum=_mat(t, per_size(t.sum), timed), xr=_mat(t, per_size(t.xr), timed),
-                      bad_words=_mat(t, per_size(t.bad_words), timed),
-                      first_bad=_mat(t, per_size(t.first_bad), timed), ms=t.ms, raw=t)
+                      bad_words=_mat(t, _sized(t, t.bad_words), timed),
+                      first_bad=_mat(t, _sized(t, t.first_bad), timed), **_curve(t, _mat))
 
 
 @dataclasses.dataclass
@@ -553,31 +539,16 @@ class CeAllToAll:
 
     @staticmethod
     def from_c(t: abi.CeAllToAllT) -> "CeAllToAll":
-        k, n, M = t.n_sizes, t.n, abi.MAX_GPUS
+        measured = _measured(t)
 
-        def row(a, per_size=False):
-            return [(list(a[r])[:k] if per_size else a[r]) if t.measured[r] else None for r in range(n)]
+        def issued(c):
+            # rank s issues a cell to every peer, and to itself only with a loop-back slice (then it copies n blocks)
+            s, d = divmod(c, abi.MAX_GPUS)
+            return t.measured[s] and (s != d or t.blocks[s] == t.n)
 
-        def checked(c):
-            return t.cell_measured[c] and t.cell_status[c] != abi.ERR_TIMEOUT
-
-        def cells(a, per_size=True):
-            return [[(list(a[s * M + d])[:k] if per_size else a[s * M + d]) if checked(s * M + d) else None
-                     for d in range(n)] for s in range(n)]
-
-        # rank s issues a cell to every peer, and to itself only with a loop-back slice (then it copies n blocks)
-        copy = [[list(t.copy_ns_median[s * M + d])[:k] if t.measured[s] and (s != d or t.blocks[s] == n) else None
-                 for d in range(n)] for s in range(n)]
-        return CeAllToAll(n=n, row_mask=t.row_mask, reps=t.reps, op=t.op, call_seq=t.call_seq,
-                          area_bytes=t.area_bytes, sizes=list(t.size)[:k],
-                          measured=[bool(t.measured[r]) for r in range(n)], status=list(t.status)[:n],
-                          blocks=row(t.blocks), t0_ns=row(t.t0_ns), peak_gbps=row(t.peak_gbps),
-                          half_bytes=row(t.half_bytes), ns_min=row(t.ns_min, True), ns_median=row(t.ns_median, True),
-                          ns_max=row(t.ns_max, True),
-                          cell_measured=[[bool(t.cell_measured[s * M + d]) for d in range(n)] for s in range(n)],
-                          cell_status=[[t.cell_status[s * M + d] for d in range(n)] for s in range(n)],
-                          bad_sizes=cells(t.bad_sizes, False), copy_ns_median=copy, bad_words=cells(t.bad_words),
-                          first_bad=cells(t.first_bad), sum=cells(t.sum), xr=cells(t.xr), ms=t.ms, raw=t)
+        return CeAllToAll(n=t.n, row_mask=t.row_mask, reps=t.reps, op=t.op, call_seq=t.call_seq,
+                          area_bytes=t.area_bytes, blocks=_row(t, t.blocks, measured), **_ladder(t, _row, measured),
+                          copy_ns_median=_mat(t, _sized(t, t.copy_ns_median), issued), **_cell_checks(t))
 
 
 @dataclasses.dataclass
@@ -630,6 +601,19 @@ class Probe:
         if rc != abi.OK:
             self._h = C.c_void_p()
             _raise(self._lib, rc, "cdprobe_open")
+
+    def _call(self, fn: str, out_type, *args):
+        """Entry point `fn` called with the handle, `args` and a new `out_type` to fill: (return code, the out struct
+        as the library left it)."""
+        out = out_type()
+        return getattr(self._lib, fn)(self._h, *args, C.byref(out)), out
+
+    def _decode(self, fn: str, result_type, call):
+        """The (return code, out struct) `call` of entry point `fn` decoded as a `result_type`; a ProbeError named
+        after `fn` when the code is not OK."""
+        rc, out = call
+        _check(self._lib, rc, fn)
+        return result_type.from_c(out)
 
     # -- Go: (*Probe).Run -------------------------------------------------------------
     def Run(self, gather: bool = False, allow_timeout: bool = False) -> Result:
@@ -702,83 +686,60 @@ class Probe:
         issuer, i.e. through the fabric; the target reads it at rest) and diffs it against the pattern.
         op: abi.OP_READ / abi.OP_WRITE or "read" / "write"."""
         op = {"read": abi.OP_READ, "write": abi.OP_WRITE}.get(op, op)
-        rc, d = self.diagnose_raw(op, issuer, target, issuer if reader is None else reader)
-        _check(self._lib, rc, "cdprobe_diagnose")
-        return Diagnosis.from_c(d)
+        reader = issuer if reader is None else reader
+        return self._decode("cdprobe_diagnose", Diagnosis, self.diagnose_raw(op, issuer, target, reader))
 
     def diagnose_raw(self, op: int, issuer: int, target: int, reader: int):
         """The bare ABI call: (return code, abi.DiagT as the library left it)."""
-        d = abi.DiagT()
-        rc = self._lib.cdprobe_diagnose(self._h, op, issuer, target, reader, C.byref(d))
-        return rc, d
+        return self._call("cdprobe_diagnose", abi.DiagT, op, issuer, target, reader)
 
     def Latency(self, hops: int = 0, reps: int = 0) -> Latency:
         """Go: (*Probe).Latency.  Dependent-load latency of every cell whose issuer is local (0: 1024 hops, 8 timed
         reps).  Needs no Run first and disturbs none."""
-        rc, t = self.latency_raw(hops, reps)
-        _check(self._lib, rc, "cdprobe_latency")
-        return Latency.from_c(t)
+        return self._decode("cdprobe_latency", Latency, self.latency_raw(hops, reps))
 
     def latency_raw(self, hops: int, reps: int):
         """The bare ABI call: (return code, abi.LatencyT as the library left it)."""
-        t = abi.LatencyT()
-        rc = self._lib.cdprobe_latency(self._h, hops, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_latency", abi.LatencyT, hops, reps)
 
     def PingPong(self, trips: int = 0, reps: int = 0, fenced: bool = False) -> PingPong:
         """Go: (*Probe).PingPong.  Signal round trip of every off-diagonal cell over the tournament's pairs (0: 256
         round trips, 8 timed reps); fenced: a fence.sys before every store.  Collective when world_size > 1.  Needs no
         Run first and disturbs none."""
-        rc, t = self.pingpong_raw(trips, reps, 1 if fenced else 0)
-        _check(self._lib, rc, "cdprobe_pingpong")
-        return PingPong.from_c(t)
+        return self._decode("cdprobe_pingpong", PingPong, self.pingpong_raw(trips, reps, 1 if fenced else 0))
 
     def pingpong_raw(self, trips: int, reps: int, fenced: int):
         """The bare ABI call: (return code, abi.PingPongT as the library left it)."""
-        t = abi.PingPongT()
-        rc = self._lib.cdprobe_pingpong(self._h, trips, reps, fenced, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_pingpong", abi.PingPongT, trips, reps, fenced)
 
     def Atomics(self, kind: int, ops: int = 0, reps: int = 0) -> Atomics:
         """Go: (*Probe).Atomics.  Remote atomics of every cell whose issuer is local (kind: abi.ATOMIC_*; 0: 1024 ops
         per lane, 8 timed reps).  One-sided, not collective.  Needs no Run first and disturbs none."""
-        rc, t = self.atomics_raw(kind, ops, reps)
-        _check(self._lib, rc, "cdprobe_atomics")
-        return Atomics.from_c(t)
+        return self._decode("cdprobe_atomics", Atomics, self.atomics_raw(kind, ops, reps))
 
     def atomics_raw(self, kind: int, ops: int, reps: int):
         """The bare ABI call: (return code, abi.AtomicsT as the library left it)."""
-        t = abi.AtomicsT()
-        rc = self._lib.cdprobe_atomics(self._h, kind, ops, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_atomics", abi.AtomicsT, kind, ops, reps)
 
     def BwCurve(self, reps: int = 0) -> BwCurve:
         """Go: (*Probe).BwCurve.  Bandwidth versus transfer size of every cell whose issuer is local, on the probe's
         read path and grid (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first and
         disturbs none."""
-        rc, t = self.bwcurve_raw(reps)
-        _check(self._lib, rc, "cdprobe_bwcurve")
-        return BwCurve.from_c(t)
+        return self._decode("cdprobe_bwcurve", BwCurve, self.bwcurve_raw(reps))
 
     def bwcurve_raw(self, reps: int):
         """The bare ABI call: (return code, abi.BwCurveT as the library left it)."""
-        t = abi.BwCurveT()
-        rc = self._lib.cdprobe_bwcurve(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_bwcurve", abi.BwCurveT, reps)
 
     def AllReduce(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReduce.  One-shot all-reduce of every rank's source buffer on every rank at once, at each
         size of the bwcurve ladder, on the probe's read path and grid (0: 8 timed reps per size).  Collective when
         world_size > 1.  Needs no Run first and disturbs none."""
-        rc, t = self.allreduce_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce", AllReduce, self.allreduce_raw(reps))
 
     def allreduce_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce", abi.AllReduceT, reps)
 
     def AllReduceTwoShot(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReduceTwoShot.  Two-shot all-reduce (reduce-scatter, then a pushed all-gather) of every
@@ -786,15 +747,11 @@ class Probe:
         grid (0: 8 timed reps per size).  The result is an AllReduce whose bad_words and first_bad cover every rep;
         the nccl-tests bus bandwidth is peak_gbps x 2 (n - 1) / n.  Collective when world_size > 1.  Needs no Run first
         and disturbs none."""
-        rc, t = self.allreduce_twoshot_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce_twoshot")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce_twoshot", AllReduce, self.allreduce_twoshot_raw(reps))
 
     def allreduce_twoshot_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce_twoshot(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce_twoshot", abi.AllReduceT, reps)
 
     def AllReduceLL(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReduceLL.  Low-latency all-reduce of every rank's source buffer on every rank at once:
@@ -802,15 +759,11 @@ class Probe:
         (the bwcurve ladder up to 1 MiB), on the probe's grids (0: 8 timed reps per size).  A rep is timed from the end
         of the rank's previous rep; path is abi.ALLREDUCE_PATH_LL.  Collective when world_size > 1.  Needs no Run
         first and disturbs none."""
-        rc, t = self.allreduce_ll_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce_ll")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce_ll", AllReduce, self.allreduce_ll_raw(reps))
 
     def allreduce_ll_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce_ll(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce_ll", abi.AllReduceT, reps)
 
     def AllReduceRing(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReduceRing.  Ring all-reduce of every rank's source buffer on every rank at once: each
@@ -818,15 +771,11 @@ class Probe:
         with no barrier or fence between them, at each size of the bwcurve ladder, on the probe's grids (0: 8 timed
         reps per size).  A rep is timed from its opening barrier to the moment the rank's output is complete; path is
         abi.ALLREDUCE_PATH_RING.  Collective when world_size > 1.  Needs no Run first and disturbs none."""
-        rc, t = self.allreduce_ring_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce_ring")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce_ring", AllReduce, self.allreduce_ring_raw(reps))
 
     def allreduce_ring_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce_ring(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce_ring", abi.AllReduceT, reps)
 
     def AllReducePush(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReducePush.  Push all-reduce of every rank's source buffer on every rank at once, every byte
@@ -835,15 +784,11 @@ class Probe:
         of the bwcurve ladder, on the probe's data path and grids (0: 8 timed reps per size).  A rep is timed from its
         opening to its closing barrier; path is the handle's.  Collective when world_size > 1.  Needs no Run first and
         disturbs none."""
-        rc, t = self.allreduce_push_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce_push")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce_push", AllReduce, self.allreduce_push_raw(reps))
 
     def allreduce_push_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce_push(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce_push", abi.AllReduceT, reps)
 
     def AllReduceNVLS(self, reps: int = 0) -> AllReduce:
         """Go: (*Probe).AllReduceNVLS.  Multicast (NVLS) all-reduce of every rank's source buffer on every rank at once:
@@ -852,29 +797,21 @@ class Probe:
         reps per size).  A rep is timed from its opening to its closing barrier; path is ALLREDUCE_PATH_NVLS.  Rows are
         ERR_UNSUPPORTED, with nothing run, where the devices, the driver or a shared device rule multicast out.
         Collective when world_size > 1.  Needs no Run first and disturbs none."""
-        rc, t = self.allreduce_nvls_raw(reps)
-        _check(self._lib, rc, "cdprobe_allreduce_nvls")
-        return AllReduce.from_c(t)
+        return self._decode("cdprobe_allreduce_nvls", AllReduce, self.allreduce_nvls_raw(reps))
 
     def allreduce_nvls_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllReduceT as the library left it)."""
-        t = abi.AllReduceT()
-        rc = self._lib.cdprobe_allreduce_nvls(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_allreduce_nvls", abi.AllReduceT, reps)
 
     def AllToAll(self, reps: int = 0) -> AllToAll:
         """Go: (*Probe).AllToAll.  One-shot all-to-all: every rank pushes a block to every peer at once, at each size of
         the bwcurve ladder, on the probe's write path and grid, and every receiver checks every word (0: 8 timed reps
         per size).  Collective when world_size > 1.  Needs no Run first and disturbs none."""
-        rc, t = self.alltoall_raw(reps)
-        _check(self._lib, rc, "cdprobe_alltoall")
-        return AllToAll.from_c(t)
+        return self._decode("cdprobe_alltoall", AllToAll, self.alltoall_raw(reps))
 
     def alltoall_raw(self, reps: int):
         """The bare ABI call: (return code, abi.AllToAllT as the library left it)."""
-        t = abi.AllToAllT()
-        rc = self._lib.cdprobe_alltoall(self._h, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_alltoall", abi.AllToAllT, reps)
 
     def Memcpy(self, op: int, reps: int = 0) -> Memcpy:
         """Go: (*Probe).Memcpy.  Copy-engine bandwidth versus transfer size of every cell whose issuer is local:
@@ -882,15 +819,11 @@ class Probe:
         abi.OP_READ, a pull) or from the issuer into the target's (abi.OP_WRITE, a push), each copy timed by CUDA events
         and every landed word checked (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first
         and disturbs none."""
-        rc, t = self.memcpy_raw(op, reps)
-        _check(self._lib, rc, "cdprobe_memcpy")
-        return Memcpy.from_c(t)
+        return self._decode("cdprobe_memcpy", Memcpy, self.memcpy_raw(op, reps))
 
     def memcpy_raw(self, op: int, reps: int):
         """The bare ABI call: (return code, abi.MemcpyT as the library left it)."""
-        t = abi.MemcpyT()
-        rc = self._lib.cdprobe_memcpy(self._h, op, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_memcpy", abi.MemcpyT, op, reps)
 
     def CeAllToAll(self, op: int, reps: int = 0) -> CeAllToAll:
         """Go: (*Probe).CeAllToAll.  Copy-engine all-to-all: in every rep every cell of Memcpy copies its block at
@@ -898,22 +831,16 @@ class Probe:
         signalling each other by stream memory operations, at each size of the bwcurve ladder; the owner of every block
         checks every word (0: 8 timed reps per size).  Collective when world_size > 1.  Needs no Run first and disturbs
         none."""
-        rc, t = self.ce_alltoall_raw(op, reps)
-        _check(self._lib, rc, "cdprobe_ce_alltoall")
-        return CeAllToAll.from_c(t)
+        return self._decode("cdprobe_ce_alltoall", CeAllToAll, self.ce_alltoall_raw(op, reps))
 
     def ce_alltoall_raw(self, op: int, reps: int):
         """The bare ABI call: (return code, abi.CeAllToAllT as the library left it)."""
-        t = abi.CeAllToAllT()
-        rc = self._lib.cdprobe_ce_alltoall(self._h, op, reps, C.byref(t))
-        return rc, t
+        return self._call("cdprobe_ce_alltoall", abi.CeAllToAllT, op, reps)
 
     def Links(self) -> Links:
         """Go: (*Probe).Links.  The per-link NVLink counters of the last Run taken with abi.OPT_LINK_COUNTERS on, one
         entry per distinct local device.  One-sided, not collective."""
-        t = abi.LinksT()
-        _check(self._lib, self._lib.cdprobe_links(self._h, C.byref(t)), "cdprobe_links")
-        return Links.from_c(t)
+        return self._decode("cdprobe_links", Links, self._call("cdprobe_links", abi.LinksT))
 
     def Close(self) -> None:
         if self._h:
