@@ -1,5 +1,5 @@
 // handle.cc — the probe handle behind the C ABI (include/cdprobe.h): open and close, peer mappings, options, fault
-// hooks and the run path.  The on-demand measurements (diagnose, latency, pingpong) are in measure.cc.
+// hooks and the run path.  The on-demand measurements are in measure.cc.
 //
 // Who calls this: the compute-domain-daemon's `run()` owns one handle for the
 // life of the pod (reference: cmd/compute-domain-daemon/main.go:212-347; the
@@ -502,6 +502,26 @@ static int set_flag(cdprobe* h, uint32_t flag, bool on) {
   }
   return rc;
 }
+
+// The option that arms each measurement's test fault (cdprobe_set_option).  Every value is accepted when it is set:
+// what it names depends on the domain and the call's arguments, so the call checks it.
+struct FaultOption {
+  uint32_t option;
+  Measurement meas;
+};
+constexpr FaultOption kFaultOptions[] = {
+    {CDPROBE_OPT_PINGPONG_FAULT, kMeasPingPong},
+    {CDPROBE_OPT_ATOMICS_FAULT, kMeasAtomics},
+    {CDPROBE_OPT_ALLREDUCE_FAULT, kMeasAllReduce},
+    {CDPROBE_OPT_ALLTOALL_FAULT, kMeasAllToAll},
+    {CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT, kMeasTwoShot},
+    {CDPROBE_OPT_ALLREDUCE_LL_FAULT, kMeasLl},
+    {CDPROBE_OPT_ALLREDUCE_RING_FAULT, kMeasRing},
+    {CDPROBE_OPT_ALLREDUCE_PUSH_FAULT, kMeasPush},
+    {CDPROBE_OPT_ALLREDUCE_NVLS_FAULT, kMeasNvls},
+    {CDPROBE_OPT_MEMCPY_FAULT, kMeasMemcpy},
+    {CDPROBE_OPT_CE_ALLTOALL_FAULT, kMeasCeAllToAll},
+};
 
 static void fill_params(const cdprobe* h, uint32_t li, const Phase* phases, uint32_t n_phases, uint32_t peer_mask,
                         ProbeParams* P) {
@@ -1294,6 +1314,12 @@ int cdprobe_trace(cdprobe_t* h, uint32_t local, cdprobe_trace_t* out) {
 
 int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
   if (h == nullptr) return CDPROBE_ERR_ARG;
+  for (const cdp::FaultOption& o : cdp::kFaultOptions) {
+    if (o.option == option) {
+      h->meas[o.meas].fault = value;
+      return CDPROBE_OK;
+    }
+  }
   switch (option) {
     case CDPROBE_OPT_EVENT_TIMING:
       h->event_timing = value != 0;
@@ -1360,42 +1386,6 @@ int cdprobe_set_option(cdprobe_t* h, uint32_t option, uint64_t value) {
       if (value == 0 || value > 65535) return CDPROBE_ERR_ARG;
       h->verify_ctas = (uint32_t)value;
       return cdp::rebuild_all(h);
-    case CDPROBE_OPT_PINGPONG_FAULT:  // checked against the call's arguments by cdprobe_pingpong
-      h->pp_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ATOMICS_FAULT:  // checked against the domain by cdprobe_atomics
-      h->at_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_FAULT:  // checked against the domain and the size ladder by cdprobe_allreduce
-      h->ar_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLTOALL_FAULT:  // checked against the domain and the size ladder by cdprobe_alltoall
-      h->a2a_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT:  // checked against the domain and the ladder by cdprobe_allreduce_twoshot
-      h->ar2_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_LL_FAULT:  // checked against the domain, the ladder and timeout_ms by cdprobe_allreduce_ll
-      h->ll_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_RING_FAULT:  // checked against the domain, the ladder, the chunks and timeout_ms by
-                                            // cdprobe_allreduce_ring
-      h->ring_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_PUSH_FAULT:  // checked against the domain, the ladder and the chunks by
-                                            // cdprobe_allreduce_push
-      h->push_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_ALLREDUCE_NVLS_FAULT:  // checked against the ladder and the chunks by cdprobe_allreduce_nvls
-      h->nvls_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_MEMCPY_FAULT:  // checked against the domain and the size ladder by cdprobe_memcpy
-      h->memcpy_fault = value;
-      return CDPROBE_OK;
-    case CDPROBE_OPT_CE_ALLTOALL_FAULT:  // checked against the domain, the size ladder and timeout_ms by
-                                         // cdprobe_ce_alltoall
-      h->cea_fault = value;
-      return CDPROBE_OK;
     case CDPROBE_OPT_LINK_COUNTERS:
       if (value > 1) return CDPROBE_ERR_ARG;
       if (value != 0 && h->links == nullptr)

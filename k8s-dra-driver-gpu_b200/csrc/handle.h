@@ -92,6 +92,24 @@ struct NvlsArea {
   bool mc_mapped[kMaxRanks] = {}, uc_mapped[kMaxRanks] = {};
 };
 
+// The measurements that keep a record on the handle (cdprobe::meas), one per entry point; the all-reduces are
+// cdprobe_allreduce, cdprobe_allreduce_twoshot, _ll, _ring, _push and _nvls.
+enum Measurement : uint32_t {
+  kMeasPingPong, kMeasAtomics, kMeasBwCurve,
+  kMeasAllReduce, kMeasTwoShot, kMeasLl, kMeasRing, kMeasPush, kMeasNvls,
+  kMeasAllToAll, kMeasMemcpy, kMeasCeAllToAll,
+  kMeasCount
+};
+
+// What a measurement keeps on the handle between calls.  `calls` counts its calls that ran, so it is the call_seq of
+// the last one; the words, flags and values its kernels exchange derive from it.  `fault` is its armed test fault, the
+// value of its CDPROBE_OPT_*_FAULT option (handle.cc, kFaultOptions), 0: disarmed; the call checks it.
+// cdprobe_bwcurve has no fault option, so its fault stays 0.
+struct MeasRecord {
+  uint64_t calls = 0;
+  uint64_t fault = 0;
+};
+
 }  // namespace cdp
 
 struct cdprobe {
@@ -133,29 +151,7 @@ struct cdprobe {
   double last_probe_ms = 0.0;    // host wall clock of the previous run (wait_rows: how long to spin hot)
   uint32_t verify_ctas = 32;  // CTAs that verify landing slots under CDPROBE_FLAG_OVERLAP_VERIFY
   int32_t fault_local = -1;   // local rank whose Ctrl holds the armed landing fault (cdprobe_corrupt_landing), -1: none
-  uint64_t pp_calls = 0;      // cdprobe_pingpong calls that ran (call_seq of the last one)
-  uint64_t pp_fault = 0;      // CDPROBE_OPT_PINGPONG_FAULT value, 0: disarmed
-  uint64_t at_calls = 0;      // cdprobe_atomics calls that ran (call_seq of the last one)
-  uint64_t at_fault = 0;      // CDPROBE_OPT_ATOMICS_FAULT value, 0: disarmed
-  uint64_t bw_calls = 0;      // cdprobe_bwcurve calls that ran (call_seq of the last one)
-  uint64_t ar_calls = 0;      // cdprobe_allreduce calls that ran (call_seq of the last one)
-  uint64_t ar_fault = 0;      // CDPROBE_OPT_ALLREDUCE_FAULT value, 0: disarmed
-  uint64_t a2a_calls = 0;     // cdprobe_alltoall calls that ran (call_seq of the last one)
-  uint64_t a2a_fault = 0;     // CDPROBE_OPT_ALLTOALL_FAULT value, 0: disarmed
-  uint64_t ar2_calls = 0;     // cdprobe_allreduce_twoshot calls that ran (call_seq of the last one)
-  uint64_t ar2_fault = 0;     // CDPROBE_OPT_ALLREDUCE_TWOSHOT_FAULT value, 0: disarmed
-  uint64_t ll_calls = 0;      // cdprobe_allreduce_ll calls that ran (call_seq of the last one)
-  uint64_t ll_fault = 0;      // CDPROBE_OPT_ALLREDUCE_LL_FAULT value, 0: disarmed
-  uint64_t ring_calls = 0;    // cdprobe_allreduce_ring calls that ran (call_seq of the last one)
-  uint64_t ring_fault = 0;    // CDPROBE_OPT_ALLREDUCE_RING_FAULT value, 0: disarmed
-  uint64_t push_calls = 0;    // cdprobe_allreduce_push calls that ran (call_seq of the last one)
-  uint64_t push_fault = 0;    // CDPROBE_OPT_ALLREDUCE_PUSH_FAULT value, 0: disarmed
-  uint64_t nvls_calls = 0;    // cdprobe_allreduce_nvls calls that ran (call_seq of the last one)
-  uint64_t nvls_fault = 0;    // CDPROBE_OPT_ALLREDUCE_NVLS_FAULT value, 0: disarmed
-  uint64_t memcpy_calls = 0;  // cdprobe_memcpy calls that ran (call_seq of the last one)
-  uint64_t memcpy_fault = 0;  // CDPROBE_OPT_MEMCPY_FAULT value, 0: disarmed
-  uint64_t cea_calls = 0;             // cdprobe_ce_alltoall calls that ran (call_seq of the last one)
-  uint64_t cea_fault = 0;             // CDPROBE_OPT_CE_ALLTOALL_FAULT value, 0: disarmed
+  cdp::MeasRecord meas[cdp::kMeasCount];  // [Measurement]
   // the pinned host block of cdprobe_memcpy and cdprobe_ce_alltoall (measure.cc), made by the first call of either:
   // the tickets their streams wait on and what their checks leave
   cdp::CopyHost* copy_host = nullptr;

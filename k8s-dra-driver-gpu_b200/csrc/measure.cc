@@ -563,8 +563,7 @@ struct ArFault {
 // One all-reduce protocol, as allreduce_call runs it.
 struct ArProtocol {
   const char* fn;                                // the entry point, which names the call in every message
-  uint64_t cdprobe::*calls;                      // its calls that ran
-  uint64_t cdprobe::*fault;                      // its armed fault, 0: disarmed
+  Measurement meas;                              // its record on the handle: calls that ran, armed fault
   uint32_t (*rule)(uint64_t, uint64_t*);         // its size ladder
   uint32_t path;                                 // out->path: kHandlePath, or its own
   SharedAlloc cdprobe::*area;                    // the shared area peers write, nullptr: none
@@ -767,45 +766,44 @@ static int nvls_launch(cdprobe* h, LocalRank& L, const DomainLines& dom, const L
 }
 
 constexpr ArProtocol kOneShot = {
-    "cdprobe_allreduce", &cdprobe::ar_calls, &cdprobe::ar_fault, bwcurve_ladder, kHandlePath, nullptr, nullptr,
-    nullptr, true, kArOff, oneshot_fault, oneshot_launch};
+    "cdprobe_allreduce", kMeasAllReduce, bwcurve_ladder, kHandlePath, nullptr, nullptr, nullptr, true, kArOff,
+    oneshot_fault, oneshot_launch};
 constexpr ArProtocol kTwoShot = {
-    "cdprobe_allreduce_twoshot", &cdprobe::ar2_calls, &cdprobe::ar2_fault, bwcurve_ladder, kHandlePath,
-    &cdprobe::gather, [](uint32_t, uint64_t s_max) { return s_max; }, nullptr, false, kAr2Off, twoshot_fault,
-    twoshot_launch};
+    "cdprobe_allreduce_twoshot", kMeasTwoShot, bwcurve_ladder, kHandlePath, &cdprobe::gather,
+    [](uint32_t, uint64_t s_max) { return s_max; }, nullptr, false, kAr2Off, twoshot_fault, twoshot_launch};
 constexpr ArProtocol kLl = {
-    "cdprobe_allreduce_ll", &cdprobe::ll_calls, &cdprobe::ll_fault, ll_ladder, CDPROBE_ALLREDUCE_PATH_LL, &cdprobe::ll,
-    ll_area_bytes, "cdprobe_allreduce_ll: zero the LL area", true, kLlOff, ll_fault, ll_launch};
+    "cdprobe_allreduce_ll", kMeasLl, ll_ladder, CDPROBE_ALLREDUCE_PATH_LL, &cdprobe::ll, ll_area_bytes,
+    "cdprobe_allreduce_ll: zero the LL area", true, kLlOff, ll_fault, ll_launch};
 constexpr ArProtocol kRing = {
-    "cdprobe_allreduce_ring", &cdprobe::ring_calls, &cdprobe::ring_fault, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_RING,
-    &cdprobe::ring, ring_area_bytes, "cdprobe_allreduce_ring: zero the ring area", false, kRingOff, ring_fault,
-    ring_launch};
+    "cdprobe_allreduce_ring", kMeasRing, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_RING, &cdprobe::ring, ring_area_bytes,
+    "cdprobe_allreduce_ring: zero the ring area", false, kRingOff, ring_fault, ring_launch};
 constexpr ArProtocol kPush = {
-    "cdprobe_allreduce_push", &cdprobe::push_calls, &cdprobe::push_fault, bwcurve_ladder, kHandlePath, &cdprobe::push,
+    "cdprobe_allreduce_push", kMeasPush, bwcurve_ladder, kHandlePath, &cdprobe::push,
     [](uint32_t, uint64_t s_max) { return s_max; }, "cdprobe_allreduce_push: zero the push area", false, kPushOff,
     push_fault, push_launch, true};
 constexpr ArProtocol kNvls = {
-    "cdprobe_allreduce_nvls", &cdprobe::nvls_calls, &cdprobe::nvls_fault, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_NVLS,
-    nullptr, nullptr, nullptr, false, kNvlsOff, nvls_fault, nvls_launch, false, true};
+    "cdprobe_allreduce_nvls", kMeasNvls, bwcurve_ladder, CDPROBE_ALLREDUCE_PATH_NVLS, nullptr, nullptr, nullptr, false,
+    kNvlsOff, nvls_fault, nvls_launch, false, true};
 
 // The all-reduces (DESIGN §5g, §5i, §5j, §5k, §5l, §5m): one call of protocol P.
 static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, const ArProtocol& P) {
   Ladder lad;
   if (const int rc = open_ladder(h, out, reps, kArDefaultReps, &lad, P.path, P.rule); rc != CDPROBE_OK) return rc;
   const uint32_t n = h->n_total;
+  MeasRecord& rec = h->meas[P.meas];
   // 1. the arguments, the armed fault, the probe mapping rows and whether any area must be zeroed; in a multi-process
   //    domain all are shared, so every process refuses, skips, zeroes or runs together.  An area that must start zeroed
   //    and is yet to be created is stale until it is zeroed
   ArFault f;
-  if (h->*P.fault != 0 && lad.bad.empty())
-    if (const char* why = P.decode(h, h->*P.fault, fault_spot(h->*P.fault, lad), lad, &f)) lad.bad = why;
+  if (rec.fault != 0 && lad.bad.empty())
+    if (const char* why = P.decode(h, rec.fault, fault_spot(rec.fault, lad), lad, &f)) lad.bad = why;
   SharedAlloc* m = P.area != nullptr ? &(h->*P.area) : nullptr;
   if (P.zeroing != nullptr) m->stale |= m->bytes == 0;
   bool zero = P.zeroing != nullptr && m->stale;
   uint32_t grid;
   int32_t st[kMaxRanks][kMaxRanks];
   bool nvls = true;
-  if (const int rc = agree(h, P.fn, lad.bad, h->*P.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero, P.native,
+  if (const int rc = agree(h, P.fn, lad.bad, rec.calls + 1, {lad.reps, 0u, 0u}, st, &grid, &zero, P.native,
                            P.nvls ? &nvls : nullptr);
       rc != CDPROBE_OK)
     return rc;
@@ -827,7 +825,7 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
     if (refused) unsupported();
     else if (rc != CDPROBE_OK) return rc;
   }
-  out->call_seq = ++(h->*P.calls);
+  out->call_seq = ++rec.calls;
   put_ladder(h, lad, out);
   // 3. every rank reads every input and writes every area: when some probe mapping or area mapping of the domain is
   //    down, nothing runs, in any process
@@ -887,7 +885,7 @@ static int allreduce_call(cdprobe* h, uint32_t reps, cdprobe_allreduce_t* out, c
   if (const int rc = domain_barrier(h); rc != CDPROBE_OK) return rc;
   for (uint32_t li = 0; li < h->n_local; ++li) {
     LocalRank& L = h->lr[li];
-    if (const int rc = P.launch(h, L, domain_lines(h, L, P.lines, h->*P.calls), lad, f, grid); rc != CDPROBE_OK)
+    if (const int rc = P.launch(h, L, domain_lines(h, L, P.lines, rec.calls), lad, f, grid); rc != CDPROBE_OK)
       return rc;
   }
 
@@ -962,14 +960,11 @@ struct CopyFault {
   uint64_t arg = 0;
 };
 
-// One copy-engine measurement, as open_copy opens it.  (Its member pointers go through an alias: nvcc's host pass warns
-// about the bare declarator, as it does for ArProtocol's.)
-using HandleCount = uint64_t cdprobe::*;
+// One copy-engine measurement, as open_copy opens it.
 struct CopyCall {
   const char* fn;                      // the entry point
   uint32_t default_reps;
-  HandleCount calls;                   // its calls that ran
-  HandleCount fault;                   // its armed fault, 0: disarmed
+  Measurement meas;                    // its record on the handle: calls that ran, armed fault
   uint64_t max_mode;                   // the highest fault mode it accepts
   const char* bad_fault;               // its refusal of an armed fault
   std::string (*refusal)(cdprobe* h);  // why this process cannot run it, empty when it can; nullptr: it always can
@@ -991,7 +986,8 @@ static int open_copy(cdprobe* h, const CopyCall& C, uint32_t op, uint32_t reps, 
   const uint32_t n = h->n_total;
   if (op != CDPROBE_OP_READ && op != CDPROBE_OP_WRITE && lad->bad.empty())
     lad->bad = "op must be CDPROBE_OP_READ or CDPROBE_OP_WRITE";
-  if (const uint64_t v = h->*C.fault; v != 0 && lad->bad.empty()) {
+  MeasRecord& rec = h->meas[C.meas];
+  if (const uint64_t v = rec.fault; v != 0 && lad->bad.empty()) {
     const uint64_t mode = v >> 48, fi = (v >> 40) & 0xffu, ft = (v >> 32) & 0xffu;
     const FaultSpot at = fault_spot(v, *lad);
     if (mode > C.max_mode || fi == 0 || fi > n || ft == 0 || ft > n || (fi == ft && !h->plan.diag) || !at.size_ok ||
@@ -1003,7 +999,7 @@ static int open_copy(cdprobe* h, const CopyCall& C, uint32_t op, uint32_t reps, 
   const std::string refusal = C.refusal != nullptr && lad->bad.empty() ? C.refusal(h) : std::string();
   bool refused = !refusal.empty();
   // agree() ors the refusal flag (its `zero`) over every process
-  if (const int rc = agree(h, C.fn, lad->bad, h->*C.calls + 1, {lad->reps, op, 0u}, st, nullptr, &refused);
+  if (const int rc = agree(h, C.fn, lad->bad, rec.calls + 1, {lad->reps, op, 0u}, st, nullptr, &refused);
       rc != CDPROBE_OK)
     return rc;
   if (refused) {
@@ -1011,7 +1007,7 @@ static int open_copy(cdprobe* h, const CopyCall& C, uint32_t op, uint32_t reps, 
     return CDPROBE_ERR_UNSUPPORTED;
   }
   if (const int rc = ensure_area(h, h->area, (size_t)n * h->plan.bpp); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++(h->*C.calls);
+  out->call_seq = ++rec.calls;
   out->area_bytes = h->area.bytes;
   put_ladder(h, *lad, out);
   return CDPROBE_OK;
@@ -1184,7 +1180,7 @@ static int memcpy_rep(cdprobe* h, const int32_t* target, uint32_t op, const Ladd
 }
 
 constexpr CopyCall kMemcpy = {
-    "cdprobe_memcpy", 8, &cdprobe::memcpy_calls, &cdprobe::memcpy_fault, 1,
+    "cdprobe_memcpy", 8, kMeasMemcpy, 1,
     "the armed memcpy fault names no cell, size or word of this call, or has a mode above 1", nullptr, nullptr};
 
 // The cells local rank li issues, one per copy stream: its peers in the order rank + 1, rank + 2, ... (mod n), then
@@ -1212,7 +1208,7 @@ static std::string ce_a2a_refusal(cdprobe* h) {
 }
 
 constexpr CopyCall kCeA2a = {
-    "cdprobe_ce_alltoall", 8, &cdprobe::cea_calls, &cdprobe::cea_fault, 2,
+    "cdprobe_ce_alltoall", 8, kMeasCeAllToAll, 2,
     "the armed copy-engine all-to-all fault names no cell, size, word or delay of this call, or has a mode above 2",
     ce_a2a_refusal,
     "cdprobe_ce_alltoall: another process cannot run it (no stream memory operations, or more streams than "
@@ -1276,7 +1272,8 @@ static int ce_a2a_rep(cdprobe* h, uint32_t op, const Ladder& lad, uint32_t k, ui
   const Plan& pl = h->plan;
   const uint32_t n = h->n_total;
   const bool push = op == CDPROBE_OP_WRITE;
-  const uint64_t ticket = ++host->issued, v = ce_a2a_value(h->cea_calls, k, rep, lad.reps), bytes = lad.size[k];
+  const uint64_t ticket = ++host->issued, bytes = lad.size[k];
+  const uint64_t v = ce_a2a_value(h->meas[kMeasCeAllToAll].calls, k, rep, lad.reps);
   const auto wait_value = [&](cudaStream_t s, CUdeviceptr a, uint64_t want) {
     return h->drv.StreamWaitValue64(s, a, want, CU_STREAM_WAIT_VALUE_GEQ);
   };
@@ -1540,9 +1537,10 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
   std::string bad;
   if (trips > cdp::kPingPongMaxTrips || reps > cdp::kMaxTimedReps || fenced > 1)
     bad = "trips must be at most 1 << 16, reps at most 64 and fenced 0 or 1";
+  cdp::MeasRecord& rec = h->meas[cdp::kMeasPingPong];
   uint32_t f_init = cdp::kPingPongNoFault, f_target = cdp::kPingPongNoFault, f_trip = cdp::kPingPongNoFault;
-  if (h->pp_fault != 0) {
-    const uint64_t fi = h->pp_fault >> 32, ft = (h->pp_fault >> 16) & 0xffffu, trip = h->pp_fault & 0xffffu;
+  if (rec.fault != 0) {
+    const uint64_t fi = rec.fault >> 32, ft = (rec.fault >> 16) & 0xffffu, trip = rec.fault & 0xffffu;
     if (fi == 0 || ft == 0 || fi > n || ft > n || fi == ft) {
       bad = "the armed pingpong fault names no off-diagonal cell";
     } else if (trip + 1 >= trips || (reps == 1 && trip + 2 == trips)) {
@@ -1556,10 +1554,9 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
   }
   // every process runs over the same pair set: the domain's mapping status, from every process's rows
   int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_pingpong", bad, h->pp_calls + 1, {trips, reps, fenced}, st);
-      rc != CDPROBE_OK)
+  if (const int rc = cdp::agree(h, "cdprobe_pingpong", bad, rec.calls + 1, {trips, reps, fenced}, st); rc != CDPROBE_OK)
     return rc;
-  out->call_seq = ++h->pp_calls;
+  out->call_seq = ++rec.calls;
   for (uint32_t li = 0; li < h->n_local; ++li) out->row_mask |= 1u << h->lr[li].grank;
   if (n == 1) {
     out->ms = cdp::now_ms() - t_begin;
@@ -1579,7 +1576,7 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
     const uint32_t g = L.grank;
     cdp::PingPongParams& p = P[li];
     memset(&p, 0, sizeof(p));
-    p.call_seq = h->pp_calls;
+    p.call_seq = rec.calls;
     p.timeout_ns = cdp::timeout_ns(h);
     p.n_rounds = pl.rounds;
     p.trips = trips;
@@ -1613,7 +1610,7 @@ int cdprobe_pingpong(cdprobe_t* h, uint32_t trips, uint32_t reps, uint32_t fence
     for (uint32_t k = 0; k < c.n; ++k) {
       const uint32_t leg = P[li].round[c.slot[k]].first ? 0u : 1u;
       for (uint32_t rep = 0; rep <= reps; ++rep)
-        c.want[k] ^= cdp::pingpong_rep_digest(h->pp_calls, c.slot[k], leg, rep, trips);
+        c.want[k] ^= cdp::pingpong_rep_digest(rec.calls, c.slot[k], leg, rep, trips);
     }
   }
 
@@ -1638,9 +1635,10 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
     cdp::set_err("kind must be a CDPROBE_ATOMIC_*, ops at most 1 << 16 and reps at most 64");
     return CDPROBE_ERR_ARG;
   }
+  cdp::MeasRecord& rec = h->meas[cdp::kMeasAtomics];
   uint32_t f_issuer = cdp::kMaxRanks, f_target = cdp::kMaxRanks;
-  if (h->at_fault != 0) {
-    const uint64_t fi = h->at_fault >> 16, ft = h->at_fault & 0xffffu;
+  if (rec.fault != 0) {
+    const uint64_t fi = rec.fault >> 16, ft = rec.fault & 0xffffu;
     if (fi == 0 || ft == 0 || fi > n || ft > n || (fi == ft && !pl.diag)) {
       cdp::set_err("the armed atomics fault names no cell of this domain");
       return CDPROBE_ERR_ARG;
@@ -1653,7 +1651,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
   reps = out->reps;
   const uint64_t total = (uint64_t)out->lanes * ops;  // increments per rep
   if (const int rc = cdp::ensure_scratch_all(h, cdp::kRepTableBytes); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++h->at_calls;
+  out->call_seq = ++rec.calls;
 
   // 1. every local issuer's cells, all launched before any is waited for; no kernel waits on another rank
   cdp::AtomicsParams P[cdp::kMaxRanks];
@@ -1664,7 +1662,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
     out->row_mask |= 1u << g;
     cdp::AtomicsParams& p = P[li];
     memset(&p, 0, sizeof(p));
-    p.call_seq = h->at_calls;
+    p.call_seq = rec.calls;
     p.timeout_ns = cdp::timeout_ns(h);
     p.ops = ops;
     p.reps = reps;
@@ -1702,7 +1700,7 @@ int cdprobe_atomics(cdprobe_t* h, uint32_t kind, uint32_t ops, uint32_t reps, cd
 
   // 2. while they run: the digest of clean reps, the same for every cell
   uint64_t want = 0;
-  for (uint32_t r = 0; r <= reps; ++r) want ^= cdp::atomics_rep_digest(cdp::atomics_start(h->at_calls, kind, r), total);
+  for (uint32_t r = 0; r <= reps; ++r) want ^= cdp::atomics_rep_digest(cdp::atomics_start(rec.calls, kind, r), total);
   for (cdp::RepCells& c : cells) std::fill(c.want, c.want + c.n, want);
 
   // 3. collect: ns per atomic of the timed reps, the digest of all of them
@@ -1719,10 +1717,11 @@ int cdprobe_bwcurve(cdprobe_t* h, uint32_t reps, cdprobe_bwcurve_t* out) {
   const uint32_t n = h->n_total;
   // 1. the arguments; in a multi-process domain the verdict is shared below, so every process refuses together.  Every
   //    cell is one-sided and the rounds come from the plan, which all processes share, so nothing else must agree
-  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", lad.bad, h->bw_calls + 1, {lad.reps, 0u, 0u}, nullptr);
+  cdp::MeasRecord& rec = h->meas[cdp::kMeasBwCurve];
+  if (const int rc = cdp::agree(h, "cdprobe_bwcurve", lad.bad, rec.calls + 1, {lad.reps, 0u, 0u}, nullptr);
       rc != CDPROBE_OK)
     return rc;
-  out->call_seq = ++h->bw_calls;
+  out->call_seq = ++rec.calls;
   cdp::put_ladder(h, lad, out);
 
   // 2. which cells run; scratch for the rep records and one cell's granule table, grown on every local rank before any
@@ -1798,9 +1797,10 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
   //    every process refuses or runs together over the same cells
   uint32_t f_send = cdp::kA2aNoFault, f_recv = cdp::kA2aNoFault, f_k = cdp::kA2aNoFault;
   uint64_t f_word = 0;
-  if (h->a2a_fault != 0 && lad.bad.empty()) {
-    const uint64_t fs = h->a2a_fault >> 40, fr = (h->a2a_fault >> 32) & 0xffu;
-    const cdp::FaultSpot at = cdp::fault_spot(h->a2a_fault, lad);
+  cdp::MeasRecord& rec = h->meas[cdp::kMeasAllToAll];
+  if (rec.fault != 0 && lad.bad.empty()) {
+    const uint64_t fs = rec.fault >> 40, fr = (rec.fault >> 32) & 0xffu;
+    const cdp::FaultSpot at = cdp::fault_spot(rec.fault, lad);
     f_word = at.word;
     if (fs == 0 || fs > n || fr == 0 || fr > n || (fs == fr && !pl.diag) || !at.word_ok) {
       lad.bad = "the armed all-to-all fault names no cell, size or word of this call";
@@ -1811,12 +1811,12 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     }
   }
   int32_t st[cdp::kMaxRanks][cdp::kMaxRanks];
-  if (const int rc = cdp::agree(h, "cdprobe_alltoall", lad.bad, h->a2a_calls + 1, {lad.reps, 0u, 0u}, st);
+  if (const int rc = cdp::agree(h, "cdprobe_alltoall", lad.bad, rec.calls + 1, {lad.reps, 0u, 0u}, st);
       rc != CDPROBE_OK)
     return rc;
   // 2. the exchange area, built once, by every process in the same call
   if (const int rc = cdp::ensure_area(h, h->area, (size_t)n * pl.bpp); rc != CDPROBE_OK) return rc;
-  out->call_seq = ++h->a2a_calls;
+  out->call_seq = ++rec.calls;
   out->area_bytes = h->area.bytes;
   cdp::put_ladder(h, lad, out);
 
@@ -1870,7 +1870,7 @@ int cdprobe_alltoall(cdprobe_t* h, uint32_t reps, cdprobe_alltoall_t* out) {
     }
     if (!joined) continue;
     p.dom.self = reinterpret_cast<uint64_t*>(va[g] + cdp::kA2aOff + (uint64_t)g * sizeof(cdp::FlagLine));
-    p.dom.call_seq = h->a2a_calls;
+    p.dom.call_seq = rec.calls;
     // the blocks, in the order rank + 1, rank + 2, ... (mod n), then the diagonal
     p.fault_k = cdp::kA2aNoFault;
     for (uint32_t d = 1; d <= n; ++d) {
